@@ -1,7 +1,7 @@
 /*
  * plaid_b200.h -- C-ABI of libplaid_b200: the PLAID search hot path of the `next-plaid` crate
  * (centroid scoring -> IVF candidates -> approximate score -> residual decompression -> MaxSim ->
- * top-k) as hand-written sm_100a CUDA, behind the entry points a Rust `extern "C"` block in
+ * top-k) as hand-written sm_90a CUDA, behind the entry points a Rust `extern "C"` block in
  * next-plaid/src/index.rs would bind (INTEGRATION.md shows that shim).
  *
  * The reference has no FFI for this path (search is hard-wired to the CPU, search.rs:85-90), so
@@ -11,7 +11,7 @@
  *   - plain pointers and sizes, no C++/torch types; every function returns a pb_status (0 = ok);
  *     pb_last_error() gives the thread-local message the shim maps to Error::Search(String)
  *     (error.rs:10-66).
- *   - there is NO CPU fallback: without a usable sm_100 device every entry point fails with
+ *   - there is NO CPU fallback: without a usable sm_90 device every entry point fails with
  *     PB_ERR_CUDA (same contract as NEXT_PLAID_FORCE_GPU, lib.rs:71-84, codec.rs:275-288).
  *   - index arrays are copied to the device at open; query / result pointers are never retained
  *     past the call; a handle may be searched from many host threads at once (state.rs:24-47).
@@ -215,14 +215,14 @@ enum {
  * candidate.  Both produce the reference's cut bit for bit; tests compare them. */
 PB_API void pb_set_fast_approx(pb_index *ix, int32_t enabled);
 
-/* Diagnostic switch for the exact stage (default on): 1 = an fp16 tcgen05 estimate with a certified error bound
+/* Diagnostic switch for the exact stage (default on): 1 = an fp16 wgmma estimate with a certified error bound
  * first picks the kept docs that can still reach the top_k, and only those are scored exactly; 0 = every kept
  * doc is scored exactly.  Same results bit for bit; tests compare both.  (PB_FAST_EXACT=0 in the environment
  * sets the default.)  The filter applies when dim is 64/96/128, queries have <= 64 tokens and no trace is asked. */
 PB_API void pb_set_fast_exact(pb_index *ix, int32_t enabled);
 
-/* Diagnostic switch for a2 (default on): 1 = the score table comes from the tcgen05 split-fp16 GEMM (k_scores16_tc) and
- * the values that decide something are recomputed as pinned-order fp32 dots; 0 = the dense fp32 FFMA2 kernel
+/* Diagnostic switch for a2 (default on): 1 = the score table comes from the wgmma split-fp16 GEMM (k_scores16_tc) and
+ * the values that decide something are recomputed as pinned-order fp32 dots; 0 = the dense fp32 FMA kernel
  * (k_centroid_scores), which is also the device-gated fallback for flagged queries and shapes outside the tensor-core
  * kernel's (dim not in {64, 96, 128}, eligibility filters, the dense variant's radix-select probe for n_ivf_probe > 64, n_ivf_probe > K/1024).  Same results bit
  * for bit; tests and bench.py compare both.  (PB_K1_TC=0 in the environment sets the default.) */
@@ -250,7 +250,7 @@ PB_API pb_status pb_last_call_ms(pb_index *ix, float *out_ms);
 enum {
     PB_KERNEL_SCORES = 0,   /* k_scores16_tc (or k_centroid_scores on the exact path) */
     PB_KERNEL_APPROX16 = 1, /* k_approx16, the first approximate pass */
-    PB_KERNEL_FILTER = 2,   /* k_exact_tc, the tcgen05 MaxSim estimate of every kept doc */
+    PB_KERNEL_FILTER = 2,   /* k_exact_tc, the wgmma MaxSim estimate of every kept doc */
     PB_KERNEL_EXACT = 3,    /* k_exact, fused decompress + MaxSim of the survivors */
     PB_KERNEL_COUNT = 4
 };
@@ -273,7 +273,7 @@ typedef struct pb_work_counters {
                                   * cells) that differ from the dense score table; 0 expected */
     int64_t n_probe_threshold;   /* sub-batches whose a3 ran threshold-first on the 16-bit table (no device fallback) */
     int64_t n_probe_list;        /* sub-batches whose a3 ran the per-lane list scan (fallback, eligibility filter, ...) */
-    int64_t n_k1_tc;             /* sub-batches whose score table came from the tcgen05 kernel (k_scores16_tc) */
+    int64_t n_k1_tc;             /* sub-batches whose score table came from the wgmma kernel (k_scores16_tc) */
     int64_t n_recheck_docs;      /* docs that got the exact fp32 approximate score (a5 second pass) */
     int64_t n_k1_tc_redo;        /* sub-batches the tensor-core pass handed back to the exact path (flagged query, list overflow) */
     int64_t n_exact_pairs;       /* (token, query token) similarities the pair form of the exact stage evaluated */
@@ -302,7 +302,7 @@ typedef struct pb_shard_group pb_shard_group;   /* in-process rank group, see "d
 PB_API pb_status pb_codec_open(int32_t device, const float *centroids, int64_t num_centroids, int32_t dim,
                                int32_t nbits, const float *bucket_cutoffs /* may be NULL */, pb_codec **out);
 PB_API void pb_codec_close(pb_codec *c);
-/* How the last compress/encode call found its codes: tokens whose argmax the tcgen05 shortlist certified
+/* How the last compress/encode call found its codes: tokens whose argmax the wgmma shortlist certified
  * vs tokens sent through the exact fp32 kernel (all of them when the filter is not in use: dim not in
  * {64, 96, 128}, K < 256, or PB_ASSIGN_EXACT set). */
 PB_API pb_status pb_codec_last_assign_stats(pb_codec *c, int64_t *n_tokens, int64_t *n_exact_fallback,

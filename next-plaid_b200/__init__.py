@@ -1,4 +1,4 @@
-"""plaid_b200: B200-native (sm_100a) PLAID search path behind next-plaid's MmapIndex interface.
+"""plaid_b200: H100-native (sm_90a) PLAID search path behind next-plaid's MmapIndex interface.
 
 The directory is named `next-plaid_b200` (the name the project brief fixes); import it as
 `next_plaid_b200` through the shim module at the repository root.

@@ -1,4 +1,4 @@
-"""Build libplaid_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Build libplaid_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -13,7 +13,7 @@ DEPS = SOURCES + sorted(f for f in os.listdir(CSRC) if f.endswith((".cuh", ".h")
     [os.path.join("..", "..", "include", "plaid_b200.h")]
 NVCC_FLAGS = [
     "-shared", "-std=c++17", "-O3", "-lineinfo",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-Xcompiler", "-fPIC,-fvisibility=hidden",
 ]
 

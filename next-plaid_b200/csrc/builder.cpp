@@ -7,7 +7,7 @@
 //   2. prepare_codec_artifacts (index.rs:182-287): held-out rows from the end of a doc sample -> bucket cutoffs /
 //      weights, avg_residual, cluster_threshold (pb_codec_train)
 //   3. per chunk of `batch_size` docs (index.rs:289-371, :420-473): nearest-centroid codes + packed residuals
-//      (pb_codec_encode_chunk: tcgen05 certified assignment), {i}.codes.npy, {i}.residuals.npy, doclens.{i}.json,
+//      (pb_codec_encode_chunk: wgmma certified assignment), {i}.codes.npy, {i}.residuals.npy, doclens.{i}.json,
 //      {i}.metadata.json
 //   4. inverted file (index.rs:850-873): built on the device by pb_index_open (no ivf given), exported to
 //      ivf.npy / ivf_lengths.npy; metadata.json, plan.json

@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for libplaid_b200 (sm_100a).
+// common.cuh -- shared device helpers for libplaid_b200 (sm_90a).
 //
 // Numerics contract (DESIGN.md "Numerics"): every floating-point operation that feeds a ranking
 // decision is written with explicit round-to-nearest intrinsics so nvcc can neither fuse nor

@@ -1,7 +1,7 @@
 // engine.cu -- host side of libplaid_b200: the device-resident index (what MmapIndex holds after
 // load, index.rs:995-1016), the search pipeline that replaces search::search_many_mmap
 // (search.rs:643) and the C-ABI of include/plaid_b200.h.  No CPU fallback anywhere: every entry
-// point needs an sm_100 device.
+// point needs an sm_90 (H100) device.
 #include "engine_internal.h"
 #include "kernels.cuh"
 
@@ -145,7 +145,7 @@ pb_status pb_fail(pb_status s, const char *fmt, ...) {
     } while (0)
 
 extern "C" const char *pb_last_error(void) { return g_err.c_str(); }
-extern "C" const char *pb_version(void) { return "plaid_b200 0.1 (sm_100a)"; }
+extern "C" const char *pb_version(void) { return "plaid_b200 0.1 (sm_90a)"; }
 
 extern "C" int32_t pb_device_count(void) {
     int n = 0;
@@ -167,8 +167,8 @@ static pb_status check_device(int device) {
     if (device < 0 || device >= n) return pb_fail(PB_ERR_INVALID, "device %d out of range (have %d)", device, n);
     cudaDeviceProp p;
     CK(cudaGetDeviceProperties(&p, device));
-    if (p.major != 10)
-        return pb_fail(PB_ERR_CUDA, "device %d is sm_%d%d; this library is built for sm_100a only", device, p.major,
+    if (p.major != 9 || p.minor != 0)
+        return pb_fail(PB_ERR_CUDA, "device %d is sm_%d%d; this library is built for sm_90a only", device, p.major,
                        p.minor);
     CK(cudaSetDevice(device));
     return PB_OK;
@@ -330,7 +330,7 @@ struct pb_index {
     int dim = 0, nbits = 0, packed = 0;
     long long K = 0, D = 0, N = 0, ivf_len = 0, doc_id_base = 0;
     int max_doclen = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     DevBuf centroids, w_rev, codes, residuals, doc_off, ivf, ivf_off, ucodes, udoc_off;
     long long n_ucodes = 0;
     bool build_ivf = false;    // no inverted file was given: built from the codes at finalize (index.rs:850-873)
@@ -341,11 +341,11 @@ struct pb_index {
     int k1_margin = 1;         // E: code units an estimate-built 16-bit code may differ from the exact one (PB_K1_TC_E widens it)
     int cent_exp = 0;          // centroids enter the tensor-core operands scaled by 2^cent_exp (max norm in [1, 2))
     bool k1_diag = false;      // also run the exact table and report the largest code difference (PB_K1_TC_DIAG=1)
-    DevBuf cent_h16t, cent_l16t;  // its centroid operands: fp16 hi / lo, UMMA tile order
+    DevBuf cent_h16t, cent_l16t;  // its centroid operands: fp16 hi / lo, MMA tile order
     int approx_grid = 8;       // k_approx16 CTAs per SM and query (PB_APPROX_GRID)
     int xtc_grid = 32;         // k_exact_tc CTAs per SM across the batch (PB_XTC_GRID)
     bool probe16 = true;       // a3 threshold-first selection on the 16-bit table (PB_PROBE16=0: per-lane lists only)
-    bool fast_exact = true;    // tcgen05 certified filter in front of the exact stage (same results either way)
+    bool fast_exact = true;    // tensor-core certified filter in front of the exact stage (same results either way)
     float vmin = 0.0f;         // smallest pre-normalisation token norm |c + w| over the index (error bound of the filter)
     float wmax = 0.0f;         // largest residual norm |w| over the index (same)
     DevBuf centroids_f16;      // [K][dim] fp16 copy for the filter (k_exact_tc, the variant without a score table)
@@ -398,7 +398,7 @@ struct pb_index {
 
 // QS: query tokens per score-table row.  Up to 32 tokens: rounded up to 8 (rows of at most 64 bytes); beyond: to a
 // multiple of 64, so that a row is whole 128-byte lines (a 96-byte row straddles lines and costs the first approximate
-// pass 2.5x instead of 1.5-2x: profiles/r02_summary.md)
+// pass extra L2 requests)
 static int query_row_tokens(int nq_max) {
     return nq_max <= 32 ? std::max(8, (nq_max + 7) & ~7) : ((nq_max + 63) & ~63);
 }
@@ -811,7 +811,7 @@ static bool k1_tc_usable(const pb_index *ix) {
     return ix->k1_tc && ix->cent_h16t.p && (ix->dim == 64 || ix->dim == 96 || ix->dim == 128) && k1_err_codes(ix->dim) < 1.0f;
 }
 
-// the 16-bit score table from the split-fp16 UMMA GEMM (k_scores16_tc) into `table`; `flags` gets the per-query
+// the 16-bit score table from the split-fp16 wgmma GEMM (k_scores16_tc) into `table`; `flags` gets the per-query
 // out-of-range bits the exact kernel would set in qflag
 static pb_status launch_k1_table(pb_index *ix, Workspace &ws, int B, int QS, unsigned short *table, int *flags) {
     const int n_groups = (int)(((long long)B * QS + 127) / 128);
@@ -830,7 +830,7 @@ static pb_status launch_k1_table(pb_index *ix, Workspace &ws, int B, int QS, uns
         auto kern = k_scores16_tc<DV>;                                                                                 \
         CKS(set_smem(kern, sm));                                                                                       \
         KEV_BEGIN(PB_KERNEL_SCORES);                                                                                   \
-        kern<<<tiles, 320, sm, ws.stream>>>(ix->cent_h16t.as<__half>(), ix->cent_l16t.as<__half>(), ix->K,             \
+        kern<<<tiles, 288, sm, ws.stream>>>(ix->cent_h16t.as<__half>(), ix->cent_l16t.as<__half>(), ix->K,             \
                                             ws.Qh16t.as<__half>(), ws.Ql16t.as<__half>(), n_groups, B, QS,             \
                                             ws.qoff.as<int>(), ws.qrange_tc.as<float2>(), table, flags);               \
         KEV_END(PB_KERNEL_SCORES);                                                                                     \
@@ -944,7 +944,7 @@ static pb_status launch_centroid_scores_exact(pb_index *ix, Workspace &ws, int B
     const int tiles = (int)((ix->K + PB_TOK_TILE - 1) / PB_TOK_TILE);
     // enough CTAs to fill the machine twice over; each CTA keeps its centroid tile in smem and walks queries
     int groups = std::max(1, std::min(B, (4 * ix->sm_count + tiles - 1) / tiles));
-    // packed fp32 FMA (FFMA2): query rows interleaved pairwise, one instruction advances two dots
+    // paired fp32 FMA tile: query rows interleaved pairwise, one 8-byte load feeds two dots
     CKS(ws.Qi.ensure((size_t)B * QS * ix->dim * 4));
     k_interleave_query_rows<<<dim3(8, B), 256, 0, ws.stream>>>(ws.Q.as<float>(), ws.qoff.as<int>(), QS, ix->dim,
                                                                ws.Qi.as<float>());
@@ -1021,7 +1021,8 @@ static pb_status launch_exact(pb_index *ix, Workspace &ws, const KeptView &kv, i
 
 static size_t smem_exact_tc(int dim, int packed, int nqt) {
     const int nbits = packed * 8 / dim;
-    return (size_t)(dim / 8) * PB_XTC_LBO + (size_t)nqt * dim * 2 + (size_t)256 * (8 / nbits) * 2 + 64;
+    return (size_t)(dim / 8) * PB_XTC_LBO + (size_t)nqt * dim * 2 + (size_t)256 * (8 / nbits) * 2 +
+           (size_t)128 * ACC_LD(nqt) * 4;
 }
 
 // error of one fp16 tensor-core similarity relative to |q| (derivation above k_exact_tc); 0 = filter unusable
@@ -1052,8 +1053,7 @@ static float filter_eps_unit2(const pb_index *ix, int E) {
 static size_t smem_maxsim_tc(int dim, int packed, int nqt) {
     const int nbits = packed * 8 / dim;
     return (size_t)2 * (dim / 8) * PB_XTC_LBO + (size_t)nqt * dim * 2 + (size_t)256 * (8 / nbits) * 2 * (nbits == 4 ? 4 : 1) +
-           4 * 128 * sizeof(MsMeta) +
-           12 * 8 + 16;
+           4 * 128 * sizeof(MsMeta) + 8 * 8 + (size_t)128 * ACC_LD(nqt) * 4;
 }
 
 // the warp-specialised linear estimate over the docs of `in`: pass 1 (pairs == nullptr) leaves per (doc, q) maxima in
@@ -1078,7 +1078,7 @@ static pb_status launch_maxsim_tc(pb_index *ix, Workspace &ws, const KeptView &i
         auto kern = k_maxsim_tc<DV, NB, NQ, EM>;                                                                       \
         CKS(set_smem(kern, sm));                                                                                       \
         if (kev >= 0) KEV_BEGIN(kev);                                                                                  \
-        kern<<<dim3(gx, B), 288, sm, ws.stream>>>(ws.Q.as<float>(), ws.qoff.as<int>(), QS, ws.ST16.as<unsigned short>(), \
+        kern<<<dim3(gx, B), 256, sm, ws.stream>>>(ws.Q.as<float>(), ws.qoff.as<int>(), QS, ws.ST16.as<unsigned short>(), \
                                                   ix->K, ws.qrange.as<float2>(), ws.qflag.as<int>(), ix->w_rev.as<float>(), \
                                                   ix->codes.as<uint32_t>(), ix->residuals.as<uint8_t>(),               \
                                                   ix->tok_inv_norm.as<float>(), ws.gbase.as<long long>(),              \
@@ -2078,7 +2078,9 @@ extern "C" pb_status pb_maxsim_scores(int32_t device, const float *query, int32_
     CKS(dmax.ensure((size_t)Mcap * QS * 4));
     CKS(dex.ensure((size_t)Mcap * 4));
     long long chunks = (total + PB_TOK_TILE - 1) / PB_TOK_TILE;
-    int gx = (int)std::max<long long>(1, std::min<long long>(chunks, 148ll * 16));
+    int sms = 0;
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+    int gx = (int)std::max<long long>(1, std::min<long long>(chunks, (long long)sms * 16));
     switch (dim) {
 #define PB_CASE(DV)                                                                                              \
     case DV: {                                                                                                   \
@@ -2214,11 +2216,11 @@ extern "C" pb_status pb_index_group_join(pb_index *ix, pb_shard_group *g, int32_
 // index-build path (SURVEY 8 a12, secondary): ResidualCodec on the device
 // ------------------------------------------------------------------------------------------
 struct pb_codec {
-    int device = 0, dim = 0, nbits = 0, sm_count = 148;
+    int device = 0, dim = 0, nbits = 0, sm_count = 132;
     long long K = 0;
     DevBuf centroids, cutoffs, cent_bf16, cent_norm;
     bool has_cutoffs = false;
-    bool use_tc = false;   // tcgen05 certified filter in front of the exact assignment
+    bool use_tc = false;   // tensor-core certified filter in front of the exact assignment
     float cmax = 0.f;
     int c_finite = 1;
     long long last_tokens = 0, last_fallback = 0;
@@ -2322,7 +2324,7 @@ static pb_status assign_codes(pb_codec *c, const float *dX, long long m, long lo
     case DV: {                                                                                             \
         auto kern = k_assign_tc<DV, false>;                                                                \
         CKS(set_smem(kern, sm));                                                                           \
-        kern<<<blocks, 320, sm>>>(xb.as<__nv_bfloat16>(), m, c->cent_bf16.as<__nv_bfloat16>(), c->K, ts.as<float>(), \
+        kern<<<blocks, 288, sm>>>(xb.as<__nv_bfloat16>(), m, c->cent_bf16.as<__nv_bfloat16>(), c->K, ts.as<float>(), \
                                   ti.as<uint32_t>(), nullptr);                                             \
     } break;
         PB_TC_CASE(64) PB_TC_CASE(96) PB_TC_CASE(128)
@@ -2521,7 +2523,7 @@ extern "C" int64_t pb_codec_heldout_tokens(int64_t num_embeddings) {  // min(0.0
     return (int64_t)std::min(0.05 * (double)num_embeddings, 50000.0);
 }
 
-// k-means assignment step.  dims 64 / 96 / 128 with K >= 256: the fp16 tcgen05 GEMM of the encode path with the
+// k-means assignment step.  dims 64 / 96 / 128 with K >= 256: the fp16 wgmma GEMM of the encode path with the
 // -|c|^2/2 bias added in its epilogue, best shortlist entry taken as is; otherwise the exact fp32 kernel.
 struct KmeansAssign {
     DevBuf xb, cb, bias, ts, ti, scratch;
@@ -2560,7 +2562,7 @@ struct KmeansAssign {
     case DV: {                                                                                                         \
         auto kern = k_assign_tc<DV, true>;                                                                             \
         CKS(set_smem(kern, sm));                                                                                       \
-        kern<<<blocks, 320, sm, st>>>(xb.as<__nv_bfloat16>(), n, cb.as<__nv_bfloat16>(), K, ts.as<float>(),            \
+        kern<<<blocks, 288, sm, st>>>(xb.as<__nv_bfloat16>(), n, cb.as<__nv_bfloat16>(), K, ts.as<float>(),            \
                                       ti.as<uint32_t>(), bias.as<float>());                                            \
     } break;
             PB_KM_CASE(64) PB_KM_CASE(96) PB_KM_CASE(128)

@@ -81,9 +81,6 @@ __global__ void k_max_row_norm(const float *__restrict__ C, long long K, int dim
 PB_DEV uint32_t pick4(const uint4 &c, int r) { return r == 0 ? c.x : (r == 1 ? c.y : (r == 2 ? c.z : c.w)); }
 
 PB_DEV uint4 gather16(const char *p) { return *reinterpret_cast<const uint4 *>(p); }
-// (ld.global.cg row gathers and a signature-sorted candidate order with contiguous slices per CTA were measured on
-// config B -- 3.10 / 3.37 ms for the stage against 3.07 -- and removed; tools/tma_gather_bench.cu has the ceiling:
-// 231 G rows/s for bare 64-byte LSU gathers, 264 G for 32-byte rows, 13.7 G through TMA gather4.)
 // LPR = lanes per row: 4 (rows up to 64 bytes: nq <= 32, eight rows per load instruction) or 8 (up to 128 bytes:
 // nq <= 64 in ONE pass over the codes, four rows per instruction).  Longer queries loop over 8*LPR-token column blocks.
 template <int LPR>

@@ -1,4 +1,4 @@
-// k_build.cuh -- index build: assignment (exact fp32 and tcgen05 certified), quantise + pack, k-means.
+// k_build.cuh -- index build: assignment (exact fp32 and tensor-core certified), quantise + pack, k-means.
 // Part of kernels.cuh (included from there, in order; not a standalone header).
 // ==========================================================================================
 // Index-build path (SURVEY 8 a12, secondary): nearest-centroid assignment, residual quantisation
@@ -189,10 +189,10 @@ __global__ void k_gather_rows(const float *__restrict__ X, const long long *__re
 }
 
 // ==========================================================================================
-// tcgen05 certified filter for nearest-centroid assignment (index-build path).
+// Tensor-core certified filter for nearest-centroid assignment (index-build path).
 //
-// The exact kernel above spends 128 fp32 FMAs per (token, centroid) pair.  Here an fp16 UMMA
-// (tcgen05.mma.kind::f16, fp32 accumulators in TMEM) scores every pair and the epilogue keeps the 4 best
+// The exact kernel above spends 128 fp32 FMAs per (token, centroid) pair.  Here an fp16 wgmma
+// (fp32 accumulators in registers) scores every pair and the epilogue keeps the 4 best
 // centroids per token.  |s_tc - s_exact| <= eps = (2^-10 + 2^-22) |x| max|c| + 2^-24 sqrt(dim) (|x| + max|c|) + 1e-5
 // (two fp16 roundings per product, Cauchy-Schwarz; the absolute spacing of fp16 subnormals; fp32 accumulation
 // slack), so if the 4th best tensor-core score is more than 2*eps below the best, the true argmax is among the
@@ -203,8 +203,8 @@ __global__ void k_gather_rows(const float *__restrict__ X, const long long *__re
 // (near ties, non-finite values) go through k_assign.  The result is therefore bit-identical to
 // compress_into_codes_cpu while ~98 % of the arithmetic runs on the tensor cores.
 //
-// One CTA = 256 tokens (two UMMA M = 128 tiles sharing every 128-centroid tile), 320 threads: warps
-// 0-7 epilogue (one TMEM lane = one token each), warp 8 loader (cp.async, 3-stage ring), warp 9 MMA issuer.
+// One CTA = 256 tokens (two 128-token tiles sharing every 128-centroid tile), 288 threads: warps
+// 0-7 two warpgroups that issue the MMAs and rank their tokens, warp 8 loader (bulk copies, 3-stage ring).
 // Operands sit in shared memory in the canonical K-major no-swizzle layout (8 rows x 16 bytes core
 // matrices; SBO = 128 B between row groups, LBO = rows/8 * 128 B between the two 8-element K
 // chunks of one MMA).
@@ -242,36 +242,70 @@ PB_DEV void bulk_g2s(void *smem_dst, const void *gsrc, uint32_t bytes, uint64_t 
                  ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
                  : "memory");
 }
-PB_DEV void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-PB_DEV void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-PB_DEV void tc_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-PB_DEV void tc_mma_bf16(uint32_t tmem_c, u64 adesc, u64 bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n"
-                 ::"r"(tmem_c), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-                 : "memory");
-}
-// shared-memory matrix descriptor, K-major, no swizzle (cute::UMMA::SmemDescriptor: start>>4 [0,14),
-// LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48), layout_type=0 [61,64))
-PB_DEV u64 tc_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// ---- Hopper warpgroup MMA (wgmma) ----
+// The 128 threads of a warpgroup issue one m64nNk16 product together (fp16 operands from shared memory, fp32
+// accumulator in registers).  Fragment of thread t of the warpgroup: d[4i + 2h + j] = element (row 16 (t/32) +
+// (t%32)/4 + 8h, column 8i + 2 (t%4) + j).
+// shared-memory matrix descriptor, K-major, no swizzle: start>>4 [0,14), LBO>>4 [16,30) = byte stride between the
+// 8-element K chunks, SBO>>4 [32,46) = byte stride between 8-row groups, layout type 0 [62,64)
+PB_DEV u64 wg_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     return (u64)((saddr >> 4) & 0x3fffu) | ((u64)((lbo_bytes >> 4) & 0x3fffu) << 16) |
-           ((u64)((sbo_bytes >> 4) & 0x3fffu) << 32) | (1ull << 46);
+           ((u64)((sbo_bytes >> 4) & 0x3fffu) << 32);
 }
-PB_DEV void tc_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+PB_DEV void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+PB_DEV void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// waits for every committed group, then pins the accumulator registers behind the wait (the compiler must not read
+// them earlier)
+template <int R> PB_DEV void wg_wait_all(float (&d)[R]) {
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// d (+)= A B^T, A = 64 rows x 16 (descriptor da), B = N rows x 16 (descriptor db); accumulate = 0 overwrites d
+template <int N> PB_DEV void wg_mma_f16(float (&d)[N / 2], u64 da, u64 db, uint32_t accumulate);
+template <> PB_DEV void wg_mma_f16<32>(float (&d)[16], u64 da, u64 db, uint32_t accumulate) {
+    asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %18, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 : "l"(da), "l"(db), "r"(accumulate));
+}
+template <> PB_DEV void wg_mma_f16<64>(float (&d)[32], u64 da, u64 db, uint32_t accumulate) {
+    asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "l"(da), "l"(db), "r"(accumulate));
+}
+template <> PB_DEV void wg_mma_f16<128>(float (&d)[64], u64 da, u64 db, uint32_t accumulate) {
+    asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(da), "l"(db), "r"(accumulate));
+}
+// The filters' epilogues work per token (thread = accumulator row).  Their warpgroup stages its m64nN fragment into a
+// row-major fp32 tile of ACC_LD(N) floats per row (+4: conflict-free 16-byte row reads) ...
+#define ACC_LD(N) ((N) + 4)
+template <int N> PB_DEV void wg_stage(float *tile, const float (&d)[N / 2]) {
+    const int t = threadIdx.x & 127;
+    float *p = tile + (16 * (t >> 5) + ((t & 31) >> 2)) * ACC_LD(N) + 2 * (t & 3);
+#pragma unroll
+    for (int i = 0; i < N / 8; ++i) {
+        *reinterpret_cast<float2 *>(p + 8 * i) = make_float2(d[4 * i], d[4 * i + 1]);
+        *reinterpret_cast<float2 *>(p + 8 * ACC_LD(N) + 8 * i) = make_float2(d[4 * i + 2], d[4 * i + 3]);
+    }
+}
+// ... and reads R consecutive columns of its own row back
+template <int R> PB_DEV void acc_row(const float *p, uint32_t (&r)[R]) {
+#pragma unroll
+    for (int i = 0; i < R / 4; ++i) {
+        const uint4 v = reinterpret_cast<const uint4 *>(p)[i];
+        r[4 * i] = v.x;
+        r[4 * i + 1] = v.y;
+        r[4 * i + 2] = v.z;
+        r[4 * i + 3] = v.w;
+    }
 }
 
-// f32 rows -> fp16 (round to nearest even; the array type says bf16 for history, the bits are fp16) in UMMA tile order
+// f32 rows -> fp16 (round to nearest even; the array type says bf16 for history, the bits are fp16) in MMA tile order
 // + the L2 norm of every row.
 // Tile order: blocks of 128 rows, each block stored exactly as the kernel wants it in shared memory --
 // K-major canonical no-swizzle layout, byte (kc*16 + r/8)*128 + (r%8)*16 + 2*e for row r, 16-byte K chunk
@@ -300,24 +334,21 @@ __global__ void k_rows_to_bf16(const float *__restrict__ X, long long n, int dim
 // BIAS: rank x.c + bias[c] instead of x.c (k-means: bias = -|c|^2 / 2 turns the maximum into the L2-nearest centroid);
 // the encode path instantiates BIAS = false.
 template <int DIM, bool BIAS>
-__global__ void __launch_bounds__(320, 1)
+__global__ void __launch_bounds__(288, 1)
 k_assign_tc(const __nv_bfloat16 *__restrict__ Xb, long long n, const __nv_bfloat16 *__restrict__ Cb, long long K,
             float *__restrict__ top_s /* [n][4] */, uint32_t *__restrict__ top_i /* [n][4] */,
             const float *__restrict__ bias /* [ceil(K/128)*128] or NULL */) {
-    // 256 tokens per CTA = two UMMA M=128 operand tiles that share every centroid tile (halves the L2
-    // traffic per token); N = 128 centroids per tile; TMEM = 2 buffers x 2 halves x 128 fp32 columns.
-    // warps 0-7 epilogue (warp w: token half w/4, TMEM lanes 32*(w%4)..), warp 8 loader, warp 9 MMA issuer.
+    // 256 tokens per CTA = two 128-token operand tiles that share every centroid tile (halves the L2 traffic per
+    // token); N = 128 centroids per tile.  warps 0-7: two consumer warpgroups (warpgroup h = token tile h, as two
+    // M = 64 slabs), warp 8: loader.
     extern __shared__ __align__(1024) unsigned char smem_tc[];
-    constexpr int KC = DIM / 8;            // 16-byte K chunks per row
-    constexpr int KSTEPS = DIM / 16;       // UMMA K = 16 for bf16
+    constexpr int KSTEPS = DIM / 16;       // wgmma K = 16 for fp16
     constexpr uint32_t A_BYTES = PB_TC_M * DIM * 2, B_BYTES = PB_TC_N * DIM * 2;   // per 128-row tile
     constexpr uint32_t LBO = (128 / 8) * 128, SBO = 128;
     unsigned char *As = smem_tc;                 // 2 tiles (token halves)
     unsigned char *Bs = smem_tc + 2 * A_BYTES;   // PB_TC_STAGES tiles
     uint64_t *bars = reinterpret_cast<uint64_t *>(Bs + PB_TC_STAGES * B_BYTES);
-    uint64_t *full = bars, *empty = bars + PB_TC_STAGES, *tfull = bars + 2 * PB_TC_STAGES, *tempty = tfull + 2;
-    uint64_t *abar = tempty + 2;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(abar + 1);
+    uint64_t *full = bars, *empty = bars + PB_TC_STAGES, *abar = bars + 2 * PB_TC_STAGES;
     const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long x0 = (long long)blockIdx.x * (2 * PB_TC_M);
     const long long n_tiles = (K + PB_TC_N - 1) / PB_TC_N;
@@ -325,33 +356,20 @@ k_assign_tc(const __nv_bfloat16 *__restrict__ Xb, long long n, const __nv_bfloat
     if (threadIdx.x == 0) {
         for (int i = 0; i < PB_TC_STAGES; ++i) {
             mbar_init(&full[i], 1);
-            mbar_init(&empty[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tfull[i], 1);
-            mbar_init(&tempty[i], 256);
+            mbar_init(&empty[i], 8);  // one arrival per consumer warp
         }
         mbar_init(abar, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (w == 9) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    // A tiles: this CTA's two 128-token tiles, one bulk copy each (the bf16 array is stored in tile order)
-    if (threadIdx.x == 0) {
-        mbar_expect_tx(abar, 2 * A_BYTES);
-        bulk_g2s(As, reinterpret_cast<const unsigned char *>(Xb) + (size_t)(2 * blockIdx.x) * A_BYTES, A_BYTES, abar);
-        bulk_g2s(As + A_BYTES, reinterpret_cast<const unsigned char *>(Xb) + (size_t)(2 * blockIdx.x + 1) * A_BYTES, A_BYTES, abar);
-    }
-    const uint32_t tmem_base = *tmem_slot;
 
     if (w == 8) {
-        // ---------------- loader: one elected lane, one 32 KB bulk copy per centroid tile ----------------
+        // ---------------- loader: one elected lane, one bulk copy per token tile and per centroid tile ----------------
         if (lane == 0) {
+            // A tiles: this CTA's two 128-token tiles (the fp16 array is stored in tile order)
+            mbar_expect_tx(abar, 2 * A_BYTES);
+            bulk_g2s(As, reinterpret_cast<const unsigned char *>(Xb) + (size_t)(2 * blockIdx.x) * A_BYTES, A_BYTES, abar);
+            bulk_g2s(As + A_BYTES, reinterpret_cast<const unsigned char *>(Xb) + (size_t)(2 * blockIdx.x + 1) * A_BYTES, A_BYTES, abar);
             for (long long t = 0; t < n_tiles; ++t) {
                 const int st = (int)(t % PB_TC_STAGES);
                 mbar_wait(&empty[st], (uint32_t)(((t / PB_TC_STAGES) & 1) ^ 1));
@@ -360,83 +378,119 @@ k_assign_tc(const __nv_bfloat16 *__restrict__ Xb, long long n, const __nv_bfloat
                          &full[st]);
             }
         }
-    } else if (w == 9) {
-        // ---------------- MMA issuer ----------------
-        // instruction descriptor (cute::UMMA::InstrDescriptor): c=f32 [4,6)=1, a=f16 [7,10)=0,
-        // b=f16 [10,13)=0, both K-major, N>>3 [17,23), M>>4 [24,29)
-        const uint32_t idesc = (1u << 4) | ((uint32_t)(PB_TC_N >> 3) << 17) | ((uint32_t)(PB_TC_M >> 4) << 24);
+    } else {
+        // ---------------- consumers: MMA, then a running top-4 per token row ----------------
+        // thread row (slab p, half h) = token 64 p + 16 (w%4) + lane/4 + 8 h of the warpgroup's tile; its 32 columns of
+        // a centroid tile are 8 i + 2 (lane%4) + j, visited in ascending order, so strict '>' keeps the lowest index
+        // among equal scores exactly as a scan over all columns would; the quad's four lists are merged at the end.
+        const int half = w >> 2;
+        float s[4][4];
+        uint32_t ix[4][4];
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                s[r][k] = -INFINITY;
+                ix[r][k] = 0xffffffffu;
+            }
+        float d[PB_TC_N / 2];
+#pragma unroll
+        for (int i = 0; i < PB_TC_N / 2; ++i) d[i] = 0.0f;
         mbar_wait(abar, 0);  // token tiles landed
         for (long long t = 0; t < n_tiles; ++t) {
-            const int st = (int)(t % PB_TC_STAGES), acc = (int)(t & 1);
+            const int st = (int)(t % PB_TC_STAGES);
             mbar_wait(&full[st], (uint32_t)((t / PB_TC_STAGES) & 1));
-            mbar_wait(&tempty[acc], (uint32_t)(((t >> 1) & 1) ^ 1));
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t a0 = smem_u32(As), b0 = smem_u32(Bs + (size_t)st * B_BYTES);
-#pragma unroll
-                for (int half = 0; half < 2; ++half)
-#pragma unroll
-                    for (int s = 0; s < KSTEPS; ++s) {
-                        const u64 ad = tc_smem_desc(a0 + half * A_BYTES + s * 2 * LBO, LBO, SBO);
-                        const u64 bd = tc_smem_desc(b0 + s * 2 * LBO, LBO, SBO);
-                        tc_mma_bf16(tmem_base + acc * 256 + half * PB_TC_N, ad, bd, idesc, s > 0 ? 1u : 0u);
-                    }
-                tc_commit(&empty[st]);   // B tile consumed
-                tc_commit(&tfull[acc]);  // accumulators ready
-            }
-            __syncwarp();
-        }
-    } else {
-        // ---------------- epilogue: thread = token row, running top-4 over all centroids ----------------
-        float s0 = -INFINITY, s1 = -INFINITY, s2 = -INFINITY, s3 = -INFINITY;
-        uint32_t i0 = 0xffffffffu, i1 = 0xffffffffu, i2 = 0xffffffffu, i3 = 0xffffffffu;
-        const int half = w >> 2, lg = w & 3;
-        for (long long t = 0; t < n_tiles; ++t) {
-            const int acc = (int)(t & 1);
-            mbar_wait(&tfull[acc], (uint32_t)((t >> 1) & 1));
-            tc_fence_after();
             const long long c0 = t * PB_TC_N;
             const bool edge = c0 + PB_TC_N > K;  // the (zero-filled) columns past K must not be ranked
-#pragma unroll 1
-            for (int cb = 0; cb < PB_TC_N / 32; ++cb) {
-                uint32_t rr[32];
-                tc_ld32(tmem_base + ((uint32_t)(32 * lg) << 16) + acc * 256 + half * PB_TC_N + cb * 32, rr);
-                if (BIAS) {  // warp-uniform addresses: one broadcast load per column
+            const uint32_t b0 = smem_u32(Bs + (size_t)st * B_BYTES);
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) rr[j] = __float_as_uint(__uint_as_float(rr[j]) + __ldg(bias + c0 + cb * 32 + j));
+            for (int p = 0; p < 2; ++p) {
+                const uint32_t a0 = smem_u32(As + half * A_BYTES) + p * 1024;  // 64 rows = 8 row groups of 128 B
+                wg_fence();
+#pragma unroll
+                for (int k = 0; k < KSTEPS; ++k)
+                    wg_mma_f16<PB_TC_N>(d, wg_desc(a0 + k * 2 * LBO, LBO, SBO), wg_desc(b0 + k * 2 * LBO, LBO, SBO), k > 0 ? 1u : 0u);
+                wg_commit();
+                wg_wait_all(d);
+                if (p == 1) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&empty[st]);  // B tile consumed
                 }
-                // one max tree per 32 columns; the insertion path runs only when the batch can matter
-                float m = __uint_as_float(rr[0]);
+                if (BIAS) {  // bias of column 8 i + 2 (lane%4) + j
 #pragma unroll
-                for (int j = 1; j < 32; ++j) m = fmaxf(m, __uint_as_float(rr[j]));
-                if (m > s3 || edge) {
+                    for (int i = 0; i < PB_TC_N / 8; ++i) {
+                        const float2 bb = __ldg(reinterpret_cast<const float2 *>(bias + c0 + 8 * i + 2 * (lane & 3)));
+                        d[4 * i] += bb.x;
+                        d[4 * i + 1] += bb.y;
+                        d[4 * i + 2] += bb.x;
+                        d[4 * i + 3] += bb.y;
+                    }
+                }
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const float v = __uint_as_float(rr[j]);
-                        const uint32_t c = (uint32_t)(c0 + cb * 32 + j);
-                        if (v > s3 && c < (uint32_t)K) {  // NaN never enters
-                            if (v > s0) { s3 = s2; i3 = i2; s2 = s1; i2 = i1; s1 = s0; i1 = i0; s0 = v; i0 = c; }
-                            else if (v > s1) { s3 = s2; i3 = i2; s2 = s1; i2 = i1; s1 = v; i1 = c; }
-                            else if (v > s2) { s3 = s2; i3 = i2; s2 = v; i2 = c; }
-                            else { s3 = v; i3 = c; }
-                        }
+                for (int h = 0; h < 2; ++h) {
+                    const int r = 2 * p + h;
+                    float s0 = s[r][0], s1 = s[r][1], s2 = s[r][2], s3 = s[r][3];
+                    uint32_t i0 = ix[r][0], i1 = ix[r][1], i2 = ix[r][2], i3 = ix[r][3];
+                    // one max tree per row; the insertion path runs only when the tile can matter
+                    float m = d[2 * h];
+#pragma unroll
+                    for (int i = 0; i < PB_TC_N / 8; ++i) m = fmaxf(m, fmaxf(d[4 * i + 2 * h], d[4 * i + 2 * h + 1]));
+                    if (m > s3 || edge) {
+#pragma unroll
+                        for (int i = 0; i < PB_TC_N / 8; ++i)
+#pragma unroll
+                            for (int j = 0; j < 2; ++j) {
+                                const float v = d[4 * i + 2 * h + j];
+                                const uint32_t c = (uint32_t)(c0 + 8 * i + 2 * (lane & 3) + j);
+                                if (v > s3 && c < (uint32_t)K) {  // NaN never enters
+                                    if (v > s0) { s3 = s2; i3 = i2; s2 = s1; i2 = i1; s1 = s0; i1 = i0; s0 = v; i0 = c; }
+                                    else if (v > s1) { s3 = s2; i3 = i2; s2 = s1; i2 = i1; s1 = v; i1 = c; }
+                                    else if (v > s2) { s3 = s2; i3 = i2; s2 = v; i2 = c; }
+                                    else { s3 = v; i3 = c; }
+                                }
+                            }
+                    }
+                    s[r][0] = s0; s[r][1] = s1; s[r][2] = s2; s[r][3] = s3;
+                    ix[r][0] = i0; ix[r][1] = i1; ix[r][2] = i2; ix[r][3] = i3;
+                }
+            }
+        }
+        // merge the quad's lists: order (score descending, index ascending), the order the scan above produces
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+#pragma unroll
+            for (int mask = 1; mask <= 2; mask <<= 1) {
+                float os[4];
+                uint32_t oi[4];
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    os[k] = __shfl_xor_sync(PB_FULL, s[r][k], mask);
+                    oi[k] = __shfl_xor_sync(PB_FULL, ix[r][k], mask);
+                }
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const float v = os[k];
+                    const uint32_t c = oi[k];
+                    auto before = [&](float a, uint32_t ia) { return v > a || (v == a && c < ia); };
+                    if (c == 0xffffffffu || !before(s[r][3], ix[r][3])) continue;  // empty slot, or not in the top 4
+                    if (before(s[r][0], ix[r][0])) {
+                        s[r][3] = s[r][2]; ix[r][3] = ix[r][2]; s[r][2] = s[r][1]; ix[r][2] = ix[r][1];
+                        s[r][1] = s[r][0]; ix[r][1] = ix[r][0]; s[r][0] = v; ix[r][0] = c;
+                    } else if (before(s[r][1], ix[r][1])) {
+                        s[r][3] = s[r][2]; ix[r][3] = ix[r][2]; s[r][2] = s[r][1]; ix[r][2] = ix[r][1]; s[r][1] = v; ix[r][1] = c;
+                    } else if (before(s[r][2], ix[r][2])) {
+                        s[r][3] = s[r][2]; ix[r][3] = ix[r][2]; s[r][2] = v; ix[r][2] = c;
+                    } else {
+                        s[r][3] = v; ix[r][3] = c;
                     }
                 }
             }
-            tc_fence_before();
-            mbar_arrive(&tempty[acc]);
+            const long long tok = x0 + half * PB_TC_M + 64 * (r >> 1) + 16 * (w & 3) + (lane >> 2) + 8 * (r & 1);
+            if ((lane & 3) == 0 && tok < n) {
+                reinterpret_cast<float4 *>(top_s)[tok] = make_float4(s[r][0], s[r][1], s[r][2], s[r][3]);
+                reinterpret_cast<uint4 *>(top_i)[tok] = make_uint4(ix[r][0], ix[r][1], ix[r][2], ix[r][3]);
+            }
         }
-        const long long tok = x0 + half * PB_TC_M + 32 * lg + lane;
-        if (tok < n) {
-            reinterpret_cast<float4 *>(top_s)[tok] = make_float4(s0, s1, s2, s3);
-            reinterpret_cast<uint4 *>(top_i)[tok] = make_uint4(i0, i1, i2, i3);
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (w == 9) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
     }
 }
 

@@ -1,12 +1,12 @@
-// k_filter_tc.cuh -- a7' tcgen05 fp16 certified filter in front of the exact stage.
+// k_filter_tc.cuh -- a7' tensor-core fp16 certified filter in front of the exact stage.
 // Part of kernels.cuh (included from there, in order; not a standalone header).
 // ==========================================================================================
-// tcgen05 certified filter in front of the exact stage (search path).
+// Tensor-core (wgmma) certified filter in front of the exact stage (search path).
 //
 // Only the top_k docs of the M kept ones need exact scores (search.rs:496-515).  k_exact_tc
 // estimates every kept doc's MaxSim on the tensor cores: tokens are decompressed approximately from an
-// fp16 copy of the centroids straight into the UMMA operand tile (canonical K-major layout, fp16),
-// the query is the N = 32 operand, sims land in TMEM, the epilogue takes per-doc column maxima.
+// fp16 copy of the centroids straight into the MMA operand tile (canonical K-major layout, fp16),
+// the query is the N = 32 operand, sims are staged to shared memory, the epilogue takes per-doc column maxima.
 // fp16 rather than bf16: every operand is a unit-scale vector, and 11 significand bits make the certified
 // band 8x narrower.  With D the exact decompressed token, D~ its estimate, u = 2^-11 the unit roundoff and
 // v = c + w the token before normalisation, v~ = h(h(c) + h(w)) what the tile holds (one fp16 add of fp16 operands),
@@ -19,9 +19,9 @@
 // estimates (fp16 overflow included) disable the filter for that query.
 // Operand tile: element (row r, 8-wide K chunk kc) at kc * LBO + (r/8) * 128 + (r%8) * 16 with
 // LBO = 2048 + 32, i.e. at kc * LBO + 16 r: the 32-byte skew makes the 16-byte cp.async scatter of a centroid
-// row bank-conflict free, and one thread decompresses one token (= its TMEM lane in the epilogue): the token is
+// row bank-conflict free, and one thread decompresses one token (= its accumulator row in the epilogue): the token is
 // stored unnormalised (h(v), same relative rounding as h(v/|v|)) and 1/|v| scales the 32 similarities instead.
-// grid = (CTAs per query, B), 128 threads, up to 4 CTAs/SM (~51 KB smem, 32 TMEM columns each).
+// grid = (CTAs per query, B), 128 threads = one warpgroup (~70 KB smem with NQT = 32, of which 18 KB staged similarities).
 // ==========================================================================================
 #define PB_XTC_LBO 2080u
 
@@ -95,8 +95,7 @@ k_exact_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, c
     // Th[byte] = the fp16 bucket weights of the 8/NBITS fields packed in that byte, first field first
     constexpr int VB = 8 / NBITS;
     __half *Th = reinterpret_cast<__half *>(Qb + QB_BYTES);  // [256][VB]
-    uint64_t *mbar = reinterpret_cast<uint64_t *>(Th + 256 * VB);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(mbar + 1);
+    float *Acc = reinterpret_cast<float *>(Th + 256 * VB);    // [128 tokens][ACC_LD(NQT)] similarities of the chunk
     const int b = blockIdx.y;
     const int nk = n_kept[b];
     const long long *tp = tok_prefix + (size_t)b * (Mcap + 1);
@@ -120,26 +119,11 @@ k_exact_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, c
         for (int e = 0; e < 8; ++e) v8[e] = __float2half_rn(r < nq ? Q[(size_t)(r0q + r) * DIM + kc * 8 + e] : 0.0f);
         *reinterpret_cast<uint4 *>(Qb + (kc * (NQT / 8) + (r >> 3)) * 128 + (r & 7) * 16) = *reinterpret_cast<uint4 *>(v8);
     }
-    if (threadIdx.x == 0) {
-        mbar_init(mbar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (w == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(NQT) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    // instruction descriptor: c = f32 [4,6) = 1, a = b = f16 (format 0), K-major, N>>3 [17,23), M>>4 [24,29)
-    const uint32_t idesc = (1u << 4) | ((uint32_t)(NQT >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    uint32_t phase = 0;
     const int hl = lane >> 4, kcl = lane & 15;  // staging: one lane per 8-wide K chunk, two centroid rows per instruction
-    const int row = threadIdx.x;                // decompression and epilogue: one thread per token (= TMEM lane)
+    const int row = threadIdx.x;                // decompression and epilogue: one thread per token (= accumulator row)
     TokMeta cur = locate_token<false>(c_lo * 128 + threadIdx.x, T, 0, nk, tp, kp, doc_off, codes);
     for (long long chunk = c_lo; chunk < c_hi; ++chunk) {
-        __syncthreads();  // previous chunk: TMEM read out, operand tile free
+        __syncthreads();  // previous chunk: similarities read out, operand tile free
         // ---- loads: each thread its own token's packed row, into registers (read once, from HBM); 16 lanes x 16 B =
         //      one fp16 centroid row, straight to its place in the operand tile ----
         uint32_t pw[NW];
@@ -233,21 +217,25 @@ k_exact_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, c
 #pragma unroll
             for (int kc = 0; kc < KC; ++kc) *reinterpret_cast<uint4 *>(As + kc * LBO_A + row * 16) = make_uint4(0, 0, 0, 0);
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        tc_fence_before();
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // the tiles are read by the async proxy
         __syncthreads();
-        if (threadIdx.x == 0) {
-            tc_fence_after();
+        {
+            // the CTA is one warpgroup: two M = 64 slabs of tokens (64 rows = 1024 bytes of the tile), staged to Acc
             const uint32_t a0 = smem_u32(As), b0 = smem_u32(Qb);
 #pragma unroll
-            for (int s = 0; s < KSTEPS; ++s)
-                tc_mma_bf16(tmem_base, tc_smem_desc(a0 + s * 2 * LBO_A, LBO_A, SBO), tc_smem_desc(b0 + s * 2 * LBO_B, LBO_B, SBO),
-                            idesc, s > 0 ? 1u : 0u);  // kind::f16 covers fp16 and bf16; idesc says which
-            tc_commit(mbar);
+            for (int p = 0; p < 2; ++p) {
+                float d[NQT / 2] = {};
+                wg_fence();
+#pragma unroll
+                for (int s = 0; s < KSTEPS; ++s)
+                    wg_mma_f16<NQT>(d, wg_desc(a0 + p * 1024 + s * 2 * LBO_A, LBO_A, SBO), wg_desc(b0 + s * 2 * LBO_B, LBO_B, SBO),
+                                    s > 0 ? 1u : 0u);
+                wg_commit();
+                wg_wait_all(d);
+                wg_stage<NQT>(Acc + p * 64 * ACC_LD(NQT), d);
+            }
         }
-        mbar_wait(mbar, phase);
-        phase ^= 1u;
-        tc_fence_after();
+        __syncthreads();
         // ---- epilogue: thread = token, 32 similarities per pass; per-doc maxima ----
         const int rank = cur.r;
         const unsigned grp = __match_any_sync(PB_FULL, rank);
@@ -255,7 +243,7 @@ k_exact_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, c
         for (int h = 0; h < NQT / 32; ++h) {
             if (32 * h >= nq) break;
             uint32_t rr[32];
-            tc_ld32(tmem_base + ((uint32_t)(32 * w) << 16) + 32 * h, rr);
+            acc_row(Acc + row * ACC_LD(NQT) + 32 * h, rr);
             // maxima are taken on the order-preserving int image of the float (x ^ ((x >> 31) & 0x7fffffff), its own
             // inverse); only the publishing lane converts to the score key.  +inf / +NaN win the max and map to key 0 =
             // "no estimate" (filter off for the query); -NaN loses, like every non-finite value in the exact path.
@@ -283,13 +271,7 @@ k_exact_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, c
                 }
             }
         }
-        tc_fence_before();
         cur = nxt;
-    }
-    __syncthreads();
-    if (w == 0) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(NQT) : "memory");
     }
 }
 
@@ -307,7 +289,7 @@ k_exact_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, c
 //     |1/|v| - inv|        <= 2^-20 / |v|
 // so |q.D - est| <= |q|max * eps_unit2 with eps_unit2 = ((E + 1.01) 2 cmax 1.0001 / 65535 + wmax (2u + u^2 + 2^-15)) / vmin
 // + 8e-6 (filter_eps_unit2 in engine.cu).  Flagged queries (no valid table) publish nothing -> no estimate -> every
-// kept doc survives.  Same grid / block / TMEM layout as k_exact_tc.
+// kept doc survives.  Same grid / block / accumulator layout as k_exact_tc.
 // ------------------------------------------------------------------------------------------
 // estimate[b][r] = sum over q of the per-token maxima (any order); resets maxkey.  one warp per kept doc.
 __global__ void __launch_bounds__(256)

@@ -1,21 +1,20 @@
-// k_maxsim_tc.cuh -- a7'/a8: the linear tcgen05 MaxSim estimate as a warp-specialised pipeline, and the exact
+// k_maxsim_tc.cuh -- a7'/a8: the linear tensor-core MaxSim estimate as a warp-specialised pipeline, and the exact
 // stage reduced to the (token, query token) pairs that can hold a per-token maximum.
 // Part of kernels.cuh (included from there, in order; not a standalone header).
 // ==========================================================================================
 // k_maxsim_tc estimates every similarity of a kept doc's tokens as sim~ = (q.w + s~(code)) / |v| (residual part on the
 // tensor cores, centroid score from the 16-bit table, stored norm; bound eps_q = |q|max * filter_eps_unit2 on every
-// similarity, DESIGN.md 4c), with the three phases of a 128-token chunk on different warps so that they overlap inside
-// one CTA (a one-loop form, every warp doing all three phases behind CTA barriers, measured the same 0.97 ms):
+// similarity, DESIGN.md 4c), with the producer and consumer phases of a 128-token chunk on different warpgroups so that
+// they overlap inside one CTA:
 //   warps 4-7  producers: locate the chunk's tokens, read the packed residuals, expand them to fp16 straight
 //              into a 2-stage operand ring (thread = token row);
-//   warp  8    one elected thread issues the KSTEPS tcgen05.mma of a chunk into one of 2 TMEM accumulators and
-//              commits to "stage free" and "accumulator full";
-//   warps 0-3  epilogue: tcgen05.ld (thread = token = TMEM lane), add the centroid score of the token's code
-//              (one 16-bit score-table row per token, fetched one chunk ahead), scale by 1/|v|, reduce per doc.
+//   warps 0-3  consumers: the KSTEPS wgmma of a chunk (two M = 64 slabs), staged to a shared fp32 tile; then the
+//              epilogue (thread = token = tile row): add the centroid score of the token's code (one 16-bit
+//              score-table row per token, fetched one chunk ahead), scale by 1/|v|, reduce per doc.
 // Token metadata travels from the producers to the epilogue through a 4-deep ring: the producer of chunk i writes
 // slot i % 4 after it finished the tile of chunk i-1, which it could only start once the MMA of chunk i-3 had
-// completed, which needed the epilogue of chunk i-5 to have drained its accumulator -- and that epilogue had read
-// the metadata of chunk i-4 before it began.
+// completed, which the consumers issue after the epilogue of chunk i-4 -- and they had read the metadata of chunk
+// i-4 before the epilogue of chunk i-5.
 //
 // EMIT = false (pass 1, every kept doc): per (doc, query token) maxima of the estimate -> maxkey.
 // EMIT = true  (pass 2, the filter's survivors): a doc's exact MaxSim needs, per query token, only the tokens whose
@@ -33,15 +32,16 @@ struct MsMeta {
 
 PB_DEV void ms_arrive(uint64_t *bar) { mbar_arrive(bar); }
 
-PB_DEV void tc_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// warp maximum of a float with NaN ignored (all NaN -> NaN), +0 above -0: one redux.sync on the order-preserving int
+// image of the float (x ^ ((x >> 31) & 0x7fffffff), its own inverse)
+PB_DEV float warp_max_f32(float x) {
+    const int i = __float_as_int(x);
+    const int m = __reduce_max_sync(PB_FULL, x == x ? i ^ ((i >> 31) & 0x7fffffff) : (int)0x80000000);
+    return __int_as_float(m ^ ((m >> 31) & 0x7fffffff));
 }
+
+// the consumer warpgroup's own barrier (the producers do not take part)
+PB_DEV void consumer_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 
 // gbase[b][r] = first token of kept doc r minus its offset in the query's kept-token stream: token s of the stream is
 // index token gbase[r] + s (one dependent load after the prefix search instead of kept -> doc_off)
@@ -82,7 +82,7 @@ PB_DEV TokMeta ms_locate(long long s, long long T, int r_lo, int nk, const long 
 }
 
 template <int DIM, int NBITS, int NQT, bool EMIT>
-__global__ void __launch_bounds__(288, 2)
+__global__ void __launch_bounds__(256, NQT == 32 ? 2 : 1)  // NQT = 64: ~129 KB of shared memory, one CTA per SM
 k_maxsim_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, const unsigned short *__restrict__ ST16,
             long long K, const float2 *__restrict__ qrange, const int *__restrict__ qflag, const float *__restrict__ w_rev,
             const uint32_t *__restrict__ codes, const uint8_t *__restrict__ residuals, const float *__restrict__ inv_norm,
@@ -108,8 +108,8 @@ k_maxsim_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, 
     __half *Th = reinterpret_cast<__half *>(Qb + QB_BYTES);       // [256][TR][VB]: fp16 bucket weights of the fields of a byte
     MsMeta *meta = reinterpret_cast<MsMeta *>(Th + 256 * VB * TR); // [4][128]
     uint64_t *bars = reinterpret_cast<uint64_t *>(meta + 4 * 128);
-    uint64_t *a_full = bars, *a_empty = bars + 2, *t_full = bars + 4, *t_empty = bars + 6, *m_full = bars + 8;  // 2,2,2,2,4
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 12);
+    uint64_t *a_full = bars, *a_empty = bars + 2, *m_full = bars + 4;  // 2,2,4
+    float *Acc = reinterpret_cast<float *>(bars + 8);                  // [128 tokens][ACC_LD(NQT)] similarities of the chunk
     const int b = blockIdx.y;
     const int nk = n_kept[b];
     const long long *tp = tok_prefix + (size_t)b * (Mcap + 1);
@@ -136,24 +136,15 @@ k_maxsim_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, 
     if (threadIdx.x == 0) {
         for (int s = 0; s < 2; ++s) {
             mbar_init(&a_full[s], 128);
-            mbar_init(&a_empty[s], 1);
-            mbar_init(&t_full[s], 1);
-            mbar_init(&t_empty[s], 128);
+            mbar_init(&a_empty[s], 4);  // one arrival per consumer warp
         }
         for (int s = 0; s < 4; ++s) mbar_init(&m_full[s], 128);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (w == 8) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(2 * NQT) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // Qb is read by the async proxy
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (w >= 4 && w < 8) {
+    if (w >= 4) {
         // ================= producers =================
         const int t = threadIdx.x - 128;
         auto load_packed = [&](const TokMeta &m, uint32_t (&pw)[NW]) __attribute__((always_inline)) {
@@ -239,31 +230,8 @@ k_maxsim_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, 
             step(i, mA, pA, mB, pB);
             if (i + 1 < n) step(i + 1, mB, pB, mA, pA);
         }
-    } else if (w == 8) {
-        // ================= MMA issuer =================
-        const uint32_t idesc = (1u << 4) | ((uint32_t)(NQT >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-        const uint32_t b0 = smem_u32(Qb);
-        for (int i = 0; i < n; ++i) {
-            const int s = i & 1;
-            const uint32_t ph = (uint32_t)(i >> 1) & 1u;
-            mbar_wait(&a_full[s], ph);
-            mbar_wait(&t_empty[s], ph ^ 1u);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t a0 = smem_u32(As + (size_t)s * A_BYTES);
-#pragma unroll
-                for (int k = 0; k < KSTEPS; ++k)
-                    tc_mma_bf16(tmem_base + s * NQT, tc_smem_desc(a0 + k * 2 * LBO_A, LBO_A, SBO),
-                                tc_smem_desc(b0 + k * 2 * LBO_B, LBO_B, SBO), idesc, k > 0 ? 1u : 0u);
-                tc_commit(&a_empty[s]);
-                tc_commit(&t_full[s]);
-            }
-            __syncwarp();
-        }
-        // both commits of the last chunks must have landed before the CTA's shared memory is released
-        for (int i = max(n - 2, 0); i < n; ++i) mbar_wait(&a_empty[i & 1], (uint32_t)(i >> 1) & 1u);
     } else {
-        // ================= epilogue =================
+        // ================= consumers: MMA + epilogue =================
         const int t = threadIdx.x;
         const float2 rg = qrange[b];
         const float inv_scale = 1.0f / rg.y, s_bias = (0.5f - rg.x) / rg.y;
@@ -318,19 +286,32 @@ k_maxsim_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, 
             load_side(nxt, swn, invn);
             load_thr(nxt, tkn);
             const int s = i & 1;
-            mbar_wait(&t_full[s], (uint32_t)(i >> 1) & 1u);
-            tc_fence_after();
+            mbar_wait(&a_full[s], (uint32_t)(i >> 1) & 1u);
+            consumer_sync();  // every thread has read the previous chunk's similarities
+            {
+                const uint32_t a0 = smem_u32(As + (size_t)s * A_BYTES), b0 = smem_u32(Qb);
+#pragma unroll
+                for (int p = 0; p < 2; ++p) {  // M = 64 slabs: tokens 64 p.. (64 rows = 1024 bytes of the tile)
+                    float d[NQT / 2] = {};
+                    wg_fence();
+#pragma unroll
+                    for (int k = 0; k < KSTEPS; ++k)
+                        wg_mma_f16<NQT>(d, wg_desc(a0 + p * 1024 + k * 2 * LBO_A, LBO_A, SBO), wg_desc(b0 + k * 2 * LBO_B, LBO_B, SBO),
+                                        k > 0 ? 1u : 0u);
+                    wg_commit();
+                    wg_wait_all(d);
+                    wg_stage<NQT>(Acc + p * 64 * ACC_LD(NQT), d);
+                }
+                __syncwarp();
+                if (lane == 0) ms_arrive(&a_empty[s]);  // operand stage free
+            }
+            consumer_sync();  // the chunk's similarities are staged
+            const float *arow = Acc + t * ACC_LD(NQT);
             const int rank = cur.r;
             const unsigned grp = __match_any_sync(PB_FULL, rank);
 #pragma unroll
             for (int h = 0; h < NQT / 32; ++h) {
-                if (32 * h >= nq) {  // (uniform) nothing to read in this half
-                    if (h == NQT / 32 - 1) {
-                        tc_fence_before();
-                        ms_arrive(&t_empty[s]);
-                    }
-                    continue;
-                }
+                if (32 * h >= nq) continue;  // (uniform) nothing to read in this half
                 if (!EMIT) {
                     // per-doc maxima, 16 query tokens at a time (16 accumulator registers live): one pass per doc
                     // present in the warp's 32 tokens (one, unless a doc boundary falls inside them).  Tokens outside
@@ -340,11 +321,7 @@ k_maxsim_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, 
 #pragma unroll
                     for (int hh = 0; hh < 2; ++hh) {
                         uint32_t r16[16];
-                        tc_ld16(tmem_base + ((uint32_t)(32 * w) << 16) + s * NQT + 32 * h + 16 * hh, r16);
-                        if (h == NQT / 32 - 1 && hh == 1) {  // the accumulator is in registers: hand it back to the MMA warp
-                            tc_fence_before();
-                            ms_arrive(&t_empty[s]);
-                        }
+                        acc_row(arow + 32 * h + 16 * hh, r16);
                         unsigned done = 0u;
                         while (valid & ~done) {
                             const int leader = __ffs(valid & ~done) - 1;
@@ -356,8 +333,7 @@ k_maxsim_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, 
                             for (int q = 0; q < 16; ++q) {
                                 const uint32_t f = __byte_perm(sw[16 * h + 8 * hh + (q >> 1)], 0x4B000000u, (q & 1) ? 0x7632 : 0x7610);
                                 const float sim = (__uint_as_float(r16[q]) + __fmaf_rn(__uint_as_float(f), inv_scale, bias_l)) * inv;
-                                float m;
-                                asm volatile("redux.sync.max.f32 %0, %1, %2;" : "=f"(m) : "f"(sim), "r"(PB_FULL));
+                                const float m = warp_max_f32(sim);
                                 if (lane == 16 * hh + q) mine = m;
                             }
                             const uint32_t key = score_key_asc(mine);
@@ -369,11 +345,7 @@ k_maxsim_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, 
                     continue;
                 }
                 uint32_t rr[32];
-                tc_ld32(tmem_base + ((uint32_t)(32 * w) << 16) + s * NQT + 32 * h, rr);
-                if (h == NQT / 32 - 1) {  // the accumulator is in registers: hand it back to the MMA warp
-                    tc_fence_before();
-                    ms_arrive(&t_empty[s]);
-                }
+                acc_row(arow + 32 * h, rr);
                 if (EMIT) {
                     // thresholds of the warp's doc: lane = query token (a warp that straddles docs reads per token)
                     const bool uni = grp == PB_FULL;
@@ -410,12 +382,6 @@ k_maxsim_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, 
             step(i, mA, sA, iA, kA, mB, sB, iB, kB);
             if (i + 1 < n) step(i + 1, mB, sB, iB, kB, mA, sA, iA, kA);
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (w == 8) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(2 * NQT) : "memory");
     }
 }
 

@@ -1,4 +1,4 @@
-// k_scores.cuh -- a2 centroid scores: tile_dots (scalar / FFMA2), tile loads, k_centroid_scores.
+// k_scores.cuh -- a2 centroid scores: tile_dots (scalar / paired rows), tile loads, k_centroid_scores.
 // Part of kernels.cuh (included from there, in order; not a standalone header).
 
 #define PB_TOK_TILE 128          // doc tokens (or centroids) per CTA tile
@@ -58,14 +58,15 @@ PB_DEV void load_rows_padded_async(float *__restrict__ dst, const float *__restr
     }
 }
 
-// tile_dots on packed fp32 pairs (sm_100 FFMA2: fma.rn.f32x2, two independent IEEE FMAs per lane and instruction,
-// one operand may be a scalar broadcast): same sequential-j FMA per dot, hence the same bits, at half the issue
-// slots.  Qi holds the 8 query rows as 4 row pairs interleaved element-wise, pair p at Qi + p*2*DIM:
-// (q_2p[0], q_2p+1[0], q_2p[1], q_2p+1[1], ...); acc[2p][k] / acc[2p+1][k] come out as the halves of one register pair.
+// tile_dots on fp32 pairs: two independent IEEE FMAs per pair with a broadcast scalar operand, the same
+// sequential-j FMA per dot, hence the same bits.  (sm_90 has no packed fp32 FMA; the pair is two FFMAs, and the
+// 8-byte operand loads of the interleaved rows stay.)  Qi holds the 8 query rows as 4 row pairs interleaved
+// element-wise, pair p at Qi + p*2*DIM: (q_2p[0], q_2p+1[0], q_2p[1], q_2p+1[1], ...); acc[2p][k] / acc[2p+1][k] come
+// out as the halves of one register pair.
 PB_DEV u64 fma2_bcast(u64 a_pair, float b, u64 c_pair) {
-    u64 d;
-    asm("{\n .reg .b64 t;\n mov.b64 t, {%2, %2};\n fma.rn.f32x2 %0, %1, t, %3;\n}\n" : "=l"(d) : "l"(a_pair), "f"(b), "l"(c_pair));
-    return d;
+    const float lo = __fmaf_rn(__uint_as_float((uint32_t)a_pair), b, __uint_as_float((uint32_t)c_pair));
+    const float hi = __fmaf_rn(__uint_as_float((uint32_t)(a_pair >> 32)), b, __uint_as_float((uint32_t)(c_pair >> 32)));
+    return ((u64)__float_as_uint(hi) << 32) | __float_as_uint(lo);
 }
 template <int DIM>
 PB_DEV void tile_dots_f2(const float *__restrict__ Qi, const float *__restrict__ Vs, float (&acc)[8][4]) {
@@ -142,7 +143,7 @@ PB_DEV void load_rows_padded(float *__restrict__ dst, const float *__restrict__ 
 // ------------------------------------------------------------------------------------------
 // a2: centroid scores.  grid = (ceil(K/128), query groups); 128 threads.
 // ------------------------------------------------------------------------------------------
-// F2: the query tiles come from the interleaved copy (k_interleave_query_rows) and the dots run on FFMA2.
+// F2: the query tiles come from the interleaved copy (k_interleave_query_rows) and the dots run on row pairs (tile_dots_f2).
 template <int DIM, bool F2>
 __global__ void __launch_bounds__(128, 2)
 k_centroid_scores(const float *__restrict__ Q, const int *__restrict__ q_off, int B, int QS,

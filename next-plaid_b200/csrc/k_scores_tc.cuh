@@ -2,8 +2,8 @@
 // Part of kernels.cuh (included from there, in order; not a standalone header).
 // ==========================================================================================
 // a2 = the one dense contraction of the path (search.rs:345 / :171-174): S = Q C^T for every query token of the
-// sub-batch against all K centroids.  k_scores16_tc computes it as a 3-product split-fp16 UMMA GEMM
-//     x = xh + xl  (xh = fp16(x), xl = fp16(x - xh));   S~ = qh.ch + qh.cl + ql.ch   (fp32 accumulator in TMEM)
+// sub-batch against all K centroids.  k_scores16_tc computes it as a 3-product split-fp16 wgmma GEMM
+//     x = xh + xl  (xh = fp16(x), xl = fp16(x - xh));   S~ = qh.ch + qh.cl + ql.ch   (fp32 accumulator in registers)
 // and writes ONLY the 16-bit fixed-point score table ST16[b][c][QS] the probe (a3) and the first approximate pass
 // (a5) stream / gather.  Nothing downstream needs a dense fp32 S: the few values that decide something
 //   - the exact selection keys of the probe winners            (k_collect16_tc)
@@ -23,11 +23,11 @@
 // E = 1.  Consumers use: code margin 2E + 1 = 3 for "could still be the maximum / in the top n", and the band
 // W = nq (1.004 + 2 err) + nq^2 / 256 + 4 for the first approximate pass (derivations at each kernel).
 // PB_K1_TC_DIAG=1 measures the largest code difference against the exact table (pb_work_counters).
-// grid = ceil(K/128) CTAs, 320 threads: warps 0-7 epilogue (warp w: TMEM lanes 32*(w%4).., column half w/4), warp 8
-// bulk-copy loader, warp 9 MMA issuer.
+// grid = ceil(K/128) CTAs, 288 threads: warps 0-7 two warpgroups that issue the MMAs of one 64-centroid half of the
+// tile each and convert their accumulators, warp 8 bulk-copy loader.
 // ==========================================================================================
 
-// fp16 hi/lo split of `n` rows, scaled by 2^kexp, into UMMA tile order (128-row tiles, K-major core matrices);
+// fp16 hi/lo split of `n` rows, scaled by 2^kexp, into MMA tile order (128-row tiles, K-major core matrices);
 // rows >= n stay zero
 __global__ void k_rows_to_f16_split_tiles(const float *__restrict__ X, long long n, int dim, int kexp,
                                           __half *__restrict__ Xh, __half *__restrict__ Xl) {
@@ -83,7 +83,7 @@ __global__ void k_query_range_tc(const float2 *__restrict__ qrange, const int *_
 }
 
 template <int DIM>
-__global__ void __launch_bounds__(320, 1)
+__global__ void __launch_bounds__(288, 1)
 k_scores16_tc(const __half *__restrict__ Ch, const __half *__restrict__ Cl, long long K, const __half *__restrict__ Qh,
               const __half *__restrict__ Ql, int n_groups, int B, int QS, const int *__restrict__ q_off,
               const float2 *__restrict__ qrange_tc, unsigned short *__restrict__ ST16, int *__restrict__ qflag) {
@@ -94,28 +94,18 @@ k_scores16_tc(const __half *__restrict__ Ch, const __half *__restrict__ Cl, long
     unsigned char *Ah = smem_k1, *Al = Ah + T_BYTES;  // this CTA's centroid tile, hi and lo
     unsigned char *Bs = Al + T_BYTES;                 // 2 stages x (hi, lo) query-row tiles
     uint64_t *bars = reinterpret_cast<uint64_t *>(Bs + 4 * T_BYTES);
-    uint64_t *full = bars, *empty = bars + 2, *tfull = bars + 4, *tempty = bars + 6, *abar = bars + 8;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 9);
+    uint64_t *full = bars, *empty = bars + 2, *abar = bars + 4;
     const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long c0 = (long long)blockIdx.x * 128;
     if (threadIdx.x == 0) {
         for (int i = 0; i < 2; ++i) {
             mbar_init(&full[i], 1);
-            mbar_init(&empty[i], 1);
-            mbar_init(&tfull[i], 1);
-            mbar_init(&tempty[i], 256);
+            mbar_init(&empty[i], 8);  // one arrival per consumer warp
         }
         mbar_init(abar, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (w == 9) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 256;" ::"r"(smem_u32(tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     if (w == 8) {
         // ---------------- loader ----------------
         if (lane == 0) {
@@ -130,77 +120,55 @@ k_scores16_tc(const __half *__restrict__ Ch, const __half *__restrict__ Cl, long
                 bulk_g2s(Bs + (size_t)(2 * st + 1) * T_BYTES, reinterpret_cast<const unsigned char *>(Ql) + (size_t)g * T_BYTES, T_BYTES, &full[st]);
             }
         }
-    } else if (w == 9) {
-        // ---------------- MMA issuer: 3 products per k-step into one fp32 accumulator ----------------
-        // instruction descriptor: c = f32, a = b = f16 (format 0), K-major, N = 128, M = 128
-        const uint32_t idesc = (1u << 4) | ((uint32_t)(128 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
+    } else {
+        // ---------------- consumers: warpgroup h = centroid rows 64 h.. of the tile (M = 64) x all 128 query rows of a
+        // group (N = 128), 3 products per k-step into one fp32 accumulator; then the codes straight from the registers:
+        // d[4 i + 2 r + j] = (centroid row 16 (w%4) + lane/4 + 8 r, query row 8 i + 2 (lane%4) + j) ----------------
+        const int h = w >> 2;
+        const int cq = 2 * (lane & 3);
+        const long long c_r0 = c0 + 64 * h + 16 * (w & 3) + (lane >> 2);
+        float d[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) d[i] = 0.0f;
         mbar_wait(abar, 0);
         for (int g = 0; g < n_groups; ++g) {
-            const int st = g & 1, acc = g & 1;
+            const int st = g & 1;
             mbar_wait(&full[st], (uint32_t)((g >> 1) & 1));
-            mbar_wait(&tempty[acc], (uint32_t)(((g >> 1) & 1) ^ 1));
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t ah = smem_u32(Ah), al = smem_u32(Al);
-                const uint32_t bh = smem_u32(Bs + (size_t)(2 * st) * T_BYTES), bl = smem_u32(Bs + (size_t)(2 * st + 1) * T_BYTES);
+            const uint32_t ah = smem_u32(Ah) + h * 1024, al = smem_u32(Al) + h * 1024;  // 64 rows = 8 row groups
+            const uint32_t bh = smem_u32(Bs + (size_t)(2 * st) * T_BYTES), bl = smem_u32(Bs + (size_t)(2 * st + 1) * T_BYTES);
+            wg_fence();
 #pragma unroll
-                for (int s = 0; s < KSTEPS; ++s) {
-                    const u64 dah = tc_smem_desc(ah + s * 2 * LBO, LBO, SBO), dal = tc_smem_desc(al + s * 2 * LBO, LBO, SBO);
-                    const u64 dbh = tc_smem_desc(bh + s * 2 * LBO, LBO, SBO), dbl = tc_smem_desc(bl + s * 2 * LBO, LBO, SBO);
-                    tc_mma_bf16(tmem_base + acc * 128, dah, dbh, idesc, s > 0 ? 1u : 0u);
-                    tc_mma_bf16(tmem_base + acc * 128, dah, dbl, idesc, 1u);
-                    tc_mma_bf16(tmem_base + acc * 128, dal, dbh, idesc, 1u);
-                }
-                tc_commit(&empty[st]);   // query tiles consumed
-                tc_commit(&tfull[acc]);  // accumulators ready
+            for (int s = 0; s < KSTEPS; ++s) {
+                const u64 dah = wg_desc(ah + s * 2 * LBO, LBO, SBO), dal = wg_desc(al + s * 2 * LBO, LBO, SBO);
+                const u64 dbh = wg_desc(bh + s * 2 * LBO, LBO, SBO), dbl = wg_desc(bl + s * 2 * LBO, LBO, SBO);
+                wg_mma_f16<128>(d, dah, dbh, s > 0 ? 1u : 0u);
+                wg_mma_f16<128>(d, dah, dbl, 1u);
+                wg_mma_f16<128>(d, dal, dbh, 1u);
             }
+            wg_commit();
+            wg_wait_all(d);
             __syncwarp();
-        }
-    } else {
-        // ---------------- epilogue: thread = centroid row (TMEM lane), 64 of the 128 padded query rows ----------------
-        const int lg = w & 3, ch = w >> 2;
-        const long long c = c0 + 32 * lg + lane;
-        for (int g = 0; g < n_groups; ++g) {
-            const int acc = g & 1;
-            mbar_wait(&tfull[acc], (uint32_t)((g >> 1) & 1));
-            tc_fence_after();
-            // (Both 32-column loads in flight and the accumulator handed back before the conversion and the stores was
-            // measured: 0.349 against 0.351 ms -- the TMEM read latency is not what bounds the epilogue.)
-#pragma unroll 1
-            for (int cb = 2 * ch; cb < 2 * ch + 2; ++cb) {
-                uint32_t rr[32];
-                tc_ld32(tmem_base + ((uint32_t)(32 * lg) << 16) + acc * 128 + cb * 32, rr);
+            if (lane == 0) mbar_arrive(&empty[st]);  // query tiles consumed
 #pragma unroll
-                for (int sub = 0; sub < 4; ++sub) {
-                    const int row0 = g * 128 + cb * 32 + sub * 8;  // 8 query rows of one query (QS % 8 == 0)
-                    const int b = row0 / QS, q = row0 - b * QS;
-                    if (b >= B || c >= K) continue;
-                    const float2 rg = qrange_tc[b];  // (R*scale, scale / 2^(kq+kc))
-                    uint32_t cd[8];
-                    bool ok = true;
+            for (int i = 0; i < 16; ++i) {
+                const int row0 = g * 128 + 8 * i;  // 8 query rows of one query (QS % 8 == 0)
+                const int b = row0 / QS, q = row0 - b * QS + cq;
+                if (b >= B) continue;
+                const float2 rg = qrange_tc[b];  // (R*scale, scale / 2^(kq+kc))
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        // code = floor(x) clamped to [0, 65535]; x outside [+0, 65536) (NaN, -0 included) raises the
-                        // query's flag and the sub-batch is redone on the exact path, so only in-range codes matter.
-                        // Padding rows hold a zero accumulator: x = R*scale, in range.
-                        const float x = __fmaf_rn(__uint_as_float(rr[sub * 8 + i]), rg.y, rg.x);
-                        ok &= __float_as_uint(x) < 0x47800000u;
-                        cd[i] = min(__float2uint_rd(x), 65535u);
-                    }
-                    if (!ok) atomicOr(&qflag[b], 1);
-                    *reinterpret_cast<uint4 *>(ST16 + ((size_t)b * K + c) * QS + q) =
-                        make_uint4(cd[0] | (cd[1] << 16), cd[2] | (cd[3] << 16), cd[4] | (cd[5] << 16), cd[6] | (cd[7] << 16));
+                for (int r = 0; r < 2; ++r) {
+                    const long long c = c_r0 + 8 * r;
+                    if (c >= K) continue;
+                    // code = floor(x) clamped to [0, 65535]; x outside [+0, 65536) (NaN, -0 included) raises the
+                    // query's flag and the sub-batch is redone on the exact path, so only in-range codes matter.
+                    // Padding rows hold a zero accumulator: x = R*scale, in range.
+                    const float x0 = __fmaf_rn(d[4 * i + 2 * r], rg.y, rg.x), x1 = __fmaf_rn(d[4 * i + 2 * r + 1], rg.y, rg.x);
+                    if (!(__float_as_uint(x0) < 0x47800000u && __float_as_uint(x1) < 0x47800000u)) atomicOr(&qflag[b], 1);
+                    *reinterpret_cast<uint32_t *>(ST16 + ((size_t)b * K + c) * QS + q) =
+                        min(__float2uint_rd(x0), 65535u) | (min(__float2uint_rd(x1), 65535u) << 16);
                 }
             }
-            tc_fence_before();
-            mbar_arrive(&tempty[acc]);
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (w == 9) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 256;" ::"r"(tmem_base) : "memory");
     }
 }
 
@@ -221,7 +189,7 @@ __global__ void k_diff16(const unsigned short *__restrict__ a, const unsigned sh
 
 // ------------------------------------------------------------------------------------------
 // Exact pinned-order score rows for a LIST of centroids per query: OUT[b][i][QS] = S[q][list[b][i]].
-// Same FFMA2 tile as k_centroid_scores<., true>; the centroid rows are gathered with cp.async.
+// Same paired-row FMA tile as k_centroid_scores<., true>; the centroid rows are gathered with cp.async.
 // grid = (ceil(cap/128), B), 128 threads.
 // ------------------------------------------------------------------------------------------
 template <int DIM>

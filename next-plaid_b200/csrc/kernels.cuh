@@ -1,7 +1,7 @@
-// kernels.cuh -- the sm_100a kernels of the PLAID search path, one per row of SURVEY.md 8(a).
+// kernels.cuh -- the sm_90a kernels of the PLAID search path, one per row of SURVEY.md 8(a).
 //
-//   k_scores16_tc ....... a2  S~ = Q*C^T as a 3-product split-fp16 tcgen05 GEMM -> 16-bit score table (default)
-//   k_centroid_scores ... a2  S = Q*C^T (fp32, packed FFMA2): the device-gated exact path   search.rs:345 / :174 / :268
+//   k_scores16_tc ....... a2  S~ = Q*C^T as a 3-product split-fp16 wgmma GEMM -> 16-bit score table (default)
+//   k_centroid_scores ... a2  S = Q*C^T (fp32 FMA, paired query rows): the device-gated exact path   search.rs:345 / :174 / :268
 //   k_chunkmax16/k_tau16/k_collect16(_tc)  a3  per-token top-n_ivf_probe, threshold first on the 16-bit table
 //   k_topn_partial/merge  a3  the same by per-lane lists (fallback), rank   search.rs:388-414 / :177-225
 //   k_cells(_unique/_thr/_emit)  a3  union + centroid_score_threshold      search.rs:417-425 / :226-251
@@ -10,7 +10,7 @@
 //   k_recheck_pairs/dots/sum (tensor-core table) | k_approx (exact table)  a5  exact re-check of the docs in the band
 //                                                                          search.rs:305-324 / :275-302
 //   k_cut ............... a6  stable top-(n_full_scores -> /4) cut        search.rs:460-469
-//   k_maxsim_tc/k_tc_finalize/k_tc_select  a7' tcgen05 certified estimate: which kept docs can reach the top_k (pass 1),
+//   k_maxsim_tc/k_tc_finalize/k_tc_select  a7' wgmma certified estimate: which kept docs can reach the top_k (pass 1),
 //                             which (token, query token) pairs of them can hold a maximum (pass 2); k_exact_tc = the
 //                             decompressing form for the table-less mode
 //   k_pair_exact ........ a7+a8 decompress + pinned fp32 dot of the listed pairs   codec.rs:423-470, maxsim.rs:270-294
@@ -18,7 +18,7 @@
 //   k_exact_finalize .... a8  q-ordered sum of per-token maxima           maxsim.rs:284-291
 //   k_topk .............. a9  stable final sort, take top_k               search.rs:496-515
 //   k_merge_cut/k_merge_topk  doc-sharded search: global cut and global top-k from the all-gathered keys
-//   k_assign_tc/k_assign_certify/k_assign/k_quantize_pack  a12  index build: nearest centroid (tcgen05 fp16
+//   k_assign_tc/k_assign_certify/k_assign/k_quantize_pack  a12  index build: nearest centroid (wgmma fp16
 //                             certified filter + exact fp32), residual quantise + pack   codec.rs:297-411
 //
 // Layouts: S is stored transposed per query, ST[b][c][QS] (one 4*QS-byte row per centroid, QS =

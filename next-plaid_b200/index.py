@@ -5,8 +5,8 @@ Names, argument meaning and error behaviour follow next-plaid/src (paths relativ
   SearchParameters, QueryResult ........................ search.rs:27-80
   Error kinds .......................................... error.rs:10-66
 
-This module is a thin ctypes binding: all work happens in hand-written sm_100a kernels behind
-include/plaid_b200.h.  There is no CPU path: if the shared library or a B200 is missing every call
+This module is a thin ctypes binding: all work happens in hand-written sm_90a kernels behind
+include/plaid_b200.h.  There is no CPU path: if the shared library or an H100 is missing every call
 raises.
 """
 from __future__ import annotations
@@ -455,7 +455,7 @@ class MmapIndex:
         load_library().pb_set_scores_tc(self._h, 1 if on else 0)
 
     def set_fast_exact(self, on: bool):
-        """tcgen05 certified filter in front of the exact stage (default on); same results either way."""
+        """wgmma certified filter in front of the exact stage (default on); same results either way."""
         load_library().pb_set_fast_exact(self._h, 1 if on else 0)
 
     def set_profiling(self, on: bool):

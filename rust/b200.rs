@@ -1,7 +1,7 @@
 //! next-plaid/src/b200.rs -- binding of libplaid_b200 (include/plaid_b200.h) for the `b200` cargo
 //! feature.  NOT COMPILED IN THIS REPOSITORY'S CI: the build image has no cargo/rustc.  It is the
 //! shim a next-plaid maintainer adds so that `MmapIndex::{load, search, search_batch}` keep their
-//! signatures (index.rs:1026, :1258, :1279) while the work runs on a B200; `colgrep` and
+//! signatures (index.rs:1026, :1258, :1279) while the work runs on an H100; `colgrep` and
 //! `next-plaid-api` link unchanged because they only see `MmapIndex`.
 #![cfg(feature = "b200")]
 

@@ -1,4 +1,4 @@
-"""CPU-side checks of the drop-in boundary: the library builds for sm_100a, loads, exports every
+"""CPU-side checks of the drop-in boundary: the library builds for sm_90a, loads, exports every
 symbol include/plaid_b200.h declares, and fails loudly (no fallback) without a device."""
 import os
 import re
@@ -26,11 +26,11 @@ def test_header_symbols_all_exported(npb):
     assert declared == set(npb.EXPORTS), declared ^ set(npb.EXPORTS)
 
 
-def test_library_targets_sm100a_only(npb):
+def test_library_targets_sm90a_only(npb):
     import subprocess
     out = subprocess.run(["cuobjdump", "-lelf", npb.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
-    assert not re.search(r"sm_(?!100a)\d+", out), out
+    assert "sm_90a" in out
+    assert not re.search(r"sm_(?!90a)\d+", out), out
 
 
 def test_default_params_match_reference(npb):

@@ -12,7 +12,7 @@ def npb():
     import next_plaid_b200 as m
     m.build_library()
     if m.device_count() < 1:
-        pytest.fail("GPU tests need a B200; the library has no CPU fallback")
+        pytest.fail("GPU tests need an H100; the library has no CPU fallback")
     return m
 
 
@@ -52,7 +52,7 @@ def test_encode_chunk_bit_exact(oracle, npb, dim, nbits, K):
     assert st["tokens"] == 1500
     assert st["tensor_cores"] == (dim in (64, 96, 128) and K >= 256)
     if st["tensor_cores"]:
-        assert st["exact_fallback"] < 150, st     # the certified tcgen05 shortlist decides >90 % of the tokens
+        assert st["exact_fallback"] < 150, st     # the certified tensor-core shortlist decides >90 % of the tokens
     assert codes.tolist() == want_codes.tolist()
     assert codes[7] == max(3, K // 2)
     assert np.array_equal(packed, want_packed)
@@ -114,7 +114,7 @@ def test_gpu_built_index_serves_searches(oracle, npb):
 
 def test_tensor_core_filter_is_exact_on_hard_inputs(oracle, npb):
     # near ties inside the fp16 error band, duplicated centroids, non-unit norms and a NaN token:
-    # whatever the tcgen05 shortlist cannot certify must fall back to the exact kernel
+    # whatever the tensor-core shortlist cannot certify must fall back to the exact kernel
     rng = np.random.default_rng(7)
     K, dim = 2048, 128
     cent = rng.standard_normal((K, dim)).astype(np.float32)
@@ -237,7 +237,7 @@ def test_data_parallel_kmeans_over_an_in_process_group(oracle, npb):
 
 
 def test_kmeans_on_the_tensor_cores_matches_the_fp32_assignment_statistically(oracle, npb, monkeypatch):
-    # dims 64/96/128 with K >= 256: the Lloyd assignment step runs as the fp16 tcgen05 GEMM with the -|c|^2/2 bias in
+    # dims 64/96/128 with K >= 256: the Lloyd assignment step runs as the fp16 wgmma GEMM with the -|c|^2/2 bias in
     # its epilogue (k_assign_tc<., true>); PB_KMEANS_EXACT=1 keeps the fp32 kernel.  Same seed -> same start; bf16
     # rounding may move points that sit between two centroids, the clustering quality must not change.
     docs = oracle.synthetic_corpus(1500, 32, dim=128, seed=8)

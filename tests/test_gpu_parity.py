@@ -13,7 +13,7 @@ def npb():
     import next_plaid_b200 as m
     m.build_library()
     if m.device_count() < 1:
-        pytest.fail("GPU tests need a B200; the library has no CPU fallback")
+        pytest.fail("GPU tests need an H100; the library has no CPU fallback")
     return m
 
 
@@ -331,7 +331,7 @@ def test_randomized_search_parity(oracle, npb):
 
 
 def test_tensor_core_filter_equals_full_exact_stage(oracle, npb, corpus):
-    # DESIGN.md "a7' certified filter": the fp16 tcgen05 estimate may only drop docs that provably cannot reach
+    # DESIGN.md "a7' certified filter": the fp16 tensor-core estimate may only drop docs that provably cannot reach
     # the top_k, so results with the filter on / off / the oracle's are the same bits
     docs, ix, qs, src, gpu = corpus
     for kw in (dict(top_k=5, n_full_scores=2048), dict(top_k=100, n_full_scores=4096, centroid_score_threshold=None),

@@ -13,7 +13,7 @@ def npb():
     import next_plaid_b200 as m
     m.build_library()
     if m.device_count() < 1:
-        pytest.fail("GPU tests need a B200; the library has no CPU fallback")
+        pytest.fail("GPU tests need an H100; the library has no CPU fallback")
     return m
 
 

@@ -6,8 +6,7 @@ vectors, each rank on its own shard.
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port 29544 \
         tools/bench_build.py --tokens 33554432 --kmeans-points 8388608                               # NCCL, 8 ranks
 
---tokens / --kmeans-points are whole-job totals, split evenly over the ranks.  Rank 0 prints one JSON line; run one rank
-under ncu for the kernel-level numbers (profiles/)."""
+--tokens / --kmeans-points are whole-job totals, split evenly over the ranks.  Rank 0 prints one JSON line."""
 import argparse
 import json
 import os
