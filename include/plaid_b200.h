@@ -124,6 +124,35 @@ PB_API int32_t pb_index_embedding_dim(const pb_index *ix);
 PB_API int32_t pb_index_nbits(const pb_index *ix);
 PB_API int32_t pb_index_device(const pb_index *ix);
 
+/* ---- incremental append ------------------------------------------------------------------ */
+
+typedef struct pb_codec pb_codec;
+
+/* MmapIndex::update_append (index.rs:1675) + reload (index.rs:1767) on a live handle.  Encodes with `codec`
+ * (same K, dim, nbits and bit-identical centroids as the index; bucket cutoffs required, codec.rs:359-362),
+ * appends the documents as ids doc_id_base + D .. + n_docs - 1, and leaves the handle exactly as
+ * pb_index_open on the concatenated arrays would.  index_dir != NULL also applies update_index's file changes
+ * (update.rs:794-1117, update_threshold = false) with chunks of batch_size docs.  Searches from other
+ * threads wait for the append; on any error neither the handle nor the directory changes.
+ *   embeddings   [sum doc_lengths][dim] f32, doc_lengths [n_docs], both in memory_space (PB_MEM_HOST | PB_MEM_DEVICE)
+ *   out_first_doc_id  may be NULL; receives doc_id_base + the old D
+ * PB_ERR_UNSUPPORTED, nothing changed: doc-sharded handles (pb_index_comm_init, pb_index_group_join), handles opened
+ * with PB_OPEN_ADOPT_RESIDUALS, index_dir with doc_id_base != 0, and totals past the limits of pb_index_open.
+ * PB_ERR_INVALID: a codec that does not match the index, a code >= K, or a directory whose metadata.json
+ * num_documents differs from the handle's.  An append of 0 documents changes nothing, on the device or on disk. */
+PB_API pb_status pb_index_append(pb_index *ix, pb_codec *codec, const float *embeddings, const int64_t *doc_lengths,
+                                 int64_t n_docs, int32_t memory_space, const char *index_dir, int64_t batch_size,
+                                 int64_t *out_first_doc_id);
+/* The same with documents already encoded (codes <i8 [n], packed residuals u1 [n][dim*nbits/8]): for callers whose
+ * codes come from elsewhere.  Device-side only (no index_dir). */
+PB_API pb_status pb_index_append_encoded(pb_index *ix, const int64_t *codes, const uint8_t *residuals,
+                                         const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
+                                         int64_t *out_first_doc_id);
+/* Pre-size the per-token and per-doc arrays so that appends up to these totals neither reallocate nor copy.
+ * Without it an append that outgrows an array reallocates it at 1.5x and copies it once, which needs the old and the
+ * new array at the same time (PB_ERR_NOMEM, nothing changed, when the device cannot hold both). */
+PB_API pb_status pb_index_reserve(pb_index *ix, int64_t num_documents, int64_t num_embeddings);
+
 /* ---- search ------------------------------------------------------------------------------ */
 
 /*
@@ -296,8 +325,8 @@ PB_API pb_status pb_search_batch_device(pb_index *ix, const float *d_queries,
  * centroids / cutoffs on the device (ResidualCodec, codec.rs:107-123) and every call is bit-identical
  * to the CPU implementation (compress_into_codes_cpu, quantize_residuals), including its last-maximum
  * tie rule -- the reference's own CUDA kernel picks the FIRST maximum (cuda.rs:202).
- * k-means: fastkmeans-rs is not in the reference tree, so pb_kmeans_fit is parity-unpinned. */
-typedef struct pb_codec pb_codec;
+ * k-means: fastkmeans-rs is not in the reference tree, so pb_kmeans_fit is parity-unpinned.  (pb_codec is declared
+ * above, with pb_index_append.) */
 typedef struct pb_shard_group pb_shard_group;   /* in-process rank group, see "doc-sharded deployment" below */
 PB_API pb_status pb_codec_open(int32_t device, const float *centroids, int64_t num_centroids, int32_t dim,
                                int32_t nbits, const float *bucket_cutoffs /* may be NULL */, pb_codec **out);

@@ -16,10 +16,13 @@
 // and the held-out sample is bit-identical to the oracle (tests/test_gpu_create_index.py).
 #include "engine_internal.h"
 
+#include <fcntl.h>
 #include <sys/stat.h>
+#include <unistd.h>
 
 #include <algorithm>
 #include <cmath>
+#include <cerrno>
 #include <cstdio>
 #include <cstring>
 #include <numeric>
@@ -75,6 +78,20 @@ pb_status write_text(const std::string &path, const std::string &txt) {
     bool ok = fwrite(txt.data(), 1, txt.size(), f) == txt.size();
     ok = (fclose(f) == 0) && ok;
     return ok ? PB_OK : pb_fail(PB_ERR_IO, "short write to %s", path.c_str());
+}
+
+// atomic_write_file (utils.rs:16-60): written and synced under a temporary name, then renamed over `path`
+template <class Write> pb_status atomic_write(const std::string &path, Write write) {
+    const std::string tmp = path + ".tmp";
+    pb_status s = write(tmp);
+    if (!s) {
+        const int fd = open(tmp.c_str(), O_RDONLY);
+        if (fd < 0 || fsync(fd) != 0) s = pb_fail(PB_ERR_IO, "cannot sync %s", tmp.c_str());
+        if (fd >= 0) close(fd);
+    }
+    if (!s && rename(tmp.c_str(), path.c_str()) != 0) s = pb_fail(PB_ERR_IO, "cannot rename %s to %s", tmp.c_str(), path.c_str());
+    if (s) remove(tmp.c_str());
+    return s;
 }
 
 struct CodecGuard {
@@ -239,4 +256,110 @@ extern "C" pb_status pb_create_index(const float *embeddings, const int64_t *doc
     if (st || !out_index) pb_index_close(ix);
     else *out_index = ix;
     return st;
+}
+
+pb_status pb_dir_append(const char *index_dir, long long old_D, long long K, int dim, int nbits, long long batch_size,
+                        const int64_t *codes, const uint8_t *residuals, const int64_t *doc_lengths, long long n_docs,
+                        const int64_t *ivf, long long ivf_total, const int32_t *ivf_lengths) {
+    const std::string dir = std::string(index_dir) + "/";
+    const long long packed = (long long)dim * nbits / 8;
+    // Metadata::load_from_path (index.rs:131-155): num_documents 0 or absent is inferred from the doclens files
+    std::string meta;
+    if (pb_status s = pb_read_text(dir + "metadata.json", meta)) return s;
+    double num_chunks = 0, mnbits = 0, num_emb = 0, avg_doclen = 0, num_docs = 0;
+    if (!pb_json_number(meta, "num_chunks", num_chunks) || !pb_json_number(meta, "nbits", mnbits) ||
+        !pb_json_number(meta, "num_embeddings", num_emb) || !pb_json_number(meta, "avg_doclen", avg_doclen))
+        return pb_fail(PB_ERR_IO, "metadata.json lacks num_chunks / nbits / num_embeddings / avg_doclen");
+    const long long n_chunks_old = (long long)num_chunks, old_N = (long long)num_emb;
+    pb_json_number(meta, "num_documents", num_docs);
+    long long meta_D = (long long)num_docs;
+    if (meta_D == 0) {
+        std::vector<int64_t> all;
+        for (long long c = 0; c < n_chunks_old; ++c) pb_read_doclens(dir + "doclens." + std::to_string(c) + ".json", all);
+        meta_D = (long long)all.size();
+    }
+    if ((int)mnbits != nbits) return pb_fail(PB_ERR_INVALID, "metadata.json nbits %d, the index has %d", (int)mnbits, nbits);
+    if (meta_D != old_D)
+        return pb_fail(PB_ERR_INVALID, "metadata.json num_documents %lld, the handle holds %lld documents", meta_D, old_D);
+
+    // a last chunk with < 2000 docs takes the first new batch (update.rs:799-827)
+    long long start = n_chunks_old, emb_off = old_N;
+    bool to_last = false;
+    if (start > 0) {
+        std::string lm;
+        const std::string last = dir + std::to_string(start - 1) + ".metadata.json";
+        double nd = 0, off = 0, ne = 0;
+        if (access(last.c_str(), F_OK) == 0) {
+            if (pb_status s = pb_read_text(last, lm)) return s;
+            if (pb_json_number(lm, "num_documents", nd) && nd < 2000) {
+                start -= 1;
+                to_last = true;
+                if (pb_json_number(lm, "embedding_offset", off)) emb_off = (long long)off;
+                else emb_off = old_N - (pb_json_number(lm, "num_embeddings", ne) ? (long long)ne : 0);
+            }
+        }
+    }
+    const long long n_new_chunks = (n_docs + batch_size - 1) / batch_size;
+    long long tok = 0;
+    for (long long i = 0; i < n_new_chunks; ++i) {
+        const std::string ci = std::to_string(start + i);
+        const long long d0 = i * batch_size, d1 = std::min(n_docs, d0 + batch_size);
+        std::vector<int64_t> cdl(doc_lengths + d0, doc_lengths + d1), ccodes;
+        long long ntok = 0;
+        for (int64_t v : cdl) ntok += v;
+        ccodes.assign(codes + tok, codes + tok + ntok);
+        std::vector<uint8_t> cres(residuals + (size_t)tok * packed, residuals + (size_t)(tok + ntok) * packed);
+        tok += ntok;
+        const std::string old_dl = dir + "doclens." + ci + ".json";
+        if (i == 0 && to_last && access(old_dl.c_str(), F_OK) == 0) {  // prepend the old chunk, read from disk
+            std::vector<int64_t> odl, ocodes;
+            std::vector<uint8_t> ores;
+            if (pb_status s = pb_read_doclens(old_dl, odl)) return s;
+            long long otok = 0;
+            for (int64_t v : odl) otok += v;
+            if (pb_status s = pb_read_chunk(dir, start + i, otok, packed, ocodes, ores)) return s;
+            cdl.insert(cdl.begin(), odl.begin(), odl.end());
+            ccodes.insert(ccodes.begin(), ocodes.begin(), ocodes.end());
+            cres.insert(cres.begin(), ores.begin(), ores.end());
+        }
+        const long long ctok = (long long)ccodes.size();
+        pb_status s = atomic_write(dir + ci + ".codes.npy", [&](const std::string &p) {
+            return write_npy(p, "<i8", {ctok}, ccodes.data(), (size_t)ctok * 8);
+        });
+        if (!s) s = atomic_write(dir + ci + ".residuals.npy", [&](const std::string &p) {
+            return write_npy(p, "|u1", {ctok, packed}, cres.data(), cres.size());
+        });
+        std::string dl = "[";
+        for (size_t d = 0; d < cdl.size(); ++d) dl += std::to_string((long long)cdl[d]) + (d + 1 < cdl.size() ? "," : "");
+        dl += "]";
+        if (!s) s = atomic_write(old_dl, [&](const std::string &p) { return write_text(p, dl); });
+        char cm[256];
+        snprintf(cm, sizeof cm, "{\n  \"num_documents\": %lld,\n  \"num_embeddings\": %lld,\n  \"embedding_offset\": %lld\n}",
+                 (long long)cdl.size(), ctok, emb_off);
+        emb_off += ctok;
+        if (!s) s = atomic_write(dir + ci + ".metadata.json", [&](const std::string &p) { return write_text(p, cm); });
+        if (s) return s;
+    }
+    pb_status s = atomic_write(dir + "ivf.npy", [&](const std::string &p) {
+        return write_npy(p, "<i8", {ivf_total}, ivf, (size_t)ivf_total * 8);
+    });
+    if (!s) s = atomic_write(dir + "ivf_lengths.npy", [&](const std::string &p) {
+        return write_npy(p, "<i4", {K}, ivf_lengths, (size_t)K * 4);
+    });
+    if (s) return s;
+    // update.rs:1085-1110: avg_doclen from the file's old value, not N / D
+    const long long total_D = old_D + n_docs;
+    const double new_avg = total_D > 0 ? (avg_doclen * (double)old_D + (double)tok) / (double)total_D : 0.0;
+    char m[512];  // struct Metadata, index.rs:105-127
+    snprintf(m, sizeof m,
+             "{\n  \"num_chunks\": %lld,\n  \"nbits\": %d,\n  \"num_partitions\": %lld,\n  \"num_embeddings\": %lld,\n"
+             "  \"avg_doclen\": %.17g,\n  \"num_documents\": %lld,\n  \"embedding_dim\": %d,\n  \"next_plaid_compatible\": true\n}",
+             start + n_new_chunks, nbits, K, old_N + tok, new_avg, total_D, dim);
+    if (pb_status s2 = atomic_write(dir + "metadata.json", [&](const std::string &p) { return write_text(p, m); })) return s2;
+    // clear_merged_files (mmap.rs:1714-1740): the merged caches no longer match the chunks
+    for (const char *f : {"merged_codes.npy", "merged_codes.npy.tmp", "merged_codes.manifest.json", "merged_codes.manifest.json.tmp",
+                          "merged_residuals.npy", "merged_residuals.npy.tmp", "merged_residuals.manifest.json",
+                          "merged_residuals.manifest.json.tmp"})
+        if (remove((dir + f).c_str()) != 0 && errno != ENOENT) return pb_fail(PB_ERR_IO, "cannot remove %s%s", dir.c_str(), f);
+    return PB_OK;
 }

@@ -20,6 +20,7 @@
 #include <cstring>
 #include <memory>
 #include <mutex>
+#include <shared_mutex>
 #include <string>
 #include <vector>
 
@@ -207,6 +208,37 @@ struct DevBuf {
         }
         return PB_OK;
     }
+    // Capacity for `bytes` that keeps the first `keep` bytes: a new allocation of max(bytes, 1.5 x the old capacity)
+    // (exactly `bytes` when !geometric) and one device-to-device copy.  On failure the old buffer is untouched.
+    pb_status grow(size_t bytes, size_t keep, bool geometric = true) {
+        if (bytes <= cap) return PB_OK;
+        if (p && !owned) return pb_fail(PB_ERR_UNSUPPORTED, "caller-owned device memory cannot grow");
+        const size_t want = geometric ? std::max(bytes, cap + cap / 2) : bytes;
+        void *q = nullptr;
+        cudaError_t e = cudaMalloc(&q, want);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return pb_fail(PB_ERR_NOMEM, "cudaMalloc(%zu bytes) failed: %s", want, cudaGetErrorString(e));
+        }
+        if (keep && p) {
+            e = cudaMemcpy(q, p, std::min(keep, cap), cudaMemcpyDeviceToDevice);
+            if (e != cudaSuccess) {
+                cudaFree(q);
+                return pb_fail(PB_ERR_CUDA, "cudaMemcpy failed: %s", cudaGetErrorString(e));
+            }
+        }
+        if (p) cudaFree(p);
+        p = q;
+        cap = want;
+        owned = true;
+        return PB_OK;
+    }
+    void swap(DevBuf &o) {
+        std::swap(p, o.p);
+        std::swap(cap, o.cap);
+        std::swap(zero_on_grow, o.zero_on_grow);
+        std::swap(owned, o.owned);
+    }
     template <class T> T *as() const { return reinterpret_cast<T *>(p); }
     ~DevBuf() {
         if (p && owned) cudaFree(p);
@@ -364,6 +396,16 @@ struct pb_index {
     int rank = 0, world = 1;
     std::mutex mu;
     std::vector<std::unique_ptr<Workspace>> pool;
+    DevBuf ivf_spare, ivf_off_spare;  // the other half of the inverted file's ping-pong: pb_index_append merges into it
+    // Readers (searches, stage entry points, accessors) share the arrays; pb_index_append / pb_index_reserve hold them
+    // alone.  A writer also holds `gate`, which every reader passes first: pthread rwlocks prefer readers, so without
+    // it a steady stream of searches could keep an append waiting forever.
+    mutable std::mutex gate;
+    mutable std::shared_mutex rw;
+    std::shared_lock<std::shared_mutex> read_lock() const {
+        { std::lock_guard<std::mutex> g(gate); }
+        return std::shared_lock<std::shared_mutex>(rw);
+    }
 
     pb_status acquire(std::unique_ptr<Workspace> &ws) {
         {
@@ -570,17 +612,18 @@ pb_status pb_index_open_begin(const pb_index_desc *d, pb_index **out) {
     return PB_OK;
 }
 
-// The inverted file of an index opened without one (index.rs:850-873), from the per-doc distinct code lists.
-static pb_status build_ivf_on_device(pb_index *ix) {
-    CKS(ix->ivf_off.ensure((size_t)(ix->K + 1) * 8));
-    const long long cap = std::max<long long>(ix->n_ucodes, 1);
-    DevBuf ka, kb, cnt, tmp;
-    CKS(ka.ensure((size_t)cap * 8));
+// The distinct (centroid, doc) pairs of docs [d0, d0 + n) as sorted keys code << 32 | (doc - d0) in `keys` (*m_out of
+// them), from the per-doc distinct code lists: k_ivf_pairs, a radix sort, and a unique pass for the raw lists of docs
+// longer than PB_UCODE_MAX.  `cap` bounds the pair count (the ucodes entries of those docs).
+static pb_status sorted_doc_pairs(pb_index *ix, long long d0, long long n, long long cap, DevBuf &keys, long long *m_out) {
+    cap = std::max<long long>(cap, 1);
+    DevBuf kb, cnt, tmp;
+    CKS(keys.ensure((size_t)cap * 8));
     CKS(kb.ensure((size_t)cap * 8));
     CKS(cnt.ensure(16));
     CK(cudaMemset(cnt.p, 0, 16));
-    if (ix->D > 0) {
-        k_ivf_pairs<<<ix->sm_count * 8, 256>>>(ix->ucodes.as<uint32_t>(), ix->udoc_off.as<long long>(), ix->D, ka.as<u64>(),
+    if (n > 0) {
+        k_ivf_pairs<<<ix->sm_count * 8, 256>>>(ix->ucodes.as<uint32_t>(), ix->udoc_off.as<long long>() + d0, n, keys.as<u64>(),
                                                cnt.as<unsigned long long>());
         CK(cudaGetLastError());
     }
@@ -590,20 +633,69 @@ static pb_status build_ivf_on_device(pb_index *ix) {
     int kbits = 1;
     while ((1ll << kbits) < ix->K) ++kbits;
     size_t tb = 0;
-    CK(cub::DeviceRadixSort::SortKeys(nullptr, tb, ka.as<u64>(), kb.as<u64>(), (int)m, 0, 32 + kbits));
+    CK(cub::DeviceRadixSort::SortKeys(nullptr, tb, keys.as<u64>(), kb.as<u64>(), (int)m, 0, 32 + kbits));
     size_t tb2 = 0;
-    CK(cub::DeviceSelect::Unique(nullptr, tb2, kb.as<u64>(), ka.as<u64>(), cnt.as<int>() + 2, (int)m));
+    CK(cub::DeviceSelect::Unique(nullptr, tb2, kb.as<u64>(), keys.as<u64>(), cnt.as<int>() + 2, (int)m));
     CKS(tmp.ensure(std::max(tb, tb2) + 16));
-    CK(cub::DeviceRadixSort::SortKeys(tmp.p, tb, ka.as<u64>(), kb.as<u64>(), (int)m, 0, 32 + kbits));
-    CK(cub::DeviceSelect::Unique(tmp.p, tb2, kb.as<u64>(), ka.as<u64>(), cnt.as<int>() + 2, (int)m));
+    CK(cub::DeviceRadixSort::SortKeys(tmp.p, tb, keys.as<u64>(), kb.as<u64>(), (int)m, 0, 32 + kbits));
+    CK(cub::DeviceSelect::Unique(tmp.p, tb2, kb.as<u64>(), keys.as<u64>(), cnt.as<int>() + 2, (int)m));
     int m2 = 0;
     CK(cudaMemcpy(&m2, cnt.as<int>() + 2, 4, cudaMemcpyDeviceToHost));
+    *m_out = m2;
+    return PB_OK;
+}
+
+// The inverted file of an index opened without one (index.rs:850-873), from the per-doc distinct code lists.
+static pb_status build_ivf_on_device(pb_index *ix) {
+    CKS(ix->ivf_off.ensure((size_t)(ix->K + 1) * 8));
+    DevBuf ka;
+    long long m2 = 0;
+    CKS(sorted_doc_pairs(ix, 0, ix->D, ix->n_ucodes, ka, &m2));
     ix->ivf_len = m2;
     CKS(ix->ivf.ensure(std::max<size_t>((size_t)m2 * 4, 16)));
     k_ivf_from_keys<<<ix->sm_count * 8, 256>>>(ka.as<u64>(), m2, ix->ivf.as<uint32_t>());
     k_ivf_offsets<<<(unsigned)((ix->K + 256) / 256), 256>>>(ka.as<u64>(), m2, ix->K, ix->ivf_off.as<long long>());
     CK(cudaGetLastError());
     CK(cudaDeviceSynchronize());
+    return PB_OK;
+}
+
+static bool filter_dim(int dim) { return dim == 64 || dim == 96 || dim == 128; }
+
+// Operands of the tensor-core kernels that depend on the centroids alone: the fp16 centroids of the filter (k_exact_tc)
+// and the scaled hi / lo tiles of the score table (k_scores16_tc).
+static pb_status build_centroid_operands(pb_index *ix) {
+    CKS(ix->centroids_f16.ensure((size_t)ix->K * ix->dim * 2));
+    k_rows_to_f16_plain<<<ix->sm_count * 8, 256>>>(ix->centroids.as<float>(), ix->K * (long long)ix->dim,
+                                                  ix->centroids_f16.as<__half>());
+    CK(cudaGetLastError());
+    if ((ix->k1_diag || ix->k1_tc) && ix->cmax > 0.0f && ix->cmax < 3.0e38f) {
+        // operands of the tensor-core score table: centroids * 2^cent_exp (max norm in [1, 2)), fp16 hi / lo parts
+        ix->cent_exp = -ilogbf(ix->cmax);
+        const size_t elems = (size_t)((ix->K + 127) / 128) * 128 * ix->dim;
+        CKS(ix->cent_h16t.ensure(elems * 2));
+        CKS(ix->cent_l16t.ensure(elems * 2));
+        CK(cudaMemset(ix->cent_h16t.p, 0, elems * 2));
+        CK(cudaMemset(ix->cent_l16t.p, 0, elems * 2));
+        k_rows_to_f16_split_tiles<<<ix->sm_count * 8, 256>>>(ix->centroids.as<float>(), ix->K, ix->dim, ix->cent_exp,
+                                                            ix->cent_h16t.as<__half>(), ix->cent_l16t.as<__half>());
+        CK(cudaGetLastError());
+    }
+    return PB_OK;
+}
+
+// 1 / |c + w| of tokens [t0, t0 + n) into tok_inv_norm; min |c + w| and max |w| over them folded into mn[0] / mn[1]
+static pb_status launch_min_vnorm(pb_index *ix, long long t0, long long n, float *mn) {
+    if (n == 0) return PB_OK;
+    const uint32_t *codes = ix->codes.as<uint32_t>() + t0;
+    const uint8_t *res = ix->residuals.as<uint8_t>() + (size_t)t0 * ix->packed;
+    float *inv = ix->tok_inv_norm.as<float>() + t0;
+    switch (ix->dim) {
+        case 64: k_min_vnorm<64><<<ix->sm_count * 8, 256>>>(ix->centroids.as<float>(), ix->w_rev.as<float>(), ix->nbits, codes, res, n, mn, inv); break;
+        case 96: k_min_vnorm<96><<<ix->sm_count * 8, 256>>>(ix->centroids.as<float>(), ix->w_rev.as<float>(), ix->nbits, codes, res, n, mn, inv); break;
+        default: k_min_vnorm<128><<<ix->sm_count * 8, 256>>>(ix->centroids.as<float>(), ix->w_rev.as<float>(), ix->nbits, codes, res, n, mn, inv); break;
+    }
+    CK(cudaGetLastError());
     return PB_OK;
 }
 
@@ -646,35 +738,15 @@ pb_status pb_index_finalize(pb_index *ix) {
         if (const char *e = getenv("PB_APPROX_GRID")) ix->approx_grid = std::max(1, atoi(e));
         if (const char *e = getenv("PB_XTC_GRID")) ix->xtc_grid = std::max(1, atoi(e));
     }
-    if ((ix->dim == 64 || ix->dim == 96 || ix->dim == 128) && ix->N > 0 && ix->K > 0) {
-        // operands of the tensor-core filter (k_exact_tc): fp16 centroids and the smallest token norm
-        CKS(ix->centroids_f16.ensure((size_t)ix->K * ix->dim * 2));
-        k_rows_to_f16_plain<<<ix->sm_count * 8, 256>>>(ix->centroids.as<float>(), ix->K * (long long)ix->dim,
-                                                      ix->centroids_f16.as<__half>());
-        CK(cudaGetLastError());
+    if (filter_dim(ix->dim) && ix->N > 0 && ix->K > 0) {
+        // operands of the tensor-core filter (k_exact_tc) and score table, and the smallest token norm
+        CKS(build_centroid_operands(ix));
         DevBuf mn;
         CKS(mn.ensure(16));
         CKS(ix->tok_inv_norm.ensure((size_t)ix->N * 4));  // 1 / |c + w| per token: operand of the linear estimate (k_maxsim_tc)
         const float init[2] = {3.0e38f, 0.0f};
         CK(cudaMemcpy(mn.p, init, 8, cudaMemcpyHostToDevice));
-        switch (ix->dim) {
-            case 64: k_min_vnorm<64><<<ix->sm_count * 8, 256>>>(ix->centroids.as<float>(), ix->w_rev.as<float>(), ix->nbits, ix->codes.as<uint32_t>(), ix->residuals.as<uint8_t>(), ix->N, mn.as<float>(), ix->tok_inv_norm.as<float>()); break;
-            case 96: k_min_vnorm<96><<<ix->sm_count * 8, 256>>>(ix->centroids.as<float>(), ix->w_rev.as<float>(), ix->nbits, ix->codes.as<uint32_t>(), ix->residuals.as<uint8_t>(), ix->N, mn.as<float>(), ix->tok_inv_norm.as<float>()); break;
-            default: k_min_vnorm<128><<<ix->sm_count * 8, 256>>>(ix->centroids.as<float>(), ix->w_rev.as<float>(), ix->nbits, ix->codes.as<uint32_t>(), ix->residuals.as<uint8_t>(), ix->N, mn.as<float>(), ix->tok_inv_norm.as<float>()); break;
-        }
-        CK(cudaGetLastError());
-        if ((ix->k1_diag || ix->k1_tc) && ix->cmax > 0.0f && ix->cmax < 3.0e38f) {
-            // operands of the tensor-core score table: centroids * 2^cent_exp (max norm in [1, 2)), fp16 hi / lo parts
-            ix->cent_exp = -ilogbf(ix->cmax);
-            const size_t elems = (size_t)((ix->K + 127) / 128) * 128 * ix->dim;
-            CKS(ix->cent_h16t.ensure(elems * 2));
-            CKS(ix->cent_l16t.ensure(elems * 2));
-            CK(cudaMemset(ix->cent_h16t.p, 0, elems * 2));
-            CK(cudaMemset(ix->cent_l16t.p, 0, elems * 2));
-            k_rows_to_f16_split_tiles<<<ix->sm_count * 8, 256>>>(ix->centroids.as<float>(), ix->K, ix->dim, ix->cent_exp,
-                                                                ix->cent_h16t.as<__half>(), ix->cent_l16t.as<__half>());
-            CK(cudaGetLastError());
-        }
+        CKS(launch_min_vnorm(ix, 0, ix->N, mn.as<float>()));
         float got[2] = {0.f, 0.f};
         CK(cudaMemcpy(got, mn.p, 8, cudaMemcpyDeviceToHost));
         ix->vmin = got[0] < 1e30f ? got[0] : 0.0f;
@@ -696,6 +768,7 @@ pb_status pb_index_finalize(pb_index *ix) {
 
 extern "C" pb_status pb_index_export_ivf(pb_index *ix, int64_t *out_ivf, int32_t *out_lengths, int64_t *out_total) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    auto rd = ix->read_lock();
     CK(cudaSetDevice(ix->device));
     if (out_total) *out_total = ix->ivf_len;
     if (!out_ivf && !out_lengths) return PB_OK;
@@ -735,10 +808,23 @@ extern "C" void pb_index_close(pb_index *ix) {
     delete ix;
 }
 
-extern "C" int64_t pb_index_num_documents(const pb_index *ix) { return ix ? ix->D : 0; }
-extern "C" int64_t pb_index_num_embeddings(const pb_index *ix) { return ix ? ix->N : 0; }
+// D and N change under pb_index_append; K, dim, nbits and the device are fixed at open
+extern "C" int64_t pb_index_num_documents(const pb_index *ix) {
+    if (!ix) return 0;
+    auto rd = ix->read_lock();
+    return ix->D;
+}
+extern "C" int64_t pb_index_num_embeddings(const pb_index *ix) {
+    if (!ix) return 0;
+    auto rd = ix->read_lock();
+    return ix->N;
+}
 extern "C" int64_t pb_index_num_partitions(const pb_index *ix) { return ix ? ix->K : 0; }
-extern "C" double pb_index_avg_doclen(const pb_index *ix) { return (ix && ix->D) ? (double)ix->N / (double)ix->D : 0.0; }
+extern "C" double pb_index_avg_doclen(const pb_index *ix) {
+    if (!ix) return 0.0;
+    auto rd = ix->read_lock();
+    return ix->D ? (double)ix->N / (double)ix->D : 0.0;
+}
 extern "C" int32_t pb_index_embedding_dim(const pb_index *ix) { return ix ? ix->dim : 0; }
 extern "C" int32_t pb_index_nbits(const pb_index *ix) { return ix ? ix->nbits : 0; }
 extern "C" int32_t pb_index_device(const pb_index *ix) { return ix ? ix->device : -1; }
@@ -1872,6 +1958,10 @@ struct LaneClock {
 static thread_local LaneClock g_lane_clock;
 
 static pb_status search_impl(pb_index *ix, const pb_search_params *p, const SearchIO &io) {
+    // the lanes' helper threads run under this caller's lock (they must not take it themselves: a waiting append
+    // would block them while this thread waits for them)
+    std::shared_lock<std::shared_mutex> rd;
+    if (ix) rd = ix->read_lock();
     // Lanes: the queries of a batch are independent, so the batch is cut into `lanes` slices searched concurrently, each
     // through the whole pipeline on its own workspace and stream (helper threads do the launching).  Not with a trace
     // (per-stage dumps), not doc-sharded (the exchanges are collective calls in batch order), not for small batches.
@@ -1972,6 +2062,7 @@ extern "C" pb_status pb_search_batch_device(pb_index *ix, const float *d_queries
 extern "C" pb_status pb_centroid_scores(pb_index *ix, const float *query_tokens, int64_t n, float *out) {
     if (!ix || (!query_tokens && n) || (!out && n)) return pb_fail(PB_ERR_INVALID, "null argument");
     if (n == 0) return PB_OK;
+    auto rd = ix->read_lock();
     CK(cudaSetDevice(ix->device));
     std::unique_ptr<Workspace> wsp;
     CKS(ix->acquire(wsp));
@@ -2006,6 +2097,7 @@ extern "C" pb_status pb_centroid_scores(pb_index *ix, const float *query_tokens,
 extern "C" pb_status pb_decompress_documents(pb_index *ix, const int64_t *doc_ids, int64_t n_docs, float *out_embeddings,
                                              int64_t *out_lengths) {
     if (!ix || (!doc_ids && n_docs) || !out_lengths) return pb_fail(PB_ERR_INVALID, "null argument");
+    auto rd = ix->read_lock();
     CK(cudaSetDevice(ix->device));
     if (n_docs == 0) return PB_OK;
     std::vector<long long> doff((size_t)ix->D + 1);
@@ -2105,6 +2197,7 @@ extern "C" pb_status pb_maxsim_scores(int32_t device, const float *query, int32_
 extern "C" pb_status pb_exhaustive_scores(pb_index *ix, const float *queries, const int64_t *q_off, int64_t n_queries,
                                           float *out_scores) {
     if (!ix || (!queries && n_queries) || !q_off || (!out_scores && n_queries)) return pb_fail(PB_ERR_INVALID, "null argument");
+    auto rd = ix->read_lock();
     CK(cudaSetDevice(ix->device));
     if (n_queries == 0 || ix->D == 0) return PB_OK;
     std::unique_ptr<Workspace> wsp;
@@ -2357,6 +2450,20 @@ extern "C" void pb_codec_close(pb_codec *c) {
     delete c;
 }
 
+// encode_index_chunk on m device-resident rows: codes (i64) and, when asked, the packed residuals and / or the f32 residuals
+static pb_status codec_encode_device(pb_codec *c, const float *dX, long long m, long long *dcodes, uint8_t *dpacked,
+                                     float *dres) {
+    CKS(assign_codes(c, dX, m, dcodes));
+    if (dpacked || dres) {
+        PB_DIM_SWITCH(c->dim, {
+            k_quantize_pack<DIM><<<c->sm_count * 8, 256>>>(dX, m, c->centroids.as<float>(), dcodes, c->cutoffs.as<float>(),
+                                                            c->nbits, dpacked, dres);
+        });
+        CK(cudaGetLastError());
+    }
+    return PB_OK;
+}
+
 // embeddings are processed in slabs so the staging buffers stay bounded
 static pb_status codec_run(pb_codec *c, const float *emb, int64_t n, int64_t *out_codes, uint8_t *out_packed,
                            float *out_residuals) {
@@ -2376,16 +2483,8 @@ static pb_status codec_run(pb_codec *c, const float *emb, int64_t n, int64_t *ou
     for (long long o = 0; o < n; o += slab) {
         const long long m = std::min(slab, n - o);
         CK(cudaMemcpy(dX.p, emb + (size_t)o * c->dim, (size_t)m * c->dim * 4, cudaMemcpyHostToDevice));
-        CKS(assign_codes(c, dX.as<float>(), m, dcodes.as<long long>()));
-        if (out_packed || out_residuals) {
-            PB_DIM_SWITCH(c->dim, {
-                k_quantize_pack<DIM><<<c->sm_count * 8, 256>>>(dX.as<float>(), m, c->centroids.as<float>(),
-                                                                dcodes.as<long long>(), c->cutoffs.as<float>(), c->nbits,
-                                                                out_packed ? dpk.as<uint8_t>() : nullptr,
-                                                                out_residuals ? dres.as<float>() : nullptr);
-            });
-            CK(cudaGetLastError());
-        }
+        CKS(codec_encode_device(c, dX.as<float>(), m, dcodes.as<long long>(), out_packed ? dpk.as<uint8_t>() : nullptr,
+                                out_residuals ? dres.as<float>() : nullptr));
         if (out_codes) CK(cudaMemcpy(out_codes + o, dcodes.p, (size_t)m * 8, cudaMemcpyDeviceToHost));
         if (out_packed) CK(cudaMemcpy(out_packed + (size_t)o * packed, dpk.p, (size_t)m * packed, cudaMemcpyDeviceToHost));
         if (out_residuals) CK(cudaMemcpy(out_residuals + (size_t)o * c->dim, dres.p, (size_t)m * c->dim * 4, cudaMemcpyDeviceToHost));
@@ -2795,5 +2894,223 @@ extern "C" pb_status pb_codec_find_outliers(pb_codec *c, const float *embeddings
             if (hf[i]) out_indices[cnt++] = o + i;
     }
     *out_count = cnt;
+    return PB_OK;
+}
+
+// ------------------------------------------------------------------------------------------
+// incremental append: MmapIndex::update_append (index.rs:1675) + reload on a live handle
+// ------------------------------------------------------------------------------------------
+static pb_status append_impl(pb_index *ix, pb_codec *codec, const float *embeddings, const int64_t *codes,
+                             const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs, int32_t space,
+                             const char *index_dir, int64_t batch_size, int64_t *out_first) {
+    if (!ix || (!doc_lengths && n_docs) || n_docs < 0) return pb_fail(PB_ERR_INVALID, "null argument");
+    if (space != PB_MEM_HOST && space != PB_MEM_DEVICE) return pb_fail(PB_ERR_INVALID, "bad memory_space %d", space);
+    std::lock_guard<std::mutex> gate(ix->gate);
+    std::unique_lock<std::shared_mutex> wr(ix->rw);
+    if (ix->comm || ix->group) return pb_fail(PB_ERR_UNSUPPORTED, "appends to a doc-sharded handle are not supported");
+    if (!ix->residuals.owned)
+        return pb_fail(PB_ERR_UNSUPPORTED, "the handle uses the caller's residual array (PB_OPEN_ADOPT_RESIDUALS)");
+    if (index_dir && ix->doc_id_base != 0) return pb_fail(PB_ERR_UNSUPPORTED, "an index directory holds doc ids from 0");
+    if (index_dir && batch_size <= 0) return pb_fail(PB_ERR_INVALID, "batch_size must be positive");
+    CK(cudaSetDevice(ix->device));
+    CK(cudaDeviceSynchronize());  // work earlier readers left queued (pb_search_batch_device) reads the arrays
+    if (codec) {  // same K, dim, nbits and bit-identical centroids as the index; cutoffs required (codec.rs:359-362)
+        if (codec->K != ix->K || codec->dim != ix->dim || codec->nbits != ix->nbits || codec->device != ix->device)
+            return pb_fail(PB_ERR_INVALID, "codec (K=%lld dim=%d nbits=%d device %d) does not match the index (K=%lld dim=%d nbits=%d device %d)",
+                           codec->K, codec->dim, codec->nbits, codec->device, ix->K, ix->dim, ix->nbits, ix->device);
+        if (!codec->has_cutoffs) return pb_fail(PB_ERR_INVALID, "bucket_cutoffs required for quantization");
+        DevBuf flag;
+        CKS(flag.ensure(16));
+        CK(cudaMemset(flag.p, 0, 4));
+        k_words_differ<<<ix->sm_count * 8, 256>>>(codec->centroids.as<uint32_t>(), ix->centroids.as<uint32_t>(),
+                                                  ix->K * (long long)ix->dim, flag.as<int>());
+        CK(cudaGetLastError());
+        int differ = 0;
+        CK(cudaMemcpy(&differ, flag.p, 4, cudaMemcpyDeviceToHost));
+        if (differ) return pb_fail(PB_ERR_INVALID, "the codec's centroids differ from the index's");
+    }
+    const long long D0 = ix->D, N0 = ix->N, U0 = ix->n_ucodes, n = n_docs;
+    if (out_first) *out_first = ix->doc_id_base + D0;
+    std::vector<int64_t> dl;
+    CKS(fetch_host(dl, doc_lengths, (size_t)n, space));
+    std::vector<long long> doff((size_t)n, 0);  // doc_off[D0 + 1 ..]
+    long long ntok = 0;
+    int maxlen = ix->max_doclen;
+    for (long long i = 0; i < n; ++i) {
+        if (dl[i] < 0 || dl[i] > (1 << 30)) return pb_fail(PB_ERR_INVALID, "doc_lengths[%lld] = %lld", i, (long long)dl[i]);
+        ntok += dl[i];
+        doff[i] = N0 + ntok;
+        maxlen = std::max<int>(maxlen, (int)dl[i]);
+    }
+    if (n == 0) return PB_OK;
+    // the limits of pb_index_open_begin for the new totals
+    if (D0 + n >= (1ll << 32) - 1 || ix->doc_id_base + D0 + n >= (1ll << 32) - 1)
+        return pb_fail(PB_ERR_UNSUPPORTED, "D and global doc ids must stay below 2^32-1");
+    if (ntok > 0 && ((codec && !embeddings) || (!codec && (!codes || !residuals)))) return pb_fail(PB_ERR_INVALID, "null argument");
+    const long long N1 = N0 + ntok, D1 = D0 + n;
+    const size_t pk = (size_t)ix->packed;
+    const bool filter = filter_dim(ix->dim) && N1 > 0;
+
+    // capacity: grown arrays keep their contents; nothing below is visible until the commit
+    CKS(ix->codes.grow((size_t)N1 * 4, (size_t)N0 * 4));
+    CKS(ix->residuals.grow((size_t)N1 * pk, (size_t)N0 * pk));
+    if (filter) CKS(ix->tok_inv_norm.grow((size_t)N1 * 4, (size_t)N0 * 4));
+    CKS(ix->doc_off.grow((size_t)(D1 + 1) * 8, (size_t)(D0 + 1) * 8));
+    CKS(ix->udoc_off.grow((size_t)(D1 + 1) * 8, (size_t)(D0 + 1) * 8));
+
+    // 1. tokens into the tails of codes / residuals: encoded on the device, or narrowed and range-checked
+    std::vector<int64_t> hcodes;  // i64 codes for the chunk files
+    if (codec) {
+        codec->last_tokens = ntok;
+        codec->last_fallback = 0;
+        const long long slab = 1ll << 20;
+        DevBuf dX, dcodes;
+        CKS(dcodes.ensure((size_t)std::max(std::min(ntok, slab), 1ll) * 8));
+        if (space == PB_MEM_HOST) CKS(dX.ensure((size_t)std::max(std::min(ntok, slab), 1ll) * ix->dim * 4));
+        if (index_dir) hcodes.resize((size_t)ntok);
+        for (long long o = 0; o < ntok; o += slab) {
+            const long long m = std::min(slab, ntok - o);
+            const float *x = embeddings + (size_t)o * ix->dim;
+            if (space == PB_MEM_HOST) {
+                CK(cudaMemcpy(dX.p, x, (size_t)m * ix->dim * 4, cudaMemcpyHostToDevice));
+                x = dX.as<float>();
+            }
+            CKS(codec_encode_device(codec, x, m, dcodes.as<long long>(), ix->residuals.as<uint8_t>() + (size_t)(N0 + o) * pk, nullptr));
+            CKS(upload_narrow(ix->codes, N0 + o, reinterpret_cast<const int64_t *>(dcodes.p), m, ix->K, PB_MEM_DEVICE, "codes"));
+            if (index_dir) CK(cudaMemcpy(hcodes.data() + o, dcodes.p, (size_t)m * 8, cudaMemcpyDeviceToHost));
+        }
+    } else if (ntok > 0) {
+        CK(cudaMemcpy(ix->residuals.as<uint8_t>() + (size_t)N0 * pk, residuals, (size_t)ntok * pk,
+                      space == PB_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+        CKS(upload_narrow(ix->codes, N0, codes, ntok, ix->K, space, "codes"));
+    }
+
+    // 2. doc offsets
+    CK(cudaMemcpy(ix->doc_off.as<long long>() + D0 + 1, doff.data(), (size_t)n * 8, cudaMemcpyHostToDevice));
+
+    // 3. distinct code lists of the new docs, after the old ones (udoc_off holds absolute positions into ucodes)
+    std::vector<long long> uoff((size_t)n);
+    {
+        DevBuf counts;
+        CKS(counts.ensure((size_t)n * 4));
+        const int blocks = (int)std::min<long long>(n, (long long)ix->sm_count * 16);
+        k_unique_codes<<<blocks, 128>>>(ix->codes.as<uint32_t>(), ix->doc_off.as<long long>() + D0, n, nullptr, nullptr,
+                                        counts.as<int>());
+        CK(cudaGetLastError());
+        std::vector<int> hc((size_t)n);
+        CK(cudaMemcpy(hc.data(), counts.p, hc.size() * 4, cudaMemcpyDeviceToHost));
+        long long u = U0;
+        for (long long i = 0; i < n; ++i) uoff[i] = u += hc[i];
+    }
+    const long long U1 = uoff[n - 1];
+    CKS(ix->ucodes.grow(std::max<size_t>((size_t)U1 * 4, 16), (size_t)U0 * 4));
+    CK(cudaMemcpy(ix->udoc_off.as<long long>() + D0 + 1, uoff.data(), (size_t)n * 8, cudaMemcpyHostToDevice));
+    {
+        const int blocks = (int)std::min<long long>(n, (long long)ix->sm_count * 16);
+        k_unique_codes<<<blocks, 128>>>(ix->codes.as<uint32_t>(), ix->doc_off.as<long long>() + D0, n,
+                                        ix->udoc_off.as<long long>() + D0, ix->ucodes.as<uint32_t>(), nullptr);
+        CK(cudaGetLastError());
+    }
+
+    // 4. 1 / |c + w| of the new tokens; min / max seeded with the index's, which is what an open over all tokens finds
+    float vmin = ix->vmin, wmax = ix->wmax;
+    if (filter) {
+        if (N0 == 0) CKS(build_centroid_operands(ix));  // an index opened empty has none yet
+        DevBuf mn;
+        CKS(mn.ensure(16));
+        const float init[2] = {N0 > 0 ? ix->vmin : 3.0e38f, N0 > 0 ? ix->wmax : 0.0f};
+        CK(cudaMemcpy(mn.p, init, 8, cudaMemcpyHostToDevice));
+        CKS(launch_min_vnorm(ix, N0, ntok, mn.as<float>()));
+        float got[2] = {0.f, 0.f};
+        CK(cudaMemcpy(got, mn.p, 8, cudaMemcpyDeviceToHost));
+        vmin = got[0] < 1e30f ? got[0] : 0.0f;
+        wmax = got[1];
+    }
+
+    // 5. inverted file: the new docs' sorted distinct (centroid, doc) pairs merged behind each centroid's old list
+    DevBuf keys, add_before;
+    long long m = 0;
+    CKS(sorted_doc_pairs(ix, D0, n, U1 - U0, keys, &m));
+    const long long L1 = ix->ivf_len + m;
+    if (L1 > (1ll << 31) - 2) return pb_fail(PB_ERR_UNSUPPORTED, "more than 2^31 (centroid, doc) pairs per shard");
+    CKS(add_before.ensure((size_t)(ix->K + 1) * 8));
+    CKS(ix->ivf_spare.grow(std::max<size_t>((size_t)L1 * 4, 16), 0));
+    CKS(ix->ivf_off_spare.ensure((size_t)(ix->K + 1) * 8));
+    k_ivf_offsets<<<(unsigned)((ix->K + 256) / 256), 256>>>(keys.as<u64>(), m, ix->K, add_before.as<long long>());
+    k_ivf_merge_old<<<ix->sm_count * 8, 256>>>(ix->ivf.as<uint32_t>(), ix->ivf_off.as<long long>(), add_before.as<long long>(),
+                                               ix->K, ix->ivf_spare.as<uint32_t>(), ix->ivf_off_spare.as<long long>());
+    if (m > 0)
+        k_ivf_merge_new<<<ix->sm_count * 8, 256>>>(keys.as<u64>(), m, ix->ivf_off.as<long long>(), (uint32_t)D0,
+                                                   ix->ivf_spare.as<uint32_t>());
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+
+    // update_index's file changes, before the commit: a failure leaves the handle as it was
+    if (index_dir) {
+        std::vector<uint8_t> hres((size_t)ntok * pk);
+        if (ntok) CK(cudaMemcpy(hres.data(), ix->residuals.as<uint8_t>() + (size_t)N0 * pk, hres.size(), cudaMemcpyDeviceToHost));
+        std::vector<int64_t> hivf((size_t)std::max(L1, 1ll));
+        std::vector<int32_t> hlen((size_t)ix->K);
+        DevBuf di, dln;
+        CKS(di.ensure(std::max<size_t>((size_t)L1 * 8, 16)));
+        CKS(dln.ensure((size_t)ix->K * 4));
+        k_ivf_export<<<ix->sm_count * 8, 256>>>(ix->ivf_spare.as<uint32_t>(), ix->ivf_off_spare.as<long long>(), L1, ix->K, 0,
+                                               di.as<long long>(), dln.as<int>());
+        CK(cudaGetLastError());
+        if (L1) CK(cudaMemcpy(hivf.data(), di.p, (size_t)L1 * 8, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(hlen.data(), dln.p, (size_t)ix->K * 4, cudaMemcpyDeviceToHost));
+        CKS(pb_dir_append(index_dir, D0, ix->K, ix->dim, ix->nbits, batch_size, hcodes.data(), hres.data(), dl.data(), n,
+                          hivf.data(), L1, hlen.data()));
+    }
+
+    // 6. commit
+    ix->ivf.swap(ix->ivf_spare);
+    ix->ivf_off.swap(ix->ivf_off_spare);
+    ix->ivf_len = L1;
+    ix->n_ucodes = U1;
+    ix->N = N1;
+    ix->D = D1;
+    ix->max_doclen = maxlen;
+    ix->vmin = vmin;
+    ix->wmax = wmax;
+    return PB_OK;
+}
+
+extern "C" pb_status pb_index_append(pb_index *ix, pb_codec *codec, const float *embeddings, const int64_t *doc_lengths,
+                                     int64_t n_docs, int32_t memory_space, const char *index_dir, int64_t batch_size,
+                                     int64_t *out_first_doc_id) {
+    if (!codec) return pb_fail(PB_ERR_INVALID, "null argument");
+    return append_impl(ix, codec, embeddings, nullptr, nullptr, doc_lengths, n_docs, memory_space, index_dir, batch_size,
+                       out_first_doc_id);
+}
+
+extern "C" pb_status pb_index_append_encoded(pb_index *ix, const int64_t *codes, const uint8_t *residuals,
+                                             const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
+                                             int64_t *out_first_doc_id) {
+    return append_impl(ix, nullptr, nullptr, codes, residuals, doc_lengths, n_docs, memory_space, nullptr, 0, out_first_doc_id);
+}
+
+extern "C" pb_status pb_index_reserve(pb_index *ix, int64_t num_documents, int64_t num_embeddings) {
+    if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    std::lock_guard<std::mutex> gate(ix->gate);
+    std::unique_lock<std::shared_mutex> wr(ix->rw);
+    if (ix->comm || ix->group) return pb_fail(PB_ERR_UNSUPPORTED, "appends to a doc-sharded handle are not supported");
+    if (!ix->residuals.owned)
+        return pb_fail(PB_ERR_UNSUPPORTED, "the handle uses the caller's residual array (PB_OPEN_ADOPT_RESIDUALS)");
+    if (num_documents >= (1ll << 32) - 1 || num_embeddings < 0) return pb_fail(PB_ERR_INVALID, "bad reserve sizes");
+    CK(cudaSetDevice(ix->device));
+    CK(cudaDeviceSynchronize());
+    const long long D1 = std::max<long long>(num_documents, ix->D), N1 = std::max<long long>(num_embeddings, ix->N);
+    const long long dd = D1 - ix->D, dn = N1 - ix->N;
+    // a new doc adds at most its length rounded up to 8 distinct-code entries, and at most that many (centroid, doc) pairs
+    const long long U1 = ix->n_ucodes + dn + 7 * dd, L1 = ix->ivf_len + dn;
+    CKS(ix->codes.grow((size_t)N1 * 4, (size_t)ix->N * 4, false));
+    CKS(ix->residuals.grow((size_t)N1 * ix->packed, (size_t)ix->N * ix->packed, false));
+    if (filter_dim(ix->dim)) CKS(ix->tok_inv_norm.grow((size_t)N1 * 4, (size_t)ix->N * 4, false));
+    CKS(ix->doc_off.grow((size_t)(D1 + 1) * 8, (size_t)(ix->D + 1) * 8, false));
+    CKS(ix->udoc_off.grow((size_t)(D1 + 1) * 8, (size_t)(ix->D + 1) * 8, false));
+    CKS(ix->ucodes.grow((size_t)U1 * 4, (size_t)ix->n_ucodes * 4, false));
+    CKS(ix->ivf.grow((size_t)L1 * 4, (size_t)ix->ivf_len * 4, false));
+    CKS(ix->ivf_spare.grow((size_t)L1 * 4, 0, false));
     return PB_OK;
 }

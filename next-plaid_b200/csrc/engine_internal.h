@@ -1,6 +1,9 @@
-// engine_internal.h -- C++-side entry points shared between engine.cu and loader.cpp (not exported).
+// engine_internal.h -- C++-side entry points shared between engine.cu, loader.cpp and builder.cpp (not exported).
 #pragma once
 #include "../../include/plaid_b200.h"
+
+#include <string>
+#include <vector>
 
 pb_status pb_fail(pb_status s, const char *fmt, ...);
 // pb_index_open without the per-token arrays; follow with pb_index_upload_tokens per chunk.
@@ -9,3 +12,19 @@ pb_status pb_index_upload_tokens(pb_index *ix, long long tok_off, const int64_t 
                                  long long n, int space);
 // call once after the last pb_index_upload_tokens
 pb_status pb_index_finalize(pb_index *ix);
+
+// The index directory, as the loader reads it: a whole file; a number of a flat JSON object; a doclens.{i}.json list;
+// the chunk file pair {i}.codes.npy <i8 [n_tokens] / {i}.residuals.npy u1 [n_tokens][packed].
+pb_status pb_read_text(const std::string &path, std::string &out);
+bool pb_json_number(const std::string &j, const char *key, double &out);
+pb_status pb_read_doclens(const std::string &path, std::vector<int64_t> &out);
+pb_status pb_read_chunk(const std::string &dir, long long chunk, long long n_tokens, long long packed,
+                        std::vector<int64_t> &codes, std::vector<uint8_t> &residuals);
+
+// update_index's file changes (update.rs:794-1117, update_threshold = false) for n_docs documents appended to the
+// index in index_dir, which holds old_D documents: chunk files in batches of batch_size docs (the first merged into a
+// last chunk of < 2000 docs), the merged inverted file ivf / ivf_lengths (global ids), metadata.json, and removal of
+// the merged_* caches.  codes i64 [sum doc_lengths], residuals packed [sum doc_lengths][dim*nbits/8].
+pb_status pb_dir_append(const char *index_dir, long long old_D, long long K, int dim, int nbits, long long batch_size,
+                        const int64_t *codes, const uint8_t *residuals, const int64_t *doc_lengths, long long n_docs,
+                        const int64_t *ivf, long long ivf_total, const int32_t *ivf_lengths);

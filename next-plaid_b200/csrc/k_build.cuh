@@ -593,6 +593,46 @@ __global__ void k_ivf_export(const uint32_t *__restrict__ ivf, const long long *
         for (long long c = i0; c < K; c += stride) out_len[c] = (int)(ivf_off[c + 1] - ivf_off[c]);
 }
 
+// ------------------------------------------------------------------------------------------
+// Incremental append (pb_index_append): the merged inverted file is, per centroid, sort + dedup(old list + new pids)
+// (update.rs:1000-1067).  The new docs' ids exceed every old id and both parts are ascending and unique, so that is the
+// old list followed by the centroid's sorted new pairs.  add_before[c] = number of new pairs whose centroid is < c (the
+// lower bound of c << 32 in the sorted new keys, k_ivf_offsets).  Out of place, into the spare half of the ping-pong:
+// old entry j of centroid c goes to old_off[c] + add_before[c] + j, one warp per centroid (coalesced on both sides);
+// new_off[c] = old_off[c] + add_before[c] for c = 0..K.
+// ------------------------------------------------------------------------------------------
+__global__ void k_ivf_merge_old(const uint32_t *__restrict__ ivf, const long long *__restrict__ old_off,
+                                const long long *__restrict__ add_before, long long K, uint32_t *__restrict__ out,
+                                long long *__restrict__ new_off) {
+    const int lane = threadIdx.x & 31;
+    const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
+    for (long long c = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c <= K; c += nw) {
+        const long long o0 = old_off[c], dst = o0 + add_before[c];
+        if (lane == 0) new_off[c] = dst;
+        if (c == K) continue;
+        const long long n = old_off[c + 1] - o0;
+        for (long long j = lane; j < n; j += 32) out[dst + j] = ivf[o0 + j];
+    }
+}
+
+// the j-th sorted new key (centroid c, doc local to the appended batch) lands right after c's old list:
+// new_off[c] + old_len[c] + (j - add_before[c]) = old_off[c + 1] + j; the doc id is offset by the old D
+__global__ void k_ivf_merge_new(const u64 *__restrict__ keys, long long m, const long long *__restrict__ old_off,
+                                uint32_t doc_base, uint32_t *__restrict__ out) {
+    for (long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x; j < m; j += (long long)gridDim.x * blockDim.x) {
+        const u64 k = keys[j];
+        out[old_off[(k >> 32) + 1] + j] = (uint32_t)k + doc_base;
+    }
+}
+
+// *flag = 1 when the two arrays differ in any bit (the codec of an append must hold the index's centroids exactly)
+__global__ void k_words_differ(const uint32_t *__restrict__ a, const uint32_t *__restrict__ b, long long n, int *__restrict__ flag) {
+    bool d = false;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        d |= a[i] != b[i];
+    if (__syncthreads_or(d) && threadIdx.x == 0) *flag = 1;
+}
+
 // codec training (index.rs:240-258): L2 norm of every residual row; per-dimension mean of |residual|
 __global__ void k_residual_stats(const float *__restrict__ R, long long n, int dim, float *__restrict__ norms) {
     const int lane = threadIdx.x & 31;

@@ -149,7 +149,9 @@ pb_status as_f32(const Npy &a, const char *name, std::vector<float> &store, cons
     return PB_OK;
 }
 
-pb_status read_text(const std::string &path, std::string &out) {
+}  // namespace
+
+pb_status pb_read_text(const std::string &path, std::string &out) {
     FILE *f = fopen(path.c_str(), "rb");
     if (!f) return pb_fail(PB_ERR_IO, "cannot open %s", path.c_str());
     char buf[1 << 16];
@@ -161,7 +163,7 @@ pb_status read_text(const std::string &path, std::string &out) {
 }
 
 // number following "key": in a flat JSON object (metadata.json, index.rs:105-127)
-bool json_number(const std::string &j, const char *key, double &out) {
+bool pb_json_number(const std::string &j, const char *key, double &out) {
     std::string k = std::string("\"") + key + "\"";
     size_t p = j.find(k);
     if (p == std::string::npos) return false;
@@ -174,18 +176,41 @@ bool json_number(const std::string &j, const char *key, double &out) {
     return end != j.c_str() + p;
 }
 
-}  // namespace
+pb_status pb_read_doclens(const std::string &path, std::vector<int64_t> &out) {
+    std::string txt;
+    if (pb_status s = pb_read_text(path, txt)) return s;
+    const char *p = txt.c_str();
+    while (*p) {
+        if (isdigit((unsigned char)*p) || (*p == '-' && isdigit((unsigned char)p[1]))) out.push_back(strtoll(p, (char **)&p, 10));
+        else ++p;
+    }
+    return PB_OK;
+}
+
+pb_status pb_read_chunk(const std::string &dir, long long chunk, long long n_tokens, long long packed,
+                        std::vector<int64_t> &codes, std::vector<uint8_t> &residuals) {
+    Npy c, r;
+    if (pb_status s = c.open(dir + std::to_string(chunk) + ".codes.npy")) return s;
+    if (pb_status s = r.open(dir + std::to_string(chunk) + ".residuals.npy")) return s;
+    if (!c.is("i8") || c.count() != n_tokens)
+        return pb_fail(PB_ERR_IO, "%lld.codes.npy must be <i8 [%lld]", chunk, n_tokens);
+    if (!r.is("u1") || r.shape.size() != 2 || r.shape[0] != n_tokens || r.shape[1] != packed)
+        return pb_fail(PB_ERR_IO, "%lld.residuals.npy must be u1 [%lld, %lld]", chunk, n_tokens, packed);
+    codes.assign((const int64_t *)c.data, (const int64_t *)c.data + n_tokens);
+    residuals.assign(r.data, r.data + (size_t)n_tokens * packed);
+    return PB_OK;
+}
 
 extern "C" pb_status pb_index_load(const char *index_dir, int32_t device, pb_index **out) {
     if (!index_dir || !out) return pb_fail(PB_ERR_INVALID, "null argument");
     *out = nullptr;
     const std::string dir = std::string(index_dir) + "/";
     std::string meta;
-    if (pb_status s = read_text(dir + "metadata.json", meta)) return s;
+    if (pb_status s = pb_read_text(dir + "metadata.json", meta)) return s;
     double num_chunks = 0, nbits = 0, num_emb = -1;
-    if (!json_number(meta, "num_chunks", num_chunks) || !json_number(meta, "nbits", nbits))
+    if (!pb_json_number(meta, "num_chunks", num_chunks) || !pb_json_number(meta, "nbits", nbits))
         return pb_fail(PB_ERR_IO, "metadata.json lacks num_chunks / nbits");
-    json_number(meta, "num_embeddings", num_emb);
+    pb_json_number(meta, "num_embeddings", num_emb);
 
     Npy cent, wts, ivf, ivfl;
     if (pb_status s = cent.open(dir + "centroids.npy")) return s;
@@ -223,17 +248,10 @@ extern "C" pb_status pb_index_load(const char *index_dir, int32_t device, pb_ind
     std::vector<int64_t> doclens;
     std::vector<long long> chunk_tokens;
     for (int c = 0; c < (int)num_chunks; ++c) {
-        std::string txt;
-        if (pb_status s = read_text(dir + "doclens." + std::to_string(c) + ".json", txt)) return s;
+        const size_t first = doclens.size();
+        if (pb_status s = pb_read_doclens(dir + "doclens." + std::to_string(c) + ".json", doclens)) return s;
         long long tok = 0;
-        const char *p = txt.c_str();
-        while (*p) {
-            if (isdigit((unsigned char)*p) || (*p == '-' && isdigit((unsigned char)p[1]))) {
-                long long v = strtoll(p, (char **)&p, 10);
-                doclens.push_back(v);
-                tok += v;
-            } else ++p;
-        }
+        for (size_t i = first; i < doclens.size(); ++i) tok += doclens[i];
         chunk_tokens.push_back(tok);
     }
     long long N = 0;

@@ -84,6 +84,7 @@ EXPORTS = [
     "pb_codec_encode_chunk", "pb_kmeans_fit", "pb_codec_train", "pb_kmeans_num_sample_docs",
     "pb_kmeans_num_partitions", "pb_codec_num_sample_docs", "pb_codec_heldout_tokens", "pb_create_index",
     "pb_create_params_default", "pb_build_comm_init", "pb_build_comm_group", "pb_build_comm_destroy", "pb_kmeans_fit_dp", "pb_codec_last_assign_stats", "pb_codec_find_outliers",
+    "pb_index_append", "pb_index_append_encoded", "pb_index_reserve",
 ]
 
 _lib = None
@@ -168,6 +169,11 @@ def load_library():
         L.pb_shard_group_destroy.argtypes = [C.c_void_p]
         L.pb_shard_group_destroy.restype = None
         L.pb_index_group_join.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
+        L.pb_index_append.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_char_p,
+                                      C.c_int64, C.c_void_p]
+        L.pb_index_append_encoded.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32,
+                                              C.c_void_p]
+        L.pb_index_reserve.argtypes = [C.c_void_p, C.c_int64, C.c_int64]
         _lib = L
     return _lib
 
@@ -358,6 +364,38 @@ class MmapIndex:
 
     def nbits(self) -> int:
         return int(load_library().pb_index_nbits(self._h))
+
+    # -- incremental append (index.rs:1675 update_append + reload) ------------------------------------
+    def append(self, embeddings: Sequence[np.ndarray], codec: "ResidualCodec", index_dir: Optional[str] = None,
+               batch_size: int = 50_000) -> List[int]:
+        """MmapIndex::update_append + reload (pb_index_append): encodes the documents on the device with `codec` (the
+        index's centroids and bucket cutoffs) and appends them; with `index_dir` also applies update_index's file
+        changes to that directory (chunks of `batch_size` docs).  Returns the assigned doc ids."""
+        dl = np.array([e.shape[0] for e in embeddings], np.int64)
+        dim = self.embedding_dim()
+        flat = (np.ascontiguousarray(np.concatenate(embeddings, 0), np.float32) if len(embeddings)
+                else np.zeros((0, dim), np.float32))
+        first = C.c_int64()
+        _check(load_library().pb_index_append(self._h, codec._h, _ptr(flat), _ptr(dl), len(dl), 0,
+                                              None if index_dir is None else os.fsencode(index_dir), batch_size,
+                                              C.byref(first)))
+        return list(range(first.value, first.value + len(dl)))
+
+    def append_encoded(self, codes: np.ndarray, residuals: np.ndarray, doc_lengths: Sequence[int]) -> List[int]:
+        """pb_index_append_encoded: documents already encoded (codes i64 [n], packed residuals u8 [n, dim*nbits/8])."""
+        cd = np.ascontiguousarray(codes, np.int64)
+        rs = np.ascontiguousarray(residuals, np.uint8)
+        dl = np.ascontiguousarray(doc_lengths, np.int64)
+        if rs.size != len(cd) * self.embedding_dim() * self.nbits() // 8 or int(dl.sum()) != len(cd):
+            raise PlaidError(PB_ERR_INVALID, f"codes {cd.shape}, residuals {rs.shape} and doc_lengths (sum "
+                                             f"{int(dl.sum())}) do not describe the same tokens")
+        first = C.c_int64()
+        _check(load_library().pb_index_append_encoded(self._h, _ptr(cd), _ptr(rs), _ptr(dl), len(dl), 0, C.byref(first)))
+        return list(range(first.value, first.value + len(dl)))
+
+    def reserve(self, num_documents: int, num_embeddings: int):
+        """pb_index_reserve: capacity for appends up to these totals without reallocation."""
+        _check(load_library().pb_index_reserve(self._h, num_documents, num_embeddings))
 
     # -- search ------------------------------------------------------------------------------
     def search(self, query: np.ndarray, params: SearchParameters,

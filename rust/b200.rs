@@ -43,6 +43,7 @@ extern "C" {
     fn pb_index_load(index_dir: *const c_char, device: i32, out: *mut *mut c_void) -> c_int;
     fn pb_index_close(ix: *mut c_void);
     fn pb_index_embedding_dim(ix: *const c_void) -> i32;
+    fn pb_index_device(ix: *const c_void) -> i32;
     fn pb_search_batch(
         ix: *mut c_void,
         queries: *const f32,
@@ -56,6 +57,15 @@ extern "C" {
         out_counts: *mut i32,
     ) -> c_int;
     fn pb_last_error() -> *const c_char;
+    fn pb_codec_open(device: i32, centroids: *const f32, k: i64, dim: i32, nbits: i32, cutoffs: *const f32,
+                     out: *mut *mut c_void) -> c_int;
+    fn pb_codec_close(c: *mut c_void);
+    fn pb_index_append(ix: *mut c_void, codec: *mut c_void, embeddings: *const f32, doc_lengths: *const i64,
+                       n_docs: i64, memory_space: i32, index_dir: *const c_char, batch_size: i64,
+                       out_first_doc_id: *mut i64) -> c_int;
+    fn pb_index_append_encoded(ix: *mut c_void, codes: *const i64, residuals: *const u8, doc_lengths: *const i64,
+                               n_docs: i64, memory_space: i32, out_first_doc_id: *mut i64) -> c_int;
+    fn pb_index_reserve(ix: *mut c_void, num_documents: i64, num_embeddings: i64) -> c_int;
 }
 
 fn last_error() -> String {
@@ -142,6 +152,55 @@ impl B200Index {
                 }
             })
             .collect())
+    }
+
+    /// `MmapIndex::update_append` (index.rs:1675) + `reload` (index.rs:1767) under the `b200` feature: the codec of the
+    /// directory (`ResidualCodec::load_from_dir`) encodes on the device, the handle grows in place (searches from other
+    /// threads wait for it) and `update_index`'s file changes are applied to `index_path` (update.rs:794-1117,
+    /// update_threshold = false).  Returns the assigned doc ids.
+    pub fn update_append(
+        &self,
+        embeddings: &[Array2<f32>],
+        index_path: &str,
+        codec: &crate::codec::ResidualCodec,
+        batch_size: usize,
+    ) -> Result<Vec<i64>> {
+        let dim = unsafe { pb_index_embedding_dim(self.handle) } as usize;
+        let mut flat: Vec<f32> = Vec::new();
+        let mut lens: Vec<i64> = Vec::with_capacity(embeddings.len());
+        for e in embeddings {
+            if e.ncols() != dim {
+                return Err(Error::Shape(format!("document has {} columns, the index embedding_dim is {}", e.ncols(), dim)));
+            }
+            flat.extend(e.as_standard_layout().iter());
+            lens.push(e.nrows() as i64);
+        }
+        let cen = codec.centroids.view().as_standard_layout().to_owned();
+        let cut = codec
+            .bucket_cutoffs
+            .as_ref()
+            .ok_or_else(|| Error::Codec("bucket_cutoffs required for quantization".into()))?
+            .as_standard_layout()
+            .to_owned();
+        let path = CString::new(index_path).map_err(|e| Error::IndexLoad(e.to_string()))?;
+        let mut c: *mut c_void = std::ptr::null_mut();
+        let st = unsafe {
+            pb_codec_open(pb_index_device(self.handle), cen.as_ptr(), cen.nrows() as i64, dim as i32, codec.nbits as i32,
+                          cut.as_ptr(), &mut c)
+        };
+        if st != 0 {
+            return Err(Error::Codec(last_error()));
+        }
+        let mut first = 0i64;
+        let st = unsafe {
+            pb_index_append(self.handle, c, flat.as_ptr(), lens.as_ptr(), lens.len() as i64, 0, path.as_ptr(),
+                            batch_size as i64, &mut first)
+        };
+        unsafe { pb_codec_close(c) };
+        if st != 0 {
+            return Err(Error::IndexLoad(last_error()));
+        }
+        Ok((first..first + lens.len() as i64).collect())
     }
 
     /// Body of `MmapIndex::search` (index.rs:1258).
