@@ -153,6 +153,32 @@ PB_API pb_status pb_index_append_encoded(pb_index *ix, const int64_t *codes, con
  * new array at the same time (PB_ERR_NOMEM, nothing changed, when the device cannot hold both). */
 PB_API pb_status pb_index_reserve(pb_index *ix, int64_t num_documents, int64_t num_embeddings);
 
+/* ---- incremental delete ------------------------------------------------------------------ */
+
+/* MmapIndex::delete_with_options (index.rs:1805) -> delete::delete_from_index (delete.rs:43), then the caller's reload
+ * (index.rs:1767), on a live handle.  Removes the documents `doc_ids` (host memory; the ids search returns, i.e.
+ * doc_id_base + local id) and leaves the handle exactly as pb_index_open on the remaining documents would: the
+ * survivors keep their order and are renumbered, a survivor's new local id being its old one minus the number of
+ * deleted ids below it (delete.rs:224-226).  Ids outside the handle's range, negative ids and repeated ids are ignored;
+ * out_deleted (may be NULL) receives the number of distinct documents removed (delete.rs:89-113).  Centroids and every
+ * centroid-derived operand are unchanged; device capacity is kept, so a following append reuses the freed space.
+ * Deleting every document leaves a valid empty handle (searches return nothing, appends work).  index_dir != NULL also
+ * applies delete_from_index's file changes (per-chunk codes / residuals / doclens / chunk metadata, ivf.npy,
+ * ivf_lengths.npy, metadata.json, removal of the merged_* caches, filtering of embeddings.npy and buffer.npy).
+ * Searches from other threads wait for the delete and see the index entirely before or after it.  Every check,
+ * allocation, the new inverted file and the directory's files come before the first in-place write to the handle's
+ * arrays; after that point only a CUDA runtime error can fail the call.  So on any other error neither the handle nor
+ * the directory changes.  A delete that removes no document changes nothing, on the device or on disk.
+ * PB_ERR_UNSUPPORTED, nothing changed: doc-sharded handles (pb_index_comm_init, pb_index_group_join), handles opened
+ * with PB_OPEN_ADOPT_RESIDUALS, and index_dir with doc_id_base != 0.  PB_ERR_INVALID, nothing changed: a directory
+ * whose metadata.json num_documents differs from the handle's. */
+PB_API pb_status pb_index_delete(pb_index *ix, const int64_t *doc_ids, int64_t n_ids, const char *index_dir,
+                                 int64_t *out_deleted);
+/* Device time of the last pb_index_delete on this handle, with pb_set_profiling(ix, 1): out_ms[0] the in-place
+ * compaction of the per-token and per-doc arrays, out_ms[1] the inverted-file kernels, out_ms[2] the norm pass
+ * (1 / |c + w|, vmin, wmax) over the remaining tokens. */
+PB_API pb_status pb_last_delete_ms(pb_index *ix, float *out_ms);
+
 /* ---- search ------------------------------------------------------------------------------ */
 
 /*

@@ -258,29 +258,74 @@ extern "C" pb_status pb_create_index(const float *embeddings, const int64_t *doc
     return st;
 }
 
-pb_status pb_dir_append(const char *index_dir, long long old_D, long long K, int dim, int nbits, long long batch_size,
-                        const int64_t *codes, const uint8_t *residuals, const int64_t *doc_lengths, long long n_docs,
-                        const int64_t *ivf, long long ivf_total, const int32_t *ivf_lengths) {
-    const std::string dir = std::string(index_dir) + "/";
-    const long long packed = (long long)dim * nbits / 8;
-    // Metadata::load_from_path (index.rs:131-155): num_documents 0 or absent is inferred from the doclens files
+// Metadata::load_from_path (index.rs:131-155) of a directory that must hold the handle's old_D documents and nbits:
+// num_documents 0 or absent is inferred from the doclens files
+static pb_status read_dir_meta(const std::string &dir, int nbits, long long old_D, long long &num_chunks, long long &num_emb,
+                               double &avg_doclen) {
     std::string meta;
     if (pb_status s = pb_read_text(dir + "metadata.json", meta)) return s;
-    double num_chunks = 0, mnbits = 0, num_emb = 0, avg_doclen = 0, num_docs = 0;
-    if (!pb_json_number(meta, "num_chunks", num_chunks) || !pb_json_number(meta, "nbits", mnbits) ||
-        !pb_json_number(meta, "num_embeddings", num_emb) || !pb_json_number(meta, "avg_doclen", avg_doclen))
+    double nc = 0, mnbits = 0, ne = 0, num_docs = 0;
+    if (!pb_json_number(meta, "num_chunks", nc) || !pb_json_number(meta, "nbits", mnbits) ||
+        !pb_json_number(meta, "num_embeddings", ne) || !pb_json_number(meta, "avg_doclen", avg_doclen))
         return pb_fail(PB_ERR_IO, "metadata.json lacks num_chunks / nbits / num_embeddings / avg_doclen");
-    const long long n_chunks_old = (long long)num_chunks, old_N = (long long)num_emb;
+    num_chunks = (long long)nc;
+    num_emb = (long long)ne;
     pb_json_number(meta, "num_documents", num_docs);
     long long meta_D = (long long)num_docs;
     if (meta_D == 0) {
         std::vector<int64_t> all;
-        for (long long c = 0; c < n_chunks_old; ++c) pb_read_doclens(dir + "doclens." + std::to_string(c) + ".json", all);
+        for (long long c = 0; c < num_chunks; ++c) pb_read_doclens(dir + "doclens." + std::to_string(c) + ".json", all);
         meta_D = (long long)all.size();
     }
     if ((int)mnbits != nbits) return pb_fail(PB_ERR_INVALID, "metadata.json nbits %d, the index has %d", (int)mnbits, nbits);
     if (meta_D != old_D)
         return pb_fail(PB_ERR_INVALID, "metadata.json num_documents %lld, the handle holds %lld documents", meta_D, old_D);
+    return PB_OK;
+}
+
+// ivf.npy / ivf_lengths.npy
+static pb_status write_ivf(const std::string &dir, long long K, const int64_t *ivf, long long ivf_total,
+                           const int32_t *ivf_lengths) {
+    pb_status s = atomic_write(dir + "ivf.npy", [&](const std::string &p) {
+        return write_npy(p, "<i8", {ivf_total}, ivf, (size_t)ivf_total * 8);
+    });
+    if (!s) s = atomic_write(dir + "ivf_lengths.npy", [&](const std::string &p) {
+        return write_npy(p, "<i4", {K}, ivf_lengths, (size_t)K * 4);
+    });
+    return s;
+}
+
+// metadata.json (struct Metadata, index.rs:105-127), then clear_merged_files (mmap.rs:1714-1740): the merged caches no
+// longer match the chunks
+static pb_status write_meta_clear_merged(const std::string &dir, long long num_chunks, int nbits, long long K, long long N,
+                                         double avg_doclen, long long D, int dim) {
+    char m[512];
+    snprintf(m, sizeof m,
+             "{\n  \"num_chunks\": %lld,\n  \"nbits\": %d,\n  \"num_partitions\": %lld,\n  \"num_embeddings\": %lld,\n"
+             "  \"avg_doclen\": %.17g,\n  \"num_documents\": %lld,\n  \"embedding_dim\": %d,\n  \"next_plaid_compatible\": true\n}",
+             num_chunks, nbits, K, N, avg_doclen, D, dim);
+    if (pb_status s = atomic_write(dir + "metadata.json", [&](const std::string &p) { return write_text(p, m); })) return s;
+    for (const char *f : {"merged_codes.npy", "merged_codes.npy.tmp", "merged_codes.manifest.json", "merged_codes.manifest.json.tmp",
+                          "merged_residuals.npy", "merged_residuals.npy.tmp", "merged_residuals.manifest.json",
+                          "merged_residuals.manifest.json.tmp"})
+        if (remove((dir + f).c_str()) != 0 && errno != ENOENT) return pb_fail(PB_ERR_IO, "cannot remove %s%s", dir.c_str(), f);
+    return PB_OK;
+}
+
+static std::string json_list(const std::vector<int64_t> &v) {
+    std::string s = "[";
+    for (size_t i = 0; i < v.size(); ++i) s += std::to_string((long long)v[i]) + (i + 1 < v.size() ? "," : "");
+    return s + "]";
+}
+
+pb_status pb_dir_append(const char *index_dir, long long old_D, long long K, int dim, int nbits, long long batch_size,
+                        const int64_t *codes, const uint8_t *residuals, const int64_t *doc_lengths, long long n_docs,
+                        const int64_t *ivf, long long ivf_total, const int32_t *ivf_lengths) {
+    const std::string dir = std::string(index_dir) + "/";
+    const long long packed = (long long)dim * nbits / 8;
+    long long n_chunks_old = 0, old_N = 0;
+    double avg_doclen = 0;
+    if (pb_status s = read_dir_meta(dir, nbits, old_D, n_chunks_old, old_N, avg_doclen)) return s;
 
     // a last chunk with < 2000 docs takes the first new batch (update.rs:799-827)
     long long start = n_chunks_old, emb_off = old_N;
@@ -329,9 +374,7 @@ pb_status pb_dir_append(const char *index_dir, long long old_D, long long K, int
         if (!s) s = atomic_write(dir + ci + ".residuals.npy", [&](const std::string &p) {
             return write_npy(p, "|u1", {ctok, packed}, cres.data(), cres.size());
         });
-        std::string dl = "[";
-        for (size_t d = 0; d < cdl.size(); ++d) dl += std::to_string((long long)cdl[d]) + (d + 1 < cdl.size() ? "," : "");
-        dl += "]";
+        const std::string dl = json_list(cdl);
         if (!s) s = atomic_write(old_dl, [&](const std::string &p) { return write_text(p, dl); });
         char cm[256];
         snprintf(cm, sizeof cm, "{\n  \"num_documents\": %lld,\n  \"num_embeddings\": %lld,\n  \"embedding_offset\": %lld\n}",
@@ -340,26 +383,122 @@ pb_status pb_dir_append(const char *index_dir, long long old_D, long long K, int
         if (!s) s = atomic_write(dir + ci + ".metadata.json", [&](const std::string &p) { return write_text(p, cm); });
         if (s) return s;
     }
-    pb_status s = atomic_write(dir + "ivf.npy", [&](const std::string &p) {
-        return write_npy(p, "<i8", {ivf_total}, ivf, (size_t)ivf_total * 8);
-    });
-    if (!s) s = atomic_write(dir + "ivf_lengths.npy", [&](const std::string &p) {
-        return write_npy(p, "<i4", {K}, ivf_lengths, (size_t)K * 4);
-    });
-    if (s) return s;
+    if (pb_status s = write_ivf(dir, K, ivf, ivf_total, ivf_lengths)) return s;
     // update.rs:1085-1110: avg_doclen from the file's old value, not N / D
     const long long total_D = old_D + n_docs;
     const double new_avg = total_D > 0 ? (avg_doclen * (double)old_D + (double)tok) / (double)total_D : 0.0;
-    char m[512];  // struct Metadata, index.rs:105-127
-    snprintf(m, sizeof m,
-             "{\n  \"num_chunks\": %lld,\n  \"nbits\": %d,\n  \"num_partitions\": %lld,\n  \"num_embeddings\": %lld,\n"
-             "  \"avg_doclen\": %.17g,\n  \"num_documents\": %lld,\n  \"embedding_dim\": %d,\n  \"next_plaid_compatible\": true\n}",
-             start + n_new_chunks, nbits, K, old_N + tok, new_avg, total_D, dim);
-    if (pb_status s2 = atomic_write(dir + "metadata.json", [&](const std::string &p) { return write_text(p, m); })) return s2;
-    // clear_merged_files (mmap.rs:1714-1740): the merged caches no longer match the chunks
-    for (const char *f : {"merged_codes.npy", "merged_codes.npy.tmp", "merged_codes.manifest.json", "merged_codes.manifest.json.tmp",
-                          "merged_residuals.npy", "merged_residuals.npy.tmp", "merged_residuals.manifest.json",
-                          "merged_residuals.manifest.json.tmp"})
-        if (remove((dir + f).c_str()) != 0 && errno != ENOENT) return pb_fail(PB_ERR_IO, "cannot remove %s%s", dir.c_str(), f);
-    return PB_OK;
+    return write_meta_clear_merged(dir, start + n_new_chunks, nbits, K, old_N + tok, new_avg, total_D, dim);
+}
+
+// clean_embeddings_files (delete.rs:286-398) for one file pair: the rows of the documents that survive, doc i of the
+// lengths file being doc id first + i; the files are removed when no document survives.  `info` (buffer_info.json) is
+// rewritten or removed with them.
+template <class Deleted>
+static pb_status clean_embeddings_file(const std::string &dir, const char *npy, const char *lengths, const char *info,
+                                       long long first_from_end, Deleted deleted) {
+    const std::string ep = dir + npy, lp = dir + lengths;
+    if (access(ep.c_str(), F_OK) != 0 || access(lp.c_str(), F_OK) != 0) return PB_OK;
+    long long rows = 0, cols = 0;
+    std::vector<float> flat, out;
+    std::vector<int64_t> lens, kept;
+    if (pb_status s = pb_read_npy_f32(ep, rows, cols, flat)) return s;
+    if (pb_status s = pb_read_doclens(lp, lens)) return s;
+    // embeddings.npy holds docs 0.., buffer.npy the last len(buffer_lengths) docs of the index before the delete
+    const long long first = first_from_end < 0 ? 0 : first_from_end - (long long)lens.size();
+    long long off = 0;
+    for (size_t i = 0; i < lens.size(); ++i) {
+        if (!deleted(first + (long long)i)) {
+            for (long long r = off; r < off + lens[i] && r < rows; ++r) out.insert(out.end(), flat.begin() + r * cols, flat.begin() + (r + 1) * cols);
+            kept.push_back(lens[i]);
+        }
+        off += lens[i];
+    }
+    if (kept.empty()) {
+        remove(ep.c_str());
+        remove(lp.c_str());
+        if (info) remove((dir + info).c_str());
+        return PB_OK;
+    }
+    const long long n_rows = cols ? (long long)out.size() / cols : 0;
+    pb_status s = atomic_write(ep, [&](const std::string &p) { return write_npy(p, "<f4", {n_rows, cols}, out.data(), out.size() * 4); });
+    const std::string lt = json_list(kept);
+    if (!s) s = atomic_write(lp, [&](const std::string &p) { return write_text(p, lt); });
+    const std::string it = "{\"num_docs\":" + std::to_string(kept.size()) + "}";
+    if (!s && info) s = atomic_write(dir + info, [&](const std::string &p) { return write_text(p, it); });
+    return s;
+}
+
+pb_status pb_dir_delete(const char *index_dir, long long old_D, long long K, int dim, int nbits, const uint32_t *deleted,
+                        const int64_t *ivf, long long ivf_total, const int32_t *ivf_lengths) {
+    const std::string dir = std::string(index_dir) + "/";
+    const long long packed = (long long)dim * nbits / 8;
+    long long n_chunks = 0, old_N = 0;
+    double avg_doclen = 0;
+    if (pb_status s = read_dir_meta(dir, nbits, old_D, n_chunks, old_N, avg_doclen)) return s;
+    auto is_del = [&](long long d) { return d >= 0 && d < old_D && ((deleted[d >> 5] >> (d & 31)) & 1u); };
+    // every chunk's doc lengths before the first write
+    std::vector<std::vector<int64_t>> dls((size_t)n_chunks);
+    long long total = 0;
+    for (long long c = 0; c < n_chunks; ++c) {
+        if (pb_status s = pb_read_doclens(dir + "doclens." + std::to_string(c) + ".json", dls[(size_t)c])) return s;
+        total += (long long)dls[(size_t)c].size();
+    }
+    if (total != old_D)
+        return pb_fail(PB_ERR_INVALID, "the doclens files hold %lld documents, the handle %lld", total, old_D);
+
+    // per chunk (delete.rs:92-185): only chunks with a deleted doc are rewritten; num_chunks stays, embedding_offset too
+    long long doc0 = 0, D1 = 0, N1 = 0;
+    for (long long c = 0; c < n_chunks; ++c) {
+        const std::vector<int64_t> &dl = dls[(size_t)c];
+        std::vector<int64_t> ndl;
+        long long ctok = 0;
+        for (size_t i = 0; i < dl.size(); ++i) {
+            ctok += dl[i];
+            if (!is_del(doc0 + (long long)i)) {
+                ndl.push_back(dl[i]);
+                N1 += dl[i];
+            }
+        }
+        D1 += (long long)ndl.size();
+        if (ndl.size() < dl.size()) {
+            const std::string ci = std::to_string(c);
+            std::vector<int64_t> codes, ncodes;
+            std::vector<uint8_t> res, nres;
+            if (pb_status s = pb_read_chunk(dir, c, ctok, packed, codes, res)) return s;
+            std::string cm;
+            if (pb_status s = pb_read_text(dir + ci + ".metadata.json", cm)) return s;
+            long long t = 0;
+            for (size_t i = 0; i < dl.size(); ++i) {
+                if (!is_del(doc0 + (long long)i)) {
+                    ncodes.insert(ncodes.end(), codes.begin() + t, codes.begin() + t + dl[i]);
+                    nres.insert(nres.end(), res.begin() + t * packed, res.begin() + (t + dl[i]) * packed);
+                }
+                t += dl[i];
+            }
+            const long long nt = (long long)ncodes.size();
+            pb_status s = atomic_write(dir + ci + ".codes.npy", [&](const std::string &p) {
+                return write_npy(p, "<i8", {nt}, ncodes.data(), (size_t)nt * 8);
+            });
+            if (!s) s = atomic_write(dir + ci + ".residuals.npy", [&](const std::string &p) {
+                return write_npy(p, "|u1", {nt, packed}, nres.data(), nres.size());
+            });
+            const std::string dtxt = json_list(ndl);
+            if (!s) s = atomic_write(dir + "doclens." + ci + ".json", [&](const std::string &p) { return write_text(p, dtxt); });
+            double eo = 0;
+            char m[256];
+            if (pb_json_number(cm, "embedding_offset", eo))
+                snprintf(m, sizeof m, "{\n  \"num_documents\": %lld,\n  \"num_embeddings\": %lld,\n  \"embedding_offset\": %lld\n}",
+                         (long long)ndl.size(), nt, (long long)eo);
+            else snprintf(m, sizeof m, "{\n  \"num_documents\": %lld,\n  \"num_embeddings\": %lld\n}", (long long)ndl.size(), nt);
+            if (!s) s = atomic_write(dir + ci + ".metadata.json", [&](const std::string &p) { return write_text(p, m); });
+            if (s) return s;
+        }
+        doc0 += (long long)dl.size();
+    }
+    if (pb_status s = write_ivf(dir, K, ivf, ivf_total, ivf_lengths)) return s;
+    // delete.rs:240-260: avg_doclen = N / D of what is left (not the append's incremental formula)
+    const double avg = D1 > 0 ? (double)N1 / (double)D1 : 0.0;
+    if (pb_status s = write_meta_clear_merged(dir, n_chunks, nbits, K, N1, avg, D1, dim)) return s;
+    if (pb_status s = clean_embeddings_file(dir, "embeddings.npy", "embeddings_lengths.json", nullptr, -1, is_del)) return s;
+    return clean_embeddings_file(dir, "buffer.npy", "buffer_lengths.json", "buffer_info.json", old_D, is_del);
 }

@@ -6,6 +6,8 @@
 #include "kernels.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_reduce.cuh>
+#include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
 
 #include <algorithm>
@@ -13,6 +15,7 @@
 #include <cmath>
 #include <condition_variable>
 #include <functional>
+#include <map>
 #include <thread>
 #include <cstdarg>
 #include <cstdio>
@@ -397,6 +400,8 @@ struct pb_index {
     std::mutex mu;
     std::vector<std::unique_ptr<Workspace>> pool;
     DevBuf ivf_spare, ivf_off_spare;  // the other half of the inverted file's ping-pong: pb_index_append merges into it
+    float delete_ms[3] = {0.f, 0.f, 0.f};  // last pb_index_delete with profiling on: compaction, inverted file, norms
+    long long delete_window = 1ll << 22;   // tokens per compaction window of pb_index_delete (PB_DELETE_WINDOW_TOKENS)
     // Readers (searches, stage entry points, accessors) share the arrays; pb_index_append / pb_index_reserve hold them
     // alone.  A writer also holds `gate`, which every reader passes first: pthread rwlocks prefer readers, so without
     // it a steady stream of searches could keep an append waiting forever.
@@ -454,8 +459,20 @@ static size_t smem_exact(int dim, int packed) {
 }
 
 template <class Kern> static pb_status set_smem(Kern k, size_t bytes) {
-    // a kernel's static shared memory counts towards the 48 KB a launch may use without opting in
-    if (bytes > 40 * 1024) CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    // a kernel's static shared memory counts towards the 48 KB a launch may use without opting in.  The opt-in only
+    // grows: lanes launch one kernel with different sizes from several threads, and a smaller value set between another
+    // lane's setting and its launch would fail that launch
+    if (bytes <= 40 * 1024) return PB_OK;
+    static std::mutex mu;
+    static std::map<std::pair<int, const void *>, size_t> opted;
+    int dev = 0;
+    CK(cudaGetDevice(&dev));
+    std::lock_guard<std::mutex> g(mu);
+    size_t &cur = opted[{dev, (const void *)k}];
+    if (bytes > cur) {
+        CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+        cur = bytes;
+    }
     return PB_OK;
 }
 
@@ -564,6 +581,7 @@ pb_status pb_index_open_begin(const pb_index_desc *d, pb_index **out) {
             long v = atol(e);
             if (v > 0) ix->st_budget = (size_t)v << 20;
         }
+    if (const char *e = getenv("PB_DELETE_WINDOW_TOKENS")) ix->delete_window = std::max(1ll, atoll(e));
     const int sp = d->memory_space;
     // doc offsets (index.rs:1107-1110)
     std::vector<int64_t> dl;
@@ -3112,5 +3130,218 @@ extern "C" pb_status pb_index_reserve(pb_index *ix, int64_t num_documents, int64
     CKS(ix->ucodes.grow((size_t)U1 * 4, (size_t)ix->n_ucodes * 4, false));
     CKS(ix->ivf.grow((size_t)L1 * 4, (size_t)ix->ivf_len * 4, false));
     CKS(ix->ivf_spare.grow((size_t)L1 * 4, 0, false));
+    return PB_OK;
+}
+
+// ------------------------------------------------------------------------------------------
+// incremental delete: MmapIndex::delete_with_options (index.rs:1805) -> delete_from_index (delete.rs:43) + reload on a
+// live handle
+// ------------------------------------------------------------------------------------------
+// out[i] = in[0] + .. + in[i - 1] for i < n
+static pb_status exclusive_sum(const long long *in, long long *out, long long n, DevBuf &tmp) {
+    size_t tb = 0;
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, in, out, n));
+    CKS(tmp.ensure(tb + 16));
+    CK(cub::DeviceScan::ExclusiveSum(tmp.p, tb, in, out, n));
+    return PB_OK;
+}
+
+struct Events {
+    cudaEvent_t e[5] = {};
+    ~Events() {
+        for (cudaEvent_t x : e)
+            if (x) cudaEventDestroy(x);
+    }
+};
+
+extern "C" pb_status pb_index_delete(pb_index *ix, const int64_t *doc_ids, int64_t n_ids, const char *index_dir,
+                                     int64_t *out_deleted) {
+    if (!ix || (!doc_ids && n_ids) || n_ids < 0) return pb_fail(PB_ERR_INVALID, "null argument");
+    if (out_deleted) *out_deleted = 0;
+    std::lock_guard<std::mutex> gate(ix->gate);
+    std::unique_lock<std::shared_mutex> wr(ix->rw);
+    if (ix->comm || ix->group) return pb_fail(PB_ERR_UNSUPPORTED, "deletes from a doc-sharded handle are not supported");
+    if (!ix->residuals.owned)
+        return pb_fail(PB_ERR_UNSUPPORTED, "the handle uses the caller's residual array (PB_OPEN_ADOPT_RESIDUALS)");
+    if (index_dir && ix->doc_id_base != 0) return pb_fail(PB_ERR_UNSUPPORTED, "an index directory holds doc ids from 0");
+    CK(cudaSetDevice(ix->device));
+    CK(cudaDeviceSynchronize());  // work earlier readers left queued (pb_search_batch_device) reads the arrays
+    const long long D0 = ix->D, K = ix->K, nw = (D0 + 31) / 32;
+    const int grid = ix->sm_count * 8;
+    const bool prof = ix->profiling;
+    Events ev;
+    if (prof)
+        for (cudaEvent_t &x : ev.e) CK(cudaEventCreate(&x));
+
+    // 1. the deleted set: one bit per doc, its per-word prefix counts, and the number of docs deleted
+    DevBuf bits, wcnt, wpre, tmp;
+    CKS(bits.ensure(std::max<size_t>((size_t)nw * 4, 16)));
+    CK(cudaMemset(bits.p, 0, (size_t)nw * 4));
+    if (n_ids > 0 && D0 > 0) {
+        const long long slab = 1ll << 20;
+        DevBuf dids;
+        CKS(dids.ensure((size_t)std::min<long long>(n_ids, slab) * 8));
+        for (long long o = 0; o < n_ids; o += slab) {
+            const long long m = std::min(slab, n_ids - o);
+            CK(cudaMemcpy(dids.p, doc_ids + o, (size_t)m * 8, cudaMemcpyHostToDevice));
+            k_del_mark<<<grid, 256>>>(dids.as<long long>(), m, ix->doc_id_base, D0, bits.as<uint32_t>());
+            CK(cudaGetLastError());
+        }
+    }
+    CKS(wcnt.ensure((size_t)(nw + 1) * 8));
+    CKS(wpre.ensure((size_t)(nw + 1) * 8));
+    k_del_popc<<<grid, 256>>>(bits.as<uint32_t>(), nw, wcnt.as<long long>());
+    CK(cudaGetLastError());
+    CKS(exclusive_sum(wcnt.as<long long>(), wpre.as<long long>(), nw + 1, tmp));
+    long long n_del = 0;
+    CK(cudaMemcpy(&n_del, wpre.as<long long>() + nw, 8, cudaMemcpyDeviceToHost));
+    if (n_del == 0) return PB_OK;
+    const long long D1 = D0 - n_del;
+
+    // 2. the survivors kept[j] and their new doc_off / udoc_off, into scratch: the old ones are read until the commit
+    DevBuf kept, tlen, ulen, new_doff, new_uoff;
+    CKS(kept.ensure((size_t)std::max(D1, 1ll) * 8));
+    CKS(tlen.ensure((size_t)(D1 + 1) * 8));
+    CKS(ulen.ensure((size_t)(D1 + 1) * 8));
+    CKS(new_doff.ensure((size_t)(D1 + 1) * 8));
+    CKS(new_uoff.ensure((size_t)(D1 + 1) * 8));
+    CK(cudaMemset(tlen.as<long long>() + D1, 0, 8));
+    CK(cudaMemset(ulen.as<long long>() + D1, 0, 8));
+    k_del_kept<<<grid, 256>>>(bits.as<uint32_t>(), wpre.as<long long>(), D0, ix->doc_off.as<long long>(),
+                              ix->udoc_off.as<long long>(), kept.as<long long>(), tlen.as<long long>(), ulen.as<long long>());
+    CK(cudaGetLastError());
+    CKS(exclusive_sum(tlen.as<long long>(), new_doff.as<long long>(), D1 + 1, tmp));
+    CKS(exclusive_sum(ulen.as<long long>(), new_uoff.as<long long>(), D1 + 1, tmp));
+    std::vector<long long> hoff((size_t)D1 + 1), hu((size_t)D1 + 1);
+    CK(cudaMemcpy(hoff.data(), new_doff.p, hoff.size() * 8, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(hu.data(), new_uoff.p, hu.size() * 8, cudaMemcpyDeviceToHost));
+    const long long N1 = hoff[D1], U1 = hu[D1];
+    int maxlen = 0;
+    for (long long j = 0; j < D1; ++j) maxlen = std::max<int>(maxlen, (int)(hoff[j + 1] - hoff[j]));
+
+    // 3. the inverted file without the deleted ids, renumbered, into the spare half
+    if (prof) CK(cudaEventRecord(ev.e[0]));
+    DevBuf icnt;
+    CKS(icnt.ensure((size_t)(K + 1) * 8));
+    CKS(ix->ivf_off_spare.ensure((size_t)(K + 1) * 8));
+    k_ivf_delete_count<<<grid, 256>>>(ix->ivf.as<uint32_t>(), ix->ivf_off.as<long long>(), K, bits.as<uint32_t>(),
+                                      icnt.as<long long>());
+    CK(cudaGetLastError());
+    CKS(exclusive_sum(icnt.as<long long>(), ix->ivf_off_spare.as<long long>(), K + 1, tmp));
+    long long L1 = 0;
+    CK(cudaMemcpy(&L1, ix->ivf_off_spare.as<long long>() + K, 8, cudaMemcpyDeviceToHost));
+    CKS(ix->ivf_spare.grow(std::max<size_t>((size_t)L1 * 4, 16), 0));
+    k_ivf_delete_write<<<grid, 256>>>(ix->ivf.as<uint32_t>(), ix->ivf_off.as<long long>(), K, bits.as<uint32_t>(),
+                                      wpre.as<long long>(), ix->ivf_off_spare.as<long long>(), ix->ivf_spare.as<uint32_t>());
+    CK(cudaGetLastError());
+    if (prof) CK(cudaEventRecord(ev.e[1]));
+
+    // 4. compaction windows over the survivors that move: those from the first deleted doc on (survivors before it keep
+    // their rows; a delete of the newest docs moves nothing).  Each window is a run of survivors whose rows fit
+    // delete_window tokens (a longer doc is a window of its own).
+    std::vector<uint32_t> hbits((size_t)nw);
+    CK(cudaMemcpy(hbits.data(), bits.p, (size_t)nw * 4, cudaMemcpyDeviceToHost));
+    long long first = 0;
+    while (hbits[(size_t)(first >> 5)] == 0) first += 32;
+    first += __builtin_ctz(hbits[(size_t)(first >> 5)]);
+    std::vector<std::pair<long long, long long>> wins;
+    long long max_tok = 0, max_u = 0;
+    for (long long j0 = first, j1; j0 < D1; j0 = j1) {
+        for (j1 = j0 + 1; j1 < D1 && hoff[j1 + 1] - hoff[j0] <= ix->delete_window; ++j1) {}
+        wins.emplace_back(j0, j1);
+        max_tok = std::max(max_tok, hoff[j1] - hoff[j0]);
+        max_u = std::max(max_u, hu[j1] - hu[j0]);
+    }
+    const size_t pk = (size_t)ix->packed;
+    DevBuf st_codes, st_res, st_u;
+    if (!wins.empty()) {
+        CKS(st_codes.ensure(std::max<size_t>((size_t)max_tok * 4, 16)));
+        CKS(st_res.ensure(std::max<size_t>((size_t)max_tok * pk, 16)));
+        CKS(st_u.ensure(std::max<size_t>((size_t)max_u * 4, 16)));
+    }
+    DevBuf mn;
+    CKS(mn.ensure(16));
+    CK(cudaDeviceSynchronize());
+
+    // delete_from_index's file changes, before the first in-place write: a failure leaves the handle as it was
+    if (index_dir) {
+        std::vector<int64_t> hivf((size_t)std::max(L1, 1ll));
+        std::vector<int32_t> hlen((size_t)K);
+        DevBuf di, dln;
+        CKS(di.ensure(std::max<size_t>((size_t)L1 * 8, 16)));
+        CKS(dln.ensure((size_t)K * 4));
+        k_ivf_export<<<grid, 256>>>(ix->ivf_spare.as<uint32_t>(), ix->ivf_off_spare.as<long long>(), L1, K, 0,
+                                    di.as<long long>(), dln.as<int>());
+        CK(cudaGetLastError());
+        if (L1) CK(cudaMemcpy(hivf.data(), di.p, (size_t)L1 * 8, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(hlen.data(), dln.p, (size_t)K * 4, cudaMemcpyDeviceToHost));
+        CKS(pb_dir_delete(index_dir, D0, K, ix->dim, ix->nbits, hbits.data(), hivf.data(), L1, hlen.data()));
+    }
+
+    // 5. in place from here on: only a CUDA runtime error can fail the call
+    if (prof) CK(cudaEventRecord(ev.e[2]));
+    for (const auto &w : wins) {
+        const long long j0 = w.first, j1 = w.second;
+        const unsigned blocks = (unsigned)std::min<long long>((j1 - j0 + 7) / 8, grid);
+        const long long *kp = kept.as<long long>();
+        k_compact_gather<uint32_t><<<blocks, 256>>>(ix->codes.as<uint8_t>(), ix->doc_off.as<long long>(), kp,
+                                                    new_doff.as<long long>(), j0, j1, 4, st_codes.as<uint8_t>());
+        if (pk % 16 == 0)  // dim * nbits / 8 is a multiple of 4 for every supported dim
+            k_compact_gather<uint4><<<blocks, 256>>>(ix->residuals.as<uint8_t>(), ix->doc_off.as<long long>(), kp,
+                                                     new_doff.as<long long>(), j0, j1, (int)pk, st_res.as<uint8_t>());
+        else
+            k_compact_gather<uint32_t><<<blocks, 256>>>(ix->residuals.as<uint8_t>(), ix->doc_off.as<long long>(), kp,
+                                                        new_doff.as<long long>(), j0, j1, (int)pk, st_res.as<uint8_t>());
+        // distinct-code blocks start at multiples of 8 codes (32 bytes)
+        k_compact_gather<uint4><<<blocks, 256>>>(ix->ucodes.as<uint8_t>(), ix->udoc_off.as<long long>(), kp,
+                                                 new_uoff.as<long long>(), j0, j1, 4, st_u.as<uint8_t>());
+        CK(cudaGetLastError());
+        const long long nt = hoff[j1] - hoff[j0], nu = hu[j1] - hu[j0];
+        CK(cudaMemcpy(ix->codes.as<uint8_t>() + (size_t)hoff[j0] * 4, st_codes.p, (size_t)nt * 4, cudaMemcpyDeviceToDevice));
+        CK(cudaMemcpy(ix->residuals.as<uint8_t>() + (size_t)hoff[j0] * pk, st_res.p, (size_t)nt * pk, cudaMemcpyDeviceToDevice));
+        CK(cudaMemcpy(ix->ucodes.as<uint8_t>() + (size_t)hu[j0] * 4, st_u.p, (size_t)nu * 4, cudaMemcpyDeviceToDevice));
+    }
+    CK(cudaMemcpy(ix->doc_off.p, new_doff.p, (size_t)(D1 + 1) * 8, cudaMemcpyDeviceToDevice));
+    CK(cudaMemcpy(ix->udoc_off.p, new_uoff.p, (size_t)(D1 + 1) * 8, cudaMemcpyDeviceToDevice));
+    if (prof) CK(cudaEventRecord(ev.e[3]));
+
+    // 6. 1 / |c + w| of the survivors in their new order, and vmin / wmax over them as an open computes them: the old
+    // constants would still bound the error, but the work counters would differ from a fresh open
+    float vmin = 0.0f, wmax = 0.0f;
+    if (filter_dim(ix->dim) && N1 > 0) {
+        const float init[2] = {3.0e38f, 0.0f};
+        CK(cudaMemcpy(mn.p, init, 8, cudaMemcpyHostToDevice));
+        CKS(launch_min_vnorm(ix, 0, N1, mn.as<float>()));
+        float got[2] = {0.f, 0.f};
+        CK(cudaMemcpy(got, mn.p, 8, cudaMemcpyDeviceToHost));
+        vmin = got[0] < 1e30f ? got[0] : 0.0f;
+        wmax = got[1];
+    }
+    if (prof) CK(cudaEventRecord(ev.e[4]));
+    CK(cudaDeviceSynchronize());
+
+    // 7. commit
+    ix->ivf.swap(ix->ivf_spare);
+    ix->ivf_off.swap(ix->ivf_off_spare);
+    ix->ivf_len = L1;
+    ix->n_ucodes = U1;
+    ix->N = N1;
+    ix->D = D1;
+    ix->max_doclen = maxlen;
+    ix->vmin = vmin;
+    ix->wmax = wmax;
+    if (prof) {
+        CK(cudaEventElapsedTime(&ix->delete_ms[0], ev.e[2], ev.e[3]));
+        CK(cudaEventElapsedTime(&ix->delete_ms[1], ev.e[0], ev.e[1]));
+        CK(cudaEventElapsedTime(&ix->delete_ms[2], ev.e[3], ev.e[4]));
+    }
+    if (out_deleted) *out_deleted = n_del;
+    return PB_OK;
+}
+
+extern "C" pb_status pb_last_delete_ms(pb_index *ix, float *out_ms) {
+    if (!ix || !out_ms) return pb_fail(PB_ERR_INVALID, "null argument");
+    auto rd = ix->read_lock();
+    memcpy(out_ms, ix->delete_ms, sizeof ix->delete_ms);
     return PB_OK;
 }

@@ -20,6 +20,8 @@ bool pb_json_number(const std::string &j, const char *key, double &out);
 pb_status pb_read_doclens(const std::string &path, std::vector<int64_t> &out);
 pb_status pb_read_chunk(const std::string &dir, long long chunk, long long n_tokens, long long packed,
                         std::vector<int64_t> &codes, std::vector<uint8_t> &residuals);
+// a 2-D <f4 NPY file (embeddings.npy, buffer.npy)
+pb_status pb_read_npy_f32(const std::string &path, long long &rows, long long &cols, std::vector<float> &out);
 
 // update_index's file changes (update.rs:794-1117, update_threshold = false) for n_docs documents appended to the
 // index in index_dir, which holds old_D documents: chunk files in batches of batch_size docs (the first merged into a
@@ -27,4 +29,11 @@ pb_status pb_read_chunk(const std::string &dir, long long chunk, long long n_tok
 // the merged_* caches.  codes i64 [sum doc_lengths], residuals packed [sum doc_lengths][dim*nbits/8].
 pb_status pb_dir_append(const char *index_dir, long long old_D, long long K, int dim, int nbits, long long batch_size,
                         const int64_t *codes, const uint8_t *residuals, const int64_t *doc_lengths, long long n_docs,
+                        const int64_t *ivf, long long ivf_total, const int32_t *ivf_lengths);
+
+// delete_from_index's file changes (delete.rs:66-273) for the documents whose bit is set in `deleted` (one bit per doc
+// of the old_D the directory holds): filtered chunk files and chunk metadata for every chunk with a deleted doc, the
+// filtered inverted file ivf / ivf_lengths, metadata.json, removal of the merged_* caches, and the filtering of
+// embeddings.npy / buffer.npy (clean_embeddings_files, delete.rs:286-398).
+pb_status pb_dir_delete(const char *index_dir, long long old_D, long long K, int dim, int nbits, const uint32_t *deleted,
                         const int64_t *ivf, long long ivf_total, const int32_t *ivf_lengths);

@@ -633,6 +633,111 @@ __global__ void k_words_differ(const uint32_t *__restrict__ a, const uint32_t *_
     if (__syncthreads_or(d) && threadIdx.x == 0) *flag = 1;
 }
 
+// ------------------------------------------------------------------------------------------
+// Incremental delete (pb_index_delete, delete.rs:43-273).  The deleted docs are one bit each in `bits` [ceil(D/32)];
+// word_pre[w] = deleted docs in words < w (exclusive scan of the per-word popcounts).  rank(d), the number of deleted
+// docs below d, is word_pre[d / 32] + the popcount of the bits below d in its word; a survivor's new id is d - rank(d)
+// (delete.rs:224-226), so the survivors keep their order.
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool del_bit(const uint32_t *__restrict__ bits, uint32_t d) { return (bits[d >> 5] >> (d & 31)) & 1u; }
+__device__ __forceinline__ long long del_rank(const uint32_t *__restrict__ bits, const long long *__restrict__ word_pre, uint32_t d) {
+    return word_pre[d >> 5] + __popc(bits[d >> 5] & ((1u << (d & 31)) - 1u));
+}
+
+// ids are global (doc_id_base + local); negative, out-of-range and repeated ids set no new bit
+__global__ void k_del_mark(const long long *__restrict__ ids, long long n, long long base, long long D, uint32_t *__restrict__ bits) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const long long id = ids[i];
+        if (id >= base && id - base < D) {
+            const long long d = id - base;
+            atomicOr(&bits[d >> 5], 1u << (d & 31));
+        }
+    }
+}
+
+// cnt[w] = deleted docs in word w (w < nw), cnt[nw] = 0: scanned into word_pre[0..nw], word_pre[nw] = all deleted docs
+__global__ void k_del_popc(const uint32_t *__restrict__ bits, long long nw, long long *__restrict__ cnt) {
+    for (long long w = (long long)blockIdx.x * blockDim.x + threadIdx.x; w <= nw; w += (long long)gridDim.x * blockDim.x)
+        cnt[w] = w < nw ? __popc(bits[w]) : 0;
+}
+
+// survivor j = d - rank(d): kept[j] = d and its token / distinct-code counts, scanned into the new doc_off / udoc_off
+__global__ void k_del_kept(const uint32_t *__restrict__ bits, const long long *__restrict__ word_pre, long long D,
+                           const long long *__restrict__ doc_off, const long long *__restrict__ udoc_off,
+                           long long *__restrict__ kept, long long *__restrict__ tlen, long long *__restrict__ ulen) {
+    for (long long d = (long long)blockIdx.x * blockDim.x + threadIdx.x; d < D; d += (long long)gridDim.x * blockDim.x) {
+        if (del_bit(bits, (uint32_t)d)) continue;
+        const long long j = d - del_rank(bits, word_pre, (uint32_t)d);
+        kept[j] = d;
+        tlen[j] = doc_off[d + 1] - doc_off[d];
+        ulen[j] = udoc_off[d + 1] - udoc_off[d];
+    }
+}
+
+// Inverted file, delete.rs:196-237: each centroid's list without the deleted ids, survivors renumbered.  One warp per
+// centroid; cnt[c] = its survivors (cnt[K] = 0), scanned into the new offsets.
+__global__ void k_ivf_delete_count(const uint32_t *__restrict__ ivf, const long long *__restrict__ off, long long K,
+                                   const uint32_t *__restrict__ bits, long long *__restrict__ cnt) {
+    const int lane = threadIdx.x & 31;
+    const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
+    for (long long c = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c <= K; c += nw) {
+        if (c == K) {
+            if (lane == 0) cnt[K] = 0;
+            continue;
+        }
+        const long long o0 = off[c], n = off[c + 1] - o0;
+        long long kept = 0;
+        for (long long b = 0; b < n; b += 32) {
+            const long long i = b + lane;
+            kept += __popc(__ballot_sync(PB_FULL, i < n && !del_bit(bits, ivf[o0 + i])));
+        }
+        if (lane == 0) cnt[c] = kept;
+    }
+}
+
+// the survivors of centroid c, in order, at new_off[c]..: compacted with a ballot, written as id - rank(id)
+__global__ void k_ivf_delete_write(const uint32_t *__restrict__ ivf, const long long *__restrict__ off, long long K,
+                                   const uint32_t *__restrict__ bits, const long long *__restrict__ word_pre,
+                                   const long long *__restrict__ new_off, uint32_t *__restrict__ out) {
+    const int lane = threadIdx.x & 31;
+    const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
+    for (long long c = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c < K; c += nw) {
+        const long long o0 = off[c], n = off[c + 1] - o0;
+        long long dst = new_off[c];
+        for (long long b = 0; b < n; b += 32) {
+            const long long i = b + lane;
+            const uint32_t id = i < n ? ivf[o0 + i] : 0u;
+            const bool keep = i < n && !del_bit(bits, id);
+            const unsigned bal = __ballot_sync(PB_FULL, keep);
+            if (keep) out[dst + __popc(bal & ((1u << lane) - 1u))] = id - (uint32_t)del_rank(bits, word_pre, id);
+            dst += __popc(bal);
+        }
+    }
+}
+
+// In-place compaction of a per-token (or per-distinct-code) array, one window of survivors [j0, j1) at a time: survivor
+// j's rows old_off[kept[j]] .. old_off[kept[j] + 1] go to staging at new_off[j] - new_off[j0], and the caller then
+// copies the staging to new_off[j0].  One warp per doc, V-wide accesses (row_bytes * every offset is a multiple of
+// sizeof(V)).
+// Invariant: new_off[j] <= old_off[kept[j]] for every j (a survivor only moves down), so a window's writes end at
+// new_off[j1] <= old_off[kept[j1]], where the next window's reads begin: windows in ascending order never read rows an
+// earlier window overwrote, and the staging is never more than one window.
+template <class V>
+__global__ void k_compact_gather(const uint8_t *__restrict__ src, const long long *__restrict__ old_off,
+                                 const long long *__restrict__ kept, const long long *__restrict__ new_off, long long j0,
+                                 long long j1, int row_bytes, uint8_t *__restrict__ stage) {
+    const int lane = threadIdx.x & 31;
+    const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
+    const long long s0 = new_off[j0];
+    for (long long j = j0 + (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); j < j1; j += nw) {
+        const long long d = kept[j], o = old_off[d];
+        const long long nv = (old_off[d + 1] - o) * row_bytes / (long long)sizeof(V);
+        const V *in = reinterpret_cast<const V *>(src + o * row_bytes);
+        V *out = reinterpret_cast<V *>(stage + (new_off[j] - s0) * row_bytes);
+        for (long long k = lane; k < nv; k += 32) out[k] = in[k];
+    }
+}
+
 // codec training (index.rs:240-258): L2 norm of every residual row; per-dimension mean of |residual|
 __global__ void k_residual_stats(const float *__restrict__ R, long long n, int dim, float *__restrict__ norms) {
     const int lane = threadIdx.x & 31;

@@ -201,6 +201,16 @@ pb_status pb_read_chunk(const std::string &dir, long long chunk, long long n_tok
     return PB_OK;
 }
 
+pb_status pb_read_npy_f32(const std::string &path, long long &rows, long long &cols, std::vector<float> &out) {
+    Npy a;
+    if (pb_status s = a.open(path)) return s;
+    if (!a.is("f4") || a.shape.size() != 2) return pb_fail(PB_ERR_IO, "%s must be <f4 [rows, cols]", path.c_str());
+    rows = a.shape[0];
+    cols = a.shape[1];
+    out.assign((const float *)a.data, (const float *)a.data + a.count());
+    return PB_OK;
+}
+
 extern "C" pb_status pb_index_load(const char *index_dir, int32_t device, pb_index **out) {
     if (!index_dir || !out) return pb_fail(PB_ERR_INVALID, "null argument");
     *out = nullptr;

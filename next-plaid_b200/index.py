@@ -85,6 +85,7 @@ EXPORTS = [
     "pb_kmeans_num_partitions", "pb_codec_num_sample_docs", "pb_codec_heldout_tokens", "pb_create_index",
     "pb_create_params_default", "pb_build_comm_init", "pb_build_comm_group", "pb_build_comm_destroy", "pb_kmeans_fit_dp", "pb_codec_last_assign_stats", "pb_codec_find_outliers",
     "pb_index_append", "pb_index_append_encoded", "pb_index_reserve",
+    "pb_index_delete", "pb_last_delete_ms",
 ]
 
 _lib = None
@@ -174,6 +175,8 @@ def load_library():
         L.pb_index_append_encoded.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32,
                                               C.c_void_p]
         L.pb_index_reserve.argtypes = [C.c_void_p, C.c_int64, C.c_int64]
+        L.pb_index_delete.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_char_p, C.c_void_p]
+        L.pb_last_delete_ms.argtypes = [C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 
@@ -396,6 +399,23 @@ class MmapIndex:
     def reserve(self, num_documents: int, num_embeddings: int):
         """pb_index_reserve: capacity for appends up to these totals without reallocation."""
         _check(load_library().pb_index_reserve(self._h, num_documents, num_embeddings))
+
+    # -- incremental delete (index.rs:1805 delete_with_options + reload) --------------------------------
+    def delete(self, doc_ids: Sequence[int], index_dir: Optional[str] = None) -> int:
+        """MmapIndex::delete + reload (pb_index_delete): removes these documents (the ids search returns; ids outside
+        the index, negative and repeated ids are ignored) and renumbers the rest in order; with `index_dir` also
+        applies delete_from_index's file changes to that directory.  Returns the number of documents removed."""
+        ids = np.ascontiguousarray(doc_ids, np.int64).reshape(-1)
+        n = C.c_int64()
+        _check(load_library().pb_index_delete(self._h, _ptr(ids), len(ids),
+                                              None if index_dir is None else os.fsencode(index_dir), C.byref(n)))
+        return int(n.value)
+
+    def last_delete_ms(self) -> dict:
+        """Device time of the last delete, with set_profiling(True): compaction, inverted file, norm pass (ms)."""
+        v = np.zeros(3, np.float32)
+        _check(load_library().pb_last_delete_ms(self._h, _ptr(v)))
+        return dict(compact_ms=float(v[0]), ivf_ms=float(v[1]), norms_ms=float(v[2]))
 
     # -- search ------------------------------------------------------------------------------
     def search(self, query: np.ndarray, params: SearchParameters,

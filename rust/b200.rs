@@ -66,6 +66,8 @@ extern "C" {
     fn pb_index_append_encoded(ix: *mut c_void, codes: *const i64, residuals: *const u8, doc_lengths: *const i64,
                                n_docs: i64, memory_space: i32, out_first_doc_id: *mut i64) -> c_int;
     fn pb_index_reserve(ix: *mut c_void, num_documents: i64, num_embeddings: i64) -> c_int;
+    fn pb_index_delete(ix: *mut c_void, doc_ids: *const i64, n_ids: i64, index_dir: *const c_char,
+                       out_deleted: *mut i64) -> c_int;
 }
 
 fn last_error() -> String {
@@ -201,6 +203,23 @@ impl B200Index {
             return Err(Error::IndexLoad(last_error()));
         }
         Ok((first..first + lens.len() as i64).collect())
+    }
+
+    /// `delete::delete_from_index` (delete.rs:43) + `reload` (index.rs:1767) inside `MmapIndex::delete_with_options`
+    /// (index.rs:1805) under the `b200` feature: the documents leave the live handle (survivors renumbered in order;
+    /// searches from other threads wait for it) and the file changes are applied to `index_path`.  Ids outside the
+    /// index, negative and repeated ids are ignored.  Returns the number of documents removed; the caller's
+    /// `metadata.db` step (`filtering::delete`) follows as before.
+    pub fn delete_with_options(&self, doc_ids: &[i64], index_path: &str) -> Result<usize> {
+        let path = CString::new(index_path).map_err(|e| Error::IndexLoad(e.to_string()))?;
+        let mut deleted = 0i64;
+        let st = unsafe {
+            pb_index_delete(self.handle, doc_ids.as_ptr(), doc_ids.len() as i64, path.as_ptr(), &mut deleted)
+        };
+        if st != 0 {
+            return Err(Error::Delete(last_error()));
+        }
+        Ok(deleted as usize)
     }
 
     /// Body of `MmapIndex::search` (index.rs:1258).
