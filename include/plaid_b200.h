@@ -104,6 +104,28 @@ PB_API void pb_search_params_default(pb_search_params *p);
  * N.codes.npy, N.residuals.npy) and uploads it to `device`. */
 PB_API pb_status pb_index_load(const char *index_dir, int32_t device, pb_index **out);
 
+/* pb_index_load restricted to documents [doc_begin, doc_end) of the directory: one shard of a doc-sharded
+ * deployment.  The handle equals pb_index_open of
+ *   centroids, bucket_weights              as in the directory
+ *   codes / residuals                      tokens doc_off[doc_begin] .. doc_off[doc_end]
+ *   doc_lengths                            doclens[doc_begin .. doc_end)
+ *   ivf / ivf_lengths                      per centroid, the entries of ivf.npy's list with doc_begin <= id < doc_end,
+ *                                          in file order, minus doc_begin; lengths = their counts
+ *   doc_id_base                            doc_begin
+ * so search returns global ids.  [0, D) gives exactly what pb_index_load gives.  Each call reads only the chunk rows
+ * of its range from disk; ivf.npy is read whole.  The directory is validated as pb_index_load validates it (every
+ * doclens file, every chunk header and size, ivf / ivf_lengths consistency, every ivf entry in [0, D)), so all ranks
+ * accept or refuse the same directory.
+ * PB_ERR_INVALID before the device is touched: doc_begin < 0, doc_end < doc_begin, doc_end > D. */
+PB_API pb_status pb_index_load_range(const char *index_dir, int32_t device, int64_t doc_begin, int64_t doc_end,
+                                     pb_index **out);
+
+/* Token-balanced contiguous split of the directory's D documents over `world` ranks (host only, reads metadata.json
+ * and the doclens files): out_bounds[0] = 0, out_bounds[world] = D, and for 0 < r < world
+ * out_bounds[r] = min { d : doc_off[d] * world >= N * r }.  Shards may be empty (world > D, N = 0).
+ * PB_ERR_INVALID: world < 1. */
+PB_API pb_status pb_index_dir_shard_bounds(const char *index_dir, int32_t world, int64_t *out_bounds /* [world+1] */);
+
 /* Same, from arrays already in memory (what a Rust MmapIndex owns after its own load). */
 PB_API pb_status pb_index_open(const pb_index_desc *desc, pb_index **out);
 

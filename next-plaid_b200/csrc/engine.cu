@@ -529,6 +529,94 @@ static pb_status upload_narrow(DevBuf &dst, long long dst_off, const int64_t *sr
     return PB_OK;
 }
 
+// out[i] = in[0] + .. + in[i - 1] for i < n
+static pb_status exclusive_sum(const long long *in, long long *out, long long n, DevBuf &tmp) {
+    size_t tb = 0;
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, in, out, n));
+    CKS(tmp.ensure(tb + 16));
+    CK(cub::DeviceScan::ExclusiveSum(tmp.p, tb, in, out, n));
+    return PB_OK;
+}
+
+// The inverted file of an index opened without one, as the part of a directory's ivf.npy (host, total entries,
+// lengths [K]) that lies in docs [b, e): every list filtered to the range in file order, ids minus b.  The file goes
+// through a staging buffer of at most 2^26 entries (PB_LOAD_IVF_SLAB sets another size): a count pass, then the
+// write pass into the exactly sized ivf, which copies the file a second time when it is more than one slab.  Any entry
+// outside [0, limit) fails.
+pb_status pb_index_upload_ivf_range(pb_index *ix, const int64_t *ivf, const int32_t *lengths, long long total,
+                                    long long limit, long long b, long long e) {
+    CK(cudaSetDevice(ix->device));
+    const long long K = ix->K;
+    std::vector<long long> foff((size_t)K + 1, 0);
+    for (long long i = 0; i < K; ++i) {
+        if (lengths[i] < 0) return pb_fail(PB_ERR_INVALID, "ivf_lengths[%lld] < 0", i);
+        foff[i + 1] = foff[i] + lengths[i];
+    }
+    long long slab = 1ll << 26;  // 64M entries = 512 MiB of i64, as upload_narrow
+    if (const char *v = getenv("PB_LOAD_IVF_SLAB")) slab = std::max(1ll, atoll(v));  // entries per slab
+    const int grid = ix->sm_count * 8;
+    DevBuf doff, cnt, stage, bad, tmp;
+    CKS(upload(doff, foff.data(), foff.size() * 8, PB_MEM_HOST));
+    CKS(cnt.ensure((size_t)(K + 1) * 8));
+    CK(cudaMemset(cnt.p, 0, (size_t)(K + 1) * 8));
+    CKS(stage.ensure(std::max<size_t>((size_t)std::min(total, slab) * 8, 16)));
+    CKS(bad.ensure(16));
+    CK(cudaMemset(bad.p, 0, 4));
+    // slab [o, o + m) overlaps the lists c0 <= c < c1: c0 the last list starting at or before o, c1 the first at or after o + m
+    auto lists = [&](long long o, long long m, long long &c0, long long &c1) {
+        c0 = std::upper_bound(foff.begin(), foff.end(), o) - foff.begin() - 1;
+        c1 = std::lower_bound(foff.begin(), foff.end(), o + m) - foff.begin();
+    };
+    // the kept entries of slab [o, o + m) at their lists' cursors
+    DevBuf cur;
+    CKS(cur.ensure((size_t)(K + 1) * 8));
+    auto write = [&](long long o, long long m, long long c0, long long c1) -> pb_status {
+        k_ivf_range_write<<<grid, 256>>>(stage.as<long long>(), o, m, doff.as<long long>(), c0, c1, b, e,
+                                         cur.as<long long>(), ix->ivf.as<uint32_t>());
+        CK(cudaGetLastError());
+        return PB_OK;
+    };
+    // For the whole index every valid entry is kept: the offsets are the file's, and each slab is written as soon as it
+    // is counted, so the file is copied once.  Otherwise the write pass waits for the scan of all the counts.
+    const bool whole = b == 0 && e >= limit;
+    CKS(ix->ivf_off.ensure((size_t)(K + 1) * 8));
+    if (whole) {
+        CK(cudaMemcpy(ix->ivf_off.p, doff.p, (size_t)(K + 1) * 8, cudaMemcpyDeviceToDevice));
+        CK(cudaMemcpy(cur.p, doff.p, (size_t)(K + 1) * 8, cudaMemcpyDeviceToDevice));
+        ix->ivf_len = total;
+        CKS(ix->ivf.ensure(std::max<size_t>((size_t)total * 4, 16)));
+    }
+    for (long long o = 0; o < total; o += slab) {
+        const long long m = std::min(slab, total - o);
+        long long c0, c1;
+        lists(o, m, c0, c1);
+        CK(cudaMemcpy(stage.p, ivf + o, (size_t)m * 8, cudaMemcpyHostToDevice));
+        k_ivf_range_count<<<grid, 256>>>(stage.as<long long>(), o, m, doff.as<long long>(), c0, c1, limit, b, e,
+                                         cnt.as<long long>(), bad.as<int>());
+        CK(cudaGetLastError());
+        if (whole) CKS(write(o, m, c0, c1));
+    }
+    int hbad = 0;
+    CK(cudaMemcpy(&hbad, bad.p, 4, cudaMemcpyDeviceToHost));
+    if (hbad) return pb_fail(PB_ERR_INVALID, "ivf contains a value outside [0, %lld)", limit);
+    if (!whole) {
+        CKS(exclusive_sum(cnt.as<long long>(), ix->ivf_off.as<long long>(), K + 1, tmp));
+        CK(cudaMemcpy(&ix->ivf_len, ix->ivf_off.as<long long>() + K, 8, cudaMemcpyDeviceToHost));
+        CKS(ix->ivf.ensure(std::max<size_t>((size_t)ix->ivf_len * 4, 16)));
+        CK(cudaMemcpy(cur.p, ix->ivf_off.p, (size_t)K * 8, cudaMemcpyDeviceToDevice));
+        for (long long o = 0; ix->ivf_len > 0 && o < total; o += slab) {
+            const long long m = std::min(slab, total - o);
+            long long c0, c1;
+            lists(o, m, c0, c1);
+            if (total > slab) CK(cudaMemcpy(stage.p, ivf + o, (size_t)m * 8, cudaMemcpyHostToDevice));
+            CKS(write(o, m, c0, c1));
+        }
+    }
+    CK(cudaDeviceSynchronize());
+    ix->build_ivf = false;
+    return PB_OK;
+}
+
 // codes + packed residuals of tokens [tok_off, tok_off+n) (one chunk file pair, or everything)
 pb_status pb_index_upload_tokens(pb_index *ix, long long tok_off, const int64_t *codes, const uint8_t *residuals,
                                  long long n, int space) {
@@ -3137,15 +3225,6 @@ extern "C" pb_status pb_index_reserve(pb_index *ix, int64_t num_documents, int64
 // incremental delete: MmapIndex::delete_with_options (index.rs:1805) -> delete_from_index (delete.rs:43) + reload on a
 // live handle
 // ------------------------------------------------------------------------------------------
-// out[i] = in[0] + .. + in[i - 1] for i < n
-static pb_status exclusive_sum(const long long *in, long long *out, long long n, DevBuf &tmp) {
-    size_t tb = 0;
-    CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, in, out, n));
-    CKS(tmp.ensure(tb + 16));
-    CK(cub::DeviceScan::ExclusiveSum(tmp.p, tb, in, out, n));
-    return PB_OK;
-}
-
 struct Events {
     cudaEvent_t e[5] = {};
     ~Events() {

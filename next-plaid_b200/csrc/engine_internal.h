@@ -12,6 +12,11 @@ pb_status pb_index_upload_tokens(pb_index *ix, long long tok_off, const int64_t 
                                  long long n, int space);
 // call once after the last pb_index_upload_tokens
 pb_status pb_index_finalize(pb_index *ix);
+// For a handle begun without an inverted file: the part of a directory's inverted file (host ivf.npy <i8 [total],
+// ivf_lengths [K], global ids, all checked against [0, limit)) that lies in docs [b, e), each list filtered in file
+// order with ids minus b, instead of the one pb_index_finalize would build from the codes.
+pb_status pb_index_upload_ivf_range(pb_index *ix, const int64_t *ivf, const int32_t *lengths, long long total,
+                                    long long limit, long long b, long long e);
 
 // The index directory, as the loader reads it: a whole file; a number of a flat JSON object; a doclens.{i}.json list;
 // the chunk file pair {i}.codes.npy <i8 [n_tokens] / {i}.residuals.npy u1 [n_tokens][packed].

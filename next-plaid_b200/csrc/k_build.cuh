@@ -715,6 +715,52 @@ __global__ void k_ivf_delete_write(const uint32_t *__restrict__ ivf, const long 
     }
 }
 
+// ------------------------------------------------------------------------------------------
+// The inverted file of a doc range [b, e) of a directory (pb_index_load_range): each list of ivf.npy filtered to the
+// range, in file order, ids minus b.  The file (i64, global ids) arrives in slabs: slab holds its entries [s0, s0 + m),
+// off [K + 1] are the file's list offsets, and the centroids c0 <= c < c1 are those whose list overlaps the slab (a list
+// may straddle slabs).  One warp per centroid; slabs go in order on one stream, so cnt[c] / cur[c] need no atomics.
+// Every entry outside [0, limit) sets *bad.
+// ------------------------------------------------------------------------------------------
+__global__ void k_ivf_range_count(const long long *__restrict__ slab, long long s0, long long m,
+                                  const long long *__restrict__ off, long long c0, long long c1, long long limit,
+                                  long long b, long long e, long long *__restrict__ cnt, int *__restrict__ bad) {
+    const int lane = threadIdx.x & 31;
+    const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
+    bool oob = false;
+    for (long long c = c0 + (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c < c1; c += nw) {
+        const long long i0 = max(off[c], s0) - s0, i1 = min(off[c + 1], s0 + m) - s0;
+        long long kept = 0;
+        for (long long i = i0 + lane; i - lane < i1; i += 32) {
+            const long long id = i < i1 ? slab[i] : -1;
+            oob |= i < i1 && (id < 0 || id >= limit);
+            kept += __popc(__ballot_sync(PB_FULL, id >= b && id < e));
+        }
+        if (lane == 0) cnt[c] += kept;
+    }
+    if (oob) *bad = 1;
+}
+
+// the kept entries of the slab's part of list c at cur[c].., compacted with a ballot, as id - b; cur[c] advances
+__global__ void k_ivf_range_write(const long long *__restrict__ slab, long long s0, long long m,
+                                  const long long *__restrict__ off, long long c0, long long c1, long long b,
+                                  long long e, long long *__restrict__ cur, uint32_t *__restrict__ out) {
+    const int lane = threadIdx.x & 31;
+    const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
+    for (long long c = c0 + (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c < c1; c += nw) {
+        const long long i0 = max(off[c], s0) - s0, i1 = min(off[c + 1], s0 + m) - s0;
+        long long dst = cur[c];
+        for (long long i = i0 + lane; i - lane < i1; i += 32) {
+            const long long id = i < i1 ? slab[i] : -1;
+            const bool keep = id >= b && id < e;
+            const unsigned bal = __ballot_sync(PB_FULL, keep);
+            if (keep) out[dst + __popc(bal & ((1u << lane) - 1u))] = (uint32_t)(id - b);
+            dst += __popc(bal);
+        }
+        if (lane == 0) cur[c] = dst;
+    }
+}
+
 // In-place compaction of a per-token (or per-distinct-code) array, one window of survivors [j0, j1) at a time: survivor
 // j's rows old_off[kept[j]] .. old_off[kept[j] + 1] go to staging at new_off[j] - new_off[j0], and the caller then
 // copies the staging to new_off[j0].  One warp per doc, V-wide accesses (row_bytes * every offset is a multiple of

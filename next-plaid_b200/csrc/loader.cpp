@@ -13,6 +13,7 @@
 #include <sys/stat.h>
 #include <unistd.h>
 
+#include <algorithm>
 #include <cctype>
 #include <cstdio>
 #include <cstdlib>
@@ -211,16 +212,45 @@ pb_status pb_read_npy_f32(const std::string &path, long long &rows, long long &c
     return PB_OK;
 }
 
-extern "C" pb_status pb_index_load(const char *index_dir, int32_t device, pb_index **out) {
-    if (!index_dir || !out) return pb_fail(PB_ERR_INVALID, "null argument");
-    *out = nullptr;
-    const std::string dir = std::string(index_dir) + "/";
-    std::string meta;
-    if (pb_status s = pb_read_text(dir + "metadata.json", meta)) return s;
+namespace {
+
+// The document layout of an index directory: metadata.json's num_chunks / nbits / num_embeddings (-1 when absent), and
+// the doc lengths of every chunk (index.rs:1096-1104) with each chunk's token count.
+struct DirLayout {
     double num_chunks = 0, nbits = 0, num_emb = -1;
-    if (!pb_json_number(meta, "num_chunks", num_chunks) || !pb_json_number(meta, "nbits", nbits))
-        return pb_fail(PB_ERR_IO, "metadata.json lacks num_chunks / nbits");
-    pb_json_number(meta, "num_embeddings", num_emb);
+    std::vector<int64_t> doclens;
+    std::vector<long long> chunk_tokens;
+    long long N = 0;
+
+    pb_status read_metadata(const std::string &dir) {
+        std::string meta;
+        if (pb_status s = pb_read_text(dir + "metadata.json", meta)) return s;
+        if (!pb_json_number(meta, "num_chunks", num_chunks) || !pb_json_number(meta, "nbits", nbits))
+            return pb_fail(PB_ERR_IO, "metadata.json lacks num_chunks / nbits");
+        pb_json_number(meta, "num_embeddings", num_emb);
+        return PB_OK;
+    }
+    pb_status read_doclens(const std::string &dir) {
+        for (int c = 0; c < (int)num_chunks; ++c) {
+            const size_t first = doclens.size();
+            if (pb_status s = pb_read_doclens(dir + "doclens." + std::to_string(c) + ".json", doclens)) return s;
+            long long tok = 0;
+            for (size_t i = first; i < doclens.size(); ++i) tok += doclens[i];
+            chunk_tokens.push_back(tok);
+        }
+        for (long long t : chunk_tokens) N += t;
+        if (num_emb >= 0 && (long long)num_emb != N)
+            return pb_fail(PB_ERR_IO, "metadata.json num_embeddings=%lld but doclens sum to %lld", (long long)num_emb, N);
+        return PB_OK;
+    }
+};
+
+// pb_index_load of documents [doc_begin, doc_end) of the directory; doc_end < 0 stands for every document
+pb_status load_range(const char *index_dir, int32_t device, long long doc_begin, long long doc_end, pb_index **out) {
+    const std::string dir = std::string(index_dir) + "/";
+    DirLayout lay;
+    if (pb_status s = lay.read_metadata(dir)) return s;
+    const double num_chunks = lay.num_chunks, nbits = lay.nbits;
 
     Npy cent, wts, ivf, ivfl;
     if (pb_status s = cent.open(dir + "centroids.npy")) return s;
@@ -254,35 +284,33 @@ extern "C" pb_status pb_index_load(const char *index_dir, int32_t device, pb_ind
     if (wts.count() != (1ll << nb)) return pb_fail(PB_ERR_IO, "bucket_weights.npy has %lld entries, expected %d", wts.count(), 1 << nb);
     if (ivfl.count() != K) return pb_fail(PB_ERR_IO, "ivf_lengths.npy has %lld entries, centroids.npy %lld rows", ivfl.count(), K);
 
-    // doc lengths from every chunk (index.rs:1096-1104)
-    std::vector<int64_t> doclens;
-    std::vector<long long> chunk_tokens;
-    for (int c = 0; c < (int)num_chunks; ++c) {
-        const size_t first = doclens.size();
-        if (pb_status s = pb_read_doclens(dir + "doclens." + std::to_string(c) + ".json", doclens)) return s;
-        long long tok = 0;
-        for (size_t i = first; i < doclens.size(); ++i) tok += doclens[i];
-        chunk_tokens.push_back(tok);
-    }
-    long long N = 0;
-    for (long long t : chunk_tokens) N += t;
-    if (num_emb >= 0 && (long long)num_emb != N)
-        return pb_fail(PB_ERR_IO, "metadata.json num_embeddings=%lld but doclens sum to %lld", (long long)num_emb, N);
+    if (pb_status s = lay.read_doclens(dir)) return s;
+    const std::vector<int64_t> &doclens = lay.doclens;
+    const std::vector<long long> &chunk_tokens = lay.chunk_tokens;
+    const long long D = (long long)doclens.size();
+    if (doc_end < 0) doc_end = D;
+    if (doc_end > D)
+        return pb_fail(PB_ERR_INVALID, "document range [%lld, %lld) outside the directory's %lld documents", doc_begin,
+                       doc_end, D);
+    // the range's tokens [t0, t1)
+    long long t0 = 0, t1 = 0;
+    for (long long i = 0; i < doc_end; ++i) (i < doc_begin ? t0 : t1) += doclens[i];
+    t1 += t0;
 
+    // the inverted file is not given to pb_index_open_begin: pb_index_upload_ivf_range slices ivf.npy on the device
     pb_index_desc d;
     memset(&d, 0, sizeof d);
     d.dim = dim;
     d.nbits = nb;
     d.num_centroids = K;
-    d.num_documents = (int64_t)doclens.size();
-    d.num_embeddings = N;
+    d.num_documents = doc_end - doc_begin;
+    d.num_embeddings = t1 - t0;
     d.centroids = cent_f32;
     d.bucket_weights = wts_f32;
-    d.doc_lengths = doclens.data();
-    d.ivf = (const int64_t *)ivf.data;
-    d.ivf_lengths = ivfl_i32;
+    d.doc_lengths = doclens.data() + doc_begin;
     d.device = device;
     d.memory_space = PB_MEM_HOST;
+    d.doc_id_base = doc_begin;
     long long ivf_sum = 0;
     for (long long i = 0; i < K; ++i) ivf_sum += ivfl_i32[i];
     if (ivf_sum != ivf.count()) return pb_fail(PB_ERR_IO, "ivf.npy has %lld entries, ivf_lengths sum to %lld", ivf.count(), ivf_sum);
@@ -305,22 +333,59 @@ extern "C" pb_status pb_index_load(const char *index_dir, int32_t device, pb_ind
     }
     pb_index *ix = nullptr;
     if (pb_status s = pb_index_open_begin(&d, &ix)) return s;
-    long long off = 0;
-    for (int c = 0; c < (int)num_chunks; ++c) {
-        if (chunk_tokens[c] == 0) continue;
+    pb_status s = pb_index_upload_ivf_range(ix, (const int64_t *)ivf.data, ivfl_i32, ivf.count(), std::max(D, 1ll),
+                                            doc_begin, doc_end);
+    // the rows of each chunk that overlap [t0, t1), straight from the chunk's mapping
+    for (long long c = 0, cs = 0; !s && c < (long long)num_chunks; cs += chunk_tokens[c++]) {
+        const long long lo = std::max(cs, t0), hi = std::min(cs + chunk_tokens[c], t1);
+        if (lo >= hi) continue;
         Npy codes, res;
-        pb_status s = open_chunk(c, codes, res);
-        if (!s) s = pb_index_upload_tokens(ix, off, (const int64_t *)codes.data, res.data, chunk_tokens[c], PB_MEM_HOST);
-        if (s) {
-            pb_index_close(ix);
-            return s;
-        }
-        off += chunk_tokens[c];
+        s = open_chunk((int)c, codes, res);
+        if (!s)
+            s = pb_index_upload_tokens(ix, lo - t0, (const int64_t *)codes.data + (lo - cs),
+                                       res.data + (size_t)(lo - cs) * packed, hi - lo, PB_MEM_HOST);
     }
-    if (pb_status s = pb_index_finalize(ix)) {
+    if (!s) s = pb_index_finalize(ix);
+    if (s) {
         pb_index_close(ix);
         return s;
     }
     *out = ix;
+    return PB_OK;
+}
+
+}  // namespace
+
+extern "C" pb_status pb_index_load(const char *index_dir, int32_t device, pb_index **out) {
+    if (!index_dir || !out) return pb_fail(PB_ERR_INVALID, "null argument");
+    *out = nullptr;
+    return load_range(index_dir, device, 0, -1, out);
+}
+
+extern "C" pb_status pb_index_load_range(const char *index_dir, int32_t device, int64_t doc_begin, int64_t doc_end,
+                                         pb_index **out) {
+    if (!index_dir || !out) return pb_fail(PB_ERR_INVALID, "null argument");
+    *out = nullptr;
+    if (doc_begin < 0 || doc_end < doc_begin)
+        return pb_fail(PB_ERR_INVALID, "bad document range [%lld, %lld)", (long long)doc_begin, (long long)doc_end);
+    return load_range(index_dir, device, doc_begin, doc_end, out);
+}
+
+extern "C" pb_status pb_index_dir_shard_bounds(const char *index_dir, int32_t world, int64_t *out_bounds) {
+    if (!index_dir || !out_bounds) return pb_fail(PB_ERR_INVALID, "null argument");
+    if (world < 1) return pb_fail(PB_ERR_INVALID, "world must be at least 1, got %d", world);
+    const std::string dir = std::string(index_dir) + "/";
+    DirLayout lay;
+    if (pb_status s = lay.read_metadata(dir)) return s;
+    if (pb_status s = lay.read_doclens(dir)) return s;
+    const long long D = (long long)lay.doclens.size();
+    // bound r = min { d : doc_off[d] * world >= N * r }, in 128-bit so that no product overflows
+    long long d = 0, off = 0;
+    out_bounds[0] = 0;
+    for (int r = 1; r < world; ++r) {
+        while (d < D && (__int128)off * world < (__int128)lay.N * r) off += lay.doclens[d++];
+        out_bounds[r] = d;
+    }
+    out_bounds[world] = D;
     return PB_OK;
 }

@@ -85,7 +85,7 @@ EXPORTS = [
     "pb_kmeans_num_partitions", "pb_codec_num_sample_docs", "pb_codec_heldout_tokens", "pb_create_index",
     "pb_create_params_default", "pb_build_comm_init", "pb_build_comm_group", "pb_build_comm_destroy", "pb_kmeans_fit_dp", "pb_codec_last_assign_stats", "pb_codec_find_outliers",
     "pb_index_append", "pb_index_append_encoded", "pb_index_reserve",
-    "pb_index_delete", "pb_last_delete_ms",
+    "pb_index_delete", "pb_last_delete_ms", "pb_index_load_range", "pb_index_dir_shard_bounds",
 ]
 
 _lib = None
@@ -122,6 +122,8 @@ def load_library():
         L.pb_set_lanes.argtypes = [C.c_void_p, C.c_int32]
         L.pb_set_lanes.restype = None
         L.pb_index_load.argtypes = [C.c_char_p, C.c_int32, C.POINTER(C.c_void_p)]
+        L.pb_index_load_range.argtypes = [C.c_char_p, C.c_int32, C.c_int64, C.c_int64, C.POINTER(C.c_void_p)]
+        L.pb_index_dir_shard_bounds.argtypes = [C.c_char_p, C.c_int32, C.c_void_p]
         L.pb_index_open.argtypes = [C.POINTER(_Desc), C.POINTER(C.c_void_p)]
         L.pb_search_batch_traced.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                              C.POINTER(_Params), C.c_void_p, C.c_int64, C.c_void_p,
@@ -243,6 +245,14 @@ def device_count() -> int:
     return int(load_library().pb_device_count())
 
 
+def shard_bounds(index_path: str, world: int) -> np.ndarray:
+    """pb_index_dir_shard_bounds: the token-balanced split of the directory's documents over `world` ranks, <i8
+    [world + 1]; rank r holds documents [bounds[r], bounds[r + 1]).  Host only."""
+    out = np.zeros(max(int(world), 0) + 1, np.int64)
+    _check(load_library().pb_index_dir_shard_bounds(os.fsencode(index_path), world, _ptr(out)))
+    return out
+
+
 @dataclass
 class SearchParameters:
     """search.rs:27-69; defaults are SearchParameters::default() (search.rs:58-69)."""
@@ -304,6 +314,22 @@ class MmapIndex:
         h = C.c_void_p()
         _check(L.pb_index_load(os.fsencode(index_path), device, C.byref(h)))
         return cls(h.value, index_path)
+
+    @classmethod
+    def load_range(cls, index_path: str, doc_begin: int, doc_end: int, device: int = 0) -> "MmapIndex":
+        """pb_index_load_range: documents [doc_begin, doc_end) of the directory as one shard of a doc-sharded
+        deployment (doc_id_base = doc_begin, so search returns global ids).  Reads only that range's chunk rows."""
+        h = C.c_void_p()
+        _check(load_library().pb_index_load_range(os.fsencode(index_path), device, doc_begin, doc_end, C.byref(h)))
+        return cls(h.value, index_path)
+
+    @classmethod
+    def load_shard(cls, index_path: str, rank: int, world: int, device: int = 0) -> "MmapIndex":
+        """Shard `rank` of `world` of the directory: load_range over shard_bounds(index_path, world)."""
+        if not 0 <= rank < world:
+            raise PlaidError(PB_ERR_INVALID, f"rank {rank} outside [0, {world})")
+        b = shard_bounds(index_path, world)
+        return cls.load_range(index_path, int(b[rank]), int(b[rank + 1]), device)
 
     @classmethod
     def from_arrays(cls, centroids, bucket_weights, codes, residuals, doc_lengths, ivf, ivf_lengths,

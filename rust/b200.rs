@@ -68,6 +68,9 @@ extern "C" {
     fn pb_index_reserve(ix: *mut c_void, num_documents: i64, num_embeddings: i64) -> c_int;
     fn pb_index_delete(ix: *mut c_void, doc_ids: *const i64, n_ids: i64, index_dir: *const c_char,
                        out_deleted: *mut i64) -> c_int;
+    fn pb_index_load_range(index_dir: *const c_char, device: i32, doc_begin: i64, doc_end: i64,
+                           out: *mut *mut c_void) -> c_int;
+    fn pb_index_dir_shard_bounds(index_dir: *const c_char, world: i32, out_bounds: *mut i64) -> c_int;
 }
 
 fn last_error() -> String {
@@ -92,6 +95,26 @@ impl B200Index {
         let st = unsafe { pb_index_load(c.as_ptr(), device, &mut handle) };
         if st != 0 {
             // No CPU fallback on this path: behaves like NEXT_PLAID_FORCE_GPU (lib.rs:71-84).
+            return Err(Error::IndexLoad(last_error()));
+        }
+        Ok(B200Index { handle })
+    }
+
+    /// Shard `rank` of `world` of the same directory for a doc-sharded deployment: the token-balanced document range
+    /// of `pb_index_dir_shard_bounds`, loaded by `pb_index_load_range` (global ids; only that range's chunk rows are
+    /// read).  Every rank then calls `pb_index_comm_init`.
+    pub fn load_shard(index_path: &str, rank: i32, world: i32, device: i32) -> Result<Self> {
+        if rank < 0 || rank >= world {
+            return Err(Error::IndexLoad(format!("rank {} outside [0, {})", rank, world)));
+        }
+        let c = CString::new(index_path).map_err(|e| Error::IndexLoad(e.to_string()))?;
+        let mut bounds = vec![0i64; world as usize + 1];
+        if unsafe { pb_index_dir_shard_bounds(c.as_ptr(), world, bounds.as_mut_ptr()) } != 0 {
+            return Err(Error::IndexLoad(last_error()));
+        }
+        let (b, e) = (bounds[rank as usize], bounds[rank as usize + 1]);
+        let mut handle: *mut c_void = std::ptr::null_mut();
+        if unsafe { pb_index_load_range(c.as_ptr(), device, b, e, &mut handle) } != 0 {
             return Err(Error::IndexLoad(last_error()));
         }
         Ok(B200Index { handle })
