@@ -355,6 +355,10 @@ typedef struct pb_work_counters {
     int64_t n_k1_tc_redo;        /* sub-batches the tensor-core pass handed back to the exact path (flagged query, list overflow) */
     int64_t n_exact_pairs;       /* (token, query token) similarities the pair form of the exact stage evaluated */
     int64_t n_pair_fallback_queries; /* queries whose pair list overflowed (or that had no estimate): scored by k_exact */
+    int64_t filter_err_ratio_e6; /* PB_FILTER_DIAG=1 only: ceil(1e6 * largest |estimate - exact| / (|q|max * eps_unit)) over
+                                  * every (kept doc, query token) maximum of the MaxSim filter; <= 1e6 = within its
+                                  * certificate; INT64_MAX = a non-finite estimate of a finite maximum; 0 otherwise */
+    int64_t filter_diag_pairs;   /* PB_FILTER_DIAG=1 only: (kept doc, query token) maxima compared for filter_err_ratio_e6 */
 } pb_work_counters;
 PB_API pb_status pb_last_work_counters(pb_index *ix, pb_work_counters *out);
 

@@ -278,7 +278,7 @@ struct Workspace {
     cudaEvent_t call_ev[2] = {};                // around a whole search call
     DevBuf Q, qoff, ST, partial, sel, cells, ncells, bitmap, cand, ncand, approx, keys, kept, nkept, tokp, maxkey,
         exact, fkeys, oids, oscores, ocounts, subset, subset_bits, elig, misc, list, counters, lkeys, ST16, qrange, qflag, lsum, cand2, ncand2,  cellbits,
-        gkeys, krank, payload, gfkeys, gpayload, cmax16, tau16, plist, pcount, Qi, Qh16t, Ql16t, ST16b, k1diag, k1rows, ulist, nulist, est, kept2, krank2, nkept2, tokp2, ktok2, qnmax, qexp, qrange_tc, mslot, slicecnt, rcmax, rcpairs, rcn, cellflags, estkey, srcrank, xpairs, xnpairs, needexact, gbase;
+        gkeys, krank, payload, gfkeys, gpayload, cmax16, tau16, plist, pcount, Qi, Qh16t, Ql16t, ST16b, k1diag, k1rows, ulist, nulist, est, kept2, krank2, nkept2, tokp2, ktok2, qnmax, qexp, qrange_tc, mslot, slicecnt, rcmax, rcpairs, rcn, cellflags, estkey, srcrank, xpairs, xnpairs, needexact, gbase, fdiag;
     HostBuf hq, hres, hcounts;
     pb_status init() {
         CK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -386,6 +386,7 @@ struct pb_index {
     DevBuf centroids_f16;      // [K][dim] fp16 copy for the filter (k_exact_tc, the variant without a score table)
     DevBuf tok_inv_norm;       // [N] 1 / |c + w| for the linear estimate (k_maxsim_tc)
     bool filter_v1 = false;    // PB_FILTER_V1=1: always the decompressing filter k_exact_tc (A/B measurement)
+    bool filter_diag = false;  // PB_FILTER_DIAG=1: score every kept doc exactly and measure the filter's estimate against it
     bool pair_exact = true;    // exact stage on the (token, query token) pairs that can hold a maximum (PB_PAIR_EXACT=0: k_exact)
     int ws_grid = 8;           // k_maxsim_tc CTAs per SM across the batch (PB_WS_GRID)
     int ws_grid2 = 8;          // the same for its pass 2 over the filter's survivors (PB_WS_GRID2; 1: 0.54, 2: 0.43, 4 and 8: 0.40 ms)
@@ -833,6 +834,7 @@ pb_status pb_index_finalize(pb_index *ix) {
         if (const char *e = getenv("PB_FAST_APPROX")) ix->fast_approx = atoi(e) != 0;
         if (const char *e = getenv("PB_FAST_EXACT")) ix->fast_exact = atoi(e) != 0;
         if (const char *e = getenv("PB_FILTER_V1")) ix->filter_v1 = atoi(e) != 0;
+        if (const char *e = getenv("PB_FILTER_DIAG")) ix->filter_diag = atoi(e) != 0;
         if (const char *e = getenv("PB_PAIR_EXACT")) ix->pair_exact = atoi(e) != 0;
         if (const char *e = getenv("PB_WS_GRID")) ix->ws_grid = std::max(1, atoi(e));
         if (const char *e = getenv("PB_WS_GRID2")) ix->ws_grid2 = std::max(1, atoi(e));
@@ -1270,8 +1272,9 @@ static pb_status launch_maxsim_tc(pb_index *ix, Workspace &ws, const KeptView &i
         auto kern = k_maxsim_tc<DV, NB, NQ, EM>;                                                                       \
         CKS(set_smem(kern, sm));                                                                                       \
         if (kev >= 0) KEV_BEGIN(kev);                                                                                  \
-        kern<<<dim3(gx, B), 256, sm, ws.stream>>>(ws.Q.as<float>(), ws.qoff.as<int>(), QS, ws.ST16.as<unsigned short>(), \
-                                                  ix->K, ws.qrange.as<float2>(), ws.qflag.as<int>(), ix->w_rev.as<float>(), \
+        kern<<<dim3(gx, B), 256, sm, ws.stream>>>(ws.Q.as<float>(), ws.qoff.as<int>(), QS, ws.qexp.as<int>(),            \
+                                                  ws.ST16.as<unsigned short>(), ix->K, ws.qrange.as<float2>(),         \
+                                                  ws.qflag.as<int>(), ix->w_rev.as<float>(),                           \
                                                   ix->codes.as<uint32_t>(), ix->residuals.as<uint8_t>(),               \
                                                   ix->tok_inv_norm.as<float>(), ws.gbase.as<long long>(),              \
                                                   in.nkept, in.tokp, Mcap, keys, src_rank, ws.qnmax.as<float>(),       \
@@ -1325,7 +1328,7 @@ static pb_status launch_filter(pb_index *ix, Workspace &ws, const KeptView &in, 
         auto kern = nqt == 32 ? k_exact_tc<DV, NB, 32> : k_exact_tc<DV, NB, 64>;                                       \
         CKS(set_smem(kern, sm));                                                                                       \
         KEV_BEGIN(PB_KERNEL_FILTER);                                                                                   \
-        kern<<<dim3(gx, B), 128, sm, ws.stream>>>(ws.Q.as<float>(), ws.qoff.as<int>(), QS,                             \
+        kern<<<dim3(gx, B), 128, sm, ws.stream>>>(ws.Q.as<float>(), ws.qoff.as<int>(), QS, ws.qexp.as<int>(),          \
                                                   ix->centroids_f16.as<__half>(), ix->w_rev.as<float>(),               \
                                                   ix->codes.as<uint32_t>(), ix->residuals.as<uint8_t>(),               \
                                                   ix->doc_off.as<long long>(), in.kept, in.nkept, in.tokp, Mcap, keys); \
@@ -1786,6 +1789,9 @@ static pb_status search_impl_inner(pb_index *ix, const pb_search_params *p, cons
         const float eps_unit = linear ? filter_eps_unit2(ix, tc ? ix->k1_margin : 0) : filter_eps_unit(ix);
         const bool filt = ix->fast_exact && !io.trace && ix->centroids_f16.p && eps_unit > 0.0f && nq_max <= 64 &&
                           top_k < Mcap && ix->packed % 4 == 0;
+        // PB_FILTER_DIAG: the filter runs as usual, then every kept doc is scored exactly (the results of
+        // pb_set_fast_exact(0)) and k_filter_diag compares the pass-1 estimate maxima with the exact ones
+        const bool diag = filt && ix->filter_diag;
         bool pairs = false;
         if (filt) {
             CKS(ws.est.ensure((size_t)B * Mcap * 4));
@@ -1794,10 +1800,11 @@ static pb_status search_impl_inner(pb_index *ix, const pb_search_params *p, cons
             CKS(ws.nkept2.ensure((size_t)B * 4 + 16));
             CKS(ws.tokp2.ensure((size_t)B * (Mcap + 1) * 8));
             CKS(ws.ktok2.ensure((size_t)B * 8 + 16));
-            if (!fast) {  // the two-pass mode computed it with the score range
+            if (!fast) {  // the two-pass mode computed them with the score range
                 CKS(ws.qnmax.ensure((size_t)B * 4 + 16));
+                CKS(ws.qexp.ensure((size_t)B * 4 + 16));
                 k_query_range<<<B, 256, 0, ws.stream>>>(ws.Q.as<float>(), ws.qoff.as<int>(), ix->dim, ix->cmax, nullptr, nullptr,
-                                                        nullptr, ws.qnmax.as<float>());
+                                                        ws.qexp.as<int>(), ws.qnmax.as<float>());
                 CK(cudaGetLastError());
                 L[PB_STAGE_EXACT] += 1;
             }
@@ -1805,15 +1812,17 @@ static pb_status search_impl_inner(pb_index *ix, const pb_search_params *p, cons
             // pair form of the exact stage: pass 2 of the estimate over the survivors lists the (token, q) pairs that can
             // hold a per-token maximum, k_pair_exact evaluates them in the pinned order; a query whose list overflows
             // (or that published no estimate) goes through k_exact
-            pairs = linear && ix->pair_exact && Mcap <= 65535 && QS <= 256;
-            if (pairs) {
+            pairs = !diag && linear && ix->pair_exact && Mcap <= 65535 && QS <= 256;
+            if (pairs || diag) {
                 CKS(ws.estkey.ensure((size_t)B * Mcap * QS * 4));
                 CKS(ws.srcrank.ensure((size_t)B * Mcap * 4));
             }
             CKS(launch_filter(ix, ws, kv, kv2, B, QS, Mcap, top_k, (long long)Mcap * std::max(ix->max_doclen, 1), eps_unit,
-                              nq_max, linear, pairs, &L[PB_STAGE_EXACT]));
-            kv = kv2;
-            if (!sharded) kv.krank = nullptr;  // survivors keep their order, so position breaks ties the same way
+                              nq_max, linear, pairs || diag, &L[PB_STAGE_EXACT]));
+            if (!diag) {
+                kv = kv2;
+                if (!sharded) kv.krank = nullptr;  // survivors keep their order, so position breaks ties the same way
+            }
         }
         if (pairs) {
             const int pair_cap = 16 * Mcap + 4096;  // ~ (top_k + ties) * nq * (1 + a few) pairs per query in practice
@@ -1850,6 +1859,16 @@ static pb_status search_impl_inner(pb_index *ix, const pb_search_params *p, cons
             KEV_END(PB_KERNEL_EXACT);
         } else {
             CKS(launch_exact(ix, ws, kv, B, QS, Mcap, 0, (long long)Mcap * std::max(ix->max_doclen, 1), &L[PB_STAGE_EXACT]));
+        }
+        if (diag) {  // before k_exact_finalize, which clears the exact maxima
+            CKS(ws.fdiag.ensure(16));
+            CK(cudaMemsetAsync(ws.fdiag.p, 0, 16, ws.stream));
+            k_filter_diag<<<dim3(4, B), 256, 0, ws.stream>>>(ws.estkey.as<uint32_t>(), ws.maxkey.as<uint32_t>(), ws.qoff.as<int>(),
+                                                             QS, kv.nkept, Mcap, ws.qnmax.as<float>(),
+                                                             linear ? ws.qflag.as<int>() : nullptr, eps_unit,
+                                                             ws.fdiag.as<unsigned long long>());
+            CK(cudaGetLastError());
+            L[PB_STAGE_EXACT] += 1;
         }
         if (sharded) {
             CKS(ws.payload.ensure((size_t)B * Mcap * 8));
@@ -1957,6 +1976,12 @@ static pb_status search_impl_inner(pb_index *ix, const pb_search_params *p, cons
                     g_stats.kernel_seen[k] = false;
                 }
         }
+        if (diag) {
+            unsigned long long got[2] = {0, 0};
+            CK(cudaMemcpy(got, ws.fdiag.p, 16, cudaMemcpyDeviceToHost));
+            g_stats.work.filter_err_ratio_e6 = std::max<long long>(g_stats.work.filter_err_ratio_e6, (long long)got[0]);
+            g_stats.work.filter_diag_pairs += (long long)got[1];
+        }
         if (fast && ix->k1_diag && ws.k1diag.p) {
             int got[2] = {0, 0};
             CK(cudaMemcpy(got, ws.k1diag.p, 8, cudaMemcpyDeviceToHost));
@@ -2052,7 +2077,9 @@ static void merge_stats(Stats &a, const Stats &b) {
     const int64_t *src = reinterpret_cast<const int64_t *>(&b.work);
     int64_t *dst = reinterpret_cast<int64_t *>(&a.work);
     const size_t kdiff = offsetof(pb_work_counters, k1_tc_max_code_diff) / 8;
-    for (size_t i = 0; i < sizeof(pb_work_counters) / 8; ++i) dst[i] = i == kdiff ? std::max(dst[i], src[i]) : dst[i] + src[i];
+    const size_t kratio = offsetof(pb_work_counters, filter_err_ratio_e6) / 8;
+    for (size_t i = 0; i < sizeof(pb_work_counters) / 8; ++i)
+        dst[i] = (i == kdiff || i == kratio) ? std::max(dst[i], src[i]) : dst[i] + src[i];
 }
 
 // events of the calling thread around a laned call (the lanes' own call events live on different streams)

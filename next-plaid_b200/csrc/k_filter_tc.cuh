@@ -13,10 +13,12 @@
 //     |v - v~| <= u (|c| + |w| + |v|) (1 + 2u)  =>  rho = |v - v~| / |v| <= u ((max|c| + max|w|) / min|v| + 1) (1 + 2u)
 //     |D - D~| <= rho / (1 - rho / 2)             (Dunkl-Williams; min|v| and max|w| are measured at index open)
 //     |q.D - h(q).D~| <= u |q| + (1 + u) |q| |D - D~| + slack               (slack: fp16 subnormals, fp32 sums)
+// with h(q) = 2^-qexp h(2^qexp q): the query enters scaled so that its largest row norm is in [1, 2) (qexp from
+// k_query_range), which keeps the subnormal slack relative to |q|max and rules out fp16 overflow at any query scale
 // so eps_q = |q|max * eps_unit (filter_eps_unit in engine.cu) bounds every similarity and nq * eps_q every
 // doc score.  k_tc_select keeps the docs whose estimate is within 2*nq*eps_q (+ slack) of the
 // top_k-th best estimate -- a superset of the true top_k -- and only those get k_exact.  Non-finite
-// estimates (fp16 overflow included) disable the filter for that query.
+// estimates disable the filter for that query.
 // Operand tile: element (row r, 8-wide K chunk kc) at kc * LBO + (r/8) * 128 + (r%8) * 16 with
 // LBO = 2048 + 32, i.e. at kc * LBO + 16 r: the 32-byte skew makes the 16-byte cp.async scatter of a centroid
 // row bank-conflict free, and one thread decompresses one token (= its accumulator row in the epilogue): the token is
@@ -75,7 +77,8 @@ k_min_vnorm(const float *__restrict__ C, const float *__restrict__ w_rev, int nb
 // reference's ONNX encoder; 3 CTAs/SM)
 template <int DIM, int NBITS, int NQT>
 __global__ void __launch_bounds__(128, NQT == 32 ? 4 : 3)
-k_exact_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, const __half *__restrict__ Ch,
+k_exact_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, const int *__restrict__ qexp,
+           const __half *__restrict__ Ch,
            const float *__restrict__ w_rev, const uint32_t *__restrict__ codes,
            const uint8_t *__restrict__ residuals, const long long *__restrict__ doc_off,
            const uint32_t *__restrict__ kept, const int *__restrict__ n_kept, const long long *__restrict__ tok_prefix,
@@ -107,16 +110,18 @@ k_exact_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, c
     const long long per = (n_chunks + gridDim.x - 1) / gridDim.x;
     const long long c_lo = (long long)blockIdx.x * per, c_hi = min(n_chunks, c_lo + per);
     if (c_lo >= c_hi || nq == 0) return;
+    // the query enters the tensor cores scaled by 2^qexp[b] and the similarities leave scaled by 2^-qexp[b] (exact)
+    const float q_up = ldexpf(1.0f, qexp[b]), q_down = ldexpf(1.0f, -qexp[b]);
     for (int i = threadIdx.x; i < 256 * VB; i += blockDim.x) {
         const int byte = i / VB, j = i - byte * VB;
         Th[i] = __float2half_rn(w_rev[(byte >> (8 - NBITS * (j + 1))) & ((1 << NBITS) - 1)]);
     }
-    // query -> fp16, canonical layout (kc * 4 + r/8) * 128 + (r%8) * 16 + 2e; rows >= nq are zero
+    // query * 2^qexp -> fp16, canonical layout (kc * 4 + r/8) * 128 + (r%8) * 16 + 2e; rows >= nq are zero
     for (int idx = threadIdx.x; idx < NQT * KC; idx += blockDim.x) {
         const int r = idx / KC, kc = idx - r * KC;
         __half v8[8];
 #pragma unroll
-        for (int e = 0; e < 8; ++e) v8[e] = __float2half_rn(r < nq ? Q[(size_t)(r0q + r) * DIM + kc * 8 + e] : 0.0f);
+        for (int e = 0; e < 8; ++e) v8[e] = __float2half_rn(r < nq ? Q[(size_t)(r0q + r) * DIM + kc * 8 + e] * q_up : 0.0f);
         *reinterpret_cast<uint4 *>(Qb + (kc * (NQT / 8) + (r >> 3)) * 128 + (r & 7) * 16) = *reinterpret_cast<uint4 *>(v8);
     }
     const int hl = lane >> 4, kcl = lane & 15;  // staging: one lane per 8-wide K chunk, two centroid rows per instruction
@@ -212,7 +217,7 @@ k_exact_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, c
                 }
                 *reinterpret_cast<uint4 *>(cell) = make_uint4(ow[0], ow[1], ow[2], ow[3]);
             }
-            inv = rsqrtf(fmaxf(p, 1e-24f));
+            inv = rsqrtf(fmaxf(p, 1e-24f)) * q_down;
         } else {
 #pragma unroll
             for (int kc = 0; kc < KC; ++kc) *reinterpret_cast<uint4 *>(As + kc * LBO_A + row * 16) = make_uint4(0, 0, 0, 0);
@@ -285,7 +290,9 @@ k_exact_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, c
 // traffic per token (64-byte table row instead of a 256-byte fp16 centroid row), about half the instructions,
 // and a tighter certificate, because the centroid part is known to a 16-bit code instead of fp16 rounding:
 //     |q.c - s~|           <= (E + 1.01) * 2R / 65535          (s~ = centre of the code; E = 0 for the exact table)
-//     |q.w - h(q).h(w)|    <= |q| max|w| (2u + u^2 + 2^-15)    (u = 2^-11; products exact, fp32 accumulation)
+//     |q.w - h(q).h(w)|    <= |q| max|w| (2u + u^2 + 2^-15)    (u = 2^-11; products exact, fp32 accumulation;
+//                                                               h(q) = 2^-qexp h(2^qexp q) as above, so the 2^-15 of
+//                                                               subnormals and fp32 sums holds at every query scale)
 //     |1/|v| - inv|        <= 2^-20 / |v|
 // so |q.D - est| <= |q|max * eps_unit2 with eps_unit2 = ((E + 1.01) 2 cmax 1.0001 / 65535 + wmax (2u + u^2 + 2^-15)) / vmin
 // + 8e-6 (filter_eps_unit2 in engine.cu).  Flagged queries (no valid table) publish nothing -> no estimate -> every
@@ -316,6 +323,45 @@ k_tc_finalize(uint32_t *__restrict__ maxkey, const int *__restrict__ q_off, int 
         tot = 0.0f;
     }
     if (lane == 0) est[(size_t)b * Mcap + r] = bad ? NAN : tot;
+}
+
+// PB_FILTER_DIAG: the pass-1 estimate of every (kept doc, query token) maximum (est) against the exact maximum of the
+// same pair (exact, k_exact's keys), in units of the certified bound qnmax[b] * eps_unit.  out[0] = ceil(1e6 * the
+// largest ratio) (INT64_MAX: a non-finite estimate of a finite maximum), out[1] += the pairs compared.  A doc without
+// tokens has no maximum; a flagged query (qflag: no estimate by design, the filter keeps all its docs) is skipped.
+__global__ void __launch_bounds__(256)
+k_filter_diag(const uint32_t *__restrict__ est, const uint32_t *__restrict__ exact, const int *__restrict__ q_off, int QS,
+              const int *__restrict__ n_kept, int Mcap, const float *__restrict__ qnmax, const int *__restrict__ qflag,
+              float eps_unit, unsigned long long *__restrict__ out) {
+    const int b = blockIdx.y;
+    if (qflag && qflag[b]) return;
+    const int nq = q_off[b + 1] - q_off[b];
+    const long long n = (long long)n_kept[b] * nq;
+    const double unit = (double)qnmax[b] * (double)eps_unit;
+    const unsigned long long sat = 0x7fffffffffffffffull;
+    unsigned long long worst = 0ull, cnt = 0ull;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const size_t at = ((size_t)b * Mcap + (size_t)(i / nq)) * QS + (size_t)(i % nq);
+        const uint32_t xk = exact[at], ek = est[at];
+        if (!xk) continue;
+        ++cnt;
+        unsigned long long v = sat;
+        if (ek) {
+            const double d = fabs((double)key_to_score(ek) - (double)key_to_score(xk));
+            const double r = unit > 0.0 ? ceil(1e6 * d / unit) : (d == 0.0 ? 0.0 : 1e300);
+            v = r < 9.0e18 ? (unsigned long long)r : sat;
+        }
+        worst = v > worst ? v : worst;
+    }
+    for (int m = 16; m >= 1; m >>= 1) {
+        const unsigned long long ow = __shfl_xor_sync(PB_FULL, worst, m), oc = __shfl_xor_sync(PB_FULL, cnt, m);
+        worst = ow > worst ? ow : worst;
+        cnt += oc;
+    }
+    if ((threadIdx.x & 31) == 0 && cnt) {
+        atomicMax(out, worst);
+        atomicAdd(out + 1, cnt);
+    }
 }
 
 // survivors of the filter, in approximate-rank order.  grid = B, 1024 threads, smem = pow2(n_kept) * 8.

@@ -3,8 +3,8 @@
 // Part of kernels.cuh (included from there, in order; not a standalone header).
 // ==========================================================================================
 // k_maxsim_tc estimates every similarity of a kept doc's tokens as sim~ = (q.w + s~(code)) / |v| (residual part on the
-// tensor cores, centroid score from the 16-bit table, stored norm; bound eps_q = |q|max * filter_eps_unit2 on every
-// similarity, DESIGN.md 4c), with the producer and consumer phases of a 128-token chunk on different warpgroups so that
+// tensor cores from the query scaled by 2^qexp, centroid score from the 16-bit table, stored norm; bound
+// eps_q = |q|max * filter_eps_unit2 on every similarity, DESIGN.md 4c), with the producer and consumer phases of a 128-token chunk on different warpgroups so that
 // they overlap inside one CTA:
 //   warps 4-7  producers: locate the chunk's tokens, read the packed residuals, expand them to fp16 straight
 //              into a 2-stage operand ring (thread = token row);
@@ -83,7 +83,8 @@ PB_DEV TokMeta ms_locate(long long s, long long T, int r_lo, int nk, const long 
 
 template <int DIM, int NBITS, int NQT, bool EMIT>
 __global__ void __launch_bounds__(256, NQT == 32 ? 2 : 1)  // NQT = 64: ~129 KB of shared memory, one CTA per SM
-k_maxsim_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, const unsigned short *__restrict__ ST16,
+k_maxsim_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, const int *__restrict__ qexp,
+            const unsigned short *__restrict__ ST16,
             long long K, const float2 *__restrict__ qrange, const int *__restrict__ qflag, const float *__restrict__ w_rev,
             const uint32_t *__restrict__ codes, const uint8_t *__restrict__ residuals, const float *__restrict__ inv_norm,
             const long long *__restrict__ gbase, const int *__restrict__ n_kept,
@@ -122,6 +123,9 @@ k_maxsim_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, 
     const long long c_lo = (long long)blockIdx.x * per, c_hi = min(n_chunks, c_lo + per);
     if (c_lo >= c_hi || nq == 0 || qflag[b]) return;
     const int n = (int)(c_hi - c_lo);
+    // the query enters the tensor cores scaled by 2^qexp[b] (largest row norm in [1, 2): no fp16 overflow, no
+    // subnormal coordinates of the rows that matter) and the products leave scaled by 2^-qexp[b]; both exact
+    const float q_up = ldexpf(1.0f, qexp[b]), q_down = ldexpf(1.0f, -qexp[b]);
     for (int i = threadIdx.x; i < 256 * VB * TR; i += blockDim.x) {
         const int byte = i / (VB * TR), j = i % VB;
         Th[i] = __float2half_rn(w_rev[(byte >> (8 - NBITS * (j + 1))) & ((1 << NBITS) - 1)]);
@@ -130,7 +134,7 @@ k_maxsim_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, 
         const int r = idx / KC, kc = idx - r * KC;
         __half v8[8];
 #pragma unroll
-        for (int e = 0; e < 8; ++e) v8[e] = __float2half_rn(r < nq ? Q[(size_t)(r0q + r) * DIM + kc * 8 + e] : 0.0f);
+        for (int e = 0; e < 8; ++e) v8[e] = __float2half_rn(r < nq ? Q[(size_t)(r0q + r) * DIM + kc * 8 + e] * q_up : 0.0f);
         *reinterpret_cast<uint4 *>(Qb + (kc * (NQT / 8) + (r >> 3)) * 128 + (r & 7) * 16) = *reinterpret_cast<uint4 *>(v8);
     }
     if (threadIdx.x == 0) {
@@ -234,11 +238,13 @@ k_maxsim_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, 
         // ================= consumers: MMA + epilogue =================
         const int t = threadIdx.x;
         const float2 rg = qrange[b];
-        const float inv_scale = 1.0f / rg.y, s_bias = (0.5f - rg.x) / rg.y;
+        const float inv_scale0 = 1.0f / rg.y, s_bias = (0.5f - rg.x) / rg.y;
         // code -> score without an int-to-float conversion: PRMT puts the 16-bit code under the exponent of 2^23
         // (float 2^23 + code, exact) and one FFMA applies scale and bias; 2^23 * inv_scale is exact, the folded
-        // constant is rounded once (<= half an ulp of ~2^8: 1.6e-5, a per-query constant that filter_eps_unit2 carries)
-        const float s_bias23 = s_bias - 8388608.0f * inv_scale;
+        // constant is rounded once (<= half an ulp of ~2^8: 1.6e-5, a per-query constant that filter_eps_unit2 carries).
+        // The centroid score joins the scaled accumulator scaled by 2^qexp too, and 1/|v| carries the 2^-qexp back:
+        // every step is the unscaled one times a power of two
+        const float inv_scale = inv_scale0 * q_up, s_bias23 = (s_bias - 8388608.0f * inv_scale0) * q_up;
         const char *STb = reinterpret_cast<const char *>(ST16 + (size_t)b * K * QS);
         const unsigned rowb = (unsigned)QS * 2u;
         const float band = EMIT ? 2.0f * band_unit * qnmax[b] + 1e-6f : 0.0f;
@@ -267,7 +273,7 @@ k_maxsim_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, 
                     sw[4 * i + 2] = t4.z;
                     sw[4 * i + 3] = t4.w;
                 }
-                inv = inv_norm[m.g];
+                inv = inv_norm[m.g] * q_down;
             } else {
 #pragma unroll
                 for (int i = 0; i < SW; ++i) sw[i] = 0u;

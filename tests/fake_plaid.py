@@ -68,7 +68,7 @@ class MmapIndex:
                          n_exact_tokens=300 * len(queries), n_filter_docs=50 * len(queries),
                          n_filter_tokens=1500 * len(queries), k1_tc_max_code_diff=0, k1_rows_mismatch=0,
                          n_probe_threshold=0, n_probe_list=0, n_k1_tc=1, n_recheck_docs=0, n_k1_tc_redo=0, n_exact_pairs=0,
-                         n_pair_fallback_queries=0)
+                         n_pair_fallback_queries=0, filter_err_ratio_e6=0, filter_diag_pairs=0)
         return out
 
     def _raw(self, qptr, offs, params, ids_ptr, sc_ptr, cn_ptr):
