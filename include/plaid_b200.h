@@ -201,6 +201,46 @@ PB_API pb_status pb_index_delete(pb_index *ix, const int64_t *doc_ids, int64_t n
  * (1 / |c + w|, vmin, wmax) over the remaining tokens. */
 PB_API pb_status pb_last_delete_ms(pb_index *ix, float *out_ms);
 
+/* ---- appends and deletes on a doc-sharded deployment --------------------------------------- */
+
+/* pb_index_delete / pb_index_append / pb_index_append_encoded on a doc-sharded deployment, collectively: the result on
+ * every rank is what the single-handle call gives on one handle holding the whole index.  Calling rules, as for a
+ * sharded search: every rank of a handle joined by pb_index_comm_init or pb_index_group_join makes the call, at the
+ * same position in its sequence of collective calls, with the same doc_ids / doc_lengths, n_*, batch_size and the
+ * same index_dir (or NULL on all).  Only rank world - 1 reads codec, embeddings, codes and residuals; the other ranks
+ * may pass NULL.  A handle outside any group is a group of one.
+ *
+ * Every call checks that the ranks' ranges [doc_id_base_r, doc_id_base_r + D_r) tile [0, D_total) in rank order
+ * (shards of pb_index_load_range over pb_index_dir_shard_bounds do), that K, dim and nbits agree, and that every rank
+ * got the same arguments.  On a local failure every rank returns the status of the lowest failing rank, with a message
+ * naming it; on a layout or argument mismatch every rank returns PB_ERR_INVALID.  Either way nothing changes on any
+ * rank or on disk.  Group members opened with PB_OPEN_ADOPT_RESIDUALS are refused with PB_ERR_UNSUPPORTED.
+ *
+ * Delete: rank r removes the ids in its range and renumbers its survivors; its doc_id_base drops by the number of
+ * documents removed from the ranks below it.  Afterwards each rank is exactly pb_index_open of its new range of the
+ * remaining documents, with that range's slice of the new inverted file; the ranges tile [0, D_total - removed) again
+ * and a rank may be left empty.  out_deleted receives the number removed over all ranks.  A delete that removes no
+ * document changes nothing anywhere.
+ * Append: the documents get ids D_total .. and all go to rank world - 1, which keeps the ranges contiguous; the other
+ * ranks change nothing.  out_first_doc_id receives D_total on every rank.  Capacity on the last rank comes from
+ * pb_index_reserve called before the handle joins the group.
+ *
+ * index_dir: rank world - 1 checks that metadata.json holds D_total documents and writes the directory's changes,
+ * computing the new ivf.npy / ivf_lengths.npy from ivf.npy as it is on disk; the files equal, byte for byte, what the
+ * single-handle call writes on a handle holding the whole index.  If the write fails no rank changes (files already
+ * renamed stay, as with the single-handle calls).
+ *
+ * After the vote every rank commits, and from there only a CUDA runtime error can fail a rank.  Such a failure leaves
+ * the group inconsistent: reload the deployment (from the directory, when one is kept in sync). */
+PB_API pb_status pb_index_delete_sharded(pb_index *ix, const int64_t *doc_ids, int64_t n_ids, const char *index_dir,
+                                         int64_t *out_deleted);
+PB_API pb_status pb_index_append_sharded(pb_index *ix, pb_codec *codec, const float *embeddings, const int64_t *doc_lengths,
+                                         int64_t n_docs, int32_t memory_space, const char *index_dir, int64_t batch_size,
+                                         int64_t *out_first_doc_id);
+PB_API pb_status pb_index_append_encoded_sharded(pb_index *ix, const int64_t *codes, const uint8_t *residuals,
+                                                 const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
+                                                 int64_t *out_first_doc_id);
+
 /* ---- search ------------------------------------------------------------------------------ */
 
 /*

@@ -283,6 +283,12 @@ static pb_status read_dir_meta(const std::string &dir, int nbits, long long old_
     return PB_OK;
 }
 
+pb_status pb_dir_check_documents(const char *index_dir, int nbits, long long D) {
+    long long num_chunks = 0, num_emb = 0;
+    double avg_doclen = 0;
+    return read_dir_meta(std::string(index_dir) + "/", nbits, D, num_chunks, num_emb, avg_doclen);
+}
+
 // ivf.npy / ivf_lengths.npy
 static pb_status write_ivf(const std::string &dir, long long K, const int64_t *ivf, long long ivf_total,
                            const int32_t *ivf_lengths) {

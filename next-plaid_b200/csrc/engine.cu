@@ -80,8 +80,9 @@ struct pb_shard_group {
     int joined = 0;
     std::vector<const void *> send;
     std::vector<int> dev;
-    // false = a peer failed or did not arrive within the timeout; the group stays broken
-    bool barrier() {
+    // false = a peer failed or did not arrive within the timeout; the group stays broken.  unbounded: wait for the
+    // peers however long they take (a peer that fails still breaks the group), for a peer known to be busy
+    bool barrier(bool unbounded = false) {
         std::unique_lock<std::mutex> g(mu);
         if (broken) return false;
         const unsigned long long my = gen;
@@ -91,7 +92,9 @@ struct pb_shard_group {
             cv.notify_all();
             return true;
         }
-        if (!cv.wait_for(g, std::chrono::seconds(60), [&] { return gen != my || broken; })) broken = true;
+        auto done = [&] { return gen != my || broken; };
+        if (unbounded) cv.wait(g, done);
+        else if (!cv.wait_for(g, std::chrono::seconds(60), done)) broken = true;
         if (broken) cv.notify_all();
         return !broken;
     }
@@ -539,13 +542,16 @@ static pb_status exclusive_sum(const long long *in, long long *out, long long n,
     return PB_OK;
 }
 
-// The inverted file of an index opened without one, as the part of a directory's ivf.npy (host, total entries,
-// lengths [K]) that lies in docs [b, e): every list filtered to the range in file order, ids minus b.  The file goes
-// through a staging buffer of at most 2^26 entries (PB_LOAD_IVF_SLAB sets another size): a count pass, then the
-// write pass into the exactly sized ivf, which copies the file a second time when it is more than one slab.  Any entry
-// outside [0, limit) fails.
-pb_status pb_index_upload_ivf_range(pb_index *ix, const int64_t *ivf, const int32_t *lengths, long long total,
-                                    long long limit, long long b, long long e) {
+// An inverted file computed from a directory's ivf.npy (host, total entries, lengths [K], global ids) into (out, out_off,
+// *out_len): every list filtered to docs [b, e) in file order, ids minus b.  With a deleted set (bits, word_pre over
+// the directory's docs, b = 0) its ids leave the lists too and survivors are renumbered (delete.rs:196-237); with
+// the sorted (centroid, doc) keys of m appended docs, each list is followed by its new pairs as ids limit + doc
+// (update.rs:1000-1067).  The file goes through a staging buffer of at most 2^26 entries (PB_LOAD_IVF_SLAB sets
+// another size): a count pass, then the write pass into the exactly sized output, which copies the file a second time
+// when it is more than one slab.  Any entry outside [0, limit) fails.
+static pb_status ivf_from_file(pb_index *ix, const int64_t *ivf, const int32_t *lengths, long long total, long long limit,
+                               long long b, long long e, const uint32_t *bits, const long long *word_pre, const u64 *keys,
+                               long long m_keys, DevBuf &out, DevBuf &out_off, long long *out_len) {
     CK(cudaSetDevice(ix->device));
     const long long K = ix->K;
     std::vector<long long> foff((size_t)K + 1, 0);
@@ -572,27 +578,38 @@ pb_status pb_index_upload_ivf_range(pb_index *ix, const int64_t *ivf, const int3
     DevBuf cur;
     CKS(cur.ensure((size_t)(K + 1) * 8));
     auto write = [&](long long o, long long m, long long c0, long long c1) -> pb_status {
-        k_ivf_range_write<<<grid, 256>>>(stage.as<long long>(), o, m, doff.as<long long>(), c0, c1, b, e,
-                                         cur.as<long long>(), ix->ivf.as<uint32_t>());
+        k_ivf_range_write<<<grid, 256>>>(stage.as<long long>(), o, m, doff.as<long long>(), c0, c1, b, e, bits, word_pre,
+                                         cur.as<long long>(), out.as<uint32_t>());
         CK(cudaGetLastError());
         return PB_OK;
     };
-    // For the whole index every valid entry is kept: the offsets are the file's, and each slab is written as soon as it
-    // is counted, so the file is copied once.  Otherwise the write pass waits for the scan of all the counts.
-    const bool whole = b == 0 && e >= limit;
-    CKS(ix->ivf_off.ensure((size_t)(K + 1) * 8));
+    // When every valid entry is kept the offsets are the file's (shifted by the new pairs before each list), and each
+    // slab is written as soon as it is counted, so the file is copied once.  Otherwise the write pass waits for the
+    // scan of all the counts.
+    const bool whole = b == 0 && e >= limit && !bits;
+    CKS(out_off.ensure((size_t)(K + 1) * 8));
     if (whole) {
-        CK(cudaMemcpy(ix->ivf_off.p, doff.p, (size_t)(K + 1) * 8, cudaMemcpyDeviceToDevice));
-        CK(cudaMemcpy(cur.p, doff.p, (size_t)(K + 1) * 8, cudaMemcpyDeviceToDevice));
-        ix->ivf_len = total;
-        CKS(ix->ivf.ensure(std::max<size_t>((size_t)total * 4, 16)));
+        if (m_keys > 0) {  // new_off[c] = file_off[c] + new pairs of the centroids below c
+            CKS(tmp.ensure((size_t)(K + 1) * 8));
+            k_ivf_offsets<<<(unsigned)((K + 256) / 256), 256>>>(keys, m_keys, K, tmp.as<long long>());
+            CK(cudaGetLastError());
+            std::vector<long long> before((size_t)K + 1);
+            CK(cudaMemcpy(before.data(), tmp.p, before.size() * 8, cudaMemcpyDeviceToHost));
+            for (long long c = 0; c <= K; ++c) before[c] += foff[c];
+            CK(cudaMemcpy(out_off.p, before.data(), before.size() * 8, cudaMemcpyHostToDevice));
+        } else {
+            CK(cudaMemcpy(out_off.p, doff.p, (size_t)(K + 1) * 8, cudaMemcpyDeviceToDevice));
+        }
+        CK(cudaMemcpy(cur.p, out_off.p, (size_t)(K + 1) * 8, cudaMemcpyDeviceToDevice));
+        *out_len = total + std::max(m_keys, 0ll);
+        CKS(out.ensure(std::max<size_t>((size_t)*out_len * 4, 16)));
     }
     for (long long o = 0; o < total; o += slab) {
         const long long m = std::min(slab, total - o);
         long long c0, c1;
         lists(o, m, c0, c1);
         CK(cudaMemcpy(stage.p, ivf + o, (size_t)m * 8, cudaMemcpyHostToDevice));
-        k_ivf_range_count<<<grid, 256>>>(stage.as<long long>(), o, m, doff.as<long long>(), c0, c1, limit, b, e,
+        k_ivf_range_count<<<grid, 256>>>(stage.as<long long>(), o, m, doff.as<long long>(), c0, c1, limit, b, e, bits,
                                          cnt.as<long long>(), bad.as<int>());
         CK(cudaGetLastError());
         if (whole) CKS(write(o, m, c0, c1));
@@ -600,12 +617,14 @@ pb_status pb_index_upload_ivf_range(pb_index *ix, const int64_t *ivf, const int3
     int hbad = 0;
     CK(cudaMemcpy(&hbad, bad.p, 4, cudaMemcpyDeviceToHost));
     if (hbad) return pb_fail(PB_ERR_INVALID, "ivf contains a value outside [0, %lld)", limit);
+    if (whole && m_keys > 0)  // the j-th new pair of centroid c after c's file list: file_off[c + 1] + j
+        k_ivf_merge_new<<<grid, 256>>>(keys, m_keys, doff.as<long long>(), (uint32_t)limit, out.as<uint32_t>());
     if (!whole) {
-        CKS(exclusive_sum(cnt.as<long long>(), ix->ivf_off.as<long long>(), K + 1, tmp));
-        CK(cudaMemcpy(&ix->ivf_len, ix->ivf_off.as<long long>() + K, 8, cudaMemcpyDeviceToHost));
-        CKS(ix->ivf.ensure(std::max<size_t>((size_t)ix->ivf_len * 4, 16)));
-        CK(cudaMemcpy(cur.p, ix->ivf_off.p, (size_t)K * 8, cudaMemcpyDeviceToDevice));
-        for (long long o = 0; ix->ivf_len > 0 && o < total; o += slab) {
+        CKS(exclusive_sum(cnt.as<long long>(), out_off.as<long long>(), K + 1, tmp));
+        CK(cudaMemcpy(out_len, out_off.as<long long>() + K, 8, cudaMemcpyDeviceToHost));
+        CKS(out.ensure(std::max<size_t>((size_t)*out_len * 4, 16)));
+        CK(cudaMemcpy(cur.p, out_off.p, (size_t)K * 8, cudaMemcpyDeviceToDevice));
+        for (long long o = 0; *out_len > 0 && o < total; o += slab) {
             const long long m = std::min(slab, total - o);
             long long c0, c1;
             lists(o, m, c0, c1);
@@ -613,7 +632,16 @@ pb_status pb_index_upload_ivf_range(pb_index *ix, const int64_t *ivf, const int3
             CKS(write(o, m, c0, c1));
         }
     }
+    CK(cudaGetLastError());
     CK(cudaDeviceSynchronize());
+    return PB_OK;
+}
+
+// The inverted file of an index opened without one, as the part of a directory's ivf.npy that lies in docs [b, e)
+pb_status pb_index_upload_ivf_range(pb_index *ix, const int64_t *ivf, const int32_t *lengths, long long total,
+                                    long long limit, long long b, long long e) {
+    CKS(ivf_from_file(ix, ivf, lengths, total, limit, b, e, nullptr, nullptr, nullptr, 0, ix->ivf, ix->ivf_off,
+                      &ix->ivf_len));
     ix->build_ivf = false;
     return PB_OK;
 }
@@ -1158,8 +1186,10 @@ static pb_status launch_centroid_scores_exact(pb_index *ix, Workspace &ws, int B
     return PB_OK;
 }
 
-// all-gather of `count` 64-bit words per rank over whichever transport the handle joined
-static pb_status shard_allgather(pb_index *ix, cudaStream_t stream, const void *send, void *recv, size_t count) {
+// all-gather of `count` 64-bit words per rank over whichever transport the handle joined.  unbounded: the in-process
+// group waits for late peers without its 60 s timeout (NCCL waits either way)
+static pb_status shard_allgather(pb_index *ix, cudaStream_t stream, const void *send, void *recv, size_t count,
+                                 bool unbounded = false) {
     if (ix->comm) {
         CKN(g_nccl.AllGather(send, recv, count, PB_NCCL_UINT64, ix->comm, stream));
         return PB_OK;
@@ -1172,7 +1202,7 @@ static pb_status shard_allgather(pb_index *ix, cudaStream_t stream, const void *
         return pb_fail(PB_ERR_CUDA, "cudaStreamSynchronize failed: %s", cudaGetErrorString(e));
     }
     g->send[ix->rank] = send;
-    if (!g->barrier()) return pb_fail(PB_ERR_COMM, "shard group: a peer failed or timed out");
+    if (!g->barrier(unbounded)) return pb_fail(PB_ERR_COMM, "shard group: a peer failed or timed out");
     for (int p = 0; p < g->world && e == cudaSuccess; ++p)
         e = cudaMemcpyPeerAsync(static_cast<char *>(recv) + (size_t)p * count * 8, ix->device, g->send[p], g->dev[p],
                                 count * 8, stream);
@@ -3033,18 +3063,53 @@ extern "C" pb_status pb_codec_find_outliers(pb_codec *c, const float *embeddings
 // ------------------------------------------------------------------------------------------
 // incremental append: MmapIndex::update_append (index.rs:1675) + reload on a live handle
 // ------------------------------------------------------------------------------------------
-static pb_status append_impl(pb_index *ix, pb_codec *codec, const float *embeddings, const int64_t *codes,
-                             const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs, int32_t space,
-                             const char *index_dir, int64_t batch_size, int64_t *out_first) {
-    if (!ix || (!doc_lengths && n_docs) || n_docs < 0) return pb_fail(PB_ERR_INVALID, "null argument");
-    if (space != PB_MEM_HOST && space != PB_MEM_DEVICE) return pb_fail(PB_ERR_INVALID, "bad memory_space %d", space);
-    std::lock_guard<std::mutex> gate(ix->gate);
-    std::unique_lock<std::shared_mutex> wr(ix->rw);
-    if (ix->comm || ix->group) return pb_fail(PB_ERR_UNSUPPORTED, "appends to a doc-sharded handle are not supported");
-    if (!ix->residuals.owned)
-        return pb_fail(PB_ERR_UNSUPPORTED, "the handle uses the caller's residual array (PB_OPEN_ADOPT_RESIDUALS)");
-    if (index_dir && ix->doc_id_base != 0) return pb_fail(PB_ERR_UNSUPPORTED, "an index directory holds doc ids from 0");
-    if (index_dir && batch_size <= 0) return pb_fail(PB_ERR_INVALID, "batch_size must be positive");
+// the u32 inverted file ivf [L] at off [K + 1] on the host in the directory's dtypes: ivf.npy <i8, ivf_lengths.npy <i4
+// (widened on the device one slab of at most 2^26 entries at a time, so the i64 copy is never whole on the device)
+static pb_status ivf_to_host(pb_index *ix, const DevBuf &ivf, const DevBuf &off, long long L, std::vector<int64_t> &hivf,
+                             std::vector<int32_t> &hlen) {
+    hivf.assign((size_t)std::max(L, 1ll), 0);
+    hlen.assign((size_t)ix->K, 0);
+    const long long slab = 1ll << 26;
+    DevBuf di, dln;
+    CKS(di.ensure(std::max<size_t>((size_t)std::min(L, slab) * 8, 16)));
+    CKS(dln.ensure((size_t)ix->K * 4));
+    for (long long o = 0; o < std::max(L, 1ll); o += slab) {  // the first launch also writes the lengths
+        const long long m = std::min(slab, L - o);
+        k_ivf_export<<<ix->sm_count * 8, 256>>>(ivf.as<uint32_t>() + o, off.as<long long>(), m, ix->K, 0,
+                                               di.as<long long>(), o == 0 ? dln.as<int>() : nullptr);
+        CK(cudaGetLastError());
+        if (m > 0) CK(cudaMemcpy(hivf.data() + o, di.p, (size_t)m * 8, cudaMemcpyDeviceToHost));
+    }
+    CK(cudaMemcpy(hlen.data(), dln.p, (size_t)ix->K * 4, cudaMemcpyDeviceToHost));
+    return PB_OK;
+}
+
+pb_status pb_index_patch_ivf(pb_index *ix, const int64_t *file_ivf, const int32_t *file_lengths, long long total, long long D,
+                             const uint32_t *bits, const long long *word_pre, const uint64_t *keys, long long m,
+                             std::vector<int64_t> &ivf, std::vector<int32_t> &lengths) {
+    DevBuf out, off;
+    long long L = 0;
+    CKS(ivf_from_file(ix, file_ivf, file_lengths, total, D, 0, D, bits, word_pre,
+                      reinterpret_cast<const u64 *>(keys), m, out, off, &L));
+    return ivf_to_host(ix, out, off, L, ivf, lengths);
+}
+
+// What an append computes before anything becomes visible: the new tokens in the tails of the per-token arrays, the
+// new docs' offsets and distinct codes, the merged inverted file in the spare half of the ping-pong, and the totals the
+// commit publishes.  keys holds the new docs' sorted (centroid << 32 | doc in the batch) pairs.
+struct AppendPrep {
+    long long D0 = 0, n = 0, ntok = 0, N1 = 0, D1 = 0, U1 = 0, L1 = 0, m = 0;
+    int maxlen = 0;
+    float vmin = 0.f, wmax = 0.f;
+    std::vector<int64_t> dl, hcodes;  // doc lengths; the i64 codes for a directory (keep_codes)
+    DevBuf keys;
+};
+
+// Every check, allocation and device write of an append that stays invisible until append_commit.  The caller holds
+// the handle's writer lock.
+static pb_status append_prepare(pb_index *ix, pb_codec *codec, const float *embeddings, const int64_t *codes,
+                                const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs, int32_t space,
+                                bool keep_codes, int64_t *out_first, AppendPrep &p) {
     CK(cudaSetDevice(ix->device));
     CK(cudaDeviceSynchronize());  // work earlier readers left queued (pb_search_batch_device) reads the arrays
     if (codec) {  // same K, dim, nbits and bit-identical centroids as the index; cutoffs required (codec.rs:359-362)
@@ -3064,7 +3129,8 @@ static pb_status append_impl(pb_index *ix, pb_codec *codec, const float *embeddi
     }
     const long long D0 = ix->D, N0 = ix->N, U0 = ix->n_ucodes, n = n_docs;
     if (out_first) *out_first = ix->doc_id_base + D0;
-    std::vector<int64_t> dl;
+    p.D0 = D0;
+    std::vector<int64_t> &dl = p.dl;
     CKS(fetch_host(dl, doc_lengths, (size_t)n, space));
     std::vector<long long> doff((size_t)n, 0);  // doc_off[D0 + 1 ..]
     long long ntok = 0;
@@ -3092,7 +3158,7 @@ static pb_status append_impl(pb_index *ix, pb_codec *codec, const float *embeddi
     CKS(ix->udoc_off.grow((size_t)(D1 + 1) * 8, (size_t)(D0 + 1) * 8));
 
     // 1. tokens into the tails of codes / residuals: encoded on the device, or narrowed and range-checked
-    std::vector<int64_t> hcodes;  // i64 codes for the chunk files
+    std::vector<int64_t> &hcodes = p.hcodes;  // i64 codes for the chunk files
     if (codec) {
         codec->last_tokens = ntok;
         codec->last_fallback = 0;
@@ -3100,7 +3166,7 @@ static pb_status append_impl(pb_index *ix, pb_codec *codec, const float *embeddi
         DevBuf dX, dcodes;
         CKS(dcodes.ensure((size_t)std::max(std::min(ntok, slab), 1ll) * 8));
         if (space == PB_MEM_HOST) CKS(dX.ensure((size_t)std::max(std::min(ntok, slab), 1ll) * ix->dim * 4));
-        if (index_dir) hcodes.resize((size_t)ntok);
+        if (keep_codes) hcodes.resize((size_t)ntok);
         for (long long o = 0; o < ntok; o += slab) {
             const long long m = std::min(slab, ntok - o);
             const float *x = embeddings + (size_t)o * ix->dim;
@@ -3110,7 +3176,7 @@ static pb_status append_impl(pb_index *ix, pb_codec *codec, const float *embeddi
             }
             CKS(codec_encode_device(codec, x, m, dcodes.as<long long>(), ix->residuals.as<uint8_t>() + (size_t)(N0 + o) * pk, nullptr));
             CKS(upload_narrow(ix->codes, N0 + o, reinterpret_cast<const int64_t *>(dcodes.p), m, ix->K, PB_MEM_DEVICE, "codes"));
-            if (index_dir) CK(cudaMemcpy(hcodes.data() + o, dcodes.p, (size_t)m * 8, cudaMemcpyDeviceToHost));
+            if (keep_codes) CK(cudaMemcpy(hcodes.data() + o, dcodes.p, (size_t)m * 8, cudaMemcpyDeviceToHost));
         }
     } else if (ntok > 0) {
         CK(cudaMemcpy(ix->residuals.as<uint8_t>() + (size_t)N0 * pk, residuals, (size_t)ntok * pk,
@@ -3161,51 +3227,84 @@ static pb_status append_impl(pb_index *ix, pb_codec *codec, const float *embeddi
     }
 
     // 5. inverted file: the new docs' sorted distinct (centroid, doc) pairs merged behind each centroid's old list
-    DevBuf keys, add_before;
+    DevBuf add_before;
     long long m = 0;
-    CKS(sorted_doc_pairs(ix, D0, n, U1 - U0, keys, &m));
+    CKS(sorted_doc_pairs(ix, D0, n, U1 - U0, p.keys, &m));
     const long long L1 = ix->ivf_len + m;
     if (L1 > (1ll << 31) - 2) return pb_fail(PB_ERR_UNSUPPORTED, "more than 2^31 (centroid, doc) pairs per shard");
     CKS(add_before.ensure((size_t)(ix->K + 1) * 8));
     CKS(ix->ivf_spare.grow(std::max<size_t>((size_t)L1 * 4, 16), 0));
     CKS(ix->ivf_off_spare.ensure((size_t)(ix->K + 1) * 8));
-    k_ivf_offsets<<<(unsigned)((ix->K + 256) / 256), 256>>>(keys.as<u64>(), m, ix->K, add_before.as<long long>());
+    k_ivf_offsets<<<(unsigned)((ix->K + 256) / 256), 256>>>(p.keys.as<u64>(), m, ix->K, add_before.as<long long>());
     k_ivf_merge_old<<<ix->sm_count * 8, 256>>>(ix->ivf.as<uint32_t>(), ix->ivf_off.as<long long>(), add_before.as<long long>(),
                                                ix->K, ix->ivf_spare.as<uint32_t>(), ix->ivf_off_spare.as<long long>());
     if (m > 0)
-        k_ivf_merge_new<<<ix->sm_count * 8, 256>>>(keys.as<u64>(), m, ix->ivf_off.as<long long>(), (uint32_t)D0,
+        k_ivf_merge_new<<<ix->sm_count * 8, 256>>>(p.keys.as<u64>(), m, ix->ivf_off.as<long long>(), (uint32_t)D0,
                                                    ix->ivf_spare.as<uint32_t>());
     CK(cudaGetLastError());
     CK(cudaDeviceSynchronize());
+    p.n = n;
+    p.ntok = ntok;
+    p.N1 = N1;
+    p.D1 = D1;
+    p.U1 = U1;
+    p.L1 = L1;
+    p.m = m;
+    p.maxlen = maxlen;
+    p.vmin = vmin;
+    p.wmax = wmax;
+    return PB_OK;
+}
 
-    // update_index's file changes, before the commit: a failure leaves the handle as it was
-    if (index_dir) {
-        std::vector<uint8_t> hres((size_t)ntok * pk);
-        if (ntok) CK(cudaMemcpy(hres.data(), ix->residuals.as<uint8_t>() + (size_t)N0 * pk, hres.size(), cudaMemcpyDeviceToHost));
-        std::vector<int64_t> hivf((size_t)std::max(L1, 1ll));
-        std::vector<int32_t> hlen((size_t)ix->K);
-        DevBuf di, dln;
-        CKS(di.ensure(std::max<size_t>((size_t)L1 * 8, 16)));
-        CKS(dln.ensure((size_t)ix->K * 4));
-        k_ivf_export<<<ix->sm_count * 8, 256>>>(ix->ivf_spare.as<uint32_t>(), ix->ivf_off_spare.as<long long>(), L1, ix->K, 0,
-                                               di.as<long long>(), dln.as<int>());
-        CK(cudaGetLastError());
-        if (L1) CK(cudaMemcpy(hivf.data(), di.p, (size_t)L1 * 8, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(hlen.data(), dln.p, (size_t)ix->K * 4, cudaMemcpyDeviceToHost));
-        CKS(pb_dir_append(index_dir, D0, ix->K, ix->dim, ix->nbits, batch_size, hcodes.data(), hres.data(), dl.data(), n,
-                          hivf.data(), L1, hlen.data()));
-    }
+// update_index's file changes for the prepared documents, on a directory of old_D documents whose new inverted file
+// is (hivf [L], hlen [K])
+static pb_status append_dir(pb_index *ix, const AppendPrep &p, const char *index_dir, long long old_D, int64_t batch_size,
+                            const std::vector<int64_t> &hivf, long long L, const std::vector<int32_t> &hlen) {
+    const size_t pk = (size_t)ix->packed;
+    std::vector<uint8_t> hres((size_t)p.ntok * pk);
+    if (p.ntok)
+        CK(cudaMemcpy(hres.data(), ix->residuals.as<uint8_t>() + (size_t)(p.N1 - p.ntok) * pk, hres.size(), cudaMemcpyDeviceToHost));
+    return pb_dir_append(index_dir, old_D, ix->K, ix->dim, ix->nbits, batch_size, p.hcodes.data(), hres.data(), p.dl.data(),
+                         p.n, hivf.data(), L, hlen.data());
+}
 
-    // 6. commit
+static void append_commit(pb_index *ix, const AppendPrep &p) {
+    if (p.n == 0) return;
     ix->ivf.swap(ix->ivf_spare);
     ix->ivf_off.swap(ix->ivf_off_spare);
-    ix->ivf_len = L1;
-    ix->n_ucodes = U1;
-    ix->N = N1;
-    ix->D = D1;
-    ix->max_doclen = maxlen;
-    ix->vmin = vmin;
-    ix->wmax = wmax;
+    ix->ivf_len = p.L1;
+    ix->n_ucodes = p.U1;
+    ix->N = p.N1;
+    ix->D = p.D1;
+    ix->max_doclen = p.maxlen;
+    ix->vmin = p.vmin;
+    ix->wmax = p.wmax;
+}
+
+static pb_status append_impl(pb_index *ix, pb_codec *codec, const float *embeddings, const int64_t *codes,
+                             const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs, int32_t space,
+                             const char *index_dir, int64_t batch_size, int64_t *out_first) {
+    if (!ix || (!doc_lengths && n_docs) || n_docs < 0) return pb_fail(PB_ERR_INVALID, "null argument");
+    if (space != PB_MEM_HOST && space != PB_MEM_DEVICE) return pb_fail(PB_ERR_INVALID, "bad memory_space %d", space);
+    std::lock_guard<std::mutex> gate(ix->gate);
+    std::unique_lock<std::shared_mutex> wr(ix->rw);
+    if (ix->comm || ix->group) return pb_fail(PB_ERR_UNSUPPORTED, "appends to a doc-sharded handle are not supported");
+    if (!ix->residuals.owned)
+        return pb_fail(PB_ERR_UNSUPPORTED, "the handle uses the caller's residual array (PB_OPEN_ADOPT_RESIDUALS)");
+    if (index_dir && ix->doc_id_base != 0) return pb_fail(PB_ERR_UNSUPPORTED, "an index directory holds doc ids from 0");
+    if (index_dir && batch_size <= 0) return pb_fail(PB_ERR_INVALID, "batch_size must be positive");
+    AppendPrep p;
+    CKS(append_prepare(ix, codec, embeddings, codes, residuals, doc_lengths, n_docs, space, index_dir != nullptr,
+                       out_first, p));
+    if (p.n == 0) return PB_OK;
+    // update_index's file changes, before the commit: a failure leaves the handle as it was
+    if (index_dir) {
+        std::vector<int64_t> hivf;
+        std::vector<int32_t> hlen;
+        CKS(ivf_to_host(ix, ix->ivf_spare, ix->ivf_off_spare, p.L1, hivf, hlen));
+        CKS(append_dir(ix, p, index_dir, p.D0, batch_size, hivf, p.L1, hlen));
+    }
+    append_commit(ix, p);
     return PB_OK;
 }
 
@@ -3260,6 +3359,197 @@ struct Events {
     }
 };
 
+// The deleted set among docs [base, base + D): one bit per doc in bits [ceil(D / 32)], its per-word prefix counts in
+// word_pre [ceil(D / 32) + 1], and the number of docs it holds
+static pb_status del_bitmap(pb_index *ix, const int64_t *doc_ids, long long n_ids, long long base, long long D, DevBuf &bits,
+                            DevBuf &wpre, long long *n_del) {
+    const long long nw = (D + 31) / 32;
+    const int grid = ix->sm_count * 8;
+    DevBuf wcnt, tmp;
+    CKS(bits.ensure(std::max<size_t>((size_t)nw * 4, 16)));
+    CK(cudaMemset(bits.p, 0, (size_t)nw * 4));
+    if (n_ids > 0 && D > 0) {
+        const long long slab = 1ll << 20;
+        DevBuf dids;
+        CKS(dids.ensure((size_t)std::min<long long>(n_ids, slab) * 8));
+        for (long long o = 0; o < n_ids; o += slab) {
+            const long long m = std::min(slab, n_ids - o);
+            CK(cudaMemcpy(dids.p, doc_ids + o, (size_t)m * 8, cudaMemcpyHostToDevice));
+            k_del_mark<<<grid, 256>>>(dids.as<long long>(), m, base, D, bits.as<uint32_t>());
+            CK(cudaGetLastError());
+        }
+    }
+    CKS(wcnt.ensure((size_t)(nw + 1) * 8));
+    CKS(wpre.ensure((size_t)(nw + 1) * 8));
+    k_del_popc<<<grid, 256>>>(bits.as<uint32_t>(), nw, wcnt.as<long long>());
+    CK(cudaGetLastError());
+    CKS(exclusive_sum(wcnt.as<long long>(), wpre.as<long long>(), nw + 1, tmp));
+    CK(cudaMemcpy(n_del, wpre.as<long long>() + nw, 8, cudaMemcpyDeviceToHost));
+    return PB_OK;
+}
+
+// What a delete computes before its first in-place write: the deleted set, the survivors and their new offsets, the
+// filtered inverted file in the spare half, the compaction windows with their staging buffers, and the new totals
+struct DeletePrep {
+    long long D0 = 0, n_del = 0, D1 = 0, N1 = 0, U1 = 0, L1 = 0;
+    int maxlen = 0;
+    DevBuf bits, wpre, kept, new_doff, new_uoff, st_codes, st_res, st_u, mn;
+    std::vector<long long> hoff, hu;
+    std::vector<uint32_t> hbits;
+    std::vector<std::pair<long long, long long>> wins;
+    Events ev;
+};
+
+// Every check and allocation of a delete and everything it computes out of place; nothing visible changes.  n_del = 0:
+// nothing to do.  The caller holds the handle's writer lock.
+static pb_status delete_prepare(pb_index *ix, const int64_t *doc_ids, int64_t n_ids, DeletePrep &p) {
+    CK(cudaSetDevice(ix->device));
+    CK(cudaDeviceSynchronize());  // work earlier readers left queued (pb_search_batch_device) reads the arrays
+    const long long D0 = ix->D, K = ix->K, nw = (D0 + 31) / 32;
+    const int grid = ix->sm_count * 8;
+    p.D0 = D0;
+    if (ix->profiling)
+        for (cudaEvent_t &x : p.ev.e) CK(cudaEventCreate(&x));
+
+    // 1. the deleted set: one bit per doc, its per-word prefix counts, and the number of docs deleted
+    CKS(del_bitmap(ix, doc_ids, n_ids, ix->doc_id_base, D0, p.bits, p.wpre, &p.n_del));
+    if (p.n_del == 0) return PB_OK;
+    const long long D1 = D0 - p.n_del;
+
+    // 2. the survivors kept[j] and their new doc_off / udoc_off, into scratch: the old ones are read until the commit
+    DevBuf tlen, ulen, tmp;
+    CKS(p.kept.ensure((size_t)std::max(D1, 1ll) * 8));
+    CKS(tlen.ensure((size_t)(D1 + 1) * 8));
+    CKS(ulen.ensure((size_t)(D1 + 1) * 8));
+    CKS(p.new_doff.ensure((size_t)(D1 + 1) * 8));
+    CKS(p.new_uoff.ensure((size_t)(D1 + 1) * 8));
+    CK(cudaMemset(tlen.as<long long>() + D1, 0, 8));
+    CK(cudaMemset(ulen.as<long long>() + D1, 0, 8));
+    k_del_kept<<<grid, 256>>>(p.bits.as<uint32_t>(), p.wpre.as<long long>(), D0, ix->doc_off.as<long long>(),
+                              ix->udoc_off.as<long long>(), p.kept.as<long long>(), tlen.as<long long>(), ulen.as<long long>());
+    CK(cudaGetLastError());
+    CKS(exclusive_sum(tlen.as<long long>(), p.new_doff.as<long long>(), D1 + 1, tmp));
+    CKS(exclusive_sum(ulen.as<long long>(), p.new_uoff.as<long long>(), D1 + 1, tmp));
+    std::vector<long long> &hoff = p.hoff, &hu = p.hu;
+    hoff.resize((size_t)D1 + 1);
+    hu.resize((size_t)D1 + 1);
+    CK(cudaMemcpy(hoff.data(), p.new_doff.p, hoff.size() * 8, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(hu.data(), p.new_uoff.p, hu.size() * 8, cudaMemcpyDeviceToHost));
+    p.D1 = D1;
+    p.N1 = hoff[D1];
+    p.U1 = hu[D1];
+    p.maxlen = 0;
+    for (long long j = 0; j < D1; ++j) p.maxlen = std::max<int>(p.maxlen, (int)(hoff[j + 1] - hoff[j]));
+
+    // 3. the inverted file without the deleted ids, renumbered, into the spare half
+    if (ix->profiling) CK(cudaEventRecord(p.ev.e[0]));
+    DevBuf icnt;
+    CKS(icnt.ensure((size_t)(K + 1) * 8));
+    CKS(ix->ivf_off_spare.ensure((size_t)(K + 1) * 8));
+    k_ivf_delete_count<<<grid, 256>>>(ix->ivf.as<uint32_t>(), ix->ivf_off.as<long long>(), K, p.bits.as<uint32_t>(),
+                                      icnt.as<long long>());
+    CK(cudaGetLastError());
+    CKS(exclusive_sum(icnt.as<long long>(), ix->ivf_off_spare.as<long long>(), K + 1, tmp));
+    CK(cudaMemcpy(&p.L1, ix->ivf_off_spare.as<long long>() + K, 8, cudaMemcpyDeviceToHost));
+    CKS(ix->ivf_spare.grow(std::max<size_t>((size_t)p.L1 * 4, 16), 0));
+    k_ivf_delete_write<<<grid, 256>>>(ix->ivf.as<uint32_t>(), ix->ivf_off.as<long long>(), K, p.bits.as<uint32_t>(),
+                                      p.wpre.as<long long>(), ix->ivf_off_spare.as<long long>(), ix->ivf_spare.as<uint32_t>());
+    CK(cudaGetLastError());
+    if (ix->profiling) CK(cudaEventRecord(p.ev.e[1]));
+
+    // 4. compaction windows over the survivors that move: those from the first deleted doc on (survivors before it keep
+    // their rows; a delete of the newest docs moves nothing).  Each window is a run of survivors whose rows fit
+    // delete_window tokens (a longer doc is a window of its own).
+    p.hbits.resize((size_t)nw);
+    CK(cudaMemcpy(p.hbits.data(), p.bits.p, (size_t)nw * 4, cudaMemcpyDeviceToHost));
+    long long first = 0;
+    while (p.hbits[(size_t)(first >> 5)] == 0) first += 32;
+    first += __builtin_ctz(p.hbits[(size_t)(first >> 5)]);
+    long long max_tok = 0, max_u = 0;
+    for (long long j0 = first, j1; j0 < D1; j0 = j1) {
+        for (j1 = j0 + 1; j1 < D1 && hoff[j1 + 1] - hoff[j0] <= ix->delete_window; ++j1) {}
+        p.wins.emplace_back(j0, j1);
+        max_tok = std::max(max_tok, hoff[j1] - hoff[j0]);
+        max_u = std::max(max_u, hu[j1] - hu[j0]);
+    }
+    const size_t pk = (size_t)ix->packed;
+    if (!p.wins.empty()) {
+        CKS(p.st_codes.ensure(std::max<size_t>((size_t)max_tok * 4, 16)));
+        CKS(p.st_res.ensure(std::max<size_t>((size_t)max_tok * pk, 16)));
+        CKS(p.st_u.ensure(std::max<size_t>((size_t)max_u * 4, 16)));
+    }
+    CKS(p.mn.ensure(16));
+    CK(cudaDeviceSynchronize());
+    return PB_OK;
+}
+
+// The in-place part of a prepared delete: only a CUDA runtime error can fail it
+static pb_status delete_commit(pb_index *ix, DeletePrep &p) {
+    if (p.n_del == 0) return PB_OK;
+    const bool prof = ix->profiling && p.ev.e[0];
+    const int grid = ix->sm_count * 8;
+    const std::vector<long long> &hoff = p.hoff, &hu = p.hu;
+    const size_t pk = (size_t)ix->packed;
+    // 5. compaction
+    if (prof) CK(cudaEventRecord(p.ev.e[2]));
+    for (const auto &w : p.wins) {
+        const long long j0 = w.first, j1 = w.second;
+        const unsigned blocks = (unsigned)std::min<long long>((j1 - j0 + 7) / 8, grid);
+        const long long *kp = p.kept.as<long long>();
+        k_compact_gather<uint32_t><<<blocks, 256>>>(ix->codes.as<uint8_t>(), ix->doc_off.as<long long>(), kp,
+                                                    p.new_doff.as<long long>(), j0, j1, 4, p.st_codes.as<uint8_t>());
+        if (pk % 16 == 0)  // dim * nbits / 8 is a multiple of 4 for every supported dim
+            k_compact_gather<uint4><<<blocks, 256>>>(ix->residuals.as<uint8_t>(), ix->doc_off.as<long long>(), kp,
+                                                     p.new_doff.as<long long>(), j0, j1, (int)pk, p.st_res.as<uint8_t>());
+        else
+            k_compact_gather<uint32_t><<<blocks, 256>>>(ix->residuals.as<uint8_t>(), ix->doc_off.as<long long>(), kp,
+                                                        p.new_doff.as<long long>(), j0, j1, (int)pk, p.st_res.as<uint8_t>());
+        // distinct-code blocks start at multiples of 8 codes (32 bytes)
+        k_compact_gather<uint4><<<blocks, 256>>>(ix->ucodes.as<uint8_t>(), ix->udoc_off.as<long long>(), kp,
+                                                 p.new_uoff.as<long long>(), j0, j1, 4, p.st_u.as<uint8_t>());
+        CK(cudaGetLastError());
+        const long long nt = hoff[j1] - hoff[j0], nu = hu[j1] - hu[j0];
+        CK(cudaMemcpy(ix->codes.as<uint8_t>() + (size_t)hoff[j0] * 4, p.st_codes.p, (size_t)nt * 4, cudaMemcpyDeviceToDevice));
+        CK(cudaMemcpy(ix->residuals.as<uint8_t>() + (size_t)hoff[j0] * pk, p.st_res.p, (size_t)nt * pk, cudaMemcpyDeviceToDevice));
+        CK(cudaMemcpy(ix->ucodes.as<uint8_t>() + (size_t)hu[j0] * 4, p.st_u.p, (size_t)nu * 4, cudaMemcpyDeviceToDevice));
+    }
+    CK(cudaMemcpy(ix->doc_off.p, p.new_doff.p, (size_t)(p.D1 + 1) * 8, cudaMemcpyDeviceToDevice));
+    CK(cudaMemcpy(ix->udoc_off.p, p.new_uoff.p, (size_t)(p.D1 + 1) * 8, cudaMemcpyDeviceToDevice));
+    if (prof) CK(cudaEventRecord(p.ev.e[3]));
+
+    // 6. 1 / |c + w| of the survivors in their new order, and vmin / wmax over them as an open computes them: the old
+    // constants would still bound the error, but the work counters would differ from a fresh open
+    float vmin = 0.0f, wmax = 0.0f;
+    if (filter_dim(ix->dim) && p.N1 > 0) {
+        const float init[2] = {3.0e38f, 0.0f};
+        CK(cudaMemcpy(p.mn.p, init, 8, cudaMemcpyHostToDevice));
+        CKS(launch_min_vnorm(ix, 0, p.N1, p.mn.as<float>()));
+        float got[2] = {0.f, 0.f};
+        CK(cudaMemcpy(got, p.mn.p, 8, cudaMemcpyDeviceToHost));
+        vmin = got[0] < 1e30f ? got[0] : 0.0f;
+        wmax = got[1];
+    }
+    if (prof) CK(cudaEventRecord(p.ev.e[4]));
+    CK(cudaDeviceSynchronize());
+
+    // 7. commit
+    ix->ivf.swap(ix->ivf_spare);
+    ix->ivf_off.swap(ix->ivf_off_spare);
+    ix->ivf_len = p.L1;
+    ix->n_ucodes = p.U1;
+    ix->N = p.N1;
+    ix->D = p.D1;
+    ix->max_doclen = p.maxlen;
+    ix->vmin = vmin;
+    ix->wmax = wmax;
+    if (prof) {
+        CK(cudaEventElapsedTime(&ix->delete_ms[0], p.ev.e[2], p.ev.e[3]));
+        CK(cudaEventElapsedTime(&ix->delete_ms[1], p.ev.e[0], p.ev.e[1]));
+        CK(cudaEventElapsedTime(&ix->delete_ms[2], p.ev.e[3], p.ev.e[4]));
+    }
+    return PB_OK;
+}
+
 extern "C" pb_status pb_index_delete(pb_index *ix, const int64_t *doc_ids, int64_t n_ids, const char *index_dir,
                                      int64_t *out_deleted) {
     if (!ix || (!doc_ids && n_ids) || n_ids < 0) return pb_fail(PB_ERR_INVALID, "null argument");
@@ -3270,179 +3560,217 @@ extern "C" pb_status pb_index_delete(pb_index *ix, const int64_t *doc_ids, int64
     if (!ix->residuals.owned)
         return pb_fail(PB_ERR_UNSUPPORTED, "the handle uses the caller's residual array (PB_OPEN_ADOPT_RESIDUALS)");
     if (index_dir && ix->doc_id_base != 0) return pb_fail(PB_ERR_UNSUPPORTED, "an index directory holds doc ids from 0");
-    CK(cudaSetDevice(ix->device));
-    CK(cudaDeviceSynchronize());  // work earlier readers left queued (pb_search_batch_device) reads the arrays
-    const long long D0 = ix->D, K = ix->K, nw = (D0 + 31) / 32;
-    const int grid = ix->sm_count * 8;
-    const bool prof = ix->profiling;
-    Events ev;
-    if (prof)
-        for (cudaEvent_t &x : ev.e) CK(cudaEventCreate(&x));
-
-    // 1. the deleted set: one bit per doc, its per-word prefix counts, and the number of docs deleted
-    DevBuf bits, wcnt, wpre, tmp;
-    CKS(bits.ensure(std::max<size_t>((size_t)nw * 4, 16)));
-    CK(cudaMemset(bits.p, 0, (size_t)nw * 4));
-    if (n_ids > 0 && D0 > 0) {
-        const long long slab = 1ll << 20;
-        DevBuf dids;
-        CKS(dids.ensure((size_t)std::min<long long>(n_ids, slab) * 8));
-        for (long long o = 0; o < n_ids; o += slab) {
-            const long long m = std::min(slab, n_ids - o);
-            CK(cudaMemcpy(dids.p, doc_ids + o, (size_t)m * 8, cudaMemcpyHostToDevice));
-            k_del_mark<<<grid, 256>>>(dids.as<long long>(), m, ix->doc_id_base, D0, bits.as<uint32_t>());
-            CK(cudaGetLastError());
-        }
-    }
-    CKS(wcnt.ensure((size_t)(nw + 1) * 8));
-    CKS(wpre.ensure((size_t)(nw + 1) * 8));
-    k_del_popc<<<grid, 256>>>(bits.as<uint32_t>(), nw, wcnt.as<long long>());
-    CK(cudaGetLastError());
-    CKS(exclusive_sum(wcnt.as<long long>(), wpre.as<long long>(), nw + 1, tmp));
-    long long n_del = 0;
-    CK(cudaMemcpy(&n_del, wpre.as<long long>() + nw, 8, cudaMemcpyDeviceToHost));
-    if (n_del == 0) return PB_OK;
-    const long long D1 = D0 - n_del;
-
-    // 2. the survivors kept[j] and their new doc_off / udoc_off, into scratch: the old ones are read until the commit
-    DevBuf kept, tlen, ulen, new_doff, new_uoff;
-    CKS(kept.ensure((size_t)std::max(D1, 1ll) * 8));
-    CKS(tlen.ensure((size_t)(D1 + 1) * 8));
-    CKS(ulen.ensure((size_t)(D1 + 1) * 8));
-    CKS(new_doff.ensure((size_t)(D1 + 1) * 8));
-    CKS(new_uoff.ensure((size_t)(D1 + 1) * 8));
-    CK(cudaMemset(tlen.as<long long>() + D1, 0, 8));
-    CK(cudaMemset(ulen.as<long long>() + D1, 0, 8));
-    k_del_kept<<<grid, 256>>>(bits.as<uint32_t>(), wpre.as<long long>(), D0, ix->doc_off.as<long long>(),
-                              ix->udoc_off.as<long long>(), kept.as<long long>(), tlen.as<long long>(), ulen.as<long long>());
-    CK(cudaGetLastError());
-    CKS(exclusive_sum(tlen.as<long long>(), new_doff.as<long long>(), D1 + 1, tmp));
-    CKS(exclusive_sum(ulen.as<long long>(), new_uoff.as<long long>(), D1 + 1, tmp));
-    std::vector<long long> hoff((size_t)D1 + 1), hu((size_t)D1 + 1);
-    CK(cudaMemcpy(hoff.data(), new_doff.p, hoff.size() * 8, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(hu.data(), new_uoff.p, hu.size() * 8, cudaMemcpyDeviceToHost));
-    const long long N1 = hoff[D1], U1 = hu[D1];
-    int maxlen = 0;
-    for (long long j = 0; j < D1; ++j) maxlen = std::max<int>(maxlen, (int)(hoff[j + 1] - hoff[j]));
-
-    // 3. the inverted file without the deleted ids, renumbered, into the spare half
-    if (prof) CK(cudaEventRecord(ev.e[0]));
-    DevBuf icnt;
-    CKS(icnt.ensure((size_t)(K + 1) * 8));
-    CKS(ix->ivf_off_spare.ensure((size_t)(K + 1) * 8));
-    k_ivf_delete_count<<<grid, 256>>>(ix->ivf.as<uint32_t>(), ix->ivf_off.as<long long>(), K, bits.as<uint32_t>(),
-                                      icnt.as<long long>());
-    CK(cudaGetLastError());
-    CKS(exclusive_sum(icnt.as<long long>(), ix->ivf_off_spare.as<long long>(), K + 1, tmp));
-    long long L1 = 0;
-    CK(cudaMemcpy(&L1, ix->ivf_off_spare.as<long long>() + K, 8, cudaMemcpyDeviceToHost));
-    CKS(ix->ivf_spare.grow(std::max<size_t>((size_t)L1 * 4, 16), 0));
-    k_ivf_delete_write<<<grid, 256>>>(ix->ivf.as<uint32_t>(), ix->ivf_off.as<long long>(), K, bits.as<uint32_t>(),
-                                      wpre.as<long long>(), ix->ivf_off_spare.as<long long>(), ix->ivf_spare.as<uint32_t>());
-    CK(cudaGetLastError());
-    if (prof) CK(cudaEventRecord(ev.e[1]));
-
-    // 4. compaction windows over the survivors that move: those from the first deleted doc on (survivors before it keep
-    // their rows; a delete of the newest docs moves nothing).  Each window is a run of survivors whose rows fit
-    // delete_window tokens (a longer doc is a window of its own).
-    std::vector<uint32_t> hbits((size_t)nw);
-    CK(cudaMemcpy(hbits.data(), bits.p, (size_t)nw * 4, cudaMemcpyDeviceToHost));
-    long long first = 0;
-    while (hbits[(size_t)(first >> 5)] == 0) first += 32;
-    first += __builtin_ctz(hbits[(size_t)(first >> 5)]);
-    std::vector<std::pair<long long, long long>> wins;
-    long long max_tok = 0, max_u = 0;
-    for (long long j0 = first, j1; j0 < D1; j0 = j1) {
-        for (j1 = j0 + 1; j1 < D1 && hoff[j1 + 1] - hoff[j0] <= ix->delete_window; ++j1) {}
-        wins.emplace_back(j0, j1);
-        max_tok = std::max(max_tok, hoff[j1] - hoff[j0]);
-        max_u = std::max(max_u, hu[j1] - hu[j0]);
-    }
-    const size_t pk = (size_t)ix->packed;
-    DevBuf st_codes, st_res, st_u;
-    if (!wins.empty()) {
-        CKS(st_codes.ensure(std::max<size_t>((size_t)max_tok * 4, 16)));
-        CKS(st_res.ensure(std::max<size_t>((size_t)max_tok * pk, 16)));
-        CKS(st_u.ensure(std::max<size_t>((size_t)max_u * 4, 16)));
-    }
-    DevBuf mn;
-    CKS(mn.ensure(16));
-    CK(cudaDeviceSynchronize());
-
+    DeletePrep p;
+    CKS(delete_prepare(ix, doc_ids, n_ids, p));
+    if (p.n_del == 0) return PB_OK;
     // delete_from_index's file changes, before the first in-place write: a failure leaves the handle as it was
     if (index_dir) {
-        std::vector<int64_t> hivf((size_t)std::max(L1, 1ll));
-        std::vector<int32_t> hlen((size_t)K);
-        DevBuf di, dln;
-        CKS(di.ensure(std::max<size_t>((size_t)L1 * 8, 16)));
-        CKS(dln.ensure((size_t)K * 4));
-        k_ivf_export<<<grid, 256>>>(ix->ivf_spare.as<uint32_t>(), ix->ivf_off_spare.as<long long>(), L1, K, 0,
-                                    di.as<long long>(), dln.as<int>());
-        CK(cudaGetLastError());
-        if (L1) CK(cudaMemcpy(hivf.data(), di.p, (size_t)L1 * 8, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(hlen.data(), dln.p, (size_t)K * 4, cudaMemcpyDeviceToHost));
-        CKS(pb_dir_delete(index_dir, D0, K, ix->dim, ix->nbits, hbits.data(), hivf.data(), L1, hlen.data()));
+        std::vector<int64_t> hivf;
+        std::vector<int32_t> hlen;
+        CKS(ivf_to_host(ix, ix->ivf_spare, ix->ivf_off_spare, p.L1, hivf, hlen));
+        CKS(pb_dir_delete(index_dir, p.D0, ix->K, ix->dim, ix->nbits, p.hbits.data(), hivf.data(), p.L1, hlen.data()));
     }
-
-    // 5. in place from here on: only a CUDA runtime error can fail the call
-    if (prof) CK(cudaEventRecord(ev.e[2]));
-    for (const auto &w : wins) {
-        const long long j0 = w.first, j1 = w.second;
-        const unsigned blocks = (unsigned)std::min<long long>((j1 - j0 + 7) / 8, grid);
-        const long long *kp = kept.as<long long>();
-        k_compact_gather<uint32_t><<<blocks, 256>>>(ix->codes.as<uint8_t>(), ix->doc_off.as<long long>(), kp,
-                                                    new_doff.as<long long>(), j0, j1, 4, st_codes.as<uint8_t>());
-        if (pk % 16 == 0)  // dim * nbits / 8 is a multiple of 4 for every supported dim
-            k_compact_gather<uint4><<<blocks, 256>>>(ix->residuals.as<uint8_t>(), ix->doc_off.as<long long>(), kp,
-                                                     new_doff.as<long long>(), j0, j1, (int)pk, st_res.as<uint8_t>());
-        else
-            k_compact_gather<uint32_t><<<blocks, 256>>>(ix->residuals.as<uint8_t>(), ix->doc_off.as<long long>(), kp,
-                                                        new_doff.as<long long>(), j0, j1, (int)pk, st_res.as<uint8_t>());
-        // distinct-code blocks start at multiples of 8 codes (32 bytes)
-        k_compact_gather<uint4><<<blocks, 256>>>(ix->ucodes.as<uint8_t>(), ix->udoc_off.as<long long>(), kp,
-                                                 new_uoff.as<long long>(), j0, j1, 4, st_u.as<uint8_t>());
-        CK(cudaGetLastError());
-        const long long nt = hoff[j1] - hoff[j0], nu = hu[j1] - hu[j0];
-        CK(cudaMemcpy(ix->codes.as<uint8_t>() + (size_t)hoff[j0] * 4, st_codes.p, (size_t)nt * 4, cudaMemcpyDeviceToDevice));
-        CK(cudaMemcpy(ix->residuals.as<uint8_t>() + (size_t)hoff[j0] * pk, st_res.p, (size_t)nt * pk, cudaMemcpyDeviceToDevice));
-        CK(cudaMemcpy(ix->ucodes.as<uint8_t>() + (size_t)hu[j0] * 4, st_u.p, (size_t)nu * 4, cudaMemcpyDeviceToDevice));
-    }
-    CK(cudaMemcpy(ix->doc_off.p, new_doff.p, (size_t)(D1 + 1) * 8, cudaMemcpyDeviceToDevice));
-    CK(cudaMemcpy(ix->udoc_off.p, new_uoff.p, (size_t)(D1 + 1) * 8, cudaMemcpyDeviceToDevice));
-    if (prof) CK(cudaEventRecord(ev.e[3]));
-
-    // 6. 1 / |c + w| of the survivors in their new order, and vmin / wmax over them as an open computes them: the old
-    // constants would still bound the error, but the work counters would differ from a fresh open
-    float vmin = 0.0f, wmax = 0.0f;
-    if (filter_dim(ix->dim) && N1 > 0) {
-        const float init[2] = {3.0e38f, 0.0f};
-        CK(cudaMemcpy(mn.p, init, 8, cudaMemcpyHostToDevice));
-        CKS(launch_min_vnorm(ix, 0, N1, mn.as<float>()));
-        float got[2] = {0.f, 0.f};
-        CK(cudaMemcpy(got, mn.p, 8, cudaMemcpyDeviceToHost));
-        vmin = got[0] < 1e30f ? got[0] : 0.0f;
-        wmax = got[1];
-    }
-    if (prof) CK(cudaEventRecord(ev.e[4]));
-    CK(cudaDeviceSynchronize());
-
-    // 7. commit
-    ix->ivf.swap(ix->ivf_spare);
-    ix->ivf_off.swap(ix->ivf_off_spare);
-    ix->ivf_len = L1;
-    ix->n_ucodes = U1;
-    ix->N = N1;
-    ix->D = D1;
-    ix->max_doclen = maxlen;
-    ix->vmin = vmin;
-    ix->wmax = wmax;
-    if (prof) {
-        CK(cudaEventElapsedTime(&ix->delete_ms[0], ev.e[2], ev.e[3]));
-        CK(cudaEventElapsedTime(&ix->delete_ms[1], ev.e[0], ev.e[1]));
-        CK(cudaEventElapsedTime(&ix->delete_ms[2], ev.e[3], ev.e[4]));
-    }
-    if (out_deleted) *out_deleted = n_del;
+    CKS(delete_commit(ix, p));
+    if (out_deleted) *out_deleted = p.n_del;
     return PB_OK;
+}
+
+// ------------------------------------------------------------------------------------------
+// appends and deletes on a doc-sharded deployment (DESIGN §4h).  Every rank prepares locally, then one all-gather of a
+// fixed record lets all ranks reach the same verdict from the same data: commit everywhere or nowhere.  Rank world - 1
+// writes the directory from ivf.npy on disk; a second exchange carries its status.  After the vote only a CUDA runtime
+// error can fail a rank.
+// ------------------------------------------------------------------------------------------
+enum { SH_STATUS, SH_RANK, SH_WORLD, SH_BASE, SH_D, SH_N, SH_K, SH_DIM, SH_NBITS, SH_NDEL, SH_PRINT, SH_WORDS };
+enum { SH_OP_DELETE = 1, SH_OP_APPEND = 2, SH_OP_APPEND_ENCODED = 3 };
+
+struct Fnv64 {  // FNV-1a over the call's arguments
+    u64 h = 14695981039346656037ull;
+    void add(const void *p, size_t n) {
+        for (size_t i = 0; i < n; ++i) h = (h ^ static_cast<const uint8_t *>(p)[i]) * 1099511628211ull;
+    }
+    template <class T> void put(T v) { add(&v, sizeof v); }
+};
+
+// every rank's `words` 64-bit words, in rank order; a handle outside any group is a group of one
+static pb_status gather_words(pb_index *ix, const long long *mine, int words, std::vector<long long> &all,
+                              bool unbounded = false) {
+    all.assign(mine, mine + words);
+    if (!ix->comm && !ix->group) return PB_OK;
+    all.resize((size_t)words * ix->world);
+    struct Stream {
+        cudaStream_t s = nullptr;
+        ~Stream() {
+            if (s) cudaStreamDestroy(s);
+        }
+    } st;
+    DevBuf send, recv;
+    CK(cudaSetDevice(ix->device));
+    CK(cudaStreamCreateWithFlags(&st.s, cudaStreamNonBlocking));
+    CKS(send.ensure((size_t)words * 8));
+    CKS(recv.ensure((size_t)words * 8 * ix->world));
+    CK(cudaMemcpy(send.p, mine, (size_t)words * 8, cudaMemcpyHostToDevice));
+    CKS(shard_allgather(ix, st.s, send.p, recv.p, (size_t)words, unbounded));
+    CK(cudaStreamSynchronize(st.s));
+    CK(cudaMemcpy(all.data(), recv.p, all.size() * 8, cudaMemcpyDeviceToHost));
+    return PB_OK;
+}
+
+// the status of the lowest failing rank, or PB_OK; the failing rank keeps its own message, the others name it
+static pb_status first_failure(pb_index *ix, const std::vector<long long> &all, int words, const char *what) {
+    for (int r = 0; r < ix->world; ++r) {
+        const pb_status s = (pb_status)all[(size_t)r * words];
+        if (s == PB_OK) continue;
+        if (r == ix->rank) {
+            const std::string own = g_err;
+            return pb_fail(s, "rank %d: %s", r, own.c_str());
+        }
+        return pb_fail(s, "rank %d of the group failed (status %d)%s", r, (int)s, what);
+    }
+    return PB_OK;
+}
+
+static pb_status sharded_update(pb_index *ix, int op, pb_codec *codec, const float *embeddings, const int64_t *codes,
+                                const uint8_t *residuals, const int64_t *doc_lengths, const int64_t *doc_ids, int64_t n,
+                                int32_t space, const char *index_dir, int64_t batch_size, int64_t *out) {
+    if (out) *out = 0;
+    std::lock_guard<std::mutex> gate(ix->gate);
+    std::unique_lock<std::shared_mutex> wr(ix->rw);
+    const bool last = ix->rank == ix->world - 1;
+    DeletePrep dp;
+    AppendPrep ap;
+    long long rec[SH_WORDS] = {};
+    // 1. local checks, the fingerprint of the arguments, and the prepare: no early return, or the peers would wait
+    auto local = [&]() -> pb_status {
+        if (n < 0 || (n && !(op == SH_OP_DELETE ? doc_ids : doc_lengths))) return pb_fail(PB_ERR_INVALID, "null argument");
+        if (op != SH_OP_DELETE && space != PB_MEM_HOST && space != PB_MEM_DEVICE)
+            return pb_fail(PB_ERR_INVALID, "bad memory_space %d", space);
+        if (!ix->residuals.owned)
+            return pb_fail(PB_ERR_UNSUPPORTED, "the handle uses the caller's residual array (PB_OPEN_ADOPT_RESIDUALS)");
+        if (index_dir && op == SH_OP_APPEND && batch_size <= 0) return pb_fail(PB_ERR_INVALID, "batch_size must be positive");
+        if (op == SH_OP_APPEND && last && !codec) return pb_fail(PB_ERR_INVALID, "null argument");
+        std::vector<int64_t> args;
+        if (op == SH_OP_DELETE) args.assign(doc_ids, doc_ids + n);
+        else CKS(fetch_host(args, doc_lengths, (size_t)n, space));
+        Fnv64 f;
+        f.put(op);
+        f.put((long long)n);
+        f.add(args.data(), args.size() * 8);
+        f.put(index_dir != nullptr);
+        if (index_dir) f.add(index_dir, strlen(index_dir) + 1);
+        f.put((long long)(op == SH_OP_APPEND ? batch_size : 0));
+        rec[SH_PRINT] = (long long)f.h;
+        if (op == SH_OP_DELETE) {
+            CKS(delete_prepare(ix, doc_ids, n, dp));
+            rec[SH_NDEL] = dp.n_del;
+        } else if (last) {
+            CKS(append_prepare(ix, codec, embeddings, codes, residuals, doc_lengths, n, space, index_dir != nullptr,
+                               nullptr, ap));
+        }
+        return PB_OK;
+    };
+    rec[SH_STATUS] = local();
+    rec[SH_RANK] = ix->rank;
+    rec[SH_WORLD] = ix->world;
+    rec[SH_BASE] = ix->doc_id_base;
+    rec[SH_D] = ix->D;
+    rec[SH_N] = ix->N;
+    rec[SH_K] = ix->K;
+    rec[SH_DIM] = ix->dim;
+    rec[SH_NBITS] = ix->nbits;
+
+    // 2. exchange A and the verdict every rank reaches from the same records
+    std::vector<long long> all;
+    CKS(gather_words(ix, rec, SH_WORDS, all));
+    const int W = ix->world;
+    CKS(first_failure(ix, all, SH_WORDS, "; nothing changed"));
+    auto at = [&](int r, int w) { return all[(size_t)r * SH_WORDS + w]; };
+    long long D_total = 0, n_del = 0, del_before = 0;
+    for (int r = 0; r < W; ++r) {
+        if (at(r, SH_RANK) != r || at(r, SH_WORLD) != W || at(r, SH_K) != at(0, SH_K) || at(r, SH_DIM) != at(0, SH_DIM) ||
+            at(r, SH_NBITS) != at(0, SH_NBITS))
+            return pb_fail(PB_ERR_INVALID, "rank %d's layout (rank %lld of %lld, K=%lld dim=%lld nbits=%lld) differs from rank 0's",
+                           r, at(r, SH_RANK), at(r, SH_WORLD), at(r, SH_K), at(r, SH_DIM), at(r, SH_NBITS));
+        if (at(r, SH_BASE) != D_total)
+            return pb_fail(PB_ERR_INVALID, "the ranks' documents do not tile [0, D): rank %d starts at %lld, not %lld", r,
+                           at(r, SH_BASE), D_total);
+        if (at(r, SH_PRINT) != at(0, SH_PRINT))
+            return pb_fail(PB_ERR_INVALID, "rank %d was called with other arguments than rank 0", r);
+        D_total += at(r, SH_D);
+        if (r < ix->rank) del_before += at(r, SH_NDEL);
+        n_del += at(r, SH_NDEL);
+    }
+    if (op == SH_OP_DELETE && n_del == 0) return PB_OK;  // nothing changes, on any rank or on disk
+    if (op != SH_OP_DELETE && out) *out = D_total;
+    if (op != SH_OP_DELETE && n == 0) return PB_OK;
+
+    // 3. the directory, written by the last rank from ivf.npy as it is on disk; exchange B carries its status
+    if (index_dir) {
+        long long wrec = PB_OK;
+        if (last) {
+            auto total = [](const std::vector<int32_t> &len) {
+                long long t = 0;
+                for (int32_t x : len) t += x;
+                return t;
+            };
+            auto write = [&]() -> pb_status {
+                CKS(pb_dir_check_documents(index_dir, ix->nbits, D_total));
+                std::vector<int64_t> hivf;
+                std::vector<int32_t> hlen;
+                if (op == SH_OP_DELETE) {
+                    DevBuf gbits, gwpre;
+                    long long g = 0;
+                    CKS(del_bitmap(ix, doc_ids, n, 0, D_total, gbits, gwpre, &g));
+                    CKS(pb_dir_patch_ivf(ix, index_dir, D_total, gbits.as<uint32_t>(), gwpre.as<long long>(), nullptr, 0, hivf, hlen));
+                    std::vector<uint32_t> hbits((size_t)(D_total + 31) / 32);
+                    CK(cudaMemcpy(hbits.data(), gbits.p, hbits.size() * 4, cudaMemcpyDeviceToHost));
+                    return pb_dir_delete(index_dir, D_total, ix->K, ix->dim, ix->nbits, hbits.data(), hivf.data(),
+                                         total(hlen), hlen.data());
+                }
+                CKS(pb_dir_patch_ivf(ix, index_dir, D_total, nullptr, nullptr, ap.keys.as<uint64_t>(), ap.m, hivf, hlen));
+                return append_dir(ix, ap, index_dir, D_total, batch_size, hivf, total(hlen), hlen);
+            };
+            wrec = write();
+        }
+        // the peers wait for the writer however long the write takes: a timeout here would leave the directory
+        // changed and every handle unchanged
+        std::vector<long long> wall;
+        CKS(gather_words(ix, &wrec, 1, wall, true));
+        CKS(first_failure(ix, wall, 1, " writing the index directory; no rank changed"));
+    }
+
+    // 4. commit everywhere: from here only a CUDA runtime error can fail a rank, and that leaves the group inconsistent
+    if (op == SH_OP_DELETE) {
+        CKS(delete_commit(ix, dp));
+        ix->doc_id_base -= del_before;
+        if (out) *out = n_del;
+    } else if (last) {
+        append_commit(ix, ap);
+    }
+    return PB_OK;
+}
+
+extern "C" pb_status pb_index_delete_sharded(pb_index *ix, const int64_t *doc_ids, int64_t n_ids, const char *index_dir,
+                                             int64_t *out_deleted) {
+    if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    return sharded_update(ix, SH_OP_DELETE, nullptr, nullptr, nullptr, nullptr, nullptr, doc_ids, n_ids, PB_MEM_HOST,
+                          index_dir, 0, out_deleted);
+}
+
+extern "C" pb_status pb_index_append_sharded(pb_index *ix, pb_codec *codec, const float *embeddings,
+                                             const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
+                                             const char *index_dir, int64_t batch_size, int64_t *out_first_doc_id) {
+    if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    return sharded_update(ix, SH_OP_APPEND, codec, embeddings, nullptr, nullptr, doc_lengths, nullptr, n_docs, memory_space,
+                          index_dir, batch_size, out_first_doc_id);
+}
+
+extern "C" pb_status pb_index_append_encoded_sharded(pb_index *ix, const int64_t *codes, const uint8_t *residuals,
+                                                     const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
+                                                     int64_t *out_first_doc_id) {
+    if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    return sharded_update(ix, SH_OP_APPEND_ENCODED, nullptr, nullptr, codes, residuals, doc_lengths, nullptr, n_docs,
+                          memory_space, nullptr, 0, out_first_doc_id);
 }
 
 extern "C" pb_status pb_last_delete_ms(pb_index *ix, float *out_ms) {

@@ -17,6 +17,16 @@ pb_status pb_index_finalize(pb_index *ix);
 // order with ids minus b, instead of the one pb_index_finalize would build from the codes.
 pb_status pb_index_upload_ivf_range(pb_index *ix, const int64_t *ivf, const int32_t *lengths, long long total,
                                     long long limit, long long b, long long e);
+// The inverted file of a directory after a change, from its ivf.npy (host, as above, ids in [0, D)) to the host, i64
+// global ids: with a deleted set (device bits / word_pre over the D docs) deleted ids leave the lists and survivors are
+// renumbered (delete.rs:196-237); with the sorted (centroid << 32 | doc) device keys of m appended docs each list is
+// followed by its new pairs as ids D + doc (update.rs:1000-1067).
+pb_status pb_index_patch_ivf(pb_index *ix, const int64_t *file_ivf, const int32_t *file_lengths, long long total, long long D,
+                             const uint32_t *bits, const long long *word_pre, const uint64_t *keys, long long m,
+                             std::vector<int64_t> &ivf, std::vector<int32_t> &lengths);
+// pb_index_patch_ivf on the directory's ivf.npy / ivf_lengths.npy as they are on disk
+pb_status pb_dir_patch_ivf(pb_index *ix, const char *index_dir, long long D, const uint32_t *bits, const long long *word_pre,
+                           const uint64_t *keys, long long m, std::vector<int64_t> &ivf, std::vector<int32_t> &lengths);
 
 // The index directory, as the loader reads it: a whole file; a number of a flat JSON object; a doclens.{i}.json list;
 // the chunk file pair {i}.codes.npy <i8 [n_tokens] / {i}.residuals.npy u1 [n_tokens][packed].
@@ -35,6 +45,9 @@ pb_status pb_read_npy_f32(const std::string &path, long long &rows, long long &c
 pb_status pb_dir_append(const char *index_dir, long long old_D, long long K, int dim, int nbits, long long batch_size,
                         const int64_t *codes, const uint8_t *residuals, const int64_t *doc_lengths, long long n_docs,
                         const int64_t *ivf, long long ivf_total, const int32_t *ivf_lengths);
+
+// PB_ERR_INVALID (PB_ERR_IO when unreadable) unless the directory's metadata.json holds D documents and nbits
+pb_status pb_dir_check_documents(const char *index_dir, int nbits, long long D);
 
 // delete_from_index's file changes (delete.rs:66-273) for the documents whose bit is set in `deleted` (one bit per doc
 // of the old_D the directory holds): filtered chunk files and chunk metadata for every chunk with a deleted doc, the

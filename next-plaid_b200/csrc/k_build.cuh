@@ -720,11 +720,14 @@ __global__ void k_ivf_delete_write(const uint32_t *__restrict__ ivf, const long 
 // range, in file order, ids minus b.  The file (i64, global ids) arrives in slabs: slab holds its entries [s0, s0 + m),
 // off [K + 1] are the file's list offsets, and the centroids c0 <= c < c1 are those whose list overlaps the slab (a list
 // may straddle slabs).  One warp per centroid; slabs go in order on one stream, so cnt[c] / cur[c] need no atomics.
-// Every entry outside [0, limit) sets *bad.
+// Every entry outside [0, limit) sets *bad.  With a deleted set (bits, word_pre over the directory's docs, b = 0) its
+// ids leave the lists too and a survivor is written as id - rank(id): delete.rs:196-237 on the file.  bits = nullptr
+// is the plain range.
 // ------------------------------------------------------------------------------------------
 __global__ void k_ivf_range_count(const long long *__restrict__ slab, long long s0, long long m,
                                   const long long *__restrict__ off, long long c0, long long c1, long long limit,
-                                  long long b, long long e, long long *__restrict__ cnt, int *__restrict__ bad) {
+                                  long long b, long long e, const uint32_t *__restrict__ bits,
+                                  long long *__restrict__ cnt, int *__restrict__ bad) {
     const int lane = threadIdx.x & 31;
     const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
     bool oob = false;
@@ -734,7 +737,7 @@ __global__ void k_ivf_range_count(const long long *__restrict__ slab, long long 
         for (long long i = i0 + lane; i - lane < i1; i += 32) {
             const long long id = i < i1 ? slab[i] : -1;
             oob |= i < i1 && (id < 0 || id >= limit);
-            kept += __popc(__ballot_sync(PB_FULL, id >= b && id < e));
+            kept += __popc(__ballot_sync(PB_FULL, id >= b && id < e && !(bits && del_bit(bits, (uint32_t)id))));
         }
         if (lane == 0) cnt[c] += kept;
     }
@@ -744,7 +747,8 @@ __global__ void k_ivf_range_count(const long long *__restrict__ slab, long long 
 // the kept entries of the slab's part of list c at cur[c].., compacted with a ballot, as id - b; cur[c] advances
 __global__ void k_ivf_range_write(const long long *__restrict__ slab, long long s0, long long m,
                                   const long long *__restrict__ off, long long c0, long long c1, long long b,
-                                  long long e, long long *__restrict__ cur, uint32_t *__restrict__ out) {
+                                  long long e, const uint32_t *__restrict__ bits, const long long *__restrict__ word_pre,
+                                  long long *__restrict__ cur, uint32_t *__restrict__ out) {
     const int lane = threadIdx.x & 31;
     const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
     for (long long c = c0 + (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c < c1; c += nw) {
@@ -752,9 +756,11 @@ __global__ void k_ivf_range_write(const long long *__restrict__ slab, long long 
         long long dst = cur[c];
         for (long long i = i0 + lane; i - lane < i1; i += 32) {
             const long long id = i < i1 ? slab[i] : -1;
-            const bool keep = id >= b && id < e;
+            const bool keep = id >= b && id < e && !(bits && del_bit(bits, (uint32_t)id));
             const unsigned bal = __ballot_sync(PB_FULL, keep);
-            if (keep) out[dst + __popc(bal & ((1u << lane) - 1u))] = (uint32_t)(id - b);
+            if (keep)
+                out[dst + __popc(bal & ((1u << lane) - 1u))] =
+                    (uint32_t)(id - b - (bits ? del_rank(bits, word_pre, (uint32_t)id) : 0));
             dst += __popc(bal);
         }
         if (lane == 0) cur[c] = dst;

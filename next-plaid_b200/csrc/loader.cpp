@@ -214,6 +214,35 @@ pb_status pb_read_npy_f32(const std::string &path, long long &rows, long long &c
 
 namespace {
 
+// A directory's inverted file: ivf.npy <i8 and ivf_lengths.npy, <i4 or (fast-plaid) <i8 narrowed into `store`
+struct DirIvf {
+    Npy ivf, ivfl;
+    std::vector<int32_t> store;
+    const int32_t *lengths = nullptr;
+    pb_status open(const std::string &dir) {
+        if (pb_status s = ivf.open(dir + "ivf.npy")) return s;
+        if (pb_status s = ivfl.open(dir + "ivf_lengths.npy")) return s;
+        if (!ivf.is("i8")) return pb_fail(PB_ERR_IO, "ivf.npy must be <i8");
+        lengths = (const int32_t *)ivfl.data;
+        if (ivfl.is("i8")) {
+            const int64_t *src = (const int64_t *)ivfl.data;
+            store.resize((size_t)ivfl.count());
+            for (long long i = 0; i < ivfl.count(); ++i) {
+                if (src[i] < 0 || src[i] > 0x7fffffffll) return pb_fail(PB_ERR_IO, "ivf_lengths.npy[%lld] out of range", i);
+                store[(size_t)i] = (int32_t)src[i];
+            }
+            lengths = store.data();
+        } else if (!ivfl.is("i4")) return pb_fail(PB_ERR_IO, "ivf_lengths.npy must be <i4 (next-plaid) or <i8 (fast-plaid)");
+        return PB_OK;
+    }
+    pb_status check_sum(long long K) const {
+        long long sum = 0;
+        for (long long i = 0; i < K; ++i) sum += lengths[i];
+        if (sum != ivf.count()) return pb_fail(PB_ERR_IO, "ivf.npy has %lld entries, ivf_lengths sum to %lld", ivf.count(), sum);
+        return PB_OK;
+    }
+};
+
 // The document layout of an index directory: metadata.json's num_chunks / nbits / num_embeddings (-1 when absent), and
 // the doc lengths of every chunk (index.rs:1096-1104) with each chunk's token count.
 struct DirLayout {
@@ -252,31 +281,21 @@ pb_status load_range(const char *index_dir, int32_t device, long long doc_begin,
     if (pb_status s = lay.read_metadata(dir)) return s;
     const double num_chunks = lay.num_chunks, nbits = lay.nbits;
 
-    Npy cent, wts, ivf, ivfl;
+    Npy cent, wts;
+    DirIvf div;
     if (pb_status s = cent.open(dir + "centroids.npy")) return s;
     if (pb_status s = wts.open(dir + "bucket_weights.npy")) return s;
-    if (pb_status s = ivf.open(dir + "ivf.npy")) return s;
-    if (pb_status s = ivfl.open(dir + "ivf_lengths.npy")) return s;
+    if (pb_status s = div.open(dir)) return s;
+    const Npy &ivf = div.ivf, &ivfl = div.ivfl;
+    const int32_t *ivfl_i32 = div.lengths;
     // fast-plaid directories (mmap.rs:1757-1811 converts them in place on the reference's first load): float tensors
     // as <f2, ivf_lengths as <i8, residuals described as <u1.  They are read as they are -- widened / narrowed in
     // memory, which gives the same values as the reference's conversion -- and never modified.
     std::vector<float> cent_store, wts_store;
-    std::vector<int32_t> ivfl_store;
     const float *cent_f32 = nullptr, *wts_f32 = nullptr;
     if (cent.shape.size() != 2) return pb_fail(PB_ERR_IO, "centroids.npy must be [K, dim]");
     if (pb_status s = as_f32(cent, "centroids.npy", cent_store, &cent_f32)) return s;
     if (pb_status s = as_f32(wts, "bucket_weights.npy", wts_store, &wts_f32)) return s;
-    if (!ivf.is("i8")) return pb_fail(PB_ERR_IO, "ivf.npy must be <i8");
-    const int32_t *ivfl_i32 = (const int32_t *)ivfl.data;
-    if (ivfl.is("i8")) {
-        const int64_t *src = (const int64_t *)ivfl.data;
-        ivfl_store.resize((size_t)ivfl.count());
-        for (long long i = 0; i < ivfl.count(); ++i) {
-            if (src[i] < 0 || src[i] > 0x7fffffffll) return pb_fail(PB_ERR_IO, "ivf_lengths.npy[%lld] out of range", i);
-            ivfl_store[(size_t)i] = (int32_t)src[i];
-        }
-        ivfl_i32 = ivfl_store.data();
-    } else if (!ivfl.is("i4")) return pb_fail(PB_ERR_IO, "ivf_lengths.npy must be <i4 (next-plaid) or <i8 (fast-plaid)");
     const long long K = cent.shape[0];
     const int dim = (int)cent.shape[1];
     const int nb = (int)nbits;
@@ -311,9 +330,7 @@ pb_status load_range(const char *index_dir, int32_t device, long long doc_begin,
     d.device = device;
     d.memory_space = PB_MEM_HOST;
     d.doc_id_base = doc_begin;
-    long long ivf_sum = 0;
-    for (long long i = 0; i < K; ++i) ivf_sum += ivfl_i32[i];
-    if (ivf_sum != ivf.count()) return pb_fail(PB_ERR_IO, "ivf.npy has %lld entries, ivf_lengths sum to %lld", ivf.count(), ivf_sum);
+    if (pb_status s = div.check_sum(K)) return s;
     const long long packed = (long long)dim * nb / 8;
     // every chunk file is checked (header, dtype, shape, payload size) before the device is touched: a bad
     // directory fails here, not after tens of GB have been uploaded
@@ -388,4 +405,15 @@ extern "C" pb_status pb_index_dir_shard_bounds(const char *index_dir, int32_t wo
     }
     out_bounds[world] = D;
     return PB_OK;
+}
+
+pb_status pb_dir_patch_ivf(pb_index *ix, const char *index_dir, long long D, const uint32_t *bits, const long long *word_pre,
+                           const uint64_t *keys, long long m, std::vector<int64_t> &ivf, std::vector<int32_t> &lengths) {
+    DirIvf div;
+    const long long K = pb_index_num_partitions(ix);
+    if (pb_status s = div.open(std::string(index_dir) + "/")) return s;
+    if (div.ivfl.count() != K) return pb_fail(PB_ERR_IO, "ivf_lengths.npy has %lld entries, the index %lld centroids", div.ivfl.count(), K);
+    if (pb_status s = div.check_sum(K)) return s;
+    return pb_index_patch_ivf(ix, (const int64_t *)div.ivf.data, div.lengths, div.ivf.count(), D, bits, word_pre, keys, m,
+                              ivf, lengths);
 }

@@ -86,6 +86,7 @@ EXPORTS = [
     "pb_create_params_default", "pb_build_comm_init", "pb_build_comm_group", "pb_build_comm_destroy", "pb_kmeans_fit_dp", "pb_codec_last_assign_stats", "pb_codec_find_outliers",
     "pb_index_append", "pb_index_append_encoded", "pb_index_reserve",
     "pb_index_delete", "pb_last_delete_ms", "pb_index_load_range", "pb_index_dir_shard_bounds",
+    "pb_index_delete_sharded", "pb_index_append_sharded", "pb_index_append_encoded_sharded",
 ]
 
 _lib = None
@@ -179,6 +180,9 @@ def load_library():
         L.pb_index_reserve.argtypes = [C.c_void_p, C.c_int64, C.c_int64]
         L.pb_index_delete.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_char_p, C.c_void_p]
         L.pb_last_delete_ms.argtypes = [C.c_void_p, C.c_void_p]
+        L.pb_index_delete_sharded.argtypes = L.pb_index_delete.argtypes
+        L.pb_index_append_sharded.argtypes = L.pb_index_append.argtypes
+        L.pb_index_append_encoded_sharded.argtypes = L.pb_index_append_encoded.argtypes
         _lib = L
     return _lib
 
@@ -193,10 +197,10 @@ def _ptr(a: Optional[np.ndarray]):
 
 
 class ShardGroup:
-    """pb_shard_group: several shard handles of ONE process searched together (one host thread per shard).
+    """pb_shard_group: several shard handles of ONE process searched and changed together (one host thread per shard).
 
-    `search_batch` runs the collective from len(shards) threads and returns rank 0's result (every rank's
-    result is identical; `all_results` keeps them for the tests)."""
+    `search_batch`, `delete`, `append` and `append_encoded` run the collective from len(shards) threads and return
+    rank 0's result (every rank's result is identical; `all_results` keeps them for the tests)."""
 
     def __init__(self, shards: Sequence["MmapIndex"]):
         self.shards = list(shards)
@@ -207,13 +211,14 @@ class ShardGroup:
             _check(load_library().pb_index_group_join(s._h, self._g, r))
         self.all_results = None
 
-    def search_batch(self, queries, params=None, subset=None):
+    def _collective(self, call):
+        """call(r, shard) from one thread per rank; the per-rank results, or the first rank's exception"""
         import threading
         out, err = [None] * len(self.shards), [None] * len(self.shards)
 
         def run(r):
             try:
-                out[r] = self.shards[r].search_batch(queries, params, subset=subset)
+                out[r] = call(r, self.shards[r])
             except Exception as e:      # noqa: BLE001 - re-raised below
                 err[r] = e
         ths = [threading.Thread(target=run, args=(r,)) for r in range(len(self.shards))]
@@ -223,7 +228,64 @@ class ShardGroup:
             if e is not None:
                 raise e
         self.all_results = out
-        return out[0]
+        return out
+
+    def search_batch(self, queries, params=None, subset=None):
+        return self._collective(lambda r, s: s.search_batch(queries, params, subset=subset))[0]
+
+    def delete(self, doc_ids: Sequence[int], index_dir: Optional[str] = None) -> int:
+        """pb_index_delete_sharded: MmapIndex.delete on the whole deployment (global ids); each rank renumbers its
+        survivors and shifts its doc_id_base, and with `index_dir` the last rank applies delete_from_index's file
+        changes.  Returns the number of documents removed over all ranks."""
+        ids = np.ascontiguousarray(doc_ids, np.int64).reshape(-1)
+        d = None if index_dir is None else os.fsencode(index_dir)
+
+        def call(r, s):
+            n = C.c_int64()
+            _check(load_library().pb_index_delete_sharded(s._h, _ptr(ids), len(ids), d, C.byref(n)))
+            return int(n.value)
+        return self._collective(call)[0]
+
+    def append(self, embeddings: Sequence[np.ndarray], codec: "ResidualCodec", index_dir: Optional[str] = None,
+               batch_size: int = 50_000) -> List[int]:
+        """pb_index_append_sharded: MmapIndex.append on the whole deployment.  The documents go to the last rank as
+        ids D_total ..; with `index_dir` the last rank applies update_index's file changes.  Returns the new ids."""
+        dl = np.array([e.shape[0] for e in embeddings], np.int64)
+        dim = self.shards[-1].embedding_dim()
+        flat = (np.ascontiguousarray(np.concatenate(embeddings, 0), np.float32) if len(embeddings)
+                else np.zeros((0, dim), np.float32))
+        d = None if index_dir is None else os.fsencode(index_dir)
+        W = len(self.shards)
+
+        def call(r, s):
+            first = C.c_int64()
+            last = r == W - 1
+            _check(load_library().pb_index_append_sharded(s._h, codec._h if last else None, _ptr(flat) if last else None,
+                                                          _ptr(dl), len(dl), 0, d, batch_size, C.byref(first)))
+            return first.value
+        first = self._collective(call)[0]
+        return list(range(first, first + len(dl)))
+
+    def append_encoded(self, codes: np.ndarray, residuals: np.ndarray, doc_lengths: Sequence[int]) -> List[int]:
+        """pb_index_append_encoded_sharded: MmapIndex.append_encoded on the whole deployment (to the last rank)."""
+        cd = np.ascontiguousarray(codes, np.int64)
+        rs = np.ascontiguousarray(residuals, np.uint8)
+        dl = np.ascontiguousarray(doc_lengths, np.int64)
+        last = self.shards[-1]
+        if rs.size != len(cd) * last.embedding_dim() * last.nbits() // 8 or int(dl.sum()) != len(cd):
+            raise PlaidError(PB_ERR_INVALID, f"codes {cd.shape}, residuals {rs.shape} and doc_lengths (sum "
+                                             f"{int(dl.sum())}) do not describe the same tokens")
+        W = len(self.shards)
+
+        def call(r, s):
+            first = C.c_int64()
+            mine = r == W - 1
+            _check(load_library().pb_index_append_encoded_sharded(s._h, _ptr(cd) if mine else None,
+                                                                  _ptr(rs) if mine else None, _ptr(dl), len(dl), 0,
+                                                                  C.byref(first)))
+            return first.value
+        first = self._collective(call)[0]
+        return list(range(first, first + len(dl)))
 
     def close(self):
         for s in self.shards:

@@ -71,6 +71,14 @@ extern "C" {
     fn pb_index_load_range(index_dir: *const c_char, device: i32, doc_begin: i64, doc_end: i64,
                            out: *mut *mut c_void) -> c_int;
     fn pb_index_dir_shard_bounds(index_dir: *const c_char, world: i32, out_bounds: *mut i64) -> c_int;
+    fn pb_index_delete_sharded(ix: *mut c_void, doc_ids: *const i64, n_ids: i64, index_dir: *const c_char,
+                               out_deleted: *mut i64) -> c_int;
+    fn pb_index_append_sharded(ix: *mut c_void, codec: *mut c_void, embeddings: *const f32, doc_lengths: *const i64,
+                               n_docs: i64, memory_space: i32, index_dir: *const c_char, batch_size: i64,
+                               out_first_doc_id: *mut i64) -> c_int;
+    fn pb_index_append_encoded_sharded(ix: *mut c_void, codes: *const i64, residuals: *const u8,
+                                       doc_lengths: *const i64, n_docs: i64, memory_space: i32,
+                                       out_first_doc_id: *mut i64) -> c_int;
 }
 
 fn last_error() -> String {
@@ -190,6 +198,31 @@ impl B200Index {
         codec: &crate::codec::ResidualCodec,
         batch_size: usize,
     ) -> Result<Vec<i64>> {
+        self.append_with(embeddings, index_path, codec, batch_size, false)
+    }
+
+    /// `update_append` on a doc-sharded deployment (`pb_index_append_sharded`): every rank calls it with the same
+    /// documents, at the same point of its sequence of collective calls.  The documents go to the last rank as ids
+    /// D_total ..; the last rank writes `index_path`, which every rank names.  Capacity comes from `pb_index_reserve`
+    /// on the last rank before it joins the group.
+    pub fn update_append_sharded(
+        &self,
+        embeddings: &[Array2<f32>],
+        index_path: &str,
+        codec: &crate::codec::ResidualCodec,
+        batch_size: usize,
+    ) -> Result<Vec<i64>> {
+        self.append_with(embeddings, index_path, codec, batch_size, true)
+    }
+
+    fn append_with(
+        &self,
+        embeddings: &[Array2<f32>],
+        index_path: &str,
+        codec: &crate::codec::ResidualCodec,
+        batch_size: usize,
+        sharded: bool,
+    ) -> Result<Vec<i64>> {
         let dim = unsafe { pb_index_embedding_dim(self.handle) } as usize;
         let mut flat: Vec<f32> = Vec::new();
         let mut lens: Vec<i64> = Vec::with_capacity(embeddings.len());
@@ -217,9 +250,10 @@ impl B200Index {
             return Err(Error::Codec(last_error()));
         }
         let mut first = 0i64;
+        let append = if sharded { pb_index_append_sharded } else { pb_index_append };
         let st = unsafe {
-            pb_index_append(self.handle, c, flat.as_ptr(), lens.as_ptr(), lens.len() as i64, 0, path.as_ptr(),
-                            batch_size as i64, &mut first)
+            append(self.handle, c, flat.as_ptr(), lens.as_ptr(), lens.len() as i64, 0, path.as_ptr(), batch_size as i64,
+                   &mut first)
         };
         unsafe { pb_codec_close(c) };
         if st != 0 {
@@ -234,11 +268,23 @@ impl B200Index {
     /// index, negative and repeated ids are ignored.  Returns the number of documents removed; the caller's
     /// `metadata.db` step (`filtering::delete`) follows as before.
     pub fn delete_with_options(&self, doc_ids: &[i64], index_path: &str) -> Result<usize> {
+        self.delete_with(doc_ids, index_path, false)
+    }
+
+    /// `delete_with_options` on a doc-sharded deployment (`pb_index_delete_sharded`): every rank calls it with the same
+    /// global ids, at the same point of its sequence of collective calls.  Each rank renumbers its survivors and moves
+    /// its doc_id_base down; the last rank writes `index_path`.  Returns the number removed over all ranks.  The
+    /// caller's `metadata.db` step (`filtering::delete`) follows once per deployment, not once per rank: the
+    /// directory is shared, and a second run would renumber `metadata.db` again.
+    pub fn delete_with_options_sharded(&self, doc_ids: &[i64], index_path: &str) -> Result<usize> {
+        self.delete_with(doc_ids, index_path, true)
+    }
+
+    fn delete_with(&self, doc_ids: &[i64], index_path: &str, sharded: bool) -> Result<usize> {
         let path = CString::new(index_path).map_err(|e| Error::IndexLoad(e.to_string()))?;
         let mut deleted = 0i64;
-        let st = unsafe {
-            pb_index_delete(self.handle, doc_ids.as_ptr(), doc_ids.len() as i64, path.as_ptr(), &mut deleted)
-        };
+        let delete = if sharded { pb_index_delete_sharded } else { pb_index_delete };
+        let st = unsafe { delete(self.handle, doc_ids.as_ptr(), doc_ids.len() as i64, path.as_ptr(), &mut deleted) };
         if st != 0 {
             return Err(Error::Delete(last_error()));
         }
