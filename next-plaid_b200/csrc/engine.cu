@@ -1018,8 +1018,6 @@ extern "C" pb_status pb_last_work_counters(pb_index *, pb_work_counters *out) {
 // ------------------------------------------------------------------------------------------
 // kernel launch helpers shared by the search pipeline and the stage entry points
 // ------------------------------------------------------------------------------------------
-static pb_status launch_centroid_scores_exact(pb_index *ix, Workspace &ws, int B, int QS, int *launches, bool with16);
-
 // a2 on the tensor cores (k_scores_tc.cuh).  err = certified bound of |exact - estimate| in 16-bit code units
 // (derivation at the top of that file); E = ceil(err) is the largest difference between an estimate-built code and
 // the exact-table code, 2E + 1 the code margin of its consumers.
@@ -1090,6 +1088,37 @@ static int probe_chunk_rows(long long K, int n, int *n_chunks) {
     return rows;
 }
 
+// entries per query token of the threshold-first probe's candidate list
+static int probe16_cap(int n) { return n * std::max(2, 128 / n); }
+
+// The threshold-first probe up to its collect kernel: the candidate lists cleared, every chunk's largest code
+// (k_chunkmax16) and each query token's threshold, the n-th largest of them (k_tau16).  *d_fallback is the device flag
+// k_tau16 and the kernels after it raise when a query cannot take this path.
+static pb_status probe16_thresholds(pb_index *ix, Workspace &ws, int B, int QS, int n, int n_chunks, int chunk_rows,
+                                    int **d_fallback) {
+    const int cap = probe16_cap(n);
+    CKS(ws.cmax16.ensure((size_t)B * n_chunks * QS * 2));
+    CKS(ws.tau16.ensure((size_t)B * QS * 4));
+    CKS(ws.plist.ensure((size_t)B * QS * cap * 8));
+    CKS(ws.pcount.ensure((size_t)B * QS * 4 + 16));
+    CK(cudaMemsetAsync(ws.plist.p, 0, (size_t)B * QS * cap * 8, ws.stream));
+    CK(cudaMemsetAsync(ws.pcount.p, 0, (size_t)B * QS * 4 + 16, ws.stream));
+    int *fb = ws.pcount.as<int>() + (size_t)B * QS;
+    k_chunkmax16<<<dim3((n_chunks + 3) / 4, B), 128, 0, ws.stream>>>(ws.ST16.as<unsigned short>(), ix->K, QS, n_chunks,
+                                                                     chunk_rows, ws.cmax16.as<unsigned short>());
+    k_tau16<<<dim3(QS, B), 32, 0, ws.stream>>>(ws.cmax16.as<unsigned short>(), ws.qoff.as<int>(), QS, n, n_chunks,
+                                              ws.qflag.as<int>(), ws.tau16.as<uint32_t>(), fb);
+    *d_fallback = fb;
+    return PB_OK;
+}
+
+// the smallest power of two >= x: the shared-memory sort and set sizes of the per-query kernels
+static int pow2_at_least(int x) {
+    int P = 1;
+    while (P < x) P <<= 1;
+    return P;
+}
+
 // a2 + a3 on the tensor-core table.  Nothing is read back here: a flagged query or a probe-list overflow raises
 // *d_fallback on the device, the kernels after it stay memory-safe, and the caller redoes the sub-batch on the
 // exact path once it sees the flag at the end.
@@ -1102,33 +1131,23 @@ static pb_status run_k1_tc(pb_index *ix, Workspace &ws, const pb_search_params *
     k_interleave_query_rows<<<dim3(8, B), 256, 0, ws.stream>>>(ws.Q.as<float>(), ws.qoff.as<int>(), QS, ix->dim, ws.Qi.as<float>());
     CKS(launch_k1_table(ix, ws, B, QS, ws.ST16.as<unsigned short>(), ws.qflag.as<int>()));
     L[PB_STAGE_CENTROID_SCORES] += 4;
-    const int cap = n * std::max(2, 128 / n);
+    const int cap = probe16_cap(n);
     const int cells_cap = (int)std::min<long long>((long long)QS * n, ix->K);
-    CKS(ws.cmax16.ensure((size_t)B * n_chunks * QS * 2));
-    CKS(ws.tau16.ensure((size_t)B * QS * 4));
-    CKS(ws.plist.ensure((size_t)B * QS * cap * 8));
-    CKS(ws.pcount.ensure((size_t)B * QS * 4 + 16));
     CKS(ws.sel.ensure((size_t)B * QS * n * 8));
     CKS(ws.cells.ensure((size_t)B * cells_cap * 4));
     CKS(ws.ncells.ensure((size_t)B * 4 + 16));
     CKS(ws.ulist.ensure((size_t)B * cells_cap * 4));
     CKS(ws.nulist.ensure((size_t)B * 4 + 16));
     CKS(ws.k1rows.ensure((size_t)B * cells_cap * QS * 4));
-    CK(cudaMemsetAsync(ws.plist.p, 0, (size_t)B * QS * cap * 8, ws.stream));
-    CK(cudaMemsetAsync(ws.pcount.p, 0, (size_t)B * QS * 4 + 16, ws.stream));
-    int *d_fallback = ws.pcount.as<int>() + (size_t)B * QS;
-    k_chunkmax16<<<dim3((n_chunks + 3) / 4, B), 128, 0, ws.stream>>>(ws.ST16.as<unsigned short>(), ix->K, QS, n_chunks,
-                                                                     chunk_rows, ws.cmax16.as<unsigned short>());
-    k_tau16<<<dim3(QS, B), 32, 0, ws.stream>>>(ws.cmax16.as<unsigned short>(), ws.qoff.as<int>(), QS, n, n_chunks,
-                                              ws.qflag.as<int>(), ws.tau16.as<uint32_t>(), d_fallback);
+    int *d_fallback = nullptr;
+    CKS(probe16_thresholds(ix, ws, B, QS, n, n_chunks, chunk_rows, &d_fallback));
     k_collect16_tc<<<dim3((n_chunks + 3) / 4, B), 128, 0, ws.stream>>>(
         ws.ST16.as<unsigned short>(), ws.Q.as<float>(), ws.qoff.as<int>(), ix->centroids.as<float>(), ix->dim, cm, ix->K, QS,
         n_chunks, chunk_rows, ws.tau16.as<uint32_t>(), cap, ws.pcount.as<int>(), ws.plist.as<u64>(), d_fallback);
     k_topn_merge<<<dim3(QS, B), 32, 0, ws.stream>>>(ws.plist.as<u64>(), ws.qoff.as<int>(), QS, n, cap / n, ws.sel.as<u64>(),
                                                   nullptr, 0);
     // the selected centroids, their exact rows, the variant's threshold rule
-    int P = 1;
-    while (P < std::max(nq_max * n, 1)) P <<= 1;
+    const int P = pow2_at_least(std::max(nq_max * n, 1));
     CKS(set_smem(k_cells_unique, (size_t)P * 8));
     k_cells_unique<<<B, 256, (size_t)P * 8, ws.stream>>>(ws.sel.as<u64>(), ws.qoff.as<int>(), QS, n, cells_cap,
                                                          ws.ulist.as<uint32_t>(), ws.nulist.as<int>());
@@ -1156,13 +1175,9 @@ static pb_status run_k1_tc(pb_index *ix, Workspace &ws, const pb_search_params *
     return PB_OK;
 }
 
+// a2 on the fp32 FMA path: the exact table, with16 also its 16-bit codes (and, with PB_K1_TC_DIAG, their comparison
+// with the tensor-core table)
 static pb_status launch_centroid_scores(pb_index *ix, Workspace &ws, int B, int QS, int *launches, bool with16 = false) {
-    CKS(launch_centroid_scores_exact(ix, ws, B, QS, launches, with16));
-    if (with16 && ix->k1_diag && ix->cent_h16t.p) CKS(launch_k1_diag(ix, ws, B, QS));
-    return PB_OK;
-}
-
-static pb_status launch_centroid_scores_exact(pb_index *ix, Workspace &ws, int B, int QS, int *launches, bool with16) {
     const int tiles = (int)((ix->K + PB_TOK_TILE - 1) / PB_TOK_TILE);
     // enough CTAs to fill the machine twice over; each CTA keeps its centroid tile in smem and walks queries
     int groups = std::max(1, std::min(B, (4 * ix->sm_count + tiles - 1) / tiles));
@@ -1183,6 +1198,7 @@ static pb_status launch_centroid_scores_exact(pb_index *ix, Workspace &ws, int B
     });
     CK(cudaGetLastError());
     if (launches) *launches += 2;
+    if (with16 && ix->k1_diag && ix->cent_h16t.p) CKS(launch_k1_diag(ix, ws, B, QS));
     return PB_OK;
 }
 
@@ -1384,8 +1400,7 @@ static pb_status launch_filter(pb_index *ix, Workspace &ws, const KeptView &in, 
     k_tc_finalize<<<dim3((Mcap + 7) / 8, B), 256, 0, ws.stream>>>(keys, ws.qoff.as<int>(), QS, in.nkept, Mcap, in.tokp,
                                                                   ws.est.as<float>(), keep_keys ? 0 : 1);
     CK(cudaGetLastError());
-    int Pm = 1;
-    while (Pm < Mcap) Pm <<= 1;
+    const int Pm = pow2_at_least(Mcap);
     CKS(set_smem(k_tc_select, (size_t)Pm * 8));
     k_tc_select<<<B, 1024, (size_t)Pm * 8, ws.stream>>>(ws.est.as<float>(), in.kept, in.krank, in.nkept, Mcap, top_k,
                                                         ws.qoff.as<int>(), ws.qnmax.as<float>(), eps_unit,
@@ -1415,7 +1430,25 @@ struct SearchIO {
     pb_trace *trace;
 };
 
-static pb_status search_impl_inner(pb_index *ix, const pb_search_params *p, const SearchIO &io) {
+// what a search call decides once, before its first sub-batch
+struct SearchPlan {
+    int64_t Bt = 0;                           // queries
+    int top_k = 0, M = 0, Mcap = 1;           // M: docs the cut keeps per query (search.rs:468)
+    bool batched = false, sharded = false;    // batched: the centroid-batched variant (search.rs:337)
+    bool empty = false;                       // every result list is empty
+    bool prof = false;                        // stage and call times (pb_set_profiling)
+    long long Wd = 0, Wk = 0;                 // 32-bit words of a doc / centroid bitmap
+    const uint32_t *d_subset_bits = nullptr;  // the subset as a doc bitmap
+    const uint32_t *d_elig = nullptr;         // the centroids holding a subset doc (dense variant with a subset)
+    long long n_elig = 0;
+    bool all_eligible = false;                // the scaled n_ivf_probe covers every eligible centroid: probe them all
+    int n_probe = 0;                          // the effective n_ivf_probe
+    bool big_probe = false;                   // beyond the streaming probe's lists: the row-wise radix select
+    int QB = 0;                               // queries per sub-batch
+};
+
+// The arguments and what follows from them alone.  Nothing is enqueued here, so a call refused here takes no workspace.
+static pb_status plan_search(pb_index *ix, const pb_search_params *p, const SearchIO &io, SearchPlan &plan) {
     if (!ix || !p) return pb_fail(PB_ERR_INVALID, "null argument");
     if (io.n_queries < 0) return pb_fail(PB_ERR_INVALID, "n_queries < 0");
     if (io.n_queries > 0 && (!io.queries || !io.q_off)) return pb_fail(PB_ERR_INVALID, "null queries");
@@ -1425,24 +1458,710 @@ static pb_status search_impl_inner(pb_index *ix, const pb_search_params *p, cons
     if (!io.out_counts) return pb_fail(PB_ERR_INVALID, "null out_counts");
     CK(cudaSetDevice(ix->device));
     g_stats = Stats();
-    const int64_t Bt = io.n_queries;
-    if (Bt == 0) return PB_OK;
-    for (int64_t b = 0; b < Bt; ++b)
+    plan.Bt = io.n_queries;
+    if (plan.Bt == 0) return PB_OK;
+    for (int64_t b = 0; b < plan.Bt; ++b)
         if (io.q_off[b + 1] < io.q_off[b]) return pb_fail(PB_ERR_INVALID, "q_tok_offsets not monotone");
-    const int top_k = (int)p->top_k;
+    plan.top_k = (int)p->top_k;
     const long long n_dec = std::max<long long>(p->n_full_scores / 4, p->top_k);  // search.rs:468
     const long long Mll = std::min<long long>(p->n_full_scores, n_dec);             // take(nfs).take(n_dec)
     if (Mll > 16384)
         return pb_fail(PB_ERR_UNSUPPORTED, "min(n_full_scores, max(n_full_scores/4, top_k)) = %lld exceeds 16384", Mll);
-    const int M = (int)Mll;
-    const int Mcap = std::max(M, 1);
-    const bool batched = p->centroid_batch_size > 0 && ix->K > p->centroid_batch_size;  // search.rs:337
-    const bool sharded = ix->world > 1;
-    if (sharded && io.has_subset && !batched)
+    plan.M = (int)Mll;
+    plan.Mcap = std::max(plan.M, 1);
+    plan.batched = p->centroid_batch_size > 0 && ix->K > p->centroid_batch_size;  // search.rs:337
+    plan.sharded = ix->world > 1;
+    if (plan.sharded && io.has_subset && !plan.batched)
         return pb_fail(PB_ERR_UNSUPPORTED, "subset with the dense variant needs the global eligible-centroid set; "
                                             "not built for doc-sharded indices");
     // a shard with no documents still takes part in the exchanges
-    const bool empty_all = (M == 0 || top_k == 0 || (ix->D == 0 && !sharded));
+    plan.empty = plan.M == 0 || plan.top_k == 0 || (ix->D == 0 && !plan.sharded);
+    plan.prof = ix->profiling;
+    return PB_OK;
+}
+
+// The subset, the probe width and the sub-batch size.  With the dense variant a subset's eligible centroids are counted
+// on the device (search.rs:350-382); none at all leaves the call empty.
+static pb_status plan_probe(pb_index *ix, Workspace &ws, const pb_search_params *p, const SearchIO &io, SearchPlan &plan) {
+    plan.Wd = (ix->D + 31) / 32;
+    plan.Wk = (ix->K + 31) / 32;
+    plan.n_probe = (int)std::min<long long>(p->n_ivf_probe, ix->K);
+    if (io.has_subset) {
+        CKS(ws.subset_bits.ensure((size_t)plan.Wd * 4));
+        CK(cudaMemsetAsync(ws.subset_bits.p, 0, (size_t)plan.Wd * 4, ws.stream));
+        if (io.n_subset > 0) {
+            CKS(ws.subset.ensure((size_t)io.n_subset * 8));
+            CK(cudaMemcpyAsync(ws.subset.p, io.subset, (size_t)io.n_subset * 8, cudaMemcpyHostToDevice, ws.stream));
+            k_subset_bits<<<296, 256, 0, ws.stream>>>(ws.subset.as<long long>(), io.n_subset, ix->doc_id_base, ix->D,
+                                                     ws.subset_bits.as<uint32_t>());
+            CK(cudaGetLastError());
+        }
+        plan.d_subset_bits = ws.subset_bits.as<uint32_t>();
+        if (!plan.batched) {
+            // eligible centroids + n_ivf_probe scaling, dense variant only
+            CKS(ws.elig.ensure((size_t)plan.Wk * 4));
+            CKS(ws.misc.ensure(64));  // [0] the eligible count; +16: k_cells_from_bits' list length (probe)
+            CK(cudaMemsetAsync(ws.elig.p, 0, (size_t)plan.Wk * 4, ws.stream));
+            CK(cudaMemsetAsync(ws.misc.p, 0, 64, ws.stream));
+            k_eligible_bits<<<ix->sm_count * 8, 256, 0, ws.stream>>>(plan.d_subset_bits, ix->D, ix->doc_off.as<long long>(),
+                                                                     ix->codes.as<uint32_t>(), ws.elig.as<uint32_t>());
+            k_popcount<<<ix->sm_count, 256, 0, ws.stream>>>(ws.elig.as<uint32_t>(), plan.Wk, ws.misc.as<unsigned long long>());
+            CK(cudaGetLastError());
+            unsigned long long ne = 0;
+            CK(cudaMemcpyAsync(&ne, ws.misc.p, 8, cudaMemcpyDeviceToHost, ws.stream));
+            CK(cudaStreamSynchronize(ws.stream));
+            plan.n_elig = (long long)ne;
+            if (plan.n_elig == 0) {  // every per-token pool is empty -> no cells -> empty results
+                plan.empty = true;
+                return PB_OK;
+            }
+            unsigned long long scaled = io.n_subset > 0 ? (unsigned long long)p->n_ivf_probe * (unsigned long long)ix->D /
+                                                              (unsigned long long)io.n_subset
+                                                        : (unsigned long long)p->n_ivf_probe;
+            scaled = std::max<unsigned long long>(scaled, (unsigned long long)p->n_ivf_probe);
+            scaled = std::min<unsigned long long>(scaled, (unsigned long long)plan.n_elig);
+            plan.d_elig = ws.elig.as<uint32_t>();
+            if ((long long)scaled >= plan.n_elig) plan.all_eligible = true;
+            else plan.n_probe = (int)scaled;
+        }
+    }
+    // effective n_ivf_probe beyond 64: the dense variant switches to a row-wise radix select; the batched variant's
+    // heap-order threshold rule is tied to the streaming formulation, whose per-lane lists hold up to 192 entries
+    const int stream_max = plan.batched ? 192 : 64;
+    plan.big_probe = !plan.all_eligible && plan.n_probe > stream_max;
+    if (plan.big_probe && plan.batched)
+        return pb_fail(PB_ERR_UNSUPPORTED, "n_ivf_probe %d > 192 with the batched variant is not built", plan.n_probe);
+
+    // ---- sub-batching: bound the transposed score matrix ----
+    const int64_t Bt = plan.Bt;
+    int nq_max_all = 0;
+    for (int64_t b = 0; b < Bt; ++b) nq_max_all = std::max<int>(nq_max_all, (int)(io.q_off[b + 1] - io.q_off[b]));
+    const int QS_all = query_row_tokens(nq_max_all);
+    if (!plan.all_eligible && !plan.big_probe && (long long)QS_all * plan.n_probe > 8192)
+        return pb_fail(PB_ERR_UNSUPPORTED, "query tokens x n_ivf_probe = %lld exceeds 8192", (long long)QS_all * plan.n_probe);
+    size_t per_q = (size_t)ix->K * QS_all * sizeof(float);
+    if (per_q >= ((size_t)1 << 32))
+        return pb_fail(PB_ERR_UNSUPPORTED, "num_centroids x query tokens x 4 = %zu bytes per query exceeds 2^32", per_q);
+    // sub-batch size: the score tables (16-bit always, fp32 only on the exact path) and the per-(query, doc) scratch
+    // (candidate lists, code sums, approximate scores, cut keys, bitmap: 24.2 bytes per document) share one budget
+    const size_t per_q_all = (size_t)ix->K * QS_all * (k1_tc_usable(ix) ? 2 : 6) + (size_t)ix->D * 24 + (size_t)ix->D / 8 + 4096;
+    int QB = (int)std::max<size_t>(1, std::min<size_t>((size_t)Bt, ix->st_budget / std::max(g_budget_div, 1) / per_q_all));
+    QB = std::min(QB, 256);
+    plan.QB = (int)((Bt + (Bt + QB - 1) / QB - 1) / ((Bt + QB - 1) / QB));  // equal sub-batches
+    return PB_OK;
+}
+
+// The pinned read-back of one pass (ws.hcounts): the query offsets that go up, then what comes back.  Placed here only.
+struct HostCounts {
+    int *qoff;                // [B + 1] query token offsets of the sub-batch
+    unsigned long long *cnt;  // [B + 2] ws.counters
+    long long *surv_tok;      // [B] tokens of the filter's survivors
+    int *cells, *cand, *kept, *surv, *recheck, *pairs, *need;  // [B] each
+    int *fell;                // the threshold-first probe's fallback flag
+};
+static pb_status map_host_counts(HostBuf &hb, int B, HostCounts &h) {
+    const size_t at_cnt = ((size_t)(B + 1) * 4 + 15) & ~(size_t)15, at_tok = at_cnt + (size_t)(B + 2) * 8,
+                 at_int = at_tok + (size_t)B * 8;
+    CKS(hb.ensure(at_int + ((size_t)7 * B + 1) * 4));
+    char *base = hb.as<char>();
+    h.qoff = reinterpret_cast<int *>(base);
+    h.cnt = reinterpret_cast<unsigned long long *>(base + at_cnt);
+    h.surv_tok = reinterpret_cast<long long *>(base + at_tok);
+    int *c = reinterpret_cast<int *>(base + at_int);
+    for (int **f : {&h.cells, &h.cand, &h.kept, &h.surv, &h.recheck, &h.pairs, &h.need, &h.fell}) *f = c, c += B;
+    return PB_OK;
+}
+
+// One pass of the pipeline over a sub-batch: its inputs, then what one stage hands to a later one
+struct Pass {
+    int64_t b0 = 0, r0 = 0, R = 0;  // first query, its first token, the sub-batch's tokens
+    int B = 0, nq_max = 0, QS = 0;
+    // use_tc: a2 + a3 on the tensor cores.  A flagged query or a probe-list overflow raises a device flag instead of
+    // being read back mid-way; the pass then finishes on (memory-safe) garbage and is redone on the exact path.
+    bool use_tc = false;
+    bool fast = false;  // the two-pass approximate stage on the 16-bit score table
+    HostCounts hc{};
+    // a2 / a3
+    int cells_cap = 0;
+    const int *d_probe_fallback = nullptr;  // device flag of the threshold-first probe (0 = it did the work)
+    bool probe_list_only = false;
+    // a5: the candidates that carry an approximate score
+    const uint32_t *cand_list = nullptr;
+    const int *cand_n = nullptr;
+    // a7: the filter's form, and the docs scored exactly
+    bool filt = false, pairs = false, diag = false;
+    KeptView kv{};
+    // a9: the results of the sub-batch on the device
+    long long *d_ids = nullptr;
+    float *d_sc = nullptr;
+    int *d_cn = nullptr;
+};
+
+// H2D: the query tokens and offsets of the sub-batch
+static pb_status upload_queries(pb_index *ix, Workspace &ws, const SearchIO &io, Pass &pass) {
+    const int B = pass.B;
+    const size_t bytes = (size_t)pass.R * ix->dim * 4;
+    CKS(ws.Q.ensure(std::max<size_t>(bytes, 16)));
+    CKS(ws.qoff.ensure((size_t)(B + 1) * 4));
+    if (pass.R > 0) {
+        const float *src = io.queries + (size_t)pass.r0 * ix->dim;
+        if (io.queries_on_device)
+            CK(cudaMemcpyAsync(ws.Q.p, src, bytes, cudaMemcpyDeviceToDevice, ws.stream));
+        else {
+            CKS(ws.hq.ensure(bytes));
+            memcpy(ws.hq.p, src, bytes);
+            CK(cudaMemcpyAsync(ws.Q.p, ws.hq.p, bytes, cudaMemcpyHostToDevice, ws.stream));
+        }
+    }
+    CKS(map_host_counts(ws.hcounts, B, pass.hc));
+    for (int b = 0; b <= B; ++b) pass.hc.qoff[b] = (int)(io.q_off[pass.b0 + b] - pass.r0);
+    CK(cudaMemcpyAsync(ws.qoff.p, pass.hc.qoff, (size_t)(B + 1) * 4, cudaMemcpyHostToDevice, ws.stream));
+    return PB_OK;
+}
+
+// a2: the centroid score table, fp32 off the tensor cores and 16-bit on a fast pass; on the tensor cores also a3
+static pb_status centroid_scores(pb_index *ix, Workspace &ws, const pb_search_params *p, const SearchPlan &plan,
+                                 Pass &pass) {
+    const int B = pass.B, QS = pass.QS;
+    int *L = g_stats.launches;
+    if (!pass.use_tc) CKS(ws.ST.ensure((size_t)B * ix->K * QS * sizeof(float)));
+    if (pass.fast) {
+        CKS(ws.ST16.ensure((size_t)B * ix->K * QS * 2));
+        CKS(ws.qrange.ensure((size_t)B * 8 + 16));
+        CKS(ws.qflag.ensure((size_t)B * 4 + 16));
+        CKS(ws.qexp.ensure((size_t)B * 4 + 16));
+        CKS(ws.qnmax.ensure((size_t)B * 4 + 16));
+        k_query_range<<<B, 256, 0, ws.stream>>>(ws.Q.as<float>(), ws.qoff.as<int>(), ix->dim, ix->cmax,
+                                                ws.qrange.as<float2>(), ws.qflag.as<int>(), ws.qexp.as<int>(),
+                                                ws.qnmax.as<float>());
+        CK(cudaGetLastError());
+        L[PB_STAGE_CENTROID_SCORES] += 1;
+    }
+    if (pass.use_tc)
+        return run_k1_tc(ix, ws, p, B, QS, pass.nq_max, plan.n_probe, plan.batched, L, &pass.cells_cap,
+                         &pass.d_probe_fallback);
+    return launch_centroid_scores(ix, ws, B, QS, &L[PB_STAGE_CENTROID_SCORES], pass.fast);
+}
+
+// a3: the cells (centroids) each query probes, on the fp32 table; the tensor-core pass placed them in a2
+static pb_status probe(pb_index *ix, Workspace &ws, const pb_search_params *p, const SearchPlan &plan, Pass &pass) {
+    if (pass.use_tc) return PB_OK;
+    const int B = pass.B, QS = pass.QS;
+    int *L = g_stats.launches;
+    if (plan.all_eligible) {
+        pass.cells_cap = (int)plan.n_elig;
+        CKS(ws.list.ensure((size_t)plan.n_elig * 4 + 16));
+        CKS(ws.cells.ensure((size_t)B * pass.cells_cap * 4));
+        CKS(ws.ncells.ensure((size_t)B * 4 + 16));
+        int *d_listn = reinterpret_cast<int *>(ws.misc.as<char>() + 16);
+        k_cells_from_bits<<<1, 1024, 0, ws.stream>>>(plan.d_elig, ix->K, ws.list.as<uint32_t>(), d_listn);
+        k_cells_filter_list<<<B, 256, 0, ws.stream>>>(ws.list.as<uint32_t>(), d_listn, ws.ST.as<float>(),
+                                                      ws.qoff.as<int>(), ix->K, QS, p->has_centroid_score_threshold,
+                                                      p->centroid_score_threshold, pass.cells_cap, ws.cells.as<uint32_t>(),
+                                                      ws.ncells.as<int>());
+        CK(cudaGetLastError());
+        L[PB_STAGE_PROBE] += 2;
+        return PB_OK;
+    }
+    const int n = plan.n_probe;
+    pass.cells_cap = (int)std::min<long long>((long long)QS * n, ix->K);
+    if (plan.big_probe) {
+        CKS(ws.cellbits.ensure((size_t)B * plan.Wk * 4));
+        CKS(ws.cells.ensure((size_t)B * pass.cells_cap * 4));
+        CKS(ws.ncells.ensure((size_t)B * 4 + 16));
+        k_topn_select_row<<<dim3(QS, B), 256, 0, ws.stream>>>(ws.ST.as<float>(), ws.qoff.as<int>(), ix->K, QS, n,
+                                                              plan.d_elig, ws.cellbits.as<uint32_t>(), plan.Wk);
+        k_cells_from_query_bits<<<B, 1024, 0, ws.stream>>>(ws.cellbits.as<uint32_t>(), plan.Wk, ws.ST.as<float>(),
+                                                           ws.qoff.as<int>(), ix->K, QS, p->has_centroid_score_threshold,
+                                                           p->centroid_score_threshold, pass.cells_cap,
+                                                           ws.cells.as<uint32_t>(), ws.ncells.as<int>());
+        CK(cudaGetLastError());
+        L[PB_STAGE_PROBE] += 2;
+        return PB_OK;
+    }
+    const int n_chunks = (int)((ix->K + 1023) / 1024);
+    CKS(ws.partial.ensure((size_t)B * QS * n_chunks * n * 8));
+    CKS(ws.sel.ensure((size_t)B * QS * n * 8));
+    CKS(ws.cells.ensure((size_t)B * pass.cells_cap * 4));
+    CKS(ws.ncells.ensure((size_t)B * 4 + 16));
+    size_t sm1 = (size_t)4 * n * 32 * 8;
+    CKS(set_smem(k_topn_partial, sm1));
+    // threshold-first selection on the 16-bit table when there is one (k_chunkmax16 / k_collect16);
+    // the per-lane list scan of k_topn_partial otherwise, or when the device raises `fallback`
+    const int GQ = QS / 8;
+    int t_chunks = 0;
+    const int t_rows = probe_chunk_rows(ix->K, n, &t_chunks);
+    const bool thr_path = pass.fast && !plan.d_elig && ix->probe16 && GQ <= 32 && t_chunks >= n && n <= 192;
+    int *d_fallback = nullptr;
+    pass.probe_list_only = !thr_path;
+    if (thr_path) {
+        const int cap = probe16_cap(n);
+        CKS(probe16_thresholds(ix, ws, B, QS, n, t_chunks, t_rows, &d_fallback));
+        pass.d_probe_fallback = d_fallback;
+        k_collect16<<<dim3((t_chunks + 3) / 4, B), 128, 0, ws.stream>>>(
+            ws.ST16.as<unsigned short>(), ws.ST.as<float>(), ix->K, QS, t_chunks, t_rows, ws.tau16.as<uint32_t>(), cap,
+            ws.pcount.as<int>(), ws.plist.as<u64>(), d_fallback);
+        k_topn_merge<<<dim3(QS, B), 32, 0, ws.stream>>>(ws.plist.as<u64>(), ws.qoff.as<int>(), QS, n, cap / n,
+                                                      ws.sel.as<u64>(), d_fallback, 0);
+        CK(cudaGetLastError());
+        L[PB_STAGE_PROBE] += 4;
+    }
+    k_topn_partial<<<dim3((n_chunks + 3) / 4, B, (QS + 31) / 32), 128, sm1, ws.stream>>>(
+        ws.ST.as<float>(), ws.qoff.as<int>(), ix->K, QS, n, plan.d_elig, ws.partial.as<u64>(), n_chunks, d_fallback, 1);
+    k_topn_merge<<<dim3(QS, B), 32, 0, ws.stream>>>(ws.partial.as<u64>(), ws.qoff.as<int>(), QS, n, n_chunks,
+                                                  ws.sel.as<u64>(), d_fallback, 1);
+    const int P = pow2_at_least(std::max(pass.nq_max * n, 1));
+    size_t sm2 = (size_t)P * 12;
+    CKS(set_smem(k_cells, sm2));
+    k_cells<<<B, 256, sm2, ws.stream>>>(ws.sel.as<u64>(), ws.ST.as<float>(), ws.qoff.as<int>(), ix->K, QS, n,
+                                        pass.cells_cap, p->has_centroid_score_threshold, p->centroid_score_threshold,
+                                        plan.batched ? 1 : 0, plan.batched ? (long long)p->centroid_batch_size : ix->K,
+                                        ws.cells.as<uint32_t>(), ws.ncells.as<int>(),
+                                        thr_path ? ws.cmax16.as<unsigned short>() : nullptr, t_chunks, t_rows,
+                                        ws.qrange.as<float2>(), d_fallback);
+    CK(cudaGetLastError());
+    L[PB_STAGE_PROBE] += 3;
+    return PB_OK;
+}
+
+// a4: the docs of the probed cells (within the subset), compacted per query
+static pb_status candidates(pb_index *ix, Workspace &ws, const SearchPlan &plan, const Pass &pass) {
+    const int B = pass.B;
+    const long long Wd = plan.Wd;
+    CKS(ws.bitmap.ensure((size_t)B * Wd * 4));
+    CKS(ws.cand.ensure((size_t)B * ix->D * 4));
+    CKS(ws.ncand.ensure((size_t)B * 4 + 16));
+    k_mark<<<dim3(pass.cells_cap, B), 128, 0, ws.stream>>>(ws.cells.as<uint32_t>(), ws.ncells.as<int>(), pass.cells_cap,
+                                                          ix->ivf.as<uint32_t>(), ix->ivf_off.as<long long>(),
+                                                          plan.d_subset_bits, ws.bitmap.as<uint32_t>(), Wd);
+    const int slices = (int)std::max<long long>(1, std::min<long long>(32, (4ll * ix->sm_count + B - 1) / B));
+    CKS(ws.slicecnt.ensure((size_t)B * slices * 4));
+    k_compact_count<<<dim3(slices, B), 256, 0, ws.stream>>>(ws.bitmap.as<uint32_t>(), Wd, ws.slicecnt.as<int>());
+    k_compact_emit<<<dim3(slices, B), 256, 0, ws.stream>>>(ws.bitmap.as<uint32_t>(), Wd, ws.slicecnt.as<int>(),
+                                                           ws.cand.as<uint32_t>(), ix->D, ws.ncand.as<int>());
+    CK(cudaGetLastError());
+    g_stats.launches[PB_STAGE_CANDIDATES] += 3;
+    return PB_OK;
+}
+
+// a5: the approximate score of every candidate; a fast pass first narrows them to the band around the cut on the
+// 16-bit table, and the tensor-core pass re-checks that band with pinned-order dots
+static pb_status approx_scores(pb_index *ix, Workspace &ws, const SearchPlan &plan, Pass &pass) {
+    const int B = pass.B, QS = pass.QS, Mcap = plan.Mcap;
+    int *L = g_stats.launches;
+    CKS(ws.counters.ensure((size_t)(B + 2) * 8));  // [0] candidate codes gathered, [1+b] kept-doc tokens, [B+1] re-check gathers
+    CK(cudaMemsetAsync(ws.counters.p, 0, (size_t)(B + 2) * 8, ws.stream));
+    CKS(ws.approx.ensure((size_t)B * ix->D * 4));
+    CKS(ws.keys.ensure((size_t)B * ix->D * 8));
+    if (pass.fast) {
+        CKS(ws.lsum.ensure((size_t)B * ix->D * 4));
+        CKS(ws.cand2.ensure((size_t)B * ix->D * 4));
+        CKS(ws.ncand2.ensure((size_t)B * 4 + 16));
+        const dim3 ga(ix->sm_count * ix->approx_grid, B);
+        const unsigned short *st16 = ws.ST16.as<unsigned short>();
+        const uint32_t *list = ws.cand.as<uint32_t>();
+        const int *list_n = ws.ncand.as<int>();
+        unsigned long long *cnt = ws.counters.as<unsigned long long>();
+        KEV_BEGIN(PB_KERNEL_APPROX16);
+        (QS <= 32 ? k_approx16<4> : k_approx16<8>)<<<ga, 256, 0, ws.stream>>>(
+            st16, ws.qoff.as<int>(), ix->K, QS, ix->ucodes.as<uint32_t>(), ix->udoc_off.as<long long>(), list, ix->D, list_n,
+            ws.lsum.as<uint32_t>(), cnt);
+        KEV_END(PB_KERNEL_APPROX16);
+        // band per query token in code units (W = band * nq + 8).  Exact table: +-1 code of rounding per token and side
+        // plus the fp32 summation error -> 4.  Estimate table (k_scores_tc.cuh): W = nq (1.004 + 2 err) + nq^2/256 + 4
+        // <= nq (ceil(1.004 + 2 err) + 1) + 8 for nq <= 256.
+        const int band_per_q =
+            pass.use_tc ? (int)ceilf(1.004f + 2.0f * std::max(k1_err_codes(ix->dim), (float)(ix->k1_margin - 1))) + 1 : 4;
+        k_select_u32<<<B, 1024, 0, ws.stream>>>(ws.lsum.as<uint32_t>(), list_n, plan.M, band_per_q, ws.lsum.as<uint32_t>(),
+                                                list, list_n, ix->D, ws.qoff.as<int>(), ws.qflag.as<int>(),
+                                                ws.cand2.as<uint32_t>(), ws.ncand2.as<int>());
+        CK(cudaGetLastError());
+        L[PB_STAGE_APPROX] += 2;
+    }
+    pass.cand_list = pass.fast ? ws.cand2.as<uint32_t>() : ws.cand.as<uint32_t>();
+    pass.cand_n = pass.fast ? ws.ncand2.as<int>() : ws.ncand.as<int>();
+    if (pass.use_tc) {  // the exact approximate score of the docs around the cut from pinned-order dots (no dense fp32 S)
+        const int rc_cap = 2 * Mcap + 1024, pair_cap = 64 * rc_cap;
+        CKS(ws.rcmax.ensure((size_t)B * rc_cap * QS * 4));
+        CKS(ws.rcpairs.ensure((size_t)B * pair_cap * 8));
+        CKS(ws.rcn.ensure((size_t)B * 4 + 16));
+        CK(cudaMemsetAsync(ws.rcn.p, 0, (size_t)B * 4, ws.stream));
+        int *d_fb = const_cast<int *>(pass.d_probe_fallback);
+        (QS <= 32 ? k_recheck_pairs<4> : k_recheck_pairs<8>)<<<dim3(ix->sm_count * 2, B), 256, 0, ws.stream>>>(
+            ws.ST16.as<unsigned short>(), ws.qoff.as<int>(), ix->K, QS, ix->ucodes.as<uint32_t>(), ix->udoc_off.as<long long>(),
+            pass.cand_list, ix->D, pass.cand_n, 2 * ix->k1_margin + 1, rc_cap, pair_cap, ws.rcpairs.as<u64>(),
+            ws.rcn.as<int>(), d_fb, ws.counters.as<unsigned long long>() + B + 1);
+        k_recheck_dots<<<dim3(ix->sm_count * 2, B), 128, 0, ws.stream>>>(ws.rcpairs.as<u64>(), ws.rcn.as<int>(), pair_cap,
+                                                                         ws.Q.as<float>(), ws.qoff.as<int>(),
+                                                                         ix->centroids.as<float>(), ix->dim, rc_cap, QS,
+                                                                         ws.rcmax.as<uint32_t>());
+        k_recheck_sum<<<dim3(ix->sm_count, B), 256, 0, ws.stream>>>(ws.rcmax.as<uint32_t>(), ws.qoff.as<int>(), QS,
+                                                                    pass.cand_list, ix->D, pass.cand_n, rc_cap,
+                                                                    ws.approx.as<float>(), ws.keys.as<u64>(),
+                                                                    (uint32_t)ix->doc_id_base);
+        L[PB_STAGE_APPROX] += 2;
+    } else
+        k_approx<<<dim3(ix->sm_count * 8, B), 256, 0, ws.stream>>>(
+            ws.ST.as<float>(), ws.qoff.as<int>(), ix->K, QS, ix->ucodes.as<uint32_t>(), ix->udoc_off.as<long long>(),
+            pass.cand_list, ix->D, pass.cand_n, ws.approx.as<float>(), ws.keys.as<u64>(),
+            pass.fast ? ws.counters.as<unsigned long long>() + B + 1 : ws.counters.as<unsigned long long>(),
+            (uint32_t)ix->doc_id_base);
+    CK(cudaGetLastError());
+    L[PB_STAGE_APPROX] += 1;
+    return PB_OK;
+}
+
+// a6: the top M by approximate score; doc-sharded, exchange 1 makes it the global cut
+static pb_status cut(pb_index *ix, Workspace &ws, const SearchPlan &plan, const Pass &pass) {
+    const int B = pass.B, M = plan.M, Mcap = plan.Mcap;
+    const bool sharded = plan.sharded;
+    CKS(ws.kept.ensure((size_t)B * Mcap * 4));
+    CKS(ws.nkept.ensure((size_t)B * 4 + 16));
+    CKS(ws.tokp.ensure((size_t)B * (Mcap + 1) * 8));
+    if (sharded) CKS(ws.lkeys.ensure((size_t)B * Mcap * 8));
+    const int Pm = pow2_at_least(Mcap);
+    CKS(set_smem(k_cut, (size_t)Pm * 8));
+    k_cut<<<B, 1024, (size_t)Pm * 8, ws.stream>>>(ws.keys.as<u64>(), ws.approx.as<float>(), ix->D, pass.cand_n, M,
+                                                  Mcap, ix->doc_off.as<long long>(), ws.kept.as<uint32_t>(),
+                                                  ws.nkept.as<int>(), ws.tokp.as<long long>(),
+                                                  ws.counters.as<long long>() + 1, (uint32_t)ix->doc_id_base,
+                                                  sharded ? ws.lkeys.as<u64>() : nullptr);
+    CK(cudaGetLastError());
+    g_stats.launches[PB_STAGE_CUT] += 1;
+    if (sharded) {
+        // exchange 1: every shard's sorted top-M cut keys -> global cut -> my members (SURVEY 8e)
+        const int G = ix->world;
+        CKS(ws.gkeys.ensure((size_t)G * B * M * 8));
+        CKS(ws.krank.ensure((size_t)B * Mcap * 4));
+        CKS(shard_allgather(ix, ws.stream, ws.lkeys.p, ws.gkeys.p, (size_t)B * M));
+        k_merge_cut<<<B, 1024, 0, ws.stream>>>(ws.gkeys.as<u64>(), G, ix->rank, B, M, (uint32_t)ix->doc_id_base, ix->D,
+                                               ix->doc_off.as<long long>(), ws.kept.as<uint32_t>(),
+                                               ws.krank.as<uint32_t>(), ws.nkept.as<int>(),
+                                               ws.tokp.as<long long>(), ws.counters.as<long long>() + 1);
+        CK(cudaGetLastError());
+        g_stats.launches[PB_STAGE_CUT] += 2;
+    }
+    return PB_OK;
+}
+
+// a7 + a8: the exact MaxSim of the kept docs.  Only the top_k need exact scores: the tensor-core filter (a7') first
+// drops the docs that provably cannot reach them, and its pass 2 lists the (token, q) pairs k_pair_exact evaluates.
+static pb_status exact_scores(pb_index *ix, Workspace &ws, const SearchIO &io, const SearchPlan &plan, Pass &pass) {
+    const int B = pass.B, QS = pass.QS, nq_max = pass.nq_max, Mcap = plan.Mcap;
+    const bool sharded = plan.sharded;
+    const long long max_tokens = (long long)Mcap * std::max(ix->max_doclen, 1);
+    int *L = g_stats.launches;
+    CKS(ws.maxkey.ensure((size_t)B * Mcap * QS * 4));
+    CKS(ws.exact.ensure((size_t)B * Mcap * 4));
+    CKS(ws.fkeys.ensure((size_t)B * Mcap * 8));
+    KeptView &kv = pass.kv;
+    kv = {ws.kept.as<uint32_t>(), ws.nkept.as<int>(), ws.tokp.as<long long>(), sharded ? ws.krank.as<uint32_t>() : nullptr};
+    // the linear form needs the 16-bit score table of this pass (a flagged query publishes no estimate and keeps
+    // every doc); without a table (PB_FAST_APPROX=0) the decompressing form estimates from fp16 centroids
+    const bool linear = pass.fast && !ix->filter_v1 && ix->tok_inv_norm.p;
+    const float eps_unit = linear ? filter_eps_unit2(ix, pass.use_tc ? ix->k1_margin : 0) : filter_eps_unit(ix);
+    pass.filt = ix->fast_exact && !io.trace && ix->centroids_f16.p && eps_unit > 0.0f && nq_max <= 64 &&
+                plan.top_k < Mcap && ix->packed % 4 == 0;
+    // PB_FILTER_DIAG: the filter runs as usual, then every kept doc is scored exactly (the results of
+    // pb_set_fast_exact(0)) and k_filter_diag compares the pass-1 estimate maxima with the exact ones
+    pass.diag = pass.filt && ix->filter_diag;
+    if (pass.filt) {
+        CKS(ws.est.ensure((size_t)B * Mcap * 4));
+        CKS(ws.kept2.ensure((size_t)B * Mcap * 4));
+        CKS(ws.krank2.ensure((size_t)B * Mcap * 4));
+        CKS(ws.nkept2.ensure((size_t)B * 4 + 16));
+        CKS(ws.tokp2.ensure((size_t)B * (Mcap + 1) * 8));
+        CKS(ws.ktok2.ensure((size_t)B * 8 + 16));
+        if (!pass.fast) {  // the two-pass mode computed them with the score range
+            CKS(ws.qnmax.ensure((size_t)B * 4 + 16));
+            CKS(ws.qexp.ensure((size_t)B * 4 + 16));
+            k_query_range<<<B, 256, 0, ws.stream>>>(ws.Q.as<float>(), ws.qoff.as<int>(), ix->dim, ix->cmax, nullptr, nullptr,
+                                                    ws.qexp.as<int>(), ws.qnmax.as<float>());
+            CK(cudaGetLastError());
+            L[PB_STAGE_EXACT] += 1;
+        }
+        KeptView kv2{ws.kept2.as<uint32_t>(), ws.nkept2.as<int>(), ws.tokp2.as<long long>(), ws.krank2.as<uint32_t>()};
+        // pair form of the exact stage: pass 2 of the estimate over the survivors lists the (token, q) pairs that can
+        // hold a per-token maximum, k_pair_exact evaluates them in the pinned order; a query whose list overflows
+        // (or that published no estimate) goes through k_exact
+        pass.pairs = !pass.diag && linear && ix->pair_exact && Mcap <= 65535 && QS <= 256;
+        if (pass.pairs || pass.diag) {
+            CKS(ws.estkey.ensure((size_t)B * Mcap * QS * 4));
+            CKS(ws.srcrank.ensure((size_t)B * Mcap * 4));
+        }
+        CKS(launch_filter(ix, ws, kv, kv2, B, QS, Mcap, plan.top_k, max_tokens, eps_unit, nq_max, linear,
+                          pass.pairs || pass.diag, &L[PB_STAGE_EXACT]));
+        if (!pass.diag) {
+            kv = kv2;
+            if (!sharded) kv.krank = nullptr;  // survivors keep their order, so position breaks ties the same way
+        }
+    }
+    if (pass.pairs) {
+        const int pair_cap = 16 * Mcap + 4096;  // ~ (top_k + ties) * nq * (1 + a few) pairs per query in practice
+        CKS(ws.xpairs.ensure((size_t)B * pair_cap * 8));
+        CKS(ws.xnpairs.ensure((size_t)B * 4 + 16));
+        CKS(ws.needexact.ensure((size_t)B * 4 + 16));
+        CK(cudaMemsetAsync(ws.xnpairs.p, 0, (size_t)B * 4, ws.stream));
+        KEV_BEGIN(PB_KERNEL_EXACT);  // pass 2 + pair evaluation + the (normally empty) k_exact of flagged queries
+        CKS(launch_maxsim_tc(ix, ws, kv, B, QS, Mcap, max_tokens, nq_max, ws.estkey.as<uint32_t>(),
+                             ws.srcrank.as<uint32_t>(), eps_unit, ws.xpairs.as<u64>(), ws.xnpairs.as<int>(), pair_cap, -1));
+        k_pair_overflow<<<(B + 255) / 256, 256, 0, ws.stream>>>(ws.xnpairs.as<int>(), pair_cap, ws.qflag.as<int>(), B,
+                                                                ws.needexact.as<int>());
+        CK(cudaGetLastError());
+        const size_t smp = ((size_t)(nq_max + 256) * (ix->dim + 1) + 256) * 4;
+        const int pe_ctas = std::max(1, std::min(16, (2 * ix->sm_count + B - 1) / B));  // about one wave over the batch
+        switch (ix->dim) {
+#define PB_PE(DV)                                                                                                      \
+    case DV: {                                                                                                         \
+        CKS(set_smem(k_pair_exact<DV>, smp));                                                                          \
+        k_pair_exact<DV><<<dim3(pe_ctas, B), 256, smp, ws.stream>>>(                                                   \
+            ws.xpairs.as<u64>(), ws.xnpairs.as<int>(), pair_cap, ws.Q.as<float>(), ws.qoff.as<int>(), QS,              \
+            ix->centroids.as<float>(), ix->w_rev.as<float>(), ix->nbits, ix->codes.as<uint32_t>(),                     \
+            ix->residuals.as<uint8_t>(), Mcap, ws.maxkey.as<uint32_t>());                                              \
+    } break;
+            PB_PE(64) PB_PE(96) PB_PE(128)
+#undef PB_PE
+            default: return pb_fail(PB_ERR_UNSUPPORTED, "pair exact: unsupported dim");
+        }
+        CK(cudaGetLastError());
+        L[PB_STAGE_EXACT] += 5;
+        CKS(launch_exact(ix, ws, kv, B, QS, Mcap, 0, max_tokens, &L[PB_STAGE_EXACT], ws.needexact.as<int>(), false));
+        KEV_END(PB_KERNEL_EXACT);
+    } else {
+        CKS(launch_exact(ix, ws, kv, B, QS, Mcap, 0, max_tokens, &L[PB_STAGE_EXACT]));
+    }
+    if (pass.diag) {  // before k_exact_finalize, which clears the exact maxima
+        CKS(ws.fdiag.ensure(16));
+        CK(cudaMemsetAsync(ws.fdiag.p, 0, 16, ws.stream));
+        k_filter_diag<<<dim3(4, B), 256, 0, ws.stream>>>(ws.estkey.as<uint32_t>(), ws.maxkey.as<uint32_t>(), ws.qoff.as<int>(),
+                                                         QS, kv.nkept, Mcap, ws.qnmax.as<float>(),
+                                                         linear ? ws.qflag.as<int>() : nullptr, eps_unit,
+                                                         ws.fdiag.as<unsigned long long>());
+        CK(cudaGetLastError());
+        L[PB_STAGE_EXACT] += 1;
+    }
+    if (sharded) {
+        CKS(ws.payload.ensure((size_t)B * Mcap * 8));
+        CK(cudaMemsetAsync(ws.fkeys.p, 0xff, (size_t)B * Mcap * 8, ws.stream));  // ~0 = no entry
+    }
+    k_exact_finalize<<<dim3((Mcap + 7) / 8, B), 256, 0, ws.stream>>>(
+        ws.maxkey.as<uint32_t>(), ws.qoff.as<int>(), QS, kv.nkept, Mcap, 0, ws.exact.as<float>(),
+        ws.fkeys.as<u64>(), kv.krank, kv.kept, (uint32_t)ix->doc_id_base, sharded ? ws.payload.as<u64>() : nullptr);
+    CK(cudaGetLastError());
+    L[PB_STAGE_EXACT] += 1;
+    return PB_OK;
+}
+
+// a9: the top_k by exact score, into the caller's device outputs or the workspace's; doc-sharded, exchange 2 merges
+// every shard's
+static pb_status select_topk(pb_index *ix, Workspace &ws, const SearchIO &io, const SearchPlan &plan, Pass &pass) {
+    const int B = pass.B, M = plan.M, top_k = plan.top_k, Mcap = plan.Mcap;
+    if (io.out_on_device) {
+        pass.d_ids = reinterpret_cast<long long *>(io.out_ids) + (size_t)pass.b0 * top_k;
+        pass.d_sc = io.out_scores + (size_t)pass.b0 * top_k;
+        pass.d_cn = io.out_counts + pass.b0;
+    } else {
+        CKS(ws.oids.ensure((size_t)B * top_k * 8));
+        CKS(ws.oscores.ensure((size_t)B * top_k * 4));
+        CKS(ws.ocounts.ensure((size_t)B * 4 + 16));
+        pass.d_ids = ws.oids.as<long long>();
+        pass.d_sc = ws.oscores.as<float>();
+        pass.d_cn = ws.ocounts.as<int>();
+    }
+    const int Pm = pow2_at_least(Mcap);
+    if (plan.sharded) {
+        // exchange 2: (exact key | global approx rank) + (doc id | score) of every shard, merged on every rank
+        const int G = ix->world;
+        CKS(ws.gfkeys.ensure((size_t)G * B * M * 8));
+        CKS(ws.gpayload.ensure((size_t)G * B * M * 8));
+        CKS(shard_allgather(ix, ws.stream, ws.fkeys.p, ws.gfkeys.p, (size_t)B * M));
+        CKS(shard_allgather(ix, ws.stream, ws.payload.p, ws.gpayload.p, (size_t)B * M));
+        CKS(ws.mslot.ensure((size_t)B * Mcap * 4));
+        CKS(set_smem(k_merge_topk, (size_t)Pm * 8));
+        k_merge_topk<<<B, 1024, (size_t)Pm * 8, ws.stream>>>(ws.gfkeys.as<u64>(), ws.gpayload.as<u64>(), G, B, M, top_k,
+                                                            ws.mslot.as<uint32_t>(), pass.d_ids, pass.d_sc, pass.d_cn);
+        CK(cudaGetLastError());
+        g_stats.launches[PB_STAGE_TOPK] += 3;
+    } else {
+        CKS(set_smem(k_topk, (size_t)Pm * 8));
+        k_topk<<<B, 1024, (size_t)Pm * 8, ws.stream>>>(ws.fkeys.as<u64>(), ws.exact.as<float>(), pass.kv.kept,
+                                                       pass.kv.nkept, Mcap, top_k, ix->doc_id_base, pass.d_ids,
+                                                       pass.d_sc, pass.d_cn);
+        CK(cudaGetLastError());
+        g_stats.launches[PB_STAGE_TOPK] += 1;
+    }
+    return PB_OK;
+}
+
+// D2H and the pass's one synchronise.  A tensor-core pass that gave up on the device stops there with *redo: its
+// launches stay counted, its stage times are not added.  Otherwise the results go out and the pass is accounted.
+static pb_status finish(pb_index *ix, Workspace &ws, const SearchIO &io, const SearchPlan &plan, const Pass &pass,
+                        bool *redo) {
+    const int B = pass.B, top_k = plan.top_k;
+    const HostCounts &hc = pass.hc;
+    *hc.fell = 0;
+    CK(cudaMemcpyAsync(hc.cells, ws.ncells.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
+    CK(cudaMemcpyAsync(hc.cand, ws.ncand.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
+    CK(cudaMemcpyAsync(hc.kept, ws.nkept.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
+    CK(cudaMemcpyAsync(hc.cnt, ws.counters.p, (size_t)(B + 2) * 8, cudaMemcpyDeviceToHost, ws.stream));
+    if (pass.filt) {
+        CK(cudaMemcpyAsync(hc.surv_tok, ws.ktok2.p, (size_t)B * 8, cudaMemcpyDeviceToHost, ws.stream));
+        CK(cudaMemcpyAsync(hc.surv, ws.nkept2.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
+    }
+    if (pass.fast) CK(cudaMemcpyAsync(hc.recheck, ws.ncand2.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
+    if (pass.pairs) {
+        CK(cudaMemcpyAsync(hc.pairs, ws.xnpairs.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
+        CK(cudaMemcpyAsync(hc.need, ws.needexact.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
+    }
+    if (pass.d_probe_fallback) CK(cudaMemcpyAsync(hc.fell, pass.d_probe_fallback, 4, cudaMemcpyDeviceToHost, ws.stream));
+    if (!io.out_on_device) {
+        size_t bytes = (size_t)B * top_k * 12 + (size_t)B * 4;
+        CKS(ws.hres.ensure(bytes));
+        char *h = ws.hres.as<char>();
+        CK(cudaMemcpyAsync(h, pass.d_ids, (size_t)B * top_k * 8, cudaMemcpyDeviceToHost, ws.stream));
+        CK(cudaMemcpyAsync(h + (size_t)B * top_k * 8, pass.d_sc, (size_t)B * top_k * 4, cudaMemcpyDeviceToHost, ws.stream));
+        CK(cudaMemcpyAsync(h + (size_t)B * top_k * 12, pass.d_cn, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
+    }
+    if (plan.prof) CK(cudaEventRecord(ws.ev[9], ws.stream));
+    CK(cudaStreamSynchronize(ws.stream));
+    if (pass.use_tc && *hc.fell) {  // the tensor-core pass gave up on the device: same sub-batch again on the exact path
+        *redo = true;
+        return PB_OK;
+    }
+    if (!io.out_on_device) {
+        char *h = ws.hres.as<char>();
+        memcpy(io.out_ids + (size_t)pass.b0 * top_k, h, (size_t)B * top_k * 8);
+        memcpy(io.out_scores + (size_t)pass.b0 * top_k, h + (size_t)B * top_k * 8, (size_t)B * top_k * 4);
+        memcpy(io.out_counts + pass.b0, h + (size_t)B * top_k * 12, (size_t)B * 4);
+    }
+    if (plan.prof) {
+        for (int s = 0; s < PB_STAGE_COUNT; ++s) {
+            float ms = 0.f;
+            CK(cudaEventElapsedTime(&ms, ws.ev[s], ws.ev[s + 1]));
+            g_stats.ms[s] += ms;
+        }
+        for (int k = 0; k < PB_KERNEL_COUNT; ++k)
+            if (g_stats.kernel_seen[k]) {
+                float ms = 0.f;
+                CK(cudaEventElapsedTime(&ms, ws.kev[2 * k], ws.kev[2 * k + 1]));
+                g_stats.kernel_ms[k] += ms;
+                g_stats.kernel_seen[k] = false;
+            }
+    }
+    pb_work_counters &w = g_stats.work;
+    if (pass.diag) {
+        unsigned long long got[2] = {0, 0};
+        CK(cudaMemcpy(got, ws.fdiag.p, 16, cudaMemcpyDeviceToHost));
+        w.filter_err_ratio_e6 = std::max<long long>(w.filter_err_ratio_e6, (long long)got[0]);
+        w.filter_diag_pairs += (long long)got[1];
+    }
+    if (pass.fast && ix->k1_diag && ws.k1diag.p) {
+        int got[2] = {0, 0};
+        CK(cudaMemcpy(got, ws.k1diag.p, 8, cudaMemcpyDeviceToHost));
+        w.k1_tc_max_code_diff = std::max<long long>(w.k1_tc_max_code_diff, got[0]);
+    }
+    w.n_queries += B;
+    w.n_query_tokens += pass.R;
+    if (pass.use_tc) w.n_k1_tc += 1;
+    else if (pass.d_probe_fallback) (*hc.fell ? w.n_probe_list : w.n_probe_threshold) += 1;
+    else if (pass.probe_list_only) w.n_probe_list += 1;
+    if (pass.fast)
+        for (int b = 0; b < B; ++b) w.n_recheck_docs += hc.recheck[b];
+    if (pass.pairs)
+        for (int b = 0; b < B; ++b) {
+            if (hc.need[b]) w.n_pair_fallback_queries += 1;
+            else w.n_exact_pairs += hc.pairs[b];
+        }
+    w.n_candidate_tokens += (long long)hc.cnt[0];
+    for (int b = 0; b < B; ++b) {
+        w.n_cells += hc.cells[b];
+        w.n_candidates += hc.cand[b];
+        if (pass.filt) {
+            w.n_filter_docs += hc.kept[b];
+            w.n_filter_tokens += (long long)hc.cnt[1 + b];
+            w.n_exact_docs += hc.surv[b];
+            w.n_exact_tokens += hc.surv_tok[b];
+        } else {
+            w.n_exact_docs += hc.kept[b];
+            w.n_exact_tokens += (long long)hc.cnt[1 + b];
+        }
+    }
+    return PB_OK;
+}
+
+// the per-stage contents of a pass into the caller's pb_trace (tests only; synchronous copies)
+static pb_status dump_trace(pb_index *ix, Workspace &ws, const SearchIO &io, const SearchPlan &plan, const Pass &pass) {
+    pb_trace *t = io.trace;
+    const HostCounts &hc = pass.hc;
+    for (int b = 0; b < pass.B; ++b) {
+        const int64_t gb = pass.b0 + b;
+        if (t->n_cells) t->n_cells[gb] = hc.cells[b];
+        if (t->n_candidates) t->n_candidates[gb] = hc.cand[b];
+        if (t->n_kept) t->n_kept[gb] = hc.kept[b];
+        if (t->cells) {
+            int n = (int)std::min<int64_t>(hc.cells[b], t->cells_cap);
+            std::vector<uint32_t> tmp(n);
+            CK(cudaMemcpy(tmp.data(), ws.cells.as<uint32_t>() + (size_t)b * pass.cells_cap, (size_t)n * 4,
+                          cudaMemcpyDeviceToHost));
+            for (int i = 0; i < n; ++i) t->cells[gb * t->cells_cap + i] = tmp[i];
+        }
+        if (t->candidates || t->approx) {
+            int n = (int)std::min<int64_t>(hc.cand[b], t->cand_cap);
+            std::vector<uint32_t> tmp(n);
+            CK(cudaMemcpy(tmp.data(), ws.cand.as<uint32_t>() + (size_t)b * ix->D, (size_t)n * 4, cudaMemcpyDeviceToHost));
+            if (t->candidates)
+                for (int i = 0; i < n; ++i) t->candidates[gb * t->cand_cap + i] = (int64_t)tmp[i] + ix->doc_id_base;
+            if (t->approx)
+                CK(cudaMemcpy(t->approx + gb * t->cand_cap, ws.approx.as<float>() + (size_t)b * ix->D, (size_t)n * 4,
+                              cudaMemcpyDeviceToHost));
+        }
+        if (t->kept || t->kept_exact) {
+            int n = (int)std::min<int64_t>(hc.kept[b], t->kept_cap);
+            std::vector<uint32_t> tmp(n);
+            CK(cudaMemcpy(tmp.data(), ws.kept.as<uint32_t>() + (size_t)b * plan.Mcap, (size_t)n * 4, cudaMemcpyDeviceToHost));
+            if (t->kept)
+                for (int i = 0; i < n; ++i) t->kept[gb * t->kept_cap + i] = (int64_t)tmp[i] + ix->doc_id_base;
+            if (t->kept_exact)
+                CK(cudaMemcpy(t->kept_exact + gb * t->kept_cap, ws.exact.as<float>() + (size_t)b * plan.Mcap, (size_t)n * 4,
+                              cudaMemcpyDeviceToHost));
+        }
+    }
+    return PB_OK;
+}
+
+// One pass of the pipeline over a sub-batch, stage by stage, with the stage events between them.  *redo: the
+// tensor-core pass gave up on the device and nothing of it went out.  `pass` is a copy, so a redo starts clean.
+static pb_status run_pass(pb_index *ix, Workspace &ws, const pb_search_params *p, const SearchIO &io,
+                          const SearchPlan &plan, Pass pass, bool *redo) {
+    *redo = false;
+    const auto mark = [&](int s) { return plan.prof ? cudaEventRecord(ws.ev[s], ws.stream) : cudaSuccess; };
+    CK(mark(0));
+    CKS(upload_queries(ix, ws, io, pass));
+    CK(mark(1));
+    CKS(centroid_scores(ix, ws, p, plan, pass));
+    CK(mark(2));
+    CKS(probe(ix, ws, p, plan, pass));
+    CK(mark(3));
+    CKS(candidates(ix, ws, plan, pass));
+    CK(mark(4));
+    CKS(approx_scores(ix, ws, plan, pass));
+    CK(mark(5));
+    CKS(cut(ix, ws, plan, pass));
+    CK(mark(6));
+    CKS(exact_scores(ix, ws, io, plan, pass));
+    CK(mark(7));
+    CKS(select_topk(ix, ws, io, plan, pass));
+    CK(mark(8));
+    CKS(finish(ix, ws, io, plan, pass, redo));  // D2H ends at ws.ev[9]
+    if (!*redo && io.trace) CKS(dump_trace(ix, ws, io, plan, pass));
+    return PB_OK;
+}
+
+// One search call (or one lane of it): the plan, the workspace, then the sub-batches in order
+static pb_status run_search(pb_index *ix, const pb_search_params *p, const SearchIO &io) {
+    SearchPlan plan;
+    CKS(plan_search(ix, p, io, plan));
+    if (plan.Bt == 0) return PB_OK;
 
     std::unique_ptr<Workspace> wsp;
     CKS(ix->acquire(wsp));
@@ -1463,633 +2182,42 @@ static pb_status search_impl_inner(pb_index *ix, const pb_search_params *p, cons
         }
     } rel{ix, wsp};
 
-    auto zero_counts = [&](int64_t b0, int64_t nb) -> pb_status {
-        if (io.out_on_device) CK(cudaMemsetAsync(io.out_counts + b0, 0, (size_t)nb * 4, ws.stream));
-        else memset(io.out_counts + b0, 0, (size_t)nb * 4);
-        return PB_OK;
-    };
-    if (empty_all) {
-        CKS(zero_counts(0, Bt));
+    if (!plan.empty) CKS(plan_probe(ix, ws, p, io, plan));
+    if (plan.empty) {
+        if (io.out_on_device) CK(cudaMemsetAsync(io.out_counts, 0, (size_t)plan.Bt * 4, ws.stream));
+        else memset(io.out_counts, 0, (size_t)plan.Bt * 4);
         CK(cudaStreamSynchronize(ws.stream));
         rel.ok = true;
         return PB_OK;
     }
 
-    // ---- subset preparation (shared by every query of the call) ----
-    const long long Wd = (ix->D + 31) / 32, Wk = (ix->K + 31) / 32;
-    const uint32_t *d_subset_bits = nullptr, *d_elig = nullptr;
-    int n_probe = (int)std::min<long long>(p->n_ivf_probe, ix->K);
-    bool all_eligible = false;
-    long long n_elig = 0;
-    if (io.has_subset) {
-        CKS(ws.subset_bits.ensure((size_t)Wd * 4));
-        CK(cudaMemsetAsync(ws.subset_bits.p, 0, (size_t)Wd * 4, ws.stream));
-        if (io.n_subset > 0) {
-            CKS(ws.subset.ensure((size_t)io.n_subset * 8));
-            CK(cudaMemcpyAsync(ws.subset.p, io.subset, (size_t)io.n_subset * 8, cudaMemcpyHostToDevice, ws.stream));
-            k_subset_bits<<<296, 256, 0, ws.stream>>>(ws.subset.as<long long>(), io.n_subset, ix->doc_id_base, ix->D,
-                                                     ws.subset_bits.as<uint32_t>());
-            CK(cudaGetLastError());
-        }
-        d_subset_bits = ws.subset_bits.as<uint32_t>();
-        if (!batched) {
-            // eligible centroids + n_ivf_probe scaling, dense variant only (search.rs:350-382)
-            CKS(ws.elig.ensure((size_t)Wk * 4));
-            CKS(ws.misc.ensure(64));
-            CK(cudaMemsetAsync(ws.elig.p, 0, (size_t)Wk * 4, ws.stream));
-            CK(cudaMemsetAsync(ws.misc.p, 0, 64, ws.stream));
-            k_eligible_bits<<<ix->sm_count * 8, 256, 0, ws.stream>>>(d_subset_bits, ix->D, ix->doc_off.as<long long>(),
-                                                                     ix->codes.as<uint32_t>(), ws.elig.as<uint32_t>());
-            k_popcount<<<ix->sm_count, 256, 0, ws.stream>>>(ws.elig.as<uint32_t>(), Wk, ws.misc.as<unsigned long long>());
-            CK(cudaGetLastError());
-            unsigned long long ne = 0;
-            CK(cudaMemcpyAsync(&ne, ws.misc.p, 8, cudaMemcpyDeviceToHost, ws.stream));
-            CK(cudaStreamSynchronize(ws.stream));
-            n_elig = (long long)ne;
-            if (n_elig == 0) {  // every per-token pool is empty -> no cells -> empty results
-                CKS(zero_counts(0, Bt));
-                CK(cudaStreamSynchronize(ws.stream));
-                rel.ok = true;
-                return PB_OK;
-            }
-            unsigned long long scaled = io.n_subset > 0 ? (unsigned long long)p->n_ivf_probe * (unsigned long long)ix->D /
-                                                              (unsigned long long)io.n_subset
-                                                        : (unsigned long long)p->n_ivf_probe;
-            scaled = std::max<unsigned long long>(scaled, (unsigned long long)p->n_ivf_probe);
-            scaled = std::min<unsigned long long>(scaled, (unsigned long long)n_elig);
-            d_elig = ws.elig.as<uint32_t>();
-            if ((long long)scaled >= n_elig) all_eligible = true;
-            else n_probe = (int)scaled;
-        }
-    }
-    // effective n_ivf_probe beyond 64: the dense variant switches to a row-wise radix select; the batched variant's
-    // heap-order threshold rule is tied to the streaming formulation, whose per-lane lists hold up to 192 entries
-    const int stream_max = batched ? 192 : 64;
-    const bool big_probe = !all_eligible && n_probe > stream_max;
-    if (big_probe && batched)
-        return pb_fail(PB_ERR_UNSUPPORTED, "n_ivf_probe %d > 192 with the batched variant is not built", n_probe);
-
-    // ---- sub-batching: bound the transposed score matrix ----
-    int nq_max_all = 0;
-    for (int64_t b = 0; b < Bt; ++b) nq_max_all = std::max<int>(nq_max_all, (int)(io.q_off[b + 1] - io.q_off[b]));
-    const int QS_all = query_row_tokens(nq_max_all);
-    if (!all_eligible && !big_probe && (long long)QS_all * n_probe > 8192)
-        return pb_fail(PB_ERR_UNSUPPORTED, "query tokens x n_ivf_probe = %lld exceeds 8192", (long long)QS_all * n_probe);
-    size_t per_q = (size_t)ix->K * QS_all * sizeof(float);
-    if (per_q >= ((size_t)1 << 32))
-        return pb_fail(PB_ERR_UNSUPPORTED, "num_centroids x query tokens x 4 = %zu bytes per query exceeds 2^32", per_q);
-    // sub-batch size: the score tables (16-bit always, fp32 only on the exact path) and the per-(query, doc) scratch
-    // (candidate lists, code sums, approximate scores, cut keys, bitmap: 24.2 bytes per document) share one budget
-    const size_t per_q_all = (size_t)ix->K * QS_all * (k1_tc_usable(ix) ? 2 : 6) + (size_t)ix->D * 24 + (size_t)ix->D / 8 + 4096;
-    int QB = (int)std::max<size_t>(1, std::min<size_t>((size_t)Bt, ix->st_budget / std::max(g_budget_div, 1) / per_q_all));
-    QB = std::min(QB, 256);
-    QB = (int)((Bt + (Bt + QB - 1) / QB - 1) / ((Bt + QB - 1) / QB));  // equal sub-batches
-
-    const bool prof = ix->profiling;
-    if (prof) CK(cudaEventRecord(ws.call_ev[0], ws.stream));
-    for (int64_t b0 = 0; b0 < Bt; b0 += QB) {
-        const int B = (int)std::min<int64_t>(QB, Bt - b0);
-        const int64_t r0 = io.q_off[b0];
-        const int64_t R = io.q_off[b0 + B] - r0;
-        int nq_max = 0;
-        std::vector<int> qoff(B + 1);
-        for (int b = 0; b <= B; ++b) qoff[b] = (int)(io.q_off[b0 + b] - r0);
-        for (int b = 0; b < B; ++b) nq_max = std::max(nq_max, qoff[b + 1] - qoff[b]);
-        const int QS = query_row_tokens(nq_max);
-        int *L = g_stats.launches;
-        const bool fast = ix->fast_approx && !io.trace;  // trace wants every candidate's exact approx score
+    if (plan.prof) CK(cudaEventRecord(ws.call_ev[0], ws.stream));
+    for (int64_t b0 = 0; b0 < plan.Bt; b0 += plan.QB) {
+        Pass pass;
+        pass.b0 = b0;
+        pass.B = (int)std::min<int64_t>(plan.QB, plan.Bt - b0);
+        pass.r0 = io.q_off[b0];
+        pass.R = io.q_off[b0 + pass.B] - pass.r0;
+        for (int b = 0; b < pass.B; ++b)
+            pass.nq_max = std::max(pass.nq_max, (int)(io.q_off[b0 + b + 1] - io.q_off[b0 + b]));
+        pass.QS = query_row_tokens(pass.nq_max);
+        pass.fast = ix->fast_approx && !io.trace;  // trace wants every candidate's exact approx score
         // the score table comes from the tensor cores unless something needs the dense fp32 S (an eligibility filter,
         // the radix-select probe, a trace) or the shape is outside the kernel's (DESIGN.md "a2")
         int n_chunks_k = 0;
-        probe_chunk_rows(ix->K, n_probe, &n_chunks_k);
-        const bool want_tc = k1_tc_usable(ix) && fast && ix->probe16 && !ix->k1_diag && !all_eligible && !big_probe && !d_elig &&
-                             QS / 8 <= 32 && n_chunks_k >= n_probe && n_probe <= 192;
-        // One pass over the sub-batch.  use_tc: a flagged query or a probe-list overflow raises a device flag instead of
-        // being read back mid-way; the pass then finishes on (memory-safe) garbage and *redo asks for the exact pass.
-        auto run_sub = [&](const bool use_tc, bool *redo) -> pb_status {
-        *redo = false;
-        if (prof) CK(cudaEventRecord(ws.ev[0], ws.stream));
-        // ---- H2D ----
-        CKS(ws.Q.ensure(std::max<size_t>((size_t)R * ix->dim * 4, 16)));
-        CKS(ws.qoff.ensure((size_t)(B + 1) * 4));
-        if (R > 0) {
-            if (io.queries_on_device)
-                CK(cudaMemcpyAsync(ws.Q.p, io.queries + (size_t)r0 * ix->dim, (size_t)R * ix->dim * 4,
-                                   cudaMemcpyDeviceToDevice, ws.stream));
-            else {
-                CKS(ws.hq.ensure((size_t)R * ix->dim * 4));
-                memcpy(ws.hq.p, io.queries + (size_t)r0 * ix->dim, (size_t)R * ix->dim * 4);
-                CK(cudaMemcpyAsync(ws.Q.p, ws.hq.p, (size_t)R * ix->dim * 4, cudaMemcpyHostToDevice, ws.stream));
-            }
-        }
-        CKS(ws.hcounts.ensure((size_t)(B + 1) * 4 + 16 + (size_t)(B + 2) * 8 + (size_t)B * 8 + (size_t)B * 7 * 4 + 192));
-        memcpy(ws.hcounts.p, qoff.data(), (size_t)(B + 1) * 4);
-        CK(cudaMemcpyAsync(ws.qoff.p, ws.hcounts.p, (size_t)(B + 1) * 4, cudaMemcpyHostToDevice, ws.stream));
-        if (prof) CK(cudaEventRecord(ws.ev[1], ws.stream));
-
-        // ---- a2 centroid scores ----
-        if (!use_tc) CKS(ws.ST.ensure((size_t)B * ix->K * QS * sizeof(float)));
-        if (fast) {
-            CKS(ws.ST16.ensure((size_t)B * ix->K * QS * 2));
-            CKS(ws.qrange.ensure((size_t)B * 8 + 16));
-            CKS(ws.qflag.ensure((size_t)B * 4 + 16));
-            CKS(ws.qexp.ensure((size_t)B * 4 + 16));
-            CKS(ws.qnmax.ensure((size_t)B * 4 + 16));
-            k_query_range<<<B, 256, 0, ws.stream>>>(ws.Q.as<float>(), ws.qoff.as<int>(), ix->dim, ix->cmax,
-                                                    ws.qrange.as<float2>(), ws.qflag.as<int>(), ws.qexp.as<int>(),
-                                                    ws.qnmax.as<float>());
-            CK(cudaGetLastError());
-            L[PB_STAGE_CENTROID_SCORES] += 1;
-        }
-        const bool tc = use_tc;
-        int cells_cap = 0;
-        const int *d_probe_fallback = nullptr;  // device flag of the threshold-first probe (0 = it did the work)
-        bool probe_list_only = false;
-        if (tc) CKS(run_k1_tc(ix, ws, p, B, QS, nq_max, n_probe, batched, L, &cells_cap, &d_probe_fallback));
-        else CKS(launch_centroid_scores(ix, ws, B, QS, &L[PB_STAGE_CENTROID_SCORES], fast));
-        if (prof) CK(cudaEventRecord(ws.ev[2], ws.stream));
-
-        // ---- a3 probe ----
-        if (tc) {
-            // cells are in place (run_k1_tc)
-        } else if (all_eligible) {
-            cells_cap = (int)n_elig;
-            CKS(ws.list.ensure((size_t)n_elig * 4 + 16));
-            CKS(ws.cells.ensure((size_t)B * cells_cap * 4));
-            CKS(ws.ncells.ensure((size_t)B * 4 + 16));
-            int *d_listn = reinterpret_cast<int *>(ws.misc.as<char>() + 16);
-            k_cells_from_bits<<<1, 1024, 0, ws.stream>>>(d_elig, ix->K, ws.list.as<uint32_t>(), d_listn);
-            k_cells_filter_list<<<B, 256, 0, ws.stream>>>(ws.list.as<uint32_t>(), d_listn, ws.ST.as<float>(),
-                                                          ws.qoff.as<int>(), ix->K, QS, p->has_centroid_score_threshold,
-                                                          p->centroid_score_threshold, cells_cap, ws.cells.as<uint32_t>(),
-                                                          ws.ncells.as<int>());
-            CK(cudaGetLastError());
-            L[PB_STAGE_PROBE] += 2;
-        } else if (big_probe) {
-            cells_cap = (int)std::min<long long>((long long)QS * n_probe, ix->K);
-            CKS(ws.cellbits.ensure((size_t)B * Wk * 4));
-            CKS(ws.cells.ensure((size_t)B * cells_cap * 4));
-            CKS(ws.ncells.ensure((size_t)B * 4 + 16));
-            k_topn_select_row<<<dim3(QS, B), 256, 0, ws.stream>>>(ws.ST.as<float>(), ws.qoff.as<int>(), ix->K, QS, n_probe,
-                                                                  d_elig, ws.cellbits.as<uint32_t>(), Wk);
-            k_cells_from_query_bits<<<B, 1024, 0, ws.stream>>>(ws.cellbits.as<uint32_t>(), Wk, ws.ST.as<float>(),
-                                                               ws.qoff.as<int>(), ix->K, QS, p->has_centroid_score_threshold,
-                                                               p->centroid_score_threshold, cells_cap, ws.cells.as<uint32_t>(),
-                                                               ws.ncells.as<int>());
-            CK(cudaGetLastError());
-            L[PB_STAGE_PROBE] += 2;
-        } else {
-            const int n = n_probe;
-            const int n_chunks = (int)((ix->K + 1023) / 1024);
-            cells_cap = (int)std::min<long long>((long long)QS * n, ix->K);
-            CKS(ws.partial.ensure((size_t)B * QS * n_chunks * n * 8));
-            CKS(ws.sel.ensure((size_t)B * QS * n * 8));
-            CKS(ws.cells.ensure((size_t)B * cells_cap * 4));
-            CKS(ws.ncells.ensure((size_t)B * 4 + 16));
-            size_t sm1 = (size_t)4 * n * 32 * 8;
-            CKS(set_smem(k_topn_partial, sm1));
-            // threshold-first selection on the 16-bit table when there is one (k_chunkmax16 / k_collect16);
-            // the per-lane list scan of k_topn_partial otherwise, or when the device raises `fallback`
-            const int GQ = QS / 8;
-            int t_chunks = 0;
-            const int t_rows = probe_chunk_rows(ix->K, n, &t_chunks);
-            const bool thr_path = fast && !d_elig && ix->probe16 && GQ <= 32 && t_chunks >= n && n <= 192;
-            int *d_fallback = nullptr;
-            probe_list_only = !thr_path;
-            if (thr_path) {
-                const int cap = n * std::max(2, 128 / n);
-                CKS(ws.cmax16.ensure((size_t)B * t_chunks * QS * 2));
-                CKS(ws.tau16.ensure((size_t)B * QS * 4));
-                CKS(ws.plist.ensure((size_t)B * QS * cap * 8));
-                CKS(ws.pcount.ensure((size_t)B * QS * 4 + 16));
-                CK(cudaMemsetAsync(ws.plist.p, 0, (size_t)B * QS * cap * 8, ws.stream));
-                CK(cudaMemsetAsync(ws.pcount.p, 0, (size_t)B * QS * 4 + 16, ws.stream));
-                d_fallback = ws.pcount.as<int>() + (size_t)B * QS;
-                d_probe_fallback = d_fallback;
-                k_chunkmax16<<<dim3((t_chunks + 3) / 4, B), 128, 0, ws.stream>>>(ws.ST16.as<unsigned short>(), ix->K, QS, t_chunks,
-                                                                                 t_rows, ws.cmax16.as<unsigned short>());
-                k_tau16<<<dim3(QS, B), 32, 0, ws.stream>>>(ws.cmax16.as<unsigned short>(), ws.qoff.as<int>(), QS, n, t_chunks,
-                                                          ws.qflag.as<int>(), ws.tau16.as<uint32_t>(), d_fallback);
-                k_collect16<<<dim3((t_chunks + 3) / 4, B), 128, 0, ws.stream>>>(
-                    ws.ST16.as<unsigned short>(), ws.ST.as<float>(), ix->K, QS, t_chunks, t_rows, ws.tau16.as<uint32_t>(), cap,
-                    ws.pcount.as<int>(), ws.plist.as<u64>(), d_fallback);
-                k_topn_merge<<<dim3(QS, B), 32, 0, ws.stream>>>(ws.plist.as<u64>(), ws.qoff.as<int>(), QS, n, cap / n,
-                                                              ws.sel.as<u64>(), d_fallback, 0);
-                CK(cudaGetLastError());
-                L[PB_STAGE_PROBE] += 4;
-            }
-            k_topn_partial<<<dim3((n_chunks + 3) / 4, B, (QS + 31) / 32), 128, sm1, ws.stream>>>(
-                ws.ST.as<float>(), ws.qoff.as<int>(), ix->K, QS, n, d_elig, ws.partial.as<u64>(), n_chunks, d_fallback, 1);
-            k_topn_merge<<<dim3(QS, B), 32, 0, ws.stream>>>(ws.partial.as<u64>(), ws.qoff.as<int>(), QS, n, n_chunks,
-                                                          ws.sel.as<u64>(), d_fallback, 1);
-            int P = 1;
-            while (P < std::max(nq_max * n, 1)) P <<= 1;
-            size_t sm2 = (size_t)P * 12;
-            CKS(set_smem(k_cells, sm2));
-            k_cells<<<B, 256, sm2, ws.stream>>>(ws.sel.as<u64>(), ws.ST.as<float>(), ws.qoff.as<int>(), ix->K, QS, n,
-                                                cells_cap, p->has_centroid_score_threshold, p->centroid_score_threshold,
-                                                batched ? 1 : 0, batched ? (long long)p->centroid_batch_size : ix->K,
-                                                ws.cells.as<uint32_t>(), ws.ncells.as<int>(),
-                                                thr_path ? ws.cmax16.as<unsigned short>() : nullptr, t_chunks, t_rows,
-                                                ws.qrange.as<float2>(), d_fallback);
-            CK(cudaGetLastError());
-            L[PB_STAGE_PROBE] += 3;
-        }
-        if (prof) CK(cudaEventRecord(ws.ev[3], ws.stream));
-
-        // ---- a4 candidates ----
-        CKS(ws.bitmap.ensure((size_t)B * Wd * 4));
-        CKS(ws.cand.ensure((size_t)B * ix->D * 4));
-        CKS(ws.ncand.ensure((size_t)B * 4 + 16));
-        k_mark<<<dim3(cells_cap, B), 128, 0, ws.stream>>>(ws.cells.as<uint32_t>(), ws.ncells.as<int>(), cells_cap,
-                                                         ix->ivf.as<uint32_t>(), ix->ivf_off.as<long long>(), d_subset_bits,
-                                                         ws.bitmap.as<uint32_t>(), Wd);
-        const int slices = (int)std::max<long long>(1, std::min<long long>(32, (4ll * ix->sm_count + B - 1) / B));
-        CKS(ws.slicecnt.ensure((size_t)B * slices * 4));
-        k_compact_count<<<dim3(slices, B), 256, 0, ws.stream>>>(ws.bitmap.as<uint32_t>(), Wd, ws.slicecnt.as<int>());
-        k_compact_emit<<<dim3(slices, B), 256, 0, ws.stream>>>(ws.bitmap.as<uint32_t>(), Wd, ws.slicecnt.as<int>(),
-                                                               ws.cand.as<uint32_t>(), ix->D, ws.ncand.as<int>());
-        CK(cudaGetLastError());
-        L[PB_STAGE_CANDIDATES] += 3;
-        if (prof) CK(cudaEventRecord(ws.ev[4], ws.stream));
-
-        // ---- a5 approximate scores ----
-        CKS(ws.counters.ensure((size_t)(B + 2) * 8));  // [0] candidate codes gathered, [1+b] kept-doc tokens, [B+1] re-check gathers
-        CK(cudaMemsetAsync(ws.counters.p, 0, (size_t)(B + 2) * 8, ws.stream));
-        CKS(ws.approx.ensure((size_t)B * ix->D * 4));
-        CKS(ws.keys.ensure((size_t)B * ix->D * 8));
-        const uint32_t *cand_list = ws.cand.as<uint32_t>();
-        const int *cand_n = ws.ncand.as<int>();
-        if (fast) {
-            CKS(ws.lsum.ensure((size_t)B * ix->D * 4));
-            CKS(ws.cand2.ensure((size_t)B * ix->D * 4));
-            CKS(ws.ncand2.ensure((size_t)B * 4 + 16));
-            const dim3 ga(ix->sm_count * ix->approx_grid, B);
-            const unsigned short *st16 = ws.ST16.as<unsigned short>();
-            const uint32_t *list = ws.cand.as<uint32_t>();
-            const int *list_n = ws.ncand.as<int>();
-            unsigned long long *cnt = ws.counters.as<unsigned long long>();
-            KEV_BEGIN(PB_KERNEL_APPROX16);
-            (QS <= 32 ? k_approx16<4> : k_approx16<8>)<<<ga, 256, 0, ws.stream>>>(
-                st16, ws.qoff.as<int>(), ix->K, QS, ix->ucodes.as<uint32_t>(), ix->udoc_off.as<long long>(), list, ix->D, list_n,
-                ws.lsum.as<uint32_t>(), cnt);
-            KEV_END(PB_KERNEL_APPROX16);
-            // band per query token in code units (W = band * nq + 8).  Exact table: +-1 code of rounding per token and side
-            // plus the fp32 summation error -> 4.  Estimate table (k_scores_tc.cuh): W = nq (1.004 + 2 err) + nq^2/256 + 4
-            // <= nq (ceil(1.004 + 2 err) + 1) + 8 for nq <= 256.
-            const int band_per_q = tc ? (int)ceilf(1.004f + 2.0f * std::max(k1_err_codes(ix->dim), (float)(ix->k1_margin - 1))) + 1 : 4;
-            k_select_u32<<<B, 1024, 0, ws.stream>>>(ws.lsum.as<uint32_t>(), list_n, M, band_per_q, ws.lsum.as<uint32_t>(), list,
-                                                    list_n, ix->D, ws.qoff.as<int>(), ws.qflag.as<int>(),
-                                                    ws.cand2.as<uint32_t>(), ws.ncand2.as<int>());
-            CK(cudaGetLastError());
-            L[PB_STAGE_APPROX] += 2;
-            cand_list = ws.cand2.as<uint32_t>();
-            cand_n = ws.ncand2.as<int>();
-        }
-        if (tc) {  // the exact approximate score of the docs around the cut from pinned-order dots (no dense fp32 S)
-            const int rc_cap = 2 * Mcap + 1024, pair_cap = 64 * rc_cap;
-            CKS(ws.rcmax.ensure((size_t)B * rc_cap * QS * 4));
-            CKS(ws.rcpairs.ensure((size_t)B * pair_cap * 8));
-            CKS(ws.rcn.ensure((size_t)B * 4 + 16));
-            CK(cudaMemsetAsync(ws.rcn.p, 0, (size_t)B * 4, ws.stream));
-            int *d_fb = const_cast<int *>(d_probe_fallback);
-            (QS <= 32 ? k_recheck_pairs<4> : k_recheck_pairs<8>)<<<dim3(ix->sm_count * 2, B), 256, 0, ws.stream>>>(
-                ws.ST16.as<unsigned short>(), ws.qoff.as<int>(), ix->K, QS, ix->ucodes.as<uint32_t>(), ix->udoc_off.as<long long>(),
-                cand_list, ix->D, cand_n, 2 * ix->k1_margin + 1, rc_cap, pair_cap, ws.rcpairs.as<u64>(), ws.rcn.as<int>(), d_fb,
-                ws.counters.as<unsigned long long>() + B + 1);
-            k_recheck_dots<<<dim3(ix->sm_count * 2, B), 128, 0, ws.stream>>>(ws.rcpairs.as<u64>(), ws.rcn.as<int>(), pair_cap,
-                                                                             ws.Q.as<float>(), ws.qoff.as<int>(),
-                                                                             ix->centroids.as<float>(), ix->dim, rc_cap, QS,
-                                                                             ws.rcmax.as<uint32_t>());
-            k_recheck_sum<<<dim3(ix->sm_count, B), 256, 0, ws.stream>>>(ws.rcmax.as<uint32_t>(), ws.qoff.as<int>(), QS, cand_list,
-                                                                        ix->D, cand_n, rc_cap, ws.approx.as<float>(),
-                                                                        ws.keys.as<u64>(), (uint32_t)ix->doc_id_base);
-            L[PB_STAGE_APPROX] += 2;
-        }
-        else
-            k_approx<<<dim3(ix->sm_count * 8, B), 256, 0, ws.stream>>>(
-                ws.ST.as<float>(), ws.qoff.as<int>(), ix->K, QS, ix->ucodes.as<uint32_t>(), ix->udoc_off.as<long long>(),
-                cand_list, ix->D, cand_n, ws.approx.as<float>(), ws.keys.as<u64>(),
-                fast ? ws.counters.as<unsigned long long>() + B + 1 : ws.counters.as<unsigned long long>(),
-                (uint32_t)ix->doc_id_base);
-        CK(cudaGetLastError());
-        L[PB_STAGE_APPROX] += 1;
-        if (prof) CK(cudaEventRecord(ws.ev[5], ws.stream));
-
-        // ---- a6 cut ----
-        CKS(ws.kept.ensure((size_t)B * Mcap * 4));
-        CKS(ws.nkept.ensure((size_t)B * 4 + 16));
-        CKS(ws.tokp.ensure((size_t)B * (Mcap + 1) * 8));
-        if (sharded) CKS(ws.lkeys.ensure((size_t)B * Mcap * 8));
-        int Pm = 1;
-        while (Pm < Mcap) Pm <<= 1;
-        CKS(set_smem(k_cut, (size_t)Pm * 8));
-        k_cut<<<B, 1024, (size_t)Pm * 8, ws.stream>>>(ws.keys.as<u64>(), ws.approx.as<float>(), ix->D, cand_n, M,
-                                                      Mcap, ix->doc_off.as<long long>(), ws.kept.as<uint32_t>(),
-                                                      ws.nkept.as<int>(), ws.tokp.as<long long>(),
-                                                      ws.counters.as<long long>() + 1, (uint32_t)ix->doc_id_base,
-                                                      sharded ? ws.lkeys.as<u64>() : nullptr);
-        CK(cudaGetLastError());
-        L[PB_STAGE_CUT] += 1;
-        if (sharded) {
-            // exchange 1: every shard's sorted top-M cut keys -> global cut -> my members (SURVEY 8e)
-            const int G = ix->world;
-            CKS(ws.gkeys.ensure((size_t)G * B * M * 8));
-            CKS(ws.krank.ensure((size_t)B * Mcap * 4));
-            CKS(shard_allgather(ix, ws.stream, ws.lkeys.p, ws.gkeys.p, (size_t)B * M));
-            k_merge_cut<<<B, 1024, 0, ws.stream>>>(ws.gkeys.as<u64>(), G, ix->rank, B, M, (uint32_t)ix->doc_id_base, ix->D,
-                                                   ix->doc_off.as<long long>(), ws.kept.as<uint32_t>(),
-                                                   ws.krank.as<uint32_t>(), ws.nkept.as<int>(),
-                                                   ws.tokp.as<long long>(), ws.counters.as<long long>() + 1);
-            CK(cudaGetLastError());
-            L[PB_STAGE_CUT] += 2;
-        }
-        if (prof) CK(cudaEventRecord(ws.ev[6], ws.stream));
-
-        // ---- a7+a8 exact ----
-        CKS(ws.maxkey.ensure((size_t)B * Mcap * QS * 4));
-        CKS(ws.exact.ensure((size_t)B * Mcap * 4));
-        CKS(ws.fkeys.ensure((size_t)B * Mcap * 8));
-        KeptView kv{ws.kept.as<uint32_t>(), ws.nkept.as<int>(), ws.tokp.as<long long>(),
-                    sharded ? ws.krank.as<uint32_t>() : nullptr};
-        // only the top_k need exact scores: the tensor-core filter drops the docs that provably cannot reach them
-        // the linear form needs the 16-bit score table of this pass (a flagged query publishes no estimate and keeps
-        // every doc); without a table (PB_FAST_APPROX=0) the decompressing form estimates from fp16 centroids
-        const bool linear = fast && !ix->filter_v1 && ix->tok_inv_norm.p;
-        const float eps_unit = linear ? filter_eps_unit2(ix, tc ? ix->k1_margin : 0) : filter_eps_unit(ix);
-        const bool filt = ix->fast_exact && !io.trace && ix->centroids_f16.p && eps_unit > 0.0f && nq_max <= 64 &&
-                          top_k < Mcap && ix->packed % 4 == 0;
-        // PB_FILTER_DIAG: the filter runs as usual, then every kept doc is scored exactly (the results of
-        // pb_set_fast_exact(0)) and k_filter_diag compares the pass-1 estimate maxima with the exact ones
-        const bool diag = filt && ix->filter_diag;
-        bool pairs = false;
-        if (filt) {
-            CKS(ws.est.ensure((size_t)B * Mcap * 4));
-            CKS(ws.kept2.ensure((size_t)B * Mcap * 4));
-            CKS(ws.krank2.ensure((size_t)B * Mcap * 4));
-            CKS(ws.nkept2.ensure((size_t)B * 4 + 16));
-            CKS(ws.tokp2.ensure((size_t)B * (Mcap + 1) * 8));
-            CKS(ws.ktok2.ensure((size_t)B * 8 + 16));
-            if (!fast) {  // the two-pass mode computed them with the score range
-                CKS(ws.qnmax.ensure((size_t)B * 4 + 16));
-                CKS(ws.qexp.ensure((size_t)B * 4 + 16));
-                k_query_range<<<B, 256, 0, ws.stream>>>(ws.Q.as<float>(), ws.qoff.as<int>(), ix->dim, ix->cmax, nullptr, nullptr,
-                                                        ws.qexp.as<int>(), ws.qnmax.as<float>());
-                CK(cudaGetLastError());
-                L[PB_STAGE_EXACT] += 1;
-            }
-            KeptView kv2{ws.kept2.as<uint32_t>(), ws.nkept2.as<int>(), ws.tokp2.as<long long>(), ws.krank2.as<uint32_t>()};
-            // pair form of the exact stage: pass 2 of the estimate over the survivors lists the (token, q) pairs that can
-            // hold a per-token maximum, k_pair_exact evaluates them in the pinned order; a query whose list overflows
-            // (or that published no estimate) goes through k_exact
-            pairs = !diag && linear && ix->pair_exact && Mcap <= 65535 && QS <= 256;
-            if (pairs || diag) {
-                CKS(ws.estkey.ensure((size_t)B * Mcap * QS * 4));
-                CKS(ws.srcrank.ensure((size_t)B * Mcap * 4));
-            }
-            CKS(launch_filter(ix, ws, kv, kv2, B, QS, Mcap, top_k, (long long)Mcap * std::max(ix->max_doclen, 1), eps_unit,
-                              nq_max, linear, pairs || diag, &L[PB_STAGE_EXACT]));
-            if (!diag) {
-                kv = kv2;
-                if (!sharded) kv.krank = nullptr;  // survivors keep their order, so position breaks ties the same way
-            }
-        }
-        if (pairs) {
-            const int pair_cap = 16 * Mcap + 4096;  // ~ (top_k + ties) * nq * (1 + a few) pairs per query in practice
-            CKS(ws.xpairs.ensure((size_t)B * pair_cap * 8));
-            CKS(ws.xnpairs.ensure((size_t)B * 4 + 16));
-            CKS(ws.needexact.ensure((size_t)B * 4 + 16));
-            CK(cudaMemsetAsync(ws.xnpairs.p, 0, (size_t)B * 4, ws.stream));
-            KEV_BEGIN(PB_KERNEL_EXACT);  // pass 2 + pair evaluation + the (normally empty) k_exact of flagged queries
-            CKS(launch_maxsim_tc(ix, ws, kv, B, QS, Mcap, (long long)Mcap * std::max(ix->max_doclen, 1), nq_max,
-                                 ws.estkey.as<uint32_t>(), ws.srcrank.as<uint32_t>(), eps_unit, ws.xpairs.as<u64>(),
-                                 ws.xnpairs.as<int>(), pair_cap, -1));
-            k_pair_overflow<<<(B + 255) / 256, 256, 0, ws.stream>>>(ws.xnpairs.as<int>(), pair_cap, ws.qflag.as<int>(), B,
-                                                                    ws.needexact.as<int>());
-            CK(cudaGetLastError());
-            const size_t smp = ((size_t)(nq_max + 256) * (ix->dim + 1) + 256) * 4;
-            const int pe_ctas = std::max(1, std::min(16, (2 * ix->sm_count + B - 1) / B));  // about one wave over the batch
-            switch (ix->dim) {
-#define PB_PE(DV)                                                                                                      \
-    case DV: {                                                                                                         \
-        CKS(set_smem(k_pair_exact<DV>, smp));                                                                          \
-        k_pair_exact<DV><<<dim3(pe_ctas, B), 256, smp, ws.stream>>>(                                                   \
-            ws.xpairs.as<u64>(), ws.xnpairs.as<int>(), pair_cap, ws.Q.as<float>(), ws.qoff.as<int>(), QS,              \
-            ix->centroids.as<float>(), ix->w_rev.as<float>(), ix->nbits, ix->codes.as<uint32_t>(),                     \
-            ix->residuals.as<uint8_t>(), Mcap, ws.maxkey.as<uint32_t>());                                              \
-    } break;
-                PB_PE(64) PB_PE(96) PB_PE(128)
-#undef PB_PE
-                default: return pb_fail(PB_ERR_UNSUPPORTED, "pair exact: unsupported dim");
-            }
-            CK(cudaGetLastError());
-            L[PB_STAGE_EXACT] += 5;
-            CKS(launch_exact(ix, ws, kv, B, QS, Mcap, 0, (long long)Mcap * std::max(ix->max_doclen, 1), &L[PB_STAGE_EXACT],
-                             ws.needexact.as<int>(), false));
-            KEV_END(PB_KERNEL_EXACT);
-        } else {
-            CKS(launch_exact(ix, ws, kv, B, QS, Mcap, 0, (long long)Mcap * std::max(ix->max_doclen, 1), &L[PB_STAGE_EXACT]));
-        }
-        if (diag) {  // before k_exact_finalize, which clears the exact maxima
-            CKS(ws.fdiag.ensure(16));
-            CK(cudaMemsetAsync(ws.fdiag.p, 0, 16, ws.stream));
-            k_filter_diag<<<dim3(4, B), 256, 0, ws.stream>>>(ws.estkey.as<uint32_t>(), ws.maxkey.as<uint32_t>(), ws.qoff.as<int>(),
-                                                             QS, kv.nkept, Mcap, ws.qnmax.as<float>(),
-                                                             linear ? ws.qflag.as<int>() : nullptr, eps_unit,
-                                                             ws.fdiag.as<unsigned long long>());
-            CK(cudaGetLastError());
-            L[PB_STAGE_EXACT] += 1;
-        }
-        if (sharded) {
-            CKS(ws.payload.ensure((size_t)B * Mcap * 8));
-            CK(cudaMemsetAsync(ws.fkeys.p, 0xff, (size_t)B * Mcap * 8, ws.stream));  // ~0 = no entry
-        }
-        k_exact_finalize<<<dim3((Mcap + 7) / 8, B), 256, 0, ws.stream>>>(
-            ws.maxkey.as<uint32_t>(), ws.qoff.as<int>(), QS, kv.nkept, Mcap, 0, ws.exact.as<float>(),
-            ws.fkeys.as<u64>(), kv.krank, kv.kept, (uint32_t)ix->doc_id_base, sharded ? ws.payload.as<u64>() : nullptr);
-        CK(cudaGetLastError());
-        L[PB_STAGE_EXACT] += 1;
-        if (prof) CK(cudaEventRecord(ws.ev[7], ws.stream));
-
-        // ---- a9 top-k ----
-        long long *d_ids;
-        float *d_sc;
-        int *d_cn;
-        if (io.out_on_device) {
-            d_ids = reinterpret_cast<long long *>(io.out_ids) + (size_t)b0 * top_k;
-            d_sc = io.out_scores + (size_t)b0 * top_k;
-            d_cn = io.out_counts + b0;
-        } else {
-            CKS(ws.oids.ensure((size_t)B * top_k * 8));
-            CKS(ws.oscores.ensure((size_t)B * top_k * 4));
-            CKS(ws.ocounts.ensure((size_t)B * 4 + 16));
-            d_ids = ws.oids.as<long long>();
-            d_sc = ws.oscores.as<float>();
-            d_cn = ws.ocounts.as<int>();
-        }
-        if (sharded) {
-            // exchange 2: (exact key | global approx rank) + (doc id | score) of every shard, merged on every rank
-            const int G = ix->world;
-            CKS(ws.gfkeys.ensure((size_t)G * B * M * 8));
-            CKS(ws.gpayload.ensure((size_t)G * B * M * 8));
-            CKS(shard_allgather(ix, ws.stream, ws.fkeys.p, ws.gfkeys.p, (size_t)B * M));
-            CKS(shard_allgather(ix, ws.stream, ws.payload.p, ws.gpayload.p, (size_t)B * M));
-            CKS(ws.mslot.ensure((size_t)B * Mcap * 4));
-            CKS(set_smem(k_merge_topk, (size_t)Pm * 8));
-            k_merge_topk<<<B, 1024, (size_t)Pm * 8, ws.stream>>>(ws.gfkeys.as<u64>(), ws.gpayload.as<u64>(), G, B, M, top_k,
-                                                                ws.mslot.as<uint32_t>(), d_ids, d_sc, d_cn);
-            CK(cudaGetLastError());
-            L[PB_STAGE_TOPK] += 3;
-        } else {
-            CKS(set_smem(k_topk, (size_t)Pm * 8));
-            k_topk<<<B, 1024, (size_t)Pm * 8, ws.stream>>>(ws.fkeys.as<u64>(), ws.exact.as<float>(), kv.kept, kv.nkept, Mcap,
-                                                           top_k, ix->doc_id_base, d_ids, d_sc, d_cn);
-            CK(cudaGetLastError());
-            L[PB_STAGE_TOPK] += 1;
-        }
-        if (prof) CK(cudaEventRecord(ws.ev[8], ws.stream));
-
-        // ---- D2H ----
-        // pinned layout after the (B + 1) query offsets: u64 counters[B + 2] | i64 survivor tokens[B] |
-        // int n_cells[B], n_cand[B], n_kept[B], survivors[B], re-checked[B], probe fallback flag
-        char *hbase = ws.hcounts.as<char>() + (((size_t)(B + 1) * 4 + 15) & ~(size_t)15);
-        unsigned long long *hcnt = reinterpret_cast<unsigned long long *>(hbase);
-        long long *hsurv_tok = reinterpret_cast<long long *>(hcnt + (B + 2));
-        int *hc = reinterpret_cast<int *>(hsurv_tok + B);
-        int *hsurv = hc + 3 * B, *hrecheck = hc + 4 * B, *hfell = hc + 5 * B, *hpairs = hc + 5 * B + 16, *hneed = hc + 6 * B + 16;
-        *hfell = 0;
-        CK(cudaMemcpyAsync(hc, ws.ncells.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
-        CK(cudaMemcpyAsync(hc + B, ws.ncand.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
-        CK(cudaMemcpyAsync(hc + 2 * B, ws.nkept.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
-        CK(cudaMemcpyAsync(hcnt, ws.counters.p, (size_t)(B + 2) * 8, cudaMemcpyDeviceToHost, ws.stream));
-        if (filt) {
-            CK(cudaMemcpyAsync(hsurv_tok, ws.ktok2.p, (size_t)B * 8, cudaMemcpyDeviceToHost, ws.stream));
-            CK(cudaMemcpyAsync(hsurv, ws.nkept2.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
-        }
-        if (fast) CK(cudaMemcpyAsync(hrecheck, ws.ncand2.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
-        if (pairs) {
-            CK(cudaMemcpyAsync(hpairs, ws.xnpairs.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
-            CK(cudaMemcpyAsync(hneed, ws.needexact.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
-        }
-        if (d_probe_fallback) CK(cudaMemcpyAsync(hfell, d_probe_fallback, 4, cudaMemcpyDeviceToHost, ws.stream));
-        if (!io.out_on_device) {
-            size_t bytes = (size_t)B * top_k * 12 + (size_t)B * 4;
-            CKS(ws.hres.ensure(bytes));
-            char *h = ws.hres.as<char>();
-            CK(cudaMemcpyAsync(h, d_ids, (size_t)B * top_k * 8, cudaMemcpyDeviceToHost, ws.stream));
-            CK(cudaMemcpyAsync(h + (size_t)B * top_k * 8, d_sc, (size_t)B * top_k * 4, cudaMemcpyDeviceToHost, ws.stream));
-            CK(cudaMemcpyAsync(h + (size_t)B * top_k * 12, d_cn, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
-        }
-        if (prof) CK(cudaEventRecord(ws.ev[9], ws.stream));
-        CK(cudaStreamSynchronize(ws.stream));
-        if (tc && *hfell) {  // the tensor-core pass gave up on the device: same sub-batch again on the exact path
-            *redo = true;
-            return PB_OK;
-        }
-        if (!io.out_on_device) {
-            char *h = ws.hres.as<char>();
-            memcpy(io.out_ids + (size_t)b0 * top_k, h, (size_t)B * top_k * 8);
-            memcpy(io.out_scores + (size_t)b0 * top_k, h + (size_t)B * top_k * 8, (size_t)B * top_k * 4);
-            memcpy(io.out_counts + b0, h + (size_t)B * top_k * 12, (size_t)B * 4);
-        }
-        if (prof) {
-            for (int s = 0; s < PB_STAGE_COUNT; ++s) {
-                float ms = 0.f;
-                CK(cudaEventElapsedTime(&ms, ws.ev[s], ws.ev[s + 1]));
-                g_stats.ms[s] += ms;
-            }
-            for (int k = 0; k < PB_KERNEL_COUNT; ++k)
-                if (g_stats.kernel_seen[k]) {
-                    float ms = 0.f;
-                    CK(cudaEventElapsedTime(&ms, ws.kev[2 * k], ws.kev[2 * k + 1]));
-                    g_stats.kernel_ms[k] += ms;
-                    g_stats.kernel_seen[k] = false;
-                }
-        }
-        if (diag) {
-            unsigned long long got[2] = {0, 0};
-            CK(cudaMemcpy(got, ws.fdiag.p, 16, cudaMemcpyDeviceToHost));
-            g_stats.work.filter_err_ratio_e6 = std::max<long long>(g_stats.work.filter_err_ratio_e6, (long long)got[0]);
-            g_stats.work.filter_diag_pairs += (long long)got[1];
-        }
-        if (fast && ix->k1_diag && ws.k1diag.p) {
-            int got[2] = {0, 0};
-            CK(cudaMemcpy(got, ws.k1diag.p, 8, cudaMemcpyDeviceToHost));
-            g_stats.work.k1_tc_max_code_diff = std::max<long long>(g_stats.work.k1_tc_max_code_diff, got[0]);
-            g_stats.work.k1_rows_mismatch += 0;
-        }
-        g_stats.work.n_queries += B;
-        g_stats.work.n_query_tokens += R;
-        if (tc) g_stats.work.n_k1_tc += 1;
-        else if (d_probe_fallback) (*hfell ? g_stats.work.n_probe_list : g_stats.work.n_probe_threshold) += 1;
-        else if (probe_list_only) g_stats.work.n_probe_list += 1;
-        if (fast)
-            for (int b = 0; b < B; ++b) g_stats.work.n_recheck_docs += hrecheck[b];
-        if (pairs)
-            for (int b = 0; b < B; ++b) {
-                if (hneed[b]) g_stats.work.n_pair_fallback_queries += 1;
-                else g_stats.work.n_exact_pairs += hpairs[b];
-            }
-        g_stats.work.n_candidate_tokens += (long long)hcnt[0];
-        for (int b = 0; b < B; ++b) {
-            g_stats.work.n_cells += hc[b];
-            g_stats.work.n_candidates += hc[B + b];
-            if (filt) {
-                g_stats.work.n_filter_docs += hc[2 * B + b];
-                g_stats.work.n_filter_tokens += (long long)hcnt[1 + b];
-                g_stats.work.n_exact_docs += hsurv[b];
-                g_stats.work.n_exact_tokens += hsurv_tok[b];
-            } else {
-                g_stats.work.n_exact_docs += hc[2 * B + b];
-                g_stats.work.n_exact_tokens += (long long)hcnt[1 + b];
-            }
-        }
-        // ---- optional trace (tests only; synchronous copies) ----
-        if (io.trace) {
-            pb_trace *t = io.trace;
-            for (int b = 0; b < B; ++b) {
-                const int64_t gb = b0 + b;
-                if (t->n_cells) t->n_cells[gb] = hc[b];
-                if (t->n_candidates) t->n_candidates[gb] = hc[B + b];
-                if (t->n_kept) t->n_kept[gb] = hc[2 * B + b];
-                if (t->cells) {
-                    int n = (int)std::min<int64_t>(hc[b], t->cells_cap);
-                    std::vector<uint32_t> tmp(n);
-                    CK(cudaMemcpy(tmp.data(), ws.cells.as<uint32_t>() + (size_t)b * cells_cap, (size_t)n * 4, cudaMemcpyDeviceToHost));
-                    for (int i = 0; i < n; ++i) t->cells[gb * t->cells_cap + i] = tmp[i];
-                }
-                if (t->candidates || t->approx) {
-                    int n = (int)std::min<int64_t>(hc[B + b], t->cand_cap);
-                    std::vector<uint32_t> tmp(n);
-                    CK(cudaMemcpy(tmp.data(), ws.cand.as<uint32_t>() + (size_t)b * ix->D, (size_t)n * 4, cudaMemcpyDeviceToHost));
-                    if (t->candidates)
-                        for (int i = 0; i < n; ++i) t->candidates[gb * t->cand_cap + i] = (int64_t)tmp[i] + ix->doc_id_base;
-                    if (t->approx)
-                        CK(cudaMemcpy(t->approx + gb * t->cand_cap, ws.approx.as<float>() + (size_t)b * ix->D, (size_t)n * 4,
-                                      cudaMemcpyDeviceToHost));
-                }
-                if (t->kept || t->kept_exact) {
-                    int n = (int)std::min<int64_t>(hc[2 * B + b], t->kept_cap);
-                    std::vector<uint32_t> tmp(n);
-                    CK(cudaMemcpy(tmp.data(), ws.kept.as<uint32_t>() + (size_t)b * Mcap, (size_t)n * 4, cudaMemcpyDeviceToHost));
-                    if (t->kept)
-                        for (int i = 0; i < n; ++i) t->kept[gb * t->kept_cap + i] = (int64_t)tmp[i] + ix->doc_id_base;
-                    if (t->kept_exact)
-                        CK(cudaMemcpy(t->kept_exact + gb * t->kept_cap, ws.exact.as<float>() + (size_t)b * Mcap, (size_t)n * 4,
-                                      cudaMemcpyDeviceToHost));
-                }
-            }
-        }
-        return PB_OK;
-        };  // run_sub
+        probe_chunk_rows(ix->K, plan.n_probe, &n_chunks_k);
+        pass.use_tc = k1_tc_usable(ix) && pass.fast && ix->probe16 && !ix->k1_diag && !plan.all_eligible &&
+                      !plan.big_probe && !plan.d_elig && pass.QS / 8 <= 32 && n_chunks_k >= plan.n_probe &&
+                      plan.n_probe <= 192;
         bool redo = false;
-        CKS(run_sub(want_tc, &redo));
+        CKS(run_pass(ix, ws, p, io, plan, pass, &redo));
         if (redo) {
             g_stats.work.n_k1_tc_redo += 1;
-            CKS(run_sub(false, &redo));
+            pass.use_tc = false;
+            CKS(run_pass(ix, ws, p, io, plan, pass, &redo));
         }
     }
-    if (prof) {
+    if (plan.prof) {
         CK(cudaEventRecord(ws.call_ev[1], ws.stream));
         CK(cudaEventSynchronize(ws.call_ev[1]));
         CK(cudaEventElapsedTime(&g_stats.call_ms, ws.call_ev[0], ws.call_ev[1]));
@@ -2137,7 +2265,7 @@ static pb_status search_impl(pb_index *ix, const pb_search_params *p, const Sear
         if (!lane_lock.owns_lock()) lanes = 1;  // another host thread is using the helpers: it already provides the overlap
     }
     if (lanes <= 1) {
-        const pb_status st = search_impl_inner(ix, p, io);
+        const pb_status st = run_search(ix, p, io);
         if (st != PB_OK && ix && ix->group) ix->group->fail();  // the peers must not wait for a rank that gave up
         return st;
     }
@@ -2169,7 +2297,7 @@ static pb_status search_impl(pb_index *ix, const pb_search_params *p, const Sear
     }
     auto run_lane = [&](int l) {
         g_budget_div = lanes;
-        sts[l] = search_impl_inner(ix, p, ios[l]);
+        sts[l] = run_search(ix, p, ios[l]);
         g_budget_div = 1;
         stats[l] = g_stats;
         if (sts[l] != PB_OK) errs[l] = g_err;
