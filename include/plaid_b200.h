@@ -241,6 +241,32 @@ PB_API pb_status pb_index_append_encoded_sharded(pb_index *ix, const int64_t *co
                                                  const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
                                                  int64_t *out_first_doc_id);
 
+/* Rebalance a doc-sharded deployment in place: rank r takes documents [bounds[r], bounds[r + 1]) of the deployment, with
+ * doc_id_base = bounds[r].  Global doc ids do not change, so the group's search results do not change either; no file
+ * is touched.  Calling rules as for pb_index_delete_sharded, with the same bounds on every rank; a handle outside any
+ * group is a group of one, whose only bounds are [0, D] (a no-op).
+ *
+ * bounds [world + 1], host memory: bounds[0] = 0, bounds[world] = D_total, non-decreasing; a rank may be left empty.
+ * NULL: the token-balanced split of pb_index_dir_shard_bounds over the deployment's documents, bounds[r] =
+ * min { d : doc_off[d] world >= N_total r }.  out_bounds [world + 1] (may be NULL) receives the bounds applied.
+ *
+ * Afterwards each rank is exactly pb_index_open of its range: its codes, residuals and doc lengths, max_doclen, the
+ * per-doc distinct codes, 1 / |c + w|, vmin and wmax over its tokens, and as inverted file the slice of the
+ * deployment's global lists (the ranks' lists rebased and concatenated in rank order, each list in its order).  When
+ * every list is sorted -- as in every index this library or the reference writes -- that is pb_index_load_range of a
+ * directory kept in sync.  Bounds equal to the current ones change nothing.
+ *
+ * Memory: a rank whose range changes builds its new arrays next to its old ones, sized to their contents (the last rank
+ * keeps the spare capacity it had, e.g. from pb_index_reserve), and frees the old ones at the end.
+ *
+ * Every failure leaves every rank unchanged, and every rank returns the same status: PB_ERR_INVALID for bounds that do
+ * not tile [0, D_total), ranks given different bounds, or ranks whose layouts disagree (as above);
+ * PB_ERR_UNSUPPORTED for a member opened with PB_OPEN_ADOPT_RESIDUALS; PB_ERR_NOMEM for a rank that cannot allocate its
+ * new arrays; PB_ERR_COMM when libnccl lacks ncclSend / ncclRecv / ncclGroupStart / ncclGroupEnd.  Unlike the calls
+ * above, a CUDA or transport error while the documents move also leaves every rank as it was: the new arrays replace
+ * the old ones only after a last vote. */
+PB_API pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bounds, int64_t *out_bounds);
+
 /* ---- search ------------------------------------------------------------------------------ */
 
 /*

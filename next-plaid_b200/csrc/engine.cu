@@ -35,7 +35,7 @@
 // ------------------------------------------------------------------------------------------
 typedef struct ncclComm *ncclComm_t;
 typedef struct { char internal[128]; } ncclUniqueId;
-enum { PB_NCCL_UINT64 = 5, PB_NCCL_FLOAT32 = 7, PB_NCCL_SUM = 0 };
+enum { PB_NCCL_UINT8 = 1, PB_NCCL_UINT64 = 5, PB_NCCL_FLOAT32 = 7, PB_NCCL_SUM = 0 };
 struct NcclApi {
     void *h = nullptr;
     int (*GetUniqueId)(ncclUniqueId *) = nullptr;
@@ -44,6 +44,12 @@ struct NcclApi {
     int (*AllGather)(const void *, void *, size_t, int, ncclComm_t, cudaStream_t) = nullptr;
     int (*AllReduce)(const void *, void *, size_t, int, int, ncclComm_t, cudaStream_t) = nullptr;
     const char *(*GetErrorString)(int) = nullptr;
+    // point-to-point, bound when present: only pb_index_rebalance_sharded needs them, so load() does not require them
+    int (*Send)(const void *, size_t, int, int, ncclComm_t, cudaStream_t) = nullptr;
+    int (*Recv)(void *, size_t, int, int, ncclComm_t, cudaStream_t) = nullptr;
+    int (*GroupStart)() = nullptr;
+    int (*GroupEnd)() = nullptr;
+    bool has_p2p() const { return Send && Recv && GroupStart && GroupEnd; }
     bool load() {
         if (h) return true;
         const char *names[] = {"libnccl.so.2", "libnccl.so"};
@@ -58,6 +64,10 @@ struct NcclApi {
         AllGather = (int (*)(const void *, void *, size_t, int, ncclComm_t, cudaStream_t))dlsym(h, "ncclAllGather");
         AllReduce = (int (*)(const void *, void *, size_t, int, int, ncclComm_t, cudaStream_t))dlsym(h, "ncclAllReduce");
         GetErrorString = (const char *(*)(int))dlsym(h, "ncclGetErrorString");
+        Send = (int (*)(const void *, size_t, int, int, ncclComm_t, cudaStream_t))dlsym(h, "ncclSend");
+        Recv = (int (*)(void *, size_t, int, int, ncclComm_t, cudaStream_t))dlsym(h, "ncclRecv");
+        GroupStart = (int (*)())dlsym(h, "ncclGroupStart");
+        GroupEnd = (int (*)())dlsym(h, "ncclGroupEnd");
         return GetUniqueId && CommInitRank && CommDestroy && AllGather && AllReduce && GetErrorString;
     }
 };
@@ -79,6 +89,7 @@ struct pb_shard_group {
     bool broken = false;
     int joined = 0;
     std::vector<const void *> send;
+    std::vector<const void *const *> table;  // per rank: the device pointers it sends in a rebalance, [destination][item]
     std::vector<int> dev;
     // false = a peer failed or did not arrive within the timeout; the group stays broken.  unbounded: wait for the
     // peers however long they take (a peer that fails still breaks the group), for a peer known to be busy
@@ -819,12 +830,10 @@ static pb_status build_centroid_operands(pb_index *ix) {
     return PB_OK;
 }
 
-// 1 / |c + w| of tokens [t0, t0 + n) into tok_inv_norm; min |c + w| and max |w| over them folded into mn[0] / mn[1]
-static pb_status launch_min_vnorm(pb_index *ix, long long t0, long long n, float *mn) {
+// 1 / |c + w| of n tokens (codes, packed residuals) into inv; min |c + w| and max |w| over them folded into mn[0] / mn[1]
+static pb_status launch_min_vnorm(pb_index *ix, const uint32_t *codes, const uint8_t *res, long long n, float *inv,
+                                  float *mn) {
     if (n == 0) return PB_OK;
-    const uint32_t *codes = ix->codes.as<uint32_t>() + t0;
-    const uint8_t *res = ix->residuals.as<uint8_t>() + (size_t)t0 * ix->packed;
-    float *inv = ix->tok_inv_norm.as<float>() + t0;
     switch (ix->dim) {
         case 64: k_min_vnorm<64><<<ix->sm_count * 8, 256>>>(ix->centroids.as<float>(), ix->w_rev.as<float>(), ix->nbits, codes, res, n, mn, inv); break;
         case 96: k_min_vnorm<96><<<ix->sm_count * 8, 256>>>(ix->centroids.as<float>(), ix->w_rev.as<float>(), ix->nbits, codes, res, n, mn, inv); break;
@@ -832,6 +841,11 @@ static pb_status launch_min_vnorm(pb_index *ix, long long t0, long long n, float
     }
     CK(cudaGetLastError());
     return PB_OK;
+}
+// the same for the handle's tokens [t0, t0 + n), into its tok_inv_norm
+static pb_status launch_min_vnorm(pb_index *ix, long long t0, long long n, float *mn) {
+    return launch_min_vnorm(ix, ix->codes.as<uint32_t>() + t0, ix->residuals.as<uint8_t>() + (size_t)t0 * ix->packed, n,
+                            ix->tok_inv_norm.as<float>() + t0, mn);
 }
 
 // Derived arrays that need every token: the per-doc distinct-code lists k_approx walks.
@@ -2578,6 +2592,7 @@ extern "C" pb_status pb_shard_group_create(int32_t world, pb_shard_group **out) 
     pb_shard_group *g = new pb_shard_group();
     g->world = world;
     g->send.assign((size_t)world, nullptr);
+    g->table.assign((size_t)world, nullptr);
     g->dev.assign((size_t)world, 0);
     *out = g;
     return PB_OK;
@@ -3899,6 +3914,404 @@ extern "C" pb_status pb_index_append_encoded_sharded(pb_index *ix, const int64_t
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
     return sharded_update(ix, SH_OP_APPEND_ENCODED, nullptr, nullptr, codes, residuals, doc_lengths, nullptr, n_docs,
                           memory_space, nullptr, 0, out_first_doc_id);
+}
+
+// ------------------------------------------------------------------------------------------
+// rebalance of a doc-sharded deployment (DESIGN §4i): the ranks take new document ranges over the same global ids.
+// Exchange A checks the layout as §4h does; balanced bounds come from one offer per boundary and rank; every rank
+// derives the same plan from the old bounds a and the new ones b: the piece s -> r is docs [max(a_s, b_r),
+// min(a_s+1, b_r+1)).  A rank whose range changes builds its new arrays out of place: its pieces' rows arrive at their
+// final offsets, then the scans, the merge of the inverted file and the norm pass run over them.  The old arrays stay
+// until the last vote, so a failure anywhere leaves every rank as it was.
+// ------------------------------------------------------------------------------------------
+enum { RB_STATUS, RB_RANK, RB_WORLD, RB_BASE, RB_D, RB_N, RB_K, RB_DIM, RB_NBITS, RB_ADOPT, RB_PRINT, RB_WORDS };
+enum { SZ_TOK, SZ_UCODES, SZ_IVF, SZ_WORDS };  // per piece in the size exchange
+// what moves with a piece of documents, in the order both ends issue it
+enum { XF_CODES, XF_RES, XF_UCODES, XF_TLEN, XF_ULEN, XF_IVF_OFF, XF_IVF, XF_ITEMS };
+
+struct RebalancePrep {
+    std::vector<long long> hoff, huoff;  // the rank's doc_off / udoc_off as they are
+    // sender: its pieces' bounds q [W + 1] in local ids, per-doc lengths, the inverted file split by destination with
+    // its offsets [W][K + 1], and where each piece's entries start in it (hsplit [W + 1])
+    DevBuf q, tlen, ulen, split, split_off;
+    std::vector<long long> hsplit;
+    // receiver: the new arrays, and the per-doc lengths and inverted-file segments of its pieces as they arrive
+    DevBuf codes, residuals, ucodes, doc_off, udoc_off, ivf, ivf_off, ivf_spare, tok_inv_norm, rlen, rulen, seg, seg_off,
+        meta, mn;
+    long long D1 = 0, N1 = 0, U1 = 0, L1 = 0;
+    int maxlen = 0;
+    float vmin = 0.f, wmax = 0.f;
+};
+
+extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bounds, int64_t *out_bounds) {
+    if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    std::lock_guard<std::mutex> gate(ix->gate);
+    std::unique_lock<std::shared_mutex> wr(ix->rw);
+    const int W = ix->world, me = ix->rank;
+    const long long K = ix->K;
+    const size_t pk = (size_t)ix->packed;
+    const int grid = ix->sm_count * 8;
+    RebalancePrep p;
+    long long rec[RB_WORDS] = {};
+    // 1. local checks, the fingerprint of the bounds and the host copies of the offsets: no early return, or the peers
+    // would wait
+    auto local = [&]() -> pb_status {
+        Fnv64 f;
+        f.put(bounds != nullptr);
+        if (bounds) f.add(bounds, (size_t)(W + 1) * 8);
+        rec[RB_PRINT] = (long long)f.h;
+        if (ix->comm && !g_nccl.has_p2p())
+            return pb_fail(PB_ERR_COMM, "the NCCL library lacks ncclSend / ncclRecv / ncclGroupStart / ncclGroupEnd");
+        CK(cudaSetDevice(ix->device));
+        CK(cudaDeviceSynchronize());  // work earlier readers left queued (pb_search_batch_device) reads the arrays
+        p.hoff.resize((size_t)ix->D + 1);
+        p.huoff.resize((size_t)ix->D + 1);
+        CK(cudaMemcpy(p.hoff.data(), ix->doc_off.p, p.hoff.size() * 8, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(p.huoff.data(), ix->udoc_off.p, p.huoff.size() * 8, cudaMemcpyDeviceToHost));
+        return PB_OK;
+    };
+    rec[RB_STATUS] = local();
+    rec[RB_RANK] = me;
+    rec[RB_WORLD] = W;
+    rec[RB_BASE] = ix->doc_id_base;
+    rec[RB_D] = ix->D;
+    rec[RB_N] = ix->N;
+    rec[RB_K] = K;
+    rec[RB_DIM] = ix->dim;
+    rec[RB_NBITS] = ix->nbits;
+    rec[RB_ADOPT] = !ix->residuals.owned;
+
+    // 2. exchange A and the verdict every rank reaches from the same records
+    std::vector<long long> all;
+    CKS(gather_words(ix, rec, RB_WORDS, all));
+    CKS(first_failure(ix, all, RB_WORDS, "; nothing changed"));
+    auto at = [&](int r, int w) { return all[(size_t)r * RB_WORDS + w]; };
+    std::vector<long long> a((size_t)W + 1, 0), tok((size_t)W + 1, 0);  // old bounds, global token offsets
+    for (int r = 0; r < W; ++r) {
+        if (at(r, RB_RANK) != r || at(r, RB_WORLD) != W || at(r, RB_K) != at(0, RB_K) || at(r, RB_DIM) != at(0, RB_DIM) ||
+            at(r, RB_NBITS) != at(0, RB_NBITS))
+            return pb_fail(PB_ERR_INVALID, "rank %d's layout (rank %lld of %lld, K=%lld dim=%lld nbits=%lld) differs from rank 0's",
+                           r, at(r, RB_RANK), at(r, RB_WORLD), at(r, RB_K), at(r, RB_DIM), at(r, RB_NBITS));
+        if (at(r, RB_BASE) != a[r])
+            return pb_fail(PB_ERR_INVALID, "the ranks' documents do not tile [0, D): rank %d starts at %lld, not %lld", r,
+                           at(r, RB_BASE), a[r]);
+        if (at(r, RB_PRINT) != at(0, RB_PRINT))
+            return pb_fail(PB_ERR_INVALID, "rank %d was called with other bounds than rank 0", r);
+        a[r + 1] = a[r] + at(r, RB_D);
+        tok[r + 1] = tok[r] + at(r, RB_N);
+    }
+    for (int r = 0; r < W; ++r)
+        if (at(r, RB_ADOPT))
+            return pb_fail(PB_ERR_UNSUPPORTED, "rank %d uses the caller's residual array (PB_OPEN_ADOPT_RESIDUALS)", r);
+    const long long D_total = a[W], N_total = tok[W];
+
+    // 3. the new bounds: the caller's, or the token-balanced split b[r] = min { d : off[d] W >= N r } of the global doc
+    // offsets.  For that each rank offers the least d of its closed range [a_me, a_me+1] that qualifies (global
+    // off[d] = tok[me] + its own doc_off), or D_total; the least offer wins.
+    std::vector<long long> b((size_t)W + 1, 0);
+    if (bounds) {
+        b.assign(bounds, bounds + W + 1);
+        bool ok = b[0] == 0 && b[W] == D_total;
+        for (int r = 0; r < W; ++r) ok = ok && b[r] <= b[r + 1];
+        if (!ok) return pb_fail(PB_ERR_INVALID, "bounds must be non-decreasing from 0 to D_total = %lld", D_total);
+    } else {
+        std::vector<long long> offer((size_t)W + 1, D_total), offers;
+        for (int r = 1; r < W; ++r) {
+            long long lo = 0, hi = ix->D + 1;  // the first local j with (tok[me] + doc_off[j]) W >= N r, or D + 1
+            while (lo < hi) {
+                const long long mid = (lo + hi) >> 1;
+                if ((tok[me] + p.hoff[mid]) * W >= N_total * r) hi = mid; else lo = mid + 1;
+            }
+            if (lo <= ix->D) offer[r] = a[me] + lo;
+        }
+        CKS(gather_words(ix, offer.data(), W + 1, offers));
+        b[W] = D_total;
+        for (int r = 1; r < W; ++r) {
+            b[r] = D_total;
+            for (int s = 0; s < W; ++s) b[r] = std::min(b[r], offers[(size_t)s * (W + 1) + r]);
+        }
+    }
+    if (b == a) {  // nothing moves
+        if (out_bounds) std::copy(b.begin(), b.end(), out_bounds);
+        return PB_OK;
+    }
+
+    // 4. the plan, and the sender's side of the prepare: per-doc lengths and the inverted file split by destination
+    auto piece = [&](int s, int r, long long &lo, long long &hi) {
+        lo = std::max(a[s], b[r]);
+        hi = std::min(a[s + 1], b[r + 1]);
+        return lo < hi;
+    };
+    const bool changes = a[me] != b[me] || a[me + 1] != b[me + 1];
+    const int SW = 1 + SZ_WORDS * W;  // status, then per destination its piece's tokens, distinct codes, ivf entries
+    std::vector<long long> srec((size_t)SW, 0);
+    auto prepare = [&]() -> pb_status {
+        if (!changes) return PB_OK;
+        const long long Dm = ix->D, n = (long long)W * (K + 1);
+        std::vector<long long> q((size_t)W + 1);
+        for (int r = 0; r <= W; ++r) q[r] = std::min(std::max(b[r] - a[me], 0ll), Dm);
+        CKS(upload(p.q, q.data(), q.size() * 8, PB_MEM_HOST));
+        CKS(p.tlen.ensure(std::max<size_t>((size_t)Dm * 8, 16)));
+        CKS(p.ulen.ensure(std::max<size_t>((size_t)Dm * 8, 16)));
+        if (Dm > 0)
+            k_doc_lengths<<<grid, 256>>>(ix->doc_off.as<long long>(), ix->udoc_off.as<long long>(), Dm,
+                                         p.tlen.as<long long>(), p.ulen.as<long long>());
+        DevBuf cnt, tmp;
+        CKS(cnt.ensure((size_t)n * 8));
+        CKS(p.split_off.ensure((size_t)n * 8));
+        CK(cudaMemset(cnt.p, 0, (size_t)n * 8));
+        k_ivf_split_count<<<grid, 256>>>(ix->ivf.as<uint32_t>(), ix->ivf_off.as<long long>(), K, p.q.as<long long>(), W,
+                                         cnt.as<long long>());
+        CK(cudaGetLastError());
+        CKS(exclusive_sum(cnt.as<long long>(), p.split_off.as<long long>(), n, tmp));
+        p.hsplit.assign((size_t)W + 1, 0);
+        for (int r = 0; r < W; ++r)
+            CK(cudaMemcpy(&p.hsplit[r], p.split_off.as<long long>() + (size_t)r * (K + 1), 8, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(&p.hsplit[W], p.split_off.as<long long>() + n - 1, 8, cudaMemcpyDeviceToHost));  // cnt[n - 1] = 0
+        CKS(p.split.ensure(std::max<size_t>((size_t)p.hsplit[W] * 4, 16)));
+        CK(cudaMemcpy(cnt.p, p.split_off.p, (size_t)n * 8, cudaMemcpyDeviceToDevice));  // the write pass's cursors
+        k_ivf_split_write<<<grid, 256>>>(ix->ivf.as<uint32_t>(), ix->ivf_off.as<long long>(), K, p.q.as<long long>(), W,
+                                         cnt.as<long long>(), p.split.as<uint32_t>());
+        CK(cudaGetLastError());
+        CK(cudaDeviceSynchronize());
+        for (int r = 0; r < W; ++r) {
+            long long lo, hi;
+            if (!piece(me, r, lo, hi)) continue;
+            lo -= a[me];
+            hi -= a[me];
+            srec[1 + SZ_WORDS * r + SZ_TOK] = p.hoff[hi] - p.hoff[lo];
+            srec[1 + SZ_WORDS * r + SZ_UCODES] = p.huoff[hi] - p.huoff[lo];
+            srec[1 + SZ_WORDS * r + SZ_IVF] = p.hsplit[r + 1] - p.hsplit[r];
+        }
+        return PB_OK;
+    };
+    srec[0] = prepare();
+    std::vector<long long> sizes;
+    CKS(gather_words(ix, srec.data(), SW, sizes));
+    CKS(first_failure(ix, sizes, SW, "; nothing changed"));
+    auto sz = [&](int s, int r, int k) { return sizes[(size_t)s * SW + 1 + SZ_WORDS * r + k]; };
+
+    // the receiver's side: where each source's piece lands, and the new arrays, sized to their contents (the last rank
+    // keeps the spare capacity it had, so appends provisioned by pb_index_reserve still need no growth copy)
+    std::vector<long long> tpos((size_t)W + 1, 0), upos((size_t)W + 1, 0), ipos((size_t)W + 1, 0);
+    for (int s = 0; s < W; ++s) {
+        tpos[s + 1] = tpos[s] + sz(s, me, SZ_TOK);
+        upos[s + 1] = upos[s] + sz(s, me, SZ_UCODES);
+        ipos[s + 1] = ipos[s] + sz(s, me, SZ_IVF);
+    }
+    auto allocate = [&]() -> pb_status {
+        if (!changes) return PB_OK;
+        p.D1 = b[me + 1] - b[me];
+        p.N1 = tpos[W];
+        p.U1 = upos[W];
+        p.L1 = ipos[W];
+        if (p.L1 > (1ll << 31) - 2) return pb_fail(PB_ERR_UNSUPPORTED, "more than 2^31 (centroid, doc) pairs per shard");
+        const bool last = me == W - 1;
+        auto alloc = [&](DevBuf &nb, const DevBuf &old, long long old_bytes, long long bytes) {
+            const size_t spare = last && (long long)old.cap > old_bytes ? old.cap - (size_t)old_bytes : 0;
+            return nb.grow(std::max<size_t>((size_t)bytes + spare, 16), 0, false);
+        };
+        const long long D0 = ix->D, N0 = ix->N, D1 = p.D1;
+        CKS(alloc(p.codes, ix->codes, N0 * 4, p.N1 * 4));
+        CKS(alloc(p.residuals, ix->residuals, N0 * (long long)pk, p.N1 * (long long)pk));
+        CKS(alloc(p.ucodes, ix->ucodes, ix->n_ucodes * 4, p.U1 * 4));
+        CKS(alloc(p.doc_off, ix->doc_off, (D0 + 1) * 8, (D1 + 1) * 8));
+        CKS(alloc(p.udoc_off, ix->udoc_off, (D0 + 1) * 8, (D1 + 1) * 8));
+        CKS(alloc(p.ivf, ix->ivf, ix->ivf_len * 4, p.L1 * 4));
+        if (last && ix->ivf_spare.cap) CKS(alloc(p.ivf_spare, ix->ivf_spare, ix->ivf_len * 4, p.L1 * 4));
+        if (filter_dim(ix->dim) && p.N1 > 0) CKS(alloc(p.tok_inv_norm, ix->tok_inv_norm, N0 * 4, p.N1 * 4));
+        CKS(p.ivf_off.grow((size_t)(K + 1) * 8, 0, false));
+        CKS(p.rlen.ensure((size_t)(D1 + 1) * 8));
+        CKS(p.rulen.ensure((size_t)(D1 + 1) * 8));
+        CKS(p.seg.ensure(std::max<size_t>((size_t)p.L1 * 4, 16)));
+        CKS(p.seg_off.ensure((size_t)W * (K + 1) * 8));
+        CK(cudaMemset(p.seg_off.p, 0, (size_t)W * (K + 1) * 8));  // a source without a piece has empty lists
+        CKS(p.mn.ensure(16));
+        std::vector<long long> meta((size_t)2 * W, 0);  // [segbase W][idoff W]
+        for (int s = 0; s < W; ++s) {
+            long long lo, hi;
+            meta[s] = ipos[s];
+            if (piece(s, me, lo, hi)) meta[W + s] = lo - b[me];
+        }
+        CKS(upload(p.meta, meta.data(), meta.size() * 8, PB_MEM_HOST));
+        return PB_OK;
+    };
+    long long vote = allocate();
+    std::vector<long long> votes;
+    CKS(gather_words(ix, &vote, 1, votes));
+    CKS(first_failure(ix, votes, 1, " allocating its new arrays; nothing changed"));
+
+    // 5. the transfer: rows of codes, residuals, distinct codes and per-doc lengths as contiguous ranges, and the
+    // inverted-file pieces, from the senders' arrays into the receivers' new arrays at their final offsets
+    std::vector<const void *> sp((size_t)W * XF_ITEMS, nullptr);  // what I send, [destination][item]
+    std::vector<size_t> sbytes((size_t)W * XF_ITEMS, 0);
+    std::vector<void *> rp((size_t)W * XF_ITEMS, nullptr);  // where I receive, [source][item]
+    std::vector<size_t> rbytes((size_t)W * XF_ITEMS, 0);
+    if (changes) {
+        for (int r = 0; r < W; ++r) {
+            long long lo, hi;
+            if (!piece(me, r, lo, hi)) continue;
+            lo -= a[me];
+            hi -= a[me];
+            const void **s = &sp[(size_t)r * XF_ITEMS];
+            size_t *n = &sbytes[(size_t)r * XF_ITEMS];
+            s[XF_CODES] = ix->codes.as<uint8_t>() + (size_t)p.hoff[lo] * 4;
+            n[XF_CODES] = (size_t)sz(me, r, SZ_TOK) * 4;
+            s[XF_RES] = ix->residuals.as<uint8_t>() + (size_t)p.hoff[lo] * pk;
+            n[XF_RES] = (size_t)sz(me, r, SZ_TOK) * pk;
+            s[XF_UCODES] = ix->ucodes.as<uint8_t>() + (size_t)p.huoff[lo] * 4;
+            n[XF_UCODES] = (size_t)sz(me, r, SZ_UCODES) * 4;
+            s[XF_TLEN] = p.tlen.as<long long>() + lo;
+            s[XF_ULEN] = p.ulen.as<long long>() + lo;
+            n[XF_TLEN] = n[XF_ULEN] = (size_t)(hi - lo) * 8;
+            s[XF_IVF_OFF] = p.split_off.as<long long>() + (size_t)r * (K + 1);
+            n[XF_IVF_OFF] = (size_t)(K + 1) * 8;
+            s[XF_IVF] = p.split.as<uint32_t>() + p.hsplit[r];
+            n[XF_IVF] = (size_t)sz(me, r, SZ_IVF) * 4;
+        }
+        for (int s = 0; s < W; ++s) {
+            long long lo, hi;
+            if (!piece(s, me, lo, hi)) continue;
+            void **d = &rp[(size_t)s * XF_ITEMS];
+            size_t *n = &rbytes[(size_t)s * XF_ITEMS];
+            d[XF_CODES] = p.codes.as<uint8_t>() + (size_t)tpos[s] * 4;
+            n[XF_CODES] = (size_t)sz(s, me, SZ_TOK) * 4;
+            d[XF_RES] = p.residuals.as<uint8_t>() + (size_t)tpos[s] * pk;
+            n[XF_RES] = (size_t)sz(s, me, SZ_TOK) * pk;
+            d[XF_UCODES] = p.ucodes.as<uint8_t>() + (size_t)upos[s] * 4;
+            n[XF_UCODES] = (size_t)sz(s, me, SZ_UCODES) * 4;
+            d[XF_TLEN] = p.rlen.as<long long>() + (lo - b[me]);
+            d[XF_ULEN] = p.rulen.as<long long>() + (lo - b[me]);
+            n[XF_TLEN] = n[XF_ULEN] = (size_t)(hi - lo) * 8;
+            d[XF_IVF_OFF] = p.seg_off.as<long long>() + (size_t)s * (K + 1);
+            n[XF_IVF_OFF] = (size_t)(K + 1) * 8;
+            d[XF_IVF] = p.seg.as<uint32_t>() + ipos[s];
+            n[XF_IVF] = (size_t)sz(s, me, SZ_IVF) * 4;
+        }
+    }
+    auto transfer = [&]() -> pb_status {
+        struct Stream {
+            cudaStream_t s = nullptr;
+            ~Stream() {
+                if (s) cudaStreamDestroy(s);
+            }
+        } st;
+        const cudaError_t ce = cudaStreamCreateWithFlags(&st.s, cudaStreamNonBlocking);
+        if (ce != cudaSuccess) {
+            if (ix->group) ix->group->fail();  // the peers must not wait for me at the barriers below
+            return pb_fail(PB_ERR_CUDA, "cudaStreamCreate failed: %s", cudaGetErrorString(ce));
+        }
+        if (ix->comm) {  // NCCL: my own piece by a local copy, the others by send / receive pairs in one group
+            for (int it = 0; it < XF_ITEMS; ++it) {
+                const size_t i = (size_t)me * XF_ITEMS + it;
+                if (rbytes[i]) CK(cudaMemcpyAsync(rp[i], sp[i], rbytes[i], cudaMemcpyDeviceToDevice, st.s));
+            }
+            int res = g_nccl.GroupStart();
+            for (int r = 0; r < W && res == 0; ++r)
+                for (int it = 0; r != me && it < XF_ITEMS && res == 0; ++it) {
+                    const size_t i = (size_t)r * XF_ITEMS + it;
+                    if (sbytes[i]) res = g_nccl.Send(sp[i], sbytes[i], PB_NCCL_UINT8, r, ix->comm, st.s);
+                }
+            for (int s = 0; s < W && res == 0; ++s)
+                for (int it = 0; s != me && it < XF_ITEMS && res == 0; ++it) {
+                    const size_t i = (size_t)s * XF_ITEMS + it;
+                    if (rbytes[i]) res = g_nccl.Recv(rp[i], rbytes[i], PB_NCCL_UINT8, s, ix->comm, st.s);
+                }
+            const int end = g_nccl.GroupEnd();
+            if (res == 0) res = end;
+            if (res != 0) return pb_fail(PB_ERR_COMM, "rebalance transfer failed: %s", g_nccl.GetErrorString(res));
+            CK(cudaStreamSynchronize(st.s));
+            return PB_OK;
+        }
+        // in-process group: every rank publishes its send pointers, then each receiver pulls its pieces
+        pb_shard_group *g = ix->group;
+        if (!g) return pb_fail(PB_ERR_COMM, "sharded handle without a transport");
+        g->table[me] = sp.data();
+        if (!g->barrier(true)) return pb_fail(PB_ERR_COMM, "shard group: a peer failed");
+        cudaError_t e = cudaSuccess;
+        for (int s = 0; s < W && e == cudaSuccess; ++s)
+            for (int it = 0; it < XF_ITEMS && e == cudaSuccess; ++it) {
+                const size_t i = (size_t)s * XF_ITEMS + it;
+                if (rbytes[i])
+                    e = cudaMemcpyPeerAsync(rp[i], ix->device, g->table[s][(size_t)me * XF_ITEMS + it], g->dev[s], rbytes[i],
+                                            st.s);
+            }
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st.s);
+        // the senders' arrays and tables are read until every receiver is past this barrier
+        const bool ok = g->barrier(true);
+        if (e != cudaSuccess) return pb_fail(PB_ERR_CUDA, "rebalance peer copy failed: %s", cudaGetErrorString(e));
+        if (!ok) return pb_fail(PB_ERR_COMM, "shard group: a peer failed");
+        return PB_OK;
+    };
+    // the receiver's new doc_off / udoc_off (scans of the arrived lengths), inverted file and norms
+    auto build = [&]() -> pb_status {
+        const long long D1 = p.D1;
+        DevBuf tmp, len;
+        CK(cudaMemset(p.rlen.as<long long>() + D1, 0, 8));
+        CK(cudaMemset(p.rulen.as<long long>() + D1, 0, 8));
+        CKS(exclusive_sum(p.rlen.as<long long>(), p.doc_off.as<long long>(), D1 + 1, tmp));
+        CKS(exclusive_sum(p.rulen.as<long long>(), p.udoc_off.as<long long>(), D1 + 1, tmp));
+        std::vector<long long> hoff((size_t)D1 + 1);
+        long long u1 = 0, l1 = 0;
+        CK(cudaMemcpy(hoff.data(), p.doc_off.p, hoff.size() * 8, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(&u1, p.udoc_off.as<long long>() + D1, 8, cudaMemcpyDeviceToHost));
+        p.maxlen = 0;
+        for (long long j = 0; j < D1; ++j) p.maxlen = std::max<int>(p.maxlen, (int)(hoff[j + 1] - hoff[j]));
+        CKS(len.ensure((size_t)(K + 1) * 8));
+        k_ivf_rebalance_count<<<(unsigned)((K + 256) / 256), 256>>>(p.seg_off.as<long long>(), W, K, len.as<long long>());
+        CK(cudaGetLastError());
+        CKS(exclusive_sum(len.as<long long>(), p.ivf_off.as<long long>(), K + 1, tmp));
+        CK(cudaMemcpy(&l1, p.ivf_off.as<long long>() + K, 8, cudaMemcpyDeviceToHost));
+        if (hoff[D1] != p.N1 || u1 != p.U1 || l1 != p.L1)
+            return pb_fail(PB_ERR_CUDA, "the received pieces (%lld tokens, %lld codes, %lld ivf entries) differ from the "
+                           "plan (%lld, %lld, %lld)", hoff[D1], u1, l1, p.N1, p.U1, p.L1);
+        if (p.L1 > 0)
+            k_ivf_rebalance_merge<<<grid, 256>>>(p.seg.as<uint32_t>(), p.seg_off.as<long long>(), p.meta.as<long long>(),
+                                                 p.meta.as<long long>() + W, W, K, p.ivf_off.as<long long>(),
+                                                 p.ivf.as<uint32_t>());
+        CK(cudaGetLastError());
+        // 1 / |c + w| of the new tokens and vmin / wmax over them, as an open computes them
+        if (filter_dim(ix->dim) && p.N1 > 0) {
+            if (ix->N == 0) CKS(build_centroid_operands(ix));  // a rank opened empty has none yet
+            const float init[2] = {3.0e38f, 0.0f};
+            CK(cudaMemcpy(p.mn.p, init, 8, cudaMemcpyHostToDevice));
+            CKS(launch_min_vnorm(ix, p.codes.as<uint32_t>(), p.residuals.as<uint8_t>(), p.N1, p.tok_inv_norm.as<float>(),
+                                 p.mn.as<float>()));
+            float got[2] = {0.f, 0.f};
+            CK(cudaMemcpy(got, p.mn.p, 8, cudaMemcpyDeviceToHost));
+            p.vmin = got[0] < 1e30f ? got[0] : 0.0f;
+            p.wmax = got[1];
+        }
+        CK(cudaDeviceSynchronize());
+        return PB_OK;
+    };
+    long long fin = transfer();
+    if (fin == PB_OK && changes) fin = build();
+
+    // 6. the last vote covers the transfer and the build; then every rank swaps in its new arrays, which cannot fail
+    CKS(gather_words(ix, &fin, 1, votes, true));
+    CKS(first_failure(ix, votes, 1, " moving the documents; nothing changed"));
+    if (changes) {
+        ix->codes.swap(p.codes);
+        ix->residuals.swap(p.residuals);
+        ix->ucodes.swap(p.ucodes);
+        ix->doc_off.swap(p.doc_off);
+        ix->udoc_off.swap(p.udoc_off);
+        ix->ivf.swap(p.ivf);
+        ix->ivf_off.swap(p.ivf_off);
+        ix->ivf_spare.swap(p.ivf_spare);
+        ix->tok_inv_norm.swap(p.tok_inv_norm);
+        ix->D = p.D1;
+        ix->N = p.N1;
+        ix->doc_id_base = b[me];
+        ix->ivf_len = p.L1;
+        ix->n_ucodes = p.U1;
+        ix->max_doclen = p.maxlen;
+        ix->vmin = p.vmin;
+        ix->wmax = p.wmax;
+    }
+    if (out_bounds) std::copy(b.begin(), b.end(), out_bounds);
+    return PB_OK;  // the old arrays are freed with p
 }
 
 extern "C" pb_status pb_last_delete_ms(pb_index *ix, float *out_ms) {

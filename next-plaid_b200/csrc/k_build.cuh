@@ -790,6 +790,103 @@ __global__ void k_compact_gather(const uint8_t *__restrict__ src, const long lon
     }
 }
 
+// ------------------------------------------------------------------------------------------
+// Rebalance of a doc-sharded deployment (pb_index_rebalance_sharded).  A sender's local ids [0, D) split into W
+// destination pieces by the bounds q [W + 1] (q[0] = 0, q[W] = D, non-decreasing; piece r = ids [q[r], q[r + 1])).
+// Each list is partitioned stably: per 32 entries the lanes bound for one piece form a __match_any_sync group whose
+// lowest lane owns that piece's counter / cursor.  cnt and cur are [W][K + 1], entry r (K + 1) + c for piece r and
+// centroid c; one warp per centroid, so neither needs atomics.  cnt[r (K + 1) + K] stays 0, so one exclusive scan of
+// cnt gives every piece's list offsets in one buffer, the pieces in destination order.
+// ------------------------------------------------------------------------------------------
+// the piece of local id `id`: the last r with q[r] <= id (empty pieces have q[r] = q[r + 1] and are skipped)
+__device__ __forceinline__ int split_piece(const long long *__restrict__ q, int W, uint32_t id) {
+    int lo = 0, hi = W - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (q[mid] <= (long long)id) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
+// cnt[r (K + 1) + c] += entries of list c bound for piece r (cnt zeroed by the caller)
+__global__ void k_ivf_split_count(const uint32_t *__restrict__ ivf, const long long *__restrict__ off, long long K,
+                                  const long long *__restrict__ q, int W, long long *__restrict__ cnt) {
+    const int lane = threadIdx.x & 31;
+    const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
+    for (long long c = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c < K; c += nw) {
+        const long long o0 = off[c], n = off[c + 1] - o0;
+        for (long long b = 0; b < n; b += 32) {
+            const long long i = b + lane;
+            const int r = i < n ? split_piece(q, W, ivf[o0 + i]) : W;
+            const unsigned same = __match_any_sync(PB_FULL, r);
+            if (r < W && lane == __ffs(same) - 1) cnt[r * (K + 1) + c] += __popc(same);
+        }
+    }
+}
+
+// the entries of list c bound for piece r, in list order, at cur[r (K + 1) + c].., as id - q[r]; cur advances
+__global__ void k_ivf_split_write(const uint32_t *__restrict__ ivf, const long long *__restrict__ off, long long K,
+                                  const long long *__restrict__ q, int W, long long *__restrict__ cur,
+                                  uint32_t *__restrict__ out) {
+    const int lane = threadIdx.x & 31;
+    const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
+    for (long long c = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c < K; c += nw) {
+        const long long o0 = off[c], n = off[c + 1] - o0;
+        for (long long b = 0; b < n; b += 32) {
+            const long long i = b + lane;
+            const uint32_t id = i < n ? ivf[o0 + i] : 0u;
+            const int r = i < n ? split_piece(q, W, id) : W;
+            const unsigned same = __match_any_sync(PB_FULL, r);
+            const int leader = __ffs(same) - 1;
+            long long base = 0;
+            if (r < W && lane == leader) base = cur[r * (K + 1) + c];
+            base = __shfl_sync(PB_FULL, base, leader);
+            if (r < W) out[base + __popc(same & ((1u << lane) - 1u))] = id - (uint32_t)q[r];
+            if (r < W && lane == leader) cur[r * (K + 1) + c] = base + __popc(same);
+        }
+    }
+}
+
+// Receiver side.  O [W][K + 1] holds each source's piece offsets as its sender scanned them (zeros for a source that
+// sends nothing); source s's entries arrived at seg[segbase[s]..].  len[c] = the new length of list c (len[K] = 0), the
+// sum over the sources, scanned by the caller into new_off.
+__global__ void k_ivf_rebalance_count(const long long *__restrict__ O, int W, long long K, long long *__restrict__ len) {
+    for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c <= K; c += (long long)gridDim.x * blockDim.x) {
+        long long n = 0;
+        if (c < K)
+            for (int s = 0; s < W; ++s) n += O[s * (K + 1) + c + 1] - O[s * (K + 1) + c];
+        len[c] = n;
+    }
+}
+
+// new list c = the sources' segments of list c concatenated in source order, ids + idoff[s] (the piece's first doc in
+// the receiver's range).  One warp per centroid, coalesced on both sides.
+__global__ void k_ivf_rebalance_merge(const uint32_t *__restrict__ seg, const long long *__restrict__ O,
+                                      const long long *__restrict__ segbase, const long long *__restrict__ idoff, int W,
+                                      long long K, const long long *__restrict__ new_off, uint32_t *__restrict__ out) {
+    const int lane = threadIdx.x & 31;
+    const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
+    for (long long c = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c < K; c += nw) {
+        long long dst = new_off[c];
+        for (int s = 0; s < W; ++s) {
+            const long long *o = O + s * (K + 1);
+            const long long src = segbase[s] + o[c] - o[0], n = o[c + 1] - o[c];
+            const uint32_t add = (uint32_t)idoff[s];
+            for (long long j = lane; j < n; j += 32) out[dst + j] = seg[src + j] + add;
+            dst += n;
+        }
+    }
+}
+
+// tlen[d] / ulen[d]: the tokens and distinct-code entries of doc d, the per-doc rows a rebalance moves with the doc
+__global__ void k_doc_lengths(const long long *__restrict__ doc_off, const long long *__restrict__ udoc_off, long long D,
+                              long long *__restrict__ tlen, long long *__restrict__ ulen) {
+    for (long long d = (long long)blockIdx.x * blockDim.x + threadIdx.x; d < D; d += (long long)gridDim.x * blockDim.x) {
+        tlen[d] = doc_off[d + 1] - doc_off[d];
+        ulen[d] = udoc_off[d + 1] - udoc_off[d];
+    }
+}
+
 // codec training (index.rs:240-258): L2 norm of every residual row; per-dimension mean of |residual|
 __global__ void k_residual_stats(const float *__restrict__ R, long long n, int dim, float *__restrict__ norms) {
     const int lane = threadIdx.x & 31;

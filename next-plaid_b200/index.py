@@ -87,6 +87,7 @@ EXPORTS = [
     "pb_index_append", "pb_index_append_encoded", "pb_index_reserve",
     "pb_index_delete", "pb_last_delete_ms", "pb_index_load_range", "pb_index_dir_shard_bounds",
     "pb_index_delete_sharded", "pb_index_append_sharded", "pb_index_append_encoded_sharded",
+    "pb_index_rebalance_sharded",
 ]
 
 _lib = None
@@ -183,6 +184,7 @@ def load_library():
         L.pb_index_delete_sharded.argtypes = L.pb_index_delete.argtypes
         L.pb_index_append_sharded.argtypes = L.pb_index_append.argtypes
         L.pb_index_append_encoded_sharded.argtypes = L.pb_index_append_encoded.argtypes
+        L.pb_index_rebalance_sharded.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 
@@ -209,6 +211,7 @@ class ShardGroup:
         self._g = h
         for r, s in enumerate(self.shards):
             _check(load_library().pb_index_group_join(s._h, self._g, r))
+            s._world = len(self.shards)
         self.all_results = None
 
     def _collective(self, call):
@@ -286,6 +289,12 @@ class ShardGroup:
             return first.value
         first = self._collective(call)[0]
         return list(range(first, first + len(dl)))
+
+    def rebalance(self, bounds: Optional[Sequence[int]] = None) -> np.ndarray:
+        """pb_index_rebalance_sharded: rank r takes documents [bounds[r], bounds[r + 1]) of the deployment (None: the
+        token-balanced split), moving them between the ranks on the device; global ids and search results do not
+        change.  Returns the bounds applied."""
+        return self._collective(lambda r, s: s.rebalance_sharded(bounds))[0]
 
     def close(self):
         for s in self.shards:
@@ -367,6 +376,7 @@ class MmapIndex:
     def __init__(self, handle: int, path: str = ""):
         self._h = C.c_void_p(handle)
         self.path = path
+        self._world = 1           # ranks of the doc-sharded deployment it joined (comm_init / ShardGroup)
 
     # -- construction ----------------------------------------------------------------------
     @classmethod
@@ -590,6 +600,20 @@ class MmapIndex:
         buf = np.frombuffer(bytes(unique_id), np.uint8).copy()
         assert buf.size == 128
         _check(load_library().pb_index_comm_init(self._h, _ptr(buf), rank, world))
+        self._world = world
+
+    def rebalance_sharded(self, bounds: Optional[Sequence[int]] = None) -> np.ndarray:
+        """pb_index_rebalance_sharded, this rank's part of the collective: every rank calls it with the same `bounds`
+        ([world + 1] document bounds, or None for the token-balanced split).  Returns the bounds applied."""
+        W = self._world
+        b = None
+        if bounds is not None:
+            b = np.ascontiguousarray(bounds, np.int64).reshape(-1)
+            if b.size != W + 1:
+                raise PlaidError(PB_ERR_INVALID, f"bounds has {b.size} entries, the deployment needs {W + 1}")
+        out = np.zeros(W + 1, np.int64)
+        _check(load_library().pb_index_rebalance_sharded(self._h, _ptr(b), _ptr(out)))
+        return out
 
     # -- measurement hooks -------------------------------------------------------------------------
     def set_fast_approx(self, mode):

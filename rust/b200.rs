@@ -79,6 +79,7 @@ extern "C" {
     fn pb_index_append_encoded_sharded(ix: *mut c_void, codes: *const i64, residuals: *const u8,
                                        doc_lengths: *const i64, n_docs: i64, memory_space: i32,
                                        out_first_doc_id: *mut i64) -> c_int;
+    fn pb_index_rebalance_sharded(ix: *mut c_void, bounds: *const i64, out_bounds: *mut i64) -> c_int;
 }
 
 fn last_error() -> String {
@@ -213,6 +214,26 @@ impl B200Index {
         batch_size: usize,
     ) -> Result<Vec<i64>> {
         self.append_with(embeddings, index_path, codec, batch_size, true)
+    }
+
+    /// Rebalance a doc-sharded deployment of `world` ranks in place (`pb_index_rebalance_sharded`): every rank calls it
+    /// with the same `bounds` ([world + 1] document bounds, or None for the token-balanced split), at the same point of
+    /// its sequence of collective calls.  Documents move between the ranks on the device; global ids, search results
+    /// and the index directory do not change.  Returns the bounds applied.  A failure leaves every rank as it was.
+    pub fn rebalance_sharded(&self, bounds: Option<&[i64]>, world: usize) -> Result<Vec<i64>> {
+        if let Some(b) = bounds {
+            if b.len() != world + 1 {
+                return Err(Error::Shape(format!("bounds has {} entries, the deployment needs {}", b.len(), world + 1)));
+            }
+        }
+        let mut out = vec![0i64; world + 1];
+        let st = unsafe {
+            pb_index_rebalance_sharded(self.handle, bounds.map_or(std::ptr::null(), |b| b.as_ptr()), out.as_mut_ptr())
+        };
+        if st != 0 {
+            return Err(Error::IndexLoad(last_error()));
+        }
+        Ok(out)
     }
 
     fn append_with(
