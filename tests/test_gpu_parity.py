@@ -120,7 +120,7 @@ def test_ragged_query_lengths_and_small_dims(oracle, npb):
         ix = oracle.create_index(docs, nbits=nbits, seed=1, num_partitions=64)
         gpu = _gpu_index(npb, ix)
         qs = []
-        for nq, seed in ((1, 1), (5, 2), (32, 3), (33, 4), (48, 5), (70, 6)):
+        for nq, seed in ((1, 1), (5, 2), (32, 3), (33, 4), (48, 5), (70, 6), (129, 7), (257, 8)):
             qs.append(oracle.synthetic_queries(docs, 1, nq=nq, seed=seed)[0][0])
         qs.append(np.zeros((0, dim), np.float32))       # empty query -> empty result
         pg, po = _params(npb, oracle, top_k=7, n_ivf_probe=4, n_full_scores=64, centroid_score_threshold=0.3)
