@@ -79,8 +79,15 @@ typedef struct pb_index_desc {
  * ADOPT_RESIDUALS: memory_space must be PB_MEM_DEVICE; the packed residuals (the largest array: 19 GB per million
  *   300-token docs at 4 bits) are used in place instead of copied -- the caller keeps them alive until pb_index_close.
  * ivf == NULL && ivf_lengths == NULL (no flag needed): the inverted file is built on the device from the codes,
- *   exactly as index.rs:850-873 does (per centroid the ascending unique doc ids); pb_index_export_ivf returns it. */
-enum { PB_OPEN_ADOPT_RESIDUALS = 1 };
+ *   exactly as index.rs:850-873 does (per centroid the ascending unique doc ids); pb_index_export_ivf returns it.
+ * HOST_RESIDUALS: the packed residuals (host or device memory_space) are copied into library-owned pinned host memory,
+ *   mapped and portable, instead of device memory; every other array stays on the device.  Each search stages the rows
+ *   of the documents its cut keeps into a device buffer of its workspace (DESIGN.md 4j), so results, counts and
+ *   pb_work_counters equal those of a handle opened without the flag; searches are slower, by the PCIe transfer.  At
+ *   4 bits and dim 128 that leaves about 11 of 75 device bytes per token.  With ADOPT_RESIDUALS: PB_ERR_INVALID.  A
+ *   failed pinned allocation: PB_ERR_NOMEM, nothing allocated.  Appends, deletes, pb_index_reserve and the sharded
+ *   mutations and rebalance refuse such handles with PB_ERR_UNSUPPORTED, as they refuse ADOPT_RESIDUALS. */
+enum { PB_OPEN_ADOPT_RESIDUALS = 1, PB_OPEN_HOST_RESIDUALS = 2 };
 
 /* search.rs:27-69 SearchParameters.  batch_size is accepted and ignored, as in the reference
  * (it is never read there). */
@@ -119,6 +126,11 @@ PB_API pb_status pb_index_load(const char *index_dir, int32_t device, pb_index *
  * PB_ERR_INVALID before the device is touched: doc_begin < 0, doc_end < doc_begin, doc_end > D. */
 PB_API pb_status pb_index_load_range(const char *index_dir, int32_t device, int64_t doc_begin, int64_t doc_end,
                                      pb_index **out);
+/* pb_index_load_range with pb_index_desc.flags (PB_OPEN_HOST_RESIDUALS: each chunk's rows go from the file mapping
+ * straight into the pinned host buffer).  pb_index_load and pb_index_load_range are this call with flags = 0; doc_end < 0
+ * stands for every document. */
+PB_API pb_status pb_index_load_range_flags(const char *index_dir, int32_t device, int64_t doc_begin, int64_t doc_end,
+                                           int32_t flags, pb_index **out);
 
 /* Token-balanced contiguous split of the directory's D documents over `world` ranks (host only, reads metadata.json
  * and the doclens files): out_bounds[0] = 0, out_bounds[world] = D, and for 0 < r < world
@@ -145,6 +157,10 @@ PB_API double pb_index_avg_doclen(const pb_index *ix);
 PB_API int32_t pb_index_embedding_dim(const pb_index *ix);
 PB_API int32_t pb_index_nbits(const pb_index *ix);
 PB_API int32_t pb_index_device(const pb_index *ix);
+/* Bytes the handle's index arrays hold (allocated capacity; per-call workspaces and a caller's adopted residual array not
+ * counted): *device_bytes on its device, *host_bytes in pinned host memory (N * dim * nbits / 8 with
+ * PB_OPEN_HOST_RESIDUALS, else 0).  Either may be NULL. */
+PB_API pb_status pb_index_memory(const pb_index *ix, int64_t *device_bytes, int64_t *host_bytes);
 
 /* ---- incremental append ------------------------------------------------------------------ */
 
@@ -427,6 +443,11 @@ typedef struct pb_work_counters {
     int64_t filter_diag_pairs;   /* PB_FILTER_DIAG=1 only: (kept doc, query token) maxima compared for filter_err_ratio_e6 */
 } pb_work_counters;
 PB_API pb_status pb_last_work_counters(pb_index *ix, pb_work_counters *out);
+/* What the calling thread's last search staged from host memory (PB_OPEN_HOST_RESIDUALS; 0 otherwise): the kept docs of
+ * every sub-batch (a doc kept by several queries counts once per query), their residual bytes, and with
+ * pb_set_profiling(ix, 1) the device time of the layout and gather kernels (part of PB_STAGE_EXACT).  Any pointer may be
+ * NULL. */
+PB_API pb_status pb_last_staging_stats(pb_index *ix, int64_t *docs, int64_t *bytes, float *ms);
 
 /* Search with queries already resident on the device and results left on the device:
  * the kernel-only timing leg of bench.py ("value"); same semantics as pb_search_batch. */

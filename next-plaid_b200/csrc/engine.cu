@@ -284,6 +284,35 @@ struct HostBuf {  // pinned
     }
 };
 
+// the packed residuals of a PB_OPEN_HOST_RESIDUALS handle: pinned, mapped and portable host memory; dev is the address
+// kernels read it at
+struct PinnedRes {
+    uint8_t *p = nullptr, *dev = nullptr;
+    size_t bytes = 0;
+    pb_status alloc(size_t n) {
+        if (n == 0) return PB_OK;
+        void *h = nullptr;
+        cudaError_t e = cudaHostAlloc(&h, n, cudaHostAllocMapped | cudaHostAllocPortable);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return pb_fail(PB_ERR_NOMEM, "cudaHostAlloc(%zu bytes, mapped) failed: %s", n, cudaGetErrorString(e));
+        }
+        void *d = nullptr;
+        e = cudaHostGetDevicePointer(&d, h, 0);
+        if (e != cudaSuccess) {
+            cudaFreeHost(h);
+            return pb_fail(PB_ERR_CUDA, "cudaHostGetDevicePointer failed: %s", cudaGetErrorString(e));
+        }
+        p = static_cast<uint8_t *>(h);
+        dev = static_cast<uint8_t *>(d);
+        bytes = n;
+        return PB_OK;
+    }
+    ~PinnedRes() {
+        if (p) cudaFreeHost(p);
+    }
+};
+
 // per-call scratch; a pool of these makes pb_search_batch re-entrant on one handle
 struct Workspace {
     cudaStream_t stream = nullptr;
@@ -293,12 +322,16 @@ struct Workspace {
     DevBuf Q, qoff, ST, partial, sel, cells, ncells, bitmap, cand, ncand, approx, keys, kept, nkept, tokp, maxkey,
         exact, fkeys, oids, oscores, ocounts, subset, subset_bits, elig, misc, list, counters, lkeys, ST16, qrange, qflag, lsum, cand2, ncand2,  cellbits,
         gkeys, krank, payload, gfkeys, gpayload, cmax16, tau16, plist, pcount, Qi, Qh16t, Ql16t, ST16b, k1diag, k1rows, ulist, nulist, est, kept2, krank2, nkept2, tokp2, ktok2, qnmax, qexp, qrange_tc, mslot, slicecnt, rcmax, rcpairs, rcn, cellflags, estkey, srcrank, xpairs, xnpairs, needexact, gbase, fdiag;
+    // host tier: the staged rows of the kept docs (residuals, codes, 1 / |v|), their slot offsets and slot list
+    DevBuf s_res, s_codes, s_inv, soff, kept_s;
+    cudaEvent_t sev[2] = {};  // around the staging kernels
     HostBuf hq, hres, hcounts;
     pb_status init() {
         CK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
         for (auto &e : ev) CK(cudaEventCreate(&e));
         for (auto &e : kev) CK(cudaEventCreate(&e));
         for (auto &e : call_ev) CK(cudaEventCreate(&e));
+        for (auto &e : sev) CK(cudaEventCreate(&e));
         bitmap.zero_on_grow = true;
         maxkey.zero_on_grow = true;
         subset_bits.zero_on_grow = true;
@@ -314,6 +347,8 @@ struct Workspace {
             if (e) cudaEventDestroy(e);
         for (auto &e : call_ev)
             if (e) cudaEventDestroy(e);
+        for (auto &e : sev)
+            if (e) cudaEventDestroy(e);
         if (stream) cudaStreamDestroy(stream);
     }
 };
@@ -325,6 +360,8 @@ struct Stats {
     float call_ms = 0.f;
     int launches[PB_STAGE_COUNT] = {};
     pb_work_counters work = {};
+    long long staged_docs = 0, staged_bytes = 0;  // host tier: pb_last_staging_stats
+    float staging_ms = 0.f;
 };
 static thread_local Stats g_stats;
 static thread_local int g_budget_div = 1;  // lanes of the current call share the workspace budget
@@ -381,6 +418,8 @@ struct pb_index {
     int max_doclen = 0;
     int sm_count = 132;
     DevBuf centroids, w_rev, codes, residuals, doc_off, ivf, ivf_off, ucodes, udoc_off;
+    bool host_tier = false;    // PB_OPEN_HOST_RESIDUALS: `residuals` stays empty, the rows live in host_res
+    PinnedRes host_res;
     long long n_ucodes = 0;
     bool build_ivf = false;    // no inverted file was given: built from the codes at finalize (index.rs:850-873)
     float cmax = 1.0f;         // largest centroid L2 norm (range of the 16-bit score table)
@@ -666,6 +705,10 @@ pb_status pb_index_upload_tokens(pb_index *ix, long long tok_off, const int64_t 
     if (!ix->residuals.owned) {  // PB_OPEN_ADOPT_RESIDUALS: the caller's array is the index
         if (tok_off != 0 || n != ix->N || residuals != ix->residuals.as<uint8_t>())
             return pb_fail(PB_ERR_INVALID, "adopted residuals cover the whole index");
+    } else if (ix->host_tier) {
+        uint8_t *dst = ix->host_res.p + (size_t)tok_off * ix->packed;
+        if (space == PB_MEM_DEVICE) CK(cudaMemcpy(dst, residuals, (size_t)n * ix->packed, cudaMemcpyDeviceToHost));
+        else memcpy(dst, residuals, (size_t)n * ix->packed);
     } else
         CK(cudaMemcpy(ix->residuals.as<uint8_t>() + (size_t)tok_off * ix->packed, residuals, (size_t)n * ix->packed,
                       space == PB_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
@@ -691,6 +734,8 @@ pb_status pb_index_open_begin(const pb_index_desc *d, pb_index **out) {
         return pb_fail(PB_ERR_INVALID, "null index array");
     if ((d->flags & PB_OPEN_ADOPT_RESIDUALS) && (d->memory_space != PB_MEM_DEVICE || !d->residuals))
         return pb_fail(PB_ERR_INVALID, "PB_OPEN_ADOPT_RESIDUALS needs device-resident residuals");
+    if ((d->flags & PB_OPEN_ADOPT_RESIDUALS) && (d->flags & PB_OPEN_HOST_RESIDUALS))
+        return pb_fail(PB_ERR_INVALID, "PB_OPEN_ADOPT_RESIDUALS and PB_OPEN_HOST_RESIDUALS exclude each other");
     CKS(check_device(d->device));
     std::unique_ptr<pb_index> ix(new pb_index());
     ix->device = d->device;
@@ -746,8 +791,10 @@ pb_status pb_index_open_begin(const pb_index_desc *d, pb_index **out) {
     for (unsigned f = 0; f < (1u << ix->nbits); ++f) wrev[f] = w[bitrev_n(f, ix->nbits)];
     CKS(upload(ix->w_rev, wrev.data(), 256 * sizeof(float), PB_MEM_HOST));
     CKS(upload(ix->centroids, d->centroids, (size_t)ix->K * ix->dim * sizeof(float), sp));
+    ix->host_tier = (d->flags & PB_OPEN_HOST_RESIDUALS) != 0;
     if (d->flags & PB_OPEN_ADOPT_RESIDUALS)
         ix->residuals.adopt(const_cast<uint8_t *>(d->residuals), (size_t)ix->N * ix->packed);
+    else if (ix->host_tier) CKS(ix->host_res.alloc((size_t)ix->N * ix->packed));
     else CKS(ix->residuals.ensure(std::max<size_t>((size_t)ix->N * ix->packed, 16)));
     CKS(ix->codes.ensure(std::max<size_t>((size_t)ix->N * 4, 16)));
     if (!ix->build_ivf) {
@@ -842,10 +889,23 @@ static pb_status launch_min_vnorm(pb_index *ix, const uint32_t *codes, const uin
     CK(cudaGetLastError());
     return PB_OK;
 }
-// the same for the handle's tokens [t0, t0 + n), into its tok_inv_norm
+// the same for the handle's tokens [t0, t0 + n), into its tok_inv_norm.  A host-tier handle's rows go through a device
+// buffer in slabs of 2^22 tokens; the per-token values and the folded min / max do not depend on the slabs, so they are
+// bit-identical to a resident open's (the filter's certificate rests on them)
 static pb_status launch_min_vnorm(pb_index *ix, long long t0, long long n, float *mn) {
-    return launch_min_vnorm(ix, ix->codes.as<uint32_t>() + t0, ix->residuals.as<uint8_t>() + (size_t)t0 * ix->packed, n,
-                            ix->tok_inv_norm.as<float>() + t0, mn);
+    if (!ix->host_tier)
+        return launch_min_vnorm(ix, ix->codes.as<uint32_t>() + t0, ix->residuals.as<uint8_t>() + (size_t)t0 * ix->packed, n,
+                                ix->tok_inv_norm.as<float>() + t0, mn);
+    const long long slab = 1ll << 22;
+    DevBuf st;
+    CKS(st.ensure((size_t)std::min(n, slab) * ix->packed + 16));
+    for (long long o = t0; o < t0 + n; o += slab) {
+        const long long m = std::min(slab, t0 + n - o);
+        CK(cudaMemcpy(st.p, ix->host_res.p + (size_t)o * ix->packed, (size_t)m * ix->packed, cudaMemcpyHostToDevice));
+        CKS(launch_min_vnorm(ix, ix->codes.as<uint32_t>() + o, st.as<uint8_t>(), m, ix->tok_inv_norm.as<float>() + o, mn));
+    }
+    CK(cudaDeviceSynchronize());
+    return PB_OK;
 }
 
 // Derived arrays that need every token: the per-doc distinct-code lists k_approx walks.
@@ -979,6 +1039,19 @@ extern "C" int32_t pb_index_embedding_dim(const pb_index *ix) { return ix ? ix->
 extern "C" int32_t pb_index_nbits(const pb_index *ix) { return ix ? ix->nbits : 0; }
 extern "C" int32_t pb_index_device(const pb_index *ix) { return ix ? ix->device : -1; }
 
+extern "C" pb_status pb_index_memory(const pb_index *ix, int64_t *device_bytes, int64_t *host_bytes) {
+    if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    auto rd = ix->read_lock();
+    size_t dev = 0;
+    for (const DevBuf *b : {&ix->centroids, &ix->w_rev, &ix->codes, &ix->residuals, &ix->doc_off, &ix->ivf, &ix->ivf_off,
+                            &ix->ucodes, &ix->udoc_off, &ix->cent_h16t, &ix->cent_l16t, &ix->centroids_f16,
+                            &ix->tok_inv_norm, &ix->ivf_spare, &ix->ivf_off_spare})
+        if (b->owned) dev += b->cap;  // adopted residuals are the caller's allocation
+    if (device_bytes) *device_bytes = (int64_t)dev;
+    if (host_bytes) *host_bytes = (int64_t)ix->host_res.bytes;
+    return PB_OK;
+}
+
 extern "C" void pb_search_params_default(pb_search_params *p) {  // search.rs:58-69
     if (!p) return;
     p->batch_size = 2000;
@@ -1026,6 +1099,12 @@ extern "C" pb_status pb_last_kernel_ms(pb_index *, float *out_ms) {
 extern "C" pb_status pb_last_work_counters(pb_index *, pb_work_counters *out) {
     if (!out) return pb_fail(PB_ERR_INVALID, "null argument");
     *out = g_stats.work;
+    return PB_OK;
+}
+extern "C" pb_status pb_last_staging_stats(pb_index *, int64_t *docs, int64_t *bytes, float *ms) {
+    if (docs) *docs = g_stats.staged_docs;
+    if (bytes) *bytes = g_stats.staged_bytes;
+    if (ms) *ms = g_stats.staging_ms;
     return PB_OK;
 }
 
@@ -1252,8 +1331,21 @@ struct KeptView {  // the docs the exact stage scores: the cut's output, or the 
     uint32_t *krank;  // global approximate rank (sharded) or nullptr
 };
 
-static pb_status launch_exact(pb_index *ix, Workspace &ws, const KeptView &kv, int B, int QS, int Mcap, int kept_shared,
-                              long long max_tokens, int *launches, const int *only_flagged = nullptr, bool timed = true) {
+// The token arrays the exact stage reads: the handle's own, or (host tier) a staged copy whose doc_off is indexed by the
+// slots the kept lists then hold (k_stage.cuh)
+struct TokView {
+    const uint32_t *codes;
+    const uint8_t *residuals;
+    const float *inv_norm;
+    const long long *doc_off;
+};
+static TokView resident_tokens(const pb_index *ix) {
+    return {ix->codes.as<uint32_t>(), ix->residuals.as<uint8_t>(), ix->tok_inv_norm.as<float>(), ix->doc_off.as<long long>()};
+}
+
+static pb_status launch_exact(pb_index *ix, Workspace &ws, const KeptView &kv, const TokView &tv, int B, int QS, int Mcap,
+                              int kept_shared, long long max_tokens, int *launches, const int *only_flagged = nullptr,
+                              bool timed = true) {
     // each CTA owns a contiguous range of chunks; aim for 8 waves of 2 CTAs/SM over the whole grid
     long long chunks = (max_tokens + PB_TOK_TILE - 1) / PB_TOK_TILE;
     long long want = std::max<long long>(1, ((long long)ix->sm_count * 16 + B - 1) / B);
@@ -1264,7 +1356,7 @@ static pb_status launch_exact(pb_index *ix, Workspace &ws, const KeptView &kv, i
         if (timed) KEV_BEGIN(PB_KERNEL_EXACT);
         kern<<<dim3(gx, B), 128, smem_exact(DIM, ix->packed), ws.stream>>>(
             ws.Q.as<float>(), ws.qoff.as<int>(), QS, ix->centroids.as<float>(), ix->w_rev.as<float>(), ix->nbits,
-            ix->codes.as<uint32_t>(), ix->residuals.as<uint8_t>(), ix->doc_off.as<long long>(), nullptr,
+            tv.codes, tv.residuals, tv.doc_off, nullptr,
             kv.kept, kv.nkept, kv.tokp, Mcap, kept_shared, ws.maxkey.as<uint32_t>(), only_flagged);
         if (timed) KEV_END(PB_KERNEL_EXACT);
     });
@@ -1312,9 +1404,9 @@ static size_t smem_maxsim_tc(int dim, int packed, int nqt) {
 
 // the warp-specialised linear estimate over the docs of `in`: pass 1 (pairs == nullptr) leaves per (doc, q) maxima in
 // `keys`; pass 2 lists the (token, q) pairs within the certified band of the maxima `keys` holds at src_rank
-static pb_status launch_maxsim_tc(pb_index *ix, Workspace &ws, const KeptView &in, int B, int QS, int Mcap, long long max_tokens,
-                                  int nq_max, uint32_t *keys, const uint32_t *src_rank, float band_unit, u64 *pairs,
-                                  int *n_pairs, int pair_cap, int kev) {
+static pb_status launch_maxsim_tc(pb_index *ix, Workspace &ws, const KeptView &in, const TokView &tv, int B, int QS, int Mcap,
+                                  long long max_tokens, int nq_max, uint32_t *keys, const uint32_t *src_rank, float band_unit,
+                                  u64 *pairs, int *n_pairs, int pair_cap, int kev) {
     const bool emit = pairs != nullptr;
     // CTAs per SM over the batch: ws_grid for pass 1 (all kept docs), ws_grid2 for pass 2 (the survivors, ~1/10 of the
     // tokens; fewer, longer CTAs measured slower: the pass is latency-bound and wants the parallelism)
@@ -1324,7 +1416,7 @@ static pb_status launch_maxsim_tc(pb_index *ix, Workspace &ws, const KeptView &i
     const int nqt = nq_max <= 32 ? 32 : 64;
     const size_t sm = smem_maxsim_tc(ix->dim, ix->packed, nqt);
     CKS(ws.gbase.ensure((size_t)B * Mcap * 8));
-    k_doc_gbase<<<dim3((Mcap + 255) / 256, B), 256, 0, ws.stream>>>(in.kept, in.nkept, in.tokp, ix->doc_off.as<long long>(), Mcap,
+    k_doc_gbase<<<dim3((Mcap + 255) / 256, B), 256, 0, ws.stream>>>(in.kept, in.nkept, in.tokp, tv.doc_off, Mcap,
                                                                     ws.gbase.as<long long>());
     CK(cudaGetLastError());
 #define PB_MS_GO(DV, NB, NQ, EM)                                                                                       \
@@ -1335,8 +1427,8 @@ static pb_status launch_maxsim_tc(pb_index *ix, Workspace &ws, const KeptView &i
         kern<<<dim3(gx, B), 256, sm, ws.stream>>>(ws.Q.as<float>(), ws.qoff.as<int>(), QS, ws.qexp.as<int>(),            \
                                                   ws.ST16.as<unsigned short>(), ix->K, ws.qrange.as<float2>(),         \
                                                   ws.qflag.as<int>(), ix->w_rev.as<float>(),                           \
-                                                  ix->codes.as<uint32_t>(), ix->residuals.as<uint8_t>(),               \
-                                                  ix->tok_inv_norm.as<float>(), ws.gbase.as<long long>(),              \
+                                                  tv.codes, tv.residuals,                                              \
+                                                  tv.inv_norm, ws.gbase.as<long long>(),                               \
                                                   in.nkept, in.tokp, Mcap, keys, src_rank, ws.qnmax.as<float>(),       \
                                                   band_unit, pairs, n_pairs, pair_cap);                                \
         if (kev >= 0) KEV_END(kev);                                                                                    \
@@ -1368,9 +1460,9 @@ static pb_status launch_maxsim_tc(pb_index *ix, Workspace &ws, const KeptView &i
 }
 
 // a7': tensor-core estimate of every kept doc, then the survivors that can still reach the top_k
-static pb_status launch_filter(pb_index *ix, Workspace &ws, const KeptView &in, const KeptView &out, int B, int QS, int Mcap,
-                               int top_k, long long max_tokens, float eps_unit, int nq_max, bool linear, bool keep_keys,
-                               int *launches) {
+static pb_status launch_filter(pb_index *ix, Workspace &ws, const KeptView &in, const KeptView &out, const TokView &tv, int B,
+                               int QS, int Mcap, int top_k, long long max_tokens, float eps_unit, int nq_max, bool linear,
+                               bool keep_keys, int *launches) {
     long long chunks = (max_tokens + 127) / 128;
     long long want = std::max<long long>(1, ((long long)ix->sm_count * ix->xtc_grid + B - 1) / B);
     int gx = (int)std::max<long long>(1, std::min<long long>(chunks, want));
@@ -1380,7 +1472,7 @@ static pb_status launch_filter(pb_index *ix, Workspace &ws, const KeptView &in, 
     uint32_t *keys = keep_keys ? ws.estkey.as<uint32_t>() : ws.maxkey.as<uint32_t>();
     if (keep_keys) CK(cudaMemsetAsync(keys, 0, (size_t)B * Mcap * QS * 4, ws.stream));
     if (linear) {
-        CKS(launch_maxsim_tc(ix, ws, in, B, QS, Mcap, max_tokens, nq_max, keys, nullptr, 0.0f, nullptr, nullptr, 0,
+        CKS(launch_maxsim_tc(ix, ws, in, tv, B, QS, Mcap, max_tokens, nq_max, keys, nullptr, 0.0f, nullptr, nullptr, 0,
                              PB_KERNEL_FILTER));
     } else {
 #define PB_TC_LAUNCH(DV, NB)                                                                                           \
@@ -1390,8 +1482,8 @@ static pb_status launch_filter(pb_index *ix, Workspace &ws, const KeptView &in, 
         KEV_BEGIN(PB_KERNEL_FILTER);                                                                                   \
         kern<<<dim3(gx, B), 128, sm, ws.stream>>>(ws.Q.as<float>(), ws.qoff.as<int>(), QS, ws.qexp.as<int>(),          \
                                                   ix->centroids_f16.as<__half>(), ix->w_rev.as<float>(),               \
-                                                  ix->codes.as<uint32_t>(), ix->residuals.as<uint8_t>(),               \
-                                                  ix->doc_off.as<long long>(), in.kept, in.nkept, in.tokp, Mcap, keys); \
+                                                  tv.codes, tv.residuals,                                              \
+                                                  tv.doc_off, in.kept, in.nkept, in.tokp, Mcap, keys);                 \
         KEV_END(PB_KERNEL_FILTER);                                                                                     \
     }
 #define PB_TC_NBITS(DV)                                                                                                \
@@ -1418,7 +1510,7 @@ static pb_status launch_filter(pb_index *ix, Workspace &ws, const KeptView &in, 
     CKS(set_smem(k_tc_select, (size_t)Pm * 8));
     k_tc_select<<<B, 1024, (size_t)Pm * 8, ws.stream>>>(ws.est.as<float>(), in.kept, in.krank, in.nkept, Mcap, top_k,
                                                         ws.qoff.as<int>(), ws.qnmax.as<float>(), eps_unit,
-                                                        ix->doc_off.as<long long>(), out.kept, out.krank, out.nkept,
+                                                        tv.doc_off, out.kept, out.krank, out.nkept,
                                                         out.tokp, ws.ktok2.as<long long>(),
                                                         keep_keys ? ws.srcrank.as<uint32_t>() : nullptr);
     CK(cudaGetLastError());
@@ -1558,7 +1650,9 @@ static pb_status plan_probe(pb_index *ix, Workspace &ws, const pb_search_params 
         return pb_fail(PB_ERR_UNSUPPORTED, "num_centroids x query tokens x 4 = %zu bytes per query exceeds 2^32", per_q);
     // sub-batch size: the score tables (16-bit always, fp32 only on the exact path) and the per-(query, doc) scratch
     // (candidate lists, code sums, approximate scores, cut keys, bitmap: 24.2 bytes per document) share one budget
-    const size_t per_q_all = (size_t)ix->K * QS_all * (k1_tc_usable(ix) ? 2 : 6) + (size_t)ix->D * 24 + (size_t)ix->D / 8 + 4096;
+    // A host-tier handle also stages up to Mcap docs of max_doclen rows per query (residuals, codes, 1 / |v|)
+    const size_t per_q_all = (size_t)ix->K * QS_all * (k1_tc_usable(ix) ? 2 : 6) + (size_t)ix->D * 24 + (size_t)ix->D / 8 + 4096 +
+                             (ix->host_tier ? (size_t)plan.Mcap * std::max(ix->max_doclen, 1) * (ix->packed + 8) : 0);
     int QB = (int)std::max<size_t>(1, std::min<size_t>((size_t)Bt, ix->st_budget / std::max(g_budget_div, 1) / per_q_all));
     QB = std::min(QB, 256);
     plan.QB = (int)((Bt + (Bt + QB - 1) / QB - 1) / ((Bt + QB - 1) / QB));  // equal sub-batches
@@ -1858,6 +1952,52 @@ static pb_status cut(pb_index *ix, Workspace &ws, const SearchPlan &plan, const 
     return PB_OK;
 }
 
+// The rows of docs[s] for the slots s of [0, n_slots) (nkept != NULL: slot b Mcap + j only for j < nkept[b]) from the
+// pinned host residuals and the device codes / 1 / |v| into the workspace's staging buffers at soff[s]; cap_tok bounds
+// the staged tokens.  Returns the staged arrays as a TokView whose doc_off is soff (indexed by slot).
+static pb_status stage_rows(pb_index *ix, Workspace &ws, const uint32_t *docs, const int *nkept, int Mcap, long long n_slots,
+                            const long long *soff, long long cap_tok, TokView &tv) {
+    const int pk = ix->packed;
+    const bool inv = ix->tok_inv_norm.p != nullptr;
+    cap_tok = std::max(cap_tok, 1ll);
+    CKS(ws.s_res.ensure((size_t)cap_tok * pk));
+    CKS(ws.s_codes.ensure((size_t)cap_tok * 4));
+    if (inv) CKS(ws.s_inv.ensure((size_t)cap_tok * 4));
+    const int grid = ix->sm_count * 8;
+    const float *src_inv = inv ? ix->tok_inv_norm.as<float>() : nullptr;
+    float *dst_inv = inv ? ws.s_inv.as<float>() : nullptr;
+    if (pk % 16 == 0)
+        k_stage_rows<uint4, 4><<<grid, 256, 0, ws.stream>>>(docs, nkept, Mcap, n_slots, ix->doc_off.as<long long>(), soff,
+                                                            ix->host_res.dev, ix->codes.as<uint32_t>(), src_inv, pk,
+                                                            ws.s_res.as<uint8_t>(), ws.s_codes.as<uint32_t>(), dst_inv);
+    else
+        k_stage_rows<uint32_t, 8><<<grid, 256, 0, ws.stream>>>(docs, nkept, Mcap, n_slots, ix->doc_off.as<long long>(), soff,
+                                                               ix->host_res.dev, ix->codes.as<uint32_t>(), src_inv, pk,
+                                                               ws.s_res.as<uint8_t>(), ws.s_codes.as<uint32_t>(), dst_inv);
+    CK(cudaGetLastError());
+    tv = {ws.s_codes.as<uint32_t>(), ws.s_res.as<uint8_t>(), dst_inv, soff};
+    return PB_OK;
+}
+
+// Host tier, after the cut: the sub-batch's kept docs laid out in slot space and staged (k_stage.cuh).  kv then lists
+// slots, tv the staged arrays; the cut's own list (ws.kept) stays as it is, and the slots go back to doc ids before
+// k_exact_finalize.
+static pb_status stage_kept(pb_index *ix, Workspace &ws, const SearchPlan &plan, const Pass &pass, KeptView &kv, TokView &tv) {
+    const int B = pass.B, Mcap = plan.Mcap;
+    const long long slots = (long long)B * Mcap;
+    CKS(ws.soff.ensure((size_t)(slots + 1) * 8));
+    CKS(ws.kept_s.ensure((size_t)slots * 4));
+    if (plan.prof) CK(cudaEventRecord(ws.sev[0], ws.stream));
+    k_stage_layout<<<dim3(std::min((Mcap + 255) / 256, 8), B), 256, 0, ws.stream>>>(
+        kv.nkept, kv.tokp, B, Mcap, ws.soff.as<long long>(), ws.kept_s.as<uint32_t>());
+    CK(cudaGetLastError());
+    CKS(stage_rows(ix, ws, kv.kept, kv.nkept, Mcap, slots, ws.soff.as<long long>(), slots * std::max(ix->max_doclen, 1), tv));
+    if (plan.prof) CK(cudaEventRecord(ws.sev[1], ws.stream));
+    g_stats.launches[PB_STAGE_EXACT] += 2;
+    kv.kept = ws.kept_s.as<uint32_t>();
+    return PB_OK;
+}
+
 // a7 + a8: the exact MaxSim of the kept docs.  Only the top_k need exact scores: the tensor-core filter (a7') first
 // drops the docs that provably cannot reach them, and its pass 2 lists the (token, q) pairs k_pair_exact evaluates.
 static pb_status exact_scores(pb_index *ix, Workspace &ws, const SearchIO &io, const SearchPlan &plan, Pass &pass) {
@@ -1870,6 +2010,8 @@ static pb_status exact_scores(pb_index *ix, Workspace &ws, const SearchIO &io, c
     CKS(ws.fkeys.ensure((size_t)B * Mcap * 8));
     KeptView &kv = pass.kv;
     kv = {ws.kept.as<uint32_t>(), ws.nkept.as<int>(), ws.tokp.as<long long>(), sharded ? ws.krank.as<uint32_t>() : nullptr};
+    TokView tv = resident_tokens(ix);
+    if (ix->host_tier) CKS(stage_kept(ix, ws, plan, pass, kv, tv));
     // the linear form needs the 16-bit score table of this pass (a flagged query publishes no estimate and keeps
     // every doc); without a table (PB_FAST_APPROX=0) the decompressing form estimates from fp16 centroids
     const bool linear = pass.fast && !ix->filter_v1 && ix->tok_inv_norm.p;
@@ -1903,7 +2045,7 @@ static pb_status exact_scores(pb_index *ix, Workspace &ws, const SearchIO &io, c
             CKS(ws.estkey.ensure((size_t)B * Mcap * QS * 4));
             CKS(ws.srcrank.ensure((size_t)B * Mcap * 4));
         }
-        CKS(launch_filter(ix, ws, kv, kv2, B, QS, Mcap, plan.top_k, max_tokens, eps_unit, nq_max, linear,
+        CKS(launch_filter(ix, ws, kv, kv2, tv, B, QS, Mcap, plan.top_k, max_tokens, eps_unit, nq_max, linear,
                           pass.pairs || pass.diag, &L[PB_STAGE_EXACT]));
         if (!pass.diag) {
             kv = kv2;
@@ -1917,7 +2059,7 @@ static pb_status exact_scores(pb_index *ix, Workspace &ws, const SearchIO &io, c
         CKS(ws.needexact.ensure((size_t)B * 4 + 16));
         CK(cudaMemsetAsync(ws.xnpairs.p, 0, (size_t)B * 4, ws.stream));
         KEV_BEGIN(PB_KERNEL_EXACT);  // pass 2 + pair evaluation + the (normally empty) k_exact of flagged queries
-        CKS(launch_maxsim_tc(ix, ws, kv, B, QS, Mcap, max_tokens, nq_max, ws.estkey.as<uint32_t>(),
+        CKS(launch_maxsim_tc(ix, ws, kv, tv, B, QS, Mcap, max_tokens, nq_max, ws.estkey.as<uint32_t>(),
                              ws.srcrank.as<uint32_t>(), eps_unit, ws.xpairs.as<u64>(), ws.xnpairs.as<int>(), pair_cap, -1));
         k_pair_overflow<<<(B + 255) / 256, 256, 0, ws.stream>>>(ws.xnpairs.as<int>(), pair_cap, ws.qflag.as<int>(), B,
                                                                 ws.needexact.as<int>());
@@ -1930,8 +2072,8 @@ static pb_status exact_scores(pb_index *ix, Workspace &ws, const SearchIO &io, c
         CKS(set_smem(k_pair_exact<DV>, smp));                                                                          \
         k_pair_exact<DV><<<dim3(pe_ctas, B), 256, smp, ws.stream>>>(                                                   \
             ws.xpairs.as<u64>(), ws.xnpairs.as<int>(), pair_cap, ws.Q.as<float>(), ws.qoff.as<int>(), QS,              \
-            ix->centroids.as<float>(), ix->w_rev.as<float>(), ix->nbits, ix->codes.as<uint32_t>(),                     \
-            ix->residuals.as<uint8_t>(), Mcap, ws.maxkey.as<uint32_t>());                                              \
+            ix->centroids.as<float>(), ix->w_rev.as<float>(), ix->nbits, tv.codes,                                     \
+            tv.residuals, Mcap, ws.maxkey.as<uint32_t>());                                                             \
     } break;
             PB_PE(64) PB_PE(96) PB_PE(128)
 #undef PB_PE
@@ -1939,10 +2081,10 @@ static pb_status exact_scores(pb_index *ix, Workspace &ws, const SearchIO &io, c
         }
         CK(cudaGetLastError());
         L[PB_STAGE_EXACT] += 5;
-        CKS(launch_exact(ix, ws, kv, B, QS, Mcap, 0, max_tokens, &L[PB_STAGE_EXACT], ws.needexact.as<int>(), false));
+        CKS(launch_exact(ix, ws, kv, tv, B, QS, Mcap, 0, max_tokens, &L[PB_STAGE_EXACT], ws.needexact.as<int>(), false));
         KEV_END(PB_KERNEL_EXACT);
     } else {
-        CKS(launch_exact(ix, ws, kv, B, QS, Mcap, 0, max_tokens, &L[PB_STAGE_EXACT]));
+        CKS(launch_exact(ix, ws, kv, tv, B, QS, Mcap, 0, max_tokens, &L[PB_STAGE_EXACT]));
     }
     if (pass.diag) {  // before k_exact_finalize, which clears the exact maxima
         CKS(ws.fdiag.ensure(16));
@@ -1951,6 +2093,11 @@ static pb_status exact_scores(pb_index *ix, Workspace &ws, const SearchIO &io, c
                                                          QS, kv.nkept, Mcap, ws.qnmax.as<float>(),
                                                          linear ? ws.qflag.as<int>() : nullptr, eps_unit,
                                                          ws.fdiag.as<unsigned long long>());
+        CK(cudaGetLastError());
+        L[PB_STAGE_EXACT] += 1;
+    }
+    if (ix->host_tier) {  // slots back to doc ids, in the list the scores belong to
+        k_unstage_kept<<<dim3((Mcap + 255) / 256, B), 256, 0, ws.stream>>>(kv.kept, kv.nkept, Mcap, ws.kept.as<uint32_t>());
         CK(cudaGetLastError());
         L[PB_STAGE_EXACT] += 1;
     }
@@ -2100,6 +2247,17 @@ static pb_status finish(pb_index *ix, Workspace &ws, const SearchIO &io, const S
             w.n_exact_tokens += (long long)hc.cnt[1 + b];
         }
     }
+    if (ix->host_tier) {  // every kept doc was staged, filter or not
+        for (int b = 0; b < B; ++b) {
+            g_stats.staged_docs += hc.kept[b];
+            g_stats.staged_bytes += (long long)hc.cnt[1 + b] * ix->packed;
+        }
+        if (plan.prof) {
+            float ms = 0.f;
+            CK(cudaEventElapsedTime(&ms, ws.sev[0], ws.sev[1]));
+            g_stats.staging_ms += ms;
+        }
+    }
     return PB_OK;
 }
 
@@ -2246,6 +2404,9 @@ static void merge_stats(Stats &a, const Stats &b) {
         a.launches[i] += b.launches[i];
     }
     for (int i = 0; i < PB_KERNEL_COUNT; ++i) a.kernel_ms[i] += b.kernel_ms[i];
+    a.staged_docs += b.staged_docs;
+    a.staged_bytes += b.staged_bytes;
+    a.staging_ms += b.staging_ms;
     const int64_t *src = reinterpret_cast<const int64_t *>(&b.work);
     int64_t *dst = reinterpret_cast<int64_t *>(&a.work);
     const size_t kdiff = offsetof(pb_work_counters, k1_tc_max_code_diff) / 8;
@@ -2421,11 +2582,28 @@ extern "C" pb_status pb_decompress_documents(pb_index *ix, const int64_t *doc_id
     }
     if (!out_embeddings || docs.empty() || prefix.back() == 0) return PB_OK;
     const long long total = prefix.back();
-    DevBuf ddocs, dpre, dout;
+    DevBuf ddocs, dpre, dout, ident;
     CKS(upload(ddocs, docs.data(), docs.size() * 4, PB_MEM_HOST));
     CKS(upload(dpre, prefix.data(), prefix.size() * 8, PB_MEM_HOST));
     const long long chunk_tok = 1ll << 22;  // bound the staging buffer (2 GiB at dim 128)
     CKS(dout.ensure((size_t)std::min(total, chunk_tok + ix->max_doclen) * ix->dim * 4));
+    // host tier: each range's docs are staged first (slot j = its j-th doc, at the range-local prefix), then decompressed
+    // from the staged rows with the identity as doc list
+    std::unique_ptr<Workspace> wsp;
+    if (ix->host_tier) {
+        CKS(ix->acquire(wsp));
+        CKS(ident.ensure(docs.size() * 4 + 16));
+        k_fill_identity<<<64, 256, 0, wsp->stream>>>(ident.as<uint32_t>(), (long long)docs.size(), 0u);
+        CK(cudaGetLastError());
+        CK(cudaStreamSynchronize(wsp->stream));
+    }
+    struct Releaser {
+        pb_index *ix;
+        std::unique_ptr<Workspace> &w;
+        ~Releaser() {
+            if (w) ix->release(w);
+        }
+    } rel{ix, wsp};
     // process doc ranges whose token count fits the staging buffer
     size_t i0 = 0;
     while (i0 < docs.size()) {
@@ -2437,10 +2615,16 @@ extern "C" pb_status pb_decompress_documents(pb_index *ix, const int64_t *doc_id
         for (int j = 0; j <= nd; ++j) local[j] = prefix[i0 + j] - prefix[i0];
         CK(cudaMemcpy(dpre.p, local.data(), local.size() * 8, cudaMemcpyHostToDevice));
         int blocks = (int)std::max<long long>(1, std::min<long long>((ntok + 7) / 8, (long long)ix->sm_count * 8));
+        TokView tv = resident_tokens(ix);
+        const uint32_t *list = ddocs.as<uint32_t>() + i0;
+        if (ix->host_tier) {
+            CKS(stage_rows(ix, *wsp, list, nullptr, nd, nd, dpre.as<long long>(), ntok, tv));
+            CK(cudaStreamSynchronize(wsp->stream));
+            list = ident.as<uint32_t>();
+        }
         PB_DIM_SWITCH(ix->dim, {
             k_decompress<DIM><<<blocks, 256>>>(ix->centroids.as<float>(), ix->w_rev.as<float>(), ix->nbits,
-                                               ix->codes.as<uint32_t>(), ix->residuals.as<uint8_t>(),
-                                               ix->doc_off.as<long long>(), ddocs.as<uint32_t>() + i0, dpre.as<long long>(),
+                                               tv.codes, tv.residuals, tv.doc_off, list, dpre.as<long long>(),
                                                nd, dout.as<float>());
         });
         CK(cudaGetLastError());
@@ -2536,13 +2720,28 @@ extern "C" pb_status pb_exhaustive_scores(pb_index *ix, const float *queries, co
         CKS(ws.maxkey.ensure((size_t)B * Mblk * QS * 4));
         CKS(ws.exact.ensure((size_t)B * Mblk * 4));
         // maxkey layout changes with QS/Mcap: rows are reset by finalize, but only those < n_kept
-        for (long long d0 = 0; d0 < ix->D; d0 += Mblk) {
-            const int nd = (int)std::min<long long>(Mblk, ix->D - d0);
-            k_fill_identity<<<64, 256, 0, ws.stream>>>(ws.kept.as<uint32_t>(), nd, (uint32_t)d0);
-            k_range_prefix<<<64, 256, 0, ws.stream>>>(ix->doc_off.as<long long>(), d0, nd, ws.tokp.as<long long>());
-            CK(cudaMemcpyAsync(ws.nkept.p, &nd, 4, cudaMemcpyHostToDevice, ws.stream));
+        for (long long d0 = 0, nd = 0; d0 < ix->D; d0 += nd) {
+            nd = std::min<long long>(Mblk, ix->D - d0);
+            // host tier: a window of at most 2^22 tokens (or one doc) is one H2D copy into the staging buffer, scored with
+            // window-local ids and offsets (the window's token prefix is its doc_off)
+            if (ix->host_tier) {
+                const long long win = std::max(1ll << 22, (long long)ix->max_doclen);
+                nd = std::upper_bound(doff.begin() + d0 + 1, doff.begin() + d0 + nd + 1, doff[d0] + win) - doff.begin() - 1 - d0;
+            }
+            const long long ntok = doff[d0 + nd] - doff[d0];
+            k_fill_identity<<<64, 256, 0, ws.stream>>>(ws.kept.as<uint32_t>(), nd, ix->host_tier ? 0u : (uint32_t)d0);
+            k_range_prefix<<<64, 256, 0, ws.stream>>>(ix->doc_off.as<long long>(), d0, (int)nd, ws.tokp.as<long long>());
+            const int nd32 = (int)nd;
+            CK(cudaMemcpyAsync(ws.nkept.p, &nd32, 4, cudaMemcpyHostToDevice, ws.stream));
             const KeptView kv{ws.kept.as<uint32_t>(), ws.nkept.as<int>(), ws.tokp.as<long long>(), nullptr};
-            CKS(launch_exact(ix, ws, kv, B, QS, Mblk, 1, doff[d0 + nd] - doff[d0], nullptr));
+            TokView tv = resident_tokens(ix);
+            if (ix->host_tier) {
+                CKS(ws.s_res.ensure((size_t)std::max(ntok, 1ll) * ix->packed));
+                CK(cudaMemcpyAsync(ws.s_res.p, ix->host_res.p + (size_t)doff[d0] * ix->packed, (size_t)ntok * ix->packed,
+                                   cudaMemcpyHostToDevice, ws.stream));
+                tv = {ix->codes.as<uint32_t>() + doff[d0], ws.s_res.as<uint8_t>(), nullptr, ws.tokp.as<long long>()};
+            }
+            CKS(launch_exact(ix, ws, kv, tv, B, QS, Mblk, 1, ntok, nullptr));
             k_exact_finalize<<<dim3((Mblk + 7) / 8, B), 256, 0, ws.stream>>>(ws.maxkey.as<uint32_t>(), ws.qoff.as<int>(), QS,
                                                                            ws.nkept.as<int>(), Mblk, 1, ws.exact.as<float>(),
                                                                            nullptr, nullptr, nullptr, 0u, nullptr);
@@ -3424,6 +3623,16 @@ static void append_commit(pb_index *ix, const AppendPrep &p) {
     ix->wmax = p.wmax;
 }
 
+// Mutations need a residual array the library owns on the device: not the caller's (PB_OPEN_ADOPT_RESIDUALS), not
+// pinned host memory (PB_OPEN_HOST_RESIDUALS)
+static pb_status refuse_fixed_residuals(const pb_index *ix) {
+    if (!ix->residuals.owned)
+        return pb_fail(PB_ERR_UNSUPPORTED, "the handle uses the caller's residual array (PB_OPEN_ADOPT_RESIDUALS)");
+    if (ix->host_tier)
+        return pb_fail(PB_ERR_UNSUPPORTED, "the handle keeps its residuals in host memory (PB_OPEN_HOST_RESIDUALS)");
+    return PB_OK;
+}
+
 static pb_status append_impl(pb_index *ix, pb_codec *codec, const float *embeddings, const int64_t *codes,
                              const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs, int32_t space,
                              const char *index_dir, int64_t batch_size, int64_t *out_first) {
@@ -3432,8 +3641,7 @@ static pb_status append_impl(pb_index *ix, pb_codec *codec, const float *embeddi
     std::lock_guard<std::mutex> gate(ix->gate);
     std::unique_lock<std::shared_mutex> wr(ix->rw);
     if (ix->comm || ix->group) return pb_fail(PB_ERR_UNSUPPORTED, "appends to a doc-sharded handle are not supported");
-    if (!ix->residuals.owned)
-        return pb_fail(PB_ERR_UNSUPPORTED, "the handle uses the caller's residual array (PB_OPEN_ADOPT_RESIDUALS)");
+    CKS(refuse_fixed_residuals(ix));
     if (index_dir && ix->doc_id_base != 0) return pb_fail(PB_ERR_UNSUPPORTED, "an index directory holds doc ids from 0");
     if (index_dir && batch_size <= 0) return pb_fail(PB_ERR_INVALID, "batch_size must be positive");
     AppendPrep p;
@@ -3470,8 +3678,7 @@ extern "C" pb_status pb_index_reserve(pb_index *ix, int64_t num_documents, int64
     std::lock_guard<std::mutex> gate(ix->gate);
     std::unique_lock<std::shared_mutex> wr(ix->rw);
     if (ix->comm || ix->group) return pb_fail(PB_ERR_UNSUPPORTED, "appends to a doc-sharded handle are not supported");
-    if (!ix->residuals.owned)
-        return pb_fail(PB_ERR_UNSUPPORTED, "the handle uses the caller's residual array (PB_OPEN_ADOPT_RESIDUALS)");
+    CKS(refuse_fixed_residuals(ix));
     if (num_documents >= (1ll << 32) - 1 || num_embeddings < 0) return pb_fail(PB_ERR_INVALID, "bad reserve sizes");
     CK(cudaSetDevice(ix->device));
     CK(cudaDeviceSynchronize());
@@ -3700,8 +3907,7 @@ extern "C" pb_status pb_index_delete(pb_index *ix, const int64_t *doc_ids, int64
     std::lock_guard<std::mutex> gate(ix->gate);
     std::unique_lock<std::shared_mutex> wr(ix->rw);
     if (ix->comm || ix->group) return pb_fail(PB_ERR_UNSUPPORTED, "deletes from a doc-sharded handle are not supported");
-    if (!ix->residuals.owned)
-        return pb_fail(PB_ERR_UNSUPPORTED, "the handle uses the caller's residual array (PB_OPEN_ADOPT_RESIDUALS)");
+    CKS(refuse_fixed_residuals(ix));
     if (index_dir && ix->doc_id_base != 0) return pb_fail(PB_ERR_UNSUPPORTED, "an index directory holds doc ids from 0");
     DeletePrep p;
     CKS(delete_prepare(ix, doc_ids, n_ids, p));
@@ -3788,8 +3994,7 @@ static pb_status sharded_update(pb_index *ix, int op, pb_codec *codec, const flo
         if (n < 0 || (n && !(op == SH_OP_DELETE ? doc_ids : doc_lengths))) return pb_fail(PB_ERR_INVALID, "null argument");
         if (op != SH_OP_DELETE && space != PB_MEM_HOST && space != PB_MEM_DEVICE)
             return pb_fail(PB_ERR_INVALID, "bad memory_space %d", space);
-        if (!ix->residuals.owned)
-            return pb_fail(PB_ERR_UNSUPPORTED, "the handle uses the caller's residual array (PB_OPEN_ADOPT_RESIDUALS)");
+        CKS(refuse_fixed_residuals(ix));
         if (index_dir && op == SH_OP_APPEND && batch_size <= 0) return pb_fail(PB_ERR_INVALID, "batch_size must be positive");
         if (op == SH_OP_APPEND && last && !codec) return pb_fail(PB_ERR_INVALID, "null argument");
         std::vector<int64_t> args;
@@ -3979,7 +4184,7 @@ extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bou
     rec[RB_K] = K;
     rec[RB_DIM] = ix->dim;
     rec[RB_NBITS] = ix->nbits;
-    rec[RB_ADOPT] = !ix->residuals.owned;
+    rec[RB_ADOPT] = !ix->residuals.owned || ix->host_tier;  // a residual array that cannot move
 
     // 2. exchange A and the verdict every rank reaches from the same records
     std::vector<long long> all;
@@ -4002,7 +4207,9 @@ extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bou
     }
     for (int r = 0; r < W; ++r)
         if (at(r, RB_ADOPT))
-            return pb_fail(PB_ERR_UNSUPPORTED, "rank %d uses the caller's residual array (PB_OPEN_ADOPT_RESIDUALS)", r);
+            return pb_fail(PB_ERR_UNSUPPORTED,
+                           "rank %d uses the caller's residual array or host memory (PB_OPEN_ADOPT_RESIDUALS / "
+                           "PB_OPEN_HOST_RESIDUALS)", r);
     const long long D_total = a[W], N_total = tok[W];
 
     // 3. the new bounds: the caller's, or the token-balanced split b[r] = min { d : off[d] W >= N r } of the global doc

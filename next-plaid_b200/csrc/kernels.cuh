@@ -16,6 +16,8 @@
 //   k_pair_exact ........ a7+a8 decompress + pinned fp32 dot of the listed pairs   codec.rs:423-470, maxsim.rs:270-294
 //   k_exact ............. a7+a8 fused residual decompress + MaxSim of every token (filter off, flagged queries, trace)
 //   k_exact_finalize .... a8  q-ordered sum of per-token maxima           maxsim.rs:284-291
+//   k_stage_layout/k_stage_rows/k_unstage_kept  a7 on a host-tier handle: the kept docs' rows staged from pinned host
+//                             memory into slot space, and the slots mapped back to doc ids before k_exact_finalize
 //   k_topk .............. a9  stable final sort, take top_k               search.rs:496-515
 //   k_merge_cut/k_merge_topk  doc-sharded search: global cut and global top-k from the all-gathered keys
 //   k_assign_tc/k_assign_certify/k_assign/k_quantize_pack  a12  index build: nearest centroid (wgmma fp16
@@ -38,3 +40,4 @@
 #include "k_filter_tc.cuh"
 #include "k_maxsim_tc.cuh"
 #include "k_scores_tc.cuh"
+#include "k_stage.cuh"

@@ -274,8 +274,10 @@ struct DirLayout {
     }
 };
 
-// pb_index_load of documents [doc_begin, doc_end) of the directory; doc_end < 0 stands for every document
-pb_status load_range(const char *index_dir, int32_t device, long long doc_begin, long long doc_end, pb_index **out) {
+// pb_index_load of documents [doc_begin, doc_end) of the directory with pb_index_desc.flags; doc_end < 0 stands for every
+// document
+pb_status load_range(const char *index_dir, int32_t device, long long doc_begin, long long doc_end, int32_t flags,
+                     pb_index **out) {
     const std::string dir = std::string(index_dir) + "/";
     DirLayout lay;
     if (pb_status s = lay.read_metadata(dir)) return s;
@@ -330,6 +332,7 @@ pb_status load_range(const char *index_dir, int32_t device, long long doc_begin,
     d.device = device;
     d.memory_space = PB_MEM_HOST;
     d.doc_id_base = doc_begin;
+    d.flags = flags;
     if (pb_status s = div.check_sum(K)) return s;
     const long long packed = (long long)dim * nb / 8;
     // every chunk file is checked (header, dtype, shape, payload size) before the device is touched: a bad
@@ -376,7 +379,7 @@ pb_status load_range(const char *index_dir, int32_t device, long long doc_begin,
 extern "C" pb_status pb_index_load(const char *index_dir, int32_t device, pb_index **out) {
     if (!index_dir || !out) return pb_fail(PB_ERR_INVALID, "null argument");
     *out = nullptr;
-    return load_range(index_dir, device, 0, -1, out);
+    return load_range(index_dir, device, 0, -1, 0, out);
 }
 
 extern "C" pb_status pb_index_load_range(const char *index_dir, int32_t device, int64_t doc_begin, int64_t doc_end,
@@ -385,7 +388,16 @@ extern "C" pb_status pb_index_load_range(const char *index_dir, int32_t device, 
     *out = nullptr;
     if (doc_begin < 0 || doc_end < doc_begin)
         return pb_fail(PB_ERR_INVALID, "bad document range [%lld, %lld)", (long long)doc_begin, (long long)doc_end);
-    return load_range(index_dir, device, doc_begin, doc_end, out);
+    return load_range(index_dir, device, doc_begin, doc_end, 0, out);
+}
+
+extern "C" pb_status pb_index_load_range_flags(const char *index_dir, int32_t device, int64_t doc_begin, int64_t doc_end,
+                                               int32_t flags, pb_index **out) {
+    if (!index_dir || !out) return pb_fail(PB_ERR_INVALID, "null argument");
+    *out = nullptr;
+    if (doc_begin < 0 || (doc_end >= 0 && doc_end < doc_begin))
+        return pb_fail(PB_ERR_INVALID, "bad document range [%lld, %lld)", (long long)doc_begin, (long long)doc_end);
+    return load_range(index_dir, device, doc_begin, doc_end, flags, out);
 }
 
 extern "C" pb_status pb_index_dir_shard_bounds(const char *index_dir, int32_t world, int64_t *out_bounds) {

@@ -87,8 +87,10 @@ EXPORTS = [
     "pb_index_append", "pb_index_append_encoded", "pb_index_reserve",
     "pb_index_delete", "pb_last_delete_ms", "pb_index_load_range", "pb_index_dir_shard_bounds",
     "pb_index_delete_sharded", "pb_index_append_sharded", "pb_index_append_encoded_sharded",
-    "pb_index_rebalance_sharded",
+    "pb_index_rebalance_sharded", "pb_index_load_range_flags", "pb_index_memory", "pb_last_staging_stats",
 ]
+
+PB_OPEN_ADOPT_RESIDUALS, PB_OPEN_HOST_RESIDUALS = 1, 2
 
 _lib = None
 
@@ -125,6 +127,10 @@ def load_library():
         L.pb_set_lanes.restype = None
         L.pb_index_load.argtypes = [C.c_char_p, C.c_int32, C.POINTER(C.c_void_p)]
         L.pb_index_load_range.argtypes = [C.c_char_p, C.c_int32, C.c_int64, C.c_int64, C.POINTER(C.c_void_p)]
+        L.pb_index_load_range_flags.argtypes = [C.c_char_p, C.c_int32, C.c_int64, C.c_int64, C.c_int32,
+                                                C.POINTER(C.c_void_p)]
+        L.pb_index_memory.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        L.pb_last_staging_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.pb_index_dir_shard_bounds.argtypes = [C.c_char_p, C.c_int32, C.c_void_p]
         L.pb_index_open.argtypes = [C.POINTER(_Desc), C.POINTER(C.c_void_p)]
         L.pb_search_batch_traced.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
@@ -380,33 +386,47 @@ class MmapIndex:
 
     # -- construction ----------------------------------------------------------------------
     @classmethod
-    def load(cls, index_path: str, device: int = 0) -> "MmapIndex":
-        """MmapIndex::load (index.rs:1026): reads the reference's index directory."""
+    def load(cls, index_path: str, device: int = 0, host_residuals: bool = False) -> "MmapIndex":
+        """MmapIndex::load (index.rs:1026): reads the reference's index directory.  host_residuals: the packed
+        residuals go to pinned host memory instead of the device (PB_OPEN_HOST_RESIDUALS; same results, slower search,
+        no appends or deletes)."""
         L = load_library()
         h = C.c_void_p()
-        _check(L.pb_index_load(os.fsencode(index_path), device, C.byref(h)))
+        if host_residuals:
+            _check(L.pb_index_load_range_flags(os.fsencode(index_path), device, 0, -1, PB_OPEN_HOST_RESIDUALS,
+                                               C.byref(h)))
+        else:
+            _check(L.pb_index_load(os.fsencode(index_path), device, C.byref(h)))
         return cls(h.value, index_path)
 
     @classmethod
-    def load_range(cls, index_path: str, doc_begin: int, doc_end: int, device: int = 0) -> "MmapIndex":
+    def load_range(cls, index_path: str, doc_begin: int, doc_end: int, device: int = 0,
+                   host_residuals: bool = False) -> "MmapIndex":
         """pb_index_load_range: documents [doc_begin, doc_end) of the directory as one shard of a doc-sharded
-        deployment (doc_id_base = doc_begin, so search returns global ids).  Reads only that range's chunk rows."""
+        deployment (doc_id_base = doc_begin, so search returns global ids).  Reads only that range's chunk rows.
+        host_residuals: as for load."""
         h = C.c_void_p()
-        _check(load_library().pb_index_load_range(os.fsencode(index_path), device, doc_begin, doc_end, C.byref(h)))
+        L = load_library()
+        if host_residuals:
+            _check(L.pb_index_load_range_flags(os.fsencode(index_path), device, doc_begin, doc_end,
+                                               PB_OPEN_HOST_RESIDUALS, C.byref(h)))
+        else:
+            _check(L.pb_index_load_range(os.fsencode(index_path), device, doc_begin, doc_end, C.byref(h)))
         return cls(h.value, index_path)
 
     @classmethod
-    def load_shard(cls, index_path: str, rank: int, world: int, device: int = 0) -> "MmapIndex":
+    def load_shard(cls, index_path: str, rank: int, world: int, device: int = 0,
+                   host_residuals: bool = False) -> "MmapIndex":
         """Shard `rank` of `world` of the directory: load_range over shard_bounds(index_path, world)."""
         if not 0 <= rank < world:
             raise PlaidError(PB_ERR_INVALID, f"rank {rank} outside [0, {world})")
         b = shard_bounds(index_path, world)
-        return cls.load_range(index_path, int(b[rank]), int(b[rank + 1]), device)
+        return cls.load_range(index_path, int(b[rank]), int(b[rank + 1]), device, host_residuals)
 
     @classmethod
     def from_arrays(cls, centroids, bucket_weights, codes, residuals, doc_lengths, ivf, ivf_lengths,
-                    nbits: int, device: int = 0, doc_id_base: int = 0) -> "MmapIndex":
-        """pb_index_open from host arrays in the reference's dtypes."""
+                    nbits: int, device: int = 0, doc_id_base: int = 0, host_residuals: bool = False) -> "MmapIndex":
+        """pb_index_open from host arrays in the reference's dtypes.  host_residuals: as for load."""
         L = load_library()
         cen = np.ascontiguousarray(centroids, np.float32)
         w = np.ascontiguousarray(bucket_weights, np.float32)
@@ -417,7 +437,8 @@ class MmapIndex:
         iv = None if ivf is None else np.ascontiguousarray(ivf, np.int64)
         il = None if ivf_lengths is None else np.ascontiguousarray(ivf_lengths, np.int32)
         d = _Desc(cen.shape[1], nbits, cen.shape[0], len(dl), len(cd), _ptr(cen), _ptr(w), _ptr(cd),
-                  _ptr(rs), _ptr(dl), _ptr(iv), _ptr(il), device, 0, doc_id_base, 0)
+                  _ptr(rs), _ptr(dl), _ptr(iv), _ptr(il), device, 0, doc_id_base,
+                  PB_OPEN_HOST_RESIDUALS if host_residuals else 0)
         h = C.c_void_p()
         _check(L.pb_index_open(C.byref(d), C.byref(h)))
         return cls(h.value)
@@ -425,13 +446,15 @@ class MmapIndex:
     @classmethod
     def from_device_pointers(cls, dim, nbits, K, D, N, centroids, bucket_weights, codes, residuals,
                              doc_lengths, ivf, ivf_lengths, device: int = 0, doc_id_base: int = 0,
-                             adopt_residuals: bool = False):
+                             adopt_residuals: bool = False, host_residuals: bool = False):
         """pb_index_open with PB_MEM_DEVICE pointers (integers), e.g. torch tensors' data_ptr().  ivf = ivf_lengths
         = None: the inverted file is built on the device (index.rs:850-873).  adopt_residuals: the packed residuals
-        are used in place (keep the array alive until close())."""
+        are used in place (keep the array alive until close()).  host_residuals: they are copied to pinned host
+        memory, as for load."""
         L = load_library()
+        flags = (PB_OPEN_ADOPT_RESIDUALS if adopt_residuals else 0) | (PB_OPEN_HOST_RESIDUALS if host_residuals else 0)
         d = _Desc(dim, nbits, K, D, N, centroids, bucket_weights, codes, residuals, doc_lengths, ivf,
-                  ivf_lengths, device, 1, doc_id_base, 1 if adopt_residuals else 0)
+                  ivf_lengths, device, 1, doc_id_base, flags)
         h = C.c_void_p()
         _check(L.pb_index_open(C.byref(d), C.byref(h)))
         return cls(h.value)
@@ -465,6 +488,12 @@ class MmapIndex:
 
     def nbits(self) -> int:
         return int(load_library().pb_index_nbits(self._h))
+
+    def memory_usage(self) -> dict:
+        """pb_index_memory: bytes the index arrays hold on the device and in pinned host memory (workspaces excluded)."""
+        dev, host = C.c_int64(), C.c_int64()
+        _check(load_library().pb_index_memory(self._h, C.byref(dev), C.byref(host)))
+        return dict(device_bytes=int(dev.value), host_bytes=int(host.value))
 
     # -- incremental append (index.rs:1675 update_append + reload) ------------------------------------
     def append(self, embeddings: Sequence[np.ndarray], codec: "ResidualCodec", index_dir: Optional[str] = None,
@@ -666,6 +695,13 @@ class MmapIndex:
         w = _Work()
         _check(load_library().pb_last_work_counters(self._h, C.byref(w)))
         return {n: int(getattr(w, n)) for n, _ in _Work._fields_}
+
+    def last_staging_stats(self) -> dict:
+        """pb_last_staging_stats: docs and residual bytes the calling thread's last search staged from host memory (0 on
+        a resident handle), and their staging time in ms (with set_profiling(True))."""
+        docs, nbytes, ms = C.c_int64(), C.c_int64(), C.c_float()
+        _check(load_library().pb_last_staging_stats(self._h, C.byref(docs), C.byref(nbytes), C.byref(ms)))
+        return dict(docs=int(docs.value), bytes=int(nbytes.value), ms=float(ms.value))
 
     def search_batch_device(self, d_queries_ptr: int, q_tok_offsets: np.ndarray, params: SearchParameters,
                             d_ids_ptr: int, d_scores_ptr: int, d_counts_ptr: int):

@@ -80,7 +80,14 @@ extern "C" {
                                        doc_lengths: *const i64, n_docs: i64, memory_space: i32,
                                        out_first_doc_id: *mut i64) -> c_int;
     fn pb_index_rebalance_sharded(ix: *mut c_void, bounds: *const i64, out_bounds: *mut i64) -> c_int;
+    fn pb_index_load_range_flags(index_dir: *const c_char, device: i32, doc_begin: i64, doc_end: i64, flags: i32,
+                                 out: *mut *mut c_void) -> c_int;
+    fn pb_index_memory(ix: *const c_void, device_bytes: *mut i64, host_bytes: *mut i64) -> c_int;
+    fn pb_last_staging_stats(ix: *mut c_void, docs: *mut i64, bytes: *mut i64, ms: *mut f32) -> c_int;
 }
+
+/// pb_index_desc.flags: the packed residuals in pinned host memory, the kept docs' rows staged per search (DESIGN §4j).
+pub const PB_OPEN_HOST_RESIDUALS: i32 = 2;
 
 fn last_error() -> String {
     unsafe { CStr::from_ptr(pb_last_error()).to_string_lossy().into_owned() }
@@ -107,6 +114,34 @@ impl B200Index {
             return Err(Error::IndexLoad(last_error()));
         }
         Ok(B200Index { handle })
+    }
+
+    /// `load` with the packed residuals in pinned host memory (`PB_OPEN_HOST_RESIDUALS`): same results, slower searches
+    /// (the kept docs' rows cross PCIe), about 11 instead of 75 device bytes per token at 4 bits and dim 128.  Such a
+    /// handle refuses appends and deletes.
+    pub fn load_host_residuals(index_path: &str, device: i32) -> Result<Self> {
+        let c = CString::new(index_path).map_err(|e| Error::IndexLoad(e.to_string()))?;
+        let mut handle: *mut c_void = std::ptr::null_mut();
+        if unsafe { pb_index_load_range_flags(c.as_ptr(), device, 0, -1, PB_OPEN_HOST_RESIDUALS, &mut handle) } != 0 {
+            return Err(Error::IndexLoad(last_error()));
+        }
+        Ok(B200Index { handle })
+    }
+
+    /// Bytes the index arrays hold: (device, pinned host) -- for capacity planning on a shared GPU.
+    pub fn memory_usage(&self) -> Result<(i64, i64)> {
+        let (mut d, mut h) = (0i64, 0i64);
+        if unsafe { pb_index_memory(self.handle, &mut d, &mut h) } != 0 {
+            return Err(Error::Search(last_error()));
+        }
+        Ok((d, h))
+    }
+
+    /// What this thread's last search staged from host memory: (docs, residual bytes, ms with profiling on).
+    pub fn last_staging_stats(&self) -> (i64, i64, f32) {
+        let (mut docs, mut bytes, mut ms) = (0i64, 0i64, 0f32);
+        unsafe { pb_last_staging_stats(self.handle, &mut docs, &mut bytes, &mut ms) };
+        (docs, bytes, ms)
     }
 
     /// Shard `rank` of `world` of the same directory for a doc-sharded deployment: the token-balanced document range
