@@ -409,7 +409,7 @@ PB_API pb_status pb_last_call_ms(pb_index *ix, float *out_ms);
 enum {
     PB_KERNEL_SCORES = 0,   /* k_scores16_tc (or k_centroid_scores on the exact path) */
     PB_KERNEL_APPROX16 = 1, /* k_approx16, the first approximate pass */
-    PB_KERNEL_FILTER = 2,   /* k_exact_tc, the wgmma MaxSim estimate of every kept doc */
+    PB_KERNEL_FILTER = 2,   /* k_maxsim_tc pass 1, the wgmma MaxSim estimate of every kept doc */
     PB_KERNEL_EXACT = 3,    /* k_exact, fused decompress + MaxSim of the survivors */
     PB_KERNEL_COUNT = 4
 };

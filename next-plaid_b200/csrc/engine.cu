@@ -431,14 +431,11 @@ struct pb_index {
     bool k1_diag = false;      // also run the exact table and report the largest code difference (PB_K1_TC_DIAG=1)
     DevBuf cent_h16t, cent_l16t;  // its centroid operands: fp16 hi / lo, MMA tile order
     int approx_grid = 8;       // k_approx16 CTAs per SM and query (PB_APPROX_GRID)
-    int xtc_grid = 32;         // k_exact_tc CTAs per SM across the batch (PB_XTC_GRID)
     bool probe16 = true;       // a3 threshold-first selection on the 16-bit table (PB_PROBE16=0: per-lane lists only)
     bool fast_exact = true;    // tensor-core certified filter in front of the exact stage (same results either way)
     float vmin = 0.0f;         // smallest pre-normalisation token norm |c + w| over the index (error bound of the filter)
     float wmax = 0.0f;         // largest residual norm |w| over the index (same)
-    DevBuf centroids_f16;      // [K][dim] fp16 copy for the filter (k_exact_tc, the variant without a score table)
     DevBuf tok_inv_norm;       // [N] 1 / |c + w| for the linear estimate (k_maxsim_tc)
-    bool filter_v1 = false;    // PB_FILTER_V1=1: always the decompressing filter k_exact_tc (A/B measurement)
     bool filter_diag = false;  // PB_FILTER_DIAG=1: score every kept doc exactly and measure the filter's estimate against it
     bool pair_exact = true;    // exact stage on the (token, query token) pairs that can hold a maximum (PB_PAIR_EXACT=0: k_exact)
     int ws_grid = 8;           // k_maxsim_tc CTAs per SM across the batch (PB_WS_GRID)
@@ -855,13 +852,9 @@ static pb_status build_ivf_on_device(pb_index *ix) {
 
 static bool filter_dim(int dim) { return dim == 64 || dim == 96 || dim == 128; }
 
-// Operands of the tensor-core kernels that depend on the centroids alone: the fp16 centroids of the filter (k_exact_tc)
-// and the scaled hi / lo tiles of the score table (k_scores16_tc).
+// Operands of the tensor-core kernels that depend on the centroids alone: the scaled hi / lo tiles of the score table
+// (k_scores16_tc).
 static pb_status build_centroid_operands(pb_index *ix) {
-    CKS(ix->centroids_f16.ensure((size_t)ix->K * ix->dim * 2));
-    k_rows_to_f16_plain<<<ix->sm_count * 8, 256>>>(ix->centroids.as<float>(), ix->K * (long long)ix->dim,
-                                                  ix->centroids_f16.as<__half>());
-    CK(cudaGetLastError());
     if ((ix->k1_diag || ix->k1_tc) && ix->cmax > 0.0f && ix->cmax < 3.0e38f) {
         // operands of the tensor-core score table: centroids * 2^cent_exp (max norm in [1, 2)), fp16 hi / lo parts
         ix->cent_exp = -ilogbf(ix->cmax);
@@ -935,7 +928,6 @@ pb_status pb_index_finalize(pb_index *ix) {
         ix->cmax = sqrtf(m2);
         if (const char *e = getenv("PB_FAST_APPROX")) ix->fast_approx = atoi(e) != 0;
         if (const char *e = getenv("PB_FAST_EXACT")) ix->fast_exact = atoi(e) != 0;
-        if (const char *e = getenv("PB_FILTER_V1")) ix->filter_v1 = atoi(e) != 0;
         if (const char *e = getenv("PB_FILTER_DIAG")) ix->filter_diag = atoi(e) != 0;
         if (const char *e = getenv("PB_PAIR_EXACT")) ix->pair_exact = atoi(e) != 0;
         if (const char *e = getenv("PB_WS_GRID")) ix->ws_grid = std::max(1, atoi(e));
@@ -946,10 +938,9 @@ pb_status pb_index_finalize(pb_index *ix) {
         if (const char *e = getenv("PB_K1_TC")) ix->k1_tc = atoi(e) != 0;
         if (const char *e = getenv("PB_K1_TC_E")) ix->k1_margin = std::max(1, atoi(e));
         if (const char *e = getenv("PB_APPROX_GRID")) ix->approx_grid = std::max(1, atoi(e));
-        if (const char *e = getenv("PB_XTC_GRID")) ix->xtc_grid = std::max(1, atoi(e));
     }
     if (filter_dim(ix->dim) && ix->N > 0 && ix->K > 0) {
-        // operands of the tensor-core filter (k_exact_tc) and score table, and the smallest token norm
+        // operands of the tensor-core score table, and the token norms of the filter
         CKS(build_centroid_operands(ix));
         DevBuf mn;
         CKS(mn.ensure(16));
@@ -1044,8 +1035,8 @@ extern "C" pb_status pb_index_memory(const pb_index *ix, int64_t *device_bytes, 
     auto rd = ix->read_lock();
     size_t dev = 0;
     for (const DevBuf *b : {&ix->centroids, &ix->w_rev, &ix->codes, &ix->residuals, &ix->doc_off, &ix->ivf, &ix->ivf_off,
-                            &ix->ucodes, &ix->udoc_off, &ix->cent_h16t, &ix->cent_l16t, &ix->centroids_f16,
-                            &ix->tok_inv_norm, &ix->ivf_spare, &ix->ivf_off_spare})
+                            &ix->ucodes, &ix->udoc_off, &ix->cent_h16t, &ix->cent_l16t, &ix->tok_inv_norm,
+                            &ix->ivf_spare, &ix->ivf_off_spare})
         if (b->owned) dev += b->cap;  // adopted residuals are the caller's allocation
     if (device_bytes) *device_bytes = (int64_t)dev;
     if (host_bytes) *host_bytes = (int64_t)ix->host_res.bytes;
@@ -1268,8 +1259,7 @@ static pb_status run_k1_tc(pb_index *ix, Workspace &ws, const pb_search_params *
     return PB_OK;
 }
 
-// a2 on the fp32 FMA path: the exact table, with16 also its 16-bit codes (and, with PB_K1_TC_DIAG, their comparison
-// with the tensor-core table)
+// a2 on the fp32 FMA path: the exact table, with16 also its 16-bit codes
 static pb_status launch_centroid_scores(pb_index *ix, Workspace &ws, int B, int QS, int *launches, bool with16 = false) {
     const int tiles = (int)((ix->K + PB_TOK_TILE - 1) / PB_TOK_TILE);
     // enough CTAs to fill the machine twice over; each CTA keeps its centroid tile in smem and walks queries
@@ -1291,7 +1281,6 @@ static pb_status launch_centroid_scores(pb_index *ix, Workspace &ws, int B, int 
     });
     CK(cudaGetLastError());
     if (launches) *launches += 2;
-    if (with16 && ix->k1_diag && ix->cent_h16t.p) CKS(launch_k1_diag(ix, ws, B, QS));
     return PB_OK;
 }
 
@@ -1365,24 +1354,8 @@ static pb_status launch_exact(pb_index *ix, Workspace &ws, const KeptView &kv, c
     return PB_OK;
 }
 
-static size_t smem_exact_tc(int dim, int packed, int nqt) {
-    const int nbits = packed * 8 / dim;
-    return (size_t)(dim / 8) * PB_XTC_LBO + (size_t)nqt * dim * 2 + (size_t)256 * (8 / nbits) * 2 +
-           (size_t)128 * ACC_LD(nqt) * 4;
-}
-
-// error of one fp16 tensor-core similarity relative to |q| (derivation above k_exact_tc); 0 = filter unusable
-static float filter_eps_unit(const pb_index *ix) {
-    const float u = 1.0f / 2048.0f;  // fp16 unit roundoff
-    const float vmin = ix->vmin * 0.9999f, wmax = ix->wmax * 1.0001f;
-    if (!(vmin > 0.0f) || !(ix->cmax < 3.0e4f) || !(wmax < 3.0e4f)) return 0.0f;  // operands must fit fp16
-    const float rho = u * ((ix->cmax + wmax) / vmin + 1.0f) * (1.0f + 2.0f * u);  // |v - v~| / |v|
-    if (!(rho < 0.25f)) return 0.0f;
-    const float sub = 3.0f * sqrtf((float)ix->dim) * 2.98e-8f / vmin;  // fp16 subnormal spacing 2^-25: h(c), h(w), their sum
-    return u + (1.0f + u) * rho / (1.0f - 0.5f * rho) + sub + 4e-5f;
-}
-
-// the same for the linear filter (derivation above k_maxsim_tc and in DESIGN.md 4c); E = code error of the score table (0 = exact table)
+// error of one tensor-core similarity estimate relative to |q| (derivation at the top of k_filter_tc.cuh and in DESIGN.md 4c);
+// E = code error of the score table (0 = exact table); 0 = filter unusable
 static float filter_eps_unit2(const pb_index *ix, int E) {
     const float u = 1.0f / 2048.0f;
     const float vmin = ix->vmin * 0.9999f, wmax = ix->wmax * 1.0001f;
@@ -1461,48 +1434,13 @@ static pb_status launch_maxsim_tc(pb_index *ix, Workspace &ws, const KeptView &i
 
 // a7': tensor-core estimate of every kept doc, then the survivors that can still reach the top_k
 static pb_status launch_filter(pb_index *ix, Workspace &ws, const KeptView &in, const KeptView &out, const TokView &tv, int B,
-                               int QS, int Mcap, int top_k, long long max_tokens, float eps_unit, int nq_max, bool linear,
+                               int QS, int Mcap, int top_k, long long max_tokens, float eps_unit, int nq_max,
                                bool keep_keys, int *launches) {
-    long long chunks = (max_tokens + 127) / 128;
-    long long want = std::max<long long>(1, ((long long)ix->sm_count * ix->xtc_grid + B - 1) / B);
-    int gx = (int)std::max<long long>(1, std::min<long long>(chunks, want));
-    const int nqt = nq_max <= 32 ? 32 : 64;
-    const size_t sm = smem_exact_tc(ix->dim, ix->packed, nqt);
     // keep_keys: the per (doc, q) maxima go to their own buffer and stay there for the pair pass of the exact stage
     uint32_t *keys = keep_keys ? ws.estkey.as<uint32_t>() : ws.maxkey.as<uint32_t>();
     if (keep_keys) CK(cudaMemsetAsync(keys, 0, (size_t)B * Mcap * QS * 4, ws.stream));
-    if (linear) {
-        CKS(launch_maxsim_tc(ix, ws, in, tv, B, QS, Mcap, max_tokens, nq_max, keys, nullptr, 0.0f, nullptr, nullptr, 0,
-                             PB_KERNEL_FILTER));
-    } else {
-#define PB_TC_LAUNCH(DV, NB)                                                                                           \
-    {                                                                                                                  \
-        auto kern = nqt == 32 ? k_exact_tc<DV, NB, 32> : k_exact_tc<DV, NB, 64>;                                       \
-        CKS(set_smem(kern, sm));                                                                                       \
-        KEV_BEGIN(PB_KERNEL_FILTER);                                                                                   \
-        kern<<<dim3(gx, B), 128, sm, ws.stream>>>(ws.Q.as<float>(), ws.qoff.as<int>(), QS, ws.qexp.as<int>(),          \
-                                                  ix->centroids_f16.as<__half>(), ix->w_rev.as<float>(),               \
-                                                  tv.codes, tv.residuals,                                              \
-                                                  tv.doc_off, in.kept, in.nkept, in.tokp, Mcap, keys);                 \
-        KEV_END(PB_KERNEL_FILTER);                                                                                     \
-    }
-#define PB_TC_NBITS(DV)                                                                                                \
-    switch (ix->nbits) {                                                                                               \
-        case 1: PB_TC_LAUNCH(DV, 1) break;                                                                             \
-        case 2: PB_TC_LAUNCH(DV, 2) break;                                                                             \
-        case 4: PB_TC_LAUNCH(DV, 4) break;                                                                             \
-        default: PB_TC_LAUNCH(DV, 8) break;                                                                            \
-    }
-        switch (ix->dim) {
-            case 64: PB_TC_NBITS(64) break;
-            case 96: PB_TC_NBITS(96) break;
-            case 128: PB_TC_NBITS(128) break;
-            default: return pb_fail(PB_ERR_UNSUPPORTED, "filter: unsupported dim");
-        }
-#undef PB_TC_NBITS
-#undef PB_TC_LAUNCH
-        CK(cudaGetLastError());
-    }
+    CKS(launch_maxsim_tc(ix, ws, in, tv, B, QS, Mcap, max_tokens, nq_max, keys, nullptr, 0.0f, nullptr, nullptr, 0,
+                         PB_KERNEL_FILTER));
     k_tc_finalize<<<dim3((Mcap + 7) / 8, B), 256, 0, ws.stream>>>(keys, ws.qoff.as<int>(), QS, in.nkept, Mcap, in.tokp,
                                                                   ws.est.as<float>(), keep_keys ? 0 : 1);
     CK(cudaGetLastError());
@@ -1696,7 +1634,8 @@ struct Pass {
     // a5: the candidates that carry an approximate score
     const uint32_t *cand_list = nullptr;
     const int *cand_n = nullptr;
-    // a7: the filter's form, and the docs scored exactly
+    // a7: whether the certified filter runs (decided before a2, which makes its 16-bit table), its form, and the docs
+    // scored exactly
     bool filt = false, pairs = false, diag = false;
     KeptView kv{};
     // a9: the results of the sub-batch on the device
@@ -1727,13 +1666,15 @@ static pb_status upload_queries(pb_index *ix, Workspace &ws, const SearchIO &io,
     return PB_OK;
 }
 
-// a2: the centroid score table, fp32 off the tensor cores and 16-bit on a fast pass; on the tensor cores also a3
+// a2: the centroid score table, fp32 off the tensor cores and 16-bit for a fast pass or the filter; on the tensor cores
+// also a3
 static pb_status centroid_scores(pb_index *ix, Workspace &ws, const pb_search_params *p, const SearchPlan &plan,
                                  Pass &pass) {
     const int B = pass.B, QS = pass.QS;
     int *L = g_stats.launches;
     if (!pass.use_tc) CKS(ws.ST.ensure((size_t)B * ix->K * QS * sizeof(float)));
-    if (pass.fast) {
+    const bool with16 = pass.fast || pass.filt;
+    if (with16) {
         CKS(ws.ST16.ensure((size_t)B * ix->K * QS * 2));
         CKS(ws.qrange.ensure((size_t)B * 8 + 16));
         CKS(ws.qflag.ensure((size_t)B * 4 + 16));
@@ -1748,7 +1689,10 @@ static pb_status centroid_scores(pb_index *ix, Workspace &ws, const pb_search_pa
     if (pass.use_tc)
         return run_k1_tc(ix, ws, p, B, QS, pass.nq_max, plan.n_probe, plan.batched, L, &pass.cells_cap,
                          &pass.d_probe_fallback);
-    return launch_centroid_scores(ix, ws, B, QS, &L[PB_STAGE_CENTROID_SCORES], pass.fast);
+    CKS(launch_centroid_scores(ix, ws, B, QS, &L[PB_STAGE_CENTROID_SCORES], with16));
+    // PB_K1_TC_DIAG: the tensor-core table next to the exact one, compared code by code
+    if (pass.fast && ix->k1_diag && ix->cent_h16t.p) CKS(launch_k1_diag(ix, ws, B, QS));
+    return PB_OK;
 }
 
 // a3: the cells (centroids) each query probes, on the fp32 table; the tensor-core pass placed them in a2
@@ -2000,7 +1944,7 @@ static pb_status stage_kept(pb_index *ix, Workspace &ws, const SearchPlan &plan,
 
 // a7 + a8: the exact MaxSim of the kept docs.  Only the top_k need exact scores: the tensor-core filter (a7') first
 // drops the docs that provably cannot reach them, and its pass 2 lists the (token, q) pairs k_pair_exact evaluates.
-static pb_status exact_scores(pb_index *ix, Workspace &ws, const SearchIO &io, const SearchPlan &plan, Pass &pass) {
+static pb_status exact_scores(pb_index *ix, Workspace &ws, const SearchPlan &plan, Pass &pass) {
     const int B = pass.B, QS = pass.QS, nq_max = pass.nq_max, Mcap = plan.Mcap;
     const bool sharded = plan.sharded;
     const long long max_tokens = (long long)Mcap * std::max(ix->max_doclen, 1);
@@ -2012,12 +1956,7 @@ static pb_status exact_scores(pb_index *ix, Workspace &ws, const SearchIO &io, c
     kv = {ws.kept.as<uint32_t>(), ws.nkept.as<int>(), ws.tokp.as<long long>(), sharded ? ws.krank.as<uint32_t>() : nullptr};
     TokView tv = resident_tokens(ix);
     if (ix->host_tier) CKS(stage_kept(ix, ws, plan, pass, kv, tv));
-    // the linear form needs the 16-bit score table of this pass (a flagged query publishes no estimate and keeps
-    // every doc); without a table (PB_FAST_APPROX=0) the decompressing form estimates from fp16 centroids
-    const bool linear = pass.fast && !ix->filter_v1 && ix->tok_inv_norm.p;
-    const float eps_unit = linear ? filter_eps_unit2(ix, pass.use_tc ? ix->k1_margin : 0) : filter_eps_unit(ix);
-    pass.filt = ix->fast_exact && !io.trace && ix->centroids_f16.p && eps_unit > 0.0f && nq_max <= 64 &&
-                plan.top_k < Mcap && ix->packed % 4 == 0;
+    const float eps_unit = filter_eps_unit2(ix, pass.use_tc ? ix->k1_margin : 0);
     // PB_FILTER_DIAG: the filter runs as usual, then every kept doc is scored exactly (the results of
     // pb_set_fast_exact(0)) and k_filter_diag compares the pass-1 estimate maxima with the exact ones
     pass.diag = pass.filt && ix->filter_diag;
@@ -2028,24 +1967,16 @@ static pb_status exact_scores(pb_index *ix, Workspace &ws, const SearchIO &io, c
         CKS(ws.nkept2.ensure((size_t)B * 4 + 16));
         CKS(ws.tokp2.ensure((size_t)B * (Mcap + 1) * 8));
         CKS(ws.ktok2.ensure((size_t)B * 8 + 16));
-        if (!pass.fast) {  // the two-pass mode computed them with the score range
-            CKS(ws.qnmax.ensure((size_t)B * 4 + 16));
-            CKS(ws.qexp.ensure((size_t)B * 4 + 16));
-            k_query_range<<<B, 256, 0, ws.stream>>>(ws.Q.as<float>(), ws.qoff.as<int>(), ix->dim, ix->cmax, nullptr, nullptr,
-                                                    ws.qexp.as<int>(), ws.qnmax.as<float>());
-            CK(cudaGetLastError());
-            L[PB_STAGE_EXACT] += 1;
-        }
         KeptView kv2{ws.kept2.as<uint32_t>(), ws.nkept2.as<int>(), ws.tokp2.as<long long>(), ws.krank2.as<uint32_t>()};
         // pair form of the exact stage: pass 2 of the estimate over the survivors lists the (token, q) pairs that can
         // hold a per-token maximum, k_pair_exact evaluates them in the pinned order; a query whose list overflows
         // (or that published no estimate) goes through k_exact
-        pass.pairs = !pass.diag && linear && ix->pair_exact && Mcap <= 65535 && QS <= 256;
+        pass.pairs = !pass.diag && ix->pair_exact && Mcap <= 65535 && QS <= 256;
         if (pass.pairs || pass.diag) {
             CKS(ws.estkey.ensure((size_t)B * Mcap * QS * 4));
             CKS(ws.srcrank.ensure((size_t)B * Mcap * 4));
         }
-        CKS(launch_filter(ix, ws, kv, kv2, tv, B, QS, Mcap, plan.top_k, max_tokens, eps_unit, nq_max, linear,
+        CKS(launch_filter(ix, ws, kv, kv2, tv, B, QS, Mcap, plan.top_k, max_tokens, eps_unit, nq_max,
                           pass.pairs || pass.diag, &L[PB_STAGE_EXACT]));
         if (!pass.diag) {
             kv = kv2;
@@ -2090,8 +2021,7 @@ static pb_status exact_scores(pb_index *ix, Workspace &ws, const SearchIO &io, c
         CKS(ws.fdiag.ensure(16));
         CK(cudaMemsetAsync(ws.fdiag.p, 0, 16, ws.stream));
         k_filter_diag<<<dim3(4, B), 256, 0, ws.stream>>>(ws.estkey.as<uint32_t>(), ws.maxkey.as<uint32_t>(), ws.qoff.as<int>(),
-                                                         QS, kv.nkept, Mcap, ws.qnmax.as<float>(),
-                                                         linear ? ws.qflag.as<int>() : nullptr, eps_unit,
+                                                         QS, kv.nkept, Mcap, ws.qnmax.as<float>(), ws.qflag.as<int>(), eps_unit,
                                                          ws.fdiag.as<unsigned long long>());
         CK(cudaGetLastError());
         L[PB_STAGE_EXACT] += 1;
@@ -2320,13 +2250,20 @@ static pb_status run_pass(pb_index *ix, Workspace &ws, const pb_search_params *p
     CK(mark(5));
     CKS(cut(ix, ws, plan, pass));
     CK(mark(6));
-    CKS(exact_scores(ix, ws, io, plan, pass));
+    CKS(exact_scores(ix, ws, plan, pass));
     CK(mark(7));
     CKS(select_topk(ix, ws, io, plan, pass));
     CK(mark(8));
     CKS(finish(ix, ws, io, plan, pass, redo));  // D2H ends at ws.ev[9]
     if (!*redo && io.trace) CKS(dump_trace(ix, ws, io, plan, pass));
     return PB_OK;
+}
+
+// a7': whether the certified filter runs on a pass; a2 then makes the pass's 16-bit table, which the estimate reads.
+// The certificate depends on the table's code error, so a tensor-core pass redone on the exact path decides again.
+static bool filter_runs(const pb_index *ix, const SearchIO &io, const SearchPlan &plan, const Pass &pass) {
+    return ix->fast_exact && !io.trace && ix->tok_inv_norm.p && filter_eps_unit2(ix, pass.use_tc ? ix->k1_margin : 0) > 0.0f &&
+           pass.nq_max <= 64 && plan.top_k < plan.Mcap && ix->packed % 4 == 0;
 }
 
 // One search call (or one lane of it): the plan, the workspace, then the sub-batches in order
@@ -2381,11 +2318,13 @@ static pb_status run_search(pb_index *ix, const pb_search_params *p, const Searc
         pass.use_tc = k1_tc_usable(ix) && pass.fast && ix->probe16 && !ix->k1_diag && !plan.all_eligible &&
                       !plan.big_probe && !plan.d_elig && pass.QS / 8 <= 32 && n_chunks_k >= plan.n_probe &&
                       plan.n_probe <= 192;
+        pass.filt = filter_runs(ix, io, plan, pass);
         bool redo = false;
         CKS(run_pass(ix, ws, p, io, plan, pass, &redo));
         if (redo) {
             g_stats.work.n_k1_tc_redo += 1;
             pass.use_tc = false;
+            pass.filt = filter_runs(ix, io, plan, pass);
             CKS(run_pass(ix, ws, p, io, plan, pass, &redo));
         }
     }

@@ -23,7 +23,11 @@
 //   pairs (a little over one per (doc, q)) are listed; k_pair_exact decompresses each token and evaluates the dot
 //   in the pinned order (codec.rs:443-467, maxsim.rs:281): the same per-token maxima as k_exact, from ~1/250 of
 //   the arithmetic.  A query whose list overflows is left to k_exact (per-query flag).
+// Residual operand tile: canonical K-major fp16, element (token row r, 8-wide K chunk kc) at
+// kc * LBO + (r/8) * 128 + (r%8) * 16 = kc * LBO + 16 r, with LBO = 2048 + 32 bytes between K chunks.
 // ==========================================================================================
+#define PB_XTC_LBO 2080u
+
 struct MsMeta {
     long long g;
     int r;

@@ -11,8 +11,7 @@
 //                                                                          search.rs:305-324 / :275-302
 //   k_cut ............... a6  stable top-(n_full_scores -> /4) cut        search.rs:460-469
 //   k_maxsim_tc/k_tc_finalize/k_tc_select  a7' wgmma certified estimate: which kept docs can reach the top_k (pass 1),
-//                             which (token, query token) pairs of them can hold a maximum (pass 2); k_exact_tc = the
-//                             decompressing form for the table-less mode
+//                             which (token, query token) pairs of them can hold a maximum (pass 2)
 //   k_pair_exact ........ a7+a8 decompress + pinned fp32 dot of the listed pairs   codec.rs:423-470, maxsim.rs:270-294
 //   k_exact ............. a7+a8 fused residual decompress + MaxSim of every token (filter off, flagged queries, trace)
 //   k_exact_finalize .... a8  q-ordered sum of per-token maxima           maxsim.rs:284-291

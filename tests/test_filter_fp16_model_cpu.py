@@ -1,4 +1,4 @@
-"""Executable statement of the residual term of the MaxSim filter's certificate (k_maxsim_tc / k_exact_tc, DESIGN.md 4c).
+"""Executable statement of the residual term of the MaxSim filter's certificate (k_maxsim_tc, DESIGN.md 4c).
 The tensor cores take q.w from fp16 operands: the query row scaled by 2^qexp (qexp = -ilogb(|q|max), so the largest
 scaled row norm is in [1, 2)), the bucket weights as they are; products are exact, sums are fp32; the result is scaled
 back by 2^-qexp.  The certificate charges this term

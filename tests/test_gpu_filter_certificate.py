@@ -1,19 +1,18 @@
-"""The MaxSim filter's certificate measured on the device (k_maxsim_tc, k_exact_tc; DESIGN.md 4c).  Every similarity
-estimate of the filter must lie within eps_q = |q|max * eps_unit of the exact one, or a doc (pass 1) or a (token, query
-token) pair (pass 2) that holds a result is dropped.  PB_FILTER_DIAG=1 scores every kept doc exactly and reports the
-largest |pass-1 estimate maximum - exact maximum| / eps_q (filter_err_ratio_e6, in millionths): here it must stay <= 1
-over the filter forms, dims, bit widths, query shapes and scales, and indexes with extreme constants.  Then near ties
-built in the codec domain -- docs and tokens whose exact scores sit inside the bands -- must come out bit for bit as
+"""The MaxSim filter's certificate measured on the device (k_maxsim_tc; DESIGN.md 4c).  Every similarity estimate of
+the filter must lie within eps_q = |q|max * eps_unit of the exact one, or a doc (pass 1) or a (token, query token) pair
+(pass 2) that holds a result is dropped.  PB_FILTER_DIAG=1 scores every kept doc exactly and reports the largest
+|pass-1 estimate maximum - exact maximum| / eps_q (filter_err_ratio_e6, in millionths): here it must stay <= 1 on the
+tensor-core table, the exact table and without a table, over dims, bit widths, query shapes and scales, and indexes
+with extreme constants.  Then near ties built in the codec domain -- docs and tokens whose exact scores sit inside the bands -- must come out bit for bit as
 the CPU oracle's while the filter really decides them."""
 import numpy as np
 import pytest
 
 pytestmark = pytest.mark.gpu
 
-MODES = {"linear_tc_table": {}, "linear_exact_table": {"PB_K1_TC": "0"}, "decompressing": {"PB_FILTER_V1": "1"},
-         "no_score_table": {"PB_FAST_APPROX": "0"}}
+MODES = {"linear_tc_table": {}, "linear_exact_table": {"PB_K1_TC": "0"}, "no_score_table": {"PB_FAST_APPROX": "0"}}
 KW = dict(top_k=10, n_ivf_probe=8, n_full_scores=256, centroid_score_threshold=None)   # any query scale finds candidates
-ENVS = ("PB_FILTER_DIAG", "PB_K1_TC", "PB_FILTER_V1", "PB_FAST_APPROX")
+ENVS = ("PB_FILTER_DIAG", "PB_K1_TC", "PB_FAST_APPROX")
 
 
 @pytest.fixture(scope="module")

@@ -423,12 +423,13 @@ def test_long_queries_keep_the_fast_paths(oracle, npb, corpus, nq):
             assert np.array_equal(r.scores, w.scores), (kw, nq)
 
 
-@pytest.mark.parametrize("env", [{"PB_FILTER_V1": "1"}, {"PB_FAST_APPROX": "0"}, {"PB_K1_TC": "0"}, {"PB_PAIR_EXACT": "0"}, {}])
-def test_both_filter_kernels_and_their_score_tables(oracle, npb, corpus, monkeypatch, env):
-    # the linear filter (k_maxsim_tc: centroid score from the 16-bit table + residual part on the tensor cores) on the
-    # tensor-core table (default) and on the exact table (PB_K1_TC=0); the decompressing filter (k_exact_tc) when
-    # forced (PB_FILTER_V1=1) or when there is no table (PB_FAST_APPROX=0); the exact stage on the (token, q) pairs
-    # inside the certified band (default) or on every token of the survivors (PB_PAIR_EXACT=0)
+@pytest.mark.parametrize("env", [{"PB_FAST_APPROX": "0"}, {"PB_K1_TC": "0"}, {"PB_PAIR_EXACT": "0"}, {},
+                                 {"PB_FAST_APPROX": "0", "PB_PAIR_EXACT": "0"}])
+def test_the_filter_on_the_tensor_core_table_the_exact_table_and_no_table(oracle, npb, corpus, monkeypatch, env):
+    # the filter (k_maxsim_tc: centroid score from the 16-bit table + residual part on the tensor cores) on the
+    # tensor-core table (default), on the exact table (PB_K1_TC=0) and without a score table (PB_FAST_APPROX=0), where
+    # a2 writes the exact table's 16-bit codes for it; the exact stage on the (token, q) pairs inside the certified
+    # band (default) or on every token of the survivors (PB_PAIR_EXACT=0)
     docs, ix, qs, src, _ = corpus
     for k, v in env.items():
         monkeypatch.setenv(k, v)
@@ -443,7 +444,7 @@ def test_both_filter_kernels_and_their_score_tables(oracle, npb, corpus, monkeyp
             res = gpu.search_batch(batch, pg)
             w = gpu.last_work_counters()
             assert 0 < w["n_exact_docs"] < w["n_filter_docs"], (env, kw, w)
-            pair_form = not env or set(env) == {"PB_K1_TC"}
+            pair_form = "PB_PAIR_EXACT" not in env
             assert (w["n_exact_pairs"] > 0) == pair_form, (env, kw, w)
             if pair_form:   # a little over one pair per (survivor, query token), never every token
                 assert w["n_pair_fallback_queries"] == 0, (env, kw, w)

@@ -16,7 +16,6 @@ VARIANTS = [
     ("approx grid x4", {"PB_APPROX_GRID": "4"}),
     ("filter off", {"PB_FAST_EXACT": "0"}),
     ("list-scan probe (exact a2)", {"PB_PROBE16": "0", "PB_K1_TC": "0"}),
-    ("decompressing filter (PB_FILTER_V1)", {"PB_FILTER_V1": "1"}),
     ("token-form exact stage (PB_PAIR_EXACT=0)", {"PB_PAIR_EXACT": "0"}),
     ("pass-2 grid 1", {"PB_WS_GRID2": "1"}),
     ("pass-2 grid 4", {"PB_WS_GRID2": "4"}),
