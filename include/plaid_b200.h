@@ -377,13 +377,14 @@ PB_API void pb_set_fast_approx(pb_index *ix, int32_t enabled);
 /* Diagnostic switch for the exact stage (default on): 1 = an fp16 wgmma estimate with a certified error bound
  * first picks the kept docs that can still reach the top_k, and only those are scored exactly; 0 = every kept
  * doc is scored exactly.  Same results bit for bit; tests compare both.  (PB_FAST_EXACT=0 in the environment
- * sets the default.)  The filter applies when dim is 64/96/128, queries have <= 64 tokens and no trace is asked. */
+ * sets the default.)  The filter applies when dim is 48/64/96/128, dim * nbits / 8 is a multiple of 4 (not at dim 48
+ * with nbits 1), queries have <= 64 tokens and no trace is asked. */
 PB_API void pb_set_fast_exact(pb_index *ix, int32_t enabled);
 
 /* Diagnostic switch for a2 (default on): 1 = the score table comes from the wgmma split-fp16 GEMM (k_scores16_tc) and
  * the values that decide something are recomputed as pinned-order fp32 dots; 0 = the dense fp32 FMA kernel
  * (k_centroid_scores), which is also the device-gated fallback for flagged queries and shapes outside the tensor-core
- * kernel's (dim not in {64, 96, 128}, eligibility filters, the dense variant's radix-select probe for n_ivf_probe > 64, n_ivf_probe > K/1024).  Same results bit
+ * kernel's (dim not in {48, 64, 96, 128}, eligibility filters, the dense variant's radix-select probe for n_ivf_probe > 64, n_ivf_probe > K/1024).  Same results bit
  * for bit; tests and bench.py compare both.  (PB_K1_TC=0 in the environment sets the default.) */
 PB_API void pb_set_scores_tc(pb_index *ix, int32_t enabled);
 
@@ -472,7 +473,7 @@ PB_API pb_status pb_codec_open(int32_t device, const float *centroids, int64_t n
 PB_API void pb_codec_close(pb_codec *c);
 /* How the last compress/encode call found its codes: tokens whose argmax the wgmma shortlist certified
  * vs tokens sent through the exact fp32 kernel (all of them when the filter is not in use: dim not in
- * {64, 96, 128}, K < 256, or PB_ASSIGN_EXACT set). */
+ * {48, 64, 96, 128}, K < 256, or PB_ASSIGN_EXACT set). */
 PB_API pb_status pb_codec_last_assign_stats(pb_codec *c, int64_t *n_tokens, int64_t *n_exact_fallback,
                                             int32_t *used_tensor_cores);
 /* ResidualCodec::compress_into_codes (codec.rs:260): out_codes[n] i64 */

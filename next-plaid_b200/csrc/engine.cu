@@ -17,6 +17,7 @@
 #include <functional>
 #include <map>
 #include <thread>
+#include <type_traits>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -482,17 +483,39 @@ struct pb_index {
 };
 
 // ------------------------------------------------------------------------------------------
-// DIM dispatch
+// DIM dispatch.  The embedding widths are listed here and nowhere else:
+//   BuiltDims  every DIM-templated kernel is instantiated for these (a handle, codec or k-means of another dim is
+//              refused with PB_ERR_UNSUPPORTED);
+//   TcDims     the tensor-core paths run at these: a2 on wgmma (k_scores16_tc), the MaxSim filter (k_maxsim_tc,
+//              k_pair_exact, the token norms it needs) and the tensor-core assignment (k_assign_tc).  A multiple of 16
+//              (wgmma K = 16) whose error bound k1_err_codes keeps E = 1; 32 and 256 stay on the fp32 kernels.
+// dispatch(d, f) calls f(std::integral_constant<int, d>) for a listed d and fails for any other: no switch falls through
+// to another width's kernel.
 // ------------------------------------------------------------------------------------------
-#define PB_DIM_SWITCH(dim, ...)                                                                    \
-    switch (dim) {                                                                                 \
-        case 32: { constexpr int DIM = 32; __VA_ARGS__; } break;                                   \
-        case 64: { constexpr int DIM = 64; __VA_ARGS__; } break;                                   \
-        case 96: { constexpr int DIM = 96; __VA_ARGS__; } break;                                   \
-        case 128: { constexpr int DIM = 128; __VA_ARGS__; } break;                                 \
-        case 256: { constexpr int DIM = 256; __VA_ARGS__; } break;                                 \
-        default: return pb_fail(PB_ERR_UNSUPPORTED, "embedding_dim %d not built (32/64/96/128/256)", dim); \
+template <int... Ds> struct DimSet {
+    static bool has(int d) { return ((d == Ds) || ...); }
+    static pb_status check(int d) {
+        if (has(d)) return PB_OK;
+        std::string list;
+        ((list += (list.empty() ? "" : "/") + std::to_string(Ds)), ...);
+        return pb_fail(PB_ERR_UNSUPPORTED, "embedding_dim %d not built (%s)", d, list.c_str());
     }
+    template <class F> static pb_status dispatch(int d, F &&f) {
+        pb_status s = PB_OK;
+        const bool hit = ((d == Ds ? (s = f(std::integral_constant<int, Ds>()), true) : false) || ...);
+        return hit ? s : check(d);
+    }
+};
+using BuiltDims = DimSet<32, 48, 64, 96, 128, 256>;
+using TcDims = DimSet<48, 64, 96, 128>;
+
+// the statements after `dim` with DIM bound to the handle's width, for every built width
+#define PB_DIM_SWITCH(dim, ...)                                                                                        \
+    CKS(BuiltDims::dispatch(dim, [&](auto dim_c) -> pb_status {                                                        \
+        constexpr int DIM = decltype(dim_c)::value;                                                                    \
+        __VA_ARGS__;                                                                                                   \
+        return PB_OK;                                                                                                  \
+    }))
 
 // QS: query tokens per score-table row.  Up to 32 tokens: rounded up to 8 (rows of at most 64 bytes); beyond: to a
 // multiple of 64, so that a row is whole 128-byte lines (a 96-byte row straddles lines and costs the first approximate
@@ -500,8 +523,6 @@ struct pb_index {
 static int query_row_tokens(int nq_max) {
     return nq_max <= 32 ? std::max(8, (nq_max + 7) & ~7) : ((nq_max + 63) & ~63);
 }
-
-static bool dim_supported(int d) { return d == 32 || d == 64 || d == 96 || d == 128 || d == 256; }
 
 static size_t smem_scores(int dim) { return (size_t)(PB_TOK_TILE + 2 * PB_Q_TILE) * (dim + 4) * sizeof(float); }
 static size_t smem_exact(int dim, int packed) {
@@ -719,7 +740,7 @@ pb_status pb_index_open_begin(const pb_index_desc *d, pb_index **out) {
     if (d->nbits <= 0 || 8 % d->nbits != 0)  // codec.rs:161-166
         return pb_fail(PB_ERR_INVALID, "nbits must be a divisor of 8, got %d", d->nbits);
     if (d->dim <= 0 || d->dim % 4 != 0) return pb_fail(PB_ERR_INVALID, "embedding_dim %d must be a positive multiple of 4", d->dim);
-    if (!dim_supported(d->dim)) return pb_fail(PB_ERR_UNSUPPORTED, "embedding_dim %d not built (32/64/96/128/256)", d->dim);
+    CKS(BuiltDims::check(d->dim));
     if (d->num_centroids <= 0 || d->num_documents < 0 || d->num_embeddings < 0)
         return pb_fail(PB_ERR_INVALID, "bad shapes K=%lld D=%lld N=%lld", (long long)d->num_centroids,
                        (long long)d->num_documents, (long long)d->num_embeddings);
@@ -850,8 +871,6 @@ static pb_status build_ivf_on_device(pb_index *ix) {
     return PB_OK;
 }
 
-static bool filter_dim(int dim) { return dim == 64 || dim == 96 || dim == 128; }
-
 // Operands of the tensor-core kernels that depend on the centroids alone: the scaled hi / lo tiles of the score table
 // (k_scores16_tc).
 static pb_status build_centroid_operands(pb_index *ix) {
@@ -874,13 +893,12 @@ static pb_status build_centroid_operands(pb_index *ix) {
 static pb_status launch_min_vnorm(pb_index *ix, const uint32_t *codes, const uint8_t *res, long long n, float *inv,
                                   float *mn) {
     if (n == 0) return PB_OK;
-    switch (ix->dim) {
-        case 64: k_min_vnorm<64><<<ix->sm_count * 8, 256>>>(ix->centroids.as<float>(), ix->w_rev.as<float>(), ix->nbits, codes, res, n, mn, inv); break;
-        case 96: k_min_vnorm<96><<<ix->sm_count * 8, 256>>>(ix->centroids.as<float>(), ix->w_rev.as<float>(), ix->nbits, codes, res, n, mn, inv); break;
-        default: k_min_vnorm<128><<<ix->sm_count * 8, 256>>>(ix->centroids.as<float>(), ix->w_rev.as<float>(), ix->nbits, codes, res, n, mn, inv); break;
-    }
-    CK(cudaGetLastError());
-    return PB_OK;
+    return TcDims::dispatch(ix->dim, [&](auto dim_c) -> pb_status {
+        k_min_vnorm<decltype(dim_c)::value><<<ix->sm_count * 8, 256>>>(ix->centroids.as<float>(), ix->w_rev.as<float>(),
+                                                                      ix->nbits, codes, res, n, mn, inv);
+        CK(cudaGetLastError());
+        return PB_OK;
+    });
 }
 // the same for the handle's tokens [t0, t0 + n), into its tok_inv_norm.  A host-tier handle's rows go through a device
 // buffer in slabs of 2^22 tokens; the per-token values and the folded min / max do not depend on the slabs, so they are
@@ -939,7 +957,7 @@ pb_status pb_index_finalize(pb_index *ix) {
         if (const char *e = getenv("PB_K1_TC_E")) ix->k1_margin = std::max(1, atoi(e));
         if (const char *e = getenv("PB_APPROX_GRID")) ix->approx_grid = std::max(1, atoi(e));
     }
-    if (filter_dim(ix->dim) && ix->N > 0 && ix->K > 0) {
+    if (TcDims::has(ix->dim) && ix->N > 0 && ix->K > 0) {
         // operands of the tensor-core score table, and the token norms of the filter
         CKS(build_centroid_operands(ix));
         DevBuf mn;
@@ -1112,7 +1130,7 @@ static float k1_err_codes(int dim) {
     return (chain + tc + sub) * 32768.0f * 1.0001f;
 }
 static bool k1_tc_usable(const pb_index *ix) {
-    return ix->k1_tc && ix->cent_h16t.p && (ix->dim == 64 || ix->dim == 96 || ix->dim == 128) && k1_err_codes(ix->dim) < 1.0f;
+    return ix->k1_tc && ix->cent_h16t.p && TcDims::has(ix->dim) && k1_err_codes(ix->dim) < 1.0f;
 }
 
 // the 16-bit score table from the split-fp16 wgmma GEMM (k_scores16_tc) into `table`; `flags` gets the per-query
@@ -1129,30 +1147,22 @@ static pb_status launch_k1_table(pb_index *ix, Workspace &ws, int B, int QS, uns
                                                             ws.qrange_tc.as<float2>());
     const int tiles = (int)((ix->K + 127) / 128);
     const size_t sm = (size_t)6 * 128 * ix->dim * 2 + 128;
-#define PB_K1_LAUNCH(DV)                                                                                               \
-    {                                                                                                                  \
-        auto kern = k_scores16_tc<DV>;                                                                                 \
-        CKS(set_smem(kern, sm));                                                                                       \
-        KEV_BEGIN(PB_KERNEL_SCORES);                                                                                   \
-        kern<<<tiles, 288, sm, ws.stream>>>(ix->cent_h16t.as<__half>(), ix->cent_l16t.as<__half>(), ix->K,             \
-                                            ws.Qh16t.as<__half>(), ws.Ql16t.as<__half>(), n_groups, B, QS,             \
-                                            ws.qoff.as<int>(), ws.qrange_tc.as<float2>(), table, flags);               \
-        KEV_END(PB_KERNEL_SCORES);                                                                                     \
-    }
-    switch (ix->dim) {
-        case 64: PB_K1_LAUNCH(64) break;
-        case 96: PB_K1_LAUNCH(96) break;
-        case 128: PB_K1_LAUNCH(128) break;
-        default: return pb_fail(PB_ERR_UNSUPPORTED, "tensor-core score table: dim must be 64, 96 or 128");
-    }
-#undef PB_K1_LAUNCH
-    CK(cudaGetLastError());
-    return PB_OK;
+    return TcDims::dispatch(ix->dim, [&](auto dim_c) -> pb_status {
+        auto kern = k_scores16_tc<decltype(dim_c)::value>;
+        CKS(set_smem(kern, sm));
+        KEV_BEGIN(PB_KERNEL_SCORES);
+        kern<<<tiles, 288, sm, ws.stream>>>(ix->cent_h16t.as<__half>(), ix->cent_l16t.as<__half>(), ix->K,
+                                            ws.Qh16t.as<__half>(), ws.Ql16t.as<__half>(), n_groups, B, QS,
+                                            ws.qoff.as<int>(), ws.qrange_tc.as<float2>(), table, flags);
+        KEV_END(PB_KERNEL_SCORES);
+        CK(cudaGetLastError());
+        return PB_OK;
+    });
 }
 
 // diagnostic twin of the score table on the tensor cores, compared code by code with the exact one
 static pb_status launch_k1_diag(pb_index *ix, Workspace &ws, int B, int QS) {
-    if (!ix->cent_h16t.p || (ix->dim != 64 && ix->dim != 96 && ix->dim != 128)) return PB_OK;
+    if (!ix->cent_h16t.p || !TcDims::has(ix->dim)) return PB_OK;
     CKS(ws.ST16b.ensure((size_t)B * ix->K * QS * 2));
     CKS(ws.k1diag.ensure((size_t)(B + 4) * 4));
     CK(cudaMemsetAsync(ws.k1diag.p, 0, (size_t)(B + 4) * 4, ws.stream));
@@ -1371,7 +1381,7 @@ static float filter_eps_unit2(const pb_index *ix, int E) {
 
 static size_t smem_maxsim_tc(int dim, int packed, int nqt) {
     const int nbits = packed * 8 / dim;
-    return (size_t)2 * (dim / 8) * PB_XTC_LBO + (size_t)nqt * dim * 2 + (size_t)256 * (8 / nbits) * 2 * (nbits == 4 ? 4 : 1) +
+    return (size_t)2 * PB_XTC_STAGE(dim) + (size_t)nqt * dim * 2 + (size_t)256 * (8 / nbits) * 2 * (nbits == 4 ? 4 : 1) +
            4 * 128 * sizeof(MsMeta) + 8 * 8 + (size_t)128 * ACC_LD(nqt) * 4;
 }
 
@@ -1412,24 +1422,26 @@ static pb_status launch_maxsim_tc(pb_index *ix, Workspace &ws, const KeptView &i
     } else {                                                                                                           \
         if (nqt == 32) PB_MS_GO(DV, NB, 32, false) else PB_MS_GO(DV, NB, 64, false)                                    \
     }
-#define PB_MS_NBITS(DV)                                                                                                \
-    switch (ix->nbits) {                                                                                               \
-        case 1: PB_MS_LAUNCH(DV, 1) break;                                                                             \
-        case 2: PB_MS_LAUNCH(DV, 2) break;                                                                             \
-        case 4: PB_MS_LAUNCH(DV, 4) break;                                                                             \
-        default: PB_MS_LAUNCH(DV, 8) break;                                                                            \
-    }
-    switch (ix->dim) {
-        case 64: PB_MS_NBITS(64) break;
-        case 96: PB_MS_NBITS(96) break;
-        case 128: PB_MS_NBITS(128) break;
-        default: return pb_fail(PB_ERR_UNSUPPORTED, "filter: unsupported dim");
-    }
-#undef PB_MS_NBITS
+    return TcDims::dispatch(ix->dim, [&](auto dim_c) -> pb_status {
+        constexpr int DV = decltype(dim_c)::value;
+        switch (ix->nbits) {
+            case 1:
+                // 1-bit rows of DV / 8 bytes: whole 32-bit words unless DV % 32 != 0 (filter_runs keeps those off)
+                if constexpr (DV % 32 == 0) {
+                    PB_MS_LAUNCH(DV, 1)
+                    break;
+                } else {
+                    return pb_fail(PB_ERR_UNSUPPORTED, "filter: %d-byte 1-bit rows are not whole 32-bit words", DV / 8);
+                }
+            case 2: PB_MS_LAUNCH(DV, 2) break;
+            case 4: PB_MS_LAUNCH(DV, 4) break;
+            default: PB_MS_LAUNCH(DV, 8) break;
+        }
+        CK(cudaGetLastError());
+        return PB_OK;
+    });
 #undef PB_MS_LAUNCH
 #undef PB_MS_GO
-    CK(cudaGetLastError());
-    return PB_OK;
 }
 
 // a7': tensor-core estimate of every kept doc, then the survivors that can still reach the top_k
@@ -1914,6 +1926,11 @@ static pb_status stage_rows(pb_index *ix, Workspace &ws, const uint32_t *docs, c
         k_stage_rows<uint4, 4><<<grid, 256, 0, ws.stream>>>(docs, nkept, Mcap, n_slots, ix->doc_off.as<long long>(), soff,
                                                             ix->host_res.dev, ix->codes.as<uint32_t>(), src_inv, pk,
                                                             ws.s_res.as<uint8_t>(), ws.s_codes.as<uint32_t>(), dst_inv);
+    else if (pk % 4 != 0)  // 1-bit rows of dim 48 (6 bytes)
+        k_stage_rows<unsigned short, 8><<<grid, 256, 0, ws.stream>>>(docs, nkept, Mcap, n_slots, ix->doc_off.as<long long>(),
+                                                                     soff, ix->host_res.dev, ix->codes.as<uint32_t>(), src_inv,
+                                                                     pk, ws.s_res.as<uint8_t>(), ws.s_codes.as<uint32_t>(),
+                                                                     dst_inv);
     else
         k_stage_rows<uint32_t, 8><<<grid, 256, 0, ws.stream>>>(docs, nkept, Mcap, n_slots, ix->doc_off.as<long long>(), soff,
                                                                ix->host_res.dev, ix->codes.as<uint32_t>(), src_inv, pk,
@@ -1997,19 +2014,15 @@ static pb_status exact_scores(pb_index *ix, Workspace &ws, const SearchPlan &pla
         CK(cudaGetLastError());
         const size_t smp = ((size_t)(nq_max + 256) * (ix->dim + 1) + 256) * 4;
         const int pe_ctas = std::max(1, std::min(16, (2 * ix->sm_count + B - 1) / B));  // about one wave over the batch
-        switch (ix->dim) {
-#define PB_PE(DV)                                                                                                      \
-    case DV: {                                                                                                         \
-        CKS(set_smem(k_pair_exact<DV>, smp));                                                                          \
-        k_pair_exact<DV><<<dim3(pe_ctas, B), 256, smp, ws.stream>>>(                                                   \
-            ws.xpairs.as<u64>(), ws.xnpairs.as<int>(), pair_cap, ws.Q.as<float>(), ws.qoff.as<int>(), QS,              \
-            ix->centroids.as<float>(), ix->w_rev.as<float>(), ix->nbits, tv.codes,                                     \
-            tv.residuals, Mcap, ws.maxkey.as<uint32_t>());                                                             \
-    } break;
-            PB_PE(64) PB_PE(96) PB_PE(128)
-#undef PB_PE
-            default: return pb_fail(PB_ERR_UNSUPPORTED, "pair exact: unsupported dim");
-        }
+        CKS(TcDims::dispatch(ix->dim, [&](auto dim_c) -> pb_status {
+            auto kern = k_pair_exact<decltype(dim_c)::value>;
+            CKS(set_smem(kern, smp));
+            kern<<<dim3(pe_ctas, B), 256, smp, ws.stream>>>(ws.xpairs.as<u64>(), ws.xnpairs.as<int>(), pair_cap,
+                                                            ws.Q.as<float>(), ws.qoff.as<int>(), QS, ix->centroids.as<float>(),
+                                                            ix->w_rev.as<float>(), ix->nbits, tv.codes, tv.residuals, Mcap,
+                                                            ws.maxkey.as<uint32_t>());
+            return PB_OK;
+        }));
         CK(cudaGetLastError());
         L[PB_STAGE_EXACT] += 5;
         CKS(launch_exact(ix, ws, kv, tv, B, QS, Mcap, 0, max_tokens, &L[PB_STAGE_EXACT], ws.needexact.as<int>(), false));
@@ -2576,7 +2589,7 @@ extern "C" pb_status pb_decompress_documents(pb_index *ix, const int64_t *doc_id
 extern "C" pb_status pb_maxsim_scores(int32_t device, const float *query, int32_t nq, int32_t dim, const float *doc_tokens,
                                       const int64_t *doc_tok_offsets, int64_t n_docs, float *out_scores) {
     if ((!query && nq) || (!doc_tok_offsets) || (!out_scores && n_docs)) return pb_fail(PB_ERR_INVALID, "null argument");
-    if (!dim_supported(dim)) return pb_fail(PB_ERR_UNSUPPORTED, "embedding_dim %d not built (32/64/96/128/256)", dim);
+    CKS(BuiltDims::check(dim));
     if (nq < 0 || n_docs < 0) return pb_fail(PB_ERR_INVALID, "negative size");
     CKS(check_device(device));
     if (n_docs == 0) return PB_OK;
@@ -2601,19 +2614,13 @@ extern "C" pb_status pb_maxsim_scores(int32_t device, const float *query, int32_
     int sms = 0;
     CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
     int gx = (int)std::max<long long>(1, std::min<long long>(chunks, (long long)sms * 16));
-    switch (dim) {
-#define PB_CASE(DV)                                                                                              \
-    case DV: {                                                                                                   \
-        auto kern = k_exact<DV, true>;                                                                           \
-        CKS(set_smem(kern, smem_exact(DV, 0)));                                                                  \
-        kern<<<dim3(gx, 1), 128, smem_exact(DV, 0)>>>(dQ.as<float>(), dqoff.as<int>(), QS, nullptr, nullptr, 8, nullptr, \
-                                                   nullptr, nullptr, dtok.as<float>(), dkept.as<uint32_t>(),    \
-                                                   dnk.as<int>(), dtp.as<long long>(), Mcap, 0, dmax.as<uint32_t>(), nullptr); \
-    } break;
-        PB_CASE(32) PB_CASE(64) PB_CASE(96) PB_CASE(128) PB_CASE(256)
-#undef PB_CASE
-        default: break;
-    }
+    PB_DIM_SWITCH(dim, {
+        auto kern = k_exact<DIM, true>;
+        CKS(set_smem(kern, smem_exact(DIM, 0)));
+        kern<<<dim3(gx, 1), 128, smem_exact(DIM, 0)>>>(dQ.as<float>(), dqoff.as<int>(), QS, nullptr, nullptr, 8, nullptr,
+                                                       nullptr, nullptr, dtok.as<float>(), dkept.as<uint32_t>(), dnk.as<int>(),
+                                                       dtp.as<long long>(), Mcap, 0, dmax.as<uint32_t>(), nullptr);
+    });
     CK(cudaGetLastError());
     k_exact_finalize<<<dim3((Mcap + 7) / 8, 1), 256>>>(dmax.as<uint32_t>(), dqoff.as<int>(), QS, dnk.as<int>(), Mcap, 0,
                                                       dex.as<float>(), nullptr, nullptr, nullptr, 0u, nullptr);
@@ -2789,7 +2796,7 @@ extern "C" pb_status pb_codec_open(int32_t device, const float *centroids, int64
     *out = nullptr;
     if (nbits <= 0 || 8 % nbits != 0) return pb_fail(PB_ERR_INVALID, "nbits must be a divisor of 8, got %d", nbits);
     if (K <= 0 || K >= (1ll << 32) - 1) return pb_fail(PB_ERR_INVALID, "bad num_centroids %lld", (long long)K);
-    if (!dim_supported(dim)) return pb_fail(PB_ERR_UNSUPPORTED, "embedding_dim %d not built (32/64/96/128/256)", dim);
+    CKS(BuiltDims::check(dim));
     CKS(check_device(device));
     std::unique_ptr<pb_codec> c(new pb_codec());
     c->device = device;
@@ -2805,7 +2812,7 @@ extern "C" pb_status pb_codec_open(int32_t device, const float *centroids, int64
         c->has_cutoffs = true;
     }
     // tensor-core filter: fp16 copy of the centroids (tile order), their largest norm, finiteness
-    c->use_tc = (dim == 64 || dim == 96 || dim == 128) && K >= 256 && !getenv("PB_ASSIGN_EXACT") &&
+    c->use_tc = TcDims::has(dim) && K >= 256 && !getenv("PB_ASSIGN_EXACT") &&
                 smem_assign_tc(dim) <= 227 * 1024;
     if (c->use_tc) {
         const size_t kpad = (size_t)((K + 127) / 128) * 128;  // tile order, zero padded
@@ -2856,18 +2863,13 @@ static pb_status assign_codes(pb_codec *c, const float *dX, long long m, long lo
     k_rows_to_bf16<<<c->sm_count * 8, 256>>>(dX, m, c->dim, xb.as<__nv_bfloat16>(), xn.as<float>());
     const unsigned blocks = (unsigned)((m + 2 * PB_TC_M - 1) / (2 * PB_TC_M));
     const size_t sm = smem_assign_tc(c->dim);
-    switch (c->dim) {
-#define PB_TC_CASE(DV)                                                                                     \
-    case DV: {                                                                                             \
-        auto kern = k_assign_tc<DV, false>;                                                                \
-        CKS(set_smem(kern, sm));                                                                           \
-        kern<<<blocks, 288, sm>>>(xb.as<__nv_bfloat16>(), m, c->cent_bf16.as<__nv_bfloat16>(), c->K, ts.as<float>(), \
-                                  ti.as<uint32_t>(), nullptr);                                             \
-    } break;
-        PB_TC_CASE(64) PB_TC_CASE(96) PB_TC_CASE(128)
-#undef PB_TC_CASE
-        default: return pb_fail(PB_ERR_UNSUPPORTED, "tensor-core assignment not built for dim %d", c->dim);
-    }
+    CKS(TcDims::dispatch(c->dim, [&](auto dim_c) -> pb_status {
+        auto kern = k_assign_tc<decltype(dim_c)::value, false>;
+        CKS(set_smem(kern, sm));
+        kern<<<blocks, 288, sm>>>(xb.as<__nv_bfloat16>(), m, c->cent_bf16.as<__nv_bfloat16>(), c->K, ts.as<float>(),
+                                  ti.as<uint32_t>(), nullptr);
+        return PB_OK;
+    }));
     CK(cudaGetLastError());
     k_assign_certify<<<c->sm_count * 8, 256>>>(dX, m, c->dim, c->centroids.as<float>(), xn.as<float>(), c->cmax, c->c_finite,
                                                ts.as<float>(), ti.as<uint32_t>(), dcodes, nfb.as<int>(), fl.as<long long>());
@@ -3066,7 +3068,7 @@ extern "C" int64_t pb_codec_heldout_tokens(int64_t num_embeddings) {  // min(0.0
     return (int64_t)std::min(0.05 * (double)num_embeddings, 50000.0);
 }
 
-// k-means assignment step.  dims 64 / 96 / 128 with K >= 256: the fp16 wgmma GEMM of the encode path with the
+// k-means assignment step.  TcDims with K >= 256: the fp16 wgmma GEMM of the encode path with the
 // -|c|^2/2 bias added in its epilogue, best shortlist entry taken as is; otherwise the exact fp32 kernel.
 struct KmeansAssign {
     DevBuf xb, cb, bias, ts, ti, scratch;
@@ -3075,7 +3077,7 @@ struct KmeansAssign {
     int dim = 0, sms = 0;
     pb_status init(const float *dX, long long n_, int dim_, long long K_, int sms_, cudaStream_t st) {
         n = n_; K = K_; dim = dim_; sms = sms_;
-        tc = (dim == 64 || dim == 96 || dim == 128) && K >= 256 && n > 0 && !getenv("PB_KMEANS_EXACT");
+        tc = TcDims::has(dim) && K >= 256 && n > 0 && !getenv("PB_KMEANS_EXACT");
         if (!tc) return PB_OK;
         const size_t npad = (size_t)((n + 255) / 256) * 256, kpad = (size_t)((K + 127) / 128) * 128;
         CKS(xb.ensure(npad * dim * 2));
@@ -3100,18 +3102,13 @@ struct KmeansAssign {
         k_half_sqnorm_padded<<<sms * 4, 256, 0, st>>>(dC, K, (long long)kpad, dim, bias.as<float>());
         const unsigned blocks = (unsigned)((n + 2 * PB_TC_M - 1) / (2 * PB_TC_M));
         const size_t sm = (size_t)2 * PB_TC_M * dim * 2 + (size_t)PB_TC_STAGES * PB_TC_N * dim * 2 + (2 * PB_TC_STAGES + 5) * 8 + 16;
-        switch (dim) {
-#define PB_KM_CASE(DV)                                                                                                 \
-    case DV: {                                                                                                         \
-        auto kern = k_assign_tc<DV, true>;                                                                             \
-        CKS(set_smem(kern, sm));                                                                                       \
-        kern<<<blocks, 288, sm, st>>>(xb.as<__nv_bfloat16>(), n, cb.as<__nv_bfloat16>(), K, ts.as<float>(),            \
-                                      ti.as<uint32_t>(), bias.as<float>());                                            \
-    } break;
-            PB_KM_CASE(64) PB_KM_CASE(96) PB_KM_CASE(128)
-#undef PB_KM_CASE
-            default: return pb_fail(PB_ERR_UNSUPPORTED, "tensor-core k-means assignment not built for dim %d", dim);
-        }
+        CKS(TcDims::dispatch(dim, [&](auto dim_c) -> pb_status {
+            auto kern = k_assign_tc<decltype(dim_c)::value, true>;
+            CKS(set_smem(kern, sm));
+            kern<<<blocks, 288, sm, st>>>(xb.as<__nv_bfloat16>(), n, cb.as<__nv_bfloat16>(), K, ts.as<float>(),
+                                          ti.as<uint32_t>(), bias.as<float>());
+            return PB_OK;
+        }));
         k_take_top1<<<sms * 4, 256, 0, st>>>(ti.as<uint32_t>(), n, codes);
         CK(cudaGetLastError());
         return PB_OK;
@@ -3122,7 +3119,7 @@ extern "C" pb_status pb_kmeans_fit(int32_t device, const float *samples, int64_t
                                    uint64_t seed, float *out_centroids) {
     if (!samples || !out_centroids) return pb_fail(PB_ERR_INVALID, "null argument");
     if (n <= 0 || K <= 0 || K > n) return pb_fail(PB_ERR_INVALID, "need 0 < K <= n (K=%lld, n=%lld)", (long long)K, (long long)n);
-    if (!dim_supported(dim)) return pb_fail(PB_ERR_UNSUPPORTED, "embedding_dim %d not built (32/64/96/128/256)", dim);
+    CKS(BuiltDims::check(dim));
     CKS(check_device(device));
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, device));
@@ -3252,7 +3249,7 @@ extern "C" pb_status pb_kmeans_fit_dp(pb_build_comm *c, const float *samples, in
                                       int32_t niters, uint64_t seed, float *out_centroids) {
     if (!c || (!samples && n_local) || !out_centroids) return pb_fail(PB_ERR_INVALID, "null argument");
     if (n_local < 0 || K <= 0) return pb_fail(PB_ERR_INVALID, "bad sizes");
-    if (!dim_supported(dim)) return pb_fail(PB_ERR_UNSUPPORTED, "embedding_dim %d not built (32/64/96/128/256)", dim);
+    CKS(BuiltDims::check(dim));
     CK(cudaSetDevice(c->device));
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, c->device));
@@ -3429,7 +3426,7 @@ static pb_status append_prepare(pb_index *ix, pb_codec *codec, const float *embe
     if (ntok > 0 && ((codec && !embeddings) || (!codec && (!codes || !residuals)))) return pb_fail(PB_ERR_INVALID, "null argument");
     const long long N1 = N0 + ntok, D1 = D0 + n;
     const size_t pk = (size_t)ix->packed;
-    const bool filter = filter_dim(ix->dim) && N1 > 0;
+    const bool filter = TcDims::has(ix->dim) && N1 > 0;
 
     // capacity: grown arrays keep their contents; nothing below is visible until the commit
     CKS(ix->codes.grow((size_t)N1 * 4, (size_t)N0 * 4));
@@ -3627,7 +3624,7 @@ extern "C" pb_status pb_index_reserve(pb_index *ix, int64_t num_documents, int64
     const long long U1 = ix->n_ucodes + dn + 7 * dd, L1 = ix->ivf_len + dn;
     CKS(ix->codes.grow((size_t)N1 * 4, (size_t)ix->N * 4, false));
     CKS(ix->residuals.grow((size_t)N1 * ix->packed, (size_t)ix->N * ix->packed, false));
-    if (filter_dim(ix->dim)) CKS(ix->tok_inv_norm.grow((size_t)N1 * 4, (size_t)ix->N * 4, false));
+    if (TcDims::has(ix->dim)) CKS(ix->tok_inv_norm.grow((size_t)N1 * 4, (size_t)ix->N * 4, false));
     CKS(ix->doc_off.grow((size_t)(D1 + 1) * 8, (size_t)(ix->D + 1) * 8, false));
     CKS(ix->udoc_off.grow((size_t)(D1 + 1) * 8, (size_t)(ix->D + 1) * 8, false));
     CKS(ix->ucodes.grow((size_t)U1 * 4, (size_t)ix->n_ucodes * 4, false));
@@ -3787,9 +3784,13 @@ static pb_status delete_commit(pb_index *ix, DeletePrep &p) {
         const long long *kp = p.kept.as<long long>();
         k_compact_gather<uint32_t><<<blocks, 256>>>(ix->codes.as<uint8_t>(), ix->doc_off.as<long long>(), kp,
                                                     p.new_doff.as<long long>(), j0, j1, 4, p.st_codes.as<uint8_t>());
-        if (pk % 16 == 0)  // dim * nbits / 8 is a multiple of 4 for every supported dim
+        if (pk % 16 == 0)
             k_compact_gather<uint4><<<blocks, 256>>>(ix->residuals.as<uint8_t>(), ix->doc_off.as<long long>(), kp,
                                                      p.new_doff.as<long long>(), j0, j1, (int)pk, p.st_res.as<uint8_t>());
+        else if (pk % 4 != 0)  // 1-bit rows of dim 48 (6 bytes)
+            k_compact_gather<unsigned short><<<blocks, 256>>>(ix->residuals.as<uint8_t>(), ix->doc_off.as<long long>(), kp,
+                                                              p.new_doff.as<long long>(), j0, j1, (int)pk,
+                                                              p.st_res.as<uint8_t>());
         else
             k_compact_gather<uint32_t><<<blocks, 256>>>(ix->residuals.as<uint8_t>(), ix->doc_off.as<long long>(), kp,
                                                         p.new_doff.as<long long>(), j0, j1, (int)pk, p.st_res.as<uint8_t>());
@@ -3809,7 +3810,7 @@ static pb_status delete_commit(pb_index *ix, DeletePrep &p) {
     // 6. 1 / |c + w| of the survivors in their new order, and vmin / wmax over them as an open computes them: the old
     // constants would still bound the error, but the work counters would differ from a fresh open
     float vmin = 0.0f, wmax = 0.0f;
-    if (filter_dim(ix->dim) && p.N1 > 0) {
+    if (TcDims::has(ix->dim) && p.N1 > 0) {
         const float init[2] = {3.0e38f, 0.0f};
         CK(cudaMemcpy(p.mn.p, init, 8, cudaMemcpyHostToDevice));
         CKS(launch_min_vnorm(ix, 0, p.N1, p.mn.as<float>()));
@@ -4265,7 +4266,7 @@ extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bou
         CKS(alloc(p.udoc_off, ix->udoc_off, (D0 + 1) * 8, (D1 + 1) * 8));
         CKS(alloc(p.ivf, ix->ivf, ix->ivf_len * 4, p.L1 * 4));
         if (last && ix->ivf_spare.cap) CKS(alloc(p.ivf_spare, ix->ivf_spare, ix->ivf_len * 4, p.L1 * 4));
-        if (filter_dim(ix->dim) && p.N1 > 0) CKS(alloc(p.tok_inv_norm, ix->tok_inv_norm, N0 * 4, p.N1 * 4));
+        if (TcDims::has(ix->dim) && p.N1 > 0) CKS(alloc(p.tok_inv_norm, ix->tok_inv_norm, N0 * 4, p.N1 * 4));
         CKS(p.ivf_off.grow((size_t)(K + 1) * 8, 0, false));
         CKS(p.rlen.ensure((size_t)(D1 + 1) * 8));
         CKS(p.rulen.ensure((size_t)(D1 + 1) * 8));
@@ -4417,7 +4418,7 @@ extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bou
                                                  p.ivf.as<uint32_t>());
         CK(cudaGetLastError());
         // 1 / |c + w| of the new tokens and vmin / wmax over them, as an open computes them
-        if (filter_dim(ix->dim) && p.N1 > 0) {
+        if (TcDims::has(ix->dim) && p.N1 > 0) {
             if (ix->N == 0) CKS(build_centroid_operands(ix));  // a rank opened empty has none yet
             const float init[2] = {3.0e38f, 0.0f};
             CK(cudaMemcpy(p.mn.p, init, 8, cudaMemcpyHostToDevice));

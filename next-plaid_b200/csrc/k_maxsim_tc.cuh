@@ -25,8 +25,12 @@
 //   the arithmetic.  A query whose list overflows is left to k_exact (per-query flag).
 // Residual operand tile: canonical K-major fp16, element (token row r, 8-wide K chunk kc) at
 // kc * LBO + (r/8) * 128 + (r%8) * 16 = kc * LBO + 16 r, with LBO = 2048 + 32 bytes between K chunks.
+// A stage is the DIM / 8 chunks rounded up to 128 bytes (PB_XTC_STAGE), so that the second stage and the query tile
+// behind the ring start on 128-byte boundaries like every other operand base here (the no-swizzle descriptors need
+// 16).  The rounding is the identity when DIM % 32 == 0 and adds 64 bytes at DIM = 48 (6 chunks = 12480 bytes).
 // ==========================================================================================
 #define PB_XTC_LBO 2080u
+#define PB_XTC_STAGE(dim) ((((unsigned)(dim) / 8u) * PB_XTC_LBO + 127u) & ~127u)
 
 struct MsMeta {
     long long g;
@@ -98,11 +102,11 @@ k_maxsim_tc(const float *__restrict__ Q, const int *__restrict__ q_off, int QS, 
     extern __shared__ __align__(128) unsigned char smem_x[];
     constexpr int KC = DIM / 8, KSTEPS = DIM / 16;
     static_assert(NQT == 32 || NQT == 64, "k_maxsim_tc: N = 32 or 64");
-    constexpr uint32_t LBO_A = PB_XTC_LBO, A_BYTES = KC * LBO_A, QB_BYTES = NQT * DIM * 2;
+    static_assert(DIM % 16 == 0, "k_maxsim_tc: whole wgmma K steps");
+    constexpr uint32_t LBO_A = PB_XTC_LBO, A_BYTES = PB_XTC_STAGE(DIM), QB_BYTES = NQT * DIM * 2;
     constexpr uint32_t LBO_B = (NQT / 8) * 128, SBO = 128;
     constexpr int PACKED = DIM * NBITS / 8, NW = PACKED / 4;
     static_assert(PACKED % 4 == 0, "k_maxsim_tc: packed rows are read in 32-bit words");
-    static_assert(A_BYTES % 128 == 0, "k_maxsim_tc: stage alignment");
     constexpr int VB = 8 / NBITS;
     // the 4-bit table (256 entries x 4 B) is kept in TR copies, lane l reads copy l % TR: 32 random lookups of one copy hit
     // the worst bank ~3.5 times, 8 lookups spread over a copy's 8 banks ~2.3 times (the kernel sits on the LSU pipe)
