@@ -442,6 +442,8 @@ typedef struct pb_work_counters {
                                   * every (kept doc, query token) maximum of the MaxSim filter; <= 1e6 = within its
                                   * certificate; INT64_MAX = a non-finite estimate of a finite maximum; 0 otherwise */
     int64_t filter_diag_pairs;   /* PB_FILTER_DIAG=1 only: (kept doc, query token) maxima compared for filter_err_ratio_e6 */
+    int64_t n_a5_live_rows;      /* score-table rows the pruned first approximate pass gathered to bound the candidates */
+    int64_t n_a5_dense_docs;     /* candidates it then scored on every row (its two rounds); 0 on the dense first pass */
 } pb_work_counters;
 PB_API pb_status pb_last_work_counters(pb_index *ix, pb_work_counters *out);
 /* What the calling thread's last search staged from host memory (PB_OPEN_HOST_RESIDUALS; 0 otherwise): the kept docs of

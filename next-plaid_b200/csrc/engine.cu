@@ -322,7 +322,8 @@ struct Workspace {
     cudaEvent_t call_ev[2] = {};                // around a whole search call
     DevBuf Q, qoff, ST, partial, sel, cells, ncells, bitmap, cand, ncand, approx, keys, kept, nkept, tokp, maxkey,
         exact, fkeys, oids, oscores, ocounts, subset, subset_bits, elig, misc, list, counters, lkeys, ST16, qrange, qflag, lsum, cand2, ncand2,  cellbits,
-        gkeys, krank, payload, gfkeys, gpayload, cmax16, tau16, plist, pcount, Qi, Qh16t, Ql16t, ST16b, k1diag, k1rows, ulist, nulist, est, kept2, krank2, nkept2, tokp2, ktok2, qnmax, qexp, qrange_tc, mslot, slicecnt, rcmax, rcpairs, rcn, cellflags, estkey, srcrank, xpairs, xnpairs, needexact, gbase, fdiag;
+        gkeys, krank, payload, gfkeys, gpayload, cmax16, tau16, plist, pcount, Qi, Qh16t, Ql16t, ST16b, k1diag, k1rows, ulist, nulist, est, kept2, krank2, nkept2, tokp2, ktok2, qnmax, qexp, qrange_tc, mslot, slicecnt, rcmax, rcpairs, rcn, cellflags, estkey, srcrank, xpairs, xnpairs, needexact, gbase, fdiag,
+        a5floor, a5live, a5n1, a5n12, a5theta;
     // host tier: the staged rows of the kept docs (residuals, codes, 1 / |v|), their slot offsets and slot list
     DevBuf s_res, s_codes, s_inv, soff, kept_s;
     cudaEvent_t sev[2] = {};  // around the staging kernels
@@ -432,6 +433,9 @@ struct pb_index {
     bool k1_diag = false;      // also run the exact table and report the largest code difference (PB_K1_TC_DIAG=1)
     DevBuf cent_h16t, cent_l16t;  // its centroid operands: fp16 hi / lo, MMA tile order
     int approx_grid = 8;       // k_approx16 CTAs per SM and query (PB_APPROX_GRID)
+    bool a5_prune = true;      // bound the first pass from the live score-table rows (PB_A5_PRUNE=0: dense first pass)
+    long long a5_live = -1;    // live rows aimed at per query token (PB_A5_LIVE; -1: K / 512)
+    float a5_m1 = 1.25f;       // round 1 of the pruned first pass keeps the M1 = a5_m1 * M best bounds (PB_A5_M1, >= 1)
     bool probe16 = true;       // a3 threshold-first selection on the 16-bit table (PB_PROBE16=0: per-lane lists only)
     bool fast_exact = true;    // tensor-core certified filter in front of the exact stage (same results either way)
     float vmin = 0.0f;         // smallest pre-normalisation token norm |c + w| over the index (error bound of the filter)
@@ -956,6 +960,9 @@ pb_status pb_index_finalize(pb_index *ix) {
         if (const char *e = getenv("PB_K1_TC")) ix->k1_tc = atoi(e) != 0;
         if (const char *e = getenv("PB_K1_TC_E")) ix->k1_margin = std::max(1, atoi(e));
         if (const char *e = getenv("PB_APPROX_GRID")) ix->approx_grid = std::max(1, atoi(e));
+        if (const char *e = getenv("PB_A5_PRUNE")) ix->a5_prune = atoi(e) != 0;
+        if (const char *e = getenv("PB_A5_LIVE")) ix->a5_live = std::max(0ll, atoll(e));
+        if (const char *e = getenv("PB_A5_M1")) ix->a5_m1 = std::max(1.0f, (float)atof(e));
     }
     if (TcDims::has(ix->dim) && ix->N > 0 && ix->K > 0) {
         // operands of the tensor-core score table, and the token norms of the filter
@@ -1599,9 +1606,10 @@ static pb_status plan_probe(pb_index *ix, Workspace &ws, const pb_search_params 
     if (per_q >= ((size_t)1 << 32))
         return pb_fail(PB_ERR_UNSUPPORTED, "num_centroids x query tokens x 4 = %zu bytes per query exceeds 2^32", per_q);
     // sub-batch size: the score tables (16-bit always, fp32 only on the exact path) and the per-(query, doc) scratch
-    // (candidate lists, code sums, approximate scores, cut keys, bitmap: 24.2 bytes per document) share one budget
+    // (candidate lists, code sums, approximate scores, cut keys, bitmap: 24.2 bytes per document; the live-row bitmap
+    // of the pruned first pass: 1 bit per centroid) share one budget
     // A host-tier handle also stages up to Mcap docs of max_doclen rows per query (residuals, codes, 1 / |v|)
-    const size_t per_q_all = (size_t)ix->K * QS_all * (k1_tc_usable(ix) ? 2 : 6) + (size_t)ix->D * 24 + (size_t)ix->D / 8 + 4096 +
+    const size_t per_q_all = (size_t)ix->K * QS_all * (k1_tc_usable(ix) ? 2 : 6) + (size_t)ix->D * 24 + (size_t)ix->D / 8 + (size_t)ix->K / 8 + 4096 +
                              (ix->host_tier ? (size_t)plan.Mcap * std::max(ix->max_doclen, 1) * (ix->packed + 8) : 0);
     int QB = (int)std::max<size_t>(1, std::min<size_t>((size_t)Bt, ix->st_budget / std::max(g_budget_div, 1) / per_q_all));
     QB = std::min(QB, 256);
@@ -1612,13 +1620,13 @@ static pb_status plan_probe(pb_index *ix, Workspace &ws, const pb_search_params 
 // The pinned read-back of one pass (ws.hcounts): the query offsets that go up, then what comes back.  Placed here only.
 struct HostCounts {
     int *qoff;                // [B + 1] query token offsets of the sub-batch
-    unsigned long long *cnt;  // [B + 2] ws.counters
+    unsigned long long *cnt;  // [B + 4] ws.counters
     long long *surv_tok;      // [B] tokens of the filter's survivors
     int *cells, *cand, *kept, *surv, *recheck, *pairs, *need;  // [B] each
     int *fell;                // the threshold-first probe's fallback flag
 };
 static pb_status map_host_counts(HostBuf &hb, int B, HostCounts &h) {
-    const size_t at_cnt = ((size_t)(B + 1) * 4 + 15) & ~(size_t)15, at_tok = at_cnt + (size_t)(B + 2) * 8,
+    const size_t at_cnt = ((size_t)(B + 1) * 4 + 15) & ~(size_t)15, at_tok = at_cnt + (size_t)(B + 4) * 8,
                  at_int = at_tok + (size_t)B * 8;
     CKS(hb.ensure(at_int + ((size_t)7 * B + 1) * 4));
     char *base = hb.as<char>();
@@ -1638,6 +1646,7 @@ struct Pass {
     // being read back mid-way; the pass then finishes on (memory-safe) garbage and is redone on the exact path.
     bool use_tc = false;
     bool fast = false;  // the two-pass approximate stage on the 16-bit score table
+    bool prune = false;  // its first pass bounded from the live table rows (QS <= 64, not on a redo)
     HostCounts hc{};
     // a2 / a3
     int cells_cap = 0;
@@ -1813,8 +1822,10 @@ static pb_status candidates(pb_index *ix, Workspace &ws, const SearchPlan &plan,
 static pb_status approx_scores(pb_index *ix, Workspace &ws, const SearchPlan &plan, Pass &pass) {
     const int B = pass.B, QS = pass.QS, Mcap = plan.Mcap;
     int *L = g_stats.launches;
-    CKS(ws.counters.ensure((size_t)(B + 2) * 8));  // [0] candidate codes gathered, [1+b] kept-doc tokens, [B+1] re-check gathers
-    CK(cudaMemsetAsync(ws.counters.p, 0, (size_t)(B + 2) * 8, ws.stream));
+    // [0] candidate codes gathered, [1+b] kept-doc tokens, [B+1] re-check gathers, [B+2] live rows gathered by the
+    // pruned first pass, [B+3] docs it scored densely
+    CKS(ws.counters.ensure((size_t)(B + 4) * 8));
+    CK(cudaMemsetAsync(ws.counters.p, 0, (size_t)(B + 4) * 8, ws.stream));
     CKS(ws.approx.ensure((size_t)B * ix->D * 4));
     CKS(ws.keys.ensure((size_t)B * ix->D * 8));
     if (pass.fast) {
@@ -1826,21 +1837,65 @@ static pb_status approx_scores(pb_index *ix, Workspace &ws, const SearchPlan &pl
         const uint32_t *list = ws.cand.as<uint32_t>();
         const int *list_n = ws.ncand.as<int>();
         unsigned long long *cnt = ws.counters.as<unsigned long long>();
-        KEV_BEGIN(PB_KERNEL_APPROX16);
-        (QS <= 32 ? k_approx16<4> : k_approx16<8>)<<<ga, 256, 0, ws.stream>>>(
-            st16, ws.qoff.as<int>(), ix->K, QS, ix->ucodes.as<uint32_t>(), ix->udoc_off.as<long long>(), list, ix->D, list_n,
-            ws.lsum.as<uint32_t>(), cnt);
-        KEV_END(PB_KERNEL_APPROX16);
+        const auto approx16 = QS <= 32 ? k_approx16<4> : k_approx16<8>;
         // band per query token in code units (W = band * nq + 8).  Exact table: +-1 code of rounding per token and side
         // plus the fp32 summation error -> 4.  Estimate table (k_scores_tc.cuh): W = nq (1.004 + 2 err) + nq^2/256 + 4
         // <= nq (ceil(1.004 + 2 err) + 1) + 8 for nq <= 256.
         const int band_per_q =
             pass.use_tc ? (int)ceilf(1.004f + 2.0f * std::max(k1_err_codes(ix->dim), (float)(ix->k1_margin - 1))) + 1 : 4;
+        KEV_BEGIN(PB_KERNEL_APPROX16);
+        if (pass.prune) {
+            // the bound U of every candidate from the live rows, then k_approx16 on the two rounds that can reach the
+            // band (k_approx16.cuh); U lives in ws.approx and the round lists in ws.keys until the re-check overwrites them
+            CKS(ws.a5floor.ensure((size_t)B * QS * 4));
+            CKS(ws.a5live.ensure((size_t)B * ((ix->K + 31) / 32) * 4));
+            CKS(ws.a5n1.ensure((size_t)B * 4 + 16));
+            CKS(ws.a5n12.ensure((size_t)B * 4 + 16));
+            CKS(ws.a5theta.ensure((size_t)B * 4 + 16));
+            const long long n_live = ix->a5_live >= 0 ? ix->a5_live : ix->K / 512;
+            const int M1 = (int)std::min<double>(ceil((double)ix->a5_m1 * plan.M), (double)INT_MAX);
+            uint32_t *ub = ws.approx.as<uint32_t>(), *rl = ws.keys.as<uint32_t>();
+            int *n1 = ws.a5n1.as<int>(), *n12 = ws.a5n12.as<int>();
+            k_a5_floor<<<dim3(QS / 8, B), 256, 0, ws.stream>>>(st16, ws.qoff.as<int>(), ix->K, QS, n_live,
+                                                               ws.a5floor.as<uint32_t>());
+            k_a5_live<<<dim3(ix->sm_count * 2, B), 256, 0, ws.stream>>>(st16, ix->K, QS, ws.a5floor.as<uint32_t>(),
+                                                                         ws.a5live.as<uint32_t>());
+            // the bitmap in shared memory up to K = 2^19 (64 KiB; three CTAs of k_a5_bound<4> still fit an SM), then
+            // 32 CTAs per SM over the batch: few enough that copying it in costs little L2
+            const auto bound = QS <= 32 ? k_a5_bound<4> : k_a5_bound<8>;
+            const size_t bits_bytes = (size_t)(ix->K + 31) / 32 * 4;
+            const bool bits_in_smem = bits_bytes <= 64 * 1024;
+            if (bits_in_smem) CKS(set_smem(bound, bits_bytes));
+            const dim3 gb = bits_in_smem ? dim3(std::max(1, ix->sm_count * 32 / B), B) : ga;
+            bound<<<gb, 256, bits_in_smem ? bits_bytes : 0, ws.stream>>>(
+                st16, ws.qoff.as<int>(), ix->K, QS, ix->ucodes.as<uint32_t>(), ix->udoc_off.as<long long>(), list, ix->D,
+                list_n, ws.a5floor.as<uint32_t>(), ws.a5live.as<uint32_t>(), bits_in_smem, ub, cnt, cnt + B + 2);
+            k_select_u32<<<B, 1024, 0, ws.stream>>>(ub, list_n, M1, 0, ub, list, list_n, ix->D, ws.qoff.as<int>(),
+                                                    ws.qflag.as<int>(), rl, n1, ws.a5theta.as<uint32_t>());
+            approx16<<<ga, 256, 0, ws.stream>>>(st16, ws.qoff.as<int>(), ix->K, QS, ix->ucodes.as<uint32_t>(),
+                                                ix->udoc_off.as<long long>(), rl, ix->D, n1, nullptr,
+                                                ws.lsum.as<uint32_t>(), nullptr);
+            k_select_u32<<<B, 1024, 0, ws.stream>>>(ws.lsum.as<uint32_t>(), n1, plan.M, band_per_q, ub, list, list_n,
+                                                    ix->D, ws.qoff.as<int>(), ws.qflag.as<int>(), rl, n12, nullptr,
+                                                    ws.a5theta.as<uint32_t>(), n1, cnt + B + 3);
+            approx16<<<ga, 256, 0, ws.stream>>>(st16, ws.qoff.as<int>(), ix->K, QS, ix->ucodes.as<uint32_t>(),
+                                                ix->udoc_off.as<long long>(), rl, ix->D, n12, n1,
+                                                ws.lsum.as<uint32_t>(), nullptr);
+            list = rl;
+            list_n = n12;
+            L[PB_STAGE_APPROX] += 7;
+        } else {
+            approx16<<<ga, 256, 0, ws.stream>>>(st16, ws.qoff.as<int>(), ix->K, QS, ix->ucodes.as<uint32_t>(),
+                                                ix->udoc_off.as<long long>(), list, ix->D, list_n, nullptr,
+                                                ws.lsum.as<uint32_t>(), cnt);
+            L[PB_STAGE_APPROX] += 1;
+        }
+        KEV_END(PB_KERNEL_APPROX16);
         k_select_u32<<<B, 1024, 0, ws.stream>>>(ws.lsum.as<uint32_t>(), list_n, plan.M, band_per_q, ws.lsum.as<uint32_t>(),
                                                 list, list_n, ix->D, ws.qoff.as<int>(), ws.qflag.as<int>(),
                                                 ws.cand2.as<uint32_t>(), ws.ncand2.as<int>());
         CK(cudaGetLastError());
-        L[PB_STAGE_APPROX] += 2;
+        L[PB_STAGE_APPROX] += 1;
     }
     pass.cand_list = pass.fast ? ws.cand2.as<uint32_t>() : ws.cand.as<uint32_t>();
     pass.cand_n = pass.fast ? ws.ncand2.as<int>() : ws.ncand.as<int>();
@@ -2107,7 +2162,7 @@ static pb_status finish(pb_index *ix, Workspace &ws, const SearchIO &io, const S
     CK(cudaMemcpyAsync(hc.cells, ws.ncells.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
     CK(cudaMemcpyAsync(hc.cand, ws.ncand.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
     CK(cudaMemcpyAsync(hc.kept, ws.nkept.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
-    CK(cudaMemcpyAsync(hc.cnt, ws.counters.p, (size_t)(B + 2) * 8, cudaMemcpyDeviceToHost, ws.stream));
+    CK(cudaMemcpyAsync(hc.cnt, ws.counters.p, (size_t)(B + 4) * 8, cudaMemcpyDeviceToHost, ws.stream));
     if (pass.filt) {
         CK(cudaMemcpyAsync(hc.surv_tok, ws.ktok2.p, (size_t)B * 8, cudaMemcpyDeviceToHost, ws.stream));
         CK(cudaMemcpyAsync(hc.surv, ws.nkept2.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
@@ -2177,6 +2232,8 @@ static pb_status finish(pb_index *ix, Workspace &ws, const SearchIO &io, const S
             else w.n_exact_pairs += hc.pairs[b];
         }
     w.n_candidate_tokens += (long long)hc.cnt[0];
+    w.n_a5_live_rows += (long long)hc.cnt[B + 2];
+    w.n_a5_dense_docs += (long long)hc.cnt[B + 3];
     for (int b = 0; b < B; ++b) {
         w.n_cells += hc.cells[b];
         w.n_candidates += hc.cand[b];
@@ -2324,6 +2381,7 @@ static pb_status run_search(pb_index *ix, const pb_search_params *p, const Searc
             pass.nq_max = std::max(pass.nq_max, (int)(io.q_off[b0 + b + 1] - io.q_off[b0 + b]));
         pass.QS = query_row_tokens(pass.nq_max);
         pass.fast = ix->fast_approx && !io.trace;  // trace wants every candidate's exact approx score
+        pass.prune = pass.fast && ix->a5_prune && pass.QS <= 64;
         // the score table comes from the tensor cores unless something needs the dense fp32 S (an eligibility filter,
         // the radix-select probe, a trace) or the shape is outside the kernel's (DESIGN.md "a2")
         int n_chunks_k = 0;
@@ -2337,6 +2395,7 @@ static pb_status run_search(pb_index *ix, const pb_search_params *p, const Searc
         if (redo) {
             g_stats.work.n_k1_tc_redo += 1;
             pass.use_tc = false;
+            pass.prune = false;
             pass.filt = filter_runs(ix, io, plan, pass);
             CKS(run_pass(ix, ws, p, io, plan, pass, &redo));
         }

@@ -88,7 +88,7 @@ __global__ void __launch_bounds__(256, LPR == 4 ? 4 : 2)
 k_approx16(const unsigned short *__restrict__ ST16, const int *__restrict__ q_off, long long K, int QS,
            const uint32_t *__restrict__ ucodes, const long long *__restrict__ udoc_off,
            const uint32_t *__restrict__ cand, long long cand_cap, const int *__restrict__ n_cand,
-           uint32_t *__restrict__ lsum, unsigned long long *__restrict__ tok_counter) {
+           const int *__restrict__ n_skip, uint32_t *__restrict__ lsum, unsigned long long *__restrict__ tok_counter) {
     constexpr int RG = 32 / LPR;   // row groups of a warp = rows per load instruction
     constexpr int QB = 8 * LPR;    // query tokens covered by one pass
     constexpr int NI = 64 / RG;    // load instructions per 64 codes
@@ -100,7 +100,8 @@ k_approx16(const unsigned short *__restrict__ ST16, const int *__restrict__ q_of
     const char *STb = reinterpret_cast<const char *>(ST16 + (size_t)b * K * QS);
     const unsigned rowb = (unsigned)QS * 2u;
     unsigned long long my_tokens = 0;
-    int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    // entries [n_skip[b], n_cand[b]) of the list (n_skip: a5's pruned second round appends to its first)
+    int i = (n_skip ? n_skip[b] : 0) + blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     uint32_t d = 0;
     long long t0 = 0, t1 = 0;
     if (i < n) {
@@ -175,18 +176,268 @@ k_approx16(const unsigned short *__restrict__ ST16, const int *__restrict__ q_of
         t0 = t0n;
         t1 = t1n;
     }
-    if (lane == 0 && my_tokens) atomicAdd(tok_counter, my_tokens);
+    if (lane == 0 && my_tokens && tok_counter) atomicAdd(tok_counter, my_tokens);
+}
+
+// ------------------------------------------------------------------------------------------
+// a5 with pruning: bound every candidate's first-pass score from the score-table rows that can matter, and run
+// k_approx16 only on the docs that can still reach the band around the cut.
+//
+// Per query token q a floor f_q (code units, k_a5_floor); a centroid c is LIVE when code[c][q] >= f_q for some
+// q < nq (k_a5_live, one bit per centroid).  Every entry of a dead row is <= f_q - 1 in its column, so in exact
+// integer arithmetic
+//     L(d) = sum_q max_{c in codes(d)} code[c][q]  <=  U(d) = sum_q max(m_live(d, q), f_q - 1)
+// (m_live = the maximum over d's live codes, 0 when none; f_q - 1 read as 0 when f_q = 0).  k_a5_bound computes U
+// with live-row gathers only.  With W the band of the final select and M the cut:
+//   round 1: theta1 = the M1-th largest U (M1 >= M), R1 = {U >= theta1} (ties at theta1 all join), L on R1 by
+//            k_approx16, tau1 = the M-th largest L over R1;
+//   round 2: R2 = {tau1 - W <= U < theta1}, L on R2 by k_approx16, appended after R1;
+//   band:    the select of the dense form, unchanged, over R1 + R2.
+// Exact: tau1 <= tau (the M-th largest L over all candidates) since R1 is a subset of them; every doc with
+// L >= tau - W >= tau1 - W has U >= L >= tau1 - W, so it is in R1 or R2; there are at least M such docs, so the
+// M-th largest L over R1 + R2 is tau and the band set {L >= tau - W} is the dense form's, doc for doc.  A query
+// with fewer than M1 candidates, or a flagged one, keeps every candidate in round 1 (theta1 = 0: R2 is empty) and is
+// the dense form.  Any floor is exact: f_q = 0 makes every row live and U = L; a floor above every code makes none
+// live and U the same for every doc, so R1 takes them all.  The floor only decides the speed.
+// ------------------------------------------------------------------------------------------
+// floor[b][q]: about the n_live-th largest code of token q, from a histogram of the high byte over a sample of
+// S = min(K, 8192) evenly spaced rows: the low edge of the highest bin with at least ceil(n_live * S / K) sampled
+// codes at or above it.  n_live = 0: 65536 (nothing live); n_live >= K: 0 (everything live); padding tokens 65536.
+// grid = (QS / 8, B), 256 threads; a CTA covers 8 query tokens, one 16-byte group of each sampled row.
+__global__ void __launch_bounds__(256)
+k_a5_floor(const unsigned short *__restrict__ ST16, const int *__restrict__ q_off, long long K, int QS, long long n_live,
+           uint32_t *__restrict__ floor_out) {
+    __shared__ int hist[8][256];
+    const int g = blockIdx.x, b = blockIdx.y, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int nq = q_off[b + 1] - q_off[b];
+    const int S = (int)min(K, 8192ll);
+    for (int i = threadIdx.x; i < 8 * 256; i += blockDim.x) (&hist[0][0])[i] = 0;
+    __syncthreads();
+    const uint4 *base = reinterpret_cast<const uint4 *>(ST16 + (size_t)b * K * QS) + g;
+    const int GQ = QS >> 3;
+    for (int j = threadIdx.x; j < S; j += blockDim.x) {
+        const uint4 v = __ldg(base + (size_t)(j * K / S) * GQ);
+        const uint32_t p[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            atomicAdd(&hist[2 * k][(p[k] >> 8) & 255u], 1);
+            atomicAdd(&hist[2 * k + 1][p[k] >> 24], 1);
+        }
+    }
+    __syncthreads();
+    const int q = 8 * g + w;  // warp w picks token w's floor
+    uint32_t f;
+    if (q >= nq || n_live <= 0) f = 65536u;
+    else if (n_live >= K) f = 0u;
+    else {
+        const int need = (int)min((long long)S, max(1ll, (n_live * S + K - 1) / K));
+        // lane l owns bins 8 (31 - l) + 7 .. 8 (31 - l): the inclusive prefix over lanes counts the codes >= 8 (31 - l)
+        int loc[8], sum = 0;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            loc[k] = hist[w][8 * (31 - lane) + 7 - k];
+            sum += loc[k];
+        }
+        int incl = sum;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(PB_FULL, incl, o);
+            if (lane >= o) incl += y;
+        }
+        const unsigned reach = __ballot_sync(PB_FULL, incl >= need);  // lane 31 always reaches it (need <= S)
+        const int hit = __ffs(reach) - 1;
+        int bin = 0;
+        if (lane == hit) {
+            int cum = incl - sum, k = 0;
+            for (; k < 7; ++k) {
+                if (cum + loc[k] >= need) break;
+                cum += loc[k];
+            }
+            bin = 8 * (31 - lane) + 7 - k;
+        }
+        f = (uint32_t)__shfl_sync(PB_FULL, bin, hit) << 8;
+    }
+    if (w < 8 && lane == 0 && q < QS) floor_out[(size_t)b * QS + q] = f;
+}
+
+// live[b][c / 32] bit c % 32: row c has a code >= floor in some real query token.  Every word is written.
+// grid = (any, B), 256 threads; a warp takes 32 rows at a time (coalesced 16-byte loads, GQ = QS / 8 <= 8 per row).
+__global__ void __launch_bounds__(256)
+k_a5_live(const unsigned short *__restrict__ ST16, long long K, int QS, const uint32_t *__restrict__ floor_in,
+          uint32_t *__restrict__ live) {
+    __shared__ uint32_t t2_s[32], m2_s[32];  // packed floors / real-token masks of token pairs (QS <= 64)
+    __shared__ uint32_t word_s[8];
+    const int b = blockIdx.y, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int GQ = QS >> 3;
+    if (threadIdx.x < QS / 2) {
+        const uint32_t a = floor_in[(size_t)b * QS + 2 * threadIdx.x], c = floor_in[(size_t)b * QS + 2 * threadIdx.x + 1];
+        t2_s[threadIdx.x] = min(a, 65535u) | (min(c, 65535u) << 16);
+        m2_s[threadIdx.x] = (a < 65536u ? 0xffffu : 0u) | (c < 65536u ? 0xffff0000u : 0u);
+    }
+    __syncthreads();
+    const long long n_words = (K + 31) / 32;
+    const uint4 *STb = reinterpret_cast<const uint4 *>(ST16 + (size_t)b * K * QS);
+    for (long long wd = (long long)blockIdx.x * 8 + w; wd < n_words; wd += (long long)gridDim.x * 8) {
+        const int rows = (int)min(32ll, K - wd * 32), total = rows * GQ;
+        const uint4 *base = STb + (size_t)wd * 32 * GQ;
+        if (lane == 0) word_s[w] = 0u;
+        __syncwarp();
+        uint4 v[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k)
+            if (k < GQ && lane + 32 * k < total) v[k] = __ldg(base + lane + 32 * k);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const int idx = lane + 32 * k;
+            if (k >= GQ || idx >= total) continue;
+            const int g = idx % GQ;
+            const uint32_t h = (__vcmpgeu2(v[k].x, t2_s[4 * g]) & m2_s[4 * g]) |
+                               (__vcmpgeu2(v[k].y, t2_s[4 * g + 1]) & m2_s[4 * g + 1]) |
+                               (__vcmpgeu2(v[k].z, t2_s[4 * g + 2]) & m2_s[4 * g + 2]) |
+                               (__vcmpgeu2(v[k].w, t2_s[4 * g + 3]) & m2_s[4 * g + 3]);
+            if (h) atomicOr(&word_s[w], 1u << (idx / GQ));
+        }
+        __syncwarp();
+        if (lane == 0) live[(size_t)b * n_words + wd] = word_s[w];
+        __syncwarp();
+    }
+}
+
+// U(d) of every candidate (bound above), one warp per doc as in k_approx16.  The kernel is latency-bound (a doc's
+// chain is cand -> offsets -> codes -> live bits -> rows), so the next doc's offsets are prefetched and up to 256 codes
+// are loaded at once; their live ones are compacted into a per-warp buffer and gathered with k_approx16's row groups,
+// 32 rows per round of independent loads.  QS <= 8 * LPR: one column pass.  Counts the doc codes read (tok_counter)
+// and the rows gathered (live_counter).  bits_in_smem: the query's bitmap is copied to dynamic shared memory first
+// (K / 8 bytes; 32 random bit tests from L1 cost up to 32 wavefronts, from shared memory about 4).
+template <int LPR>
+__global__ void __launch_bounds__(256, LPR == 4 ? 3 : 2)  // (4 CTAs of LPR = 4 would spill)
+k_a5_bound(const unsigned short *__restrict__ ST16, const int *__restrict__ q_off, long long K, int QS,
+           const uint32_t *__restrict__ ucodes, const long long *__restrict__ udoc_off,
+           const uint32_t *__restrict__ cand, long long cand_cap, const int *__restrict__ n_cand,
+           const uint32_t *__restrict__ floor_in, const uint32_t *__restrict__ live, bool bits_in_smem,
+           uint32_t *__restrict__ ubound, unsigned long long *__restrict__ tok_counter,
+           unsigned long long *__restrict__ live_counter) {
+    constexpr int RG = 32 / LPR;  // rows per load instruction
+    constexpr int NE = 32 / RG;   // load instructions per round of 32 rows
+    __shared__ uint32_t buf_s[8][256];
+    extern __shared__ uint32_t bits_s[];
+    const int b = blockIdx.y, w = threadIdx.x >> 5;
+    const int nq = q_off[b + 1] - q_off[b];
+    const int n = n_cand[b];
+    const int lane = threadIdx.x & 31, r = lane / LPR, sl = lane % LPR;
+    const int warps_per_grid = gridDim.x * (blockDim.x >> 5);
+    const bool in_row = 8 * sl < QS;
+    const char *col = reinterpret_cast<const char *>(ST16 + (size_t)b * K * QS) + (in_row ? 16 * sl : 0);
+    const unsigned rowb = (unsigned)QS * 2u;
+    const uint32_t *liveb = live + (size_t)b * ((K + 31) / 32);
+    if (bits_in_smem) {
+        for (long long k = threadIdx.x; k < (K + 31) / 32; k += blockDim.x) bits_s[k] = liveb[k];
+        __syncthreads();
+    }
+    uint32_t *buf = buf_s[w];
+    // this lane's dead-row maxima f_q - 1 (0 for f_q = 0), packed as the maxima are
+    uint32_t dm[4] = {0u, 0u, 0u, 0u};
+    if (in_row)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const uint32_t f = floor_in[(size_t)b * QS + 8 * sl + j];
+            dm[j >> 1] |= (f ? min(f - 1u, 65535u) : 0u) << (16 * (j & 1));
+        }
+    unsigned long long my_tokens = 0, my_live = 0;
+    int i = blockIdx.x * (blockDim.x >> 5) + w;
+    long long t0 = 0, t1 = 0;
+    if (i < n) {
+        const uint32_t d = cand[(size_t)b * cand_cap + i];
+        t0 = udoc_off[d];
+        t1 = udoc_off[d + 1];
+    }
+    for (; i < n; i += warps_per_grid) {
+        const int i2 = i + warps_per_grid;
+        long long t0n = 0, t1n = 0;
+        if (i2 < n) {
+            const uint32_t dn = cand[(size_t)b * cand_cap + i2];
+            t0n = udoc_off[dn];
+            t1n = udoc_off[dn + 1];
+        }
+        my_tokens += (unsigned long long)(t1 - t0);
+        uint32_t m0 = dm[0], m1 = dm[1], m2 = dm[2], m3 = dm[3];
+        for (long long tb = t0; tb < t1; tb += 256) {
+            uint32_t cc[8];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+                const long long t = tb + 32 * k + lane;
+                cc[k] = t < t1 ? ucodes[t] : 0u;
+            }
+            int cnt = 0;
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+                const uint32_t c = cc[k];
+                const uint32_t word = bits_in_smem ? bits_s[c >> 5] : __ldg(liveb + (c >> 5));
+                const bool lv = tb + 32 * k + lane < t1 && ((word >> (c & 31)) & 1u);
+                const unsigned bal = __ballot_sync(PB_FULL, lv);
+                if (lv) buf[cnt + __popc(bal & ((1u << lane) - 1u))] = c;
+                cnt += __popc(bal);
+            }
+            __syncwarp();
+            for (int base = 0; base < cnt; base += 32) {
+                uint4 v[NE];
+#pragma unroll
+                for (int e = 0; e < NE; ++e)
+                    if (base + RG * e + r < cnt)
+                        v[e] = *reinterpret_cast<const uint4 *>(col + (size_t)buf[base + RG * e + r] * rowb);
+#pragma unroll
+                for (int e = 0; e < NE; ++e)
+                    if (base + RG * e + r < cnt) {
+                        m0 = __vmaxu2(m0, v[e].x);
+                        m1 = __vmaxu2(m1, v[e].y);
+                        m2 = __vmaxu2(m2, v[e].z);
+                        m3 = __vmaxu2(m3, v[e].w);
+                    }
+            }
+            my_live += (unsigned long long)cnt;
+            __syncwarp();
+        }
+#pragma unroll
+        for (int m = LPR; m < 32; m <<= 1) {
+            m0 = __vmaxu2(m0, __shfl_xor_sync(PB_FULL, m0, m));
+            m1 = __vmaxu2(m1, __shfl_xor_sync(PB_FULL, m1, m));
+            m2 = __vmaxu2(m2, __shfl_xor_sync(PB_FULL, m2, m));
+            m3 = __vmaxu2(m3, __shfl_xor_sync(PB_FULL, m3, m));
+        }
+        const int q0 = 8 * sl;
+        uint32_t part = 0;
+        if (in_row && r == 0) {
+            const uint32_t mm[4] = {m0, m1, m2, m3};
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                if (q0 + 2 * j < nq) part += mm[j] & 0xffffu;
+                if (q0 + 2 * j + 1 < nq) part += mm[j] >> 16;
+            }
+        }
+        const uint32_t total = __reduce_add_sync(PB_FULL, part);
+        if (lane == 0) ubound[(size_t)b * cand_cap + i] = total;
+        t0 = t0n;
+        t1 = t1n;
+    }
+    if (lane == 0) {
+        if (my_tokens) atomicAdd(tok_counter, my_tokens);
+        if (my_live) atomicAdd(live_counter, my_live);
+    }
 }
 
 // "N-th largest with a band" selection.  Per query:
 //   tau = N-th largest of sel_keys[0..sel_n) (0 when sel_n < N or the query is flagged),
-//   thr = tau - (band_per_q * nq + 8) (0 when band_per_q < 0 ... see callers), and the output is every
+//   thr = tau - (band_per_q * nq + 8) (thr = tau when band_per_q <= 0), and the output is every
 //   entry of filt_list whose filt_key >= thr (unordered).  grid = B, 1024 threads.
+// The pruned a5 rounds use the optional arguments: thr_out[b] = thr; filt_hi[b] also caps the key (filt_key <
+// filt_hi[b]); the output goes after out_base[b] entries and out_n[b] counts them too; tally adds up the out_n.
 __global__ void __launch_bounds__(1024)
 k_select_u32(const uint32_t *__restrict__ sel_keys, const int *__restrict__ sel_n, int N, int band_per_q,
              const uint32_t *__restrict__ filt_keys, const uint32_t *__restrict__ filt_list,
              const int *__restrict__ filt_n, long long stride, const int *__restrict__ q_off,
-             const int *__restrict__ qflag, uint32_t *__restrict__ out_list, int *__restrict__ out_n) {
+             const int *__restrict__ qflag, uint32_t *__restrict__ out_list, int *__restrict__ out_n,
+             uint32_t *__restrict__ thr_out = nullptr, const uint32_t *__restrict__ filt_hi = nullptr,
+             const int *__restrict__ out_base = nullptr, unsigned long long *__restrict__ tally = nullptr) {
     // one histogram per warp: the keys of a query share their high digits (sums of nq 16-bit codes), so a single
     // histogram serialises every thread of the CTA on one or two shared-memory words (0.15 ms); a warp whose 32 keys
     // fall in one bin adds 32 with one atomic
@@ -276,7 +527,13 @@ k_select_u32(const uint32_t *__restrict__ sel_keys, const int *__restrict__ sel_
         const uint32_t W = band_per_q > 0 ? (uint32_t)band_per_q * (uint32_t)nq + 8u : 0u;
         thr = tau > W ? tau - W : 0u;
     }
-    if (threadIdx.x == 0) fill_s = 0;
+    const int base0 = out_base ? out_base[b] : 0;
+    const uint32_t hi = filt_hi ? filt_hi[b] : 0xffffffffu;
+    if (threadIdx.x == 0) {
+        fill_s = 0;
+        if (thr_out) thr_out[b] = thr;
+    }
+    cout += base0;
     __syncthreads();
     const int lane = threadIdx.x & 31;
     for (int base = 0; base < nf; base += blockDim.x * 8) {
@@ -290,7 +547,7 @@ k_select_u32(const uint32_t *__restrict__ sel_keys, const int *__restrict__ sel_
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             const int i = base + j * (int)blockDim.x + (int)threadIdx.x;
-            const bool keep = i < nf && fv[j] >= thr;
+            const bool keep = i < nf && fv[j] >= thr && (!filt_hi || fv[j] < hi);
             const unsigned bal = __ballot_sync(PB_FULL, keep);
             if (!bal) continue;
             int off = 0;
@@ -300,6 +557,9 @@ k_select_u32(const uint32_t *__restrict__ sel_keys, const int *__restrict__ sel_
         }
     }
     __syncthreads();
-    if (threadIdx.x == 0) out_n[b] = fill_s;
+    if (threadIdx.x == 0) {
+        out_n[b] = base0 + fill_s;
+        if (tally) atomicAdd(tally, (unsigned long long)(base0 + fill_s));
+    }
 }
 

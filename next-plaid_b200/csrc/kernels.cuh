@@ -7,6 +7,8 @@
 //   k_cells(_unique/_thr/_emit)  a3  union + centroid_score_threshold      search.rs:417-425 / :226-251
 //   k_mark/k_compact .... a4  IVF posting-list union (sorted, unique)     index.rs:1142-1156
 //   k_approx16/k_select_u32  a5  sum_q max_t S[q, code_t] on the 16-bit table, band around the cut
+//   k_a5_floor/k_a5_live/k_a5_bound  a5  an upper bound of it from the live table rows: k_approx16 runs on the few
+//                             candidates that can still reach the band
 //   k_recheck_pairs/dots/sum (tensor-core table) | k_approx (exact table)  a5  exact re-check of the docs in the band
 //                                                                          search.rs:305-324 / :275-302
 //   k_cut ............... a6  stable top-(n_full_scores -> /4) cut        search.rs:460-469

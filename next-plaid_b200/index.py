@@ -68,7 +68,8 @@ class _Work(C.Structure):
                                          "n_filter_docs", "n_filter_tokens", "k1_tc_max_code_diff",
                                          "k1_rows_mismatch", "n_probe_threshold", "n_probe_list", "n_k1_tc",
                                          "n_recheck_docs", "n_k1_tc_redo", "n_exact_pairs",
-                                         "n_pair_fallback_queries", "filter_err_ratio_e6", "filter_diag_pairs")]
+                                         "n_pair_fallback_queries", "filter_err_ratio_e6", "filter_diag_pairs",
+                                         "n_a5_live_rows", "n_a5_dense_docs")]
 
 
 EXPORTS = [
