@@ -327,6 +327,20 @@ PB_API pb_status pb_search_batch_traced(pb_index *ix, const float *queries,
                                         int64_t n_subset, int64_t *out_ids, float *out_scores,
                                         int32_t *out_counts, pb_trace *trace);
 
+/* pb_search_batch with an Option<&[i64]> subset per query: result i equals pb_search_batch of query i alone with
+ * subset_ids[subset_offsets[i] .. subset_offsets[i+1]) when has_subset[i] != 0, and with no subset (None) when
+ * has_subset[i] == 0.  has_subset == NULL: every query has one.  subset_offsets == NULL: no query has one.
+ * trace may be NULL (as pb_search_batch_traced).  On a doc-sharded handle it is a collective like pb_search_batch:
+ * every rank passes the same arguments; ranks given different subsets all return PB_ERR_INVALID.
+ * Queries of different subsets share the batch's passes, so a server can put concurrent filtered requests into one
+ * call.  Any limit that would refuse pb_search_batch of one query with its subset refuses the whole call; malformed
+ * offsets return PB_ERR_INVALID before anything runs. */
+PB_API pb_status pb_search_batch_subsets(pb_index *ix, const float *queries, const int64_t *q_tok_offsets,
+                                         int64_t n_queries, const pb_search_params *params,
+                                         const int64_t *subset_offsets /* [n_queries + 1], [0] == 0 */,
+                                         const int64_t *subset_ids, const uint8_t *has_subset /* [n_queries] */,
+                                         int64_t *out_ids, float *out_scores, int32_t *out_counts, pb_trace *trace);
+
 /* ---- stage entry points (each is one kernel of the path; used by tests, bench and ncu) ---- */
 
 /* Stage 1, S = Q * C^T (search.rs:345).  out: [n_query_tokens][K] row-major f32, host. */

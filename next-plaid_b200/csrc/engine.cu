@@ -321,9 +321,12 @@ struct Workspace {
     cudaEvent_t kev[2 * PB_KERNEL_COUNT] = {};  // begin / end around the main kernel of a stage
     cudaEvent_t call_ev[2] = {};                // around a whole search call
     DevBuf Q, qoff, ST, partial, sel, cells, ncells, bitmap, cand, ncand, approx, keys, kept, nkept, tokp, maxkey,
-        exact, fkeys, oids, oscores, ocounts, subset, subset_bits, elig, misc, list, counters, lkeys, ST16, qrange, qflag, lsum, cand2, ncand2,  cellbits,
+        exact, fkeys, oids, oscores, ocounts, subset, subset_bits, elig, list, counters, lkeys, ST16, qrange, qflag, lsum, cand2, ncand2,  cellbits,
         gkeys, krank, payload, gfkeys, gpayload, cmax16, tau16, plist, pcount, Qi, Qh16t, Ql16t, ST16b, k1diag, k1rows, ulist, nulist, est, kept2, krank2, nkept2, tokp2, ktok2, qnmax, qexp, qrange_tc, mslot, slicecnt, rcmax, rcpairs, rcn, cellflags, estkey, srcrank, xpairs, xnpairs, needexact, gbase, fdiag,
         a5floor, a5live, a5n1, a5n12, a5theta;
+    // subsets: the call's ids, its rows' spans, the passes' per-query rows and n, the all-eligible lists' lengths, the
+    // eligible counts, and the doc-sharded exchanges (plan record, every rank's eligibility rows)
+    DevBuf subspan, qsub, listn, eligcnt, xrec, xall, gelig;
     // host tier: the staged rows of the kept docs (residuals, codes, 1 / |v|), their slot offsets and slot list
     DevBuf s_res, s_codes, s_inv, soff, kept_s;
     cudaEvent_t sev[2] = {};  // around the staging kernels
@@ -1246,7 +1249,7 @@ static pb_status run_k1_tc(pb_index *ix, Workspace &ws, const pb_search_params *
         ws.ST16.as<unsigned short>(), ws.Q.as<float>(), ws.qoff.as<int>(), ix->centroids.as<float>(), ix->dim, cm, ix->K, QS,
         n_chunks, chunk_rows, ws.tau16.as<uint32_t>(), cap, ws.pcount.as<int>(), ws.plist.as<u64>(), d_fallback);
     k_topn_merge<<<dim3(QS, B), 32, 0, ws.stream>>>(ws.plist.as<u64>(), ws.qoff.as<int>(), QS, n, cap / n, ws.sel.as<u64>(),
-                                                  nullptr, 0);
+                                                  nullptr, 0, nullptr);
     // the selected centroids, their exact rows, the variant's threshold rule
     const int P = pow2_at_least(std::max(nq_max * n, 1));
     CKS(set_smem(k_cells_unique, (size_t)P * 8));
@@ -1478,20 +1481,51 @@ static pb_status launch_filter(pb_index *ix, Workspace &ws, const KeptView &in, 
 // ------------------------------------------------------------------------------------------
 // the search pipeline
 // ------------------------------------------------------------------------------------------
+struct Fnv64 {  // FNV-1a over the call's arguments
+    u64 h = 14695981039346656037ull;
+    void add(const void *p, size_t n) {
+        for (size_t i = 0; i < n; ++i) h = (h ^ static_cast<const uint8_t *>(p)[i]) * 1099511628211ull;
+    }
+    template <class T> void put(T v) { add(&v, sizeof v); }
+};
+
 struct SearchIO {
     const float *queries;  // host or device
     bool queries_on_device;
     const int64_t *q_off;  // host
     int64_t n_queries;
-    const int64_t *subset;  // host
-    int64_t n_subset;
-    bool has_subset;
+    // Subsets (host).  Per query: query b's ids are sub_ids[sub_off[b] .. sub_off[b + 1]) when has_sub[b] != 0 (has_sub
+    // null: every query has one; sub_off null: none has).  shared_sub: every query has sub_ids[0 .. n_shared).
+    const int64_t *sub_ids;
+    const int64_t *sub_off;
+    const uint8_t *has_sub;
+    int64_t n_shared;
+    bool shared_sub;
     int64_t *out_ids;  // host or device
     float *out_scores;
     int32_t *out_counts;
     bool out_on_device;
     pb_trace *trace;
 };
+
+// query b's id list [*s, *e) of io.sub_ids, or false when it has no subset
+static bool query_subset(const SearchIO &io, int64_t b, int64_t *s, int64_t *e) {
+    if (io.shared_sub) {
+        *s = 0;
+        *e = io.n_shared;
+        return true;
+    }
+    if (!io.sub_off || (io.has_sub && !io.has_sub[b])) return false;
+    *s = io.sub_off[b];
+    *e = io.sub_off[b + 1];
+    return true;
+}
+
+// How a query's cells are selected (a3); a pass holds queries of one kind.  TABLE: no eligibility row, the streaming
+// probe (the tensor-core table where it applies).  STREAM: the streaming probe over the query's eligible centroids.
+// BIG: the row-wise radix select (effective n_ivf_probe beyond the streaming lists).  ALL: every eligible centroid.
+// NONE: nothing eligible, an empty result without a pass.
+enum ProbeKind : uint8_t { PROBE_TABLE, PROBE_STREAM, PROBE_BIG, PROBE_ALL, PROBE_NONE };
 
 // what a search call decides once, before its first sub-batch
 struct SearchPlan {
@@ -1501,13 +1535,18 @@ struct SearchPlan {
     bool empty = false;                       // every result list is empty
     bool prof = false;                        // stage and call times (pb_set_profiling)
     long long Wd = 0, Wk = 0;                 // 32-bit words of a doc / centroid bitmap
-    const uint32_t *d_subset_bits = nullptr;  // the subset as a doc bitmap
-    const uint32_t *d_elig = nullptr;         // the centroids holding a subset doc (dense variant with a subset)
-    long long n_elig = 0;
-    bool all_eligible = false;                // the scaled n_ivf_probe covers every eligible centroid: probe them all
-    int n_probe = 0;                          // the effective n_ivf_probe
-    bool big_probe = false;                   // beyond the streaming probe's lists: the row-wise radix select
-    int QB = 0;                               // queries per sub-batch
+    long long Wke = 0;                        // words of an eligibility row (even: rows travel as 64-bit words)
+    long long D_total = 0;                    // documents of the deployment (doc-sharded: over every rank)
+    int n_probe = 0;                          // n_ivf_probe, capped at K
+    // subsets: one row per distinct id list; the doc bitmap rows, and (dense variant) the eligible-centroid rows
+    int rows = 0;
+    const uint32_t *d_subset_bits = nullptr;
+    const uint32_t *d_elig = nullptr;
+    std::vector<int> qrow;          // [Bt] the query's row, -1 = no subset
+    std::vector<int> qn;            // [Bt] its effective n_ivf_probe (ALL: its eligible count)
+    std::vector<uint8_t> kind;      // [Bt] ProbeKind
+    std::vector<int64_t> order;     // the queries in pass order
+    std::vector<std::pair<int64_t, int>> passes;  // (first position in `order`, queries)
 };
 
 // The arguments and what follows from them alone.  Nothing is enqueued here, so a call refused here takes no workspace.
@@ -1534,86 +1573,235 @@ static pb_status plan_search(pb_index *ix, const pb_search_params *p, const Sear
     plan.Mcap = std::max(plan.M, 1);
     plan.batched = p->centroid_batch_size > 0 && ix->K > p->centroid_batch_size;  // search.rs:337
     plan.sharded = ix->world > 1;
-    if (plan.sharded && io.has_subset && !plan.batched)
-        return pb_fail(PB_ERR_UNSUPPORTED, "subset with the dense variant needs the global eligible-centroid set; "
-                                            "not built for doc-sharded indices");
     // a shard with no documents still takes part in the exchanges
     plan.empty = plan.M == 0 || plan.top_k == 0 || (ix->D == 0 && !plan.sharded);
     plan.prof = ix->profiling;
     return PB_OK;
 }
 
-// The subset, the probe width and the sub-batch size.  With the dense variant a subset's eligible centroids are counted
-// on the device (search.rs:350-382); none at all leaves the call empty.
+// a sharded call's refusal that every rank reached from the same exchanged data: the group stays usable
+static thread_local bool g_search_agreed = false;
+
+// Doc-sharded: the plan-time exchange of one record per rank (status, D, raw sub-batch bound, fingerprint of the
+// subset arguments).  Every rank takes the least bound (equal sub-batches, so the later exchanges agree in size) and
+// the deployment's D for the n_ivf_probe scaling; differing subsets refuse the call on every rank.
+enum { PX_STATUS, PX_D, PX_QB, PX_PRINT, PX_WORDS };
+static pb_status plan_exchange(pb_index *ix, Workspace &ws, pb_status local, u64 print, int *QB, SearchPlan &plan) {
+    const int G = ix->world;
+    long long mine[PX_WORDS] = {(long long)local, ix->D, *QB, (long long)print};
+    std::vector<long long> all((size_t)G * PX_WORDS);
+    CKS(ws.xrec.ensure(PX_WORDS * 8));
+    CKS(ws.xall.ensure((size_t)G * PX_WORDS * 8));
+    CK(cudaMemcpyAsync(ws.xrec.p, mine, PX_WORDS * 8, cudaMemcpyHostToDevice, ws.stream));
+    CKS(shard_allgather(ix, ws.stream, ws.xrec.p, ws.xall.p, PX_WORDS));
+    CK(cudaMemcpyAsync(all.data(), ws.xall.p, all.size() * 8, cudaMemcpyDeviceToHost, ws.stream));
+    CK(cudaStreamSynchronize(ws.stream));
+    g_search_agreed = true;  // from here on every rank decides from the same words
+    for (int r = 0; r < G; ++r) {
+        const pb_status s = (pb_status)all[(size_t)r * PX_WORDS + PX_STATUS];
+        if (s == PB_OK) continue;
+        if (r == ix->rank) return s;  // g_err holds my own message
+        return pb_fail(s, "rank %d of the group failed (status %d)", r, (int)s);
+    }
+    plan.D_total = 0;
+    for (int r = 0; r < G; ++r) {
+        const long long *w = all.data() + (size_t)r * PX_WORDS;
+        if ((u64)w[PX_PRINT] != print)
+            return pb_fail(PB_ERR_INVALID, "the ranks were given different subsets (rank %d differs from rank %d)", r,
+                           ix->rank);
+        plan.D_total += w[PX_D];
+        *QB = (int)std::min<long long>(*QB, w[PX_QB]);
+    }
+    g_search_agreed = false;
+    return PB_OK;
+}
+
+// The subsets, each query's probe kind and width, and the passes.  Subset rows: one doc bitmap per distinct id list,
+// and with the dense variant its eligible centroids (search.rs:350-382), counted on the device and read back once.
 static pb_status plan_probe(pb_index *ix, Workspace &ws, const pb_search_params *p, const SearchIO &io, SearchPlan &plan) {
+    const int64_t Bt = plan.Bt;
     plan.Wd = (ix->D + 31) / 32;
     plan.Wk = (ix->K + 31) / 32;
+    plan.Wke = (plan.Wk + 1) & ~1ll;
+    plan.D_total = ix->D;
     plan.n_probe = (int)std::min<long long>(p->n_ivf_probe, ix->K);
-    if (io.has_subset) {
-        CKS(ws.subset_bits.ensure((size_t)plan.Wd * 4));
-        CK(cudaMemsetAsync(ws.subset_bits.p, 0, (size_t)plan.Wd * 4, ws.stream));
-        if (io.n_subset > 0) {
-            CKS(ws.subset.ensure((size_t)io.n_subset * 8));
-            CK(cudaMemcpyAsync(ws.subset.p, io.subset, (size_t)io.n_subset * 8, cudaMemcpyHostToDevice, ws.stream));
-            k_subset_bits<<<296, 256, 0, ws.stream>>>(ws.subset.as<long long>(), io.n_subset, ix->doc_id_base, ix->D,
-                                                     ws.subset_bits.as<uint32_t>());
-            CK(cudaGetLastError());
-        }
-        plan.d_subset_bits = ws.subset_bits.as<uint32_t>();
-        if (!plan.batched) {
-            // eligible centroids + n_ivf_probe scaling, dense variant only
-            CKS(ws.elig.ensure((size_t)plan.Wk * 4));
-            CKS(ws.misc.ensure(64));  // [0] the eligible count; +16: k_cells_from_bits' list length (probe)
-            CK(cudaMemsetAsync(ws.elig.p, 0, (size_t)plan.Wk * 4, ws.stream));
-            CK(cudaMemsetAsync(ws.misc.p, 0, 64, ws.stream));
-            k_eligible_bits<<<ix->sm_count * 8, 256, 0, ws.stream>>>(plan.d_subset_bits, ix->D, ix->doc_off.as<long long>(),
-                                                                     ix->codes.as<uint32_t>(), ws.elig.as<uint32_t>());
-            k_popcount<<<ix->sm_count, 256, 0, ws.stream>>>(ws.elig.as<uint32_t>(), plan.Wk, ws.misc.as<unsigned long long>());
-            CK(cudaGetLastError());
-            unsigned long long ne = 0;
-            CK(cudaMemcpyAsync(&ne, ws.misc.p, 8, cudaMemcpyDeviceToHost, ws.stream));
-            CK(cudaStreamSynchronize(ws.stream));
-            plan.n_elig = (long long)ne;
-            if (plan.n_elig == 0) {  // every per-token pool is empty -> no cells -> empty results
-                plan.empty = true;
-                return PB_OK;
-            }
-            unsigned long long scaled = io.n_subset > 0 ? (unsigned long long)p->n_ivf_probe * (unsigned long long)ix->D /
-                                                              (unsigned long long)io.n_subset
-                                                        : (unsigned long long)p->n_ivf_probe;
-            scaled = std::max<unsigned long long>(scaled, (unsigned long long)p->n_ivf_probe);
-            scaled = std::min<unsigned long long>(scaled, (unsigned long long)plan.n_elig);
-            plan.d_elig = ws.elig.as<uint32_t>();
-            if ((long long)scaled >= plan.n_elig) plan.all_eligible = true;
-            else plan.n_probe = (int)scaled;
-        }
-    }
-    // effective n_ivf_probe beyond 64: the dense variant switches to a row-wise radix select; the batched variant's
-    // heap-order threshold rule is tied to the streaming formulation, whose per-lane lists hold up to 192 entries
-    const int stream_max = plan.batched ? 192 : 64;
-    plan.big_probe = !plan.all_eligible && plan.n_probe > stream_max;
-    if (plan.big_probe && plan.batched)
-        return pb_fail(PB_ERR_UNSUPPORTED, "n_ivf_probe %d > 192 with the batched variant is not built", plan.n_probe);
 
-    // ---- sub-batching: bound the transposed score matrix ----
-    const int64_t Bt = plan.Bt;
+    // ---- subset rows: queries with the same id list share one; every empty list is the same row ----
+    plan.qrow.assign((size_t)Bt, -1);
+    std::vector<long long> span;  // [2 rows] into sub_ids, then relative to `lo`
+    std::map<std::pair<int64_t, int64_t>, int> row_of;
+    int64_t lo = INT64_MAX, hi = 0;
+    for (int64_t b = 0; b < Bt; ++b) {
+        int64_t s, e;
+        if (!query_subset(io, b, &s, &e)) continue;
+        if (s == e) s = e = 0;
+        auto it = row_of.emplace(std::make_pair(s, e), (int)(span.size() / 2));
+        if (it.second) {
+            span.push_back(s);
+            span.push_back(e);
+            if (s < e) lo = std::min(lo, s), hi = std::max(hi, e);
+        }
+        plan.qrow[(size_t)b] = it.first->second;
+    }
+    plan.rows = (int)(span.size() / 2);
+    if (lo > hi) lo = hi = 0;
+    const bool elig = plan.rows > 0 && !plan.batched;
+
+    // ---- the raw sub-batch bound: the score tables (16-bit always, fp32 only on the exact path) and the per-(query,
+    // doc) scratch (candidate lists, code sums, approximate scores, cut keys, bitmap: 24.2 bytes per document; the
+    // live-row bitmap of the pruned first pass: 1 bit per centroid) share one budget.  A host-tier handle also stages up
+    // to Mcap docs of max_doclen rows per query (residuals, codes, 1 / |v|); a call with subsets holds a doc row and
+    // (dense variant) an eligibility row per query that has one.
     int nq_max_all = 0;
     for (int64_t b = 0; b < Bt; ++b) nq_max_all = std::max<int>(nq_max_all, (int)(io.q_off[b + 1] - io.q_off[b]));
     const int QS_all = query_row_tokens(nq_max_all);
-    if (!plan.all_eligible && !plan.big_probe && (long long)QS_all * plan.n_probe > 8192)
-        return pb_fail(PB_ERR_UNSUPPORTED, "query tokens x n_ivf_probe = %lld exceeds 8192", (long long)QS_all * plan.n_probe);
-    size_t per_q = (size_t)ix->K * QS_all * sizeof(float);
-    if (per_q >= ((size_t)1 << 32))
-        return pb_fail(PB_ERR_UNSUPPORTED, "num_centroids x query tokens x 4 = %zu bytes per query exceeds 2^32", per_q);
-    // sub-batch size: the score tables (16-bit always, fp32 only on the exact path) and the per-(query, doc) scratch
-    // (candidate lists, code sums, approximate scores, cut keys, bitmap: 24.2 bytes per document; the live-row bitmap
-    // of the pruned first pass: 1 bit per centroid) share one budget
-    // A host-tier handle also stages up to Mcap docs of max_doclen rows per query (residuals, codes, 1 / |v|)
     const size_t per_q_all = (size_t)ix->K * QS_all * (k1_tc_usable(ix) ? 2 : 6) + (size_t)ix->D * 24 + (size_t)ix->D / 8 + (size_t)ix->K / 8 + 4096 +
-                             (ix->host_tier ? (size_t)plan.Mcap * std::max(ix->max_doclen, 1) * (ix->packed + 8) : 0);
+                             (ix->host_tier ? (size_t)plan.Mcap * std::max(ix->max_doclen, 1) * (ix->packed + 8) : 0) +
+                             (plan.rows ? (size_t)plan.Wd * 4 + (elig ? (size_t)plan.Wke * 4 : 0) : 0);
     int QB = (int)std::max<size_t>(1, std::min<size_t>((size_t)Bt, ix->st_budget / std::max(g_budget_div, 1) / per_q_all));
     QB = std::min(QB, 256);
-    plan.QB = (int)((Bt + (Bt + QB - 1) / QB - 1) / ((Bt + QB - 1) / QB));  // equal sub-batches
+
+    // ---- the rows on the device: every id of the call in one copy ----
+    auto build_rows = [&]() -> pb_status {
+        if (!plan.rows) return PB_OK;
+        for (size_t i = 0; i < span.size(); i += 2)  // relative to the uploaded ids; empty lists stay [0, 0)
+            if (span[i] < span[i + 1]) span[i] -= lo, span[i + 1] -= lo;
+        CKS(ws.subset.ensure((size_t)std::max<int64_t>(hi - lo, 2) * 8));
+        CKS(ws.subspan.ensure(span.size() * 8));
+        if (hi > lo)
+            CK(cudaMemcpyAsync(ws.subset.p, io.sub_ids + lo, (size_t)(hi - lo) * 8, cudaMemcpyHostToDevice, ws.stream));
+        CK(cudaMemcpyAsync(ws.subspan.p, span.data(), span.size() * 8, cudaMemcpyHostToDevice, ws.stream));
+        long long len_max = 0;
+        for (int r = 0; r < plan.rows; ++r) len_max = std::max(len_max, span[2 * r + 1] - span[2 * r]);
+        const unsigned gx = (unsigned)std::max<long long>(1, std::min<long long>((len_max + 255) / 256,
+                                                                                  std::max(1, ix->sm_count * 4 / plan.rows)));
+        CKS(ws.subset_bits.ensure(std::max<size_t>((size_t)plan.rows * plan.Wd * 4, 16)));
+        CK(cudaMemsetAsync(ws.subset_bits.p, 0, (size_t)plan.rows * plan.Wd * 4, ws.stream));
+        k_subset_bits<<<dim3(gx, plan.rows), 256, 0, ws.stream>>>(ws.subset.as<long long>(), ws.subspan.as<long long>(),
+                                                                 ix->doc_id_base, ix->D, ws.subset_bits.as<uint32_t>(),
+                                                                 plan.Wd);
+        plan.d_subset_bits = ws.subset_bits.as<uint32_t>();
+        if (elig) {
+            CKS(ws.elig.ensure((size_t)plan.rows * plan.Wke * 4));
+            CK(cudaMemsetAsync(ws.elig.p, 0, (size_t)plan.rows * plan.Wke * 4, ws.stream));
+            // a warp per listed doc; the row in shared memory while it fits (K <= 2^19)
+            const size_t sm = (size_t)plan.Wk * 4;
+            const bool in_smem = sm <= 64 * 1024;
+            if (in_smem) CKS(set_smem(k_eligible_bits, sm));
+            const unsigned ge = (unsigned)std::max<long long>(1, std::min<long long>((len_max + 63) / 64,
+                                                                                      std::max(1, ix->sm_count * 2 / plan.rows)));
+            k_eligible_bits<<<dim3(ge, plan.rows), 256, in_smem ? sm : 0, ws.stream>>>(
+                ws.subset.as<long long>(), ws.subspan.as<long long>(), ix->doc_id_base, ix->D, ix->doc_off.as<long long>(),
+                ix->codes.as<uint32_t>(), ws.elig.as<uint32_t>(), plan.Wk, plan.Wke, in_smem ? 1 : 0);
+            plan.d_elig = ws.elig.as<uint32_t>();
+        }
+        CK(cudaGetLastError());
+        return PB_OK;
+    };
+    pb_status local = build_rows();
+    if (plan.sharded) {
+        Fnv64 f;  // the subset arguments as the caller gave them
+        f.put(Bt);
+        for (int64_t b = 0; b < Bt; ++b) {
+            int64_t s = 0, e = 0;
+            const uint8_t has = query_subset(io, b, &s, &e) ? 1 : 0;
+            f.put(has);
+            f.put(e - s);
+            if (has && e > s && !io.shared_sub) f.add(io.sub_ids + s, (size_t)(e - s) * 8);
+        }
+        if (io.shared_sub && io.n_shared > 0) f.add(io.sub_ids, (size_t)io.n_shared * 8);
+        CKS(plan_exchange(ix, ws, local, f.h, &QB, plan));
+        if (elig) {  // global eligibility: every rank's rows, OR-ed on the device
+            const size_t words = (size_t)plan.rows * plan.Wke;
+            CKS(ws.gelig.ensure(words * 4 * ix->world));
+            CKS(shard_allgather(ix, ws.stream, ws.elig.p, ws.gelig.p, words / 2));
+            k_or_ranks<<<ix->sm_count * 4, 256, 0, ws.stream>>>(ws.gelig.as<uint32_t>(), ix->world, (long long)words,
+                                                               ws.elig.as<uint32_t>());
+            CK(cudaGetLastError());
+        }
+    } else CKS(local);
+
+    // ---- every query's kind and n: the eligible counts come back in one read ----
+    std::vector<unsigned long long> ne((size_t)plan.rows, 0ull);
+    if (elig) {
+        CKS(ws.eligcnt.ensure((size_t)plan.rows * 8));
+        CK(cudaMemsetAsync(ws.eligcnt.p, 0, (size_t)plan.rows * 8, ws.stream));
+        const unsigned gp = (unsigned)std::max<long long>(1, std::min<long long>((plan.Wk + 4095) / 4096, 8));
+        k_popcount<<<dim3(gp, plan.rows), 256, 0, ws.stream>>>(ws.elig.as<uint32_t>(), plan.Wke,
+                                                              ws.eligcnt.as<unsigned long long>());
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(ne.data(), ws.eligcnt.p, (size_t)plan.rows * 8, cudaMemcpyDeviceToHost, ws.stream));
+        CK(cudaStreamSynchronize(ws.stream));
+    }
+    if (plan.sharded) g_search_agreed = true;  // the refusals below follow from exchanged data alone
+    // effective n_ivf_probe beyond 64: the dense variant switches to a row-wise radix select; the batched variant's
+    // heap-order threshold rule is tied to the streaming formulation, whose per-lane lists hold up to 192 entries
+    const int stream_max = plan.batched ? 192 : 64;
+    if (plan.batched && plan.n_probe > stream_max)
+        return pb_fail(PB_ERR_UNSUPPORTED, "n_ivf_probe %d > 192 with the batched variant is not built", plan.n_probe);
+    plan.qn.assign((size_t)Bt, plan.n_probe);
+    plan.kind.assign((size_t)Bt, PROBE_TABLE);
+    for (int64_t b = 0; b < Bt; ++b) {
+        const int r = plan.qrow[(size_t)b];
+        int n = plan.n_probe;
+        uint8_t k = n > stream_max ? PROBE_BIG : PROBE_TABLE;
+        if (elig && r >= 0) {
+            const unsigned long long n_elig = ne[(size_t)r];
+            const unsigned long long len = (unsigned long long)(io.shared_sub ? io.n_shared : io.sub_off[b + 1] - io.sub_off[b]);
+            // n_ivf_probe scaled by D / |subset| (raw length, duplicates and out-of-range ids counted)
+            unsigned long long scaled = len > 0 ? (unsigned long long)p->n_ivf_probe * (unsigned long long)plan.D_total / len
+                                                : (unsigned long long)p->n_ivf_probe;
+            scaled = std::max<unsigned long long>(scaled, (unsigned long long)p->n_ivf_probe);
+            scaled = std::min<unsigned long long>(scaled, n_elig);
+            if (n_elig == 0) k = PROBE_NONE, n = 0;  // every per-token pool is empty -> no cells
+            else if (scaled >= n_elig) k = PROBE_ALL, n = (int)n_elig;
+            else n = (int)scaled, k = n > stream_max ? PROBE_BIG : PROBE_STREAM;
+        }
+        plan.kind[(size_t)b] = k;
+        plan.qn[(size_t)b] = n;
+    }
+    // the limits of pb_search_batch, query by query
+    for (int64_t b = 0; b < Bt; ++b) {
+        const uint8_t k = plan.kind[(size_t)b];
+        if (k == PROBE_NONE) continue;
+        const int QS = query_row_tokens((int)(io.q_off[b + 1] - io.q_off[b]));
+        if ((k == PROBE_TABLE || k == PROBE_STREAM) && (long long)QS * plan.qn[(size_t)b] > 8192)
+            return pb_fail(PB_ERR_UNSUPPORTED, "query tokens x n_ivf_probe = %lld exceeds 8192",
+                           (long long)QS * plan.qn[(size_t)b]);
+        const size_t per_q = (size_t)ix->K * QS * sizeof(float);
+        if (per_q >= ((size_t)1 << 32))
+            return pb_fail(PB_ERR_UNSUPPORTED, "num_centroids x query tokens x 4 = %zu bytes per query exceeds 2^32", per_q);
+    }
+    g_search_agreed = false;
+
+    // ---- passes: the queries of each kind in input order, in equal sub-batches of at most QB; a streaming pass also
+    // keeps its widest query row x its largest n within 8192 ----
+    for (uint8_t k = PROBE_TABLE; k < PROBE_NONE; ++k) {
+        std::vector<int64_t> run;
+        for (int64_t b = 0; b < Bt; ++b)
+            if (plan.kind[(size_t)b] == k) run.push_back(b);
+        if (run.empty()) continue;
+        const int64_t L = (int64_t)run.size();
+        const int64_t per = (L + (L + QB - 1) / QB - 1) / ((L + QB - 1) / QB);  // equal sub-batches
+        int64_t at = (int64_t)plan.order.size();
+        int cur = 0, qs_max = 0, n_max = 0;
+        for (int64_t b : run) {
+            const int QS = query_row_tokens((int)(io.q_off[b + 1] - io.q_off[b]));
+            const int qs2 = std::max(qs_max, QS), n2 = std::max(n_max, plan.qn[(size_t)b]);
+            const bool wide = (k == PROBE_TABLE || k == PROBE_STREAM) && (long long)qs2 * n2 > 8192;
+            if (cur > 0 && (cur == per || wide)) {
+                plan.passes.emplace_back(at, cur);
+                at += cur;
+                cur = 0;
+                qs_max = n_max = 0;
+            }
+            qs_max = std::max(qs_max, QS);
+            n_max = std::max(n_max, plan.qn[(size_t)b]);
+            plan.order.push_back(b);
+            ++cur;
+        }
+        plan.passes.emplace_back(at, cur);
+    }
     return PB_OK;
 }
 
@@ -1623,25 +1811,34 @@ struct HostCounts {
     unsigned long long *cnt;  // [B + 4] ws.counters
     long long *surv_tok;      // [B] tokens of the filter's survivors
     int *cells, *cand, *kept, *surv, *recheck, *pairs, *need;  // [B] each
+    int *qrow, *qn;           // [B] each, up: the queries' subset rows and n_ivf_probe (Pass::rows)
     int *fell;                // the threshold-first probe's fallback flag
 };
 static pb_status map_host_counts(HostBuf &hb, int B, HostCounts &h) {
     const size_t at_cnt = ((size_t)(B + 1) * 4 + 15) & ~(size_t)15, at_tok = at_cnt + (size_t)(B + 4) * 8,
                  at_int = at_tok + (size_t)B * 8;
-    CKS(hb.ensure(at_int + ((size_t)7 * B + 1) * 4));
+    CKS(hb.ensure(at_int + ((size_t)9 * B + 1) * 4));
     char *base = hb.as<char>();
     h.qoff = reinterpret_cast<int *>(base);
     h.cnt = reinterpret_cast<unsigned long long *>(base + at_cnt);
     h.surv_tok = reinterpret_cast<long long *>(base + at_tok);
     int *c = reinterpret_cast<int *>(base + at_int);
-    for (int **f : {&h.cells, &h.cand, &h.kept, &h.surv, &h.recheck, &h.pairs, &h.need, &h.fell}) *f = c, c += B;
+    for (int **f : {&h.cells, &h.cand, &h.kept, &h.surv, &h.recheck, &h.pairs, &h.need, &h.qrow, &h.qn, &h.fell})
+        *f = c, c += B;
     return PB_OK;
 }
 
 // One pass of the pipeline over a sub-batch: its inputs, then what one stage hands to a later one
 struct Pass {
-    int64_t b0 = 0, r0 = 0, R = 0;  // first query, its first token, the sub-batch's tokens
+    const int64_t *q = nullptr;  // [B] the input positions of its queries (ascending within a kind)
+    int64_t R = 0;               // the sub-batch's tokens
     int B = 0, nq_max = 0, QS = 0;
+    // the probe kind of its queries and their largest n_ivf_probe; rows: the queries' subset rows and n on the device
+    // (d_qrow / d_qn), when any query has a row or its own n
+    uint8_t kind = PROBE_TABLE;
+    int n = 0;
+    bool rows = false;
+    const int *d_qrow = nullptr, *d_qn = nullptr;
     // use_tc: a2 + a3 on the tensor cores.  A flagged query or a probe-list overflow raises a device flag instead of
     // being read back mid-way; the pass then finishes on (memory-safe) garbage and is redone on the exact path.
     bool use_tc = false;
@@ -1665,25 +1862,38 @@ struct Pass {
     int *d_cn = nullptr;
 };
 
-// H2D: the query tokens and offsets of the sub-batch
-static pb_status upload_queries(pb_index *ix, Workspace &ws, const SearchIO &io, Pass &pass) {
+// H2D: the query tokens and offsets of the sub-batch, gathered from their input positions, and their subset rows
+static pb_status upload_queries(pb_index *ix, Workspace &ws, const SearchIO &io, const SearchPlan &plan, Pass &pass) {
     const int B = pass.B;
-    const size_t bytes = (size_t)pass.R * ix->dim * 4;
+    const size_t bytes = (size_t)pass.R * ix->dim * 4, row = (size_t)ix->dim * 4;
     CKS(ws.Q.ensure(std::max<size_t>(bytes, 16)));
     CKS(ws.qoff.ensure((size_t)(B + 1) * 4));
+    CKS(map_host_counts(ws.hcounts, B, pass.hc));
+    pass.hc.qoff[0] = 0;
+    for (int b = 0; b < B; ++b) pass.hc.qoff[b + 1] = pass.hc.qoff[b] + (int)(io.q_off[pass.q[b] + 1] - io.q_off[pass.q[b]]);
     if (pass.R > 0) {
-        const float *src = io.queries + (size_t)pass.r0 * ix->dim;
-        if (io.queries_on_device)
+        if (io.queries_on_device) {  // no subsets: the queries of a pass are consecutive
+            const float *src = io.queries + (size_t)io.q_off[pass.q[0]] * ix->dim;
             CK(cudaMemcpyAsync(ws.Q.p, src, bytes, cudaMemcpyDeviceToDevice, ws.stream));
-        else {
+        } else {
             CKS(ws.hq.ensure(bytes));
-            memcpy(ws.hq.p, src, bytes);
+            for (int b = 0; b < B; ++b)
+                memcpy(ws.hq.as<char>() + (size_t)pass.hc.qoff[b] * row, io.queries + (size_t)io.q_off[pass.q[b]] * ix->dim,
+                       (size_t)(pass.hc.qoff[b + 1] - pass.hc.qoff[b]) * row);
             CK(cudaMemcpyAsync(ws.Q.p, ws.hq.p, bytes, cudaMemcpyHostToDevice, ws.stream));
         }
     }
-    CKS(map_host_counts(ws.hcounts, B, pass.hc));
-    for (int b = 0; b <= B; ++b) pass.hc.qoff[b] = (int)(io.q_off[pass.b0 + b] - pass.r0);
     CK(cudaMemcpyAsync(ws.qoff.p, pass.hc.qoff, (size_t)(B + 1) * 4, cudaMemcpyHostToDevice, ws.stream));
+    if (pass.rows) {
+        for (int b = 0; b < B; ++b) {
+            pass.hc.qrow[b] = plan.qrow[(size_t)pass.q[b]];
+            pass.hc.qn[b] = plan.qn[(size_t)pass.q[b]];
+        }
+        CKS(ws.qsub.ensure((size_t)B * 8));
+        CK(cudaMemcpyAsync(ws.qsub.p, pass.hc.qrow, (size_t)B * 8, cudaMemcpyHostToDevice, ws.stream));  // qrow, qn adjacent
+        pass.d_qrow = ws.qsub.as<int>();
+        pass.d_qn = ws.qsub.as<int>() + B;
+    }
     return PB_OK;
 }
 
@@ -1708,7 +1918,7 @@ static pb_status centroid_scores(pb_index *ix, Workspace &ws, const pb_search_pa
         L[PB_STAGE_CENTROID_SCORES] += 1;
     }
     if (pass.use_tc)
-        return run_k1_tc(ix, ws, p, B, QS, pass.nq_max, plan.n_probe, plan.batched, L, &pass.cells_cap,
+        return run_k1_tc(ix, ws, p, B, QS, pass.nq_max, pass.n, plan.batched, L, &pass.cells_cap,
                          &pass.d_probe_fallback);
     CKS(launch_centroid_scores(ix, ws, B, QS, &L[PB_STAGE_CENTROID_SCORES], with16));
     // PB_K1_TC_DIAG: the tensor-core table next to the exact one, compared code by code
@@ -1721,14 +1931,17 @@ static pb_status probe(pb_index *ix, Workspace &ws, const pb_search_params *p, c
     if (pass.use_tc) return PB_OK;
     const int B = pass.B, QS = pass.QS;
     int *L = g_stats.launches;
-    if (plan.all_eligible) {
-        pass.cells_cap = (int)plan.n_elig;
-        CKS(ws.list.ensure((size_t)plan.n_elig * 4 + 16));
+    // each query reads its own eligibility row and n (pass.d_qrow / d_qn); lists are sized by the pass's largest n
+    const uint32_t *elig = pass.rows ? plan.d_elig : nullptr;
+    if (pass.kind == PROBE_ALL) {
+        pass.cells_cap = pass.n;  // the largest eligible count of the pass
+        CKS(ws.list.ensure((size_t)B * pass.n * 4 + 16));
+        CKS(ws.listn.ensure((size_t)B * 4 + 16));
         CKS(ws.cells.ensure((size_t)B * pass.cells_cap * 4));
         CKS(ws.ncells.ensure((size_t)B * 4 + 16));
-        int *d_listn = reinterpret_cast<int *>(ws.misc.as<char>() + 16);
-        k_cells_from_bits<<<1, 1024, 0, ws.stream>>>(plan.d_elig, ix->K, ws.list.as<uint32_t>(), d_listn);
-        k_cells_filter_list<<<B, 256, 0, ws.stream>>>(ws.list.as<uint32_t>(), d_listn, ws.ST.as<float>(),
+        k_cells_from_bits<<<B, 1024, 0, ws.stream>>>(plan.d_elig, pass.d_qrow, plan.Wke, ix->K, ws.list.as<uint32_t>(),
+                                                     pass.n, ws.listn.as<int>());
+        k_cells_filter_list<<<B, 256, 0, ws.stream>>>(ws.list.as<uint32_t>(), pass.n, ws.listn.as<int>(), ws.ST.as<float>(),
                                                       ws.qoff.as<int>(), ix->K, QS, p->has_centroid_score_threshold,
                                                       p->centroid_score_threshold, pass.cells_cap, ws.cells.as<uint32_t>(),
                                                       ws.ncells.as<int>());
@@ -1736,14 +1949,15 @@ static pb_status probe(pb_index *ix, Workspace &ws, const pb_search_params *p, c
         L[PB_STAGE_PROBE] += 2;
         return PB_OK;
     }
-    const int n = plan.n_probe;
+    const int n = pass.n;
     pass.cells_cap = (int)std::min<long long>((long long)QS * n, ix->K);
-    if (plan.big_probe) {
+    if (pass.kind == PROBE_BIG) {
         CKS(ws.cellbits.ensure((size_t)B * plan.Wk * 4));
         CKS(ws.cells.ensure((size_t)B * pass.cells_cap * 4));
         CKS(ws.ncells.ensure((size_t)B * 4 + 16));
-        k_topn_select_row<<<dim3(QS, B), 256, 0, ws.stream>>>(ws.ST.as<float>(), ws.qoff.as<int>(), ix->K, QS, n,
-                                                              plan.d_elig, ws.cellbits.as<uint32_t>(), plan.Wk);
+        k_topn_select_row<<<dim3(QS, B), 256, 0, ws.stream>>>(ws.ST.as<float>(), ws.qoff.as<int>(), ix->K, QS, pass.d_qn,
+                                                              elig, pass.d_qrow, plan.Wke, ws.cellbits.as<uint32_t>(),
+                                                              plan.Wk);
         k_cells_from_query_bits<<<B, 1024, 0, ws.stream>>>(ws.cellbits.as<uint32_t>(), plan.Wk, ws.ST.as<float>(),
                                                            ws.qoff.as<int>(), ix->K, QS, p->has_centroid_score_threshold,
                                                            p->centroid_score_threshold, pass.cells_cap,
@@ -1764,7 +1978,7 @@ static pb_status probe(pb_index *ix, Workspace &ws, const pb_search_params *p, c
     const int GQ = QS / 8;
     int t_chunks = 0;
     const int t_rows = probe_chunk_rows(ix->K, n, &t_chunks);
-    const bool thr_path = pass.fast && !plan.d_elig && ix->probe16 && GQ <= 32 && t_chunks >= n && n <= 192;
+    const bool thr_path = pass.fast && pass.kind == PROBE_TABLE && ix->probe16 && GQ <= 32 && t_chunks >= n && n <= 192;
     int *d_fallback = nullptr;
     pass.probe_list_only = !thr_path;
     if (thr_path) {
@@ -1775,14 +1989,15 @@ static pb_status probe(pb_index *ix, Workspace &ws, const pb_search_params *p, c
             ws.ST16.as<unsigned short>(), ws.ST.as<float>(), ix->K, QS, t_chunks, t_rows, ws.tau16.as<uint32_t>(), cap,
             ws.pcount.as<int>(), ws.plist.as<u64>(), d_fallback);
         k_topn_merge<<<dim3(QS, B), 32, 0, ws.stream>>>(ws.plist.as<u64>(), ws.qoff.as<int>(), QS, n, cap / n,
-                                                      ws.sel.as<u64>(), d_fallback, 0);
+                                                      ws.sel.as<u64>(), d_fallback, 0, nullptr);
         CK(cudaGetLastError());
         L[PB_STAGE_PROBE] += 4;
     }
     k_topn_partial<<<dim3((n_chunks + 3) / 4, B, (QS + 31) / 32), 128, sm1, ws.stream>>>(
-        ws.ST.as<float>(), ws.qoff.as<int>(), ix->K, QS, n, plan.d_elig, ws.partial.as<u64>(), n_chunks, d_fallback, 1);
+        ws.ST.as<float>(), ws.qoff.as<int>(), ix->K, QS, n, elig, pass.d_qrow, plan.Wke, pass.d_qn, ws.partial.as<u64>(),
+        n_chunks, d_fallback, 1);
     k_topn_merge<<<dim3(QS, B), 32, 0, ws.stream>>>(ws.partial.as<u64>(), ws.qoff.as<int>(), QS, n, n_chunks,
-                                                  ws.sel.as<u64>(), d_fallback, 1);
+                                                  ws.sel.as<u64>(), d_fallback, 1, pass.d_qn);
     const int P = pow2_at_least(std::max(pass.nq_max * n, 1));
     size_t sm2 = (size_t)P * 12;
     CKS(set_smem(k_cells, sm2));
@@ -1806,7 +2021,8 @@ static pb_status candidates(pb_index *ix, Workspace &ws, const SearchPlan &plan,
     CKS(ws.ncand.ensure((size_t)B * 4 + 16));
     k_mark<<<dim3(pass.cells_cap, B), 128, 0, ws.stream>>>(ws.cells.as<uint32_t>(), ws.ncells.as<int>(), pass.cells_cap,
                                                           ix->ivf.as<uint32_t>(), ix->ivf_off.as<long long>(),
-                                                          plan.d_subset_bits, ws.bitmap.as<uint32_t>(), Wd);
+                                                          pass.rows ? plan.d_subset_bits : nullptr, pass.d_qrow,
+                                                          ws.bitmap.as<uint32_t>(), Wd);
     const int slices = (int)std::max<long long>(1, std::min<long long>(32, (4ll * ix->sm_count + B - 1) / B));
     CKS(ws.slicecnt.ensure((size_t)B * slices * 4));
     k_compact_count<<<dim3(slices, B), 256, 0, ws.stream>>>(ws.bitmap.as<uint32_t>(), Wd, ws.slicecnt.as<int>());
@@ -2115,10 +2331,10 @@ static pb_status exact_scores(pb_index *ix, Workspace &ws, const SearchPlan &pla
 // every shard's
 static pb_status select_topk(pb_index *ix, Workspace &ws, const SearchIO &io, const SearchPlan &plan, Pass &pass) {
     const int B = pass.B, M = plan.M, top_k = plan.top_k, Mcap = plan.Mcap;
-    if (io.out_on_device) {
-        pass.d_ids = reinterpret_cast<long long *>(io.out_ids) + (size_t)pass.b0 * top_k;
-        pass.d_sc = io.out_scores + (size_t)pass.b0 * top_k;
-        pass.d_cn = io.out_counts + pass.b0;
+    if (io.out_on_device) {  // no subsets: the queries of a pass are consecutive
+        pass.d_ids = reinterpret_cast<long long *>(io.out_ids) + (size_t)pass.q[0] * top_k;
+        pass.d_sc = io.out_scores + (size_t)pass.q[0] * top_k;
+        pass.d_cn = io.out_counts + pass.q[0];
     } else {
         CKS(ws.oids.ensure((size_t)B * top_k * 8));
         CKS(ws.oscores.ensure((size_t)B * top_k * 4));
@@ -2187,11 +2403,14 @@ static pb_status finish(pb_index *ix, Workspace &ws, const SearchIO &io, const S
         *redo = true;
         return PB_OK;
     }
-    if (!io.out_on_device) {
-        char *h = ws.hres.as<char>();
-        memcpy(io.out_ids + (size_t)pass.b0 * top_k, h, (size_t)B * top_k * 8);
-        memcpy(io.out_scores + (size_t)pass.b0 * top_k, h + (size_t)B * top_k * 8, (size_t)B * top_k * 4);
-        memcpy(io.out_counts + pass.b0, h + (size_t)B * top_k * 12, (size_t)B * 4);
+    if (!io.out_on_device) {  // back to the queries' input positions
+        const char *h = ws.hres.as<char>();
+        for (int b = 0; b < B; ++b) {
+            const int64_t g = pass.q[b];
+            memcpy(io.out_ids + (size_t)g * top_k, h + (size_t)b * top_k * 8, (size_t)top_k * 8);
+            memcpy(io.out_scores + (size_t)g * top_k, h + (size_t)B * top_k * 8 + (size_t)b * top_k * 4, (size_t)top_k * 4);
+            memcpy(io.out_counts + g, h + (size_t)B * top_k * 12 + (size_t)b * 4, 4);
+        }
     }
     if (plan.prof) {
         for (int s = 0; s < PB_STAGE_COUNT; ++s) {
@@ -2266,7 +2485,7 @@ static pb_status dump_trace(pb_index *ix, Workspace &ws, const SearchIO &io, con
     pb_trace *t = io.trace;
     const HostCounts &hc = pass.hc;
     for (int b = 0; b < pass.B; ++b) {
-        const int64_t gb = pass.b0 + b;
+        const int64_t gb = pass.q[b];
         if (t->n_cells) t->n_cells[gb] = hc.cells[b];
         if (t->n_candidates) t->n_candidates[gb] = hc.cand[b];
         if (t->n_kept) t->n_kept[gb] = hc.kept[b];
@@ -2308,7 +2527,7 @@ static pb_status run_pass(pb_index *ix, Workspace &ws, const pb_search_params *p
     *redo = false;
     const auto mark = [&](int s) { return plan.prof ? cudaEventRecord(ws.ev[s], ws.stream) : cudaSuccess; };
     CK(mark(0));
-    CKS(upload_queries(ix, ws, io, pass));
+    CKS(upload_queries(ix, ws, io, plan, pass));
     CK(mark(1));
     CKS(centroid_scores(ix, ws, p, plan, pass));
     CK(mark(2));
@@ -2362,33 +2581,46 @@ static pb_status run_search(pb_index *ix, const pb_search_params *p, const Searc
     } rel{ix, wsp};
 
     if (!plan.empty) CKS(plan_probe(ix, ws, p, io, plan));
-    if (plan.empty) {
-        if (io.out_on_device) CK(cudaMemsetAsync(io.out_counts, 0, (size_t)plan.Bt * 4, ws.stream));
-        else memset(io.out_counts, 0, (size_t)plan.Bt * 4);
+    // empty results: the whole call, or the queries with nothing eligible (they get no pass)
+    for (int64_t b = 0; b < plan.Bt; ++b) {
+        if (!plan.empty && plan.kind[(size_t)b] != PROBE_NONE) continue;
+        if (io.out_on_device) CK(cudaMemsetAsync(io.out_counts + b, 0, 4, ws.stream));
+        else io.out_counts[b] = 0;
+        if (pb_trace *t = io.trace) {
+            if (t->n_cells) t->n_cells[b] = 0;
+            if (t->n_candidates) t->n_candidates[b] = 0;
+            if (t->n_kept) t->n_kept[b] = 0;
+        }
+    }
+    if (plan.empty || plan.passes.empty()) {
         CK(cudaStreamSynchronize(ws.stream));
         rel.ok = true;
         return PB_OK;
     }
 
     if (plan.prof) CK(cudaEventRecord(ws.call_ev[0], ws.stream));
-    for (int64_t b0 = 0; b0 < plan.Bt; b0 += plan.QB) {
+    for (const auto &pp : plan.passes) {
         Pass pass;
-        pass.b0 = b0;
-        pass.B = (int)std::min<int64_t>(plan.QB, plan.Bt - b0);
-        pass.r0 = io.q_off[b0];
-        pass.R = io.q_off[b0 + pass.B] - pass.r0;
-        for (int b = 0; b < pass.B; ++b)
-            pass.nq_max = std::max(pass.nq_max, (int)(io.q_off[b0 + b + 1] - io.q_off[b0 + b]));
+        pass.q = plan.order.data() + pp.first;
+        pass.B = pp.second;
+        for (int b = 0; b < pass.B; ++b) {
+            const int64_t g = pass.q[b];
+            pass.R += io.q_off[g + 1] - io.q_off[g];
+            pass.nq_max = std::max(pass.nq_max, (int)(io.q_off[g + 1] - io.q_off[g]));
+            pass.n = std::max(pass.n, plan.qn[(size_t)g]);
+            pass.rows = pass.rows || plan.qrow[(size_t)g] >= 0;
+        }
+        pass.kind = plan.kind[(size_t)pass.q[0]];
+        pass.rows = pass.rows || pass.kind != PROBE_TABLE;
         pass.QS = query_row_tokens(pass.nq_max);
         pass.fast = ix->fast_approx && !io.trace;  // trace wants every candidate's exact approx score
         pass.prune = pass.fast && ix->a5_prune && pass.QS <= 64;
         // the score table comes from the tensor cores unless something needs the dense fp32 S (an eligibility filter,
         // the radix-select probe, a trace) or the shape is outside the kernel's (DESIGN.md "a2")
         int n_chunks_k = 0;
-        probe_chunk_rows(ix->K, plan.n_probe, &n_chunks_k);
-        pass.use_tc = k1_tc_usable(ix) && pass.fast && ix->probe16 && !ix->k1_diag && !plan.all_eligible &&
-                      !plan.big_probe && !plan.d_elig && pass.QS / 8 <= 32 && n_chunks_k >= plan.n_probe &&
-                      plan.n_probe <= 192;
+        probe_chunk_rows(ix->K, pass.n, &n_chunks_k);
+        pass.use_tc = k1_tc_usable(ix) && pass.fast && ix->probe16 && !ix->k1_diag && pass.kind == PROBE_TABLE &&
+                      pass.QS / 8 <= 32 && n_chunks_k >= pass.n && pass.n <= 192;
         pass.filt = filter_runs(ix, io, plan, pass);
         bool redo = false;
         CKS(run_pass(ix, ws, p, io, plan, pass, &redo));
@@ -2439,6 +2671,7 @@ static pb_status search_impl(pb_index *ix, const pb_search_params *p, const Sear
     // would block them while this thread waits for them)
     std::shared_lock<std::shared_mutex> rd;
     if (ix) rd = ix->read_lock();
+    g_search_agreed = false;
     // Lanes: the queries of a batch are independent, so the batch is cut into `lanes` slices searched concurrently, each
     // through the whole pipeline on its own workspace and stream (helper threads do the launching).  Not with a trace
     // (per-stage dumps), not doc-sharded (the exchanges are collective calls in batch order), not for small batches.
@@ -2452,7 +2685,8 @@ static pb_status search_impl(pb_index *ix, const pb_search_params *p, const Sear
     }
     if (lanes <= 1) {
         const pb_status st = run_search(ix, p, io);
-        if (st != PB_OK && ix && ix->group) ix->group->fail();  // the peers must not wait for a rank that gave up
+        // the peers must not wait for a rank that gave up; a refusal every rank reached together leaves the group usable
+        if (st != PB_OK && ix && ix->group && !g_search_agreed) ix->group->fail();
         return st;
     }
     while ((int)ix->lane_workers.size() < lanes - 1) ix->lane_workers.emplace_back(new LaneWorker());
@@ -2476,6 +2710,8 @@ static pb_status search_impl(pb_index *ix, const pb_search_params *p, const Sear
     for (int l = 0; l < lanes; ++l) {
         const int64_t b0 = Bt * l / lanes, b1 = Bt * (l + 1) / lanes;
         ios[l].q_off = io.q_off + b0;
+        if (io.sub_off) ios[l].sub_off = io.sub_off + b0;  // the offsets stay absolute into sub_ids
+        if (io.has_sub) ios[l].has_sub = io.has_sub + b0;
         ios[l].n_queries = b1 - b0;
         if (io.out_ids) ios[l].out_ids = io.out_ids + b0 * top_k;
         if (io.out_scores) ios[l].out_scores = io.out_scores + b0 * top_k;
@@ -2513,7 +2749,27 @@ extern "C" pb_status pb_search_batch_traced(pb_index *ix, const float *queries, 
                                             int64_t n_queries, const pb_search_params *params, const int64_t *subset,
                                             int64_t n_subset, int64_t *out_ids, float *out_scores, int32_t *out_counts,
                                             pb_trace *trace) {
-    SearchIO io{queries, false, q_tok_offsets, n_queries, subset, subset ? n_subset : 0, subset != nullptr,
+    if (subset && n_subset < 0) return pb_fail(PB_ERR_INVALID, "n_subset < 0");
+    SearchIO io{queries, false, q_tok_offsets, n_queries, subset, nullptr, nullptr, subset ? n_subset : 0,
+                subset != nullptr, out_ids, out_scores, out_counts, false, trace};
+    return search_impl(ix, params, io);
+}
+
+extern "C" pb_status pb_search_batch_subsets(pb_index *ix, const float *queries, const int64_t *q_tok_offsets,
+                                             int64_t n_queries, const pb_search_params *params,
+                                             const int64_t *subset_offsets, const int64_t *subset_ids,
+                                             const uint8_t *has_subset, int64_t *out_ids, float *out_scores,
+                                             int32_t *out_counts, pb_trace *trace) {
+    // the subset arguments, checked whole before any lane takes its slice
+    if (n_queries < 0) return pb_fail(PB_ERR_INVALID, "n_queries < 0");
+    if (subset_offsets) {
+        if (subset_offsets[0] != 0) return pb_fail(PB_ERR_INVALID, "subset_offsets[0] must be 0");
+        for (int64_t b = 0; b < n_queries; ++b)
+            if (subset_offsets[b + 1] < subset_offsets[b]) return pb_fail(PB_ERR_INVALID, "subset_offsets not monotone");
+        if (n_queries > 0 && subset_offsets[n_queries] > 0 && !subset_ids)
+            return pb_fail(PB_ERR_INVALID, "null subset_ids");
+    }
+    SearchIO io{queries, false, q_tok_offsets, n_queries, subset_ids, subset_offsets, has_subset, 0, false,
                 out_ids, out_scores, out_counts, false, trace};
     return search_impl(ix, params, io);
 }
@@ -2528,7 +2784,7 @@ extern "C" pb_status pb_search_batch(pb_index *ix, const float *queries, const i
 extern "C" pb_status pb_search_batch_device(pb_index *ix, const float *d_queries, const int64_t *q_tok_offsets_host,
                                             int64_t n_queries, const pb_search_params *params, int64_t *d_out_ids,
                                             float *d_out_scores, int32_t *d_out_counts) {
-    SearchIO io{d_queries, true, q_tok_offsets_host, n_queries, nullptr, 0, false,
+    SearchIO io{d_queries, true, q_tok_offsets_host, n_queries, nullptr, nullptr, nullptr, 0, false,
                 d_out_ids, d_out_scores, d_out_counts, true, nullptr};
     return search_impl(ix, params, io);
 }
@@ -3931,14 +4187,6 @@ extern "C" pb_status pb_index_delete(pb_index *ix, const int64_t *doc_ids, int64
 // ------------------------------------------------------------------------------------------
 enum { SH_STATUS, SH_RANK, SH_WORLD, SH_BASE, SH_D, SH_N, SH_K, SH_DIM, SH_NBITS, SH_NDEL, SH_PRINT, SH_WORDS };
 enum { SH_OP_DELETE = 1, SH_OP_APPEND = 2, SH_OP_APPEND_ENCODED = 3 };
-
-struct Fnv64 {  // FNV-1a over the call's arguments
-    u64 h = 14695981039346656037ull;
-    void add(const void *p, size_t n) {
-        for (size_t i = 0; i < n; ++i) h = (h ^ static_cast<const uint8_t *>(p)[i]) * 1099511628211ull;
-    }
-    template <class T> void put(T v) { add(&v, sizeof v); }
-};
 
 // every rank's `words` 64-bit words, in rank order; a handle outside any group is a group of one
 static pb_status gather_words(pb_index *ix, const long long *mine, int words, std::vector<long long> &all,

@@ -2,20 +2,23 @@
 // Part of kernels.cuh (included from there, in order; not a standalone header).
 // ------------------------------------------------------------------------------------------
 // a4: candidates = sorted unique union of the posting lists of the surviving cells.
-// k_mark: grid = (cells_cap, B): set one bit per (query, doc).  k_compact_count / k_compact_emit turn the bitmap
+// k_mark: grid = (cells_cap, B): set one bit per (query, doc) of the query's subset row, if it has one.  k_compact_count / k_compact_emit turn the bitmap
 // into an ascending doc-id list (and clear it for the next call).
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128)
 k_mark(const uint32_t *__restrict__ cells, const int *__restrict__ n_cells, int cells_cap,
        const uint32_t *__restrict__ ivf, const long long *__restrict__ ivf_off,
-       const uint32_t *__restrict__ subset_bits, uint32_t *__restrict__ bitmap, long long W) {
+       const uint32_t *__restrict__ subset_bits, const int *__restrict__ qrow, uint32_t *__restrict__ bitmap,
+       long long W) {
     const int b = blockIdx.y;
     if ((int)blockIdx.x >= n_cells[b]) return;
     const uint32_t c = cells[(size_t)b * cells_cap + blockIdx.x];
     uint32_t *bm = bitmap + (size_t)b * W;
+    // the query's subset row (k_subset_bits), or none
+    const uint32_t *sb = (subset_bits && qrow[b] >= 0) ? subset_bits + (size_t)qrow[b] * W : nullptr;
     for (long long i = ivf_off[c] + threadIdx.x; i < ivf_off[c + 1]; i += blockDim.x) {
         uint32_t d = ivf[i];
-        if (subset_bits && !((subset_bits[d >> 5] >> (d & 31)) & 1u)) continue;
+        if (sb && !((sb[d >> 5] >> (d & 31)) & 1u)) continue;
         atomicOr(&bm[d >> 5], 1u << (d & 31));
     }
 }

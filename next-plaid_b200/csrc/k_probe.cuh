@@ -8,16 +8,20 @@
 // centroid rows, lane = query token, per-lane list of the n best keys in shared memory.
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128)
-k_topn_partial(const float *__restrict__ ST, const int *__restrict__ q_off, long long K, int QS, int n,
-               const uint32_t *__restrict__ eligible, u64 *__restrict__ partial, int n_chunks,
+k_topn_partial(const float *__restrict__ ST, const int *__restrict__ q_off, long long K, int QS, int n_max,
+               const uint32_t *__restrict__ elig_rows, const int *__restrict__ qrow, long long Wke,
+               const int *__restrict__ qn, u64 *__restrict__ partial, int n_chunks,
                const int *__restrict__ gate, int gate_want) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     if (gate && (*gate != 0) != (gate_want != 0)) return;  // the threshold path (k_collect16) did the work
-    u64 *lists = reinterpret_cast<u64 *>(smem_raw);  // [4 warps][n][32 lanes]
+    u64 *lists = reinterpret_cast<u64 *>(smem_raw);  // [4 warps][n_max][32 lanes]
     const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int b = blockIdx.y, q = blockIdx.z * 32 + lane;
     const int nq = q_off[b + 1] - q_off[b];
-    u64 *mine = lists + (size_t)w * n * 32 + lane;
+    // the query's own n and eligibility row (per-query subsets), lists laid out for the pass's n_max
+    const int n = qn ? qn[b] : n_max;
+    const uint32_t *eligible = (elig_rows && qrow[b] >= 0) ? elig_rows + (size_t)qrow[b] * Wke : nullptr;
+    u64 *mine = lists + (size_t)w * n_max * 32 + lane;
     const int wchunk = blockIdx.x * 4 + w;  // 1024-centroid chunk index
     long long c_begin = (long long)wchunk * 1024, c_end = min(K, c_begin + 1024);
     int cnt = 0, minslot = 0;
@@ -65,8 +69,8 @@ k_topn_partial(const float *__restrict__ ST, const int *__restrict__ q_off, long
         }
     }
     if (q < QS && wchunk < n_chunks) {
-        u64 *out = partial + (((size_t)b * QS + q) * n_chunks + wchunk) * n;
-        for (int s = 0; s < n; ++s) out[s] = (active && s < cnt) ? mine[(size_t)s * 32] : 0ull;
+        u64 *out = partial + (((size_t)b * QS + q) * n_chunks + wchunk) * n_max;
+        for (int s = 0; s < n_max; ++s) out[s] = (active && s < cnt) ? mine[(size_t)s * 32] : 0ull;
     }
 }
 
@@ -201,9 +205,11 @@ k_collect16(const unsigned short *__restrict__ ST16, const float *__restrict__ S
 }
 
 // k_topn_merge: one warp per (b, q): n rounds of "largest key strictly below the previous winner".
-// grid = (QS, B), 32 threads.  sel[b][q][n] gets the winning keys in rank order (0 = none).
+// grid = (QS, B), 32 threads.  sel[b][q][n] gets the winning keys in rank order (0 = none).  qn: each query's own n
+// (rows keep the stride n, the rest zero), or null.
 __global__ void k_topn_merge(const u64 *__restrict__ partial, const int *__restrict__ q_off, int QS,
-                             int n, int n_chunks, u64 *__restrict__ sel, const int *__restrict__ gate, int gate_want) {
+                             int n, int n_chunks, u64 *__restrict__ sel, const int *__restrict__ gate, int gate_want,
+                             const int *__restrict__ qn) {
     if (gate && (*gate != 0) != (gate_want != 0)) return;
     const int q = blockIdx.x, b = blockIdx.y, lane = threadIdx.x;
     const int nq = q_off[b + 1] - q_off[b];
@@ -214,8 +220,10 @@ __global__ void k_topn_merge(const u64 *__restrict__ partial, const int *__restr
     }
     const u64 *in = partial + ((size_t)b * QS + q) * n_chunks * n;
     const int P = n_chunks * n;
+    const int nb = qn ? qn[b] : n;
+    for (int s = nb + lane; s < n; s += 32) out[s] = 0ull;
     u64 bound = ~0ull;
-    for (int r = 0; r < n; ++r) {
+    for (int r = 0; r < nb; ++r) {
         u64 best = 0ull;
         for (int i = lane; i < P; i += 32) {
             u64 k = in[i];
@@ -224,7 +232,7 @@ __global__ void k_topn_merge(const u64 *__restrict__ partial, const int *__restr
         best = warp_max_u64(best);
         if (lane == 0) out[r] = best;
         if (best == 0ull) {
-            for (int s = r + 1 + lane; s < n; s += 32) out[s] = 0ull;
+            for (int s = r + 1 + lane; s < nb; s += 32) out[s] = 0ull;
             break;
         }
         bound = best;

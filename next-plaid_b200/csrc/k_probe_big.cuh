@@ -4,17 +4,22 @@
 // a3 for large effective n_ivf_probe (dense variant; the subset rule scales n_ivf_probe by
 // D / |subset|, search.rs:370-382, far beyond the 64 the streaming lists hold).  One CTA per query
 // token: MSB radix select of the n-th best selection key among the eligible centroids, then every
-// centroid at or above it is marked in the query's cell bitmap.  grid = (QS, B), 256 threads.
+// centroid at or above it is marked in the query's cell bitmap.  grid = (QS, B), 256 threads.  Each query reads its own
+// n and eligibility row, so queries of different subsets share a launch.
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
-k_topn_select_row(const float *__restrict__ ST, const int *__restrict__ q_off, long long K, int QS, long long n,
-                  const uint32_t *__restrict__ eligible, uint32_t *__restrict__ cellbits, long long Wk) {
+k_topn_select_row(const float *__restrict__ ST, const int *__restrict__ q_off, long long K, int QS,
+                  const int *__restrict__ qn, const uint32_t *__restrict__ elig_rows, const int *__restrict__ qrow,
+                  long long Wke, uint32_t *__restrict__ cellbits, long long Wk) {
     __shared__ int hist[256];
     __shared__ u64 prefix_s, mask_s;
     __shared__ long long remaining_s;
     const int q = blockIdx.x, b = blockIdx.y;
     const int nq = q_off[b + 1] - q_off[b];
     if (q >= nq) return;
+    // the query's own n and eligibility row (per-query subsets), or none
+    const long long n = qn[b];
+    const uint32_t *eligible = (elig_rows && qrow[b] >= 0) ? elig_rows + (size_t)qrow[b] * Wke : nullptr;
     const float *col = ST + (size_t)b * K * QS + q;
     uint32_t *bits = cellbits + (size_t)b * Wk;
     if (threadIdx.x == 0) {

@@ -1,69 +1,107 @@
 // k_subset_shard.cuh -- subset pre-filter helpers and the doc-sharded merges.
 // Part of kernels.cuh (included from there, in order; not a standalone header).
-// subset -> doc bitmap (ids outside [base, base+D) are ignored: `candidates.retain` can never match them)
-__global__ void k_subset_bits(const long long *__restrict__ subset, long long n, long long base, long long D,
-                              uint32_t *__restrict__ bits) {
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-        long long d = subset[i] - base;
-        if (d >= 0 && d < D) atomicOr(&bits[d >> 5], 1u << (d & 31));
+// Subsets are per query.  A call's ids are uploaded once; subset row r lists ids[span[2r] .. span[2r + 1]) and every
+// query with that list reads row r (a query without a subset reads none).
+// k_subset_bits: row r's doc bitmap.  Ids outside [base, base+D) set nothing: `candidates.retain` can never match
+// them.  grid = (x, rows)
+__global__ void k_subset_bits(const long long *__restrict__ ids, const long long *__restrict__ span, long long base,
+                              long long D, uint32_t *__restrict__ bits, long long Wd) {
+    const long long s = span[2 * blockIdx.y], e = span[2 * blockIdx.y + 1];
+    uint32_t *row = bits + (size_t)blockIdx.y * Wd;
+    for (long long i = s + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < e; i += (long long)gridDim.x * blockDim.x) {
+        const long long d = ids[i] - base;
+        if (d >= 0 && d < D) atomicOr(&row[d >> 5], 1u << (d & 31));
     }
 }
 
-// eligible centroids of a subset (search.rs:350-364): every code of every subset doc
-__global__ void k_eligible_bits(const uint32_t *__restrict__ subset_bits, long long D,
-                                const long long *__restrict__ doc_off, const uint32_t *__restrict__ codes,
-                                uint32_t *__restrict__ elig) {
-    const int lane = threadIdx.x & 31;
-    const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
-    for (long long d = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); d < D; d += nw) {
-        if (!((subset_bits[d >> 5] >> (d & 31)) & 1u)) continue;
+// k_eligible_bits: row r's eligible centroids (search.rs:350-364), every code of every listed in-range doc; a warp per
+// listed id, so the cost is the subset's tokens.  With `smem` the CTA ORs into a shared copy of the row (Wk words) and
+// flushes its non-zero words once.  grid = (x, rows), 256 threads
+__global__ void __launch_bounds__(256)
+k_eligible_bits(const long long *__restrict__ ids, const long long *__restrict__ span, long long base, long long D,
+                const long long *__restrict__ doc_off, const uint32_t *__restrict__ codes, uint32_t *__restrict__ elig,
+                long long Wk, long long Wke, int smem) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    uint32_t *sh = reinterpret_cast<uint32_t *>(smem_raw);
+    uint32_t *row = elig + (size_t)blockIdx.y * Wke;
+    uint32_t *dst = smem ? sh : row;
+    if (smem) {
+        for (long long i = threadIdx.x; i < Wk; i += blockDim.x) sh[i] = 0u;
+        __syncthreads();
+    }
+    const long long s = span[2 * blockIdx.y], e = span[2 * blockIdx.y + 1];
+    const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+    for (long long i = s + (long long)blockIdx.x * wpb + (threadIdx.x >> 5); i < e; i += (long long)gridDim.x * wpb) {
+        const long long d = ids[i] - base;
+        if (d < 0 || d >= D) continue;  // warp-uniform
         for (long long t = doc_off[d] + lane; t < doc_off[d + 1]; t += 32) {
-            uint32_t c = codes[t];
-            atomicOr(&elig[c >> 5], 1u << (c & 31));
+            const uint32_t c = codes[t];
+            atomicOr(&dst[c >> 5], 1u << (c & 31));
         }
     }
+    if (smem) {
+        __syncthreads();
+        for (long long i = threadIdx.x; i < Wk; i += blockDim.x)
+            if (sh[i]) atomicOr(&row[i], sh[i]);
+    }
 }
 
+// doc-sharded: the OR of every rank's eligibility rows (`words` 32-bit words per rank) into `out`
+__global__ void k_or_ranks(const uint32_t *__restrict__ gathered, int G, long long words, uint32_t *__restrict__ out) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < words; i += (long long)gridDim.x * blockDim.x) {
+        uint32_t v = 0u;
+        for (int g = 0; g < G; ++g) v |= gathered[(size_t)g * words + i];
+        out[i] = v;
+    }
+}
+
+// out[r] += the set bits of row r.  grid = (x, rows)
 __global__ void k_popcount(const uint32_t *__restrict__ bits, long long W, unsigned long long *__restrict__ out) {
+    const uint32_t *row = bits + (size_t)blockIdx.y * W;
     unsigned long long c = 0;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < W; i += (long long)gridDim.x * blockDim.x)
-        c += __popc(bits[i]);
+        c += __popc(row[i]);
     for (int m = 16; m >= 1; m >>= 1) c += __shfl_xor_sync(PB_FULL, c, m);
-    if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, c);
+    if ((threadIdx.x & 31) == 0 && c) atomicAdd(out + blockIdx.y, c);
 }
 
-// "all eligible centroids" as the selected set (n_probe_eff >= |eligible|, search.rs:379)
-__global__ void k_cells_from_bits(const uint32_t *__restrict__ elig, long long K, uint32_t *__restrict__ list,
-                                  int *__restrict__ count) {
-    // single CTA, ascending output
+// "all eligible centroids" as the selected set (n_probe_eff >= |eligible|, search.rs:379): query b's row, ascending,
+// into list[b][lcap].  grid = B, 1024 threads
+__global__ void k_cells_from_bits(const uint32_t *__restrict__ elig, const int *__restrict__ qrow, long long Wke,
+                                  long long K, uint32_t *__restrict__ list, int lcap, int *__restrict__ count) {
     __shared__ int scan_tmp[33];
+    const int b = blockIdx.x;
+    const uint32_t *row = elig + (size_t)qrow[b] * Wke;
+    uint32_t *out = list + (size_t)b * lcap;
     const long long W = (K + 31) / 32;
     const long long per = (W + blockDim.x - 1) / blockDim.x;
     const long long w0 = min(W, (long long)threadIdx.x * per), w1 = min(W, w0 + per);
     int cnt = 0;
-    for (long long i = w0; i < w1; ++i) cnt += __popc(elig[i]);
+    for (long long i = w0; i < w1; ++i) cnt += __popc(row[i]);
     int total;
     int pos = block_exclusive_scan(cnt, scan_tmp, &total);
     for (long long i = w0; i < w1; ++i) {
-        uint32_t x = elig[i];
+        uint32_t x = row[i];
         while (x) {
             int bit = __ffs(x) - 1;
             x &= x - 1;
-            list[pos++] = (uint32_t)(i * 32 + bit);
+            if (pos < lcap) out[pos] = (uint32_t)(i * 32 + bit);
+            ++pos;
         }
     }
-    if (threadIdx.x == 0) *count = total;
+    if (threadIdx.x == 0) count[b] = min(total, lcap);
 }
 
-// threshold filter over a shared centroid list (dense variant only; subset path)
+// threshold filter over each query's centroid list (dense variant only; subset path).  grid = B, 256 threads
 __global__ void __launch_bounds__(256)
-k_cells_filter_list(const uint32_t *__restrict__ list, const int *__restrict__ list_n, const float *__restrict__ ST,
-                    const int *__restrict__ q_off, long long K, int QS, int has_thr, float thr, int cells_cap,
-                    uint32_t *__restrict__ cells, int *__restrict__ n_cells) {
+k_cells_filter_list(const uint32_t *__restrict__ list, int lcap, const int *__restrict__ list_n,
+                    const float *__restrict__ ST, const int *__restrict__ q_off, long long K, int QS, int has_thr,
+                    float thr, int cells_cap, uint32_t *__restrict__ cells, int *__restrict__ n_cells) {
     __shared__ int scan_tmp[33];
     const int b = blockIdx.x;
     const int nq = q_off[b + 1] - q_off[b];
-    const int n = *list_n;
+    const int n = list_n[b];
+    const uint32_t *lst = list + (size_t)b * lcap;
     const float *STb = ST + (size_t)b * K * QS;
     int outn = 0;
     for (int base = 0; base < n; base += blockDim.x) {
@@ -71,7 +109,7 @@ k_cells_filter_list(const uint32_t *__restrict__ list, const int *__restrict__ l
         int f = 0;
         uint32_t c = 0;
         if (i < n && nq > 0) {
-            c = list[i];
+            c = lst[i];
             f = 1;
             if (has_thr) {
                 const float *row = STb + (size_t)c * QS;

@@ -56,6 +56,20 @@ extern "C" {
         out_scores: *mut f32,
         out_counts: *mut i32,
     ) -> c_int;
+    fn pb_search_batch_subsets(
+        ix: *mut c_void,
+        queries: *const f32,
+        q_tok_offsets: *const i64,
+        n_queries: i64,
+        params: *const PbSearchParams,
+        subset_offsets: *const i64,
+        subset_ids: *const i64,
+        has_subset: *const u8,
+        out_ids: *mut i64,
+        out_scores: *mut f32,
+        out_counts: *mut i32,
+        trace: *mut c_void,
+    ) -> c_int;
     fn pb_last_error() -> *const c_char;
     fn pb_codec_open(device: i32, centroids: *const f32, k: i64, dim: i32, nbits: i32, cutoffs: *const f32,
                      out: *mut *mut c_void) -> c_int;
@@ -206,6 +220,76 @@ impl B200Index {
                 ids.as_mut_ptr(),
                 scores.as_mut_ptr(),
                 counts.as_mut_ptr(),
+            )
+        };
+        if st != 0 {
+            return Err(Error::Search(last_error()));
+        }
+        Ok((0..queries.len())
+            .map(|i| {
+                let n = counts[i] as usize;
+                QueryResult {
+                    query_id: i, // search.rs:661
+                    passage_ids: ids[i * k..i * k + n].to_vec(),
+                    scores: scores[i * k..i * k + n].to_vec(),
+                }
+            })
+            .collect())
+    }
+
+    /// `search_batch` with its own `Option<&[i64]>` subset per query (one per request, e.g. each request's
+    /// `filter_condition`): result i equals `search_batch(&queries[i..i + 1], params, subsets[i])`.  Concurrent filtered
+    /// requests can share one call this way (INTEGRATION.md).
+    pub fn search_batch_subsets(
+        &self,
+        queries: &[Array2<f32>],
+        params: &SearchParameters,
+        subsets: &[Option<&[i64]>],
+    ) -> Result<Vec<QueryResult>> {
+        if subsets.len() != queries.len() {
+            return Err(Error::Shape(format!("{} subsets for {} queries", subsets.len(), queries.len())));
+        }
+        let dim = unsafe { pb_index_embedding_dim(self.handle) } as usize;
+        let mut offsets = Vec::with_capacity(queries.len() + 1);
+        offsets.push(0i64);
+        let mut flat: Vec<f32> = Vec::new();
+        for q in queries {
+            if q.ncols() != dim {
+                return Err(Error::Shape(format!("query has {} columns, the index embedding_dim is {}", q.ncols(), dim)));
+            }
+            flat.extend(q.as_standard_layout().iter());
+            offsets.push(offsets.last().unwrap() + q.nrows() as i64);
+        }
+        let mut sub_off = Vec::with_capacity(subsets.len() + 1);
+        sub_off.push(0i64);
+        let mut sub_ids: Vec<i64> = Vec::new();
+        let mut has: Vec<u8> = Vec::with_capacity(subsets.len());
+        for s in subsets {
+            has.push(s.is_some() as u8);
+            if let Some(ids) = s {
+                sub_ids.extend_from_slice(ids);
+            }
+            sub_off.push(sub_ids.len() as i64);
+        }
+        let k = params.top_k;
+        let mut ids = vec![0i64; queries.len() * k.max(1)];
+        let mut scores = vec![0f32; queries.len() * k.max(1)];
+        let mut counts = vec![0i32; queries.len()];
+        let p = PbSearchParams::from(params);
+        let st = unsafe {
+            pb_search_batch_subsets(
+                self.handle,
+                flat.as_ptr(),
+                offsets.as_ptr(),
+                queries.len() as i64,
+                &p,
+                sub_off.as_ptr(),
+                if sub_ids.is_empty() { std::ptr::null() } else { sub_ids.as_ptr() },
+                has.as_ptr(),
+                ids.as_mut_ptr(),
+                scores.as_mut_ptr(),
+                counts.as_mut_ptr(),
+                std::ptr::null_mut(),
             )
         };
         if st != 0 {
