@@ -341,6 +341,20 @@ PB_API pb_status pb_search_batch_subsets(pb_index *ix, const float *queries, con
                                          const int64_t *subset_ids, const uint8_t *has_subset /* [n_queries] */,
                                          int64_t *out_ids, float *out_scores, int32_t *out_counts, pb_trace *trace);
 
+/* pb_search_batch_subsets with search parameters per query: result i equals pb_search_batch_subsets of query i alone
+ * with params[i] (and its subset).  Row i of out_ids / out_scores starts at i * max_i(params[i].top_k); entries past
+ * out_counts[i] are not part of the result.  Each params[i] is checked as pb_search_batch checks its one struct, and a
+ * query that would be refused alone refuses the whole call with the same status, before anything runs; params == NULL
+ * is PB_ERR_INVALID.  A query with top_k == 0 or min(n_full_scores, max(n_full_scores / 4, top_k)) == 0 gets count 0.
+ * Queries with different top_k, n_full_scores, n_ivf_probe or threshold share the batch's passes, so a server can put
+ * concurrent requests with their own parameters into one call.  On a doc-sharded handle it is a collective: ranks
+ * given different parameters (or subsets) all return PB_ERR_INVALID and the group stays usable. */
+PB_API pb_status pb_search_batch_params(pb_index *ix, const float *queries, const int64_t *q_tok_offsets,
+                                        int64_t n_queries, const pb_search_params *params /* [n_queries] */,
+                                        const int64_t *subset_offsets, const int64_t *subset_ids,
+                                        const uint8_t *has_subset, int64_t *out_ids, float *out_scores,
+                                        int32_t *out_counts, pb_trace *trace);
+
 /* ---- stage entry points (each is one kernel of the path; used by tests, bench and ncu) ---- */
 
 /* Stage 1, S = Q * C^T (search.rs:345).  out: [n_query_tokens][K] row-major f32, host. */

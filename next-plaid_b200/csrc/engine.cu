@@ -1199,7 +1199,7 @@ static int probe16_cap(int n) { return n * std::max(2, 128 / n); }
 // (k_chunkmax16) and each query token's threshold, the n-th largest of them (k_tau16).  *d_fallback is the device flag
 // k_tau16 and the kernels after it raise when a query cannot take this path.
 static pb_status probe16_thresholds(pb_index *ix, Workspace &ws, int B, int QS, int n, int n_chunks, int chunk_rows,
-                                    int **d_fallback) {
+                                    const int *qn, int **d_fallback) {
     const int cap = probe16_cap(n);
     CKS(ws.cmax16.ensure((size_t)B * n_chunks * QS * 2));
     CKS(ws.tau16.ensure((size_t)B * QS * 4));
@@ -1211,7 +1211,7 @@ static pb_status probe16_thresholds(pb_index *ix, Workspace &ws, int B, int QS, 
     k_chunkmax16<<<dim3((n_chunks + 3) / 4, B), 128, 0, ws.stream>>>(ws.ST16.as<unsigned short>(), ix->K, QS, n_chunks,
                                                                      chunk_rows, ws.cmax16.as<unsigned short>());
     k_tau16<<<dim3(QS, B), 32, 0, ws.stream>>>(ws.cmax16.as<unsigned short>(), ws.qoff.as<int>(), QS, n, n_chunks,
-                                              ws.qflag.as<int>(), ws.tau16.as<uint32_t>(), fb);
+                                              ws.qflag.as<int>(), ws.tau16.as<uint32_t>(), fb, qn);
     *d_fallback = fb;
     return PB_OK;
 }
@@ -1226,8 +1226,10 @@ static int pow2_at_least(int x) {
 // a2 + a3 on the tensor-core table.  Nothing is read back here: a flagged query or a probe-list overflow raises
 // *d_fallback on the device, the kernels after it stay memory-safe, and the caller redoes the sub-batch on the
 // exact path once it sees the flag at the end.
-static pb_status run_k1_tc(pb_index *ix, Workspace &ws, const pb_search_params *p, int B, int QS, int nq_max, int n,
-                           bool batched, int *L, int *cells_cap_out, const int **d_fallback_out) {
+// n: the pass's largest n_ivf_probe; qn / qhas / qthr: each query's own n and threshold, or null (uniform pass).
+static pb_status run_k1_tc(pb_index *ix, Workspace &ws, int B, int QS, int nq_max, int n, const int *qn, int has_thr,
+                           float thr, const int *qhas, const float *qthr, bool batched, long long slab, int *L,
+                           int *cells_cap_out, const int **d_fallback_out) {
     int n_chunks = 0;
     const int chunk_rows = probe_chunk_rows(ix->K, n, &n_chunks);
     const int cm = 2 * ix->k1_margin + 1;
@@ -1244,12 +1246,12 @@ static pb_status run_k1_tc(pb_index *ix, Workspace &ws, const pb_search_params *
     CKS(ws.nulist.ensure((size_t)B * 4 + 16));
     CKS(ws.k1rows.ensure((size_t)B * cells_cap * QS * 4));
     int *d_fallback = nullptr;
-    CKS(probe16_thresholds(ix, ws, B, QS, n, n_chunks, chunk_rows, &d_fallback));
+    CKS(probe16_thresholds(ix, ws, B, QS, n, n_chunks, chunk_rows, qn, &d_fallback));
     k_collect16_tc<<<dim3((n_chunks + 3) / 4, B), 128, 0, ws.stream>>>(
         ws.ST16.as<unsigned short>(), ws.Q.as<float>(), ws.qoff.as<int>(), ix->centroids.as<float>(), ix->dim, cm, ix->K, QS,
         n_chunks, chunk_rows, ws.tau16.as<uint32_t>(), cap, ws.pcount.as<int>(), ws.plist.as<u64>(), d_fallback);
     k_topn_merge<<<dim3(QS, B), 32, 0, ws.stream>>>(ws.plist.as<u64>(), ws.qoff.as<int>(), QS, n, cap / n, ws.sel.as<u64>(),
-                                                  nullptr, 0, nullptr);
+                                                  nullptr, 0, qn);
     // the selected centroids, their exact rows, the variant's threshold rule
     const int P = pow2_at_least(std::max(nq_max * n, 1));
     CKS(set_smem(k_cells_unique, (size_t)P * 8));
@@ -1266,10 +1268,9 @@ static pb_status run_k1_tc(pb_index *ix, Workspace &ws, const pb_search_params *
     CKS(ws.cellflags.ensure((size_t)B * cells_cap * 4));
     k_cells_thr<<<dim3(8, B), 256, 0, ws.stream>>>(
         ws.sel.as<u64>(), ws.k1rows.as<float>(), ws.ulist.as<uint32_t>(), ws.nulist.as<int>(), ws.qoff.as<int>(), ix->K, QS, n,
-        cells_cap, p->has_centroid_score_threshold, p->centroid_score_threshold, batched ? 1 : 0,
-        batched ? (long long)p->centroid_batch_size : ix->K, ws.cellflags.as<int>(), ws.ST16.as<unsigned short>(),
+        cells_cap, has_thr, thr, batched ? 1 : 0, slab, ws.cellflags.as<int>(), ws.ST16.as<unsigned short>(),
         ws.qrange.as<float2>(), cm, ws.Q.as<float>(), ix->centroids.as<float>(), ix->dim, ws.cmax16.as<unsigned short>(),
-        n_chunks, chunk_rows);
+        n_chunks, chunk_rows, qn, qhas, qthr);
     k_cells_emit<<<B, 256, 0, ws.stream>>>(ws.ulist.as<uint32_t>(), ws.nulist.as<int>(), ws.cellflags.as<int>(), cells_cap,
                                            ws.cells.as<uint32_t>(), ws.ncells.as<int>());
     CK(cudaGetLastError());
@@ -1456,8 +1457,8 @@ static pb_status launch_maxsim_tc(pb_index *ix, Workspace &ws, const KeptView &i
 
 // a7': tensor-core estimate of every kept doc, then the survivors that can still reach the top_k
 static pb_status launch_filter(pb_index *ix, Workspace &ws, const KeptView &in, const KeptView &out, const TokView &tv, int B,
-                               int QS, int Mcap, int top_k, long long max_tokens, float eps_unit, int nq_max,
-                               bool keep_keys, int *launches) {
+                               int QS, int Mcap, int top_k, const int *qtopk, long long max_tokens, float eps_unit,
+                               int nq_max, bool keep_keys, int *launches) {
     // keep_keys: the per (doc, q) maxima go to their own buffer and stay there for the pair pass of the exact stage
     uint32_t *keys = keep_keys ? ws.estkey.as<uint32_t>() : ws.maxkey.as<uint32_t>();
     if (keep_keys) CK(cudaMemsetAsync(keys, 0, (size_t)B * Mcap * QS * 4, ws.stream));
@@ -1472,7 +1473,7 @@ static pb_status launch_filter(pb_index *ix, Workspace &ws, const KeptView &in, 
                                                         ws.qoff.as<int>(), ws.qnmax.as<float>(), eps_unit,
                                                         tv.doc_off, out.kept, out.krank, out.nkept,
                                                         out.tokp, ws.ktok2.as<long long>(),
-                                                        keep_keys ? ws.srcrank.as<uint32_t>() : nullptr);
+                                                        keep_keys ? ws.srcrank.as<uint32_t>() : nullptr, qtopk);
     CK(cudaGetLastError());
     if (launches) *launches += 3 + (keep_keys ? 1 : 0);
     return PB_OK;
@@ -1506,7 +1507,14 @@ struct SearchIO {
     int32_t *out_counts;
     bool out_on_device;
     pb_trace *trace;
+    // search parameters: query b's are qp[b * qp_stride] (stride 0: one struct for the call); rows of out_ids /
+    // out_scores are out_stride entries apart (the call's largest top_k)
+    const pb_search_params *qp;
+    int64_t qp_stride;
+    int64_t out_stride;
 };
+
+static const pb_search_params &query_params(const SearchIO &io, int64_t b) { return io.qp[b * io.qp_stride]; }
 
 // query b's id list [*s, *e) of io.sub_ids, or false when it has no subset
 static bool query_subset(const SearchIO &io, int64_t b, int64_t *s, int64_t *e) {
@@ -1530,14 +1538,19 @@ enum ProbeKind : uint8_t { PROBE_TABLE, PROBE_STREAM, PROBE_BIG, PROBE_ALL, PROB
 // what a search call decides once, before its first sub-batch
 struct SearchPlan {
     int64_t Bt = 0;                           // queries
-    int top_k = 0, M = 0, Mcap = 1;           // M: docs the cut keeps per query (search.rs:468)
-    bool batched = false, sharded = false;    // batched: the centroid-batched variant (search.rs:337)
+    int Mcap = 1, top_k_max = 0;              // the largest M and top_k of the call: buffer strides and budget
+    bool sharded = false;
     bool empty = false;                       // every result list is empty
     bool prof = false;                        // stage and call times (pb_set_profiling)
     long long Wd = 0, Wk = 0;                 // 32-bit words of a doc / centroid bitmap
     long long Wke = 0;                        // words of an eligibility row (even: rows travel as 64-bit words)
     long long D_total = 0;                    // documents of the deployment (doc-sharded: over every rank)
-    int n_probe = 0;                          // n_ivf_probe, capped at K
+    // each query's search parameters (DESIGN.md 4l): M = the docs the cut keeps (search.rs:468), M1 = the first round
+    // of the pruned a5 pass, the threshold (has / value), the variant (batched: search.rs:337) and its slab width
+    std::vector<int> qtopk, qM, qM1, qhas;
+    std::vector<float> qthr;
+    std::vector<uint8_t> qbatched;
+    std::vector<long long> qslab;
     // subsets: one row per distinct id list; the doc bitmap rows, and (dense variant) the eligible-centroid rows
     int rows = 0;
     const uint32_t *d_subset_bits = nullptr;
@@ -1550,13 +1563,20 @@ struct SearchPlan {
 };
 
 // The arguments and what follows from them alone.  Nothing is enqueued here, so a call refused here takes no workspace.
-static pb_status plan_search(pb_index *ix, const pb_search_params *p, const SearchIO &io, SearchPlan &plan) {
-    if (!ix || !p) return pb_fail(PB_ERR_INVALID, "null argument");
+static pb_status plan_search(pb_index *ix, const SearchIO &io, SearchPlan &plan) {
+    if (!ix || !io.qp) return pb_fail(PB_ERR_INVALID, "null argument");
     if (io.n_queries < 0) return pb_fail(PB_ERR_INVALID, "n_queries < 0");
     if (io.n_queries > 0 && (!io.queries || !io.q_off)) return pb_fail(PB_ERR_INVALID, "null queries");
-    if (p->top_k < 0 || p->n_full_scores < 0) return pb_fail(PB_ERR_INVALID, "top_k / n_full_scores must be >= 0");
-    if (p->n_ivf_probe < 1) return pb_fail(PB_ERR_INVALID, "n_ivf_probe must be >= 1");
-    if (p->top_k > 0 && (!io.out_ids || !io.out_scores)) return pb_fail(PB_ERR_INVALID, "null outputs");
+    // every query's parameters as pb_search_batch checks its one struct (one struct: also for an empty batch)
+    const int64_t n_par = io.qp_stride ? io.n_queries : 1;
+    long long top_k_max = 0;
+    for (int64_t b = 0; b < n_par; ++b) {
+        const pb_search_params &p = query_params(io, b);
+        if (p.top_k < 0 || p.n_full_scores < 0) return pb_fail(PB_ERR_INVALID, "top_k / n_full_scores must be >= 0");
+        if (p.n_ivf_probe < 1) return pb_fail(PB_ERR_INVALID, "n_ivf_probe must be >= 1");
+        top_k_max = std::max<long long>(top_k_max, p.top_k);
+    }
+    if (top_k_max > 0 && (!io.out_ids || !io.out_scores)) return pb_fail(PB_ERR_INVALID, "null outputs");
     if (!io.out_counts) return pb_fail(PB_ERR_INVALID, "null out_counts");
     CK(cudaSetDevice(ix->device));
     g_stats = Stats();
@@ -1564,20 +1584,40 @@ static pb_status plan_search(pb_index *ix, const pb_search_params *p, const Sear
     if (plan.Bt == 0) return PB_OK;
     for (int64_t b = 0; b < plan.Bt; ++b)
         if (io.q_off[b + 1] < io.q_off[b]) return pb_fail(PB_ERR_INVALID, "q_tok_offsets not monotone");
-    plan.top_k = (int)p->top_k;
-    const long long n_dec = std::max<long long>(p->n_full_scores / 4, p->top_k);  // search.rs:468
-    const long long Mll = std::min<long long>(p->n_full_scores, n_dec);             // take(nfs).take(n_dec)
-    if (Mll > 16384)
-        return pb_fail(PB_ERR_UNSUPPORTED, "min(n_full_scores, max(n_full_scores/4, top_k)) = %lld exceeds 16384", Mll);
-    plan.M = (int)Mll;
-    plan.Mcap = std::max(plan.M, 1);
-    plan.batched = p->centroid_batch_size > 0 && ix->K > p->centroid_batch_size;  // search.rs:337
+    const size_t Bt = (size_t)plan.Bt;
+    plan.qtopk.resize(Bt), plan.qM.resize(Bt), plan.qM1.resize(Bt), plan.qhas.resize(Bt), plan.qthr.resize(Bt);
+    plan.qbatched.resize(Bt), plan.qslab.resize(Bt);
+    bool all_empty = true;
+    int M_max = 0;
+    for (int64_t b = 0; b < plan.Bt; ++b) {
+        const pb_search_params &p = query_params(io, b);
+        const long long n_dec = std::max<long long>(p.n_full_scores / 4, p.top_k);  // search.rs:468
+        const long long Mll = std::min<long long>(p.n_full_scores, n_dec);          // take(nfs).take(n_dec)
+        if (Mll > 16384)
+            return pb_fail(PB_ERR_UNSUPPORTED, "min(n_full_scores, max(n_full_scores/4, top_k)) = %lld exceeds 16384", Mll);
+        const int M = (int)Mll;
+        const bool batched = p.centroid_batch_size > 0 && ix->K > p.centroid_batch_size;  // search.rs:337
+        plan.qtopk[(size_t)b] = (int)p.top_k;
+        plan.qM[(size_t)b] = M;
+        plan.qM1[(size_t)b] = (int)std::min<double>(ceil((double)ix->a5_m1 * M), (double)INT_MAX);
+        plan.qhas[(size_t)b] = p.has_centroid_score_threshold ? 1 : 0;
+        plan.qthr[(size_t)b] = p.centroid_score_threshold;
+        plan.qbatched[(size_t)b] = batched ? 1 : 0;
+        plan.qslab[(size_t)b] = batched ? (long long)p.centroid_batch_size : ix->K;
+        all_empty = all_empty && (M == 0 || p.top_k == 0);
+        M_max = std::max(M_max, M);
+    }
+    plan.Mcap = std::max(M_max, 1);
+    plan.top_k_max = (int)top_k_max;
     plan.sharded = ix->world > 1;
     // a shard with no documents still takes part in the exchanges
-    plan.empty = plan.M == 0 || plan.top_k == 0 || (ix->D == 0 && !plan.sharded);
+    plan.empty = all_empty || (ix->D == 0 && !plan.sharded);
     plan.prof = ix->profiling;
     return PB_OK;
 }
+
+// a query whose parameters leave nothing to return (top_k == 0 or M == 0): count 0, no pass
+static bool query_empty(const SearchPlan &plan, int64_t b) { return plan.qtopk[(size_t)b] == 0 || plan.qM[(size_t)b] == 0; }
 
 // a sharded call's refusal that every rank reached from the same exchanged data: the group stays usable
 static thread_local bool g_search_agreed = false;
@@ -1607,7 +1647,8 @@ static pb_status plan_exchange(pb_index *ix, Workspace &ws, pb_status local, u64
     for (int r = 0; r < G; ++r) {
         const long long *w = all.data() + (size_t)r * PX_WORDS;
         if ((u64)w[PX_PRINT] != print)
-            return pb_fail(PB_ERR_INVALID, "the ranks were given different subsets (rank %d differs from rank %d)", r,
+            return pb_fail(PB_ERR_INVALID,
+                           "the ranks were given different subsets or parameters (rank %d differs from rank %d)", r,
                            ix->rank);
         plan.D_total += w[PX_D];
         *QB = (int)std::min<long long>(*QB, w[PX_QB]);
@@ -1618,13 +1659,12 @@ static pb_status plan_exchange(pb_index *ix, Workspace &ws, pb_status local, u64
 
 // The subsets, each query's probe kind and width, and the passes.  Subset rows: one doc bitmap per distinct id list,
 // and with the dense variant its eligible centroids (search.rs:350-382), counted on the device and read back once.
-static pb_status plan_probe(pb_index *ix, Workspace &ws, const pb_search_params *p, const SearchIO &io, SearchPlan &plan) {
+static pb_status plan_probe(pb_index *ix, Workspace &ws, const SearchIO &io, SearchPlan &plan) {
     const int64_t Bt = plan.Bt;
     plan.Wd = (ix->D + 31) / 32;
     plan.Wk = (ix->K + 31) / 32;
     plan.Wke = (plan.Wk + 1) & ~1ll;
     plan.D_total = ix->D;
-    plan.n_probe = (int)std::min<long long>(p->n_ivf_probe, ix->K);
 
     // ---- subset rows: queries with the same id list share one; every empty list is the same row ----
     plan.qrow.assign((size_t)Bt, -1);
@@ -1645,7 +1685,9 @@ static pb_status plan_probe(pb_index *ix, Workspace &ws, const pb_search_params 
     }
     plan.rows = (int)(span.size() / 2);
     if (lo > hi) lo = hi = 0;
-    const bool elig = plan.rows > 0 && !plan.batched;
+    // eligible-centroid rows: for the dense-variant queries with a subset
+    bool elig = false;
+    for (int64_t b = 0; b < Bt; ++b) elig = elig || (plan.qrow[(size_t)b] >= 0 && !plan.qbatched[(size_t)b]);
 
     // ---- the raw sub-batch bound: the score tables (16-bit always, fp32 only on the exact path) and the per-(query,
     // doc) scratch (candidate lists, code sums, approximate scores, cut keys, bitmap: 24.2 bytes per document; the
@@ -1710,6 +1752,11 @@ static pb_status plan_probe(pb_index *ix, Workspace &ws, const pb_search_params 
             if (has && e > s && !io.shared_sub) f.add(io.sub_ids + s, (size_t)(e - s) * 8);
         }
         if (io.shared_sub && io.n_shared > 0) f.add(io.sub_ids, (size_t)io.n_shared * 8);
+        for (int64_t b = 0; b < Bt; ++b) {  // the parameters (field by field: the struct has padding)
+            const pb_search_params &q = query_params(io, b);
+            f.put(q.n_full_scores), f.put(q.top_k), f.put(q.n_ivf_probe), f.put(q.centroid_batch_size);
+            f.put(q.has_centroid_score_threshold), f.put(q.centroid_score_threshold);
+        }
         CKS(plan_exchange(ix, ws, local, f.h, &QB, plan));
         if (elig) {  // global eligibility: every rank's rows, OR-ed on the device
             const size_t words = (size_t)plan.rows * plan.Wke;
@@ -1736,22 +1783,27 @@ static pb_status plan_probe(pb_index *ix, Workspace &ws, const pb_search_params 
     if (plan.sharded) g_search_agreed = true;  // the refusals below follow from exchanged data alone
     // effective n_ivf_probe beyond 64: the dense variant switches to a row-wise radix select; the batched variant's
     // heap-order threshold rule is tied to the streaming formulation, whose per-lane lists hold up to 192 entries
-    const int stream_max = plan.batched ? 192 : 64;
-    if (plan.batched && plan.n_probe > stream_max)
-        return pb_fail(PB_ERR_UNSUPPORTED, "n_ivf_probe %d > 192 with the batched variant is not built", plan.n_probe);
-    plan.qn.assign((size_t)Bt, plan.n_probe);
+    for (int64_t b = 0; b < Bt; ++b) {
+        const long long n_probe = std::min<long long>(query_params(io, b).n_ivf_probe, ix->K);
+        if (!query_empty(plan, b) && plan.qbatched[(size_t)b] && n_probe > 192)
+            return pb_fail(PB_ERR_UNSUPPORTED, "n_ivf_probe %d > 192 with the batched variant is not built", (int)n_probe);
+    }
+    plan.qn.assign((size_t)Bt, 0);
     plan.kind.assign((size_t)Bt, PROBE_TABLE);
     for (int64_t b = 0; b < Bt; ++b) {
+        const pb_search_params &p = query_params(io, b);
         const int r = plan.qrow[(size_t)b];
-        int n = plan.n_probe;
+        const int stream_max = plan.qbatched[(size_t)b] ? 192 : 64;
+        int n = (int)std::min<long long>(p.n_ivf_probe, ix->K);
         uint8_t k = n > stream_max ? PROBE_BIG : PROBE_TABLE;
-        if (elig && r >= 0) {
+        if (query_empty(plan, b)) k = PROBE_NONE, n = 0;
+        else if (!plan.qbatched[(size_t)b] && r >= 0) {
             const unsigned long long n_elig = ne[(size_t)r];
             const unsigned long long len = (unsigned long long)(io.shared_sub ? io.n_shared : io.sub_off[b + 1] - io.sub_off[b]);
             // n_ivf_probe scaled by D / |subset| (raw length, duplicates and out-of-range ids counted)
-            unsigned long long scaled = len > 0 ? (unsigned long long)p->n_ivf_probe * (unsigned long long)plan.D_total / len
-                                                : (unsigned long long)p->n_ivf_probe;
-            scaled = std::max<unsigned long long>(scaled, (unsigned long long)p->n_ivf_probe);
+            unsigned long long scaled = len > 0 ? (unsigned long long)p.n_ivf_probe * (unsigned long long)plan.D_total / len
+                                                : (unsigned long long)p.n_ivf_probe;
+            scaled = std::max<unsigned long long>(scaled, (unsigned long long)p.n_ivf_probe);
             scaled = std::min<unsigned long long>(scaled, n_elig);
             if (n_elig == 0) k = PROBE_NONE, n = 0;  // every per-token pool is empty -> no cells
             else if (scaled >= n_elig) k = PROBE_ALL, n = (int)n_elig;
@@ -1774,33 +1826,50 @@ static pb_status plan_probe(pb_index *ix, Workspace &ws, const pb_search_params 
     }
     g_search_agreed = false;
 
-    // ---- passes: the queries of each kind in input order, in equal sub-batches of at most QB; a streaming pass also
-    // keeps its widest query row x its largest n within 8192 ----
+    // ---- passes: the queries of each pass key in input order, in equal sub-batches of at most QB; a streaming pass
+    // also keeps its widest query row x its largest n within 8192.  The key is (probe kind, variant, slab width,
+    // whether the query's own n admits the tensor-core table): the batched threshold rule depends on the slab width,
+    // and a query whose n rules out the table path must not pull the others of its pass off it ----
+    std::vector<uint8_t> tc_ok((size_t)Bt, 0);
+    for (int64_t b = 0; b < Bt; ++b) {
+        if (plan.kind[(size_t)b] != PROBE_TABLE) continue;
+        int n_chunks = 0;
+        const int n = plan.qn[(size_t)b];
+        probe_chunk_rows(ix->K, n, &n_chunks);
+        tc_ok[(size_t)b] = n_chunks >= n && n <= 192;
+    }
+    const auto same_key = [&](int64_t a, int64_t b) {
+        return plan.kind[(size_t)a] == plan.kind[(size_t)b] && plan.qbatched[(size_t)a] == plan.qbatched[(size_t)b] &&
+               plan.qslab[(size_t)a] == plan.qslab[(size_t)b] && tc_ok[(size_t)a] == tc_ok[(size_t)b];
+    };
+    std::vector<uint8_t> placed((size_t)Bt, 0);
     for (uint8_t k = PROBE_TABLE; k < PROBE_NONE; ++k) {
-        std::vector<int64_t> run;
-        for (int64_t b = 0; b < Bt; ++b)
-            if (plan.kind[(size_t)b] == k) run.push_back(b);
-        if (run.empty()) continue;
-        const int64_t L = (int64_t)run.size();
-        const int64_t per = (L + (L + QB - 1) / QB - 1) / ((L + QB - 1) / QB);  // equal sub-batches
-        int64_t at = (int64_t)plan.order.size();
-        int cur = 0, qs_max = 0, n_max = 0;
-        for (int64_t b : run) {
-            const int QS = query_row_tokens((int)(io.q_off[b + 1] - io.q_off[b]));
-            const int qs2 = std::max(qs_max, QS), n2 = std::max(n_max, plan.qn[(size_t)b]);
-            const bool wide = (k == PROBE_TABLE || k == PROBE_STREAM) && (long long)qs2 * n2 > 8192;
-            if (cur > 0 && (cur == per || wide)) {
-                plan.passes.emplace_back(at, cur);
-                at += cur;
-                cur = 0;
-                qs_max = n_max = 0;
+        for (int64_t first = 0; first < Bt; ++first) {
+            if (placed[(size_t)first] || plan.kind[(size_t)first] != k) continue;
+            std::vector<int64_t> run;
+            for (int64_t b = first; b < Bt; ++b)
+                if (!placed[(size_t)b] && same_key(first, b)) run.push_back(b), placed[(size_t)b] = 1;
+            const int64_t L = (int64_t)run.size();
+            const int64_t per = (L + (L + QB - 1) / QB - 1) / ((L + QB - 1) / QB);  // equal sub-batches
+            int64_t at = (int64_t)plan.order.size();
+            int cur = 0, qs_max = 0, n_max = 0;
+            for (int64_t b : run) {
+                const int QS = query_row_tokens((int)(io.q_off[b + 1] - io.q_off[b]));
+                const int qs2 = std::max(qs_max, QS), n2 = std::max(n_max, plan.qn[(size_t)b]);
+                const bool wide = (k == PROBE_TABLE || k == PROBE_STREAM) && (long long)qs2 * n2 > 8192;
+                if (cur > 0 && (cur == per || wide)) {
+                    plan.passes.emplace_back(at, cur);
+                    at += cur;
+                    cur = 0;
+                    qs_max = n_max = 0;
+                }
+                qs_max = std::max(qs_max, QS);
+                n_max = std::max(n_max, plan.qn[(size_t)b]);
+                plan.order.push_back(b);
+                ++cur;
             }
-            qs_max = std::max(qs_max, QS);
-            n_max = std::max(n_max, plan.qn[(size_t)b]);
-            plan.order.push_back(b);
-            ++cur;
+            plan.passes.emplace_back(at, cur);
         }
-        plan.passes.emplace_back(at, cur);
     }
     return PB_OK;
 }
@@ -1811,20 +1880,27 @@ struct HostCounts {
     unsigned long long *cnt;  // [B + 4] ws.counters
     long long *surv_tok;      // [B] tokens of the filter's survivors
     int *cells, *cand, *kept, *surv, *recheck, *pairs, *need;  // [B] each
-    int *qrow, *qn;           // [B] each, up: the queries' subset rows and n_ivf_probe (Pass::rows)
+    // [B] each, up in one copy: the queries' subset rows and n_ivf_probe (Pass::rows), then their M, M1, top_k and
+    // threshold (Pass::mixed)
+    int *qrow, *qn, *qM, *qM1, *qtopk, *qhas;
+    float *qthr;
     int *fell;                // the threshold-first probe's fallback flag
 };
+enum { HC_UP_WORDS = 7 };  // the per-query words from qrow to qthr
 static pb_status map_host_counts(HostBuf &hb, int B, HostCounts &h) {
     const size_t at_cnt = ((size_t)(B + 1) * 4 + 15) & ~(size_t)15, at_tok = at_cnt + (size_t)(B + 4) * 8,
                  at_int = at_tok + (size_t)B * 8;
-    CKS(hb.ensure(at_int + ((size_t)9 * B + 1) * 4));
+    CKS(hb.ensure(at_int + ((size_t)14 * B + 1) * 4));
     char *base = hb.as<char>();
     h.qoff = reinterpret_cast<int *>(base);
     h.cnt = reinterpret_cast<unsigned long long *>(base + at_cnt);
     h.surv_tok = reinterpret_cast<long long *>(base + at_tok);
     int *c = reinterpret_cast<int *>(base + at_int);
-    for (int **f : {&h.cells, &h.cand, &h.kept, &h.surv, &h.recheck, &h.pairs, &h.need, &h.qrow, &h.qn, &h.fell})
+    for (int **f : {&h.cells, &h.cand, &h.kept, &h.surv, &h.recheck, &h.pairs, &h.need, &h.qrow, &h.qn, &h.qM, &h.qM1,
+                    &h.qtopk, &h.qhas})
         *f = c, c += B;
+    h.qthr = reinterpret_cast<float *>(c), c += B;
+    h.fell = c;
     return PB_OK;
 }
 
@@ -1839,6 +1915,16 @@ struct Pass {
     int n = 0;
     bool rows = false;
     const int *d_qrow = nullptr, *d_qn = nullptr;
+    // the search parameters: the variant and slab width are the pass's (its key); M, M1, top_k and the threshold are
+    // its first query's, and with `mixed` (its queries differ in them) each query's on the device (d_qM ...)
+    bool batched = false;
+    long long slab = 0;
+    int M = 0, M1 = 0, top_k = 0, has_thr = 0;
+    float thr = 0.0f;
+    bool mixed = false;
+    bool some_top_k_below_M = false;  // the certified filter has something to drop
+    const int *d_qM = nullptr, *d_qM1 = nullptr, *d_qtopk = nullptr, *d_qhas = nullptr;
+    const float *d_qthr = nullptr;
     // use_tc: a2 + a3 on the tensor cores.  A flagged query or a probe-list overflow raises a device flag instead of
     // being read back mid-way; the pass then finishes on (memory-safe) garbage and is redone on the exact path.
     bool use_tc = false;
@@ -1884,23 +1970,32 @@ static pb_status upload_queries(pb_index *ix, Workspace &ws, const SearchIO &io,
         }
     }
     CK(cudaMemcpyAsync(ws.qoff.p, pass.hc.qoff, (size_t)(B + 1) * 4, cudaMemcpyHostToDevice, ws.stream));
-    if (pass.rows) {
+    if (pass.rows || pass.mixed) {
         for (int b = 0; b < B; ++b) {
-            pass.hc.qrow[b] = plan.qrow[(size_t)pass.q[b]];
-            pass.hc.qn[b] = plan.qn[(size_t)pass.q[b]];
+            const size_t g = (size_t)pass.q[b];
+            pass.hc.qrow[b] = plan.qrow[g];
+            pass.hc.qn[b] = plan.qn[g];
+            pass.hc.qM[b] = plan.qM[g];
+            pass.hc.qM1[b] = plan.qM1[g];
+            pass.hc.qtopk[b] = plan.qtopk[g];
+            pass.hc.qhas[b] = plan.qhas[g];
+            pass.hc.qthr[b] = plan.qthr[g];
         }
-        CKS(ws.qsub.ensure((size_t)B * 8));
-        CK(cudaMemcpyAsync(ws.qsub.p, pass.hc.qrow, (size_t)B * 8, cudaMemcpyHostToDevice, ws.stream));  // qrow, qn adjacent
-        pass.d_qrow = ws.qsub.as<int>();
-        pass.d_qn = ws.qsub.as<int>() + B;
+        CKS(ws.qsub.ensure((size_t)B * HC_UP_WORDS * 4));
+        CK(cudaMemcpyAsync(ws.qsub.p, pass.hc.qrow, (size_t)B * HC_UP_WORDS * 4, cudaMemcpyHostToDevice, ws.stream));
+        const int *up = ws.qsub.as<int>();
+        if (pass.rows) pass.d_qrow = up, pass.d_qn = up + B;
+        if (pass.mixed) {
+            pass.d_qM = up + 2 * B, pass.d_qM1 = up + 3 * B, pass.d_qtopk = up + 4 * B, pass.d_qhas = up + 5 * B;
+            pass.d_qthr = ws.qsub.as<float>() + 6 * B;
+        }
     }
     return PB_OK;
 }
 
 // a2: the centroid score table, fp32 off the tensor cores and 16-bit for a fast pass or the filter; on the tensor cores
 // also a3
-static pb_status centroid_scores(pb_index *ix, Workspace &ws, const pb_search_params *p, const SearchPlan &plan,
-                                 Pass &pass) {
+static pb_status centroid_scores(pb_index *ix, Workspace &ws, Pass &pass) {
     const int B = pass.B, QS = pass.QS;
     int *L = g_stats.launches;
     if (!pass.use_tc) CKS(ws.ST.ensure((size_t)B * ix->K * QS * sizeof(float)));
@@ -1918,8 +2013,8 @@ static pb_status centroid_scores(pb_index *ix, Workspace &ws, const pb_search_pa
         L[PB_STAGE_CENTROID_SCORES] += 1;
     }
     if (pass.use_tc)
-        return run_k1_tc(ix, ws, p, B, QS, pass.nq_max, pass.n, plan.batched, L, &pass.cells_cap,
-                         &pass.d_probe_fallback);
+        return run_k1_tc(ix, ws, B, QS, pass.nq_max, pass.n, pass.d_qn, pass.has_thr, pass.thr, pass.d_qhas, pass.d_qthr,
+                         pass.batched, pass.slab, L, &pass.cells_cap, &pass.d_probe_fallback);
     CKS(launch_centroid_scores(ix, ws, B, QS, &L[PB_STAGE_CENTROID_SCORES], with16));
     // PB_K1_TC_DIAG: the tensor-core table next to the exact one, compared code by code
     if (pass.fast && ix->k1_diag && ix->cent_h16t.p) CKS(launch_k1_diag(ix, ws, B, QS));
@@ -1927,7 +2022,7 @@ static pb_status centroid_scores(pb_index *ix, Workspace &ws, const pb_search_pa
 }
 
 // a3: the cells (centroids) each query probes, on the fp32 table; the tensor-core pass placed them in a2
-static pb_status probe(pb_index *ix, Workspace &ws, const pb_search_params *p, const SearchPlan &plan, Pass &pass) {
+static pb_status probe(pb_index *ix, Workspace &ws, const SearchPlan &plan, Pass &pass) {
     if (pass.use_tc) return PB_OK;
     const int B = pass.B, QS = pass.QS;
     int *L = g_stats.launches;
@@ -1942,9 +2037,9 @@ static pb_status probe(pb_index *ix, Workspace &ws, const pb_search_params *p, c
         k_cells_from_bits<<<B, 1024, 0, ws.stream>>>(plan.d_elig, pass.d_qrow, plan.Wke, ix->K, ws.list.as<uint32_t>(),
                                                      pass.n, ws.listn.as<int>());
         k_cells_filter_list<<<B, 256, 0, ws.stream>>>(ws.list.as<uint32_t>(), pass.n, ws.listn.as<int>(), ws.ST.as<float>(),
-                                                      ws.qoff.as<int>(), ix->K, QS, p->has_centroid_score_threshold,
-                                                      p->centroid_score_threshold, pass.cells_cap, ws.cells.as<uint32_t>(),
-                                                      ws.ncells.as<int>());
+                                                      ws.qoff.as<int>(), ix->K, QS, pass.has_thr, pass.thr, pass.cells_cap,
+                                                      ws.cells.as<uint32_t>(), ws.ncells.as<int>(), pass.d_qhas,
+                                                      pass.d_qthr);
         CK(cudaGetLastError());
         L[PB_STAGE_PROBE] += 2;
         return PB_OK;
@@ -1959,9 +2054,9 @@ static pb_status probe(pb_index *ix, Workspace &ws, const pb_search_params *p, c
                                                               elig, pass.d_qrow, plan.Wke, ws.cellbits.as<uint32_t>(),
                                                               plan.Wk);
         k_cells_from_query_bits<<<B, 1024, 0, ws.stream>>>(ws.cellbits.as<uint32_t>(), plan.Wk, ws.ST.as<float>(),
-                                                           ws.qoff.as<int>(), ix->K, QS, p->has_centroid_score_threshold,
-                                                           p->centroid_score_threshold, pass.cells_cap,
-                                                           ws.cells.as<uint32_t>(), ws.ncells.as<int>());
+                                                           ws.qoff.as<int>(), ix->K, QS, pass.has_thr, pass.thr,
+                                                           pass.cells_cap, ws.cells.as<uint32_t>(), ws.ncells.as<int>(),
+                                                           pass.d_qhas, pass.d_qthr);
         CK(cudaGetLastError());
         L[PB_STAGE_PROBE] += 2;
         return PB_OK;
@@ -1983,13 +2078,13 @@ static pb_status probe(pb_index *ix, Workspace &ws, const pb_search_params *p, c
     pass.probe_list_only = !thr_path;
     if (thr_path) {
         const int cap = probe16_cap(n);
-        CKS(probe16_thresholds(ix, ws, B, QS, n, t_chunks, t_rows, &d_fallback));
+        CKS(probe16_thresholds(ix, ws, B, QS, n, t_chunks, t_rows, pass.d_qn, &d_fallback));
         pass.d_probe_fallback = d_fallback;
         k_collect16<<<dim3((t_chunks + 3) / 4, B), 128, 0, ws.stream>>>(
             ws.ST16.as<unsigned short>(), ws.ST.as<float>(), ix->K, QS, t_chunks, t_rows, ws.tau16.as<uint32_t>(), cap,
             ws.pcount.as<int>(), ws.plist.as<u64>(), d_fallback);
         k_topn_merge<<<dim3(QS, B), 32, 0, ws.stream>>>(ws.plist.as<u64>(), ws.qoff.as<int>(), QS, n, cap / n,
-                                                      ws.sel.as<u64>(), d_fallback, 0, nullptr);
+                                                      ws.sel.as<u64>(), d_fallback, 0, pass.d_qn);
         CK(cudaGetLastError());
         L[PB_STAGE_PROBE] += 4;
     }
@@ -2002,11 +2097,10 @@ static pb_status probe(pb_index *ix, Workspace &ws, const pb_search_params *p, c
     size_t sm2 = (size_t)P * 12;
     CKS(set_smem(k_cells, sm2));
     k_cells<<<B, 256, sm2, ws.stream>>>(ws.sel.as<u64>(), ws.ST.as<float>(), ws.qoff.as<int>(), ix->K, QS, n,
-                                        pass.cells_cap, p->has_centroid_score_threshold, p->centroid_score_threshold,
-                                        plan.batched ? 1 : 0, plan.batched ? (long long)p->centroid_batch_size : ix->K,
+                                        pass.cells_cap, pass.has_thr, pass.thr, pass.batched ? 1 : 0, pass.slab,
                                         ws.cells.as<uint32_t>(), ws.ncells.as<int>(),
                                         thr_path ? ws.cmax16.as<unsigned short>() : nullptr, t_chunks, t_rows,
-                                        ws.qrange.as<float2>(), d_fallback);
+                                        ws.qrange.as<float2>(), d_fallback, pass.d_qn, pass.d_qhas, pass.d_qthr);
     CK(cudaGetLastError());
     L[PB_STAGE_PROBE] += 3;
     return PB_OK;
@@ -2069,7 +2163,7 @@ static pb_status approx_scores(pb_index *ix, Workspace &ws, const SearchPlan &pl
             CKS(ws.a5n12.ensure((size_t)B * 4 + 16));
             CKS(ws.a5theta.ensure((size_t)B * 4 + 16));
             const long long n_live = ix->a5_live >= 0 ? ix->a5_live : ix->K / 512;
-            const int M1 = (int)std::min<double>(ceil((double)ix->a5_m1 * plan.M), (double)INT_MAX);
+            const int M1 = pass.M1;
             uint32_t *ub = ws.approx.as<uint32_t>(), *rl = ws.keys.as<uint32_t>();
             int *n1 = ws.a5n1.as<int>(), *n12 = ws.a5n12.as<int>();
             k_a5_floor<<<dim3(QS / 8, B), 256, 0, ws.stream>>>(st16, ws.qoff.as<int>(), ix->K, QS, n_live,
@@ -2087,13 +2181,14 @@ static pb_status approx_scores(pb_index *ix, Workspace &ws, const SearchPlan &pl
                 st16, ws.qoff.as<int>(), ix->K, QS, ix->ucodes.as<uint32_t>(), ix->udoc_off.as<long long>(), list, ix->D,
                 list_n, ws.a5floor.as<uint32_t>(), ws.a5live.as<uint32_t>(), bits_in_smem, ub, cnt, cnt + B + 2);
             k_select_u32<<<B, 1024, 0, ws.stream>>>(ub, list_n, M1, 0, ub, list, list_n, ix->D, ws.qoff.as<int>(),
-                                                    ws.qflag.as<int>(), rl, n1, ws.a5theta.as<uint32_t>());
+                                                    ws.qflag.as<int>(), rl, n1, ws.a5theta.as<uint32_t>(), nullptr,
+                                                    nullptr, nullptr, pass.d_qM1);
             approx16<<<ga, 256, 0, ws.stream>>>(st16, ws.qoff.as<int>(), ix->K, QS, ix->ucodes.as<uint32_t>(),
                                                 ix->udoc_off.as<long long>(), rl, ix->D, n1, nullptr,
                                                 ws.lsum.as<uint32_t>(), nullptr);
-            k_select_u32<<<B, 1024, 0, ws.stream>>>(ws.lsum.as<uint32_t>(), n1, plan.M, band_per_q, ub, list, list_n,
+            k_select_u32<<<B, 1024, 0, ws.stream>>>(ws.lsum.as<uint32_t>(), n1, pass.M, band_per_q, ub, list, list_n,
                                                     ix->D, ws.qoff.as<int>(), ws.qflag.as<int>(), rl, n12, nullptr,
-                                                    ws.a5theta.as<uint32_t>(), n1, cnt + B + 3);
+                                                    ws.a5theta.as<uint32_t>(), n1, cnt + B + 3, pass.d_qM);
             approx16<<<ga, 256, 0, ws.stream>>>(st16, ws.qoff.as<int>(), ix->K, QS, ix->ucodes.as<uint32_t>(),
                                                 ix->udoc_off.as<long long>(), rl, ix->D, n12, n1,
                                                 ws.lsum.as<uint32_t>(), nullptr);
@@ -2107,9 +2202,10 @@ static pb_status approx_scores(pb_index *ix, Workspace &ws, const SearchPlan &pl
             L[PB_STAGE_APPROX] += 1;
         }
         KEV_END(PB_KERNEL_APPROX16);
-        k_select_u32<<<B, 1024, 0, ws.stream>>>(ws.lsum.as<uint32_t>(), list_n, plan.M, band_per_q, ws.lsum.as<uint32_t>(),
+        k_select_u32<<<B, 1024, 0, ws.stream>>>(ws.lsum.as<uint32_t>(), list_n, pass.M, band_per_q, ws.lsum.as<uint32_t>(),
                                                 list, list_n, ix->D, ws.qoff.as<int>(), ws.qflag.as<int>(),
-                                                ws.cand2.as<uint32_t>(), ws.ncand2.as<int>());
+                                                ws.cand2.as<uint32_t>(), ws.ncand2.as<int>(), nullptr, nullptr, nullptr,
+                                                nullptr, pass.d_qM);
         CK(cudaGetLastError());
         L[PB_STAGE_APPROX] += 1;
     }
@@ -2148,7 +2244,7 @@ static pb_status approx_scores(pb_index *ix, Workspace &ws, const SearchPlan &pl
 
 // a6: the top M by approximate score; doc-sharded, exchange 1 makes it the global cut
 static pb_status cut(pb_index *ix, Workspace &ws, const SearchPlan &plan, const Pass &pass) {
-    const int B = pass.B, M = plan.M, Mcap = plan.Mcap;
+    const int B = pass.B, Mcap = plan.Mcap;
     const bool sharded = plan.sharded;
     CKS(ws.kept.ensure((size_t)B * Mcap * 4));
     CKS(ws.nkept.ensure((size_t)B * 4 + 16));
@@ -2156,23 +2252,24 @@ static pb_status cut(pb_index *ix, Workspace &ws, const SearchPlan &plan, const 
     if (sharded) CKS(ws.lkeys.ensure((size_t)B * Mcap * 8));
     const int Pm = pow2_at_least(Mcap);
     CKS(set_smem(k_cut, (size_t)Pm * 8));
-    k_cut<<<B, 1024, (size_t)Pm * 8, ws.stream>>>(ws.keys.as<u64>(), ws.approx.as<float>(), ix->D, pass.cand_n, M,
+    k_cut<<<B, 1024, (size_t)Pm * 8, ws.stream>>>(ws.keys.as<u64>(), ws.approx.as<float>(), ix->D, pass.cand_n, pass.M,
                                                   Mcap, ix->doc_off.as<long long>(), ws.kept.as<uint32_t>(),
                                                   ws.nkept.as<int>(), ws.tokp.as<long long>(),
                                                   ws.counters.as<long long>() + 1, (uint32_t)ix->doc_id_base,
-                                                  sharded ? ws.lkeys.as<u64>() : nullptr);
+                                                  sharded ? ws.lkeys.as<u64>() : nullptr, pass.d_qM);
     CK(cudaGetLastError());
     g_stats.launches[PB_STAGE_CUT] += 1;
     if (sharded) {
-        // exchange 1: every shard's sorted top-M cut keys -> global cut -> my members (SURVEY 8e)
+        // exchange 1: every shard's sorted top-M cut keys (Mcap per query, ~0 past its M) -> global cut -> my members
+        // (SURVEY 8e)
         const int G = ix->world;
-        CKS(ws.gkeys.ensure((size_t)G * B * M * 8));
+        CKS(ws.gkeys.ensure((size_t)G * B * Mcap * 8));
         CKS(ws.krank.ensure((size_t)B * Mcap * 4));
-        CKS(shard_allgather(ix, ws.stream, ws.lkeys.p, ws.gkeys.p, (size_t)B * M));
-        k_merge_cut<<<B, 1024, 0, ws.stream>>>(ws.gkeys.as<u64>(), G, ix->rank, B, M, (uint32_t)ix->doc_id_base, ix->D,
-                                               ix->doc_off.as<long long>(), ws.kept.as<uint32_t>(),
+        CKS(shard_allgather(ix, ws.stream, ws.lkeys.p, ws.gkeys.p, (size_t)B * Mcap));
+        k_merge_cut<<<B, 1024, 0, ws.stream>>>(ws.gkeys.as<u64>(), G, ix->rank, B, pass.M, Mcap, (uint32_t)ix->doc_id_base,
+                                               ix->D, ix->doc_off.as<long long>(), ws.kept.as<uint32_t>(),
                                                ws.krank.as<uint32_t>(), ws.nkept.as<int>(),
-                                               ws.tokp.as<long long>(), ws.counters.as<long long>() + 1);
+                                               ws.tokp.as<long long>(), ws.counters.as<long long>() + 1, pass.d_qM);
         CK(cudaGetLastError());
         g_stats.launches[PB_STAGE_CUT] += 2;
     }
@@ -2264,7 +2361,7 @@ static pb_status exact_scores(pb_index *ix, Workspace &ws, const SearchPlan &pla
             CKS(ws.estkey.ensure((size_t)B * Mcap * QS * 4));
             CKS(ws.srcrank.ensure((size_t)B * Mcap * 4));
         }
-        CKS(launch_filter(ix, ws, kv, kv2, tv, B, QS, Mcap, plan.top_k, max_tokens, eps_unit, nq_max,
+        CKS(launch_filter(ix, ws, kv, kv2, tv, B, QS, Mcap, pass.top_k, pass.d_qtopk, max_tokens, eps_unit, nq_max,
                           pass.pairs || pass.diag, &L[PB_STAGE_EXACT]));
         if (!pass.diag) {
             kv = kv2;
@@ -2330,14 +2427,16 @@ static pb_status exact_scores(pb_index *ix, Workspace &ws, const SearchPlan &pla
 // a9: the top_k by exact score, into the caller's device outputs or the workspace's; doc-sharded, exchange 2 merges
 // every shard's
 static pb_status select_topk(pb_index *ix, Workspace &ws, const SearchIO &io, const SearchPlan &plan, Pass &pass) {
-    const int B = pass.B, M = plan.M, top_k = plan.top_k, Mcap = plan.Mcap;
+    // rows of the outputs: the caller's stride on the device, the call's largest top_k in the workspace
+    const int B = pass.B, Mcap = plan.Mcap;
+    const int ostride = io.out_on_device ? (int)io.out_stride : plan.top_k_max;
     if (io.out_on_device) {  // no subsets: the queries of a pass are consecutive
-        pass.d_ids = reinterpret_cast<long long *>(io.out_ids) + (size_t)pass.q[0] * top_k;
-        pass.d_sc = io.out_scores + (size_t)pass.q[0] * top_k;
+        pass.d_ids = reinterpret_cast<long long *>(io.out_ids) + (size_t)pass.q[0] * ostride;
+        pass.d_sc = io.out_scores + (size_t)pass.q[0] * ostride;
         pass.d_cn = io.out_counts + pass.q[0];
     } else {
-        CKS(ws.oids.ensure((size_t)B * top_k * 8));
-        CKS(ws.oscores.ensure((size_t)B * top_k * 4));
+        CKS(ws.oids.ensure((size_t)B * ostride * 8));
+        CKS(ws.oscores.ensure((size_t)B * ostride * 4));
         CKS(ws.ocounts.ensure((size_t)B * 4 + 16));
         pass.d_ids = ws.oids.as<long long>();
         pass.d_sc = ws.oscores.as<float>();
@@ -2347,21 +2446,22 @@ static pb_status select_topk(pb_index *ix, Workspace &ws, const SearchIO &io, co
     if (plan.sharded) {
         // exchange 2: (exact key | global approx rank) + (doc id | score) of every shard, merged on every rank
         const int G = ix->world;
-        CKS(ws.gfkeys.ensure((size_t)G * B * M * 8));
-        CKS(ws.gpayload.ensure((size_t)G * B * M * 8));
-        CKS(shard_allgather(ix, ws.stream, ws.fkeys.p, ws.gfkeys.p, (size_t)B * M));
-        CKS(shard_allgather(ix, ws.stream, ws.payload.p, ws.gpayload.p, (size_t)B * M));
+        CKS(ws.gfkeys.ensure((size_t)G * B * Mcap * 8));
+        CKS(ws.gpayload.ensure((size_t)G * B * Mcap * 8));
+        CKS(shard_allgather(ix, ws.stream, ws.fkeys.p, ws.gfkeys.p, (size_t)B * Mcap));
+        CKS(shard_allgather(ix, ws.stream, ws.payload.p, ws.gpayload.p, (size_t)B * Mcap));
         CKS(ws.mslot.ensure((size_t)B * Mcap * 4));
         CKS(set_smem(k_merge_topk, (size_t)Pm * 8));
-        k_merge_topk<<<B, 1024, (size_t)Pm * 8, ws.stream>>>(ws.gfkeys.as<u64>(), ws.gpayload.as<u64>(), G, B, M, top_k,
-                                                            ws.mslot.as<uint32_t>(), pass.d_ids, pass.d_sc, pass.d_cn);
+        k_merge_topk<<<B, 1024, (size_t)Pm * 8, ws.stream>>>(ws.gfkeys.as<u64>(), ws.gpayload.as<u64>(), G, B, Mcap,
+                                                            pass.top_k, ws.mslot.as<uint32_t>(), pass.d_ids, pass.d_sc,
+                                                            pass.d_cn, pass.d_qtopk, ostride);
         CK(cudaGetLastError());
         g_stats.launches[PB_STAGE_TOPK] += 3;
     } else {
         CKS(set_smem(k_topk, (size_t)Pm * 8));
         k_topk<<<B, 1024, (size_t)Pm * 8, ws.stream>>>(ws.fkeys.as<u64>(), ws.exact.as<float>(), pass.kv.kept,
-                                                       pass.kv.nkept, Mcap, top_k, ix->doc_id_base, pass.d_ids,
-                                                       pass.d_sc, pass.d_cn);
+                                                       pass.kv.nkept, Mcap, pass.top_k, ix->doc_id_base, pass.d_ids,
+                                                       pass.d_sc, pass.d_cn, pass.d_qtopk, ostride);
         CK(cudaGetLastError());
         g_stats.launches[PB_STAGE_TOPK] += 1;
     }
@@ -2372,7 +2472,7 @@ static pb_status select_topk(pb_index *ix, Workspace &ws, const SearchIO &io, co
 // launches stay counted, its stage times are not added.  Otherwise the results go out and the pass is accounted.
 static pb_status finish(pb_index *ix, Workspace &ws, const SearchIO &io, const SearchPlan &plan, const Pass &pass,
                         bool *redo) {
-    const int B = pass.B, top_k = plan.top_k;
+    const int B = pass.B, top_k = plan.top_k_max;  // the workspace's row stride (select_topk)
     const HostCounts &hc = pass.hc;
     *hc.fell = 0;
     CK(cudaMemcpyAsync(hc.cells, ws.ncells.p, (size_t)B * 4, cudaMemcpyDeviceToHost, ws.stream));
@@ -2407,8 +2507,9 @@ static pb_status finish(pb_index *ix, Workspace &ws, const SearchIO &io, const S
         const char *h = ws.hres.as<char>();
         for (int b = 0; b < B; ++b) {
             const int64_t g = pass.q[b];
-            memcpy(io.out_ids + (size_t)g * top_k, h + (size_t)b * top_k * 8, (size_t)top_k * 8);
-            memcpy(io.out_scores + (size_t)g * top_k, h + (size_t)B * top_k * 8 + (size_t)b * top_k * 4, (size_t)top_k * 4);
+            const size_t kq = (size_t)plan.qtopk[(size_t)g], os = (size_t)io.out_stride;
+            memcpy(io.out_ids + (size_t)g * os, h + (size_t)b * top_k * 8, kq * 8);
+            memcpy(io.out_scores + (size_t)g * os, h + (size_t)B * top_k * 8 + (size_t)b * top_k * 4, kq * 4);
             memcpy(io.out_counts + g, h + (size_t)B * top_k * 12 + (size_t)b * 4, 4);
         }
     }
@@ -2522,16 +2623,16 @@ static pb_status dump_trace(pb_index *ix, Workspace &ws, const SearchIO &io, con
 
 // One pass of the pipeline over a sub-batch, stage by stage, with the stage events between them.  *redo: the
 // tensor-core pass gave up on the device and nothing of it went out.  `pass` is a copy, so a redo starts clean.
-static pb_status run_pass(pb_index *ix, Workspace &ws, const pb_search_params *p, const SearchIO &io,
-                          const SearchPlan &plan, Pass pass, bool *redo) {
+static pb_status run_pass(pb_index *ix, Workspace &ws, const SearchIO &io, const SearchPlan &plan, Pass pass,
+                          bool *redo) {
     *redo = false;
     const auto mark = [&](int s) { return plan.prof ? cudaEventRecord(ws.ev[s], ws.stream) : cudaSuccess; };
     CK(mark(0));
     CKS(upload_queries(ix, ws, io, plan, pass));
     CK(mark(1));
-    CKS(centroid_scores(ix, ws, p, plan, pass));
+    CKS(centroid_scores(ix, ws, pass));
     CK(mark(2));
-    CKS(probe(ix, ws, p, plan, pass));
+    CKS(probe(ix, ws, plan, pass));
     CK(mark(3));
     CKS(candidates(ix, ws, plan, pass));
     CK(mark(4));
@@ -2550,15 +2651,16 @@ static pb_status run_pass(pb_index *ix, Workspace &ws, const pb_search_params *p
 
 // a7': whether the certified filter runs on a pass; a2 then makes the pass's 16-bit table, which the estimate reads.
 // The certificate depends on the table's code error, so a tensor-core pass redone on the exact path decides again.
-static bool filter_runs(const pb_index *ix, const SearchIO &io, const SearchPlan &plan, const Pass &pass) {
+// It runs when some query of the pass has top_k < M; a query whose top_k reaches its kept count keeps every kept doc.
+static bool filter_runs(const pb_index *ix, const SearchIO &io, const Pass &pass) {
     return ix->fast_exact && !io.trace && ix->tok_inv_norm.p && filter_eps_unit2(ix, pass.use_tc ? ix->k1_margin : 0) > 0.0f &&
-           pass.nq_max <= 64 && plan.top_k < plan.Mcap && ix->packed % 4 == 0;
+           pass.nq_max <= 64 && pass.some_top_k_below_M && ix->packed % 4 == 0;
 }
 
 // One search call (or one lane of it): the plan, the workspace, then the sub-batches in order
-static pb_status run_search(pb_index *ix, const pb_search_params *p, const SearchIO &io) {
+static pb_status run_search(pb_index *ix, const SearchIO &io) {
     SearchPlan plan;
-    CKS(plan_search(ix, p, io, plan));
+    CKS(plan_search(ix, io, plan));
     if (plan.Bt == 0) return PB_OK;
 
     std::unique_ptr<Workspace> wsp;
@@ -2580,7 +2682,7 @@ static pb_status run_search(pb_index *ix, const pb_search_params *p, const Searc
         }
     } rel{ix, wsp};
 
-    if (!plan.empty) CKS(plan_probe(ix, ws, p, io, plan));
+    if (!plan.empty) CKS(plan_probe(ix, ws, io, plan));
     // empty results: the whole call, or the queries with nothing eligible (they get no pass)
     for (int64_t b = 0; b < plan.Bt; ++b) {
         if (!plan.empty && plan.kind[(size_t)b] != PROBE_NONE) continue;
@@ -2610,7 +2712,20 @@ static pb_status run_search(pb_index *ix, const pb_search_params *p, const Searc
             pass.n = std::max(pass.n, plan.qn[(size_t)g]);
             pass.rows = pass.rows || plan.qrow[(size_t)g] >= 0;
         }
-        pass.kind = plan.kind[(size_t)pass.q[0]];
+        const size_t g0 = (size_t)pass.q[0];
+        pass.kind = plan.kind[g0];
+        pass.batched = plan.qbatched[g0] != 0;
+        pass.slab = plan.qslab[g0];
+        pass.M = plan.qM[g0], pass.M1 = plan.qM1[g0], pass.top_k = plan.qtopk[g0], pass.has_thr = plan.qhas[g0];
+        pass.thr = plan.qthr[g0];
+        for (int b = 0; b < pass.B; ++b) {
+            const size_t g = (size_t)pass.q[b];
+            pass.rows = pass.rows || plan.qn[g] != pass.n;  // queries of their own n
+            pass.mixed = pass.mixed || plan.qM[g] != pass.M || plan.qM1[g] != pass.M1 || plan.qtopk[g] != pass.top_k ||
+                         plan.qhas[g] != pass.has_thr ||
+                         (pass.has_thr && __builtin_memcmp(&plan.qthr[g], &pass.thr, 4) != 0);
+            pass.some_top_k_below_M = pass.some_top_k_below_M || plan.qtopk[g] < plan.qM[g];
+        }
         pass.rows = pass.rows || pass.kind != PROBE_TABLE;
         pass.QS = query_row_tokens(pass.nq_max);
         pass.fast = ix->fast_approx && !io.trace;  // trace wants every candidate's exact approx score
@@ -2621,15 +2736,15 @@ static pb_status run_search(pb_index *ix, const pb_search_params *p, const Searc
         probe_chunk_rows(ix->K, pass.n, &n_chunks_k);
         pass.use_tc = k1_tc_usable(ix) && pass.fast && ix->probe16 && !ix->k1_diag && pass.kind == PROBE_TABLE &&
                       pass.QS / 8 <= 32 && n_chunks_k >= pass.n && pass.n <= 192;
-        pass.filt = filter_runs(ix, io, plan, pass);
+        pass.filt = filter_runs(ix, io, pass);
         bool redo = false;
-        CKS(run_pass(ix, ws, p, io, plan, pass, &redo));
+        CKS(run_pass(ix, ws, io, plan, pass, &redo));
         if (redo) {
             g_stats.work.n_k1_tc_redo += 1;
             pass.use_tc = false;
             pass.prune = false;
-            pass.filt = filter_runs(ix, io, plan, pass);
-            CKS(run_pass(ix, ws, p, io, plan, pass, &redo));
+            pass.filt = filter_runs(ix, io, pass);
+            CKS(run_pass(ix, ws, io, plan, pass, &redo));
         }
     }
     if (plan.prof) {
@@ -2666,7 +2781,7 @@ struct LaneClock {
 };
 static thread_local LaneClock g_lane_clock;
 
-static pb_status search_impl(pb_index *ix, const pb_search_params *p, const SearchIO &io) {
+static pb_status search_impl(pb_index *ix, const SearchIO &io) {
     // the lanes' helper threads run under this caller's lock (they must not take it themselves: a waiting append
     // would block them while this thread waits for them)
     std::shared_lock<std::shared_mutex> rd;
@@ -2676,7 +2791,7 @@ static pb_status search_impl(pb_index *ix, const pb_search_params *p, const Sear
     // through the whole pipeline on its own workspace and stream (helper threads do the launching).  Not with a trace
     // (per-stage dumps), not doc-sharded (the exchanges are collective calls in batch order), not for small batches.
     int lanes = 1;
-    if (ix && p && ix->lanes > 1 && !io.trace && ix->world == 1 && io.n_queries >= 16)
+    if (ix && io.qp && ix->lanes > 1 && !io.trace && ix->world == 1 && io.n_queries >= 16)
         lanes = (int)std::min<int64_t>(ix->lanes, io.n_queries / 8);
     std::unique_lock<std::mutex> lane_lock;
     if (lanes > 1) {
@@ -2684,7 +2799,7 @@ static pb_status search_impl(pb_index *ix, const pb_search_params *p, const Sear
         if (!lane_lock.owns_lock()) lanes = 1;  // another host thread is using the helpers: it already provides the overlap
     }
     if (lanes <= 1) {
-        const pb_status st = run_search(ix, p, io);
+        const pb_status st = run_search(ix, io);
         // the peers must not wait for a rank that gave up; a refusal every rank reached together leaves the group usable
         if (st != PB_OK && ix && ix->group && !g_search_agreed) ix->group->fail();
         return st;
@@ -2706,20 +2821,21 @@ static pb_status search_impl(pb_index *ix, const pb_search_params *p, const Sear
     std::vector<pb_status> sts(lanes, PB_OK);
     std::vector<Stats> stats(lanes);
     std::vector<std::string> errs(lanes);
-    const int64_t Bt = io.n_queries, top_k = p->top_k;
+    const int64_t Bt = io.n_queries, top_k = io.out_stride;
     for (int l = 0; l < lanes; ++l) {
         const int64_t b0 = Bt * l / lanes, b1 = Bt * (l + 1) / lanes;
         ios[l].q_off = io.q_off + b0;
         if (io.sub_off) ios[l].sub_off = io.sub_off + b0;  // the offsets stay absolute into sub_ids
         if (io.has_sub) ios[l].has_sub = io.has_sub + b0;
         ios[l].n_queries = b1 - b0;
+        ios[l].qp = io.qp + b0 * io.qp_stride;
         if (io.out_ids) ios[l].out_ids = io.out_ids + b0 * top_k;
         if (io.out_scores) ios[l].out_scores = io.out_scores + b0 * top_k;
         ios[l].out_counts = io.out_counts ? io.out_counts + b0 : nullptr;
     }
     auto run_lane = [&](int l) {
         g_budget_div = lanes;
-        sts[l] = run_search(ix, p, ios[l]);
+        sts[l] = run_search(ix, ios[l]);
         g_budget_div = 1;
         stats[l] = g_stats;
         if (sts[l] != PB_OK) errs[l] = g_err;
@@ -2751,15 +2867,16 @@ extern "C" pb_status pb_search_batch_traced(pb_index *ix, const float *queries, 
                                             pb_trace *trace) {
     if (subset && n_subset < 0) return pb_fail(PB_ERR_INVALID, "n_subset < 0");
     SearchIO io{queries, false, q_tok_offsets, n_queries, subset, nullptr, nullptr, subset ? n_subset : 0,
-                subset != nullptr, out_ids, out_scores, out_counts, false, trace};
-    return search_impl(ix, params, io);
+                subset != nullptr, out_ids, out_scores, out_counts, false, trace,
+                params, 0, params ? params->top_k : 0};
+    return search_impl(ix, io);
 }
 
-extern "C" pb_status pb_search_batch_subsets(pb_index *ix, const float *queries, const int64_t *q_tok_offsets,
-                                             int64_t n_queries, const pb_search_params *params,
-                                             const int64_t *subset_offsets, const int64_t *subset_ids,
-                                             const uint8_t *has_subset, int64_t *out_ids, float *out_scores,
-                                             int32_t *out_counts, pb_trace *trace) {
+// pb_search_batch_subsets and pb_search_batch_params: params[b * params_stride] are query b's parameters
+static pb_status search_subsets(pb_index *ix, const float *queries, const int64_t *q_tok_offsets, int64_t n_queries,
+                                const pb_search_params *params, int64_t params_stride, const int64_t *subset_offsets,
+                                const int64_t *subset_ids, const uint8_t *has_subset, int64_t *out_ids,
+                                float *out_scores, int32_t *out_counts, pb_trace *trace) {
     // the subset arguments, checked whole before any lane takes its slice
     if (n_queries < 0) return pb_fail(PB_ERR_INVALID, "n_queries < 0");
     if (subset_offsets) {
@@ -2769,9 +2886,32 @@ extern "C" pb_status pb_search_batch_subsets(pb_index *ix, const float *queries,
         if (n_queries > 0 && subset_offsets[n_queries] > 0 && !subset_ids)
             return pb_fail(PB_ERR_INVALID, "null subset_ids");
     }
+    int64_t out_stride = 0;  // the call's largest top_k (negative ones are refused in plan_search)
+    if (params)
+        for (int64_t b = 0; b < (params_stride ? n_queries : 1); ++b)
+            out_stride = std::max<int64_t>(out_stride, params[b * params_stride].top_k);
     SearchIO io{queries, false, q_tok_offsets, n_queries, subset_ids, subset_offsets, has_subset, 0, false,
-                out_ids, out_scores, out_counts, false, trace};
-    return search_impl(ix, params, io);
+                out_ids, out_scores, out_counts, false, trace, params, params_stride, out_stride};
+    return search_impl(ix, io);
+}
+
+extern "C" pb_status pb_search_batch_subsets(pb_index *ix, const float *queries, const int64_t *q_tok_offsets,
+                                             int64_t n_queries, const pb_search_params *params,
+                                             const int64_t *subset_offsets, const int64_t *subset_ids,
+                                             const uint8_t *has_subset, int64_t *out_ids, float *out_scores,
+                                             int32_t *out_counts, pb_trace *trace) {
+    return search_subsets(ix, queries, q_tok_offsets, n_queries, params, 0, subset_offsets, subset_ids, has_subset,
+                          out_ids, out_scores, out_counts, trace);
+}
+
+extern "C" pb_status pb_search_batch_params(pb_index *ix, const float *queries, const int64_t *q_tok_offsets,
+                                            int64_t n_queries, const pb_search_params *params,
+                                            const int64_t *subset_offsets, const int64_t *subset_ids,
+                                            const uint8_t *has_subset, int64_t *out_ids, float *out_scores,
+                                            int32_t *out_counts, pb_trace *trace) {
+    if (!params) return pb_fail(PB_ERR_INVALID, "null params");
+    return search_subsets(ix, queries, q_tok_offsets, n_queries, params, 1, subset_offsets, subset_ids, has_subset,
+                          out_ids, out_scores, out_counts, trace);
 }
 
 extern "C" pb_status pb_search_batch(pb_index *ix, const float *queries, const int64_t *q_tok_offsets, int64_t n_queries,
@@ -2785,8 +2925,8 @@ extern "C" pb_status pb_search_batch_device(pb_index *ix, const float *d_queries
                                             int64_t n_queries, const pb_search_params *params, int64_t *d_out_ids,
                                             float *d_out_scores, int32_t *d_out_counts) {
     SearchIO io{d_queries, true, q_tok_offsets_host, n_queries, nullptr, nullptr, nullptr, 0, false,
-                d_out_ids, d_out_scores, d_out_counts, true, nullptr};
-    return search_impl(ix, params, io);
+                d_out_ids, d_out_scores, d_out_counts, true, nullptr, params, 0, params ? params->top_k : 0};
+    return search_impl(ix, io);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -431,13 +431,15 @@ k_a5_bound(const unsigned short *__restrict__ ST16, const int *__restrict__ q_of
 //   entry of filt_list whose filt_key >= thr (unordered).  grid = B, 1024 threads.
 // The pruned a5 rounds use the optional arguments: thr_out[b] = thr; filt_hi[b] also caps the key (filt_key <
 // filt_hi[b]); the output goes after out_base[b] entries and out_n[b] counts them too; tally adds up the out_n.
+// qN: each query's own N (DESIGN.md 4l), or null.
 __global__ void __launch_bounds__(1024)
 k_select_u32(const uint32_t *__restrict__ sel_keys, const int *__restrict__ sel_n, int N, int band_per_q,
              const uint32_t *__restrict__ filt_keys, const uint32_t *__restrict__ filt_list,
              const int *__restrict__ filt_n, long long stride, const int *__restrict__ q_off,
              const int *__restrict__ qflag, uint32_t *__restrict__ out_list, int *__restrict__ out_n,
              uint32_t *__restrict__ thr_out = nullptr, const uint32_t *__restrict__ filt_hi = nullptr,
-             const int *__restrict__ out_base = nullptr, unsigned long long *__restrict__ tally = nullptr) {
+             const int *__restrict__ out_base = nullptr, unsigned long long *__restrict__ tally = nullptr,
+             const int *__restrict__ qN = nullptr) {
     // one histogram per warp: the keys of a query share their high digits (sums of nq 16-bit codes), so a single
     // histogram serialises every thread of the CTA on one or two shared-memory words (0.15 ms); a warp whose 32 keys
     // fall in one bin adds 32 with one atomic
@@ -446,6 +448,7 @@ k_select_u32(const uint32_t *__restrict__ sel_keys, const int *__restrict__ sel_
     __shared__ int remaining_s, fill_s;
     const int b = blockIdx.x;
     const int ns = sel_n[b], nf = filt_n[b];
+    if (qN) N = qN[b];
     const int nq = q_off[b + 1] - q_off[b];
     const uint32_t *L = sel_keys + (size_t)b * stride;
     const uint32_t *F = filt_keys + (size_t)b * stride;

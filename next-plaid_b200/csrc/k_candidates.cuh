@@ -251,13 +251,13 @@ k_unique_codes(const uint32_t *__restrict__ codes, const long long *__restrict__
 // ------------------------------------------------------------------------------------------
 // a6: per query, the M smallest cut keys in ascending order (M = min(n_full_scores, n_decompress)),
 // via MSB radix select + bitonic sort; also the token prefix sums the exact stage walks.
-// grid = B, 1024 threads, dynamic smem = Mpow2*8 bytes.
+// qM: each query's own M (or null: M); lists keep the stride Mcap.  grid = B, 1024 threads, dynamic smem = Mpow2*8 bytes.
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(1024)
 k_cut(const u64 *__restrict__ keys, const float *__restrict__ approx_in, long long cand_cap,
       const int *__restrict__ n_cand, int M, int Mcap, const long long *__restrict__ doc_off,
       uint32_t *__restrict__ kept, int *__restrict__ n_kept, long long *__restrict__ tok_prefix,
-      long long *__restrict__ kept_tokens, uint32_t doc_id_base, u64 *__restrict__ out_keys) {
+      long long *__restrict__ kept_tokens, uint32_t doc_id_base, u64 *__restrict__ out_keys, const int *__restrict__ qM) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     u64 *sk = reinterpret_cast<u64 *>(smem_raw);
     __shared__ int hist[256];
@@ -266,6 +266,7 @@ k_cut(const u64 *__restrict__ keys, const float *__restrict__ approx_in, long lo
     __shared__ int remaining_s, fill_s;
     const int b = blockIdx.x;
     const int n = n_cand[b];
+    if (qM) M = qM[b];
     const int Mq = min(M, n);
     const u64 *kb = keys + (size_t)b * cand_cap;
     const int P = next_pow2(max(Mq, 1));
@@ -311,8 +312,9 @@ k_cut(const u64 *__restrict__ keys, const float *__restrict__ approx_in, long lo
         __syncthreads();
     }
     bitonic_sort_u64(sk, P);
-    if (out_keys) {  // doc-sharded mode: the shard's sorted top-M goes to the all-gather; kept docs come from k_merge_cut
-        for (int i = threadIdx.x; i < M; i += blockDim.x) out_keys[(size_t)b * M + i] = i < Mq ? sk[i] : ~0ull;
+    if (out_keys) {  // doc-sharded mode: the shard's sorted top-M goes to the all-gather (Mcap keys, ~0 past M); kept
+                     // docs come from k_merge_cut
+        for (int i = threadIdx.x; i < Mcap; i += blockDim.x) out_keys[(size_t)b * Mcap + i] = i < Mq ? sk[i] : ~0ull;
         return;
     }
     // outputs + token prefix sums

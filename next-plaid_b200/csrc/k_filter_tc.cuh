@@ -133,13 +133,15 @@ k_filter_diag(const uint32_t *__restrict__ est, const uint32_t *__restrict__ exa
     }
 }
 
-// survivors of the filter, in approximate-rank order.  grid = B, 1024 threads, smem = pow2(n_kept) * 8.
+// survivors of the filter, in approximate-rank order.  qtopk: each query's own top_k (or null: top_k); a query whose
+// top_k reaches its kept count keeps every kept doc.  grid = B, 1024 threads, smem = pow2(n_kept) * 8.
 __global__ void __launch_bounds__(1024)
 k_tc_select(const float *__restrict__ est, const uint32_t *__restrict__ kept, const uint32_t *__restrict__ krank,
             const int *__restrict__ n_kept, int Mcap, int top_k, const int *__restrict__ q_off,
             const float *__restrict__ qnmax, float eps_unit, const long long *__restrict__ doc_off,
             uint32_t *__restrict__ kept2, uint32_t *__restrict__ krank2, int *__restrict__ n_kept2,
-            long long *__restrict__ tok_prefix2, long long *__restrict__ kept_tokens2, uint32_t *__restrict__ src_rank2) {
+            long long *__restrict__ tok_prefix2, long long *__restrict__ kept_tokens2, uint32_t *__restrict__ src_rank2,
+            const int *__restrict__ qtopk) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     u64 *sk = reinterpret_cast<u64 *>(smem_raw);
     __shared__ int scan_tmp[33];
@@ -147,6 +149,7 @@ k_tc_select(const float *__restrict__ est, const uint32_t *__restrict__ kept, co
     const int b = blockIdx.x;
     const int nk = n_kept[b];
     const int nq = q_off[b + 1] - q_off[b];
+    if (qtopk) top_k = qtopk[b];
     const float *e = est + (size_t)b * Mcap;
     if (threadIdx.x == 0) any_bad = 0;
     __syncthreads();

@@ -137,10 +137,15 @@ k_chunkmax16(const unsigned short *__restrict__ ST16, long long K, int QS, int n
 }
 
 // tau[b][q] = the largest t with at least n chunk maxima >= t; 65536 for padding rows.  grid = (QS, B), 32 threads.
+// qn: each query's own n (or null: n).  The chunk geometry is the pass's, chosen for its largest n, and any chunking
+// with n_chunks >= n is exact for n: n entries with code >= tau exist (the n chunks whose maxima reach it), so an entry
+// below tau is beaten by n others, whatever the chunk size.
 __global__ void k_tau16(const unsigned short *__restrict__ cmax, const int *__restrict__ q_off, int QS, int n, int n_chunks,
-                        const int *__restrict__ qflag, uint32_t *__restrict__ tau, int *__restrict__ fallback) {
+                        const int *__restrict__ qflag, uint32_t *__restrict__ tau, int *__restrict__ fallback,
+                        const int *__restrict__ qn) {
     const int q = blockIdx.x, b = blockIdx.y, lane = threadIdx.x;
     const int nq = q_off[b + 1] - q_off[b];
+    if (qn) n = qn[b];
     if (q == 0 && lane == 0 && qflag[b]) atomicOr(fallback, 1);
     if (q >= nq) {
         if (lane == 0) tau[(size_t)b * QS + q] = 65536u;
@@ -250,11 +255,15 @@ k_cells(const u64 *__restrict__ sel, const float *__restrict__ ST, const int *__
         long long K, int QS, int n, int cells_cap, int has_thr, float thr, int batched,
         long long slab, uint32_t *__restrict__ cells, int *__restrict__ n_cells,
         const unsigned short *__restrict__ cmax16, int n_chunks, int chunk_rows, const float2 *__restrict__ qrange,
-        const int *__restrict__ gate) {
+        const int *__restrict__ gate, const int *__restrict__ qn, const int *__restrict__ qhas,
+        const float *__restrict__ qthr) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int b = blockIdx.x;
     const int nq = q_off[b + 1] - q_off[b];
-    const int total = nq * n;
+    const int total = nq * n;  // sel rows keep the pass's stride n; entries past a query's own n are 0
+    // per-query parameters (DESIGN.md 4l): the query's own n (the batched slab-heap size) and threshold
+    const int nb = qn ? qn[b] : n;
+    if (qhas) has_thr = qhas[b], thr = qthr[b];
     const int P = next_pow2(max(total, 1));
     // chunk maxima of the 16-bit table (threshold-first probe) prune the slab-prefix scan below; not when the
     // probe fell back (flagged query: no valid table)
@@ -350,7 +359,7 @@ k_cells(const u64 *__restrict__ sel, const float *__restrict__ ST, const int *__
                                 cnt += (score_key_asc(STb[(size_t)c2 * QS + q]) >= kv) ? 1 : 0;
 #pragma unroll
                         for (int m = 16; m >= 1; m >>= 1) cnt += __shfl_xor_sync(PB_FULL, cnt, m);
-                        if (cnt < n) keep = 1;
+                        if (cnt < nb) keep = 1;
                     }
                 }
             }

@@ -73,10 +73,12 @@ k_topn_select_row(const float *__restrict__ ST, const int *__restrict__ q_off, l
 __global__ void __launch_bounds__(1024)
 k_cells_from_query_bits(uint32_t *__restrict__ cellbits, long long Wk, const float *__restrict__ ST,
                         const int *__restrict__ q_off, long long K, int QS, int has_thr, float thr, int cells_cap,
-                        uint32_t *__restrict__ cells, int *__restrict__ n_cells) {
+                        uint32_t *__restrict__ cells, int *__restrict__ n_cells, const int *__restrict__ qhas,
+                        const float *__restrict__ qthr) {
     __shared__ int scan_tmp[33];
     const int b = blockIdx.x;
     const int nq = q_off[b + 1] - q_off[b];
+    if (qhas) has_thr = qhas[b], thr = qthr[b];  // the query's own threshold (DESIGN.md 4l)
     uint32_t *bits = cellbits + (size_t)b * Wk;
     const float *STb = ST + (size_t)b * K * QS;
     const long long per = (Wk + blockDim.x - 1) / blockDim.x;

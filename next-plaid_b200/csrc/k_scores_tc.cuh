@@ -346,10 +346,12 @@ k_cells_thr(const u64 *__restrict__ sel, const float *__restrict__ rows, const u
             float thr, int batched, long long slab, int *__restrict__ flags,
             const unsigned short *__restrict__ ST16, const float2 *__restrict__ qrange, int code_margin,
             const float *__restrict__ Q, const float *__restrict__ C, int dim, const unsigned short *__restrict__ cmax16,
-            int n_chunks, int chunk_rows) {
+            int n_chunks, int chunk_rows, const int *__restrict__ qn, const int *__restrict__ qhas,
+            const float *__restrict__ qthr) {
     const int b = blockIdx.y;
     const int nq = q_off[b + 1] - q_off[b];
     const int nu = n_u[b];
+    if (qhas) has_thr = qhas[b], thr = qthr[b];  // the query's own threshold (DESIGN.md 4l)
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
     for (int u = blockIdx.x * nwarps + w; u < nu; u += gridDim.x * nwarps) {
         const uint32_t c = ulist[(size_t)b * cap + u];
@@ -381,6 +383,7 @@ k_cells_thr(const u64 *__restrict__ sel, const float *__restrict__ rows, const u
                     // another token may have recorded a score >= thr for c while scanning its slab
                     const long long s0 = (long long)(c / slab) * slab;
                     const float2 rg = qrange[b];
+                    const int nb = qn ? qn[b] : n;  // the query's own n: its slab-heap size
                     for (int q = 0; q < nq && !keep; ++q) {
                         const float v = row[q];
                         const uint32_t kv = score_key_asc(v);
@@ -416,7 +419,7 @@ k_cells_thr(const u64 *__restrict__ sel, const float *__restrict__ rows, const u
                         }
 #pragma unroll
                         for (int m = 16; m >= 1; m >>= 1) cnt += __shfl_xor_sync(PB_FULL, cnt, m);
-                        if (cnt < n) keep = 1;
+                        if (cnt < nb) keep = 1;
                     }
                 }
             }

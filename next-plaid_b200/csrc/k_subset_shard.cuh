@@ -96,11 +96,13 @@ __global__ void k_cells_from_bits(const uint32_t *__restrict__ elig, const int *
 __global__ void __launch_bounds__(256)
 k_cells_filter_list(const uint32_t *__restrict__ list, int lcap, const int *__restrict__ list_n,
                     const float *__restrict__ ST, const int *__restrict__ q_off, long long K, int QS, int has_thr,
-                    float thr, int cells_cap, uint32_t *__restrict__ cells, int *__restrict__ n_cells) {
+                    float thr, int cells_cap, uint32_t *__restrict__ cells, int *__restrict__ n_cells,
+                    const int *__restrict__ qhas, const float *__restrict__ qthr) {
     __shared__ int scan_tmp[33];
     const int b = blockIdx.x;
     const int nq = q_off[b + 1] - q_off[b];
     const int n = list_n[b];
+    if (qhas) has_thr = qhas[b], thr = qthr[b];  // the query's own threshold (DESIGN.md 4l)
     const uint32_t *lst = list + (size_t)b * lcap;
     const float *STb = ST + (size_t)b * K * QS;
     int outn = 0;
@@ -136,14 +138,17 @@ k_cells_filter_list(const uint32_t *__restrict__ list, int lcap, const int *__re
 // ------------------------------------------------------------------------------------------
 // k_merge_cut: every shard's list is sorted (best first) and keys are unique (global doc id in the low word), so the
 // global rank of my j-th entry is j + the number of smaller keys in every other shard's list (one binary search
-// each); it is in the global cut iff that rank < M.  No sort, no shared memory: any number of shards.
+// each); it is in the global cut iff that rank < M.  No sort, no shared memory: any number of shards.  Lists are Mcap
+// keys per query (~0 past the shard's own); qM: each query's own M (or null: M).
 __global__ void __launch_bounds__(1024)
-k_merge_cut(const u64 *__restrict__ gkeys, int G, int my_rank, int B, int M, uint32_t doc_id_base, long long D,
+k_merge_cut(const u64 *__restrict__ gkeys, int G, int my_rank, int B, int M, int Mcap, uint32_t doc_id_base, long long D,
             const long long *__restrict__ doc_off, uint32_t *__restrict__ kept, uint32_t *__restrict__ krank,
-            int *__restrict__ n_kept, long long *__restrict__ tok_prefix, long long *__restrict__ kept_tokens) {
+            int *__restrict__ n_kept, long long *__restrict__ tok_prefix, long long *__restrict__ kept_tokens,
+            const int *__restrict__ qM) {
     __shared__ int scan_tmp[33];
     const int b = blockIdx.x;
-    const u64 *mine = gkeys + ((size_t)my_rank * B + b) * M;
+    if (qM) M = qM[b];
+    const u64 *mine = gkeys + ((size_t)my_rank * B + b) * Mcap;
     long long run = 0;
     int outn = 0;
     for (int base = 0; base < M; base += blockDim.x) {
@@ -155,7 +160,7 @@ k_merge_cut(const u64 *__restrict__ gkeys, int G, int my_rank, int B, int M, uin
             int r = j;
             for (int g = 0; g < G && r < M; ++g) {
                 if (g == my_rank) continue;
-                const u64 *lst = gkeys + ((size_t)g * B + b) * M;
+                const u64 *lst = gkeys + ((size_t)g * B + b) * Mcap;
                 int lo = 0, hi = M;  // first position with lst[pos] >= key (~0 padding sorts last)
                 while (lo < hi) {
                     const int mid = (lo + hi) >> 1;
@@ -175,15 +180,15 @@ k_merge_cut(const u64 *__restrict__ gkeys, int G, int my_rank, int B, int M, uin
         const int pos = block_exclusive_scan(f, scan_tmp, &tot);
         const int tpos = block_exclusive_scan(len, scan_tmp, &ttot);
         if (f) {
-            kept[(size_t)b * M + outn + pos] = d;
-            krank[(size_t)b * M + outn + pos] = grank;
-            tok_prefix[(size_t)b * (M + 1) + outn + pos] = run + tpos;
+            kept[(size_t)b * Mcap + outn + pos] = d;
+            krank[(size_t)b * Mcap + outn + pos] = grank;
+            tok_prefix[(size_t)b * (Mcap + 1) + outn + pos] = run + tpos;
         }
         outn += tot;
         run += ttot;
     }
     if (threadIdx.x == 0) {
-        tok_prefix[(size_t)b * (M + 1) + outn] = run;
+        tok_prefix[(size_t)b * (Mcap + 1) + outn] = run;
         n_kept[b] = outn;
         kept_tokens[b] = run;
     }
@@ -191,13 +196,15 @@ k_merge_cut(const u64 *__restrict__ gkeys, int G, int my_rank, int B, int M, uin
 
 // k_merge_topk: the global cut has at most M members and every global approximate rank belongs to exactly one shard,
 // so the real entries of all shards fit M slots indexed by rank: sort those (smem = pow2(M) keys), payloads stay in
-// global memory.  `slot` is scratch [B][M] (source position of every rank).
+// global memory.  `slot` is scratch [B][M] (source position of every rank).  Lists are M = Mcap entries per query;
+// qtopk: each query's own top_k (or null: top_k); rows of the outputs are `ostride` apart.
 __global__ void __launch_bounds__(1024)
 k_merge_topk(const u64 *__restrict__ gfkeys, const u64 *__restrict__ gpayload, int G, int B, int M, int top_k,
              uint32_t *__restrict__ slot, long long *__restrict__ out_ids, float *__restrict__ out_scores,
-             int *__restrict__ out_counts) {
+             int *__restrict__ out_counts, const int *__restrict__ qtopk, int ostride) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int b = blockIdx.x;
+    if (qtopk) top_k = qtopk[b];
     const int P = next_pow2(max(M, 1));
     u64 *sk = reinterpret_cast<u64 *>(smem_raw);  // [P], indexed by global approximate rank before the sort
     uint32_t *sl = slot + (size_t)b * M;
@@ -225,8 +232,8 @@ k_merge_topk(const u64 *__restrict__ gfkeys, const u64 *__restrict__ gpayload, i
         const uint32_t src = sl[(uint32_t)sk[i]];
         const int g = (int)(src / (uint32_t)M), j = (int)(src - (uint32_t)g * (uint32_t)M);
         const u64 pv = gpayload[((size_t)g * B + b) * M + j];
-        out_ids[(size_t)b * top_k + i] = (long long)(pv >> 32);
-        out_scores[(size_t)b * top_k + i] = __uint_as_float((uint32_t)pv);
+        out_ids[(size_t)b * ostride + i] = (long long)(pv >> 32);
+        out_scores[(size_t)b * ostride + i] = __uint_as_float((uint32_t)pv);
     }
     if (threadIdx.x == 0) out_counts[b] = cnt;
 }

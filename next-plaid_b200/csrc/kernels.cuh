@@ -26,6 +26,10 @@
 //
 // Layouts: S is stored transposed per query, ST[b][c][QS] (one 4*QS-byte row per centroid, QS =
 // query tokens rounded up to 8), so the approximate stage gathers one contiguous row per doc token.
+//
+// Per-query search parameters (DESIGN.md 4l): a kernel that reads n_ivf_probe, the threshold, M or top_k takes the
+// pass's value as a scalar and an optional per-query array (qn, qhas / qthr, qM / qN, qtopk).  With the array it reads
+// its query's entry once per CTA, before any loop; buffers keep the pass's (n) or the call's (Mcap, top_k) stride.
 #pragma once
 #include "common.cuh"
 

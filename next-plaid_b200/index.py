@@ -76,7 +76,7 @@ EXPORTS = [
     "pb_search_params_default", "pb_index_load", "pb_index_open", "pb_index_close",
     "pb_index_num_documents", "pb_index_num_embeddings", "pb_index_num_partitions",
     "pb_index_avg_doclen", "pb_index_embedding_dim", "pb_index_nbits", "pb_index_device",
-    "pb_search_batch", "pb_search_batch_traced", "pb_search_batch_subsets", "pb_centroid_scores", "pb_decompress_documents",
+    "pb_search_batch", "pb_search_batch_traced", "pb_search_batch_subsets", "pb_search_batch_params", "pb_centroid_scores", "pb_decompress_documents",
     "pb_maxsim_scores", "pb_exhaustive_scores", "pb_set_profiling", "pb_last_stage_stats",
     "pb_last_work_counters", "pb_search_batch_device", "pb_last_error", "pb_version",
     "pb_device_count", "pb_comm_unique_id", "pb_index_comm_init", "pb_shard_group_create", "pb_shard_group_destroy",
@@ -141,6 +141,7 @@ def load_library():
         L.pb_search_batch_subsets.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(_Params),
                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                               C.c_void_p]
+        L.pb_search_batch_params.argtypes = list(L.pb_search_batch_subsets.argtypes)
         L.pb_search_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                              C.POINTER(_Params), C.c_void_p, C.c_void_p, C.c_void_p]
         L.pb_centroid_scores.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
@@ -249,6 +250,10 @@ class ShardGroup:
     def search_batch_subsets(self, queries, params, subsets, trace=False):
         """MmapIndex.search_batch_subsets on the whole deployment (global ids; every rank gets the same subsets)."""
         return self._collective(lambda r, s: s.search_batch_subsets(queries, params, subsets, trace=trace))[0]
+
+    def search_batch_params(self, queries, params, subsets=None, trace=False):
+        """MmapIndex.search_batch_params on the whole deployment (every rank gets the same parameters and subsets)."""
+        return self._collective(lambda r, s: s.search_batch_params(queries, params, subsets, trace=trace))[0]
 
     def delete(self, doc_ids: Sequence[int], index_dir: Optional[str] = None) -> int:
         """pb_index_delete_sharded: MmapIndex.delete on the whole deployment (global ids); each rank renumbers its
@@ -369,6 +374,21 @@ class SearchTrace:
     approx: List[np.ndarray]
     kept: List[np.ndarray]
     kept_exact: List[np.ndarray]
+
+
+def _subset_args(subsets, n_queries):
+    """(offsets, ids, has) of pb_search_batch_subsets for a list of Option<&[i64]> subsets (None: no query has one)"""
+    if subsets is None:
+        subsets = [None] * n_queries
+    if len(subsets) != n_queries:
+        raise PlaidError(PB_ERR_INVALID, f"{len(subsets)} subsets for {n_queries} queries")
+    has = np.array([s is not None for s in subsets], np.uint8)
+    lists = [np.ascontiguousarray(s, np.int64).reshape(-1) if s is not None else np.zeros(0, np.int64)
+             for s in subsets]
+    so = np.zeros(len(lists) + 1, np.int64)
+    so[1:] = np.cumsum([len(x) for x in lists])
+    si = np.ascontiguousarray(np.concatenate(lists) if lists else np.zeros(0, np.int64), np.int64)
+    return so, si, has
 
 
 def _pack_queries(queries: Sequence[np.ndarray], dim: int):
@@ -577,33 +597,47 @@ class MmapIndex:
         """pb_search_batch_subsets: search_batch with its own Option<&[i64]> subset per query (None: no filter, []:
         nothing eligible).  Result i equals search_batch([queries[i]], params, subset=subsets[i])[0]."""
         L = load_library()
-        if len(subsets) != len(queries):
-            raise PlaidError(PB_ERR_INVALID, f"{len(subsets)} subsets for {len(queries)} queries")
-        has = np.array([s is not None for s in subsets], np.uint8)
-        lists = [np.ascontiguousarray(s, np.int64).reshape(-1) if s is not None else np.zeros(0, np.int64)
-                 for s in subsets]
-        so = np.zeros(len(lists) + 1, np.int64)
-        so[1:] = np.cumsum([len(x) for x in lists])
-        si = np.ascontiguousarray(np.concatenate(lists) if lists else np.zeros(0, np.int64), np.int64)
+        so, si, has = _subset_args(subsets, len(queries))
         return self._search(queries, params, trace, bool(has.any()),
                             lambda flat, offs, B, p, ids, sc, cn, tr: L.pb_search_batch_subsets(
                                 self._h, _ptr(flat), _ptr(offs), B, p, _ptr(so), _ptr(si), _ptr(has),
                                 _ptr(ids), _ptr(sc), _ptr(cn), tr))
 
+    def search_batch_params(self, queries: Sequence[np.ndarray], params: Sequence[SearchParameters],
+                            subsets: Optional[Sequence[Optional[Sequence[int]]]] = None, trace: bool = False):
+        """pb_search_batch_params: search_batch_subsets with its own SearchParameters per query.  Result i equals
+        search_batch([queries[i]], params[i], subset=subsets[i])[0], cut to its own count."""
+        L = load_library()
+        params = list(params)
+        if len(params) != len(queries):
+            raise PlaidError(PB_ERR_INVALID, f"{len(params)} parameter sets for {len(queries)} queries")
+        so, si, has = _subset_args(subsets, len(queries))
+        return self._search(queries, params, trace, bool(has.any()),
+                            lambda flat, offs, B, p, ids, sc, cn, tr: L.pb_search_batch_params(
+                                self._h, _ptr(flat), _ptr(offs), B, p, None if subsets is None else _ptr(so),
+                                _ptr(si), _ptr(has), _ptr(ids), _ptr(sc), _ptr(cn), tr))
+
     def _search(self, queries, params, trace, any_subset, invoke):
         """the outputs (and trace buffers) of one search call; invoke(flat, offs, B, params, ids, scores, counts,
-        trace pointer) makes the call"""
+        trace pointer) makes the call.  params: one SearchParameters, or a list of one per query"""
         flat, offs = _pack_queries(queries, self.embedding_dim())
-        B, k = len(queries), max(int(params.top_k), 0)
+        plist = params if isinstance(params, list) else [params]
+        B, k = len(queries), max([int(q.top_k) for q in plist] + [0])
         ids = np.zeros((B, max(k, 1)), np.int64)
         sc = np.zeros((B, max(k, 1)), np.float32)
         cn = np.zeros(B, np.int32)
-        p = params._c()
+        if isinstance(params, list):
+            p = (_Params * max(B, 1))(*[q._c() for q in params])
+            p_arg = C.cast(p, C.POINTER(_Params)) if B else None
+        else:
+            p = params._c()
+            p_arg = C.byref(p)
         tr, bufs = None, None
         if trace:
             D, K = self.num_documents(), self.num_partitions()
-            M = max(min(params.n_full_scores, max(params.n_full_scores // 4, params.top_k)), 1)
-            cc = min(K, max(int(offs[-1]) * max(params.n_ivf_probe, 1), 1)) if not any_subset else K
+            M = max([min(q.n_full_scores, max(q.n_full_scores // 4, q.top_k)) for q in plist] + [1])
+            n_probe = max([max(q.n_ivf_probe, 1) for q in plist] + [1])
+            cc = min(K, max(int(offs[-1]) * n_probe, 1)) if not any_subset else K
             bufs = dict(cells=np.zeros((B, cc), np.int64), n_cells=np.zeros(B, np.int32),
                         cand=np.zeros((B, max(D, 1)), np.int64), approx=np.zeros((B, max(D, 1)), np.float32),
                         n_cand=np.zeros(B, np.int32), kept=np.zeros((B, M), np.int64),
@@ -611,7 +645,7 @@ class MmapIndex:
             tr = _Trace(_ptr(bufs["cells"]), _ptr(bufs["n_cells"]), cc, _ptr(bufs["cand"]),
                         _ptr(bufs["approx"]), _ptr(bufs["n_cand"]), max(D, 1), _ptr(bufs["kept"]),
                         _ptr(bufs["kex"]), _ptr(bufs["n_kept"]), M)
-        _check(invoke(flat, offs, B, C.byref(p), ids, sc, cn, None if tr is None else C.cast(C.pointer(tr), C.c_void_p)))
+        _check(invoke(flat, offs, B, p_arg, ids, sc, cn, None if tr is None else C.cast(C.pointer(tr), C.c_void_p)))
         res = [QueryResult(i, ids[i, :cn[i]].copy(), sc[i, :cn[i]].copy()) for i in range(B)]
         if trace:
             t = SearchTrace(

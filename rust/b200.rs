@@ -70,6 +70,20 @@ extern "C" {
         out_counts: *mut i32,
         trace: *mut c_void,
     ) -> c_int;
+    fn pb_search_batch_params(
+        ix: *mut c_void,
+        queries: *const f32,
+        q_tok_offsets: *const i64,
+        n_queries: i64,
+        params: *const PbSearchParams, // [n_queries]
+        subset_offsets: *const i64,
+        subset_ids: *const i64,
+        has_subset: *const u8,
+        out_ids: *mut i64, // row i at i * max top_k
+        out_scores: *mut f32,
+        out_counts: *mut i32,
+        trace: *mut c_void,
+    ) -> c_int;
     fn pb_last_error() -> *const c_char;
     fn pb_codec_open(device: i32, centroids: *const f32, k: i64, dim: i32, nbits: i32, cutoffs: *const f32,
                      out: *mut *mut c_void) -> c_int;
