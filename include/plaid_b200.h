@@ -355,6 +355,61 @@ PB_API pb_status pb_search_batch_params(pb_index *ix, const float *queries, cons
                                         const uint8_t *has_subset, int64_t *out_ids, float *out_scores,
                                         int32_t *out_counts, pb_trace *trace);
 
+/* MmapIndex::search (index.rs:1258 -> search_one_mmap, search.rs:327): one query per call, the way a server's worker
+ * threads enter the library (next-plaid-api/src/state.rs:24-47, handlers/search.rs:221).
+ *   query        [n_query_tokens][dim] f32 row-major (host memory)
+ *   subset       Option<&[i64]>: NULL = None; otherwise n_subset doc ids (may be empty)
+ *   out_ids / out_scores [params->top_k], *out_count the number of valid entries
+ * With coalescing off (the default) it is pb_search_batch_params with n_queries = 1 and nothing more: same result,
+ * statuses, messages and thread-local stats.  With coalescing on (pb_index_set_coalescing) the calls that arrive from
+ * different host threads while the device is busy are merged into one pb_search_batch_params call; each caller blocks
+ * until its own request is answered and gets, bit for bit, what it would get alone.
+ *   - A request that pb_search_batch_params would refuse alone (PB_ERR_INVALID: null pointers, negative sizes, top_k or
+ *     n_full_scores < 0, n_ivf_probe < 1; PB_ERR_UNSUPPORTED: the limits of pb_search_batch) is refused on its own
+ *     thread before it is queued and never affects another caller.
+ *   - A merged call that fails with PB_ERR_CUDA fails every request in it.  Any other failure (PB_ERR_NOMEM for the
+ *     workspace, a limit only the device can evaluate) re-runs the members alone, each getting the status of its own run.
+ *   - pb_last_error() is the caller's own message.  pb_last_work_counters, pb_last_stage_stats, pb_last_kernel_ms,
+ *     pb_last_call_ms and pb_last_staging_stats report the merged batch the request rode in (n_queries counts that
+ *     batch's queries), on every thread of that batch alike; after a re-run alone, the request's own run.
+ *   - Appends and deletes are seen entirely or not at all, as by any search.
+ * Doc-sharded handles always run the plain batch of one (a collective, called on every rank in step). */
+PB_API pb_status pb_search(pb_index *ix, const float *query, int64_t n_query_tokens, const pb_search_params *params,
+                           const int64_t *subset, int64_t n_subset, int64_t *out_ids /* [top_k] */,
+                           float *out_scores /* [top_k] */, int32_t *out_count);
+
+/* Coalescing of concurrent pb_search calls on one handle (no reference analogue: next-plaid searches each request on its
+ * own rayon task).  No thread is created: the caller at the head of the handle's queue runs the next batch -- up to
+ * max_queries requests in arrival order -- as soon as fewer than max_inflight batches are running, and wakes the
+ * callers that rode in it; a caller never serves a second batch.  With max_wait_us = 0 an idle handle answers a
+ * request at once, alone; batches form from what arrives while max_inflight batches are on the device.
+ * Environment defaults, read at open: PB_COALESCE (max_queries), PB_COALESCE_WAIT_US, PB_COALESCE_INFLIGHT; unset = off.
+ * May be called while searches run: requests already queued are still answered.
+ * Measured on config B (DESIGN.md 4m, one H100): with 32 or more caller threads, 32 / 200 / 2 gives 1.8-2.4x the
+ * throughput of coalescing off and a p99 latency 2-3x lower; max_wait_us = 0 costs a lone caller nothing but leaves a
+ * long p99 tail under load, and max_wait_us = 200 costs a lone caller more than a millisecond.
+ * PB_ERR_INVALID: max_queries < 1, max_inflight < 1, max_wait_us < 0.  PB_ERR_UNSUPPORTED: max_queries > 1 on a
+ * doc-sharded handle; pb_index_comm_init and pb_index_group_join turn coalescing off. */
+typedef struct pb_coalesce_config {
+    int32_t max_queries;   /* largest merged batch; 1 = off */
+    int32_t max_wait_us;   /* how long the leader of a batch of fewer than max_queries waits for more; 0 = never; at most 10 000 */
+    int32_t max_inflight;  /* merged batches that may run at once on the handle */
+} pb_coalesce_config;
+PB_API pb_status pb_index_set_coalescing(pb_index *ix, const pb_coalesce_config *cfg /* NULL = off */);
+
+typedef struct pb_coalesce_stats {
+    int64_t n_requests;       /* pb_search calls that went through the queue */
+    int64_t n_batches;        /* merged calls run */
+    int64_t n_bypassed;       /* pb_search calls that ran as a plain batch of one (coalescing off, doc-sharded) */
+    int64_t n_refused;        /* requests refused by their own validation, never queued */
+    int64_t n_rerun_alone;    /* members re-run alone after their merged call failed */
+    int64_t max_batch;        /* largest merged batch so far */
+    int64_t batch_hist[8];    /* merged batches of size 1, 2, 3-4, 5-8, 9-16, 17-32, 33-64, > 64 */
+    int64_t queue_wait_us;    /* sum over requests: enqueue -> start of their merged call */
+} pb_coalesce_stats;
+/* Counters of the handle's queue since open or the last reset (reset != 0 clears them after the read). */
+PB_API pb_status pb_index_coalesce_stats(pb_index *ix, pb_coalesce_stats *out, int32_t reset);
+
 /* ---- stage entry points (each is one kernel of the path; used by tests, bench and ncu) ---- */
 
 /* Stage 1, S = Q * C^T (search.rs:345).  out: [n_query_tokens][K] row-major f32, host. */

@@ -2,6 +2,7 @@
 // load, index.rs:995-1016), the search pipeline that replaces search::search_many_mmap
 // (search.rs:643) and the C-ABI of include/plaid_b200.h.  No CPU fallback anywhere: every entry
 // point needs an sm_90 (H100) device.
+#include "coalesce.h"
 #include "engine_internal.h"
 #include "kernels.cuh"
 
@@ -416,6 +417,20 @@ struct LaneWorker {
     }
 };
 
+// pb_search's request queue (coalesce.h, DESIGN.md 4m) runs a merged batch through this: run_coalesced, below the
+// search entry points
+struct CoalescedRun {
+    pb_index *ix;
+    int operator()(pbq::Request *const *reqs, size_t n, std::string &err) const;
+};
+struct GatherBuf {  // host scratch of one merged batch: the arguments of its pb_search_batch_params call
+    std::vector<float> queries, scores;
+    std::vector<int64_t> q_off, sub_off, sub_ids, ids;
+    std::vector<pb_search_params> params;
+    std::vector<uint8_t> has_sub;
+    std::vector<int32_t> counts;
+};
+
 struct pb_index {
     int device = 0;
     int dim = 0, nbits = 0, packed = 0;
@@ -458,6 +473,10 @@ struct pb_index {
     int rank = 0, world = 1;
     std::mutex mu;
     std::vector<std::unique_ptr<Workspace>> pool;
+    // pb_search: concurrent single-query callers merged into shared batches (pb_index_set_coalescing; off by default)
+    pbq::Queue<CoalescedRun> coalescer{CoalescedRun{this}, PB_ERR_CUDA};
+    std::atomic<bool> coalesce_on{false};
+    std::vector<std::unique_ptr<GatherBuf>> gather_pool;  // under mu
     DevBuf ivf_spare, ivf_off_spare;  // the other half of the inverted file's ping-pong: pb_index_append merges into it
     float delete_ms[3] = {0.f, 0.f, 0.f};  // last pb_index_delete with profiling on: compaction, inverted file, norms
     long long delete_window = 1ll << 22;   // tokens per compaction window of pb_index_delete (PB_DELETE_WINDOW_TOKENS)
@@ -966,6 +985,13 @@ pb_status pb_index_finalize(pb_index *ix) {
         if (const char *e = getenv("PB_A5_PRUNE")) ix->a5_prune = atoi(e) != 0;
         if (const char *e = getenv("PB_A5_LIVE")) ix->a5_live = std::max(0ll, atoll(e));
         if (const char *e = getenv("PB_A5_M1")) ix->a5_m1 = std::max(1.0f, (float)atof(e));
+        if (const char *e = getenv("PB_COALESCE")) {
+            pb_coalesce_config c = {atoi(e), 0, 2};
+            if (const char *w = getenv("PB_COALESCE_WAIT_US")) c.max_wait_us = std::max(0, atoi(w));
+            if (const char *f = getenv("PB_COALESCE_INFLIGHT")) c.max_inflight = std::max(1, atoi(f));
+            c.max_queries = std::max(1, c.max_queries);
+            CKS(pb_index_set_coalescing(ix, &c));
+        }
     }
     if (TcDims::has(ix->dim) && ix->N > 0 && ix->K > 0) {
         // operands of the tensor-core score table, and the token norms of the filter
@@ -1091,6 +1117,31 @@ extern "C" void pb_set_scores_tc(pb_index *ix, int32_t enabled) {
 }
 extern "C" void pb_set_lanes(pb_index *ix, int32_t lanes) {
     if (ix) ix->lanes = std::min(8, std::max(1, (int)lanes));
+}
+extern "C" pb_status pb_index_set_coalescing(pb_index *ix, const pb_coalesce_config *cfg) {
+    if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    pbq::Config c;  // off
+    if (cfg) {
+        if (cfg->max_queries < 1 || cfg->max_wait_us < 0 || cfg->max_inflight < 1)
+            return pb_fail(PB_ERR_INVALID, "coalescing: max_queries and max_inflight must be >= 1, max_wait_us >= 0");
+        if (cfg->max_queries > 1 && (ix->world > 1 || ix->group || ix->comm))
+            return pb_fail(PB_ERR_UNSUPPORTED, "coalescing on a doc-sharded handle: a collective needs the same order on every rank");
+        c.max_queries = cfg->max_queries;
+        c.max_wait_us = std::min(cfg->max_wait_us, 10000);
+        c.max_inflight = cfg->max_inflight;
+    }
+    ix->coalescer.configure(c);
+    ix->coalesce_on = c.max_queries > 1;
+    return PB_OK;
+}
+extern "C" pb_status pb_index_coalesce_stats(pb_index *ix, pb_coalesce_stats *out, int32_t reset) {
+    if (!ix || !out) return pb_fail(PB_ERR_INVALID, "null argument");
+    const pbq::Counters c = ix->coalescer.counters(reset != 0);
+    out->n_requests = c.n_requests, out->n_batches = c.n_batches, out->n_bypassed = c.n_bypassed;
+    out->n_refused = c.n_refused, out->n_rerun_alone = c.n_rerun_alone, out->max_batch = c.max_batch;
+    for (int i = 0; i < 8; ++i) out->batch_hist[i] = c.batch_hist[i];
+    out->queue_wait_us = c.queue_wait_us;
+    return PB_OK;
 }
 extern "C" void pb_set_fast_exact(pb_index *ix, int32_t enabled) {
     if (ix) ix->fast_exact = enabled != 0;
@@ -1562,6 +1613,45 @@ struct SearchPlan {
     std::vector<std::pair<int64_t, int>> passes;  // (first position in `order`, queries)
 };
 
+// The checks a query must pass whatever batch it is in.  plan_search and plan_probe apply them to every query of a call
+// and pb_search applies them to a request before it joins a merged batch (check_request), so a request refused alone is
+// refused before it can fail its neighbours.
+static pb_status check_query_args(const pb_search_params &p) {
+    if (p.top_k < 0 || p.n_full_scores < 0) return pb_fail(PB_ERR_INVALID, "top_k / n_full_scores must be >= 0");
+    if (p.n_ivf_probe < 1) return pb_fail(PB_ERR_INVALID, "n_ivf_probe must be >= 1");
+    return PB_OK;
+}
+// M, the docs the cut keeps
+static pb_status query_kept_docs(const pb_search_params &p, int *M) {
+    const long long n_dec = std::max<long long>(p.n_full_scores / 4, p.top_k);  // search.rs:468
+    const long long Mll = std::min<long long>(p.n_full_scores, n_dec);          // take(nfs).take(n_dec)
+    if (Mll > 16384)
+        return pb_fail(PB_ERR_UNSUPPORTED, "min(n_full_scores, max(n_full_scores/4, top_k)) = %lld exceeds 16384", Mll);
+    *M = (int)Mll;
+    return PB_OK;
+}
+static bool query_batched(const pb_index *ix, const pb_search_params &p) {
+    return p.centroid_batch_size > 0 && ix->K > p.centroid_batch_size;  // search.rs:337
+}
+// effective n_ivf_probe beyond 64: the dense variant switches to a row-wise radix select; the batched variant's
+// heap-order threshold rule is tied to the streaming formulation, whose per-lane lists hold up to 192 entries
+static pb_status check_batched_probe(const pb_index *ix, const pb_search_params &p) {
+    const long long n_probe = std::min<long long>(p.n_ivf_probe, ix->K);
+    if (n_probe > 192)
+        return pb_fail(PB_ERR_UNSUPPORTED, "n_ivf_probe %d > 192 with the batched variant is not built", (int)n_probe);
+    return PB_OK;
+}
+// the limits of a query of n_tokens tokens whose probe is of `kind` with effective width n
+static pb_status check_query_rows(const pb_index *ix, uint8_t kind, int n, int n_tokens) {
+    const int QS = query_row_tokens(n_tokens);
+    if ((kind == PROBE_TABLE || kind == PROBE_STREAM) && (long long)QS * n > 8192)
+        return pb_fail(PB_ERR_UNSUPPORTED, "query tokens x n_ivf_probe = %lld exceeds 8192", (long long)QS * n);
+    const size_t per_q = (size_t)ix->K * QS * sizeof(float);
+    if (per_q >= ((size_t)1 << 32))
+        return pb_fail(PB_ERR_UNSUPPORTED, "num_centroids x query tokens x 4 = %zu bytes per query exceeds 2^32", per_q);
+    return PB_OK;
+}
+
 // The arguments and what follows from them alone.  Nothing is enqueued here, so a call refused here takes no workspace.
 static pb_status plan_search(pb_index *ix, const SearchIO &io, SearchPlan &plan) {
     if (!ix || !io.qp) return pb_fail(PB_ERR_INVALID, "null argument");
@@ -1572,8 +1662,7 @@ static pb_status plan_search(pb_index *ix, const SearchIO &io, SearchPlan &plan)
     long long top_k_max = 0;
     for (int64_t b = 0; b < n_par; ++b) {
         const pb_search_params &p = query_params(io, b);
-        if (p.top_k < 0 || p.n_full_scores < 0) return pb_fail(PB_ERR_INVALID, "top_k / n_full_scores must be >= 0");
-        if (p.n_ivf_probe < 1) return pb_fail(PB_ERR_INVALID, "n_ivf_probe must be >= 1");
+        CKS(check_query_args(p));
         top_k_max = std::max<long long>(top_k_max, p.top_k);
     }
     if (top_k_max > 0 && (!io.out_ids || !io.out_scores)) return pb_fail(PB_ERR_INVALID, "null outputs");
@@ -1591,12 +1680,9 @@ static pb_status plan_search(pb_index *ix, const SearchIO &io, SearchPlan &plan)
     int M_max = 0;
     for (int64_t b = 0; b < plan.Bt; ++b) {
         const pb_search_params &p = query_params(io, b);
-        const long long n_dec = std::max<long long>(p.n_full_scores / 4, p.top_k);  // search.rs:468
-        const long long Mll = std::min<long long>(p.n_full_scores, n_dec);          // take(nfs).take(n_dec)
-        if (Mll > 16384)
-            return pb_fail(PB_ERR_UNSUPPORTED, "min(n_full_scores, max(n_full_scores/4, top_k)) = %lld exceeds 16384", Mll);
-        const int M = (int)Mll;
-        const bool batched = p.centroid_batch_size > 0 && ix->K > p.centroid_batch_size;  // search.rs:337
+        int M = 0;
+        CKS(query_kept_docs(p, &M));
+        const bool batched = query_batched(ix, p);
         plan.qtopk[(size_t)b] = (int)p.top_k;
         plan.qM[(size_t)b] = M;
         plan.qM1[(size_t)b] = (int)std::min<double>(ceil((double)ix->a5_m1 * M), (double)INT_MAX);
@@ -1781,13 +1867,8 @@ static pb_status plan_probe(pb_index *ix, Workspace &ws, const SearchIO &io, Sea
         CK(cudaStreamSynchronize(ws.stream));
     }
     if (plan.sharded) g_search_agreed = true;  // the refusals below follow from exchanged data alone
-    // effective n_ivf_probe beyond 64: the dense variant switches to a row-wise radix select; the batched variant's
-    // heap-order threshold rule is tied to the streaming formulation, whose per-lane lists hold up to 192 entries
-    for (int64_t b = 0; b < Bt; ++b) {
-        const long long n_probe = std::min<long long>(query_params(io, b).n_ivf_probe, ix->K);
-        if (!query_empty(plan, b) && plan.qbatched[(size_t)b] && n_probe > 192)
-            return pb_fail(PB_ERR_UNSUPPORTED, "n_ivf_probe %d > 192 with the batched variant is not built", (int)n_probe);
-    }
+    for (int64_t b = 0; b < Bt; ++b)
+        if (!query_empty(plan, b) && plan.qbatched[(size_t)b]) CKS(check_batched_probe(ix, query_params(io, b)));
     plan.qn.assign((size_t)Bt, 0);
     plan.kind.assign((size_t)Bt, PROBE_TABLE);
     for (int64_t b = 0; b < Bt; ++b) {
@@ -1816,13 +1897,7 @@ static pb_status plan_probe(pb_index *ix, Workspace &ws, const SearchIO &io, Sea
     for (int64_t b = 0; b < Bt; ++b) {
         const uint8_t k = plan.kind[(size_t)b];
         if (k == PROBE_NONE) continue;
-        const int QS = query_row_tokens((int)(io.q_off[b + 1] - io.q_off[b]));
-        if ((k == PROBE_TABLE || k == PROBE_STREAM) && (long long)QS * plan.qn[(size_t)b] > 8192)
-            return pb_fail(PB_ERR_UNSUPPORTED, "query tokens x n_ivf_probe = %lld exceeds 8192",
-                           (long long)QS * plan.qn[(size_t)b]);
-        const size_t per_q = (size_t)ix->K * QS * sizeof(float);
-        if (per_q >= ((size_t)1 << 32))
-            return pb_fail(PB_ERR_UNSUPPORTED, "num_centroids x query tokens x 4 = %zu bytes per query exceeds 2^32", per_q);
+        CKS(check_query_rows(ix, k, plan.qn[(size_t)b], (int)(io.q_off[b + 1] - io.q_off[b])));
     }
     g_search_agreed = false;
 
@@ -2914,6 +2989,128 @@ extern "C" pb_status pb_search_batch_params(pb_index *ix, const float *queries, 
                           out_ids, out_scores, out_counts, trace);
 }
 
+// ---- pb_search: one query per call, merged with the other callers' when coalescing is on (DESIGN.md 4m) ----
+struct SearchRequest : pbq::Request {
+    const float *query;
+    int64_t n_tokens;
+    const pb_search_params *params;
+    const int64_t *subset;  // null = None
+    int64_t n_subset;
+    int64_t *out_ids;
+    float *out_scores;
+    int32_t *out_count;
+    Stats stats;  // of the call the request was answered by; installed in the caller's thread-local slot
+};
+
+// a request as a batch of one, straight into its own outputs
+static pb_status search_alone(pb_index *ix, const SearchRequest &r) {
+    const int64_t q_off[2] = {0, r.n_tokens}, sub_off[2] = {0, r.subset ? r.n_subset : 0};
+    const uint8_t has = r.subset ? 1 : 0;
+    return pb_search_batch_params(ix, r.query, q_off, 1, r.params, r.subset ? sub_off : nullptr, r.subset, &has,
+                                  r.out_ids, r.out_scores, r.out_count, nullptr);
+}
+
+// What pb_search_batch_params of the request alone would refuse, as far as the host can tell (the caller holds the
+// read lock: K decides the variant).  Not covered: a dense-variant query with a subset, whose effective n_ivf_probe
+// follows from its eligible centroids, counted on the device; such a request can still fail its merged call, which
+// then re-runs its members alone.
+static pb_status check_request(const pb_index *ix, const SearchRequest &r) {
+    if (!r.params) return pb_fail(PB_ERR_INVALID, "null params");
+    if (r.subset && r.n_subset < 0) return pb_fail(PB_ERR_INVALID, "subset_offsets not monotone");
+    if (!r.query) return pb_fail(PB_ERR_INVALID, "null queries");
+    const pb_search_params &p = *r.params;
+    CKS(check_query_args(p));
+    if (p.top_k > 0 && (!r.out_ids || !r.out_scores)) return pb_fail(PB_ERR_INVALID, "null outputs");
+    if (!r.out_count) return pb_fail(PB_ERR_INVALID, "null out_counts");
+    if (r.n_tokens < 0) return pb_fail(PB_ERR_INVALID, "q_tok_offsets not monotone");
+    int M = 0;
+    CKS(query_kept_docs(p, &M));
+    if (M == 0 || p.top_k == 0 || ix->D == 0) return PB_OK;  // an empty result, no pass
+    const bool batched = query_batched(ix, p);
+    if (batched) CKS(check_batched_probe(ix, p));
+    const int n = (int)std::min<long long>(p.n_ivf_probe, ix->K);
+    const uint8_t kind = (!batched && r.subset) ? PROBE_ALL : n > (batched ? 192 : 64) ? PROBE_BIG : PROBE_TABLE;
+    return check_query_rows(ix, kind, n, (int)r.n_tokens);
+}
+
+int CoalescedRun::operator()(pbq::Request *const *reqs, size_t n, std::string &err) const {
+    pb_status st;
+    if (n == 1) st = search_alone(ix, *static_cast<SearchRequest *>(reqs[0]));
+    else {
+        std::unique_ptr<GatherBuf> gb;
+        {
+            std::lock_guard<std::mutex> g(ix->mu);
+            if (!ix->gather_pool.empty()) {
+                gb = std::move(ix->gather_pool.back());
+                ix->gather_pool.pop_back();
+            }
+        }
+        if (!gb) gb.reset(new GatherBuf());
+        GatherBuf &g = *gb;
+        g.queries.clear(), g.q_off.assign(1, 0), g.sub_off.assign(1, 0), g.sub_ids.clear(), g.params.clear(), g.has_sub.clear();
+        int64_t top_k = 0;
+        bool any_subset = false;
+        for (size_t i = 0; i < n; ++i) {
+            const SearchRequest &r = *static_cast<SearchRequest *>(reqs[i]);
+            g.queries.insert(g.queries.end(), r.query, r.query + (size_t)r.n_tokens * ix->dim);
+            g.q_off.push_back(g.q_off.back() + r.n_tokens);
+            if (r.subset) g.sub_ids.insert(g.sub_ids.end(), r.subset, r.subset + r.n_subset);
+            g.sub_off.push_back((int64_t)g.sub_ids.size());
+            g.has_sub.push_back(r.subset ? 1 : 0);
+            any_subset = any_subset || r.subset;
+            g.params.push_back(*r.params);
+            top_k = std::max(top_k, r.params->top_k);
+        }
+        g.ids.resize(n * (size_t)top_k), g.scores.resize(n * (size_t)top_k), g.counts.resize(n);
+        if (g.queries.empty()) g.queries.push_back(0.f);  // every query has no tokens: the pointer must not be null
+        st = pb_search_batch_params(ix, g.queries.data(), g.q_off.data(), (int64_t)n, g.params.data(),
+                                    any_subset ? g.sub_off.data() : nullptr, g.sub_ids.data(), g.has_sub.data(),
+                                    g.ids.data(), g.scores.data(), g.counts.data(), nullptr);
+        if (st == PB_OK)
+            for (size_t i = 0; i < n; ++i) {
+                const SearchRequest &r = *static_cast<SearchRequest *>(reqs[i]);
+                const size_t c = (size_t)g.counts[i];
+                *r.out_count = g.counts[i];
+                if (c) {
+                    memcpy(r.out_ids, g.ids.data() + i * (size_t)top_k, c * 8);
+                    memcpy(r.out_scores, g.scores.data() + i * (size_t)top_k, c * 4);
+                }
+            }
+        std::lock_guard<std::mutex> lk(ix->mu);
+        ix->gather_pool.push_back(std::move(gb));
+    }
+    if (st != PB_OK) err = g_err;
+    for (size_t i = 0; i < n; ++i) static_cast<SearchRequest *>(reqs[i])->stats = g_stats;
+    return (int)st;
+}
+
+extern "C" pb_status pb_search(pb_index *ix, const float *query, int64_t n_query_tokens, const pb_search_params *params,
+                               const int64_t *subset, int64_t n_subset, int64_t *out_ids, float *out_scores,
+                               int32_t *out_count) {
+    if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    SearchRequest r;
+    r.query = query, r.n_tokens = n_query_tokens, r.params = params, r.subset = subset, r.n_subset = n_subset;
+    r.out_ids = out_ids, r.out_scores = out_scores, r.out_count = out_count;
+    // a doc-sharded search is a collective, issued in the same order on every rank: never queued
+    if (!ix->coalesce_on || ix->world > 1 || ix->group || ix->comm) {
+        ix->coalescer.count_bypassed();
+        return search_alone(ix, r);
+    }
+    pb_status st;
+    {
+        auto rd = ix->read_lock();
+        st = check_request(ix, r);
+    }
+    if (st != PB_OK) {
+        ix->coalescer.count_refused();
+        return st;
+    }
+    ix->coalescer.submit(r);
+    g_stats = r.stats;
+    if (r.status != 0) g_err = r.error;
+    return (pb_status)r.status;
+}
+
 extern "C" pb_status pb_search_batch(pb_index *ix, const float *queries, const int64_t *q_tok_offsets, int64_t n_queries,
                                      const pb_search_params *params, const int64_t *subset, int64_t n_subset,
                                      int64_t *out_ids, float *out_scores, int32_t *out_counts) {
@@ -3181,6 +3378,7 @@ extern "C" pb_status pb_index_comm_init(pb_index *ix, const uint8_t *id128, int3
     ncclUniqueId id;
     memcpy(id.internal, id128, 128);
     CKN(g_nccl.CommInitRank(&ix->comm, world, id, rank));
+    pb_index_set_coalescing(ix, nullptr);  // a sharded search is a collective: arrival order is not a rank-agreed order
     ix->rank = rank;
     ix->world = world;
     return PB_OK;
@@ -3205,6 +3403,7 @@ extern "C" pb_status pb_index_group_join(pb_index *ix, pb_shard_group *g, int32_
     std::lock_guard<std::mutex> lk(g->mu);
     g->dev[rank] = ix->device;
     ++g->joined;
+    pb_index_set_coalescing(ix, nullptr);  // as pb_index_comm_init
     ix->group = g;
     ix->rank = rank;
     ix->world = g->world;

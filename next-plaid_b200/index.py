@@ -72,6 +72,16 @@ class _Work(C.Structure):
                                          "n_a5_live_rows", "n_a5_dense_docs")]
 
 
+class _CoalesceConfig(C.Structure):
+    _fields_ = [("max_queries", C.c_int32), ("max_wait_us", C.c_int32), ("max_inflight", C.c_int32)]
+
+
+class _CoalesceStats(C.Structure):
+    _fields_ = [("n_requests", C.c_int64), ("n_batches", C.c_int64), ("n_bypassed", C.c_int64),
+                ("n_refused", C.c_int64), ("n_rerun_alone", C.c_int64), ("max_batch", C.c_int64),
+                ("batch_hist", C.c_int64 * 8), ("queue_wait_us", C.c_int64)]
+
+
 EXPORTS = [
     "pb_search_params_default", "pb_index_load", "pb_index_open", "pb_index_close",
     "pb_index_num_documents", "pb_index_num_embeddings", "pb_index_num_partitions",
@@ -89,6 +99,7 @@ EXPORTS = [
     "pb_index_delete", "pb_last_delete_ms", "pb_index_load_range", "pb_index_dir_shard_bounds",
     "pb_index_delete_sharded", "pb_index_append_sharded", "pb_index_append_encoded_sharded",
     "pb_index_rebalance_sharded", "pb_index_load_range_flags", "pb_index_memory", "pb_last_staging_stats",
+    "pb_search", "pb_index_set_coalescing", "pb_index_coalesce_stats",
 ]
 
 PB_OPEN_ADOPT_RESIDUALS, PB_OPEN_HOST_RESIDUALS = 1, 2
@@ -142,6 +153,10 @@ def load_library():
                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                               C.c_void_p]
         L.pb_search_batch_params.argtypes = list(L.pb_search_batch_subsets.argtypes)
+        L.pb_search.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(_Params), C.c_void_p, C.c_int64,
+                                C.c_void_p, C.c_void_p, C.c_void_p]
+        L.pb_index_set_coalescing.argtypes = [C.c_void_p, C.POINTER(_CoalesceConfig)]
+        L.pb_index_coalesce_stats.argtypes = [C.c_void_p, C.POINTER(_CoalesceStats), C.c_int32]
         L.pb_search_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                              C.POINTER(_Params), C.c_void_p, C.c_void_p, C.c_void_p]
         L.pb_centroid_scores.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
@@ -575,10 +590,35 @@ class MmapIndex:
     # -- search ------------------------------------------------------------------------------
     def search(self, query: np.ndarray, params: SearchParameters,
                subset: Optional[Sequence[int]] = None) -> QueryResult:
-        """MmapIndex::search (index.rs:1258)."""
-        r = self.search_batch([query], params, True, subset)[0]
-        r.query_id = 0
-        return r
+        """MmapIndex::search (index.rs:1258), pb_search: one query per call.  The call releases the GIL, so with
+        set_coalescing the searches of concurrent Python threads share batches."""
+        q = np.asarray(query)
+        if q.ndim != 2 or q.shape[1] != self.embedding_dim():
+            raise PlaidError(PB_ERR_INVALID, f"query has shape {q.shape}, expected [tokens, {self.embedding_dim()}]")
+        q = np.ascontiguousarray(q, np.float32)
+        ss = None if subset is None else np.ascontiguousarray(subset, np.int64).reshape(-1)
+        k = max(int(params.top_k), 1)
+        ids, sc, cn = np.zeros(k, np.int64), np.zeros(k, np.float32), C.c_int32()
+        p = params._c()
+        _check(load_library().pb_search(self._h, _ptr(q), q.shape[0], C.byref(p), _ptr(ss),
+                                        0 if ss is None else len(ss), _ptr(ids), _ptr(sc), C.byref(cn)))
+        return QueryResult(0, ids[:cn.value].copy(), sc[:cn.value].copy())
+
+    def set_coalescing(self, max_queries: int, max_wait_us: int = 0, max_inflight: int = 2):
+        """pb_index_set_coalescing: merge the `search` calls of concurrent threads into batches of up to max_queries
+        (1 = off), with at most max_inflight batches running at once; a leader whose batch is short waits up to
+        max_wait_us for more requests (0 = never)."""
+        c = _CoalesceConfig(int(max_queries), int(max_wait_us), int(max_inflight))
+        _check(load_library().pb_index_set_coalescing(self._h, C.byref(c)))
+
+    def coalesce_stats(self, reset: bool = False) -> dict:
+        """pb_index_coalesce_stats: the counters of the handle's request queue (batch_hist: merged batches of size
+        1, 2, 3-4, 5-8, 9-16, 17-32, 33-64, > 64)."""
+        st = _CoalesceStats()
+        _check(load_library().pb_index_coalesce_stats(self._h, C.byref(st), 1 if reset else 0))
+        out = {n: int(getattr(st, n)) for n, _ in _CoalesceStats._fields_ if n != "batch_hist"}
+        out["batch_hist"] = [int(v) for v in st.batch_hist]
+        return out
 
     def search_batch(self, queries: Sequence[np.ndarray], params: SearchParameters,
                      parallel: bool = True, subset: Optional[Sequence[int]] = None,

@@ -38,6 +38,14 @@ impl From<&SearchParameters> for PbSearchParams {
     }
 }
 
+/// `pb_coalesce_config`
+#[repr(C)]
+struct PbCoalesceConfig {
+    max_queries: i32,
+    max_wait_us: i32,
+    max_inflight: i32,
+}
+
 #[link(name = "plaid_b200")]
 extern "C" {
     fn pb_index_load(index_dir: *const c_char, device: i32, out: *mut *mut c_void) -> c_int;
@@ -84,6 +92,18 @@ extern "C" {
         out_counts: *mut i32,
         trace: *mut c_void,
     ) -> c_int;
+    fn pb_search(
+        ix: *mut c_void,
+        query: *const f32,
+        n_query_tokens: i64,
+        params: *const PbSearchParams,
+        subset: *const i64,
+        n_subset: i64,
+        out_ids: *mut i64, // [top_k]
+        out_scores: *mut f32,
+        out_count: *mut i32,
+    ) -> c_int;
+    fn pb_index_set_coalescing(ix: *mut c_void, cfg: *const PbCoalesceConfig) -> c_int;
     fn pb_last_error() -> *const c_char;
     fn pb_codec_open(device: i32, centroids: *const f32, k: i64, dim: i32, nbits: i32, cutoffs: *const f32,
                      out: *mut *mut c_void) -> c_int;
@@ -445,17 +465,49 @@ impl B200Index {
         Ok(deleted as usize)
     }
 
-    /// Body of `MmapIndex::search` (index.rs:1258).
+    /// Body of `MmapIndex::search` (index.rs:1258): `pb_search`, one query per call.  With `set_coalescing` the calls
+    /// of concurrent worker threads share batches inside the library; each gets what it would get alone.
     pub fn search(
         &self,
         query: &Array2<f32>,
         params: &SearchParameters,
         subset: Option<&[i64]>,
     ) -> Result<QueryResult> {
-        let mut r = self.search_batch(std::slice::from_ref(query), params, subset)?;
-        let mut r = r.remove(0);
-        r.query_id = 0;
-        Ok(r)
+        let dim = unsafe { pb_index_embedding_dim(self.handle) } as usize;
+        if query.ncols() != dim {
+            return Err(Error::Shape(format!("query has {} columns, the index embedding_dim is {}", query.ncols(), dim)));
+        }
+        let q = query.as_standard_layout();
+        let k = params.top_k;
+        let mut ids = vec![0i64; k.max(1)];
+        let mut scores = vec![0f32; k.max(1)];
+        let mut count = 0i32;
+        let p = PbSearchParams::from(params);
+        let (sp, sn) = match subset {
+            Some(s) if !s.is_empty() => (s.as_ptr(), s.len() as i64),
+            Some(_) => (std::ptr::NonNull::<i64>::dangling().as_ptr() as *const i64, 0),
+            None => (std::ptr::null(), 0),
+        };
+        let st = unsafe {
+            pb_search(self.handle, q.as_ptr(), q.nrows() as i64, &p, sp, sn, ids.as_mut_ptr(), scores.as_mut_ptr(),
+                      &mut count)
+        };
+        if st != 0 {
+            return Err(Error::Search(last_error()));
+        }
+        let n = count as usize;
+        Ok(QueryResult { query_id: 0, passage_ids: ids[..n].to_vec(), scores: scores[..n].to_vec() })
+    }
+
+    /// `pb_index_set_coalescing`: merge the `search` calls of concurrent threads into batches of up to `max_queries`
+    /// (1 = off), at most `max_inflight` of them running at once; a leader with a short batch waits up to
+    /// `max_wait_us` for more requests.  A server sets this once after `load` (INTEGRATION.md).
+    pub fn set_coalescing(&self, max_queries: i32, max_wait_us: i32, max_inflight: i32) -> Result<()> {
+        let cfg = PbCoalesceConfig { max_queries, max_wait_us, max_inflight };
+        if unsafe { pb_index_set_coalescing(self.handle, &cfg) } != 0 {
+            return Err(Error::Search(last_error()));
+        }
+        Ok(())
     }
 }
 
