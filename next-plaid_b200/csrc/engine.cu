@@ -17,6 +17,7 @@
 #include <condition_variable>
 #include <functional>
 #include <map>
+#include <tuple>
 #include <thread>
 #include <type_traits>
 #include <cstdarg>
@@ -454,6 +455,7 @@ struct pb_index {
     bool a5_prune = true;      // bound the first pass from the live score-table rows (PB_A5_PRUNE=0: dense first pass)
     long long a5_live = -1;    // live rows aimed at per query token (PB_A5_LIVE; -1: K / 512)
     float a5_m1 = 1.25f;       // round 1 of the pruned first pass keeps the M1 = a5_m1 * M best bounds (PB_A5_M1, >= 1)
+    int a5_waves = 8;          // k_a5_bound's grid in waves of resident CTAs, over the batch (PB_A5_WAVES)
     bool probe16 = true;       // a3 threshold-first selection on the 16-bit table (PB_PROBE16=0: per-lane lists only)
     bool fast_exact = true;    // tensor-core certified filter in front of the exact stage (same results either way)
     float vmin = 0.0f;         // smallest pre-normalisation token norm |c + w| over the index (error bound of the filter)
@@ -571,6 +573,25 @@ template <class Kern> static pb_status set_smem(Kern k, size_t bytes) {
         CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
         cur = bytes;
     }
+    return PB_OK;
+}
+
+// CTAs of a kernel that fit one SM at this block size and dynamic shared memory (at least 1), asked of the runtime
+// once per (device, kernel, threads, bytes)
+template <class Kern> static pb_status resident_ctas(Kern k, int threads, size_t smem, int *out) {
+    static std::mutex mu;
+    static std::map<std::tuple<int, const void *, int, size_t>, int> known;
+    int dev = 0;
+    CK(cudaGetDevice(&dev));
+    std::lock_guard<std::mutex> g(mu);
+    const auto key = std::make_tuple(dev, (const void *)k, threads, smem);
+    auto it = known.find(key);
+    if (it == known.end()) {
+        int n = 0;
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k, threads, smem));
+        it = known.emplace(key, std::max(1, n)).first;
+    }
+    *out = it->second;
     return PB_OK;
 }
 
@@ -985,6 +1006,7 @@ pb_status pb_index_finalize(pb_index *ix) {
         if (const char *e = getenv("PB_A5_PRUNE")) ix->a5_prune = atoi(e) != 0;
         if (const char *e = getenv("PB_A5_LIVE")) ix->a5_live = std::max(0ll, atoll(e));
         if (const char *e = getenv("PB_A5_M1")) ix->a5_m1 = std::max(1.0f, (float)atof(e));
+        if (const char *e = getenv("PB_A5_WAVES")) ix->a5_waves = std::max(1, atoi(e));
         if (const char *e = getenv("PB_COALESCE")) {
             pb_coalesce_config c = {atoi(e), 0, 2};
             if (const char *w = getenv("PB_COALESCE_WAIT_US")) c.max_wait_us = std::max(0, atoi(w));
@@ -2233,7 +2255,8 @@ static pb_status approx_scores(pb_index *ix, Workspace &ws, const SearchPlan &pl
             // the bound U of every candidate from the live rows, then k_approx16 on the two rounds that can reach the
             // band (k_approx16.cuh); U lives in ws.approx and the round lists in ws.keys until the re-check overwrites them
             CKS(ws.a5floor.ensure((size_t)B * QS * 4));
-            CKS(ws.a5live.ensure((size_t)B * ((ix->K + 31) / 32) * 4));
+            const long long live_stride = ((ix->K + 31) / 32 + 3) & ~3ll;  // words per query, 16-byte rows
+            CKS(ws.a5live.ensure((size_t)B * live_stride * 4));
             CKS(ws.a5n1.ensure((size_t)B * 4 + 16));
             CKS(ws.a5n12.ensure((size_t)B * 4 + 16));
             CKS(ws.a5theta.ensure((size_t)B * 4 + 16));
@@ -2244,17 +2267,22 @@ static pb_status approx_scores(pb_index *ix, Workspace &ws, const SearchPlan &pl
             k_a5_floor<<<dim3(QS / 8, B), 256, 0, ws.stream>>>(st16, ws.qoff.as<int>(), ix->K, QS, n_live,
                                                                ws.a5floor.as<uint32_t>());
             k_a5_live<<<dim3(ix->sm_count * 2, B), 256, 0, ws.stream>>>(st16, ix->K, QS, ws.a5floor.as<uint32_t>(),
-                                                                         ws.a5live.as<uint32_t>());
-            // the bitmap in shared memory up to K = 2^19 (64 KiB; three CTAs of k_a5_bound<4> still fit an SM), then
-            // 32 CTAs per SM over the batch: few enough that copying it in costs little L2
+                                                                         ws.a5live.as<uint32_t>(), live_stride);
+            // the bitmap in shared memory up to K = 2^19 (64 KiB, two CTAs per SM), then a5_waves waves of resident
+            // CTAs spread over the batch, each a contiguous range of its query's candidates (k_approx16.cuh; the
+            // default of 8 waves is measured in DESIGN.md 4b)
             const auto bound = QS <= 32 ? k_a5_bound<4> : k_a5_bound<8>;
-            const size_t bits_bytes = (size_t)(ix->K + 31) / 32 * 4;
-            const bool bits_in_smem = bits_bytes <= 64 * 1024;
-            if (bits_in_smem) CKS(set_smem(bound, bits_bytes));
-            const dim3 gb = bits_in_smem ? dim3(std::max(1, ix->sm_count * 32 / B), B) : ga;
-            bound<<<gb, 256, bits_in_smem ? bits_bytes : 0, ws.stream>>>(
-                st16, ws.qoff.as<int>(), ix->K, QS, ix->ucodes.as<uint32_t>(), ix->udoc_off.as<long long>(), list, ix->D,
-                list_n, ws.a5floor.as<uint32_t>(), ws.a5live.as<uint32_t>(), bits_in_smem, ub, cnt, cnt + B + 2);
+            const bool bits_in_smem = live_stride * 4 <= 64 * 1024;
+            const size_t smb = a5_bound_smem(live_stride, bits_in_smem);
+            CKS(set_smem(bound, smb));
+            int resident = 1;
+            CKS(resident_ctas(bound, 256, smb, &resident));
+            const long long ctas = (long long)resident * ix->sm_count * ix->a5_waves;
+            const dim3 gb((unsigned)std::max(1ll, (ctas + B - 1) / B), B);
+            bound<<<gb, 256, smb, ws.stream>>>(st16, ws.qoff.as<int>(), ix->K, QS, ix->ucodes.as<uint32_t>(),
+                                               ix->udoc_off.as<long long>(), list, ix->D, list_n,
+                                               ws.a5floor.as<uint32_t>(), ws.a5live.as<uint32_t>(), live_stride,
+                                               bits_in_smem, ub, cnt, cnt + B + 2);
             k_select_u32<<<B, 1024, 0, ws.stream>>>(ub, list_n, M1, 0, ub, list, list_n, ix->D, ws.qoff.as<int>(),
                                                     ws.qflag.as<int>(), rl, n1, ws.a5theta.as<uint32_t>(), nullptr,
                                                     nullptr, nullptr, pass.d_qM1);

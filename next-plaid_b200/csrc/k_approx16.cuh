@@ -260,11 +260,13 @@ k_a5_floor(const unsigned short *__restrict__ ST16, const int *__restrict__ q_of
     if (w < 8 && lane == 0 && q < QS) floor_out[(size_t)b * QS + q] = f;
 }
 
-// live[b][c / 32] bit c % 32: row c has a code >= floor in some real query token.  Every word is written.
+// live[b * stride + c / 32] bit c % 32: row c has a code >= floor in some real query token.  Every word below
+// (K + 31) / 32 is written; stride rounds that up to a multiple of 4 words, so that k_a5_bound can bulk-copy a query's
+// bitmap (16-byte aligned rows).
 // grid = (any, B), 256 threads; a warp takes 32 rows at a time (coalesced 16-byte loads, GQ = QS / 8 <= 8 per row).
 __global__ void __launch_bounds__(256)
 k_a5_live(const unsigned short *__restrict__ ST16, long long K, int QS, const uint32_t *__restrict__ floor_in,
-          uint32_t *__restrict__ live) {
+          uint32_t *__restrict__ live, long long stride) {
     __shared__ uint32_t t2_s[32], m2_s[32];  // packed floors / real-token masks of token pairs (QS <= 64)
     __shared__ uint32_t word_s[8];
     const int b = blockIdx.y, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -298,43 +300,137 @@ k_a5_live(const unsigned short *__restrict__ ST16, long long K, int QS, const ui
             if (h) atomicOr(&word_s[w], 1u << (idx / GQ));
         }
         __syncwarp();
-        if (lane == 0) live[(size_t)b * n_words + wd] = word_s[w];
+        if (lane == 0) live[(size_t)b * stride + wd] = word_s[w];
         __syncwarp();
     }
 }
 
-// U(d) of every candidate (bound above), one warp per doc as in k_approx16.  The kernel is latency-bound (a doc's
-// chain is cand -> offsets -> codes -> live bits -> rows), so the next doc's offsets are prefetched and up to 256 codes
-// are loaded at once; their live ones are compacted into a per-warp buffer and gathered with k_approx16's row groups,
-// 32 rows per round of independent loads.  QS <= 8 * LPR: one column pass.  Counts the doc codes read (tok_counter)
-// and the rows gathered (live_counter).  bits_in_smem: the query's bitmap is copied to dynamic shared memory first
-// (K / 8 bytes; 32 random bit tests from L1 cost up to 32 wavefronts, from shared memory about 4).
+// U(d) of every candidate (bound above).  Each warp streams its docs' distinct-code lists into its own ring of shared
+// memory slots with TMA 1-D bulk copies, PB_A5_SPW slots ahead of the doc it bounds.  (The one-warp-per-doc form loaded
+// the codes itself and waited on HBM latency for every doc: cand -> offsets -> codes -> live bits -> rows.)
+//   CTA (x, b): the contiguous range [lo, hi) = [n x / X, n (x + 1) / X) of query b's candidate list (ascending doc ids,
+//   so the code lists are read in ascending address order).  Warp w bounds docs lo + w, lo + w + 8, ...
+//   Offsets: the warp loads 32 of its docs' candidate ids and udoc_off pairs at once (one doc per lane), the next 32
+//   while it works through these.
+//   Staging: lane 0 issues one cp.async.bulk per slot of PB_A5_SLOT codes (1 KiB), the warp's chunk sequence being its
+//   docs' lists in order, each cut into slots (a list longer than a slot -- more than 256 distinct codes, or a doc
+//   above PB_UCODE_MAX tokens with its raw list -- fills consecutive slots).  A slot holds its size word (codes, bit 31
+//   = the doc's last slot) and a full mbarrier, armed with expect_tx and completed by the copy's bytes.  The warp
+//   refills a slot as soon as it has read it, so no other warp's pace holds it up (a producer warp feeding all eight,
+//   one lane per consumer, reconverged after every wait and so waited on the slowest of them: DESIGN.md 4b).
+//   Bounding, per slot: the live test against the bitmap, the ballot compaction into the warp's buffer, then the
+//   gather of those rows with k_approx16's row groups, 32 rows per round of independent loads.  QS <= 8 * LPR: one
+//   column pass.  The packed maxima start at the dead-row floor f_q - 1 and are summed over the real tokens.
+// Bulk-copy condition: source 16-byte aligned, size a multiple of 16.  Every list satisfies it because k_unique_codes
+// pads lists to a multiple of 8 codes and udoc_off is the scan of those padded lengths from 0 -- at index open, on
+// append (new lists start at the old total), after delete (whole lists compacted, offsets rescanned) and after a
+// rebalance (offsets scanned from the arrived padded lengths) -- so a list starts 32-byte aligned and every slot of it
+// is a multiple of 32 bytes.
+// Counts the doc codes read (tok_counter) and the rows gathered (live_counter), as the dense pass does.
+// bits_in_smem: the query's bitmap (live_stride words, a multiple of 4) is bulk-copied into shared memory at CTA start
+// (K <= 2^19: up to 64 KiB); for larger K the bits are tested from global memory through L1.
+// Dynamic shared memory: a5_bound_smem().
+#define PB_A5_SLOT 256  // codes per ring slot (1 KiB): an average list (~212 distinct codes at 300 tokens) fits one
+#define PB_A5_SPW 4     // ring slots per warp: 32 KiB of codes in flight per CTA
+constexpr int PB_A5_RING = 8 * PB_A5_SPW;
+// shared-memory layout: ring [PB_A5_RING][PB_A5_SLOT] u32, live buffers [8][PB_A5_SLOT] u32, slot sizes [PB_A5_RING] u32,
+// full mbarriers [PB_A5_RING] + the bitmap's, then the bitmap from PB_A5_BITS_AT (16-byte aligned for its bulk copy)
+constexpr size_t PB_A5_BITS_AT = 41 * 1024;
+static_assert((size_t)(PB_A5_RING + 8) * PB_A5_SLOT * 4 + PB_A5_RING * 4 + (PB_A5_RING + 1) * 8 <= PB_A5_BITS_AT,
+              "k_a5_bound: ring, buffers, sizes and mbarriers overrun the bitmap");
+static_assert(PB_A5_BITS_AT % 16 == 0 && (PB_A5_RING * PB_A5_SLOT * 4 + 8 * PB_A5_SLOT * 4 + PB_A5_RING * 4) % 8 == 0,
+              "k_a5_bound: misaligned shared-memory layout");
+static inline size_t a5_bound_smem(long long live_stride, bool bits_in_smem) {
+    return PB_A5_BITS_AT + (bits_in_smem ? (size_t)live_stride * 4 : 0);
+}
 template <int LPR>
-__global__ void __launch_bounds__(256, LPR == 4 ? 3 : 2)  // (4 CTAs of LPR = 4 would spill)
+__global__ void __launch_bounds__(256, LPR == 4 ? 3 : 2)  // (sm_90a: 80 / 112 registers, no spills)
 k_a5_bound(const unsigned short *__restrict__ ST16, const int *__restrict__ q_off, long long K, int QS,
            const uint32_t *__restrict__ ucodes, const long long *__restrict__ udoc_off,
            const uint32_t *__restrict__ cand, long long cand_cap, const int *__restrict__ n_cand,
-           const uint32_t *__restrict__ floor_in, const uint32_t *__restrict__ live, bool bits_in_smem,
-           uint32_t *__restrict__ ubound, unsigned long long *__restrict__ tok_counter,
+           const uint32_t *__restrict__ floor_in, const uint32_t *__restrict__ live, long long live_stride,
+           bool bits_in_smem, uint32_t *__restrict__ ubound, unsigned long long *__restrict__ tok_counter,
            unsigned long long *__restrict__ live_counter) {
     constexpr int RG = 32 / LPR;  // rows per load instruction
     constexpr int NE = 32 / RG;   // load instructions per round of 32 rows
-    __shared__ uint32_t buf_s[8][256];
-    extern __shared__ uint32_t bits_s[];
-    const int b = blockIdx.y, w = threadIdx.x >> 5;
+    extern __shared__ __align__(128) unsigned char smem_a5[];
+    uint32_t *ring = reinterpret_cast<uint32_t *>(smem_a5);  // [PB_A5_RING][PB_A5_SLOT]
+    uint32_t *bufs = ring + PB_A5_RING * PB_A5_SLOT;           // [8][PB_A5_SLOT]
+    uint32_t *slot_n = bufs + 8 * PB_A5_SLOT;                  // [PB_A5_RING]
+    uint64_t *full = reinterpret_cast<uint64_t *>(slot_n + PB_A5_RING), *bits_bar = full + PB_A5_RING;
+    uint32_t *bits_s = reinterpret_cast<uint32_t *>(smem_a5 + PB_A5_BITS_AT);
+    const int b = blockIdx.y, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long long n = n_cand[b];
+    const int lo = (int)(n * blockIdx.x / gridDim.x), hi = (int)(n * (blockIdx.x + 1) / gridDim.x);
+    if (lo >= hi) return;  // (the whole CTA)
+    const uint32_t *liveb = live + (size_t)b * live_stride;
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < PB_A5_RING; ++s) mbar_init(&full[s], 1);
+        mbar_init(bits_bar, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    if (bits_in_smem && threadIdx.x == 0) {
+        mbar_expect_tx(bits_bar, (uint32_t)live_stride * 4u);
+        bulk_g2s(bits_s, liveb, (uint32_t)live_stride * 4u, bits_bar);
+    }
+
+    // ---- this warp's docs j = lo + w + 8 k, k < nd, and their staging ----
+    const int nd = hi - lo > w ? (hi - lo - w + 7) / 8 : 0;
+    const uint32_t *cl = cand + (size_t)b * cand_cap + lo + w;
+    long long ta = 0, tb = 0, na = 0, nb = 0;  // lane l: offsets of doc k = 32 p + l (this batch) and of the next batch
+    if (lane < nd) {
+        const uint32_t d = cl[8 * lane];
+        ta = udoc_off[d];
+        tb = udoc_off[d + 1];
+    }
+    if (32 + lane < nd) {
+        const uint32_t d = cl[8 * (32 + lane)];
+        na = udoc_off[d];
+        nb = udoc_off[d + 1];
+    }
+    // the fill position (warp-uniform): doc fk, codes [ft, fe) of it still to stage; slots issued / consumed so far
+    int fk = 0;
+    long long ft = (long long)shfl_u64((u64)ta, 0), fe = (long long)shfl_u64((u64)tb, 0);
+    uint32_t issued = 0, seq = 0;
+    auto stage = [&]() {
+        while (fk < nd && issued - seq < PB_A5_SPW) {
+            const int nc = (int)min((long long)PB_A5_SLOT, fe - ft);
+            const int s = w * PB_A5_SPW + (int)(issued % PB_A5_SPW);
+            if (lane == 0) {
+                slot_n[s] = (uint32_t)nc | (ft + nc >= fe ? 0x80000000u : 0u);
+                if (nc > 0) {
+                    mbar_expect_tx(&full[s], (uint32_t)nc * 4u);
+                    bulk_g2s(ring + s * PB_A5_SLOT, ucodes + ft, (uint32_t)nc * 4u, &full[s]);
+                } else
+                    mbar_arrive(&full[s]);  // (an empty list: no codes, the bound is the dead-row floor)
+            }
+            ++issued;
+            ft += nc;
+            if (ft >= fe && ++fk < nd) {
+                if ((fk & 31) == 0) {  // the next batch of offsets becomes current; load the one after it
+                    ta = na;
+                    tb = nb;
+                    na = nb = 0;
+                    if (fk + 32 + lane < nd) {
+                        const uint32_t d = cl[8 * (fk + 32 + lane)];
+                        na = udoc_off[d];
+                        nb = udoc_off[d + 1];
+                    }
+                }
+                ft = (long long)shfl_u64((u64)ta, fk & 31);
+                fe = (long long)shfl_u64((u64)tb, fk & 31);
+            }
+        }
+    };
+    stage();
+
     const int nq = q_off[b + 1] - q_off[b];
-    const int n = n_cand[b];
-    const int lane = threadIdx.x & 31, r = lane / LPR, sl = lane % LPR;
-    const int warps_per_grid = gridDim.x * (blockDim.x >> 5);
+    const int r = lane / LPR, sl = lane % LPR;
     const bool in_row = 8 * sl < QS;
     const char *col = reinterpret_cast<const char *>(ST16 + (size_t)b * K * QS) + (in_row ? 16 * sl : 0);
     const unsigned rowb = (unsigned)QS * 2u;
-    const uint32_t *liveb = live + (size_t)b * ((K + 31) / 32);
-    if (bits_in_smem) {
-        for (long long k = threadIdx.x; k < (K + 31) / 32; k += blockDim.x) bits_s[k] = liveb[k];
-        __syncthreads();
-    }
-    uint32_t *buf = buf_s[w];
+    uint32_t *buf = bufs + w * PB_A5_SLOT;
     // this lane's dead-row maxima f_q - 1 (0 for f_q = 0), packed as the maxima are
     uint32_t dm[4] = {0u, 0u, 0u, 0u};
     if (in_row)
@@ -343,42 +439,36 @@ k_a5_bound(const unsigned short *__restrict__ ST16, const int *__restrict__ q_of
             const uint32_t f = floor_in[(size_t)b * QS + 8 * sl + j];
             dm[j >> 1] |= (f ? min(f - 1u, 65535u) : 0u) << (16 * (j & 1));
         }
+    if (bits_in_smem) mbar_wait(bits_bar, 0u);
     unsigned long long my_tokens = 0, my_live = 0;
-    int i = blockIdx.x * (blockDim.x >> 5) + w;
-    long long t0 = 0, t1 = 0;
-    if (i < n) {
-        const uint32_t d = cand[(size_t)b * cand_cap + i];
-        t0 = udoc_off[d];
-        t1 = udoc_off[d + 1];
-    }
-    for (; i < n; i += warps_per_grid) {
-        const int i2 = i + warps_per_grid;
-        long long t0n = 0, t1n = 0;
-        if (i2 < n) {
-            const uint32_t dn = cand[(size_t)b * cand_cap + i2];
-            t0n = udoc_off[dn];
-            t1n = udoc_off[dn + 1];
-        }
-        my_tokens += (unsigned long long)(t1 - t0);
+    for (int k = 0; k < nd; ++k) {
         uint32_t m0 = dm[0], m1 = dm[1], m2 = dm[2], m3 = dm[3];
-        for (long long tb = t0; tb < t1; tb += 256) {
-            uint32_t cc[8];
+        bool last;
+        do {
+            const int s = w * PB_A5_SPW + (int)(seq % PB_A5_SPW);
+            mbar_wait(&full[s], (seq / PB_A5_SPW) & 1u);
+            const uint32_t sz = slot_n[s];
+            const int nc = (int)(sz & 0xffffu);
+            last = (sz >> 31) != 0u;
+            const uint32_t *codes = ring + s * PB_A5_SLOT;
+            uint32_t cc[PB_A5_SLOT / 32];
 #pragma unroll
-            for (int k = 0; k < 8; ++k) {
-                const long long t = tb + 32 * k + lane;
-                cc[k] = t < t1 ? ucodes[t] : 0u;
-            }
+            for (int j = 0; j < PB_A5_SLOT / 32; ++j) cc[j] = 32 * j + lane < nc ? codes[32 * j + lane] : 0u;
             int cnt = 0;
 #pragma unroll
-            for (int k = 0; k < 8; ++k) {
-                const uint32_t c = cc[k];
+            for (int j = 0; j < PB_A5_SLOT / 32; ++j) {
+                const uint32_t c = cc[j];
                 const uint32_t word = bits_in_smem ? bits_s[c >> 5] : __ldg(liveb + (c >> 5));
-                const bool lv = tb + 32 * k + lane < t1 && ((word >> (c & 31)) & 1u);
+                const bool lv = 32 * j + lane < nc && ((word >> (c & 31)) & 1u);
                 const unsigned bal = __ballot_sync(PB_FULL, lv);
                 if (lv) buf[cnt + __popc(bal & ((1u << lane) - 1u))] = c;
                 cnt += __popc(bal);
             }
             __syncwarp();
+            ++seq;
+            // the slot is read: order those reads before the copy that refills it (async proxy), then refill
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            stage();
             for (int base = 0; base < cnt; base += 32) {
                 uint4 v[NE];
 #pragma unroll
@@ -394,9 +484,10 @@ k_a5_bound(const unsigned short *__restrict__ ST16, const int *__restrict__ q_of
                         m3 = __vmaxu2(m3, v[e].w);
                     }
             }
+            my_tokens += (unsigned long long)nc;
             my_live += (unsigned long long)cnt;
             __syncwarp();
-        }
+        } while (!last);
 #pragma unroll
         for (int m = LPR; m < 32; m <<= 1) {
             m0 = __vmaxu2(m0, __shfl_xor_sync(PB_FULL, m0, m));
@@ -415,9 +506,7 @@ k_a5_bound(const unsigned short *__restrict__ ST16, const int *__restrict__ q_of
             }
         }
         const uint32_t total = __reduce_add_sync(PB_FULL, part);
-        if (lane == 0) ubound[(size_t)b * cand_cap + i] = total;
-        t0 = t0n;
-        t1 = t1n;
+        if (lane == 0) ubound[(size_t)b * cand_cap + lo + w + 8 * k] = total;
     }
     if (lane == 0) {
         if (my_tokens) atomicAdd(tok_counter, my_tokens);

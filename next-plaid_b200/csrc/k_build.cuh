@@ -216,32 +216,7 @@ __global__ void k_gather_rows(const float *__restrict__ X, const long long *__re
 #define PB_TC_N 128
 #define PB_TC_STAGES 3
 
-PB_DEV uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-PB_DEV void mbar_init(uint64_t *bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-PB_DEV void mbar_arrive(uint64_t *bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-PB_DEV void mbar_wait(uint64_t *bar, uint32_t parity) {
-    uint32_t done = 0;
-    const uint32_t a = smem_u32(bar);
-    do {
-        asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}\n"
-                     : "=r"(done)
-                     : "r"(a), "r"(parity)
-                     : "memory");
-    } while (!done);
-}
-PB_DEV void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-// TMA 1-D bulk copy global -> shared, completion counted in bytes on an mbarrier
-PB_DEV void bulk_g2s(void *smem_dst, const void *gsrc, uint32_t bytes, uint64_t *bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
+// (smem_u32, the mbarrier helpers and bulk_g2s are in common.cuh)
 // ---- Hopper warpgroup MMA (wgmma) ----
 // The 128 threads of a warpgroup issue one m64nNk16 product together (fp16 operands from shared memory, fp32
 // accumulator in registers).  Fragment of thread t of the warpgroup: d[4i + 2h + j] = element (row 16 (t/32) +
