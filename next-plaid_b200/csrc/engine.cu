@@ -12,6 +12,7 @@
 #include <cub/device/device_select.cuh>
 
 #include <algorithm>
+#include <array>
 #include <chrono>
 #include <cmath>
 #include <condition_variable>
@@ -432,16 +433,35 @@ struct GatherBuf {  // host scratch of one merged batch: the arguments of its pb
     std::vector<int32_t> counts;
 };
 
-struct pb_index {
+// The totals of an index's documents.  Open derives them; append, delete and rebalance prepare new ones and publish
+// them in one place (publish), so that the handle equals a fresh open of its documents.
+struct DocTotals {
+    long long D = 0, N = 0, ivf_len = 0, n_ucodes = 0;
+    int max_doclen = 0;
+    float vmin = 0.0f;  // smallest pre-normalisation token norm |c + w| over the index (error bound of the filter)
+    float wmax = 0.0f;  // largest residual norm |w| over the index (same)
+};
+
+// The arrays derived from an index's documents, with their totals
+struct DocArrays : DocTotals {
+    DevBuf codes, residuals, doc_off, ucodes, udoc_off, ivf, ivf_off;
+    DevBuf tok_inv_norm;               // [N] 1 / |c + w| for the linear estimate (k_maxsim_tc)
+    DevBuf ivf_spare, ivf_off_spare;   // the other half of the inverted file's ping-pong: append / delete write into it
+    // every buffer, in one list (the memory count and the rebalance's swap walk it)
+    template <class A> static auto buffers(A &a) {
+        return std::array{&a.codes, &a.residuals, &a.doc_off, &a.ucodes, &a.udoc_off, &a.ivf,
+                          &a.ivf_off, &a.tok_inv_norm, &a.ivf_spare, &a.ivf_off_spare};
+    }
+};
+
+struct pb_index : DocArrays {
     int device = 0;
     int dim = 0, nbits = 0, packed = 0;
-    long long K = 0, D = 0, N = 0, ivf_len = 0, doc_id_base = 0;
-    int max_doclen = 0;
+    long long K = 0, doc_id_base = 0;
     int sm_count = 132;
-    DevBuf centroids, w_rev, codes, residuals, doc_off, ivf, ivf_off, ucodes, udoc_off;
+    DevBuf centroids, w_rev;
     bool host_tier = false;    // PB_OPEN_HOST_RESIDUALS: `residuals` stays empty, the rows live in host_res
     PinnedRes host_res;
-    long long n_ucodes = 0;
     bool build_ivf = false;    // no inverted file was given: built from the codes at finalize (index.rs:850-873)
     float cmax = 1.0f;         // largest centroid L2 norm (range of the 16-bit score table)
     bool fast_approx = true;   // two-pass approximate stage (exact cut either way)
@@ -458,9 +478,6 @@ struct pb_index {
     int a5_waves = 8;          // k_a5_bound's grid in waves of resident CTAs, over the batch (PB_A5_WAVES)
     bool probe16 = true;       // a3 threshold-first selection on the 16-bit table (PB_PROBE16=0: per-lane lists only)
     bool fast_exact = true;    // tensor-core certified filter in front of the exact stage (same results either way)
-    float vmin = 0.0f;         // smallest pre-normalisation token norm |c + w| over the index (error bound of the filter)
-    float wmax = 0.0f;         // largest residual norm |w| over the index (same)
-    DevBuf tok_inv_norm;       // [N] 1 / |c + w| for the linear estimate (k_maxsim_tc)
     bool filter_diag = false;  // PB_FILTER_DIAG=1: score every kept doc exactly and measure the filter's estimate against it
     bool pair_exact = true;    // exact stage on the (token, query token) pairs that can hold a maximum (PB_PAIR_EXACT=0: k_exact)
     int ws_grid = 8;           // k_maxsim_tc CTAs per SM across the batch (PB_WS_GRID)
@@ -479,7 +496,6 @@ struct pb_index {
     pbq::Queue<CoalescedRun> coalescer{CoalescedRun{this}, PB_ERR_CUDA};
     std::atomic<bool> coalesce_on{false};
     std::vector<std::unique_ptr<GatherBuf>> gather_pool;  // under mu
-    DevBuf ivf_spare, ivf_off_spare;  // the other half of the inverted file's ping-pong: pb_index_append merges into it
     float delete_ms[3] = {0.f, 0.f, 0.f};  // last pb_index_delete with profiling on: compaction, inverted file, norms
     long long delete_window = 1ll << 22;   // tokens per compaction window of pb_index_delete (PB_DELETE_WINDOW_TOKENS)
     // Readers (searches, stage entry points, accessors) share the arrays; pb_index_append / pb_index_reserve hold them
@@ -491,22 +507,43 @@ struct pb_index {
         { std::lock_guard<std::mutex> g(gate); }
         return std::shared_lock<std::shared_mutex>(rw);
     }
+};
 
-    pb_status acquire(std::unique_ptr<Workspace> &ws) {
+// A workspace of the handle's pool for one call.  It goes back to the pool only after a call that ran to completion
+// (done): its scratch invariants (cleared bitmaps, zeroed maxima) are restored by the kernels themselves, so a call
+// that fails half way must not hand its buffers to the next caller; its workspace is synchronized and dropped.
+struct WorkspaceLease {
+    pb_index *ix;
+    std::unique_ptr<Workspace> ws;
+    bool done = false;
+    pb_status acquire() {
         {
-            std::lock_guard<std::mutex> g(mu);
-            if (!pool.empty()) {
-                ws = std::move(pool.back());
-                pool.pop_back();
+            std::lock_guard<std::mutex> g(ix->mu);
+            if (!ix->pool.empty()) {
+                ws = std::move(ix->pool.back());
+                ix->pool.pop_back();
                 return PB_OK;
             }
         }
         ws.reset(new Workspace());
         return ws->init();
     }
-    void release(std::unique_ptr<Workspace> &ws) {
-        std::lock_guard<std::mutex> g(mu);
-        pool.push_back(std::move(ws));
+    ~WorkspaceLease() {
+        if (!ws) return;
+        if (done) {
+            std::lock_guard<std::mutex> g(ix->mu);
+            ix->pool.push_back(std::move(ws));
+        } else {
+            cudaStreamSynchronize(ws->stream);
+        }
+    }
+};
+
+// a non-blocking stream of one collective call, destroyed with it
+struct OwnedStream {
+    cudaStream_t s = nullptr;
+    ~OwnedStream() {
+        if (s) cudaStreamDestroy(s);
     }
 };
 
@@ -780,6 +817,25 @@ pb_status pb_index_upload_tokens(pb_index *ix, long long tok_off, const int64_t 
     return upload_narrow(ix->codes, tok_off, codes, n, ix->K, space, "codes");
 }
 
+// The offsets of docs of lengths dl starting at token t0 (off[0] = t0, dl.size() + 1 of them); the longest doc is
+// folded into *maxlen.  A length outside [0, 2^30] fails.
+static pb_status doc_offsets(const std::vector<int64_t> &dl, long long t0, std::vector<long long> &off, int *maxlen) {
+    off.assign(dl.size() + 1, t0);
+    for (size_t i = 0; i < dl.size(); ++i) {
+        if (dl[i] < 0 || dl[i] > (1 << 30)) return pb_fail(PB_ERR_INVALID, "doc_lengths[%zu] = %lld", i, (long long)dl[i]);
+        off[i + 1] = off[i] + dl[i];
+        *maxlen = std::max<int>(*maxlen, (int)dl[i]);
+    }
+    return PB_OK;
+}
+
+// the longest of the D docs at host offsets off
+static int longest_doc(const std::vector<long long> &off, long long D) {
+    int m = 0;
+    for (long long j = 0; j < D; ++j) m = std::max<int>(m, (int)(off[j + 1] - off[j]));
+    return m;
+}
+
 // Everything except the per-token arrays (d->codes / d->residuals may be NULL here).
 pb_status pb_index_open_begin(const pb_index_desc *d, pb_index **out) {
     if (!d || !out) return pb_fail(PB_ERR_INVALID, "null argument");
@@ -824,16 +880,10 @@ pb_status pb_index_open_begin(const pb_index_desc *d, pb_index **out) {
     // doc offsets (index.rs:1107-1110)
     std::vector<int64_t> dl;
     CKS(fetch_host(dl, d->doc_lengths, (size_t)ix->D, sp));
-    std::vector<long long> doff((size_t)ix->D + 1, 0);
-    int maxlen = 0;
-    for (long long i = 0; i < ix->D; ++i) {
-        if (dl[i] < 0 || dl[i] > (1 << 30)) return pb_fail(PB_ERR_INVALID, "doc_lengths[%lld] = %lld", i, (long long)dl[i]);
-        doff[i + 1] = doff[i] + dl[i];
-        maxlen = std::max<int>(maxlen, (int)dl[i]);
-    }
+    std::vector<long long> doff;
+    CKS(doc_offsets(dl, 0, doff, &ix->max_doclen));
     if (doff[ix->D] != ix->N)
         return pb_fail(PB_ERR_INVALID, "sum(doc_lengths)=%lld != num_embeddings=%lld", doff[ix->D], ix->N);
-    ix->max_doclen = maxlen;
     CKS(upload(ix->doc_off, doff.data(), doff.size() * 8, PB_MEM_HOST));
     // ivf offsets (index.rs:1089-1094); without an inverted file it is built from the codes in pb_index_finalize
     ix->build_ivf = d->ivf_lengths == nullptr;
@@ -947,41 +997,72 @@ static pb_status launch_min_vnorm(pb_index *ix, const uint32_t *codes, const uin
         return PB_OK;
     });
 }
-// the same for the handle's tokens [t0, t0 + n), into its tok_inv_norm.  A host-tier handle's rows go through a device
-// buffer in slabs of 2^22 tokens; the per-token values and the folded min / max do not depend on the slabs, so they are
-// bit-identical to a resident open's (the filter's certificate rests on them)
-static pb_status launch_min_vnorm(pb_index *ix, long long t0, long long n, float *mn) {
-    if (!ix->host_tier)
-        return launch_min_vnorm(ix, ix->codes.as<uint32_t>() + t0, ix->residuals.as<uint8_t>() + (size_t)t0 * ix->packed, n,
-                                ix->tok_inv_norm.as<float>() + t0, mn);
-    const long long slab = 1ll << 22;
-    DevBuf st;
-    CKS(st.ensure((size_t)std::min(n, slab) * ix->packed + 16));
-    for (long long o = t0; o < t0 + n; o += slab) {
-        const long long m = std::min(slab, t0 + n - o);
-        CK(cudaMemcpy(st.p, ix->host_res.p + (size_t)o * ix->packed, (size_t)m * ix->packed, cudaMemcpyHostToDevice));
-        CKS(launch_min_vnorm(ix, ix->codes.as<uint32_t>() + o, st.as<uint8_t>(), m, ix->tok_inv_norm.as<float>() + o, mn));
+// The filter's token norms of tokens [t0, t.N) of `a` (the handle's arrays, or a rebalance's new ones), at the
+// tensor-core widths: 1 / |c + w| into a.tok_inv_norm, and into t.vmin / t.wmax the least |c + w| and the largest |w|
+// over those tokens and the seed (0 / 0 over nothing).  An append seeds with the handle's values; open, delete and
+// rebalance, which cover every token, with {3e38, 0}.  A handle that had no tokens gets its centroid operands first.
+// A host-tier handle's rows go through a device buffer in slabs of 2^22 tokens; the per-token values and the folded
+// min / max do not depend on the slabs, so they are bit-identical to a resident open's (the filter's certificate rests
+// on them).  mn: 8 bytes of scratch.
+static pb_status token_norms(pb_index *ix, DocArrays &a, long long t0, const float seed[2], DocTotals &t, DevBuf &mn) {
+    float got[2] = {seed[0], seed[1]};
+    if (TcDims::has(ix->dim) && t.N > 0) {
+        if (ix->N == 0) CKS(build_centroid_operands(ix));
+        const long long n = t.N - t0, slab = ix->host_tier ? 1ll << 22 : std::max(n, 1ll);
+        DevBuf st;
+        if (ix->host_tier) CKS(st.ensure((size_t)std::min(n, slab) * ix->packed + 16));
+        CKS(mn.ensure(16));
+        CK(cudaMemcpy(mn.p, seed, 8, cudaMemcpyHostToDevice));
+        for (long long o = t0; o < t.N; o += slab) {
+            const long long m = std::min(slab, t.N - o);
+            const uint8_t *res = st.as<uint8_t>();
+            if (ix->host_tier)
+                CK(cudaMemcpy(st.p, ix->host_res.p + (size_t)o * ix->packed, (size_t)m * ix->packed, cudaMemcpyHostToDevice));
+            else
+                res = a.residuals.as<uint8_t>() + (size_t)o * ix->packed;
+            CKS(launch_min_vnorm(ix, a.codes.as<uint32_t>() + o, res, m, a.tok_inv_norm.as<float>() + o, mn.as<float>()));
+        }
+        CK(cudaMemcpy(got, mn.p, 8, cudaMemcpyDeviceToHost));
     }
-    CK(cudaDeviceSynchronize());
+    t.vmin = got[0] < 1e30f ? got[0] : 0.0f;
+    t.wmax = got[1];
     return PB_OK;
 }
 
-// Derived arrays that need every token: the per-doc distinct-code lists k_approx walks.
+// The distinct-code lists k_approx walks, of docs [d0, d0 + n) of the handle, after the u0 entries of the docs before
+// them: a count pass, the offsets on the host into udoc_off [d0, d0 + n] (udoc_off holds d0 + n + 1 entries, absolute
+// positions into ucodes), then the lists into ucodes.  ucodes is sized as a first allocation is, or grows keeping its
+// first u0 entries.  The new entry count goes to *u1.
+static pb_status unique_codes(pb_index *ix, long long d0, long long n, long long u0, long long *u1) {
+    std::vector<long long> uoff((size_t)n + 1, u0);
+    const int blocks = (int)std::min<long long>(n, (long long)ix->sm_count * 16);
+    if (n > 0) {
+        DevBuf counts;
+        CKS(counts.ensure((size_t)n * 4));
+        k_unique_codes<<<blocks, 128>>>(ix->codes.as<uint32_t>(), ix->doc_off.as<long long>() + d0, n, nullptr, nullptr,
+                                        counts.as<int>());
+        CK(cudaGetLastError());
+        std::vector<int> hc((size_t)n);
+        CK(cudaMemcpy(hc.data(), counts.p, hc.size() * 4, cudaMemcpyDeviceToHost));
+        for (long long i = 0; i < n; ++i) uoff[i + 1] = uoff[i] + hc[i];
+    }
+    *u1 = uoff[n];
+    const size_t bytes = std::max<size_t>((size_t)*u1 * 4, 16);
+    CKS(ix->ucodes.p ? ix->ucodes.grow(bytes, (size_t)u0 * 4) : ix->ucodes.ensure(bytes));
+    CK(cudaMemcpy(ix->udoc_off.as<long long>() + d0, uoff.data(), uoff.size() * 8, cudaMemcpyHostToDevice));
+    if (n > 0) {
+        k_unique_codes<<<blocks, 128>>>(ix->codes.as<uint32_t>(), ix->doc_off.as<long long>() + d0, n,
+                                        ix->udoc_off.as<long long>() + d0, ix->ucodes.as<uint32_t>(), nullptr);
+        CK(cudaGetLastError());
+    }
+    return PB_OK;
+}
+
+// Derived arrays that need every token: the per-doc distinct-code lists, the token norms, and the inverted file of an
+// index opened without one.
 pb_status pb_index_finalize(pb_index *ix) {
     CK(cudaSetDevice(ix->device));
     if ((unsigned long long)ix->K * 1024ull * 4ull >= (1ull << 40)) return pb_fail(PB_ERR_UNSUPPORTED, "K too large");
-    std::vector<long long> uoff((size_t)ix->D + 1, 0);
-    if (ix->D > 0) {
-        DevBuf counts;
-        CKS(counts.ensure((size_t)ix->D * 4));
-        const int blocks = (int)std::min<long long>(ix->D, (long long)ix->sm_count * 16);
-        k_unique_codes<<<blocks, 128>>>(ix->codes.as<uint32_t>(), ix->doc_off.as<long long>(), ix->D, nullptr, nullptr,
-                                        counts.as<int>());
-        CK(cudaGetLastError());
-        std::vector<int> hc((size_t)ix->D);
-        CK(cudaMemcpy(hc.data(), counts.p, hc.size() * 4, cudaMemcpyDeviceToHost));
-        for (long long i = 0; i < ix->D; ++i) uoff[i + 1] = uoff[i] + hc[i];
-    }
     {
         DevBuf mx;
         CKS(mx.ensure(16));
@@ -1015,30 +1096,17 @@ pb_status pb_index_finalize(pb_index *ix) {
             CKS(pb_index_set_coalescing(ix, &c));
         }
     }
-    if (TcDims::has(ix->dim) && ix->N > 0 && ix->K > 0) {
+    if (TcDims::has(ix->dim) && ix->N > 0) {
         // operands of the tensor-core score table, and the token norms of the filter
         CKS(build_centroid_operands(ix));
+        CKS(ix->tok_inv_norm.ensure((size_t)ix->N * 4));
         DevBuf mn;
-        CKS(mn.ensure(16));
-        CKS(ix->tok_inv_norm.ensure((size_t)ix->N * 4));  // 1 / |c + w| per token: operand of the linear estimate (k_maxsim_tc)
-        const float init[2] = {3.0e38f, 0.0f};
-        CK(cudaMemcpy(mn.p, init, 8, cudaMemcpyHostToDevice));
-        CKS(launch_min_vnorm(ix, 0, ix->N, mn.as<float>()));
-        float got[2] = {0.f, 0.f};
-        CK(cudaMemcpy(got, mn.p, 8, cudaMemcpyDeviceToHost));
-        ix->vmin = got[0] < 1e30f ? got[0] : 0.0f;
-        ix->wmax = got[1];
+        const float seed[2] = {3.0e38f, 0.0f};
+        CKS(token_norms(ix, *ix, 0, seed, *ix, mn));
     }
-    ix->n_ucodes = uoff[ix->D];
-    CKS(upload(ix->udoc_off, uoff.data(), uoff.size() * 8, PB_MEM_HOST));
-    CKS(ix->ucodes.ensure(std::max<size_t>((size_t)ix->n_ucodes * 4, 16)));
-    if (ix->D > 0) {
-        const int blocks = (int)std::min<long long>(ix->D, (long long)ix->sm_count * 16);
-        k_unique_codes<<<blocks, 128>>>(ix->codes.as<uint32_t>(), ix->doc_off.as<long long>(), ix->D,
-                                        ix->udoc_off.as<long long>(), ix->ucodes.as<uint32_t>(), nullptr);
-        CK(cudaGetLastError());
-        CK(cudaDeviceSynchronize());
-    }
+    CKS(ix->udoc_off.ensure(std::max<size_t>((size_t)(ix->D + 1) * 8, 16)));
+    CKS(unique_codes(ix, 0, ix->D, 0, &ix->n_ucodes));
+    CK(cudaDeviceSynchronize());
     if (ix->build_ivf) CKS(build_ivf_on_device(ix));
     return PB_OK;
 }
@@ -1109,10 +1177,8 @@ extern "C" int32_t pb_index_device(const pb_index *ix) { return ix ? ix->device 
 extern "C" pb_status pb_index_memory(const pb_index *ix, int64_t *device_bytes, int64_t *host_bytes) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
     auto rd = ix->read_lock();
-    size_t dev = 0;
-    for (const DevBuf *b : {&ix->centroids, &ix->w_rev, &ix->codes, &ix->residuals, &ix->doc_off, &ix->ivf, &ix->ivf_off,
-                            &ix->ucodes, &ix->udoc_off, &ix->cent_h16t, &ix->cent_l16t, &ix->tok_inv_norm,
-                            &ix->ivf_spare, &ix->ivf_off_spare})
+    size_t dev = ix->centroids.cap + ix->w_rev.cap + ix->cent_h16t.cap + ix->cent_l16t.cap;
+    for (const DevBuf *b : DocArrays::buffers(*ix))
         if (b->owned) dev += b->cap;  // adopted residuals are the caller's allocation
     if (device_bytes) *device_bytes = (int64_t)dev;
     if (host_bytes) *host_bytes = (int64_t)ix->host_res.bytes;
@@ -2766,24 +2832,9 @@ static pb_status run_search(pb_index *ix, const SearchIO &io) {
     CKS(plan_search(ix, io, plan));
     if (plan.Bt == 0) return PB_OK;
 
-    std::unique_ptr<Workspace> wsp;
-    CKS(ix->acquire(wsp));
-    Workspace &ws = *wsp;
-    // A workspace goes back to the pool only after a search that ran to completion: its scratch
-    // invariants (cleared bitmaps, zeroed maxima) are restored by the kernels themselves, so a call that
-    // fails half way must not hand its buffers to the next caller.
-    struct Releaser {
-        pb_index *ix;
-        std::unique_ptr<Workspace> &w;
-        bool ok = false;
-        ~Releaser() {
-            if (ok) ix->release(w);
-            else {
-                cudaStreamSynchronize(w->stream);
-                w.reset();
-            }
-        }
-    } rel{ix, wsp};
+    WorkspaceLease lease{ix};
+    CKS(lease.acquire());
+    Workspace &ws = *lease.ws;
 
     if (!plan.empty) CKS(plan_probe(ix, ws, io, plan));
     // empty results: the whole call, or the queries with nothing eligible (they get no pass)
@@ -2799,7 +2850,7 @@ static pb_status run_search(pb_index *ix, const SearchIO &io) {
     }
     if (plan.empty || plan.passes.empty()) {
         CK(cudaStreamSynchronize(ws.stream));
-        rel.ok = true;
+        lease.done = true;
         return PB_OK;
     }
 
@@ -2855,7 +2906,7 @@ static pb_status run_search(pb_index *ix, const SearchIO &io) {
         CK(cudaEventSynchronize(ws.call_ev[1]));
         CK(cudaEventElapsedTime(&g_stats.call_ms, ws.call_ev[0], ws.call_ev[1]));
     }
-    rel.ok = true;
+    lease.done = true;
     return PB_OK;
 }
 
@@ -3162,14 +3213,9 @@ extern "C" pb_status pb_centroid_scores(pb_index *ix, const float *query_tokens,
     if (n == 0) return PB_OK;
     auto rd = ix->read_lock();
     CK(cudaSetDevice(ix->device));
-    std::unique_ptr<Workspace> wsp;
-    CKS(ix->acquire(wsp));
-    Workspace &ws = *wsp;
-    struct Releaser {
-        pb_index *ix;
-        std::unique_ptr<Workspace> &w;
-        ~Releaser() { ix->release(w); }
-    } rel{ix, wsp};
+    WorkspaceLease lease{ix};
+    CKS(lease.acquire());
+    Workspace &ws = *lease.ws;
     // one pseudo-query per block of <= 64 tokens keeps the per-query transposed layout small
     const int blk = 64;
     DevBuf S;
@@ -3189,6 +3235,7 @@ extern "C" pb_status pb_centroid_scores(pb_index *ix, const float *query_tokens,
         CK(cudaMemcpyAsync(out + (size_t)r0 * ix->K, S.p, (size_t)nq * ix->K * 4, cudaMemcpyDeviceToHost, ws.stream));
         CK(cudaStreamSynchronize(ws.stream));
     }
+    lease.done = true;
     return PB_OK;
 }
 
@@ -3221,21 +3268,14 @@ extern "C" pb_status pb_decompress_documents(pb_index *ix, const int64_t *doc_id
     CKS(dout.ensure((size_t)std::min(total, chunk_tok + ix->max_doclen) * ix->dim * 4));
     // host tier: each range's docs are staged first (slot j = its j-th doc, at the range-local prefix), then decompressed
     // from the staged rows with the identity as doc list
-    std::unique_ptr<Workspace> wsp;
+    WorkspaceLease lease{ix};
     if (ix->host_tier) {
-        CKS(ix->acquire(wsp));
+        CKS(lease.acquire());
         CKS(ident.ensure(docs.size() * 4 + 16));
-        k_fill_identity<<<64, 256, 0, wsp->stream>>>(ident.as<uint32_t>(), (long long)docs.size(), 0u);
+        k_fill_identity<<<64, 256, 0, lease.ws->stream>>>(ident.as<uint32_t>(), (long long)docs.size(), 0u);
         CK(cudaGetLastError());
-        CK(cudaStreamSynchronize(wsp->stream));
+        CK(cudaStreamSynchronize(lease.ws->stream));
     }
-    struct Releaser {
-        pb_index *ix;
-        std::unique_ptr<Workspace> &w;
-        ~Releaser() {
-            if (w) ix->release(w);
-        }
-    } rel{ix, wsp};
     // process doc ranges whose token count fits the staging buffer
     size_t i0 = 0;
     while (i0 < docs.size()) {
@@ -3250,8 +3290,8 @@ extern "C" pb_status pb_decompress_documents(pb_index *ix, const int64_t *doc_id
         TokView tv = resident_tokens(ix);
         const uint32_t *list = ddocs.as<uint32_t>() + i0;
         if (ix->host_tier) {
-            CKS(stage_rows(ix, *wsp, list, nullptr, nd, nd, dpre.as<long long>(), ntok, tv));
-            CK(cudaStreamSynchronize(wsp->stream));
+            CKS(stage_rows(ix, *lease.ws, list, nullptr, nd, nd, dpre.as<long long>(), ntok, tv));
+            CK(cudaStreamSynchronize(lease.ws->stream));
             list = ident.as<uint32_t>();
         }
         PB_DIM_SWITCH(ix->dim, {
@@ -3263,6 +3303,7 @@ extern "C" pb_status pb_decompress_documents(pb_index *ix, const int64_t *doc_id
         CK(cudaMemcpy(out_embeddings + (size_t)prefix[i0] * ix->dim, dout.p, (size_t)ntok * ix->dim * 4, cudaMemcpyDeviceToHost));
         i0 = i1;
     }
+    lease.done = true;
     return PB_OK;
 }
 
@@ -3315,14 +3356,9 @@ extern "C" pb_status pb_exhaustive_scores(pb_index *ix, const float *queries, co
     auto rd = ix->read_lock();
     CK(cudaSetDevice(ix->device));
     if (n_queries == 0 || ix->D == 0) return PB_OK;
-    std::unique_ptr<Workspace> wsp;
-    CKS(ix->acquire(wsp));
-    Workspace &ws = *wsp;
-    struct Releaser {
-        pb_index *ix;
-        std::unique_ptr<Workspace> &w;
-        ~Releaser() { ix->release(w); }
-    } rel{ix, wsp};
+    WorkspaceLease lease{ix};
+    CKS(lease.acquire());
+    Workspace &ws = *lease.ws;
     std::vector<long long> doff((size_t)ix->D + 1);
     CK(cudaMemcpy(doff.data(), ix->doc_off.p, doff.size() * 8, cudaMemcpyDeviceToHost));
     const int QBmax = 32;
@@ -3378,6 +3414,7 @@ extern "C" pb_status pb_exhaustive_scores(pb_index *ix, const float *queries, co
             CK(cudaStreamSynchronize(ws.stream));
         }
     }
+    lease.done = true;
     return PB_OK;
 }
 
@@ -4058,14 +4095,37 @@ pb_status pb_index_patch_ivf(pb_index *ix, const int64_t *file_ivf, const int32_
 // new docs' offsets and distinct codes, the merged inverted file in the spare half of the ping-pong, and the totals the
 // commit publishes.  keys holds the new docs' sorted (centroid << 32 | doc in the batch) pairs.
 struct AppendPrep {
-    long long D0 = 0, n = 0, ntok = 0, N1 = 0, D1 = 0, U1 = 0, L1 = 0, m = 0;
-    int maxlen = 0;
-    float vmin = 0.f, wmax = 0.f;
+    long long D0 = 0, n = 0, ntok = 0, m = 0;
+    DocTotals t;
     std::vector<int64_t> dl, hcodes;  // doc lengths; the i64 codes for a directory (keep_codes)
     DevBuf keys;
 };
 
-// Every check, allocation and device write of an append that stays invisible until append_commit.  The caller holds
+// Capacity for D1 docs of N1 tokens in the per-token and per-doc arrays, keeping their contents
+static pb_status grow_docs(pb_index *ix, long long D1, long long N1, bool geometric) {
+    const size_t pk = (size_t)ix->packed;
+    CKS(ix->codes.grow((size_t)N1 * 4, (size_t)ix->N * 4, geometric));
+    CKS(ix->residuals.grow((size_t)N1 * pk, (size_t)ix->N * pk, geometric));
+    if (TcDims::has(ix->dim)) CKS(ix->tok_inv_norm.grow((size_t)N1 * 4, (size_t)ix->N * 4, geometric));
+    CKS(ix->doc_off.grow((size_t)(D1 + 1) * 8, (size_t)(ix->D + 1) * 8, geometric));
+    CKS(ix->udoc_off.grow((size_t)(D1 + 1) * 8, (size_t)(ix->D + 1) * 8, geometric));
+    return PB_OK;
+}
+
+// Makes a prepared mutation visible: its totals, with either the inverted file an append or a delete merged into the
+// spare halves, or (rebalance) a whole set of arrays built out of place, swapped in; the old ones leave with `fresh`
+static void publish(pb_index *ix, const DocTotals &t, DocArrays *fresh = nullptr) {
+    if (fresh) {
+        const auto mine = DocArrays::buffers(*ix), theirs = DocArrays::buffers(*fresh);
+        for (size_t i = 0; i < mine.size(); ++i) mine[i]->swap(*theirs[i]);
+    } else {
+        ix->ivf.swap(ix->ivf_spare);
+        ix->ivf_off.swap(ix->ivf_off_spare);
+    }
+    static_cast<DocTotals &>(*ix) = t;
+}
+
+// Every check, allocation and device write of an append that stays invisible until publish.  The caller holds
 // the handle's writer lock.
 static pb_status append_prepare(pb_index *ix, pb_codec *codec, const float *embeddings, const int64_t *codes,
                                 const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs, int32_t space,
@@ -4087,35 +4147,27 @@ static pb_status append_prepare(pb_index *ix, pb_codec *codec, const float *embe
         CK(cudaMemcpy(&differ, flag.p, 4, cudaMemcpyDeviceToHost));
         if (differ) return pb_fail(PB_ERR_INVALID, "the codec's centroids differ from the index's");
     }
-    const long long D0 = ix->D, N0 = ix->N, U0 = ix->n_ucodes, n = n_docs;
+    const long long D0 = ix->D, N0 = ix->N, n = n_docs;
     if (out_first) *out_first = ix->doc_id_base + D0;
     p.D0 = D0;
-    std::vector<int64_t> &dl = p.dl;
-    CKS(fetch_host(dl, doc_lengths, (size_t)n, space));
-    std::vector<long long> doff((size_t)n, 0);  // doc_off[D0 + 1 ..]
-    long long ntok = 0;
-    int maxlen = ix->max_doclen;
-    for (long long i = 0; i < n; ++i) {
-        if (dl[i] < 0 || dl[i] > (1 << 30)) return pb_fail(PB_ERR_INVALID, "doc_lengths[%lld] = %lld", i, (long long)dl[i]);
-        ntok += dl[i];
-        doff[i] = N0 + ntok;
-        maxlen = std::max<int>(maxlen, (int)dl[i]);
-    }
+    DocTotals &t = p.t;
+    t.max_doclen = ix->max_doclen;
+    CKS(fetch_host(p.dl, doc_lengths, (size_t)n, space));
+    std::vector<long long> doff;  // doc_off[D0 ..]
+    CKS(doc_offsets(p.dl, N0, doff, &t.max_doclen));
     if (n == 0) return PB_OK;
+    const long long ntok = doff[n] - N0;
     // the limits of pb_index_open_begin for the new totals
     if (D0 + n >= (1ll << 32) - 1 || ix->doc_id_base + D0 + n >= (1ll << 32) - 1)
         return pb_fail(PB_ERR_UNSUPPORTED, "D and global doc ids must stay below 2^32-1");
     if (ntok > 0 && ((codec && !embeddings) || (!codec && (!codes || !residuals)))) return pb_fail(PB_ERR_INVALID, "null argument");
-    const long long N1 = N0 + ntok, D1 = D0 + n;
+    p.ntok = ntok;
+    t.N = N0 + ntok;
+    t.D = D0 + n;
     const size_t pk = (size_t)ix->packed;
-    const bool filter = TcDims::has(ix->dim) && N1 > 0;
 
     // capacity: grown arrays keep their contents; nothing below is visible until the commit
-    CKS(ix->codes.grow((size_t)N1 * 4, (size_t)N0 * 4));
-    CKS(ix->residuals.grow((size_t)N1 * pk, (size_t)N0 * pk));
-    if (filter) CKS(ix->tok_inv_norm.grow((size_t)N1 * 4, (size_t)N0 * 4));
-    CKS(ix->doc_off.grow((size_t)(D1 + 1) * 8, (size_t)(D0 + 1) * 8));
-    CKS(ix->udoc_off.grow((size_t)(D1 + 1) * 8, (size_t)(D0 + 1) * 8));
+    CKS(grow_docs(ix, t.D, t.N, true));
 
     // 1. tokens into the tails of codes / residuals: encoded on the device, or narrowed and range-checked
     std::vector<int64_t> &hcodes = p.hcodes;  // i64 codes for the chunk files
@@ -4145,55 +4197,24 @@ static pb_status append_prepare(pb_index *ix, pb_codec *codec, const float *embe
     }
 
     // 2. doc offsets
-    CK(cudaMemcpy(ix->doc_off.as<long long>() + D0 + 1, doff.data(), (size_t)n * 8, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(ix->doc_off.as<long long>() + D0 + 1, doff.data() + 1, (size_t)n * 8, cudaMemcpyHostToDevice));
 
-    // 3. distinct code lists of the new docs, after the old ones (udoc_off holds absolute positions into ucodes)
-    std::vector<long long> uoff((size_t)n);
-    {
-        DevBuf counts;
-        CKS(counts.ensure((size_t)n * 4));
-        const int blocks = (int)std::min<long long>(n, (long long)ix->sm_count * 16);
-        k_unique_codes<<<blocks, 128>>>(ix->codes.as<uint32_t>(), ix->doc_off.as<long long>() + D0, n, nullptr, nullptr,
-                                        counts.as<int>());
-        CK(cudaGetLastError());
-        std::vector<int> hc((size_t)n);
-        CK(cudaMemcpy(hc.data(), counts.p, hc.size() * 4, cudaMemcpyDeviceToHost));
-        long long u = U0;
-        for (long long i = 0; i < n; ++i) uoff[i] = u += hc[i];
-    }
-    const long long U1 = uoff[n - 1];
-    CKS(ix->ucodes.grow(std::max<size_t>((size_t)U1 * 4, 16), (size_t)U0 * 4));
-    CK(cudaMemcpy(ix->udoc_off.as<long long>() + D0 + 1, uoff.data(), (size_t)n * 8, cudaMemcpyHostToDevice));
-    {
-        const int blocks = (int)std::min<long long>(n, (long long)ix->sm_count * 16);
-        k_unique_codes<<<blocks, 128>>>(ix->codes.as<uint32_t>(), ix->doc_off.as<long long>() + D0, n,
-                                        ix->udoc_off.as<long long>() + D0, ix->ucodes.as<uint32_t>(), nullptr);
-        CK(cudaGetLastError());
-    }
+    // 3. distinct code lists of the new docs, after the old ones
+    CKS(unique_codes(ix, D0, n, ix->n_ucodes, &t.n_ucodes));
 
     // 4. 1 / |c + w| of the new tokens; min / max seeded with the index's, which is what an open over all tokens finds
-    float vmin = ix->vmin, wmax = ix->wmax;
-    if (filter) {
-        if (N0 == 0) CKS(build_centroid_operands(ix));  // an index opened empty has none yet
-        DevBuf mn;
-        CKS(mn.ensure(16));
-        const float init[2] = {N0 > 0 ? ix->vmin : 3.0e38f, N0 > 0 ? ix->wmax : 0.0f};
-        CK(cudaMemcpy(mn.p, init, 8, cudaMemcpyHostToDevice));
-        CKS(launch_min_vnorm(ix, N0, ntok, mn.as<float>()));
-        float got[2] = {0.f, 0.f};
-        CK(cudaMemcpy(got, mn.p, 8, cudaMemcpyDeviceToHost));
-        vmin = got[0] < 1e30f ? got[0] : 0.0f;
-        wmax = got[1];
-    }
+    DevBuf mn;
+    const float seed[2] = {N0 > 0 ? ix->vmin : 3.0e38f, N0 > 0 ? ix->wmax : 0.0f};
+    CKS(token_norms(ix, *ix, N0, seed, t, mn));
 
     // 5. inverted file: the new docs' sorted distinct (centroid, doc) pairs merged behind each centroid's old list
     DevBuf add_before;
     long long m = 0;
-    CKS(sorted_doc_pairs(ix, D0, n, U1 - U0, p.keys, &m));
-    const long long L1 = ix->ivf_len + m;
-    if (L1 > (1ll << 31) - 2) return pb_fail(PB_ERR_UNSUPPORTED, "more than 2^31 (centroid, doc) pairs per shard");
+    CKS(sorted_doc_pairs(ix, D0, n, t.n_ucodes - ix->n_ucodes, p.keys, &m));
+    t.ivf_len = ix->ivf_len + m;
+    if (t.ivf_len > (1ll << 31) - 2) return pb_fail(PB_ERR_UNSUPPORTED, "more than 2^31 (centroid, doc) pairs per shard");
     CKS(add_before.ensure((size_t)(ix->K + 1) * 8));
-    CKS(ix->ivf_spare.grow(std::max<size_t>((size_t)L1 * 4, 16), 0));
+    CKS(ix->ivf_spare.grow(std::max<size_t>((size_t)t.ivf_len * 4, 16), 0));
     CKS(ix->ivf_off_spare.ensure((size_t)(ix->K + 1) * 8));
     k_ivf_offsets<<<(unsigned)((ix->K + 256) / 256), 256>>>(p.keys.as<u64>(), m, ix->K, add_before.as<long long>());
     k_ivf_merge_old<<<ix->sm_count * 8, 256>>>(ix->ivf.as<uint32_t>(), ix->ivf_off.as<long long>(), add_before.as<long long>(),
@@ -4204,15 +4225,7 @@ static pb_status append_prepare(pb_index *ix, pb_codec *codec, const float *embe
     CK(cudaGetLastError());
     CK(cudaDeviceSynchronize());
     p.n = n;
-    p.ntok = ntok;
-    p.N1 = N1;
-    p.D1 = D1;
-    p.U1 = U1;
-    p.L1 = L1;
     p.m = m;
-    p.maxlen = maxlen;
-    p.vmin = vmin;
-    p.wmax = wmax;
     return PB_OK;
 }
 
@@ -4223,22 +4236,9 @@ static pb_status append_dir(pb_index *ix, const AppendPrep &p, const char *index
     const size_t pk = (size_t)ix->packed;
     std::vector<uint8_t> hres((size_t)p.ntok * pk);
     if (p.ntok)
-        CK(cudaMemcpy(hres.data(), ix->residuals.as<uint8_t>() + (size_t)(p.N1 - p.ntok) * pk, hres.size(), cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(hres.data(), ix->residuals.as<uint8_t>() + (size_t)(p.t.N - p.ntok) * pk, hres.size(), cudaMemcpyDeviceToHost));
     return pb_dir_append(index_dir, old_D, ix->K, ix->dim, ix->nbits, batch_size, p.hcodes.data(), hres.data(), p.dl.data(),
                          p.n, hivf.data(), L, hlen.data());
-}
-
-static void append_commit(pb_index *ix, const AppendPrep &p) {
-    if (p.n == 0) return;
-    ix->ivf.swap(ix->ivf_spare);
-    ix->ivf_off.swap(ix->ivf_off_spare);
-    ix->ivf_len = p.L1;
-    ix->n_ucodes = p.U1;
-    ix->N = p.N1;
-    ix->D = p.D1;
-    ix->max_doclen = p.maxlen;
-    ix->vmin = p.vmin;
-    ix->wmax = p.wmax;
 }
 
 // Mutations need a residual array the library owns on the device: not the caller's (PB_OPEN_ADOPT_RESIDUALS), not
@@ -4270,10 +4270,10 @@ static pb_status append_impl(pb_index *ix, pb_codec *codec, const float *embeddi
     if (index_dir) {
         std::vector<int64_t> hivf;
         std::vector<int32_t> hlen;
-        CKS(ivf_to_host(ix, ix->ivf_spare, ix->ivf_off_spare, p.L1, hivf, hlen));
-        CKS(append_dir(ix, p, index_dir, p.D0, batch_size, hivf, p.L1, hlen));
+        CKS(ivf_to_host(ix, ix->ivf_spare, ix->ivf_off_spare, p.t.ivf_len, hivf, hlen));
+        CKS(append_dir(ix, p, index_dir, p.D0, batch_size, hivf, p.t.ivf_len, hlen));
     }
-    append_commit(ix, p);
+    publish(ix, p.t);
     return PB_OK;
 }
 
@@ -4304,11 +4304,7 @@ extern "C" pb_status pb_index_reserve(pb_index *ix, int64_t num_documents, int64
     const long long dd = D1 - ix->D, dn = N1 - ix->N;
     // a new doc adds at most its length rounded up to 8 distinct-code entries, and at most that many (centroid, doc) pairs
     const long long U1 = ix->n_ucodes + dn + 7 * dd, L1 = ix->ivf_len + dn;
-    CKS(ix->codes.grow((size_t)N1 * 4, (size_t)ix->N * 4, false));
-    CKS(ix->residuals.grow((size_t)N1 * ix->packed, (size_t)ix->N * ix->packed, false));
-    if (TcDims::has(ix->dim)) CKS(ix->tok_inv_norm.grow((size_t)N1 * 4, (size_t)ix->N * 4, false));
-    CKS(ix->doc_off.grow((size_t)(D1 + 1) * 8, (size_t)(ix->D + 1) * 8, false));
-    CKS(ix->udoc_off.grow((size_t)(D1 + 1) * 8, (size_t)(ix->D + 1) * 8, false));
+    CKS(grow_docs(ix, D1, N1, false));
     CKS(ix->ucodes.grow((size_t)U1 * 4, (size_t)ix->n_ucodes * 4, false));
     CKS(ix->ivf.grow((size_t)L1 * 4, (size_t)ix->ivf_len * 4, false));
     CKS(ix->ivf_spare.grow((size_t)L1 * 4, 0, false));
@@ -4359,8 +4355,8 @@ static pb_status del_bitmap(pb_index *ix, const int64_t *doc_ids, long long n_id
 // What a delete computes before its first in-place write: the deleted set, the survivors and their new offsets, the
 // filtered inverted file in the spare half, the compaction windows with their staging buffers, and the new totals
 struct DeletePrep {
-    long long D0 = 0, n_del = 0, D1 = 0, N1 = 0, U1 = 0, L1 = 0;
-    int maxlen = 0;
+    long long D0 = 0, n_del = 0;
+    DocTotals t;
     DevBuf bits, wpre, kept, new_doff, new_uoff, st_codes, st_res, st_u, mn;
     std::vector<long long> hoff, hu;
     std::vector<uint32_t> hbits;
@@ -4403,11 +4399,10 @@ static pb_status delete_prepare(pb_index *ix, const int64_t *doc_ids, int64_t n_
     hu.resize((size_t)D1 + 1);
     CK(cudaMemcpy(hoff.data(), p.new_doff.p, hoff.size() * 8, cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(hu.data(), p.new_uoff.p, hu.size() * 8, cudaMemcpyDeviceToHost));
-    p.D1 = D1;
-    p.N1 = hoff[D1];
-    p.U1 = hu[D1];
-    p.maxlen = 0;
-    for (long long j = 0; j < D1; ++j) p.maxlen = std::max<int>(p.maxlen, (int)(hoff[j + 1] - hoff[j]));
+    p.t.D = D1;
+    p.t.N = hoff[D1];
+    p.t.n_ucodes = hu[D1];
+    p.t.max_doclen = longest_doc(hoff, D1);
 
     // 3. the inverted file without the deleted ids, renumbered, into the spare half
     if (ix->profiling) CK(cudaEventRecord(p.ev.e[0]));
@@ -4418,8 +4413,8 @@ static pb_status delete_prepare(pb_index *ix, const int64_t *doc_ids, int64_t n_
                                       icnt.as<long long>());
     CK(cudaGetLastError());
     CKS(exclusive_sum(icnt.as<long long>(), ix->ivf_off_spare.as<long long>(), K + 1, tmp));
-    CK(cudaMemcpy(&p.L1, ix->ivf_off_spare.as<long long>() + K, 8, cudaMemcpyDeviceToHost));
-    CKS(ix->ivf_spare.grow(std::max<size_t>((size_t)p.L1 * 4, 16), 0));
+    CK(cudaMemcpy(&p.t.ivf_len, ix->ivf_off_spare.as<long long>() + K, 8, cudaMemcpyDeviceToHost));
+    CKS(ix->ivf_spare.grow(std::max<size_t>((size_t)p.t.ivf_len * 4, 16), 0));
     k_ivf_delete_write<<<grid, 256>>>(ix->ivf.as<uint32_t>(), ix->ivf_off.as<long long>(), K, p.bits.as<uint32_t>(),
                                       p.wpre.as<long long>(), ix->ivf_off_spare.as<long long>(), ix->ivf_spare.as<uint32_t>());
     CK(cudaGetLastError());
@@ -4485,35 +4480,19 @@ static pb_status delete_commit(pb_index *ix, DeletePrep &p) {
         CK(cudaMemcpy(ix->residuals.as<uint8_t>() + (size_t)hoff[j0] * pk, p.st_res.p, (size_t)nt * pk, cudaMemcpyDeviceToDevice));
         CK(cudaMemcpy(ix->ucodes.as<uint8_t>() + (size_t)hu[j0] * 4, p.st_u.p, (size_t)nu * 4, cudaMemcpyDeviceToDevice));
     }
-    CK(cudaMemcpy(ix->doc_off.p, p.new_doff.p, (size_t)(p.D1 + 1) * 8, cudaMemcpyDeviceToDevice));
-    CK(cudaMemcpy(ix->udoc_off.p, p.new_uoff.p, (size_t)(p.D1 + 1) * 8, cudaMemcpyDeviceToDevice));
+    CK(cudaMemcpy(ix->doc_off.p, p.new_doff.p, (size_t)(p.t.D + 1) * 8, cudaMemcpyDeviceToDevice));
+    CK(cudaMemcpy(ix->udoc_off.p, p.new_uoff.p, (size_t)(p.t.D + 1) * 8, cudaMemcpyDeviceToDevice));
     if (prof) CK(cudaEventRecord(p.ev.e[3]));
 
     // 6. 1 / |c + w| of the survivors in their new order, and vmin / wmax over them as an open computes them: the old
     // constants would still bound the error, but the work counters would differ from a fresh open
-    float vmin = 0.0f, wmax = 0.0f;
-    if (TcDims::has(ix->dim) && p.N1 > 0) {
-        const float init[2] = {3.0e38f, 0.0f};
-        CK(cudaMemcpy(p.mn.p, init, 8, cudaMemcpyHostToDevice));
-        CKS(launch_min_vnorm(ix, 0, p.N1, p.mn.as<float>()));
-        float got[2] = {0.f, 0.f};
-        CK(cudaMemcpy(got, p.mn.p, 8, cudaMemcpyDeviceToHost));
-        vmin = got[0] < 1e30f ? got[0] : 0.0f;
-        wmax = got[1];
-    }
+    const float seed[2] = {3.0e38f, 0.0f};
+    CKS(token_norms(ix, *ix, 0, seed, p.t, p.mn));
     if (prof) CK(cudaEventRecord(p.ev.e[4]));
     CK(cudaDeviceSynchronize());
 
     // 7. commit
-    ix->ivf.swap(ix->ivf_spare);
-    ix->ivf_off.swap(ix->ivf_off_spare);
-    ix->ivf_len = p.L1;
-    ix->n_ucodes = p.U1;
-    ix->N = p.N1;
-    ix->D = p.D1;
-    ix->max_doclen = p.maxlen;
-    ix->vmin = vmin;
-    ix->wmax = wmax;
+    publish(ix, p.t);
     if (prof) {
         CK(cudaEventElapsedTime(&ix->delete_ms[0], p.ev.e[2], p.ev.e[3]));
         CK(cudaEventElapsedTime(&ix->delete_ms[1], p.ev.e[0], p.ev.e[1]));
@@ -4538,8 +4517,8 @@ extern "C" pb_status pb_index_delete(pb_index *ix, const int64_t *doc_ids, int64
     if (index_dir) {
         std::vector<int64_t> hivf;
         std::vector<int32_t> hlen;
-        CKS(ivf_to_host(ix, ix->ivf_spare, ix->ivf_off_spare, p.L1, hivf, hlen));
-        CKS(pb_dir_delete(index_dir, p.D0, ix->K, ix->dim, ix->nbits, p.hbits.data(), hivf.data(), p.L1, hlen.data()));
+        CKS(ivf_to_host(ix, ix->ivf_spare, ix->ivf_off_spare, p.t.ivf_len, hivf, hlen));
+        CKS(pb_dir_delete(index_dir, p.D0, ix->K, ix->dim, ix->nbits, p.hbits.data(), hivf.data(), p.t.ivf_len, hlen.data()));
     }
     CKS(delete_commit(ix, p));
     if (out_deleted) *out_deleted = p.n_del;
@@ -4552,7 +4531,10 @@ extern "C" pb_status pb_index_delete(pb_index *ix, const int64_t *doc_ids, int64
 // writes the directory from ivf.npy on disk; a second exchange carries its status.  After the vote only a CUDA runtime
 // error can fail a rank.
 // ------------------------------------------------------------------------------------------
-enum { SH_STATUS, SH_RANK, SH_WORLD, SH_BASE, SH_D, SH_N, SH_K, SH_DIM, SH_NBITS, SH_NDEL, SH_PRINT, SH_WORDS };
+// The first exchange of a sharded collective (update or rebalance) carries one record per rank: this head, then the
+// operation's own word (the local deletion count of an update, the adopt flag of a rebalance), then an FNV-1a
+// fingerprint of the arguments
+enum { LR_STATUS, LR_RANK, LR_WORLD, LR_BASE, LR_D, LR_N, LR_K, LR_DIM, LR_NBITS, LR_OWN, LR_PRINT, LR_WORDS };
 enum { SH_OP_DELETE = 1, SH_OP_APPEND = 2, SH_OP_APPEND_ENCODED = 3 };
 
 // every rank's `words` 64-bit words, in rank order; a handle outside any group is a group of one
@@ -4561,12 +4543,7 @@ static pb_status gather_words(pb_index *ix, const long long *mine, int words, st
     all.assign(mine, mine + words);
     if (!ix->comm && !ix->group) return PB_OK;
     all.resize((size_t)words * ix->world);
-    struct Stream {
-        cudaStream_t s = nullptr;
-        ~Stream() {
-            if (s) cudaStreamDestroy(s);
-        }
-    } st;
+    OwnedStream st;
     DevBuf send, recv;
     CK(cudaSetDevice(ix->device));
     CK(cudaStreamCreateWithFlags(&st.s, cudaStreamNonBlocking));
@@ -4593,6 +4570,43 @@ static pb_status first_failure(pb_index *ix, const std::vector<long long> &all, 
     return PB_OK;
 }
 
+// Exchange A of a sharded collective and the verdict every rank reaches from the same records.  The caller has set
+// the status, its own word and the fingerprint of `rec`; the head is filled in here.  The lowest failing rank's
+// status, a rank whose layout differs from rank 0's, documents that do not tile [0, D) and a fingerprint that differs
+// from rank 0's (a call with other `args`) fail every rank.  Gives every rank's record (all), the ranks' first
+// documents (base [W + 1], base[W] = D_total) and first tokens (tok [W + 1]).
+static pb_status layout_vote(pb_index *ix, long long *rec, const char *args, std::vector<long long> &all,
+                             std::vector<long long> &base, std::vector<long long> &tok) {
+    const int W = ix->world;
+    rec[LR_RANK] = ix->rank;
+    rec[LR_WORLD] = W;
+    rec[LR_BASE] = ix->doc_id_base;
+    rec[LR_D] = ix->D;
+    rec[LR_N] = ix->N;
+    rec[LR_K] = ix->K;
+    rec[LR_DIM] = ix->dim;
+    rec[LR_NBITS] = ix->nbits;
+    CKS(gather_words(ix, rec, LR_WORDS, all));
+    CKS(first_failure(ix, all, LR_WORDS, "; nothing changed"));
+    auto at = [&](int r, int w) { return all[(size_t)r * LR_WORDS + w]; };
+    base.assign((size_t)W + 1, 0);
+    tok.assign((size_t)W + 1, 0);
+    for (int r = 0; r < W; ++r) {
+        if (at(r, LR_RANK) != r || at(r, LR_WORLD) != W || at(r, LR_K) != at(0, LR_K) || at(r, LR_DIM) != at(0, LR_DIM) ||
+            at(r, LR_NBITS) != at(0, LR_NBITS))
+            return pb_fail(PB_ERR_INVALID, "rank %d's layout (rank %lld of %lld, K=%lld dim=%lld nbits=%lld) differs from rank 0's",
+                           r, at(r, LR_RANK), at(r, LR_WORLD), at(r, LR_K), at(r, LR_DIM), at(r, LR_NBITS));
+        if (at(r, LR_BASE) != base[r])
+            return pb_fail(PB_ERR_INVALID, "the ranks' documents do not tile [0, D): rank %d starts at %lld, not %lld", r,
+                           at(r, LR_BASE), base[r]);
+        if (at(r, LR_PRINT) != at(0, LR_PRINT))
+            return pb_fail(PB_ERR_INVALID, "rank %d was called with other %s than rank 0", r, args);
+        base[r + 1] = base[r] + at(r, LR_D);
+        tok[r + 1] = tok[r] + at(r, LR_N);
+    }
+    return PB_OK;
+}
+
 static pb_status sharded_update(pb_index *ix, int op, pb_codec *codec, const float *embeddings, const int64_t *codes,
                                 const uint8_t *residuals, const int64_t *doc_lengths, const int64_t *doc_ids, int64_t n,
                                 int32_t space, const char *index_dir, int64_t batch_size, int64_t *out) {
@@ -4602,7 +4616,7 @@ static pb_status sharded_update(pb_index *ix, int op, pb_codec *codec, const flo
     const bool last = ix->rank == ix->world - 1;
     DeletePrep dp;
     AppendPrep ap;
-    long long rec[SH_WORDS] = {};
+    long long rec[LR_WORDS] = {};
     // 1. local checks, the fingerprint of the arguments, and the prepare: no early return, or the peers would wait
     auto local = [&]() -> pb_status {
         if (n < 0 || (n && !(op == SH_OP_DELETE ? doc_ids : doc_lengths))) return pb_fail(PB_ERR_INVALID, "null argument");
@@ -4621,46 +4635,26 @@ static pb_status sharded_update(pb_index *ix, int op, pb_codec *codec, const flo
         f.put(index_dir != nullptr);
         if (index_dir) f.add(index_dir, strlen(index_dir) + 1);
         f.put((long long)(op == SH_OP_APPEND ? batch_size : 0));
-        rec[SH_PRINT] = (long long)f.h;
+        rec[LR_PRINT] = (long long)f.h;
         if (op == SH_OP_DELETE) {
             CKS(delete_prepare(ix, doc_ids, n, dp));
-            rec[SH_NDEL] = dp.n_del;
+            rec[LR_OWN] = dp.n_del;
         } else if (last) {
             CKS(append_prepare(ix, codec, embeddings, codes, residuals, doc_lengths, n, space, index_dir != nullptr,
                                nullptr, ap));
         }
         return PB_OK;
     };
-    rec[SH_STATUS] = local();
-    rec[SH_RANK] = ix->rank;
-    rec[SH_WORLD] = ix->world;
-    rec[SH_BASE] = ix->doc_id_base;
-    rec[SH_D] = ix->D;
-    rec[SH_N] = ix->N;
-    rec[SH_K] = ix->K;
-    rec[SH_DIM] = ix->dim;
-    rec[SH_NBITS] = ix->nbits;
+    rec[LR_STATUS] = local();
 
     // 2. exchange A and the verdict every rank reaches from the same records
-    std::vector<long long> all;
-    CKS(gather_words(ix, rec, SH_WORDS, all));
-    const int W = ix->world;
-    CKS(first_failure(ix, all, SH_WORDS, "; nothing changed"));
-    auto at = [&](int r, int w) { return all[(size_t)r * SH_WORDS + w]; };
-    long long D_total = 0, n_del = 0, del_before = 0;
-    for (int r = 0; r < W; ++r) {
-        if (at(r, SH_RANK) != r || at(r, SH_WORLD) != W || at(r, SH_K) != at(0, SH_K) || at(r, SH_DIM) != at(0, SH_DIM) ||
-            at(r, SH_NBITS) != at(0, SH_NBITS))
-            return pb_fail(PB_ERR_INVALID, "rank %d's layout (rank %lld of %lld, K=%lld dim=%lld nbits=%lld) differs from rank 0's",
-                           r, at(r, SH_RANK), at(r, SH_WORLD), at(r, SH_K), at(r, SH_DIM), at(r, SH_NBITS));
-        if (at(r, SH_BASE) != D_total)
-            return pb_fail(PB_ERR_INVALID, "the ranks' documents do not tile [0, D): rank %d starts at %lld, not %lld", r,
-                           at(r, SH_BASE), D_total);
-        if (at(r, SH_PRINT) != at(0, SH_PRINT))
-            return pb_fail(PB_ERR_INVALID, "rank %d was called with other arguments than rank 0", r);
-        D_total += at(r, SH_D);
-        if (r < ix->rank) del_before += at(r, SH_NDEL);
-        n_del += at(r, SH_NDEL);
+    std::vector<long long> all, base, tok;
+    CKS(layout_vote(ix, rec, "arguments", all, base, tok));
+    const long long D_total = base[ix->world];
+    long long n_del = 0, del_before = 0;
+    for (int r = 0; r < ix->world; ++r) {
+        if (r < ix->rank) del_before += all[(size_t)r * LR_WORDS + LR_OWN];
+        n_del += all[(size_t)r * LR_WORDS + LR_OWN];
     }
     if (op == SH_OP_DELETE && n_del == 0) return PB_OK;  // nothing changes, on any rank or on disk
     if (op != SH_OP_DELETE && out) *out = D_total;
@@ -4707,7 +4701,7 @@ static pb_status sharded_update(pb_index *ix, int op, pb_codec *codec, const flo
         ix->doc_id_base -= del_before;
         if (out) *out = n_del;
     } else if (last) {
-        append_commit(ix, ap);
+        publish(ix, ap.t);
     }
     return PB_OK;
 }
@@ -4743,7 +4737,6 @@ extern "C" pb_status pb_index_append_encoded_sharded(pb_index *ix, const int64_t
 // final offsets, then the scans, the merge of the inverted file and the norm pass run over them.  The old arrays stay
 // until the last vote, so a failure anywhere leaves every rank as it was.
 // ------------------------------------------------------------------------------------------
-enum { RB_STATUS, RB_RANK, RB_WORLD, RB_BASE, RB_D, RB_N, RB_K, RB_DIM, RB_NBITS, RB_ADOPT, RB_PRINT, RB_WORDS };
 enum { SZ_TOK, SZ_UCODES, SZ_IVF, SZ_WORDS };  // per piece in the size exchange
 // what moves with a piece of documents, in the order both ends issue it
 enum { XF_CODES, XF_RES, XF_UCODES, XF_TLEN, XF_ULEN, XF_IVF_OFF, XF_IVF, XF_ITEMS };
@@ -4754,12 +4747,10 @@ struct RebalancePrep {
     // its offsets [W][K + 1], and where each piece's entries start in it (hsplit [W + 1])
     DevBuf q, tlen, ulen, split, split_off;
     std::vector<long long> hsplit;
-    // receiver: the new arrays, and the per-doc lengths and inverted-file segments of its pieces as they arrive
-    DevBuf codes, residuals, ucodes, doc_off, udoc_off, ivf, ivf_off, ivf_spare, tok_inv_norm, rlen, rulen, seg, seg_off,
-        meta, mn;
-    long long D1 = 0, N1 = 0, U1 = 0, L1 = 0;
-    int maxlen = 0;
-    float vmin = 0.f, wmax = 0.f;
+    // receiver: the new arrays with their totals, and the per-doc lengths and inverted-file segments of its pieces as
+    // they arrive
+    DocArrays nx;
+    DevBuf rlen, rulen, seg, seg_off, meta, mn;
 };
 
 extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bounds, int64_t *out_bounds) {
@@ -4771,14 +4762,14 @@ extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bou
     const size_t pk = (size_t)ix->packed;
     const int grid = ix->sm_count * 8;
     RebalancePrep p;
-    long long rec[RB_WORDS] = {};
+    long long rec[LR_WORDS] = {};
     // 1. local checks, the fingerprint of the bounds and the host copies of the offsets: no early return, or the peers
     // would wait
     auto local = [&]() -> pb_status {
         Fnv64 f;
         f.put(bounds != nullptr);
         if (bounds) f.add(bounds, (size_t)(W + 1) * 8);
-        rec[RB_PRINT] = (long long)f.h;
+        rec[LR_PRINT] = (long long)f.h;
         if (ix->comm && !g_nccl.has_p2p())
             return pb_fail(PB_ERR_COMM, "the NCCL library lacks ncclSend / ncclRecv / ncclGroupStart / ncclGroupEnd");
         CK(cudaSetDevice(ix->device));
@@ -4789,38 +4780,14 @@ extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bou
         CK(cudaMemcpy(p.huoff.data(), ix->udoc_off.p, p.huoff.size() * 8, cudaMemcpyDeviceToHost));
         return PB_OK;
     };
-    rec[RB_STATUS] = local();
-    rec[RB_RANK] = me;
-    rec[RB_WORLD] = W;
-    rec[RB_BASE] = ix->doc_id_base;
-    rec[RB_D] = ix->D;
-    rec[RB_N] = ix->N;
-    rec[RB_K] = K;
-    rec[RB_DIM] = ix->dim;
-    rec[RB_NBITS] = ix->nbits;
-    rec[RB_ADOPT] = !ix->residuals.owned || ix->host_tier;  // a residual array that cannot move
+    rec[LR_STATUS] = local();
+    rec[LR_OWN] = !ix->residuals.owned || ix->host_tier;  // a residual array that cannot move
 
     // 2. exchange A and the verdict every rank reaches from the same records
-    std::vector<long long> all;
-    CKS(gather_words(ix, rec, RB_WORDS, all));
-    CKS(first_failure(ix, all, RB_WORDS, "; nothing changed"));
-    auto at = [&](int r, int w) { return all[(size_t)r * RB_WORDS + w]; };
-    std::vector<long long> a((size_t)W + 1, 0), tok((size_t)W + 1, 0);  // old bounds, global token offsets
-    for (int r = 0; r < W; ++r) {
-        if (at(r, RB_RANK) != r || at(r, RB_WORLD) != W || at(r, RB_K) != at(0, RB_K) || at(r, RB_DIM) != at(0, RB_DIM) ||
-            at(r, RB_NBITS) != at(0, RB_NBITS))
-            return pb_fail(PB_ERR_INVALID, "rank %d's layout (rank %lld of %lld, K=%lld dim=%lld nbits=%lld) differs from rank 0's",
-                           r, at(r, RB_RANK), at(r, RB_WORLD), at(r, RB_K), at(r, RB_DIM), at(r, RB_NBITS));
-        if (at(r, RB_BASE) != a[r])
-            return pb_fail(PB_ERR_INVALID, "the ranks' documents do not tile [0, D): rank %d starts at %lld, not %lld", r,
-                           at(r, RB_BASE), a[r]);
-        if (at(r, RB_PRINT) != at(0, RB_PRINT))
-            return pb_fail(PB_ERR_INVALID, "rank %d was called with other bounds than rank 0", r);
-        a[r + 1] = a[r] + at(r, RB_D);
-        tok[r + 1] = tok[r] + at(r, RB_N);
-    }
+    std::vector<long long> all, a, tok;  // records, old bounds, global token offsets
+    CKS(layout_vote(ix, rec, "bounds", all, a, tok));
     for (int r = 0; r < W; ++r)
-        if (at(r, RB_ADOPT))
+        if (all[(size_t)r * LR_WORDS + LR_OWN])
             return pb_fail(PB_ERR_UNSUPPORTED,
                            "rank %d uses the caller's residual array or host memory (PB_OPEN_ADOPT_RESIDUALS / "
                            "PB_OPEN_HOST_RESIDUALS)", r);
@@ -4920,31 +4887,34 @@ extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bou
         upos[s + 1] = upos[s] + sz(s, me, SZ_UCODES);
         ipos[s + 1] = ipos[s] + sz(s, me, SZ_IVF);
     }
+    DocArrays &nx = p.nx;
     auto allocate = [&]() -> pb_status {
         if (!changes) return PB_OK;
-        p.D1 = b[me + 1] - b[me];
-        p.N1 = tpos[W];
-        p.U1 = upos[W];
-        p.L1 = ipos[W];
-        if (p.L1 > (1ll << 31) - 2) return pb_fail(PB_ERR_UNSUPPORTED, "more than 2^31 (centroid, doc) pairs per shard");
+        nx.D = b[me + 1] - b[me];
+        nx.N = tpos[W];
+        nx.n_ucodes = upos[W];
+        nx.ivf_len = ipos[W];
+        if (nx.ivf_len > (1ll << 31) - 2) return pb_fail(PB_ERR_UNSUPPORTED, "more than 2^31 (centroid, doc) pairs per shard");
         const bool last = me == W - 1;
         auto alloc = [&](DevBuf &nb, const DevBuf &old, long long old_bytes, long long bytes) {
             const size_t spare = last && (long long)old.cap > old_bytes ? old.cap - (size_t)old_bytes : 0;
             return nb.grow(std::max<size_t>((size_t)bytes + spare, 16), 0, false);
         };
-        const long long D0 = ix->D, N0 = ix->N, D1 = p.D1;
-        CKS(alloc(p.codes, ix->codes, N0 * 4, p.N1 * 4));
-        CKS(alloc(p.residuals, ix->residuals, N0 * (long long)pk, p.N1 * (long long)pk));
-        CKS(alloc(p.ucodes, ix->ucodes, ix->n_ucodes * 4, p.U1 * 4));
-        CKS(alloc(p.doc_off, ix->doc_off, (D0 + 1) * 8, (D1 + 1) * 8));
-        CKS(alloc(p.udoc_off, ix->udoc_off, (D0 + 1) * 8, (D1 + 1) * 8));
-        CKS(alloc(p.ivf, ix->ivf, ix->ivf_len * 4, p.L1 * 4));
-        if (last && ix->ivf_spare.cap) CKS(alloc(p.ivf_spare, ix->ivf_spare, ix->ivf_len * 4, p.L1 * 4));
-        if (TcDims::has(ix->dim) && p.N1 > 0) CKS(alloc(p.tok_inv_norm, ix->tok_inv_norm, N0 * 4, p.N1 * 4));
-        CKS(p.ivf_off.grow((size_t)(K + 1) * 8, 0, false));
+        const long long D0 = ix->D, N0 = ix->N, D1 = nx.D;
+        CKS(alloc(nx.codes, ix->codes, N0 * 4, nx.N * 4));
+        CKS(alloc(nx.residuals, ix->residuals, N0 * (long long)pk, nx.N * (long long)pk));
+        CKS(alloc(nx.ucodes, ix->ucodes, ix->n_ucodes * 4, nx.n_ucodes * 4));
+        CKS(alloc(nx.doc_off, ix->doc_off, (D0 + 1) * 8, (D1 + 1) * 8));
+        CKS(alloc(nx.udoc_off, ix->udoc_off, (D0 + 1) * 8, (D1 + 1) * 8));
+        CKS(alloc(nx.ivf, ix->ivf, ix->ivf_len * 4, nx.ivf_len * 4));
+        if (last && ix->ivf_spare.cap) CKS(alloc(nx.ivf_spare, ix->ivf_spare, ix->ivf_len * 4, nx.ivf_len * 4));
+        if (TcDims::has(ix->dim) && nx.N > 0) CKS(alloc(nx.tok_inv_norm, ix->tok_inv_norm, N0 * 4, nx.N * 4));
+        CKS(nx.ivf_off.grow((size_t)(K + 1) * 8, 0, false));
+        // the spare offsets hold K + 1 entries whatever the documents: a rank that had them keeps their capacity
+        if (ix->ivf_off_spare.cap) CKS(nx.ivf_off_spare.grow(ix->ivf_off_spare.cap, 0, false));
         CKS(p.rlen.ensure((size_t)(D1 + 1) * 8));
         CKS(p.rulen.ensure((size_t)(D1 + 1) * 8));
-        CKS(p.seg.ensure(std::max<size_t>((size_t)p.L1 * 4, 16)));
+        CKS(p.seg.ensure(std::max<size_t>((size_t)nx.ivf_len * 4, 16)));
         CKS(p.seg_off.ensure((size_t)W * (K + 1) * 8));
         CK(cudaMemset(p.seg_off.p, 0, (size_t)W * (K + 1) * 8));  // a source without a piece has empty lists
         CKS(p.mn.ensure(16));
@@ -4995,11 +4965,11 @@ extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bou
             if (!piece(s, me, lo, hi)) continue;
             void **d = &rp[(size_t)s * XF_ITEMS];
             size_t *n = &rbytes[(size_t)s * XF_ITEMS];
-            d[XF_CODES] = p.codes.as<uint8_t>() + (size_t)tpos[s] * 4;
+            d[XF_CODES] = nx.codes.as<uint8_t>() + (size_t)tpos[s] * 4;
             n[XF_CODES] = (size_t)sz(s, me, SZ_TOK) * 4;
-            d[XF_RES] = p.residuals.as<uint8_t>() + (size_t)tpos[s] * pk;
+            d[XF_RES] = nx.residuals.as<uint8_t>() + (size_t)tpos[s] * pk;
             n[XF_RES] = (size_t)sz(s, me, SZ_TOK) * pk;
-            d[XF_UCODES] = p.ucodes.as<uint8_t>() + (size_t)upos[s] * 4;
+            d[XF_UCODES] = nx.ucodes.as<uint8_t>() + (size_t)upos[s] * 4;
             n[XF_UCODES] = (size_t)sz(s, me, SZ_UCODES) * 4;
             d[XF_TLEN] = p.rlen.as<long long>() + (lo - b[me]);
             d[XF_ULEN] = p.rulen.as<long long>() + (lo - b[me]);
@@ -5011,12 +4981,7 @@ extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bou
         }
     }
     auto transfer = [&]() -> pb_status {
-        struct Stream {
-            cudaStream_t s = nullptr;
-            ~Stream() {
-                if (s) cudaStreamDestroy(s);
-            }
-        } st;
+        OwnedStream st;
         const cudaError_t ce = cudaStreamCreateWithFlags(&st.s, cudaStreamNonBlocking);
         if (ce != cudaSuccess) {
             if (ix->group) ix->group->fail();  // the peers must not wait for me at the barriers below
@@ -5066,43 +5031,33 @@ extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bou
     };
     // the receiver's new doc_off / udoc_off (scans of the arrived lengths), inverted file and norms
     auto build = [&]() -> pb_status {
-        const long long D1 = p.D1;
+        const long long D1 = nx.D;
         DevBuf tmp, len;
         CK(cudaMemset(p.rlen.as<long long>() + D1, 0, 8));
         CK(cudaMemset(p.rulen.as<long long>() + D1, 0, 8));
-        CKS(exclusive_sum(p.rlen.as<long long>(), p.doc_off.as<long long>(), D1 + 1, tmp));
-        CKS(exclusive_sum(p.rulen.as<long long>(), p.udoc_off.as<long long>(), D1 + 1, tmp));
+        CKS(exclusive_sum(p.rlen.as<long long>(), nx.doc_off.as<long long>(), D1 + 1, tmp));
+        CKS(exclusive_sum(p.rulen.as<long long>(), nx.udoc_off.as<long long>(), D1 + 1, tmp));
         std::vector<long long> hoff((size_t)D1 + 1);
         long long u1 = 0, l1 = 0;
-        CK(cudaMemcpy(hoff.data(), p.doc_off.p, hoff.size() * 8, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(&u1, p.udoc_off.as<long long>() + D1, 8, cudaMemcpyDeviceToHost));
-        p.maxlen = 0;
-        for (long long j = 0; j < D1; ++j) p.maxlen = std::max<int>(p.maxlen, (int)(hoff[j + 1] - hoff[j]));
+        CK(cudaMemcpy(hoff.data(), nx.doc_off.p, hoff.size() * 8, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(&u1, nx.udoc_off.as<long long>() + D1, 8, cudaMemcpyDeviceToHost));
+        nx.max_doclen = longest_doc(hoff, D1);
         CKS(len.ensure((size_t)(K + 1) * 8));
         k_ivf_rebalance_count<<<(unsigned)((K + 256) / 256), 256>>>(p.seg_off.as<long long>(), W, K, len.as<long long>());
         CK(cudaGetLastError());
-        CKS(exclusive_sum(len.as<long long>(), p.ivf_off.as<long long>(), K + 1, tmp));
-        CK(cudaMemcpy(&l1, p.ivf_off.as<long long>() + K, 8, cudaMemcpyDeviceToHost));
-        if (hoff[D1] != p.N1 || u1 != p.U1 || l1 != p.L1)
+        CKS(exclusive_sum(len.as<long long>(), nx.ivf_off.as<long long>(), K + 1, tmp));
+        CK(cudaMemcpy(&l1, nx.ivf_off.as<long long>() + K, 8, cudaMemcpyDeviceToHost));
+        if (hoff[D1] != nx.N || u1 != nx.n_ucodes || l1 != nx.ivf_len)
             return pb_fail(PB_ERR_CUDA, "the received pieces (%lld tokens, %lld codes, %lld ivf entries) differ from the "
-                           "plan (%lld, %lld, %lld)", hoff[D1], u1, l1, p.N1, p.U1, p.L1);
-        if (p.L1 > 0)
+                           "plan (%lld, %lld, %lld)", hoff[D1], u1, l1, nx.N, nx.n_ucodes, nx.ivf_len);
+        if (nx.ivf_len > 0)
             k_ivf_rebalance_merge<<<grid, 256>>>(p.seg.as<uint32_t>(), p.seg_off.as<long long>(), p.meta.as<long long>(),
-                                                 p.meta.as<long long>() + W, W, K, p.ivf_off.as<long long>(),
-                                                 p.ivf.as<uint32_t>());
+                                                 p.meta.as<long long>() + W, W, K, nx.ivf_off.as<long long>(),
+                                                 nx.ivf.as<uint32_t>());
         CK(cudaGetLastError());
         // 1 / |c + w| of the new tokens and vmin / wmax over them, as an open computes them
-        if (TcDims::has(ix->dim) && p.N1 > 0) {
-            if (ix->N == 0) CKS(build_centroid_operands(ix));  // a rank opened empty has none yet
-            const float init[2] = {3.0e38f, 0.0f};
-            CK(cudaMemcpy(p.mn.p, init, 8, cudaMemcpyHostToDevice));
-            CKS(launch_min_vnorm(ix, p.codes.as<uint32_t>(), p.residuals.as<uint8_t>(), p.N1, p.tok_inv_norm.as<float>(),
-                                 p.mn.as<float>()));
-            float got[2] = {0.f, 0.f};
-            CK(cudaMemcpy(got, p.mn.p, 8, cudaMemcpyDeviceToHost));
-            p.vmin = got[0] < 1e30f ? got[0] : 0.0f;
-            p.wmax = got[1];
-        }
+        const float seed[2] = {3.0e38f, 0.0f};
+        CKS(token_norms(ix, nx, 0, seed, nx, p.mn));
         CK(cudaDeviceSynchronize());
         return PB_OK;
     };
@@ -5113,23 +5068,8 @@ extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bou
     CKS(gather_words(ix, &fin, 1, votes, true));
     CKS(first_failure(ix, votes, 1, " moving the documents; nothing changed"));
     if (changes) {
-        ix->codes.swap(p.codes);
-        ix->residuals.swap(p.residuals);
-        ix->ucodes.swap(p.ucodes);
-        ix->doc_off.swap(p.doc_off);
-        ix->udoc_off.swap(p.udoc_off);
-        ix->ivf.swap(p.ivf);
-        ix->ivf_off.swap(p.ivf_off);
-        ix->ivf_spare.swap(p.ivf_spare);
-        ix->tok_inv_norm.swap(p.tok_inv_norm);
-        ix->D = p.D1;
-        ix->N = p.N1;
+        publish(ix, nx, &nx);
         ix->doc_id_base = b[me];
-        ix->ivf_len = p.L1;
-        ix->n_ucodes = p.U1;
-        ix->max_doclen = p.maxlen;
-        ix->vmin = p.vmin;
-        ix->wmax = p.wmax;
     }
     if (out_bounds) std::copy(b.begin(), b.end(), out_bounds);
     return PB_OK;  // the old arrays are freed with p
