@@ -78,49 +78,6 @@ struct NcclApi {
 static NcclApi g_nccl;
 
 // ------------------------------------------------------------------------------------------
-// In-process shard group: the same two exchanges without NCCL, for ONE process that drives several shards
-// from several host threads (any mix of devices, including all shards on one GPU -- which is how the merge
-// kernels run under `pytest -m gpu` on a single-GPU box).  An all-gather is a host barrier, one
-// cudaMemcpyPeerAsync per peer into the caller's receive buffer, and a second barrier so nobody reuses a
-// send buffer that is still being read.
-// ------------------------------------------------------------------------------------------
-struct pb_shard_group {
-    int world = 0;
-    std::mutex mu;
-    std::condition_variable cv;
-    int arrived = 0;
-    unsigned long long gen = 0;
-    bool broken = false;
-    int joined = 0;
-    std::vector<const void *> send;
-    std::vector<const void *const *> table;  // per rank: the device pointers it sends in a rebalance, [destination][item]
-    std::vector<int> dev;
-    // false = a peer failed or did not arrive within the timeout; the group stays broken.  unbounded: wait for the
-    // peers however long they take (a peer that fails still breaks the group), for a peer known to be busy
-    bool barrier(bool unbounded = false) {
-        std::unique_lock<std::mutex> g(mu);
-        if (broken) return false;
-        const unsigned long long my = gen;
-        if (++arrived == world) {
-            arrived = 0;
-            ++gen;
-            cv.notify_all();
-            return true;
-        }
-        auto done = [&] { return gen != my || broken; };
-        if (unbounded) cv.wait(g, done);
-        else if (!cv.wait_for(g, std::chrono::seconds(60), done)) broken = true;
-        if (broken) cv.notify_all();
-        return !broken;
-    }
-    void fail() {
-        std::lock_guard<std::mutex> g(mu);
-        broken = true;
-        cv.notify_all();
-    }
-};
-
-// ------------------------------------------------------------------------------------------
 // errors
 // ------------------------------------------------------------------------------------------
 static thread_local std::string g_err;
@@ -317,6 +274,182 @@ struct PinnedRes {
     }
 };
 
+// ------------------------------------------------------------------------------------------
+// Cross-rank exchanges.  A rank reaches its peers over NCCL (one process per GPU) or through an in-process shard group:
+// ONE process drives several shards from several host threads (any mix of devices, including all shards on one GPU --
+// which is how the sharded paths run under `pytest -m gpu` on a single-GPU box).  ShardComm is one rank's end of
+// either; the search, the sharded update, the rebalance and the data-parallel k-means see only its collectives.
+// ------------------------------------------------------------------------------------------
+struct pb_shard_group {
+    int world = 0;
+    std::mutex mu;
+    std::condition_variable cv;
+    int arrived = 0;
+    unsigned long long gen = 0;
+    bool broken = false, failing = false;
+    std::vector<const void *const *> table;  // per rank: the device pointers it sends, [destination][item]
+    std::vector<int> dev;
+    // false = a peer failed or did not arrive within the timeout; the group stays broken.  unbounded: wait for the
+    // peers however long they take (a peer that fails still breaks the group), for a peer known to be busy.  ok =
+    // false: this rank failed; the group breaks once every rank has arrived, and every rank returns false
+    bool barrier(bool unbounded = false, bool ok = true) {
+        std::unique_lock<std::mutex> g(mu);
+        if (broken) return false;
+        const unsigned long long my = gen;
+        failing = failing || !ok;
+        if (++arrived == world) {
+            arrived = 0;
+            ++gen;
+            broken = failing;
+            cv.notify_all();
+            return !broken;
+        }
+        auto done = [&] { return gen != my || broken; };
+        if (unbounded) cv.wait(g, done);
+        else if (!cv.wait_for(g, std::chrono::seconds(60), done)) broken = true;
+        if (broken) cv.notify_all();
+        return !broken;
+    }
+    void fail() {
+        std::lock_guard<std::mutex> g(mu);
+        broken = true;
+        cv.notify_all();
+    }
+};
+
+struct ShardComm {
+    int rank = 0, world = 1, device = 0;
+    ncclComm_t nccl = nullptr;        // owned
+    pb_shard_group *group = nullptr;  // or a member of this group
+    ShardComm() = default;
+    ShardComm(const ShardComm &) = delete;  // the NCCL communicator is destroyed once
+    ShardComm &operator=(const ShardComm &) = delete;
+    ~ShardComm() {
+        if (nccl) g_nccl.CommDestroy(nccl);
+    }
+
+    // world 1 is a group of one and needs no NCCL
+    pb_status init_nccl(const uint8_t *id128, int r, int w, int dev) {
+        if (w < 1 || r < 0 || r >= w) return pb_fail(PB_ERR_INVALID, "bad rank %d / world %d", r, w);
+        if (joined()) return pb_fail(PB_ERR_INVALID, "communicator already initialised");
+        if (w > 1) {
+            if (!g_nccl.load()) return pb_fail(PB_ERR_COMM, "libnccl.so.2 not found (%s)", dlerror());
+            CK(cudaSetDevice(dev));
+            ncclUniqueId id;
+            memcpy(id.internal, id128, 128);
+            CKN(g_nccl.CommInitRank(&nccl, w, id, r));
+        }
+        rank = r, world = w, device = dev;
+        return PB_OK;
+    }
+    pb_status join(pb_shard_group *g, int r, int dev) {
+        if (r < 0 || r >= g->world) return pb_fail(PB_ERR_INVALID, "bad rank %d / world %d", r, g->world);
+        if (joined()) return pb_fail(PB_ERR_INVALID, "communicator already initialised");
+        std::lock_guard<std::mutex> lk(g->mu);
+        g->dev[r] = dev;
+        group = g, rank = r, world = g->world, device = dev;
+        return PB_OK;
+    }
+    bool joined() const { return nccl || group; }
+    // the peers must not wait for a rank that gave up: breaks an in-process group (NCCL keeps no such state)
+    void fail() {
+        if (group) group->fail();
+    }
+    // exchange() over NCCL needs its optional point-to-point symbols
+    bool has_p2p() const { return !nccl || g_nccl.has_p2p(); }
+
+    // every rank's `words` 64-bit words at `send`, into `recv` in rank order.  unbounded: the in-process group waits
+    // for late peers without its 60 s timeout (NCCL waits either way)
+    pb_status allgather(cudaStream_t stream, const void *send, void *recv, size_t words, bool unbounded = false) {
+        if (nccl) {
+            CKN(g_nccl.AllGather(send, recv, words, PB_NCCL_UINT64, nccl, stream));
+            return PB_OK;
+        }
+        return gather(stream, send, recv, words * 8, unbounded);
+    }
+
+    // in-place sum of `count` floats over the ranks, synchronized; the result is bit-identical on every rank (the
+    // in-process group gathers every rank's buffer into `stage` and sums it in rank order)
+    pb_status allreduce_sum(cudaStream_t stream, float *buf, size_t count, DevBuf &stage) {
+        if (world == 1) return PB_OK;
+        if (nccl) {
+            CKN(g_nccl.AllReduce(buf, buf, count, PB_NCCL_FLOAT32, PB_NCCL_SUM, nccl, stream));
+            CK(cudaStreamSynchronize(stream));
+            return PB_OK;
+        }
+        CKS(stage.ensure((size_t)world * count * 4));
+        CKS(gather(stream, buf, stage.p, count * 4, false));
+        k_sum_ranks<<<stage.cap ? 296 : 1, 256, 0, stream>>>(stage.as<float>(), world, (long long)count, buf);
+        CK(cudaGetLastError());
+        CK(cudaStreamSynchronize(stream));
+        return PB_OK;
+    }
+
+    // `items` pieces between every pair of ranks, synchronized: send_* are [destination][item], recv_* [source][item],
+    // and a piece's sizes agree at both ends.  Waits for late peers.  NCCL: my own piece by a device copy, the others
+    // by send / receive pairs in one group (has_p2p() must hold)
+    pb_status exchange(cudaStream_t stream, int items, const void *const *send_ptrs, const size_t *send_bytes,
+                       void *const *recv_ptrs, const size_t *recv_bytes) {
+        if (!nccl) return pull(stream, items, send_ptrs, recv_ptrs, recv_bytes, true, true);
+        for (int it = 0; it < items; ++it) {
+            const size_t i = (size_t)rank * items + it;
+            if (recv_bytes[i])
+                CK(cudaMemcpyAsync(recv_ptrs[i], send_ptrs[i], recv_bytes[i], cudaMemcpyDeviceToDevice, stream));
+        }
+        int res = g_nccl.GroupStart();
+        for (int r = 0; r < world && res == 0; ++r)
+            for (int it = 0; r != rank && it < items && res == 0; ++it) {
+                const size_t i = (size_t)r * items + it;
+                if (send_bytes[i]) res = g_nccl.Send(send_ptrs[i], send_bytes[i], PB_NCCL_UINT8, r, nccl, stream);
+            }
+        for (int s = 0; s < world && res == 0; ++s)
+            for (int it = 0; s != rank && it < items && res == 0; ++it) {
+                const size_t i = (size_t)s * items + it;
+                if (recv_bytes[i]) res = g_nccl.Recv(recv_ptrs[i], recv_bytes[i], PB_NCCL_UINT8, s, nccl, stream);
+            }
+        const int end = g_nccl.GroupEnd();
+        if (res == 0) res = end;
+        if (res != 0) return pb_fail(PB_ERR_COMM, "rebalance transfer failed: %s", g_nccl.GetErrorString(res));
+        CK(cudaStreamSynchronize(stream));
+        return PB_OK;
+    }
+
+  private:
+    // The in-process protocol of every collective: publish my table of send pointers ([destination][item]), a barrier,
+    // pull my pieces (recv / bytes [source][item]) from each source by peer copies, and a second barrier, after which
+    // the sources may reuse their tables and buffers.  A rank whose CUDA work fails still takes both barriers, so that
+    // no rank leaves while a peer reads its table or buffers; the barrier it fails at fails every rank and breaks the
+    // group, unless keep_group (the caller reports the error to its peers itself).  A CUDA error returns PB_ERR_CUDA, a
+    // broken or timed-out barrier PB_ERR_COMM.
+    pb_status pull(cudaStream_t stream, int items, const void *const *send, void *const *recv, const size_t *bytes,
+                   bool unbounded, bool keep_group) {
+        if (!group) return pb_fail(PB_ERR_COMM, "sharded handle without a transport");
+        cudaError_t e = cudaStreamSynchronize(stream);  // my send buffers are complete
+        group->table[rank] = send;
+        bool ok = group->barrier(unbounded, e == cudaSuccess || keep_group);
+        for (int s = 0; s < world && ok && e == cudaSuccess; ++s)
+            for (int it = 0; it < items && e == cudaSuccess; ++it) {
+                const size_t i = (size_t)s * items + it;
+                if (bytes[i])
+                    e = cudaMemcpyPeerAsync(recv[i], device, group->table[s][(size_t)rank * items + it], group->dev[s],
+                                            bytes[i], stream);
+            }
+        if (ok && e == cudaSuccess) e = cudaStreamSynchronize(stream);
+        ok = ok && group->barrier(unbounded, e == cudaSuccess || keep_group);
+        if (e != cudaSuccess) return pb_fail(PB_ERR_CUDA, "shard group exchange failed: %s", cudaGetErrorString(e));
+        if (!ok) return pb_fail(PB_ERR_COMM, "shard group: a peer failed or timed out");
+        return PB_OK;
+    }
+    // an all-gather of `bytes` per rank: every destination's entry is the one send buffer
+    pb_status gather(cudaStream_t stream, const void *send, void *recv, size_t bytes, bool unbounded) {
+        const std::vector<const void *> table((size_t)world, send);
+        std::vector<void *> dst((size_t)world);
+        for (int s = 0; s < world; ++s) dst[s] = static_cast<char *>(recv) + (size_t)s * bytes;
+        const std::vector<size_t> n((size_t)world, bytes);
+        return pull(stream, 1, table.data(), dst.data(), n.data(), unbounded, false);
+    }
+};
+
 // per-call scratch; a pool of these makes pb_search_batch re-entrant on one handle
 struct Workspace {
     cudaStream_t stream = nullptr;
@@ -487,9 +620,6 @@ struct pb_index : DocArrays {
     std::vector<std::unique_ptr<LaneWorker>> lane_workers;
     bool profiling = false;
     size_t st_budget = (size_t)8 << 30;  // workspace budget of one search call (PB_WS_BUDGET_MB)
-    ncclComm_t comm = nullptr;  // doc-sharded deployment: one rank per GPU
-    pb_shard_group *group = nullptr;  // or one host thread per shard inside this process (pb_index_group_join)
-    int rank = 0, world = 1;
     std::mutex mu;
     std::vector<std::unique_ptr<Workspace>> pool;
     // pb_search: concurrent single-query callers merged into shared batches (pb_index_set_coalescing; off by default)
@@ -507,6 +637,9 @@ struct pb_index : DocArrays {
         { std::lock_guard<std::mutex> g(gate); }
         return std::shared_lock<std::shared_mutex>(rw);
     }
+    // doc-sharded deployment (pb_index_comm_init / pb_index_group_join).  Declared last, so destroyed first: an NCCL
+    // communicator goes before the workspace streams it ran on
+    ShardComm comm;
 };
 
 // A workspace of the handle's pool for one call.  It goes back to the pool only after a call that ran to completion
@@ -1149,7 +1282,6 @@ extern "C" void pb_index_close(pb_index *ix) {
     cudaSetDevice(ix->device);
     ix->lane_workers.clear();  // joins the helper threads
     cudaDeviceSynchronize();
-    if (ix->comm) g_nccl.CommDestroy(ix->comm);
     delete ix;
 }
 
@@ -1212,7 +1344,7 @@ extern "C" pb_status pb_index_set_coalescing(pb_index *ix, const pb_coalesce_con
     if (cfg) {
         if (cfg->max_queries < 1 || cfg->max_wait_us < 0 || cfg->max_inflight < 1)
             return pb_fail(PB_ERR_INVALID, "coalescing: max_queries and max_inflight must be >= 1, max_wait_us >= 0");
-        if (cfg->max_queries > 1 && (ix->world > 1 || ix->group || ix->comm))
+        if (cfg->max_queries > 1 && ix->comm.joined())
             return pb_fail(PB_ERR_UNSUPPORTED, "coalescing on a doc-sharded handle: a collective needs the same order on every rank");
         c.max_queries = cfg->max_queries;
         c.max_wait_us = std::min(cfg->max_wait_us, 10000);
@@ -1441,35 +1573,6 @@ static pb_status launch_centroid_scores(pb_index *ix, Workspace &ws, int B, int 
     });
     CK(cudaGetLastError());
     if (launches) *launches += 2;
-    return PB_OK;
-}
-
-// all-gather of `count` 64-bit words per rank over whichever transport the handle joined.  unbounded: the in-process
-// group waits for late peers without its 60 s timeout (NCCL waits either way)
-static pb_status shard_allgather(pb_index *ix, cudaStream_t stream, const void *send, void *recv, size_t count,
-                                 bool unbounded = false) {
-    if (ix->comm) {
-        CKN(g_nccl.AllGather(send, recv, count, PB_NCCL_UINT64, ix->comm, stream));
-        return PB_OK;
-    }
-    pb_shard_group *g = ix->group;
-    if (!g) return pb_fail(PB_ERR_COMM, "sharded handle without a transport");
-    cudaError_t e = cudaStreamSynchronize(stream);  // my send buffer is complete
-    if (e != cudaSuccess) {
-        g->fail();
-        return pb_fail(PB_ERR_CUDA, "cudaStreamSynchronize failed: %s", cudaGetErrorString(e));
-    }
-    g->send[ix->rank] = send;
-    if (!g->barrier(unbounded)) return pb_fail(PB_ERR_COMM, "shard group: a peer failed or timed out");
-    for (int p = 0; p < g->world && e == cudaSuccess; ++p)
-        e = cudaMemcpyPeerAsync(static_cast<char *>(recv) + (size_t)p * count * 8, ix->device, g->send[p], g->dev[p],
-                                count * 8, stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);  // peers may reuse their send buffers after the barrier
-    if (e != cudaSuccess) {
-        g->fail();
-        return pb_fail(PB_ERR_CUDA, "shard group copy failed: %s", cudaGetErrorString(e));
-    }
-    if (!g->barrier()) return pb_fail(PB_ERR_COMM, "shard group: a peer failed or timed out");
     return PB_OK;
 }
 
@@ -1783,7 +1886,7 @@ static pb_status plan_search(pb_index *ix, const SearchIO &io, SearchPlan &plan)
     }
     plan.Mcap = std::max(M_max, 1);
     plan.top_k_max = (int)top_k_max;
-    plan.sharded = ix->world > 1;
+    plan.sharded = ix->comm.world > 1;
     // a shard with no documents still takes part in the exchanges
     plan.empty = all_empty || (ix->D == 0 && !plan.sharded);
     plan.prof = ix->profiling;
@@ -1801,20 +1904,20 @@ static thread_local bool g_search_agreed = false;
 // the deployment's D for the n_ivf_probe scaling; differing subsets refuse the call on every rank.
 enum { PX_STATUS, PX_D, PX_QB, PX_PRINT, PX_WORDS };
 static pb_status plan_exchange(pb_index *ix, Workspace &ws, pb_status local, u64 print, int *QB, SearchPlan &plan) {
-    const int G = ix->world;
+    const int G = ix->comm.world;
     long long mine[PX_WORDS] = {(long long)local, ix->D, *QB, (long long)print};
     std::vector<long long> all((size_t)G * PX_WORDS);
     CKS(ws.xrec.ensure(PX_WORDS * 8));
     CKS(ws.xall.ensure((size_t)G * PX_WORDS * 8));
     CK(cudaMemcpyAsync(ws.xrec.p, mine, PX_WORDS * 8, cudaMemcpyHostToDevice, ws.stream));
-    CKS(shard_allgather(ix, ws.stream, ws.xrec.p, ws.xall.p, PX_WORDS));
+    CKS(ix->comm.allgather(ws.stream, ws.xrec.p, ws.xall.p, PX_WORDS));
     CK(cudaMemcpyAsync(all.data(), ws.xall.p, all.size() * 8, cudaMemcpyDeviceToHost, ws.stream));
     CK(cudaStreamSynchronize(ws.stream));
     g_search_agreed = true;  // from here on every rank decides from the same words
     for (int r = 0; r < G; ++r) {
         const pb_status s = (pb_status)all[(size_t)r * PX_WORDS + PX_STATUS];
         if (s == PB_OK) continue;
-        if (r == ix->rank) return s;  // g_err holds my own message
+        if (r == ix->comm.rank) return s;  // g_err holds my own message
         return pb_fail(s, "rank %d of the group failed (status %d)", r, (int)s);
     }
     plan.D_total = 0;
@@ -1823,7 +1926,7 @@ static pb_status plan_exchange(pb_index *ix, Workspace &ws, pb_status local, u64
         if ((u64)w[PX_PRINT] != print)
             return pb_fail(PB_ERR_INVALID,
                            "the ranks were given different subsets or parameters (rank %d differs from rank %d)", r,
-                           ix->rank);
+                           ix->comm.rank);
         plan.D_total += w[PX_D];
         *QB = (int)std::min<long long>(*QB, w[PX_QB]);
     }
@@ -1934,9 +2037,9 @@ static pb_status plan_probe(pb_index *ix, Workspace &ws, const SearchIO &io, Sea
         CKS(plan_exchange(ix, ws, local, f.h, &QB, plan));
         if (elig) {  // global eligibility: every rank's rows, OR-ed on the device
             const size_t words = (size_t)plan.rows * plan.Wke;
-            CKS(ws.gelig.ensure(words * 4 * ix->world));
-            CKS(shard_allgather(ix, ws.stream, ws.elig.p, ws.gelig.p, words / 2));
-            k_or_ranks<<<ix->sm_count * 4, 256, 0, ws.stream>>>(ws.gelig.as<uint32_t>(), ix->world, (long long)words,
+            CKS(ws.gelig.ensure(words * 4 * ix->comm.world));
+            CKS(ix->comm.allgather(ws.stream, ws.elig.p, ws.gelig.p, words / 2));
+            k_or_ranks<<<ix->sm_count * 4, 256, 0, ws.stream>>>(ws.gelig.as<uint32_t>(), ix->comm.world, (long long)words,
                                                                ws.elig.as<uint32_t>());
             CK(cudaGetLastError());
         }
@@ -2431,11 +2534,11 @@ static pb_status cut(pb_index *ix, Workspace &ws, const SearchPlan &plan, const 
     if (sharded) {
         // exchange 1: every shard's sorted top-M cut keys (Mcap per query, ~0 past its M) -> global cut -> my members
         // (SURVEY 8e)
-        const int G = ix->world;
+        const int G = ix->comm.world;
         CKS(ws.gkeys.ensure((size_t)G * B * Mcap * 8));
         CKS(ws.krank.ensure((size_t)B * Mcap * 4));
-        CKS(shard_allgather(ix, ws.stream, ws.lkeys.p, ws.gkeys.p, (size_t)B * Mcap));
-        k_merge_cut<<<B, 1024, 0, ws.stream>>>(ws.gkeys.as<u64>(), G, ix->rank, B, pass.M, Mcap, (uint32_t)ix->doc_id_base,
+        CKS(ix->comm.allgather(ws.stream, ws.lkeys.p, ws.gkeys.p, (size_t)B * Mcap));
+        k_merge_cut<<<B, 1024, 0, ws.stream>>>(ws.gkeys.as<u64>(), G, ix->comm.rank, B, pass.M, Mcap, (uint32_t)ix->doc_id_base,
                                                ix->D, ix->doc_off.as<long long>(), ws.kept.as<uint32_t>(),
                                                ws.krank.as<uint32_t>(), ws.nkept.as<int>(),
                                                ws.tokp.as<long long>(), ws.counters.as<long long>() + 1, pass.d_qM);
@@ -2614,11 +2717,11 @@ static pb_status select_topk(pb_index *ix, Workspace &ws, const SearchIO &io, co
     const int Pm = pow2_at_least(Mcap);
     if (plan.sharded) {
         // exchange 2: (exact key | global approx rank) + (doc id | score) of every shard, merged on every rank
-        const int G = ix->world;
+        const int G = ix->comm.world;
         CKS(ws.gfkeys.ensure((size_t)G * B * Mcap * 8));
         CKS(ws.gpayload.ensure((size_t)G * B * Mcap * 8));
-        CKS(shard_allgather(ix, ws.stream, ws.fkeys.p, ws.gfkeys.p, (size_t)B * Mcap));
-        CKS(shard_allgather(ix, ws.stream, ws.payload.p, ws.gpayload.p, (size_t)B * Mcap));
+        CKS(ix->comm.allgather(ws.stream, ws.fkeys.p, ws.gfkeys.p, (size_t)B * Mcap));
+        CKS(ix->comm.allgather(ws.stream, ws.payload.p, ws.gpayload.p, (size_t)B * Mcap));
         CKS(ws.mslot.ensure((size_t)B * Mcap * 4));
         CKS(set_smem(k_merge_topk, (size_t)Pm * 8));
         k_merge_topk<<<B, 1024, (size_t)Pm * 8, ws.stream>>>(ws.gfkeys.as<u64>(), ws.gpayload.as<u64>(), G, B, Mcap,
@@ -2945,7 +3048,7 @@ static pb_status search_impl(pb_index *ix, const SearchIO &io) {
     // through the whole pipeline on its own workspace and stream (helper threads do the launching).  Not with a trace
     // (per-stage dumps), not doc-sharded (the exchanges are collective calls in batch order), not for small batches.
     int lanes = 1;
-    if (ix && io.qp && ix->lanes > 1 && !io.trace && ix->world == 1 && io.n_queries >= 16)
+    if (ix && io.qp && ix->lanes > 1 && !io.trace && ix->comm.world == 1 && io.n_queries >= 16)
         lanes = (int)std::min<int64_t>(ix->lanes, io.n_queries / 8);
     std::unique_lock<std::mutex> lane_lock;
     if (lanes > 1) {
@@ -2955,7 +3058,7 @@ static pb_status search_impl(pb_index *ix, const SearchIO &io) {
     if (lanes <= 1) {
         const pb_status st = run_search(ix, io);
         // the peers must not wait for a rank that gave up; a refusal every rank reached together leaves the group usable
-        if (st != PB_OK && ix && ix->group && !g_search_agreed) ix->group->fail();
+        if (st != PB_OK && ix && !g_search_agreed) ix->comm.fail();
         return st;
     }
     while ((int)ix->lane_workers.size() < lanes - 1) ix->lane_workers.emplace_back(new LaneWorker());
@@ -3171,7 +3274,7 @@ extern "C" pb_status pb_search(pb_index *ix, const float *query, int64_t n_query
     r.query = query, r.n_tokens = n_query_tokens, r.params = params, r.subset = subset, r.n_subset = n_subset;
     r.out_ids = out_ids, r.out_scores = out_scores, r.out_count = out_count;
     // a doc-sharded search is a collective, issued in the same order on every rank: never queued
-    if (!ix->coalesce_on || ix->world > 1 || ix->group || ix->comm) {
+    if (!ix->coalesce_on || ix->comm.joined()) {
         ix->coalescer.count_bypassed();
         return search_alone(ix, r);
     }
@@ -3435,17 +3538,9 @@ extern "C" pb_status pb_comm_unique_id(uint8_t *out128) {
 
 extern "C" pb_status pb_index_comm_init(pb_index *ix, const uint8_t *id128, int32_t rank, int32_t world) {
     if (!ix || !id128) return pb_fail(PB_ERR_INVALID, "null argument");
-    if (world < 1 || rank < 0 || rank >= world) return pb_fail(PB_ERR_INVALID, "bad rank %d / world %d", rank, world);
-    if (ix->comm) return pb_fail(PB_ERR_INVALID, "communicator already initialised");
-    if (world == 1) return PB_OK;
-    if (!g_nccl.load()) return pb_fail(PB_ERR_COMM, "libnccl.so.2 not found (%s)", dlerror());
-    CK(cudaSetDevice(ix->device));
-    ncclUniqueId id;
-    memcpy(id.internal, id128, 128);
-    CKN(g_nccl.CommInitRank(&ix->comm, world, id, rank));
-    pb_index_set_coalescing(ix, nullptr);  // a sharded search is a collective: arrival order is not a rank-agreed order
-    ix->rank = rank;
-    ix->world = world;
+    CKS(ix->comm.init_nccl(id128, rank, world, ix->device));
+    // a sharded search is a collective: arrival order is not a rank-agreed order
+    if (ix->comm.joined()) pb_index_set_coalescing(ix, nullptr);
     return PB_OK;
 }
 
@@ -3454,7 +3549,6 @@ extern "C" pb_status pb_shard_group_create(int32_t world, pb_shard_group **out) 
     if (!out || world < 1 || world > 64) return pb_fail(PB_ERR_INVALID, "shard group: world must be in [1, 64]");
     pb_shard_group *g = new pb_shard_group();
     g->world = world;
-    g->send.assign((size_t)world, nullptr);
     g->table.assign((size_t)world, nullptr);
     g->dev.assign((size_t)world, 0);
     *out = g;
@@ -3463,15 +3557,8 @@ extern "C" pb_status pb_shard_group_create(int32_t world, pb_shard_group **out) 
 extern "C" void pb_shard_group_destroy(pb_shard_group *g) { delete g; }
 extern "C" pb_status pb_index_group_join(pb_index *ix, pb_shard_group *g, int32_t rank) {
     if (!ix || !g) return pb_fail(PB_ERR_INVALID, "null argument");
-    if (rank < 0 || rank >= g->world) return pb_fail(PB_ERR_INVALID, "bad rank %d / world %d", rank, g->world);
-    if (ix->comm || ix->group) return pb_fail(PB_ERR_INVALID, "communicator already initialised");
-    std::lock_guard<std::mutex> lk(g->mu);
-    g->dev[rank] = ix->device;
-    ++g->joined;
+    CKS(ix->comm.join(g, rank, ix->device));
     pb_index_set_coalescing(ix, nullptr);  // as pb_index_comm_init
-    ix->group = g;
-    ix->rank = rank;
-    ix->world = g->world;
     return PB_OK;
 }
 
@@ -3885,83 +3972,33 @@ extern "C" pb_status pb_kmeans_fit(int32_t device, const float *samples, int64_t
 // group (peer copies + a rank-ordered sum, identical on every rank) when it came from pb_build_comm_group.
 // ------------------------------------------------------------------------------------------
 struct pb_build_comm {
-    int device = 0, rank = 0, world = 1;
-    ncclComm_t nccl = nullptr;
-    pb_shard_group *group = nullptr;
-    cudaStream_t stream = nullptr;
-    DevBuf stage;
+    OwnedStream stream;
+    DevBuf stage;  // every rank's buffer, gathered by the in-process all-reduce
+    ShardComm comm;  // declared last, so destroyed first: an NCCL communicator goes before the stream it ran on
 };
 
 extern "C" pb_status pb_build_comm_init(const uint8_t *id128, int32_t rank, int32_t world, int32_t device, pb_build_comm **out) {
     if (!id128 || !out) return pb_fail(PB_ERR_INVALID, "null argument");
-    if (world < 1 || rank < 0 || rank >= world) return pb_fail(PB_ERR_INVALID, "bad rank %d / world %d", rank, world);
     CKS(check_device(device));
     std::unique_ptr<pb_build_comm> c(new pb_build_comm());
-    c->device = device;
-    c->rank = rank;
-    c->world = world;
-    CK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-    if (world > 1) {
-        if (!g_nccl.load()) return pb_fail(PB_ERR_COMM, "libnccl.so.2 not found (%s)", dlerror());
-        ncclUniqueId id;
-        memcpy(id.internal, id128, 128);
-        CKN(g_nccl.CommInitRank(&c->nccl, world, id, rank));
-    }
+    CK(cudaStreamCreateWithFlags(&c->stream.s, cudaStreamNonBlocking));
+    CKS(c->comm.init_nccl(id128, rank, world, device));
     *out = c.release();
     return PB_OK;
 }
 extern "C" pb_status pb_build_comm_group(pb_shard_group *g, int32_t rank, int32_t device, pb_build_comm **out) {
     if (!g || !out) return pb_fail(PB_ERR_INVALID, "null argument");
-    if (rank < 0 || rank >= g->world) return pb_fail(PB_ERR_INVALID, "bad rank %d / world %d", rank, g->world);
     CKS(check_device(device));
     std::unique_ptr<pb_build_comm> c(new pb_build_comm());
-    c->device = device;
-    c->rank = rank;
-    c->world = g->world;
-    c->group = g;
-    CK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-    {
-        std::lock_guard<std::mutex> lk(g->mu);
-        g->dev[rank] = device;
-    }
+    CK(cudaStreamCreateWithFlags(&c->stream.s, cudaStreamNonBlocking));
+    CKS(c->comm.join(g, rank, device));
     *out = c.release();
     return PB_OK;
 }
 extern "C" void pb_build_comm_destroy(pb_build_comm *c) {
     if (!c) return;
-    cudaSetDevice(c->device);
-    if (c->nccl) g_nccl.CommDestroy(c->nccl);
-    if (c->stream) cudaStreamDestroy(c->stream);
+    cudaSetDevice(c->comm.device);
     delete c;
-}
-
-// in-place sum of `count` floats over the ranks; the result is bit-identical on every rank
-static pb_status build_allreduce(pb_build_comm *c, float *buf, size_t count) {
-    if (c->world == 1) return PB_OK;
-    if (c->nccl) {
-        CKN(g_nccl.AllReduce(buf, buf, count, PB_NCCL_FLOAT32, PB_NCCL_SUM, c->nccl, c->stream));
-        CK(cudaStreamSynchronize(c->stream));
-        return PB_OK;
-    }
-    pb_shard_group *g = c->group;
-    CKS(c->stage.ensure((size_t)c->world * count * 4));
-    cudaError_t e = cudaStreamSynchronize(c->stream);
-    g->send[c->rank] = buf;
-    if (e != cudaSuccess || !g->barrier()) {
-        g->fail();
-        return pb_fail(PB_ERR_COMM, "shard group: a peer failed or timed out");
-    }
-    for (int p = 0; p < g->world && e == cudaSuccess; ++p)
-        e = cudaMemcpyPeerAsync(c->stage.as<float>() + (size_t)p * count, c->device, g->send[p], g->dev[p], count * 4, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (e != cudaSuccess || !g->barrier()) {  // everyone has read every buffer: they may be overwritten now
-        g->fail();
-        return pb_fail(PB_ERR_COMM, "shard group all-reduce failed");
-    }
-    k_sum_ranks<<<c->stage.cap ? 296 : 1, 256, 0, c->stream>>>(c->stage.as<float>(), c->world, (long long)count, buf);
-    CK(cudaGetLastError());
-    CK(cudaStreamSynchronize(c->stream));
-    return PB_OK;
 }
 
 extern "C" pb_status pb_kmeans_fit_dp(pb_build_comm *c, const float *samples, int64_t n_local, int32_t dim, int64_t K,
@@ -3969,15 +4006,15 @@ extern "C" pb_status pb_kmeans_fit_dp(pb_build_comm *c, const float *samples, in
     if (!c || (!samples && n_local) || !out_centroids) return pb_fail(PB_ERR_INVALID, "null argument");
     if (n_local < 0 || K <= 0) return pb_fail(PB_ERR_INVALID, "bad sizes");
     CKS(BuiltDims::check(dim));
-    CK(cudaSetDevice(c->device));
+    CK(cudaSetDevice(c->comm.device));
     cudaDeviceProp prop;
-    CK(cudaGetDeviceProperties(&prop, c->device));
+    CK(cudaGetDeviceProperties(&prop, c->comm.device));
     const int sms = prop.multiProcessorCount;
     const long long n = n_local;
     // rank r seeds centroids [k0, k1) with distinct points of its shard; one all-reduce of the zero-padded table
     // gives every rank the same start
-    const long long k0 = K * c->rank / c->world, k1 = K * (c->rank + 1) / c->world, kmine = k1 - k0;
-    if (kmine > n) return pb_fail(PB_ERR_INVALID, "rank %d holds %lld points but seeds %lld centroids", c->rank, n, kmine);
+    const long long k0 = K * c->comm.rank / c->comm.world, k1 = K * (c->comm.rank + 1) / c->comm.world, kmine = k1 - k0;
+    if (kmine > n) return pb_fail(PB_ERR_INVALID, "rank %d holds %lld points but seeds %lld centroids", c->comm.rank, n, kmine);
     DevBuf dX, dC, dbias, dcodes, dacc, didx;
     CKS(upload(dX, samples, (size_t)std::max<long long>(n, 1) * dim * 4, PB_MEM_HOST));
     CKS(dC.ensure((size_t)K * dim * 4));
@@ -3986,35 +4023,35 @@ extern "C" pb_status pb_kmeans_fit_dp(pb_build_comm *c, const float *samples, in
     CKS(dacc.ensure((size_t)K * (dim + 1) * 4));  // [K][dim] sums followed by [K] counts: one all-reduce
     std::vector<long long> perm((size_t)n);
     for (long long i = 0; i < n; ++i) perm[i] = i;
-    uint64_t s = (seed + 0x9e3779b97f4a7c15ull * (uint64_t)(c->rank + 1)) * 6364136223846793005ull + 1442695040888963407ull;
+    uint64_t s = (seed + 0x9e3779b97f4a7c15ull * (uint64_t)(c->comm.rank + 1)) * 6364136223846793005ull + 1442695040888963407ull;
     for (long long i = 0; i < kmine; ++i) {
         s = s * 6364136223846793005ull + 1442695040888963407ull;
         long long j = i + (long long)((s >> 11) % (uint64_t)(n - i));
         std::swap(perm[i], perm[j]);
     }
-    CK(cudaMemsetAsync(dC.p, 0, (size_t)K * dim * 4, c->stream));
+    CK(cudaMemsetAsync(dC.p, 0, (size_t)K * dim * 4, c->stream.s));
     if (kmine > 0) {
         CKS(upload(didx, perm.data(), (size_t)kmine * 8, PB_MEM_HOST));
-        k_gather_rows<<<sms * 4, 256, 0, c->stream>>>(dX.as<float>(), didx.as<long long>(), kmine, dim, dC.as<float>() + (size_t)k0 * dim);
+        k_gather_rows<<<sms * 4, 256, 0, c->stream.s>>>(dX.as<float>(), didx.as<long long>(), kmine, dim, dC.as<float>() + (size_t)k0 * dim);
         CK(cudaGetLastError());
     }
-    CKS(build_allreduce(c, dC.as<float>(), (size_t)K * dim));
+    CKS(c->comm.allreduce_sum(c->stream.s, dC.as<float>(), (size_t)K * dim, c->stage));
     float *sums = dacc.as<float>(), *counts = dacc.as<float>() + (size_t)K * dim;
     KmeansAssign ka;
-    CKS(ka.init(dX.as<float>(), n, dim, K, sms, c->stream));
+    CKS(ka.init(dX.as<float>(), n, dim, K, sms, c->stream.s));
     for (int it = 0; it < niters; ++it) {
-        CKS(ka.run(dX.as<float>(), dC.as<float>(), dbias.as<float>(), dcodes.as<uint32_t>(), c->stream));
-        CK(cudaMemsetAsync(dacc.p, 0, (size_t)K * (dim + 1) * 4, c->stream));
-        if (n > 0) k_accumulate<<<sms * 8, 256, 0, c->stream>>>(dX.as<float>(), n, dim, dcodes.as<uint32_t>(), sums, counts);
+        CKS(ka.run(dX.as<float>(), dC.as<float>(), dbias.as<float>(), dcodes.as<uint32_t>(), c->stream.s));
+        CK(cudaMemsetAsync(dacc.p, 0, (size_t)K * (dim + 1) * 4, c->stream.s));
+        if (n > 0) k_accumulate<<<sms * 8, 256, 0, c->stream.s>>>(dX.as<float>(), n, dim, dcodes.as<uint32_t>(), sums, counts);
         CK(cudaGetLastError());
-        CKS(build_allreduce(c, dacc.as<float>(), (size_t)K * (dim + 1)));
-        k_update_centroids<<<sms * 4, 256, 0, c->stream>>>(dC.as<float>(), K, dim, sums, counts);
+        CKS(c->comm.allreduce_sum(c->stream.s, dacc.as<float>(), (size_t)K * (dim + 1), c->stage));
+        k_update_centroids<<<sms * 4, 256, 0, c->stream.s>>>(dC.as<float>(), K, dim, sums, counts);
         CK(cudaGetLastError());
     }
-    k_normalize_rows<<<sms * 4, 256, 0, c->stream>>>(dC.as<float>(), K, dim);  // kmeans.rs:415-419
+    k_normalize_rows<<<sms * 4, 256, 0, c->stream.s>>>(dC.as<float>(), K, dim);  // kmeans.rs:415-419
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(out_centroids, dC.p, (size_t)K * dim * 4, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaStreamSynchronize(c->stream));
+    CK(cudaMemcpyAsync(out_centroids, dC.p, (size_t)K * dim * 4, cudaMemcpyDeviceToHost, c->stream.s));
+    CK(cudaStreamSynchronize(c->stream.s));
     return PB_OK;
 }
 
@@ -4258,7 +4295,7 @@ static pb_status append_impl(pb_index *ix, pb_codec *codec, const float *embeddi
     if (space != PB_MEM_HOST && space != PB_MEM_DEVICE) return pb_fail(PB_ERR_INVALID, "bad memory_space %d", space);
     std::lock_guard<std::mutex> gate(ix->gate);
     std::unique_lock<std::shared_mutex> wr(ix->rw);
-    if (ix->comm || ix->group) return pb_fail(PB_ERR_UNSUPPORTED, "appends to a doc-sharded handle are not supported");
+    if (ix->comm.joined()) return pb_fail(PB_ERR_UNSUPPORTED, "appends to a doc-sharded handle are not supported");
     CKS(refuse_fixed_residuals(ix));
     if (index_dir && ix->doc_id_base != 0) return pb_fail(PB_ERR_UNSUPPORTED, "an index directory holds doc ids from 0");
     if (index_dir && batch_size <= 0) return pb_fail(PB_ERR_INVALID, "batch_size must be positive");
@@ -4295,7 +4332,7 @@ extern "C" pb_status pb_index_reserve(pb_index *ix, int64_t num_documents, int64
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
     std::lock_guard<std::mutex> gate(ix->gate);
     std::unique_lock<std::shared_mutex> wr(ix->rw);
-    if (ix->comm || ix->group) return pb_fail(PB_ERR_UNSUPPORTED, "appends to a doc-sharded handle are not supported");
+    if (ix->comm.joined()) return pb_fail(PB_ERR_UNSUPPORTED, "appends to a doc-sharded handle are not supported");
     CKS(refuse_fixed_residuals(ix));
     if (num_documents >= (1ll << 32) - 1 || num_embeddings < 0) return pb_fail(PB_ERR_INVALID, "bad reserve sizes");
     CK(cudaSetDevice(ix->device));
@@ -4507,7 +4544,7 @@ extern "C" pb_status pb_index_delete(pb_index *ix, const int64_t *doc_ids, int64
     if (out_deleted) *out_deleted = 0;
     std::lock_guard<std::mutex> gate(ix->gate);
     std::unique_lock<std::shared_mutex> wr(ix->rw);
-    if (ix->comm || ix->group) return pb_fail(PB_ERR_UNSUPPORTED, "deletes from a doc-sharded handle are not supported");
+    if (ix->comm.joined()) return pb_fail(PB_ERR_UNSUPPORTED, "deletes from a doc-sharded handle are not supported");
     CKS(refuse_fixed_residuals(ix));
     if (index_dir && ix->doc_id_base != 0) return pb_fail(PB_ERR_UNSUPPORTED, "an index directory holds doc ids from 0");
     DeletePrep p;
@@ -4541,16 +4578,16 @@ enum { SH_OP_DELETE = 1, SH_OP_APPEND = 2, SH_OP_APPEND_ENCODED = 3 };
 static pb_status gather_words(pb_index *ix, const long long *mine, int words, std::vector<long long> &all,
                               bool unbounded = false) {
     all.assign(mine, mine + words);
-    if (!ix->comm && !ix->group) return PB_OK;
-    all.resize((size_t)words * ix->world);
+    if (!ix->comm.joined()) return PB_OK;
+    all.resize((size_t)words * ix->comm.world);
     OwnedStream st;
     DevBuf send, recv;
     CK(cudaSetDevice(ix->device));
     CK(cudaStreamCreateWithFlags(&st.s, cudaStreamNonBlocking));
     CKS(send.ensure((size_t)words * 8));
-    CKS(recv.ensure((size_t)words * 8 * ix->world));
+    CKS(recv.ensure((size_t)words * 8 * ix->comm.world));
     CK(cudaMemcpy(send.p, mine, (size_t)words * 8, cudaMemcpyHostToDevice));
-    CKS(shard_allgather(ix, st.s, send.p, recv.p, (size_t)words, unbounded));
+    CKS(ix->comm.allgather(st.s, send.p, recv.p, (size_t)words, unbounded));
     CK(cudaStreamSynchronize(st.s));
     CK(cudaMemcpy(all.data(), recv.p, all.size() * 8, cudaMemcpyDeviceToHost));
     return PB_OK;
@@ -4558,10 +4595,10 @@ static pb_status gather_words(pb_index *ix, const long long *mine, int words, st
 
 // the status of the lowest failing rank, or PB_OK; the failing rank keeps its own message, the others name it
 static pb_status first_failure(pb_index *ix, const std::vector<long long> &all, int words, const char *what) {
-    for (int r = 0; r < ix->world; ++r) {
+    for (int r = 0; r < ix->comm.world; ++r) {
         const pb_status s = (pb_status)all[(size_t)r * words];
         if (s == PB_OK) continue;
-        if (r == ix->rank) {
+        if (r == ix->comm.rank) {
             const std::string own = g_err;
             return pb_fail(s, "rank %d: %s", r, own.c_str());
         }
@@ -4577,8 +4614,8 @@ static pb_status first_failure(pb_index *ix, const std::vector<long long> &all, 
 // documents (base [W + 1], base[W] = D_total) and first tokens (tok [W + 1]).
 static pb_status layout_vote(pb_index *ix, long long *rec, const char *args, std::vector<long long> &all,
                              std::vector<long long> &base, std::vector<long long> &tok) {
-    const int W = ix->world;
-    rec[LR_RANK] = ix->rank;
+    const int W = ix->comm.world;
+    rec[LR_RANK] = ix->comm.rank;
     rec[LR_WORLD] = W;
     rec[LR_BASE] = ix->doc_id_base;
     rec[LR_D] = ix->D;
@@ -4613,7 +4650,7 @@ static pb_status sharded_update(pb_index *ix, int op, pb_codec *codec, const flo
     if (out) *out = 0;
     std::lock_guard<std::mutex> gate(ix->gate);
     std::unique_lock<std::shared_mutex> wr(ix->rw);
-    const bool last = ix->rank == ix->world - 1;
+    const bool last = ix->comm.rank == ix->comm.world - 1;
     DeletePrep dp;
     AppendPrep ap;
     long long rec[LR_WORDS] = {};
@@ -4650,10 +4687,10 @@ static pb_status sharded_update(pb_index *ix, int op, pb_codec *codec, const flo
     // 2. exchange A and the verdict every rank reaches from the same records
     std::vector<long long> all, base, tok;
     CKS(layout_vote(ix, rec, "arguments", all, base, tok));
-    const long long D_total = base[ix->world];
+    const long long D_total = base[ix->comm.world];
     long long n_del = 0, del_before = 0;
-    for (int r = 0; r < ix->world; ++r) {
-        if (r < ix->rank) del_before += all[(size_t)r * LR_WORDS + LR_OWN];
+    for (int r = 0; r < ix->comm.world; ++r) {
+        if (r < ix->comm.rank) del_before += all[(size_t)r * LR_WORDS + LR_OWN];
         n_del += all[(size_t)r * LR_WORDS + LR_OWN];
     }
     if (op == SH_OP_DELETE && n_del == 0) return PB_OK;  // nothing changes, on any rank or on disk
@@ -4757,7 +4794,7 @@ extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bou
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
     std::lock_guard<std::mutex> gate(ix->gate);
     std::unique_lock<std::shared_mutex> wr(ix->rw);
-    const int W = ix->world, me = ix->rank;
+    const int W = ix->comm.world, me = ix->comm.rank;
     const long long K = ix->K;
     const size_t pk = (size_t)ix->packed;
     const int grid = ix->sm_count * 8;
@@ -4770,7 +4807,7 @@ extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bou
         f.put(bounds != nullptr);
         if (bounds) f.add(bounds, (size_t)(W + 1) * 8);
         rec[LR_PRINT] = (long long)f.h;
-        if (ix->comm && !g_nccl.has_p2p())
+        if (!ix->comm.has_p2p())
             return pb_fail(PB_ERR_COMM, "the NCCL library lacks ncclSend / ncclRecv / ncclGroupStart / ncclGroupEnd");
         CK(cudaSetDevice(ix->device));
         CK(cudaDeviceSynchronize());  // work earlier readers left queued (pb_search_batch_device) reads the arrays
@@ -4984,50 +5021,10 @@ extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bou
         OwnedStream st;
         const cudaError_t ce = cudaStreamCreateWithFlags(&st.s, cudaStreamNonBlocking);
         if (ce != cudaSuccess) {
-            if (ix->group) ix->group->fail();  // the peers must not wait for me at the barriers below
+            ix->comm.fail();  // the peers must not wait for me at the barriers of the exchange
             return pb_fail(PB_ERR_CUDA, "cudaStreamCreate failed: %s", cudaGetErrorString(ce));
         }
-        if (ix->comm) {  // NCCL: my own piece by a local copy, the others by send / receive pairs in one group
-            for (int it = 0; it < XF_ITEMS; ++it) {
-                const size_t i = (size_t)me * XF_ITEMS + it;
-                if (rbytes[i]) CK(cudaMemcpyAsync(rp[i], sp[i], rbytes[i], cudaMemcpyDeviceToDevice, st.s));
-            }
-            int res = g_nccl.GroupStart();
-            for (int r = 0; r < W && res == 0; ++r)
-                for (int it = 0; r != me && it < XF_ITEMS && res == 0; ++it) {
-                    const size_t i = (size_t)r * XF_ITEMS + it;
-                    if (sbytes[i]) res = g_nccl.Send(sp[i], sbytes[i], PB_NCCL_UINT8, r, ix->comm, st.s);
-                }
-            for (int s = 0; s < W && res == 0; ++s)
-                for (int it = 0; s != me && it < XF_ITEMS && res == 0; ++it) {
-                    const size_t i = (size_t)s * XF_ITEMS + it;
-                    if (rbytes[i]) res = g_nccl.Recv(rp[i], rbytes[i], PB_NCCL_UINT8, s, ix->comm, st.s);
-                }
-            const int end = g_nccl.GroupEnd();
-            if (res == 0) res = end;
-            if (res != 0) return pb_fail(PB_ERR_COMM, "rebalance transfer failed: %s", g_nccl.GetErrorString(res));
-            CK(cudaStreamSynchronize(st.s));
-            return PB_OK;
-        }
-        // in-process group: every rank publishes its send pointers, then each receiver pulls its pieces
-        pb_shard_group *g = ix->group;
-        if (!g) return pb_fail(PB_ERR_COMM, "sharded handle without a transport");
-        g->table[me] = sp.data();
-        if (!g->barrier(true)) return pb_fail(PB_ERR_COMM, "shard group: a peer failed");
-        cudaError_t e = cudaSuccess;
-        for (int s = 0; s < W && e == cudaSuccess; ++s)
-            for (int it = 0; it < XF_ITEMS && e == cudaSuccess; ++it) {
-                const size_t i = (size_t)s * XF_ITEMS + it;
-                if (rbytes[i])
-                    e = cudaMemcpyPeerAsync(rp[i], ix->device, g->table[s][(size_t)me * XF_ITEMS + it], g->dev[s], rbytes[i],
-                                            st.s);
-            }
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st.s);
-        // the senders' arrays and tables are read until every receiver is past this barrier
-        const bool ok = g->barrier(true);
-        if (e != cudaSuccess) return pb_fail(PB_ERR_CUDA, "rebalance peer copy failed: %s", cudaGetErrorString(e));
-        if (!ok) return pb_fail(PB_ERR_COMM, "shard group: a peer failed");
-        return PB_OK;
+        return ix->comm.exchange(st.s, XF_ITEMS, sp.data(), sbytes.data(), rp.data(), rbytes.data());
     };
     // the receiver's new doc_off / udoc_off (scans of the arrived lengths), inverted file and norms
     auto build = [&]() -> pb_status {

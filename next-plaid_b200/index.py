@@ -224,6 +224,26 @@ def _ptr(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
+def _per_rank(n: int, call) -> list:
+    """call(r) for r in range(n), one host thread per rank (the ranks of an in-process shard group); the results in
+    rank order, or the first rank's exception once every thread has finished"""
+    import threading
+    out, err = [None] * n, [None] * n
+
+    def run(r):
+        try:
+            out[r] = call(r)
+        except Exception as e:      # noqa: BLE001 - re-raised below
+            err[r] = e
+    ths = [threading.Thread(target=run, args=(r,)) for r in range(n)]
+    [t.start() for t in ths]
+    [t.join() for t in ths]
+    for e in err:
+        if e is not None:
+            raise e
+    return out
+
+
 class ShardGroup:
     """pb_shard_group: several shard handles of ONE process searched and changed together (one host thread per shard).
 
@@ -242,22 +262,8 @@ class ShardGroup:
 
     def _collective(self, call):
         """call(r, shard) from one thread per rank; the per-rank results, or the first rank's exception"""
-        import threading
-        out, err = [None] * len(self.shards), [None] * len(self.shards)
-
-        def run(r):
-            try:
-                out[r] = call(r, self.shards[r])
-            except Exception as e:      # noqa: BLE001 - re-raised below
-                err[r] = e
-        ths = [threading.Thread(target=run, args=(r,)) for r in range(len(self.shards))]
-        [t.start() for t in ths]
-        [t.join() for t in ths]
-        for e in err:
-            if e is not None:
-                raise e
-        self.all_results = out
-        return out
+        self.all_results = _per_rank(len(self.shards), lambda r: call(r, self.shards[r]))
+        return self.all_results
 
     def search_batch(self, queries, params=None, subset=None):
         return self._collective(lambda r, s: s.search_batch(queries, params, subset=subset))[0]
@@ -871,32 +877,24 @@ def kmeans_fit_dp(shards: Sequence[np.ndarray], K: int, niters: int = 4, seed: i
         finally:
             L.pb_build_comm_destroy(h)
         return out
-    import threading
     G = len(shards)
     g = C.c_void_p()
     _check(L.pb_shard_group_create(G, C.byref(g)))
-    outs, errs = [None] * G, [None] * G
 
     def run(r):
+        h = C.c_void_p()
+        _check(L.pb_build_comm_group(g, r, device, C.byref(h)))
+        x = np.ascontiguousarray(shards[r], np.float32)
+        out = np.zeros((K, dim), np.float32)
         try:
-            h = C.c_void_p()
-            _check(L.pb_build_comm_group(g, r, device, C.byref(h)))
-            x = np.ascontiguousarray(shards[r], np.float32)
-            out = np.zeros((K, dim), np.float32)
-            try:
-                _check(L.pb_kmeans_fit_dp(h, _ptr(x), x.shape[0], dim, K, niters, seed, _ptr(out)))
-            finally:
-                L.pb_build_comm_destroy(h)
-            outs[r] = out
-        except Exception as e:      # noqa: BLE001 - re-raised below
-            errs[r] = e
-    ths = [threading.Thread(target=run, args=(r,)) for r in range(G)]
-    [t.start() for t in ths]
-    [t.join() for t in ths]
-    L.pb_shard_group_destroy(g)
-    for e in errs:
-        if e is not None:
-            raise e
+            _check(L.pb_kmeans_fit_dp(h, _ptr(x), x.shape[0], dim, K, niters, seed, _ptr(out)))
+        finally:
+            L.pb_build_comm_destroy(h)
+        return out
+    try:
+        outs = _per_rank(G, run)
+    finally:
+        L.pb_shard_group_destroy(g)
     for o in outs[1:]:
         assert np.array_equal(o, outs[0]), "ranks disagree on the centroids"
     return outs[0]
