@@ -527,6 +527,10 @@ typedef struct pb_work_counters {
     int64_t filter_diag_pairs;   /* PB_FILTER_DIAG=1 only: (kept doc, query token) maxima compared for filter_err_ratio_e6 */
     int64_t n_a5_live_rows;      /* score-table rows the pruned first approximate pass gathered to bound the candidates */
     int64_t n_a5_dense_docs;     /* candidates it then scored on every row (its two rounds); 0 on the dense first pass */
+    int64_t table_diag_mismatch; /* PB_TABLE_DIAG=1 only: 32-bit words of the tensor-core probe's chunk maxima (from the
+                                  * GEMM epilogue) and of its live-row bitmap (from the collect kernel) that differ from
+                                  * what k_chunkmax16 and k_a5_live compute on the same table, over the sub-batches
+                                  * that were not redone on the exact path; 0 expected */
 } pb_work_counters;
 PB_API pb_status pb_last_work_counters(pb_index *ix, pb_work_counters *out);
 /* What the calling thread's last search staged from host memory (PB_OPEN_HOST_RESIDUALS; 0 otherwise): the kept docs of

@@ -459,7 +459,7 @@ struct Workspace {
     DevBuf Q, qoff, ST, partial, sel, cells, ncells, bitmap, cand, ncand, approx, keys, kept, nkept, tokp, maxkey,
         exact, fkeys, oids, oscores, ocounts, subset, subset_bits, elig, list, counters, lkeys, ST16, qrange, qflag, lsum, cand2, ncand2,  cellbits,
         gkeys, krank, payload, gfkeys, gpayload, cmax16, tau16, plist, pcount, Qi, Qh16t, Ql16t, ST16b, k1diag, k1rows, ulist, nulist, est, kept2, krank2, nkept2, tokp2, ktok2, qnmax, qexp, qrange_tc, mslot, slicecnt, rcmax, rcpairs, rcn, cellflags, estkey, srcrank, xpairs, xnpairs, needexact, gbase, fdiag,
-        a5floor, a5live, a5n1, a5n12, a5theta;
+        a5floor, a5live, a5n1, a5n12, a5theta, smax, tdlive, tdcmax, tdiag;
     // subsets: the call's ids, its rows' spans, the passes' per-query rows and n, the all-eligible lists' lengths, the
     // eligible counts, and the doc-sharded exchanges (plan record, every rank's eligibility rows)
     DevBuf subspan, qsub, listn, eligcnt, xrec, xall, gelig;
@@ -603,6 +603,8 @@ struct pb_index : DocArrays {
     int k1_margin = 1;         // E: code units an estimate-built 16-bit code may differ from the exact one (PB_K1_TC_E widens it)
     int cent_exp = 0;          // centroids enter the tensor-core operands scaled by 2^cent_exp (max norm in [1, 2))
     bool k1_diag = false;      // also run the exact table and report the largest code difference (PB_K1_TC_DIAG=1)
+    bool table_diag = false;   // PB_TABLE_DIAG=1: rerun k_chunkmax16 and k_a5_live on the tensor-core table and count the
+                               // words the fused chunk maxima and live bits differ in
     DevBuf cent_h16t, cent_l16t;  // its centroid operands: fp16 hi / lo, MMA tile order
     int approx_grid = 8;       // k_approx16 CTAs per SM and query (PB_APPROX_GRID)
     bool a5_prune = true;      // bound the first pass from the live score-table rows (PB_A5_PRUNE=0: dense first pass)
@@ -1214,6 +1216,7 @@ pb_status pb_index_finalize(pb_index *ix) {
         if (const char *e = getenv("PB_LANES")) ix->lanes = std::min(8, std::max(1, atoi(e)));
         if (const char *e = getenv("PB_PROBE16")) ix->probe16 = atoi(e) != 0;
         if (const char *e = getenv("PB_K1_TC_DIAG")) ix->k1_diag = atoi(e) != 0;
+        if (const char *e = getenv("PB_TABLE_DIAG")) ix->table_diag = atoi(e) != 0;
         if (const char *e = getenv("PB_K1_TC")) ix->k1_tc = atoi(e) != 0;
         if (const char *e = getenv("PB_K1_TC_E")) ix->k1_margin = std::max(1, atoi(e));
         if (const char *e = getenv("PB_APPROX_GRID")) ix->approx_grid = std::max(1, atoi(e));
@@ -1415,8 +1418,11 @@ static bool k1_tc_usable(const pb_index *ix) {
 }
 
 // the 16-bit score table from the split-fp16 wgmma GEMM (k_scores16_tc) into `table`; `flags` gets the per-query
-// out-of-range bits the exact kernel would set in qflag
-static pb_status launch_k1_table(pb_index *ix, Workspace &ws, int B, int QS, unsigned short *table, int *flags) {
+// out-of-range bits the exact kernel would set in qflag; slab_max (or null) the table's 16-row slab maxima
+// (8 ceil(K / 128) slabs of k1_slab_rows(B, QS) codes)
+static int k1_slab_rows(int B, int QS) { return (int)(((long long)B * QS + 127) / 128) * 128; }
+static pb_status launch_k1_table(pb_index *ix, Workspace &ws, int B, int QS, unsigned short *table, int *flags,
+                                 unsigned short *slab_max) {
     const int n_groups = (int)(((long long)B * QS + 127) / 128);
     const size_t qelems = (size_t)n_groups * 128 * ix->dim;
     CKS(ws.Qh16t.ensure(qelems * 2));
@@ -1434,7 +1440,7 @@ static pb_status launch_k1_table(pb_index *ix, Workspace &ws, int B, int QS, uns
         KEV_BEGIN(PB_KERNEL_SCORES);
         kern<<<tiles, 288, sm, ws.stream>>>(ix->cent_h16t.as<__half>(), ix->cent_l16t.as<__half>(), ix->K,
                                             ws.Qh16t.as<__half>(), ws.Ql16t.as<__half>(), n_groups, B, QS,
-                                            ws.qoff.as<int>(), ws.qrange_tc.as<float2>(), table, flags);
+                                            ws.qoff.as<int>(), ws.qrange_tc.as<float2>(), table, flags, slab_max);
         KEV_END(PB_KERNEL_SCORES);
         CK(cudaGetLastError());
         return PB_OK;
@@ -1447,7 +1453,7 @@ static pb_status launch_k1_diag(pb_index *ix, Workspace &ws, int B, int QS) {
     CKS(ws.ST16b.ensure((size_t)B * ix->K * QS * 2));
     CKS(ws.k1diag.ensure((size_t)(B + 4) * 4));
     CK(cudaMemsetAsync(ws.k1diag.p, 0, (size_t)(B + 4) * 4, ws.stream));
-    CKS(launch_k1_table(ix, ws, B, QS, ws.ST16b.as<unsigned short>(), ws.k1diag.as<int>() + 4));
+    CKS(launch_k1_table(ix, ws, B, QS, ws.ST16b.as<unsigned short>(), ws.k1diag.as<int>() + 4, nullptr));
     k_diff16<<<dim3(ix->sm_count, B), 256, 0, ws.stream>>>(ws.ST16.as<unsigned short>(), ws.ST16b.as<unsigned short>(),
                                                           ws.qoff.as<int>(), ix->K, QS, ws.k1diag.as<int>());
     CK(cudaGetLastError());
@@ -1467,10 +1473,11 @@ static int probe_chunk_rows(long long K, int n, int *n_chunks) {
 static int probe16_cap(int n) { return n * std::max(2, 128 / n); }
 
 // The threshold-first probe up to its collect kernel: the candidate lists cleared, every chunk's largest code
-// (k_chunkmax16) and each query token's threshold, the n-th largest of them (k_tau16).  *d_fallback is the device flag
-// k_tau16 and the kernels after it raise when a query cannot take this path.
+// (k_chunkmax16 from the table, or k_chunkmax_slabs from the slab maxima the tensor-core table's epilogue kept) and
+// each query token's threshold, the n-th largest of them (k_tau16).  *d_fallback is the device flag k_tau16 and the
+// kernels after it raise when a query cannot take this path.
 static pb_status probe16_thresholds(pb_index *ix, Workspace &ws, int B, int QS, int n, int n_chunks, int chunk_rows,
-                                    const int *qn, int **d_fallback) {
+                                    const int *qn, const unsigned short *slab_max, int **d_fallback) {
     const int cap = probe16_cap(n);
     CKS(ws.cmax16.ensure((size_t)B * n_chunks * QS * 2));
     CKS(ws.tau16.ensure((size_t)B * QS * 4));
@@ -1479,8 +1486,12 @@ static pb_status probe16_thresholds(pb_index *ix, Workspace &ws, int B, int QS, 
     CK(cudaMemsetAsync(ws.plist.p, 0, (size_t)B * QS * cap * 8, ws.stream));
     CK(cudaMemsetAsync(ws.pcount.p, 0, (size_t)B * QS * 4 + 16, ws.stream));
     int *fb = ws.pcount.as<int>() + (size_t)B * QS;
-    k_chunkmax16<<<dim3((n_chunks + 3) / 4, B), 128, 0, ws.stream>>>(ws.ST16.as<unsigned short>(), ix->K, QS, n_chunks,
-                                                                     chunk_rows, ws.cmax16.as<unsigned short>());
+    if (slab_max)
+        k_chunkmax_slabs<<<dim3(n_chunks, (B * QS + 511) / 512), 256, 0, ws.stream>>>(
+            slab_max, ix->K, B, QS, k1_slab_rows(B, QS) / 128, n_chunks, chunk_rows, ws.cmax16.as<unsigned short>());
+    else
+        k_chunkmax16<<<dim3((n_chunks + 3) / 4, B), 128, 0, ws.stream>>>(ws.ST16.as<unsigned short>(), ix->K, QS,
+                                                                         n_chunks, chunk_rows, ws.cmax16.as<unsigned short>());
     k_tau16<<<dim3(QS, B), 32, 0, ws.stream>>>(ws.cmax16.as<unsigned short>(), ws.qoff.as<int>(), QS, n, n_chunks,
                                               ws.qflag.as<int>(), ws.tau16.as<uint32_t>(), fb, qn);
     *d_fallback = fb;
@@ -1494,19 +1505,31 @@ static int pow2_at_least(int x) {
     return P;
 }
 
+// live rows the pruned first approximate pass aims at per query token (k_a5_floor), and the words per query of its
+// live-row bitmap (16-byte rows, so that k_a5_bound can bulk-copy one)
+static long long a5_live_rows(const pb_index *ix) { return ix->a5_live >= 0 ? ix->a5_live : ix->K / 512; }
+static long long a5_live_stride(long long K) { return ((K + 31) / 32 + 3) & ~3ll; }
+
 // a2 + a3 on the tensor-core table.  Nothing is read back here: a flagged query or a probe-list overflow raises
 // *d_fallback on the device, the kernels after it stay memory-safe, and the caller redoes the sub-batch on the
 // exact path once it sees the flag at the end.
 // n: the pass's largest n_ivf_probe; qn / qhas / qthr: each query's own n and threshold, or null (uniform pass).
+// live: the pass prunes its first approximate pass; the floors of a5 (k_a5_floor, on a sample of the table) are taken
+// before the collect kernel, which then also writes the live-row bitmap from its one stream of the table (ws.a5floor,
+// ws.a5live, read by approx_scores).  On a pass that raises *d_fallback the bitmap may be stale or partly written;
+// approx_scores still runs on it (memory-safe: the bits only select among a doc's own code rows) and the redo on the
+// exact path replaces everything that pass produced.
 static pb_status run_k1_tc(pb_index *ix, Workspace &ws, int B, int QS, int nq_max, int n, const int *qn, int has_thr,
-                           float thr, const int *qhas, const float *qthr, bool batched, long long slab, int *L,
-                           int *cells_cap_out, const int **d_fallback_out) {
+                           float thr, const int *qhas, const float *qthr, bool batched, long long slab, bool live,
+                           int *L, int *cells_cap_out, const int **d_fallback_out) {
     int n_chunks = 0;
     const int chunk_rows = probe_chunk_rows(ix->K, n, &n_chunks);
     const int cm = 2 * ix->k1_margin + 1;
     CKS(ws.Qi.ensure((size_t)B * QS * ix->dim * 4));
     k_interleave_query_rows<<<dim3(8, B), 256, 0, ws.stream>>>(ws.Q.as<float>(), ws.qoff.as<int>(), QS, ix->dim, ws.Qi.as<float>());
-    CKS(launch_k1_table(ix, ws, B, QS, ws.ST16.as<unsigned short>(), ws.qflag.as<int>()));
+    const int tiles = (int)((ix->K + 127) / 128);
+    CKS(ws.smax.ensure((size_t)tiles * 8 * k1_slab_rows(B, QS) * 2));
+    CKS(launch_k1_table(ix, ws, B, QS, ws.ST16.as<unsigned short>(), ws.qflag.as<int>(), ws.smax.as<unsigned short>()));
     L[PB_STAGE_CENTROID_SCORES] += 4;
     const int cap = probe16_cap(n);
     const int cells_cap = (int)std::min<long long>((long long)QS * n, ix->K);
@@ -1517,10 +1540,42 @@ static pb_status run_k1_tc(pb_index *ix, Workspace &ws, int B, int QS, int nq_ma
     CKS(ws.nulist.ensure((size_t)B * 4 + 16));
     CKS(ws.k1rows.ensure((size_t)B * cells_cap * QS * 4));
     int *d_fallback = nullptr;
-    CKS(probe16_thresholds(ix, ws, B, QS, n, n_chunks, chunk_rows, qn, &d_fallback));
-    k_collect16_tc<<<dim3((n_chunks + 3) / 4, B), 128, 0, ws.stream>>>(
+    CKS(probe16_thresholds(ix, ws, B, QS, n, n_chunks, chunk_rows, qn, ws.smax.as<unsigned short>(), &d_fallback));
+    const long long live_stride = a5_live_stride(ix->K);
+    if (live) {
+        CKS(ws.a5floor.ensure((size_t)B * QS * 4));
+        CKS(ws.a5live.ensure((size_t)B * live_stride * 4));
+        k_a5_floor<<<dim3(QS / 8, B), 256, 0, ws.stream>>>(ws.ST16.as<unsigned short>(), ws.qoff.as<int>(), ix->K, QS,
+                                                           a5_live_rows(ix), ws.a5floor.as<uint32_t>());
+        L[PB_STAGE_PROBE] += 1;
+    }
+    (live ? k_collect16_tc<true> : k_collect16_tc<false>)<<<dim3((n_chunks + 3) / 4, B), 128, 0, ws.stream>>>(
         ws.ST16.as<unsigned short>(), ws.Q.as<float>(), ws.qoff.as<int>(), ix->centroids.as<float>(), ix->dim, cm, ix->K, QS,
-        n_chunks, chunk_rows, ws.tau16.as<uint32_t>(), cap, ws.pcount.as<int>(), ws.plist.as<u64>(), d_fallback);
+        n_chunks, chunk_rows, ws.tau16.as<uint32_t>(), cap, ws.pcount.as<int>(), ws.plist.as<u64>(), d_fallback,
+        live ? ws.a5floor.as<uint32_t>() : nullptr, live ? ws.a5live.as<uint32_t>() : nullptr, live_stride);
+    // PB_TABLE_DIAG: the standalone kernels on the same table, compared word by word with the chunk maxima from the
+    // slab maxima and with the collect kernel's live bits
+    if (ix->table_diag) {
+        CKS(ws.tdcmax.ensure((size_t)B * n_chunks * QS * 2));
+        CKS(ws.tdiag.ensure(16));
+        CK(cudaMemsetAsync(ws.tdiag.p, 0, 16, ws.stream));
+        k_chunkmax16<<<dim3((n_chunks + 3) / 4, B), 128, 0, ws.stream>>>(ws.ST16.as<unsigned short>(), ix->K, QS, n_chunks,
+                                                                         chunk_rows, ws.tdcmax.as<unsigned short>());
+        k_words_diff<<<dim3(4, B), 256, 0, ws.stream>>>(ws.cmax16.as<uint32_t>(), ws.tdcmax.as<uint32_t>(),
+                                                        (long long)n_chunks * QS / 2, (long long)n_chunks * QS / 2,
+                                                        d_fallback, ws.tdiag.as<unsigned long long>());
+        L[PB_STAGE_PROBE] += 2;
+        if (live) {
+            CKS(ws.tdlive.ensure((size_t)B * live_stride * 4));
+            k_a5_live<<<dim3(ix->sm_count * 2, B), 256, 0, ws.stream>>>(ws.ST16.as<unsigned short>(), ix->K, QS,
+                                                                         ws.a5floor.as<uint32_t>(), ws.tdlive.as<uint32_t>(),
+                                                                         live_stride);
+            k_words_diff<<<dim3(4, B), 256, 0, ws.stream>>>(ws.a5live.as<uint32_t>(), ws.tdlive.as<uint32_t>(),
+                                                            (ix->K + 31) / 32, live_stride, d_fallback,
+                                                            ws.tdiag.as<unsigned long long>());
+            L[PB_STAGE_PROBE] += 2;
+        }
+    }
     k_topn_merge<<<dim3(QS, B), 32, 0, ws.stream>>>(ws.plist.as<u64>(), ws.qoff.as<int>(), QS, n, cap / n, ws.sel.as<u64>(),
                                                   nullptr, 0, qn);
     // the selected centroids, their exact rows, the variant's threshold rule
@@ -1966,7 +2021,8 @@ static pb_status plan_probe(pb_index *ix, Workspace &ws, const SearchIO &io, Sea
     bool elig = false;
     for (int64_t b = 0; b < Bt; ++b) elig = elig || (plan.qrow[(size_t)b] >= 0 && !plan.qbatched[(size_t)b]);
 
-    // ---- the raw sub-batch bound: the score tables (16-bit always, fp32 only on the exact path) and the per-(query,
+    // ---- the raw sub-batch bound: the score tables (16-bit always, fp32 only on the exact path, the 16-row slab maxima
+    // of the 16-bit one on the tensor-core path) and the per-(query,
     // doc) scratch (candidate lists, code sums, approximate scores, cut keys, bitmap: 24.2 bytes per document; the
     // live-row bitmap of the pruned first pass: 1 bit per centroid) share one budget.  A host-tier handle also stages up
     // to Mcap docs of max_doclen rows per query (residuals, codes, 1 / |v|); a call with subsets holds a doc row and
@@ -1974,7 +2030,8 @@ static pb_status plan_probe(pb_index *ix, Workspace &ws, const SearchIO &io, Sea
     int nq_max_all = 0;
     for (int64_t b = 0; b < Bt; ++b) nq_max_all = std::max<int>(nq_max_all, (int)(io.q_off[b + 1] - io.q_off[b]));
     const int QS_all = query_row_tokens(nq_max_all);
-    const size_t per_q_all = (size_t)ix->K * QS_all * (k1_tc_usable(ix) ? 2 : 6) + (size_t)ix->D * 24 + (size_t)ix->D / 8 + (size_t)ix->K / 8 + 4096 +
+    const size_t per_q_all = (size_t)ix->K * QS_all * (k1_tc_usable(ix) ? 2 : 6) +
+                             (k1_tc_usable(ix) ? (size_t)ix->K * QS_all / 8 : 0) + (size_t)ix->D * 24 + (size_t)ix->D / 8 + (size_t)ix->K / 8 + 4096 +
                              (ix->host_tier ? (size_t)plan.Mcap * std::max(ix->max_doclen, 1) * (ix->packed + 8) : 0) +
                              (plan.rows ? (size_t)plan.Wd * 4 + (elig ? (size_t)plan.Wke * 4 : 0) : 0);
     int QB = (int)std::max<size_t>(1, std::min<size_t>((size_t)Bt, ix->st_budget / std::max(g_budget_div, 1) / per_q_all));
@@ -2280,7 +2337,7 @@ static pb_status centroid_scores(pb_index *ix, Workspace &ws, Pass &pass) {
     }
     if (pass.use_tc)
         return run_k1_tc(ix, ws, B, QS, pass.nq_max, pass.n, pass.d_qn, pass.has_thr, pass.thr, pass.d_qhas, pass.d_qthr,
-                         pass.batched, pass.slab, L, &pass.cells_cap, &pass.d_probe_fallback);
+                         pass.batched, pass.slab, pass.prune, L, &pass.cells_cap, &pass.d_probe_fallback);
     CKS(launch_centroid_scores(ix, ws, B, QS, &L[PB_STAGE_CENTROID_SCORES], with16));
     // PB_K1_TC_DIAG: the tensor-core table next to the exact one, compared code by code
     if (pass.fast && ix->k1_diag && ix->cent_h16t.p) CKS(launch_k1_diag(ix, ws, B, QS));
@@ -2344,7 +2401,7 @@ static pb_status probe(pb_index *ix, Workspace &ws, const SearchPlan &plan, Pass
     pass.probe_list_only = !thr_path;
     if (thr_path) {
         const int cap = probe16_cap(n);
-        CKS(probe16_thresholds(ix, ws, B, QS, n, t_chunks, t_rows, pass.d_qn, &d_fallback));
+        CKS(probe16_thresholds(ix, ws, B, QS, n, t_chunks, t_rows, pass.d_qn, nullptr, &d_fallback));
         pass.d_probe_fallback = d_fallback;
         k_collect16<<<dim3((t_chunks + 3) / 4, B), 128, 0, ws.stream>>>(
             ws.ST16.as<unsigned short>(), ws.ST.as<float>(), ix->K, QS, t_chunks, t_rows, ws.tau16.as<uint32_t>(), cap,
@@ -2423,20 +2480,22 @@ static pb_status approx_scores(pb_index *ix, Workspace &ws, const SearchPlan &pl
         if (pass.prune) {
             // the bound U of every candidate from the live rows, then k_approx16 on the two rounds that can reach the
             // band (k_approx16.cuh); U lives in ws.approx and the round lists in ws.keys until the re-check overwrites them
-            CKS(ws.a5floor.ensure((size_t)B * QS * 4));
-            const long long live_stride = ((ix->K + 31) / 32 + 3) & ~3ll;  // words per query, 16-byte rows
-            CKS(ws.a5live.ensure((size_t)B * live_stride * 4));
+            const long long live_stride = a5_live_stride(ix->K);
             CKS(ws.a5n1.ensure((size_t)B * 4 + 16));
             CKS(ws.a5n12.ensure((size_t)B * 4 + 16));
             CKS(ws.a5theta.ensure((size_t)B * 4 + 16));
-            const long long n_live = ix->a5_live >= 0 ? ix->a5_live : ix->K / 512;
             const int M1 = pass.M1;
             uint32_t *ub = ws.approx.as<uint32_t>(), *rl = ws.keys.as<uint32_t>();
             int *n1 = ws.a5n1.as<int>(), *n12 = ws.a5n12.as<int>();
-            k_a5_floor<<<dim3(QS / 8, B), 256, 0, ws.stream>>>(st16, ws.qoff.as<int>(), ix->K, QS, n_live,
-                                                               ws.a5floor.as<uint32_t>());
-            k_a5_live<<<dim3(ix->sm_count * 2, B), 256, 0, ws.stream>>>(st16, ix->K, QS, ws.a5floor.as<uint32_t>(),
-                                                                         ws.a5live.as<uint32_t>(), live_stride);
+            if (!pass.use_tc) {  // the tensor-core pass took the floors and the live bits with its probe (run_k1_tc)
+                CKS(ws.a5floor.ensure((size_t)B * QS * 4));
+                CKS(ws.a5live.ensure((size_t)B * live_stride * 4));
+                k_a5_floor<<<dim3(QS / 8, B), 256, 0, ws.stream>>>(st16, ws.qoff.as<int>(), ix->K, QS, a5_live_rows(ix),
+                                                                   ws.a5floor.as<uint32_t>());
+                k_a5_live<<<dim3(ix->sm_count * 2, B), 256, 0, ws.stream>>>(st16, ix->K, QS, ws.a5floor.as<uint32_t>(),
+                                                                             ws.a5live.as<uint32_t>(), live_stride);
+                L[PB_STAGE_APPROX] += 2;
+            }
             // the bitmap in shared memory up to K = 2^19 (64 KiB, two CTAs per SM), then a5_waves waves of resident
             // CTAs spread over the batch, each a contiguous range of its query's candidates (k_approx16.cuh; the
             // default of 8 waves is measured in DESIGN.md 4b)
@@ -2466,7 +2525,7 @@ static pb_status approx_scores(pb_index *ix, Workspace &ws, const SearchPlan &pl
                                                 ws.lsum.as<uint32_t>(), nullptr);
             list = rl;
             list_n = n12;
-            L[PB_STAGE_APPROX] += 7;
+            L[PB_STAGE_APPROX] += 5;
         } else {
             approx16<<<ga, 256, 0, ws.stream>>>(st16, ws.qoff.as<int>(), ix->K, QS, ix->ucodes.as<uint32_t>(),
                                                 ix->udoc_off.as<long long>(), list, ix->D, list_n, nullptr,
@@ -2805,6 +2864,11 @@ static pb_status finish(pb_index *ix, Workspace &ws, const SearchIO &io, const S
         CK(cudaMemcpy(got, ws.fdiag.p, 16, cudaMemcpyDeviceToHost));
         w.filter_err_ratio_e6 = std::max<long long>(w.filter_err_ratio_e6, (long long)got[0]);
         w.filter_diag_pairs += (long long)got[1];
+    }
+    if (pass.use_tc && ix->table_diag) {
+        unsigned long long got = 0;
+        CK(cudaMemcpy(&got, ws.tdiag.p, 8, cudaMemcpyDeviceToHost));
+        w.table_diag_mismatch += (long long)got;
     }
     if (pass.fast && ix->k1_diag && ws.k1diag.p) {
         int got[2] = {0, 0};

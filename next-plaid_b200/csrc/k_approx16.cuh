@@ -260,7 +260,8 @@ k_a5_floor(const unsigned short *__restrict__ ST16, const int *__restrict__ q_of
     if (w < 8 && lane == 0 && q < QS) floor_out[(size_t)b * QS + q] = f;
 }
 
-// live[b * stride + c / 32] bit c % 32: row c has a code >= floor in some real query token.  Every word below
+// live[b * stride + c / 32] bit c % 32: row c has a code >= floor in some real query token (on the exact table; the
+// tensor-core pass takes the same bits with its probe's stream of the table, k_collect16_tc).  Every word below
 // (K + 31) / 32 is written; stride rounds that up to a multiple of 4 words, so that k_a5_bound can bulk-copy a query's
 // bitmap (16-byte aligned rows).
 // grid = (any, B), 256 threads; a warp takes 32 rows at a time (coalesced 16-byte loads, GQ = QS / 8 <= 8 per row).

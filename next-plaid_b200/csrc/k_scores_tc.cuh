@@ -25,6 +25,9 @@
 // PB_K1_TC_DIAG=1 measures the largest code difference against the exact table (pb_work_counters).
 // grid = ceil(K/128) CTAs, 288 threads: warps 0-7 two warpgroups that issue the MMAs of one 64-centroid half of the
 // tile each and convert their accumulators, warp 8 bulk-copy loader.
+// With SMAX the epilogue also keeps the largest stored code of every 16-centroid slab (one warp's rows) and query row:
+// SMAX[s][row] (row = b QS + q, n_groups * 128 rows per slab, slabs up to 8 ceil(K/128)), from which
+// k_chunkmax_slabs forms the probe's chunk maxima without reading the table back.
 // ==========================================================================================
 
 // fp16 hi/lo split of `n` rows, scaled by 2^kexp, into MMA tile order (128-row tiles, K-major core matrices);
@@ -86,7 +89,8 @@ template <int DIM>
 __global__ void __launch_bounds__(288, 1)
 k_scores16_tc(const __half *__restrict__ Ch, const __half *__restrict__ Cl, long long K, const __half *__restrict__ Qh,
               const __half *__restrict__ Ql, int n_groups, int B, int QS, const int *__restrict__ q_off,
-              const float2 *__restrict__ qrange_tc, unsigned short *__restrict__ ST16, int *__restrict__ qflag) {
+              const float2 *__restrict__ qrange_tc, unsigned short *__restrict__ ST16, int *__restrict__ qflag,
+              unsigned short *__restrict__ SMAX) {
     extern __shared__ __align__(128) unsigned char smem_k1[];
     constexpr int KSTEPS = DIM / 16;
     constexpr uint32_t T_BYTES = 128 * DIM * 2;  // one 128-row fp16 tile
@@ -149,8 +153,10 @@ k_scores16_tc(const __half *__restrict__ Ch, const __half *__restrict__ Cl, long
             wg_wait_all(d);
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty[st]);  // query tiles consumed
+            uint32_t m[16];  // m[i]: packed maxima of this thread's stored words of query rows 8 i + cq, + 1
 #pragma unroll
             for (int i = 0; i < 16; ++i) {
+                m[i] = 0u;
                 const int row0 = g * 128 + 8 * i;  // 8 query rows of one query (QS % 8 == 0)
                 const int b = row0 / QS, q = row0 - b * QS + cq;
                 if (b >= B) continue;
@@ -164,12 +170,57 @@ k_scores16_tc(const __half *__restrict__ Ch, const __half *__restrict__ Cl, long
                     // Padding rows hold a zero accumulator: x = R*scale, in range.
                     const float x0 = __fmaf_rn(d[4 * i + 2 * r], rg.y, rg.x), x1 = __fmaf_rn(d[4 * i + 2 * r + 1], rg.y, rg.x);
                     if (!(__float_as_uint(x0) < 0x47800000u && __float_as_uint(x1) < 0x47800000u)) atomicOr(&qflag[b], 1);
-                    *reinterpret_cast<uint32_t *>(ST16 + ((size_t)b * K + c) * QS + q) =
-                        min(__float2uint_rd(x0), 65535u) | (min(__float2uint_rd(x1), 65535u) << 16);
+                    const uint32_t word = min(__float2uint_rd(x0), 65535u) | (min(__float2uint_rd(x1), 65535u) << 16);
+                    *reinterpret_cast<uint32_t *>(ST16 + ((size_t)b * K + c) * QS + q) = word;
+                    m[i] = __vmaxu2(m[i], word);
                 }
+            }
+            if (SMAX) {
+                // the warp's 16 centroid rows are the 8 lanes of equal lane % 4 times r: reduce m over lanes ^16, ^8, ^4,
+                // each step keeping half of the values (the lane bit picks the half), so that lane l ends with
+                // m[k] = the slab maximum of query rows 8 (k + 2 (l / 4)) + cq, + 1 for k = 0, 1
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                    const bool hi = lane & 16;
+                    const uint32_t keep = hi ? m[i + 8] : m[i], send = hi ? m[i] : m[i + 8];
+                    m[i] = __vmaxu2(keep, __shfl_xor_sync(PB_FULL, send, 16));
+                }
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const bool hi = lane & 8;
+                    const uint32_t keep = hi ? m[i + 4] : m[i], send = hi ? m[i] : m[i + 4];
+                    m[i] = __vmaxu2(keep, __shfl_xor_sync(PB_FULL, send, 8));
+                }
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const bool hi = lane & 4;
+                    const uint32_t keep = hi ? m[i + 2] : m[i], send = hi ? m[i] : m[i + 2];
+                    m[i] = __vmaxu2(keep, __shfl_xor_sync(PB_FULL, send, 4));
+                }
+                uint32_t *srow = reinterpret_cast<uint32_t *>(SMAX + ((size_t)blockIdx.x * 8 + w) * n_groups * 128 + g * 128 + cq);
+                srow[4 * (2 * (lane >> 2))] = m[0];
+                srow[4 * (2 * (lane >> 2) + 1)] = m[1];
             }
         }
     }
+}
+
+// cmax[b][chunk][q] = the largest code of rows chunk * chunk_rows .. of the table, what k_chunkmax16 reads from it, as
+// the maximum of the slab maxima of k_scores16_tc (chunk_rows is a multiple of 16).  grid = (n_chunks,
+// ceil(B QS / 512)), 256 threads, a thread per pair of query rows: a slab row is contiguous over the batch.
+__global__ void __launch_bounds__(256)
+k_chunkmax_slabs(const unsigned short *__restrict__ SMAX, long long K, int B, int QS, int n_groups, int n_chunks,
+                 int chunk_rows, unsigned short *__restrict__ cmax) {
+    const int chunk = blockIdx.x, j = blockIdx.y * blockDim.x + threadIdx.x;
+    if (2 * j >= B * QS) return;
+    const long long s0 = (long long)chunk * chunk_rows / 16, s1 = (min((long long)(chunk + 1) * chunk_rows, K) + 15) / 16;
+    const uint32_t *col = reinterpret_cast<const uint32_t *>(SMAX) + j;
+    const size_t words = (size_t)n_groups * 64;  // 32-bit words per slab
+    uint32_t m = 0u;
+#pragma unroll 8
+    for (long long s = s0; s < s1; ++s) m = __vmaxu2(m, __ldg(col + (size_t)s * words));
+    const int b = 2 * j / QS, q = 2 * j - b * QS;
+    *reinterpret_cast<uint32_t *>(cmax + ((size_t)b * n_chunks + chunk) * QS + q) = m;
 }
 
 // largest |a - b| over the codes of real query tokens (PB_K1_TC_DIAG)
@@ -185,6 +236,19 @@ __global__ void k_diff16(const unsigned short *__restrict__ a, const unsigned sh
     }
     best = __reduce_max_sync(PB_FULL, best);
     if ((threadIdx.x & 31) == 0 && best) atomicMax(out_max, best);
+}
+
+// words of a[b][0..n) that differ from b_[b][0..n) (rows `stride` words apart), added to *out; nothing when *fallback is
+// raised (PB_TABLE_DIAG: the fused outputs of a tensor-core pass against the standalone kernels).  grid = (any, B).
+__global__ void k_words_diff(const uint32_t *__restrict__ a, const uint32_t *__restrict__ b_, long long n, long long stride,
+                             const int *__restrict__ fallback, unsigned long long *__restrict__ out) {
+    if (*fallback) return;
+    const size_t o = (size_t)blockIdx.y * stride;
+    unsigned cnt = 0;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        cnt += a[o + i] != b_[o + i] ? 1u : 0u;
+    cnt = __reduce_add_sync(PB_FULL, cnt);
+    if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(out, (unsigned long long)cnt);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -245,59 +309,102 @@ PB_DEV float pinned_dot(const float *__restrict__ q, const float *__restrict__ c
     return s;
 }
 
+// the probe candidates of one row group of k_collect16_tc: each hit (bit 16 j' of h[j'/2], query token q0 + j') gets a
+// list slot and its exact selection key.  Out of line: hits are rare, and the fused live test of the kernel needs the
+// registers.
+__device__ __noinline__ void collect_hits(uint32_t hx, uint32_t hy, uint32_t hz, uint32_t hw, int q0, int b, long long c,
+                                          const float *__restrict__ Q, const int *__restrict__ q_off,
+                                          const float *__restrict__ C, int dim, int QS, int cap, int *__restrict__ counts,
+                                          u64 *__restrict__ list, int *__restrict__ fallback) {
+    const uint32_t hits[4] = {hx, hy, hz, hw};
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        if (!((hits[j >> 1] >> (16 * (j & 1))) & 1u)) continue;
+        const int q = q0 + j;
+        const int slot = atomicAdd(&counts[(size_t)b * QS + q], 1);
+        if (slot < cap) {
+            const float s = pinned_dot(Q + (size_t)(q_off[b] + q) * dim, C + (size_t)c * dim, dim);
+            list[((size_t)b * QS + q) * cap + slot] = ((u64)score_key_asc(s) << 32) | (uint32_t)(~(uint32_t)c);
+        } else atomicOr(fallback, 1);
+    }
+}
+
 // ------------------------------------------------------------------------------------------
-// a3 on the tensor-core table.  k_chunkmax16 / k_tau16 (k_probe.cuh) run unchanged: tau = the n-th largest chunk
-// maximum of a token's ESTIMATE codes, so n entries with code >= tau exist (set A).  An entry x of the exact top n
+// a3 on the tensor-core table.  k_tau16 (k_probe.cuh) runs unchanged on the chunk maxima of k_chunkmax_slabs (the
+// values k_chunkmax16 would read from the table): tau = the n-th largest chunk maximum of a token's ESTIMATE codes,
+// so n entries with code >= tau exist (set A).  An entry x of the exact top n
 // outside A displaces some a in A with e(x) >= e(a), hence t(x) >= t(a) - 2 delta and code(x) >= code(a) - (2E + 1)
 // >= tau - code_margin: k_collect16_tc lowers the thresholds by code_margin and takes the exact selection key of
 // every hit from a pinned-order dot, so k_topn_merge ranks exactly the keys the exact path would.
-// ------------------------------------------------------------------------------------------
+// LIVE: the same loads also give the live bits of the pruned first approximate pass (k_approx16.cuh), which k_a5_live
+// computes on the exact table: bit c % 32 of live[b * live_stride + c / 32] = row c has a code >= floor_in[b][q] in
+// some real query token q.  A warp owns a whole chunk (a multiple of 32 rows), so it sets its words' bits in shared
+// memory and writes every word of the chunk once.  A pass that raised *fallback writes no bits (or only those of the
+// chunks that ran before the flag): the bitmap keeps what earlier work left there, and k_a5_bound still reads it before
+// the host sees the flag.  That is memory-safe -- a bit only decides which of a doc's own code rows get gathered -- and
+// the pass's results and counters are discarded when it is redone on the exact path.
+template <bool LIVE>
 __global__ void __launch_bounds__(128)
 k_collect16_tc(const unsigned short *__restrict__ ST16, const float *__restrict__ Q, const int *__restrict__ q_off,
                const float *__restrict__ C, int dim, int code_margin, long long K, int QS, int n_chunks, int chunk_rows,
                const uint32_t *__restrict__ tau, int cap, int *__restrict__ counts, u64 *__restrict__ list,
-               int *__restrict__ fallback) {
+               int *__restrict__ fallback, const uint32_t *__restrict__ floor_in, uint32_t *__restrict__ live_out,
+               long long live_stride) {
+    __shared__ uint32_t live_s[LIVE ? 4 : 1][LIVE ? 32 : 1];  // a chunk's words (chunk_rows <= 1024)
     const int w = threadIdx.x >> 5, lane = threadIdx.x & 31, b = blockIdx.y;
     const int chunk = blockIdx.x * 4 + w;
     if (chunk >= n_chunks || *fallback) return;
     const int GQ = QS >> 3, L = (32 / GQ) * GQ, g = lane % GQ;  // lane -> query-token group as in k_chunkmax16
-    if (lane >= L) return;
     const long long c0 = (long long)chunk * chunk_rows;
     const int rows = (int)min((long long)chunk_rows, K - c0);
-    const uint4 *base = reinterpret_cast<const uint4 *>(ST16 + ((size_t)b * K + c0) * QS);
-    const int total = rows * GQ;
-    // this lane's 8 thresholds as packed halfwords; padding rows (tau = 65536) never match
-    uint32_t t2[4], live[4];
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-        uint32_t a = tau[(size_t)b * QS + 8 * g + 2 * e], c = tau[(size_t)b * QS + 8 * g + 2 * e + 1];
-        if (a < 65536u) a = a > (uint32_t)code_margin ? a - (uint32_t)code_margin : 0u;
-        if (c < 65536u) c = c > (uint32_t)code_margin ? c - (uint32_t)code_margin : 0u;
-        t2[e] = min(a, 65535u) | (min(c, 65535u) << 16);
-        live[e] = (a < 65536u ? 0xffffu : 0u) | (c < 65536u ? 0xffff0000u : 0u);
+    if (LIVE) {
+        live_s[w][lane] = 0u;
+        __syncwarp();
     }
-    for (int i0 = lane; i0 < total; i0 += 8 * L) {
-        uint4 v[8];
+    if (lane < L) {
+        const uint4 *base = reinterpret_cast<const uint4 *>(ST16 + ((size_t)b * K + c0) * QS);
+        const int total = rows * GQ;
+        // this lane's 8 thresholds as packed halfwords; padding rows (tau = 65536) never match
+        uint32_t t2[4], live[4], f2[4];
+        bool lv = false;
 #pragma unroll
-        for (int e = 0; e < 8; ++e) v[e] = (i0 + L * e < total) ? __ldg(base + i0 + L * e) : make_uint4(0, 0, 0, 0);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-            const uint32_t hx = __vcmpgeu2(v[e].x, t2[0]) & live[0], hy = __vcmpgeu2(v[e].y, t2[1]) & live[1];
-            const uint32_t hz = __vcmpgeu2(v[e].z, t2[2]) & live[2], hw = __vcmpgeu2(v[e].w, t2[3]) & live[3];
-            if ((hx | hy | hz | hw) == 0u || i0 + L * e >= total) continue;  // the common case
-            const long long c = c0 + (i0 + L * e) / GQ;
-            const uint32_t hits[4] = {hx, hy, hz, hw};
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                if (!((hits[j >> 1] >> (16 * (j & 1))) & 1u)) continue;
-                const int q = 8 * g + j;
-                const int slot = atomicAdd(&counts[(size_t)b * QS + q], 1);
-                if (slot < cap) {
-                    const float s = pinned_dot(Q + (size_t)(q_off[b] + q) * dim, C + (size_t)c * dim, dim);
-                    list[((size_t)b * QS + q) * cap + slot] = ((u64)score_key_asc(s) << 32) | (uint32_t)(~(uint32_t)c);
-                } else atomicOr(fallback, 1);
+        for (int e = 0; e < 4; ++e) {
+            uint32_t a = tau[(size_t)b * QS + 8 * g + 2 * e], c = tau[(size_t)b * QS + 8 * g + 2 * e + 1];
+            if (a < 65536u) a = a > (uint32_t)code_margin ? a - (uint32_t)code_margin : 0u;
+            if (c < 65536u) c = c > (uint32_t)code_margin ? c - (uint32_t)code_margin : 0u;
+            t2[e] = min(a, 65535u) | (min(c, 65535u) << 16);
+            live[e] = (a < 65536u ? 0xffffu : 0u) | (c < 65536u ? 0xffff0000u : 0u);
+            // the floors, packed as k_a5_live packs them.  k_a5_live masks a token whose floor is 65536; k_a5_floor gives
+            // that to the padding tokens (masked by live[] here too) and, when nothing is to be live, to every token
+            // (lv false)
+            if (LIVE) {
+                const uint32_t fa = floor_in[(size_t)b * QS + 8 * g + 2 * e], fc = floor_in[(size_t)b * QS + 8 * g + 2 * e + 1];
+                f2[e] = min(fa, 65535u) | (min(fc, 65535u) << 16);
+                lv |= fa < 65536u || fc < 65536u;
             }
         }
+        for (int i0 = lane; i0 < total; i0 += 8 * L) {
+            uint4 v[8];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) v[e] = (i0 + L * e < total) ? __ldg(base + i0 + L * e) : make_uint4(0, 0, 0, 0);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                const uint32_t hx = __vcmpgeu2(v[e].x, t2[0]) & live[0], hy = __vcmpgeu2(v[e].y, t2[1]) & live[1];
+                const uint32_t hz = __vcmpgeu2(v[e].z, t2[2]) & live[2], hw = __vcmpgeu2(v[e].w, t2[3]) & live[3];
+                const uint32_t hf = LIVE && lv ? (__vcmpgeu2(v[e].x, f2[0]) & live[0]) | (__vcmpgeu2(v[e].y, f2[1]) & live[1]) |
+                                                     (__vcmpgeu2(v[e].z, f2[2]) & live[2]) | (__vcmpgeu2(v[e].w, f2[3]) & live[3])
+                                               : 0u;
+                if ((hx | hy | hz | hw | hf) == 0u || i0 + L * e >= total) continue;  // the common case
+                const int r = (i0 + L * e) / GQ;
+                if (LIVE && hf) atomicOr(&live_s[w][r >> 5], 1u << (r & 31));
+                if ((hx | hy | hz | hw) == 0u) continue;
+                collect_hits(hx, hy, hz, hw, 8 * g, b, c0 + r, Q, q_off, C, dim, QS, cap, counts, list, fallback);
+            }
+        }
+    }
+    if (LIVE) {
+        __syncwarp();
+        if (lane < (rows + 31) / 32) live_out[(size_t)b * live_stride + c0 / 32 + lane] = live_s[w][lane];
     }
 }
 

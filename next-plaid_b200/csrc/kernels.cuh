@@ -1,13 +1,16 @@
 // kernels.cuh -- the sm_90a kernels of the PLAID search path, one per row of SURVEY.md 8(a).
 //
-//   k_scores16_tc ....... a2  S~ = Q*C^T as a 3-product split-fp16 wgmma GEMM -> 16-bit score table (default)
+//   k_scores16_tc ....... a2  S~ = Q*C^T as a 3-product split-fp16 wgmma GEMM -> 16-bit score table (default), and
+//                             the table's 16-row slab maxima, from which k_chunkmax_slabs forms a3's chunk maxima
 //   k_centroid_scores ... a2  S = Q*C^T (fp32 FMA, paired query rows): the device-gated exact path   search.rs:345 / :174 / :268
 //   k_chunkmax16/k_tau16/k_collect16(_tc)  a3  per-token top-n_ivf_probe, threshold first on the 16-bit table
+//                             (k_collect16_tc also writes a5's live-row bitmap from the same loads)
 //   k_topn_partial/merge  a3  the same by per-lane lists (fallback), rank   search.rs:388-414 / :177-225
 //   k_cells(_unique/_thr/_emit)  a3  union + centroid_score_threshold      search.rs:417-425 / :226-251
 //   k_mark/k_compact .... a4  IVF posting-list union (sorted, unique)     index.rs:1142-1156
 //   k_approx16/k_select_u32  a5  sum_q max_t S[q, code_t] on the 16-bit table, band around the cut
-//   k_a5_floor/k_a5_live/k_a5_bound  a5  an upper bound of it from the live table rows: k_approx16 runs on the few
+//   k_a5_floor/k_a5_live/k_a5_bound  a5  an upper bound of it from the live table rows (k_a5_live on the exact table
+//                             only): k_approx16 runs on the few
 //                             candidates that can still reach the band (k_a5_bound stages the code lists into shared
 //                             memory with TMA bulk copies, each warp its own ring, and tests them against the live bitmap)
 //   k_recheck_pairs/dots/sum (tensor-core table) | k_approx (exact table)  a5  exact re-check of the docs in the band

@@ -69,7 +69,7 @@ class _Work(C.Structure):
                                          "k1_rows_mismatch", "n_probe_threshold", "n_probe_list", "n_k1_tc",
                                          "n_recheck_docs", "n_k1_tc_redo", "n_exact_pairs",
                                          "n_pair_fallback_queries", "filter_err_ratio_e6", "filter_diag_pairs",
-                                         "n_a5_live_rows", "n_a5_dense_docs")]
+                                         "n_a5_live_rows", "n_a5_dense_docs", "table_diag_mismatch")]
 
 
 class _CoalesceConfig(C.Structure):
