@@ -602,7 +602,8 @@ PB_API pb_status pb_kmeans_fit(int32_t device, const float *samples, int64_t n, 
  * the sample points; per iteration one all-reduce of the [K][dim] sums + [K] counts.  A pb_build_comm is an NCCL
  * communicator (one process per GPU; ship pb_comm_unique_id's 128 bytes as for search) or a member of an in-process
  * pb_shard_group (one host thread per rank).  Every rank receives the same L2-normalised centroids.  The encode
- * that follows needs no communication: each rank runs pb_codec_encode_chunk on its own documents. */
+ * that follows needs no communication: each rank runs pb_codec_encode_chunk on its own documents.
+ * pb_create_index_sharded (below) runs the whole build -- plan, k-means, codec, encode, every file -- on it. */
 typedef struct pb_build_comm pb_build_comm;
 PB_API pb_status pb_build_comm_init(const uint8_t *id128, int32_t rank, int32_t world, int32_t device, pb_build_comm **out);
 PB_API pb_status pb_build_comm_group(pb_shard_group *g, int32_t rank, int32_t device, pb_build_comm **out);
@@ -631,6 +632,44 @@ typedef struct pb_create_params {  /* IndexConfig, index.rs:73-102 */
 PB_API void pb_create_params_default(pb_create_params *p);
 PB_API pb_status pb_create_index(const float *embeddings, const int64_t *doc_lengths, int64_t n_docs, int32_t dim,
                                  const pb_create_params *params, const char *index_dir, pb_index **out_index);
+
+/* MmapIndex::create_with_kmeans (index.rs:1392) -- or create_index_files (index.rs:551) when centroids are given --
+ * for a corpus spread over the ranks of a build communicator, collectively (DESIGN §4n).  pb_create_index is this
+ * call on a group of one.
+ *   Calling rules: a collective over c (pb_build_comm_init or pb_build_comm_group); every rank calls it.  Rank r's
+ *   documents get global ids base_r .. base_r + n_docs - 1, base_r being the sum of n_docs over the lower ranks;
+ *   *out_first_doc_id receives base_r.  n_docs = 0 is allowed on any rank, the total must be > 0.  The rank's device is
+ *   the communicator's (params->device is ignored).  index_dir names the same directory on every rank (with ranks on
+ *   several hosts: a shared filesystem).  doc_lengths is host memory; embeddings [sum doc_lengths][dim] f32 is in
+ *   memory_space.  centroids: host [num_centroids][dim], the same on every rank, or NULL for k-means.
+ *   Result on disk: the directory pb_create_index writes for the rank-order concatenation of the documents with the
+ *   same params and the same centroids, file for file and byte for byte.  With centroids == NULL, sample membership, K
+ *   (kmeans.rs:304-309 over the global sample), the fit subsample and the initial seeds are pb_create_index's; only the
+ *   k-means iterations differ in the last bits (float atomics, as on one GPU).  With centroids given,
+ *   num_partitions, kmeans_niters and max_points_per_centroid are not used and the centroids are written as given.
+ *   Codec training sees pb_create_index's held-out rows in its order.  metadata.json is written last.
+ *   Result in memory: *out_shard (may be NULL) is rank r's range opened on its device, joined to no group: the same
+ *   arrays, totals and inverted-file slice as pb_index_load_range(index_dir, base_r, base_r + n_docs), built from the
+ *   encode output already on the device.  Join the handles with pb_index_group_join / pb_index_comm_init to search.
+ *   What a rank holds: its own documents, its k-means fit points, the held-out rows (rank 0, which trains the codec and
+ *   shares its numbers) and the rows of a chunk that crosses its boundary (the chunk's writer, the rank holding its
+ *   first document).  The global inverted file is never assembled in one place: each rank writes its lists' pieces
+ *   into ivf.npy at offsets from an all-gather of the per-centroid lengths.  Host memory: O(D) words for the plan.
+ *   Failure: a first vote checks the arguments (dim, nbits, every params field but device, the centroids' and
+ *   index_dir's fingerprints, null or negative arguments) and that every rank sees the directory rank 0 creates.  A
+ *   refusal returns the same status on every rank (the lowest failing rank's) and no handle, and writes nothing (the
+ *   directory may be created): argument mismatches PB_ERR_INVALID, a dim not built PB_ERR_UNSUPPORTED, a directory not
+ *   seen by every rank PB_ERR_IO.  Limits are pb_index_open's per shard.  Every later phase ends in a vote, so a
+ *   failed write on one rank fails every rank; the directory is then left as a failed pb_create_index leaves it.  A
+ *   CUDA error inside a collective step may break the group (PB_ERR_COMM on the peers). */
+PB_API pb_status pb_create_index_sharded(pb_build_comm *c, const float *embeddings, const int64_t *doc_lengths,
+                                         int64_t n_docs, int32_t dim, int32_t memory_space, const float *centroids,
+                                         int64_t num_centroids, const pb_create_params *params, const char *index_dir,
+                                         pb_index **out_shard, int64_t *out_first_doc_id);
+/* wall time of the calling thread's last pb_create_index / pb_create_index_sharded per phase, ms: plan, k-means,
+ * codec training, encode, shard (inverted file and derived arrays on the device), chunk files, ivf.npy and the
+ * remaining files */
+PB_API pb_status pb_last_create_ms(float *out_ms /* [7] */);
 
 /* ---- doc-sharded deployment (SURVEY 8e; no reference analogue: the reference is single-process) ----
  *

@@ -1,18 +1,9 @@
-// builder.cpp -- pb_create_index: MmapIndex::create_with_kmeans (index.rs:1392 -> kmeans.rs:261-422 ->
-// index.rs:551-911) with every numeric step on the GPU and the reference's index directory as the result
-// (file set of index.rs:394-525, SURVEY.md appendix B), so the reference -- or pb_index_load -- can open it.
-//
-//   1. compute_kmeans (kmeans.rs:273-419): sample docs, K = 2^floor(log2(16 sqrt(avg_doclen D))), at most
-//      256 points per centroid, Lloyd iterations on the device (pb_kmeans_fit), L2-normalised centroids
-//   2. prepare_codec_artifacts (index.rs:182-287): held-out rows from the end of a doc sample -> bucket cutoffs /
-//      weights, avg_residual, cluster_threshold (pb_codec_train)
-//   3. per chunk of `batch_size` docs (index.rs:289-371, :420-473): nearest-centroid codes + packed residuals
-//      (pb_codec_encode_chunk: wgmma certified assignment), {i}.codes.npy, {i}.residuals.npy, doclens.{i}.json,
-//      {i}.metadata.json
-//   4. inverted file (index.rs:850-873): built on the device by pb_index_open (no ivf given), exported to
-//      ivf.npy / ivf_lengths.npy; metadata.json, plan.json
+// builder.cpp -- the index directory's files: what pb_create_index / pb_create_index_sharded write (file set of
+// index.rs:394-525, SURVEY.md appendix B, so the reference -- or pb_index_load -- can open it), and the file changes of
+// append and delete.  The build itself (sample plan, k-means, codec training, encode, inverted file) is
+// create_collective in engine.cu; pb_create_index is its one-rank case (DESIGN §4n).
 // Sample membership (ChaCha8 shuffles in the reference) and the k-means iteration itself (fastkmeans-rs) are
-// parity-unpinned (SURVEY 8c): this file uses its own splitmix64 shuffles.  Everything downstream of the centroids
+// parity-unpinned (SURVEY 8c): the build uses the splitmix64 shuffles below.  Everything downstream of the centroids
 // and the held-out sample is bit-identical to the oracle (tests/test_gpu_create_index.py).
 #include "engine_internal.h"
 
@@ -29,16 +20,13 @@
 #include <string>
 #include <vector>
 
-namespace {
-
-uint64_t splitmix64(uint64_t &s) {
+static uint64_t splitmix64(uint64_t &s) {
     uint64_t z = (s += 0x9e3779b97f4a7c15ull);
     z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
     z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
     return z ^ (z >> 31);
 }
 
-// first `take` entries of a seeded Fisher-Yates shuffle of 0..n-1
 std::vector<long long> shuffled_prefix(long long n, long long take, uint64_t seed) {
     std::vector<long long> p((size_t)n);
     std::iota(p.begin(), p.end(), 0ll);
@@ -53,8 +41,7 @@ std::vector<long long> shuffled_prefix(long long n, long long take, uint64_t see
 }
 
 // NPY v1.0, header padded so the payload starts on a 64-byte boundary (what numpy and mmap.rs:1177-1250 write)
-pb_status write_npy(const std::string &path, const char *descr, const std::vector<long long> &shape, const void *data,
-                    size_t bytes) {
+static std::string npy_header(const char *descr, const std::vector<long long> &shape) {
     std::string dict = std::string("{'descr': '") + descr + "', 'fortran_order': False, 'shape': (";
     for (size_t i = 0; i < shape.size(); ++i) dict += std::to_string(shape[i]) + (shape.size() == 1 || i + 1 < shape.size() ? "," : "") + (i + 1 < shape.size() ? " " : "");
     dict += "), }";
@@ -62,13 +49,45 @@ pb_status write_npy(const std::string &path, const char *descr, const std::vecto
     const size_t pad = (64 - total % 64) % 64;
     dict.append(pad, ' ');
     dict.push_back('\n');
-    FILE *f = fopen(path.c_str(), "wb");
-    if (!f) return pb_fail(PB_ERR_IO, "cannot create %s", path.c_str());
     const unsigned char magic[8] = {0x93, 'N', 'U', 'M', 'P', 'Y', 1, 0};
     const uint16_t hlen = (uint16_t)dict.size();
-    bool ok = fwrite(magic, 1, 8, f) == 8 && fwrite(&hlen, 2, 1, f) == 1 && fwrite(dict.data(), 1, dict.size(), f) == dict.size();
+    return std::string((const char *)magic, 8) + std::string((const char *)&hlen, 2) + dict;
+}
+
+pb_status write_npy(const std::string &path, const char *descr, const std::vector<long long> &shape, const void *data,
+                    size_t bytes) {
+    const std::string h = npy_header(descr, shape);
+    FILE *f = fopen(path.c_str(), "wb");
+    if (!f) return pb_fail(PB_ERR_IO, "cannot create %s", path.c_str());
+    bool ok = fwrite(h.data(), 1, h.size(), f) == h.size();
     if (ok && bytes) ok = fwrite(data, 1, bytes, f) == bytes;
     ok = (fclose(f) == 0) && ok;
+    return ok ? PB_OK : pb_fail(PB_ERR_IO, "short write to %s", path.c_str());
+}
+
+pb_status npy_create(const std::string &path, const char *descr, const std::vector<long long> &shape, size_t bytes) {
+    const std::string h = npy_header(descr, shape);
+    const int fd = open(path.c_str(), O_WRONLY | O_CREAT | O_TRUNC, 0666);
+    if (fd < 0) return pb_fail(PB_ERR_IO, "cannot create %s", path.c_str());
+    bool ok = write(fd, h.data(), h.size()) == (ssize_t)h.size() && ftruncate(fd, (off_t)(h.size() + bytes)) == 0;
+    ok = (close(fd) == 0) && ok;
+    return ok ? PB_OK : pb_fail(PB_ERR_IO, "short write to %s", path.c_str());
+}
+
+pb_status npy_put(const std::string &path, const char *descr, const std::vector<long long> &shape,
+                  const std::vector<NpyPiece> &pieces) {
+    const size_t h = npy_header(descr, shape).size();
+    const int fd = open(path.c_str(), O_WRONLY);
+    if (fd < 0) return pb_fail(PB_ERR_IO, "cannot open %s", path.c_str());
+    bool ok = true;
+    for (const NpyPiece &p : pieces) {
+        for (size_t done = 0; ok && done < p.bytes;) {
+            const ssize_t w = pwrite(fd, p.src + done, p.bytes - done, (off_t)(h + p.offset + done));
+            ok = w > 0;
+            if (ok) done += (size_t)w;
+        }
+    }
+    ok = (close(fd) == 0) && ok;
     return ok ? PB_OK : pb_fail(PB_ERR_IO, "short write to %s", path.c_str());
 }
 
@@ -79,6 +98,8 @@ pb_status write_text(const std::string &path, const std::string &txt) {
     ok = (fclose(f) == 0) && ok;
     return ok ? PB_OK : pb_fail(PB_ERR_IO, "short write to %s", path.c_str());
 }
+
+namespace {
 
 // atomic_write_file (utils.rs:16-60): written and synced under a temporary name, then renamed over `path`
 template <class Write> pb_status atomic_write(const std::string &path, Write write) {
@@ -93,13 +114,6 @@ template <class Write> pb_status atomic_write(const std::string &path, Write wri
     if (s) remove(tmp.c_str());
     return s;
 }
-
-struct CodecGuard {
-    pb_codec *c = nullptr;
-    ~CodecGuard() {
-        if (c) pb_codec_close(c);
-    }
-};
 
 }  // namespace
 
@@ -123,139 +137,58 @@ extern "C" pb_status pb_create_index(const float *embeddings, const int64_t *doc
     if (cfg.nbits <= 0 || 8 % cfg.nbits != 0) return pb_fail(PB_ERR_INVALID, "nbits must be a divisor of 8, got %d", cfg.nbits);
     if (cfg.batch_size <= 0 || cfg.kmeans_niters < 0 || cfg.max_points_per_centroid <= 0)
         return pb_fail(PB_ERR_INVALID, "bad create parameters");
-    const long long D = n_docs;
-    std::vector<long long> off((size_t)D + 1, 0);
-    for (long long i = 0; i < D; ++i) {
+    long long N = 0;
+    for (long long i = 0; i < n_docs; ++i) {
         if (doc_lengths[i] < 0) return pb_fail(PB_ERR_INVALID, "doc_lengths[%lld] < 0", i);
-        off[(size_t)i + 1] = off[(size_t)i] + doc_lengths[i];
+        N += doc_lengths[i];
     }
-    const long long N = off[(size_t)D];
     if (N <= 0) return pb_fail(PB_ERR_INVALID, "no embeddings");
-    mkdir(index_dir, 0777);
-    const std::string dir = std::string(index_dir) + "/";
-    const int packed = dim * cfg.nbits / 8;
+    return pb_create_local(embeddings, doc_lengths, n_docs, dim, params, index_dir, out_index);
+}
 
-    // ---- 1. centroids (kmeans.rs:273-419) ----
-    const long long n_sdocs = pb_kmeans_num_sample_docs(D);
-    const std::vector<long long> sdocs = shuffled_prefix(D, n_sdocs, cfg.seed);
-    long long n_stok = 0;
-    for (long long d : sdocs) n_stok += doc_lengths[d];
-    if (n_stok <= 0) return pb_fail(PB_ERR_INVALID, "the k-means sample holds no embeddings");
-    long long K = cfg.num_partitions > 0 ? std::min<long long>(cfg.num_partitions, n_stok)
-                                         : pb_kmeans_num_partitions(D, (double)n_stok / (double)n_sdocs, n_stok);
-    std::vector<float> samples((size_t)n_stok * dim);
-    {
-        size_t w = 0;
-        for (long long d : sdocs) {
-            const size_t n = (size_t)doc_lengths[d] * dim;
-            memcpy(samples.data() + w, embeddings + (size_t)off[(size_t)d] * dim, n * sizeof(float));
-            w += n;
-        }
-    }
-    long long n_fit = n_stok;
-    if (n_stok > K * (long long)cfg.max_points_per_centroid) {  // at most max_points_per_centroid points per centroid
-        n_fit = K * (long long)cfg.max_points_per_centroid;
-        const std::vector<long long> pick = shuffled_prefix(n_stok, n_fit, cfg.seed ^ 0x5bd1e995u);
-        std::vector<float> sub((size_t)n_fit * dim);
-        for (long long i = 0; i < n_fit; ++i)
-            memcpy(sub.data() + (size_t)i * dim, samples.data() + (size_t)pick[(size_t)i] * dim, (size_t)dim * sizeof(float));
-        samples.swap(sub);
-    }
-    std::vector<float> centroids((size_t)K * dim);
-    if (pb_status s = pb_kmeans_fit(cfg.device, samples.data(), n_fit, dim, K, cfg.kmeans_niters, cfg.seed, centroids.data()))
-        return s;
-    std::vector<float>().swap(samples);
+// {i}.codes.npy, {i}.residuals.npy, doclens.{i}.json, {i}.metadata.json (index.rs:420-473)
+pb_status pb_write_chunk(const std::string &dir, long long c, const int64_t *codes, const uint8_t *residuals, long long n,
+                         int packed, const int64_t *doc_lengths, long long n_docs, long long t0) {
+    const std::string ci = std::to_string(c);
+    if (pb_status s = write_npy(dir + ci + ".codes.npy", "<i8", {n}, codes, (size_t)n * 8)) return s;
+    if (pb_status s = write_npy(dir + ci + ".residuals.npy", "|u1", {n, packed}, residuals, (size_t)n * packed)) return s;
+    std::string dl = "[";
+    for (long long d = 0; d < n_docs; ++d) dl += std::to_string((long long)doc_lengths[d]) + (d + 1 < n_docs ? "," : "");
+    dl += "]";
+    if (pb_status s = write_text(dir + "doclens." + ci + ".json", dl)) return s;
+    char meta[256];
+    snprintf(meta, sizeof meta, "{\n  \"num_documents\": %lld,\n  \"num_embeddings\": %lld,\n  \"embedding_offset\": %lld\n}",
+             n_docs, n, t0);
+    return write_text(dir + ci + ".metadata.json", meta);
+}
 
-    // ---- 2. codec training on held-out rows (index.rs:195-287) ----
-    CodecGuard cg;
-    if (pb_status s = pb_codec_open(cfg.device, centroids.data(), K, dim, cfg.nbits, nullptr, &cg.c)) return s;
-    const long long n_cdocs = pb_codec_num_sample_docs(D);
-    const std::vector<long long> cdocs = shuffled_prefix(D, n_cdocs, cfg.seed + 1);
-    const long long want = pb_codec_heldout_tokens(N);
-    std::vector<float> heldout;
-    long long got = 0;
-    for (long long i = (long long)cdocs.size() - 1; i >= 0 && got < want; --i) {  // from the end of the sample list
-        const long long d = cdocs[(size_t)i];
-        const long long take = std::min<long long>(want - got, doc_lengths[d]);
-        heldout.insert(heldout.end(), embeddings + (size_t)off[(size_t)d] * dim, embeddings + (size_t)(off[(size_t)d] + take) * dim);
-        got += take;
-    }
-    const int nopt = 1 << cfg.nbits;
-    std::vector<float> cutoffs((size_t)std::max(nopt - 1, 1)), weights((size_t)nopt), avg_res((size_t)dim);
-    float threshold = 0.0f;
-    if (pb_status s = pb_codec_train(cg.c, heldout.data(), got, cutoffs.data(), weights.data(), avg_res.data(), &threshold))
-        return s;
-
-    // ---- 3. encode chunk by chunk, write the chunk files (index.rs:420-473) ----
-    std::vector<int64_t> codes((size_t)N);
-    std::vector<uint8_t> residuals((size_t)N * packed);
-    const long long n_chunks = (D + cfg.batch_size - 1) / cfg.batch_size;
-    for (long long c = 0; c < n_chunks; ++c) {
-        const long long d0 = c * cfg.batch_size, d1 = std::min<long long>(D, d0 + cfg.batch_size);
-        const long long t0 = off[(size_t)d0], n = off[(size_t)d1] - t0;
-        if (pb_status s = pb_codec_encode_chunk(cg.c, embeddings + (size_t)t0 * dim, n, codes.data() + t0,
-                                                residuals.data() + (size_t)t0 * packed))
-            return s;
-        const std::string ci = std::to_string(c);
-        if (pb_status s = write_npy(dir + ci + ".codes.npy", "<i8", {n}, codes.data() + t0, (size_t)n * 8)) return s;
-        if (pb_status s = write_npy(dir + ci + ".residuals.npy", "|u1", {n, packed}, residuals.data() + (size_t)t0 * packed,
-                                    (size_t)n * packed))
-            return s;
-        std::string dl = "[";
-        for (long long d = d0; d < d1; ++d) dl += std::to_string((long long)doc_lengths[d]) + (d + 1 < d1 ? "," : "");
-        dl += "]";
-        if (pb_status s = write_text(dir + "doclens." + ci + ".json", dl)) return s;
-        char meta[256];
-        snprintf(meta, sizeof meta, "{\n  \"num_documents\": %lld,\n  \"num_embeddings\": %lld,\n  \"embedding_offset\": %lld\n}",
-                 d1 - d0, n, t0);
-        if (pb_status s = write_text(dir + ci + ".metadata.json", meta)) return s;
-    }
-
-    // ---- 4. inverted file on the device, remaining files ----
-    pb_index_desc desc;
-    memset(&desc, 0, sizeof desc);
-    desc.dim = dim;
-    desc.nbits = cfg.nbits;
-    desc.num_centroids = K;
-    desc.num_documents = D;
-    desc.num_embeddings = N;
-    desc.centroids = centroids.data();
-    desc.bucket_weights = weights.data();
-    desc.codes = codes.data();
-    desc.residuals = residuals.data();
-    desc.doc_lengths = doc_lengths;
-    desc.device = cfg.device;
-    desc.memory_space = PB_MEM_HOST;
-    pb_index *ix = nullptr;
-    if (pb_status s = pb_index_open(&desc, &ix)) return s;
-    int64_t ivf_total = 0;
-    pb_status st = pb_index_export_ivf(ix, nullptr, nullptr, &ivf_total);
-    std::vector<int64_t> ivf((size_t)std::max<int64_t>(ivf_total, 1));
-    std::vector<int32_t> ivf_len((size_t)K);
-    if (!st) st = pb_index_export_ivf(ix, ivf.data(), ivf_len.data(), &ivf_total);
-    if (!st) st = write_npy(dir + "ivf.npy", "<i8", {(long long)ivf_total}, ivf.data(), (size_t)ivf_total * 8);
-    if (!st) st = write_npy(dir + "ivf_lengths.npy", "<i4", {K}, ivf_len.data(), (size_t)K * 4);
-    if (!st) st = write_npy(dir + "centroids.npy", "<f4", {K, dim}, centroids.data(), (size_t)K * dim * 4);
-    if (!st) st = write_npy(dir + "bucket_cutoffs.npy", "<f4", {(long long)nopt - 1}, cutoffs.data(), (size_t)(nopt - 1) * 4);
-    if (!st) st = write_npy(dir + "bucket_weights.npy", "<f4", {(long long)nopt}, weights.data(), (size_t)nopt * 4);
-    if (!st) st = write_npy(dir + "avg_residual.npy", "<f4", {(long long)dim}, avg_res.data(), (size_t)dim * 4);
+// centroids.npy, the codec's files and plan.json
+pb_status pb_write_codec_files(const std::string &dir, long long K, int dim, int nbits, const float *centroids,
+                               const float *cutoffs, const float *weights, const float *avg_res, float threshold,
+                               long long n_chunks) {
+    const int nopt = 1 << nbits;
+    pb_status st = write_npy(dir + "centroids.npy", "<f4", {K, dim}, centroids, (size_t)K * dim * 4);
+    if (!st) st = write_npy(dir + "bucket_cutoffs.npy", "<f4", {(long long)nopt - 1}, cutoffs, (size_t)(nopt - 1) * 4);
+    if (!st) st = write_npy(dir + "bucket_weights.npy", "<f4", {(long long)nopt}, weights, (size_t)nopt * 4);
+    if (!st) st = write_npy(dir + "avg_residual.npy", "<f4", {(long long)dim}, avg_res, (size_t)dim * 4);
     if (!st) st = write_npy(dir + "cluster_threshold.npy", "<f4", {1}, &threshold, 4);
     if (!st) {
         char plan[128];
-        snprintf(plan, sizeof plan, "{\n  \"nbits\": %d,\n  \"num_chunks\": %lld\n}", cfg.nbits, n_chunks);
+        snprintf(plan, sizeof plan, "{\n  \"nbits\": %d,\n  \"num_chunks\": %lld\n}", nbits, n_chunks);
         st = write_text(dir + "plan.json", plan);
     }
-    if (!st) {
-        char meta[512];  // struct Metadata, index.rs:105-127
-        snprintf(meta, sizeof meta,
-                 "{\n  \"num_chunks\": %lld,\n  \"nbits\": %d,\n  \"num_partitions\": %lld,\n  \"num_embeddings\": %lld,\n"
-                 "  \"avg_doclen\": %.17g,\n  \"num_documents\": %lld,\n  \"embedding_dim\": %d,\n  \"next_plaid_compatible\": true\n}",
-                 n_chunks, cfg.nbits, K, N, (double)N / (double)D, D, dim);
-        st = write_text(dir + "metadata.json", meta);
-    }
-    if (st || !out_index) pb_index_close(ix);
-    else *out_index = ix;
     return st;
+}
+
+// metadata.json of a new index (struct Metadata, index.rs:105-127)
+pb_status pb_write_create_meta(const std::string &dir, long long n_chunks, int nbits, long long K, long long N, long long D,
+                               int dim) {
+    char meta[512];
+    snprintf(meta, sizeof meta,
+             "{\n  \"num_chunks\": %lld,\n  \"nbits\": %d,\n  \"num_partitions\": %lld,\n  \"num_embeddings\": %lld,\n"
+             "  \"avg_doclen\": %.17g,\n  \"num_documents\": %lld,\n  \"embedding_dim\": %d,\n  \"next_plaid_compatible\": true\n}",
+             n_chunks, nbits, K, N, (double)N / (double)D, D, dim);
+    return write_text(dir + "metadata.json", meta);
 }
 
 // Metadata::load_from_path (index.rs:131-155) of a directory that must hold the handle's old_D documents and nbits:
@@ -508,3 +441,18 @@ pb_status pb_dir_delete(const char *index_dir, long long old_D, long long K, int
     if (pb_status s = clean_embeddings_file(dir, "embeddings.npy", "embeddings_lengths.json", nullptr, -1, is_del)) return s;
     return clean_embeddings_file(dir, "buffer.npy", "buffer_lengths.json", "buffer_info.json", old_D, is_del);
 }
+
+// The directory check of a collective build: rank 0 creates the directory and a file holding a token, every other rank
+// reads it back, and rank 0 removes it.  A rank that does not find the token does not see rank 0's directory.
+static std::string token_path(const char *index_dir) { return std::string(index_dir) + "/.pb_create_check"; }
+pb_status pb_dir_token_put(const char *index_dir, long long token) {
+    mkdir(index_dir, 0777);
+    return write_text(token_path(index_dir), std::to_string(token));
+}
+pb_status pb_dir_token_check(const char *index_dir, long long token) {
+    std::string got;
+    if (pb_read_text(token_path(index_dir), got) || got != std::to_string(token))
+        return pb_fail(PB_ERR_IO, "%s is not the directory rank 0 created (no shared filesystem?)", index_dir);
+    return PB_OK;
+}
+void pb_dir_token_drop(const char *index_dir) { remove(token_path(index_dir).c_str()); }

@@ -3985,6 +3985,46 @@ struct KmeansAssign {
     }
 };
 
+// Lloyd iterations from the K centroids in dC over the n points dX (k-means assignment, coordinate sums and counts,
+// new centroids), then L2 normalisation (kmeans.rs:415-419).  With `comm`, the points are this rank's share and one
+// all-reduce per iteration sums every rank's [K][dim] sums and [K] counts, so every rank moves the same centroids.
+static pb_status lloyd(ShardComm *comm, DevBuf *stage, cudaStream_t st, const float *dX, long long n, int dim, long long K,
+                       int niters, int sms, float *dC) {
+    DevBuf dbias, dcodes, dacc;
+    CKS(dbias.ensure((size_t)K * 4));
+    CKS(dcodes.ensure((size_t)std::max<long long>(n, 1) * 4));
+    CKS(dacc.ensure((size_t)K * (dim + 1) * 4));  // [K][dim] sums followed by [K] counts: one all-reduce
+    float *sums = dacc.as<float>(), *counts = dacc.as<float>() + (size_t)K * dim;
+    KmeansAssign ka;
+    CKS(ka.init(dX, n, dim, K, sms, st));
+    for (int it = 0; it < niters; ++it) {
+        CKS(ka.run(dX, dC, dbias.as<float>(), dcodes.as<uint32_t>(), st));
+        CK(cudaMemsetAsync(dacc.p, 0, (size_t)K * (dim + 1) * 4, st));
+        if (n > 0) k_accumulate<<<sms * 8, 256, 0, st>>>(dX, n, dim, dcodes.as<uint32_t>(), sums, counts);
+        CK(cudaGetLastError());
+        if (comm) CKS(comm->allreduce_sum(st, dacc.as<float>(), (size_t)K * (dim + 1), *stage));
+        k_update_centroids<<<sms * 4, 256, 0, st>>>(dC, K, dim, sums, counts);
+        CK(cudaGetLastError());
+    }
+    k_normalize_rows<<<sms * 4, 256, 0, st>>>(dC, K, dim);
+    CK(cudaGetLastError());
+    return PB_OK;
+}
+
+// the first K entries of a partial Fisher-Yates shuffle of 0..n-1 with a 64-bit LCG from state s: the sample points
+// pb_kmeans_fit starts from
+static std::vector<long long> lcg_seeds(long long n, long long K, uint64_t s) {
+    std::vector<long long> perm((size_t)n);
+    for (long long i = 0; i < n; ++i) perm[i] = i;
+    for (long long i = 0; i < K; ++i) {
+        s = s * 6364136223846793005ull + 1442695040888963407ull;
+        long long j = i + (long long)((s >> 11) % (uint64_t)(n - i));
+        std::swap(perm[i], perm[j]);
+    }
+    perm.resize((size_t)K);
+    return perm;
+}
+
 extern "C" pb_status pb_kmeans_fit(int32_t device, const float *samples, int64_t n, int32_t dim, int64_t K, int32_t niters,
                                    uint64_t seed, float *out_centroids) {
     if (!samples || !out_centroids) return pb_fail(PB_ERR_INVALID, "null argument");
@@ -3994,37 +4034,15 @@ extern "C" pb_status pb_kmeans_fit(int32_t device, const float *samples, int64_t
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, device));
     const int sms = prop.multiProcessorCount;
-    DevBuf dX, dC, dbias, dcodes, dsums, dcnt, didx;
+    DevBuf dX, dC, didx;
     CKS(upload(dX, samples, (size_t)n * dim * 4, PB_MEM_HOST));
     CKS(dC.ensure((size_t)K * dim * 4));
-    CKS(dbias.ensure((size_t)K * 4));
-    CKS(dcodes.ensure((size_t)n * 4));
-    CKS(dsums.ensure((size_t)K * dim * 4));
-    CKS(dcnt.ensure((size_t)K * 4));
-    // initial centroids: K distinct sample points (partial Fisher-Yates with a 64-bit LCG)
-    std::vector<long long> perm((size_t)n);
-    for (long long i = 0; i < n; ++i) perm[i] = i;
-    uint64_t s = seed * 6364136223846793005ull + 1442695040888963407ull;
-    for (long long i = 0; i < K; ++i) {
-        s = s * 6364136223846793005ull + 1442695040888963407ull;
-        long long j = i + (long long)((s >> 11) % (uint64_t)(n - i));
-        std::swap(perm[i], perm[j]);
-    }
+    // initial centroids: K distinct sample points
+    const std::vector<long long> perm = lcg_seeds(n, K, seed * 6364136223846793005ull + 1442695040888963407ull);
     CKS(upload(didx, perm.data(), (size_t)K * 8, PB_MEM_HOST));
     k_gather_rows<<<sms * 4, 256>>>(dX.as<float>(), didx.as<long long>(), K, dim, dC.as<float>());
     CK(cudaGetLastError());
-    KmeansAssign ka;
-    CKS(ka.init(dX.as<float>(), n, dim, K, sms, 0));
-    for (int it = 0; it < niters; ++it) {
-        CKS(ka.run(dX.as<float>(), dC.as<float>(), dbias.as<float>(), dcodes.as<uint32_t>(), 0));
-        CK(cudaMemset(dsums.p, 0, (size_t)K * dim * 4));
-        CK(cudaMemset(dcnt.p, 0, (size_t)K * 4));
-        k_accumulate<<<sms * 8, 256>>>(dX.as<float>(), n, dim, dcodes.as<uint32_t>(), dsums.as<float>(), dcnt.as<float>());
-        k_update_centroids<<<sms * 4, 256>>>(dC.as<float>(), K, dim, dsums.as<float>(), dcnt.as<float>());
-        CK(cudaGetLastError());
-    }
-    k_normalize_rows<<<sms * 4, 256>>>(dC.as<float>(), K, dim);  // kmeans.rs:415-419
-    CK(cudaGetLastError());
+    CKS(lloyd(nullptr, nullptr, 0, dX.as<float>(), n, dim, K, niters, sms, dC.as<float>()));
     CK(cudaMemcpy(out_centroids, dC.p, (size_t)K * dim * 4, cudaMemcpyDeviceToHost));
     return PB_OK;
 }
@@ -4079,20 +4097,11 @@ extern "C" pb_status pb_kmeans_fit_dp(pb_build_comm *c, const float *samples, in
     // gives every rank the same start
     const long long k0 = K * c->comm.rank / c->comm.world, k1 = K * (c->comm.rank + 1) / c->comm.world, kmine = k1 - k0;
     if (kmine > n) return pb_fail(PB_ERR_INVALID, "rank %d holds %lld points but seeds %lld centroids", c->comm.rank, n, kmine);
-    DevBuf dX, dC, dbias, dcodes, dacc, didx;
+    DevBuf dX, dC, didx;
     CKS(upload(dX, samples, (size_t)std::max<long long>(n, 1) * dim * 4, PB_MEM_HOST));
     CKS(dC.ensure((size_t)K * dim * 4));
-    CKS(dbias.ensure((size_t)K * 4));
-    CKS(dcodes.ensure((size_t)std::max<long long>(n, 1) * 4));
-    CKS(dacc.ensure((size_t)K * (dim + 1) * 4));  // [K][dim] sums followed by [K] counts: one all-reduce
-    std::vector<long long> perm((size_t)n);
-    for (long long i = 0; i < n; ++i) perm[i] = i;
-    uint64_t s = (seed + 0x9e3779b97f4a7c15ull * (uint64_t)(c->comm.rank + 1)) * 6364136223846793005ull + 1442695040888963407ull;
-    for (long long i = 0; i < kmine; ++i) {
-        s = s * 6364136223846793005ull + 1442695040888963407ull;
-        long long j = i + (long long)((s >> 11) % (uint64_t)(n - i));
-        std::swap(perm[i], perm[j]);
-    }
+    const std::vector<long long> perm = lcg_seeds(
+        n, kmine, (seed + 0x9e3779b97f4a7c15ull * (uint64_t)(c->comm.rank + 1)) * 6364136223846793005ull + 1442695040888963407ull);
     CK(cudaMemsetAsync(dC.p, 0, (size_t)K * dim * 4, c->stream.s));
     if (kmine > 0) {
         CKS(upload(didx, perm.data(), (size_t)kmine * 8, PB_MEM_HOST));
@@ -4100,20 +4109,7 @@ extern "C" pb_status pb_kmeans_fit_dp(pb_build_comm *c, const float *samples, in
         CK(cudaGetLastError());
     }
     CKS(c->comm.allreduce_sum(c->stream.s, dC.as<float>(), (size_t)K * dim, c->stage));
-    float *sums = dacc.as<float>(), *counts = dacc.as<float>() + (size_t)K * dim;
-    KmeansAssign ka;
-    CKS(ka.init(dX.as<float>(), n, dim, K, sms, c->stream.s));
-    for (int it = 0; it < niters; ++it) {
-        CKS(ka.run(dX.as<float>(), dC.as<float>(), dbias.as<float>(), dcodes.as<uint32_t>(), c->stream.s));
-        CK(cudaMemsetAsync(dacc.p, 0, (size_t)K * (dim + 1) * 4, c->stream.s));
-        if (n > 0) k_accumulate<<<sms * 8, 256, 0, c->stream.s>>>(dX.as<float>(), n, dim, dcodes.as<uint32_t>(), sums, counts);
-        CK(cudaGetLastError());
-        CKS(c->comm.allreduce_sum(c->stream.s, dacc.as<float>(), (size_t)K * (dim + 1), c->stage));
-        k_update_centroids<<<sms * 4, 256, 0, c->stream.s>>>(dC.as<float>(), K, dim, sums, counts);
-        CK(cudaGetLastError());
-    }
-    k_normalize_rows<<<sms * 4, 256, 0, c->stream.s>>>(dC.as<float>(), K, dim);  // kmeans.rs:415-419
-    CK(cudaGetLastError());
+    CKS(lloyd(&c->comm, &c->stage, c->stream.s, dX.as<float>(), n, dim, K, niters, sms, dC.as<float>()));
     CK(cudaMemcpyAsync(out_centroids, dC.p, (size_t)K * dim * 4, cudaMemcpyDeviceToHost, c->stream.s));
     CK(cudaStreamSynchronize(c->stream.s));
     return PB_OK;
@@ -4638,37 +4634,44 @@ extern "C" pb_status pb_index_delete(pb_index *ix, const int64_t *doc_ids, int64
 enum { LR_STATUS, LR_RANK, LR_WORLD, LR_BASE, LR_D, LR_N, LR_K, LR_DIM, LR_NBITS, LR_OWN, LR_PRINT, LR_WORDS };
 enum { SH_OP_DELETE = 1, SH_OP_APPEND = 2, SH_OP_APPEND_ENCODED = 3 };
 
-// every rank's `words` 64-bit words, in rank order; a handle outside any group is a group of one
-static pb_status gather_words(pb_index *ix, const long long *mine, int words, std::vector<long long> &all,
+// every rank's `words` 64-bit words, in rank order; a communicator outside any group is a group of one
+static pb_status gather_words(ShardComm &comm, const long long *mine, int words, std::vector<long long> &all,
                               bool unbounded = false) {
     all.assign(mine, mine + words);
-    if (!ix->comm.joined()) return PB_OK;
-    all.resize((size_t)words * ix->comm.world);
+    if (!comm.joined()) return PB_OK;
+    all.resize((size_t)words * comm.world);
     OwnedStream st;
     DevBuf send, recv;
-    CK(cudaSetDevice(ix->device));
+    CK(cudaSetDevice(comm.device));
     CK(cudaStreamCreateWithFlags(&st.s, cudaStreamNonBlocking));
     CKS(send.ensure((size_t)words * 8));
-    CKS(recv.ensure((size_t)words * 8 * ix->comm.world));
+    CKS(recv.ensure((size_t)words * 8 * comm.world));
     CK(cudaMemcpy(send.p, mine, (size_t)words * 8, cudaMemcpyHostToDevice));
-    CKS(ix->comm.allgather(st.s, send.p, recv.p, (size_t)words, unbounded));
+    CKS(comm.allgather(st.s, send.p, recv.p, (size_t)words, unbounded));
     CK(cudaStreamSynchronize(st.s));
     CK(cudaMemcpy(all.data(), recv.p, all.size() * 8, cudaMemcpyDeviceToHost));
     return PB_OK;
 }
+static pb_status gather_words(pb_index *ix, const long long *mine, int words, std::vector<long long> &all,
+                              bool unbounded = false) {
+    return gather_words(ix->comm, mine, words, all, unbounded);
+}
 
 // the status of the lowest failing rank, or PB_OK; the failing rank keeps its own message, the others name it
-static pb_status first_failure(pb_index *ix, const std::vector<long long> &all, int words, const char *what) {
-    for (int r = 0; r < ix->comm.world; ++r) {
+static pb_status first_failure(const ShardComm &comm, const std::vector<long long> &all, int words, const char *what) {
+    for (int r = 0; r < comm.world; ++r) {
         const pb_status s = (pb_status)all[(size_t)r * words];
         if (s == PB_OK) continue;
-        if (r == ix->comm.rank) {
+        if (r == comm.rank) {
             const std::string own = g_err;
             return pb_fail(s, "rank %d: %s", r, own.c_str());
         }
         return pb_fail(s, "rank %d of the group failed (status %d)%s", r, (int)s, what);
     }
     return PB_OK;
+}
+static pb_status first_failure(pb_index *ix, const std::vector<long long> &all, int words, const char *what) {
+    return first_failure(ix->comm, all, words, what);
 }
 
 // Exchange A of a sharded collective and the verdict every rank reaches from the same records.  The caller has set
@@ -5140,5 +5143,473 @@ extern "C" pb_status pb_last_delete_ms(pb_index *ix, float *out_ms) {
     if (!ix || !out_ms) return pb_fail(PB_ERR_INVALID, "null argument");
     auto rd = ix->read_lock();
     memcpy(out_ms, ix->delete_ms, sizeof ix->delete_ms);
+    return PB_OK;
+}
+
+// ------------------------------------------------------------------------------------------
+// Collective index build (DESIGN §4n): pb_create_index_sharded, with pb_create_index as its one-rank case.  Every rank
+// computes the same sample plan over global doc ids; it uploads only its own rows (k-means fit points and seeds, and
+// held-out rows for the trainer, rank 0), encodes its documents straight into its shard, writes the chunks that start
+// in its range (the head of a chunk that crosses into a later rank comes over the communicator) and its pieces of
+// ivf.npy.  A vote ends every phase that can fail on one rank alone.
+// ------------------------------------------------------------------------------------------
+enum { CV_STATUS, CV_RANK, CV_WORLD, CV_D, CV_N, CV_DIM, CV_NBITS, CV_NITERS, CV_MPP, CV_PARTS, CV_BATCH, CV_SEED, CV_K,
+       CV_CENT, CV_DIR, CV_TOKEN, CV_WORDS };
+enum { CP_PLAN, CP_KMEANS, CP_CODEC, CP_ENCODE, CP_SHARD, CP_CHUNKS, CP_IVF, CP_COUNT };
+static thread_local float g_create_ms[CP_COUNT];
+
+// one word per rank: the lowest failing rank's status on every rank.  Waits for late peers (a phase may keep one rank
+// busy much longer than the others)
+static pb_status create_vote(ShardComm &comm, pb_status local, const char *what) {
+    const long long v = local;
+    std::vector<long long> all;
+    CKS(gather_words(comm, &v, 1, all, true));
+    return first_failure(comm, all, 1, what);
+}
+
+// rows `tok` (this rank's token ids) of its embeddings [N][dim] (host or device) into out, in that order
+static pb_status gather_rows(const float *emb, int space, int dim, const std::vector<long long> &tok, DevBuf &out, int sms,
+                             cudaStream_t st) {
+    CKS(out.ensure(std::max<size_t>(tok.size() * dim * 4, 16)));
+    if (tok.empty()) return PB_OK;
+    if (space == PB_MEM_HOST) {
+        std::vector<float> h(tok.size() * dim);
+        for (size_t i = 0; i < tok.size(); ++i) memcpy(h.data() + i * dim, emb + (size_t)tok[i] * dim, (size_t)dim * 4);
+        CK(cudaMemcpy(out.p, h.data(), h.size() * 4, cudaMemcpyHostToDevice));
+        return PB_OK;
+    }
+    DevBuf idx;
+    CKS(upload(idx, tok.data(), tok.size() * 8, PB_MEM_HOST));
+    k_gather_rows_i64<<<sms * 8, 256, 0, st>>>(emb, idx.as<long long>(), (long long)tok.size(), dim, out.as<float>());
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(st));
+    return PB_OK;
+}
+
+struct IndexCloser {
+    void operator()(pb_index *ix) const { pb_index_close(ix); }
+};
+
+static pb_status create_collective(pb_build_comm *c, const float *emb, const int64_t *doc_lengths, int64_t n_docs, int dim,
+                                   int space, const float *centroids_in, int64_t num_centroids, const pb_create_params *params,
+                                   const char *index_dir, pb_index **out_shard, int64_t *out_first) {
+    using clock = std::chrono::steady_clock;
+    for (float &v : g_create_ms) v = 0.0f;
+    auto t_lap = clock::now();
+    auto lap = [&](int phase) {
+        const auto now = clock::now();
+        g_create_ms[phase] += std::chrono::duration<float, std::milli>(now - t_lap).count();
+        t_lap = now;
+    };
+    ShardComm &comm = c->comm;
+    const int R = comm.rank, W = comm.world;
+    cudaStream_t st = c->stream.s;
+    CK(cudaSetDevice(comm.device));
+
+    // ---- 1. the vote on the arguments, and the directory check ----
+    long long rec[CV_WORDS] = {};
+    long long n_tok = 0;
+    bool token = false;
+    auto local = [&]() -> pb_status {
+        if (!params || !index_dir || n_docs < 0 || (n_docs && !doc_lengths)) return pb_fail(PB_ERR_INVALID, "null or negative argument");
+        if (space != PB_MEM_HOST && space != PB_MEM_DEVICE) return pb_fail(PB_ERR_INVALID, "bad memory_space %d", space);
+        const pb_create_params &p = *params;
+        if (p.nbits <= 0 || 8 % p.nbits != 0) return pb_fail(PB_ERR_INVALID, "nbits must be a divisor of 8, got %d", p.nbits);
+        if (p.batch_size <= 0 || p.kmeans_niters < 0 || p.max_points_per_centroid <= 0)
+            return pb_fail(PB_ERR_INVALID, "bad create parameters");
+        if (centroids_in && (num_centroids <= 0 || num_centroids >= (1ll << 32) - 1))
+            return pb_fail(PB_ERR_INVALID, "bad num_centroids %lld", (long long)num_centroids);
+        for (long long i = 0; i < n_docs; ++i) {
+            if (doc_lengths[i] < 0 || doc_lengths[i] > (1 << 30))
+                return pb_fail(PB_ERR_INVALID, "doc_lengths[%lld] = %lld", i, (long long)doc_lengths[i]);
+            n_tok += doc_lengths[i];
+        }
+        if (n_tok && !emb) return pb_fail(PB_ERR_INVALID, "null argument");
+        if (W > 1 && !comm.has_p2p()) return pb_fail(PB_ERR_COMM, "libnccl.so.2 lacks ncclSend / ncclRecv");
+        CKS(BuiltDims::check(dim));
+        const long long words[] = {dim, p.nbits, p.kmeans_niters, p.max_points_per_centroid, (long long)p.num_partitions,
+                                   (long long)p.batch_size, (long long)p.seed, centroids_in ? (long long)num_centroids : 0};
+        memcpy(rec + CV_DIM, words, sizeof words);
+        Fnv64 fc, fd;
+        if (centroids_in) fc.add(centroids_in, (size_t)num_centroids * dim * 4);
+        fd.add(index_dir, strlen(index_dir) + 1);
+        rec[CV_CENT] = (long long)fc.h;
+        rec[CV_DIR] = (long long)fd.h;
+        if (R == 0) {
+            Fnv64 ft;
+            ft.put(clock::now().time_since_epoch().count());
+            ft.put((uintptr_t)c);
+            rec[CV_TOKEN] = (long long)(ft.h >> 1);
+            token = true;
+            CKS(pb_dir_token_put(index_dir, rec[CV_TOKEN]));
+        }
+        return PB_OK;
+    };
+    rec[CV_STATUS] = local();
+    rec[CV_RANK] = R;
+    rec[CV_WORLD] = W;
+    rec[CV_D] = n_docs;
+    rec[CV_N] = n_tok;
+    std::vector<long long> all;
+    pb_status s = gather_words(comm, rec, CV_WORDS, all, true);
+    if (!s) s = first_failure(comm, all, CV_WORDS, "; nothing was written");
+    auto at = [&](int r, int w) { return all[(size_t)r * CV_WORDS + w]; };
+    std::vector<long long> base((size_t)W + 1, 0), tokb((size_t)W + 1, 0);
+    for (int r = 0; r < W && !s; ++r) {
+        bool same = at(r, CV_RANK) == r && at(r, CV_WORLD) == W;
+        for (int w = CV_DIM; w <= CV_DIR; ++w) same = same && at(r, w) == at(0, w);
+        if (!same) s = pb_fail(PB_ERR_INVALID, "rank %d was called with other arguments than rank 0", r);
+        base[r + 1] = base[r] + at(r, CV_D);
+        tokb[r + 1] = tokb[r] + at(r, CV_N);
+    }
+    const long long D = base[W], N = tokb[W];
+    if (!s && D <= 0) s = pb_fail(PB_ERR_INVALID, "no documents");
+    if (!s && N <= 0) s = pb_fail(PB_ERR_INVALID, "no embeddings");
+    if (!s && D >= (1ll << 32) - 1) s = pb_fail(PB_ERR_UNSUPPORTED, "global doc ids must stay below 2^32-1");
+    if (!s) s = create_vote(comm, R ? pb_dir_token_check(index_dir, at(0, CV_TOKEN)) : PB_OK,
+                            " finding the index directory; nothing was written");
+    if (token) pb_dir_token_drop(index_dir);
+    if (s) return s;
+    const pb_create_params &cfg = *params;
+    const std::string dir = std::string(index_dir) + "/";
+    const int packed = dim * cfg.nbits / 8, nopt = 1 << cfg.nbits;
+    const long long T0 = tokb[R];
+    cudaDeviceProp prop;
+    CK(cudaGetDeviceProperties(&prop, comm.device));
+    const int sms = prop.multiProcessorCount;
+
+    // every document's length: O(D) host words, as pb_create_index's own plan
+    long long maxD = 0;
+    for (int r = 0; r < W; ++r) maxD = std::max(maxD, at(r, CV_D));
+    std::vector<long long> mine((size_t)maxD, 0), gl;
+    for (long long i = 0; i < n_docs; ++i) mine[i] = doc_lengths[i];
+    CKS(gather_words(comm, mine.data(), (int)maxD, gl, true));
+    std::vector<int64_t> lens((size_t)D);
+    std::vector<long long> off((size_t)D + 1, 0);
+    for (int r = 0; r < W; ++r)
+        for (long long i = 0; i < at(r, CV_D); ++i) lens[base[r] + i] = gl[(size_t)r * maxD + i];
+    for (long long d = 0; d < D; ++d) off[d + 1] = off[d] + lens[d];
+    std::vector<long long>().swap(gl);
+    auto owner_tok = [&](long long t) { return (int)(std::upper_bound(tokb.begin(), tokb.end(), t) - tokb.begin()) - 1; };
+    auto owner_doc = [&](long long d) { return (int)(std::upper_bound(base.begin(), base.end(), d) - base.begin()) - 1; };
+    lap(CP_PLAN);
+
+    // ---- 2. centroids (kmeans.rs:273-419): this rank's fit points in global fit order, its seeds, one Lloyd loop ----
+    long long K = num_centroids;
+    std::vector<float> cent;
+    if (centroids_in) {
+        cent.assign(centroids_in, centroids_in + (size_t)K * dim);
+    } else {
+        const long long n_sdocs = pb_kmeans_num_sample_docs(D);
+        const std::vector<long long> sdocs = shuffled_prefix(D, n_sdocs, cfg.seed);
+        std::vector<long long> srow((size_t)n_sdocs + 1, 0);  // first sample row of each sampled doc
+        for (long long j = 0; j < n_sdocs; ++j) srow[j + 1] = srow[j] + lens[sdocs[j]];
+        const long long n_stok = srow[n_sdocs];
+        if (n_stok <= 0) return pb_fail(PB_ERR_INVALID, "the k-means sample holds no embeddings");
+        K = cfg.num_partitions > 0 ? std::min<long long>(cfg.num_partitions, n_stok)
+                                   : pb_kmeans_num_partitions(D, (double)n_stok / (double)n_sdocs, n_stok);
+        long long n_fit = n_stok;
+        std::vector<long long> pick;  // at most max_points_per_centroid points per centroid
+        if (n_stok > K * (long long)cfg.max_points_per_centroid) {
+            n_fit = K * (long long)cfg.max_points_per_centroid;
+            pick = shuffled_prefix(n_stok, n_fit, cfg.seed ^ 0x5bd1e995u);
+        }
+        std::vector<long long> my_fit, my_tok;  // my fit points: their fit indices (ascending) and my token ids
+        for (long long i = 0; i < n_fit; ++i) {
+            const long long r = pick.empty() ? i : pick[i];
+            const long long j = (long long)(std::upper_bound(srow.begin(), srow.end(), r) - srow.begin()) - 1;
+            const long long t = off[sdocs[j]] + (r - srow[j]);
+            if (owner_tok(t) == R) {
+                my_fit.push_back(i);
+                my_tok.push_back(t - T0);
+            }
+        }
+        const std::vector<long long> seeds = lcg_seeds(n_fit, K, cfg.seed * 6364136223846793005ull + 1442695040888963407ull);
+        std::vector<long long> sidx((size_t)K, -1);  // my fit point of each seed I own
+        for (long long k = 0; k < K; ++k) {
+            auto it = std::lower_bound(my_fit.begin(), my_fit.end(), seeds[k]);
+            if (it != my_fit.end() && *it == seeds[k]) sidx[k] = it - my_fit.begin();
+        }
+        DevBuf dX, dC, didx;
+        auto prep = [&]() -> pb_status {
+            CKS(gather_rows(emb, space, dim, my_tok, dX, sms, st));
+            CKS(dC.ensure((size_t)K * dim * 4));
+            CKS(upload(didx, sidx.data(), (size_t)K * 8, PB_MEM_HOST));
+            k_seed_rows<<<sms * 4, 256, 0, st>>>(dX.as<float>(), didx.as<long long>(), K, dim, dC.as<float>());
+            CK(cudaGetLastError());
+            return PB_OK;
+        };
+        CKS(create_vote(comm, prep(), " gathering its k-means points; nothing was written"));
+        CKS(comm.allreduce_sum(st, dC.as<float>(), (size_t)K * dim, c->stage));
+        CKS(lloyd(comm.joined() ? &comm : nullptr, &c->stage, st, dX.as<float>(), (long long)my_tok.size(), dim, K,
+                  cfg.kmeans_niters, sms, dC.as<float>()));
+        cent.resize((size_t)K * dim);
+        CK(cudaMemcpyAsync(cent.data(), dC.p, cent.size() * 4, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+    }
+    lap(CP_KMEANS);
+
+    // ---- 3. codec training on rank 0, on pb_create_index's held-out rows in its order (index.rs:195-287) ----
+    const long long n_cdocs = pb_codec_num_sample_docs(D);
+    const std::vector<long long> cdocs = shuffled_prefix(D, n_cdocs, cfg.seed + 1);
+    const long long want = pb_codec_heldout_tokens(N);
+    std::vector<std::pair<long long, long long>> held;  // (first global token, rows), from the end of the sample list
+    std::vector<long long> my_held, held_rows((size_t)W, 0);
+    long long got = 0;
+    for (long long i = (long long)cdocs.size() - 1; i >= 0 && got < want; --i) {
+        const long long d = cdocs[(size_t)i], take = std::min<long long>(want - got, lens[d]);
+        got += take;
+        if (!take) continue;
+        held.emplace_back(off[d], take);
+        const int r = owner_doc(d);
+        held_rows[r] += take;
+        if (r == R)
+            for (long long t = 0; t < take; ++t) my_held.push_back(off[d] - T0 + t);
+    }
+    std::vector<float> cutoffs((size_t)std::max(nopt - 1, 1)), weights((size_t)nopt), avg_res((size_t)dim);
+    float threshold = 0.0f;
+    {
+        DevBuf hs, hr;
+        std::vector<size_t> first((size_t)W + 1, 0);
+        for (int r = 0; r < W; ++r) first[r + 1] = first[r] + (size_t)held_rows[r] * dim * 4;
+        auto gather = [&]() -> pb_status {
+            CKS(gather_rows(emb, space, dim, my_held, hs, sms, st));
+            if (R == 0) CKS(hr.ensure(std::max<size_t>(first[W], 16)));
+            return PB_OK;
+        };
+        CKS(create_vote(comm, gather(), " gathering its held-out rows; nothing was written"));
+        std::vector<float> rows(R == 0 ? (size_t)got * dim : 0);
+        if (comm.joined()) {
+            std::vector<const void *> sp((size_t)W, nullptr);
+            std::vector<void *> rp((size_t)W, nullptr);
+            std::vector<size_t> sb((size_t)W, 0), rb((size_t)W, 0);
+            sp[0] = hs.p;
+            sb[0] = first[R + 1] - first[R];
+            for (int r = 0; r < W && R == 0; ++r) {
+                rp[r] = hr.as<char>() + first[r];
+                rb[r] = first[r + 1] - first[r];
+            }
+            CKS(comm.exchange(st, 1, sp.data(), sb.data(), rp.data(), rb.data()));
+            if (R == 0 && got) CK(cudaMemcpy(rows.data(), hr.p, first[W], cudaMemcpyDeviceToHost));
+        } else if (got) {
+            CK(cudaMemcpy(rows.data(), hs.p, first[W], cudaMemcpyDeviceToHost));
+        }
+        // the trainer reassembles the sample order from the ranks' pieces, trains, and shares the codec's numbers
+        const int nf = (nopt - 1) + nopt + dim + 1, words = 1 + (nf + 1) / 2;
+        std::vector<long long> mine_w((size_t)words, 0), allw;
+        if (R == 0) {
+            auto train = [&]() -> pb_status {
+                std::vector<float> heldout((size_t)got * dim);
+                std::vector<size_t> cur(first.begin(), first.end() - 1);
+                size_t w = 0;
+                for (const auto &pc : held) {
+                    const int r = owner_tok(pc.first);
+                    const size_t b = (size_t)pc.second * dim * 4;
+                    memcpy(reinterpret_cast<char *>(heldout.data()) + w, reinterpret_cast<char *>(rows.data()) + cur[r], b);
+                    cur[r] += b;
+                    w += b;
+                }
+                pb_codec *tc = nullptr;
+                CKS(pb_codec_open(comm.device, cent.data(), K, dim, cfg.nbits, nullptr, &tc));
+                pb_status ts = pb_codec_train(tc, heldout.data(), got, cutoffs.data(), weights.data(), avg_res.data(), &threshold);
+                pb_codec_close(tc);
+                return ts;
+            };
+            mine_w[0] = train();
+            float *f = reinterpret_cast<float *>(mine_w.data() + 1);
+            memcpy(f, cutoffs.data(), (size_t)(nopt - 1) * 4);
+            memcpy(f + nopt - 1, weights.data(), (size_t)nopt * 4);
+            memcpy(f + 2 * nopt - 1, avg_res.data(), (size_t)dim * 4);
+            f[nf - 1] = threshold;
+        }
+        CKS(gather_words(comm, mine_w.data(), words, allw, true));
+        CKS(first_failure(comm, allw, words, " training the codec; nothing was written"));
+        const float *f = reinterpret_cast<const float *>(allw.data() + 1);  // rank 0's record
+        memcpy(cutoffs.data(), f, (size_t)(nopt - 1) * 4);
+        memcpy(weights.data(), f + nopt - 1, (size_t)nopt * 4);
+        memcpy(avg_res.data(), f + 2 * nopt - 1, (size_t)dim * 4);
+        threshold = f[nf - 1];
+    }
+    lap(CP_CODEC);
+
+    // ---- 4. encode this rank's documents straight into its shard, slab by slab ----
+    std::unique_ptr<pb_index, IndexCloser> ix;
+    pb_codec *enc = nullptr;
+    auto encode = [&]() -> pb_status {
+        CKS(pb_codec_open(comm.device, cent.data(), K, dim, cfg.nbits, cutoffs.data(), &enc));
+        pb_index_desc d;
+        memset(&d, 0, sizeof d);
+        d.dim = dim;
+        d.nbits = cfg.nbits;
+        d.num_centroids = K;
+        d.num_documents = n_docs;
+        d.num_embeddings = n_tok;
+        d.centroids = cent.data();
+        d.bucket_weights = weights.data();
+        d.doc_lengths = doc_lengths;
+        d.device = comm.device;
+        d.memory_space = PB_MEM_HOST;
+        d.doc_id_base = base[R];
+        pb_index *h = nullptr;
+        CKS(pb_index_open_begin(&d, &h));
+        ix.reset(h);
+        const long long slab = 1ll << 20;
+        DevBuf dX, dcodes, dpk;
+        if (space == PB_MEM_HOST) CKS(dX.ensure((size_t)std::min(n_tok, slab) * dim * 4 + 16));
+        CKS(dcodes.ensure((size_t)std::min(n_tok, slab) * 8 + 16));
+        CKS(dpk.ensure((size_t)std::min(n_tok, slab) * packed + 16));
+        for (long long o = 0; o < n_tok; o += slab) {
+            const long long m = std::min(slab, n_tok - o);
+            const float *x = emb + (size_t)o * dim;
+            if (space == PB_MEM_HOST) {
+                CK(cudaMemcpy(dX.p, x, (size_t)m * dim * 4, cudaMemcpyHostToDevice));
+                x = dX.as<float>();
+            }
+            CKS(codec_encode_device(enc, x, m, dcodes.as<long long>(), dpk.as<uint8_t>(), nullptr));
+            CKS(pb_index_upload_tokens(ix.get(), o, dcodes.as<int64_t>(), dpk.as<uint8_t>(), m, PB_MEM_DEVICE));
+        }
+        lap(CP_ENCODE);
+        CKS(pb_index_finalize(ix.get()));
+        lap(CP_SHARD);
+        return PB_OK;
+    };
+    s = encode();
+    if (enc) pb_codec_close(enc);
+    CKS(create_vote(comm, s, " encoding its documents; nothing was written"));
+
+    // ---- 5. chunk files: chunk i is written by the rank holding its first document; the head of a rank's range that
+    // lies in a chunk begun on an earlier rank goes to that chunk's writer ----
+    const long long bs = cfg.batch_size, n_chunks = (D + bs - 1) / bs;
+    std::vector<int> head_to((size_t)W, -1);  // writer of each rank's head, or -1
+    std::vector<long long> head_end((size_t)W, 0);
+    bool any_head = false;
+    for (int r = 0; r < W; ++r) {
+        if (base[r] == base[r + 1] || base[r] % bs == 0) continue;
+        const long long c0 = base[r] / bs * bs;
+        head_to[r] = owner_doc(c0);
+        head_end[r] = std::min(c0 + bs, base[r + 1]);
+        any_head = true;
+    }
+    DevBuf rc, rr;  // the heads this rank receives, in rank order
+    std::vector<long long> recv_tok((size_t)W + 1, 0);
+    for (int r = 0; r < W; ++r)
+        recv_tok[r + 1] = recv_tok[r] + (head_to[r] == R && r != R ? off[head_end[r]] - off[base[r]] : 0);
+    if (any_head) {
+        CKS(rc.ensure((size_t)recv_tok[W] * 4 + 16));
+        CKS(rr.ensure((size_t)recv_tok[W] * packed + 16));
+        std::vector<const void *> sp((size_t)W * 2, nullptr);
+        std::vector<void *> rp((size_t)W * 2, nullptr);
+        std::vector<size_t> sb((size_t)W * 2, 0), rb((size_t)W * 2, 0);
+        if (head_to[R] >= 0) {
+            const long long n = off[head_end[R]] - off[base[R]];
+            sp[(size_t)head_to[R] * 2] = ix->codes.p;
+            sp[(size_t)head_to[R] * 2 + 1] = ix->residuals.p;
+            sb[(size_t)head_to[R] * 2] = (size_t)n * 4;
+            sb[(size_t)head_to[R] * 2 + 1] = (size_t)n * packed;
+        }
+        for (int r = 0; r < W; ++r) {
+            const long long n = recv_tok[r + 1] - recv_tok[r];
+            rp[(size_t)r * 2] = rc.as<uint32_t>() + recv_tok[r];
+            rp[(size_t)r * 2 + 1] = rr.as<uint8_t>() + (size_t)recv_tok[r] * packed;
+            rb[(size_t)r * 2] = (size_t)n * 4;
+            rb[(size_t)r * 2 + 1] = (size_t)n * packed;
+        }
+        CKS(comm.exchange(st, 2, sp.data(), sb.data(), rp.data(), rb.data()));
+    }
+    auto write_chunks = [&]() -> pb_status {
+        for (long long ch = (base[R] + bs - 1) / bs; n_docs && ch * bs < base[R + 1]; ++ch) {
+            const long long d0 = ch * bs, d1 = std::min(D, d0 + bs), dm = std::min(d1, base[R + 1]);
+            const long long t0 = off[d0], n_own = off[dm] - t0, n = off[d1] - t0;
+            const long long n_in = dm < d1 ? recv_tok[W] : 0;  // only the last chunk crosses into later ranks
+            std::vector<uint32_t> c32((size_t)n);
+            std::vector<int64_t> codes((size_t)n);
+            std::vector<uint8_t> res((size_t)n * packed);
+            if (n_own) {
+                CK(cudaMemcpy(c32.data(), ix->codes.as<uint32_t>() + (t0 - T0), (size_t)n_own * 4, cudaMemcpyDeviceToHost));
+                CK(cudaMemcpy(res.data(), ix->residuals.as<uint8_t>() + (size_t)(t0 - T0) * packed, (size_t)n_own * packed,
+                              cudaMemcpyDeviceToHost));
+            }
+            if (n_in) {
+                CK(cudaMemcpy(c32.data() + n_own, rc.p, (size_t)n_in * 4, cudaMemcpyDeviceToHost));
+                CK(cudaMemcpy(res.data() + (size_t)n_own * packed, rr.p, (size_t)n_in * packed, cudaMemcpyDeviceToHost));
+            }
+            if (n_own + n_in != n) return pb_fail(PB_ERR_INVALID, "chunk %lld: %lld of %lld rows", ch, n_own + n_in, n);
+            for (long long i = 0; i < n; ++i) codes[i] = c32[i];
+            CKS(pb_write_chunk(dir, ch, codes.data(), res.data(), n, packed, lens.data() + d0, d1 - d0, t0));
+        }
+        return PB_OK;
+    };
+    CKS(create_vote(comm, write_chunks(), " writing its chunk files"));
+    lap(CP_CHUNKS);
+
+    // ---- 6. ivf.npy: list k is the ranks' lists of k in rank order (each ascending, so the whole list is); rank 0
+    // creates the file at its final size and every rank writes its pieces at their offsets.  Then the codec's files,
+    // and metadata.json last ----
+    int64_t my_total = 0;
+    std::vector<int64_t> my_ivf;
+    std::vector<int32_t> my_len((size_t)K);
+    CKS(create_vote(comm, [&]() -> pb_status {
+        CKS(pb_index_export_ivf(ix.get(), nullptr, nullptr, &my_total));
+        my_ivf.resize((size_t)std::max<int64_t>(my_total, 1));
+        return pb_index_export_ivf(ix.get(), my_ivf.data(), my_len.data(), &my_total);
+    }(), " exporting its inverted file"));
+    const int lw = (int)((K + 1) / 2);
+    std::vector<long long> lw_mine((size_t)lw, 0), lw_all;
+    memcpy(lw_mine.data(), my_len.data(), (size_t)K * 4);
+    CKS(gather_words(comm, lw_mine.data(), lw, lw_all, true));
+    auto len_of = [&](int r, long long k) { return (long long)reinterpret_cast<const int32_t *>(lw_all.data() + (size_t)r * lw)[k]; };
+    std::vector<int32_t> tot((size_t)K, 0);
+    std::vector<NpyPiece> pieces;
+    long long ivf_total = 0, src = 0;
+    for (long long k = 0; k < K; ++k) {
+        long long before = 0;
+        for (int r = 0; r < W; ++r) {
+            if (r < R) before += len_of(r, k);
+            tot[k] += (int32_t)len_of(r, k);
+        }
+        if (my_len[k])
+            pieces.push_back({(size_t)(ivf_total + before) * 8, (size_t)my_len[k] * 8, reinterpret_cast<const char *>(my_ivf.data() + src)});
+        src += my_len[k];
+        ivf_total += tot[k];
+    }
+    CKS(create_vote(comm, R ? PB_OK : [&]() -> pb_status {
+        CKS(npy_create(dir + "ivf.npy", "<i8", {ivf_total}, (size_t)ivf_total * 8));
+        CKS(write_npy(dir + "ivf_lengths.npy", "<i4", {K}, tot.data(), (size_t)K * 4));
+        return pb_write_codec_files(dir, K, dim, cfg.nbits, cent.data(), cutoffs.data(), weights.data(), avg_res.data(),
+                                    threshold, n_chunks);
+    }(), " writing the index files"));
+    CKS(create_vote(comm, npy_put(dir + "ivf.npy", "<i8", {ivf_total}, pieces), " writing its part of ivf.npy"));
+    CKS(create_vote(comm, R ? PB_OK : pb_write_create_meta(dir, n_chunks, cfg.nbits, K, N, D, dim), " writing metadata.json"));
+    lap(CP_IVF);
+    if (out_first) *out_first = base[R];
+    if (out_shard) *out_shard = ix.release();
+    return PB_OK;
+}
+
+extern "C" pb_status pb_create_index_sharded(pb_build_comm *c, const float *embeddings, const int64_t *doc_lengths,
+                                             int64_t n_docs, int32_t dim, int32_t memory_space, const float *centroids,
+                                             int64_t num_centroids, const pb_create_params *params, const char *index_dir,
+                                             pb_index **out_shard, int64_t *out_first_doc_id) {
+    if (out_shard) *out_shard = nullptr;
+    if (out_first_doc_id) *out_first_doc_id = 0;
+    if (!c) return pb_fail(PB_ERR_INVALID, "null argument");
+    return create_collective(c, embeddings, doc_lengths, n_docs, dim, memory_space, centroids, num_centroids, params,
+                             index_dir, out_shard, out_first_doc_id);
+}
+
+pb_status pb_create_local(const float *embeddings, const int64_t *doc_lengths, int64_t n_docs, int32_t dim,
+                          const pb_create_params *params, const char *index_dir, pb_index **out_index) {
+    CKS(check_device(params->device));
+    pb_build_comm c;
+    c.comm.device = params->device;
+    CK(cudaSetDevice(params->device));
+    CK(cudaStreamCreateWithFlags(&c.stream.s, cudaStreamNonBlocking));
+    return create_collective(&c, embeddings, doc_lengths, n_docs, dim, PB_MEM_HOST, nullptr, 0, params, index_dir, out_index,
+                             nullptr);
+}
+
+extern "C" pb_status pb_last_create_ms(float *out_ms) {
+    if (!out_ms) return pb_fail(PB_ERR_INVALID, "null argument");
+    memcpy(out_ms, g_create_ms, sizeof g_create_ms);
     return PB_OK;
 }

@@ -46,6 +46,40 @@ pb_status pb_dir_append(const char *index_dir, long long old_D, long long K, int
                         const int64_t *codes, const uint8_t *residuals, const int64_t *doc_lengths, long long n_docs,
                         const int64_t *ivf, long long ivf_total, const int32_t *ivf_lengths);
 
+// Index build (builder.cpp).  The first `take` entries of a seeded Fisher-Yates shuffle of 0..n-1 (splitmix64): the
+// sample plan of pb_create_index.
+std::vector<long long> shuffled_prefix(long long n, long long take, uint64_t seed);
+// NPY v1.0 files: a whole file; a file of `bytes` payload bytes whose payload is written later, in pieces (byte offset
+// into the payload), by any process
+pb_status write_npy(const std::string &path, const char *descr, const std::vector<long long> &shape, const void *data,
+                    size_t bytes);
+pb_status write_text(const std::string &path, const std::string &txt);
+struct NpyPiece {
+    size_t offset, bytes;
+    const char *src;
+};
+pb_status npy_create(const std::string &path, const char *descr, const std::vector<long long> &shape, size_t bytes);
+pb_status npy_put(const std::string &path, const char *descr, const std::vector<long long> &shape,
+                  const std::vector<NpyPiece> &pieces);
+// chunk c's four files: n tokens starting at token t0 of the index, its n_docs documents' lengths
+pb_status pb_write_chunk(const std::string &dir, long long c, const int64_t *codes, const uint8_t *residuals, long long n,
+                         int packed, const int64_t *doc_lengths, long long n_docs, long long t0);
+// centroids.npy, bucket_cutoffs.npy, bucket_weights.npy, avg_residual.npy, cluster_threshold.npy, plan.json
+pb_status pb_write_codec_files(const std::string &dir, long long K, int dim, int nbits, const float *centroids,
+                               const float *cutoffs, const float *weights, const float *avg_res, float threshold,
+                               long long n_chunks);
+// metadata.json of a new index of D documents and N tokens
+pb_status pb_write_create_meta(const std::string &dir, long long n_chunks, int nbits, long long K, long long N, long long D,
+                               int dim);
+// the directory check of a collective build: rank 0 creates index_dir and a token file in it, the other ranks check
+// that they read the same token (PB_ERR_IO otherwise), rank 0 removes the file
+pb_status pb_dir_token_put(const char *index_dir, long long token);
+pb_status pb_dir_token_check(const char *index_dir, long long token);
+void pb_dir_token_drop(const char *index_dir);
+// pb_create_index after its argument checks: pb_create_index_sharded over a group of one on params->device
+pb_status pb_create_local(const float *embeddings, const int64_t *doc_lengths, int64_t n_docs, int32_t dim,
+                          const pb_create_params *params, const char *index_dir, pb_index **out_index);
+
 // PB_ERR_INVALID (PB_ERR_IO when unreadable) unless the directory's metadata.json holds D documents and nbits
 pb_status pb_dir_check_documents(const char *index_dir, int nbits, long long D);
 

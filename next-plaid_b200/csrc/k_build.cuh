@@ -188,6 +188,15 @@ __global__ void k_gather_rows(const float *__restrict__ X, const long long *__re
         out[i] = X[(size_t)idx[i / dim] * dim + (i % dim)];
 }
 
+// k_gather_rows where idx[k] < 0 gives a zero row: one rank's part of a seed table that an all-reduce completes
+__global__ void k_seed_rows(const float *__restrict__ X, const long long *__restrict__ idx, long long K, int dim,
+                            float *__restrict__ out) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < K * dim; i += (long long)gridDim.x * blockDim.x) {
+        const long long r = idx[i / dim];
+        out[i] = r >= 0 ? X[(size_t)r * dim + (i % dim)] : 0.0f;
+    }
+}
+
 // ==========================================================================================
 // Tensor-core certified filter for nearest-centroid assignment (index-build path).
 //

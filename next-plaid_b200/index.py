@@ -99,7 +99,7 @@ EXPORTS = [
     "pb_index_delete", "pb_last_delete_ms", "pb_index_load_range", "pb_index_dir_shard_bounds",
     "pb_index_delete_sharded", "pb_index_append_sharded", "pb_index_append_encoded_sharded",
     "pb_index_rebalance_sharded", "pb_index_load_range_flags", "pb_index_memory", "pb_last_staging_stats",
-    "pb_search", "pb_index_set_coalescing", "pb_index_coalesce_stats",
+    "pb_search", "pb_index_set_coalescing", "pb_index_coalesce_stats", "pb_create_index_sharded", "pb_last_create_ms",
 ]
 
 PB_OPEN_ADOPT_RESIDUALS, PB_OPEN_HOST_RESIDUALS = 1, 2
@@ -194,6 +194,9 @@ def load_library():
         L.pb_build_comm_destroy.argtypes = [C.c_void_p]
         L.pb_build_comm_destroy.restype = None
         L.pb_kmeans_fit_dp.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_int32, C.c_uint64, C.c_void_p]
+        L.pb_create_index_sharded.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32,
+                                              C.c_void_p, C.c_int64, C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p]
+        L.pb_last_create_ms.argtypes = [C.c_void_p]
         L.pb_comm_unique_id.argtypes = [C.c_void_p]
         L.pb_index_comm_init.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32]
         L.pb_shard_group_create.argtypes = [C.c_int32, C.c_void_p]
@@ -856,6 +859,90 @@ def create_index(embeddings: Sequence[np.ndarray], index_dir: str, nbits: int = 
     h = C.c_void_p()
     _check(L.pb_create_index(_ptr(flat), _ptr(dl), len(dl), flat.shape[1], C.byref(p), index_dir.encode(), C.byref(h)))
     return MmapIndex(h.value)
+
+
+CREATE_PHASES = ["plan", "kmeans", "codec", "encode", "shard", "chunks", "ivf"]
+
+
+def last_create_ms() -> dict:
+    """pb_last_create_ms: the calling thread's last create_index / create_index_sharded rank, wall ms per phase."""
+    v = np.zeros(len(CREATE_PHASES), np.float32)
+    _check(load_library().pb_last_create_ms(_ptr(v)))
+    return dict(zip(CREATE_PHASES, v.tolist()))
+
+
+def _rank_docs(docs, dim):
+    """(embeddings pointer, memory_space, lengths, keep-alive) of one rank's documents: numpy arrays (host) or CUDA
+    tensors (device, memory_space 1)"""
+    lens = np.array([int(d.shape[0]) for d in docs], np.int64)
+    if len(docs) and not isinstance(docs[0], np.ndarray) and getattr(docs[0], "is_cuda", False):
+        import torch
+        flat = torch.cat([d.reshape(-1, dim) for d in docs], 0).to(torch.float32).contiguous()
+        return flat.data_ptr() if flat.numel() else None, 1, lens, flat
+    flat = (np.ascontiguousarray(np.concatenate([np.asarray(d) for d in docs], 0), np.float32) if len(docs)
+            else np.zeros((0, dim), np.float32))
+    return _ptr(flat), 0, lens, flat
+
+
+def create_index_sharded(shards: Sequence[Sequence], index_dir: str, centroids: Optional[np.ndarray] = None,
+                         nbits: int = 4, kmeans_niters: int = 4, num_partitions: int = 0, batch_size: int = 50_000,
+                         seed: int = 42, device=0, max_points_per_centroid: int = 256, nccl: Optional[tuple] = None,
+                         dim: Optional[int] = None):
+    """pb_create_index_sharded: create_index for a corpus split over the ranks of a doc-sharded deployment.  Rank r's
+    documents (numpy arrays or CUDA tensors) get global ids after every lower rank's; the directory equals what
+    create_index writes for their concatenation.  centroids: [K, dim], or None for k-means.  Without `nccl`: one host
+    thread per rank through an in-process group on `device` (one device, or one per rank); returns one MmapIndex per
+    rank (each with .first_doc_id and .create_ms, its phase times), ready for ShardGroup.  With nccl = (unique_id, rank, world): shards[0] is this
+    rank's documents and this rank's MmapIndex is returned."""
+    L = load_library()
+    if dim is None:
+        dim = next((int(d.shape[1]) for docs in shards for d in docs),
+                   0 if centroids is None else int(np.asarray(centroids).shape[-1]))
+    cen = None if centroids is None else np.ascontiguousarray(centroids, np.float32)
+    if cen is not None and (cen.ndim != 2 or cen.shape[1] != dim):
+        raise PlaidError(PB_ERR_INVALID, f"centroids have shape {cen.shape}, the documents dim {dim}")
+    path = os.fsencode(index_dir)
+
+    def build(comm, r, docs, dev):
+        emb, space, lens, keep = _rank_docs(docs, dim)
+        p = _CreateParams(nbits, kmeans_niters, max_points_per_centroid, dev, num_partitions, batch_size, seed)
+        h, first = C.c_void_p(), C.c_int64()
+        _check(L.pb_create_index_sharded(comm, emb, _ptr(lens), len(lens), dim, space, _ptr(cen),
+                                         0 if cen is None else cen.shape[0], C.byref(p), path, C.byref(h),
+                                         C.byref(first)))
+        del keep
+        ix = MmapIndex(h.value, index_dir)
+        ix.first_doc_id = int(first.value)
+        ix.create_ms = last_create_ms()         # this rank's phase times (thread-local in the library)
+        return ix
+
+    if nccl is not None:
+        uid, rank, world = nccl
+        buf = np.frombuffer(bytes(uid), np.uint8).copy()
+        dev = device if isinstance(device, int) else device[rank]
+        h = C.c_void_p()
+        _check(L.pb_build_comm_init(_ptr(buf), rank, world, dev, C.byref(h)))
+        try:
+            return build(h, rank, shards[0], dev)
+        finally:
+            L.pb_build_comm_destroy(h)
+    G = len(shards)
+    devs = [device] * G if isinstance(device, int) else list(device)
+    g = C.c_void_p()
+    _check(L.pb_shard_group_create(G, C.byref(g)))
+
+    def run(r):
+        h = C.c_void_p()
+        _check(L.pb_build_comm_group(g, r, devs[r], C.byref(h)))
+        try:
+            return build(h, r, shards[r], devs[r])
+        finally:
+            L.pb_build_comm_destroy(h)
+    try:
+        out = _per_rank(G, run)
+    finally:
+        L.pb_shard_group_destroy(g)
+    return out
 
 
 def kmeans_fit_dp(shards: Sequence[np.ndarray], K: int, niters: int = 4, seed: int = 42, device: int = 0,

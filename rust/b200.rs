@@ -132,6 +132,11 @@ extern "C" {
                                  out: *mut *mut c_void) -> c_int;
     fn pb_index_memory(ix: *const c_void, device_bytes: *mut i64, host_bytes: *mut i64) -> c_int;
     fn pb_last_staging_stats(ix: *mut c_void, docs: *mut i64, bytes: *mut i64, ms: *mut f32) -> c_int;
+    // pb_create_index_sharded (DESIGN §4n): `comm` is a pb_build_comm, `params` a pb_create_params
+    fn pb_create_index_sharded(comm: *mut c_void, embeddings: *const f32, doc_lengths: *const i64, n_docs: i64, dim: i32,
+                               memory_space: i32, centroids: *const f32, num_centroids: i64, params: *const c_void,
+                               index_dir: *const c_char, out_shard: *mut *mut c_void, out_first_doc_id: *mut i64)
+                               -> c_int;
 }
 
 /// pb_index_desc.flags: the packed residuals in pinned host memory, the kept docs' rows staged per search (DESIGN §4j).
