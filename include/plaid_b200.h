@@ -373,7 +373,8 @@ PB_API pb_status pb_search_batch_params(pb_index *ix, const float *queries, cons
  *     pb_last_call_ms and pb_last_staging_stats report the merged batch the request rode in (n_queries counts that
  *     batch's queries), on every thread of that batch alike; after a re-run alone, the request's own run.
  *   - Appends and deletes are seen entirely or not at all, as by any search.
- * Doc-sharded handles always run the plain batch of one (a collective, called on every rank in step). */
+ * Doc-sharded handles always run the plain batch of one (a collective, called on every rank in step); a handle of
+ * pb_index_load_devices coalesces as one handle does. */
 PB_API pb_status pb_search(pb_index *ix, const float *query, int64_t n_query_tokens, const pb_search_params *params,
                            const int64_t *subset, int64_t n_subset, int64_t *out_ids /* [top_k] */,
                            float *out_scores /* [top_k] */, int32_t *out_count);
@@ -389,7 +390,8 @@ PB_API pb_status pb_search(pb_index *ix, const float *query, int64_t n_query_tok
  * throughput of coalescing off and a p99 latency 2-3x lower; max_wait_us = 0 costs a lone caller nothing but leaves a
  * long p99 tail under load, and max_wait_us = 200 costs a lone caller more than a millisecond.
  * PB_ERR_INVALID: max_queries < 1, max_inflight < 1, max_wait_us < 0.  PB_ERR_UNSUPPORTED: max_queries > 1 on a
- * doc-sharded handle; pb_index_comm_init and pb_index_group_join turn coalescing off. */
+ * doc-sharded handle; pb_index_comm_init and pb_index_group_join turn coalescing off.  A handle of
+ * pb_index_load_devices is one index to its caller and coalesces (see there). */
 typedef struct pb_coalesce_config {
     int32_t max_queries;   /* largest merged batch; 1 = off */
     int32_t max_wait_us;   /* how long the leader of a batch of fewer than max_queries waits for more; 0 = never; at most 10 000 */
@@ -689,6 +691,56 @@ PB_API pb_status pb_index_comm_init(pb_index *ix, const uint8_t *id128, int32_t 
 PB_API pb_status pb_shard_group_create(int32_t world, pb_shard_group **out);
 PB_API void pb_shard_group_destroy(pb_shard_group *g);
 PB_API pb_status pb_index_group_join(pb_index *ix, pb_shard_group *g, int32_t rank);
+
+/* ---- a deployment behind one handle (DESIGN.md 4o) --------------------------------------------
+ *
+ * MmapIndex::load(path) over several devices of this process: rank r holds documents [bounds[r], bounds[r+1]) of
+ * pb_index_dir_shard_bounds(index_dir, n_devices) on devices[r], loaded as pb_index_load_range_flags does, the ranks
+ * joined in an in-process group.  devices may repeat (several ranks on one GPU).  flags as for
+ * pb_index_load_range_flags (PB_OPEN_HOST_RESIDUALS applies to every rank).
+ * Checks before any device is touched, in this order: a NULL index_dir, devices or out, or n_devices outside [1, 64]:
+ * PB_ERR_INVALID; no usable device: PB_ERR_CUDA (no CPU fallback); a device id outside [0, pb_device_count()):
+ * PB_ERR_INVALID.  The ranks load concurrently, one per thread; if any fails the call returns the lowest failing rank's
+ * status and message (a missing directory: PB_ERR_IO, as pb_index_load) and leaves nothing behind.
+ *
+ * The handle is one index to its caller; the ranks and their threads live inside the library (rank 0 runs on the
+ * calling thread, ranks 1..n-1 on one worker thread each, created here and joined by pb_index_close).  Every collective
+ * takes one lock of the deployment, so concurrent callers, coalesced batches and mutations reach every rank in one
+ * order.  The accessors, pb_index_memory and pb_index_shard_layout wait for a running mutation, as on one handle, but
+ * not for a running search; pb_decompress_documents and pb_exhaustive_scores use the ranks' threads and so wait for a
+ * running collective.  On such a handle:
+ *   pb_search_batch, pb_search_batch_traced (trace NULL), pb_search_batch_subsets, pb_search_batch_params, pb_search:
+ *     the sharded collective on every rank with the caller's arguments; results equal pb_index_load's bit for bit.
+ *   pb_index_set_coalescing, pb_index_coalesce_stats: the deployment's own queue (PB_COALESCE* read at load).  A request
+ *     is validated as a pb_index_load handle of the directory would validate it, and a merged batch is one
+ *     pb_search_batch_params collective, so the ranks see it in one order.  The group runs one collective at a time:
+ *     merged batches run one after another whatever max_inflight says, while requests gather into the next batch.
+ *   pb_index_num_documents, pb_index_num_embeddings, pb_index_memory: sums over the ranks; pb_index_avg_doclen,
+ *     num_partitions, embedding_dim, nbits: those of pb_index_load; pb_index_device: devices[0].
+ *   pb_decompress_documents: each id is answered by the rank holding it (ranks in parallel, output in input order).
+ *   pb_exhaustive_scores: rank r fills columns [bounds[r], bounds[r+1]) of each D-wide row.
+ *   pb_centroid_scores: rank 0 (the centroids are replicated).
+ *   pb_index_delete, pb_index_append, pb_index_append_encoded: the _sharded twin on every rank (its rules apply;
+ *     index_dir is allowed and the last rank writes it).  Only the last rank receives the codec and the documents: a
+ *     codec on another device than the last rank's is PB_ERR_INVALID, nothing changed.
+ *   pb_index_rebalance_sharded: on every rank with the same bounds.
+ *   pb_set_fast_approx, pb_set_scores_tc, pb_set_fast_exact, pb_set_profiling, pb_set_lanes: applied to every rank.
+ *   pb_last_* per-call stats: rank 0's, for the calling thread's last call.
+ * PB_ERR_UNSUPPORTED, the handle unchanged and usable: pb_index_comm_init, pb_index_group_join, pb_index_delete_sharded,
+ * pb_index_append_sharded, pb_index_append_encoded_sharded (call the plain names), pb_index_reserve (a group member's
+ * capacity is reserved before it joins), pb_index_export_ivf, pb_last_delete_ms, pb_search_batch_device (its pointers
+ * belong to one device), and a search with a non-NULL trace.
+ * A failed collective returns the status of the lowest rank whose status is not PB_ERR_COMM (PB_ERR_COMM if every rank
+ * reports it), with that rank's pb_last_error() text; when that text only says another rank failed (a sharded call
+ * gives every rank the failing rank's status), the failing rank's own text.  A CUDA error inside an exchange breaks
+ * the group: every later collective that reaches an exchange fails with PB_ERR_COMM (a rank whose own CUDA calls fail
+ * first reports PB_ERR_CUDA, and a call that reaches no exchange may still succeed).  The deployment must then be
+ * closed and loaded again. */
+PB_API pb_status pb_index_load_devices(const char *index_dir, const int32_t *devices, int32_t n_devices, int32_t flags,
+                                       pb_index **out);
+/* The ranks behind a handle: *out_world, and (each may be NULL) out_bounds [world+1] global doc ranges and
+ * out_devices [world].  A handle that is not a deployment reports world 1, [doc_id_base, doc_id_base + D], its device. */
+PB_API pb_status pb_index_shard_layout(const pb_index *ix, int32_t *out_world, int64_t *out_bounds, int32_t *out_devices);
 
 /* ---- misc ----------------------------------------------------------------------------- */
 

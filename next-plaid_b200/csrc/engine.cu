@@ -639,6 +639,8 @@ struct pb_index : DocArrays {
         { std::lock_guard<std::mutex> g(gate); }
         return std::shared_lock<std::shared_mutex>(rw);
     }
+    // pb_index_load_devices: this handle holds no documents and stands for the ranks of `dep` (deployment.cpp)
+    Deployment *dep = nullptr;
     // doc-sharded deployment (pb_index_comm_init / pb_index_group_join).  Declared last, so destroyed first: an NCCL
     // communicator goes before the workspace streams it ran on
     ShardComm comm;
@@ -1193,6 +1195,35 @@ static pb_status unique_codes(pb_index *ix, long long d0, long long n, long long
     return PB_OK;
 }
 
+// The coalescing a handle starts with: PB_COALESCE (max_queries), PB_COALESCE_WAIT_US, PB_COALESCE_INFLIGHT
+static pb_status coalesce_env_defaults(pb_index *ix) {
+    if (const char *e = getenv("PB_COALESCE")) {
+        pb_coalesce_config c = {atoi(e), 0, 2};
+        if (const char *w = getenv("PB_COALESCE_WAIT_US")) c.max_wait_us = std::max(0, atoi(w));
+        if (const char *f = getenv("PB_COALESCE_INFLIGHT")) c.max_inflight = std::max(1, atoi(f));
+        c.max_queries = std::max(1, c.max_queries);
+        CKS(pb_index_set_coalescing(ix, &c));
+    }
+    return PB_OK;
+}
+
+// A deployment's handle (deployment.cpp): no documents of its own; what every rank shares, from rank 0
+pb_index *pb_index_new_deployment(Deployment *d, const pb_index *rank0) {
+    pb_index *ix = new pb_index();
+    ix->dep = d;
+    ix->device = rank0->device, ix->dim = rank0->dim, ix->nbits = rank0->nbits, ix->packed = rank0->packed;
+    ix->K = rank0->K;
+    coalesce_env_defaults(ix);  // cannot fail: the handle joins no group
+    return ix;
+}
+
+// The calls a deployment refuses: each addresses one rank's handle, or one device
+static pb_status refuse_deployment(const pb_index *ix, const char *call) {
+    if (ix && ix->dep)
+        return pb_fail(PB_ERR_UNSUPPORTED, "%s on a multi-device handle (pb_index_load_devices) is not supported", call);
+    return PB_OK;
+}
+
 // Derived arrays that need every token: the per-doc distinct-code lists, the token norms, and the inverted file of an
 // index opened without one.
 pb_status pb_index_finalize(pb_index *ix) {
@@ -1224,13 +1255,7 @@ pb_status pb_index_finalize(pb_index *ix) {
         if (const char *e = getenv("PB_A5_LIVE")) ix->a5_live = std::max(0ll, atoll(e));
         if (const char *e = getenv("PB_A5_M1")) ix->a5_m1 = std::max(1.0f, (float)atof(e));
         if (const char *e = getenv("PB_A5_WAVES")) ix->a5_waves = std::max(1, atoi(e));
-        if (const char *e = getenv("PB_COALESCE")) {
-            pb_coalesce_config c = {atoi(e), 0, 2};
-            if (const char *w = getenv("PB_COALESCE_WAIT_US")) c.max_wait_us = std::max(0, atoi(w));
-            if (const char *f = getenv("PB_COALESCE_INFLIGHT")) c.max_inflight = std::max(1, atoi(f));
-            c.max_queries = std::max(1, c.max_queries);
-            CKS(pb_index_set_coalescing(ix, &c));
-        }
+        CKS(coalesce_env_defaults(ix));
     }
     if (TcDims::has(ix->dim) && ix->N > 0) {
         // operands of the tensor-core score table, and the token norms of the filter
@@ -1249,6 +1274,7 @@ pb_status pb_index_finalize(pb_index *ix) {
 
 extern "C" pb_status pb_index_export_ivf(pb_index *ix, int64_t *out_ivf, int32_t *out_lengths, int64_t *out_total) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    CKS(refuse_deployment(ix, "pb_index_export_ivf"));
     auto rd = ix->read_lock();
     CK(cudaSetDevice(ix->device));
     if (out_total) *out_total = ix->ivf_len;
@@ -1282,6 +1308,7 @@ extern "C" pb_status pb_index_open(const pb_index_desc *d, pb_index **out) {
 
 extern "C" void pb_index_close(pb_index *ix) {
     if (!ix) return;
+    if (ix->dep) pb_dep_close(ix->dep);  // joins its threads, closes its ranks, destroys its group
     cudaSetDevice(ix->device);
     ix->lane_workers.clear();  // joins the helper threads
     cudaDeviceSynchronize();
@@ -1291,17 +1318,23 @@ extern "C" void pb_index_close(pb_index *ix) {
 // D and N change under pb_index_append; K, dim, nbits and the device are fixed at open
 extern "C" int64_t pb_index_num_documents(const pb_index *ix) {
     if (!ix) return 0;
+    long long D, N;
+    if (ix->dep) return pb_dep_totals(ix->dep, &D, &N) == PB_OK ? D : 0;
     auto rd = ix->read_lock();
     return ix->D;
 }
 extern "C" int64_t pb_index_num_embeddings(const pb_index *ix) {
     if (!ix) return 0;
+    long long D, N;
+    if (ix->dep) return pb_dep_totals(ix->dep, &D, &N) == PB_OK ? N : 0;
     auto rd = ix->read_lock();
     return ix->N;
 }
 extern "C" int64_t pb_index_num_partitions(const pb_index *ix) { return ix ? ix->K : 0; }
 extern "C" double pb_index_avg_doclen(const pb_index *ix) {
     if (!ix) return 0.0;
+    long long D, N;
+    if (ix->dep) return pb_dep_totals(ix->dep, &D, &N) == PB_OK && D ? (double)N / (double)D : 0.0;
     auto rd = ix->read_lock();
     return ix->D ? (double)ix->N / (double)ix->D : 0.0;
 }
@@ -1311,12 +1344,23 @@ extern "C" int32_t pb_index_device(const pb_index *ix) { return ix ? ix->device 
 
 extern "C" pb_status pb_index_memory(const pb_index *ix, int64_t *device_bytes, int64_t *host_bytes) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    if (ix->dep) return pb_dep_memory(ix->dep, device_bytes, host_bytes);
     auto rd = ix->read_lock();
     size_t dev = ix->centroids.cap + ix->w_rev.cap + ix->cent_h16t.cap + ix->cent_l16t.cap;
     for (const DevBuf *b : DocArrays::buffers(*ix))
         if (b->owned) dev += b->cap;  // adopted residuals are the caller's allocation
     if (device_bytes) *device_bytes = (int64_t)dev;
     if (host_bytes) *host_bytes = (int64_t)ix->host_res.bytes;
+    return PB_OK;
+}
+
+extern "C" pb_status pb_index_shard_layout(const pb_index *ix, int32_t *out_world, int64_t *out_bounds, int32_t *out_devices) {
+    if (!ix || !out_world) return pb_fail(PB_ERR_INVALID, "null argument");
+    if (ix->dep) return pb_dep_layout(ix->dep, out_world, out_bounds, out_devices);
+    auto rd = ix->read_lock();
+    *out_world = 1;
+    if (out_bounds) out_bounds[0] = ix->doc_id_base, out_bounds[1] = ix->doc_id_base + ix->D;
+    if (out_devices) out_devices[0] = ix->device;
     return PB_OK;
 }
 
@@ -1333,12 +1377,15 @@ extern "C" void pb_search_params_default(pb_search_params *p) {  // search.rs:58
 
 extern "C" void pb_set_fast_approx(pb_index *ix, int32_t enabled) {
     if (!ix) return;
+    if (ix->dep) return pb_dep_each(ix->dep, [&](pb_index *m) { pb_set_fast_approx(m, enabled); });
     ix->fast_approx = enabled != 0;  // 0 = single exact pass over every candidate, otherwise two-pass
 }
 extern "C" void pb_set_scores_tc(pb_index *ix, int32_t enabled) {
+    if (ix && ix->dep) return pb_dep_each(ix->dep, [&](pb_index *m) { pb_set_scores_tc(m, enabled); });
     if (ix) ix->k1_tc = enabled != 0;  // effective when the tensor-core operands were built at open (k1_tc_usable)
 }
 extern "C" void pb_set_lanes(pb_index *ix, int32_t lanes) {
+    if (ix && ix->dep) return pb_dep_each(ix->dep, [&](pb_index *m) { pb_set_lanes(m, lanes); });
     if (ix) ix->lanes = std::min(8, std::max(1, (int)lanes));
 }
 extern "C" pb_status pb_index_set_coalescing(pb_index *ix, const pb_coalesce_config *cfg) {
@@ -1367,9 +1414,11 @@ extern "C" pb_status pb_index_coalesce_stats(pb_index *ix, pb_coalesce_stats *ou
     return PB_OK;
 }
 extern "C" void pb_set_fast_exact(pb_index *ix, int32_t enabled) {
+    if (ix && ix->dep) return pb_dep_each(ix->dep, [&](pb_index *m) { pb_set_fast_exact(m, enabled); });
     if (ix) ix->fast_exact = enabled != 0;
 }
 extern "C" void pb_set_profiling(pb_index *ix, int32_t enabled) {
+    if (ix && ix->dep) return pb_dep_each(ix->dep, [&](pb_index *m) { pb_set_profiling(m, enabled); });
     if (ix) ix->profiling = enabled != 0;
 }
 extern "C" pb_status pb_last_stage_stats(pb_index *, float *out_ms, int32_t *out_launches) {
@@ -3186,6 +3235,13 @@ extern "C" pb_status pb_search_batch_traced(pb_index *ix, const float *queries, 
                                             int64_t n_queries, const pb_search_params *params, const int64_t *subset,
                                             int64_t n_subset, int64_t *out_ids, float *out_scores, int32_t *out_counts,
                                             pb_trace *trace) {
+    if (trace) CKS(refuse_deployment(ix, "pb_search_batch_traced with a trace"));
+    if (ix && ix->dep)
+        return pb_dep_search(ix->dep, n_queries, params ? params->top_k : 0, out_ids, out_scores, out_counts,
+                             [&](pb_index *m, int64_t *ids, float *sc, int32_t *cn) {
+                                 return pb_search_batch_traced(m, queries, q_tok_offsets, n_queries, params, subset,
+                                                               n_subset, ids, sc, cn, nullptr);
+                             });
     if (subset && n_subset < 0) return pb_fail(PB_ERR_INVALID, "n_subset < 0");
     SearchIO io{queries, false, q_tok_offsets, n_queries, subset, nullptr, nullptr, subset ? n_subset : 0,
                 subset != nullptr, out_ids, out_scores, out_counts, false, trace,
@@ -3211,6 +3267,14 @@ static pb_status search_subsets(pb_index *ix, const float *queries, const int64_
     if (params)
         for (int64_t b = 0; b < (params_stride ? n_queries : 1); ++b)
             out_stride = std::max<int64_t>(out_stride, params[b * params_stride].top_k);
+    if (ix && ix->dep) {
+        if (trace) CKS(refuse_deployment(ix, "a search with a trace"));
+        return pb_dep_search(ix->dep, n_queries, out_stride, out_ids, out_scores, out_counts,
+                             [&](pb_index *m, int64_t *ids, float *sc, int32_t *cn) {
+                                 return search_subsets(m, queries, q_tok_offsets, n_queries, params, params_stride,
+                                                       subset_offsets, subset_ids, has_subset, ids, sc, cn, nullptr);
+                             });
+    }
     SearchIO io{queries, false, q_tok_offsets, n_queries, subset_ids, subset_offsets, has_subset, 0, false,
                 out_ids, out_scores, out_counts, false, trace, params, params_stride, out_stride};
     return search_impl(ix, io);
@@ -3256,11 +3320,11 @@ static pb_status search_alone(pb_index *ix, const SearchRequest &r) {
                                   r.out_ids, r.out_scores, r.out_count, nullptr);
 }
 
-// What pb_search_batch_params of the request alone would refuse, as far as the host can tell (the caller holds the
-// read lock: K decides the variant).  Not covered: a dense-variant query with a subset, whose effective n_ivf_probe
-// follows from its eligible centroids, counted on the device; such a request can still fail its merged call, which
-// then re-runs its members alone.
-static pb_status check_request(const pb_index *ix, const SearchRequest &r) {
+// What pb_search_batch_params of the request alone would refuse, as far as the host can tell, on a handle of D
+// documents with ix's K (the caller holds ix's read lock: K decides the variant).  Not covered: a dense-variant query
+// with a subset, whose effective n_ivf_probe follows from its eligible centroids, counted on the device; such a request
+// can still fail its merged call, which then re-runs its members alone.
+static pb_status check_request(const pb_index *ix, long long D, const SearchRequest &r) {
     if (!r.params) return pb_fail(PB_ERR_INVALID, "null params");
     if (r.subset && r.n_subset < 0) return pb_fail(PB_ERR_INVALID, "subset_offsets not monotone");
     if (!r.query) return pb_fail(PB_ERR_INVALID, "null queries");
@@ -3271,7 +3335,7 @@ static pb_status check_request(const pb_index *ix, const SearchRequest &r) {
     if (r.n_tokens < 0) return pb_fail(PB_ERR_INVALID, "q_tok_offsets not monotone");
     int M = 0;
     CKS(query_kept_docs(p, &M));
-    if (M == 0 || p.top_k == 0 || ix->D == 0) return PB_OK;  // an empty result, no pass
+    if (M == 0 || p.top_k == 0 || D == 0) return PB_OK;  // an empty result, no pass
     const bool batched = query_batched(ix, p);
     if (batched) CKS(check_batched_probe(ix, p));
     const int n = (int)std::min<long long>(p.n_ivf_probe, ix->K);
@@ -3343,9 +3407,14 @@ extern "C" pb_status pb_search(pb_index *ix, const float *query, int64_t n_query
         return search_alone(ix, r);
     }
     pb_status st;
-    {
+    if (ix->dep) {  // as one handle of the whole index: every rank's K, the deployment's D (rank 0 may be empty)
+        const long long D = pb_index_num_documents(ix);
+        const pb_index *m = pb_dep_rank(ix->dep, 0);
+        auto rd = m->read_lock();
+        st = check_request(m, D, r);
+    } else {
         auto rd = ix->read_lock();
-        st = check_request(ix, r);
+        st = check_request(ix, ix->D, r);
     }
     if (st != PB_OK) {
         ix->coalescer.count_refused();
@@ -3367,6 +3436,7 @@ extern "C" pb_status pb_search_batch(pb_index *ix, const float *queries, const i
 extern "C" pb_status pb_search_batch_device(pb_index *ix, const float *d_queries, const int64_t *q_tok_offsets_host,
                                             int64_t n_queries, const pb_search_params *params, int64_t *d_out_ids,
                                             float *d_out_scores, int32_t *d_out_counts) {
+    CKS(refuse_deployment(ix, "pb_search_batch_device"));
     SearchIO io{d_queries, true, q_tok_offsets_host, n_queries, nullptr, nullptr, nullptr, 0, false,
                 d_out_ids, d_out_scores, d_out_counts, true, nullptr, params, 0, params ? params->top_k : 0};
     return search_impl(ix, io);
@@ -3376,6 +3446,7 @@ extern "C" pb_status pb_search_batch_device(pb_index *ix, const float *d_queries
 // stage entry points
 // ------------------------------------------------------------------------------------------
 extern "C" pb_status pb_centroid_scores(pb_index *ix, const float *query_tokens, int64_t n, float *out) {
+    if (ix && ix->dep) return pb_centroid_scores(pb_dep_rank(ix->dep, 0), query_tokens, n, out);  // centroids replicated
     if (!ix || (!query_tokens && n) || (!out && n)) return pb_fail(PB_ERR_INVALID, "null argument");
     if (n == 0) return PB_OK;
     auto rd = ix->read_lock();
@@ -3408,6 +3479,7 @@ extern "C" pb_status pb_centroid_scores(pb_index *ix, const float *query_tokens,
 
 extern "C" pb_status pb_decompress_documents(pb_index *ix, const int64_t *doc_ids, int64_t n_docs, float *out_embeddings,
                                              int64_t *out_lengths) {
+    if (ix && ix->dep) return pb_dep_decompress(ix->dep, doc_ids, n_docs, out_embeddings, out_lengths);
     if (!ix || (!doc_ids && n_docs) || !out_lengths) return pb_fail(PB_ERR_INVALID, "null argument");
     auto rd = ix->read_lock();
     CK(cudaSetDevice(ix->device));
@@ -3519,6 +3591,7 @@ extern "C" pb_status pb_maxsim_scores(int32_t device, const float *query, int32_
 
 extern "C" pb_status pb_exhaustive_scores(pb_index *ix, const float *queries, const int64_t *q_off, int64_t n_queries,
                                           float *out_scores) {
+    if (ix && ix->dep) return pb_dep_exhaustive(ix->dep, queries, q_off, n_queries, out_scores);
     if (!ix || (!queries && n_queries) || !q_off || (!out_scores && n_queries)) return pb_fail(PB_ERR_INVALID, "null argument");
     auto rd = ix->read_lock();
     CK(cudaSetDevice(ix->device));
@@ -3602,6 +3675,7 @@ extern "C" pb_status pb_comm_unique_id(uint8_t *out128) {
 
 extern "C" pb_status pb_index_comm_init(pb_index *ix, const uint8_t *id128, int32_t rank, int32_t world) {
     if (!ix || !id128) return pb_fail(PB_ERR_INVALID, "null argument");
+    CKS(refuse_deployment(ix, "pb_index_comm_init"));
     CKS(ix->comm.init_nccl(id128, rank, world, ix->device));
     // a sharded search is a collective: arrival order is not a rank-agreed order
     if (ix->comm.joined()) pb_index_set_coalescing(ix, nullptr);
@@ -3621,6 +3695,7 @@ extern "C" pb_status pb_shard_group_create(int32_t world, pb_shard_group **out) 
 extern "C" void pb_shard_group_destroy(pb_shard_group *g) { delete g; }
 extern "C" pb_status pb_index_group_join(pb_index *ix, pb_shard_group *g, int32_t rank) {
     if (!ix || !g) return pb_fail(PB_ERR_INVALID, "null argument");
+    CKS(refuse_deployment(ix, "pb_index_group_join"));
     CKS(ix->comm.join(g, rank, ix->device));
     pb_index_set_coalescing(ix, nullptr);  // as pb_index_comm_init
     return PB_OK;
@@ -4378,6 +4453,9 @@ extern "C" pb_status pb_index_append(pb_index *ix, pb_codec *codec, const float 
                                      int64_t n_docs, int32_t memory_space, const char *index_dir, int64_t batch_size,
                                      int64_t *out_first_doc_id) {
     if (!codec) return pb_fail(PB_ERR_INVALID, "null argument");
+    if (ix && ix->dep)
+        return pb_dep_append(ix->dep, codec, embeddings, nullptr, nullptr, doc_lengths, n_docs, memory_space, index_dir,
+                             batch_size, out_first_doc_id);
     return append_impl(ix, codec, embeddings, nullptr, nullptr, doc_lengths, n_docs, memory_space, index_dir, batch_size,
                        out_first_doc_id);
 }
@@ -4385,11 +4463,15 @@ extern "C" pb_status pb_index_append(pb_index *ix, pb_codec *codec, const float 
 extern "C" pb_status pb_index_append_encoded(pb_index *ix, const int64_t *codes, const uint8_t *residuals,
                                              const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
                                              int64_t *out_first_doc_id) {
+    if (ix && ix->dep)
+        return pb_dep_append(ix->dep, nullptr, nullptr, codes, residuals, doc_lengths, n_docs, memory_space, nullptr, 0,
+                             out_first_doc_id);
     return append_impl(ix, nullptr, nullptr, codes, residuals, doc_lengths, n_docs, memory_space, nullptr, 0, out_first_doc_id);
 }
 
 extern "C" pb_status pb_index_reserve(pb_index *ix, int64_t num_documents, int64_t num_embeddings) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    CKS(refuse_deployment(ix, "pb_index_reserve (reserve a rank's capacity before it joins a group)"));
     std::lock_guard<std::mutex> gate(ix->gate);
     std::unique_lock<std::shared_mutex> wr(ix->rw);
     if (ix->comm.joined()) return pb_fail(PB_ERR_UNSUPPORTED, "appends to a doc-sharded handle are not supported");
@@ -4602,6 +4684,7 @@ extern "C" pb_status pb_index_delete(pb_index *ix, const int64_t *doc_ids, int64
                                      int64_t *out_deleted) {
     if (!ix || (!doc_ids && n_ids) || n_ids < 0) return pb_fail(PB_ERR_INVALID, "null argument");
     if (out_deleted) *out_deleted = 0;
+    if (ix->dep) return pb_dep_delete(ix->dep, doc_ids, n_ids, index_dir, out_deleted);
     std::lock_guard<std::mutex> gate(ix->gate);
     std::unique_lock<std::shared_mutex> wr(ix->rw);
     if (ix->comm.joined()) return pb_fail(PB_ERR_UNSUPPORTED, "deletes from a doc-sharded handle are not supported");
@@ -4813,6 +4896,7 @@ static pb_status sharded_update(pb_index *ix, int op, pb_codec *codec, const flo
 extern "C" pb_status pb_index_delete_sharded(pb_index *ix, const int64_t *doc_ids, int64_t n_ids, const char *index_dir,
                                              int64_t *out_deleted) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    CKS(refuse_deployment(ix, "pb_index_delete_sharded (call pb_index_delete)"));
     return sharded_update(ix, SH_OP_DELETE, nullptr, nullptr, nullptr, nullptr, nullptr, doc_ids, n_ids, PB_MEM_HOST,
                           index_dir, 0, out_deleted);
 }
@@ -4821,6 +4905,7 @@ extern "C" pb_status pb_index_append_sharded(pb_index *ix, pb_codec *codec, cons
                                              const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
                                              const char *index_dir, int64_t batch_size, int64_t *out_first_doc_id) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    CKS(refuse_deployment(ix, "pb_index_append_sharded (call pb_index_append)"));
     return sharded_update(ix, SH_OP_APPEND, codec, embeddings, nullptr, nullptr, doc_lengths, nullptr, n_docs, memory_space,
                           index_dir, batch_size, out_first_doc_id);
 }
@@ -4829,6 +4914,7 @@ extern "C" pb_status pb_index_append_encoded_sharded(pb_index *ix, const int64_t
                                                      const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
                                                      int64_t *out_first_doc_id) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    CKS(refuse_deployment(ix, "pb_index_append_encoded_sharded (call pb_index_append_encoded)"));
     return sharded_update(ix, SH_OP_APPEND_ENCODED, nullptr, nullptr, codes, residuals, doc_lengths, nullptr, n_docs,
                           memory_space, nullptr, 0, out_first_doc_id);
 }
@@ -4859,6 +4945,7 @@ struct RebalancePrep {
 
 extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bounds, int64_t *out_bounds) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    if (ix->dep) return pb_dep_rebalance(ix->dep, bounds, out_bounds);
     std::lock_guard<std::mutex> gate(ix->gate);
     std::unique_lock<std::shared_mutex> wr(ix->rw);
     const int W = ix->comm.world, me = ix->comm.rank;
@@ -5141,6 +5228,7 @@ extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bou
 
 extern "C" pb_status pb_last_delete_ms(pb_index *ix, float *out_ms) {
     if (!ix || !out_ms) return pb_fail(PB_ERR_INVALID, "null argument");
+    CKS(refuse_deployment(ix, "pb_last_delete_ms"));
     auto rd = ix->read_lock();
     memcpy(out_ms, ix->delete_ms, sizeof ix->delete_ms);
     return PB_OK;

@@ -1,11 +1,44 @@
-// engine_internal.h -- C++-side entry points shared between engine.cu, loader.cpp and builder.cpp (not exported).
+// engine_internal.h -- C++-side entry points shared between engine.cu, loader.cpp, builder.cpp and deployment.cpp (not
+// exported).
 #pragma once
 #include "../../include/plaid_b200.h"
 
+#include <functional>
 #include <string>
 #include <vector>
 
 pb_status pb_fail(pb_status s, const char *fmt, ...);
+
+// A deployment (pb_index_load_devices, deployment.cpp, DESIGN §4o): the ranks of a doc-sharded index in one process,
+// driven through the public entry points by the library's own threads.  Its handle is a pb_index that holds no
+// documents; the entry points of engine.cu hand such a handle to the functions below.
+struct Deployment;
+// the handle: K, dim, nbits and device copied from rank 0; the PB_COALESCE* defaults applied
+pb_index *pb_index_new_deployment(Deployment *d, const pb_index *rank0);
+// rank r's handle
+pb_index *pb_dep_rank(Deployment *d, int r);
+// Stops and joins the threads, closes the ranks, destroys the group and d
+void pb_dep_close(Deployment *d);
+// call(m) on every rank's handle, on the caller's thread (the pb_set_* switches)
+void pb_dep_each(Deployment *d, const std::function<void(pb_index *)> &call);
+// A search collective: call(m, ids, scores, counts) on every rank at once, rank 0 with the caller's outputs and the
+// others with scratch outputs of n_queries rows of `stride` (null where the caller's is null)
+pb_status pb_dep_search(Deployment *d, int64_t n_queries, int64_t stride, int64_t *out_ids, float *out_scores,
+                        int32_t *out_counts,
+                        const std::function<pb_status(pb_index *, int64_t *, float *, int32_t *)> &call);
+pb_status pb_dep_totals(Deployment *d, long long *D, long long *N);
+pb_status pb_dep_memory(Deployment *d, int64_t *device_bytes, int64_t *host_bytes);
+pb_status pb_dep_layout(Deployment *d, int32_t *out_world, int64_t *out_bounds, int32_t *out_devices);
+pb_status pb_dep_decompress(Deployment *d, const int64_t *doc_ids, int64_t n_docs, float *out_embeddings,
+                            int64_t *out_lengths);
+pb_status pb_dep_exhaustive(Deployment *d, const float *queries, const int64_t *q_off, int64_t n_queries,
+                            float *out_scores);
+pb_status pb_dep_delete(Deployment *d, const int64_t *doc_ids, int64_t n_ids, const char *index_dir, int64_t *out_deleted);
+// pb_index_append (codec != null) or pb_index_append_encoded
+pb_status pb_dep_append(Deployment *d, pb_codec *codec, const float *embeddings, const int64_t *codes,
+                        const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
+                        const char *index_dir, int64_t batch_size, int64_t *out_first_doc_id);
+pb_status pb_dep_rebalance(Deployment *d, const int64_t *bounds, int64_t *out_bounds);
 // pb_index_open without the per-token arrays; follow with pb_index_upload_tokens per chunk.
 pb_status pb_index_open_begin(const pb_index_desc *d, pb_index **out);
 pb_status pb_index_upload_tokens(pb_index *ix, long long tok_off, const int64_t *codes, const uint8_t *residuals,

@@ -100,6 +100,7 @@ EXPORTS = [
     "pb_index_delete_sharded", "pb_index_append_sharded", "pb_index_append_encoded_sharded",
     "pb_index_rebalance_sharded", "pb_index_load_range_flags", "pb_index_memory", "pb_last_staging_stats",
     "pb_search", "pb_index_set_coalescing", "pb_index_coalesce_stats", "pb_create_index_sharded", "pb_last_create_ms",
+    "pb_index_load_devices", "pb_index_shard_layout",
 ]
 
 PB_OPEN_ADOPT_RESIDUALS, PB_OPEN_HOST_RESIDUALS = 1, 2
@@ -214,6 +215,8 @@ def load_library():
         L.pb_index_append_sharded.argtypes = L.pb_index_append.argtypes
         L.pb_index_append_encoded_sharded.argtypes = L.pb_index_append_encoded.argtypes
         L.pb_index_rebalance_sharded.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        L.pb_index_load_devices.argtypes = [C.c_char_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
+        L.pb_index_shard_layout.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 
@@ -465,6 +468,28 @@ class MmapIndex:
         else:
             _check(L.pb_index_load_range(os.fsencode(index_path), device, doc_begin, doc_end, C.byref(h)))
         return cls(h.value, index_path)
+
+    @classmethod
+    def load_devices(cls, index_path: str, devices: Sequence[int], host_residuals: bool = False) -> "MmapIndex":
+        """pb_index_load_devices: the directory doc-sharded over `devices` of this process (rank r holds the r-th range
+        of shard_bounds(index_path, len(devices)) on devices[r]; devices may repeat) behind one handle.  Every method
+        then works as on a handle from load, with the same results; the ranks and their threads live in the library."""
+        dv = np.ascontiguousarray(list(devices), np.int32)
+        h = C.c_void_p()
+        _check(load_library().pb_index_load_devices(os.fsencode(index_path), _ptr(dv), len(dv),
+                                                    PB_OPEN_HOST_RESIDUALS if host_residuals else 0, C.byref(h)))
+        ix = cls(h.value, index_path)
+        ix._world = len(dv)
+        return ix
+
+    def shard_layout(self):
+        """pb_index_shard_layout: (bounds [world + 1] global document ranges, devices [world]) of the ranks behind the
+        handle; a handle that is not a deployment is one rank."""
+        w = C.c_int32()
+        _check(load_library().pb_index_shard_layout(self._h, C.byref(w), None, None))
+        b, d = np.zeros(w.value + 1, np.int64), np.zeros(w.value, np.int32)
+        _check(load_library().pb_index_shard_layout(self._h, C.byref(w), _ptr(b), _ptr(d)))
+        return b, d
 
     @classmethod
     def load_shard(cls, index_path: str, rank: int, world: int, device: int = 0,

@@ -130,6 +130,8 @@ extern "C" {
     fn pb_index_rebalance_sharded(ix: *mut c_void, bounds: *const i64, out_bounds: *mut i64) -> c_int;
     fn pb_index_load_range_flags(index_dir: *const c_char, device: i32, doc_begin: i64, doc_end: i64, flags: i32,
                                  out: *mut *mut c_void) -> c_int;
+    fn pb_index_load_devices(index_dir: *const c_char, devices: *const i32, n_devices: i32, flags: i32,
+                             out: *mut *mut c_void) -> c_int;
     fn pb_index_memory(ix: *const c_void, device_bytes: *mut i64, host_bytes: *mut i64) -> c_int;
     fn pb_last_staging_stats(ix: *mut c_void, docs: *mut i64, bytes: *mut i64, ms: *mut f32) -> c_int;
     // pb_create_index_sharded (DESIGN §4n): `comm` is a pb_build_comm, `params` a pb_create_params
@@ -176,6 +178,20 @@ impl B200Index {
         let c = CString::new(index_path).map_err(|e| Error::IndexLoad(e.to_string()))?;
         let mut handle: *mut c_void = std::ptr::null_mut();
         if unsafe { pb_index_load_range_flags(c.as_ptr(), device, 0, -1, PB_OPEN_HOST_RESIDUALS, &mut handle) } != 0 {
+            return Err(Error::IndexLoad(last_error()));
+        }
+        Ok(B200Index { handle })
+    }
+
+    /// `load` doc-sharded over several GPUs of this process (`pb_index_load_devices`, DESIGN §4o): rank r holds the
+    /// r-th token-balanced document range on `devices[r]`, and the library keeps one thread per extra rank.  The
+    /// handle is then used exactly as one from `load`: `search`, `search_batch`, `set_coalescing`, `update_append`
+    /// and `delete_with_options` reach every rank in one order, results equal those of `load`.
+    pub fn load_devices(index_path: &str, devices: &[i32]) -> Result<Self> {
+        let c = CString::new(index_path).map_err(|e| Error::IndexLoad(e.to_string()))?;
+        let mut handle: *mut c_void = std::ptr::null_mut();
+        let st = unsafe { pb_index_load_devices(c.as_ptr(), devices.as_ptr(), devices.len() as i32, 0, &mut handle) };
+        if st != 0 {
             return Err(Error::IndexLoad(last_error()));
         }
         Ok(B200Index { handle })
