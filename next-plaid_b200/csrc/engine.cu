@@ -1487,7 +1487,7 @@ static pb_status launch_k1_table(pb_index *ix, Workspace &ws, int B, int QS, uns
         auto kern = k_scores16_tc<decltype(dim_c)::value>;
         CKS(set_smem(kern, sm));
         KEV_BEGIN(PB_KERNEL_SCORES);
-        kern<<<tiles, 288, sm, ws.stream>>>(ix->cent_h16t.as<__half>(), ix->cent_l16t.as<__half>(), ix->K,
+        kern<<<tiles, 384, sm, ws.stream>>>(ix->cent_h16t.as<__half>(), ix->cent_l16t.as<__half>(), ix->K,
                                             ws.Qh16t.as<__half>(), ws.Ql16t.as<__half>(), n_groups, B, QS,
                                             ws.qoff.as<int>(), ws.qrange_tc.as<float2>(), table, flags, slab_max);
         KEV_END(PB_KERNEL_SCORES);

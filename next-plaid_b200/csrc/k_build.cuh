@@ -238,13 +238,15 @@ PB_DEV u64 wg_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
 }
 PB_DEV void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 PB_DEV void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-// waits for every committed group, then pins the accumulator registers behind the wait (the compiler must not read
-// them earlier)
-template <int R> PB_DEV void wg_wait_all(float (&d)[R]) {
-    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+// waits until at most N committed groups are pending, then pins the accumulator registers of a retired group behind
+// the wait (the compiler must not read them earlier).  With N > 0 the newest groups keep running: their accumulators
+// must not be passed here.
+template <int N, int R> PB_DEV void wg_wait(float (&d)[R]) {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 #pragma unroll
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+template <int R> PB_DEV void wg_wait_all(float (&d)[R]) { wg_wait<0>(d); }
 // d (+)= A B^T, A = 64 rows x 16 (descriptor da), B = N rows x 16 (descriptor db); accumulate = 0 overwrites d
 template <int N> PB_DEV void wg_mma_f16(float (&d)[N / 2], u64 da, u64 db, uint32_t accumulate);
 template <> PB_DEV void wg_mma_f16<32>(float (&d)[16], u64 da, u64 db, uint32_t accumulate) {

@@ -23,8 +23,9 @@
 // E = 1.  Consumers use: code margin 2E + 1 = 3 for "could still be the maximum / in the top n", and the band
 // W = nq (1.004 + 2 err) + nq^2 / 256 + 4 for the first approximate pass (derivations at each kernel).
 // PB_K1_TC_DIAG=1 measures the largest code difference against the exact table (pb_work_counters).
-// grid = ceil(K/128) CTAs, 288 threads: warps 0-7 two warpgroups that issue the MMAs of one 64-centroid half of the
-// tile each and convert their accumulators, warp 8 bulk-copy loader.
+// grid = ceil(K/128) CTAs, 384 threads: warps 0-7 two warpgroups that issue the MMAs of one 64-centroid half of the
+// tile each and convert their accumulators, warp 8 bulk-copy loader.  The third warpgroup exists so that setmaxnreg can
+// move its registers to the consumers (40 each for it, 232 for them), which hold two accumulators (k_scores16_tc).
 // With SMAX the epilogue also keeps the largest stored code of every 16-centroid slab (one warp's rows) and query row:
 // SMAX[s][row] (row = b QS + q, n_groups * 128 rows per slab, slabs up to 8 ceil(K/128)), from which
 // k_chunkmax_slabs forms the probe's chunk maxima without reading the table back.
@@ -85,16 +86,104 @@ __global__ void k_query_range_tc(const float2 *__restrict__ qrange, const int *_
     qrange_tc[b] = make_float2(rg.x, ldexpf(rg.y, -(qexp[b] + kc)));
 }
 
+// the 3 dim/16 products of query group g (stage st of the ring) into d, committed as one wgmma group: the
+// accumulator's instructions and their order are those of every group, so the codes do not depend on the pipelining
 template <int DIM>
-__global__ void __launch_bounds__(288, 1)
+PB_DEV void k1_issue(float (&d)[64], uint32_t ah, uint32_t al, const unsigned char *Bs, int st) {
+    constexpr uint32_t T_BYTES = 128 * DIM * 2, LBO = 16 * 128, SBO = 128;
+    const uint32_t bh = smem_u32(Bs + (size_t)(2 * st) * T_BYTES), bl = smem_u32(Bs + (size_t)(2 * st + 1) * T_BYTES);
+    wg_fence();
+#pragma unroll
+    for (int s = 0; s < DIM / 16; ++s) {
+        const u64 dah = wg_desc(ah + s * 2 * LBO, LBO, SBO), dal = wg_desc(al + s * 2 * LBO, LBO, SBO);
+        const u64 dbh = wg_desc(bh + s * 2 * LBO, LBO, SBO), dbl = wg_desc(bl + s * 2 * LBO, LBO, SBO);
+        wg_mma_f16<128>(d, dah, dbh, s > 0 ? 1u : 0u);
+        wg_mma_f16<128>(d, dah, dbl, 1u);
+        wg_mma_f16<128>(d, dal, dbh, 1u);
+    }
+    wg_commit();
+}
+
+// the epilogue of query group g from its accumulator: codes into ST16, out-of-range flags into qflag and, with SMAX,
+// the warp's slab maxima.  d[4 i + 2 r + j] = (centroid row c_r0 + 8 r, query row g 128 + 8 i + cq + j).  The 8 query
+// rows of one i belong to one query (QS % 8 == 0), so (b, q) and the row pointer step by 8 rows from one division per
+// group.
+PB_DEV void k1_store_group(const float (&d)[64], int g, int n_groups, int w, int lane, long long c_r0, long long K,
+                           int B, int QS, const float2 *__restrict__ qrange_tc, unsigned short *__restrict__ ST16,
+                           int *__restrict__ qflag, unsigned short *__restrict__ SMAX) {
+    const int cq = 2 * (lane & 3);
+    const bool in0 = c_r0 < K, in1 = c_r0 + 8 < K;
+    const size_t wrap = (size_t)(K - 1) * QS;  // pointer step from (b, QS - 8) to (b + 1, 0), less the 8 rows
+    int b = (g * 128) / QS, q = g * 128 - b * QS;
+    unsigned short *p = ST16 + ((size_t)b * K + c_r0) * QS + q + cq;
+    float2 rg = b < B ? qrange_tc[b] : make_float2(0.0f, 0.0f);  // (R*scale, scale / 2^(kq+kc))
+    // the warp's 16 centroid rows are the 8 lanes of equal lane % 4 times r.  mi = the packed maximum of this thread's
+    // stored words of query rows 8 i + cq, + 1; the slab maxima reduce them over lanes ^16, ^8, ^4, each step keeping
+    // half of the values (the lane bit picks the half), so that lane l ends with m[k] = the slab maximum of query rows
+    // 8 (k + 2 (l / 4)) + cq, + 1 for k = 0, 1.  The ^16 step pairs i with i + 8 and runs as soon as mi is known.
+    uint32_t m[8];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+        uint32_t mi = 0u;
+        if (b < B) {
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                if (!(r ? in1 : in0)) continue;
+                // code = floor(x) clamped to [0, 65535]; x outside [+0, 65536) (NaN, -0 included) raises the
+                // query's flag and the sub-batch is redone on the exact path, so only in-range codes matter.
+                // Padding rows hold a zero accumulator: x = R*scale, in range.
+                const float x0 = __fmaf_rn(d[4 * i + 2 * r], rg.y, rg.x), x1 = __fmaf_rn(d[4 * i + 2 * r + 1], rg.y, rg.x);
+                if (!(__float_as_uint(x0) < 0x47800000u && __float_as_uint(x1) < 0x47800000u)) atomicOr(&qflag[b], 1);
+                const uint32_t word = min(__float2uint_rd(x0), 65535u) | (min(__float2uint_rd(x1), 65535u) << 16);
+                *reinterpret_cast<uint32_t *>(p + (r ? 8 * QS : 0)) = word;
+                mi = __vmaxu2(mi, word);
+            }
+        }
+        if (i < 8) {
+            m[i] = mi;
+        } else if (SMAX) {
+            const bool hi = lane & 16;
+            const uint32_t keep = hi ? mi : m[i - 8], send = hi ? m[i - 8] : mi;
+            m[i - 8] = __vmaxu2(keep, __shfl_xor_sync(PB_FULL, send, 16));
+        }
+        if (i < 15) {
+            q += 8;
+            p += 8;
+            if (q == QS) {
+                q = 0;
+                ++b;
+                p += wrap;
+                if (b < B) rg = qrange_tc[b];
+            }
+        }
+    }
+    if (SMAX) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const bool hi = lane & 8;
+            const uint32_t keep = hi ? m[i + 4] : m[i], send = hi ? m[i] : m[i + 4];
+            m[i] = __vmaxu2(keep, __shfl_xor_sync(PB_FULL, send, 8));
+        }
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const bool hi = lane & 4;
+            const uint32_t keep = hi ? m[i + 2] : m[i], send = hi ? m[i] : m[i + 2];
+            m[i] = __vmaxu2(keep, __shfl_xor_sync(PB_FULL, send, 4));
+        }
+        uint32_t *srow = reinterpret_cast<uint32_t *>(SMAX + ((size_t)blockIdx.x * 8 + w) * n_groups * 128 + g * 128 + cq);
+        srow[4 * (2 * (lane >> 2))] = m[0];
+        srow[4 * (2 * (lane >> 2) + 1)] = m[1];
+    }
+}
+
+template <int DIM>
+__global__ void __launch_bounds__(384, 1)
 k_scores16_tc(const __half *__restrict__ Ch, const __half *__restrict__ Cl, long long K, const __half *__restrict__ Qh,
               const __half *__restrict__ Ql, int n_groups, int B, int QS, const int *__restrict__ q_off,
               const float2 *__restrict__ qrange_tc, unsigned short *__restrict__ ST16, int *__restrict__ qflag,
               unsigned short *__restrict__ SMAX) {
     extern __shared__ __align__(128) unsigned char smem_k1[];
-    constexpr int KSTEPS = DIM / 16;
     constexpr uint32_t T_BYTES = 128 * DIM * 2;  // one 128-row fp16 tile
-    constexpr uint32_t LBO = 16 * 128, SBO = 128;
     unsigned char *Ah = smem_k1, *Al = Ah + T_BYTES;  // this CTA's centroid tile, hi and lo
     unsigned char *Bs = Al + T_BYTES;                 // 2 stages x (hi, lo) query-row tiles
     uint64_t *bars = reinterpret_cast<uint64_t *>(Bs + 4 * T_BYTES);
@@ -110,9 +199,10 @@ k_scores16_tc(const __half *__restrict__ Ch, const __half *__restrict__ Cl, long
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    if (w == 8) {
-        // ---------------- loader ----------------
-        if (lane == 0) {
+    if (w >= 8) {
+        // ---------------- loader: warpgroup 2 hands its registers to the consumers, warp 8 issues the copies ----------------
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+        if (w == 8 && lane == 0) {
             mbar_expect_tx(abar, 2 * T_BYTES);
             bulk_g2s(Ah, reinterpret_cast<const unsigned char *>(Ch) + (size_t)blockIdx.x * T_BYTES, T_BYTES, abar);
             bulk_g2s(Al, reinterpret_cast<const unsigned char *>(Cl) + (size_t)blockIdx.x * T_BYTES, T_BYTES, abar);
@@ -126,80 +216,48 @@ k_scores16_tc(const __half *__restrict__ Ch, const __half *__restrict__ Cl, long
         }
     } else {
         // ---------------- consumers: warpgroup h = centroid rows 64 h.. of the tile (M = 64) x all 128 query rows of a
-        // group (N = 128), 3 products per k-step into one fp32 accumulator; then the codes straight from the registers:
-        // d[4 i + 2 r + j] = (centroid row 16 (w%4) + lane/4 + 8 r, query row 8 i + 2 (lane%4) + j) ----------------
+        // group (N = 128), 3 products per k-step into an fp32 accumulator; then the codes straight from the registers.
+        // Two accumulators per thread: group g + 1's MMAs are issued into one before group g's epilogue runs from the
+        // other, so the tensor cores work through every epilogue but the last.  wait_group 1 retires group g alone,
+        // which frees its stage for the loader (group g + 2) while g + 1 still reads the other one. ----------------
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
         const int h = w >> 2;
-        const int cq = 2 * (lane & 3);
         const long long c_r0 = c0 + 64 * h + 16 * (w & 3) + (lane >> 2);
-        float d[64];
+        const uint32_t ah = smem_u32(Ah) + h * 1024, al = smem_u32(Al) + h * 1024;  // 64 rows = 8 row groups
+        float d0[64], d1[64];  // the accumulators of the even and of the odd groups
 #pragma unroll
-        for (int i = 0; i < 64; ++i) d[i] = 0.0f;
+        for (int i = 0; i < 64; ++i) d0[i] = d1[i] = 0.0f;
         mbar_wait(abar, 0);
-        for (int g = 0; g < n_groups; ++g) {
-            const int st = g & 1;
-            mbar_wait(&full[st], (uint32_t)((g >> 1) & 1));
-            const uint32_t ah = smem_u32(Ah) + h * 1024, al = smem_u32(Al) + h * 1024;  // 64 rows = 8 row groups
-            const uint32_t bh = smem_u32(Bs + (size_t)(2 * st) * T_BYTES), bl = smem_u32(Bs + (size_t)(2 * st + 1) * T_BYTES);
-            wg_fence();
-#pragma unroll
-            for (int s = 0; s < KSTEPS; ++s) {
-                const u64 dah = wg_desc(ah + s * 2 * LBO, LBO, SBO), dal = wg_desc(al + s * 2 * LBO, LBO, SBO);
-                const u64 dbh = wg_desc(bh + s * 2 * LBO, LBO, SBO), dbl = wg_desc(bl + s * 2 * LBO, LBO, SBO);
-                wg_mma_f16<128>(d, dah, dbh, s > 0 ? 1u : 0u);
-                wg_mma_f16<128>(d, dah, dbl, 1u);
-                wg_mma_f16<128>(d, dal, dbh, 1u);
+        if (n_groups > 0) {
+            // every branch below starts with group g in flight in d0 and ends with nothing pending, so the compiler
+            // sees one state at each join and keeps the MMAs asynchronous
+            mbar_wait(&full[0], 0u);
+            k1_issue<DIM>(d0, ah, al, Bs, 0);
+            int g = 0;
+            for (; g + 2 < n_groups; g += 2) {
+                mbar_wait(&full[1], (uint32_t)((g >> 1) & 1));
+                k1_issue<DIM>(d1, ah, al, Bs, 1);
+                wg_wait<1>(d0);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[0]);  // group g's query tiles consumed
+                k1_store_group(d0, g, n_groups, w, lane, c_r0, K, B, QS, qrange_tc, ST16, qflag, SMAX);
+                mbar_wait(&full[0], (uint32_t)(((g + 2) >> 1) & 1));
+                k1_issue<DIM>(d0, ah, al, Bs, 0);
+                wg_wait<1>(d1);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[1]);
+                k1_store_group(d1, g + 1, n_groups, w, lane, c_r0, K, B, QS, qrange_tc, ST16, qflag, SMAX);
             }
-            wg_commit();
-            wg_wait_all(d);
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty[st]);  // query tiles consumed
-            uint32_t m[16];  // m[i]: packed maxima of this thread's stored words of query rows 8 i + cq, + 1
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-                m[i] = 0u;
-                const int row0 = g * 128 + 8 * i;  // 8 query rows of one query (QS % 8 == 0)
-                const int b = row0 / QS, q = row0 - b * QS + cq;
-                if (b >= B) continue;
-                const float2 rg = qrange_tc[b];  // (R*scale, scale / 2^(kq+kc))
-#pragma unroll
-                for (int r = 0; r < 2; ++r) {
-                    const long long c = c_r0 + 8 * r;
-                    if (c >= K) continue;
-                    // code = floor(x) clamped to [0, 65535]; x outside [+0, 65536) (NaN, -0 included) raises the
-                    // query's flag and the sub-batch is redone on the exact path, so only in-range codes matter.
-                    // Padding rows hold a zero accumulator: x = R*scale, in range.
-                    const float x0 = __fmaf_rn(d[4 * i + 2 * r], rg.y, rg.x), x1 = __fmaf_rn(d[4 * i + 2 * r + 1], rg.y, rg.x);
-                    if (!(__float_as_uint(x0) < 0x47800000u && __float_as_uint(x1) < 0x47800000u)) atomicOr(&qflag[b], 1);
-                    const uint32_t word = min(__float2uint_rd(x0), 65535u) | (min(__float2uint_rd(x1), 65535u) << 16);
-                    *reinterpret_cast<uint32_t *>(ST16 + ((size_t)b * K + c) * QS + q) = word;
-                    m[i] = __vmaxu2(m[i], word);
-                }
-            }
-            if (SMAX) {
-                // the warp's 16 centroid rows are the 8 lanes of equal lane % 4 times r: reduce m over lanes ^16, ^8, ^4,
-                // each step keeping half of the values (the lane bit picks the half), so that lane l ends with
-                // m[k] = the slab maximum of query rows 8 (k + 2 (l / 4)) + cq, + 1 for k = 0, 1
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const bool hi = lane & 16;
-                    const uint32_t keep = hi ? m[i + 8] : m[i], send = hi ? m[i] : m[i + 8];
-                    m[i] = __vmaxu2(keep, __shfl_xor_sync(PB_FULL, send, 16));
-                }
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const bool hi = lane & 8;
-                    const uint32_t keep = hi ? m[i + 4] : m[i], send = hi ? m[i] : m[i + 4];
-                    m[i] = __vmaxu2(keep, __shfl_xor_sync(PB_FULL, send, 8));
-                }
-#pragma unroll
-                for (int i = 0; i < 2; ++i) {
-                    const bool hi = lane & 4;
-                    const uint32_t keep = hi ? m[i + 2] : m[i], send = hi ? m[i] : m[i + 2];
-                    m[i] = __vmaxu2(keep, __shfl_xor_sync(PB_FULL, send, 4));
-                }
-                uint32_t *srow = reinterpret_cast<uint32_t *>(SMAX + ((size_t)blockIdx.x * 8 + w) * n_groups * 128 + g * 128 + cq);
-                srow[4 * (2 * (lane >> 2))] = m[0];
-                srow[4 * (2 * (lane >> 2) + 1)] = m[1];
+            if (g + 1 < n_groups) {  // the last two groups
+                mbar_wait(&full[1], (uint32_t)((g >> 1) & 1));
+                k1_issue<DIM>(d1, ah, al, Bs, 1);
+                wg_wait<1>(d0);
+                k1_store_group(d0, g, n_groups, w, lane, c_r0, K, B, QS, qrange_tc, ST16, qflag, SMAX);
+                wg_wait<0>(d1);
+                k1_store_group(d1, g + 1, n_groups, w, lane, c_r0, K, B, QS, qrange_tc, ST16, qflag, SMAX);
+            } else {  // the last group
+                wg_wait<0>(d0);
+                k1_store_group(d0, g, n_groups, w, lane, c_r0, K, B, QS, qrange_tc, ST16, qflag, SMAX);
             }
         }
     }

@@ -13,6 +13,11 @@ under torch.profiler (CUDA activities), and writes DIR/profile_step.json:
   a5_bound             k_a5_bound's device time per step and its achieved rate on the bytes the algorithm needs:
                        n_candidate_tokens x 4 (the distinct-code lists, from HBM) plus n_a5_live_rows x 2 QS (the live
                        rows of the 16-bit score table, from L2), QS = query tokens rounded up to 8
+  scores_tc            k_scores16_tc's device time per step and its rates on what its shapes make it do, per
+                       tensor-core pass (n_k1_tc of them per step; R = B QS rows padded to 128-row groups, T = ceil(K/128)
+                       centroid tiles): issued fp16 FLOP 3 x 2 R (128 T) dim (three split products), table bytes
+                       written B QS K 2 plus the slab maxima 8 T R 2, and operand bytes read from L2: every CTA reads
+                       the hi and lo query tiles of every group, T R dim 4, plus its centroid tile, K dim 4
 The profiler slows the host, so its step times are not bench.py's queries/s; use bench.py for that.
 """
 from __future__ import annotations
@@ -107,6 +112,16 @@ def main():
     bound_ms = sum(v for k, v in kms.items() if k.startswith("k_a5_bound"))
     hbm = wps.get("n_candidate_tokens", 0) * 4.0
     l2 = wps.get("n_a5_live_rows", 0) * 2.0 * QS
+    K, dim, B = 1 << args.log2k, args.dim, args.batch
+    passes = wps.get("n_k1_tc", 0)
+    R, T = (B * QS + 127) // 128 * 128, (K + 127) // 128
+    sc_ms = sum(v for k, v in kms.items() if k.startswith("k_scores16_tc"))
+    flop = passes * 3 * 2 * R * 128 * T * dim
+    wr = passes * (B * QS * K * 2 + 8 * T * R * 2)
+    l2r = passes * (T * R * dim * 4 + K * dim * 4)
+
+    def rate(x):
+        return x / (sc_ms * 1e-3) if sc_ms > 0 else None
     out = {
         "gpu": bench.gpu_info(0),
         "workload": bench.workload_config(args, 1)["workload"],
@@ -117,11 +132,14 @@ def main():
         "a5_bound": {"ms": bound_ms, "code_bytes_hbm": hbm, "live_row_bytes_l2": l2,
                      "gbs": (hbm + l2) / (bound_ms * 1e-3) / 1e9 if bound_ms > 0 else None,
                      "code_gbs": hbm / (bound_ms * 1e-3) / 1e9 if bound_ms > 0 else None},
+        "scores_tc": {"ms": sc_ms, "passes": passes, "flop": flop, "table_write_bytes": wr, "operand_l2_bytes": l2r,
+                      "tflops": rate(flop / 1e12), "table_write_gbs": rate(wr / 1e9),
+                      "operand_l2_gbs": rate(l2r / 1e9)},
     }
     os.makedirs(own.out, exist_ok=True)
     with open(os.path.join(own.out, "profile_step.json"), "w") as f:
         json.dump(out, f, indent=1)
-    print(json.dumps({"gpu": out["gpu"], "a5_bound": out["a5_bound"],
+    print(json.dumps({"gpu": out["gpu"], "a5_bound": out["a5_bound"], "scores_tc": out["scores_tc"],
                       "top": dict(list(kms.items())[:8])}))
     gpu.close()
 
