@@ -438,6 +438,33 @@ PB_API pb_status pb_exhaustive_scores(pb_index *ix, const float *queries,
                                       const int64_t *q_tok_offsets, int64_t n_queries,
                                       float *out_scores);
 
+/* ---- token pooling ------------------------------------------------------------------------ */
+
+/* pool_document_embeddings (next-plaid-onnx lib.rs:1632) on the device: token 0 kept, the rest clustered by Ward's
+ * nearest-neighbour chain and averaged, bit-identical to the reference's CPU arithmetic (DESIGN.md 4p).
+ *
+ * pb_pooled_doc_length: the rows pool_embeddings_hierarchical(doc, pool_factor, 1) returns for a document of n_tokens
+ * rows: n_tokens when pool_factor <= 1, n_tokens <= 2 or k = max((n_tokens - 1) / pool_factor, 1) >= n_tokens - 1,
+ * otherwise 1 + k; -1 for a negative argument.  Size out_embeddings with it.
+ *
+ * pb_pool_embeddings: embeddings [sum doc_lengths][dim] f32 and out_embeddings [sum pooled lengths][dim] f32 in
+ * memory_space (PB_MEM_HOST | PB_MEM_DEVICE, on `device`); doc_lengths and out_doc_lengths [n_docs] on the host.  Each
+ * output row equals the reference's f32 row bit for bit, documents in input order.  Re-entrant: concurrent calls on
+ * one device each use their own stream and workspace.
+ * Refused before the device is touched: PB_ERR_INVALID for a negative n_docs, pool_factor or length, a NULL pointer
+ * that must hold data, or another memory_space; PB_ERR_UNSUPPORTED for a dim outside the built widths
+ * (32/48/64/96/128/256) or a document of more than 8193 tokens that is clustered.  PB_ERR_INVALID, nothing written, for
+ * an input value that is not finite (the reference panics or returns NaN rows there).  A host-memory call stages the
+ * whole input and output on the device; the clustering runs in waves of documents whose t x t f64 distance matrices
+ * (t = tokens - 1) fit 1 GiB. */
+PB_API int64_t pb_pooled_doc_length(int64_t n_tokens, int64_t pool_factor);
+PB_API pb_status pb_pool_embeddings(int32_t device, const float *embeddings, const int64_t *doc_lengths, int64_t n_docs,
+                                    int32_t dim, int64_t pool_factor, int32_t memory_space,
+                                    float *out_embeddings, int64_t *out_doc_lengths);
+/* device time of the calling thread's last pb_pool_embeddings per phase, ms (CUDA events): distances, chain, cut and
+ * means */
+PB_API pb_status pb_last_pool_ms(float *out_ms /* [3] */);
+
 /* ---- timing hooks for bench.py (device-side, CUDA events on the library's own stream) ----- */
 
 /* Stage ids for pb_last_stage_ms */

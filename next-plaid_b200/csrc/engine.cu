@@ -3589,6 +3589,181 @@ extern "C" pb_status pb_maxsim_scores(int32_t device, const float *query, int32_
     return PB_OK;
 }
 
+// ------------------------------------------------------------------------------------------
+// pool_document_embeddings (next-plaid-onnx lib.rs:1632, DESIGN §4p)
+// ------------------------------------------------------------------------------------------
+// pool_embeddings_hierarchical's length rule (lib.rs:1636-1641, :2257-2266) with protected_tokens = 1
+extern "C" int64_t pb_pooled_doc_length(int64_t n_tokens, int64_t pool_factor) {
+    if (n_tokens < 0 || pool_factor < 0) return -1;
+    if (pool_factor <= 1 || n_tokens <= 2) return n_tokens;
+    const int64_t t = n_tokens - 1, k = std::max<int64_t>(t / pool_factor, 1);
+    return k >= t ? n_tokens : 1 + k;
+}
+
+static thread_local float g_pool_ms[3];
+extern "C" pb_status pb_last_pool_ms(float *out_ms) {
+    if (!out_ms) return pb_fail(PB_ERR_INVALID, "null argument");
+    memcpy(out_ms, g_pool_ms, sizeof g_pool_ms);
+    return PB_OK;
+}
+
+// d^2 workspace of one wave of documents (a document that needs more runs alone)
+static constexpr size_t POOL_WAVE_BYTES = size_t(1) << 30;
+
+extern "C" pb_status pb_pool_embeddings(int32_t device, const float *embeddings, const int64_t *doc_lengths,
+                                        int64_t n_docs, int32_t dim, int64_t pool_factor, int32_t memory_space,
+                                        float *out_embeddings, int64_t *out_doc_lengths) {
+    if (n_docs < 0 || pool_factor < 0) return pb_fail(PB_ERR_INVALID, "negative n_docs or pool_factor");
+    if (n_docs > INT_MAX) return pb_fail(PB_ERR_UNSUPPORTED, "more than %d documents in one call", INT_MAX);
+    if (n_docs && (!doc_lengths || !out_doc_lengths)) return pb_fail(PB_ERR_INVALID, "null argument");
+    if (memory_space != PB_MEM_HOST && memory_space != PB_MEM_DEVICE)
+        return pb_fail(PB_ERR_INVALID, "memory_space %d is neither PB_MEM_HOST nor PB_MEM_DEVICE", memory_space);
+    CKS(BuiltDims::check(dim));
+    std::vector<PoolDoc> docs(n_docs);
+    long long total = 0, total_out = 0;
+    for (int64_t i = 0; i < n_docs; ++i) {
+        const int64_t n = doc_lengths[i];
+        if (n < 0) return pb_fail(PB_ERR_INVALID, "doc_lengths[%lld] = %lld is negative", (long long)i, (long long)n);
+        const int64_t o = pb_pooled_doc_length(n, pool_factor);
+        const int k = o < n ? (int)(o - 1) : 0;
+        if (n > INT_MAX || (k && n - 1 > PB_POOL_MAX_T))
+            return pb_fail(PB_ERR_UNSUPPORTED, "document %lld has %lld tokens; pooling clusters at most %d", (long long)i,
+                           (long long)n, PB_POOL_MAX_T);
+        docs[i] = PoolDoc{total, total_out, 0, 0, (int)n, k};
+        total += n;
+        total_out += o;
+    }
+    if ((total && !embeddings) || (total_out && !out_embeddings)) return pb_fail(PB_ERR_INVALID, "null argument");
+    CKS(check_device(device));
+    memset(g_pool_ms, 0, sizeof g_pool_ms);
+    // waves: consecutive documents whose d^2 matrices fit POOL_WAVE_BYTES; per wave the pooled documents and the
+    // (doc, I, J) tiles of k_pool_dist
+    struct Wave {
+        int d0, d1;
+        size_t p0, p1, i0, i1;
+        int max_t, max_means_smem;
+    };
+    std::vector<Wave> waves;
+    std::vector<int> pooled;
+    std::vector<int4> items;
+    size_t ws_max = 0, par_max = 0;
+    for (int64_t i = 0; i < n_docs;) {
+        Wave w{(int)i, (int)i, pooled.size(), 0, items.size(), 0, 0, 0};
+        size_t ws = 0, par = 0;
+        for (; i < n_docs; ++i) {
+            PoolDoc &d = docs[i];
+            const size_t t = d.n - 1, need = d.k ? t * t : 0;
+            if (w.d1 > w.d0 && (ws + need) * sizeof(double) > POOL_WAVE_BYTES) break;
+            if (d.k) {
+                d.ws_off = (long long)ws;
+                d.par_off = (long long)par;
+                ws += need;
+                par += t;
+                pooled.push_back((int)i);
+                const int nb = (int)((t + PB_POOL_TILE - 1) / PB_POOL_TILE);
+                for (int I = 0; I < nb; ++I)
+                    for (int J = I; J < nb; ++J) items.push_back(make_int4((int)i, I, J, 0));
+                w.max_t = std::max(w.max_t, (int)t);
+                w.max_means_smem = std::max(w.max_means_smem, (int)(4 * t + 2 * d.k) * 4);
+            }
+            w.d1 = (int)i + 1;
+        }
+        w.p1 = pooled.size();
+        w.i1 = items.size();
+        ws_max = std::max(ws_max, ws);
+        par_max = std::max(par_max, par);
+        waves.push_back(w);
+    }
+
+    OwnedStream st;
+    CK(cudaStreamCreateWithFlags(&st.s, cudaStreamNonBlocking));
+    DevBuf din, dout, ddocs, dpooled, ditems, dws, dpar, derr;
+    const size_t in_bytes = (size_t)total * dim * 4, out_bytes = (size_t)total_out * dim * 4;
+    const float *x = embeddings;
+    float *y = out_embeddings;
+    if (memory_space == PB_MEM_HOST) {
+        CKS(din.ensure(std::max<size_t>(in_bytes, 16)));
+        CKS(dout.ensure(std::max<size_t>(out_bytes, 16)));
+        if (in_bytes) CK(cudaMemcpyAsync(din.p, embeddings, in_bytes, cudaMemcpyHostToDevice, st.s));
+        x = din.as<float>();
+        y = dout.as<float>();
+    }
+    CKS(derr.ensure(16));
+    CK(cudaMemsetAsync(derr.p, 0, 4, st.s));
+    int sms = 0, err = 0;
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+    if (total) {
+        const long long nv = total * dim;
+        k_pool_finite<<<(int)std::min<long long>((nv + 255) / 256, (long long)sms * 8), 256, 0, st.s>>>(x, nv, derr.as<int>());
+        CK(cudaGetLastError());
+    }
+    CK(cudaMemcpyAsync(&err, derr.p, 4, cudaMemcpyDeviceToHost, st.s));
+    CK(cudaStreamSynchronize(st.s));
+    if (err & 1) return pb_fail(PB_ERR_INVALID, "the embeddings hold a value that is not finite");
+
+    CKS(ddocs.ensure(std::max<size_t>(docs.size() * sizeof(PoolDoc), 16)));
+    CKS(dpooled.ensure(std::max<size_t>(pooled.size() * 4, 16)));
+    CKS(ditems.ensure(std::max<size_t>(items.size() * sizeof(int4), 16)));
+    CKS(dws.ensure(std::max<size_t>(ws_max * sizeof(double), 16)));
+    CKS(dpar.ensure(std::max<size_t>(par_max * 4, 16)));
+    if (n_docs) CK(cudaMemcpyAsync(ddocs.p, docs.data(), docs.size() * sizeof(PoolDoc), cudaMemcpyHostToDevice, st.s));
+    if (!pooled.empty()) CK(cudaMemcpyAsync(dpooled.p, pooled.data(), pooled.size() * 4, cudaMemcpyHostToDevice, st.s));
+    if (!items.empty())
+        CK(cudaMemcpyAsync(ditems.p, items.data(), items.size() * sizeof(int4), cudaMemcpyHostToDevice, st.s));
+    struct Events {
+        cudaEvent_t e[4] = {};
+        ~Events() {
+            for (cudaEvent_t v : e)
+                if (v) cudaEventDestroy(v);
+        }
+    } ev;
+    for (cudaEvent_t &v : ev.e) CK(cudaEventCreate(&v));
+    for (const Wave &w : waves) {
+        const int np = (int)(w.p1 - w.p0), ni = (int)(w.i1 - w.i0);
+        CK(cudaEventRecord(ev.e[0], st.s));
+        if (ni) {
+            PB_DIM_SWITCH(dim, {
+                k_pool_dist<DIM><<<ni, 256, 0, st.s>>>(x, ddocs.as<PoolDoc>(), ditems.as<int4>() + w.i0, dws.as<double>());
+            });
+            CK(cudaGetLastError());
+        }
+        CK(cudaEventRecord(ev.e[1], st.s));
+        if (np) {
+            const size_t smem = (size_t)w.max_t * 24;
+            CKS(set_smem(k_pool_chain, smem));
+            k_pool_chain<<<np, 32, smem, st.s>>>(ddocs.as<PoolDoc>(), dpooled.as<int>() + w.p0, dws.as<double>(),
+                                                 dpar.as<int>(), derr.as<int>());
+            CK(cudaGetLastError());
+        }
+        CK(cudaEventRecord(ev.e[2], st.s));
+        PB_DIM_SWITCH(dim, {
+            auto kern = k_pool_means<DIM>;
+            CKS(set_smem(kern, w.max_means_smem));
+            kern<<<w.d1 - w.d0, 256, w.max_means_smem, st.s>>>(x, ddocs.as<PoolDoc>(), w.d0, dpar.as<int>(), y,
+                                                              derr.as<int>());
+        });
+        CK(cudaGetLastError());
+        CK(cudaEventRecord(ev.e[3], st.s));
+        CK(cudaEventSynchronize(ev.e[3]));
+        for (int p = 0; p < 3; ++p) {
+            float ms = 0.f;
+            CK(cudaEventElapsedTime(&ms, ev.e[p], ev.e[p + 1]));
+            g_pool_ms[p] += ms;
+        }
+    }
+    CK(cudaMemcpyAsync(&err, derr.p, 4, cudaMemcpyDeviceToHost, st.s));
+    CK(cudaStreamSynchronize(st.s));
+    if (err & 2)
+        return pb_fail(PB_ERR_UNSUPPORTED, "a nearest-neighbour chain revisited a cluster (the reference does not terminate)");
+    if (err) return pb_fail(PB_ERR_CUDA, "pooling cut did not give the expected number of clusters (error bits %d)", err);
+    if (memory_space == PB_MEM_HOST && out_bytes) {
+        CK(cudaMemcpyAsync(out_embeddings, dout.p, out_bytes, cudaMemcpyDeviceToHost, st.s));
+        CK(cudaStreamSynchronize(st.s));
+    }
+    for (int64_t i = 0; i < n_docs; ++i) out_doc_lengths[i] = pb_pooled_doc_length(doc_lengths[i], pool_factor);
+    return PB_OK;
+}
+
 extern "C" pb_status pb_exhaustive_scores(pb_index *ix, const float *queries, const int64_t *q_off, int64_t n_queries,
                                           float *out_scores) {
     if (ix && ix->dep) return pb_dep_exhaustive(ix->dep, queries, q_off, n_queries, out_scores);

@@ -25,6 +25,8 @@
 //                             memory into slot space, and the slots mapped back to doc ids before k_exact_finalize
 //   k_topk .............. a9  stable final sort, take top_k               search.rs:496-515
 //   k_merge_cut/k_merge_topk  doc-sharded search: global cut and global top-k from the all-gathered keys
+//   k_pool_dist/k_pool_chain/k_pool_means  pool_document_embeddings: cosine d^2 (f64), Ward's nearest-neighbour chain,
+//                             cut + cluster means   next-plaid-onnx lib.rs:2249-2317, hierarchy.rs:128-284, :426-504, :599-653
 //   k_assign_tc/k_assign_certify/k_assign/k_quantize_pack  a12  index build: nearest centroid (wgmma fp16
 //                             certified filter + exact fp32), residual quantise + pack   codec.rs:297-411
 //
@@ -50,3 +52,4 @@
 #include "k_maxsim_tc.cuh"
 #include "k_scores_tc.cuh"
 #include "k_stage.cuh"
+#include "k_pool.cuh"

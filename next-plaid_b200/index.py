@@ -100,7 +100,7 @@ EXPORTS = [
     "pb_index_delete_sharded", "pb_index_append_sharded", "pb_index_append_encoded_sharded",
     "pb_index_rebalance_sharded", "pb_index_load_range_flags", "pb_index_memory", "pb_last_staging_stats",
     "pb_search", "pb_index_set_coalescing", "pb_index_coalesce_stats", "pb_create_index_sharded", "pb_last_create_ms",
-    "pb_index_load_devices", "pb_index_shard_layout",
+    "pb_index_load_devices", "pb_index_shard_layout", "pb_pooled_doc_length", "pb_pool_embeddings", "pb_last_pool_ms",
 ]
 
 PB_OPEN_ADOPT_RESIDUALS, PB_OPEN_HOST_RESIDUALS = 1, 2
@@ -217,6 +217,11 @@ def load_library():
         L.pb_index_rebalance_sharded.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         L.pb_index_load_devices.argtypes = [C.c_char_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
         L.pb_index_shard_layout.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.pb_pooled_doc_length.argtypes = [C.c_int64, C.c_int64]
+        L.pb_pooled_doc_length.restype = C.c_int64
+        L.pb_pool_embeddings.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_int32,
+                                         C.c_void_p, C.c_void_p]
+        L.pb_last_pool_ms.argtypes = [C.c_void_p]
         _lib = L
     return _lib
 
@@ -907,6 +912,48 @@ def _rank_docs(docs, dim):
     flat = (np.ascontiguousarray(np.concatenate([np.asarray(d) for d in docs], 0), np.float32) if len(docs)
             else np.zeros((0, dim), np.float32))
     return _ptr(flat), 0, lens, flat
+
+
+def pooled_doc_length(n_tokens: int, pool_factor: int) -> int:
+    """pb_pooled_doc_length: the rows pool_document_embeddings returns for a document of n_tokens rows."""
+    return int(load_library().pb_pooled_doc_length(n_tokens, pool_factor))
+
+
+def pool_document_embeddings(embeddings: Sequence, pool_factor: Optional[int], device: int = 0) -> list:
+    """pool_document_embeddings (next-plaid-onnx lib.rs:1632) on the device (pb_pool_embeddings): token 0 of each
+    document kept, the others clustered by Ward linkage and averaged, bit-identical to the reference.  Takes and returns
+    a list of f32 [tokens, dim] numpy arrays, or of CUDA tensors (pooled on their device, the result on it too)."""
+    if not len(embeddings):
+        return []
+    L = load_library()
+    pf = 0 if pool_factor is None else pool_factor
+    dim = int(embeddings[0].shape[1])
+    ptr, space, lens, keep = _rank_docs(embeddings, dim)
+    olens = np.array([L.pb_pooled_doc_length(int(n), pf) for n in lens], np.int64)
+    if (olens < 0).any():
+        raise PlaidError(PB_ERR_INVALID, "negative pool_factor")
+    got = np.zeros(len(lens), np.int64)
+    total = int(olens.sum())
+    if space == 1:
+        import torch
+        out = torch.empty((total, dim), dtype=torch.float32, device=keep.device)
+        with torch.cuda.device(keep.device):
+            torch.cuda.current_stream().synchronize()
+        _check(L.pb_pool_embeddings(keep.device.index, ptr, _ptr(lens), len(lens), dim, pf, 1,
+                                    out.data_ptr() if total else None, _ptr(got)))
+    else:
+        out = np.zeros((total, dim), np.float32)
+        _check(L.pb_pool_embeddings(device, ptr, _ptr(lens), len(lens), dim, pf, 0, _ptr(out) if total else None,
+                                    _ptr(got)))
+    offs = np.concatenate([[0], np.cumsum(got)]).tolist()
+    return [out[offs[i]:offs[i + 1]] for i in range(len(got))]
+
+
+def last_pool_ms() -> dict:
+    """pb_last_pool_ms: device ms per phase of the calling thread's last pool_document_embeddings."""
+    v = np.zeros(3, np.float32)
+    _check(load_library().pb_last_pool_ms(_ptr(v)))
+    return dict(zip(["distances", "chain", "cut_means"], v.tolist()))
 
 
 def create_index_sharded(shards: Sequence[Sequence], index_dir: str, centroids: Optional[np.ndarray] = None,

@@ -48,6 +48,10 @@ struct PbCoalesceConfig {
 
 #[link(name = "plaid_b200")]
 extern "C" {
+    fn pb_pooled_doc_length(n_tokens: i64, pool_factor: i64) -> i64;
+    fn pb_pool_embeddings(device: i32, embeddings: *const f32, doc_lengths: *const i64, n_docs: i64, dim: i32,
+                          pool_factor: i64, memory_space: i32, out_embeddings: *mut f32, out_doc_lengths: *mut i64)
+                          -> c_int;
     fn pb_index_load(index_dir: *const c_char, device: i32, out: *mut *mut c_void) -> c_int;
     fn pb_index_close(ix: *mut c_void);
     fn pb_index_embedding_dim(ix: *const c_void) -> i32;
@@ -536,4 +540,50 @@ impl Drop for B200Index {
     fn drop(&mut self) {
         unsafe { pb_index_close(self.handle) }
     }
+}
+
+/// `pool_document_embeddings` (next-plaid-onnx lib.rs:1632) on `device`: token 0 of each document kept, the others
+/// clustered by Ward linkage and averaged, every row bit-identical to the reference's.  Same signature as the
+/// reference's plus the device; `pool_factor` None or <= 1 returns the input.
+pub fn pool_document_embeddings(
+    embeddings: &[Array2<f32>],
+    pool_factor: Option<usize>,
+    device: i32,
+) -> Result<Vec<Array2<f32>>> {
+    let pf = match pool_factor {
+        Some(pf) if pf > 1 => pf as i64,
+        _ => return Ok(embeddings.to_vec()),
+    };
+    if embeddings.is_empty() {
+        return Ok(Vec::new());
+    }
+    let dim = embeddings[0].ncols();
+    if let Some(e) = embeddings.iter().find(|e| e.ncols() != dim) {
+        return Err(Error::Shape(format!("documents have {} and {} columns", dim, e.ncols())));
+    }
+    let lens: Vec<i64> = embeddings.iter().map(|e| e.nrows() as i64).collect();
+    let out_lens: Vec<i64> = lens.iter().map(|&n| unsafe { pb_pooled_doc_length(n, pf) }).collect();
+    let mut flat = Vec::with_capacity(lens.iter().sum::<i64>() as usize * dim);
+    for e in embeddings {
+        flat.extend(e.iter().copied());
+    }
+    let mut out = vec![0f32; out_lens.iter().sum::<i64>() as usize * dim];
+    let mut got = vec![0i64; lens.len()];
+    let st = unsafe {
+        pb_pool_embeddings(device, flat.as_ptr(), lens.as_ptr(), lens.len() as i64, dim as i32, pf, 0,
+                           out.as_mut_ptr(), got.as_mut_ptr())
+    };
+    if st != 0 {
+        return Err(Error::Shape(last_error()));
+    }
+    let mut docs = Vec::with_capacity(got.len());
+    let mut off = 0usize;
+    for &n in &got {
+        let rows = n as usize;
+        let a = Array2::from_shape_vec((rows, dim), out[off * dim..(off + rows) * dim].to_vec())
+            .map_err(|e| Error::Shape(e.to_string()))?;
+        docs.push(a);
+        off += rows;
+    }
+    Ok(docs)
 }
