@@ -769,6 +769,48 @@ PB_API pb_status pb_index_load_devices(const char *index_dir, const int32_t *dev
  * out_devices [world].  A handle that is not a deployment reports world 1, [doc_id_base, doc_id_base + D], its device. */
 PB_API pb_status pb_index_shard_layout(const pb_index *ix, int32_t *out_world, int64_t *out_bounds, int32_t *out_devices);
 
+/* ---- replicas behind one handle (DESIGN.md 4q) --------------------------------------------
+ *
+ * R full copies of an index directory, each spread over S devices, behind one handle: n_devices = R * S, and replica g
+ * uses devices[g*S .. g*S + S-1] (devices may repeat).  With S = 1 each replica is a handle of pb_index_load; with S > 1
+ * a deployment of pb_index_load_devices.  flags as for pb_index_load_range_flags.  Replica 0 is loaded from the
+ * directory; every other replica is a device-to-device copy of it (derived arrays included; the sm count and the grids
+ * sized from it are the copy's device's own), made concurrently.  With PB_OPEN_HOST_RESIDUALS rank r of every replica
+ * reads replica 0's rank r's one pinned array, freed with the last of them.
+ * Checks before any device is touched, in this order: a NULL index_dir, devices or out, n_shards < 1, n_devices not a
+ * positive multiple of n_shards, n_devices > 64: PB_ERR_INVALID; no usable device: PB_ERR_CUDA; a device id outside
+ * [0, pb_device_count()): PB_ERR_INVALID.  A failed load returns the lowest failing replica's status and message and
+ * leaves nothing allocated.
+ * Every entry point behaves as on replica 0's kind of handle, with results equal to it bit for bit, and refuses where it
+ * refuses; on top of that:
+ *   searches: a call of n queries is cut into k = min(R, ceil(n / 32)) contiguous slices, each served by one of the k
+ *     replicas with the fewest queries in flight (ties: the lowest index); slice 0 runs on the calling thread, the others
+ *     on library threads.  A traced call, and a call whose arguments the host checks of a plain handle refuse, runs
+ *     whole on one replica; a cut call that a slice refuses on the device runs again whole on one replica, for the
+ *     plain handle's status and message.  pb_last_error() is the call's; the pb_last_* stats of the calling thread are every slice's, merged as
+ *     lanes merge them (per-sub-batch counters count each slice's sub-batches).
+ *   pb_search with coalescing: each merged batch goes whole to the least-loaded replica; max_inflight is per replica.
+ *   pb_decompress_documents, pb_exhaustive_scores, pb_centroid_scores, pb_index_export_ivf: on one replica.
+ *   pb_index_memory: device bytes of every replica; host bytes of each pinned array once.
+ *   mutations (append, append_encoded, delete, reserve, rebalance) hold the set alone: a search sees every replica
+ *     before a mutation or every replica after it.  With a codec, only replica 0 (its last rank) encodes; the others
+ *     take its encoded rows, and pb_codec_last_assign_stats counts the tokens once.  The directory is written once,
+ *     byte-identical to the single handle's.  Every replica prepares, the directory is written, every replica
+ *     commits (S > 1: the replicas' ranks vote together around their groups' own votes), so a failure before the
+ *     commit changes no replica and no file.  After a commit only a CUDA runtime error can fail, and the set must then
+ *     be reloaded.  pb_index_reserve only adds capacity: a replica that reserved before another failed keeps it.
+ *   refused with PB_ERR_UNSUPPORTED, handle unchanged: pb_search_batch_device, pb_index_comm_init,
+ *     pb_index_group_join and the _sharded mutations. */
+PB_API pb_status pb_index_load_replicas(const char *index_dir, const int32_t *devices, int32_t n_devices,
+                                        int32_t n_shards, int32_t flags, pb_index **out);
+/* *out_replicas = R, *out_shards = S and (may be NULL) out_devices [R*S].  Any other handle is one replica of its
+ * pb_index_shard_layout ranks. */
+PB_API pb_status pb_index_replica_layout(const pb_index *ix, int32_t *out_replicas, int32_t *out_shards,
+                                         int32_t *out_devices /* [R*S], may be NULL */);
+/* Per replica, since load or the last reset: calls or slices it served (out_calls [R]) and queries (out_queries [R]);
+ * either may be NULL.  PB_ERR_INVALID on a handle that is not a replica set. */
+PB_API pb_status pb_index_replica_stats(pb_index *ix, int64_t *out_calls, int64_t *out_queries, int32_t reset);
+
 /* ---- misc ----------------------------------------------------------------------------- */
 
 PB_API const char *pb_last_error(void);       /* thread-local, never NULL */

@@ -8,7 +8,7 @@ import sys
 PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libplaid_b200.so")
-SOURCES = ["engine.cu", "loader.cpp", "builder.cpp", "deployment.cpp"]
+SOURCES = ["engine.cu", "loader.cpp", "builder.cpp", "deployment.cpp", "replicas.cpp"]
 DEPS = SOURCES + sorted(f for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + \
     [os.path.join("..", "..", "include", "plaid_b200.h")]
 NVCC_FLAGS = [

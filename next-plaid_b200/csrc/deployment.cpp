@@ -19,56 +19,6 @@
 
 namespace {
 
-using Job = std::function<pb_status(int rank)>;
-
-// A rank's thread: waits for a job, runs it, records its status and pb_last_error() text
-struct RankWorker {
-    int rank;
-    std::thread th;
-    std::mutex m;
-    std::condition_variable cv;
-    const Job *job = nullptr;
-    bool done = false, quit = false;
-    pb_status status = PB_OK;
-    std::string error;
-    explicit RankWorker(int r) : rank(r) {
-        th = std::thread([this] {
-            std::unique_lock<std::mutex> lk(m);
-            for (;;) {
-                cv.wait(lk, [this] { return job || quit; });
-                if (quit) return;
-                const Job *j = job;
-                lk.unlock();
-                const pb_status s = (*j)(rank);
-                std::string e = s == PB_OK ? std::string() : std::string(pb_last_error());
-                lk.lock();
-                status = s, error = std::move(e);
-                job = nullptr;
-                done = true;
-                cv.notify_all();
-            }
-        });
-    }
-    void submit(const Job &j) {
-        std::lock_guard<std::mutex> lk(m);
-        job = &j;
-        done = false;
-        cv.notify_all();
-    }
-    void wait() {
-        std::unique_lock<std::mutex> lk(m);
-        cv.wait(lk, [this] { return done; });
-    }
-    ~RankWorker() {
-        {
-            std::lock_guard<std::mutex> lk(m);
-            quit = true;
-            cv.notify_all();
-        }
-        if (th.joinable()) th.join();
-    }
-};
-
 struct SearchScratch {  // one rank's copy of a search's outputs (ranks >= 1)
     std::vector<int64_t> ids;
     std::vector<float> scores;
@@ -139,6 +89,16 @@ struct Deployment {
         return PB_OK;
     }
 
+    // joins the loaded ranks in the group and makes the handle; on failure the caller deletes this
+    pb_status finish(pb_index **out) {
+        for (int r = 0; r < world(); ++r) {
+            pb_status s = pb_index_group_join(ranks[r], group, r);
+            if (s != PB_OK) return s;
+        }
+        *out = pb_index_new_deployment(this, ranks[0]);
+        return PB_OK;
+    }
+
     ~Deployment() {
         workers.clear();  // joins the threads
         for (pb_index *ix : ranks) pb_index_close(ix);
@@ -180,11 +140,23 @@ extern "C" pb_status pb_index_load_devices(const char *index_dir, const int32_t 
     }, false);
     d->ranks.erase(std::remove(d->ranks.begin(), d->ranks.end(), nullptr), d->ranks.end());
     if (s != PB_OK) return s;  // ~Deployment closes the ranks that loaded
-    for (int r = 0; r < n_devices; ++r)
-        if ((s = pb_index_group_join(d->ranks[r], d->group, r)) != PB_OK) return s;
-    pb_index *ix = pb_index_new_deployment(d.get(), d->ranks[0]);
+    if ((s = d->finish(out)) != PB_OK) return s;
     d.release();
-    *out = ix;
+    return PB_OK;
+}
+
+pb_status pb_dep_assemble(std::vector<pb_index *> ranks, const std::vector<int> &devices, pb_index **out) {
+    const int n = (int)ranks.size();
+    std::unique_ptr<Deployment> d(new Deployment());
+    d->ranks = std::move(ranks);  // closed by ~Deployment on failure
+    d->devices = devices;
+    d->scratch.resize((size_t)n);
+    pb_status s = pb_shard_group_create(n, &d->group);
+    if (s != PB_OK) return s;
+    d->workers.resize((size_t)n);
+    for (int r = 1; r < n; ++r) d->workers[r].reset(new RankWorker(r));
+    if ((s = d->finish(out)) != PB_OK) return s;
+    d.release();
     return PB_OK;
 }
 

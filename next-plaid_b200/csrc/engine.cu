@@ -246,10 +246,11 @@ struct HostBuf {  // pinned
 };
 
 // the packed residuals of a PB_OPEN_HOST_RESIDUALS handle: pinned, mapped and portable host memory; dev is the address
-// kernels read it at
+// kernels read it at.  The replicas of a set share one allocation (share), freed with the last of them.
 struct PinnedRes {
     uint8_t *p = nullptr, *dev = nullptr;
     size_t bytes = 0;
+    std::shared_ptr<uint8_t> keep;  // owns p
     pb_status alloc(size_t n) {
         if (n == 0) return PB_OK;
         void *h = nullptr;
@@ -265,12 +266,20 @@ struct PinnedRes {
             return pb_fail(PB_ERR_CUDA, "cudaHostGetDevicePointer failed: %s", cudaGetErrorString(e));
         }
         p = static_cast<uint8_t *>(h);
+        keep.reset(p, [](uint8_t *q) { cudaFreeHost(q); });
         dev = static_cast<uint8_t *>(d);
         bytes = n;
         return PB_OK;
     }
-    ~PinnedRes() {
-        if (p) cudaFreeHost(p);
+    // o's allocation, read from the current device
+    pb_status share(const PinnedRes &o) {
+        if (!o.p) return PB_OK;
+        void *d = nullptr;
+        cudaError_t e = cudaHostGetDevicePointer(&d, o.p, 0);
+        if (e != cudaSuccess) return pb_fail(PB_ERR_CUDA, "cudaHostGetDevicePointer failed: %s", cudaGetErrorString(e));
+        p = o.p, keep = o.keep, bytes = o.bytes;
+        dev = static_cast<uint8_t *>(d);
+        return PB_OK;
     }
 };
 
@@ -641,6 +650,11 @@ struct pb_index : DocArrays {
     }
     // pb_index_load_devices: this handle holds no documents and stands for the ranks of `dep` (deployment.cpp)
     Deployment *dep = nullptr;
+    // pb_index_load_replicas: this handle holds no documents and stands for the replicas of `rep` (replicas.cpp)
+    Replicas *rep = nullptr;
+    // a rank of a replica of such a set, during one of its mutations: the vote it takes with the other replicas
+    RepVote *rep_vote = nullptr;
+    int rep_index = 0;
     // doc-sharded deployment (pb_index_comm_init / pb_index_group_join).  Declared last, so destroyed first: an NCCL
     // communicator goes before the workspace streams it ran on
     ShardComm comm;
@@ -1217,10 +1231,22 @@ pb_index *pb_index_new_deployment(Deployment *d, const pb_index *rank0) {
     return ix;
 }
 
-// The calls a deployment refuses: each addresses one rank's handle, or one device
+// A replica set's handle (replicas.cpp): no documents of its own; K, dim, nbits and device from replica 0
+pb_index *pb_index_new_replicas(Replicas *rs, const pb_index *member0) {
+    pb_index *ix = new pb_index();
+    ix->rep = rs;
+    ix->device = member0->device, ix->dim = member0->dim, ix->nbits = member0->nbits, ix->packed = member0->packed;
+    ix->K = member0->K;
+    coalesce_env_defaults(ix);  // cannot fail: the handle joins no group
+    return ix;
+}
+
+// The calls a deployment or a replica set refuses: each addresses one rank's handle, one device, or one group
 static pb_status refuse_deployment(const pb_index *ix, const char *call) {
     if (ix && ix->dep)
         return pb_fail(PB_ERR_UNSUPPORTED, "%s on a multi-device handle (pb_index_load_devices) is not supported", call);
+    if (ix && ix->rep)
+        return pb_fail(PB_ERR_UNSUPPORTED, "%s on a replica set (pb_index_load_replicas) is not supported", call);
     return PB_OK;
 }
 
@@ -1274,6 +1300,8 @@ pb_status pb_index_finalize(pb_index *ix) {
 
 extern "C" pb_status pb_index_export_ivf(pb_index *ix, int64_t *out_ivf, int32_t *out_lengths, int64_t *out_total) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    if (ix->rep)
+        return pb_rep_whole(ix->rep, 0, [&](pb_index *m) { return pb_index_export_ivf(m, out_ivf, out_lengths, out_total); });
     CKS(refuse_deployment(ix, "pb_index_export_ivf"));
     auto rd = ix->read_lock();
     CK(cudaSetDevice(ix->device));
@@ -1309,6 +1337,7 @@ extern "C" pb_status pb_index_open(const pb_index_desc *d, pb_index **out) {
 extern "C" void pb_index_close(pb_index *ix) {
     if (!ix) return;
     if (ix->dep) pb_dep_close(ix->dep);  // joins its threads, closes its ranks, destroys its group
+    if (ix->rep) pb_rep_close(ix->rep);  // joins its threads, closes its replicas
     cudaSetDevice(ix->device);
     ix->lane_workers.clear();  // joins the helper threads
     cudaDeviceSynchronize();
@@ -1320,6 +1349,7 @@ extern "C" int64_t pb_index_num_documents(const pb_index *ix) {
     if (!ix) return 0;
     long long D, N;
     if (ix->dep) return pb_dep_totals(ix->dep, &D, &N) == PB_OK ? D : 0;
+    if (ix->rep) return pb_index_num_documents(pb_rep_member(ix->rep, 0));
     auto rd = ix->read_lock();
     return ix->D;
 }
@@ -1327,6 +1357,7 @@ extern "C" int64_t pb_index_num_embeddings(const pb_index *ix) {
     if (!ix) return 0;
     long long D, N;
     if (ix->dep) return pb_dep_totals(ix->dep, &D, &N) == PB_OK ? N : 0;
+    if (ix->rep) return pb_index_num_embeddings(pb_rep_member(ix->rep, 0));
     auto rd = ix->read_lock();
     return ix->N;
 }
@@ -1335,6 +1366,7 @@ extern "C" double pb_index_avg_doclen(const pb_index *ix) {
     if (!ix) return 0.0;
     long long D, N;
     if (ix->dep) return pb_dep_totals(ix->dep, &D, &N) == PB_OK && D ? (double)N / (double)D : 0.0;
+    if (ix->rep) return pb_index_avg_doclen(pb_rep_member(ix->rep, 0));
     auto rd = ix->read_lock();
     return ix->D ? (double)ix->N / (double)ix->D : 0.0;
 }
@@ -1345,6 +1377,7 @@ extern "C" int32_t pb_index_device(const pb_index *ix) { return ix ? ix->device 
 extern "C" pb_status pb_index_memory(const pb_index *ix, int64_t *device_bytes, int64_t *host_bytes) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
     if (ix->dep) return pb_dep_memory(ix->dep, device_bytes, host_bytes);
+    if (ix->rep) return pb_rep_memory(ix->rep, device_bytes, host_bytes);
     auto rd = ix->read_lock();
     size_t dev = ix->centroids.cap + ix->w_rev.cap + ix->cent_h16t.cap + ix->cent_l16t.cap;
     for (const DevBuf *b : DocArrays::buffers(*ix))
@@ -1357,6 +1390,7 @@ extern "C" pb_status pb_index_memory(const pb_index *ix, int64_t *device_bytes, 
 extern "C" pb_status pb_index_shard_layout(const pb_index *ix, int32_t *out_world, int64_t *out_bounds, int32_t *out_devices) {
     if (!ix || !out_world) return pb_fail(PB_ERR_INVALID, "null argument");
     if (ix->dep) return pb_dep_layout(ix->dep, out_world, out_bounds, out_devices);
+    if (ix->rep) return pb_index_shard_layout(pb_rep_member(ix->rep, 0), out_world, out_bounds, out_devices);
     auto rd = ix->read_lock();
     *out_world = 1;
     if (out_bounds) out_bounds[0] = ix->doc_id_base, out_bounds[1] = ix->doc_id_base + ix->D;
@@ -1378,14 +1412,17 @@ extern "C" void pb_search_params_default(pb_search_params *p) {  // search.rs:58
 extern "C" void pb_set_fast_approx(pb_index *ix, int32_t enabled) {
     if (!ix) return;
     if (ix->dep) return pb_dep_each(ix->dep, [&](pb_index *m) { pb_set_fast_approx(m, enabled); });
+    if (ix->rep) return pb_rep_each(ix->rep, [&](pb_index *m) { pb_set_fast_approx(m, enabled); });
     ix->fast_approx = enabled != 0;  // 0 = single exact pass over every candidate, otherwise two-pass
 }
 extern "C" void pb_set_scores_tc(pb_index *ix, int32_t enabled) {
     if (ix && ix->dep) return pb_dep_each(ix->dep, [&](pb_index *m) { pb_set_scores_tc(m, enabled); });
+    if (ix && ix->rep) return pb_rep_each(ix->rep, [&](pb_index *m) { pb_set_scores_tc(m, enabled); });
     if (ix) ix->k1_tc = enabled != 0;  // effective when the tensor-core operands were built at open (k1_tc_usable)
 }
 extern "C" void pb_set_lanes(pb_index *ix, int32_t lanes) {
     if (ix && ix->dep) return pb_dep_each(ix->dep, [&](pb_index *m) { pb_set_lanes(m, lanes); });
+    if (ix && ix->rep) return pb_rep_each(ix->rep, [&](pb_index *m) { pb_set_lanes(m, lanes); });
     if (ix) ix->lanes = std::min(8, std::max(1, (int)lanes));
 }
 extern "C" pb_status pb_index_set_coalescing(pb_index *ix, const pb_coalesce_config *cfg) {
@@ -1398,7 +1435,8 @@ extern "C" pb_status pb_index_set_coalescing(pb_index *ix, const pb_coalesce_con
             return pb_fail(PB_ERR_UNSUPPORTED, "coalescing on a doc-sharded handle: a collective needs the same order on every rank");
         c.max_queries = cfg->max_queries;
         c.max_wait_us = std::min(cfg->max_wait_us, 10000);
-        c.max_inflight = cfg->max_inflight;
+        // a replica set runs max_inflight merged batches per replica
+        c.max_inflight = ix->rep ? cfg->max_inflight * pb_rep_count(ix->rep) : cfg->max_inflight;
     }
     ix->coalescer.configure(c);
     ix->coalesce_on = c.max_queries > 1;
@@ -1415,10 +1453,12 @@ extern "C" pb_status pb_index_coalesce_stats(pb_index *ix, pb_coalesce_stats *ou
 }
 extern "C" void pb_set_fast_exact(pb_index *ix, int32_t enabled) {
     if (ix && ix->dep) return pb_dep_each(ix->dep, [&](pb_index *m) { pb_set_fast_exact(m, enabled); });
+    if (ix && ix->rep) return pb_rep_each(ix->rep, [&](pb_index *m) { pb_set_fast_exact(m, enabled); });
     if (ix) ix->fast_exact = enabled != 0;
 }
 extern "C" void pb_set_profiling(pb_index *ix, int32_t enabled) {
     if (ix && ix->dep) return pb_dep_each(ix->dep, [&](pb_index *m) { pb_set_profiling(m, enabled); });
+    if (ix && ix->rep) return pb_rep_each(ix->rep, [&](pb_index *m) { pb_set_profiling(m, enabled); });
     if (ix) ix->profiling = enabled != 0;
 }
 extern "C" pb_status pb_last_stage_stats(pb_index *, float *out_ms, int32_t *out_launches) {
@@ -3231,10 +3271,72 @@ static pb_status search_impl(pb_index *ix, const SearchIO &io) {
     return PB_OK;
 }
 
+// A replica set's search (replicas.cpp): contiguous slices of the batch, each on one of the least-loaded replicas.
+// run(m, b0, b1) searches queries [b0, b1) on member m into the caller's rows; (0, n) passes the caller's arguments as
+// they are.  A call that the host checks of a plain handle refuse (null or non-monotone offsets, a query's parameters)
+// is not cut: it runs whole on one replica, so it is refused there, once, with the plain handle's status, message and
+// outputs.  A cut call that a slice still refuses on the device runs again whole on one replica, for the plain
+// handle's status and message.  The caller's stats are every slice's, merged as the lanes' are.
+static pb_status replica_search(pb_index *ix, const float *queries, const int64_t *q_off, int64_t n_queries,
+                                const int64_t *sub_off, const pb_search_params *params, int64_t params_stride,
+                                const std::function<pb_status(pb_index *, int64_t, int64_t)> &run) {
+    auto whole = [&] { return pb_rep_whole(ix->rep, n_queries, [&](pb_index *m) { return run(m, 0, n_queries); }); };
+    bool cut = n_queries > 1 && queries && q_off && params && (!sub_off || sub_off[0] == 0);
+    for (int64_t b = 0; cut && b < n_queries; ++b) {
+        cut = q_off[b + 1] >= q_off[b] && (!sub_off || sub_off[b + 1] >= sub_off[b]);
+        int M = 0;
+        const pb_search_params &p = params[b * params_stride];
+        cut = cut && check_query_args(p) == PB_OK && query_kept_docs(p, &M) == PB_OK;
+    }
+    if (!cut) return whole();
+    std::vector<Stats> stats((size_t)pb_rep_count(ix->rep));
+    std::vector<char> ran(stats.size(), 0);
+    const pb_status st = pb_rep_search(ix->rep, n_queries, [&](pb_index *m, int64_t b0, int64_t b1, int k) {
+        const pb_status r = run(m, b0, b1);
+        stats[k] = g_stats, ran[k] = 1;
+        return r;
+    });
+    if (st != PB_OK) return whole();
+    Stats total = stats[0];
+    for (size_t k = 1; k < stats.size(); ++k)
+        if (ran[k]) {
+            merge_stats(total, stats[k]);
+            total.call_ms = std::max(total.call_ms, stats[k].call_ms);
+        }
+    g_stats = total;
+    return PB_OK;
+}
+
+// q_tok_offsets [b0, b1] of a slice, from 0
+static std::vector<int64_t> slice_offsets(const int64_t *off, int64_t b0, int64_t b1) {
+    std::vector<int64_t> o((size_t)(b1 - b0 + 1));
+    for (int64_t i = b0; i <= b1; ++i) o[(size_t)(i - b0)] = off[i] - off[b0];
+    return o;
+}
+
 extern "C" pb_status pb_search_batch_traced(pb_index *ix, const float *queries, const int64_t *q_tok_offsets,
                                             int64_t n_queries, const pb_search_params *params, const int64_t *subset,
                                             int64_t n_subset, int64_t *out_ids, float *out_scores, int32_t *out_counts,
                                             pb_trace *trace) {
+    if (ix && ix->rep) {
+        if (trace || !params)  // a trace follows one call through the pipeline: never cut
+            return pb_rep_whole(ix->rep, n_queries, [&](pb_index *m) {
+                return pb_search_batch_traced(m, queries, q_tok_offsets, n_queries, params, subset, n_subset, out_ids,
+                                              out_scores, out_counts, trace);
+            });
+        const int64_t k = std::max<int64_t>(params->top_k, 0);
+        return replica_search(ix, queries, q_tok_offsets, n_queries, nullptr, params, 0,
+                              [&](pb_index *m, int64_t b0, int64_t b1) {
+            if (b0 == 0 && b1 == n_queries)
+                return pb_search_batch_traced(m, queries, q_tok_offsets, n_queries, params, subset, n_subset, out_ids,
+                                              out_scores, out_counts, nullptr);
+            const std::vector<int64_t> qo = slice_offsets(q_tok_offsets, b0, b1);
+            return pb_search_batch_traced(m, queries + q_tok_offsets[b0] * ix->dim, qo.data(), b1 - b0, params, subset,
+                                          n_subset, out_ids ? out_ids + b0 * k : nullptr,
+                                          out_scores ? out_scores + b0 * k : nullptr,
+                                          out_counts ? out_counts + b0 : nullptr, nullptr);
+        });
+    }
     if (trace) CKS(refuse_deployment(ix, "pb_search_batch_traced with a trace"));
     if (ix && ix->dep)
         return pb_dep_search(ix->dep, n_queries, params ? params->top_k : 0, out_ids, out_scores, out_counts,
@@ -3267,6 +3369,40 @@ static pb_status search_subsets(pb_index *ix, const float *queries, const int64_
     if (params)
         for (int64_t b = 0; b < (params_stride ? n_queries : 1); ++b)
             out_stride = std::max<int64_t>(out_stride, params[b * params_stride].top_k);
+    if (ix && ix->rep && trace)
+        return pb_rep_whole(ix->rep, n_queries, [&](pb_index *m) {
+            return search_subsets(m, queries, q_tok_offsets, n_queries, params, params_stride, subset_offsets,
+                                  subset_ids, has_subset, out_ids, out_scores, out_counts, trace);
+        });
+    if (ix && ix->rep)
+        return replica_search(ix, queries, q_tok_offsets, n_queries, subset_offsets, params, params_stride,
+                              [&](pb_index *m, int64_t b0, int64_t b1) {
+            if (b0 == 0 && b1 == n_queries)
+                return search_subsets(m, queries, q_tok_offsets, n_queries, params, params_stride, subset_offsets,
+                                      subset_ids, has_subset, out_ids, out_scores, out_counts, nullptr);
+            const std::vector<int64_t> qo = slice_offsets(q_tok_offsets, b0, b1);
+            std::vector<int64_t> so;
+            if (subset_offsets) so = slice_offsets(subset_offsets, b0, b1);
+            const pb_search_params *pp = params + b0 * params_stride;
+            int64_t stride = 0;  // the slice's largest top_k: its rows are that far apart
+            for (int64_t b = 0; b < (params_stride ? b1 - b0 : 1); ++b) stride = std::max<int64_t>(stride, pp[b * params_stride].top_k);
+            const bool direct = stride == out_stride;
+            std::vector<int64_t> ids(direct || !out_ids ? 0 : (size_t)(b1 - b0) * stride);
+            std::vector<float> sc(direct || !out_scores ? 0 : (size_t)(b1 - b0) * stride);
+            const pb_status st = search_subsets(
+                m, queries + q_tok_offsets[b0] * ix->dim, qo.data(), b1 - b0, pp, params_stride,
+                subset_offsets ? so.data() : nullptr, subset_ids && subset_offsets ? subset_ids + subset_offsets[b0] : subset_ids,
+                has_subset ? has_subset + b0 : nullptr, !out_ids ? nullptr : direct ? out_ids + b0 * out_stride : ids.data(),
+                !out_scores ? nullptr : direct ? out_scores + b0 * out_stride : sc.data(),
+                out_counts ? out_counts + b0 : nullptr, nullptr);
+            if (st != PB_OK || direct) return st;
+            for (int64_t b = 0; b < b1 - b0; ++b) {  // each row's own top_k entries, as the search writes them
+                const size_t kq = (size_t)std::max<int64_t>(pp[b * params_stride].top_k, 0);
+                if (out_ids) std::copy_n(ids.data() + b * stride, kq, out_ids + (b0 + b) * out_stride);
+                if (out_scores) std::copy_n(sc.data() + b * stride, kq, out_scores + (b0 + b) * out_stride);
+            }
+            return st;
+        });
     if (ix && ix->dep) {
         if (trace) CKS(refuse_deployment(ix, "a search with a trace"));
         return pb_dep_search(ix->dep, n_queries, out_stride, out_ids, out_scores, out_counts,
@@ -3344,6 +3480,11 @@ static pb_status check_request(const pb_index *ix, long long D, const SearchRequ
 }
 
 int CoalescedRun::operator()(pbq::Request *const *reqs, size_t n, std::string &err) const {
+    if (ix->rep) {  // a replica set: the merged batch goes whole to the least-loaded replica
+        int r = 0;
+        pb_rep_whole(ix->rep, (int64_t)n, [&](pb_index *m) { return (pb_status)(r = CoalescedRun{m}(reqs, n, err)); });
+        return r;
+    }
     pb_status st;
     if (n == 1) st = search_alone(ix, *static_cast<SearchRequest *>(reqs[0]));
     else {
@@ -3407,9 +3548,10 @@ extern "C" pb_status pb_search(pb_index *ix, const float *query, int64_t n_query
         return search_alone(ix, r);
     }
     pb_status st;
-    if (ix->dep) {  // as one handle of the whole index: every rank's K, the deployment's D (rank 0 may be empty)
+    if (ix->dep || ix->rep) {  // as one handle of the whole index: every rank's K, the deployment's D (rank 0 may be empty)
         const long long D = pb_index_num_documents(ix);
-        const pb_index *m = pb_dep_rank(ix->dep, 0);
+        const pb_index *m = ix->rep ? pb_rep_member(ix->rep, 0) : ix;
+        if (m->dep) m = pb_dep_rank(m->dep, 0);
         auto rd = m->read_lock();
         st = check_request(m, D, r);
     } else {
@@ -3436,7 +3578,7 @@ extern "C" pb_status pb_search_batch(pb_index *ix, const float *queries, const i
 extern "C" pb_status pb_search_batch_device(pb_index *ix, const float *d_queries, const int64_t *q_tok_offsets_host,
                                             int64_t n_queries, const pb_search_params *params, int64_t *d_out_ids,
                                             float *d_out_scores, int32_t *d_out_counts) {
-    CKS(refuse_deployment(ix, "pb_search_batch_device"));
+    CKS(refuse_deployment(ix, "pb_search_batch_device"));  // its pointers belong to one device
     SearchIO io{d_queries, true, q_tok_offsets_host, n_queries, nullptr, nullptr, nullptr, 0, false,
                 d_out_ids, d_out_scores, d_out_counts, true, nullptr, params, 0, params ? params->top_k : 0};
     return search_impl(ix, io);
@@ -3447,6 +3589,7 @@ extern "C" pb_status pb_search_batch_device(pb_index *ix, const float *d_queries
 // ------------------------------------------------------------------------------------------
 extern "C" pb_status pb_centroid_scores(pb_index *ix, const float *query_tokens, int64_t n, float *out) {
     if (ix && ix->dep) return pb_centroid_scores(pb_dep_rank(ix->dep, 0), query_tokens, n, out);  // centroids replicated
+    if (ix && ix->rep) return pb_rep_whole(ix->rep, 0, [&](pb_index *m) { return pb_centroid_scores(m, query_tokens, n, out); });
     if (!ix || (!query_tokens && n) || (!out && n)) return pb_fail(PB_ERR_INVALID, "null argument");
     if (n == 0) return PB_OK;
     auto rd = ix->read_lock();
@@ -3480,6 +3623,10 @@ extern "C" pb_status pb_centroid_scores(pb_index *ix, const float *query_tokens,
 extern "C" pb_status pb_decompress_documents(pb_index *ix, const int64_t *doc_ids, int64_t n_docs, float *out_embeddings,
                                              int64_t *out_lengths) {
     if (ix && ix->dep) return pb_dep_decompress(ix->dep, doc_ids, n_docs, out_embeddings, out_lengths);
+    if (ix && ix->rep)
+        return pb_rep_whole(ix->rep, 0, [&](pb_index *m) {
+            return pb_decompress_documents(m, doc_ids, n_docs, out_embeddings, out_lengths);
+        });
     if (!ix || (!doc_ids && n_docs) || !out_lengths) return pb_fail(PB_ERR_INVALID, "null argument");
     auto rd = ix->read_lock();
     CK(cudaSetDevice(ix->device));
@@ -3767,6 +3914,8 @@ extern "C" pb_status pb_pool_embeddings(int32_t device, const float *embeddings,
 extern "C" pb_status pb_exhaustive_scores(pb_index *ix, const float *queries, const int64_t *q_off, int64_t n_queries,
                                           float *out_scores) {
     if (ix && ix->dep) return pb_dep_exhaustive(ix->dep, queries, q_off, n_queries, out_scores);
+    if (ix && ix->rep)
+        return pb_rep_whole(ix->rep, 0, [&](pb_index *m) { return pb_exhaustive_scores(m, queries, q_off, n_queries, out_scores); });
     if (!ix || (!queries && n_queries) || !q_off || (!out_scores && n_queries)) return pb_fail(PB_ERR_INVALID, "null argument");
     auto rd = ix->read_lock();
     CK(cudaSetDevice(ix->device));
@@ -4601,27 +4750,9 @@ static pb_status refuse_fixed_residuals(const pb_index *ix) {
 static pb_status append_impl(pb_index *ix, pb_codec *codec, const float *embeddings, const int64_t *codes,
                              const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs, int32_t space,
                              const char *index_dir, int64_t batch_size, int64_t *out_first) {
-    if (!ix || (!doc_lengths && n_docs) || n_docs < 0) return pb_fail(PB_ERR_INVALID, "null argument");
-    if (space != PB_MEM_HOST && space != PB_MEM_DEVICE) return pb_fail(PB_ERR_INVALID, "bad memory_space %d", space);
-    std::lock_guard<std::mutex> gate(ix->gate);
-    std::unique_lock<std::shared_mutex> wr(ix->rw);
-    if (ix->comm.joined()) return pb_fail(PB_ERR_UNSUPPORTED, "appends to a doc-sharded handle are not supported");
-    CKS(refuse_fixed_residuals(ix));
-    if (index_dir && ix->doc_id_base != 0) return pb_fail(PB_ERR_UNSUPPORTED, "an index directory holds doc ids from 0");
-    if (index_dir && batch_size <= 0) return pb_fail(PB_ERR_INVALID, "batch_size must be positive");
-    AppendPrep p;
-    CKS(append_prepare(ix, codec, embeddings, codes, residuals, doc_lengths, n_docs, space, index_dir != nullptr,
-                       out_first, p));
-    if (p.n == 0) return PB_OK;
-    // update_index's file changes, before the commit: a failure leaves the handle as it was
-    if (index_dir) {
-        std::vector<int64_t> hivf;
-        std::vector<int32_t> hlen;
-        CKS(ivf_to_host(ix, ix->ivf_spare, ix->ivf_off_spare, p.t.ivf_len, hivf, hlen));
-        CKS(append_dir(ix, p, index_dir, p.D0, batch_size, hivf, p.t.ivf_len, hlen));
-    }
-    publish(ix, p.t);
-    return PB_OK;
+    if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    return pb_members_append({ix}, codec, embeddings, codes, residuals, doc_lengths, n_docs, space, index_dir, batch_size,
+                             out_first);
 }
 
 extern "C" pb_status pb_index_append(pb_index *ix, pb_codec *codec, const float *embeddings, const int64_t *doc_lengths,
@@ -4630,6 +4761,9 @@ extern "C" pb_status pb_index_append(pb_index *ix, pb_codec *codec, const float 
     if (!codec) return pb_fail(PB_ERR_INVALID, "null argument");
     if (ix && ix->dep)
         return pb_dep_append(ix->dep, codec, embeddings, nullptr, nullptr, doc_lengths, n_docs, memory_space, index_dir,
+                             batch_size, out_first_doc_id);
+    if (ix && ix->rep)
+        return pb_rep_append(ix->rep, codec, embeddings, nullptr, nullptr, doc_lengths, n_docs, memory_space, index_dir,
                              batch_size, out_first_doc_id);
     return append_impl(ix, codec, embeddings, nullptr, nullptr, doc_lengths, n_docs, memory_space, index_dir, batch_size,
                        out_first_doc_id);
@@ -4641,11 +4775,15 @@ extern "C" pb_status pb_index_append_encoded(pb_index *ix, const int64_t *codes,
     if (ix && ix->dep)
         return pb_dep_append(ix->dep, nullptr, nullptr, codes, residuals, doc_lengths, n_docs, memory_space, nullptr, 0,
                              out_first_doc_id);
+    if (ix && ix->rep)
+        return pb_rep_append(ix->rep, nullptr, nullptr, codes, residuals, doc_lengths, n_docs, memory_space, nullptr, 0,
+                             out_first_doc_id);
     return append_impl(ix, nullptr, nullptr, codes, residuals, doc_lengths, n_docs, memory_space, nullptr, 0, out_first_doc_id);
 }
 
 extern "C" pb_status pb_index_reserve(pb_index *ix, int64_t num_documents, int64_t num_embeddings) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    if (ix->rep) return pb_rep_reserve(ix->rep, num_documents, num_embeddings);
     CKS(refuse_deployment(ix, "pb_index_reserve (reserve a rank's capacity before it joins a group)"));
     std::lock_guard<std::mutex> gate(ix->gate);
     std::unique_lock<std::shared_mutex> wr(ix->rw);
@@ -4860,23 +4998,161 @@ extern "C" pb_status pb_index_delete(pb_index *ix, const int64_t *doc_ids, int64
     if (!ix || (!doc_ids && n_ids) || n_ids < 0) return pb_fail(PB_ERR_INVALID, "null argument");
     if (out_deleted) *out_deleted = 0;
     if (ix->dep) return pb_dep_delete(ix->dep, doc_ids, n_ids, index_dir, out_deleted);
-    std::lock_guard<std::mutex> gate(ix->gate);
-    std::unique_lock<std::shared_mutex> wr(ix->rw);
-    if (ix->comm.joined()) return pb_fail(PB_ERR_UNSUPPORTED, "deletes from a doc-sharded handle are not supported");
+    if (ix->rep) return pb_rep_delete(ix->rep, doc_ids, n_ids, index_dir, out_deleted);
+    return pb_members_delete({ix}, doc_ids, n_ids, index_dir, out_deleted);
+}
+
+// ------------------------------------------------------------------------------------------
+// replicas (DESIGN §4q): a handle copied onto another device, and appends and deletes applied to several plain handles
+// of the same documents as one
+// ------------------------------------------------------------------------------------------
+// dst: a copy of src's whole allocation (on the current device, which is dst_dev), issued on st
+static pb_status clone_buf(DevBuf &dst, const DevBuf &src, int dst_dev, int src_dev, cudaStream_t st) {
+    if (!src.p) return PB_OK;
+    cudaError_t e = cudaMalloc(&dst.p, src.cap);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        dst.p = nullptr;
+        return pb_fail(PB_ERR_NOMEM, "cudaMalloc(%zu bytes) failed: %s", src.cap, cudaGetErrorString(e));
+    }
+    dst.cap = src.cap, dst.owned = true, dst.zero_on_grow = src.zero_on_grow;
+    CK(cudaMemcpyPeerAsync(dst.p, dst_dev, src.p, src_dev, src.cap, st));
+    return PB_OK;
+}
+
+pb_status pb_index_clone(const pb_index *src, int device, pb_index **out) {
+    *out = nullptr;
+    auto rd = src->read_lock();
+    CKS(check_device(device));
+    std::unique_ptr<pb_index> ix(new pb_index());
+    static_cast<DocTotals &>(*ix) = static_cast<const DocTotals &>(*src);
+    ix->device = device;
+    cudaDeviceProp prop;
+    CK(cudaGetDeviceProperties(&prop, device));
+    ix->sm_count = prop.multiProcessorCount;  // the grids sized from it follow the copy's device
+    ix->dim = src->dim, ix->nbits = src->nbits, ix->packed = src->packed, ix->K = src->K, ix->doc_id_base = src->doc_id_base;
+    ix->host_tier = src->host_tier, ix->build_ivf = src->build_ivf, ix->cmax = src->cmax, ix->cent_exp = src->cent_exp;
+    ix->fast_approx = src->fast_approx, ix->k1_tc = src->k1_tc, ix->k1_margin = src->k1_margin, ix->k1_diag = src->k1_diag;
+    ix->table_diag = src->table_diag, ix->approx_grid = src->approx_grid, ix->a5_prune = src->a5_prune;
+    ix->a5_live = src->a5_live, ix->a5_m1 = src->a5_m1, ix->a5_waves = src->a5_waves, ix->probe16 = src->probe16;
+    ix->fast_exact = src->fast_exact, ix->filter_diag = src->filter_diag, ix->pair_exact = src->pair_exact;
+    ix->ws_grid = src->ws_grid, ix->ws_grid2 = src->ws_grid2, ix->lanes = src->lanes, ix->profiling = src->profiling;
+    ix->st_budget = src->st_budget, ix->delete_window = src->delete_window;
+    if (src->host_tier) CKS(ix->host_res.share(src->host_res));
+    OwnedStream st;
+    CK(cudaStreamCreateWithFlags(&st.s, cudaStreamNonBlocking));
+    const auto mine = DocArrays::buffers(*ix);
+    const auto theirs = DocArrays::buffers(*src);
+    for (size_t i = 0; i < mine.size(); ++i) CKS(clone_buf(*mine[i], *theirs[i], device, src->device, st.s));
+    CKS(clone_buf(ix->centroids, src->centroids, device, src->device, st.s));
+    CKS(clone_buf(ix->w_rev, src->w_rev, device, src->device, st.s));
+    CKS(clone_buf(ix->cent_h16t, src->cent_h16t, device, src->device, st.s));
+    CKS(clone_buf(ix->cent_l16t, src->cent_l16t, device, src->device, st.s));
+    CK(cudaStreamSynchronize(st.s));
+    CKS(coalesce_env_defaults(ix.get()));
+    *out = ix.release();
+    return PB_OK;
+}
+
+// The encoded rows of tokens [t0, t0 + n) of a handle, on the host: codes widened to i64 and packed residual rows
+static pb_status tail_rows(const pb_index *ix, long long t0, long long n, std::vector<int64_t> &codes,
+                           std::vector<uint8_t> &res) {
+    const size_t pk = (size_t)ix->packed;
+    std::vector<uint32_t> c32((size_t)n);
+    res.resize((size_t)n * pk);
+    if (n) {
+        CK(cudaSetDevice(ix->device));
+        CK(cudaMemcpy(c32.data(), ix->codes.as<uint32_t>() + t0, (size_t)n * 4, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(res.data(), ix->residuals.as<uint8_t>() + (size_t)t0 * pk, res.size(), cudaMemcpyDeviceToHost));
+    }
+    codes.assign(c32.begin(), c32.end());
+    return PB_OK;
+}
+
+Replicas *pb_replicas_of(const pb_index *ix) { return ix ? ix->rep : nullptr; }
+pb_index *pb_rank_of(pb_index *ix, int r) { return ix->dep ? pb_dep_rank(ix->dep, r) : ix; }
+
+// Every member's writer lock, in member order
+struct MembersLock {
+    std::vector<std::unique_lock<std::mutex>> gates;
+    std::vector<std::unique_lock<std::shared_mutex>> rws;
+    explicit MembersLock(const std::vector<pb_index *> &ms) {
+        for (pb_index *m : ms) {
+            gates.emplace_back(m->gate);
+            rws.emplace_back(m->rw);
+        }
+    }
+};
+
+pb_status pb_members_append(const std::vector<pb_index *> &ms, pb_codec *codec, const float *embeddings,
+                            const int64_t *codes, const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs,
+                            int32_t space, const char *index_dir, int64_t batch_size, int64_t *out_first) {
+    pb_index *ix = ms[0];
+    // append_impl's checks, in its order
+    if ((!doc_lengths && n_docs) || n_docs < 0) return pb_fail(PB_ERR_INVALID, "null argument");
+    if (space != PB_MEM_HOST && space != PB_MEM_DEVICE) return pb_fail(PB_ERR_INVALID, "bad memory_space %d", space);
+    MembersLock lock(ms);
+    if (ix->comm.joined()) return pb_fail(PB_ERR_UNSUPPORTED, "appends to a doc-sharded handle are not supported");
     CKS(refuse_fixed_residuals(ix));
     if (index_dir && ix->doc_id_base != 0) return pb_fail(PB_ERR_UNSUPPORTED, "an index directory holds doc ids from 0");
-    DeletePrep p;
-    CKS(delete_prepare(ix, doc_ids, n_ids, p));
-    if (p.n_del == 0) return PB_OK;
-    // delete_from_index's file changes, before the first in-place write: a failure leaves the handle as it was
+    if (index_dir && batch_size <= 0) return pb_fail(PB_ERR_INVALID, "batch_size must be positive");
+    std::vector<std::unique_ptr<AppendPrep>> p;
+    for (size_t g = 0; g < ms.size(); ++g) p.emplace_back(new AppendPrep());
+    // 1. prepare: member 0 as one handle would (with a codec, the only encode); the others from its encoded rows
+    CKS(append_prepare(ix, codec, embeddings, codes, residuals, doc_lengths, n_docs, space, index_dir != nullptr,
+                       out_first, *p[0]));
+    if (p[0]->n == 0) return PB_OK;
+    if (ms.size() > 1) {
+        const AppendPrep &a = *p[0];
+        std::vector<int64_t> hc;
+        std::vector<uint8_t> hr;
+        CKS(tail_rows(ix, a.t.N - a.ntok, a.ntok, hc, hr));
+        for (size_t g = 1; g < ms.size(); ++g)
+            CKS(append_prepare(ms[g], nullptr, nullptr, hc.data(), hr.data(), a.dl.data(), n_docs, PB_MEM_HOST, false,
+                               nullptr, *p[g]));
+    }
+    // 2. the directory, once, before any commit: a failure leaves every member as it was
     if (index_dir) {
         std::vector<int64_t> hivf;
         std::vector<int32_t> hlen;
-        CKS(ivf_to_host(ix, ix->ivf_spare, ix->ivf_off_spare, p.t.ivf_len, hivf, hlen));
-        CKS(pb_dir_delete(index_dir, p.D0, ix->K, ix->dim, ix->nbits, p.hbits.data(), hivf.data(), p.t.ivf_len, hlen.data()));
+        CK(cudaSetDevice(ix->device));
+        CKS(ivf_to_host(ix, ix->ivf_spare, ix->ivf_off_spare, p[0]->t.ivf_len, hivf, hlen));
+        CKS(append_dir(ix, *p[0], index_dir, p[0]->D0, batch_size, hivf, p[0]->t.ivf_len, hlen));
     }
-    CKS(delete_commit(ix, p));
-    if (out_deleted) *out_deleted = p.n_del;
+    // 3. commit everywhere
+    for (size_t g = 0; g < ms.size(); ++g) publish(ms[g], p[g]->t);
+    return PB_OK;
+}
+
+pb_status pb_members_delete(const std::vector<pb_index *> &ms, const int64_t *doc_ids, int64_t n_ids, const char *index_dir,
+                            int64_t *out_deleted) {
+    pb_index *ix = ms[0];
+    if (out_deleted) *out_deleted = 0;
+    MembersLock lock(ms);
+    // pb_index_delete's checks, in its order
+    if (ix->comm.joined()) return pb_fail(PB_ERR_UNSUPPORTED, "deletes from a doc-sharded handle are not supported");
+    CKS(refuse_fixed_residuals(ix));
+    if (index_dir && ix->doc_id_base != 0) return pb_fail(PB_ERR_UNSUPPORTED, "an index directory holds doc ids from 0");
+    std::vector<std::unique_ptr<DeletePrep>> p;
+    for (size_t g = 0; g < ms.size(); ++g) {
+        p.emplace_back(new DeletePrep());
+        CKS(delete_prepare(ms[g], doc_ids, n_ids, *p[g]));
+        if (p[0]->n_del == 0) return PB_OK;
+    }
+    if (index_dir) {
+        std::vector<int64_t> hivf;
+        std::vector<int32_t> hlen;
+        CK(cudaSetDevice(ix->device));
+        CKS(ivf_to_host(ix, ix->ivf_spare, ix->ivf_off_spare, p[0]->t.ivf_len, hivf, hlen));
+        CKS(pb_dir_delete(index_dir, p[0]->D0, ix->K, ix->dim, ix->nbits, p[0]->hbits.data(), hivf.data(), p[0]->t.ivf_len,
+                          hlen.data()));
+    }
+    // from here only a CUDA runtime error can fail a member, and that leaves the set to be reloaded
+    for (size_t g = 0; g < ms.size(); ++g) {
+        CK(cudaSetDevice(ms[g]->device));
+        CKS(delete_commit(ms[g], *p[g]));
+    }
+    if (out_deleted) *out_deleted = p[0]->n_del;
     return PB_OK;
 }
 
@@ -4969,24 +5245,151 @@ static pb_status layout_vote(pb_index *ix, long long *rec, const char *args, std
     return PB_OK;
 }
 
+// ------------------------------------------------------------------------------------------
+// The replicas of a set of deployments (S > 1, replicas.cpp, DESIGN §4q) vote on a mutation together, so that it
+// commits on every replica or on none: every rank of every replica takes the same rounds, and a rank that returns
+// early counts, for every later round, with the status it returned.  A round fails with the lowest failing replica's
+// status.  With a codec, replica 0's last rank also hands the rows it encoded to the other replicas, which wait for them
+// before they prepare: the append encodes once.
+// ------------------------------------------------------------------------------------------
+struct RepVote {
+    int ranks = 0;
+    bool with_dir = false, share_rows = false;
+    std::mutex mu;
+    std::condition_variable cv;
+    struct Entry {
+        int round, replica;
+        pb_status st;
+        std::string msg;
+        bool left;
+    };
+    std::vector<Entry> entries;
+    bool rows_ready = false;
+    pb_status rows_st = PB_OK;
+    std::string rows_msg;
+    std::vector<int64_t> dl, codes;
+    std::vector<uint8_t> res;
+    // round k's votes: the ranks that voted in it and the ranks that left before or at it
+    int count(int k) const {
+        int c = 0;
+        for (const Entry &e : entries) c += e.left ? e.round <= k : e.round == k;
+        return c;
+    }
+    const Entry *failure(int k) const {
+        const Entry *f = nullptr;
+        for (const Entry &e : entries)
+            if (e.st != PB_OK && (e.left ? e.round <= k : e.round == k) && (!f || e.replica < f->replica)) f = &e;
+        return f;
+    }
+};
+
+RepVote *pb_rep_vote_new(int ranks, bool with_dir, bool share_rows) {
+    RepVote *v = new RepVote();
+    v->ranks = ranks, v->with_dir = with_dir, v->share_rows = share_rows;
+    return v;
+}
+void pb_rep_vote_free(RepVote *v) { delete v; }
+void pb_index_set_rep_vote(pb_index *member, RepVote *v, int replica) {
+    auto set = [&](pb_index *r) { r->rep_vote = v, r->rep_index = replica; };
+    if (member->dep) pb_dep_each(member->dep, set);
+    else set(member);
+}
+
+// One rank's turns in its replica set's vote (nothing without one)
+struct RepTurn {
+    RepVote *v;
+    int replica, round = 0;
+    explicit RepTurn(const pb_index *ix) : v(ix->rep_vote), replica(ix->rep_index) {}
+    bool with_dir() const { return v && v->with_dir; }
+    // waits for every rank; the round's verdict (a failing rank keeps its own message)
+    pb_status vote(pb_status mine) {
+        if (!v) return mine;
+        const std::string msg = mine == PB_OK ? std::string() : g_err;
+        std::unique_lock<std::mutex> lk(v->mu);
+        const int k = round++;
+        v->entries.push_back({k, replica, mine, msg, false});
+        v->cv.notify_all();
+        v->cv.wait(lk, [&] { return v->count(k) >= v->ranks; });
+        const RepVote::Entry *f = v->failure(k);
+        if (!f) return PB_OK;
+        if (mine != PB_OK) return mine;
+        return pb_fail(f->st, "replica %d failed (%s); nothing changed", f->replica, f->msg.c_str());
+    }
+    // the rank returns with status st: it counts so for the rounds it did not take
+    void leave(pb_status st) {
+        if (!v) return;
+        std::lock_guard<std::mutex> lk(v->mu);
+        v->entries.push_back({round, replica, st, st == PB_OK ? std::string() : g_err, true});
+        if (v->share_rows && replica == 0 && !v->rows_ready && st != PB_OK)  // replica 0 failed before it could share
+            v->rows_ready = true, v->rows_st = st, v->rows_msg = g_err;
+        v->cv.notify_all();
+    }
+    // replica 0's last rank: the rows its prepare encoded (or why it failed), for the other replicas
+    void share(pb_status st, pb_index *ix, const AppendPrep &ap) {
+        std::vector<int64_t> codes;
+        std::vector<uint8_t> res;
+        if (st == PB_OK && ap.n > 0) st = tail_rows(ix, ap.t.N - ap.ntok, ap.ntok, codes, res);
+        std::lock_guard<std::mutex> lk(v->mu);
+        v->rows_st = st, v->rows_msg = st == PB_OK ? std::string() : g_err;
+        v->dl = ap.dl, v->codes = std::move(codes), v->res = std::move(res);
+        v->rows_ready = true;
+        v->cv.notify_all();
+    }
+    // another replica's rank: replica 0's encoded rows, once they are there
+    pb_status rows(const std::vector<int64_t> *&dl, const std::vector<int64_t> *&codes, const std::vector<uint8_t> *&res) {
+        std::unique_lock<std::mutex> lk(v->mu);
+        v->cv.wait(lk, [&] { return v->rows_ready; });
+        if (v->rows_st != PB_OK) return pb_fail(v->rows_st, "replica 0 failed (%s); nothing changed", v->rows_msg.c_str());
+        dl = &v->dl, codes = &v->codes, res = &v->res;
+        return PB_OK;
+    }
+};
+
+static pb_status sharded_update_body(pb_index *ix, RepTurn &turn, int op, pb_codec *codec, const float *embeddings,
+                                     const int64_t *codes, const uint8_t *residuals, const int64_t *doc_lengths,
+                                     const int64_t *doc_ids, int64_t n, int32_t space, const char *index_dir,
+                                     int64_t batch_size, int64_t *out);
+
 static pb_status sharded_update(pb_index *ix, int op, pb_codec *codec, const float *embeddings, const int64_t *codes,
                                 const uint8_t *residuals, const int64_t *doc_lengths, const int64_t *doc_ids, int64_t n,
                                 int32_t space, const char *index_dir, int64_t batch_size, int64_t *out) {
     if (out) *out = 0;
     std::lock_guard<std::mutex> gate(ix->gate);
     std::unique_lock<std::shared_mutex> wr(ix->rw);
+    RepTurn turn(ix);
+    const pb_status s = sharded_update_body(ix, turn, op, codec, embeddings, codes, residuals, doc_lengths, doc_ids, n,
+                                            space, index_dir, batch_size, out);
+    turn.leave(s);
+    return s;
+}
+
+static pb_status sharded_update_body(pb_index *ix, RepTurn &turn, int op, pb_codec *codec, const float *embeddings,
+                                     const int64_t *codes, const uint8_t *residuals, const int64_t *doc_lengths,
+                                     const int64_t *doc_ids, int64_t n, int32_t space, const char *index_dir,
+                                     int64_t batch_size, int64_t *out) {
     const bool last = ix->comm.rank == ix->comm.world - 1;
     DeletePrep dp;
     AppendPrep ap;
     long long rec[LR_WORDS] = {};
+    // a replica other than 0 of an append with a codec: every rank waits for replica 0's encoded rows, so that the
+    // group's exchange below does not time out while replica 0 encodes; the last rank appends them
+    const bool takes_rows = turn.v && turn.v->share_rows && turn.replica > 0;
+    pb_status rows_st = PB_OK;
+    if (takes_rows) {
+        const std::vector<int64_t> *dl = nullptr, *cd = nullptr;
+        const std::vector<uint8_t> *rs = nullptr;
+        rows_st = turn.rows(dl, cd, rs);
+        if (rows_st == PB_OK) codes = cd->data(), residuals = rs->data(), doc_lengths = dl->data(), space = PB_MEM_HOST;
+    }
     // 1. local checks, the fingerprint of the arguments, and the prepare: no early return, or the peers would wait
     auto local = [&]() -> pb_status {
+        CKS(rows_st);
         if (n < 0 || (n && !(op == SH_OP_DELETE ? doc_ids : doc_lengths))) return pb_fail(PB_ERR_INVALID, "null argument");
         if (op != SH_OP_DELETE && space != PB_MEM_HOST && space != PB_MEM_DEVICE)
             return pb_fail(PB_ERR_INVALID, "bad memory_space %d", space);
         CKS(refuse_fixed_residuals(ix));
         if (index_dir && op == SH_OP_APPEND && batch_size <= 0) return pb_fail(PB_ERR_INVALID, "batch_size must be positive");
-        if (op == SH_OP_APPEND && last && !codec) return pb_fail(PB_ERR_INVALID, "null argument");
+        if (op == SH_OP_APPEND && last && !codec && !takes_rows) return pb_fail(PB_ERR_INVALID, "null argument");
         std::vector<int64_t> args;
         if (op == SH_OP_DELETE) args.assign(doc_ids, doc_ids + n);
         else CKS(fetch_host(args, doc_lengths, (size_t)n, space));
@@ -5002,12 +5405,13 @@ static pb_status sharded_update(pb_index *ix, int op, pb_codec *codec, const flo
             CKS(delete_prepare(ix, doc_ids, n, dp));
             rec[LR_OWN] = dp.n_del;
         } else if (last) {
-            CKS(append_prepare(ix, codec, embeddings, codes, residuals, doc_lengths, n, space, index_dir != nullptr,
-                               nullptr, ap));
+            CKS(append_prepare(ix, takes_rows ? nullptr : codec, embeddings, codes, residuals, doc_lengths, n, space,
+                               index_dir != nullptr, nullptr, ap));
         }
         return PB_OK;
     };
     rec[LR_STATUS] = local();
+    if (turn.v && turn.v->share_rows && turn.replica == 0 && last) turn.share((pb_status)rec[LR_STATUS], ix, ap);
 
     // 2. exchange A and the verdict every rank reaches from the same records
     std::vector<long long> all, base, tok;
@@ -5021,6 +5425,9 @@ static pb_status sharded_update(pb_index *ix, int op, pb_codec *codec, const flo
     if (op == SH_OP_DELETE && n_del == 0) return PB_OK;  // nothing changes, on any rank or on disk
     if (op != SH_OP_DELETE && out) *out = D_total;
     if (op != SH_OP_DELETE && n == 0) return PB_OK;
+
+    // the replicas of a set: every replica prepared, or none writes the directory
+    CKS(turn.vote(PB_OK));
 
     // 3. the directory, written by the last rank from ivf.npy as it is on disk; exchange B carries its status
     if (index_dir) {
@@ -5056,6 +5463,8 @@ static pb_status sharded_update(pb_index *ix, int op, pb_codec *codec, const flo
         CKS(gather_words(ix, &wrec, 1, wall, true));
         CKS(first_failure(ix, wall, 1, " writing the index directory; no rank changed"));
     }
+
+    if (turn.with_dir()) CKS(turn.vote(PB_OK));  // replica 0 wrote the directory
 
     // 4. commit everywhere: from here only a CUDA runtime error can fail a rank, and that leaves the group inconsistent
     if (op == SH_OP_DELETE) {
@@ -5118,11 +5527,21 @@ struct RebalancePrep {
     DevBuf rlen, rulen, seg, seg_off, meta, mn;
 };
 
+static pb_status rebalance_body(pb_index *ix, RepTurn &turn, const int64_t *bounds, int64_t *out_bounds);
+
 extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bounds, int64_t *out_bounds) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
     if (ix->dep) return pb_dep_rebalance(ix->dep, bounds, out_bounds);
+    if (ix->rep) return pb_rep_rebalance(ix->rep, bounds, out_bounds);
     std::lock_guard<std::mutex> gate(ix->gate);
     std::unique_lock<std::shared_mutex> wr(ix->rw);
+    RepTurn turn(ix);
+    const pb_status s = rebalance_body(ix, turn, bounds, out_bounds);
+    turn.leave(s);
+    return s;
+}
+
+static pb_status rebalance_body(pb_index *ix, RepTurn &turn, const int64_t *bounds, int64_t *out_bounds) {
     const int W = ix->comm.world, me = ix->comm.rank;
     const long long K = ix->K;
     const size_t pk = (size_t)ix->packed;
@@ -5393,6 +5812,7 @@ extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bou
     // 6. the last vote covers the transfer and the build; then every rank swaps in its new arrays, which cannot fail
     CKS(gather_words(ix, &fin, 1, votes, true));
     CKS(first_failure(ix, votes, 1, " moving the documents; nothing changed"));
+    CKS(turn.vote(PB_OK));  // the replicas of a set: every replica moved its documents, or none commits
     if (changes) {
         publish(ix, nx, &nx);
         ix->doc_id_base = b[me];
@@ -5403,6 +5823,7 @@ extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bou
 
 extern "C" pb_status pb_last_delete_ms(pb_index *ix, float *out_ms) {
     if (!ix || !out_ms) return pb_fail(PB_ERR_INVALID, "null argument");
+    if (ix->rep) return pb_last_delete_ms(pb_rep_member(ix->rep, 0), out_ms);  // the set's last delete ran there too
     CKS(refuse_deployment(ix, "pb_last_delete_ms"));
     auto rd = ix->read_lock();
     memcpy(out_ms, ix->delete_ms, sizeof ix->delete_ms);

@@ -3,11 +3,66 @@
 #pragma once
 #include "../../include/plaid_b200.h"
 
+#include <condition_variable>
 #include <functional>
+#include <memory>
+#include <mutex>
 #include <string>
+#include <thread>
 #include <vector>
 
 pb_status pb_fail(pb_status s, const char *fmt, ...);
+
+using Job = std::function<pb_status(int rank)>;
+
+// A library thread of a deployment's rank or a replica set's slice: waits for a job, runs it, records its status and
+// pb_last_error() text
+struct RankWorker {
+    int rank;
+    std::thread th;
+    std::mutex m;
+    std::condition_variable cv;
+    const Job *job = nullptr;
+    bool done = false, quit = false;
+    pb_status status = PB_OK;
+    std::string error;
+    explicit RankWorker(int r) : rank(r) {
+        th = std::thread([this] {
+            std::unique_lock<std::mutex> lk(m);
+            for (;;) {
+                cv.wait(lk, [this] { return job || quit; });
+                if (quit) return;
+                const Job *j = job;
+                lk.unlock();
+                const pb_status s = (*j)(rank);
+                std::string e = s == PB_OK ? std::string() : std::string(pb_last_error());
+                lk.lock();
+                status = s, error = std::move(e);
+                job = nullptr;
+                done = true;
+                cv.notify_all();
+            }
+        });
+    }
+    void submit(const Job &j) {
+        std::lock_guard<std::mutex> lk(m);
+        job = &j;
+        done = false;
+        cv.notify_all();
+    }
+    void wait() {
+        std::unique_lock<std::mutex> lk(m);
+        cv.wait(lk, [this] { return done; });
+    }
+    ~RankWorker() {
+        {
+            std::lock_guard<std::mutex> lk(m);
+            quit = true;
+            cv.notify_all();
+        }
+        if (th.joinable()) th.join();
+    }
+};
 
 // A deployment (pb_index_load_devices, deployment.cpp, DESIGN §4o): the ranks of a doc-sharded index in one process,
 // driven through the public entry points by the library's own threads.  Its handle is a pb_index that holds no
@@ -39,6 +94,56 @@ pb_status pb_dep_append(Deployment *d, pb_codec *codec, const float *embeddings,
                         const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
                         const char *index_dir, int64_t batch_size, int64_t *out_first_doc_id);
 pb_status pb_dep_rebalance(Deployment *d, const int64_t *bounds, int64_t *out_bounds);
+// A deployment of ranks already loaded (ranks[r] on devices[r], not yet in a group): joins them in a new group and
+// returns its handle.  On failure the ranks are closed.
+pb_status pb_dep_assemble(std::vector<pb_index *> ranks, const std::vector<int> &devices, pb_index **out);
+
+// A replica set (pb_index_load_replicas, replicas.cpp, DESIGN §4q): R full copies of an index, each a plain handle or a
+// deployment, behind one pb_index that holds no documents; the entry points of engine.cu hand such a handle to the
+// functions below.
+struct Replicas;
+pb_index *pb_index_new_replicas(Replicas *rs, const pb_index *member0);
+pb_index *pb_rep_member(Replicas *rs, int g);
+int pb_rep_count(const Replicas *rs);
+void pb_rep_close(Replicas *rs);
+void pb_rep_each(Replicas *rs, const std::function<void(pb_index *)> &call);
+// A routed search of n queries: cut into contiguous slices [b0, b1), each run by call(member, b0, b1, slice) on one of
+// the least-loaded replicas, slice 0 on the caller's thread.  Returns the lowest failing slice's status.
+pb_status pb_rep_search(Replicas *rs, int64_t n_queries,
+                        const std::function<pb_status(pb_index *, int64_t, int64_t, int)> &call);
+// call(member) on the least-loaded replica for a whole request of n queries (a merged batch, a reader)
+pb_status pb_rep_whole(Replicas *rs, int64_t n_queries, const std::function<pb_status(pb_index *)> &call);
+pb_status pb_rep_memory(Replicas *rs, int64_t *device_bytes, int64_t *host_bytes);
+// the mutations, under the set's writer lock
+pb_status pb_rep_delete(Replicas *rs, const int64_t *doc_ids, int64_t n_ids, const char *index_dir, int64_t *out_deleted);
+pb_status pb_rep_append(Replicas *rs, pb_codec *codec, const float *embeddings, const int64_t *codes,
+                        const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
+                        const char *index_dir, int64_t batch_size, int64_t *out_first_doc_id);
+pb_status pb_rep_reserve(Replicas *rs, int64_t num_documents, int64_t num_embeddings);
+pb_status pb_rep_rebalance(Replicas *rs, const int64_t *bounds, int64_t *out_bounds);
+
+// A copy of a plain handle (or one rank of a deployment, outside its group) on `device`: every array, derived ones
+// included, copied device to device; a host-tier handle shares src's pinned residuals.  The copy's device-dependent
+// scalars are its own.
+pb_status pb_index_clone(const pb_index *src, int device, pb_index **out);
+// Appends and deletes on plain handles that hold the same documents, as one: every member prepares, the directory is
+// written once, then every member commits.  An append with a codec encodes on members[0] only; the others take its
+// encoded rows.
+pb_status pb_members_append(const std::vector<pb_index *> &members, pb_codec *codec, const float *embeddings,
+                            const int64_t *codes, const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs,
+                            int32_t space, const char *index_dir, int64_t batch_size, int64_t *out_first);
+pb_status pb_members_delete(const std::vector<pb_index *> &members, const int64_t *doc_ids, int64_t n_ids,
+                            const char *index_dir, int64_t *out_deleted);
+// The vote a set's replicas take together on a mutation, so that it commits on every replica or on none (engine.cu):
+// for `ranks` ranks in all; with_dir: replica 0 writes the directory; share_rows: an append with a codec, which replica
+// 0 encodes for every replica.  Set on every rank of replica g's handle for the mutation (null clears it).
+struct RepVote;
+RepVote *pb_rep_vote_new(int ranks, bool with_dir, bool share_rows);
+void pb_rep_vote_free(RepVote *v);
+void pb_index_set_rep_vote(pb_index *member, RepVote *v, int replica);
+// the set behind a handle (null for any other handle); rank r of a deployment's handle (the handle itself otherwise)
+Replicas *pb_replicas_of(const pb_index *ix);
+pb_index *pb_rank_of(pb_index *ix, int r);
 // pb_index_open without the per-token arrays; follow with pb_index_upload_tokens per chunk.
 pb_status pb_index_open_begin(const pb_index_desc *d, pb_index **out);
 pb_status pb_index_upload_tokens(pb_index *ix, long long tok_off, const int64_t *codes, const uint8_t *residuals,

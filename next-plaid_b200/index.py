@@ -101,6 +101,7 @@ EXPORTS = [
     "pb_index_rebalance_sharded", "pb_index_load_range_flags", "pb_index_memory", "pb_last_staging_stats",
     "pb_search", "pb_index_set_coalescing", "pb_index_coalesce_stats", "pb_create_index_sharded", "pb_last_create_ms",
     "pb_index_load_devices", "pb_index_shard_layout", "pb_pooled_doc_length", "pb_pool_embeddings", "pb_last_pool_ms",
+    "pb_index_load_replicas", "pb_index_replica_layout", "pb_index_replica_stats",
 ]
 
 PB_OPEN_ADOPT_RESIDUALS, PB_OPEN_HOST_RESIDUALS = 1, 2
@@ -217,6 +218,10 @@ def load_library():
         L.pb_index_rebalance_sharded.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         L.pb_index_load_devices.argtypes = [C.c_char_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
         L.pb_index_shard_layout.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.pb_index_load_replicas.argtypes = [C.c_char_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                             C.POINTER(C.c_void_p)]
+        L.pb_index_replica_layout.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.pb_index_replica_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]
         L.pb_pooled_doc_length.argtypes = [C.c_int64, C.c_int64]
         L.pb_pooled_doc_length.restype = C.c_int64
         L.pb_pool_embeddings.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_int32,
@@ -495,6 +500,37 @@ class MmapIndex:
         b, d = np.zeros(w.value + 1, np.int64), np.zeros(w.value, np.int32)
         _check(load_library().pb_index_shard_layout(self._h, C.byref(w), _ptr(b), _ptr(d)))
         return b, d
+
+    @classmethod
+    def load_replicas(cls, index_path: str, devices: Sequence[int], shards: int = 1,
+                      host_residuals: bool = False) -> "MmapIndex":
+        """pb_index_load_replicas: len(devices) / shards full copies of the directory behind one handle, replica g on
+        devices[g * shards : (g + 1) * shards] (a plain handle when shards == 1, else a doc-sharded deployment; devices
+        may repeat).  Searches are spread over the replicas, mutations applied to all of them at once; every method
+        works as on a handle from load (shards == 1) or load_devices, with the same results."""
+        dv = np.ascontiguousarray(list(devices), np.int32)
+        h = C.c_void_p()
+        _check(load_library().pb_index_load_replicas(os.fsencode(index_path), _ptr(dv), len(dv), shards,
+                                                     PB_OPEN_HOST_RESIDUALS if host_residuals else 0, C.byref(h)))
+        ix = cls(h.value, index_path)
+        ix._world = shards
+        return ix
+
+    def replica_layout(self):
+        """pb_index_replica_layout: (replicas, shards, devices [replicas, shards]); any other handle is one replica."""
+        r, s = C.c_int32(), C.c_int32()
+        _check(load_library().pb_index_replica_layout(self._h, C.byref(r), C.byref(s), None))
+        d = np.zeros(r.value * s.value, np.int32)
+        _check(load_library().pb_index_replica_layout(self._h, C.byref(r), C.byref(s), _ptr(d)))
+        return r.value, s.value, d.reshape(r.value, s.value)
+
+    def replica_stats(self, reset: bool = False):
+        """pb_index_replica_stats: per replica since load or the last reset, (calls or slices served, queries)."""
+        r, s = C.c_int32(), C.c_int32()
+        _check(load_library().pb_index_replica_layout(self._h, C.byref(r), C.byref(s), None))
+        calls, queries = np.zeros(r.value, np.int64), np.zeros(r.value, np.int64)
+        _check(load_library().pb_index_replica_stats(self._h, _ptr(calls), _ptr(queries), int(reset)))
+        return calls, queries
 
     @classmethod
     def load_shard(cls, index_path: str, rank: int, world: int, device: int = 0,

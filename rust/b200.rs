@@ -136,6 +136,8 @@ extern "C" {
                                  out: *mut *mut c_void) -> c_int;
     fn pb_index_load_devices(index_dir: *const c_char, devices: *const i32, n_devices: i32, flags: i32,
                              out: *mut *mut c_void) -> c_int;
+    fn pb_index_load_replicas(index_dir: *const c_char, devices: *const i32, n_devices: i32, n_shards: i32, flags: i32,
+                              out: *mut *mut c_void) -> c_int;
     fn pb_index_memory(ix: *const c_void, device_bytes: *mut i64, host_bytes: *mut i64) -> c_int;
     fn pb_last_staging_stats(ix: *mut c_void, docs: *mut i64, bytes: *mut i64, ms: *mut f32) -> c_int;
     // pb_create_index_sharded (DESIGN §4n): `comm` is a pb_build_comm, `params` a pb_create_params
@@ -195,6 +197,22 @@ impl B200Index {
         let c = CString::new(index_path).map_err(|e| Error::IndexLoad(e.to_string()))?;
         let mut handle: *mut c_void = std::ptr::null_mut();
         let st = unsafe { pb_index_load_devices(c.as_ptr(), devices.as_ptr(), devices.len() as i32, 0, &mut handle) };
+        if st != 0 {
+            return Err(Error::IndexLoad(last_error()));
+        }
+        Ok(B200Index { handle })
+    }
+
+    /// `devices.len() / shards` full copies of the index behind one handle (`pb_index_load_replicas`, DESIGN §4q):
+    /// replica g on `devices[g * shards .. (g + 1) * shards]`, a `load` handle when `shards == 1`, else a `load_devices`
+    /// deployment.  Searches are spread over the replicas, `update_append` and `delete_with_options` reach all of them
+    /// at once (encoded once, the directory written once); results equal those of `load` / `load_devices`.
+    pub fn load_replicas(index_path: &str, devices: &[i32], shards: i32) -> Result<Self> {
+        let c = CString::new(index_path).map_err(|e| Error::IndexLoad(e.to_string()))?;
+        let mut handle: *mut c_void = std::ptr::null_mut();
+        let st = unsafe {
+            pb_index_load_replicas(c.as_ptr(), devices.as_ptr(), devices.len() as i32, shards, 0, &mut handle)
+        };
         if st != 0 {
             return Err(Error::IndexLoad(last_error()));
         }
