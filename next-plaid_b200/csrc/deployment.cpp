@@ -38,28 +38,13 @@ struct Deployment {
 
     int world() const { return (int)ranks.size(); }
 
-    // job(r) for every rank at once; the status of each, and the pb_last_error() text of each failure
-    void run(const Job &job, std::vector<pb_status> &st, std::vector<std::string> &err) {
-        const int W = world();
-        st.assign((size_t)W, PB_OK);
-        err.assign((size_t)W, std::string());
-        for (int r = 1; r < W; ++r) workers[r]->submit(job);
-        st[0] = job(0);
-        if (st[0] != PB_OK) err[0] = pb_last_error();
-        for (int r = 1; r < W; ++r) {
-            workers[r]->wait();
-            st[r] = workers[r]->status;
-            err[r] = workers[r]->error;
-        }
-    }
-
-    // run() whose result is one status: the lowest failing rank's, where with skip_comm a rank reporting PB_ERR_COMM
-    // (a peer's failure seen through the group) gives way to a rank with a failure of its own.  That rank's message
-    // becomes the caller's.
+    // job(r) for every rank at once, whose result is one status: the lowest failing rank's, where with skip_comm a rank
+    // reporting PB_ERR_COMM (a peer's failure seen through the group) gives way to a rank with a failure of its own.
+    // That rank's message becomes the caller's.
     pb_status run_one(const Job &job, bool skip_comm = true) {
         std::vector<pb_status> st;
         std::vector<std::string> err;
-        run(job, st, err);
+        run_slots(world(), job, workers.data() + 1, st, err);
         int pick = -1;
         for (int r = 0; r < world() && pick < 0; ++r)
             if (st[r] != PB_OK && !(skip_comm && st[r] == PB_ERR_COMM)) pick = r;

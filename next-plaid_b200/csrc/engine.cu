@@ -516,51 +516,6 @@ struct Stats {
 static thread_local Stats g_stats;
 static thread_local int g_budget_div = 1;  // lanes of the current call share the workspace budget
 
-// One helper thread of a laned search call (search_impl): runs the pipeline of a slice of the batch on its own workspace
-// and stream while the caller runs another slice, so that one slice's latency-bound kernels overlap the other's
-// bandwidth-bound ones.
-struct LaneWorker {
-    std::thread th;
-    std::mutex m;
-    std::condition_variable cv;
-    std::function<void()> job;
-    bool has_job = false, done = false, quit = false;
-    LaneWorker() {
-        th = std::thread([this] {
-            std::unique_lock<std::mutex> lk(m);
-            for (;;) {
-                cv.wait(lk, [this] { return has_job || quit; });
-                if (quit) return;
-                lk.unlock();
-                job();
-                lk.lock();
-                has_job = false;
-                done = true;
-                cv.notify_all();
-            }
-        });
-    }
-    void submit(std::function<void()> f) {
-        std::lock_guard<std::mutex> lk(m);
-        job = std::move(f);
-        has_job = true;
-        done = false;
-        cv.notify_all();
-    }
-    void wait() {
-        std::unique_lock<std::mutex> lk(m);
-        cv.wait(lk, [this] { return done; });
-    }
-    ~LaneWorker() {
-        {
-            std::lock_guard<std::mutex> lk(m);
-            quit = true;
-            cv.notify_all();
-        }
-        if (th.joinable()) th.join();
-    }
-};
-
 // pb_search's request queue (coalesce.h, DESIGN.md 4m) runs a merged batch through this: run_coalesced, below the
 // search entry points
 struct CoalescedRun {
@@ -628,7 +583,7 @@ struct pb_index : DocArrays {
     int ws_grid2 = 8;          // the same for its pass 2 over the filter's survivors (PB_WS_GRID2; 1: 0.54, 2: 0.43, 4 and 8: 0.40 ms)
     int lanes = 1;             // slices of a batch searched concurrently, each on its own stream (pb_set_lanes / PB_LANES; 1 = off)
     std::mutex lane_mu;        // one laned call at a time per handle (a second concurrent caller runs un-laned)
-    std::vector<std::unique_ptr<LaneWorker>> lane_workers;
+    std::vector<std::unique_ptr<RankWorker>> lane_workers;  // lane_workers[l - 1] runs lane l
     bool profiling = false;
     size_t st_budget = (size_t)8 << 30;  // workspace budget of one search call (PB_WS_BUDGET_MB)
     std::mutex mu;
@@ -1901,6 +1856,21 @@ struct SearchIO {
 };
 
 static const pb_search_params &query_params(const SearchIO &io, int64_t b) { return io.qp[b * io.qp_stride]; }
+
+// Queries [b0, b1) of a call, as lanes and replica slices search them: the offsets stay absolute into the call's
+// queries and subset ids, and the output rows stay io.out_stride apart (a search writes each row's own top_k entries)
+static SearchIO slice_io(const SearchIO &io, int64_t b0, int64_t b1) {
+    SearchIO s = io;
+    s.n_queries = b1 - b0;
+    if (io.q_off) s.q_off = io.q_off + b0;
+    if (io.sub_off) s.sub_off = io.sub_off + b0;
+    if (io.has_sub) s.has_sub = io.has_sub + b0;
+    if (io.qp) s.qp = io.qp + b0 * io.qp_stride;
+    if (io.out_ids) s.out_ids = io.out_ids + b0 * io.out_stride;
+    if (io.out_scores) s.out_scores = io.out_scores + b0 * io.out_stride;
+    if (io.out_counts) s.out_counts = io.out_counts + b0;
+    return s;
+}
 
 // query b's id list [*s, *e) of io.sub_ids, or false when it has no subset
 static bool query_subset(const SearchIO &io, int64_t b, int64_t *s, int64_t *e) {
@@ -3183,6 +3153,16 @@ static void merge_stats(Stats &a, const Stats &b) {
         dst[i] = (i == kdiff || i == kratio) ? std::max(dst[i], src[i]) : dst[i] + src[i];
 }
 
+// the stats of a call cut into the slices s[0 .. n) (lanes, replica slices): merged, with the longest slice's call time
+static Stats merge_slices(const Stats *s, size_t n) {
+    Stats total = s[0];
+    for (size_t i = 1; i < n; ++i) {
+        merge_stats(total, s[i]);
+        total.call_ms = std::max(total.call_ms, s[i].call_ms);
+    }
+    return total;
+}
+
 // events of the calling thread around a laned call (the lanes' own call events live on different streams)
 struct LaneClock {
     cudaStream_t stream = nullptr;
@@ -3214,7 +3194,8 @@ static pb_status search_impl(pb_index *ix, const SearchIO &io) {
         if (st != PB_OK && ix && !g_search_agreed) ix->comm.fail();
         return st;
     }
-    while ((int)ix->lane_workers.size() < lanes - 1) ix->lane_workers.emplace_back(new LaneWorker());
+    while ((int)ix->lane_workers.size() < lanes - 1)
+        ix->lane_workers.emplace_back(new RankWorker((int)ix->lane_workers.size() + 1));
     const bool prof = ix->profiling;
     LaneClock &clk = g_lane_clock;
     if (prof) {
@@ -3227,36 +3208,18 @@ static pb_status search_impl(pb_index *ix, const SearchIO &io) {
         }
         CK(cudaEventRecord(clk.ev[0], clk.stream));
     }
-    std::vector<SearchIO> ios(lanes, io);
-    std::vector<pb_status> sts(lanes, PB_OK);
     std::vector<Stats> stats(lanes);
-    std::vector<std::string> errs(lanes);
-    const int64_t Bt = io.n_queries, top_k = io.out_stride;
-    for (int l = 0; l < lanes; ++l) {
-        const int64_t b0 = Bt * l / lanes, b1 = Bt * (l + 1) / lanes;
-        ios[l].q_off = io.q_off + b0;
-        if (io.sub_off) ios[l].sub_off = io.sub_off + b0;  // the offsets stay absolute into sub_ids
-        if (io.has_sub) ios[l].has_sub = io.has_sub + b0;
-        ios[l].n_queries = b1 - b0;
-        ios[l].qp = io.qp + b0 * io.qp_stride;
-        if (io.out_ids) ios[l].out_ids = io.out_ids + b0 * top_k;
-        if (io.out_scores) ios[l].out_scores = io.out_scores + b0 * top_k;
-        ios[l].out_counts = io.out_counts ? io.out_counts + b0 : nullptr;
-    }
-    auto run_lane = [&](int l) {
+    std::vector<pb_status> sts;
+    std::vector<std::string> errs;
+    const int64_t Bt = io.n_queries;
+    run_slots(lanes, [&](int l) {
         g_budget_div = lanes;
-        sts[l] = run_search(ix, ios[l]);
+        const pb_status st = run_search(ix, slice_io(io, Bt * l / lanes, Bt * (l + 1) / lanes));
         g_budget_div = 1;
         stats[l] = g_stats;
-        if (sts[l] != PB_OK) errs[l] = g_err;
-    };
-    for (int l = 1; l < lanes; ++l) ix->lane_workers[l - 1]->submit([&, l] { run_lane(l); });
-    run_lane(0);
-    for (int l = 1; l < lanes; ++l) ix->lane_workers[l - 1]->wait();
-    Stats total = stats[0];
-    for (int l = 1; l < lanes; ++l) merge_stats(total, stats[l]);
-    total.call_ms = 0.f;
-    for (int l = 0; l < lanes; ++l) total.call_ms = std::max(total.call_ms, stats[l].call_ms);
+        return st;
+    }, ix->lane_workers.data(), sts, errs);
+    Stats total = merge_slices(stats.data(), lanes);
     if (prof) {
         CK(cudaEventRecord(clk.ev[1], clk.stream));
         CK(cudaEventSynchronize(clk.ev[1]));
@@ -3271,84 +3234,62 @@ static pb_status search_impl(pb_index *ix, const SearchIO &io) {
     return PB_OK;
 }
 
-// A replica set's search (replicas.cpp): contiguous slices of the batch, each on one of the least-loaded replicas.
-// run(m, b0, b1) searches queries [b0, b1) on member m into the caller's rows; (0, n) passes the caller's arguments as
-// they are.  A call that the host checks of a plain handle refuse (null or non-monotone offsets, a query's parameters)
-// is not cut: it runs whole on one replica, so it is refused there, once, with the plain handle's status, message and
-// outputs.  A cut call that a slice still refuses on the device runs again whole on one replica, for the plain
-// handle's status and message.  The caller's stats are every slice's, merged as the lanes' are.
-static pb_status replica_search(pb_index *ix, const float *queries, const int64_t *q_off, int64_t n_queries,
-                                const int64_t *sub_off, const pb_search_params *params, int64_t params_stride,
-                                const std::function<pb_status(pb_index *, int64_t, int64_t)> &run) {
-    auto whole = [&] { return pb_rep_whole(ix->rep, n_queries, [&](pb_index *m) { return run(m, 0, n_queries); }); };
-    bool cut = n_queries > 1 && queries && q_off && params && (!sub_off || sub_off[0] == 0);
-    for (int64_t b = 0; cut && b < n_queries; ++b) {
-        cut = q_off[b + 1] >= q_off[b] && (!sub_off || sub_off[b + 1] >= sub_off[b]);
-        int M = 0;
-        const pb_search_params &p = params[b * params_stride];
-        cut = cut && check_query_args(p) == PB_OK && query_kept_docs(p, &M) == PB_OK;
-    }
-    if (!cut) return whole();
-    std::vector<Stats> stats((size_t)pb_rep_count(ix->rep));
-    std::vector<char> ran(stats.size(), 0);
-    const pb_status st = pb_rep_search(ix->rep, n_queries, [&](pb_index *m, int64_t b0, int64_t b1, int k) {
-        const pb_status r = run(m, b0, b1);
-        stats[k] = g_stats, ran[k] = 1;
-        return r;
-    });
-    if (st != PB_OK) return whole();
-    Stats total = stats[0];
-    for (size_t k = 1; k < stats.size(); ++k)
-        if (ran[k]) {
-            merge_stats(total, stats[k]);
-            total.call_ms = std::max(total.call_ms, stats[k].call_ms);
+// One batch search on any handle; each batch entry point builds its SearchIO and calls this.  `traced` names the call
+// in a deployment's refusal of a trace.
+// - A replica set (replicas.cpp) cuts the call into contiguous slices, each searched as slice_io on one of the
+//   least-loaded replicas.  A call that the host checks of a plain handle refuse (null or non-monotone offsets, a
+//   query's parameters) is not cut: it runs whole on one replica, so it is refused there, once, with the plain handle's
+//   status, message and outputs.  A cut call that a slice still refuses on the device runs again whole on one
+//   replica, for the plain handle's status and message.  A trace follows one call through the pipeline: never cut.
+// - A deployment runs the call on every rank, rank 0 into the caller's outputs.
+// - A plain handle searches it.
+static pb_status search_io(pb_index *ix, const SearchIO &io, const char *traced) {
+    if (ix && ix->rep) {
+        auto whole = [&] {
+            return pb_rep_whole(ix->rep, io.n_queries, [&](pb_index *m) { return search_io(m, io, traced); });
+        };
+        bool cut = !io.trace && io.n_queries > 1 && io.queries && io.q_off && io.qp;
+        for (int64_t b = 0; cut && b < io.n_queries; ++b) {
+            int M = 0;
+            const pb_search_params &p = query_params(io, b);
+            cut = io.q_off[b + 1] >= io.q_off[b] && (!io.sub_off || io.sub_off[b + 1] >= io.sub_off[b]) &&
+                  check_query_args(p) == PB_OK && query_kept_docs(p, &M) == PB_OK;
         }
-    g_stats = total;
-    return PB_OK;
-}
-
-// q_tok_offsets [b0, b1] of a slice, from 0
-static std::vector<int64_t> slice_offsets(const int64_t *off, int64_t b0, int64_t b1) {
-    std::vector<int64_t> o((size_t)(b1 - b0 + 1));
-    for (int64_t i = b0; i <= b1; ++i) o[(size_t)(i - b0)] = off[i] - off[b0];
-    return o;
+        if (!cut) return whole();
+        std::vector<Stats> stats((size_t)pb_rep_count(ix->rep));
+        size_t slices = 0;
+        const pb_status st = pb_rep_search(ix->rep, io.n_queries, [&](pb_index *m, int64_t b0, int64_t b1, int k) {
+            const pb_status r = search_io(m, slice_io(io, b0, b1), traced);
+            stats[k] = g_stats;
+            if (b1 == io.n_queries) slices = k + 1;  // the last slice ends the call
+            return r;
+        });
+        if (st != PB_OK) return whole();
+        g_stats = merge_slices(stats.data(), slices);
+        return PB_OK;
+    }
+    if (ix && ix->dep) {
+        if (io.trace) CKS(refuse_deployment(ix, traced));
+        return pb_dep_search(ix->dep, io.n_queries, io.out_stride, io.out_ids, io.out_scores, io.out_counts,
+                             [&](pb_index *m, int64_t *ids, float *sc, int32_t *cn) {
+                                 SearchIO rank = io;
+                                 rank.out_ids = ids, rank.out_scores = sc, rank.out_counts = cn;
+                                 return search_io(m, rank, traced);
+                             });
+    }
+    // before search_impl: a refusal there leaves a deployment's group broken
+    if (io.shared_sub && io.n_shared < 0) return pb_fail(PB_ERR_INVALID, "n_subset < 0");
+    return search_impl(ix, io);
 }
 
 extern "C" pb_status pb_search_batch_traced(pb_index *ix, const float *queries, const int64_t *q_tok_offsets,
                                             int64_t n_queries, const pb_search_params *params, const int64_t *subset,
                                             int64_t n_subset, int64_t *out_ids, float *out_scores, int32_t *out_counts,
                                             pb_trace *trace) {
-    if (ix && ix->rep) {
-        if (trace || !params)  // a trace follows one call through the pipeline: never cut
-            return pb_rep_whole(ix->rep, n_queries, [&](pb_index *m) {
-                return pb_search_batch_traced(m, queries, q_tok_offsets, n_queries, params, subset, n_subset, out_ids,
-                                              out_scores, out_counts, trace);
-            });
-        const int64_t k = std::max<int64_t>(params->top_k, 0);
-        return replica_search(ix, queries, q_tok_offsets, n_queries, nullptr, params, 0,
-                              [&](pb_index *m, int64_t b0, int64_t b1) {
-            if (b0 == 0 && b1 == n_queries)
-                return pb_search_batch_traced(m, queries, q_tok_offsets, n_queries, params, subset, n_subset, out_ids,
-                                              out_scores, out_counts, nullptr);
-            const std::vector<int64_t> qo = slice_offsets(q_tok_offsets, b0, b1);
-            return pb_search_batch_traced(m, queries + q_tok_offsets[b0] * ix->dim, qo.data(), b1 - b0, params, subset,
-                                          n_subset, out_ids ? out_ids + b0 * k : nullptr,
-                                          out_scores ? out_scores + b0 * k : nullptr,
-                                          out_counts ? out_counts + b0 : nullptr, nullptr);
-        });
-    }
-    if (trace) CKS(refuse_deployment(ix, "pb_search_batch_traced with a trace"));
-    if (ix && ix->dep)
-        return pb_dep_search(ix->dep, n_queries, params ? params->top_k : 0, out_ids, out_scores, out_counts,
-                             [&](pb_index *m, int64_t *ids, float *sc, int32_t *cn) {
-                                 return pb_search_batch_traced(m, queries, q_tok_offsets, n_queries, params, subset,
-                                                               n_subset, ids, sc, cn, nullptr);
-                             });
-    if (subset && n_subset < 0) return pb_fail(PB_ERR_INVALID, "n_subset < 0");
     SearchIO io{queries, false, q_tok_offsets, n_queries, subset, nullptr, nullptr, subset ? n_subset : 0,
                 subset != nullptr, out_ids, out_scores, out_counts, false, trace,
                 params, 0, params ? params->top_k : 0};
-    return search_impl(ix, io);
+    return search_io(ix, io, "pb_search_batch_traced with a trace");
 }
 
 // pb_search_batch_subsets and pb_search_batch_params: params[b * params_stride] are query b's parameters
@@ -3356,7 +3297,7 @@ static pb_status search_subsets(pb_index *ix, const float *queries, const int64_
                                 const pb_search_params *params, int64_t params_stride, const int64_t *subset_offsets,
                                 const int64_t *subset_ids, const uint8_t *has_subset, int64_t *out_ids,
                                 float *out_scores, int32_t *out_counts, pb_trace *trace) {
-    // the subset arguments, checked whole before any lane takes its slice
+    // the subset arguments, checked whole before any slice is taken
     if (n_queries < 0) return pb_fail(PB_ERR_INVALID, "n_queries < 0");
     if (subset_offsets) {
         if (subset_offsets[0] != 0) return pb_fail(PB_ERR_INVALID, "subset_offsets[0] must be 0");
@@ -3369,51 +3310,9 @@ static pb_status search_subsets(pb_index *ix, const float *queries, const int64_
     if (params)
         for (int64_t b = 0; b < (params_stride ? n_queries : 1); ++b)
             out_stride = std::max<int64_t>(out_stride, params[b * params_stride].top_k);
-    if (ix && ix->rep && trace)
-        return pb_rep_whole(ix->rep, n_queries, [&](pb_index *m) {
-            return search_subsets(m, queries, q_tok_offsets, n_queries, params, params_stride, subset_offsets,
-                                  subset_ids, has_subset, out_ids, out_scores, out_counts, trace);
-        });
-    if (ix && ix->rep)
-        return replica_search(ix, queries, q_tok_offsets, n_queries, subset_offsets, params, params_stride,
-                              [&](pb_index *m, int64_t b0, int64_t b1) {
-            if (b0 == 0 && b1 == n_queries)
-                return search_subsets(m, queries, q_tok_offsets, n_queries, params, params_stride, subset_offsets,
-                                      subset_ids, has_subset, out_ids, out_scores, out_counts, nullptr);
-            const std::vector<int64_t> qo = slice_offsets(q_tok_offsets, b0, b1);
-            std::vector<int64_t> so;
-            if (subset_offsets) so = slice_offsets(subset_offsets, b0, b1);
-            const pb_search_params *pp = params + b0 * params_stride;
-            int64_t stride = 0;  // the slice's largest top_k: its rows are that far apart
-            for (int64_t b = 0; b < (params_stride ? b1 - b0 : 1); ++b) stride = std::max<int64_t>(stride, pp[b * params_stride].top_k);
-            const bool direct = stride == out_stride;
-            std::vector<int64_t> ids(direct || !out_ids ? 0 : (size_t)(b1 - b0) * stride);
-            std::vector<float> sc(direct || !out_scores ? 0 : (size_t)(b1 - b0) * stride);
-            const pb_status st = search_subsets(
-                m, queries + q_tok_offsets[b0] * ix->dim, qo.data(), b1 - b0, pp, params_stride,
-                subset_offsets ? so.data() : nullptr, subset_ids && subset_offsets ? subset_ids + subset_offsets[b0] : subset_ids,
-                has_subset ? has_subset + b0 : nullptr, !out_ids ? nullptr : direct ? out_ids + b0 * out_stride : ids.data(),
-                !out_scores ? nullptr : direct ? out_scores + b0 * out_stride : sc.data(),
-                out_counts ? out_counts + b0 : nullptr, nullptr);
-            if (st != PB_OK || direct) return st;
-            for (int64_t b = 0; b < b1 - b0; ++b) {  // each row's own top_k entries, as the search writes them
-                const size_t kq = (size_t)std::max<int64_t>(pp[b * params_stride].top_k, 0);
-                if (out_ids) std::copy_n(ids.data() + b * stride, kq, out_ids + (b0 + b) * out_stride);
-                if (out_scores) std::copy_n(sc.data() + b * stride, kq, out_scores + (b0 + b) * out_stride);
-            }
-            return st;
-        });
-    if (ix && ix->dep) {
-        if (trace) CKS(refuse_deployment(ix, "a search with a trace"));
-        return pb_dep_search(ix->dep, n_queries, out_stride, out_ids, out_scores, out_counts,
-                             [&](pb_index *m, int64_t *ids, float *sc, int32_t *cn) {
-                                 return search_subsets(m, queries, q_tok_offsets, n_queries, params, params_stride,
-                                                       subset_offsets, subset_ids, has_subset, ids, sc, cn, nullptr);
-                             });
-    }
     SearchIO io{queries, false, q_tok_offsets, n_queries, subset_ids, subset_offsets, has_subset, 0, false,
                 out_ids, out_scores, out_counts, false, trace, params, params_stride, out_stride};
-    return search_impl(ix, io);
+    return search_io(ix, io, "a search with a trace");
 }
 
 extern "C" pb_status pb_search_batch_subsets(pb_index *ix, const float *queries, const int64_t *q_tok_offsets,

@@ -15,8 +15,8 @@ pb_status pb_fail(pb_status s, const char *fmt, ...);
 
 using Job = std::function<pb_status(int rank)>;
 
-// A library thread of a deployment's rank or a replica set's slice: waits for a job, runs it, records its status and
-// pb_last_error() text
+// A library thread of a deployment's rank, a replica set's slice or a search lane: waits for a job, runs it, records
+// its status and pb_last_error() text
 struct RankWorker {
     int rank;
     std::thread th;
@@ -63,6 +63,22 @@ struct RankWorker {
         if (th.joinable()) th.join();
     }
 };
+
+// job(i) for slots 0..k-1 at once: slot 0 on the caller's thread, slot i >= 1 on helpers[i - 1], a RankWorker of rank
+// i.  st[i] is slot i's status and err[i] its pb_last_error() text when it failed; the caller picks the one it reports.
+inline void run_slots(int k, const Job &job, const std::unique_ptr<RankWorker> *helpers, std::vector<pb_status> &st,
+                      std::vector<std::string> &err) {
+    st.assign((size_t)k, PB_OK);
+    err.assign((size_t)k, std::string());
+    for (int i = 1; i < k; ++i) helpers[i - 1]->submit(job);
+    st[0] = job(0);
+    if (st[0] != PB_OK) err[0] = pb_last_error();
+    for (int i = 1; i < k; ++i) {
+        helpers[i - 1]->wait();
+        st[i] = helpers[i - 1]->status;
+        err[i] = helpers[i - 1]->error;
+    }
+}
 
 // A deployment (pb_index_load_devices, deployment.cpp, DESIGN §4o): the ranks of a doc-sharded index in one process,
 // driven through the public entry points by the library's own threads.  Its handle is a pb_index that holds no

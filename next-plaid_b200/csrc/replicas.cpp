@@ -88,18 +88,16 @@ struct Replicas {
     pb_status each(const std::function<pb_status(pb_index *, int)> &op, RepVote *vote = nullptr) {
         for (int g = 0; g < R() && vote; ++g) pb_index_set_rep_vote(members[g], vote, g);
         std::unique_ptr<Crew> crew = take_crew();
-        const Job job = [&](int g) { return op(members[g], g); };
-        for (int g = 1; g < R(); ++g) crew->w[g - 1]->submit(job);
-        pb_status st = job(0);
-        std::string err = st == PB_OK ? std::string() : std::string(pb_last_error());
-        for (int g = 1; g < R(); ++g) {
-            crew->w[g - 1]->wait();
-            if (st == PB_OK && crew->w[g - 1]->status != PB_OK)
-                st = crew->w[g - 1]->status, err = "replica " + std::to_string(g) + ": " + crew->w[g - 1]->error;
-        }
+        std::vector<pb_status> st;
+        std::vector<std::string> err;
+        run_slots(R(), [&](int g) { return op(members[g], g); }, crew->w.data(), st, err);
         give_crew(std::move(crew));
         for (int g = 0; g < R() && vote; ++g) pb_index_set_rep_vote(members[g], nullptr, 0);
-        return st == PB_OK ? PB_OK : pb_fail(st, "%s", err.c_str());
+        for (int g = 0; g < R(); ++g)
+            if (st[g] != PB_OK)
+                return g == 0 ? pb_fail(st[0], "%s", err[0].c_str())
+                              : pb_fail(st[g], "replica %d: %s", g, err[g].c_str());
+        return PB_OK;
     }
     // each() of a mutation on deployments, with the vote that makes it commit on every replica or on none
     pb_status voted(bool with_dir, bool share_rows, const std::function<pb_status(pb_index *, int)> &op) {
@@ -180,21 +178,17 @@ pb_status pb_rep_search(Replicas *rs, int64_t n, const std::function<pb_status(p
     for (int i = 0; i <= k; ++i) b[i] = n * i / k;
     for (int i = 0; i < k; ++i) share[i] = b[i + 1] - b[i];
     const std::vector<int> who = rs->pick(share);
-    const Job job = [&](int i) { return call(rs->members[who[i]], b[i], b[i + 1], i); };
     std::unique_ptr<Crew> crew;
-    if (k > 1) {
-        crew = rs->take_crew();
-        for (int i = 1; i < k; ++i) crew->w[i - 1]->submit(job);
-    }
-    pb_status st = job(0);
-    std::string err = st == PB_OK ? std::string() : std::string(pb_last_error());
-    for (int i = 1; i < k; ++i) {
-        crew->w[i - 1]->wait();
-        if (st == PB_OK && crew->w[i - 1]->status != PB_OK) st = crew->w[i - 1]->status, err = crew->w[i - 1]->error;
-    }
+    if (k > 1) crew = rs->take_crew();
+    std::vector<pb_status> st;
+    std::vector<std::string> err;
+    run_slots(k, [&](int i) { return call(rs->members[who[i]], b[i], b[i + 1], i); }, crew ? crew->w.data() : nullptr,
+              st, err);
     if (crew) rs->give_crew(std::move(crew));
     rs->done(who, share);
-    return st == PB_OK ? PB_OK : pb_fail(st, "%s", err.c_str());
+    for (int i = 0; i < k; ++i)
+        if (st[i] != PB_OK) return pb_fail(st[i], "%s", err[i].c_str());
+    return PB_OK;
 }
 
 pb_status pb_rep_whole(Replicas *rs, int64_t n, const std::function<pb_status(pb_index *)> &call) {
