@@ -85,9 +85,16 @@ typedef struct pb_index_desc {
  *   of the documents its cut keeps into a device buffer of its workspace (DESIGN.md 4j), so results, counts and
  *   pb_work_counters equal those of a handle opened without the flag; searches are slower, by the PCIe transfer.  At
  *   4 bits and dim 128 that leaves about 11 of 75 device bytes per token.  With ADOPT_RESIDUALS: PB_ERR_INVALID.  A
- *   failed pinned allocation: PB_ERR_NOMEM, nothing allocated.  Appends, deletes, pb_index_reserve and the sharded
- *   mutations and rebalance refuse such handles with PB_ERR_UNSUPPORTED, as they refuse ADOPT_RESIDUALS. */
-enum { PB_OPEN_ADOPT_RESIDUALS = 1, PB_OPEN_HOST_RESIDUALS = 2 };
+ *   failed pinned allocation: PB_ERR_NOMEM, nothing allocated.  The rows are held in pinned segments of 2^28 bytes
+ *   (PB_HOST_SEGMENT_BYTES, read at open: a power of two of at least 256, else PB_ERR_INVALID); the last is as long
+ *   as the rows need.  Without HOST_MUTABLE, appends, deletes, pb_index_reserve and the sharded mutations refuse
+ *   such handles with PB_ERR_UNSUPPORTED, as they refuse ADOPT_RESIDUALS; the rebalance always refuses them.
+ * HOST_MUTABLE: only with HOST_RESIDUALS (else PB_ERR_INVALID).  Appends, deletes, pb_index_reserve and the sharded
+ *   appends and deletes run on the handle as on a resident one, with results equal to a fresh open of the resulting
+ *   arrays (DESIGN.md 4r): new rows go to the tail of the segments, which grow one segment at a time (a failed
+ *   allocation: PB_ERR_NOMEM, nothing changed), and a delete compacts the rows in place.  Capacity is never given
+ *   back.  A replica set writes each shared row store once, through replica 0. */
+enum { PB_OPEN_ADOPT_RESIDUALS = 1, PB_OPEN_HOST_RESIDUALS = 2, PB_OPEN_HOST_MUTABLE = 4 };
 
 /* search.rs:27-69 SearchParameters.  batch_size is accepted and ignored, as in the reference
  * (it is never read there). */
@@ -158,8 +165,8 @@ PB_API int32_t pb_index_embedding_dim(const pb_index *ix);
 PB_API int32_t pb_index_nbits(const pb_index *ix);
 PB_API int32_t pb_index_device(const pb_index *ix);
 /* Bytes the handle's index arrays hold (allocated capacity; per-call workspaces and a caller's adopted residual array not
- * counted): *device_bytes on its device, *host_bytes in pinned host memory (N * dim * nbits / 8 with
- * PB_OPEN_HOST_RESIDUALS, else 0).  Either may be NULL. */
+ * counted): *device_bytes on its device, *host_bytes the pinned host memory held (with PB_OPEN_HOST_RESIDUALS
+ * N * dim * nbits / 8 until a PB_OPEN_HOST_MUTABLE mutation grows it by whole segments, else 0).  Either may be NULL. */
 PB_API pb_status pb_index_memory(const pb_index *ix, int64_t *device_bytes, int64_t *host_bytes);
 
 /* ---- incremental append ------------------------------------------------------------------ */
@@ -175,9 +182,12 @@ typedef struct pb_codec pb_codec;
  *   embeddings   [sum doc_lengths][dim] f32, doc_lengths [n_docs], both in memory_space (PB_MEM_HOST | PB_MEM_DEVICE)
  *   out_first_doc_id  may be NULL; receives doc_id_base + the old D
  * PB_ERR_UNSUPPORTED, nothing changed: doc-sharded handles (pb_index_comm_init, pb_index_group_join), handles opened
- * with PB_OPEN_ADOPT_RESIDUALS, index_dir with doc_id_base != 0, and totals past the limits of pb_index_open.
+ * with PB_OPEN_ADOPT_RESIDUALS or with PB_OPEN_HOST_RESIDUALS but not PB_OPEN_HOST_MUTABLE, index_dir with
+ * doc_id_base != 0, and totals past the limits of pb_index_open.
  * PB_ERR_INVALID: a codec that does not match the index, a code >= K, or a directory whose metadata.json
- * num_documents differs from the handle's.  An append of 0 documents changes nothing, on the device or on disk. */
+ * num_documents differs from the handle's.  An append of 0 documents changes nothing, on the device or on disk.
+ * On a PB_OPEN_HOST_MUTABLE handle the new rows go to the tail of the pinned segments, which grow first (a failed
+ * pinned allocation: PB_ERR_NOMEM, nothing changed). */
 PB_API pb_status pb_index_append(pb_index *ix, pb_codec *codec, const float *embeddings, const int64_t *doc_lengths,
                                  int64_t n_docs, int32_t memory_space, const char *index_dir, int64_t batch_size,
                                  int64_t *out_first_doc_id);
@@ -188,7 +198,10 @@ PB_API pb_status pb_index_append_encoded(pb_index *ix, const int64_t *codes, con
                                          int64_t *out_first_doc_id);
 /* Pre-size the per-token and per-doc arrays so that appends up to these totals neither reallocate nor copy.
  * Without it an append that outgrows an array reallocates it at 1.5x and copies it once, which needs the old and the
- * new array at the same time (PB_ERR_NOMEM, nothing changed, when the device cannot hold both). */
+ * new array at the same time (PB_ERR_NOMEM, nothing changed, when the device cannot hold both).  On a
+ * PB_OPEN_HOST_MUTABLE handle it also adds the pinned segments for num_embeddings; an append's own growth adds
+ * segments without copying the rows, except that the first growth replaces the exact-size last segment of the open.
+ * Refused (PB_ERR_UNSUPPORTED) as pb_index_delete refuses. */
 PB_API pb_status pb_index_reserve(pb_index *ix, int64_t num_documents, int64_t num_embeddings);
 
 /* ---- incremental delete ------------------------------------------------------------------ */
@@ -208,8 +221,10 @@ PB_API pb_status pb_index_reserve(pb_index *ix, int64_t num_documents, int64_t n
  * arrays; after that point only a CUDA runtime error can fail the call.  So on any other error neither the handle nor
  * the directory changes.  A delete that removes no document changes nothing, on the device or on disk.
  * PB_ERR_UNSUPPORTED, nothing changed: doc-sharded handles (pb_index_comm_init, pb_index_group_join), handles opened
- * with PB_OPEN_ADOPT_RESIDUALS, and index_dir with doc_id_base != 0.  PB_ERR_INVALID, nothing changed: a directory
- * whose metadata.json num_documents differs from the handle's. */
+ * with PB_OPEN_ADOPT_RESIDUALS or with PB_OPEN_HOST_RESIDUALS but not PB_OPEN_HOST_MUTABLE, and index_dir with
+ * doc_id_base != 0.  PB_ERR_INVALID, nothing changed: a directory whose metadata.json num_documents differs from the
+ * handle's.  On a PB_OPEN_HOST_MUTABLE handle the survivors' rows are compacted in place in the pinned segments, whose
+ * capacity is kept. */
 PB_API pb_status pb_index_delete(pb_index *ix, const int64_t *doc_ids, int64_t n_ids, const char *index_dir,
                                  int64_t *out_deleted);
 /* Device time of the last pb_index_delete on this handle, with pb_set_profiling(ix, 1): out_ms[0] the in-place
@@ -776,7 +791,9 @@ PB_API pb_status pb_index_shard_layout(const pb_index *ix, int32_t *out_world, i
  * a deployment of pb_index_load_devices.  flags as for pb_index_load_range_flags.  Replica 0 is loaded from the
  * directory; every other replica is a device-to-device copy of it (derived arrays included; the sm count and the grids
  * sized from it are the copy's device's own), made concurrently.  With PB_OPEN_HOST_RESIDUALS rank r of every replica
- * reads replica 0's rank r's one pinned array, freed with the last of them.
+ * reads replica 0's rank r's one pinned row store, freed with the last of them.  With PB_OPEN_HOST_MUTABLE replica 0
+ * writes and moves the shared rows once, and every replica its own device arrays; a mutation first synchronizes every
+ * replica's devices.
  * Checks before any device is touched, in this order: a NULL index_dir, devices or out, n_shards < 1, n_devices not a
  * positive multiple of n_shards, n_devices > 64: PB_ERR_INVALID; no usable device: PB_ERR_CUDA; a device id outside
  * [0, pb_device_count()): PB_ERR_INVALID.  A failed load returns the lowest failing replica's status and message and

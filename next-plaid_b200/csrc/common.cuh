@@ -28,6 +28,22 @@ PB_DEV float key_to_score(uint32_t k) {
     return __uint_as_float((k & 0x80000000u) ? (k ^ 0x80000000u) : ~k);
 }
 
+// A row array addressed by byte.  FlatRows: one allocation.  SegRows: the pinned host segments of a host-tier handle
+// (DESIGN.md 4r), 2^shift bytes each, read over the mapping through the device's segment table: byte b is at
+// seg[b >> shift] + (b & (2^shift - 1)).  The segment size is a multiple of 16 and a load unit of V (2, 4 or 16 bytes)
+// sits at a multiple of sizeof(V) from the array start, so no unit straddles two segments.
+struct FlatRows {
+    const uint8_t *p;
+    template <class V> PB_DEV const V *at(long long b) const { return reinterpret_cast<const V *>(p + b); }
+};
+struct SegRows {
+    const uint8_t *const *seg;
+    int shift;
+    template <class V> PB_DEV const V *at(long long b) const {
+        return reinterpret_cast<const V *>(seg[b >> shift] + (b & ((1ll << shift) - 1)));
+    }
+};
+
 PB_DEV u64 shfl_u64(u64 v, int src) {
     uint32_t lo = __shfl_sync(PB_FULL, (uint32_t)v, src);
     uint32_t hi = __shfl_sync(PB_FULL, (uint32_t)(v >> 32), src);

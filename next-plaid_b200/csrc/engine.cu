@@ -245,42 +245,114 @@ struct HostBuf {  // pinned
     }
 };
 
-// the packed residuals of a PB_OPEN_HOST_RESIDUALS handle: pinned, mapped and portable host memory; dev is the address
-// kernels read it at.  The replicas of a set share one allocation (share), freed with the last of them.
-struct PinnedRes {
-    uint8_t *p = nullptr, *dev = nullptr;
-    size_t bytes = 0;
-    std::shared_ptr<uint8_t> keep;  // owns p
-    pb_status alloc(size_t n) {
-        if (n == 0) return PB_OK;
-        void *h = nullptr;
-        cudaError_t e = cudaHostAlloc(&h, n, cudaHostAllocMapped | cudaHostAllocPortable);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            return pb_fail(PB_ERR_NOMEM, "cudaHostAlloc(%zu bytes, mapped) failed: %s", n, cudaGetErrorString(e));
+// One pinned, mapped and portable host allocation of n bytes
+static pb_status pinned_segment(size_t n, std::shared_ptr<uint8_t> &out) {
+    void *h = nullptr;
+    cudaError_t e = cudaHostAlloc(&h, n, cudaHostAllocMapped | cudaHostAllocPortable);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return pb_fail(PB_ERR_NOMEM, "cudaHostAlloc(%zu bytes, mapped) failed: %s", n, cudaGetErrorString(e));
+    }
+    out.reset(static_cast<uint8_t *>(h), [](uint8_t *q) { cudaFreeHost(q); });
+    return PB_OK;
+}
+
+// The packed residuals of a PB_OPEN_HOST_RESIDUALS handle (DESIGN.md 4r): segments of 2^shift bytes, each one pinned
+// host allocation; byte b of the row array is at seg[b >> shift] + (b & (2^shift - 1)).  An open makes the last segment
+// exactly as long as the rows need; the first growth replaces it by a full one (a copy of at most one segment), and
+// later growths only add segments.  The replicas of a set share one store, freed with the last of them; each reads it
+// through its own device table of the segments' mapped addresses (HostTier).  mu serialises growths.
+struct HostRows {
+    int shift = 28;
+    std::vector<std::shared_ptr<uint8_t>> seg;
+    size_t bytes = 0;             // pinned bytes held: the capacity, since only the last segment can be short
+    unsigned long long gen = 0;   // changes whenever a segment's address does
+    std::mutex mu;
+    size_t seg_bytes() const { return (size_t)1 << shift; }
+    pb_status open(size_t n) {
+        for (size_t o = 0; o < n; o += seg_bytes()) {
+            seg.emplace_back();
+            CKS(pinned_segment(std::min(seg_bytes(), n - o), seg.back()));
+            bytes += std::min(seg_bytes(), n - o);
         }
-        void *d = nullptr;
-        e = cudaHostGetDevicePointer(&d, h, 0);
-        if (e != cudaSuccess) {
-            cudaFreeHost(h);
-            return pb_fail(PB_ERR_CUDA, "cudaHostGetDevicePointer failed: %s", cudaGetErrorString(e));
-        }
-        p = static_cast<uint8_t *>(h);
-        keep.reset(p, [](uint8_t *q) { cudaFreeHost(q); });
-        dev = static_cast<uint8_t *>(d);
-        bytes = n;
+        ++gen;
         return PB_OK;
     }
-    // o's allocation, read from the current device
-    pb_status share(const PinnedRes &o) {
-        if (!o.p) return PB_OK;
-        void *d = nullptr;
-        cudaError_t e = cudaHostGetDevicePointer(&d, o.p, 0);
-        if (e != cudaSuccess) return pb_fail(PB_ERR_CUDA, "cudaHostGetDevicePointer failed: %s", cudaGetErrorString(e));
-        p = o.p, keep = o.keep, bytes = o.bytes;
-        dev = static_cast<uint8_t *>(d);
+    // capacity for `want` bytes; every allocation before the first change, so a failure changes nothing
+    pb_status grow(size_t want) {
+        if (want <= bytes) return PB_OK;
+        const size_t S = seg_bytes(), tail = bytes & (S - 1), need = (want + S - 1) / S;
+        std::shared_ptr<uint8_t> full;
+        if (tail) CKS(pinned_segment(S, full));
+        std::vector<std::shared_ptr<uint8_t>> add(need - seg.size());
+        for (auto &x : add) CKS(pinned_segment(S, x));
+        if (tail) {
+            memcpy(full.get(), seg.back().get(), tail);
+            seg.back() = std::move(full);
+        }
+        for (auto &x : add) seg.push_back(std::move(x));
+        bytes = seg.size() * S;
+        ++gen;
         return PB_OK;
     }
+    // f(host address, offset into the range, length) for each segment piece of bytes [b, b + n)
+    template <class F> pb_status pieces(size_t b, size_t n, F &&f) const {
+        for (size_t done = 0; done < n;) {
+            const size_t o = (b + done) & (seg_bytes() - 1), m = std::min(n - done, seg_bytes() - o);
+            CKS(f(seg[(b + done) >> shift].get() + o, done, m));
+            done += m;
+        }
+        return PB_OK;
+    }
+    // bytes [b, b + n) from src (host or device memory), or to dst (host memory)
+    pb_status write(size_t b, const uint8_t *src, size_t n, int space) const {
+        return pieces(b, n, [&](uint8_t *h, size_t o, size_t m) -> pb_status {
+            if (space == PB_MEM_DEVICE) CK(cudaMemcpy(h, src + o, m, cudaMemcpyDeviceToHost));
+            else memcpy(h, src + o, m);
+            return PB_OK;
+        });
+    }
+    pb_status read(size_t b, uint8_t *dst, size_t n) const {
+        return pieces(b, n, [&](uint8_t *h, size_t o, size_t m) -> pb_status {
+            memcpy(dst + o, h, m);
+            return PB_OK;
+        });
+    }
+    // bytes [b, b + n) to device memory, one copy per piece on st
+    pb_status to_device(size_t b, uint8_t *dst, size_t n, cudaStream_t st) const {
+        return pieces(b, n, [&](uint8_t *h, size_t o, size_t m) -> pb_status {
+            CK(cudaMemcpyAsync(dst + o, h, m, cudaMemcpyHostToDevice, st));
+            return PB_OK;
+        });
+    }
+};
+
+// One handle's view of its host rows: the store, and the store's segment table as this handle's device reads it
+struct HostTier {
+    std::shared_ptr<HostRows> rows;
+    DevBuf table;                        // [segments] mapped addresses on the handle's device
+    unsigned long long table_gen = ~0ull;
+    // the table after a change of the store's segments (the current device is the handle's)
+    pb_status sync() {
+        if (!rows || table_gen == rows->gen) return PB_OK;
+        std::vector<const uint8_t *> a(rows->seg.size());
+        for (size_t k = 0; k < a.size(); ++k) {
+            void *d = nullptr;
+            CK(cudaHostGetDevicePointer(&d, rows->seg[k].get(), 0));
+            a[k] = static_cast<const uint8_t *>(d);
+        }
+        CKS(table.ensure(std::max<size_t>(a.size() * 8, 16)));
+        if (!a.empty()) CK(cudaMemcpy(table.p, a.data(), a.size() * 8, cudaMemcpyHostToDevice));
+        table_gen = rows->gen;
+        return PB_OK;
+    }
+    // capacity for `want` bytes, and this handle's table to match
+    pb_status grow(size_t want) {
+        std::lock_guard<std::mutex> g(rows->mu);
+        CKS(rows->grow(want));
+        return sync();
+    }
+    SegRows dev() const { return SegRows{table.as<const uint8_t *const>(), rows->shift}; }
 };
 
 // ------------------------------------------------------------------------------------------
@@ -557,8 +629,9 @@ struct pb_index : DocArrays {
     long long K = 0, doc_id_base = 0;
     int sm_count = 132;
     DevBuf centroids, w_rev;
-    bool host_tier = false;    // PB_OPEN_HOST_RESIDUALS: `residuals` stays empty, the rows live in host_res
-    PinnedRes host_res;
+    bool host_tier = false;    // PB_OPEN_HOST_RESIDUALS: `residuals` stays empty, the rows live in host.rows
+    bool host_mutable = false; // PB_OPEN_HOST_MUTABLE: appends and deletes write the host rows
+    HostTier host;
     bool build_ivf = false;    // no inverted file was given: built from the codes at finalize (index.rs:850-873)
     float cmax = 1.0f;         // largest centroid L2 norm (range of the 16-bit score table)
     bool fast_approx = true;   // two-pass approximate stage (exact cut either way)
@@ -914,9 +987,7 @@ pb_status pb_index_upload_tokens(pb_index *ix, long long tok_off, const int64_t 
         if (tok_off != 0 || n != ix->N || residuals != ix->residuals.as<uint8_t>())
             return pb_fail(PB_ERR_INVALID, "adopted residuals cover the whole index");
     } else if (ix->host_tier) {
-        uint8_t *dst = ix->host_res.p + (size_t)tok_off * ix->packed;
-        if (space == PB_MEM_DEVICE) CK(cudaMemcpy(dst, residuals, (size_t)n * ix->packed, cudaMemcpyDeviceToHost));
-        else memcpy(dst, residuals, (size_t)n * ix->packed);
+        CKS(ix->host.rows->write((size_t)tok_off * ix->packed, residuals, (size_t)n * ix->packed, space));
     } else
         CK(cudaMemcpy(ix->residuals.as<uint8_t>() + (size_t)tok_off * ix->packed, residuals, (size_t)n * ix->packed,
                       space == PB_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
@@ -963,6 +1034,15 @@ pb_status pb_index_open_begin(const pb_index_desc *d, pb_index **out) {
         return pb_fail(PB_ERR_INVALID, "PB_OPEN_ADOPT_RESIDUALS needs device-resident residuals");
     if ((d->flags & PB_OPEN_ADOPT_RESIDUALS) && (d->flags & PB_OPEN_HOST_RESIDUALS))
         return pb_fail(PB_ERR_INVALID, "PB_OPEN_ADOPT_RESIDUALS and PB_OPEN_HOST_RESIDUALS exclude each other");
+    if ((d->flags & PB_OPEN_HOST_MUTABLE) && !(d->flags & PB_OPEN_HOST_RESIDUALS))
+        return pb_fail(PB_ERR_INVALID, "PB_OPEN_HOST_MUTABLE needs PB_OPEN_HOST_RESIDUALS");
+    int seg_shift = 28;
+    if (const char *e = getenv("PB_HOST_SEGMENT_BYTES"); e && (d->flags & PB_OPEN_HOST_RESIDUALS)) {
+        const long long v = atoll(e);
+        if (v < 256 || v > (1ll << 40) || (v & (v - 1)))
+            return pb_fail(PB_ERR_INVALID, "PB_HOST_SEGMENT_BYTES=%s is not a power of two in [256, 2^40]", e);
+        seg_shift = __builtin_ctzll((unsigned long long)v);
+    }
     CKS(check_device(d->device));
     std::unique_ptr<pb_index> ix(new pb_index());
     ix->device = d->device;
@@ -1013,9 +1093,16 @@ pb_status pb_index_open_begin(const pb_index_desc *d, pb_index **out) {
     CKS(upload(ix->w_rev, wrev.data(), 256 * sizeof(float), PB_MEM_HOST));
     CKS(upload(ix->centroids, d->centroids, (size_t)ix->K * ix->dim * sizeof(float), sp));
     ix->host_tier = (d->flags & PB_OPEN_HOST_RESIDUALS) != 0;
+    ix->host_mutable = (d->flags & PB_OPEN_HOST_MUTABLE) != 0;
     if (d->flags & PB_OPEN_ADOPT_RESIDUALS)
         ix->residuals.adopt(const_cast<uint8_t *>(d->residuals), (size_t)ix->N * ix->packed);
-    else if (ix->host_tier) CKS(ix->host_res.alloc((size_t)ix->N * ix->packed));
+    else if (ix->host_tier) {
+        ix->host.rows = std::make_shared<HostRows>();
+        ix->host.rows->shift = seg_shift;
+        CKS(ix->host.rows->open((size_t)ix->N * ix->packed));
+        CK(cudaSetDevice(ix->device));
+        CKS(ix->host.sync());
+    }
     else CKS(ix->residuals.ensure(std::max<size_t>((size_t)ix->N * ix->packed, 16)));
     CKS(ix->codes.ensure(std::max<size_t>((size_t)ix->N * 4, 16)));
     if (!ix->build_ivf) {
@@ -1122,9 +1209,10 @@ static pb_status token_norms(pb_index *ix, DocArrays &a, long long t0, const flo
         for (long long o = t0; o < t.N; o += slab) {
             const long long m = std::min(slab, t.N - o);
             const uint8_t *res = st.as<uint8_t>();
-            if (ix->host_tier)
-                CK(cudaMemcpy(st.p, ix->host_res.p + (size_t)o * ix->packed, (size_t)m * ix->packed, cudaMemcpyHostToDevice));
-            else
+            if (ix->host_tier) {
+                CKS(ix->host.rows->to_device((size_t)o * ix->packed, st.as<uint8_t>(), (size_t)m * ix->packed, 0));
+                CK(cudaStreamSynchronize(0));
+            } else
                 res = a.residuals.as<uint8_t>() + (size_t)o * ix->packed;
             CKS(launch_min_vnorm(ix, a.codes.as<uint32_t>() + o, res, m, a.tok_inv_norm.as<float>() + o, mn.as<float>()));
         }
@@ -1338,7 +1426,7 @@ extern "C" pb_status pb_index_memory(const pb_index *ix, int64_t *device_bytes, 
     for (const DevBuf *b : DocArrays::buffers(*ix))
         if (b->owned) dev += b->cap;  // adopted residuals are the caller's allocation
     if (device_bytes) *device_bytes = (int64_t)dev;
-    if (host_bytes) *host_bytes = (int64_t)ix->host_res.bytes;
+    if (host_bytes) *host_bytes = ix->host.rows ? (int64_t)ix->host.rows->bytes : 0;
     return PB_OK;
 }
 
@@ -2682,16 +2770,16 @@ static pb_status stage_rows(pb_index *ix, Workspace &ws, const uint32_t *docs, c
     float *dst_inv = inv ? ws.s_inv.as<float>() : nullptr;
     if (pk % 16 == 0)
         k_stage_rows<uint4, 4><<<grid, 256, 0, ws.stream>>>(docs, nkept, Mcap, n_slots, ix->doc_off.as<long long>(), soff,
-                                                            ix->host_res.dev, ix->codes.as<uint32_t>(), src_inv, pk,
+                                                            ix->host.dev(), ix->codes.as<uint32_t>(), src_inv, pk,
                                                             ws.s_res.as<uint8_t>(), ws.s_codes.as<uint32_t>(), dst_inv);
     else if (pk % 4 != 0)  // 1-bit rows of dim 48 (6 bytes)
         k_stage_rows<unsigned short, 8><<<grid, 256, 0, ws.stream>>>(docs, nkept, Mcap, n_slots, ix->doc_off.as<long long>(),
-                                                                     soff, ix->host_res.dev, ix->codes.as<uint32_t>(), src_inv,
+                                                                     soff, ix->host.dev(), ix->codes.as<uint32_t>(), src_inv,
                                                                      pk, ws.s_res.as<uint8_t>(), ws.s_codes.as<uint32_t>(),
                                                                      dst_inv);
     else
         k_stage_rows<uint32_t, 8><<<grid, 256, 0, ws.stream>>>(docs, nkept, Mcap, n_slots, ix->doc_off.as<long long>(), soff,
-                                                               ix->host_res.dev, ix->codes.as<uint32_t>(), src_inv, pk,
+                                                               ix->host.dev(), ix->codes.as<uint32_t>(), src_inv, pk,
                                                                ws.s_res.as<uint8_t>(), ws.s_codes.as<uint32_t>(), dst_inv);
     CK(cudaGetLastError());
     tv = {ws.s_codes.as<uint32_t>(), ws.s_res.as<uint8_t>(), dst_inv, soff};
@@ -3862,8 +3950,8 @@ extern "C" pb_status pb_exhaustive_scores(pb_index *ix, const float *queries, co
             TokView tv = resident_tokens(ix);
             if (ix->host_tier) {
                 CKS(ws.s_res.ensure((size_t)std::max(ntok, 1ll) * ix->packed));
-                CK(cudaMemcpyAsync(ws.s_res.p, ix->host_res.p + (size_t)doff[d0] * ix->packed, (size_t)ntok * ix->packed,
-                                   cudaMemcpyHostToDevice, ws.stream));
+                CKS(ix->host.rows->to_device((size_t)doff[d0] * ix->packed, ws.s_res.as<uint8_t>(), (size_t)ntok * ix->packed,
+                                             ws.stream));
                 tv = {ix->codes.as<uint32_t>() + doff[d0], ws.s_res.as<uint8_t>(), nullptr, ws.tokp.as<long long>()};
             }
             CKS(launch_exact(ix, ws, kv, tv, B, QS, Mblk, 1, ntok, nullptr));
@@ -4500,7 +4588,7 @@ struct AppendPrep {
 static pb_status grow_docs(pb_index *ix, long long D1, long long N1, bool geometric) {
     const size_t pk = (size_t)ix->packed;
     CKS(ix->codes.grow((size_t)N1 * 4, (size_t)ix->N * 4, geometric));
-    CKS(ix->residuals.grow((size_t)N1 * pk, (size_t)ix->N * pk, geometric));
+    if (!ix->host_tier) CKS(ix->residuals.grow((size_t)N1 * pk, (size_t)ix->N * pk, geometric));
     if (TcDims::has(ix->dim)) CKS(ix->tok_inv_norm.grow((size_t)N1 * 4, (size_t)ix->N * 4, geometric));
     CKS(ix->doc_off.grow((size_t)(D1 + 1) * 8, (size_t)(ix->D + 1) * 8, geometric));
     CKS(ix->udoc_off.grow((size_t)(D1 + 1) * 8, (size_t)(ix->D + 1) * 8, geometric));
@@ -4521,10 +4609,11 @@ static void publish(pb_index *ix, const DocTotals &t, DocArrays *fresh = nullptr
 }
 
 // Every check, allocation and device write of an append that stays invisible until publish.  The caller holds
-// the handle's writer lock.
+// the handle's writer lock.  A host-tier handle's new rows go to its store's tail, past the rows a search reads;
+// write_rows = false: another replica sharing the store has written them.
 static pb_status append_prepare(pb_index *ix, pb_codec *codec, const float *embeddings, const int64_t *codes,
                                 const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs, int32_t space,
-                                bool keep_codes, int64_t *out_first, AppendPrep &p) {
+                                bool keep_codes, int64_t *out_first, AppendPrep &p, bool write_rows = true) {
     CK(cudaSetDevice(ix->device));
     CK(cudaDeviceSynchronize());  // work earlier readers left queued (pb_search_batch_device) reads the arrays
     if (codec) {  // same K, dim, nbits and bit-identical centroids as the index; cutoffs required (codec.rs:359-362)
@@ -4562,6 +4651,7 @@ static pb_status append_prepare(pb_index *ix, pb_codec *codec, const float *embe
     const size_t pk = (size_t)ix->packed;
 
     // capacity: grown arrays keep their contents; nothing below is visible until the commit
+    if (ix->host_tier) CKS(write_rows ? ix->host.grow((size_t)t.N * pk) : ix->host.sync());
     CKS(grow_docs(ix, t.D, t.N, true));
 
     // 1. tokens into the tails of codes / residuals: encoded on the device, or narrowed and range-checked
@@ -4570,9 +4660,10 @@ static pb_status append_prepare(pb_index *ix, pb_codec *codec, const float *embe
         codec->last_tokens = ntok;
         codec->last_fallback = 0;
         const long long slab = 1ll << 20;
-        DevBuf dX, dcodes;
+        DevBuf dX, dcodes, dres;  // dres: a host-tier slab's rows on their way to the store
         CKS(dcodes.ensure((size_t)std::max(std::min(ntok, slab), 1ll) * 8));
         if (space == PB_MEM_HOST) CKS(dX.ensure((size_t)std::max(std::min(ntok, slab), 1ll) * ix->dim * 4));
+        if (ix->host_tier) CKS(dres.ensure((size_t)std::max(std::min(ntok, slab), 1ll) * pk));
         if (keep_codes) hcodes.resize((size_t)ntok);
         for (long long o = 0; o < ntok; o += slab) {
             const long long m = std::min(slab, ntok - o);
@@ -4581,13 +4672,18 @@ static pb_status append_prepare(pb_index *ix, pb_codec *codec, const float *embe
                 CK(cudaMemcpy(dX.p, x, (size_t)m * ix->dim * 4, cudaMemcpyHostToDevice));
                 x = dX.as<float>();
             }
-            CKS(codec_encode_device(codec, x, m, dcodes.as<long long>(), ix->residuals.as<uint8_t>() + (size_t)(N0 + o) * pk, nullptr));
+            uint8_t *res = ix->host_tier ? dres.as<uint8_t>() : ix->residuals.as<uint8_t>() + (size_t)(N0 + o) * pk;
+            CKS(codec_encode_device(codec, x, m, dcodes.as<long long>(), res, nullptr));
+            if (ix->host_tier) CKS(ix->host.rows->write((size_t)(N0 + o) * pk, res, (size_t)m * pk, PB_MEM_DEVICE));
             CKS(upload_narrow(ix->codes, N0 + o, reinterpret_cast<const int64_t *>(dcodes.p), m, ix->K, PB_MEM_DEVICE, "codes"));
             if (keep_codes) CK(cudaMemcpy(hcodes.data() + o, dcodes.p, (size_t)m * 8, cudaMemcpyDeviceToHost));
         }
     } else if (ntok > 0) {
-        CK(cudaMemcpy(ix->residuals.as<uint8_t>() + (size_t)N0 * pk, residuals, (size_t)ntok * pk,
-                      space == PB_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+        if (!ix->host_tier)
+            CK(cudaMemcpy(ix->residuals.as<uint8_t>() + (size_t)N0 * pk, residuals, (size_t)ntok * pk,
+                          space == PB_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+        else if (write_rows)
+            CKS(ix->host.rows->write((size_t)N0 * pk, residuals, (size_t)ntok * pk, space));
         CKS(upload_narrow(ix->codes, N0, codes, ntok, ix->K, space, "codes"));
     }
 
@@ -4624,24 +4720,32 @@ static pb_status append_prepare(pb_index *ix, pb_codec *codec, const float *embe
     return PB_OK;
 }
 
+// the packed rows of tokens [t0, t0 + n) into host memory, from the device array or the host tier's store
+static pb_status rows_to_host(const pb_index *ix, long long t0, long long n, uint8_t *dst) {
+    const size_t pk = (size_t)ix->packed;
+    if (n == 0) return PB_OK;
+    if (ix->host_tier) return ix->host.rows->read((size_t)t0 * pk, dst, (size_t)n * pk);
+    CK(cudaMemcpy(dst, ix->residuals.as<uint8_t>() + (size_t)t0 * pk, (size_t)n * pk, cudaMemcpyDeviceToHost));
+    return PB_OK;
+}
+
 // update_index's file changes for the prepared documents, on a directory of old_D documents whose new inverted file
 // is (hivf [L], hlen [K])
 static pb_status append_dir(pb_index *ix, const AppendPrep &p, const char *index_dir, long long old_D, int64_t batch_size,
                             const std::vector<int64_t> &hivf, long long L, const std::vector<int32_t> &hlen) {
     const size_t pk = (size_t)ix->packed;
     std::vector<uint8_t> hres((size_t)p.ntok * pk);
-    if (p.ntok)
-        CK(cudaMemcpy(hres.data(), ix->residuals.as<uint8_t>() + (size_t)(p.t.N - p.ntok) * pk, hres.size(), cudaMemcpyDeviceToHost));
+    CKS(rows_to_host(ix, p.t.N - p.ntok, p.ntok, hres.data()));
     return pb_dir_append(index_dir, old_D, ix->K, ix->dim, ix->nbits, batch_size, p.hcodes.data(), hres.data(), p.dl.data(),
                          p.n, hivf.data(), L, hlen.data());
 }
 
-// Mutations need a residual array the library owns on the device: not the caller's (PB_OPEN_ADOPT_RESIDUALS), not
-// pinned host memory (PB_OPEN_HOST_RESIDUALS)
+// Mutations need residual rows the library owns and may grow: not the caller's array (PB_OPEN_ADOPT_RESIDUALS), not
+// pinned host memory opened without PB_OPEN_HOST_MUTABLE
 static pb_status refuse_fixed_residuals(const pb_index *ix) {
     if (!ix->residuals.owned)
         return pb_fail(PB_ERR_UNSUPPORTED, "the handle uses the caller's residual array (PB_OPEN_ADOPT_RESIDUALS)");
-    if (ix->host_tier)
+    if (ix->host_tier && !ix->host_mutable)
         return pb_fail(PB_ERR_UNSUPPORTED, "the handle keeps its residuals in host memory (PB_OPEN_HOST_RESIDUALS)");
     return PB_OK;
 }
@@ -4695,6 +4799,7 @@ extern "C" pb_status pb_index_reserve(pb_index *ix, int64_t num_documents, int64
     const long long dd = D1 - ix->D, dn = N1 - ix->N;
     // a new doc adds at most its length rounded up to 8 distinct-code entries, and at most that many (centroid, doc) pairs
     const long long U1 = ix->n_ucodes + dn + 7 * dd, L1 = ix->ivf_len + dn;
+    if (ix->host_tier) CKS(ix->host.grow((size_t)N1 * ix->packed));
     CKS(grow_docs(ix, D1, N1, false));
     CKS(ix->ucodes.grow((size_t)U1 * 4, (size_t)ix->n_ucodes * 4, false));
     CKS(ix->ivf.grow((size_t)L1 * 4, (size_t)ix->ivf_len * 4, false));
@@ -4837,8 +4942,11 @@ static pb_status delete_prepare(pb_index *ix, const int64_t *doc_ids, int64_t n_
     return PB_OK;
 }
 
-// The in-place part of a prepared delete: only a CUDA runtime error can fail it
-static pb_status delete_commit(pb_index *ix, DeletePrep &p) {
+// The in-place part of a prepared delete, in two steps (delete_move, then delete_finish): only a CUDA runtime error
+// can fail them.  delete_move compacts the arrays; a host-tier handle's survivors are gathered over the mapping into
+// the device staging and copied back to the store at their new offsets, one copy per segment piece.  write_rows =
+// false: another replica sharing the store moves them, before this handle's delete_finish reads them.
+static pb_status delete_move(pb_index *ix, DeletePrep &p, bool write_rows) {
     if (p.n_del == 0) return PB_OK;
     const bool prof = ix->profiling && p.ev.e[0];
     const int grid = ix->sm_count * 8;
@@ -4850,31 +4958,43 @@ static pb_status delete_commit(pb_index *ix, DeletePrep &p) {
         const long long j0 = w.first, j1 = w.second;
         const unsigned blocks = (unsigned)std::min<long long>((j1 - j0 + 7) / 8, grid);
         const long long *kp = p.kept.as<long long>();
-        k_compact_gather<uint32_t><<<blocks, 256>>>(ix->codes.as<uint8_t>(), ix->doc_off.as<long long>(), kp,
+        k_compact_gather<uint32_t><<<blocks, 256>>>(FlatRows{ix->codes.as<uint8_t>()}, ix->doc_off.as<long long>(), kp,
                                                     p.new_doff.as<long long>(), j0, j1, 4, p.st_codes.as<uint8_t>());
-        if (pk % 16 == 0)
-            k_compact_gather<uint4><<<blocks, 256>>>(ix->residuals.as<uint8_t>(), ix->doc_off.as<long long>(), kp,
-                                                     p.new_doff.as<long long>(), j0, j1, (int)pk, p.st_res.as<uint8_t>());
-        else if (pk % 4 != 0)  // 1-bit rows of dim 48 (6 bytes)
-            k_compact_gather<unsigned short><<<blocks, 256>>>(ix->residuals.as<uint8_t>(), ix->doc_off.as<long long>(), kp,
-                                                              p.new_doff.as<long long>(), j0, j1, (int)pk,
-                                                              p.st_res.as<uint8_t>());
-        else
-            k_compact_gather<uint32_t><<<blocks, 256>>>(ix->residuals.as<uint8_t>(), ix->doc_off.as<long long>(), kp,
-                                                        p.new_doff.as<long long>(), j0, j1, (int)pk, p.st_res.as<uint8_t>());
+        auto gather_rows = [&](auto src) {
+            if (pk % 16 == 0)
+                k_compact_gather<uint4><<<blocks, 256>>>(src, ix->doc_off.as<long long>(), kp, p.new_doff.as<long long>(), j0,
+                                                         j1, (int)pk, p.st_res.as<uint8_t>());
+            else if (pk % 4 != 0)  // 1-bit rows of dim 48 (6 bytes)
+                k_compact_gather<unsigned short><<<blocks, 256>>>(src, ix->doc_off.as<long long>(), kp,
+                                                                  p.new_doff.as<long long>(), j0, j1, (int)pk,
+                                                                  p.st_res.as<uint8_t>());
+            else
+                k_compact_gather<uint32_t><<<blocks, 256>>>(src, ix->doc_off.as<long long>(), kp, p.new_doff.as<long long>(),
+                                                            j0, j1, (int)pk, p.st_res.as<uint8_t>());
+        };
+        if (!ix->host_tier) gather_rows(FlatRows{ix->residuals.as<uint8_t>()});
+        else if (write_rows) gather_rows(ix->host.dev());
         // distinct-code blocks start at multiples of 8 codes (32 bytes)
-        k_compact_gather<uint4><<<blocks, 256>>>(ix->ucodes.as<uint8_t>(), ix->udoc_off.as<long long>(), kp,
+        k_compact_gather<uint4><<<blocks, 256>>>(FlatRows{ix->ucodes.as<uint8_t>()}, ix->udoc_off.as<long long>(), kp,
                                                  p.new_uoff.as<long long>(), j0, j1, 4, p.st_u.as<uint8_t>());
         CK(cudaGetLastError());
         const long long nt = hoff[j1] - hoff[j0], nu = hu[j1] - hu[j0];
         CK(cudaMemcpy(ix->codes.as<uint8_t>() + (size_t)hoff[j0] * 4, p.st_codes.p, (size_t)nt * 4, cudaMemcpyDeviceToDevice));
-        CK(cudaMemcpy(ix->residuals.as<uint8_t>() + (size_t)hoff[j0] * pk, p.st_res.p, (size_t)nt * pk, cudaMemcpyDeviceToDevice));
+        if (!ix->host_tier)
+            CK(cudaMemcpy(ix->residuals.as<uint8_t>() + (size_t)hoff[j0] * pk, p.st_res.p, (size_t)nt * pk, cudaMemcpyDeviceToDevice));
+        else if (write_rows)
+            CKS(ix->host.rows->write((size_t)hoff[j0] * pk, p.st_res.as<uint8_t>(), (size_t)nt * pk, PB_MEM_DEVICE));
         CK(cudaMemcpy(ix->ucodes.as<uint8_t>() + (size_t)hu[j0] * 4, p.st_u.p, (size_t)nu * 4, cudaMemcpyDeviceToDevice));
     }
     CK(cudaMemcpy(ix->doc_off.p, p.new_doff.p, (size_t)(p.t.D + 1) * 8, cudaMemcpyDeviceToDevice));
     CK(cudaMemcpy(ix->udoc_off.p, p.new_uoff.p, (size_t)(p.t.D + 1) * 8, cudaMemcpyDeviceToDevice));
     if (prof) CK(cudaEventRecord(p.ev.e[3]));
+    return PB_OK;
+}
 
+static pb_status delete_finish(pb_index *ix, DeletePrep &p) {
+    if (p.n_del == 0) return PB_OK;
+    const bool prof = ix->profiling && p.ev.e[0];
     // 6. 1 / |c + w| of the survivors in their new order, and vmin / wmax over them as an open computes them: the old
     // constants would still bound the error, but the work counters would differ from a fresh open
     const float seed[2] = {3.0e38f, 0.0f};
@@ -4890,6 +5010,11 @@ static pb_status delete_commit(pb_index *ix, DeletePrep &p) {
         CK(cudaEventElapsedTime(&ix->delete_ms[2], p.ev.e[3], p.ev.e[4]));
     }
     return PB_OK;
+}
+
+static pb_status delete_commit(pb_index *ix, DeletePrep &p, bool write_rows = true) {
+    CKS(delete_move(ix, p, write_rows));
+    return delete_finish(ix, p);
 }
 
 extern "C" pb_status pb_index_delete(pb_index *ix, const int64_t *doc_ids, int64_t n_ids, const char *index_dir,
@@ -4937,7 +5062,12 @@ pb_status pb_index_clone(const pb_index *src, int device, pb_index **out) {
     ix->fast_exact = src->fast_exact, ix->filter_diag = src->filter_diag, ix->pair_exact = src->pair_exact;
     ix->ws_grid = src->ws_grid, ix->ws_grid2 = src->ws_grid2, ix->lanes = src->lanes, ix->profiling = src->profiling;
     ix->st_budget = src->st_budget, ix->delete_window = src->delete_window;
-    if (src->host_tier) CKS(ix->host_res.share(src->host_res));
+    ix->host_mutable = src->host_mutable;
+    if (src->host_tier) {  // the store is shared; the table is the copy's device's own
+        ix->host.rows = src->host.rows;
+        CK(cudaSetDevice(device));
+        CKS(ix->host.sync());
+    }
     OwnedStream st;
     CK(cudaStreamCreateWithFlags(&st.s, cudaStreamNonBlocking));
     const auto mine = DocArrays::buffers(*ix);
@@ -4962,7 +5092,7 @@ static pb_status tail_rows(const pb_index *ix, long long t0, long long n, std::v
     if (n) {
         CK(cudaSetDevice(ix->device));
         CK(cudaMemcpy(c32.data(), ix->codes.as<uint32_t>() + t0, (size_t)n * 4, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(res.data(), ix->residuals.as<uint8_t>() + (size_t)t0 * pk, res.size(), cudaMemcpyDeviceToHost));
+        CKS(rows_to_host(ix, t0, n, res.data()));
     }
     codes.assign(c32.begin(), c32.end());
     return PB_OK;
@@ -4970,6 +5100,17 @@ static pb_status tail_rows(const pb_index *ix, long long t0, long long n, std::v
 
 Replicas *pb_replicas_of(const pb_index *ix) { return ix ? ix->rep : nullptr; }
 pb_index *pb_rank_of(pb_index *ix, int r) { return ix->dep ? pb_dep_rank(ix->dep, r) : ix; }
+bool pb_host_rows_shared(pb_index *ix) { return pb_rank_of(ix, 0)->host_mutable; }
+pb_status pb_sync_devices(pb_index *ix) {
+    pb_status st = PB_OK;
+    auto sync = [&](pb_index *r) {
+        if (st == PB_OK && (cudaSetDevice(r->device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess))
+            st = pb_fail(PB_ERR_CUDA, "synchronizing device %d failed", r->device);
+    };
+    if (ix->dep) pb_dep_each(ix->dep, sync);
+    else sync(ix);
+    return st;
+}
 
 // Every member's writer lock, in member order
 struct MembersLock {
@@ -4998,8 +5139,15 @@ pb_status pb_members_append(const std::vector<pb_index *> &ms, pb_codec *codec, 
     std::vector<std::unique_ptr<AppendPrep>> p;
     for (size_t g = 0; g < ms.size(); ++g) p.emplace_back(new AppendPrep());
     // 1. prepare: member 0 as one handle would (with a codec, the only encode); the others from its encoded rows
-    CKS(append_prepare(ix, codec, embeddings, codes, residuals, doc_lengths, n_docs, space, index_dir != nullptr,
-                       out_first, *p[0]));
+    pb_status st = append_prepare(ix, codec, embeddings, codes, residuals, doc_lengths, n_docs, space,
+                                  index_dir != nullptr, out_first, *p[0]);
+    // host tier: member 0 wrote the rows to the store the members share, and may have moved its segments
+    for (size_t g = 1; g < ms.size() && ix->host_tier; ++g) {
+        CK(cudaSetDevice(ms[g]->device));
+        const pb_status s = ms[g]->host.sync();
+        if (st == PB_OK) st = s;
+    }
+    CKS(st);
     if (p[0]->n == 0) return PB_OK;
     if (ms.size() > 1) {
         const AppendPrep &a = *p[0];
@@ -5008,7 +5156,7 @@ pb_status pb_members_append(const std::vector<pb_index *> &ms, pb_codec *codec, 
         CKS(tail_rows(ix, a.t.N - a.ntok, a.ntok, hc, hr));
         for (size_t g = 1; g < ms.size(); ++g)
             CKS(append_prepare(ms[g], nullptr, nullptr, hc.data(), hr.data(), a.dl.data(), n_docs, PB_MEM_HOST, false,
-                               nullptr, *p[g]));
+                               nullptr, *p[g], false));
     }
     // 2. the directory, once, before any commit: a failure leaves every member as it was
     if (index_dir) {
@@ -5046,10 +5194,11 @@ pb_status pb_members_delete(const std::vector<pb_index *> &ms, const int64_t *do
         CKS(pb_dir_delete(index_dir, p[0]->D0, ix->K, ix->dim, ix->nbits, p[0]->hbits.data(), hivf.data(), p[0]->t.ivf_len,
                           hlen.data()));
     }
-    // from here only a CUDA runtime error can fail a member, and that leaves the set to be reloaded
+    // from here only a CUDA runtime error can fail a member, and that leaves the set to be reloaded.  Host tier: member
+    // 0 moves the rows of the store the members share, and every member's norm pass reads them after it
     for (size_t g = 0; g < ms.size(); ++g) {
         CK(cudaSetDevice(ms[g]->device));
-        CKS(delete_commit(ms[g], *p[g]));
+        CKS(delete_commit(ms[g], *p[g], g == 0));
     }
     if (out_deleted) *out_deleted = p[0]->n_del;
     return PB_OK;
@@ -5273,12 +5422,20 @@ static pb_status sharded_update_body(pb_index *ix, RepTurn &turn, int op, pb_cod
     // a replica other than 0 of an append with a codec: every rank waits for replica 0's encoded rows, so that the
     // group's exchange below does not time out while replica 0 encodes; the last rank appends them
     const bool takes_rows = turn.v && turn.v->share_rows && turn.replica > 0;
+    // host tier: rank r of every replica shares replica 0's rank r's row store, which only replica 0 writes
+    const bool write_rows = !(ix->host_tier && turn.v && turn.replica > 0);
     pb_status rows_st = PB_OK;
     if (takes_rows) {
         const std::vector<int64_t> *dl = nullptr, *cd = nullptr;
         const std::vector<uint8_t> *rs = nullptr;
         rows_st = turn.rows(dl, cd, rs);
         if (rows_st == PB_OK) codes = cd->data(), residuals = rs->data(), doc_lengths = dl->data(), space = PB_MEM_HOST;
+        // replica 0's prepare may have moved the store's segments, whether it then failed or not
+        if (ix->host_tier) {
+            pb_status s = cudaSetDevice(ix->device) == cudaSuccess ? ix->host.sync()
+                                                                    : pb_fail(PB_ERR_CUDA, "cudaSetDevice failed");
+            if (rows_st == PB_OK) rows_st = s;
+        }
     }
     // 1. local checks, the fingerprint of the arguments, and the prepare: no early return, or the peers would wait
     auto local = [&]() -> pb_status {
@@ -5305,7 +5462,7 @@ static pb_status sharded_update_body(pb_index *ix, RepTurn &turn, int op, pb_cod
             rec[LR_OWN] = dp.n_del;
         } else if (last) {
             CKS(append_prepare(ix, takes_rows ? nullptr : codec, embeddings, codes, residuals, doc_lengths, n, space,
-                               index_dir != nullptr, nullptr, ap));
+                               index_dir != nullptr, nullptr, ap, write_rows));
         }
         return PB_OK;
     };
@@ -5367,7 +5524,10 @@ static pb_status sharded_update_body(pb_index *ix, RepTurn &turn, int op, pb_cod
 
     // 4. commit everywhere: from here only a CUDA runtime error can fail a rank, and that leaves the group inconsistent
     if (op == SH_OP_DELETE) {
-        CKS(delete_commit(ix, dp));
+        CKS(delete_move(ix, dp, write_rows));
+        // host tier: every replica's norm pass reads the rows replica 0 has just moved
+        if (ix->host_tier && turn.v) CKS(turn.vote(PB_OK));
+        CKS(delete_finish(ix, dp));
         ix->doc_id_base -= del_before;
         if (out) *out = n_del;
     } else if (last) {

@@ -160,6 +160,10 @@ void pb_index_set_rep_vote(pb_index *member, RepVote *v, int replica);
 // the set behind a handle (null for any other handle); rank r of a deployment's handle (the handle itself otherwise)
 Replicas *pb_replicas_of(const pb_index *ix);
 pb_index *pb_rank_of(pb_index *ix, int r);
+// a mutable host-tier handle or deployment: the replicas of a set write one shared row store, through replica 0 only
+bool pb_host_rows_shared(pb_index *ix);
+// cudaDeviceSynchronize on the device of ix, or of each of its ranks
+pb_status pb_sync_devices(pb_index *ix);
 // pb_index_open without the per-token arrays; follow with pb_index_upload_tokens per chunk.
 pb_status pb_index_open_begin(const pb_index_desc *d, pb_index **out);
 pb_status pb_index_upload_tokens(pb_index *ix, long long tok_off, const int64_t *codes, const uint8_t *residuals,

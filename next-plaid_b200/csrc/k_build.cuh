@@ -756,12 +756,12 @@ __global__ void k_ivf_range_write(const long long *__restrict__ slab, long long 
 // In-place compaction of a per-token (or per-distinct-code) array, one window of survivors [j0, j1) at a time: survivor
 // j's rows old_off[kept[j]] .. old_off[kept[j] + 1] go to staging at new_off[j] - new_off[j0], and the caller then
 // copies the staging to new_off[j0].  One warp per doc, V-wide accesses (row_bytes * every offset is a multiple of
-// sizeof(V)).
+// sizeof(V)).  src is a device array (FlatRows) or a host-tier handle's pinned segments (SegRows).
 // Invariant: new_off[j] <= old_off[kept[j]] for every j (a survivor only moves down), so a window's writes end at
 // new_off[j1] <= old_off[kept[j1]], where the next window's reads begin: windows in ascending order never read rows an
 // earlier window overwrote, and the staging is never more than one window.
-template <class V>
-__global__ void k_compact_gather(const uint8_t *__restrict__ src, const long long *__restrict__ old_off,
+template <class V, class Src>
+__global__ void k_compact_gather(Src src, const long long *__restrict__ old_off,
                                  const long long *__restrict__ kept, const long long *__restrict__ new_off, long long j0,
                                  long long j1, int row_bytes, uint8_t *__restrict__ stage) {
     const int lane = threadIdx.x & 31;
@@ -770,9 +770,8 @@ __global__ void k_compact_gather(const uint8_t *__restrict__ src, const long lon
     for (long long j = j0 + (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); j < j1; j += nw) {
         const long long d = kept[j], o = old_off[d];
         const long long nv = (old_off[d + 1] - o) * row_bytes / (long long)sizeof(V);
-        const V *in = reinterpret_cast<const V *>(src + o * row_bytes);
         V *out = reinterpret_cast<V *>(stage + (new_off[j] - s0) * row_bytes);
-        for (long long k = lane; k < nv; k += 32) out[k] = in[k];
+        for (long long k = lane; k < nv; k += 32) out[k] = *src.template at<V>(o * row_bytes + k * (long long)sizeof(V));
     }
 }
 

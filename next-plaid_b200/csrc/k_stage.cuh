@@ -34,14 +34,15 @@ __global__ void __launch_bounds__(256) k_stage_layout(const int *__restrict__ nk
 }
 
 // One warp per slot: the rows [doc_off[d], doc_off[d + 1]) of doc d = kept[s] go to staged rows [soff[s], ..).  The
-// packed residuals come from mapped host memory in V-sized words (16 bytes when the row length allows), U loads in flight
-// per lane before the stores, since this kernel's PCIe read rate sets the speed of the tier; codes and 1 / |v| (inv_norm
-// may be NULL) come from their device arrays.  nkept == NULL: every slot of [0, n_slots) holds a doc.  No launch bounds:
-// with __launch_bounds__(256) ptxas spills the uint4 form at 40 registers; without, it takes 56 and spills nothing.
+// packed residuals come from the mapped host segments in V-sized words (16 bytes when the row length allows), each
+// located through the segment table, U loads in flight per lane before the stores, since this kernel's PCIe read rate
+// sets the speed of the tier; codes and 1 / |v| (inv_norm may be NULL) come from their device arrays.  nkept == NULL:
+// every slot of [0, n_slots) holds a doc.  No launch bounds: with __launch_bounds__(256) ptxas spills the uint4 form at
+// 40 registers; without, it takes 56 and spills nothing.
 template <class V, int U>
 __global__ void k_stage_rows(const uint32_t *__restrict__ kept, const int *__restrict__ nkept, int Mcap, long long n_slots,
                              const long long *__restrict__ doc_off, const long long *__restrict__ soff,
-                             const uint8_t *host_res, const uint32_t *__restrict__ codes,
+                             SegRows host_res, const uint32_t *__restrict__ codes,
                              const float *__restrict__ inv_norm, int packed, uint8_t *__restrict__ s_res,
                              uint32_t *__restrict__ s_codes, float *__restrict__ s_inv) {
     const int lane = threadIdx.x & 31;
@@ -58,17 +59,17 @@ __global__ void k_stage_rows(const uint32_t *__restrict__ kept, const int *__res
             if (inv_norm) s_inv[t0 + t] = inv_norm[g0 + t];
         }
         const long long nv = len * packed / (long long)sizeof(V);
-        const V *src = reinterpret_cast<const V *>(host_res + (size_t)g0 * packed);
+        const long long b0 = g0 * packed;
         V *dst = reinterpret_cast<V *>(s_res + (size_t)t0 * packed);
         long long i = lane;
         for (; i + 32 * (U - 1) < nv; i += 32 * U) {
             V r[U];
 #pragma unroll
-            for (int u = 0; u < U; ++u) r[u] = src[i + 32 * u];
+            for (int u = 0; u < U; ++u) r[u] = *host_res.at<V>(b0 + (i + 32 * u) * (long long)sizeof(V));
 #pragma unroll
             for (int u = 0; u < U; ++u) dst[i + 32 * u] = r[u];
         }
-        for (; i < nv; i += 32) dst[i] = src[i];
+        for (; i < nv; i += 32) dst[i] = *host_res.at<V>(b0 + i * (long long)sizeof(V));
     }
 }
 

@@ -215,9 +215,19 @@ pb_status pb_rep_memory(Replicas *rs, int64_t *device_bytes, int64_t *host_bytes
     return PB_OK;
 }
 
+// A mutable host-tier set: replica 0 grows and rewrites the row stores every replica reads, so no replica may have
+// work in flight when a mutation starts (the set's writer lock keeps new work out until it ends)
+static pb_status quiesce(Replicas *rs) {
+    if (!pb_host_rows_shared(rs->members[0])) return PB_OK;
+    for (pb_index *m : rs->members)
+        if (pb_status s = pb_sync_devices(m)) return s;
+    return PB_OK;
+}
+
 pb_status pb_rep_delete(Replicas *rs, const int64_t *doc_ids, int64_t n_ids, const char *index_dir, int64_t *out_deleted) {
     std::lock_guard<std::mutex> g(rs->gate);
     std::unique_lock<std::shared_mutex> wr(rs->rw);
+    if (pb_status s = quiesce(rs)) return s;
     if (rs->S == 1) return pb_members_delete(rs->members, doc_ids, n_ids, index_dir, out_deleted);
     // replica 0 writes the directory
     return rs->voted(index_dir != nullptr, false, [&](pb_index *m, int r) {
@@ -233,11 +243,14 @@ pb_status pb_rep_append(Replicas *rs, pb_codec *codec, const float *embeddings, 
                         const char *index_dir, int64_t batch_size, int64_t *out_first_doc_id) {
     std::lock_guard<std::mutex> g(rs->gate);
     std::unique_lock<std::shared_mutex> wr(rs->rw);
+    if (pb_status s = quiesce(rs)) return s;
     if (rs->S == 1)
         return pb_members_append(rs->members, codec, embeddings, codes, residuals, doc_lengths, n_docs, memory_space,
                                  index_dir, batch_size, out_first_doc_id);
-    // with a codec replica 0's last rank encodes and writes the directory; the other replicas append its rows
-    return rs->voted(index_dir != nullptr, codec != nullptr, [&](pb_index *m, int r) -> pb_status {
+    // with a codec replica 0's last rank encodes and writes the directory; the other replicas append its rows.  On a
+    // mutable host tier they also wait for it without a codec: its prepare writes the rows they read
+    return rs->voted(index_dir != nullptr, codec != nullptr || pb_host_rows_shared(rs->members[0]),
+                     [&](pb_index *m, int r) -> pb_status {
         if (r == 0)
             return codec ? pb_index_append(m, codec, embeddings, doc_lengths, n_docs, memory_space, index_dir, batch_size,
                                            out_first_doc_id)
@@ -251,6 +264,7 @@ pb_status pb_rep_append(Replicas *rs, pb_codec *codec, const float *embeddings, 
 pb_status pb_rep_reserve(Replicas *rs, int64_t num_documents, int64_t num_embeddings) {
     std::lock_guard<std::mutex> g(rs->gate);
     std::unique_lock<std::shared_mutex> wr(rs->rw);
+    if (pb_status s = quiesce(rs)) return s;
     return rs->each([&](pb_index *m, int) { return pb_index_reserve(m, num_documents, num_embeddings); });
 }
 

@@ -104,7 +104,12 @@ EXPORTS = [
     "pb_index_load_replicas", "pb_index_replica_layout", "pb_index_replica_stats",
 ]
 
-PB_OPEN_ADOPT_RESIDUALS, PB_OPEN_HOST_RESIDUALS = 1, 2
+PB_OPEN_ADOPT_RESIDUALS, PB_OPEN_HOST_RESIDUALS, PB_OPEN_HOST_MUTABLE = 1, 2, 4
+
+
+def _host_flags(host_residuals: bool, mutable: bool) -> int:
+    """pb_index_desc.flags of host_residuals / mutable (mutable alone is refused by the library: PB_ERR_INVALID)"""
+    return (PB_OPEN_HOST_RESIDUALS if host_residuals else 0) | (PB_OPEN_HOST_MUTABLE if mutable else 0)
 
 _lib = None
 
@@ -451,43 +456,47 @@ class MmapIndex:
 
     # -- construction ----------------------------------------------------------------------
     @classmethod
-    def load(cls, index_path: str, device: int = 0, host_residuals: bool = False) -> "MmapIndex":
+    def load(cls, index_path: str, device: int = 0, host_residuals: bool = False,
+             mutable: bool = False) -> "MmapIndex":
         """MmapIndex::load (index.rs:1026): reads the reference's index directory.  host_residuals: the packed
         residuals go to pinned host memory instead of the device (PB_OPEN_HOST_RESIDUALS; same results, slower search,
-        no appends or deletes)."""
+        no appends or deletes unless mutable).  mutable: with host_residuals only, appends, deletes and reserve work
+        on the handle, its pinned rows growing in segments (PB_OPEN_HOST_MUTABLE)."""
         L = load_library()
         h = C.c_void_p()
-        if host_residuals:
-            _check(L.pb_index_load_range_flags(os.fsencode(index_path), device, 0, -1, PB_OPEN_HOST_RESIDUALS,
-                                               C.byref(h)))
+        flags = _host_flags(host_residuals, mutable)
+        if flags:
+            _check(L.pb_index_load_range_flags(os.fsencode(index_path), device, 0, -1, flags, C.byref(h)))
         else:
             _check(L.pb_index_load(os.fsencode(index_path), device, C.byref(h)))
         return cls(h.value, index_path)
 
     @classmethod
     def load_range(cls, index_path: str, doc_begin: int, doc_end: int, device: int = 0,
-                   host_residuals: bool = False) -> "MmapIndex":
+                   host_residuals: bool = False, mutable: bool = False) -> "MmapIndex":
         """pb_index_load_range: documents [doc_begin, doc_end) of the directory as one shard of a doc-sharded
         deployment (doc_id_base = doc_begin, so search returns global ids).  Reads only that range's chunk rows.
-        host_residuals: as for load."""
+        host_residuals, mutable: as for load."""
         h = C.c_void_p()
         L = load_library()
-        if host_residuals:
-            _check(L.pb_index_load_range_flags(os.fsencode(index_path), device, doc_begin, doc_end,
-                                               PB_OPEN_HOST_RESIDUALS, C.byref(h)))
+        flags = _host_flags(host_residuals, mutable)
+        if flags:
+            _check(L.pb_index_load_range_flags(os.fsencode(index_path), device, doc_begin, doc_end, flags, C.byref(h)))
         else:
             _check(L.pb_index_load_range(os.fsencode(index_path), device, doc_begin, doc_end, C.byref(h)))
         return cls(h.value, index_path)
 
     @classmethod
-    def load_devices(cls, index_path: str, devices: Sequence[int], host_residuals: bool = False) -> "MmapIndex":
+    def load_devices(cls, index_path: str, devices: Sequence[int], host_residuals: bool = False,
+                     mutable: bool = False) -> "MmapIndex":
         """pb_index_load_devices: the directory doc-sharded over `devices` of this process (rank r holds the r-th range
         of shard_bounds(index_path, len(devices)) on devices[r]; devices may repeat) behind one handle.  Every method
-        then works as on a handle from load, with the same results; the ranks and their threads live in the library."""
+        then works as on a handle from load, with the same results; the ranks and their threads live in the library.
+        host_residuals, mutable: as for load, on every rank."""
         dv = np.ascontiguousarray(list(devices), np.int32)
         h = C.c_void_p()
         _check(load_library().pb_index_load_devices(os.fsencode(index_path), _ptr(dv), len(dv),
-                                                    PB_OPEN_HOST_RESIDUALS if host_residuals else 0, C.byref(h)))
+                                                    _host_flags(host_residuals, mutable), C.byref(h)))
         ix = cls(h.value, index_path)
         ix._world = len(dv)
         return ix
@@ -503,15 +512,16 @@ class MmapIndex:
 
     @classmethod
     def load_replicas(cls, index_path: str, devices: Sequence[int], shards: int = 1,
-                      host_residuals: bool = False) -> "MmapIndex":
+                      host_residuals: bool = False, mutable: bool = False) -> "MmapIndex":
         """pb_index_load_replicas: len(devices) / shards full copies of the directory behind one handle, replica g on
         devices[g * shards : (g + 1) * shards] (a plain handle when shards == 1, else a doc-sharded deployment; devices
         may repeat).  Searches are spread over the replicas, mutations applied to all of them at once; every method
-        works as on a handle from load (shards == 1) or load_devices, with the same results."""
+        works as on a handle from load (shards == 1) or load_devices, with the same results.  host_residuals: the
+        replicas share one copy of the rows in pinned host memory; mutable: as for load."""
         dv = np.ascontiguousarray(list(devices), np.int32)
         h = C.c_void_p()
         _check(load_library().pb_index_load_replicas(os.fsencode(index_path), _ptr(dv), len(dv), shards,
-                                                     PB_OPEN_HOST_RESIDUALS if host_residuals else 0, C.byref(h)))
+                                                     _host_flags(host_residuals, mutable), C.byref(h)))
         ix = cls(h.value, index_path)
         ix._world = shards
         return ix
@@ -534,17 +544,18 @@ class MmapIndex:
 
     @classmethod
     def load_shard(cls, index_path: str, rank: int, world: int, device: int = 0,
-                   host_residuals: bool = False) -> "MmapIndex":
+                   host_residuals: bool = False, mutable: bool = False) -> "MmapIndex":
         """Shard `rank` of `world` of the directory: load_range over shard_bounds(index_path, world)."""
         if not 0 <= rank < world:
             raise PlaidError(PB_ERR_INVALID, f"rank {rank} outside [0, {world})")
         b = shard_bounds(index_path, world)
-        return cls.load_range(index_path, int(b[rank]), int(b[rank + 1]), device, host_residuals)
+        return cls.load_range(index_path, int(b[rank]), int(b[rank + 1]), device, host_residuals, mutable)
 
     @classmethod
     def from_arrays(cls, centroids, bucket_weights, codes, residuals, doc_lengths, ivf, ivf_lengths,
-                    nbits: int, device: int = 0, doc_id_base: int = 0, host_residuals: bool = False) -> "MmapIndex":
-        """pb_index_open from host arrays in the reference's dtypes.  host_residuals: as for load."""
+                    nbits: int, device: int = 0, doc_id_base: int = 0, host_residuals: bool = False,
+                    mutable: bool = False) -> "MmapIndex":
+        """pb_index_open from host arrays in the reference's dtypes.  host_residuals, mutable: as for load."""
         L = load_library()
         cen = np.ascontiguousarray(centroids, np.float32)
         w = np.ascontiguousarray(bucket_weights, np.float32)
@@ -556,7 +567,7 @@ class MmapIndex:
         il = None if ivf_lengths is None else np.ascontiguousarray(ivf_lengths, np.int32)
         d = _Desc(cen.shape[1], nbits, cen.shape[0], len(dl), len(cd), _ptr(cen), _ptr(w), _ptr(cd),
                   _ptr(rs), _ptr(dl), _ptr(iv), _ptr(il), device, 0, doc_id_base,
-                  PB_OPEN_HOST_RESIDUALS if host_residuals else 0)
+                  _host_flags(host_residuals, mutable))
         h = C.c_void_p()
         _check(L.pb_index_open(C.byref(d), C.byref(h)))
         return cls(h.value)
@@ -564,13 +575,13 @@ class MmapIndex:
     @classmethod
     def from_device_pointers(cls, dim, nbits, K, D, N, centroids, bucket_weights, codes, residuals,
                              doc_lengths, ivf, ivf_lengths, device: int = 0, doc_id_base: int = 0,
-                             adopt_residuals: bool = False, host_residuals: bool = False):
+                             adopt_residuals: bool = False, host_residuals: bool = False, mutable: bool = False):
         """pb_index_open with PB_MEM_DEVICE pointers (integers), e.g. torch tensors' data_ptr().  ivf = ivf_lengths
         = None: the inverted file is built on the device (index.rs:850-873).  adopt_residuals: the packed residuals
         are used in place (keep the array alive until close()).  host_residuals: they are copied to pinned host
-        memory, as for load."""
+        memory, as for load; mutable: as for load."""
         L = load_library()
-        flags = (PB_OPEN_ADOPT_RESIDUALS if adopt_residuals else 0) | (PB_OPEN_HOST_RESIDUALS if host_residuals else 0)
+        flags = (PB_OPEN_ADOPT_RESIDUALS if adopt_residuals else 0) | _host_flags(host_residuals, mutable)
         d = _Desc(dim, nbits, K, D, N, centroids, bucket_weights, codes, residuals, doc_lengths, ivf,
                   ivf_lengths, device, 1, doc_id_base, flags)
         h = C.c_void_p()

@@ -149,6 +149,8 @@ extern "C" {
 
 /// pb_index_desc.flags: the packed residuals in pinned host memory, the kept docs' rows staged per search (DESIGN §4j).
 pub const PB_OPEN_HOST_RESIDUALS: i32 = 2;
+/// with `PB_OPEN_HOST_RESIDUALS` only: appends and deletes work on the host-tier handle (DESIGN §4r)
+pub const PB_OPEN_HOST_MUTABLE: i32 = 4;
 
 fn last_error() -> String {
     unsafe { CStr::from_ptr(pb_last_error()).to_string_lossy().into_owned() }
