@@ -169,6 +169,40 @@ PB_API int32_t pb_index_device(const pb_index *ix);
  * N * dim * nbits / 8 until a PB_OPEN_HOST_MUTABLE mutation grows it by whole segments, else 0).  Either may be NULL. */
 PB_API pb_status pb_index_memory(const pb_index *ix, int64_t *device_bytes, int64_t *host_bytes);
 
+/* Device cache of packed residual rows for a PB_OPEN_HOST_RESIDUALS handle (DESIGN.md 4s).  Search staging copies a
+ * cached doc's rows device to device instead of reading them over PCIe; results, counts and pb_work_counters are the
+ * same at every cache state.  Off by default; with the cache off nothing about the handle changes.
+ *
+ * pb_index_set_row_cache: the budget, in bytes of rows, on the handle's device; 0 = off, the default.  A budget
+ *   allocates two per-doc arrays (an i64 map to each doc's offset in the cache, a u32 count of how often search staging
+ *   kept the doc), which appends grow and deletes compact with the other per-doc arrays; 0 frees them and the cache.
+ *   A budget below the bytes the cache holds (cached_bytes + dead_bytes) empties it.  PB_ERR_UNSUPPORTED on a resident
+ *   handle or one opened with PB_OPEN_ADOPT_RESIDUALS; PB_ERR_INVALID for max_bytes < 0; PB_ERR_NOMEM when the arrays
+ *   cannot be allocated, with the handle as it was.
+ * pb_index_fill_row_cache: replaces the cached set.  doc_ids == NULL: the docs with a nonzero count, most kept first and
+ *   ties by ascending id, then the counts reset; else the n_ids ids in the caller's order, ids outside the handle's range
+ *   and repeats ignored.  Each doc is taken when its rows still fit the budget and skipped otherwise.  out_ids (may be
+ *   NULL) receives at most out_cap of the cached ids in the order they were taken, *out_n their number.  The new cache
+ *   is built out of place while searches run on the old one (mutations wait), then swapped in, so a search sees the old
+ *   set or the new one: the peak is the old cache plus the new one.  Docs already cached are copied device to device.
+ *   Every allocation comes before the swap; a failure leaves the old cache in place.  PB_ERR_INVALID without a budget.
+ * pb_index_row_cache_stats: the fields below; reset != 0 clears the staging counters after the read.
+ * A delete keeps the survivors' map entries and counts; a deleted doc's cached rows count as dead_bytes until the next
+ *   fill.  Appended docs are not cached.  pb_index_memory counts the cache, the map and the counts while they exist.
+ * pb_index_load_devices: per rank, each on its device; a fill by counts fills every rank from its own counts, a fill
+ *   with ids gives every rank the ids in its range; out_ids lists rank 0's ids first.  A replica set: every replica has
+ *   its own cache and counts, set and filled under the set's writer lock; out_ids lists replica 0's ids first.  Stats
+ *   are sums over the ranks or replicas. */
+typedef struct pb_row_cache_stats {
+    int64_t budget_bytes, cached_docs, cached_bytes, dead_bytes;  /* dead: rows of docs deleted since the fill */
+    int64_t staged_docs, hit_docs, hit_bytes;                      /* search staging since the last reset */
+    float last_fill_ms;                                            /* wall time of the last fill */
+} pb_row_cache_stats;
+PB_API pb_status pb_index_set_row_cache(pb_index *ix, int64_t max_bytes);
+PB_API pb_status pb_index_fill_row_cache(pb_index *ix, const int64_t *doc_ids, int64_t n_ids,
+                                         int64_t *out_ids /* may be NULL */, int64_t out_cap, int64_t *out_n);
+PB_API pb_status pb_index_row_cache_stats(pb_index *ix, pb_row_cache_stats *out, int32_t reset);
+
 /* ---- incremental append ------------------------------------------------------------------ */
 
 typedef struct pb_codec pb_codec;

@@ -280,6 +280,16 @@ pb_status pb_dep_delete(Deployment *d, const int64_t *doc_ids, int64_t n_ids, co
     return s;
 }
 
+pb_status pb_dep_ranks(Deployment *d, const std::function<pb_status(pb_index *)> &call) {
+    std::shared_lock<std::shared_mutex> g(d->layout);
+    for (int r = 0; r < d->world(); ++r)
+        if (pb_status s = call(d->ranks[r])) {
+            const std::string e = pb_last_error();
+            return d->world() == 1 ? s : pb_fail(s, "rank %d: %s", r, e.c_str());
+        }
+    return PB_OK;
+}
+
 // Only the last rank receives the codec and the documents: an append goes to the end of the deployment
 pb_status pb_dep_append(Deployment *d, pb_codec *codec, const float *embeddings, const int64_t *codes,
                         const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,

@@ -546,6 +546,7 @@ struct Workspace {
     DevBuf subspan, qsub, listn, eligcnt, xrec, xall, gelig;
     // host tier: the staged rows of the kept docs (residuals, codes, 1 / |v|), their slot offsets and slot list
     DevBuf s_res, s_codes, s_inv, soff, kept_s;
+    DevBuf rc_hits;  // with a row cache: the slots staged from it and their bytes, this pass
     cudaEvent_t sev[2] = {};  // around the staging kernels
     HostBuf hq, hres, hcounts;
     pb_status init() {
@@ -616,11 +617,25 @@ struct DocArrays : DocTotals {
     DevBuf codes, residuals, doc_off, ucodes, udoc_off, ivf, ivf_off;
     DevBuf tok_inv_norm;               // [N] 1 / |c + w| for the linear estimate (k_maxsim_tc)
     DevBuf ivf_spare, ivf_off_spare;   // the other half of the inverted file's ping-pong: append / delete write into it
+    // host tier with a row cache (pb_index_set_row_cache, DESIGN.md 4s): [D] i64 token offset of each doc's rows in the
+    // cache or -1, and [D] u32 how often search staging kept each doc since the last fill by counts; empty otherwise
+    DevBuf cache_off, kept_count;
     // every buffer, in one list (the memory count and the rebalance's swap walk it)
     template <class A> static auto buffers(A &a) {
         return std::array{&a.codes, &a.residuals, &a.doc_off, &a.ucodes, &a.udoc_off, &a.ivf,
-                          &a.ivf_off, &a.tok_inv_norm, &a.ivf_spare, &a.ivf_off_spare};
+                          &a.ivf_off, &a.tok_inv_norm, &a.ivf_spare, &a.ivf_off_spare, &a.cache_off, &a.kept_count};
     }
+};
+
+// The rest of a host-tier handle's row cache: the rows, the budget they fit, what they hold, and the search staging
+// counters since the last reset.  The map and the counts are per-doc arrays (DocArrays).
+struct RowCacheState {
+    size_t budget = 0;       // 0: off, and cache_off / kept_count are empty
+    DevBuf rows;             // the cached docs' packed rows, each doc's at a token offset
+    long long docs = 0, bytes = 0, dead = 0;  // live cached docs and their row bytes; bytes of docs deleted since the fill
+    float fill_ms = 0.f;
+    std::atomic<long long> staged{0}, hit_docs{0}, hit_bytes{0};
+    std::mutex fill_mu;      // one pb_index_set_row_cache / pb_index_fill_row_cache at a time
 };
 
 struct pb_index : DocArrays {
@@ -632,6 +647,8 @@ struct pb_index : DocArrays {
     bool host_tier = false;    // PB_OPEN_HOST_RESIDUALS: `residuals` stays empty, the rows live in host.rows
     bool host_mutable = false; // PB_OPEN_HOST_MUTABLE: appends and deletes write the host rows
     HostTier host;
+    RowCacheState rc;
+    unsigned long long doc_gen = 0;  // changes with every publish: a fill built out of place checks it before its swap
     bool build_ivf = false;    // no inverted file was given: built from the codes at finalize (index.rs:850-873)
     float cmax = 1.0f;         // largest centroid L2 norm (range of the 16-bit score table)
     bool fast_approx = true;   // two-pass approximate stage (exact cut either way)
@@ -1422,7 +1439,7 @@ extern "C" pb_status pb_index_memory(const pb_index *ix, int64_t *device_bytes, 
     if (ix->dep) return pb_dep_memory(ix->dep, device_bytes, host_bytes);
     if (ix->rep) return pb_rep_memory(ix->rep, device_bytes, host_bytes);
     auto rd = ix->read_lock();
-    size_t dev = ix->centroids.cap + ix->w_rev.cap + ix->cent_h16t.cap + ix->cent_l16t.cap;
+    size_t dev = ix->centroids.cap + ix->w_rev.cap + ix->cent_h16t.cap + ix->cent_l16t.cap + ix->rc.rows.cap;
     for (const DevBuf *b : DocArrays::buffers(*ix))
         if (b->owned) dev += b->cap;  // adopted residuals are the caller's allocation
     if (device_bytes) *device_bytes = (int64_t)dev;
@@ -2754,34 +2771,56 @@ static pb_status cut(pb_index *ix, Workspace &ws, const SearchPlan &plan, const 
     return PB_OK;
 }
 
+// k_stage_rows in the form the row length allows, on st: the rows of docs[s] for the slots s of [0, n_slots) (nkept !=
+// NULL: slot b Mcap + j only for j < nkept[b]) to s_res / s_codes / s_inv at soff[s] (s_codes == NULL: rows only)
+static pb_status launch_stage_rows(pb_index *ix, cudaStream_t st, const uint32_t *docs, const int *nkept, int Mcap,
+                                   long long n_slots, const long long *soff, RowCache cache, uint8_t *s_res,
+                                   uint32_t *s_codes, float *s_inv) {
+    const int pk = ix->packed, grid = ix->sm_count * 8;
+    const float *src_inv = s_inv ? ix->tok_inv_norm.as<float>() : nullptr;
+    const long long *doff = ix->doc_off.as<long long>();
+    const uint32_t *codes = ix->codes.as<uint32_t>();
+    if (pk % 16 == 0)
+        k_stage_rows<uint4, 4><<<grid, 256, 0, st>>>(docs, nkept, Mcap, n_slots, doff, soff, ix->host.dev(), cache, codes,
+                                                     src_inv, pk, s_res, s_codes, s_inv);
+    else if (pk % 4 != 0)  // 1-bit rows of dim 48 (6 bytes)
+        k_stage_rows<unsigned short, 8><<<grid, 256, 0, st>>>(docs, nkept, Mcap, n_slots, doff, soff, ix->host.dev(), cache,
+                                                              codes, src_inv, pk, s_res, s_codes, s_inv);
+    else
+        k_stage_rows<uint32_t, 8><<<grid, 256, 0, st>>>(docs, nkept, Mcap, n_slots, doff, soff, ix->host.dev(), cache,
+                                                        codes, src_inv, pk, s_res, s_codes, s_inv);
+    CK(cudaGetLastError());
+    return PB_OK;
+}
+
+// The handle's row cache as k_stage_rows reads it; count: also the keep counts and the workspace's hit counters
+// (search staging only)
+static RowCache row_cache_view(const pb_index *ix, Workspace *ws, bool count) {
+    if (!ix->cache_off.p) return RowCache{nullptr, FlatRows{nullptr}, nullptr, nullptr};
+    return RowCache{ix->cache_off.as<const long long>(), FlatRows{ix->rc.rows.as<uint8_t>()},
+                    count ? ix->kept_count.as<uint32_t>() : nullptr,
+                    count ? ws->rc_hits.as<unsigned long long>() : nullptr};
+}
+
 // The rows of docs[s] for the slots s of [0, n_slots) (nkept != NULL: slot b Mcap + j only for j < nkept[b]) from the
-// pinned host residuals and the device codes / 1 / |v| into the workspace's staging buffers at soff[s]; cap_tok bounds
-// the staged tokens.  Returns the staged arrays as a TokView whose doc_off is soff (indexed by slot).
+// row cache or the pinned host residuals, and the device codes / 1 / |v|, into the workspace's staging buffers at
+// soff[s]; cap_tok bounds the staged tokens.  count: a search's staging, which the row cache counts.  Returns the
+// staged arrays as a TokView whose doc_off is soff (indexed by slot).
 static pb_status stage_rows(pb_index *ix, Workspace &ws, const uint32_t *docs, const int *nkept, int Mcap, long long n_slots,
-                            const long long *soff, long long cap_tok, TokView &tv) {
+                            const long long *soff, long long cap_tok, bool count, TokView &tv) {
     const int pk = ix->packed;
     const bool inv = ix->tok_inv_norm.p != nullptr;
     cap_tok = std::max(cap_tok, 1ll);
     CKS(ws.s_res.ensure((size_t)cap_tok * pk));
     CKS(ws.s_codes.ensure((size_t)cap_tok * 4));
     if (inv) CKS(ws.s_inv.ensure((size_t)cap_tok * 4));
-    const int grid = ix->sm_count * 8;
-    const float *src_inv = inv ? ix->tok_inv_norm.as<float>() : nullptr;
     float *dst_inv = inv ? ws.s_inv.as<float>() : nullptr;
-    if (pk % 16 == 0)
-        k_stage_rows<uint4, 4><<<grid, 256, 0, ws.stream>>>(docs, nkept, Mcap, n_slots, ix->doc_off.as<long long>(), soff,
-                                                            ix->host.dev(), ix->codes.as<uint32_t>(), src_inv, pk,
-                                                            ws.s_res.as<uint8_t>(), ws.s_codes.as<uint32_t>(), dst_inv);
-    else if (pk % 4 != 0)  // 1-bit rows of dim 48 (6 bytes)
-        k_stage_rows<unsigned short, 8><<<grid, 256, 0, ws.stream>>>(docs, nkept, Mcap, n_slots, ix->doc_off.as<long long>(),
-                                                                     soff, ix->host.dev(), ix->codes.as<uint32_t>(), src_inv,
-                                                                     pk, ws.s_res.as<uint8_t>(), ws.s_codes.as<uint32_t>(),
-                                                                     dst_inv);
-    else
-        k_stage_rows<uint32_t, 8><<<grid, 256, 0, ws.stream>>>(docs, nkept, Mcap, n_slots, ix->doc_off.as<long long>(), soff,
-                                                               ix->host.dev(), ix->codes.as<uint32_t>(), src_inv, pk,
-                                                               ws.s_res.as<uint8_t>(), ws.s_codes.as<uint32_t>(), dst_inv);
-    CK(cudaGetLastError());
+    if (count && ix->cache_off.p) {
+        CKS(ws.rc_hits.ensure(16));
+        CK(cudaMemsetAsync(ws.rc_hits.p, 0, 16, ws.stream));
+    }
+    CKS(launch_stage_rows(ix, ws.stream, docs, nkept, Mcap, n_slots, soff, row_cache_view(ix, &ws, count),
+                          ws.s_res.as<uint8_t>(), ws.s_codes.as<uint32_t>(), dst_inv));
     tv = {ws.s_codes.as<uint32_t>(), ws.s_res.as<uint8_t>(), dst_inv, soff};
     return PB_OK;
 }
@@ -2798,7 +2837,8 @@ static pb_status stage_kept(pb_index *ix, Workspace &ws, const SearchPlan &plan,
     k_stage_layout<<<dim3(std::min((Mcap + 255) / 256, 8), B), 256, 0, ws.stream>>>(
         kv.nkept, kv.tokp, B, Mcap, ws.soff.as<long long>(), ws.kept_s.as<uint32_t>());
     CK(cudaGetLastError());
-    CKS(stage_rows(ix, ws, kv.kept, kv.nkept, Mcap, slots, ws.soff.as<long long>(), slots * std::max(ix->max_doclen, 1), tv));
+    CKS(stage_rows(ix, ws, kv.kept, kv.nkept, Mcap, slots, ws.soff.as<long long>(), slots * std::max(ix->max_doclen, 1), true,
+                   tv));
     if (plan.prof) CK(cudaEventRecord(ws.sev[1], ws.stream));
     g_stats.launches[PB_STAGE_EXACT] += 2;
     kv.kept = ws.kept_s.as<uint32_t>();
@@ -3059,6 +3099,16 @@ static pb_status finish(pb_index *ix, Workspace &ws, const SearchIO &io, const S
             float ms = 0.f;
             CK(cudaEventElapsedTime(&ms, ws.sev[0], ws.sev[1]));
             g_stats.staging_ms += ms;
+        }
+        if (ix->cache_off.p) {  // the row cache's staging counters
+            unsigned long long hits[2] = {0, 0};
+            CK(cudaMemcpyAsync(hits, ws.rc_hits.p, 16, cudaMemcpyDeviceToHost, ws.stream));
+            CK(cudaStreamSynchronize(ws.stream));
+            long long kept = 0;
+            for (int b = 0; b < B; ++b) kept += hc.kept[b];
+            ix->rc.staged += kept;
+            ix->rc.hit_docs += (long long)hits[0];
+            ix->rc.hit_bytes += (long long)hits[1];
         }
     }
     return PB_OK;
@@ -3663,7 +3713,7 @@ extern "C" pb_status pb_decompress_documents(pb_index *ix, const int64_t *doc_id
         TokView tv = resident_tokens(ix);
         const uint32_t *list = ddocs.as<uint32_t>() + i0;
         if (ix->host_tier) {
-            CKS(stage_rows(ix, *lease.ws, list, nullptr, nd, nd, dpre.as<long long>(), ntok, tv));
+            CKS(stage_rows(ix, *lease.ws, list, nullptr, nd, nd, dpre.as<long long>(), ntok, false, tv));
             CK(cudaStreamSynchronize(lease.ws->stream));
             list = ident.as<uint32_t>();
         }
@@ -4592,6 +4642,10 @@ static pb_status grow_docs(pb_index *ix, long long D1, long long N1, bool geomet
     if (TcDims::has(ix->dim)) CKS(ix->tok_inv_norm.grow((size_t)N1 * 4, (size_t)ix->N * 4, geometric));
     CKS(ix->doc_off.grow((size_t)(D1 + 1) * 8, (size_t)(ix->D + 1) * 8, geometric));
     CKS(ix->udoc_off.grow((size_t)(D1 + 1) * 8, (size_t)(ix->D + 1) * 8, geometric));
+    if (ix->cache_off.p) {
+        CKS(ix->cache_off.grow((size_t)D1 * 8, (size_t)ix->D * 8, geometric));
+        CKS(ix->kept_count.grow((size_t)D1 * 4, (size_t)ix->D * 4, geometric));
+    }
     return PB_OK;
 }
 
@@ -4606,6 +4660,7 @@ static void publish(pb_index *ix, const DocTotals &t, DocArrays *fresh = nullptr
         ix->ivf_off.swap(ix->ivf_off_spare);
     }
     static_cast<DocTotals &>(*ix) = t;
+    ++ix->doc_gen;
 }
 
 // Every check, allocation and device write of an append that stays invisible until publish.  The caller holds
@@ -4687,8 +4742,12 @@ static pb_status append_prepare(pb_index *ix, pb_codec *codec, const float *embe
         CKS(upload_narrow(ix->codes, N0, codes, ntok, ix->K, space, "codes"));
     }
 
-    // 2. doc offsets
+    // 2. doc offsets; with a row cache the new docs are not cached and have not been kept
     CK(cudaMemcpy(ix->doc_off.as<long long>() + D0 + 1, doff.data() + 1, (size_t)n * 8, cudaMemcpyHostToDevice));
+    if (ix->cache_off.p) {
+        CK(cudaMemset(ix->cache_off.as<long long>() + D0, 0xff, (size_t)n * 8));
+        CK(cudaMemset(ix->kept_count.as<uint32_t>() + D0, 0, (size_t)n * 4));
+    }
 
     // 3. distinct code lists of the new docs, after the old ones
     CKS(unique_codes(ix, D0, n, ix->n_ucodes, &t.n_ucodes));
@@ -4854,6 +4913,8 @@ struct DeletePrep {
     long long D0 = 0, n_del = 0;
     DocTotals t;
     DevBuf bits, wpre, kept, new_doff, new_uoff, st_codes, st_res, st_u, mn;
+    DevBuf cache_off, kept_count;  // with a row cache: the survivors' map and counts under their new ids
+    long long dead_docs = 0, dead_tok = 0;  // the cached docs among the deleted ones, and their tokens
     std::vector<long long> hoff, hu;
     std::vector<uint32_t> hbits;
     std::vector<std::pair<long long, long long>> wins;
@@ -4899,6 +4960,21 @@ static pb_status delete_prepare(pb_index *ix, const int64_t *doc_ids, int64_t n_
     p.t.N = hoff[D1];
     p.t.n_ucodes = hu[D1];
     p.t.max_doclen = longest_doc(hoff, D1);
+    if (ix->cache_off.p) {  // the row cache: survivors keep their entries, deleted cached docs' rows become dead
+        DevBuf dead;
+        CKS(p.cache_off.ensure((size_t)std::max(D1, 1ll) * 8));
+        CKS(p.kept_count.ensure((size_t)std::max(D1, 1ll) * 4));
+        CKS(dead.ensure(16));
+        CK(cudaMemset(dead.p, 0, 16));
+        k_cache_compact<<<grid, 256>>>(ix->cache_off.as<long long>(), ix->kept_count.as<uint32_t>(), p.kept.as<long long>(),
+                                       D1, p.cache_off.as<long long>(), p.kept_count.as<uint32_t>());
+        k_cache_dead<<<grid, 256>>>(ix->cache_off.as<long long>(), p.bits.as<uint32_t>(), ix->doc_off.as<long long>(), D0,
+                                    dead.as<unsigned long long>());
+        CK(cudaGetLastError());
+        long long got[2] = {0, 0};
+        CK(cudaMemcpy(got, dead.p, 16, cudaMemcpyDeviceToHost));
+        p.dead_docs = got[0], p.dead_tok = got[1];
+    }
 
     // 3. the inverted file without the deleted ids, renumbered, into the spare half
     if (ix->profiling) CK(cudaEventRecord(p.ev.e[0]));
@@ -4988,6 +5064,12 @@ static pb_status delete_move(pb_index *ix, DeletePrep &p, bool write_rows) {
     }
     CK(cudaMemcpy(ix->doc_off.p, p.new_doff.p, (size_t)(p.t.D + 1) * 8, cudaMemcpyDeviceToDevice));
     CK(cudaMemcpy(ix->udoc_off.p, p.new_uoff.p, (size_t)(p.t.D + 1) * 8, cudaMemcpyDeviceToDevice));
+    if (ix->cache_off.p) {
+        ix->cache_off.swap(p.cache_off);
+        ix->kept_count.swap(p.kept_count);
+        const long long b = p.dead_tok * ix->packed;
+        ix->rc.docs -= p.dead_docs, ix->rc.bytes -= b, ix->rc.dead += b;
+    }
     if (prof) CK(cudaEventRecord(p.ev.e[3]));
     return PB_OK;
 }
@@ -5024,6 +5106,190 @@ extern "C" pb_status pb_index_delete(pb_index *ix, const int64_t *doc_ids, int64
     if (ix->dep) return pb_dep_delete(ix->dep, doc_ids, n_ids, index_dir, out_deleted);
     if (ix->rep) return pb_rep_delete(ix->rep, doc_ids, n_ids, index_dir, out_deleted);
     return pb_members_delete({ix}, doc_ids, n_ids, index_dir, out_deleted);
+}
+
+// ------------------------------------------------------------------------------------------
+// device row cache of a host-tier handle (DESIGN.md 4s): the rows of a chosen set of docs, in spare device memory, which
+// search staging copies device to device instead of over PCIe
+// ------------------------------------------------------------------------------------------
+static pb_status refuse_row_cache(const pb_index *ix) {
+    if (!ix->residuals.owned)
+        return pb_fail(PB_ERR_UNSUPPORTED, "the handle uses the caller's residual array (PB_OPEN_ADOPT_RESIDUALS)");
+    if (!ix->host_tier)
+        return pb_fail(PB_ERR_UNSUPPORTED, "a row cache serves host-tier handles (PB_OPEN_HOST_RESIDUALS) only");
+    return PB_OK;
+}
+
+// The cache emptied: no rows, every map entry -1.  The caller holds the writer lock.
+static pb_status row_cache_clear(pb_index *ix) {
+    CK(cudaDeviceSynchronize());  // pb_search_batch_device may have left staging work that reads the rows
+    DevBuf().swap(ix->rc.rows);
+    CK(cudaMemset(ix->cache_off.p, 0xff, (size_t)ix->D * 8));
+    ix->rc.docs = ix->rc.bytes = ix->rc.dead = 0;
+    return PB_OK;
+}
+
+extern "C" pb_status pb_index_set_row_cache(pb_index *ix, int64_t max_bytes) {
+    if (max_bytes < 0) return pb_fail(PB_ERR_INVALID, "row cache budget %lld < 0", (long long)max_bytes);
+    if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
+    if (ix->dep) return pb_dep_ranks(ix->dep, [&](pb_index *m) { return pb_index_set_row_cache(m, max_bytes); });
+    if (ix->rep) return pb_rep_members(ix->rep, true, [&](pb_index *m) { return pb_index_set_row_cache(m, max_bytes); });
+    CKS(refuse_row_cache(ix));
+    std::lock_guard<std::mutex> f(ix->rc.fill_mu);
+    DevBuf off, cnt;  // the old arrays leave with these, after the locks
+    std::lock_guard<std::mutex> gate(ix->gate);
+    std::unique_lock<std::shared_mutex> wr(ix->rw);
+    CK(cudaSetDevice(ix->device));
+    if (max_bytes == 0) {
+        if (ix->cache_off.p) CKS(row_cache_clear(ix));
+        ix->cache_off.swap(off);
+        ix->kept_count.swap(cnt);
+        ix->rc.budget = 0;
+        return PB_OK;
+    }
+    if (!ix->cache_off.p) {  // every allocation before the first change
+        CKS(off.ensure((size_t)std::max(ix->D, 1ll) * 8));
+        CKS(cnt.ensure((size_t)std::max(ix->D, 1ll) * 4));
+        CK(cudaMemset(off.p, 0xff, (size_t)ix->D * 8));
+        CK(cudaMemset(cnt.p, 0, (size_t)ix->D * 4));
+        ix->cache_off.swap(off);
+        ix->kept_count.swap(cnt);
+    }
+    ix->rc.budget = (size_t)max_bytes;
+    if ((size_t)(ix->rc.bytes + ix->rc.dead) > ix->rc.budget) CKS(row_cache_clear(ix));
+    return PB_OK;
+}
+
+// The docs a fill caches, in the order it takes them: by counts (doc_ids == NULL) the docs kept at least once, most
+// kept first and ties by id, else the caller's ids in its order, those outside [0, D) and repeats ignored; each taken
+// when its rows still fit the budget, skipped otherwise.  off: their token offsets in the new cache, and the total.
+static void row_cache_pick(const std::vector<long long> &doff, const std::vector<uint32_t> *count, const int64_t *doc_ids,
+                           int64_t n_ids, long long base, long long pk, size_t budget, std::vector<uint32_t> &pick,
+                           std::vector<long long> &off) {
+    const long long D = (long long)doff.size() - 1;
+    std::vector<uint32_t> order;
+    if (count) {
+        for (long long d = 0; d < D; ++d)
+            if ((*count)[d]) order.push_back((uint32_t)d);
+        std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return (*count)[a] > (*count)[b]; });
+    } else {
+        std::vector<uint8_t> seen((size_t)D, 0);
+        for (int64_t i = 0; i < n_ids; ++i) {
+            const long long d = doc_ids[i] - base;
+            if (d < 0 || d >= D || seen[d]) continue;
+            seen[d] = 1;
+            order.push_back((uint32_t)d);
+        }
+    }
+    off.assign(1, 0);
+    for (uint32_t d : order) {
+        const long long len = doff[d + 1] - doff[d];
+        if ((size_t)((off.back() + len) * pk) > budget) continue;
+        pick.push_back(d);
+        off.push_back(off.back() + len);
+    }
+}
+
+// A plain handle's fill: the new map and rows built out of place under the reader lock, so that searches go on with
+// the old cache and mutations wait; then swapped under the writer lock.  A mutation that ran between the two (the
+// reader lock cannot become the writer lock in place) makes the fill start again on the new documents.
+static pb_status row_cache_fill(pb_index *ix, const int64_t *doc_ids, int64_t n_ids, int64_t *out_ids, int64_t out_cap,
+                                int64_t *out_n) {
+    CKS(refuse_row_cache(ix));
+    std::lock_guard<std::mutex> f(ix->rc.fill_mu);
+    const auto t0 = std::chrono::steady_clock::now();
+    for (;;) {
+        std::vector<uint32_t> pick;
+        std::vector<long long> off;
+        DevBuf map, rows, dpick, doff;  // the new cache; after the swap the old one, freed after the locks
+        unsigned long long gen = 0;
+        {
+            auto rd = ix->read_lock();
+            if (!ix->rc.budget) return pb_fail(PB_ERR_INVALID, "the handle has no row cache budget (pb_index_set_row_cache)");
+            CK(cudaSetDevice(ix->device));
+            gen = ix->doc_gen;
+            const long long D = ix->D;
+            std::vector<long long> hoff((size_t)D + 1);
+            CK(cudaMemcpy(hoff.data(), ix->doc_off.p, hoff.size() * 8, cudaMemcpyDeviceToHost));
+            std::vector<uint32_t> count;
+            if (!doc_ids) {
+                count.resize((size_t)D);
+                CK(cudaMemcpy(count.data(), ix->kept_count.p, (size_t)D * 4, cudaMemcpyDeviceToHost));
+            }
+            row_cache_pick(hoff, doc_ids ? nullptr : &count, doc_ids, n_ids, ix->doc_id_base, ix->packed, ix->rc.budget,
+                           pick, off);
+            std::vector<long long> hmap((size_t)D, -1);
+            for (size_t i = 0; i < pick.size(); ++i) hmap[pick[i]] = off[i];
+            CKS(map.ensure((size_t)std::max(D, 1ll) * 8));
+            if (D) CK(cudaMemcpy(map.p, hmap.data(), (size_t)D * 8, cudaMemcpyHostToDevice));
+            const long long tok = off.back();
+            if (tok > 0) {  // the chosen docs' rows: already cached ones device to device, the others over PCIe
+                CKS(rows.grow((size_t)tok * ix->packed, 0, false));
+                CKS(upload(dpick, pick.data(), pick.size() * 4, PB_MEM_HOST));
+                CKS(upload(doff, off.data(), off.size() * 8, PB_MEM_HOST));
+                CKS(launch_stage_rows(ix, 0, dpick.as<uint32_t>(), nullptr, 0, (long long)pick.size(), doff.as<long long>(),
+                                      row_cache_view(ix, nullptr, false), rows.as<uint8_t>(), nullptr, nullptr));
+                CK(cudaStreamSynchronize(0));
+            }
+        }
+        std::lock_guard<std::mutex> gate(ix->gate);
+        std::unique_lock<std::shared_mutex> wr(ix->rw);
+        if (ix->doc_gen != gen) continue;
+        CK(cudaSetDevice(ix->device));
+        CK(cudaDeviceSynchronize());  // pb_search_batch_device may have left staging work that reads the old cache
+        ix->cache_off.swap(map);
+        ix->rc.rows.swap(rows);
+        if (!doc_ids) CK(cudaMemset(ix->kept_count.p, 0, (size_t)ix->D * 4));
+        ix->rc.docs = (long long)pick.size();
+        ix->rc.bytes = off.back() * ix->packed;
+        ix->rc.dead = 0;
+        ix->rc.fill_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+        *out_n = (int64_t)pick.size();
+        for (size_t i = 0; out_ids && i < pick.size() && (int64_t)i < out_cap; ++i)
+            out_ids[i] = (int64_t)pick[i] + ix->doc_id_base;
+        return PB_OK;
+    }
+}
+
+extern "C" pb_status pb_index_fill_row_cache(pb_index *ix, const int64_t *doc_ids, int64_t n_ids, int64_t *out_ids,
+                                             int64_t out_cap, int64_t *out_n) {
+    if (!ix || !out_n || (!doc_ids && n_ids > 0) || (doc_ids && n_ids < 0) || (out_ids && out_cap < 0))
+        return pb_fail(PB_ERR_INVALID, "null argument");
+    *out_n = 0;
+    if (!ix->dep && !ix->rep) return row_cache_fill(ix, doc_ids, n_ids, out_ids, out_cap, out_n);
+    // ranks or replicas in order, each writing its ids after the previous ones'
+    auto one = [&](pb_index *m) {
+        const int64_t at = std::min(*out_n, out_cap);
+        int64_t n = 0;
+        const pb_status s = pb_index_fill_row_cache(m, doc_ids, n_ids, out_ids ? out_ids + at : nullptr, out_cap - at, &n);
+        *out_n += n;
+        return s;
+    };
+    return ix->dep ? pb_dep_ranks(ix->dep, one) : pb_rep_members(ix->rep, true, one);
+}
+
+extern "C" pb_status pb_index_row_cache_stats(pb_index *ix, pb_row_cache_stats *out, int32_t reset) {
+    if (!ix || !out) return pb_fail(PB_ERR_INVALID, "null argument");
+    *out = pb_row_cache_stats{};
+    if (ix->dep || ix->rep) {  // sums over the ranks or replicas
+        auto one = [&](pb_index *m) {
+            pb_row_cache_stats s{};
+            CKS(pb_index_row_cache_stats(m, &s, reset));
+            out->budget_bytes += s.budget_bytes, out->cached_docs += s.cached_docs, out->cached_bytes += s.cached_bytes;
+            out->dead_bytes += s.dead_bytes, out->staged_docs += s.staged_docs, out->hit_docs += s.hit_docs;
+            out->hit_bytes += s.hit_bytes, out->last_fill_ms += s.last_fill_ms;
+            return PB_OK;
+        };
+        return ix->dep ? pb_dep_ranks(ix->dep, one) : pb_rep_members(ix->rep, false, one);
+    }
+    auto rd = ix->read_lock();
+    RowCacheState &c = ix->rc;
+    out->budget_bytes = (int64_t)c.budget, out->cached_docs = c.docs, out->cached_bytes = c.bytes;
+    out->dead_bytes = c.dead, out->last_fill_ms = c.fill_ms;
+    out->staged_docs = reset ? c.staged.exchange(0) : c.staged.load();
+    out->hit_docs = reset ? c.hit_docs.exchange(0) : c.hit_docs.load();
+    out->hit_bytes = reset ? c.hit_bytes.exchange(0) : c.hit_bytes.load();
+    return PB_OK;
 }
 
 // ------------------------------------------------------------------------------------------

@@ -110,6 +110,9 @@ pb_status pb_dep_append(Deployment *d, pb_codec *codec, const float *embeddings,
                         const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
                         const char *index_dir, int64_t batch_size, int64_t *out_first_doc_id);
 pb_status pb_dep_rebalance(Deployment *d, const int64_t *bounds, int64_t *out_bounds);
+// call(rank) on every rank in turn, the lowest rank's failure first; mutations wait, searches go on (the row cache's
+// entry points, which are rank-local)
+pb_status pb_dep_ranks(Deployment *d, const std::function<pb_status(pb_index *)> &call);
 // A deployment of ranks already loaded (ranks[r] on devices[r], not yet in a group): joins them in a new group and
 // returns its handle.  On failure the ranks are closed.
 pb_status pb_dep_assemble(std::vector<pb_index *> ranks, const std::vector<int> &devices, pb_index **out);
@@ -137,6 +140,9 @@ pb_status pb_rep_append(Replicas *rs, pb_codec *codec, const float *embeddings, 
                         const char *index_dir, int64_t batch_size, int64_t *out_first_doc_id);
 pb_status pb_rep_reserve(Replicas *rs, int64_t num_documents, int64_t num_embeddings);
 pb_status pb_rep_rebalance(Replicas *rs, const int64_t *bounds, int64_t *out_bounds);
+// call(member) on every replica in turn, under the set's writer lock (writer) or its reader lock; the lowest replica's
+// failure first (the row cache's entry points)
+pb_status pb_rep_members(Replicas *rs, bool writer, const std::function<pb_status(pb_index *)> &call);
 
 // A copy of a plain handle (or one rank of a deployment, outside its group) on `device`: every array, derived ones
 // included, copied device to device; a host-tier handle shares src's pinned residuals.  The copy's device-dependent

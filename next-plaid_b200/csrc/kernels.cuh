@@ -22,7 +22,8 @@
 //   k_exact ............. a7+a8 fused residual decompress + MaxSim of every token (filter off, flagged queries, trace)
 //   k_exact_finalize .... a8  q-ordered sum of per-token maxima           maxsim.rs:284-291
 //   k_stage_layout/k_stage_rows/k_unstage_kept  a7 on a host-tier handle: the kept docs' rows staged from pinned host
-//                             memory into slot space, and the slots mapped back to doc ids before k_exact_finalize
+//                             memory (or from the device row cache) into slot space, and the slots mapped back to doc
+//                             ids before k_exact_finalize; k_cache_compact/k_cache_dead carry the row cache through a delete
 //   k_topk .............. a9  stable final sort, take top_k               search.rs:496-515
 //   k_merge_cut/k_merge_topk  doc-sharded search: global cut and global top-k from the all-gathered keys
 //   k_pool_dist/k_pool_chain/k_pool_means  pool_document_embeddings: cosine d^2 (f64), Ward's nearest-neighbour chain,

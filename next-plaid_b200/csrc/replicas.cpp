@@ -276,6 +276,20 @@ pb_status pb_rep_rebalance(Replicas *rs, const int64_t *bounds, int64_t *out_bou
     });
 }
 
+pb_status pb_rep_members(Replicas *rs, bool writer, const std::function<pb_status(pb_index *)> &call) {
+    std::unique_lock<std::mutex> g(rs->gate);
+    std::unique_lock<std::shared_mutex> wr(rs->rw, std::defer_lock);
+    std::shared_lock<std::shared_mutex> rd(rs->rw, std::defer_lock);
+    if (writer) wr.lock();
+    else g.unlock(), rd.lock();
+    for (int i = 0; i < rs->R(); ++i)
+        if (pb_status s = call(rs->members[i])) {
+            const std::string e = pb_last_error();
+            return i == 0 ? s : pb_fail(s, "replica %d: %s", i, e.c_str());
+        }
+    return PB_OK;
+}
+
 extern "C" pb_status pb_index_replica_layout(const pb_index *ix, int32_t *out_replicas, int32_t *out_shards,
                                              int32_t *out_devices) {
     if (!ix || !out_replicas || !out_shards) return pb_fail(PB_ERR_INVALID, "null argument");

@@ -76,6 +76,12 @@ class _CoalesceConfig(C.Structure):
     _fields_ = [("max_queries", C.c_int32), ("max_wait_us", C.c_int32), ("max_inflight", C.c_int32)]
 
 
+class _RowCacheStats(C.Structure):
+    _fields_ = [("budget_bytes", C.c_int64), ("cached_docs", C.c_int64), ("cached_bytes", C.c_int64),
+                ("dead_bytes", C.c_int64), ("staged_docs", C.c_int64), ("hit_docs", C.c_int64),
+                ("hit_bytes", C.c_int64), ("last_fill_ms", C.c_float)]
+
+
 class _CoalesceStats(C.Structure):
     _fields_ = [("n_requests", C.c_int64), ("n_batches", C.c_int64), ("n_bypassed", C.c_int64),
                 ("n_refused", C.c_int64), ("n_rerun_alone", C.c_int64), ("max_batch", C.c_int64),
@@ -102,6 +108,7 @@ EXPORTS = [
     "pb_search", "pb_index_set_coalescing", "pb_index_coalesce_stats", "pb_create_index_sharded", "pb_last_create_ms",
     "pb_index_load_devices", "pb_index_shard_layout", "pb_pooled_doc_length", "pb_pool_embeddings", "pb_last_pool_ms",
     "pb_index_load_replicas", "pb_index_replica_layout", "pb_index_replica_stats",
+    "pb_index_set_row_cache", "pb_index_fill_row_cache", "pb_index_row_cache_stats",
 ]
 
 PB_OPEN_ADOPT_RESIDUALS, PB_OPEN_HOST_RESIDUALS, PB_OPEN_HOST_MUTABLE = 1, 2, 4
@@ -227,6 +234,9 @@ def load_library():
                                              C.POINTER(C.c_void_p)]
         L.pb_index_replica_layout.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.pb_index_replica_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]
+        L.pb_index_set_row_cache.argtypes = [C.c_void_p, C.c_int64]
+        L.pb_index_fill_row_cache.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]
+        L.pb_index_row_cache_stats.argtypes = [C.c_void_p, C.POINTER(_RowCacheStats), C.c_int32]
         L.pb_pooled_doc_length.argtypes = [C.c_int64, C.c_int64]
         L.pb_pooled_doc_length.restype = C.c_int64
         L.pb_pool_embeddings.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_int32,
@@ -623,6 +633,32 @@ class MmapIndex:
         dev, host = C.c_int64(), C.c_int64()
         _check(load_library().pb_index_memory(self._h, C.byref(dev), C.byref(host)))
         return dict(device_bytes=int(dev.value), host_bytes=int(host.value))
+
+    # -- device row cache of a host-tier handle (DESIGN.md 4s) ---------------------------------------------
+    def set_row_cache(self, max_bytes: int) -> None:
+        """pb_index_set_row_cache: the budget, in bytes of rows, of the device cache of a host-tier handle's most-kept
+        documents (0 = off, the default)."""
+        _check(load_library().pb_index_set_row_cache(self._h, int(max_bytes)))
+
+    def fill_row_cache(self, doc_ids: Optional[Sequence[int]] = None) -> np.ndarray:
+        """pb_index_fill_row_cache: replaces the cached set, by the keep counts of the searches since the last such fill
+        (doc_ids None) or with doc_ids in order, each doc taken while its rows fit the budget.  Returns the cached ids in
+        the order they were taken (per rank, then per replica)."""
+        replicas = self.replica_layout()[0]
+        ids = None if doc_ids is None else np.ascontiguousarray(doc_ids, np.int64)
+        cap = replicas * (self.num_documents() if ids is None else len(ids))
+        out, n = np.zeros(max(cap, 1), np.int64), C.c_int64()
+        _check(load_library().pb_index_fill_row_cache(self._h, None if ids is None else _ptr(ids),
+                                                      0 if ids is None else len(ids), _ptr(out), cap, C.byref(n)))
+        return out[:min(n.value, cap)].copy()
+
+    def row_cache_stats(self, reset: bool = False) -> dict:
+        """pb_index_row_cache_stats: the cache's budget and contents, and search staging since the last reset."""
+        st = _RowCacheStats()
+        _check(load_library().pb_index_row_cache_stats(self._h, C.byref(st), 1 if reset else 0))
+        out = {n: int(getattr(st, n)) for n, _ in _RowCacheStats._fields_ if n != "last_fill_ms"}
+        out["last_fill_ms"] = float(st.last_fill_ms)
+        return out
 
     # -- incremental append (index.rs:1675 update_append + reload) ------------------------------------
     def append(self, embeddings: Sequence[np.ndarray], codec: "ResidualCodec", index_dir: Optional[str] = None,

@@ -39,6 +39,22 @@ impl From<&SearchParameters> for PbSearchParams {
 }
 
 /// `pb_coalesce_config`
+/// `pb_row_cache_stats`: a host-tier handle's device row cache (DESIGN §4s)
+#[repr(C)]
+#[derive(Default, Debug, Clone, Copy)]
+pub struct PbRowCacheStats {
+    pub budget_bytes: i64,
+    pub cached_docs: i64,
+    pub cached_bytes: i64,
+    /// rows of docs deleted since the fill
+    pub dead_bytes: i64,
+    /// search staging since the last reset
+    pub staged_docs: i64,
+    pub hit_docs: i64,
+    pub hit_bytes: i64,
+    pub last_fill_ms: f32,
+}
+
 #[repr(C)]
 struct PbCoalesceConfig {
     max_queries: i32,
@@ -140,6 +156,10 @@ extern "C" {
                               out: *mut *mut c_void) -> c_int;
     fn pb_index_memory(ix: *const c_void, device_bytes: *mut i64, host_bytes: *mut i64) -> c_int;
     fn pb_last_staging_stats(ix: *mut c_void, docs: *mut i64, bytes: *mut i64, ms: *mut f32) -> c_int;
+    fn pb_index_set_row_cache(ix: *mut c_void, max_bytes: i64) -> c_int;
+    fn pb_index_fill_row_cache(ix: *mut c_void, doc_ids: *const i64, n_ids: i64, out_ids: *mut i64, out_cap: i64,
+                               out_n: *mut i64) -> c_int;
+    fn pb_index_row_cache_stats(ix: *mut c_void, out: *mut PbRowCacheStats, reset: i32) -> c_int;
     // pb_create_index_sharded (DESIGN §4n): `comm` is a pb_build_comm, `params` a pb_create_params
     fn pb_create_index_sharded(comm: *mut c_void, embeddings: *const f32, doc_lengths: *const i64, n_docs: i64, dim: i32,
                                memory_space: i32, centroids: *const f32, num_centroids: i64, params: *const c_void,
@@ -228,6 +248,36 @@ impl B200Index {
             return Err(Error::Search(last_error()));
         }
         Ok((d, h))
+    }
+
+    /// The budget of the device row cache of a host-tier handle (`pb_index_set_row_cache`, DESIGN §4s); 0 = off.
+    pub fn set_row_cache(&self, max_bytes: i64) -> Result<()> {
+        if unsafe { pb_index_set_row_cache(self.handle, max_bytes) } != 0 {
+            return Err(Error::Search(last_error()));
+        }
+        Ok(())
+    }
+
+    /// Replaces the cached set (`pb_index_fill_row_cache`): by the keep counts (`doc_ids` None) or with the given ids in
+    /// order, each doc taken while its rows fit the budget.  Returns at most `cap` of the cached ids, in the order taken.
+    pub fn fill_row_cache(&self, doc_ids: Option<&[i64]>, cap: usize) -> Result<Vec<i64>> {
+        let mut out = vec![0i64; cap.max(1)];
+        let mut n = 0i64;
+        let (p, len) = doc_ids.map_or((std::ptr::null(), 0), |d| (d.as_ptr(), d.len() as i64));
+        if unsafe { pb_index_fill_row_cache(self.handle, p, len, out.as_mut_ptr(), cap as i64, &mut n) } != 0 {
+            return Err(Error::Search(last_error()));
+        }
+        out.truncate((n as usize).min(cap));
+        Ok(out)
+    }
+
+    /// The row cache's budget and contents, and search staging since the last reset (`pb_index_row_cache_stats`).
+    pub fn row_cache_stats(&self, reset: bool) -> Result<PbRowCacheStats> {
+        let mut st = PbRowCacheStats::default();
+        if unsafe { pb_index_row_cache_stats(self.handle, &mut st, reset as i32) } != 0 {
+            return Err(Error::Search(last_error()));
+        }
+        Ok(st)
     }
 
     /// What this thread's last search staged from host memory: (docs, residual bytes, ms with profiling on).
