@@ -818,6 +818,41 @@ PB_API pb_status pb_index_load_devices(const char *index_dir, const int32_t *dev
  * out_devices [world].  A handle that is not a deployment reports world 1, [doc_id_base, doc_id_base + D], its device. */
 PB_API pb_status pb_index_shard_layout(const pb_index *ix, int32_t *out_world, int64_t *out_bounds, int32_t *out_devices);
 
+/* ---- changing a deployment's number of ranks (DESIGN.md 4t) -------------------------------
+ *
+ * A live deployment of pb_index_load_devices gains or loses ranks without a reload: the documents move on the device
+ * (pb_index_rebalance_sharded's transfer), global doc ids stay, and no file is touched.  Afterwards every entry point
+ * gives what it gave before, and what pb_index_load_devices of an in-sync directory on the new devices gives; rank order
+ * stays document order, so later appends go to the new last rank.  Both calls hold the deployment alone: searches,
+ * coalesced requests and mutations wait and then run on the new layout.
+ *
+ * Balanced bounds (bounds NULL): b[r] = min { d : doc_off[d] W' >= N r } over the new world W', i.e.
+ * pb_index_dir_shard_bounds(dir, W') of a directory in sync.  Explicit bounds [W' + 1], host memory: non-decreasing from
+ * 0 to D_total; a rank may be left empty.  out_bounds [W' + 1] (may be NULL) receives the bounds applied.
+ *
+ * Refusals, the handle unchanged and usable: PB_ERR_INVALID for a NULL ix / devices / ranks, a device id outside
+ * [0, pb_device_count()), a new world outside [1, 64], a rank outside [0, world) or listed twice, removing every rank, or
+ * bounds that do not tile [0, D_total); PB_ERR_UNSUPPORTED for a handle that is not such a deployment (a single index,
+ * an NCCL-joined rank, a replica set) and for ranks opened with PB_OPEN_HOST_RESIDUALS or PB_OPEN_ADOPT_RESIDUALS.
+ * A failure while the documents move (PB_ERR_NOMEM for a rank that cannot allocate its new arrays, a CUDA or transport
+ * error) also leaves every rank as it was: pb_index_add_devices then closes its new ranks and puts the old ones back in
+ * their group.  What cannot be undone is a CUDA error that leaves a device unusable: the handle must then be closed,
+ * as after any such error.
+ *
+ * Memory: as for pb_index_rebalance_sharded, a rank whose range changes holds its old and new arrays until the end; a
+ * new rank also holds a copy of the centroids from the start. */
+/* n_devices ranks join after the last rank, on devices[i] (they may repeat, or be devices the deployment already uses),
+ * each opened empty from rank 0 by device-to-device copies; then the documents move so that rank r of the new world
+ * holds [b[r], b[r+1]): bounds [world + n_devices + 1], or NULL for the balanced split. */
+PB_API pb_status pb_index_add_devices(pb_index *ix, const int32_t *devices, int32_t n_devices, const int64_t *bounds,
+                                      int64_t *out_bounds);
+/* The listed ranks (distinct, in [0, world), not all of them) leave: their documents go to the remaining ranks, which
+ * keep their order, so that rank r of the new world holds [b[r], b[r+1]) (bounds [world - n_ranks + 1] over the new
+ * world, or NULL for the balanced split).  The leaving ranks are then closed and their device memory freed;
+ * pb_index_device follows the new rank 0. */
+PB_API pb_status pb_index_remove_ranks(pb_index *ix, const int32_t *ranks, int32_t n_ranks, const int64_t *bounds,
+                                       int64_t *out_bounds);
+
 /* ---- replicas behind one handle (DESIGN.md 4q) --------------------------------------------
  *
  * R full copies of an index directory, each spread over S devices, behind one handle: n_devices = R * S, and replica g

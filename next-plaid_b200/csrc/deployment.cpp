@@ -74,6 +74,20 @@ struct Deployment {
         return PB_OK;
     }
 
+    // A resize's new layout: next[r] becomes rank r of g, on devs[r].  The threads and scratch follow the world: worker
+    // r serves slot r, so the workers of the slots both worlds have stay, and those of the slots it loses are joined.
+    // Under mu and layout, with no collective running; cannot fail.
+    void reform(std::vector<pb_index *> next, std::vector<int> devs, pb_shard_group *g) {
+        for (size_t r = 0; r < next.size(); ++r) pb_index_group_move(next[r], g, (int)r);  // r < g's world: succeeds
+        ranks = std::move(next);
+        devices = std::move(devs);
+        group = g;
+        workers.resize((size_t)world());
+        for (int r = 1; r < world(); ++r)
+            if (!workers[r]) workers[r].reset(new RankWorker(r));
+        scratch.resize((size_t)world());
+    }
+
     // joins the loaded ranks in the group and makes the handle; on failure the caller deletes this
     pb_status finish(pb_index **out) {
         for (int r = 0; r < world(); ++r) {
@@ -94,7 +108,13 @@ struct Deployment {
 pb_index *pb_dep_rank(Deployment *d, int r) { return d->ranks[r]; }
 void pb_dep_close(Deployment *d) { delete d; }
 
+pb_status pb_dep_first(Deployment *d, const std::function<pb_status(pb_index *)> &call) {
+    std::shared_lock<std::shared_mutex> g(d->layout);
+    return call(d->ranks[0]);
+}
+
 void pb_dep_each(Deployment *d, const std::function<void(pb_index *)> &call) {
+    std::shared_lock<std::shared_mutex> g(d->layout);
     for (pb_index *ix : d->ranks) call(ix);
 }
 
@@ -319,4 +339,123 @@ pb_status pb_dep_rebalance(Deployment *d, const int64_t *bounds, int64_t *out_bo
     pb_status s = d->run_one([&](int r) { return pb_index_rebalance_sharded(d->ranks[r], bounds, got[r].data()); });
     if (s == PB_OK && out_bounds) std::copy(got[0].begin(), got[0].end(), out_bounds);
     return s;
+}
+
+// bounds [W + 1] (host) tile [0, D): non-decreasing from 0 to D
+static pb_status check_tiling(const int64_t *b, int W, long long D) {
+    bool ok = b[0] == 0 && b[W] == D;
+    for (int r = 0; r < W; ++r) ok = ok && b[r] <= b[r + 1];
+    if (ok) return PB_OK;
+    return pb_fail(PB_ERR_INVALID, "bounds must be non-decreasing from 0 to D_total = %lld over the %d ranks of the new "
+                   "world", D, W);
+}
+
+// New ranks open empty after the last one, every rank moves to a group of the new world, and the rebalance moves the
+// documents.  If the rebalance fails every rank is as it was: the old ranks go back to their group (never used in the
+// meantime, so whole) and the new ones are closed.
+pb_status pb_dep_add_devices(Deployment *d, const int32_t *devices, int32_t n, const int64_t *bounds, int64_t *out_bounds) {
+    std::lock_guard<std::mutex> g(d->mu);
+    std::unique_lock<std::shared_mutex> l(d->layout);
+    const int W = d->world();
+    if (n < 1 || W + n > 64)
+        return pb_fail(PB_ERR_INVALID, "adding %d ranks to %d: the new world must be in [%d, 64] (the shard group's limit)",
+                       (int)n, W, W + 1);
+    const int have = pb_device_count();
+    for (int i = 0; i < n; ++i)
+        if (devices[i] < 0 || devices[i] >= have)
+            return pb_fail(PB_ERR_INVALID, "devices[%d] = %d out of range (have %d)", i, (int)devices[i], have);
+    const int W1 = W + n;
+    std::vector<int64_t> base;
+    pb_status s = d->bounds(base);
+    if (s == PB_OK && bounds) s = check_tiling(bounds, W1, base[W]);
+    if (s != PB_OK) return s;
+    std::vector<pb_index *> prev = d->ranks, next = d->ranks;
+    std::vector<int> prev_dev = d->devices, devs = d->devices;
+    auto drop = [&] {
+        for (int r = W; r < (int)next.size(); ++r) pb_index_close(next[r]);
+    };
+    for (int i = 0; i < n && s == PB_OK; ++i) {
+        pb_index *e = nullptr;
+        s = pb_index_clone_empty(d->ranks[0], devices[i], base[W], &e);
+        if (s == PB_OK) next.push_back(e), devs.push_back(devices[i]);
+    }
+    pb_shard_group *g1 = nullptr;
+    if (s == PB_OK) s = pb_shard_group_create(W1, &g1);
+    if (s != PB_OK) {
+        drop();
+        return s;
+    }
+    pb_shard_group *g0 = d->group;
+    d->reform(next, devs, g1);
+    std::vector<std::vector<int64_t>> got((size_t)W1, std::vector<int64_t>((size_t)W1 + 1, 0));
+    s = d->run_one([&](int r) { return pb_index_rebalance_sharded(d->ranks[r], bounds, got[r].data()); });
+    if (s != PB_OK) {
+        const std::string e = pb_last_error();
+        d->reform(prev, prev_dev, g0);
+        drop();
+        pb_shard_group_destroy(g1);
+        return pb_fail(s, "%s", e.c_str());
+    }
+    pb_shard_group_destroy(g0);
+    if (out_bounds) std::copy(got[0].begin(), got[0].end(), out_bounds);
+    return PB_OK;
+}
+
+// The rebalance runs over the current group, the leaving ranks taking empty ranges at their positions; then they are
+// closed and the others move, in their order, to a group of the new world (created first, so that nothing can fail
+// after the documents have moved).  If the rebalance fails every rank is as it was.
+pb_status pb_dep_remove_ranks(Deployment *d, pb_index *handle, const int32_t *ranks, int32_t n, const int64_t *bounds,
+                              int64_t *out_bounds) {
+    std::lock_guard<std::mutex> g(d->mu);
+    std::unique_lock<std::shared_mutex> l(d->layout);
+    const int W = d->world();
+    if (n < 1 || n >= W)
+        return pb_fail(PB_ERR_INVALID, "removing %d of %d ranks: at least one must leave and one stay", (int)n, W);
+    std::vector<uint8_t> stays((size_t)W, 1);
+    for (int i = 0; i < n; ++i) {
+        const int r = ranks[i];
+        if (r < 0 || r >= W) return pb_fail(PB_ERR_INVALID, "ranks[%d] = %d outside [0, %d)", i, r, W);
+        if (!stays[r]) return pb_fail(PB_ERR_INVALID, "rank %d is listed twice", r);
+        stays[r] = 0;
+    }
+    const int W1 = W - n;
+    std::vector<int64_t> base, b;
+    pb_status s = d->bounds(base);
+    if (s == PB_OK && bounds) s = check_tiling(bounds, W1, base[W]);
+    if (s != PB_OK) return s;
+    if (bounds) {  // over the old world: a leaving rank gets the empty range where the next staying rank starts
+        b.assign((size_t)W + 1, base[W]);
+        for (int r = 0, j = 0; r < W; ++r) {
+            b[r] = bounds[j];
+            j += stays[r];
+        }
+    }
+    pb_shard_group *g1 = nullptr;
+    if ((s = pb_shard_group_create(W1, &g1)) != PB_OK) return s;
+    std::vector<std::vector<int64_t>> got((size_t)W, std::vector<int64_t>((size_t)W + 1, 0));
+    s = d->run_one([&](int r) {
+        return pb_index_rebalance_shares(d->ranks[r], bounds ? b.data() : nullptr, bounds ? nullptr : stays.data(),
+                                         got[r].data());
+    });
+    if (s != PB_OK) {
+        pb_shard_group_destroy(g1);
+        return s;
+    }
+    std::vector<pb_index *> next, gone;
+    std::vector<int> devs;
+    for (int r = 0; r < W; ++r) {
+        (stays[r] ? next : gone).push_back(d->ranks[r]);
+        if (stays[r]) devs.push_back(d->devices[r]);
+    }
+    pb_shard_group *g0 = d->group;
+    d->reform(next, devs, g1);
+    for (pb_index *x : gone) pb_index_close(x);
+    pb_shard_group_destroy(g0);
+    pb_index_deployment_rank0(handle, d->ranks[0]);
+    if (out_bounds) {
+        for (int r = 0, j = 0; r < W; ++r)
+            if (stays[r]) out_bounds[j++] = got[0][r];
+        out_bounds[W1] = base[W];
+    }
+    return PB_OK;
 }

@@ -432,6 +432,11 @@ struct ShardComm {
         return PB_OK;
     }
     bool joined() const { return nccl || group; }
+    // an in-process rank leaves its group, so that it can join another (a deployment changing its number of ranks).
+    // No collective of the group may be running.  An NCCL communicator stays as it is.
+    void leave() {
+        if (!nccl) group = nullptr, rank = 0, world = 1;
+    }
     // the peers must not wait for a rank that gave up: breaks an in-process group (NCCL keeps no such state)
     void fail() {
         if (group) group->fail();
@@ -1285,10 +1290,13 @@ static pb_status coalesce_env_defaults(pb_index *ix) {
 pb_index *pb_index_new_deployment(Deployment *d, const pb_index *rank0) {
     pb_index *ix = new pb_index();
     ix->dep = d;
-    ix->device = rank0->device, ix->dim = rank0->dim, ix->nbits = rank0->nbits, ix->packed = rank0->packed;
-    ix->K = rank0->K;
+    pb_index_deployment_rank0(ix, rank0);
     coalesce_env_defaults(ix);  // cannot fail: the handle joins no group
     return ix;
+}
+void pb_index_deployment_rank0(pb_index *ix, const pb_index *rank0) {
+    ix->device = rank0->device, ix->dim = rank0->dim, ix->nbits = rank0->nbits, ix->packed = rank0->packed;
+    ix->K = rank0->K;
 }
 
 // A replica set's handle (replicas.cpp): no documents of its own; K, dim, nbits and device from replica 0
@@ -1432,7 +1440,12 @@ extern "C" double pb_index_avg_doclen(const pb_index *ix) {
 }
 extern "C" int32_t pb_index_embedding_dim(const pb_index *ix) { return ix ? ix->dim : 0; }
 extern "C" int32_t pb_index_nbits(const pb_index *ix) { return ix ? ix->nbits : 0; }
-extern "C" int32_t pb_index_device(const pb_index *ix) { return ix ? ix->device : -1; }
+extern "C" int32_t pb_index_device(const pb_index *ix) {
+    if (!ix) return -1;
+    int32_t dv = ix->device;  // a deployment's: its rank 0's, which pb_index_remove_ranks may change
+    if (ix->dep) pb_dep_first(ix->dep, [&](pb_index *r0) { return dv = r0->device, PB_OK; });
+    return dv;
+}
 
 extern "C" pb_status pb_index_memory(const pb_index *ix, int64_t *device_bytes, int64_t *host_bytes) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
@@ -3587,10 +3600,12 @@ extern "C" pb_status pb_search(pb_index *ix, const float *query, int64_t n_query
     pb_status st;
     if (ix->dep || ix->rep) {  // as one handle of the whole index: every rank's K, the deployment's D (rank 0 may be empty)
         const long long D = pb_index_num_documents(ix);
-        const pb_index *m = ix->rep ? pb_rep_member(ix->rep, 0) : ix;
-        if (m->dep) m = pb_dep_rank(m->dep, 0);
-        auto rd = m->read_lock();
-        st = check_request(m, D, r);
+        pb_index *m = ix->rep ? pb_rep_member(ix->rep, 0) : ix;
+        auto check = [&](pb_index *h) {
+            auto rd = h->read_lock();
+            return check_request(h, D, r);
+        };
+        st = m->dep ? pb_dep_first(m->dep, check) : check(m);
     } else {
         auto rd = ix->read_lock();
         st = check_request(ix, ix->D, r);
@@ -3625,7 +3640,8 @@ extern "C" pb_status pb_search_batch_device(pb_index *ix, const float *d_queries
 // stage entry points
 // ------------------------------------------------------------------------------------------
 extern "C" pb_status pb_centroid_scores(pb_index *ix, const float *query_tokens, int64_t n, float *out) {
-    if (ix && ix->dep) return pb_centroid_scores(pb_dep_rank(ix->dep, 0), query_tokens, n, out);  // centroids replicated
+    if (ix && ix->dep)  // the centroids are replicated
+        return pb_dep_first(ix->dep, [&](pb_index *r0) { return pb_centroid_scores(r0, query_tokens, n, out); });
     if (ix && ix->rep) return pb_rep_whole(ix->rep, 0, [&](pb_index *m) { return pb_centroid_scores(m, query_tokens, n, out); });
     if (!ix || (!query_tokens && n) || (!out && n)) return pb_fail(PB_ERR_INVALID, "null argument");
     if (n == 0) return PB_OK;
@@ -4060,6 +4076,10 @@ extern "C" pb_status pb_index_group_join(pb_index *ix, pb_shard_group *g, int32_
     CKS(ix->comm.join(g, rank, ix->device));
     pb_index_set_coalescing(ix, nullptr);  // as pb_index_comm_init
     return PB_OK;
+}
+pb_status pb_index_group_move(pb_index *ix, pb_shard_group *g, int rank) {
+    ix->comm.leave();
+    return pb_index_group_join(ix, g, rank);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -5349,6 +5369,43 @@ pb_status pb_index_clone(const pb_index *src, int device, pb_index **out) {
     return PB_OK;
 }
 
+pb_status pb_index_clone_empty(const pb_index *src, int device, long long doc_id_base, pb_index **out) {
+    *out = nullptr;
+    auto rd = src->read_lock();
+    if (!src->residuals.owned || src->host_tier)
+        return pb_fail(PB_ERR_UNSUPPORTED, "an empty rank beside one that uses the caller's residual array or host memory "
+                                           "(PB_OPEN_ADOPT_RESIDUALS / PB_OPEN_HOST_RESIDUALS)");
+    CKS(check_device(device));
+    std::unique_ptr<pb_index> ix(new pb_index());
+    ix->device = device;
+    cudaDeviceProp prop;
+    CK(cudaGetDeviceProperties(&prop, device));
+    ix->sm_count = prop.multiProcessorCount;
+    ix->dim = src->dim, ix->nbits = src->nbits, ix->packed = src->packed, ix->K = src->K, ix->doc_id_base = doc_id_base;
+    ix->cmax = src->cmax;
+    ix->fast_approx = src->fast_approx, ix->k1_tc = src->k1_tc, ix->k1_margin = src->k1_margin, ix->k1_diag = src->k1_diag;
+    ix->table_diag = src->table_diag, ix->approx_grid = src->approx_grid, ix->a5_prune = src->a5_prune;
+    ix->a5_live = src->a5_live, ix->a5_m1 = src->a5_m1, ix->a5_waves = src->a5_waves, ix->probe16 = src->probe16;
+    ix->fast_exact = src->fast_exact, ix->filter_diag = src->filter_diag, ix->pair_exact = src->pair_exact;
+    ix->ws_grid = src->ws_grid, ix->ws_grid2 = src->ws_grid2, ix->lanes = src->lanes, ix->profiling = src->profiling;
+    ix->st_budget = src->st_budget, ix->delete_window = src->delete_window;
+    // the per-doc arrays of no documents, allocated as an open of an empty range allocates them
+    const long long zero = 0;
+    CKS(upload(ix->doc_off, &zero, 8, PB_MEM_HOST));
+    CKS(upload(ix->udoc_off, &zero, 8, PB_MEM_HOST));
+    CKS(ix->ivf_off.ensure((size_t)(ix->K + 1) * 8));
+    for (DevBuf *b : {&ix->codes, &ix->residuals, &ix->ucodes, &ix->ivf}) CKS(b->ensure(16));
+    OwnedStream st;
+    CK(cudaStreamCreateWithFlags(&st.s, cudaStreamNonBlocking));
+    CK(cudaMemsetAsync(ix->ivf_off.p, 0, (size_t)(ix->K + 1) * 8, st.s));
+    CKS(clone_buf(ix->centroids, src->centroids, device, src->device, st.s));
+    CKS(clone_buf(ix->w_rev, src->w_rev, device, src->device, st.s));
+    CK(cudaStreamSynchronize(st.s));
+    CKS(coalesce_env_defaults(ix.get()));
+    *out = ix.release();
+    return PB_OK;
+}
+
 // The encoded rows of tokens [t0, t0 + n) of a handle, on the host: codes widened to i64 and packed residual rows
 static pb_status tail_rows(const pb_index *ix, long long t0, long long n, std::vector<int64_t> &codes,
                            std::vector<uint8_t> &res) {
@@ -5852,21 +5909,50 @@ struct RebalancePrep {
     DevBuf rlen, rulen, seg, seg_off, meta, mn;
 };
 
-static pb_status rebalance_body(pb_index *ix, RepTurn &turn, const int64_t *bounds, int64_t *out_bounds);
+static pb_status rebalance_body(pb_index *ix, RepTurn &turn, const int64_t *bounds, const uint8_t *shares,
+                                int64_t *out_bounds);
 
 extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bounds, int64_t *out_bounds) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
     if (ix->dep) return pb_dep_rebalance(ix->dep, bounds, out_bounds);
     if (ix->rep) return pb_rep_rebalance(ix->rep, bounds, out_bounds);
+    return pb_index_rebalance_shares(ix, bounds, nullptr, out_bounds);
+}
+
+// The calls that change a deployment's number of ranks (DESIGN §4t) address a deployment of pb_index_load_devices only
+static pb_status refuse_resize(const pb_index *ix, const char *call) {
+    if (ix->rep) return pb_fail(PB_ERR_UNSUPPORTED, "%s on a replica set (pb_index_load_replicas) is not supported", call);
+    if (!ix->dep)
+        return pb_fail(PB_ERR_UNSUPPORTED, "%s needs a multi-device handle of pb_index_load_devices (this handle is %s)",
+                       call, ix->comm.joined() ? "a rank of a doc-sharded group" : "a single index");
+    return PB_OK;
+}
+
+extern "C" pb_status pb_index_add_devices(pb_index *ix, const int32_t *devices, int32_t n_devices, const int64_t *bounds,
+                                          int64_t *out_bounds) {
+    if (!ix || !devices) return pb_fail(PB_ERR_INVALID, "null argument");
+    CKS(refuse_resize(ix, "pb_index_add_devices"));
+    return pb_dep_add_devices(ix->dep, devices, n_devices, bounds, out_bounds);
+}
+
+extern "C" pb_status pb_index_remove_ranks(pb_index *ix, const int32_t *ranks, int32_t n_ranks, const int64_t *bounds,
+                                           int64_t *out_bounds) {
+    if (!ix || !ranks) return pb_fail(PB_ERR_INVALID, "null argument");
+    CKS(refuse_resize(ix, "pb_index_remove_ranks"));
+    return pb_dep_remove_ranks(ix->dep, ix, ranks, n_ranks, bounds, out_bounds);
+}
+
+pb_status pb_index_rebalance_shares(pb_index *ix, const int64_t *bounds, const uint8_t *shares, int64_t *out_bounds) {
     std::lock_guard<std::mutex> gate(ix->gate);
     std::unique_lock<std::shared_mutex> wr(ix->rw);
     RepTurn turn(ix);
-    const pb_status s = rebalance_body(ix, turn, bounds, out_bounds);
+    const pb_status s = rebalance_body(ix, turn, bounds, shares, out_bounds);
     turn.leave(s);
     return s;
 }
 
-static pb_status rebalance_body(pb_index *ix, RepTurn &turn, const int64_t *bounds, int64_t *out_bounds) {
+static pb_status rebalance_body(pb_index *ix, RepTurn &turn, const int64_t *bounds, const uint8_t *shares,
+                                int64_t *out_bounds) {
     const int W = ix->comm.world, me = ix->comm.rank;
     const long long K = ix->K;
     const size_t pk = (size_t)ix->packed;
@@ -5879,6 +5965,8 @@ static pb_status rebalance_body(pb_index *ix, RepTurn &turn, const int64_t *boun
         Fnv64 f;
         f.put(bounds != nullptr);
         if (bounds) f.add(bounds, (size_t)(W + 1) * 8);
+        f.put(shares != nullptr);
+        if (shares) f.add(shares, (size_t)W);
         rec[LR_PRINT] = (long long)f.h;
         if (!ix->comm.has_p2p())
             return pb_fail(PB_ERR_COMM, "the NCCL library lacks ncclSend / ncclRecv / ncclGroupStart / ncclGroupEnd");
@@ -5903,9 +5991,11 @@ static pb_status rebalance_body(pb_index *ix, RepTurn &turn, const int64_t *boun
                            "PB_OPEN_HOST_RESIDUALS)", r);
     const long long D_total = a[W], N_total = tok[W];
 
-    // 3. the new bounds: the caller's, or the token-balanced split b[r] = min { d : off[d] W >= N r } of the global doc
-    // offsets.  For that each rank offers the least d of its closed range [a_me, a_me+1] that qualifies (global
-    // off[d] = tok[me] + its own doc_off), or D_total; the least offer wins.
+    // 3. the new bounds: the caller's, or the token-balanced split c[j] = min { d : off[d] S >= N j } of the global doc
+    // offsets over the S ranks that take a share (every rank, unless `shares` leaves some out).  For that each rank
+    // offers the least d of its closed range [a_me, a_me+1] that qualifies (global off[d] = tok[me] + its own
+    // doc_off), or D_total; the least offer wins.  The j-th sharing rank takes [c[j], c[j+1]), and a rank without a
+    // share the empty range where the next sharing rank starts.
     std::vector<long long> b((size_t)W + 1, 0);
     if (bounds) {
         b.assign(bounds, bounds + W + 1);
@@ -5913,21 +6003,27 @@ static pb_status rebalance_body(pb_index *ix, RepTurn &turn, const int64_t *boun
         for (int r = 0; r < W; ++r) ok = ok && b[r] <= b[r + 1];
         if (!ok) return pb_fail(PB_ERR_INVALID, "bounds must be non-decreasing from 0 to D_total = %lld", D_total);
     } else {
-        std::vector<long long> offer((size_t)W + 1, D_total), offers;
-        for (int r = 1; r < W; ++r) {
-            long long lo = 0, hi = ix->D + 1;  // the first local j with (tok[me] + doc_off[j]) W >= N r, or D + 1
+        int S = 0;
+        for (int r = 0; r < W; ++r) S += !shares || shares[r];
+        if (S == 0) return pb_fail(PB_ERR_INVALID, "no rank takes a share of the documents");
+        std::vector<long long> offer((size_t)S + 1, D_total), offers, c((size_t)S + 1, D_total);
+        for (int j = 1; j < S; ++j) {
+            long long lo = 0, hi = ix->D + 1;  // the first local i with (tok[me] + doc_off[i]) S >= N j, or D + 1
             while (lo < hi) {
                 const long long mid = (lo + hi) >> 1;
-                if ((tok[me] + p.hoff[mid]) * W >= N_total * r) hi = mid; else lo = mid + 1;
+                if ((tok[me] + p.hoff[mid]) * S >= N_total * j) hi = mid; else lo = mid + 1;
             }
-            if (lo <= ix->D) offer[r] = a[me] + lo;
+            if (lo <= ix->D) offer[j] = a[me] + lo;
         }
-        CKS(gather_words(ix, offer.data(), W + 1, offers));
+        CKS(gather_words(ix, offer.data(), S + 1, offers));
+        c[0] = 0;
+        for (int j = 1; j < S; ++j)
+            for (int s = 0; s < W; ++s) c[j] = std::min(c[j], offers[(size_t)s * (S + 1) + j]);
+        for (int r = 0, j = 0; r < W; ++r) {
+            b[r] = c[j];
+            j += !shares || shares[r];
+        }
         b[W] = D_total;
-        for (int r = 1; r < W; ++r) {
-            b[r] = D_total;
-            for (int s = 0; s < W; ++s) b[r] = std::min(b[r], offers[(size_t)s * (W + 1) + r]);
-        }
     }
     if (b == a) {  // nothing moves
         if (out_bounds) std::copy(b.begin(), b.end(), out_bounds);

@@ -84,13 +84,18 @@ inline void run_slots(int k, const Job &job, const std::unique_ptr<RankWorker> *
 // driven through the public entry points by the library's own threads.  Its handle is a pb_index that holds no
 // documents; the entry points of engine.cu hand such a handle to the functions below.
 struct Deployment;
-// the handle: K, dim, nbits and device copied from rank 0; the PB_COALESCE* defaults applied
+// the handle: K, dim, nbits and device copied from rank 0 (pb_index_deployment_rank0); the PB_COALESCE* defaults applied
 pb_index *pb_index_new_deployment(Deployment *d, const pb_index *rank0);
-// rank r's handle
+// the handle's fields taken from rank 0 again, after a resize gave it another rank 0
+void pb_index_deployment_rank0(pb_index *ix, const pb_index *rank0);
+// rank r's handle, unlocked: only for a deployment whose ranks cannot change (a replica set's member, which refuses
+// pb_index_add_devices / pb_index_remove_ranks); elsewhere pb_dep_first or pb_dep_ranks
 pb_index *pb_dep_rank(Deployment *d, int r);
+// call(rank 0's handle) on the caller's thread; a resize waits for it
+pb_status pb_dep_first(Deployment *d, const std::function<pb_status(pb_index *)> &call);
 // Stops and joins the threads, closes the ranks, destroys the group and d
 void pb_dep_close(Deployment *d);
-// call(m) on every rank's handle, on the caller's thread (the pb_set_* switches)
+// call(m) on every rank's handle, on the caller's thread (the pb_set_* switches); mutations wait for it
 void pb_dep_each(Deployment *d, const std::function<void(pb_index *)> &call);
 // A search collective: call(m, ids, scores, counts) on every rank at once, rank 0 with the caller's outputs and the
 // others with scratch outputs of n_queries rows of `stride` (null where the caller's is null)
@@ -110,6 +115,11 @@ pb_status pb_dep_append(Deployment *d, pb_codec *codec, const float *embeddings,
                         const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
                         const char *index_dir, int64_t batch_size, int64_t *out_first_doc_id);
 pb_status pb_dep_rebalance(Deployment *d, const int64_t *bounds, int64_t *out_bounds);
+// pb_index_add_devices / pb_index_remove_ranks after the handle's checks.  `handle` is the deployment's own: its rank-0
+// fields follow a new rank 0.
+pb_status pb_dep_add_devices(Deployment *d, const int32_t *devices, int32_t n, const int64_t *bounds, int64_t *out_bounds);
+pb_status pb_dep_remove_ranks(Deployment *d, pb_index *handle, const int32_t *ranks, int32_t n, const int64_t *bounds,
+                              int64_t *out_bounds);
 // call(rank) on every rank in turn, the lowest rank's failure first; mutations wait, searches go on (the row cache's
 // entry points, which are rank-local)
 pb_status pb_dep_ranks(Deployment *d, const std::function<pb_status(pb_index *)> &call);
@@ -148,6 +158,18 @@ pb_status pb_rep_members(Replicas *rs, bool writer, const std::function<pb_statu
 // included, copied device to device; a host-tier handle shares src's pinned residuals.  The copy's device-dependent
 // scalars are its own.
 pb_status pb_index_clone(const pb_index *src, int device, pb_index **out);
+// An empty rank on `device` opened from a peer src (a handle of the same index, one deployment rank): src's centroids,
+// bucket weights and search switches copied, no documents, global ids from doc_id_base.  It equals pb_index_load_range
+// of an empty range at doc_id_base -- scalars, arrays and pb_index_memory -- and reads no file.  As such a load it holds
+// no tensor-core centroid operands: they are built when its first tokens arrive.  PB_ERR_UNSUPPORTED when src is
+// host-tier or uses the caller's residual array (a deployment's ranks cannot move their documents then).
+pb_status pb_index_clone_empty(const pb_index *src, int device, long long doc_id_base, pb_index **out);
+// A rank of an in-process group leaves it and joins g as `rank`; no collective of either group may be running
+pb_status pb_index_group_move(pb_index *ix, pb_shard_group *g, int rank);
+// pb_index_rebalance_sharded on one rank of a group, where shares [world] (null: every rank) says which ranks take a
+// share of the token-balanced split when bounds is null: the others get empty ranges at their positions (a rank that
+// leaves its deployment).  Every rank passes the same shares.
+pb_status pb_index_rebalance_shares(pb_index *ix, const int64_t *bounds, const uint8_t *shares, int64_t *out_bounds);
 // Appends and deletes on plain handles that hold the same documents, as one: every member prepares, the directory is
 // written once, then every member commits.  An append with a codec encodes on members[0] only; the others take its
 // encoded rows.

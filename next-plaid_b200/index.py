@@ -13,6 +13,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import threading
 from dataclasses import dataclass
 from typing import List, Optional, Sequence
 
@@ -107,6 +108,7 @@ EXPORTS = [
     "pb_index_rebalance_sharded", "pb_index_load_range_flags", "pb_index_memory", "pb_last_staging_stats",
     "pb_search", "pb_index_set_coalescing", "pb_index_coalesce_stats", "pb_create_index_sharded", "pb_last_create_ms",
     "pb_index_load_devices", "pb_index_shard_layout", "pb_pooled_doc_length", "pb_pool_embeddings", "pb_last_pool_ms",
+    "pb_index_add_devices", "pb_index_remove_ranks",
     "pb_index_load_replicas", "pb_index_replica_layout", "pb_index_replica_stats",
     "pb_index_set_row_cache", "pb_index_fill_row_cache", "pb_index_row_cache_stats",
 ]
@@ -230,6 +232,8 @@ def load_library():
         L.pb_index_rebalance_sharded.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         L.pb_index_load_devices.argtypes = [C.c_char_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
         L.pb_index_shard_layout.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.pb_index_add_devices.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+        L.pb_index_remove_ranks.argtypes = L.pb_index_add_devices.argtypes
         L.pb_index_load_replicas.argtypes = [C.c_char_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                              C.POINTER(C.c_void_p)]
         L.pb_index_replica_layout.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -519,6 +523,42 @@ class MmapIndex:
         b, d = np.zeros(w.value + 1, np.int64), np.zeros(w.value, np.int32)
         _check(load_library().pb_index_shard_layout(self._h, C.byref(w), _ptr(b), _ptr(d)))
         return b, d
+
+    # one resize at a time from this process: the bounds' length is checked against the world a resize starts from
+    _resize_lock = threading.Lock()
+
+    def _resize(self, call, n: int, grow: bool, bounds):
+        with MmapIndex._resize_lock:
+            w = C.c_int32()
+            _check(load_library().pb_index_shard_layout(self._h, C.byref(w), None, None))
+            W = w.value + n if grow else w.value - n
+            b = None
+            if bounds is not None:
+                b = np.ascontiguousarray(bounds, np.int64).reshape(-1)
+                if b.size != W + 1:
+                    raise PlaidError(PB_ERR_INVALID, f"bounds has {b.size} entries, the new world needs {W + 1}")
+            out = np.zeros(max(W, 0) + 1, np.int64)
+            _check(call(_ptr(b), _ptr(out)))
+            self._world = W
+            return out
+
+    def add_devices(self, devices: Sequence[int], bounds: Optional[Sequence[int]] = None) -> np.ndarray:
+        """pb_index_add_devices: a load_devices handle gains one rank per entry of `devices` after its last rank, each
+        opened empty on its device, and the documents move on the device so that rank r of the new world holds
+        [bounds[r], bounds[r + 1]) (None: the token-balanced split, shard_bounds of the new world).  Ids, results and
+        the directory do not change.  Returns the bounds applied."""
+        dv = np.ascontiguousarray(list(devices), np.int32)
+        return self._resize(lambda b, out: load_library().pb_index_add_devices(self._h, _ptr(dv), len(dv), b, out),
+                            len(dv), True, bounds)
+
+    def remove_ranks(self, ranks: Sequence[int], bounds: Optional[Sequence[int]] = None) -> np.ndarray:
+        """pb_index_remove_ranks: the listed ranks of a load_devices handle leave it, their documents moving on the
+        device to the remaining ranks (which keep their order) so that rank r of the new world holds
+        [bounds[r], bounds[r + 1]) (None: the token-balanced split).  Their device memory is freed.  Returns the
+        bounds applied."""
+        rk = np.ascontiguousarray(list(ranks), np.int32)
+        return self._resize(lambda b, out: load_library().pb_index_remove_ranks(self._h, _ptr(rk), len(rk), b, out),
+                            len(rk), False, bounds)
 
     @classmethod
     def load_replicas(cls, index_path: str, devices: Sequence[int], shards: int = 1,

@@ -152,6 +152,11 @@ extern "C" {
                                  out: *mut *mut c_void) -> c_int;
     fn pb_index_load_devices(index_dir: *const c_char, devices: *const i32, n_devices: i32, flags: i32,
                              out: *mut *mut c_void) -> c_int;
+    fn pb_index_shard_layout(ix: *const c_void, out_world: *mut i32, out_bounds: *mut i64, out_devices: *mut i32) -> c_int;
+    fn pb_index_add_devices(ix: *mut c_void, devices: *const i32, n_devices: i32, bounds: *const i64,
+                            out_bounds: *mut i64) -> c_int;
+    fn pb_index_remove_ranks(ix: *mut c_void, ranks: *const i32, n_ranks: i32, bounds: *const i64,
+                             out_bounds: *mut i64) -> c_int;
     fn pb_index_load_replicas(index_dir: *const c_char, devices: *const i32, n_devices: i32, n_shards: i32, flags: i32,
                               out: *mut *mut c_void) -> c_int;
     fn pb_index_memory(ix: *const c_void, device_bytes: *mut i64, host_bytes: *mut i64) -> c_int;
@@ -479,6 +484,51 @@ impl B200Index {
             pb_index_rebalance_sharded(self.handle, bounds.map_or(std::ptr::null(), |b| b.as_ptr()), out.as_mut_ptr())
         };
         if st != 0 {
+            return Err(Error::IndexLoad(last_error()));
+        }
+        Ok(out)
+    }
+
+    /// Add one rank per entry of `devices` after the last rank of a `load_devices` handle (`pb_index_add_devices`,
+    /// DESIGN §4t): each opens empty on its device, then the documents move on the device so that rank r of the new
+    /// world holds `[bounds[r], bounds[r + 1])` (None: the token-balanced split of the new world).  Ids, results and the
+    /// index directory do not change; a failure leaves the handle as it was.  Returns the bounds applied.  `bounds`
+    /// is checked against the world the call starts from: resizes of one handle from several threads need an order.
+    pub fn add_devices(&self, devices: &[i32], bounds: Option<&[i64]>) -> Result<Vec<i64>> {
+        let world = self.world()? + devices.len();
+        self.resize(bounds, world, |b, out| unsafe {
+            pb_index_add_devices(self.handle, devices.as_ptr(), devices.len() as i32, b, out)
+        })
+    }
+
+    /// The listed ranks leave a `load_devices` handle (`pb_index_remove_ranks`, DESIGN §4t): their documents move on
+    /// the device to the remaining ranks, which keep their order, so that rank r of the new world holds
+    /// `[bounds[r], bounds[r + 1])` (None: the token-balanced split), and their device memory is freed.  As
+    /// `add_devices` otherwise.
+    pub fn remove_ranks(&self, ranks: &[i32], bounds: Option<&[i64]>) -> Result<Vec<i64>> {
+        let world = self.world()?.saturating_sub(ranks.len());
+        self.resize(bounds, world, |b, out| unsafe {
+            pb_index_remove_ranks(self.handle, ranks.as_ptr(), ranks.len() as i32, b, out)
+        })
+    }
+
+    fn world(&self) -> Result<usize> {
+        let mut w = 0i32;
+        if unsafe { pb_index_shard_layout(self.handle, &mut w, std::ptr::null_mut(), std::ptr::null_mut()) } != 0 {
+            return Err(Error::IndexLoad(last_error()));
+        }
+        Ok(w as usize)
+    }
+
+    fn resize(&self, bounds: Option<&[i64]>, world: usize, call: impl FnOnce(*const i64, *mut i64) -> c_int)
+              -> Result<Vec<i64>> {
+        if let Some(b) = bounds {
+            if b.len() != world + 1 {
+                return Err(Error::Shape(format!("bounds has {} entries, the new world needs {}", b.len(), world + 1)));
+            }
+        }
+        let mut out = vec![0i64; world + 1];
+        if call(bounds.map_or(std::ptr::null(), |b| b.as_ptr()), out.as_mut_ptr()) != 0 {
             return Err(Error::IndexLoad(last_error()));
         }
         Ok(out)
