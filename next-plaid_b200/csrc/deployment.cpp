@@ -27,7 +27,7 @@ struct SearchScratch {  // one rank's copy of a search's outputs (ranks >= 1)
 
 }  // namespace
 
-struct Deployment {
+struct Deployment : Group {
     std::vector<pb_index *> ranks;
     std::vector<int> devices;
     pb_shard_group *group = nullptr;
@@ -94,29 +94,48 @@ struct Deployment {
             pb_status s = pb_index_group_join(ranks[r], group, r);
             if (s != PB_OK) return s;
         }
-        *out = pb_index_new_deployment(this, ranks[0]);
+        *out = pb_index_new_group(this, ranks[0]);
         return PB_OK;
     }
 
-    ~Deployment() {
+    // stops and joins the threads, closes the ranks, destroys the group
+    ~Deployment() override {
         workers.clear();  // joins the threads
         for (pb_index *ix : ranks) pb_index_close(ix);
         pb_shard_group_destroy(group);
     }
+
+    const char *kind() const override { return "a multi-device handle (pb_index_load_devices)"; }
+    Deployment *as_deployment() override { return this; }
+    pb_index *member(int r) override { return ranks[r]; }
+    int size() override { return world(); }
+    void totals(long long *D, long long *N) override;
+    pb_status memory(int64_t *device_bytes, int64_t *host_bytes) override;
+    pb_status shard_layout(int32_t *out_world, int64_t *out_bounds, int32_t *out_devices) override;
+    pb_status append(pb_codec *codec, const float *embeddings, const int64_t *codes, const uint8_t *residuals,
+                     const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space, const char *index_dir,
+                     int64_t batch_size, int64_t *out_first_doc_id) override;
+    pb_status del(const int64_t *doc_ids, int64_t n_ids, const char *index_dir, int64_t *out_deleted) override;
+    pb_status rebalance(const int64_t *bounds, int64_t *out_bounds) override;
+    pb_status decompress(const int64_t *doc_ids, int64_t n_docs, float *out_embeddings, int64_t *out_lengths) override;
+    pb_status exhaustive(const float *queries, const int64_t *q_off, int64_t n_queries, float *out_scores) override;
+    // each addresses one rank's handle
+    pb_status reserve(int64_t, int64_t) override {
+        return refuse("pb_index_reserve (reserve a rank's capacity before it joins a group)");
+    }
+    pb_status export_ivf(int64_t *, int32_t *, int64_t *) override { return refuse("pb_index_export_ivf"); }
+    pb_status last_delete_ms(float *) override { return refuse("pb_last_delete_ms"); }
+    // the ranks as they are: a resize waits for these, a search does not
+    void each(const std::function<void(pb_index *)> &call) override {
+        std::shared_lock<std::shared_mutex> g(layout);
+        for (pb_index *ix : ranks) call(ix);
+    }
+    pb_status in_turn(bool, const std::function<pb_status(pb_index *)> &call) override;
+    pb_status one(int64_t, const std::function<pb_status(pb_index *)> &call) override {
+        std::shared_lock<std::shared_mutex> g(layout);
+        return call(ranks[0]);
+    }
 };
-
-pb_index *pb_dep_rank(Deployment *d, int r) { return d->ranks[r]; }
-void pb_dep_close(Deployment *d) { delete d; }
-
-pb_status pb_dep_first(Deployment *d, const std::function<pb_status(pb_index *)> &call) {
-    std::shared_lock<std::shared_mutex> g(d->layout);
-    return call(d->ranks[0]);
-}
-
-void pb_dep_each(Deployment *d, const std::function<void(pb_index *)> &call) {
-    std::shared_lock<std::shared_mutex> g(d->layout);
-    for (pb_index *ix : d->ranks) call(ix);
-}
 
 extern "C" pb_status pb_index_load_devices(const char *index_dir, const int32_t *devices, int32_t n_devices,
                                            int32_t flags, pb_index **out) {
@@ -183,20 +202,19 @@ pb_status pb_dep_search(Deployment *d, int64_t n_queries, int64_t stride, int64_
     });
 }
 
-pb_status pb_dep_totals(Deployment *d, long long *D, long long *N) {
-    std::shared_lock<std::shared_mutex> g(d->layout);
+void Deployment::totals(long long *D, long long *N) {
+    std::shared_lock<std::shared_mutex> g(layout);
     *D = *N = 0;
-    for (pb_index *ix : d->ranks) {
+    for (pb_index *ix : ranks) {
         *D += pb_index_num_documents(ix);
         *N += pb_index_num_embeddings(ix);
     }
-    return PB_OK;
 }
 
-pb_status pb_dep_memory(Deployment *d, int64_t *device_bytes, int64_t *host_bytes) {
-    std::shared_lock<std::shared_mutex> g(d->layout);
+pb_status Deployment::memory(int64_t *device_bytes, int64_t *host_bytes) {
+    std::shared_lock<std::shared_mutex> g(layout);
     int64_t dev = 0, host = 0;
-    for (pb_index *ix : d->ranks) {
+    for (pb_index *ix : ranks) {
         int64_t a = 0, b = 0;
         pb_status s = pb_index_memory(ix, &a, &b);
         if (s != PB_OK) return s;
@@ -207,27 +225,26 @@ pb_status pb_dep_memory(Deployment *d, int64_t *device_bytes, int64_t *host_byte
     return PB_OK;
 }
 
-pb_status pb_dep_layout(Deployment *d, int32_t *out_world, int64_t *out_bounds, int32_t *out_devices) {
-    std::shared_lock<std::shared_mutex> g(d->layout);
+pb_status Deployment::shard_layout(int32_t *out_world, int64_t *out_bounds, int32_t *out_devices) {
+    std::shared_lock<std::shared_mutex> g(layout);
     std::vector<int64_t> base;
-    pb_status s = d->bounds(base);
+    pb_status s = bounds(base);
     if (s != PB_OK) return s;
-    *out_world = d->world();
+    *out_world = world();
     if (out_bounds) std::copy(base.begin(), base.end(), out_bounds);
-    if (out_devices) std::copy(d->devices.begin(), d->devices.end(), out_devices);
+    if (out_devices) std::copy(devices.begin(), devices.end(), out_devices);
     return PB_OK;
 }
 
 // Each id goes to the rank holding it, in input order; the ranks run in parallel and write disjoint rows of the output
-pb_status pb_dep_decompress(Deployment *d, const int64_t *doc_ids, int64_t n_docs, float *out_embeddings,
-                            int64_t *out_lengths) {
+pb_status Deployment::decompress(const int64_t *doc_ids, int64_t n_docs, float *out_embeddings, int64_t *out_lengths) {
     if ((!doc_ids && n_docs) || !out_lengths) return pb_fail(PB_ERR_INVALID, "null argument");
     if (n_docs <= 0) return PB_OK;
-    std::lock_guard<std::mutex> g(d->mu);  // the rank threads; mutations, which move the ranges, wait
+    std::lock_guard<std::mutex> g(mu);  // the rank threads; mutations, which move the ranges, wait
     std::vector<int64_t> base;
-    pb_status s = d->bounds(base);
+    pb_status s = bounds(base);
     if (s != PB_OK) return s;
-    const int W = d->world();
+    const int W = world();
     std::vector<std::vector<int64_t>> ids((size_t)W), pos((size_t)W), lens((size_t)W);
     for (int64_t i = 0; i < n_docs; ++i) {
         out_lengths[i] = 0;  // an id no rank holds: length 0, as on one handle
@@ -237,10 +254,10 @@ pb_status pb_dep_decompress(Deployment *d, const int64_t *doc_ids, int64_t n_doc
         ids[r].push_back(id);
         pos[r].push_back(i);
     }
-    s = d->run_one([&](int r) {
+    s = run_one([&](int r) {
         lens[r].assign(ids[r].size(), 0);
         return ids[r].empty() ? PB_OK
-                              : pb_decompress_documents(d->ranks[r], ids[r].data(), (int64_t)ids[r].size(), nullptr,
+                              : pb_decompress_documents(ranks[r], ids[r].data(), (int64_t)ids[r].size(), nullptr,
                                                         lens[r].data());
     }, false);
     if (s != PB_OK) return s;
@@ -249,14 +266,14 @@ pb_status pb_dep_decompress(Deployment *d, const int64_t *doc_ids, int64_t n_doc
     if (!out_embeddings) return PB_OK;
     std::vector<int64_t> start((size_t)n_docs + 1, 0);  // row of each input id in the output
     for (int64_t i = 0; i < n_docs; ++i) start[i + 1] = start[i] + out_lengths[i];
-    const size_t dim = (size_t)pb_index_embedding_dim(d->ranks[0]);
-    return d->run_one([&](int r) {
+    const size_t dim = (size_t)pb_index_embedding_dim(ranks[0]);
+    return run_one([&](int r) {
         int64_t rows = 0;
         for (int64_t l : lens[r]) rows += l;
         if (rows == 0) return PB_OK;
         std::vector<float> buf((size_t)rows * dim);
         std::vector<int64_t> got(ids[r].size());
-        pb_status st = pb_decompress_documents(d->ranks[r], ids[r].data(), (int64_t)ids[r].size(), buf.data(), got.data());
+        pb_status st = pb_decompress_documents(ranks[r], ids[r].data(), (int64_t)ids[r].size(), buf.data(), got.data());
         if (st != PB_OK) return st;
         const float *src = buf.data();
         for (size_t j = 0; j < pos[r].size(); ++j) {
@@ -268,20 +285,19 @@ pb_status pb_dep_decompress(Deployment *d, const int64_t *doc_ids, int64_t n_doc
 }
 
 // Rank r fills columns [base[r], base[r + 1]) of each D_total-wide row
-pb_status pb_dep_exhaustive(Deployment *d, const float *queries, const int64_t *q_off, int64_t n_queries,
-                            float *out_scores) {
+pb_status Deployment::exhaustive(const float *queries, const int64_t *q_off, int64_t n_queries, float *out_scores) {
     if ((!queries && n_queries) || !q_off || (!out_scores && n_queries)) return pb_fail(PB_ERR_INVALID, "null argument");
     if (n_queries <= 0) return PB_OK;
-    std::lock_guard<std::mutex> g(d->mu);  // the rank threads; mutations, which move the ranges, wait
+    std::lock_guard<std::mutex> g(mu);  // the rank threads; mutations, which move the ranges, wait
     std::vector<int64_t> base;
-    pb_status s = d->bounds(base);
+    pb_status s = bounds(base);
     if (s != PB_OK) return s;
-    const size_t D = (size_t)(base[d->world()] - base[0]);
-    return d->run_one([&](int r) {
+    const size_t D = (size_t)(base[world()] - base[0]);
+    return run_one([&](int r) {
         const size_t Dr = (size_t)(base[r + 1] - base[r]), c0 = (size_t)(base[r] - base[0]);
         if (Dr == 0) return PB_OK;
         std::vector<float> buf((size_t)n_queries * Dr);
-        pb_status st = pb_exhaustive_scores(d->ranks[r], queries, q_off, n_queries, buf.data());
+        pb_status st = pb_exhaustive_scores(ranks[r], queries, q_off, n_queries, buf.data());
         if (st != PB_OK) return st;
         for (int64_t q = 0; q < n_queries; ++q)
             std::copy(buf.data() + (size_t)q * Dr, buf.data() + (size_t)(q + 1) * Dr, out_scores + (size_t)q * D + c0);
@@ -289,37 +305,37 @@ pb_status pb_dep_exhaustive(Deployment *d, const float *queries, const int64_t *
     }, false);
 }
 
-pb_status pb_dep_delete(Deployment *d, const int64_t *doc_ids, int64_t n_ids, const char *index_dir, int64_t *out_deleted) {
-    std::lock_guard<std::mutex> g(d->mu);
-    std::unique_lock<std::shared_mutex> l(d->layout);
-    std::vector<int64_t> n((size_t)d->world(), 0);
-    pb_status s = d->run_one([&](int r) {
-        return pb_index_delete_sharded(d->ranks[r], doc_ids, n_ids, index_dir, &n[r]);
+pb_status Deployment::del(const int64_t *doc_ids, int64_t n_ids, const char *index_dir, int64_t *out_deleted) {
+    std::lock_guard<std::mutex> g(mu);
+    std::unique_lock<std::shared_mutex> l(layout);
+    std::vector<int64_t> n((size_t)world(), 0);
+    pb_status s = run_one([&](int r) {
+        return pb_index_delete_sharded(ranks[r], doc_ids, n_ids, index_dir, &n[r]);
     });
     if (out_deleted) *out_deleted = s == PB_OK ? n[0] : 0;
     return s;
 }
 
-pb_status pb_dep_ranks(Deployment *d, const std::function<pb_status(pb_index *)> &call) {
-    std::shared_lock<std::shared_mutex> g(d->layout);
-    for (int r = 0; r < d->world(); ++r)
-        if (pb_status s = call(d->ranks[r])) {
+pb_status Deployment::in_turn(bool, const std::function<pb_status(pb_index *)> &call) {
+    std::shared_lock<std::shared_mutex> g(layout);
+    for (int r = 0; r < world(); ++r)
+        if (pb_status s = call(ranks[r])) {
             const std::string e = pb_last_error();
-            return d->world() == 1 ? s : pb_fail(s, "rank %d: %s", r, e.c_str());
+            return world() == 1 ? s : pb_fail(s, "rank %d: %s", r, e.c_str());
         }
     return PB_OK;
 }
 
 // Only the last rank receives the codec and the documents: an append goes to the end of the deployment
-pb_status pb_dep_append(Deployment *d, pb_codec *codec, const float *embeddings, const int64_t *codes,
-                        const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
-                        const char *index_dir, int64_t batch_size, int64_t *out_first_doc_id) {
-    std::lock_guard<std::mutex> g(d->mu);
-    std::unique_lock<std::shared_mutex> l(d->layout);
-    const int last = d->world() - 1;
-    std::vector<int64_t> first((size_t)d->world(), 0);
-    pb_status s = d->run_one([&](int r) {
-        pb_index *ix = d->ranks[r];
+pb_status Deployment::append(pb_codec *codec, const float *embeddings, const int64_t *codes, const uint8_t *residuals,
+                             const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space, const char *index_dir,
+                             int64_t batch_size, int64_t *out_first_doc_id) {
+    std::lock_guard<std::mutex> g(mu);
+    std::unique_lock<std::shared_mutex> l(layout);
+    const int last = world() - 1;
+    std::vector<int64_t> first((size_t)world(), 0);
+    pb_status s = run_one([&](int r) {
+        pb_index *ix = ranks[r];
         const bool mine = r == last;
         if (codec)
             return pb_index_append_sharded(ix, mine ? codec : nullptr, mine ? embeddings : nullptr, doc_lengths, n_docs,
@@ -331,12 +347,12 @@ pb_status pb_dep_append(Deployment *d, pb_codec *codec, const float *embeddings,
     return s;
 }
 
-pb_status pb_dep_rebalance(Deployment *d, const int64_t *bounds, int64_t *out_bounds) {
-    std::lock_guard<std::mutex> g(d->mu);
-    std::unique_lock<std::shared_mutex> l(d->layout);
-    const size_t W1 = (size_t)d->world() + 1;
-    std::vector<std::vector<int64_t>> got((size_t)d->world(), std::vector<int64_t>(W1, 0));
-    pb_status s = d->run_one([&](int r) { return pb_index_rebalance_sharded(d->ranks[r], bounds, got[r].data()); });
+pb_status Deployment::rebalance(const int64_t *bounds, int64_t *out_bounds) {
+    std::lock_guard<std::mutex> g(mu);
+    std::unique_lock<std::shared_mutex> l(layout);
+    const size_t W1 = (size_t)world() + 1;
+    std::vector<std::vector<int64_t>> got((size_t)world(), std::vector<int64_t>(W1, 0));
+    pb_status s = run_one([&](int r) { return pb_index_rebalance_sharded(ranks[r], bounds, got[r].data()); });
     if (s == PB_OK && out_bounds) std::copy(got[0].begin(), got[0].end(), out_bounds);
     return s;
 }

@@ -643,28 +643,16 @@ struct RowCacheState {
     std::mutex fill_mu;      // one pb_index_set_row_cache / pb_index_fill_row_cache at a time
 };
 
-struct pb_index : DocArrays {
-    int device = 0;
-    int dim = 0, nbits = 0, packed = 0;
-    long long K = 0, doc_id_base = 0;
-    int sm_count = 132;
-    DevBuf centroids, w_rev;
-    bool host_tier = false;    // PB_OPEN_HOST_RESIDUALS: `residuals` stays empty, the rows live in host.rows
-    bool host_mutable = false; // PB_OPEN_HOST_MUTABLE: appends and deletes write the host rows
-    HostTier host;
-    RowCacheState rc;
-    unsigned long long doc_gen = 0;  // changes with every publish: a fill built out of place checks it before its swap
-    bool build_ivf = false;    // no inverted file was given: built from the codes at finalize (index.rs:850-873)
-    float cmax = 1.0f;         // largest centroid L2 norm (range of the 16-bit score table)
+// A handle's switches of the search pipeline and the delete: defaults, the environment at open (pb_index_finalize), the
+// pb_set_* calls.  A copy of a handle (pb_index_clone, pb_index_clone_empty) takes its source's.
+struct Switches {
     bool fast_approx = true;   // two-pass approximate stage (exact cut either way)
     bool k1_tc = true;         // a2 on the tensor cores (k_scores16_tc) with its certified consumers: the default;
                                // PB_K1_TC=0 keeps every sub-batch on the exact fp32 kernel (the device-gated fallback)
     int k1_margin = 1;         // E: code units an estimate-built 16-bit code may differ from the exact one (PB_K1_TC_E widens it)
-    int cent_exp = 0;          // centroids enter the tensor-core operands scaled by 2^cent_exp (max norm in [1, 2))
     bool k1_diag = false;      // also run the exact table and report the largest code difference (PB_K1_TC_DIAG=1)
     bool table_diag = false;   // PB_TABLE_DIAG=1: rerun k_chunkmax16 and k_a5_live on the tensor-core table and count the
                                // words the fused chunk maxima and live bits differ in
-    DevBuf cent_h16t, cent_l16t;  // its centroid operands: fp16 hi / lo, MMA tile order
     int approx_grid = 8;       // k_approx16 CTAs per SM and query (PB_APPROX_GRID)
     bool a5_prune = true;      // bound the first pass from the live score-table rows (PB_A5_PRUNE=0: dense first pass)
     long long a5_live = -1;    // live rows aimed at per query token (PB_A5_LIVE; -1: K / 512)
@@ -677,10 +665,28 @@ struct pb_index : DocArrays {
     int ws_grid = 8;           // k_maxsim_tc CTAs per SM across the batch (PB_WS_GRID)
     int ws_grid2 = 8;          // the same for its pass 2 over the filter's survivors (PB_WS_GRID2; 1: 0.54, 2: 0.43, 4 and 8: 0.40 ms)
     int lanes = 1;             // slices of a batch searched concurrently, each on its own stream (pb_set_lanes / PB_LANES; 1 = off)
-    std::mutex lane_mu;        // one laned call at a time per handle (a second concurrent caller runs un-laned)
-    std::vector<std::unique_ptr<RankWorker>> lane_workers;  // lane_workers[l - 1] runs lane l
     bool profiling = false;
     size_t st_budget = (size_t)8 << 30;  // workspace budget of one search call (PB_WS_BUDGET_MB)
+    long long delete_window = 1ll << 22;   // tokens per compaction window of pb_index_delete (PB_DELETE_WINDOW_TOKENS)
+};
+
+struct pb_index : DocArrays, Switches {
+    int device = 0;
+    int dim = 0, nbits = 0, packed = 0;
+    long long K = 0, doc_id_base = 0;
+    int sm_count = 132;
+    DevBuf centroids, w_rev;
+    bool host_tier = false;    // PB_OPEN_HOST_RESIDUALS: `residuals` stays empty, the rows live in host.rows
+    bool host_mutable = false; // PB_OPEN_HOST_MUTABLE: appends and deletes write the host rows
+    HostTier host;
+    RowCacheState rc;
+    unsigned long long doc_gen = 0;  // changes with every publish: a fill built out of place checks it before its swap
+    bool build_ivf = false;    // no inverted file was given: built from the codes at finalize (index.rs:850-873)
+    float cmax = 1.0f;         // largest centroid L2 norm (range of the 16-bit score table)
+    int cent_exp = 0;          // centroids enter the tensor-core operands scaled by 2^cent_exp (max norm in [1, 2))
+    DevBuf cent_h16t, cent_l16t;  // its centroid operands: fp16 hi / lo, MMA tile order
+    std::mutex lane_mu;        // one laned call at a time per handle (a second concurrent caller runs un-laned)
+    std::vector<std::unique_ptr<RankWorker>> lane_workers;  // lane_workers[l - 1] runs lane l
     std::mutex mu;
     std::vector<std::unique_ptr<Workspace>> pool;
     // pb_search: concurrent single-query callers merged into shared batches (pb_index_set_coalescing; off by default)
@@ -688,7 +694,6 @@ struct pb_index : DocArrays {
     std::atomic<bool> coalesce_on{false};
     std::vector<std::unique_ptr<GatherBuf>> gather_pool;  // under mu
     float delete_ms[3] = {0.f, 0.f, 0.f};  // last pb_index_delete with profiling on: compaction, inverted file, norms
-    long long delete_window = 1ll << 22;   // tokens per compaction window of pb_index_delete (PB_DELETE_WINDOW_TOKENS)
     // Readers (searches, stage entry points, accessors) share the arrays; pb_index_append / pb_index_reserve hold them
     // alone.  A writer also holds `gate`, which every reader passes first: pthread rwlocks prefer readers, so without
     // it a steady stream of searches could keep an append waiting forever.
@@ -698,10 +703,9 @@ struct pb_index : DocArrays {
         { std::lock_guard<std::mutex> g(gate); }
         return std::shared_lock<std::shared_mutex>(rw);
     }
-    // pb_index_load_devices: this handle holds no documents and stands for the ranks of `dep` (deployment.cpp)
-    Deployment *dep = nullptr;
-    // pb_index_load_replicas: this handle holds no documents and stands for the replicas of `rep` (replicas.cpp)
-    Replicas *rep = nullptr;
+    // pb_index_load_devices / pb_index_load_replicas: this handle holds no documents and stands for the members of
+    // `group` (deployment.cpp, replicas.cpp)
+    std::unique_ptr<Group> group;
     // a rank of a replica of such a set, during one of its mutations: the vote it takes with the other replicas
     RepVote *rep_vote = nullptr;
     int rep_index = 0;
@@ -1286,11 +1290,11 @@ static pb_status coalesce_env_defaults(pb_index *ix) {
     return PB_OK;
 }
 
-// A deployment's handle (deployment.cpp): no documents of its own; what every rank shares, from rank 0
-pb_index *pb_index_new_deployment(Deployment *d, const pb_index *rank0) {
+// A deployment's or replica set's handle: no documents of its own; what every member shares, from the first
+pb_index *pb_index_new_group(Group *g, const pb_index *first) {
     pb_index *ix = new pb_index();
-    ix->dep = d;
-    pb_index_deployment_rank0(ix, rank0);
+    ix->group.reset(g);
+    pb_index_deployment_rank0(ix, first);
     coalesce_env_defaults(ix);  // cannot fail: the handle joins no group
     return ix;
 }
@@ -1299,23 +1303,9 @@ void pb_index_deployment_rank0(pb_index *ix, const pb_index *rank0) {
     ix->K = rank0->K;
 }
 
-// A replica set's handle (replicas.cpp): no documents of its own; K, dim, nbits and device from replica 0
-pb_index *pb_index_new_replicas(Replicas *rs, const pb_index *member0) {
-    pb_index *ix = new pb_index();
-    ix->rep = rs;
-    ix->device = member0->device, ix->dim = member0->dim, ix->nbits = member0->nbits, ix->packed = member0->packed;
-    ix->K = member0->K;
-    coalesce_env_defaults(ix);  // cannot fail: the handle joins no group
-    return ix;
-}
-
 // The calls a deployment or a replica set refuses: each addresses one rank's handle, one device, or one group
 static pb_status refuse_deployment(const pb_index *ix, const char *call) {
-    if (ix && ix->dep)
-        return pb_fail(PB_ERR_UNSUPPORTED, "%s on a multi-device handle (pb_index_load_devices) is not supported", call);
-    if (ix && ix->rep)
-        return pb_fail(PB_ERR_UNSUPPORTED, "%s on a replica set (pb_index_load_replicas) is not supported", call);
-    return PB_OK;
+    return ix && ix->group ? ix->group->refuse(call) : PB_OK;
 }
 
 // Derived arrays that need every token: the per-doc distinct-code lists, the token norms, and the inverted file of an
@@ -1368,9 +1358,7 @@ pb_status pb_index_finalize(pb_index *ix) {
 
 extern "C" pb_status pb_index_export_ivf(pb_index *ix, int64_t *out_ivf, int32_t *out_lengths, int64_t *out_total) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
-    if (ix->rep)
-        return pb_rep_whole(ix->rep, 0, [&](pb_index *m) { return pb_index_export_ivf(m, out_ivf, out_lengths, out_total); });
-    CKS(refuse_deployment(ix, "pb_index_export_ivf"));
+    if (ix->group) return ix->group->export_ivf(out_ivf, out_lengths, out_total);
     auto rd = ix->read_lock();
     CK(cudaSetDevice(ix->device));
     if (out_total) *out_total = ix->ivf_len;
@@ -1404,8 +1392,7 @@ extern "C" pb_status pb_index_open(const pb_index_desc *d, pb_index **out) {
 
 extern "C" void pb_index_close(pb_index *ix) {
     if (!ix) return;
-    if (ix->dep) pb_dep_close(ix->dep);  // joins its threads, closes its ranks, destroys its group
-    if (ix->rep) pb_rep_close(ix->rep);  // joins its threads, closes its replicas
+    ix->group.reset();  // first: joins its threads, closes its members
     cudaSetDevice(ix->device);
     ix->lane_workers.clear();  // joins the helper threads
     cudaDeviceSynchronize();
@@ -1413,44 +1400,39 @@ extern "C" void pb_index_close(pb_index *ix) {
 }
 
 // D and N change under pb_index_append; K, dim, nbits and the device are fixed at open
-extern "C" int64_t pb_index_num_documents(const pb_index *ix) {
-    if (!ix) return 0;
-    long long D, N;
-    if (ix->dep) return pb_dep_totals(ix->dep, &D, &N) == PB_OK ? D : 0;
-    if (ix->rep) return pb_index_num_documents(pb_rep_member(ix->rep, 0));
+void pb_index_totals(const pb_index *ix, long long *D, long long *N) {
+    if (ix->group) return ix->group->totals(D, N);
     auto rd = ix->read_lock();
-    return ix->D;
+    *D = ix->D, *N = ix->N;
+}
+extern "C" int64_t pb_index_num_documents(const pb_index *ix) {
+    long long D = 0, N = 0;
+    if (ix) pb_index_totals(ix, &D, &N);
+    return D;
 }
 extern "C" int64_t pb_index_num_embeddings(const pb_index *ix) {
-    if (!ix) return 0;
-    long long D, N;
-    if (ix->dep) return pb_dep_totals(ix->dep, &D, &N) == PB_OK ? N : 0;
-    if (ix->rep) return pb_index_num_embeddings(pb_rep_member(ix->rep, 0));
-    auto rd = ix->read_lock();
-    return ix->N;
+    long long D = 0, N = 0;
+    if (ix) pb_index_totals(ix, &D, &N);
+    return N;
 }
 extern "C" int64_t pb_index_num_partitions(const pb_index *ix) { return ix ? ix->K : 0; }
 extern "C" double pb_index_avg_doclen(const pb_index *ix) {
-    if (!ix) return 0.0;
-    long long D, N;
-    if (ix->dep) return pb_dep_totals(ix->dep, &D, &N) == PB_OK && D ? (double)N / (double)D : 0.0;
-    if (ix->rep) return pb_index_avg_doclen(pb_rep_member(ix->rep, 0));
-    auto rd = ix->read_lock();
-    return ix->D ? (double)ix->N / (double)ix->D : 0.0;
+    long long D = 0, N = 0;
+    if (ix) pb_index_totals(ix, &D, &N);
+    return D ? (double)N / (double)D : 0.0;
 }
 extern "C" int32_t pb_index_embedding_dim(const pb_index *ix) { return ix ? ix->dim : 0; }
 extern "C" int32_t pb_index_nbits(const pb_index *ix) { return ix ? ix->nbits : 0; }
 extern "C" int32_t pb_index_device(const pb_index *ix) {
     if (!ix) return -1;
     int32_t dv = ix->device;  // a deployment's: its rank 0's, which pb_index_remove_ranks may change
-    if (ix->dep) pb_dep_first(ix->dep, [&](pb_index *r0) { return dv = r0->device, PB_OK; });
+    if (ix->group && ix->group->as_deployment()) ix->group->one(0, [&](pb_index *r0) { return dv = r0->device, PB_OK; });
     return dv;
 }
 
 extern "C" pb_status pb_index_memory(const pb_index *ix, int64_t *device_bytes, int64_t *host_bytes) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
-    if (ix->dep) return pb_dep_memory(ix->dep, device_bytes, host_bytes);
-    if (ix->rep) return pb_rep_memory(ix->rep, device_bytes, host_bytes);
+    if (ix->group) return ix->group->memory(device_bytes, host_bytes);
     auto rd = ix->read_lock();
     size_t dev = ix->centroids.cap + ix->w_rev.cap + ix->cent_h16t.cap + ix->cent_l16t.cap + ix->rc.rows.cap;
     for (const DevBuf *b : DocArrays::buffers(*ix))
@@ -1462,8 +1444,7 @@ extern "C" pb_status pb_index_memory(const pb_index *ix, int64_t *device_bytes, 
 
 extern "C" pb_status pb_index_shard_layout(const pb_index *ix, int32_t *out_world, int64_t *out_bounds, int32_t *out_devices) {
     if (!ix || !out_world) return pb_fail(PB_ERR_INVALID, "null argument");
-    if (ix->dep) return pb_dep_layout(ix->dep, out_world, out_bounds, out_devices);
-    if (ix->rep) return pb_index_shard_layout(pb_rep_member(ix->rep, 0), out_world, out_bounds, out_devices);
+    if (ix->group) return ix->group->shard_layout(out_world, out_bounds, out_devices);
     auto rd = ix->read_lock();
     *out_world = 1;
     if (out_bounds) out_bounds[0] = ix->doc_id_base, out_bounds[1] = ix->doc_id_base + ix->D;
@@ -1484,18 +1465,15 @@ extern "C" void pb_search_params_default(pb_search_params *p) {  // search.rs:58
 
 extern "C" void pb_set_fast_approx(pb_index *ix, int32_t enabled) {
     if (!ix) return;
-    if (ix->dep) return pb_dep_each(ix->dep, [&](pb_index *m) { pb_set_fast_approx(m, enabled); });
-    if (ix->rep) return pb_rep_each(ix->rep, [&](pb_index *m) { pb_set_fast_approx(m, enabled); });
+    if (ix->group) return ix->group->each([&](pb_index *m) { pb_set_fast_approx(m, enabled); });
     ix->fast_approx = enabled != 0;  // 0 = single exact pass over every candidate, otherwise two-pass
 }
 extern "C" void pb_set_scores_tc(pb_index *ix, int32_t enabled) {
-    if (ix && ix->dep) return pb_dep_each(ix->dep, [&](pb_index *m) { pb_set_scores_tc(m, enabled); });
-    if (ix && ix->rep) return pb_rep_each(ix->rep, [&](pb_index *m) { pb_set_scores_tc(m, enabled); });
+    if (ix && ix->group) return ix->group->each([&](pb_index *m) { pb_set_scores_tc(m, enabled); });
     if (ix) ix->k1_tc = enabled != 0;  // effective when the tensor-core operands were built at open (k1_tc_usable)
 }
 extern "C" void pb_set_lanes(pb_index *ix, int32_t lanes) {
-    if (ix && ix->dep) return pb_dep_each(ix->dep, [&](pb_index *m) { pb_set_lanes(m, lanes); });
-    if (ix && ix->rep) return pb_rep_each(ix->rep, [&](pb_index *m) { pb_set_lanes(m, lanes); });
+    if (ix && ix->group) return ix->group->each([&](pb_index *m) { pb_set_lanes(m, lanes); });
     if (ix) ix->lanes = std::min(8, std::max(1, (int)lanes));
 }
 extern "C" pb_status pb_index_set_coalescing(pb_index *ix, const pb_coalesce_config *cfg) {
@@ -1509,7 +1487,7 @@ extern "C" pb_status pb_index_set_coalescing(pb_index *ix, const pb_coalesce_con
         c.max_queries = cfg->max_queries;
         c.max_wait_us = std::min(cfg->max_wait_us, 10000);
         // a replica set runs max_inflight merged batches per replica
-        c.max_inflight = ix->rep ? cfg->max_inflight * pb_rep_count(ix->rep) : cfg->max_inflight;
+        c.max_inflight = pb_replicas_of(ix) ? cfg->max_inflight * ix->group->size() : cfg->max_inflight;
     }
     ix->coalescer.configure(c);
     ix->coalesce_on = c.max_queries > 1;
@@ -1525,13 +1503,11 @@ extern "C" pb_status pb_index_coalesce_stats(pb_index *ix, pb_coalesce_stats *ou
     return PB_OK;
 }
 extern "C" void pb_set_fast_exact(pb_index *ix, int32_t enabled) {
-    if (ix && ix->dep) return pb_dep_each(ix->dep, [&](pb_index *m) { pb_set_fast_exact(m, enabled); });
-    if (ix && ix->rep) return pb_rep_each(ix->rep, [&](pb_index *m) { pb_set_fast_exact(m, enabled); });
+    if (ix && ix->group) return ix->group->each([&](pb_index *m) { pb_set_fast_exact(m, enabled); });
     if (ix) ix->fast_exact = enabled != 0;
 }
 extern "C" void pb_set_profiling(pb_index *ix, int32_t enabled) {
-    if (ix && ix->dep) return pb_dep_each(ix->dep, [&](pb_index *m) { pb_set_profiling(m, enabled); });
-    if (ix && ix->rep) return pb_rep_each(ix->rep, [&](pb_index *m) { pb_set_profiling(m, enabled); });
+    if (ix && ix->group) return ix->group->each([&](pb_index *m) { pb_set_profiling(m, enabled); });
     if (ix) ix->profiling = enabled != 0;
 }
 extern "C" pb_status pb_last_stage_stats(pb_index *, float *out_ms, int32_t *out_launches) {
@@ -3395,9 +3371,9 @@ static pb_status search_impl(pb_index *ix, const SearchIO &io) {
 // - A deployment runs the call on every rank, rank 0 into the caller's outputs.
 // - A plain handle searches it.
 static pb_status search_io(pb_index *ix, const SearchIO &io, const char *traced) {
-    if (ix && ix->rep) {
+    if (Replicas *rs = pb_replicas_of(ix)) {
         auto whole = [&] {
-            return pb_rep_whole(ix->rep, io.n_queries, [&](pb_index *m) { return search_io(m, io, traced); });
+            return ix->group->one(io.n_queries, [&](pb_index *m) { return search_io(m, io, traced); });
         };
         bool cut = !io.trace && io.n_queries > 1 && io.queries && io.q_off && io.qp;
         for (int64_t b = 0; cut && b < io.n_queries; ++b) {
@@ -3407,9 +3383,9 @@ static pb_status search_io(pb_index *ix, const SearchIO &io, const char *traced)
                   check_query_args(p) == PB_OK && query_kept_docs(p, &M) == PB_OK;
         }
         if (!cut) return whole();
-        std::vector<Stats> stats((size_t)pb_rep_count(ix->rep));
+        std::vector<Stats> stats((size_t)ix->group->size());
         size_t slices = 0;
-        const pb_status st = pb_rep_search(ix->rep, io.n_queries, [&](pb_index *m, int64_t b0, int64_t b1, int k) {
+        const pb_status st = pb_rep_search(rs, io.n_queries, [&](pb_index *m, int64_t b0, int64_t b1, int k) {
             const pb_status r = search_io(m, slice_io(io, b0, b1), traced);
             stats[k] = g_stats;
             if (b1 == io.n_queries) slices = k + 1;  // the last slice ends the call
@@ -3419,9 +3395,9 @@ static pb_status search_io(pb_index *ix, const SearchIO &io, const char *traced)
         g_stats = merge_slices(stats.data(), slices);
         return PB_OK;
     }
-    if (ix && ix->dep) {
+    if (Deployment *d = ix && ix->group ? ix->group->as_deployment() : nullptr) {
         if (io.trace) CKS(refuse_deployment(ix, traced));
-        return pb_dep_search(ix->dep, io.n_queries, io.out_stride, io.out_ids, io.out_scores, io.out_counts,
+        return pb_dep_search(d, io.n_queries, io.out_stride, io.out_ids, io.out_scores, io.out_counts,
                              [&](pb_index *m, int64_t *ids, float *sc, int32_t *cn) {
                                  SearchIO rank = io;
                                  rank.out_ids = ids, rank.out_scores = sc, rank.out_counts = cn;
@@ -3530,9 +3506,9 @@ static pb_status check_request(const pb_index *ix, long long D, const SearchRequ
 }
 
 int CoalescedRun::operator()(pbq::Request *const *reqs, size_t n, std::string &err) const {
-    if (ix->rep) {  // a replica set: the merged batch goes whole to the least-loaded replica
+    if (pb_replicas_of(ix)) {  // a replica set: the merged batch goes whole to the least-loaded replica
         int r = 0;
-        pb_rep_whole(ix->rep, (int64_t)n, [&](pb_index *m) { return (pb_status)(r = CoalescedRun{m}(reqs, n, err)); });
+        ix->group->one((int64_t)n, [&](pb_index *m) { return (pb_status)(r = CoalescedRun{m}(reqs, n, err)); });
         return r;
     }
     pb_status st;
@@ -3598,14 +3574,14 @@ extern "C" pb_status pb_search(pb_index *ix, const float *query, int64_t n_query
         return search_alone(ix, r);
     }
     pb_status st;
-    if (ix->dep || ix->rep) {  // as one handle of the whole index: every rank's K, the deployment's D (rank 0 may be empty)
+    if (ix->group) {  // as one handle of the whole index: every rank's K, the deployment's D (rank 0 may be empty)
         const long long D = pb_index_num_documents(ix);
-        pb_index *m = ix->rep ? pb_rep_member(ix->rep, 0) : ix;
+        pb_index *m = pb_replicas_of(ix) ? ix->group->member(0) : ix;
         auto check = [&](pb_index *h) {
             auto rd = h->read_lock();
             return check_request(h, D, r);
         };
-        st = m->dep ? pb_dep_first(m->dep, check) : check(m);
+        st = m->group ? m->group->one(0, check) : check(m);
     } else {
         auto rd = ix->read_lock();
         st = check_request(ix, ix->D, r);
@@ -3640,9 +3616,8 @@ extern "C" pb_status pb_search_batch_device(pb_index *ix, const float *d_queries
 // stage entry points
 // ------------------------------------------------------------------------------------------
 extern "C" pb_status pb_centroid_scores(pb_index *ix, const float *query_tokens, int64_t n, float *out) {
-    if (ix && ix->dep)  // the centroids are replicated
-        return pb_dep_first(ix->dep, [&](pb_index *r0) { return pb_centroid_scores(r0, query_tokens, n, out); });
-    if (ix && ix->rep) return pb_rep_whole(ix->rep, 0, [&](pb_index *m) { return pb_centroid_scores(m, query_tokens, n, out); });
+    if (ix && ix->group)  // the centroids are replicated: a deployment's rank 0, a replica
+        return ix->group->one(0, [&](pb_index *m) { return pb_centroid_scores(m, query_tokens, n, out); });
     if (!ix || (!query_tokens && n) || (!out && n)) return pb_fail(PB_ERR_INVALID, "null argument");
     if (n == 0) return PB_OK;
     auto rd = ix->read_lock();
@@ -3675,11 +3650,7 @@ extern "C" pb_status pb_centroid_scores(pb_index *ix, const float *query_tokens,
 
 extern "C" pb_status pb_decompress_documents(pb_index *ix, const int64_t *doc_ids, int64_t n_docs, float *out_embeddings,
                                              int64_t *out_lengths) {
-    if (ix && ix->dep) return pb_dep_decompress(ix->dep, doc_ids, n_docs, out_embeddings, out_lengths);
-    if (ix && ix->rep)
-        return pb_rep_whole(ix->rep, 0, [&](pb_index *m) {
-            return pb_decompress_documents(m, doc_ids, n_docs, out_embeddings, out_lengths);
-        });
+    if (ix && ix->group) return ix->group->decompress(doc_ids, n_docs, out_embeddings, out_lengths);
     if (!ix || (!doc_ids && n_docs) || !out_lengths) return pb_fail(PB_ERR_INVALID, "null argument");
     auto rd = ix->read_lock();
     CK(cudaSetDevice(ix->device));
@@ -3966,9 +3937,7 @@ extern "C" pb_status pb_pool_embeddings(int32_t device, const float *embeddings,
 
 extern "C" pb_status pb_exhaustive_scores(pb_index *ix, const float *queries, const int64_t *q_off, int64_t n_queries,
                                           float *out_scores) {
-    if (ix && ix->dep) return pb_dep_exhaustive(ix->dep, queries, q_off, n_queries, out_scores);
-    if (ix && ix->rep)
-        return pb_rep_whole(ix->rep, 0, [&](pb_index *m) { return pb_exhaustive_scores(m, queries, q_off, n_queries, out_scores); });
+    if (ix && ix->group) return ix->group->exhaustive(queries, q_off, n_queries, out_scores);
     if (!ix || (!queries && n_queries) || !q_off || (!out_scores && n_queries)) return pb_fail(PB_ERR_INVALID, "null argument");
     auto rd = ix->read_lock();
     CK(cudaSetDevice(ix->device));
@@ -4841,12 +4810,9 @@ extern "C" pb_status pb_index_append(pb_index *ix, pb_codec *codec, const float 
                                      int64_t n_docs, int32_t memory_space, const char *index_dir, int64_t batch_size,
                                      int64_t *out_first_doc_id) {
     if (!codec) return pb_fail(PB_ERR_INVALID, "null argument");
-    if (ix && ix->dep)
-        return pb_dep_append(ix->dep, codec, embeddings, nullptr, nullptr, doc_lengths, n_docs, memory_space, index_dir,
-                             batch_size, out_first_doc_id);
-    if (ix && ix->rep)
-        return pb_rep_append(ix->rep, codec, embeddings, nullptr, nullptr, doc_lengths, n_docs, memory_space, index_dir,
-                             batch_size, out_first_doc_id);
+    if (ix && ix->group)
+        return ix->group->append(codec, embeddings, nullptr, nullptr, doc_lengths, n_docs, memory_space, index_dir,
+                                 batch_size, out_first_doc_id);
     return append_impl(ix, codec, embeddings, nullptr, nullptr, doc_lengths, n_docs, memory_space, index_dir, batch_size,
                        out_first_doc_id);
 }
@@ -4854,19 +4820,15 @@ extern "C" pb_status pb_index_append(pb_index *ix, pb_codec *codec, const float 
 extern "C" pb_status pb_index_append_encoded(pb_index *ix, const int64_t *codes, const uint8_t *residuals,
                                              const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
                                              int64_t *out_first_doc_id) {
-    if (ix && ix->dep)
-        return pb_dep_append(ix->dep, nullptr, nullptr, codes, residuals, doc_lengths, n_docs, memory_space, nullptr, 0,
-                             out_first_doc_id);
-    if (ix && ix->rep)
-        return pb_rep_append(ix->rep, nullptr, nullptr, codes, residuals, doc_lengths, n_docs, memory_space, nullptr, 0,
-                             out_first_doc_id);
+    if (ix && ix->group)
+        return ix->group->append(nullptr, nullptr, codes, residuals, doc_lengths, n_docs, memory_space, nullptr, 0,
+                                 out_first_doc_id);
     return append_impl(ix, nullptr, nullptr, codes, residuals, doc_lengths, n_docs, memory_space, nullptr, 0, out_first_doc_id);
 }
 
 extern "C" pb_status pb_index_reserve(pb_index *ix, int64_t num_documents, int64_t num_embeddings) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
-    if (ix->rep) return pb_rep_reserve(ix->rep, num_documents, num_embeddings);
-    CKS(refuse_deployment(ix, "pb_index_reserve (reserve a rank's capacity before it joins a group)"));
+    if (ix->group) return ix->group->reserve(num_documents, num_embeddings);
     std::lock_guard<std::mutex> gate(ix->gate);
     std::unique_lock<std::shared_mutex> wr(ix->rw);
     if (ix->comm.joined()) return pb_fail(PB_ERR_UNSUPPORTED, "appends to a doc-sharded handle are not supported");
@@ -5123,8 +5085,7 @@ extern "C" pb_status pb_index_delete(pb_index *ix, const int64_t *doc_ids, int64
                                      int64_t *out_deleted) {
     if (!ix || (!doc_ids && n_ids) || n_ids < 0) return pb_fail(PB_ERR_INVALID, "null argument");
     if (out_deleted) *out_deleted = 0;
-    if (ix->dep) return pb_dep_delete(ix->dep, doc_ids, n_ids, index_dir, out_deleted);
-    if (ix->rep) return pb_rep_delete(ix->rep, doc_ids, n_ids, index_dir, out_deleted);
+    if (ix->group) return ix->group->del(doc_ids, n_ids, index_dir, out_deleted);
     return pb_members_delete({ix}, doc_ids, n_ids, index_dir, out_deleted);
 }
 
@@ -5152,8 +5113,7 @@ static pb_status row_cache_clear(pb_index *ix) {
 extern "C" pb_status pb_index_set_row_cache(pb_index *ix, int64_t max_bytes) {
     if (max_bytes < 0) return pb_fail(PB_ERR_INVALID, "row cache budget %lld < 0", (long long)max_bytes);
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
-    if (ix->dep) return pb_dep_ranks(ix->dep, [&](pb_index *m) { return pb_index_set_row_cache(m, max_bytes); });
-    if (ix->rep) return pb_rep_members(ix->rep, true, [&](pb_index *m) { return pb_index_set_row_cache(m, max_bytes); });
+    if (ix->group) return ix->group->in_turn(true, [&](pb_index *m) { return pb_index_set_row_cache(m, max_bytes); });
     CKS(refuse_row_cache(ix));
     std::lock_guard<std::mutex> f(ix->rc.fill_mu);
     DevBuf off, cnt;  // the old arrays leave with these, after the locks
@@ -5276,7 +5236,7 @@ extern "C" pb_status pb_index_fill_row_cache(pb_index *ix, const int64_t *doc_id
     if (!ix || !out_n || (!doc_ids && n_ids > 0) || (doc_ids && n_ids < 0) || (out_ids && out_cap < 0))
         return pb_fail(PB_ERR_INVALID, "null argument");
     *out_n = 0;
-    if (!ix->dep && !ix->rep) return row_cache_fill(ix, doc_ids, n_ids, out_ids, out_cap, out_n);
+    if (!ix->group) return row_cache_fill(ix, doc_ids, n_ids, out_ids, out_cap, out_n);
     // ranks or replicas in order, each writing its ids after the previous ones'
     auto one = [&](pb_index *m) {
         const int64_t at = std::min(*out_n, out_cap);
@@ -5285,13 +5245,13 @@ extern "C" pb_status pb_index_fill_row_cache(pb_index *ix, const int64_t *doc_id
         *out_n += n;
         return s;
     };
-    return ix->dep ? pb_dep_ranks(ix->dep, one) : pb_rep_members(ix->rep, true, one);
+    return ix->group->in_turn(true, one);
 }
 
 extern "C" pb_status pb_index_row_cache_stats(pb_index *ix, pb_row_cache_stats *out, int32_t reset) {
     if (!ix || !out) return pb_fail(PB_ERR_INVALID, "null argument");
     *out = pb_row_cache_stats{};
-    if (ix->dep || ix->rep) {  // sums over the ranks or replicas
+    if (ix->group) {  // sums over the ranks or replicas
         auto one = [&](pb_index *m) {
             pb_row_cache_stats s{};
             CKS(pb_index_row_cache_stats(m, &s, reset));
@@ -5300,7 +5260,7 @@ extern "C" pb_status pb_index_row_cache_stats(pb_index *ix, pb_row_cache_stats *
             out->hit_bytes += s.hit_bytes, out->last_fill_ms += s.last_fill_ms;
             return PB_OK;
         };
-        return ix->dep ? pb_dep_ranks(ix->dep, one) : pb_rep_members(ix->rep, false, one);
+        return ix->group->in_turn(false, one);
     }
     auto rd = ix->read_lock();
     RowCacheState &c = ix->rc;
@@ -5342,12 +5302,7 @@ pb_status pb_index_clone(const pb_index *src, int device, pb_index **out) {
     ix->sm_count = prop.multiProcessorCount;  // the grids sized from it follow the copy's device
     ix->dim = src->dim, ix->nbits = src->nbits, ix->packed = src->packed, ix->K = src->K, ix->doc_id_base = src->doc_id_base;
     ix->host_tier = src->host_tier, ix->build_ivf = src->build_ivf, ix->cmax = src->cmax, ix->cent_exp = src->cent_exp;
-    ix->fast_approx = src->fast_approx, ix->k1_tc = src->k1_tc, ix->k1_margin = src->k1_margin, ix->k1_diag = src->k1_diag;
-    ix->table_diag = src->table_diag, ix->approx_grid = src->approx_grid, ix->a5_prune = src->a5_prune;
-    ix->a5_live = src->a5_live, ix->a5_m1 = src->a5_m1, ix->a5_waves = src->a5_waves, ix->probe16 = src->probe16;
-    ix->fast_exact = src->fast_exact, ix->filter_diag = src->filter_diag, ix->pair_exact = src->pair_exact;
-    ix->ws_grid = src->ws_grid, ix->ws_grid2 = src->ws_grid2, ix->lanes = src->lanes, ix->profiling = src->profiling;
-    ix->st_budget = src->st_budget, ix->delete_window = src->delete_window;
+    static_cast<Switches &>(*ix) = static_cast<const Switches &>(*src);
     ix->host_mutable = src->host_mutable;
     if (src->host_tier) {  // the store is shared; the table is the copy's device's own
         ix->host.rows = src->host.rows;
@@ -5383,12 +5338,7 @@ pb_status pb_index_clone_empty(const pb_index *src, int device, long long doc_id
     ix->sm_count = prop.multiProcessorCount;
     ix->dim = src->dim, ix->nbits = src->nbits, ix->packed = src->packed, ix->K = src->K, ix->doc_id_base = doc_id_base;
     ix->cmax = src->cmax;
-    ix->fast_approx = src->fast_approx, ix->k1_tc = src->k1_tc, ix->k1_margin = src->k1_margin, ix->k1_diag = src->k1_diag;
-    ix->table_diag = src->table_diag, ix->approx_grid = src->approx_grid, ix->a5_prune = src->a5_prune;
-    ix->a5_live = src->a5_live, ix->a5_m1 = src->a5_m1, ix->a5_waves = src->a5_waves, ix->probe16 = src->probe16;
-    ix->fast_exact = src->fast_exact, ix->filter_diag = src->filter_diag, ix->pair_exact = src->pair_exact;
-    ix->ws_grid = src->ws_grid, ix->ws_grid2 = src->ws_grid2, ix->lanes = src->lanes, ix->profiling = src->profiling;
-    ix->st_budget = src->st_budget, ix->delete_window = src->delete_window;
+    static_cast<Switches &>(*ix) = static_cast<const Switches &>(*src);
     // the per-doc arrays of no documents, allocated as an open of an empty range allocates them
     const long long zero = 0;
     CKS(upload(ix->doc_off, &zero, 8, PB_MEM_HOST));
@@ -5421,8 +5371,8 @@ static pb_status tail_rows(const pb_index *ix, long long t0, long long n, std::v
     return PB_OK;
 }
 
-Replicas *pb_replicas_of(const pb_index *ix) { return ix ? ix->rep : nullptr; }
-pb_index *pb_rank_of(pb_index *ix, int r) { return ix->dep ? pb_dep_rank(ix->dep, r) : ix; }
+Replicas *pb_replicas_of(const pb_index *ix) { return ix && ix->group ? ix->group->as_replicas() : nullptr; }
+pb_index *pb_rank_of(pb_index *ix, int r) { return ix->group && ix->group->as_deployment() ? ix->group->member(r) : ix; }
 bool pb_host_rows_shared(pb_index *ix) { return pb_rank_of(ix, 0)->host_mutable; }
 pb_status pb_sync_devices(pb_index *ix) {
     pb_status st = PB_OK;
@@ -5430,7 +5380,7 @@ pb_status pb_sync_devices(pb_index *ix) {
         if (st == PB_OK && (cudaSetDevice(r->device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess))
             st = pb_fail(PB_ERR_CUDA, "synchronizing device %d failed", r->device);
     };
-    if (ix->dep) pb_dep_each(ix->dep, sync);
+    if (ix->group) ix->group->each(sync);
     else sync(ix);
     return st;
 }
@@ -5662,7 +5612,7 @@ RepVote *pb_rep_vote_new(int ranks, bool with_dir, bool share_rows) {
 void pb_rep_vote_free(RepVote *v) { delete v; }
 void pb_index_set_rep_vote(pb_index *member, RepVote *v, int replica) {
     auto set = [&](pb_index *r) { r->rep_vote = v, r->rep_index = replica; };
-    if (member->dep) pb_dep_each(member->dep, set);
+    if (member->group) member->group->each(set);
     else set(member);
 }
 
@@ -5914,32 +5864,29 @@ static pb_status rebalance_body(pb_index *ix, RepTurn &turn, const int64_t *boun
 
 extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bounds, int64_t *out_bounds) {
     if (!ix) return pb_fail(PB_ERR_INVALID, "null argument");
-    if (ix->dep) return pb_dep_rebalance(ix->dep, bounds, out_bounds);
-    if (ix->rep) return pb_rep_rebalance(ix->rep, bounds, out_bounds);
+    if (ix->group) return ix->group->rebalance(bounds, out_bounds);
     return pb_index_rebalance_shares(ix, bounds, nullptr, out_bounds);
 }
 
 // The calls that change a deployment's number of ranks (DESIGN §4t) address a deployment of pb_index_load_devices only
 static pb_status refuse_resize(const pb_index *ix, const char *call) {
-    if (ix->rep) return pb_fail(PB_ERR_UNSUPPORTED, "%s on a replica set (pb_index_load_replicas) is not supported", call);
-    if (!ix->dep)
-        return pb_fail(PB_ERR_UNSUPPORTED, "%s needs a multi-device handle of pb_index_load_devices (this handle is %s)",
-                       call, ix->comm.joined() ? "a rank of a doc-sharded group" : "a single index");
-    return PB_OK;
+    if (ix->group) return ix->group->as_deployment() ? PB_OK : ix->group->refuse(call);
+    return pb_fail(PB_ERR_UNSUPPORTED, "%s needs a multi-device handle of pb_index_load_devices (this handle is %s)",
+                   call, ix->comm.joined() ? "a rank of a doc-sharded group" : "a single index");
 }
 
 extern "C" pb_status pb_index_add_devices(pb_index *ix, const int32_t *devices, int32_t n_devices, const int64_t *bounds,
                                           int64_t *out_bounds) {
     if (!ix || !devices) return pb_fail(PB_ERR_INVALID, "null argument");
     CKS(refuse_resize(ix, "pb_index_add_devices"));
-    return pb_dep_add_devices(ix->dep, devices, n_devices, bounds, out_bounds);
+    return pb_dep_add_devices(ix->group->as_deployment(), devices, n_devices, bounds, out_bounds);
 }
 
 extern "C" pb_status pb_index_remove_ranks(pb_index *ix, const int32_t *ranks, int32_t n_ranks, const int64_t *bounds,
                                            int64_t *out_bounds) {
     if (!ix || !ranks) return pb_fail(PB_ERR_INVALID, "null argument");
     CKS(refuse_resize(ix, "pb_index_remove_ranks"));
-    return pb_dep_remove_ranks(ix->dep, ix, ranks, n_ranks, bounds, out_bounds);
+    return pb_dep_remove_ranks(ix->group->as_deployment(), ix, ranks, n_ranks, bounds, out_bounds);
 }
 
 pb_status pb_index_rebalance_shares(pb_index *ix, const int64_t *bounds, const uint8_t *shares, int64_t *out_bounds) {
@@ -6244,8 +6191,7 @@ static pb_status rebalance_body(pb_index *ix, RepTurn &turn, const int64_t *boun
 
 extern "C" pb_status pb_last_delete_ms(pb_index *ix, float *out_ms) {
     if (!ix || !out_ms) return pb_fail(PB_ERR_INVALID, "null argument");
-    if (ix->rep) return pb_last_delete_ms(pb_rep_member(ix->rep, 0), out_ms);  // the set's last delete ran there too
-    CKS(refuse_deployment(ix, "pb_last_delete_ms"));
+    if (ix->group) return ix->group->last_delete_ms(out_ms);
     auto rd = ix->read_lock();
     memcpy(out_ms, ix->delete_ms, sizeof ix->delete_ms);
     return PB_OK;

@@ -80,79 +80,72 @@ inline void run_slots(int k, const Job &job, const std::unique_ptr<RankWorker> *
     }
 }
 
-// A deployment (pb_index_load_devices, deployment.cpp, DESIGN §4o): the ranks of a doc-sharded index in one process,
-// driven through the public entry points by the library's own threads.  Its handle is a pb_index that holds no
-// documents; the entry points of engine.cu hand such a handle to the functions below.
+// A handle that holds no documents and stands for other handles, its members: a deployment (pb_index_load_devices,
+// deployment.cpp, DESIGN §4o) for the ranks of a doc-sharded index in one process, driven by the library's own
+// threads; a replica set (pb_index_load_replicas, replicas.cpp, DESIGN §4q) for R full copies of an index, each a plain
+// handle or a deployment.  The members are driven through the public entry points.  Such a handle's pb_index owns its
+// Group; the entry points of engine.cu check their arguments and hand the call to it.
 struct Deployment;
-// the handle: K, dim, nbits and device copied from rank 0 (pb_index_deployment_rank0); the PB_COALESCE* defaults applied
-pb_index *pb_index_new_deployment(Deployment *d, const pb_index *rank0);
+struct Replicas;
+struct Group {
+    virtual ~Group() = default;
+    // what the handle is called in a refusal
+    virtual const char *kind() const = 0;
+    pb_status refuse(const char *call) const {
+        return pb_fail(PB_ERR_UNSUPPORTED, "%s on %s is not supported", call, kind());
+    }
+    // the concrete group, for the calls only one kind serves (search, resize); null for the other kind
+    virtual Deployment *as_deployment() { return nullptr; }
+    virtual Replicas *as_replicas() { return nullptr; }
+    // member i's handle, unlocked: only for a group whose members cannot change (a replica set, or a deployment that is
+    // a replica set's member and so refuses pb_index_add_devices / pb_index_remove_ranks); elsewhere one() or in_turn()
+    virtual pb_index *member(int i) = 0;
+    virtual int size() = 0;
+    // the whole index's documents and tokens, read together
+    virtual void totals(long long *D, long long *N) = 0;
+    virtual pb_status memory(int64_t *device_bytes, int64_t *host_bytes) = 0;
+    virtual pb_status shard_layout(int32_t *out_world, int64_t *out_bounds, int32_t *out_devices) = 0;
+    // pb_index_append (codec != null) or pb_index_append_encoded
+    virtual pb_status append(pb_codec *codec, const float *embeddings, const int64_t *codes, const uint8_t *residuals,
+                             const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space, const char *index_dir,
+                             int64_t batch_size, int64_t *out_first_doc_id) = 0;
+    virtual pb_status del(const int64_t *doc_ids, int64_t n_ids, const char *index_dir, int64_t *out_deleted) = 0;
+    virtual pb_status rebalance(const int64_t *bounds, int64_t *out_bounds) = 0;
+    virtual pb_status reserve(int64_t num_documents, int64_t num_embeddings) = 0;
+    virtual pb_status decompress(const int64_t *doc_ids, int64_t n_docs, float *out_embeddings, int64_t *out_lengths) = 0;
+    virtual pb_status exhaustive(const float *queries, const int64_t *q_off, int64_t n_queries, float *out_scores) = 0;
+    virtual pb_status export_ivf(int64_t *out_ivf, int32_t *out_lengths, int64_t *out_total) = 0;
+    virtual pb_status last_delete_ms(float *out_ms) = 0;
+    // call(m) on every member's handle, on the caller's thread, outside the group's collectives (the pb_set_* switches)
+    virtual void each(const std::function<void(pb_index *)> &call) = 0;
+    // call(m) on every member in turn, the lowest member's failure first, as a writer or a reader of the group (the row
+    // cache's entry points)
+    virtual pb_status in_turn(bool writer, const std::function<pb_status(pb_index *)> &call) = 0;
+    // call(m) on one member, on the caller's thread, for a whole request of n queries (a merged batch, a reader)
+    virtual pb_status one(int64_t n_queries, const std::function<pb_status(pb_index *)> &call) = 0;
+};
+// A group's handle, owning g: K, dim, nbits and device copied from g's first member (pb_index_deployment_rank0); the
+// PB_COALESCE* defaults applied
+pb_index *pb_index_new_group(Group *g, const pb_index *first);
 // the handle's fields taken from rank 0 again, after a resize gave it another rank 0
 void pb_index_deployment_rank0(pb_index *ix, const pb_index *rank0);
-// rank r's handle, unlocked: only for a deployment whose ranks cannot change (a replica set's member, which refuses
-// pb_index_add_devices / pb_index_remove_ranks); elsewhere pb_dep_first or pb_dep_ranks
-pb_index *pb_dep_rank(Deployment *d, int r);
-// call(rank 0's handle) on the caller's thread; a resize waits for it
-pb_status pb_dep_first(Deployment *d, const std::function<pb_status(pb_index *)> &call);
-// Stops and joins the threads, closes the ranks, destroys the group and d
-void pb_dep_close(Deployment *d);
-// call(m) on every rank's handle, on the caller's thread (the pb_set_* switches); mutations wait for it
-void pb_dep_each(Deployment *d, const std::function<void(pb_index *)> &call);
 // A search collective: call(m, ids, scores, counts) on every rank at once, rank 0 with the caller's outputs and the
 // others with scratch outputs of n_queries rows of `stride` (null where the caller's is null)
 pb_status pb_dep_search(Deployment *d, int64_t n_queries, int64_t stride, int64_t *out_ids, float *out_scores,
                         int32_t *out_counts,
                         const std::function<pb_status(pb_index *, int64_t *, float *, int32_t *)> &call);
-pb_status pb_dep_totals(Deployment *d, long long *D, long long *N);
-pb_status pb_dep_memory(Deployment *d, int64_t *device_bytes, int64_t *host_bytes);
-pb_status pb_dep_layout(Deployment *d, int32_t *out_world, int64_t *out_bounds, int32_t *out_devices);
-pb_status pb_dep_decompress(Deployment *d, const int64_t *doc_ids, int64_t n_docs, float *out_embeddings,
-                            int64_t *out_lengths);
-pb_status pb_dep_exhaustive(Deployment *d, const float *queries, const int64_t *q_off, int64_t n_queries,
-                            float *out_scores);
-pb_status pb_dep_delete(Deployment *d, const int64_t *doc_ids, int64_t n_ids, const char *index_dir, int64_t *out_deleted);
-// pb_index_append (codec != null) or pb_index_append_encoded
-pb_status pb_dep_append(Deployment *d, pb_codec *codec, const float *embeddings, const int64_t *codes,
-                        const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
-                        const char *index_dir, int64_t batch_size, int64_t *out_first_doc_id);
-pb_status pb_dep_rebalance(Deployment *d, const int64_t *bounds, int64_t *out_bounds);
 // pb_index_add_devices / pb_index_remove_ranks after the handle's checks.  `handle` is the deployment's own: its rank-0
 // fields follow a new rank 0.
 pb_status pb_dep_add_devices(Deployment *d, const int32_t *devices, int32_t n, const int64_t *bounds, int64_t *out_bounds);
 pb_status pb_dep_remove_ranks(Deployment *d, pb_index *handle, const int32_t *ranks, int32_t n, const int64_t *bounds,
                               int64_t *out_bounds);
-// call(rank) on every rank in turn, the lowest rank's failure first; mutations wait, searches go on (the row cache's
-// entry points, which are rank-local)
-pb_status pb_dep_ranks(Deployment *d, const std::function<pb_status(pb_index *)> &call);
 // A deployment of ranks already loaded (ranks[r] on devices[r], not yet in a group): joins them in a new group and
 // returns its handle.  On failure the ranks are closed.
 pb_status pb_dep_assemble(std::vector<pb_index *> ranks, const std::vector<int> &devices, pb_index **out);
-
-// A replica set (pb_index_load_replicas, replicas.cpp, DESIGN §4q): R full copies of an index, each a plain handle or a
-// deployment, behind one pb_index that holds no documents; the entry points of engine.cu hand such a handle to the
-// functions below.
-struct Replicas;
-pb_index *pb_index_new_replicas(Replicas *rs, const pb_index *member0);
-pb_index *pb_rep_member(Replicas *rs, int g);
-int pb_rep_count(const Replicas *rs);
-void pb_rep_close(Replicas *rs);
-void pb_rep_each(Replicas *rs, const std::function<void(pb_index *)> &call);
 // A routed search of n queries: cut into contiguous slices [b0, b1), each run by call(member, b0, b1, slice) on one of
 // the least-loaded replicas, slice 0 on the caller's thread.  Returns the lowest failing slice's status.
 pb_status pb_rep_search(Replicas *rs, int64_t n_queries,
                         const std::function<pb_status(pb_index *, int64_t, int64_t, int)> &call);
-// call(member) on the least-loaded replica for a whole request of n queries (a merged batch, a reader)
-pb_status pb_rep_whole(Replicas *rs, int64_t n_queries, const std::function<pb_status(pb_index *)> &call);
-pb_status pb_rep_memory(Replicas *rs, int64_t *device_bytes, int64_t *host_bytes);
-// the mutations, under the set's writer lock
-pb_status pb_rep_delete(Replicas *rs, const int64_t *doc_ids, int64_t n_ids, const char *index_dir, int64_t *out_deleted);
-pb_status pb_rep_append(Replicas *rs, pb_codec *codec, const float *embeddings, const int64_t *codes,
-                        const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
-                        const char *index_dir, int64_t batch_size, int64_t *out_first_doc_id);
-pb_status pb_rep_reserve(Replicas *rs, int64_t num_documents, int64_t num_embeddings);
-pb_status pb_rep_rebalance(Replicas *rs, const int64_t *bounds, int64_t *out_bounds);
-// call(member) on every replica in turn, under the set's writer lock (writer) or its reader lock; the lowest replica's
-// failure first (the row cache's entry points)
-pb_status pb_rep_members(Replicas *rs, bool writer, const std::function<pb_status(pb_index *)> &call);
 
 // A copy of a plain handle (or one rank of a deployment, outside its group) on `device`: every array, derived ones
 // included, copied device to device; a host-tier handle shares src's pinned residuals.  The copy's device-dependent
@@ -188,6 +181,8 @@ void pb_index_set_rep_vote(pb_index *member, RepVote *v, int replica);
 // the set behind a handle (null for any other handle); rank r of a deployment's handle (the handle itself otherwise)
 Replicas *pb_replicas_of(const pb_index *ix);
 pb_index *pb_rank_of(pb_index *ix, int r);
+// a handle's documents and tokens, read together
+void pb_index_totals(const pb_index *ix, long long *D, long long *N);
 // a mutable host-tier handle or deployment: the replicas of a set write one shared row store, through replica 0 only
 bool pb_host_rows_shared(pb_index *ix);
 // cudaDeviceSynchronize on the device of ix, or of each of its ranks

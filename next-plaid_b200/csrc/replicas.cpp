@@ -30,7 +30,7 @@ struct Crew {  // helper threads of one routed call: slices 1..R-1
 
 }  // namespace
 
-struct Replicas {
+struct Replicas : Group {
     int S = 1;
     std::vector<pb_index *> members;  // [R]: plain handles (S = 1) or deployments (S > 1)
     std::vector<int> devices;         // [R * S]
@@ -85,7 +85,7 @@ struct Replicas {
     }
     // op(member, g) on every replica at once, slice-thread style (replica 0 on the caller's thread); the lowest failing
     // replica's status and message.  With a vote (S > 1 mutations) the replicas' ranks take it together.
-    pb_status each(const std::function<pb_status(pb_index *, int)> &op, RepVote *vote = nullptr) {
+    pb_status at_once(const std::function<pb_status(pb_index *, int)> &op, RepVote *vote = nullptr) {
         for (int g = 0; g < R() && vote; ++g) pb_index_set_rep_vote(members[g], vote, g);
         std::unique_ptr<Crew> crew = take_crew();
         std::vector<pb_status> st;
@@ -99,24 +99,54 @@ struct Replicas {
                               : pb_fail(st[g], "replica %d: %s", g, err[g].c_str());
         return PB_OK;
     }
-    // each() of a mutation on deployments, with the vote that makes it commit on every replica or on none
+    // at_once() of a mutation on deployments, with the vote that makes it commit on every replica or on none
     pb_status voted(bool with_dir, bool share_rows, const std::function<pb_status(pb_index *, int)> &op) {
         std::unique_ptr<RepVote, void (*)(RepVote *)> v(pb_rep_vote_new(R() * S, with_dir, share_rows), pb_rep_vote_free);
-        return each(op, v.get());
+        return at_once(op, v.get());
     }
-    ~Replicas() {
+    // joins the threads, closes the replicas
+    ~Replicas() override {
         crews.clear();  // joins the threads
         for (pb_index *m : members)
             if (m) pb_index_close(m);
     }
-};
 
-pb_index *pb_rep_member(Replicas *rs, int g) { return rs->members[g]; }
-int pb_rep_count(const Replicas *rs) { return rs->R(); }
-void pb_rep_close(Replicas *rs) { delete rs; }
-void pb_rep_each(Replicas *rs, const std::function<void(pb_index *)> &call) {
-    for (pb_index *m : rs->members) call(m);
-}
+    const char *kind() const override { return "a replica set (pb_index_load_replicas)"; }
+    Replicas *as_replicas() override { return this; }
+    pb_index *member(int g) override { return members[g]; }
+    int size() override { return R(); }
+    // what every replica holds, from replica 0
+    void totals(long long *D, long long *N) override { pb_index_totals(members[0], D, N); }
+    pb_status shard_layout(int32_t *out_world, int64_t *out_bounds, int32_t *out_devices) override {
+        return pb_index_shard_layout(members[0], out_world, out_bounds, out_devices);
+    }
+    pb_status last_delete_ms(float *out_ms) override {
+        return pb_last_delete_ms(members[0], out_ms);  // the set's last delete ran there too
+    }
+    pb_status memory(int64_t *device_bytes, int64_t *host_bytes) override;
+    // the mutations, under the set's writer lock
+    pb_status append(pb_codec *codec, const float *embeddings, const int64_t *codes, const uint8_t *residuals,
+                     const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space, const char *index_dir,
+                     int64_t batch_size, int64_t *out_first_doc_id) override;
+    pb_status del(const int64_t *doc_ids, int64_t n_ids, const char *index_dir, int64_t *out_deleted) override;
+    pb_status rebalance(const int64_t *bounds, int64_t *out_bounds) override;
+    pb_status reserve(int64_t num_documents, int64_t num_embeddings) override;
+    // the readers of one whole copy, on the least-loaded replica
+    pb_status decompress(const int64_t *doc_ids, int64_t n_docs, float *out_embeddings, int64_t *out_lengths) override {
+        return one(0, [&](pb_index *m) { return pb_decompress_documents(m, doc_ids, n_docs, out_embeddings, out_lengths); });
+    }
+    pb_status exhaustive(const float *queries, const int64_t *q_off, int64_t n_queries, float *out_scores) override {
+        return one(0, [&](pb_index *m) { return pb_exhaustive_scores(m, queries, q_off, n_queries, out_scores); });
+    }
+    pb_status export_ivf(int64_t *out_ivf, int32_t *out_lengths, int64_t *out_total) override {
+        return one(0, [&](pb_index *m) { return pb_index_export_ivf(m, out_ivf, out_lengths, out_total); });
+    }
+    void each(const std::function<void(pb_index *)> &call) override {
+        for (pb_index *m : members) call(m);
+    }
+    pb_status in_turn(bool writer, const std::function<pb_status(pb_index *)> &call) override;
+    pb_status one(int64_t n, const std::function<pb_status(pb_index *)> &call) override;
+};
 
 extern "C" pb_status pb_index_load_replicas(const char *index_dir, const int32_t *devices, int32_t n_devices,
                                             int32_t n_shards, int32_t flags, pb_index **out) {
@@ -166,7 +196,7 @@ extern "C" pb_status pb_index_load_replicas(const char *index_dir, const int32_t
     for (auto &x : w)
         if (x->status != PB_OK) return pb_fail(x->status, "%s", x->error.c_str());  // ~Replicas closes what loaded
     w.clear();
-    *out = pb_index_new_replicas(rs.get(), m0);
+    *out = pb_index_new_group(rs.get(), m0);
     rs.release();
     return PB_OK;
 }
@@ -191,21 +221,21 @@ pb_status pb_rep_search(Replicas *rs, int64_t n, const std::function<pb_status(p
     return PB_OK;
 }
 
-pb_status pb_rep_whole(Replicas *rs, int64_t n, const std::function<pb_status(pb_index *)> &call) {
-    auto rd = rs->read_lock();
+pb_status Replicas::one(int64_t n, const std::function<pb_status(pb_index *)> &call) {
+    auto rd = read_lock();
     const std::vector<int64_t> share(1, std::max<int64_t>(n, 0));
-    const std::vector<int> who = rs->pick(share);
-    const pb_status st = call(rs->members[who[0]]);
-    rs->done(who, share);
+    const std::vector<int> who = pick(share);
+    const pb_status st = call(members[who[0]]);
+    done(who, share);
     return st;
 }
 
 // device bytes over every member; host bytes once: every replica reads replica 0's pinned arrays
-pb_status pb_rep_memory(Replicas *rs, int64_t *device_bytes, int64_t *host_bytes) {
+pb_status Replicas::memory(int64_t *device_bytes, int64_t *host_bytes) {
     int64_t dev = 0, host = 0;
-    for (int g = 0; g < rs->R(); ++g) {
+    for (int g = 0; g < R(); ++g) {
         int64_t a = 0, h = 0;
-        pb_status s = pb_index_memory(rs->members[g], &a, &h);
+        pb_status s = pb_index_memory(members[g], &a, &h);
         if (s != PB_OK) return s;
         dev += a;
         if (g == 0) host = h;
@@ -224,13 +254,13 @@ static pb_status quiesce(Replicas *rs) {
     return PB_OK;
 }
 
-pb_status pb_rep_delete(Replicas *rs, const int64_t *doc_ids, int64_t n_ids, const char *index_dir, int64_t *out_deleted) {
-    std::lock_guard<std::mutex> g(rs->gate);
-    std::unique_lock<std::shared_mutex> wr(rs->rw);
-    if (pb_status s = quiesce(rs)) return s;
-    if (rs->S == 1) return pb_members_delete(rs->members, doc_ids, n_ids, index_dir, out_deleted);
+pb_status Replicas::del(const int64_t *doc_ids, int64_t n_ids, const char *index_dir, int64_t *out_deleted) {
+    std::lock_guard<std::mutex> g(gate);
+    std::unique_lock<std::shared_mutex> wr(rw);
+    if (pb_status s = quiesce(this)) return s;
+    if (S == 1) return pb_members_delete(members, doc_ids, n_ids, index_dir, out_deleted);
     // replica 0 writes the directory
-    return rs->voted(index_dir != nullptr, false, [&](pb_index *m, int r) {
+    return voted(index_dir != nullptr, false, [&](pb_index *m, int r) {
         int64_t d = 0;
         const pb_status s = pb_index_delete(m, doc_ids, n_ids, r == 0 ? index_dir : nullptr, &d);
         if (r == 0 && out_deleted) *out_deleted = d;
@@ -238,18 +268,18 @@ pb_status pb_rep_delete(Replicas *rs, const int64_t *doc_ids, int64_t n_ids, con
     });
 }
 
-pb_status pb_rep_append(Replicas *rs, pb_codec *codec, const float *embeddings, const int64_t *codes,
-                        const uint8_t *residuals, const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space,
-                        const char *index_dir, int64_t batch_size, int64_t *out_first_doc_id) {
-    std::lock_guard<std::mutex> g(rs->gate);
-    std::unique_lock<std::shared_mutex> wr(rs->rw);
-    if (pb_status s = quiesce(rs)) return s;
-    if (rs->S == 1)
-        return pb_members_append(rs->members, codec, embeddings, codes, residuals, doc_lengths, n_docs, memory_space,
+pb_status Replicas::append(pb_codec *codec, const float *embeddings, const int64_t *codes, const uint8_t *residuals,
+                           const int64_t *doc_lengths, int64_t n_docs, int32_t memory_space, const char *index_dir,
+                           int64_t batch_size, int64_t *out_first_doc_id) {
+    std::lock_guard<std::mutex> g(gate);
+    std::unique_lock<std::shared_mutex> wr(rw);
+    if (pb_status s = quiesce(this)) return s;
+    if (S == 1)
+        return pb_members_append(members, codec, embeddings, codes, residuals, doc_lengths, n_docs, memory_space,
                                  index_dir, batch_size, out_first_doc_id);
     // with a codec replica 0's last rank encodes and writes the directory; the other replicas append its rows.  On a
     // mutable host tier they also wait for it without a codec: its prepare writes the rows they read
-    return rs->voted(index_dir != nullptr, codec != nullptr || pb_host_rows_shared(rs->members[0]),
+    return voted(index_dir != nullptr, codec != nullptr || pb_host_rows_shared(members[0]),
                      [&](pb_index *m, int r) -> pb_status {
         if (r == 0)
             return codec ? pb_index_append(m, codec, embeddings, doc_lengths, n_docs, memory_space, index_dir, batch_size,
@@ -261,29 +291,29 @@ pb_status pb_rep_append(Replicas *rs, pb_codec *codec, const float *embeddings, 
 }
 
 // Capacity only: a replica that reserved before another failed keeps it, and no result depends on it
-pb_status pb_rep_reserve(Replicas *rs, int64_t num_documents, int64_t num_embeddings) {
-    std::lock_guard<std::mutex> g(rs->gate);
-    std::unique_lock<std::shared_mutex> wr(rs->rw);
-    if (pb_status s = quiesce(rs)) return s;
-    return rs->each([&](pb_index *m, int) { return pb_index_reserve(m, num_documents, num_embeddings); });
+pb_status Replicas::reserve(int64_t num_documents, int64_t num_embeddings) {
+    std::lock_guard<std::mutex> g(gate);
+    std::unique_lock<std::shared_mutex> wr(rw);
+    if (pb_status s = quiesce(this)) return s;
+    return at_once([&](pb_index *m, int) { return pb_index_reserve(m, num_documents, num_embeddings); });
 }
 
-pb_status pb_rep_rebalance(Replicas *rs, const int64_t *bounds, int64_t *out_bounds) {
-    std::lock_guard<std::mutex> g(rs->gate);
-    std::unique_lock<std::shared_mutex> wr(rs->rw);
-    return rs->voted(false, false, [&](pb_index *m, int r) {
+pb_status Replicas::rebalance(const int64_t *bounds, int64_t *out_bounds) {
+    std::lock_guard<std::mutex> g(gate);
+    std::unique_lock<std::shared_mutex> wr(rw);
+    return voted(false, false, [&](pb_index *m, int r) {
         return pb_index_rebalance_sharded(m, bounds, r == 0 ? out_bounds : nullptr);
     });
 }
 
-pb_status pb_rep_members(Replicas *rs, bool writer, const std::function<pb_status(pb_index *)> &call) {
-    std::unique_lock<std::mutex> g(rs->gate);
-    std::unique_lock<std::shared_mutex> wr(rs->rw, std::defer_lock);
-    std::shared_lock<std::shared_mutex> rd(rs->rw, std::defer_lock);
+pb_status Replicas::in_turn(bool writer, const std::function<pb_status(pb_index *)> &call) {
+    std::unique_lock<std::mutex> g(gate);
+    std::unique_lock<std::shared_mutex> wr(rw, std::defer_lock);
+    std::shared_lock<std::shared_mutex> rd(rw, std::defer_lock);
     if (writer) wr.lock();
     else g.unlock(), rd.lock();
-    for (int i = 0; i < rs->R(); ++i)
-        if (pb_status s = call(rs->members[i])) {
+    for (int i = 0; i < R(); ++i)
+        if (pb_status s = call(members[i])) {
             const std::string e = pb_last_error();
             return i == 0 ? s : pb_fail(s, "replica %d: %s", i, e.c_str());
         }

@@ -230,7 +230,7 @@ def test_accessors_and_readers(npb, corpus):
     full = npb.MmapIndex.load(path)
     try:
         acc = lambda h: [h.num_documents(), h.num_embeddings(), h.num_partitions(), h.avg_doclen(),  # noqa: E731
-                         h.embedding_dim(), h.nbits()]
+                         h.embedding_dim(), h.nbits(), npb.load_library().pb_index_device(h._h)]
         ids = [899, 0, 450, 450, 200, 199, 5, -1, 900, 10 ** 9, 3]
         e_full, l_full = full.decompress_documents(ids)
         ex_full = full.exhaustive_scores(qs)

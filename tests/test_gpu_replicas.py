@@ -127,7 +127,8 @@ def test_search_routing_and_readers(npb, corpus):
             assert calls.tolist() == [1] * R and queries.tolist() == [32] * R, (R, S, calls, queries)
             assert _searches(npb, rep, qs, D, R) == _searches(npb, plain, qs, D, R), (R, S)
             acc = lambda h: [h.num_documents(), h.num_embeddings(), h.num_partitions(), h.avg_doclen(),  # noqa: E731
-                             h.embedding_dim(), h.nbits(), h.shard_layout()[0].tolist()]
+                             h.embedding_dim(), h.nbits(), h.shard_layout()[0].tolist(),
+                             npb.load_library().pb_index_device(h._h)]
             assert acc(rep) == acc(plain)
             e1, l1 = rep.decompress_documents(ids)
             e2, l2 = plain.decompress_documents(ids)
@@ -137,6 +138,7 @@ def test_search_routing_and_readers(npb, corpus):
             if S == 1:
                 a, b = rep.export_ivf(), plain.export_ivf()
                 assert all(np.array_equal(x, y) for x, y in zip(a, b))
+                assert rep.last_delete_ms() == plain.last_delete_ms()
             m1, m0 = rep.memory_usage(), plain.memory_usage()
             assert m1 == {"device_bytes": R * m0["device_bytes"], "host_bytes": 0}, (m1, m0)
         finally:
