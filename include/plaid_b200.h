@@ -890,12 +890,49 @@ PB_API pb_status pb_index_remove_ranks(pb_index *ix, const int32_t *ranks, int32
 PB_API pb_status pb_index_load_replicas(const char *index_dir, const int32_t *devices, int32_t n_devices,
                                         int32_t n_shards, int32_t flags, pb_index **out);
 /* *out_replicas = R, *out_shards = S and (may be NULL) out_devices [R*S].  Any other handle is one replica of its
- * pb_index_shard_layout ranks. */
+ * pb_index_shard_layout ranks.  R may change between calls (pb_index_add_replicas): an out_devices of 64 entries, the
+ * member limit, is always large enough. */
 PB_API pb_status pb_index_replica_layout(const pb_index *ix, int32_t *out_replicas, int32_t *out_shards,
                                          int32_t *out_devices /* [R*S], may be NULL */);
 /* Per replica, since load or the last reset: calls or slices it served (out_calls [R]) and queries (out_queries [R]);
- * either may be NULL.  PB_ERR_INVALID on a handle that is not a replica set. */
+ * either may be NULL.  PB_ERR_INVALID on a handle that is not a replica set.  Arrays of 64 entries are always large
+ * enough, whatever resize comes between a caller's pb_index_replica_layout and this call. */
 PB_API pb_status pb_index_replica_stats(pb_index *ix, int64_t *out_calls, int64_t *out_queries, int32_t reset);
+
+/* ---- changing a replica set's number of replicas (DESIGN.md 4u) ---------------------------
+ *
+ * A live replica set of pb_index_load_replicas gains or loses whole replicas without a reload; nothing changes but R.
+ * Afterwards every entry point gives what it gave before, and what pb_index_load_replicas(dir, new devices, S, flags)
+ * of an in-sync directory gives, bit for bit: every search form, coalesced pb_search, decompression, exhaustive scores,
+ * the accessors and pb_index_memory.  New replicas go after the last one; a removal keeps the order of the replicas
+ * that stay.  Replica 0 may be removed: the next replica becomes replica 0, writes the directory in later mutations and
+ * the shared row store of a PB_OPEN_HOST_MUTABLE set, and pb_index_device follows it.  Each replica keeps its
+ * pb_index_replica_stats counts; a new one starts at 0.  Coalescing's max_inflight stays per replica.
+ *
+ * An add copies replica 0 (pb_index_clone of each of its ranks, peer to peer, as at load) while the set keeps serving:
+ * searches, coalesced batches and readers go on on the replicas it has.  Mutations (append, append_encoded, delete,
+ * reserve, rebalance), pb_index_set_row_cache / pb_index_fill_row_cache and another resize wait until it ends, so no
+ * copy mixes the state before a mutation with the state after it.  The new replicas enter the rotation at once, with
+ * the switches replica 0 has then: a search sees the old set or the new one.  A removal waits for the routed calls and
+ * merged batches in flight; requests queued on the coalescer are answered by the replicas that stay.
+ *
+ * Refusals, checked before anything is allocated, the handle unchanged and usable, in this order: PB_ERR_INVALID for a
+ * NULL ix / devices / replicas; PB_ERR_UNSUPPORTED for a handle that is not a replica set (a single index, a
+ * deployment, a rank of a doc-sharded group: to grow from one copy, load the directory with pb_index_load_replicas at
+ * R = 1); PB_ERR_INVALID for n_devices not a positive multiple of S, more than 64 devices in all, a device id outside
+ * [0, pb_device_count()), n_replicas < 1, removing every replica, and a replica outside [0, R) or listed twice.  A copy
+ * that fails (PB_ERR_NOMEM on the target device, a CUDA error) closes the copies made so far and returns the lowest
+ * failing replica's status and message; the set is as it was.
+ *
+ * Memory: a new replica holds what replica 0 holds on its devices, capacity included, and a row cache's rows; host
+ * bytes are counted once, as every replica reads one pinned row store.  A removal frees the leaving replicas' device
+ * memory; the host store is freed with the last replica. */
+/* n_devices / S new replicas after the last one; replica R + i uses devices[i*S .. i*S + S-1] (devices may repeat or
+ * be devices the set already uses).  Each is copied device to device from replica 0 while the set keeps serving. */
+PB_API pb_status pb_index_add_replicas(pb_index *ix, const int32_t *devices, int32_t n_devices);
+/* The listed replicas (distinct, in [0, R), not all of them) leave the set once the calls they serve have finished;
+ * the others keep their order; their device memory is freed.  pb_index_device follows the new replica 0. */
+PB_API pb_status pb_index_remove_replicas(pb_index *ix, const int32_t *replicas, int32_t n_replicas);
 
 /* ---- misc ----------------------------------------------------------------------------- */
 

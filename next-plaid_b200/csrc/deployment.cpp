@@ -108,7 +108,6 @@ struct Deployment : Group {
     const char *kind() const override { return "a multi-device handle (pb_index_load_devices)"; }
     Deployment *as_deployment() override { return this; }
     pb_index *member(int r) override { return ranks[r]; }
-    int size() override { return world(); }
     void totals(long long *D, long long *N) override;
     pb_status memory(int64_t *device_bytes, int64_t *host_bytes) override;
     pb_status shard_layout(int32_t *out_world, int64_t *out_bounds, int32_t *out_devices) override;
@@ -131,7 +130,8 @@ struct Deployment : Group {
         for (pb_index *ix : ranks) call(ix);
     }
     pb_status in_turn(bool, const std::function<pb_status(pb_index *)> &call) override;
-    pb_status one(int64_t, const std::function<pb_status(pb_index *)> &call) override {
+    pb_status one(int64_t, const std::function<pb_status(pb_index *)> &call) override { return first(call); }
+    pb_status first(const std::function<pb_status(pb_index *)> &call) override {
         std::shared_lock<std::shared_mutex> g(layout);
         return call(ranks[0]);
     }

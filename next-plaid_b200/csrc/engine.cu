@@ -692,6 +692,7 @@ struct pb_index : DocArrays, Switches {
     // pb_search: concurrent single-query callers merged into shared batches (pb_index_set_coalescing; off by default)
     pbq::Queue<CoalescedRun> coalescer{CoalescedRun{this}, PB_ERR_CUDA};
     std::atomic<bool> coalesce_on{false};
+    pbq::Config coalesce_cfg;  // as the caller set it: a replica set's max_inflight is per replica
     std::vector<std::unique_ptr<GatherBuf>> gather_pool;  // under mu
     float delete_ms[3] = {0.f, 0.f, 0.f};  // last pb_index_delete with profiling on: compaction, inverted file, norms
     // Readers (searches, stage entry points, accessors) share the arrays; pb_index_append / pb_index_reserve hold them
@@ -1425,8 +1426,8 @@ extern "C" int32_t pb_index_embedding_dim(const pb_index *ix) { return ix ? ix->
 extern "C" int32_t pb_index_nbits(const pb_index *ix) { return ix ? ix->nbits : 0; }
 extern "C" int32_t pb_index_device(const pb_index *ix) {
     if (!ix) return -1;
-    int32_t dv = ix->device;  // a deployment's: its rank 0's, which pb_index_remove_ranks may change
-    if (ix->group && ix->group->as_deployment()) ix->group->one(0, [&](pb_index *r0) { return dv = r0->device, PB_OK; });
+    int32_t dv = ix->device;  // a group's: its first member's, which a resize may change
+    if (ix->group) ix->group->first([&](pb_index *m) { return dv = pb_index_device(m), PB_OK; });
     return dv;
 }
 
@@ -1486,12 +1487,22 @@ extern "C" pb_status pb_index_set_coalescing(pb_index *ix, const pb_coalesce_con
             return pb_fail(PB_ERR_UNSUPPORTED, "coalescing on a doc-sharded handle: a collective needs the same order on every rank");
         c.max_queries = cfg->max_queries;
         c.max_wait_us = std::min(cfg->max_wait_us, 10000);
-        // a replica set runs max_inflight merged batches per replica
-        c.max_inflight = pb_replicas_of(ix) ? cfg->max_inflight * ix->group->size() : cfg->max_inflight;
+        c.max_inflight = cfg->max_inflight;
     }
+    auto set = [&](int R) {
+        ix->coalesce_cfg = c;
+        pb_index_apply_coalescing(ix, R);
+    };
+    if (Replicas *rs = pb_replicas_of(ix)) pb_rep_sized(rs, set);  // a resize rescales it
+    else set(1);
+    return PB_OK;
+}
+// a replica set runs max_inflight merged batches per replica
+void pb_index_apply_coalescing(pb_index *ix, int R) {
+    pbq::Config c = ix->coalesce_cfg;
+    c.max_inflight *= R;
     ix->coalescer.configure(c);
     ix->coalesce_on = c.max_queries > 1;
-    return PB_OK;
 }
 extern "C" pb_status pb_index_coalesce_stats(pb_index *ix, pb_coalesce_stats *out, int32_t reset) {
     if (!ix || !out) return pb_fail(PB_ERR_INVALID, "null argument");
@@ -3383,7 +3394,7 @@ static pb_status search_io(pb_index *ix, const SearchIO &io, const char *traced)
                   check_query_args(p) == PB_OK && query_kept_docs(p, &M) == PB_OK;
         }
         if (!cut) return whole();
-        std::vector<Stats> stats((size_t)ix->group->size());
+        std::vector<Stats> stats(PB_MAX_MEMBERS);  // a slice per replica: R may change until pb_rep_search holds the set
         size_t slices = 0;
         const pb_status st = pb_rep_search(rs, io.n_queries, [&](pb_index *m, int64_t b0, int64_t b1, int k) {
             const pb_status r = search_io(m, slice_io(io, b0, b1), traced);
@@ -3576,12 +3587,12 @@ extern "C" pb_status pb_search(pb_index *ix, const float *query, int64_t n_query
     pb_status st;
     if (ix->group) {  // as one handle of the whole index: every rank's K, the deployment's D (rank 0 may be empty)
         const long long D = pb_index_num_documents(ix);
-        pb_index *m = pb_replicas_of(ix) ? ix->group->member(0) : ix;
         auto check = [&](pb_index *h) {
             auto rd = h->read_lock();
             return check_request(h, D, r);
         };
-        st = m->group ? m->group->one(0, check) : check(m);
+        // a deployment's rank 0; a replica set's replica 0, or its rank 0
+        st = ix->group->first([&](pb_index *m) { return m->group ? m->group->first(check) : check(m); });
     } else {
         auto rd = ix->read_lock();
         st = check_request(ix, ix->D, r);
@@ -5318,6 +5329,9 @@ pb_status pb_index_clone(const pb_index *src, int device, pb_index **out) {
     CKS(clone_buf(ix->w_rev, src->w_rev, device, src->device, st.s));
     CKS(clone_buf(ix->cent_h16t, src->cent_h16t, device, src->device, st.s));
     CKS(clone_buf(ix->cent_l16t, src->cent_l16t, device, src->device, st.s));
+    // a row cache: its map and counts are per-doc arrays (above), its rows and what they hold follow
+    CKS(clone_buf(ix->rc.rows, src->rc.rows, device, src->device, st.s));
+    ix->rc.budget = src->rc.budget, ix->rc.docs = src->rc.docs, ix->rc.bytes = src->rc.bytes, ix->rc.dead = src->rc.dead;
     CK(cudaStreamSynchronize(st.s));
     CKS(coalesce_env_defaults(ix.get()));
     *out = ix.release();
@@ -5372,6 +5386,15 @@ static pb_status tail_rows(const pb_index *ix, long long t0, long long n, std::v
 }
 
 Replicas *pb_replicas_of(const pb_index *ix) { return ix && ix->group ? ix->group->as_replicas() : nullptr; }
+void pb_index_copy_switches(pb_index *dst, pb_index *src) {
+    if (!dst->group) {
+        static_cast<Switches &>(*dst) = static_cast<const Switches &>(*src);
+        return;
+    }
+    int32_t world = 0;
+    pb_index_shard_layout(dst, &world, nullptr, nullptr);
+    for (int r = 0; r < world; ++r) pb_index_copy_switches(pb_rank_of(dst, r), pb_rank_of(src, r));
+}
 pb_index *pb_rank_of(pb_index *ix, int r) { return ix->group && ix->group->as_deployment() ? ix->group->member(r) : ix; }
 bool pb_host_rows_shared(pb_index *ix) { return pb_rank_of(ix, 0)->host_mutable; }
 pb_status pb_sync_devices(pb_index *ix) {
@@ -5868,11 +5891,16 @@ extern "C" pb_status pb_index_rebalance_sharded(pb_index *ix, const int64_t *bou
     return pb_index_rebalance_shares(ix, bounds, nullptr, out_bounds);
 }
 
-// The calls that change a deployment's number of ranks (DESIGN §4t) address a deployment of pb_index_load_devices only
-static pb_status refuse_resize(const pb_index *ix, const char *call) {
-    if (ix->group) return ix->group->as_deployment() ? PB_OK : ix->group->refuse(call);
-    return pb_fail(PB_ERR_UNSUPPORTED, "%s needs a multi-device handle of pb_index_load_devices (this handle is %s)",
-                   call, ix->comm.joined() ? "a rank of a doc-sharded group" : "a single index");
+// The calls that change a deployment's number of ranks (DESIGN §4t) address a deployment of pb_index_load_devices only;
+// those that change a replica set's number of replicas (§4u), a replica set of pb_index_load_replicas only
+static pb_status refuse_resize(const pb_index *ix, const char *call, bool replicas = false) {
+    if (ix->group) {
+        const bool mine = replicas ? ix->group->as_replicas() != nullptr : ix->group->as_deployment() != nullptr;
+        return mine ? PB_OK : ix->group->refuse(call);
+    }
+    return pb_fail(PB_ERR_UNSUPPORTED, "%s needs %s (this handle is %s)", call,
+                   replicas ? "a replica set of pb_index_load_replicas" : "a multi-device handle of pb_index_load_devices",
+                   ix->comm.joined() ? "a rank of a doc-sharded group" : "a single index");
 }
 
 extern "C" pb_status pb_index_add_devices(pb_index *ix, const int32_t *devices, int32_t n_devices, const int64_t *bounds,
@@ -5887,6 +5915,18 @@ extern "C" pb_status pb_index_remove_ranks(pb_index *ix, const int32_t *ranks, i
     if (!ix || !ranks) return pb_fail(PB_ERR_INVALID, "null argument");
     CKS(refuse_resize(ix, "pb_index_remove_ranks"));
     return pb_dep_remove_ranks(ix->group->as_deployment(), ix, ranks, n_ranks, bounds, out_bounds);
+}
+
+extern "C" pb_status pb_index_add_replicas(pb_index *ix, const int32_t *devices, int32_t n_devices) {
+    if (!ix || !devices) return pb_fail(PB_ERR_INVALID, "null argument");
+    CKS(refuse_resize(ix, "pb_index_add_replicas", true));
+    return pb_rep_add(ix->group->as_replicas(), ix, devices, n_devices);
+}
+
+extern "C" pb_status pb_index_remove_replicas(pb_index *ix, const int32_t *replicas, int32_t n_replicas) {
+    if (!ix || !replicas) return pb_fail(PB_ERR_INVALID, "null argument");
+    CKS(refuse_resize(ix, "pb_index_remove_replicas", true));
+    return pb_rep_remove(ix->group->as_replicas(), ix, replicas, n_replicas);
 }
 
 pb_status pb_index_rebalance_shares(pb_index *ix, const int64_t *bounds, const uint8_t *shares, int64_t *out_bounds) {

@@ -97,10 +97,10 @@ struct Group {
     // the concrete group, for the calls only one kind serves (search, resize); null for the other kind
     virtual Deployment *as_deployment() { return nullptr; }
     virtual Replicas *as_replicas() { return nullptr; }
-    // member i's handle, unlocked: only for a group whose members cannot change (a replica set, or a deployment that is
-    // a replica set's member and so refuses pb_index_add_devices / pb_index_remove_ranks); elsewhere one() or in_turn()
+    // member i's handle, unlocked: only for a group whose members cannot change (a deployment that is a replica set's
+    // member and so refuses pb_index_add_devices / pb_index_remove_ranks) or while the caller holds the group's lock;
+    // elsewhere first(), one() or in_turn().  Both kinds of group change their members while live (DESIGN §4t, §4u).
     virtual pb_index *member(int i) = 0;
-    virtual int size() = 0;
     // the whole index's documents and tokens, read together
     virtual void totals(long long *D, long long *N) = 0;
     virtual pb_status memory(int64_t *device_bytes, int64_t *host_bytes) = 0;
@@ -123,7 +123,12 @@ struct Group {
     virtual pb_status in_turn(bool writer, const std::function<pb_status(pb_index *)> &call) = 0;
     // call(m) on one member, on the caller's thread, for a whole request of n queries (a merged batch, a reader)
     virtual pb_status one(int64_t n_queries, const std::function<pb_status(pb_index *)> &call) = 0;
+    // call(m) on member 0 (a deployment's rank 0, a replica set's replica 0), under the group's lock and counted as no
+    // request: what every member shares (pb_search's request check, pb_index_device)
+    virtual pb_status first(const std::function<pb_status(pb_index *)> &call) = 0;
 };
+// The most members a group has: ranks of a deployment, devices of a replica set (R * S)
+constexpr int PB_MAX_MEMBERS = 64;
 // A group's handle, owning g: K, dim, nbits and device copied from g's first member (pb_index_deployment_rank0); the
 // PB_COALESCE* defaults applied
 pb_index *pb_index_new_group(Group *g, const pb_index *first);
@@ -146,10 +151,20 @@ pb_status pb_dep_assemble(std::vector<pb_index *> ranks, const std::vector<int> 
 // the least-loaded replicas, slice 0 on the caller's thread.  Returns the lowest failing slice's status.
 pb_status pb_rep_search(Replicas *rs, int64_t n_queries,
                         const std::function<pb_status(pb_index *, int64_t, int64_t, int)> &call);
+// pb_index_add_replicas / pb_index_remove_replicas after the null checks.  `handle` is the set's own: its replica-0
+// fields and its coalescing limit follow the new set.
+pb_status pb_rep_add(Replicas *rs, pb_index *handle, const int32_t *devices, int32_t n_devices);
+pb_status pb_rep_remove(Replicas *rs, pb_index *handle, const int32_t *replicas, int32_t n_replicas);
+// call(R) under the lock that a change of the set's number of replicas R takes (pb_index_set_coalescing)
+void pb_rep_sized(Replicas *rs, const std::function<void(int)> &call);
+// the handle's coalescing configuration applied to its queue, max_inflight scaled by R (a replica set's replicas)
+void pb_index_apply_coalescing(pb_index *ix, int R);
+// dst's pb_set_* switches (each rank's, for a deployment) made src's; no search may be running on dst
+void pb_index_copy_switches(pb_index *dst, pb_index *src);
 
 // A copy of a plain handle (or one rank of a deployment, outside its group) on `device`: every array, derived ones
-// included, copied device to device; a host-tier handle shares src's pinned residuals.  The copy's device-dependent
-// scalars are its own.
+// included, copied device to device; a host-tier handle shares src's pinned residuals.  A row cache comes with its rows
+// and what they hold, its staging counters at 0.  The copy's device-dependent scalars are its own.
 pb_status pb_index_clone(const pb_index *src, int device, pb_index **out);
 // An empty rank on `device` opened from a peer src (a handle of the same index, one deployment rank): src's centroids,
 // bucket weights and search switches copied, no documents, global ids from doc_id_base.  It equals pb_index_load_range

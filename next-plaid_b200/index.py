@@ -110,6 +110,7 @@ EXPORTS = [
     "pb_index_load_devices", "pb_index_shard_layout", "pb_pooled_doc_length", "pb_pool_embeddings", "pb_last_pool_ms",
     "pb_index_add_devices", "pb_index_remove_ranks",
     "pb_index_load_replicas", "pb_index_replica_layout", "pb_index_replica_stats",
+    "pb_index_add_replicas", "pb_index_remove_replicas",
     "pb_index_set_row_cache", "pb_index_fill_row_cache", "pb_index_row_cache_stats",
 ]
 
@@ -238,6 +239,8 @@ def load_library():
                                              C.POINTER(C.c_void_p)]
         L.pb_index_replica_layout.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.pb_index_replica_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]
+        L.pb_index_add_replicas.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
+        L.pb_index_remove_replicas.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
         L.pb_index_set_row_cache.argtypes = [C.c_void_p, C.c_int64]
         L.pb_index_fill_row_cache.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]
         L.pb_index_row_cache_stats.argtypes = [C.c_void_p, C.POINTER(_RowCacheStats), C.c_int32]
@@ -576,21 +579,37 @@ class MmapIndex:
         ix._world = shards
         return ix
 
+    # the member limit: arrays of this many entries hold any layout, whatever resize comes between two calls
+    _MAX_MEMBERS = 64
+
     def replica_layout(self):
         """pb_index_replica_layout: (replicas, shards, devices [replicas, shards]); any other handle is one replica."""
         r, s = C.c_int32(), C.c_int32()
-        _check(load_library().pb_index_replica_layout(self._h, C.byref(r), C.byref(s), None))
-        d = np.zeros(r.value * s.value, np.int32)
+        d = np.zeros(self._MAX_MEMBERS, np.int32)
         _check(load_library().pb_index_replica_layout(self._h, C.byref(r), C.byref(s), _ptr(d)))
-        return r.value, s.value, d.reshape(r.value, s.value)
+        return r.value, s.value, d[:r.value * s.value].reshape(r.value, s.value)
 
     def replica_stats(self, reset: bool = False):
-        """pb_index_replica_stats: per replica since load or the last reset, (calls or slices served, queries)."""
-        r, s = C.c_int32(), C.c_int32()
-        _check(load_library().pb_index_replica_layout(self._h, C.byref(r), C.byref(s), None))
-        calls, queries = np.zeros(r.value, np.int64), np.zeros(r.value, np.int64)
+        """pb_index_replica_stats: per replica since load or the last reset, (calls or slices served, queries).  Under
+        a concurrent resize the arrays have the length of the layout read after the counts."""
+        calls, queries = np.zeros(self._MAX_MEMBERS, np.int64), np.zeros(self._MAX_MEMBERS, np.int64)
         _check(load_library().pb_index_replica_stats(self._h, _ptr(calls), _ptr(queries), int(reset)))
-        return calls, queries
+        r = self.replica_layout()[0]
+        return calls[:r], queries[:r]
+
+    def add_replicas(self, devices: Sequence[int]) -> None:
+        """pb_index_add_replicas: len(devices) / shards new replicas after the last one of a load_replicas set, replica
+        R + i on devices[i * shards : (i + 1) * shards], each copied device to device from replica 0 while the set keeps
+        serving.  Results do not change."""
+        dv = np.ascontiguousarray(list(devices), np.int32)
+        _check(load_library().pb_index_add_replicas(self._h, _ptr(dv), len(dv)))
+
+    def remove_replicas(self, replicas: Sequence[int]) -> None:
+        """pb_index_remove_replicas: the listed replicas (distinct, not all) leave a load_replicas set once the calls
+        they serve have finished; the others keep their order and the next one becomes replica 0 when replica 0 leaves.
+        Their device memory is freed.  Results do not change."""
+        rp = np.ascontiguousarray(list(replicas), np.int32)
+        _check(load_library().pb_index_remove_replicas(self._h, _ptr(rp), len(rp)))
 
     @classmethod
     def load_shard(cls, index_path: str, rank: int, world: int, device: int = 0,

@@ -159,6 +159,8 @@ extern "C" {
                              out_bounds: *mut i64) -> c_int;
     fn pb_index_load_replicas(index_dir: *const c_char, devices: *const i32, n_devices: i32, n_shards: i32, flags: i32,
                               out: *mut *mut c_void) -> c_int;
+    fn pb_index_add_replicas(ix: *mut c_void, devices: *const i32, n_devices: i32) -> c_int;
+    fn pb_index_remove_replicas(ix: *mut c_void, replicas: *const i32, n_replicas: i32) -> c_int;
     fn pb_index_memory(ix: *const c_void, device_bytes: *mut i64, host_bytes: *mut i64) -> c_int;
     fn pb_last_staging_stats(ix: *mut c_void, docs: *mut i64, bytes: *mut i64, ms: *mut f32) -> c_int;
     fn pb_index_set_row_cache(ix: *mut c_void, max_bytes: i64) -> c_int;
@@ -518,6 +520,27 @@ impl B200Index {
             return Err(Error::IndexLoad(last_error()));
         }
         Ok(w as usize)
+    }
+
+    /// Add `devices.len() / shards` replicas after the last one of a `load_replicas` set (`pb_index_add_replicas`,
+    /// DESIGN §4u): replica R + i on `devices[i * shards .. (i + 1) * shards]`, each copied device to device from
+    /// replica 0 while the set keeps serving searches; mutations wait for it.  Results do not change; a failure leaves
+    /// the set as it was.
+    pub fn add_replicas(&self, devices: &[i32]) -> Result<()> {
+        if unsafe { pb_index_add_replicas(self.handle, devices.as_ptr(), devices.len() as i32) } != 0 {
+            return Err(Error::IndexLoad(last_error()));
+        }
+        Ok(())
+    }
+
+    /// The listed replicas (distinct, not all) leave a `load_replicas` set once the calls they serve have finished
+    /// (`pb_index_remove_replicas`, DESIGN §4u); the others keep their order, the next becoming replica 0 if replica 0
+    /// leaves, and the leaving replicas' device memory is freed.  Results do not change.
+    pub fn remove_replicas(&self, replicas: &[i32]) -> Result<()> {
+        if unsafe { pb_index_remove_replicas(self.handle, replicas.as_ptr(), replicas.len() as i32) } != 0 {
+            return Err(Error::IndexLoad(last_error()));
+        }
+        Ok(())
     }
 
     fn resize(&self, bounds: Option<&[i64]>, world: usize, call: impl FnOnce(*const i64, *mut i64) -> c_int)
